@@ -45,20 +45,12 @@ def parse_args():
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-parity", action="store_true", help="skip the CPU-oracle check of the first sample (the GPU-side digests still run)")
     ap.add_argument("--no-vxgi", action="store_true")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write the image the timed path returned for its last step to DIR/*.npy (float32)")
     ap.add_argument("--global-slots", action="store_true",
                     help="N > 1: IDKPT_CREATE_GLOBAL_SLOTS -- per-bounce exchange of per-stripe alive counts over NVLink, the N-GPU image is "
                          "bit-identical to the 1-GPU image (SURVEY 8e option ii); parity_check then compares against a 1-GPU frame")
     return ap.parse_args()
-
-
-def measured_traffic():
-    """ncu --set full figures of the current kernels (profiles/traffic.json, regenerated by scripts/ncu_summary.py from the
-    round's capture): DRAM bytes per launch and DRAM utilisation of the heaviest traversal launches, or None."""
-    p = os.path.join(REPO, "profiles", "traffic.json")
-    try:
-        return json.load(open(p))
-    except Exception:
-        return None
 
 
 def measured_peaks():
@@ -68,11 +60,11 @@ def measured_peaks():
             return float(json.load(open(p))["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs)"
         except Exception:
             pass
-    return 6650.0, "fallback (B200_PROFILING.md 6.65 TB/s)"
+    return 3350.0, "fallback (H100 SXM data sheet 3.35 TB/s)"
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons during the timed region (B200_PROFILING.md recipe)."""
+    """nvidia-smi clocks / throttle reasons during the timed region."""
     Q = "index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.active,clocks_event_reasons.hw_slowdown," \
         "clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap"
 
@@ -117,6 +109,19 @@ class ClockSampler:
         return {"sm_mhz": float(np.median(sm)), "sm_max_mhz": float(max(mx)), "reasons": sorted(reasons), "samples": len(sm)}
 
 
+def gpu_info(device):
+    """The card a number was measured on: name and power limit (a power-capped card runs lower clocks)."""
+    import torch
+    info = {"name": torch.cuda.get_device_name(device), "power_limit_w": None}
+    try:
+        out = subprocess.run(["nvidia-smi", "--query-gpu=power.limit", "--format=csv,noheader,nounits", "-i", str(device)],
+                             capture_output=True, text=True, timeout=30).stdout.strip()
+        info["power_limit_w"] = float(out.splitlines()[0])
+    except Exception:
+        pass
+    return info
+
+
 def build_scene(args):
     from idkengine_b200 import scenes
     if args.workload == "config3":
@@ -142,7 +147,7 @@ def workload_config(args, world, scene):
                        f"FinalDraw over NVLink peer memory (IDKPT_GATHER=nccl: one NCCL all-gather per frame)",
         "slots": ("global (IDKPT_CREATE_GLOBAL_SLOTS): per-stripe alive counts exchanged over NVLink every bounce, image == 1-GPU image"
                   if (getattr(args, "global_slots", False) and world > 1) else "tile-local (one collective per frame; image reproducible per GPU count)"),
-        "l2": "per-step working set (2x64B path state + hits, ~330 MB at 1080p) exceeds the 126 MB L2; the 22 MB BVH is "
+        "l2": "per-step working set (2x64B path state + hits, ~330 MB at 1080p) exceeds the 50 MB L2; the 22 MB BVH is "
               "re-read every bounce and is L2-resident by design (SURVEY 8d)",
     }
 
@@ -299,6 +304,24 @@ def vxgi_record(scene, frame, pt, args):
             "mipmap_unique_gbs": gbs(mip_bytes, best.MipmapMs), "mipmap_frac": gbs(mip_bytes, best.MipmapMs) / peak,
             "cone_texel_gbs": gbs(cone_bytes, cone.ConeTraceMs),
             "parity": "tests/test_configs_gpu.py::test_config5_vxgi_384_cubed (every level and the cone image == oracle)"}
+
+
+DUMP_LIMIT = 64 << 20
+
+
+def dump_outputs(out_dir, image):
+    """image.npy: the rgba32f accumulated image, H x W x 4. A larger image (4K) is written as a fixed sample instead:
+    image_sample.npy (n x 4) at the pixels image_sample_index.npy (row-major pixel index, float64), chosen with seed 0."""
+    os.makedirs(out_dir, exist_ok=True)
+    image = np.ascontiguousarray(image, np.float32)
+    if image.nbytes <= DUMP_LIMIT:
+        np.save(os.path.join(out_dir, "image.npy"), image)
+        return
+    flat = image.reshape(-1, image.shape[-1])
+    n = DUMP_LIMIT // (flat.shape[1] * 4 + 8)
+    idx = np.sort(np.random.default_rng(0).choice(len(flat), n, replace=False))
+    np.save(os.path.join(out_dir, "image_sample.npy"), flat[idx])
+    np.save(os.path.join(out_dir, "image_sample_index.npy"), idx.astype(np.float64))
 
 
 def bind_to_gpu_numa_node(local_rank):
@@ -459,6 +482,7 @@ def run_ours(args, rank, world, local_rank):
         pipe_ms = pe0.elapsed_time(pe1)
         assert pt.AccumulatedSamples == args.steps
         digest_pipelined = digest(pt.Result[rows])
+    timed_image = pt.Result[rows] if args.dump_outputs else None      # what the pass behind `value` returned for its last step
 
     # ---- timed region 2: end to end through the public API with host buffers (frame H2D, result D2H every step)
     pt.ResetAccumulation()
@@ -471,6 +495,8 @@ def run_ours(args, rank, world, local_rank):
     barrier()
     e2e_ms = (time.perf_counter() - t0) * 1e3
     final_host = host.np[(args.steps - 1) & 1]
+    if args.dump_outputs and rank == 0:     # N > 1: the full frame every rank presented into (parity_check: == the timed tiles)
+        dump_outputs(args.dump_outputs, timed_image if world == 1 else final_host)
 
     # ---- parity of what was just timed (untimed). Everything is compared bit for bit.
     #  a) serial pass == pipelined pass == the image the e2e pass left in the host frame (same K samples from a reset);
@@ -554,7 +580,6 @@ def run_ours(args, rank, world, local_rank):
 
     if rank == 0:
         peak, peak_src = measured_peaks()
-        traffic = measured_traffic()
         trav_bytes = 64 * S + 52 * T + 48 * I + 52 * R      # DESIGN.md: algorithmic bytes of k_traverse (rank 0's tile)
         achieved = trav_bytes / (trav_ms * 1e-3) / 1e9
         shade_only_ms = shade_ms - compact_ms
@@ -581,16 +606,14 @@ def run_ours(args, rank, world, local_rank):
                          "frac_measured_in": "serial pass of the same K steps: algorithmic bytes / CUDA-event time of the traversal launches",
                          "frac_pipelined": (trav_bytes / (job_ms * 1e-3) / 1e9) / peak if world == 1 else None,
                          "frac_pipelined_is": "the same algorithmic bytes / the WHOLE pipelined step (traversal overlaps the shading of other samples): a lower bound for the kernel, the figure behind `value`",
-                         "dram_frac": (traffic or {}).get("dram_frac"), "traffic": (traffic or {}).get("dram_bytes_per_launch"),
-                         "traffic_source": (traffic or {}).get("source"),
-                         "bound_note": "the BVH (26 MB) is L2-resident by design: DRAM traffic is far below the algorithmic bytes and the kernel is paced by L1/L2 transactions and SIMT divergence, not by HBM (profiles/r02_*)",
+                         "bound_note": "the BVH (26 MB) is kept L2-resident by a persisting access-policy window: the algorithmic bytes overstate the DRAM traffic",
                          "peak_source": peak_src,
                          "algorithmic_bytes_per_launch": trav_bytes / max(trav_launches, 1),
                          "launch_ms": trav_ms / max(trav_launches, 1),
                          "per_ray": {"node_pair_fetches": S / R, "triangle_tests": T / R, "instances": I / R},
                          "other_kernels": {
                              "k_shade": {"ms_per_step": shade_only_ms / args.steps, "algorithmic_gbs": gbs(shade_bytes, shade_only_ms), "frac": gbs(shade_bytes, shade_only_ms) / peak,
-                                         "bytes_per_ray": shade_bytes / R, "dram_frac": (traffic or {}).get("shade_dram_frac")},
+                                         "bytes_per_ray": shade_bytes / R},
                              "k_compact": {"ms_per_step": compact_ms / args.steps, "algorithmic_gbs": gbs(compact_bytes, compact_ms), "frac": (gbs(compact_bytes, compact_ms) or 0) / peak,
                                            "note": "8 launches per sample over 4-byte entries: launch-latency bound"},
                              "k_accumulate": {"ms_per_step": acc_ms / args.steps, "algorithmic_gbs": gbs(acc_bytes, acc_ms), "frac": (gbs(acc_bytes, acc_ms) or 0) / peak}}},
@@ -602,6 +625,7 @@ def run_ours(args, rank, world, local_rank):
             "parity_check": parity,
             "gpu_launches": total_launches,
             "clocks": clocks,
+            "gpu": gpu_info(local_rank),
         }
         if per_rank is not None:
             line["per_rank_ms"] = per_rank

@@ -1,6 +1,6 @@
 """Build helpers: compile the in-tree native libraries.
 
-  libidkpt.so   -- the product: CUDA kernels for sm_100a + the C ABI (include/idkpt.h)
+  libidkpt.so   -- the product: CUDA kernels for sm_90a (H100) + the C ABI (include/idkpt.h)
   libidkhost.so -- host-side mirror of the engine's C# BVH builder (no CUDA)
 
 The oracle (oracle/) has its own recipe, oracle/build.py: it is test infrastructure and
@@ -20,7 +20,7 @@ LIBIDKPT = os.path.join(CSRC_DIR, "libidkpt.so")
 LIBIDKHOST = os.path.join(HOST_DIR, "libidkhost.so")
 
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a",
+    "-gencode", "arch=compute_90a,code=sm_90a",
     "-O3", "-lineinfo", "-std=c++17",
     # Parity contract (DESIGN.md "Float semantics"): no FMA contraction, IEEE div/sqrt.
     "-fmad=false", "-prec-div=true", "-prec-sqrt=true", "-ftz=false",

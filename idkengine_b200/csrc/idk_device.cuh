@@ -1,10 +1,10 @@
-// Device-side math for libidkpt (sm_100a). Float semantics contract (DESIGN.md):
+// Device-side math for libidkpt (sm_90a). Float semantics contract (DESIGN.md):
 // fp32, left-to-right evaluation, NO fused multiply-add (the TU is compiled with
 // -fmad=false), IEEE divide / sqrt (-prec-div=true -prec-sqrt=true), fminf/fmaxf
 // return the non-NaN operand. normalize(v) = v * (1/sqrt(dot)), pow(x,5) by
 // squaring, sin/cos/exp = the polynomial routines below.
 //
-// GLSL sources restated (relative to /root/reference/IDKEngine/Resource/Shaders):
+// GLSL sources restated (relative to the reference repository's IDKEngine/Resource/Shaders):
 //   include/IntersectionRoutines.glsl:6-69, include/Random.glsl:16-33,
 //   include/Sampling.glsl:4-19,59-68,86-114, include/Compression.glsl:11-73,
 //   include/Math.glsl:6-15,41-57,104-137
@@ -283,11 +283,8 @@ __device__ __forceinline__ bool ray_sphere(f3 o, f3 d, f3 position, float radius
 __device__ __forceinline__ float4 ldg4(const float4* p) { return __ldg(p); }
 
 // ---- experiment switches (defaults = the measured best; scripts/variant_probe.py builds and times the alternatives)
-#ifndef IDK_NODE_V8
-#define IDK_NODE_V8 1        // sibling pair = 2 x 256-bit loads (LDG.E.256, new on sm_100) instead of 4 x 128-bit
-#endif
 #ifndef IDK_TRI_STRIDE
-#define IDK_TRI_STRIDE 4     // float4s per device-private triangle record: 3 = packed 48 B, 4 = 64 B (one 128-B line, 2 x LDG.E.256)
+#define IDK_TRI_STRIDE 4     // float4s per device-private triangle record: 3 = packed 48 B, 4 = 64 B (never straddles a 128-B line)
 #endif
 #ifndef IDK_REG_STACK
 #define IDK_REG_STACK 0      // k_traverse2: top N entries of the traversal stack live in registers (0 = all in shared memory)
@@ -309,30 +306,15 @@ __device__ __forceinline__ float4 ldg4(const float4* p) { return __ldg(p); }
 // One GpuBlasNode sibling pair (64 bytes, children are adjacent: BLAS.cs:16-22) / two adjacent GpuTlasNodes.
 struct NodePair { float4 lA, lB, rA, rB; };
 
-__device__ __forceinline__ void ldg256(const void* p, float4& a, float4& b) {   // p 32-byte aligned, read-only data
-    asm("ld.global.nc.v8.f32 {%0,%1,%2,%3,%4,%5,%6,%7}, [%8];"
-        : "=f"(a.x), "=f"(a.y), "=f"(a.z), "=f"(a.w), "=f"(b.x), "=f"(b.y), "=f"(b.z), "=f"(b.w) : "l"(p));
-}
-
+// 4 x 128-bit read-only loads (the widest global load sm_90 has)
 __device__ __forceinline__ NodePair ldg_pair(const float4* np) {
     NodePair r;
-#if IDK_NODE_V8
-    ldg256(np, r.lA, r.lB);
-    ldg256(np + 2, r.rA, r.rB);
-#else
     r.lA = ldg4(np); r.lB = ldg4(np + 1); r.rA = ldg4(np + 2); r.rB = ldg4(np + 3);
-#endif
     return r;
 }
 
 // Device-private triangle record i: (p0.xyz,e1.x) (e1.yz,e2.xy) (e2.z,n.xyz) [pad]
 __device__ __forceinline__ void ldg_tri(const float4* triRec, size_t i, float4& a, float4& b, float4& c) {
     const float4* tr = triRec + IDK_TRI_STRIDE * i;
-#if IDK_TRI_STRIDE == 4 && IDK_NODE_V8
-    float4 pad;
-    ldg256(tr, a, b);
-    ldg256(tr + 2, c, pad);
-#else
     a = ldg4(tr); b = ldg4(tr + 1); c = ldg4(tr + 2);
-#endif
 }

@@ -1,4 +1,4 @@
-// Wavefront path-tracing kernels for sm_100a (B200). See DESIGN.md for the HBM layout and the
+// Wavefront path-tracing kernels for sm_90a (H100). See DESIGN.md for the HBM layout and the
 // algorithmic-byte accounting of each kernel.
 //
 //   k_prepare_triangles/vertices/surfaces  scene upload: 48-byte triangle records, decoded vertex frames, per-mesh surfaces
@@ -389,7 +389,7 @@ __device__ __forceinline__ void tma_stage_treelet(void* smemDst, const void* gme
 // and the ticket of the batch after that is already in a register. A SETUP round then hands rays out of shared memory
 // instead of walking the dependent chain atomicAdd -> alive[] -> PathState (three L2/HBM round trips) for a dozen lanes at
 // a time; that makes SETUP rounds cheap enough to run them for few waiting lanes (lower setupThreshold, fewer idle lanes
-// in the BOX rounds: profiles/r02_phase_stats.txt). Which lane traces which ray changes; what is traced does not.
+// in the BOX rounds). Which lane traces which ray changes; what is traced does not.
 #ifndef IDK_STAGE_CG
 #define IDK_STAGE_CG 0
 #endif
@@ -665,12 +665,7 @@ __global__ void __launch_bounds__(IDK_T2_BLOCK) k_traverse2(TraverseArgs a, Trav
                 nodes = sc.nodes + 2 * (size_t)nodeOffset;
                 curXf = bi.MeshTransformId;
                 if (STATS) I++;
-                float4 ra, rb;
-#if IDK_NODE_V8
-                ldg256(nodes + 2, ra, rb);
-#else
-                ra = ldg4(nodes + 2); rb = ldg4(nodes + 3);
-#endif
+                const float4 ra = ldg4(nodes + 2), rb = ldg4(nodes + 3);
                 float tRoot;
                 if (ray_box(lo, inv, ra, rb, tRoot) && tRoot < hit.t) {
                     state = ST_BOX;

@@ -1,4 +1,4 @@
-// VXGI kernels for sm_100a over a linear rgba16f 3D grid in HBM (all mip levels in one allocation).
+// VXGI kernels for sm_90a over a linear rgba16f 3D grid in HBM (all mip levels in one allocation).
 //
 //   k_vx_voxelize_small / k_vx_voxelize_large   Voxelize/{vertex,geometry,fragment}.glsl + MergeIntermediates
 //   k_vx_mipmap                                 Voxelize/Mipmap/compute.glsl

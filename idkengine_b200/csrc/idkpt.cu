@@ -1,4 +1,4 @@
-// libidkpt: C ABI (include/idkpt.h) over the sm_100a wavefront kernels (idk_kernels.cuh).
+// libidkpt: C ABI (include/idkpt.h) over the sm_90a wavefront kernels (idk_kernels.cuh).
 // Host sequencing mirrors PathTracer.Compute(), IDKEngine/Source/Render/PathTracer.cs:214-297, with
 // every GL dispatch replaced by a CUDA launch on one stream and no CPU read-back inside the loop
 // (alive counts stay on the device, like the reference's indirect dispatch).
@@ -49,7 +49,7 @@ struct Lane {
 
 struct IdkPtCtx {
     int device = 0;
-    int smCount = 148;
+    int smCount = 132;
     cudaStream_t stream = nullptr;
     std::string lastError;
 
@@ -89,7 +89,7 @@ struct IdkPtCtx {
 
     // wavefront buffers: one set per lane. A lane is one sample in flight (ray-gen .. last shade) on its own stream; with
     // several lanes the latency-bound tail bounces of one sample overlap the throughput-bound head of the next
-    // (profiles/r01h_overlap_probe.json). Lane 0 also serves the synchronous path (stats, export, debug).
+    // Lane 0 also serves the synchronous path (stats, export, debug).
     Lane lanes[IDK_MAX_LANES];
     int laneCount = 8;             // lanes used by asynchronous idkpt_compute (stats == NULL); IDKPT_LANES / CreateInfo.Flags
     int nextLane = 0;
@@ -107,8 +107,8 @@ struct IdkPtCtx {
     int traverseBlocksLane = 0, traverse1BlocksLane = 0;   // grids of the asynchronous path: the resident-block budget split between the lanes
     int traverseVariant = 3;       // 1 = k_traverse (one ray per lane, reference loop), 2 = k_traverse2 (phase-scheduled warps),
                                    // 3 = k_traverse for the coherent primary rays, k_traverse2 for every bounce (default)
-    TraverseTuning tune = {12, 4, 0, 6, 0};   // swept on B200 (profiles/r01b_tuning.txt); packRays is set per launch
-    int packCta = 0;                 // IDKPT_PACK_CTA: pipelined launches let only ceil(rays / (256 * k)) CTAs take part (0 = all; measured neutral at k = 1, slower at 2 / 4: profiles/r02_traverse_experiments.txt)
+    TraverseTuning tune = {12, 4, 0, 6, 0};   // thresholds of the phase vote (IDKPT_TUNE_*); packRays is set per launch
+    int packCta = 0;                 // IDKPT_PACK_CTA: pipelined launches let only ceil(rays / (256 * k)) CTAs take part (0 = all)
     int packAsync = 1;               // IDKPT_PACK_ASYNC: asynchronous (pipelined) launches pack 32 rays per warp instead of spreading few rays over all warps
     size_t stackBytes = 0;
     size_t traverse2Smem = 0;      // treelet + stacks
@@ -125,7 +125,7 @@ struct IdkPtCtx {
     bool peerMapped[IDK_MAX_PEERS] = {};
     uint32_t gatherEpoch = 0;
     double gatherTimeoutMs = 30000.0;                                     // arrival wait bound (IDKPT_GATHER_TIMEOUT_MS); a dead peer becomes an error, not a hung GPU
-    int clockKHz = 1965000;
+    int clockKHz = 1980000;
     int gatherCurrent = -1;                                               // buffer holding the last completed frame
     bool peerIsIpc = false;                                               // peers mapped with cudaIpcOpenMemHandle (else: same-process pointers)
     // global slots (IDKPT_CREATE_GLOBAL_SLOTS): per-stripe alive counts exchanged every bounce; table = [lane][parity][stripe] u64
@@ -238,11 +238,11 @@ static int configure_launches(IdkPtCtx* ctx) {
     CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&n, k_compact, IDK_BLOCK, 0));
     ctx->compactBlocks = std::max(1, std::min(n, 4)) * ctx->smCount;
     // asynchronous path: `laneCount` samples in flight share the SMs; each lane's persistent traversal grid takes its share of
-    // the resident-block budget (profiles/r01h_overlap_probe.json: 4 x 1 block/SM beats 4 x full grid by 24 % on a 1/8 tile)
+    // the resident-block budget
     {
         const int lanes = std::max(1, ctx->laneCount);
         const int perSm2 = (ctx->traverseBlocks / ctx->smCount + lanes - 1) / lanes, perSm1 = (ctx->traverse1Blocks / ctx->smCount + lanes - 1) / lanes;
-        ctx->traverseBlocksLane = std::max(1, perSm2) * ctx->smCount;      // profiles/r01h_lanes_probe.json: 3 lanes x 2 blocks/SM, 4+ lanes x 1
+        ctx->traverseBlocksLane = std::max(1, perSm2) * ctx->smCount;
         ctx->traverse1BlocksLane = std::max(1, perSm1) * ctx->smCount;
     }
     if (const char* v = getenv("IDKPT_LANE_BLOCKS_PER_SM")) {        // developer knob
@@ -536,9 +536,9 @@ IDKPT_API int idkpt_create(const IdkPtCreateInfo* ci, IdkPtCtx** out) {
     if (cudaSetDevice(ci->Device) != cudaSuccess) return fail(nullptr, IDKPT_ERR_CUDA, "idkpt_create: cudaSetDevice failed");
     cudaDeviceProp prop;
     if (cudaGetDeviceProperties(&prop, ci->Device) != cudaSuccess) return fail(nullptr, IDKPT_ERR_CUDA, "idkpt_create: cudaGetDeviceProperties failed");
-    if (prop.major < 10) {
+    if (prop.major != 9 || prop.minor != 0) {
         char buf[512];
-        snprintf(buf, sizeof(buf), "idkpt_create: device '%s' is sm_%d%d; libidkpt is built for sm_100a only", prop.name, prop.major, prop.minor);
+        snprintf(buf, sizeof(buf), "idkpt_create: device '%s' is sm_%d%d; libidkpt is built for sm_90a only", prop.name, prop.major, prop.minor);
         return fail(nullptr, IDKPT_ERR_NO_DEVICE, buf);
     }
     IdkPtCtx* ctx = new IdkPtCtx();
@@ -668,7 +668,7 @@ IDKPT_API int idkpt_set_scene(IdkPtCtx* ctx, const IdkPtSceneDesc* s) {
     std::vector<GpuBlasNode> relaid;
     {
         const char* env = getenv("IDKPT_TREELET_PAIRS");
-        const uint32_t wantPairs = env ? (uint32_t)std::min(768, std::max(0, atoi(env))) : 0u;   // default off: measured no gain over the L1 (profiles/r01d_treelet.txt)
+        const uint32_t wantPairs = env ? (uint32_t)std::min(768, std::max(0, atoi(env))) : 0u;   // default off
         if (wantPairs > 0 && !s->UseTlas && s->BlasInstanceCount == 1 && s->BlasDescCount == 1 && s->BlasDescs[0].NodeOffset == 0 &&
             s->BlasNodeCount < (1ull << 31) && (s->BlasNodeCount & 1) == 0) {
             const int got = relayout_treelet(s->BlasNodes, (uint32_t)s->BlasNodeCount, wantPairs, relaid);
@@ -738,7 +738,7 @@ IDKPT_API int idkpt_set_scene(IdkPtCtx* ctx, const IdkPtSceneDesc* s) {
     ctx->hostDescs.assign(s->BlasDescs, s->BlasDescs + s->BlasDescCount);
     ctx->nodeBytes = nodeBytes;
     if ((rc = configure_launches(ctx))) return rc;
-    // Keep the BVH resident in the 126 MB L2: persisting access-policy window over [nodes | triRec] on the render stream.
+    // Keep the BVH resident in the 50 MB L2: persisting access-policy window over [nodes | triRec] on the render stream.
     // The wavefront buffers (hundreds of MB per frame) stream through the rest of the cache without evicting the tree.
     {
         cudaDeviceProp prop;

@@ -17,7 +17,7 @@
 static thread_local std::string g_vxCreateError;
 
 struct IdkVxCtx {
-    int device = 0, smCount = 148;
+    int device = 0, smCount = 132;
     cudaStream_t stream = nullptr;
     std::string lastError;
     VxGridDev grid = {};
@@ -85,7 +85,7 @@ IDKPT_API int idkvx_create(const IdkVxCreateInfo* ci, IdkVxCtx** out) {
     if (cudaSetDevice(ci->Device) != cudaSuccess) return vfail(nullptr, IDKPT_ERR_CUDA, "idkvx_create: cudaSetDevice failed");
     cudaDeviceProp prop;
     if (cudaGetDeviceProperties(&prop, ci->Device) != cudaSuccess) return vfail(nullptr, IDKPT_ERR_CUDA, "idkvx_create: cudaGetDeviceProperties failed");
-    if (prop.major < 10) return vfail(nullptr, IDKPT_ERR_NO_DEVICE, "idkvx_create: libidkpt is built for sm_100a only");
+    if (prop.major != 9 || prop.minor != 0) return vfail(nullptr, IDKPT_ERR_NO_DEVICE, "idkvx_create: libidkpt is built for sm_90a only");
     IdkVxCtx* ctx = new IdkVxCtx();
     ctx->device = ci->Device;
     ctx->smCount = prop.multiProcessorCount;
@@ -269,8 +269,8 @@ IDKPT_API int idkvx_voxelize(IdkVxCtx* ctx, IdkVxStats* stats) {
         // levels that halve exactly on every axis and are big enough to fill the machine take the shared-memory tiled kernel
         const VxGridDev& gd = ctx->grid;
         const bool halves = gd.sx[l - 1] == 2 * gd.sx[l] && gd.sy[l - 1] == 2 * gd.sy[l] && gd.sz[l - 1] == 2 * gd.sz[l];
-        // measured on B200 (bench.py vxgi record, 384^3): tiled 0.82 ms vs 0.43 ms for the direct kernel -- the direct kernel's 7x
-        // re-reads are L1 hits and the filter is bound by its ~640 fp32 operations per texel, not by memory; opt-in only (cross-check)
+        // the direct kernel's 7x re-reads are L1 hits and the filter is bound by its ~640 fp32 operations per texel, not by
+        // memory, so the tiled kernel is opt-in only (cross-check)
         const bool tiledOn = getenv("IDKVX_MIP_TILED") && atoi(getenv("IDKVX_MIP_TILED")) != 0;
         if (halves && n >= 4096 && tiledOn) {
             const int tiles = ((gd.sx[l] + IDKVX_MT_X - 1) / IDKVX_MT_X) * ((gd.sy[l] + IDKVX_MT_Y - 1) / IDKVX_MT_Y) * ((gd.sz[l] + IDKVX_MT_Z - 1) / IDKVX_MT_Z);

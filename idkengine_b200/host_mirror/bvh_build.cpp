@@ -3,7 +3,7 @@
 // BVH build and camera"). It exists here because this image has no .NET; it
 // produces exactly the arrays the engine uploads to SSBO 20-23.
 //
-// Mirrors (file:line relative to /root/reference/IDKEngine/Source):
+// Mirrors (file:line relative to the reference repository's IDKEngine/Source):
 //   Bvh/PreSplitting.cs:26-160   PreSplit (early split clipping)
 //   Bvh/BLAS.cs:128-157          GetBuildData (3 radix sorts by centroid key)
 //   Bvh/BLAS.cs:159-274          Build / ProcessBuildTask / RemoveEmptySubtrees

@@ -1,5 +1,4 @@
-"""Synthetic scene generators for the configs of BASELINE.json (SURVEY.md section 8d) plus a loader for
-the reference's own Sponza geometry (used only by local tests; /root/reference does not exist on the GPU box).
+"""Synthetic scene generators for the configs of BASELINE.json (SURVEY.md section 8d) plus a minimal glTF geometry loader.
 
 All generators are seeded and deterministic; all materials use constant (1x1) textures, i.e. factors only
 (the reference's own fallback for missing maps, SRC/Utils/ModelLoader.cs:877-885).
@@ -431,10 +430,7 @@ def texturize(scene, size=512, count=8, seed=11):
     return scene
 
 
-# --------------------------------------------------------------------------- real Sponza (local only)
-REFERENCE_SPONZA = "/root/reference/IDKEngine/Resource/Models/SponzaCompressed/Sponza.gltf"
-
-
+# --------------------------------------------------------------------------- glTF geometry
 def load_gltf_geometry(path):
     """Minimal glTF reader: float32 POSITION/NORMAL/TEXCOORD_0 + integer indices, factor-only materials."""
     with open(path) as f:
@@ -476,35 +472,6 @@ def load_gltf_geometry(path):
             mesh_mat.append(prim.get("material", 0))
             nv += len(p)
     return g, pos, nrm, uv, idx, tri_mesh, mesh_mat
-
-
-def sponza_reference(threads=None):
-    """Config 2 with the reference's real Sponza.bin geometry (262,267 triangles). Materials from glTF factors with
-    metallic=0, roughness=0.8 (SURVEY 8d 'constant-texture semantics'); emissive biases per SRC/Application.cs:449-457."""
-    g, pos, nrm, uv, idx, tri_mesh, mesh_mat = load_gltf_geometry(REFERENCE_SPONZA)
-    gm = g.get("materials", [{}])
-    mats = gt.default_material(len(gm))
-    for k, m in enumerate(gm):
-        pbr = m.get("pbrMetallicRoughness", {})
-        mats["BaseColorFactor"][k] = gt.pack_unorm4x8(np.array(pbr.get("baseColorFactor", [1, 1, 1, 1])))
-        mats["MetallicFactor"][k] = 0.0
-        mats["RoughnessFactor"][k] = 0.8
-        mats["EmissiveFactor"][k] = m.get("emissiveFactor", [0, 0, 0])
-        mode = m.get("alphaMode", "OPAQUE")
-        mats["AlphaCutoff"][k] = 0.0 if mode == "OPAQUE" else (m.get("alphaCutoff", 0.5) if mode == "MASK" else 2.0)
-        mats["IsDoubleSided"][k] = 1 if m.get("doubleSided", False) else 0
-    meshes = gt.default_mesh(len(mesh_mat))
-    meshes["MaterialId"] = np.array(mesh_mat, np.int32)
-    for mid, bias in {63: 10.0, 70: 20.0, 3: 12.0, 99: 15.0, 97: 9.0, 42: 20.0, 38: 20.0, 40: 20.0}.items():
-        if mid < len(meshes):
-            meshes["EmissiveBias"][mid] = bias
-    normals = None if any(n is None for n in nrm) else np.concatenate(nrm)
-    model = Model(np.concatenate(pos), np.concatenate(idx), np.concatenate(tri_mesh), normals=normals,
-                  texcoords=np.concatenate(uv), meshes=meshes, materials=mats,
-                  model_matrix=trs_matrix(1.815, 0.0, (0.0, -1.0, 0.0)), name="sponza")
-    scene = Scene().add(model, threads=threads)
-    cam = dict(position=(7.63, 2.71, 0.8), view_dir=tuple(view_dir_from_angles(360.0 - 165.4, 90.0 - 7.4)), fov_y_deg=102.0)
-    return scene, cam
 
 
 def camera_frame(cam, width, height):

@@ -1,5 +1,5 @@
 /*
- * idkpt.h -- C ABI of libidkpt, the B200-native replacement for the body of
+ * idkpt.h -- C ABI of libidkpt, the H100-native replacement for the body of
  * IDKEngine.Render.PathTracer (reference: IDKEngine/Source/Render/PathTracer.cs).
  *
  * The C# class keeps its public surface (ctor / Compute / SetSize /

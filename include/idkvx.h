@@ -1,5 +1,5 @@
 /*
- * idkvx.h -- C ABI of the VXGI passes of libidkpt: voxelise, mipmap and cone-trace GI as sm_100a kernels over a
+ * idkvx.h -- C ABI of the VXGI passes of libidkpt: voxelise, mipmap and cone-trace GI as sm_90a kernels over a
  * linear 3D rgba16f grid in HBM (BASELINE.json configs[4]).
  *
  * Replaces (reference paths relative to IDKEngine/):

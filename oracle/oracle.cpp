@@ -11,7 +11,7 @@
 // (b) a brute-force all-triangles intersector, (c) the builder's structural
 // invariants (tests/test_bvh_build.py).
 //
-// Restated sources (relative to /root/reference/IDKEngine):
+// Restated sources (relative to the reference repository's IDKEngine):
 //   Resource/Shaders/include/BVHIntersect.glsl:27-105,183-291  IntersectBlas, TraceRay (closest, no-TLAS + TLAS)
 //   Resource/Shaders/include/IntersectionRoutines.glsl:6-69   ray/triangle, ray/box, ray/sphere
 //   Resource/Shaders/include/Ray.glsl:7-12                    RayTransform

@@ -1,9 +1,9 @@
-"""A/B harness for kernel experiments: build libidkpt with -D switches into gpurun-travelling side files here (CPU), then
-time every variant on the GPU box in its own process (same scene, same samples) and check that all of them produce the
+"""A/B harness for kernel experiments: build libidkpt with -D switches into side files (CPU), then
+time every variant on the GPU in its own process (same scene, same samples) and check that all of them produce the
 same image and the same S/T/I counters as the default build.
 
-    python scripts/variant_probe.py --build name:-DIDK_NODE_V8=0 name2:-DIDK_REG_STACK=0,-DIDK_TRI_STRIDE=3   (here)
-    python scripts/variant_probe.py --run [--eighth]                                                            (under gpurun)
+    python scripts/variant_probe.py --build name:-DIDK_REG_STACK=2 name2:-DIDK_TRI_STRIDE=3   (build machine)
+    python scripts/variant_probe.py --run [--eighth]                                             (GPU machine)
 """
 import hashlib
 import json

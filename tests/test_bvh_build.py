@@ -1,11 +1,9 @@
 """Host-side BLAS builder (mirror of SRC/Bvh/BLAS.cs + PreSplitting.cs): structural invariants of the
 BLAS.cs:16-22 doc comment, and BVH traversal == brute force over all triangles (config 1 of BASELINE.json)."""
 import numpy as np
-import pytest
 
 import oracle_lib as ol
 from idkengine_b200 import scenes, host
-from idkengine_b200 import gpu_types as gt
 
 
 def check_invariants(scene):
@@ -138,65 +136,6 @@ def test_build_deterministic_and_threads_agree():
     s2, _ = scenes.atrium(40000, threads=4)
     assert np.array_equal(s1.blas_nodes, s2.blas_nodes)
     assert np.array_equal(s1.blas_triangles, s2.blas_triangles)
-
-
-@pytest.mark.skipif(not __import__("os").path.exists(scenes.REFERENCE_SPONZA), reason="reference assets not present")
-def test_real_sponza_builds_like_the_readme_says():
-    """Readme.md:515-522,820: Sponza 262,267 triangles; presplit 0.3 adds ~45k fragments -> ~41k after dedup."""
-    scene, cam = scenes.sponza_reference()
-    info = scene.build_info[0]
-    assert info["source_triangles"] == 262267
-    added_frag = info["fragments"] - info["source_triangles"]
-    added_tris = info["triangles"] - info["source_triangles"]
-    assert 30000 < added_frag < 60000 and 25000 < added_tris <= added_frag
-    assert 10 <= info["required_stack_size"] <= 30
-    frame = scenes.camera_frame(cam, 96, 54)
-    rays = ol.primary_rays(frame, 96, 54)
-    _compare_to_brute_force(scene, rays)
-
-
-@pytest.mark.skipif(not __import__("os").path.exists(scenes.REFERENCE_SPONZA), reason="reference assets not present")
-def test_readme_known_answers_on_real_sponza():
-    """The only reference-published numbers for this path: Readme.md:812-824, Sponza (262k), `TRAVERSAL_COST=1.0`,
-    `TriangleCost=1.1`, max 8 primitives per leaf, OptimizeStackSize disabled.
-
-        SplitFactor          0.0      0.3               1.0
-        New Triangles        0        45124 => 41150    188554 => 166664
-        SAH                  76.7     73.2              78.85
-        Stack Size           26       24                24
-
-    Asserted EXACTLY where the builder reproduces the README (fragment count at 0.3, stack sizes at 0.0 / 0.3, SAH at 0.0
-    to the README's precision) and pinned to this builder's own exact values elsewhere, with the README delta stated.
-    The README table was produced on commit e7ff348, not on the snapshot under /root/reference, so small deltas cannot
-    be attributed; ruled out here: the rounding of cbrtf (a correctly rounded cbrt gives the same counts) and the
-    summation order of totalPriority (serial, as PreSplitting.cs:33-37)."""
-    g, pos, nrm, uv, idx, tri_mesh, mesh_mat = scenes.load_gltf_geometry(scenes.REFERENCE_SPONZA)
-    P = np.concatenate(pos).astype(np.float32)
-    I = np.concatenate(idx).astype(np.uint32).reshape(-1, 3)
-    positions = np.zeros(len(P), gt.PackedVec3)
-    positions["x"], positions["y"], positions["z"] = P[:, 0], P[:, 1], P[:, 2]
-    tris = np.zeros(len(I), gt.GpuBlasTriangle)
-    tris["X"], tris["Y"], tris["Z"], tris["MeshId"] = I[:, 0], I[:, 1], I[:, 2], np.concatenate(tri_mesh)
-    assert len(I) == 262267
-    got = {}
-    for sf in (0.0, 0.3, 1.0):
-        st = host.default_build_settings()
-        st.MaxLeafTriangleCount = 8
-        st.StackOptThreshold = 1 << 30          # OptimizeStackSize disabled
-        st.SplitFactor = sf
-        b = host.build_blas(positions, tris, presplit=sf > 0, threads=4, settings=st)
-        got[sf] = (b["fragment_count"] - len(I), len(b["triangles"]) - len(I), b["sah"], b["required_stack_size"])
-    # README-exact
-    assert got[0.0][0] == 0 and got[0.0][1] == 0
-    assert got[0.3][0] == 45124                                   # "45124 =>"
-    assert got[0.0][3] == 26 and got[0.3][3] == 24                # Stack Size
-    assert round(got[0.0][2], 1) == 76.7                          # SAH 76.7
-    assert abs(got[0.3][2] - 73.2) < 0.1                          # SAH 73.2 (this builder: 73.145)
-    # this builder's exact values where the README differs in the last digits (README: 41150; 188554 => 166664; 78.85; 24)
-    assert got[0.3][1] == 41089
-    assert got[1.0][:2] == (188552, 166867) and got[1.0][3] == 25
-    assert abs(got[0.0][2] - 76.657) < 2e-3 and abs(got[0.3][2] - 73.145) < 2e-3 and abs(got[1.0][2] - 79.330) < 2e-3
-    assert abs(got[1.0][0] - 188554) <= 2 and abs(got[1.0][1] - 166664) / 166664 < 2e-3 and abs(got[0.3][1] - 41150) / 41150 < 2e-3
 
 
 def test_tlas_ploc_structure_and_equivalence(multi_blas):

@@ -449,8 +449,8 @@ def test_resize_and_snapshot_restore(cornell):
 
 
 def test_multi_gpu_peer_gather():
-    """Fused FinalDraw + NVLink peer-memory gather vs NCCL all-gather vs per-tile oracle (needs >= 2 GPUs; the single-GPU
-    driver box skips it, scripts/gpu_multi.sh runs the same script under gpurun --gpus N)."""
+    """Fused FinalDraw + NVLink peer-memory gather vs NCCL all-gather vs per-tile oracle (needs >= 2 GPUs; skipped
+    on a single-GPU machine)."""
     import os
     import subprocess
     import sys
