@@ -211,7 +211,7 @@ def load(path=None):
     global _lib
     if _lib is not None and path is None:
         return _lib
-    path = path or os.environ.get("IDKPT_LIB") or _build.LIBIDKPT     # IDKPT_LIB: an experiment build (scripts/variant_probe.py)
+    path = path or _build.LIBIDKPT
     if not os.path.exists(path):
         raise RuntimeError(f"{path} is missing: build it with `python -m idkengine_b200.build` "
                            "(libidkpt has no CPU fallback)")

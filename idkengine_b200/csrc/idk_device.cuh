@@ -282,27 +282,6 @@ __device__ __forceinline__ bool ray_sphere(f3 o, f3 d, f3 position, float radius
 
 __device__ __forceinline__ float4 ldg4(const float4* p) { return __ldg(p); }
 
-// ---- experiment switches (defaults = the measured best; scripts/variant_probe.py builds and times the alternatives)
-#ifndef IDK_TRI_STRIDE
-#define IDK_TRI_STRIDE 4     // float4s per device-private triangle record: 3 = packed 48 B, 4 = 64 B (never straddles a 128-B line)
-#endif
-#ifndef IDK_REG_STACK
-#define IDK_REG_STACK 0      // k_traverse2: top N entries of the traversal stack live in registers (0 = all in shared memory)
-#endif
-
-#ifndef IDK_STAGED_FETCH
-#define IDK_STAGED_FETCH 0   // k_traverse2: rays are prefetched into shared memory one batch ahead (cp.async) instead of fetched in the SETUP round
-#endif
-#ifndef IDK_FAST_VOTE
-#define IDK_FAST_VOTE 0      // k_traverse2: one ballot instead of four when (nearly) every lane is in the BOX phase
-#endif
-#ifndef IDK_BOX_LOOP
-#define IDK_BOX_LOOP 0       // k_traverse2: stay in the BOX phase with one ballot per round while >= 33 - min(thresholds) lanes are in it
-#endif
-#ifndef IDK_LEAF_LOOP
-#define IDK_LEAF_LOOP 0      // k_traverse2: a LEAF round tests a lane's whole pending range instead of one triangle
-#endif
-
 // One GpuBlasNode sibling pair (64 bytes, children are adjacent: BLAS.cs:16-22) / two adjacent GpuTlasNodes.
 struct NodePair { float4 lA, lB, rA, rB; };
 
@@ -313,8 +292,8 @@ __device__ __forceinline__ NodePair ldg_pair(const float4* np) {
     return r;
 }
 
-// Device-private triangle record i: (p0.xyz,e1.x) (e1.yz,e2.xy) (e2.z,n.xyz) [pad]
+// Device-private triangle record i, 64 B so that it never straddles a 128-B line: (p0.xyz,e1.x) (e1.yz,e2.xy) (e2.z,n.xyz) [pad]
 __device__ __forceinline__ void ldg_tri(const float4* triRec, size_t i, float4& a, float4& b, float4& c) {
-    const float4* tr = triRec + IDK_TRI_STRIDE * i;
+    const float4* tr = triRec + 4 * i;
     a = ldg4(tr); b = ldg4(tr + 1); c = ldg4(tr + 2);
 }

@@ -112,9 +112,9 @@ __global__ void __launch_bounds__(256) k_refit_climb(RefitArgs a) {
         lo = mk3(fminf(fminf(fminf(lo.x, p0.x), p1.x), p2.x), fminf(fminf(fminf(lo.y, p0.y), p1.y), p2.y), fminf(fminf(fminf(lo.z, p0.z), p1.z), p2.z));
         hi = mk3(fmaxf(fmaxf(fmaxf(hi.x, p0.x), p1.x), p2.x), fmaxf(fmaxf(fmaxf(hi.y, p0.y), p1.y), p2.y), fmaxf(fmaxf(fmaxf(hi.z, p0.z), p1.z), p2.z));
         const f3 e1 = p1 - p0, e2 = p2 - p0, n = cross3(e1, e2);
-        a.triRec[IDK_TRI_STRIDE * (size_t)k + 0] = make_float4(p0.x, p0.y, p0.z, e1.x);
-        a.triRec[IDK_TRI_STRIDE * (size_t)k + 1] = make_float4(e1.y, e1.z, e2.x, e2.y);
-        a.triRec[IDK_TRI_STRIDE * (size_t)k + 2] = make_float4(e2.z, n.x, n.y, n.z);
+        a.triRec[4 * (size_t)k + 0] = make_float4(p0.x, p0.y, p0.z, e1.x);
+        a.triRec[4 * (size_t)k + 1] = make_float4(e1.y, e1.z, e2.x, e2.y);
+        a.triRec[4 * (size_t)k + 2] = make_float4(e2.z, n.x, n.y, n.z);
     }
     a.nodes[2 * (size_t)i] = make_float4(lo.x, lo.y, lo.z, nA.w);
     a.nodes[2 * (size_t)i + 1] = make_float4(hi.x, hi.y, hi.z, nB.w);

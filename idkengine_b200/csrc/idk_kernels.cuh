@@ -1,7 +1,7 @@
 // Wavefront path-tracing kernels for sm_90a (H100). See DESIGN.md for the HBM layout and the
 // algorithmic-byte accounting of each kernel.
 //
-//   k_prepare_triangles/vertices/surfaces  scene upload: 48-byte triangle records, decoded vertex frames, per-mesh surfaces
+//   k_prepare_triangles/vertices/surfaces  scene upload: 64-byte triangle records, decoded vertex frames, per-mesh surfaces
 //   k_init_sample        per sample: zero alive counts and work tickets
 //   k_raygen             FirstHit/compute.glsl:44-81   ray generation (camera, jitter, thin lens)
 //   k_traverse           BVHIntersect.glsl:27-105,183-291  closest hit, one ray per lane (primary rays, TLAS walk)
@@ -16,13 +16,11 @@
 
 #define IDK_BLOCK 256
 #define IDK_WARPS (IDK_BLOCK / 32)
-#ifndef IDK_T2_BLOCK
-#define IDK_T2_BLOCK 256     // threads per block of k_traverse2 (smaller blocks hand their registers / shared memory back sooner in the tail of a launch)
-#endif
+#define IDK_T2_BLOCK 256     // threads per block of k_traverse2
 
 struct DeviceScene {
     const float4* nodes;          // 2 x float4 per GpuBlasNode
-    const float4* triRec;         // IDK_TRI_STRIDE x float4 per triangle: (p0.xyz,e1.x) (e1.yz,e2.xy) (e2.z,n.xyz) [pad]
+    const float4* triRec;         // 4 x float4 per triangle: (p0.xyz,e1.x) (e1.yz,e2.xy) (e2.z,n.xyz) [pad]
     const int4* blasTris;         // GpuBlasTriangle
     const GpuBlasDesc* descs;
     const GpuBlasInstance* instances;
@@ -39,7 +37,6 @@ struct DeviceScene {
     int skyFaceSize;
     const float4* tlasNodes;      // 2 x float4 per GpuTlasNode, root at 0 (USE_TLAS path, BVHIntersect.glsl:205-272)
     int useTlas;
-    int treeletNodes;             // node indices < treeletNodes (BFS-first re-layout, single-BLAS scenes) are staged in shared memory
     const float4* vtxFrame;       // device-private, 2 x float4 per vertex: decoded (normal.xyz, tangent.x) (tangent.yz, 0, 0)
     const float4* surfRec;        // device-private, 5 x float4 per mesh: GetSurface + SurfaceApplyModificatons, see k_prepare_surfaces
     const struct TexRec* textures; // material texture table (handle k > 0 = textures[k - 1]; 0 = the reference's 1x1 white fallback)
@@ -65,11 +62,7 @@ static_assert(sizeof(PathState) == 64, "PathState must be 64 bytes");
 
 struct HitRec { float bx, by, t; uint32_t tri; };   // 16 bytes, + uint32 transform id in a second array
 
-struct TraceCounters { unsigned long long steps, tris, instances, hits; unsigned int maxSteps[64];
-                       unsigned long long phaseRounds[4], phaseLanes[4], boxIdle[4]; };   // IDK_PHASE_STATS builds: warp rounds / active lanes per phase (SETUP, BOX, LEAF, TLAS)
-#ifndef IDK_PHASE_STATS
-#define IDK_PHASE_STATS 0
-#endif
+struct TraceCounters { unsigned long long steps, tris, instances, hits; unsigned int maxSteps[64]; };
 
 // ------------------------------------------------------------------------------------------------
 // Per sample: zero the alive counts and the work tickets, counts[0] = number of primary rays.
@@ -88,12 +81,10 @@ __global__ void k_prepare_triangles(const int4* __restrict__ tris, const float* 
     f3 p2 = mk3(positions[3 * t.z], positions[3 * t.z + 1], positions[3 * t.z + 2]);
     f3 e1 = p1 - p0, e2 = p2 - p0;
     f3 n = cross3(e1, e2);
-    triRec[IDK_TRI_STRIDE * (size_t)i + 0] = make_float4(p0.x, p0.y, p0.z, e1.x);
-    triRec[IDK_TRI_STRIDE * (size_t)i + 1] = make_float4(e1.y, e1.z, e2.x, e2.y);
-    triRec[IDK_TRI_STRIDE * (size_t)i + 2] = make_float4(e2.z, n.x, n.y, n.z);
-#if IDK_TRI_STRIDE == 4
-    triRec[IDK_TRI_STRIDE * (size_t)i + 3] = make_float4(0.0f, 0.0f, 0.0f, 0.0f);
-#endif
+    triRec[4 * (size_t)i + 0] = make_float4(p0.x, p0.y, p0.z, e1.x);
+    triRec[4 * (size_t)i + 1] = make_float4(e1.y, e1.z, e2.x, e2.y);
+    triRec[4 * (size_t)i + 2] = make_float4(e2.z, n.x, n.y, n.z);
+    triRec[4 * (size_t)i + 3] = make_float4(0.0f, 0.0f, 0.0f, 0.0f);
 }
 
 // Scene upload: DecompressSR11G11B10 of every vertex normal / tangent (Compression.glsl:11-32), hoisted out of the
@@ -355,69 +346,16 @@ __global__ void __launch_bounds__(IDK_BLOCK) k_traverse(TraverseArgs a) {
 //   LEAF   lanes with a pending range test ONE triangle.
 // Each iteration the warp votes (ballots) which phase to run: a phase runs when enough lanes wait for it or nothing
 // else can run. Traversal stacks live in shared memory, one column per thread (the reference's layout).
-struct TraverseTuning { int setupThreshold; int leafThreshold; int packRays; int setupThresholdStaged; int packCta; };   // packRays: 32 rays per warp whatever the count (throughput mode: several samples share the SMs)
+struct TraverseTuning { int setupThreshold; int leafThreshold; int packRays; };   // packRays: 32 rays per warp whatever the count (throughput mode: several samples share the SMs)
+#define IDK_T2_SETUP_THRESHOLD 12   // SETUP runs when this many lanes wait in it (capped at 3/8 of the rays a warp carries)
+#define IDK_T2_LEAF_THRESHOLD 4     // LEAF runs when this many lanes wait in it (capped at 1/8 of the rays a warp carries)
 
-// TMA (bulk async copy) staging of the hot top of the BVH into shared memory: one elected thread arms an mbarrier with
-// the byte count and issues cp.async.bulk global -> shared; every thread then waits on the barrier phase.
-__device__ __forceinline__ void tma_stage_treelet(void* smemDst, const void* gmemSrc, uint32_t bytes, uint64_t* mbar) {
-    const uint32_t bar = (uint32_t)__cvta_generic_to_shared(mbar);
-    if (threadIdx.x == 0) {
-        asm volatile("mbarrier.init.shared::cta.b64 [%0], 1;" ::"r"(bar));
-        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-    }
-    __syncthreads();
-    if (threadIdx.x == 0) {
-        asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(bar), "r"(bytes) : "memory");
-        const uint32_t dst = (uint32_t)__cvta_generic_to_shared(smemDst);
-        const uint32_t chunk = 16384u;
-        for (uint32_t off = 0; off < bytes; off += chunk) {
-            const uint32_t n = min(chunk, bytes - off);
-            asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
-                         ::"r"(dst + off), "l"((const char*)gmemSrc + off), "r"(n), "r"(bar) : "memory");
-        }
-    }
-    uint32_t done = 0;
-    while (!done) {
-        asm volatile("{\n\t.reg .pred p;\n\tmbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n\tselp.u32 %0, 1, 0, p;\n\t}"
-                     : "=r"(done) : "r"(bar), "r"(0u) : "memory");
-    }
-}
-
-// Staged ray fetch (IDK_STAGED_FETCH): in the bulk regime every warp owns a double-buffered shared-memory staging area of
-// 2 x 32 ray records. A batch = one ticket of 32 consecutive alive-list slots; its alive-list indices are loaded coalesced
-// and the 32-byte head of every ray's PathState is copied global -> shared with cp.async (LDGSTS) one batch AHEAD of its use,
-// and the ticket of the batch after that is already in a register. A SETUP round then hands rays out of shared memory
-// instead of walking the dependent chain atomicAdd -> alive[] -> PathState (three L2/HBM round trips) for a dozen lanes at
-// a time; that makes SETUP rounds cheap enough to run them for few waiting lanes (lower setupThreshold, fewer idle lanes
-// in the BOX rounds). Which lane traces which ray changes; what is traced does not.
-#ifndef IDK_STAGE_CG
-#define IDK_STAGE_CG 0
-#endif
-#ifndef IDK_STAGE_GSS
-#define IDK_STAGE_GSS 1
-#endif
-#define IDK_STAGE_BYTES ((IDK_T2_BLOCK / 32) * 2 * 32 * 32)
-__device__ __forceinline__ void cp_async16(void* smemDst, const void* gmemSrc) {
-#if IDK_STAGE_CG
-    asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"((uint32_t)__cvta_generic_to_shared(smemDst)), "l"(gmemSrc) : "memory");
-#else
-    asm volatile("cp.async.ca.shared.global [%0], [%1], 16;" ::"r"((uint32_t)__cvta_generic_to_shared(smemDst)), "l"(gmemSrc) : "memory");
-#endif
-}
-__device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commit_group;" ::: "memory"); }
-template <int N> __device__ __forceinline__ void cp_async_wait() { asm volatile("cp.async.wait_group %0;" ::"n"(N) : "memory"); }
-
-template <bool STATS, bool TREELET, bool TLAS>
+template <bool STATS, bool TLAS>
 __global__ void __launch_bounds__(IDK_T2_BLOCK) k_traverse2(TraverseArgs a, TraverseTuning tune) {
-    // dynamic shared memory: [treelet: treeletNodes x 32 B][traversal stacks: stackSize x IDK_T2_BLOCK x 4 B][ray staging: IDK_STAGE_BYTES]
+    // dynamic shared memory: traversal stacks, stackSize x IDK_T2_BLOCK x 4 B
     extern __shared__ __align__(128) unsigned char s_dyn[];
-    __shared__ __align__(8) uint64_t s_mbar;
     const DeviceScene& sc = a.sc;
-    const uint32_t treeletNodes = TREELET ? (uint32_t)sc.treeletNodes : 0u;
-    const float4* s_treelet = reinterpret_cast<const float4*>(s_dyn);
-    uint32_t* s_stack = reinterpret_cast<uint32_t*>(s_dyn + (size_t)treeletNodes * 32);
-    if (TREELET && treeletNodes) tma_stage_treelet(s_dyn, sc.nodes, treeletNodes * 32u, &s_mbar);
-    uint32_t* stack = s_stack + threadIdx.x;
+    uint32_t* stack = reinterpret_cast<uint32_t*>(s_dyn) + threadIdx.x;
     const uint32_t lane = threadIdx.x & 31;
     const uint32_t laneLt = (1u << lane) - 1u;
     const uint32_t count = *a.count;
@@ -425,22 +363,10 @@ __global__ void __launch_bounds__(IDK_T2_BLOCK) k_traverse2(TraverseArgs a, Trav
     // Latency regime (few rays, e.g. late bounces or a 1/8 screen tile): spread the rays over ALL resident warps instead
     // of packing 32 per warp -- a warp that carries few rays has short BOX/LEAF/SETUP rounds and little L1 wavefront
     // serialisation, so the longest ray (which bounds the launch) finishes sooner. quota = rays per warp, 32 in the bulk.
-    // Pipelined launches (packRays): a launch with few rays needs few CTAs. Only the first ceil(count / (block * packRays)) CTAs take
-    // part, the others retire at once and leave their registers / shared memory to the other samples' kernels (a CTA that keeps one
-    // busy warp holds a quarter of an SM). packCta = rays per thread a participating CTA is expected to take (1 = tightest packing, 0 = every CTA takes part).
-    if (tune.packCta > 0 && (uint64_t)blockIdx.x * (IDK_T2_BLOCK * (uint32_t)tune.packCta) >= (uint64_t)count && blockIdx.x > 0) return;
     const uint32_t totalWarps = gridDim.x * (IDK_T2_BLOCK / 32);
     const uint32_t quota = tune.packRays ? 32u : min(32u, max(1u, (count + totalWarps - 1) / totalWarps));
-#if IDK_STAGED_FETCH
-    const bool bulk = quota == 32u;     // staged fetch in the throughput regime only; the latency regime keeps one ticket per SETUP round
-    const int setupThreshold = max(1, min(bulk ? tune.setupThresholdStaged : tune.setupThreshold, (int)(quota * 3 / 8)));
-#else
     const int setupThreshold = max(1, min(tune.setupThreshold, (int)(quota * 3 / 8)));
-#endif
     const int leafThreshold = max(1, min(tune.leafThreshold, (int)(quota / 8)));
-#if IDK_FAST_VOTE
-    const int fastBox = 33 - min(setupThreshold, leafThreshold);   // > 32 (never) when a threshold is 1
-#endif
 
     int state = ST_SETUP;
     bool haveRay = false, finished = false, blasHit = false;
@@ -453,106 +379,18 @@ __global__ void __launch_bounds__(IDK_T2_BLOCK) k_traverse2(TraverseArgs a, Trav
     uint32_t triOffset = 0, top = 2, sp = 0, first = 0, end = 0;
     uint32_t S = 0, T = 0, I = 0, H = 0, rayS0 = 0;
     float cost = 0.0f;
-    // Traversal stack: the top IDK_REG_STACK entries live in registers (rs[0] = top, `rc` of them valid), everything below
-    // them in this thread's shared-memory column (`sp` entries). Registers spill one entry when full and refill one when
-    // empty, so a ray that oscillates around one depth never touches shared memory and a pop's next node index is
-    // available without a load in the dependent chain. The sequence of popped values is that of the reference's array stack.
-#if IDK_REG_STACK > 0
-    uint32_t rs[IDK_REG_STACK];
-#pragma unroll
-    for (int k = 0; k < IDK_REG_STACK; k++) rs[k] = 0;
-    uint32_t rc = 0;
-#endif
     // TLAS walk (BVHIntersect.glsl:205-272): per-lane stack of IDK_TLAS_STACK_SIZE entries (local memory: touched once per
     // TLAS node, i.e. rarely next to the BLAS steps), `ttop` = the TLAS node to visit next.
     uint32_t tstack[TLAS ? IDK_TLAS_STACK_SIZE : 1];
     uint32_t tsp = 0, ttop = 0;
     f3 winv = wd;
 
-#if IDK_REG_STACK > 0
-#define IDK_STACK_RESET() do { sp = 0; rc = 0; } while (0)
-#define IDK_STACK_EMPTY() (rc == 0u && sp == 0u)
-#define IDK_STACK_PUSH(x) do {                                                         \
-        if (rc == IDK_REG_STACK) { stack[(sp++) * IDK_T2_BLOCK] = rs[IDK_REG_STACK - 1]; rc = IDK_REG_STACK - 1; } \
-        _Pragma("unroll") for (int k_ = IDK_REG_STACK - 1; k_ > 0; k_--) rs[k_] = rs[k_ - 1]; \
-        rs[0] = (x); rc++;                                                             \
-    } while (0)
-#define IDK_STACK_POP(dst) do {                                                        \
-        if (rc == 0u) { rs[0] = stack[(--sp) * IDK_T2_BLOCK]; rc = 1; }                   \
-        (dst) = rs[0];                                                                 \
-        _Pragma("unroll") for (int k_ = 0; k_ < IDK_REG_STACK - 1; k_++) rs[k_] = rs[k_ + 1]; \
-        rc--;                                                                          \
-    } while (0)
-#else
-#define IDK_STACK_RESET() do { sp = 0; } while (0)
-#define IDK_STACK_EMPTY() (sp == 0u)
-#define IDK_STACK_PUSH(x) do { stack[(sp++) * IDK_T2_BLOCK] = (x); } while (0)
-#define IDK_STACK_POP(dst) do { (dst) = stack[(--sp) * IDK_T2_BLOCK]; } while (0)
-#endif
-    // a BLAS has been exhausted: commit its hit, then the instance loop advances (SETUP) or the TLAS walk pops / ends
-#define IDK_BLAS_DONE() do {                                                           \
-        if (blasHit) hitXf = curXf;                                                    \
-        if (TLAS) {                                                                    \
-            if (tsp == 0u) { inst = 0xFFFFFFFFu; state = ST_SETUP; }                   \
-            else { ttop = tstack[--tsp]; state = ST_TLAS; }                            \
-        } else { inst++; state = ST_SETUP; }                                           \
-    } while (0)
-
-#if IDK_STAGED_FETCH
-    float4* const stage = reinterpret_cast<float4*>(s_dyn + (size_t)treeletNodes * 32 + (size_t)sc.stackSize * IDK_T2_BLOCK * 4) + (size_t)(threadIdx.x >> 5) * (2 * 32 * 2);
-    uint32_t curBase = 0, curCount = 0, curNext = 0, nxtBase = 0, pendBase = 0, bufCur = 0, nxtCnt = 32, pendCnt = 32, lastBase = 0;
-    // Guided self-scheduling: a ticket covers 32 slots while plenty of rays remain and shrinks to 4 as the list drains (judged
-    // from the newest ticket this warp has seen), so that the batches a warp holds in advance do not unbalance the tail.
-#define IDK_GRAB(dst, cnt) do {                                                          \
-        const uint32_t rem_ = count > lastBase ? count - lastBase : 0u;                  \
-        (cnt) = IDK_STAGE_GSS ? min(32u, max(4u, rem_ / (2u * totalWarps))) : 32u;       \
-        uint32_t b_ = 0; if (lane == 0) b_ = atomicAdd(a.ticket, (cnt));                 \
-        (dst) = __shfl_sync(0xffffffffu, b_, 0); lastBase = (dst);                       \
-    } while (0)
-#define IDK_ISSUE(buf, base, cnt) do {                                                   \
-        const uint32_t g_ = (base) + lane;                                               \
-        if (lane < (cnt) && g_ < count) {                                                \
-            const uint32_t src_ = a.perm ? a.perm[g_] : g_;                              \
-            const float4* sp_ = reinterpret_cast<const float4*>(a.state + src_);         \
-            float4* d_ = stage + ((buf) * 32 + lane) * 2;                                \
-            cp_async16(d_, sp_); cp_async16(d_ + 1, sp_ + 1);                            \
-        }                                                                                \
-        cp_async_commit();                                                               \
-    } while (0)
-    if (bulk) {
-        uint32_t b1, c0;
-        IDK_GRAB(curBase, c0); IDK_ISSUE(0u, curBase, c0);
-        IDK_GRAB(b1, nxtCnt); IDK_ISSUE(1u, b1, nxtCnt);
-        IDK_GRAB(pendBase, pendCnt);
-        nxtBase = b1;
-        curCount = curBase < count ? min(c0, count - curBase) : 0u;
-        cp_async_wait<1>();
-        __syncwarp();
-    }
-#endif
-#if IDK_PHASE_STATS
-    uint32_t pr0 = 0, pr1 = 0, pr2 = 0, pl0 = 0, pl1 = 0, pl2 = 0, pw0 = 0, pw2 = 0, pwx = 0;   // pw*: lanes idle during BOX rounds (waiting for SETUP / LEAF, exited)
-#endif
     for (;;) {
         const uint32_t mBox = __ballot_sync(0xffffffffu, state == ST_BOX);
-#if IDK_FAST_VOTE
-        // Fast path: with this many lanes in BOX neither the SETUP nor the LEAF (nor the TLAS) threshold can be met by the
-        // remaining lanes, so the full vote would pick BOX anyway -- skip its three other ballots (same schedule, fewer instructions).
-        const bool boxOnly = __popc(mBox) >= fastBox;
-        const uint32_t mSetup = boxOnly ? 0u : __ballot_sync(0xffffffffu, state == ST_SETUP);
-        const uint32_t mLeaf = boxOnly ? 0u : __ballot_sync(0xffffffffu, state == ST_LEAF);
-        const uint32_t mTlas = (TLAS && !boxOnly) ? __ballot_sync(0xffffffffu, state == ST_TLAS) : 0u;
-#else
         const uint32_t mSetup = __ballot_sync(0xffffffffu, state == ST_SETUP);
         const uint32_t mLeaf = __ballot_sync(0xffffffffu, state == ST_LEAF);
         const uint32_t mTlas = TLAS ? __ballot_sync(0xffffffffu, state == ST_TLAS) : 0u;
-#endif
         if ((mSetup | mBox | mLeaf | mTlas) == 0u) break;
-#if IDK_PHASE_STATS
-        if (mSetup && (__popc(mSetup) >= setupThreshold || (mBox | mLeaf | mTlas) == 0u)) { pr0++; pl0 += __popc(mSetup); }
-        else if (mLeaf && (__popc(mLeaf) >= leafThreshold || mBox == 0u)) { pr2++; pl2 += __popc(mLeaf); }
-        else { pr1++; pl1 += __popc(mBox); pw0 += __popc(mSetup); pw2 += __popc(mLeaf); pwx += 32 - __popc(mSetup | mBox | mLeaf | mTlas); }
-#endif
 
         if (mSetup && (__popc(mSetup) >= setupThreshold || (mBox | mLeaf | mTlas) == 0u)) {
             // ------------------------------------------------------------------ SETUP
@@ -571,55 +409,19 @@ __global__ void __launch_bounds__(IDK_T2_BLOCK) k_traverse2(TraverseArgs a, Trav
             if (mine && !haveRay && lane >= quota) state = ST_EXIT;
             const uint32_t fm = __ballot_sync(0xffffffffu, needFetch);
             if (fm) {
-                bool got = false, exhausted = true;     // exhausted: a lane that got no ray will never get one (end of the alive list)
+                const int leader = __ffs(fm) - 1;
+                uint32_t base = 0;
+                if ((int)lane == leader) base = atomicAdd(a.ticket, (uint32_t)__popc(fm));
+                base = __shfl_sync(0xffffffffu, base, leader);
+                bool got = false;
                 float4 s0 = make_float4(0.0f, 0.0f, 0.0f, 0.0f), s1 = s0;
-#if IDK_STAGED_FETCH
-                if (bulk) {
-                    const uint32_t need = (uint32_t)__popc(fm), rank = (uint32_t)__popc(fm & laneLt);
-                    if (needFetch && curNext + rank < curCount) {
-                        const float4* r_ = stage + (bufCur * 32 + curNext + rank) * 2;
-                        s0 = r_[0]; s1 = r_[1];
-                        gid = curBase + curNext + rank;
+                if (needFetch) {
+                    gid = base + __popc(fm & laneLt);
+                    if (gid < count) {
+                        const uint32_t src = a.perm ? a.perm[gid] : gid;
+                        const float4* spp = reinterpret_cast<const float4*>(a.state + src);
+                        s0 = spp[0]; s1 = spp[1];
                         got = true;
-                    }
-                    if (curNext + need >= curCount) {
-                        // current batch used up: the prefetched one becomes current, the vacated buffer receives the batch whose
-                        // ticket is already here, and the ticket after that is requested (its value is needed one swap later)
-                        const uint32_t served = curCount - curNext;
-                        cp_async_wait<0>();
-                        __syncwarp();
-                        bufCur ^= 1u;
-                        curBase = nxtBase;
-                        curCount = curBase < count ? min(nxtCnt, count - curBase) : 0u;
-                        IDK_ISSUE(bufCur ^ 1u, pendBase, pendCnt);
-                        nxtBase = pendBase; nxtCnt = pendCnt;
-                        IDK_GRAB(pendBase, pendCnt);
-                        if (needFetch && !got && rank - served < curCount) {
-                            const float4* r_ = stage + (bufCur * 32 + (rank - served)) * 2;
-                            s0 = r_[0]; s1 = r_[1];
-                            gid = curBase + (rank - served);
-                            got = true;
-                        }
-                        curNext = min(curCount, need - served);
-                    } else {
-                        curNext += need;
-                    }
-                    exhausted = curBase >= count;    // otherwise an unserved lane (small guided batches) asks again next SETUP round
-                } else
-#endif
-                {
-                    const int leader = __ffs(fm) - 1;
-                    uint32_t base = 0;
-                    if ((int)lane == leader) base = atomicAdd(a.ticket, (uint32_t)__popc(fm));
-                    base = __shfl_sync(0xffffffffu, base, leader);
-                    if (needFetch) {
-                        gid = base + __popc(fm & laneLt);
-                        if (gid < count) {
-                            const uint32_t src = a.perm ? a.perm[gid] : gid;
-                            const float4* spp = reinterpret_cast<const float4*>(a.state + src);
-                            s0 = spp[0]; s1 = spp[1];
-                            got = true;
-                        }
                     }
                 }
                 if (needFetch) {
@@ -648,8 +450,8 @@ __global__ void __launch_bounds__(IDK_T2_BLOCK) k_traverse2(TraverseArgs a, Trav
                             ttop = 0; tsp = 0;
                             state = ST_TLAS;
                         }
-                    } else if (exhausted) {
-                        state = ST_EXIT;
+                    } else {
+                        state = ST_EXIT;     // end of the alive list: this lane will never get a ray
                     }
                 }
             }
@@ -669,7 +471,7 @@ __global__ void __launch_bounds__(IDK_T2_BLOCK) k_traverse2(TraverseArgs a, Trav
                 float tRoot;
                 if (ray_box(lo, inv, ra, rb, tRoot) && tRoot < hit.t) {
                     state = ST_BOX;
-                    top = 2; IDK_STACK_RESET(); blasHit = false; finished = false;
+                    top = 2; sp = 0; blasHit = false; finished = false;
                 } else {
                     inst++;
                 }
@@ -694,7 +496,7 @@ __global__ void __launch_bounds__(IDK_T2_BLOCK) k_traverse2(TraverseArgs a, Trav
                     curXf = bi.MeshTransformId;
                     if (STATS) I++;
                     state = ST_BOX;
-                    top = 2; IDK_STACK_RESET(); blasHit = false; finished = false;
+                    top = 2; sp = 0; blasHit = false; finished = false;
                 } else {
                     const NodePair pr = ldg_pair(sc.tlasNodes + 2 * (size_t)id);
                     float tMinLeft, tMinRight;
@@ -719,9 +521,6 @@ __global__ void __launch_bounds__(IDK_T2_BLOCK) k_traverse2(TraverseArgs a, Trav
         } else if (mLeaf && (__popc(mLeaf) >= leafThreshold || mBox == 0u)) {
             // ------------------------------------------------------------------ LEAF (one triangle)
             if (state == ST_LEAF) {
-#if IDK_LEAF_LOOP
-                do {      // the lane's whole pending range in one round (leaves hold 1-2 triangles with the reference's build settings)
-#endif
                 float4 ta, tb, tc;
                 ldg_tri(sc.triRec, first, ta, tb, tc);
                 float bx, by, t;
@@ -730,32 +529,25 @@ __global__ void __launch_bounds__(IDK_T2_BLOCK) k_traverse2(TraverseArgs a, Trav
                     hit.tri = first; hit.bx = bx; hit.by = by; hit.t = t;
                 }
                 first++;
-#if IDK_LEAF_LOOP
-                } while (first != end);
-#endif
                 if (first == end) {
-                    if (finished) IDK_BLAS_DONE();
-                    else state = ST_BOX;
+                    if (finished) {
+                        // the BLAS is exhausted: commit its hit, then the instance loop advances (SETUP) or the TLAS walk pops / ends
+                        if (blasHit) hitXf = curXf;
+                        if (TLAS) {
+                            if (tsp == 0u) { inst = 0xFFFFFFFFu; state = ST_SETUP; }
+                            else { ttop = tstack[--tsp]; state = ST_TLAS; }
+                        } else { inst++; state = ST_SETUP; }
+                    } else {
+                        state = ST_BOX;
+                    }
                 }
             }
         } else {
             // ------------------------------------------------------------------ BOX (one sibling pair)
-#if IDK_BOX_LOOP
-            // While (nearly) every lane stays in BOX no other phase can reach its threshold, so the full four-ballot vote would pick
-            // BOX again: stay in this loop with one ballot per round instead (same schedule, fewer instructions).
-            const int boxStay = 33 - min(setupThreshold, leafThreshold);
-            do {
-#endif
             if (state == ST_BOX) {
                 if (STATS) { S++; cost += 1.0f; }
-                float4 lA, lB, rA, rB;
-                if (TREELET && top < treeletNodes) {       // hot top of the tree: shared memory (single-BLAS scenes, nodes == sc.nodes)
-                    const float4* np = s_treelet + 2 * (size_t)top;
-                    lA = np[0]; lB = np[1]; rA = np[2]; rB = np[3];
-                } else {
-                    const NodePair pr = ldg_pair(nodes + 2 * (size_t)top);
-                    lA = pr.lA; lB = pr.lB; rA = pr.rA; rB = pr.rB;
-                }
+                const NodePair pr = ldg_pair(nodes + 2 * (size_t)top);
+                const float4 lA = pr.lA, lB = pr.lB, rA = pr.rA, rB = pr.rB;
                 const int lChild = __float_as_int(lA.w), lCount = __float_as_int(lB.w);
                 const int rChild = __float_as_int(rA.w), rCount = __float_as_int(rB.w);
                 float tMinLeft, tMinRight;
@@ -776,44 +568,28 @@ __global__ void __launch_bounds__(IDK_T2_BLOCK) k_traverse2(TraverseArgs a, Trav
                     if (traverseLeft && traverseRight) {
                         const bool leftCloser = tMinLeft < tMinRight;
                         top = leftCloser ? (uint32_t)lChild : (uint32_t)rChild;
-                        IDK_STACK_PUSH(leftCloser ? (uint32_t)rChild : (uint32_t)lChild);
+                        stack[(sp++) * IDK_T2_BLOCK] = leftCloser ? (uint32_t)rChild : (uint32_t)lChild;
                     } else {
                         top = traverseLeft ? (uint32_t)lChild : (uint32_t)rChild;
                     }
-                } else if (IDK_STACK_EMPTY()) {
+                } else if (sp == 0u) {
                     finished = true;
                 } else {
-                    IDK_STACK_POP(top);
+                    top = stack[(--sp) * IDK_T2_BLOCK];
                 }
                 if (pending) {
                     state = ST_LEAF;
                 } else if (finished) {
-                    IDK_BLAS_DONE();
+                    // the BLAS is exhausted: same hand-over as at the end of a LEAF round
+                    if (blasHit) hitXf = curXf;
+                    if (TLAS) {
+                        if (tsp == 0u) { inst = 0xFFFFFFFFu; state = ST_SETUP; }
+                        else { ttop = tstack[--tsp]; state = ST_TLAS; }
+                    } else { inst++; state = ST_SETUP; }
                 }
             }
-#if IDK_BOX_LOOP
-            } while (__popc(__ballot_sync(0xffffffffu, state == ST_BOX)) >= boxStay);
-#endif
         }
     }
-#undef IDK_STACK_RESET
-#undef IDK_STACK_EMPTY
-#undef IDK_STACK_PUSH
-#undef IDK_STACK_POP
-#undef IDK_BLAS_DONE
-#if IDK_STAGED_FETCH
-#undef IDK_GRAB
-#undef IDK_ISSUE
-    cp_async_wait<0>();     // a prefetched batch beyond the end of the list may still be in flight
-#endif
-#if IDK_PHASE_STATS
-    if (lane == 0) {
-        atomicAdd(&a.counters->phaseRounds[0], (unsigned long long)pr0); atomicAdd(&a.counters->phaseLanes[0], (unsigned long long)pl0);
-        atomicAdd(&a.counters->phaseRounds[1], (unsigned long long)pr1); atomicAdd(&a.counters->phaseLanes[1], (unsigned long long)pl1);
-        atomicAdd(&a.counters->phaseRounds[2], (unsigned long long)pr2); atomicAdd(&a.counters->phaseLanes[2], (unsigned long long)pl2);
-        atomicAdd(&a.counters->boxIdle[0], (unsigned long long)pw0); atomicAdd(&a.counters->boxIdle[1], (unsigned long long)pw2); atomicAdd(&a.counters->boxIdle[2], (unsigned long long)pwx);
-    }
-#endif
     if (STATS) {
         for (int off = 16; off > 0; off >>= 1) {
             S += __shfl_down_sync(0xffffffffu, S, off);
@@ -1079,11 +855,8 @@ __device__ __forceinline__ uint32_t status_epoch(unsigned long long sv) { return
 // One thread per alive ray, no block-level cooperation: every warp runs at its own pace (the ordered compaction of
 // the reference's atomic alive list is a separate, uniform-cost pass over 4-byte entries: k_compact).
 // TEX = the scene has material textures (idkpt_set_scene); the untextured instantiation is the north-star path.
-#ifndef IDK_SHADE_MIN_BLOCKS
-#define IDK_SHADE_MIN_BLOCKS 3
-#endif
 template <bool TEX>
-__global__ void __launch_bounds__(IDK_BLOCK, IDK_SHADE_MIN_BLOCKS) k_shade(ShadeArgs a) {
+__global__ void __launch_bounds__(IDK_BLOCK, 3) k_shade(ShadeArgs a) {
     const uint32_t count = *a.count;
     const DeviceScene& sc = a.sc;
     const FrameParams& f = a.f;
@@ -1182,7 +955,7 @@ __global__ void __launch_bounds__(IDK_BLOCK, IDK_SHADE_MIN_BLOCKS) k_shade(Shade
                         const f3 B = normalize3(cross3(N, T));
                         const f3 tbnN = (T * s.Normal.x + B * s.Normal.y) + N * s.Normal.z;
                         s.Normal = normalize3(mix3(worldNormal, tbnN, normalMapStrength));
-                        const float4 tr = ldg4(sc.triRec + IDK_TRI_STRIDE * (size_t)hitTri + 2);
+                        const float4 tr = ldg4(sc.triRec + 4 * (size_t)hitTri + 2);
                         geometricNormal = normalize3(mk3(tr.y, tr.z, tr.w));   // GetTriangleNormal
                         geometricNormal = normalize3(xform_normal(r0, r1, r2, geometricNormal));
                     }

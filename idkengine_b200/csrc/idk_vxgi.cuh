@@ -304,73 +304,6 @@ __global__ void __launch_bounds__(256) k_vx_mipmap(VxGridDev g, int level) {
     }
 }
 
-// Tiled variant for the levels that halve exactly (source = 2 x destination on every axis, i.e. every big level of a
-// power-of-two-ish grid): a CTA produces an 8 x 8 x 4 block of destination texels from the (2*8+2) x (2*8+2) x (2*4+2) source
-// texels around it. The tile is fetched from HBM ONCE (coalesced rows), converted half -> float ONCE and kept in shared
-// memory as float4; the 7 trilinear taps then read shared memory. The arithmetic of every destination texel -- coordinates,
-// weights, lerp order, tap order, /7, RNE conversion -- is that of k_vx_mipmap, so the result is bit-identical; what changes
-// is that a source texel is read and converted once per tile instead of ~7 times per neighbourhood (the r01 kernel ran at
-// 21 % of the HBM rate, bound by the 56 global fetches + 224 half conversions per destination texel).
-#define IDKVX_MT_X 8
-#define IDKVX_MT_Y 8
-#define IDKVX_MT_Z 4
-#define IDKVX_MS_X (2 * IDKVX_MT_X + 2)
-#define IDKVX_MS_Y (2 * IDKVX_MT_Y + 2)
-#define IDKVX_MS_Z (2 * IDKVX_MT_Z + 2)
-#define IDKVX_MIP_TILE_SMEM (IDKVX_MS_X * IDKVX_MS_Y * IDKVX_MS_Z * 16)
-
-__device__ __forceinline__ float4 vx_tile_trilinear(const float4* tile, int bx, int by, int bz, int sx, int sy, int sz,
-                                                    float u, float v, float w, int ox, int oy, int oz) {
-    const float px = u * (float)sx - 0.5f, py = v * (float)sy - 0.5f, pz = w * (float)sz - 0.5f;
-    const float fx0 = floorf(px), fy0 = floorf(py), fz0 = floorf(pz);
-    const float fx = px - fx0, fy = py - fy0, fz = pz - fz0;
-    // tile entry (i, j, k) holds source texel (clamp(bx + i), clamp(by + j), clamp(bz + k)): indexing with the UNCLAMPED
-    // coordinate relative to the tile origin returns exactly what clamp-then-fetch returns in vx_trilinear
-    const int x0 = (int)fx0 + ox - bx, y0 = (int)fy0 + oy - by, z0 = (int)fz0 + oz - bz;
-#define T_(i, j, k) tile[((k) * IDKVX_MS_Y + (j)) * IDKVX_MS_X + (i)]
-    const float4 c00 = lerp4(T_(x0, y0, z0), T_(x0 + 1, y0, z0), fx);
-    const float4 c10 = lerp4(T_(x0, y0 + 1, z0), T_(x0 + 1, y0 + 1, z0), fx);
-    const float4 c01 = lerp4(T_(x0, y0, z0 + 1), T_(x0 + 1, y0, z0 + 1), fx);
-    const float4 c11 = lerp4(T_(x0, y0 + 1, z0 + 1), T_(x0 + 1, y0 + 1, z0 + 1), fx);
-#undef T_
-    return lerp4(lerp4(c00, c10, fy), lerp4(c01, c11, fy), fz);
-}
-
-__global__ void __launch_bounds__(256) k_vx_mipmap_tiled(VxGridDev g, int level) {
-    extern __shared__ __align__(16) float4 s_tile[];
-    const int sx = g.sx[level], sy = g.sy[level], sz = g.sz[level];
-    const int px_ = g.sx[level - 1], py_ = g.sy[level - 1], pz_ = g.sz[level - 1];      // source = 2 x destination on every axis
-    const int tilesX = (sx + IDKVX_MT_X - 1) / IDKVX_MT_X, tilesY = (sy + IDKVX_MT_Y - 1) / IDKVX_MT_Y, tilesZ = (sz + IDKVX_MT_Z - 1) / IDKVX_MT_Z;
-    const int nTiles = tilesX * tilesY * tilesZ;
-    for (int tIdx = blockIdx.x; tIdx < nTiles; tIdx += gridDim.x) {
-        const int tx = tIdx % tilesX, ty = (tIdx / tilesX) % tilesY, tz = tIdx / (tilesX * tilesY);
-        const int X0 = tx * IDKVX_MT_X, Y0 = ty * IDKVX_MT_Y, Z0 = tz * IDKVX_MT_Z;
-        const int bx = 2 * X0 - 1, by = 2 * Y0 - 1, bz = 2 * Z0 - 1;      // source coordinate of tile entry (0, 0, 0)
-        __syncthreads();                                                    // the previous tile has been consumed
-        for (int e = threadIdx.x; e < IDKVX_MS_X * IDKVX_MS_Y * IDKVX_MS_Z; e += blockDim.x) {
-            const int i = e % IDKVX_MS_X, j = (e / IDKVX_MS_X) % IDKVX_MS_Y, k = e / (IDKVX_MS_X * IDKVX_MS_Y);
-            s_tile[e] = vx_fetch(g, level - 1, clampi(bx + i, 0, px_ - 1), clampi(by + j, 0, py_ - 1), clampi(bz + k, 0, pz_ - 1));
-        }
-        __syncthreads();
-        const int lx = threadIdx.x % IDKVX_MT_X, ly = (threadIdx.x / IDKVX_MT_X) % IDKVX_MT_Y, lz = threadIdx.x / (IDKVX_MT_X * IDKVX_MT_Y);
-        const int x = X0 + lx, y = Y0 + ly, z = Z0 + lz;
-        if (x < sx && y < sy && z < sz) {
-            const float u = ((float)x + 0.5f) / (float)sx, v = ((float)y + 0.5f) / (float)sy, w = ((float)z + 0.5f) / (float)sz;
-            float4 r = vx_tile_trilinear(s_tile, bx, by, bz, px_, py_, pz_, u, v, w, 0, 0, 0);
-            float4 s;
-            s = vx_tile_trilinear(s_tile, bx, by, bz, px_, py_, pz_, u, v, w, -1, 0, 0); r = make_float4(r.x + s.x, r.y + s.y, r.z + s.z, r.w + s.w);
-            s = vx_tile_trilinear(s_tile, bx, by, bz, px_, py_, pz_, u, v, w, 1, 0, 0); r = make_float4(r.x + s.x, r.y + s.y, r.z + s.z, r.w + s.w);
-            s = vx_tile_trilinear(s_tile, bx, by, bz, px_, py_, pz_, u, v, w, 0, -1, 0); r = make_float4(r.x + s.x, r.y + s.y, r.z + s.z, r.w + s.w);
-            s = vx_tile_trilinear(s_tile, bx, by, bz, px_, py_, pz_, u, v, w, 0, 1, 0); r = make_float4(r.x + s.x, r.y + s.y, r.z + s.z, r.w + s.w);
-            s = vx_tile_trilinear(s_tile, bx, by, bz, px_, py_, pz_, u, v, w, 0, 0, -1); r = make_float4(r.x + s.x, r.y + s.y, r.z + s.z, r.w + s.w);
-            s = vx_tile_trilinear(s_tile, bx, by, bz, px_, py_, pz_, u, v, w, 0, 0, 1); r = make_float4(r.x + s.x, r.y + s.y, r.z + s.z, r.w + s.w);
-            const uint32_t lo = (uint32_t)__half_as_ushort(__float2half_rn(r.x / 7.0f)) | ((uint32_t)__half_as_ushort(__float2half_rn(r.y / 7.0f)) << 16);
-            const uint32_t hi = (uint32_t)__half_as_ushort(__float2half_rn(r.z / 7.0f)) | ((uint32_t)__half_as_ushort(__float2half_rn(r.w / 7.0f)) << 16);
-            g.level[level][((size_t)z * sy + y) * sx + x] = (unsigned long long)lo | ((unsigned long long)hi << 32);
-        }
-    }
-}
-
 // ------------------------------------------------------------------------------------------------ cone tracing
 struct VxConeArgs {
     VxGridDev g;

@@ -105,14 +105,8 @@ struct IdkPtCtx {
     int traverseBlocks = 0, traverseBlocksStats = 0, shadeBlocks = 0, traceRaysBlocks = 0, compactBlocks = 0;
     int traverse1Blocks = 0, traverse1BlocksStats = 0;
     int traverseBlocksLane = 0, traverse1BlocksLane = 0;   // grids of the asynchronous path: the resident-block budget split between the lanes
-    int traverseVariant = 3;       // 1 = k_traverse (one ray per lane, reference loop), 2 = k_traverse2 (phase-scheduled warps),
-                                   // 3 = k_traverse for the coherent primary rays, k_traverse2 for every bounce (default)
-    TraverseTuning tune = {12, 4, 0, 6, 0};   // thresholds of the phase vote (IDKPT_TUNE_*); packRays is set per launch
-    int packCta = 0;                 // IDKPT_PACK_CTA: pipelined launches let only ceil(rays / (256 * k)) CTAs take part (0 = all)
-    int packAsync = 1;               // IDKPT_PACK_ASYNC: asynchronous (pipelined) launches pack 32 rays per warp instead of spreading few rays over all warps
     size_t stackBytes = 0;
-    size_t traverse2Smem = 0;      // treelet + stacks
-    int treeletNodes = 0;
+    size_t traverse2Smem = 0;      // k_traverse2 stacks (IDK_T2_BLOCK columns)
 
     std::vector<cudaEvent_t> events;
     cudaStreamAttrValue l2Window = {};   // persisting-L2 window over [nodes | triRec]; applied to the main stream and every lane stream
@@ -200,35 +194,25 @@ static int configure_launches(IdkPtCtx* ctx) {
     CK(cudaFuncSetAttribute(k_trace_rays, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)ctx->stackBytes));
     CK(cudaFuncSetAttribute(k_trace_rays_any, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)ctx->stackBytes));
     CK(cudaFuncSetAttribute(k_shadows_ray_traced, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)ctx->stackBytes));
-    ctx->traverse2Smem = (size_t)stackSize * IDK_T2_BLOCK * sizeof(uint32_t) + (size_t)ctx->treeletNodes * 32 + (IDK_STAGED_FETCH ? IDK_STAGE_BYTES : 0);
-    if (const char* v = getenv("IDKPT_EXTRA_SMEM")) ctx->traverse2Smem += (size_t)std::max(0, atoi(v));   // experiment: L1 capacity sensitivity
-    CK(cudaFuncSetAttribute(k_traverse2<false, false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)ctx->traverse2Smem));
-    CK(cudaFuncSetAttribute(k_traverse2<true, false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)ctx->traverse2Smem));
-    CK(cudaFuncSetAttribute(k_traverse2<false, true, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)ctx->traverse2Smem));
-    CK(cudaFuncSetAttribute(k_traverse2<true, true, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)ctx->traverse2Smem));
-    CK(cudaFuncSetAttribute(k_traverse2<false, false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)ctx->traverse2Smem));
-    CK(cudaFuncSetAttribute(k_traverse2<true, false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)ctx->traverse2Smem));
+    ctx->traverse2Smem = (size_t)stackSize * IDK_T2_BLOCK * sizeof(uint32_t);
+    CK(cudaFuncSetAttribute(k_traverse2<false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)ctx->traverse2Smem));
+    CK(cudaFuncSetAttribute(k_traverse2<true, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)ctx->traverse2Smem));
+    CK(cudaFuncSetAttribute(k_traverse2<false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)ctx->traverse2Smem));
+    CK(cudaFuncSetAttribute(k_traverse2<true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)ctx->traverse2Smem));
     int n = 0;
     CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&n, k_traverse<false>, IDK_BLOCK, ctx->stackBytes));
     ctx->traverse1Blocks = std::max(1, n) * ctx->smCount;
     CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&n, k_traverse<true>, IDK_BLOCK, ctx->stackBytes));
     ctx->traverse1BlocksStats = std::max(1, n) * ctx->smCount;
-    if (ctx->traverseVariant == 1) {
-        CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&n, k_traverse<false>, IDK_BLOCK, ctx->stackBytes));
+    if (ctx->sc.useTlas) {
+        CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&n, k_traverse2<false, true>, IDK_T2_BLOCK, ctx->traverse2Smem));
         ctx->traverseBlocks = std::max(1, n) * ctx->smCount;
-        CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&n, k_traverse<true>, IDK_BLOCK, ctx->stackBytes));
-        ctx->traverseBlocksStats = std::max(1, n) * ctx->smCount;
-    } else if (ctx->sc.useTlas) {
-        CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&n, k_traverse2<false, false, true>, IDK_T2_BLOCK, ctx->traverse2Smem));
-        ctx->traverseBlocks = std::max(1, n) * ctx->smCount;
-        CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&n, k_traverse2<true, false, true>, IDK_T2_BLOCK, ctx->traverse2Smem));
+        CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&n, k_traverse2<true, true>, IDK_T2_BLOCK, ctx->traverse2Smem));
         ctx->traverseBlocksStats = std::max(1, n) * ctx->smCount;
     } else {
-        if (ctx->treeletNodes) CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&n, k_traverse2<false, true, false>, IDK_T2_BLOCK, ctx->traverse2Smem));
-        else CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&n, k_traverse2<false, false, false>, IDK_T2_BLOCK, ctx->traverse2Smem));
+        CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&n, k_traverse2<false, false>, IDK_T2_BLOCK, ctx->traverse2Smem));
         ctx->traverseBlocks = std::max(1, n) * ctx->smCount;
-        if (ctx->treeletNodes) CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&n, k_traverse2<true, true, false>, IDK_T2_BLOCK, ctx->traverse2Smem));
-        else CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&n, k_traverse2<true, false, false>, IDK_T2_BLOCK, ctx->traverse2Smem));
+        CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&n, k_traverse2<true, false>, IDK_T2_BLOCK, ctx->traverse2Smem));
         ctx->traverseBlocksStats = std::max(1, n) * ctx->smCount;
     }
     CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&n, k_trace_rays, IDK_BLOCK, ctx->stackBytes));
@@ -244,31 +228,6 @@ static int configure_launches(IdkPtCtx* ctx) {
         const int perSm2 = (ctx->traverseBlocks / ctx->smCount + lanes - 1) / lanes, perSm1 = (ctx->traverse1Blocks / ctx->smCount + lanes - 1) / lanes;
         ctx->traverseBlocksLane = std::max(1, perSm2) * ctx->smCount;
         ctx->traverse1BlocksLane = std::max(1, perSm1) * ctx->smCount;
-    }
-    if (const char* v = getenv("IDKPT_LANE_BLOCKS_PER_SM")) {        // developer knob
-        const int b = std::max(1, atoi(v));
-        ctx->traverseBlocksLane = std::min(ctx->traverseBlocks, b * ctx->smCount);
-        ctx->traverse1BlocksLane = std::min(ctx->traverse1Blocks, b * ctx->smCount);
-    }
-    if (const char* v = getenv("IDKPT_TRAVERSE_BLOCKS_PER_SM")) {   // developer knob
-        const int b = std::max(1, atoi(v));
-        ctx->traverseBlocks = std::min(ctx->traverseBlocks, b * ctx->smCount);
-        ctx->traverseBlocksStats = std::min(ctx->traverseBlocksStats, b * ctx->smCount);
-    }
-    if (const char* v = getenv("IDKPT_CARVEOUT")) {                 // developer knob: same shared-memory carve-out for every kernel
-        const int pct = atoi(v);
-        if (pct >= 0) {
-            cudaFuncSetAttribute(k_traverse<false>, cudaFuncAttributePreferredSharedMemoryCarveout, pct);
-            cudaFuncSetAttribute(k_traverse<true>, cudaFuncAttributePreferredSharedMemoryCarveout, pct);
-            cudaFuncSetAttribute(k_traverse2<false, false, false>, cudaFuncAttributePreferredSharedMemoryCarveout, pct);
-            cudaFuncSetAttribute(k_traverse2<true, false, false>, cudaFuncAttributePreferredSharedMemoryCarveout, pct);
-            cudaFuncSetAttribute(k_shade<false>, cudaFuncAttributePreferredSharedMemoryCarveout, pct);
-            cudaFuncSetAttribute(k_shade<true>, cudaFuncAttributePreferredSharedMemoryCarveout, pct);
-            cudaFuncSetAttribute(k_compact, cudaFuncAttributePreferredSharedMemoryCarveout, pct);
-            cudaFuncSetAttribute(k_raygen, cudaFuncAttributePreferredSharedMemoryCarveout, pct);
-            cudaFuncSetAttribute(k_accumulate, cudaFuncAttributePreferredSharedMemoryCarveout, pct);
-            cudaFuncSetAttribute(k_init_sample, cudaFuncAttributePreferredSharedMemoryCarveout, pct);
-        }
     }
     return IDKPT_OK;
 }
@@ -367,52 +326,6 @@ static int allocate_wavefront(IdkPtCtx* ctx) {
     }
     CK(ensure(ctx->counters, sizeof(TraceCounters)));
     return IDKPT_OK;
-}
-
-// Device-private node layout for single-BLAS scenes: the first `pairs` sibling pairs in breadth-first order are moved to
-// the front of the array (node indices 2 .. 2*pairs+1) so that the hot top of the tree is one contiguous block that a
-// single bulk copy (TMA) can stage into shared memory; all remaining pairs keep their relative order. Child pointers are
-// rewritten; leaves (triangle ranges) are untouched, so traversal order and results are unchanged.
-static int relayout_treelet(const GpuBlasNode* src, uint32_t nodeCount, uint32_t wantPairs, std::vector<GpuBlasNode>& out) {
-    const uint32_t pairCount = nodeCount / 2;            // pair p = nodes 2p, 2p+1 (pair 0 = pad + root)
-    if (pairCount < 2) return 0;
-    std::vector<uint32_t> newOf(pairCount, 0xFFFFFFFFu), order;
-    order.reserve(pairCount);
-    std::vector<uint32_t> queue;
-    queue.push_back(1);                                  // children of the root
-    size_t head = 0;
-    const uint32_t treeletPairs = std::min(wantPairs, pairCount - 1);
-    while (head < queue.size() && order.size() < treeletPairs) {
-        const uint32_t p = queue[head++];
-        newOf[p] = (uint32_t)order.size() + 1;
-        order.push_back(p);
-        for (int c = 0; c < 2; c++) {
-            const GpuBlasNode& n = src[2 * p + c];
-            if (n.TriCount == 0) {
-                if (n.TriStartOrChild < 2 || (uint32_t)n.TriStartOrChild + 1 >= nodeCount || (n.TriStartOrChild & 1)) return -1;
-                queue.push_back((uint32_t)n.TriStartOrChild / 2);
-            }
-        }
-    }
-    const uint32_t inTreelet = (uint32_t)order.size();
-    for (uint32_t p = 1; p < pairCount; p++)
-        if (newOf[p] == 0xFFFFFFFFu) { newOf[p] = (uint32_t)order.size() + 1; order.push_back(p); }
-    out.assign(nodeCount, GpuBlasNode{});
-    out[0] = src[0];
-    out[1] = src[1];
-    if (src[1].TriCount == 0) out[1].TriStartOrChild = 2;
-    for (uint32_t i = 0; i < order.size(); i++) {
-        const uint32_t p = order[i], np = i + 1;
-        for (int c = 0; c < 2; c++) {
-            GpuBlasNode n = src[2 * p + c];
-            if (n.TriCount == 0) {
-                if (n.TriStartOrChild < 2 || (uint32_t)n.TriStartOrChild + 1 >= nodeCount || (n.TriStartOrChild & 1)) return -1;
-                n.TriStartOrChild = (int32_t)(2 * newOf[(uint32_t)n.TriStartOrChild / 2]);
-            }
-            out[2 * np + c] = n;
-        }
-    }
-    return (int)inTreelet;
 }
 
 // Structural validation of one BLAS before its arrays reach the kernels (a malformed host array must become an error
@@ -553,13 +466,6 @@ IDKPT_API int idkpt_create(const IdkPtCreateInfo* ci, IdkPtCtx** out) {
         delete ctx;
         return fail(nullptr, IDKPT_ERR_CUDA, "idkpt_create: cudaStreamCreate failed");
     }
-    // developer knobs (kernel variant / scheduling thresholds); results are identical for every setting
-    if (const char* v = getenv("IDKPT_TRAVERSE_VARIANT")) ctx->traverseVariant = std::max(1, std::min(3, atoi(v)));
-    if (const char* v = getenv("IDKPT_TUNE_SETUP")) ctx->tune.setupThreshold = std::max(1, std::min(32, atoi(v)));
-    if (const char* v = getenv("IDKPT_TUNE_LEAF")) ctx->tune.leafThreshold = std::max(1, std::min(32, atoi(v)));
-    if (const char* v = getenv("IDKPT_TUNE_SETUP_STAGED")) ctx->tune.setupThresholdStaged = std::max(1, std::min(32, atoi(v)));
-    if (const char* v = getenv("IDKPT_PACK_ASYNC")) ctx->packAsync = atoi(v) != 0;
-    if (const char* v = getenv("IDKPT_PACK_CTA")) ctx->packCta = std::max(0, atoi(v));
     if (const int fl = (ci->Flags >> 8) & 15) ctx->laneCount = std::min(IDK_MAX_LANES, fl);   // IDKPT_CREATE_LANES(n)
     ctx->globalSlots = (ci->Flags & IDKPT_CREATE_GLOBAL_SLOTS) != 0;
     if (const char* v = getenv("IDKPT_LANES")) ctx->laneCount = std::max(1, std::min(IDK_MAX_LANES, atoi(v)));
@@ -662,22 +568,9 @@ IDKPT_API int idkpt_set_scene(IdkPtCtx* ctx, const IdkPtSceneDesc* s) {
     int rc;
     // nodes and triangle records share one allocation ("bvh"): [nodes | triRec], so that one L2 access-policy window covers both
     const size_t nodeBytes = ((s->BlasNodeCount * sizeof(GpuBlasNode)) + 255) & ~(size_t)255;
-    const size_t triRecBytes = std::max<size_t>(s->BlasTriangleCount, 1) * (16 * IDK_TRI_STRIDE);
+    const size_t triRecBytes = std::max<size_t>(s->BlasTriangleCount, 1) * 64;
     CK(ensure(ctx->nodes, nodeBytes + triRecBytes));
-    ctx->treeletNodes = 0;
-    std::vector<GpuBlasNode> relaid;
-    {
-        const char* env = getenv("IDKPT_TREELET_PAIRS");
-        const uint32_t wantPairs = env ? (uint32_t)std::min(768, std::max(0, atoi(env))) : 0u;   // default off
-        if (wantPairs > 0 && !s->UseTlas && s->BlasInstanceCount == 1 && s->BlasDescCount == 1 && s->BlasDescs[0].NodeOffset == 0 &&
-            s->BlasNodeCount < (1ull << 31) && (s->BlasNodeCount & 1) == 0) {
-            const int got = relayout_treelet(s->BlasNodes, (uint32_t)s->BlasNodeCount, wantPairs, relaid);
-            if (got > 0) ctx->treeletNodes = 2 * got + 2;
-            else relaid.clear();
-        }
-    }
-    CK(cudaMemcpyAsync(ctx->nodes.p, relaid.empty() ? s->BlasNodes : relaid.data(), s->BlasNodeCount * sizeof(GpuBlasNode), cudaMemcpyHostToDevice, ctx->stream));
-    CK(cudaStreamSynchronize(ctx->stream));   // `relaid` is a local
+    CK(cudaMemcpyAsync(ctx->nodes.p, s->BlasNodes, s->BlasNodeCount * sizeof(GpuBlasNode), cudaMemcpyHostToDevice, ctx->stream));
     if ((rc = upload(ctx, ctx->blasTris, s->BlasTriangles, s->BlasTriangleCount * sizeof(GpuBlasTriangle)))) return rc;
     if ((rc = upload(ctx, ctx->positions, s->VertexPositions, s->VertexPositionCount * sizeof(PackedVec3)))) return rc;
     if ((rc = upload(ctx, ctx->descs, s->BlasDescs, s->BlasDescCount * sizeof(GpuBlasDesc)))) return rc;
@@ -728,7 +621,6 @@ IDKPT_API int idkpt_set_scene(IdkPtCtx* ctx, const IdkPtSceneDesc* s) {
     sc.stackSize = std::max(1, s->BlasStackSize);
     sc.tlasNodes = (const float4*)ctx->tlas.p;
     sc.useTlas = s->UseTlas ? 1 : 0;
-    sc.treeletNodes = ctx->treeletNodes;
     sc.vtxFrame = (const float4*)ctx->vtxFrame.p;
     sc.surfRec = (const float4*)ctx->surfRec.p;
     sc.textures = (const TexRec*)ctx->texRecs.p;
@@ -743,11 +635,9 @@ IDKPT_API int idkpt_set_scene(IdkPtCtx* ctx, const IdkPtSceneDesc* s) {
     {
         cudaDeviceProp prop;
         CK(cudaGetDeviceProperties(&prop, ctx->device));
-        const char* env = getenv("IDKPT_L2_PERSIST");
-        const bool want = !(env && atoi(env) == 0);
         cudaStreamAttrValue& attr = ctx->l2Window;
         memset(&attr, 0, sizeof(attr));
-        if (want && prop.persistingL2CacheMaxSize > 0 && prop.accessPolicyMaxWindowSize > 0) {
+        if (prop.persistingL2CacheMaxSize > 0 && prop.accessPolicyMaxWindowSize > 0) {
             const size_t bvhBytes = nodeBytes + triRecBytes;
             const size_t setAside = std::min<size_t>((size_t)prop.persistingL2CacheMaxSize, std::max<size_t>(bvhBytes, 1 << 20));
             CK(cudaDeviceSetLimit(cudaLimitPersistingL2CacheSize, setAside));
@@ -943,19 +833,7 @@ IDKPT_API int idkpt_stream_handle(IdkPtCtx* ctx, void** stream) {
 IDKPT_API int idkpt_sync(IdkPtCtx* ctx) {
     if (!ctx) return IDKPT_ERR_INVALID_ARGUMENT;
     CK(cudaSetDevice(ctx->device));
-    int rc = check_device_errors(ctx, drain(ctx), "idkpt_sync");
-#if IDK_PHASE_STATS
-    if (rc == IDKPT_OK && ctx->counters.p) {   // instrumented build: phase statistics of everything since the last dump (asynchronous path included)
-        TraceCounters tc;
-        CK(cudaMemcpy(&tc, ctx->counters.p, sizeof(tc), cudaMemcpyDeviceToHost));
-        CK(cudaMemset(ctx->counters.p, 0, sizeof(tc)));
-        const double bs = 32.0 * (double)tc.phaseRounds[1];
-        fprintf(stderr, "[idkpt phase stats @sync] rounds SETUP %llu BOX %llu LEAF %llu | lanes/round SETUP %.1f BOX %.1f LEAF %.1f | BOX lane slots: active %.1f%% wait-SETUP %.1f%% wait-LEAF %.1f%% exited %.1f%%\n",
-                tc.phaseRounds[0], tc.phaseRounds[1], tc.phaseRounds[2], (double)tc.phaseLanes[0] / std::max(1ull, tc.phaseRounds[0]), (double)tc.phaseLanes[1] / std::max(1ull, tc.phaseRounds[1]),
-                (double)tc.phaseLanes[2] / std::max(1ull, tc.phaseRounds[2]), 100.0 * tc.phaseLanes[1] / std::max(1.0, bs), 100.0 * tc.boxIdle[0] / std::max(1.0, bs), 100.0 * tc.boxIdle[1] / std::max(1.0, bs), 100.0 * tc.boxIdle[2] / std::max(1.0, bs));
-    }
-#endif
-    return rc;
+    return check_device_errors(ctx, drain(ctx), "idkpt_sync");
 }
 
 IDKPT_API int idkpt_compute(IdkPtCtx* ctx, const GpuPerFrameData* frame, const IdkPtSettings* st, IdkPtStats* stats) {
@@ -1088,23 +966,18 @@ IDKPT_API int idkpt_compute(IdkPtCtx* ctx, const GpuPerFrameData* frame, const I
             ta.traceLights = st->Gpu.DoTraceLights;
             ta.bounce = j;
             e0 = ev.begin();
-            if (ctx->traverseVariant == 1 || (ctx->traverseVariant == 3 && first)) {
+            if (first) {     // the coherent primary rays: one ray per lane
                 if (wantStats) k_traverse<true><<<ctx->traverse1BlocksStats, IDK_BLOCK, ctx->stackBytes, ls>>>(ta);
                 else k_traverse<false><<<async ? ctx->traverse1BlocksLane : ctx->traverse1Blocks, IDK_BLOCK, ctx->stackBytes, ls>>>(ta);
-            } else {
+            } else {         // every later bounce: phase-scheduled warps
                 const int tb = async ? ctx->traverseBlocksLane : ctx->traverseBlocks;
-                TraverseTuning tune = ctx->tune;
-                tune.packRays = (async && ctx->packAsync) ? 1 : 0;
-                tune.packCta = (async && ctx->packAsync) ? ctx->packCta : 0;
+                const TraverseTuning tune = {IDK_T2_SETUP_THRESHOLD, IDK_T2_LEAF_THRESHOLD, async ? 1 : 0};
                 if (ctx->sc.useTlas) {       // the TLAS walk is a fourth phase of the production kernel (BVHIntersect.glsl:205-272)
-                    if (wantStats) k_traverse2<true, false, true><<<ctx->traverseBlocksStats, IDK_T2_BLOCK, ctx->traverse2Smem, ls>>>(ta, tune);
-                    else k_traverse2<false, false, true><<<tb, IDK_T2_BLOCK, ctx->traverse2Smem, ls>>>(ta, tune);
-                } else if (ctx->treeletNodes) {
-                    if (wantStats) k_traverse2<true, true, false><<<ctx->traverseBlocksStats, IDK_T2_BLOCK, ctx->traverse2Smem, ls>>>(ta, tune);
-                    else k_traverse2<false, true, false><<<tb, IDK_T2_BLOCK, ctx->traverse2Smem, ls>>>(ta, tune);
+                    if (wantStats) k_traverse2<true, true><<<ctx->traverseBlocksStats, IDK_T2_BLOCK, ctx->traverse2Smem, ls>>>(ta, tune);
+                    else k_traverse2<false, true><<<tb, IDK_T2_BLOCK, ctx->traverse2Smem, ls>>>(ta, tune);
                 } else {
-                    if (wantStats) k_traverse2<true, false, false><<<ctx->traverseBlocksStats, IDK_T2_BLOCK, ctx->traverse2Smem, ls>>>(ta, tune);
-                    else k_traverse2<false, false, false><<<tb, IDK_T2_BLOCK, ctx->traverse2Smem, ls>>>(ta, tune);
+                    if (wantStats) k_traverse2<true, false><<<ctx->traverseBlocksStats, IDK_T2_BLOCK, ctx->traverse2Smem, ls>>>(ta, tune);
+                    else k_traverse2<false, false><<<tb, IDK_T2_BLOCK, ctx->traverse2Smem, ls>>>(ta, tune);
                 }
             }
             ev.end(e0, 0, j);
@@ -1227,12 +1100,6 @@ IDKPT_API int idkpt_compute(IdkPtCtx* ctx, const GpuPerFrameData* frame, const I
             stats->TriangleTests = tc.tris;
             stats->InstanceVisits = tc.instances;
             stats->Hits = tc.hits;
-#if IDK_PHASE_STATS
-            fprintf(stderr, "[idkpt phase stats] SETUP rounds %llu lanes %llu | BOX rounds %llu lanes %llu | LEAF rounds %llu lanes %llu\n", tc.phaseRounds[0], tc.phaseLanes[0],
-                    tc.phaseRounds[1], tc.phaseLanes[1], tc.phaseRounds[2], tc.phaseLanes[2]);
-            fprintf(stderr, "[idkpt phase stats] during BOX rounds, idle lanes: waiting SETUP %llu, waiting LEAF %llu, exited %llu\n", tc.boxIdle[0], tc.boxIdle[1], tc.boxIdle[2]);
-            { double mx = 0; for (int j = 0; j < st->RayDepth; j++) mx += tc.maxSteps[j]; fprintf(stderr, "[idkpt phase stats] sum over bounces of the longest ray: %.0f steps\n", mx); }
-#endif
             for (int j = 0; j < IDKPT_MAX_RAY_DEPTH; j++) stats->BounceMaxSteps[j] = tc.maxSteps[j];
         }
         for (const EventPool::Span& sp : ev.spans) {
@@ -1387,8 +1254,8 @@ static int preload_kernels(IdkPtCtx* ctx) {
 #define IDK_PRELOAD(k) CK(cudaFuncGetAttributes(&fa, k))
     IDK_PRELOAD(k_init_sample); IDK_PRELOAD(k_prepare_triangles); IDK_PRELOAD(k_prepare_vertices); IDK_PRELOAD(k_prepare_surfaces);
     IDK_PRELOAD(k_raygen); IDK_PRELOAD(k_traverse<false>); IDK_PRELOAD(k_traverse<true>);
-    IDK_PRELOAD((k_traverse2<false, false, false>)); IDK_PRELOAD((k_traverse2<true, false, false>)); IDK_PRELOAD((k_traverse2<false, true, false>));
-    IDK_PRELOAD((k_traverse2<true, true, false>)); IDK_PRELOAD((k_traverse2<false, false, true>)); IDK_PRELOAD((k_traverse2<true, false, true>));
+    IDK_PRELOAD((k_traverse2<false, false>)); IDK_PRELOAD((k_traverse2<true, false>));
+    IDK_PRELOAD((k_traverse2<false, true>)); IDK_PRELOAD((k_traverse2<true, true>));
     IDK_PRELOAD(k_shade<false>); IDK_PRELOAD(k_shade<true>); IDK_PRELOAD(k_compact); IDK_PRELOAD(k_slot_exchange);
     IDK_PRELOAD(k_accumulate); IDK_PRELOAD(k_accumulate_aov); IDK_PRELOAD(k_accumulate_scatter); IDK_PRELOAD(k_gather_wait);
     IDK_PRELOAD(k_sort_histogram); IDK_PRELOAD(k_sort_scan); IDK_PRELOAD(k_sort_scatter);
@@ -1810,7 +1677,6 @@ IDKPT_API int idkpt_blas_refit(IdkPtCtx* ctx, uint32_t first, uint32_t count, fl
     DRAIN_PENDING("idkpt_blas_refit");
     if (!ctx->haveScene) return fail(ctx, IDKPT_ERR_NO_SCENE, "idkpt_blas_refit: no scene");
     if ((uint64_t)first + count > ctx->hostDescs.size()) return fail(ctx, IDKPT_ERR_INVALID_ARGUMENT, "idkpt_blas_refit: BLAS range outside BlasDescs");
-    if (ctx->treeletNodes) return fail(ctx, IDKPT_ERR_UNSUPPORTED, "idkpt_blas_refit: not available with the treelet node layout (IDKPT_TREELET_PAIRS)");
     if (kernelMs) *kernelMs = 0.0f;
     CK(cudaSetDevice(ctx->device));
     int maxNodes = 0;
@@ -1851,7 +1717,6 @@ IDKPT_API int idkpt_tlas_build(IdkPtCtx* ctx, int32_t searchRadius, float* kerne
     if (searchRadius < 1 || searchRadius > 1024) return fail(ctx, IDKPT_ERR_INVALID_ARGUMENT, "idkpt_tlas_build: search radius out of range (TLAS.BuildSettings.SearchRadius, default 15)");
     const uint64_t n = ctx->counts.BlasInstanceCount;
     if (n > 16384) return fail(ctx, IDKPT_ERR_UNSUPPORTED, "idkpt_tlas_build: more than 16384 instances (single-CTA build); build on the host and idkpt_update_range");
-    if (ctx->treeletNodes) return fail(ctx, IDKPT_ERR_UNSUPPORTED, "idkpt_tlas_build: not available with the treelet node layout (IDKPT_TREELET_PAIRS)");
     CK(cudaSetDevice(ctx->device));
     const size_t nodeCount = 2 * n - 1;
     const size_t tempOff = 0, leavesOff = nodeCount * 32, keysOff = leavesOff + n * 32, prefOff = keysOff + n * 4, needOff = prefOff + n * 4;
@@ -1896,7 +1761,6 @@ IDKPT_API int idkpt_read_range(IdkPtCtx* ctx, IdkPtArrayId which, uint64_t first
         case IDKPT_ARRAY_TLAS_NODES: b = &ctx->tlas; elem = sizeof(GpuTlasNode); limit = ctx->counts.UseTlas ? ctx->counts.TlasNodeCount : 0; break;
         default: return fail(ctx, IDKPT_ERR_INVALID_ARGUMENT, "idkpt_read_range: array id not readable");
     }
-    if (which == IDKPT_ARRAY_BLAS_NODES && ctx->treeletNodes) return fail(ctx, IDKPT_ERR_UNSUPPORTED, "idkpt_read_range: BLAS nodes are re-laid out (IDKPT_TREELET_PAIRS)");
     if (first > limit || count > limit - first) return fail(ctx, IDKPT_ERR_INVALID_ARGUMENT, "idkpt_read_range: range outside the array");
     CK(cudaSetDevice(ctx->device));
     if (count) CK(cudaMemcpyAsync(out, (const char*)b->p + first * elem, count * elem, cudaMemcpyDeviceToHost, ctx->stream));

@@ -89,7 +89,6 @@ IDKPT_API int idkvx_create(const IdkVxCreateInfo* ci, IdkVxCtx** out) {
     IdkVxCtx* ctx = new IdkVxCtx();
     ctx->device = ci->Device;
     ctx->smCount = prop.multiProcessorCount;
-    cudaFuncSetAttribute(k_vx_mipmap_tiled, cudaFuncAttributeMaxDynamicSharedMemorySize, IDKVX_MIP_TILE_SMEM);
     if (cudaStreamCreateWithFlags(&ctx->stream, cudaStreamNonBlocking) != cudaSuccess) { delete ctx; return vfail(nullptr, IDKPT_ERR_CUDA, "idkvx_create: stream creation failed"); }
     // Texture.GetMaxMipmapLevel: levels down to 1 texel of the largest extent
     const int mx = std::max(ci->Width, std::max(ci->Height, ci->Depth));
@@ -266,18 +265,7 @@ IDKPT_API int idkvx_voxelize(IdkVxCtx* ctx, IdkVxStats* stats) {
     for (int l = 1; l < (ctx->slabMode ? 1 : ctx->grid.levels); l++) {
         const size_t n = ctx->levelTexels[l];
         const int blocks = (int)std::min<size_t>((n + 255) / 256, (size_t)ctx->smCount * 16);
-        // levels that halve exactly on every axis and are big enough to fill the machine take the shared-memory tiled kernel
-        const VxGridDev& gd = ctx->grid;
-        const bool halves = gd.sx[l - 1] == 2 * gd.sx[l] && gd.sy[l - 1] == 2 * gd.sy[l] && gd.sz[l - 1] == 2 * gd.sz[l];
-        // the direct kernel's 7x re-reads are L1 hits and the filter is bound by its ~640 fp32 operations per texel, not by
-        // memory, so the tiled kernel is opt-in only (cross-check)
-        const bool tiledOn = getenv("IDKVX_MIP_TILED") && atoi(getenv("IDKVX_MIP_TILED")) != 0;
-        if (halves && n >= 4096 && tiledOn) {
-            const int tiles = ((gd.sx[l] + IDKVX_MT_X - 1) / IDKVX_MT_X) * ((gd.sy[l] + IDKVX_MT_Y - 1) / IDKVX_MT_Y) * ((gd.sz[l] + IDKVX_MT_Z - 1) / IDKVX_MT_Z);
-            k_vx_mipmap_tiled<<<std::min(tiles, ctx->smCount * 4), 256, IDKVX_MIP_TILE_SMEM, ctx->stream>>>(ctx->grid, l);
-        } else {
-            k_vx_mipmap<<<blocks, 256, 0, ctx->stream>>>(ctx->grid, l);
-        }
+        k_vx_mipmap<<<blocks, 256, 0, ctx->stream>>>(ctx->grid, l);
         launches++;
     }
     VCK(cudaEventRecord(ev[3], ctx->stream));

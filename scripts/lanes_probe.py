@@ -13,26 +13,23 @@ out = {}
 K = 40
 for tname, tile in (("full", (8, 0, 1)), ("eighth", (8, 0, 8))):
     for lanes in (1, 2, 3, 4, 6, 8):
-        for lb in ((0,) if lanes == 1 else (0, 2)):
-            if lb: os.environ["IDKPT_LANE_BLOCKS_PER_SM"] = str(lb)
-            s = capi.default_settings(); s.RayDepth = args.ray_depth
-            pt = PathTracer(args.width, args.height, s, device=0, tile=tile, lanes=lanes)
-            pt.SetScene(scene); pt.SetSky(bench.SKY); pt.SetFrame(frame)
-            os.environ.pop("IDKPT_LANE_BLOCKS_PER_SM", None)
-            rays = pt.Compute().Rays
-            ext = torch.cuda.ExternalStream(pt.StreamHandle())
-            e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-            for rep in range(2):
-                pt.ResetAccumulation()
-                torch.cuda.synchronize()
-                e0.record(ext)
-                for _ in range(K if rep else 8):
-                    pt.ComputeAsync() if lanes > 1 else pt.Compute(want_stats=False)
-                e1.record(ext)
-                pt.Sync()
-            ms = e0.elapsed_time(e1) / K
-            key = f"{tname}_lanes{lanes}" + (f"_{lb}blk" if lb else "")
-            out[key] = {"ms_per_sample": ms, "mrays_s": rays / ms / 1e3}
-            print(key, out[key], flush=True)
-            pt.Dispose()
+        s = capi.default_settings(); s.RayDepth = args.ray_depth
+        pt = PathTracer(args.width, args.height, s, device=0, tile=tile, lanes=lanes)
+        pt.SetScene(scene); pt.SetSky(bench.SKY); pt.SetFrame(frame)
+        rays = pt.Compute().Rays
+        ext = torch.cuda.ExternalStream(pt.StreamHandle())
+        e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+        for rep in range(2):
+            pt.ResetAccumulation()
+            torch.cuda.synchronize()
+            e0.record(ext)
+            for _ in range(K if rep else 8):
+                pt.ComputeAsync() if lanes > 1 else pt.Compute(want_stats=False)
+            e1.record(ext)
+            pt.Sync()
+        ms = e0.elapsed_time(e1) / K
+        key = f"{tname}_lanes{lanes}"
+        out[key] = {"ms_per_sample": ms, "mrays_s": rays / ms / 1e3}
+        print(key, out[key], flush=True)
+        pt.Dispose()
 json.dump(out, open("gpurun_out/lanes_probe.json", "w"), indent=1)

@@ -1,5 +1,5 @@
 """Can two samples in flight hide the tail-bounce latency? Emulated with several contexts on one GPU, one host thread
-each (idkpt_compute blocks, ctypes releases the GIL). Reports aggregate Mrays/s per variant."""
+each (idkpt_compute blocks, ctypes releases the GIL). Reports aggregate Mrays/s per context count."""
 import json, os, sys, threading, time
 sys.path.insert(0, os.path.join(os.path.dirname(os.path.abspath(__file__)), ".."))
 import numpy as np
@@ -13,17 +13,13 @@ scene, cam, frame = bench.build_scene(args)
 K = 24
 out = {}
 
-def run(name, nctx, tile, env):
-    for k, v in env.items():
-        os.environ[k] = v
+def run(name, nctx, tile):
     s = capi.default_settings(); s.RayDepth = args.ray_depth
     pts = []
     for _ in range(nctx):
         pt = PathTracer(args.width, args.height, s, device=0, tile=tile)
         pt.SetScene(scene); pt.SetSky(bench.SKY); pt.SetFrame(frame)
         pts.append(pt)
-    for k in env:
-        del os.environ[k]
     rays = [0] * nctx
     def worker(i, n):
         for _ in range(n):
@@ -40,13 +36,10 @@ def run(name, nctx, tile, env):
     for pt in pts: pt.Dispose()
 
 full, eighth = (8, 0, 1), (8, 0, 8)
-run("full_1ctx", 1, full, {})
-run("full_2ctx_default", 2, full, {})
-run("full_2ctx_2blocks", 2, full, {"IDKPT_TRAVERSE_BLOCKS_PER_SM": "2"})
-run("full_3ctx_default", 3, full, {})
-run("eighth_1ctx", 1, eighth, {})
-run("eighth_2ctx_default", 2, eighth, {})
-run("eighth_2ctx_2blocks", 2, eighth, {"IDKPT_TRAVERSE_BLOCKS_PER_SM": "2"})
-run("eighth_4ctx_1block", 4, eighth, {"IDKPT_TRAVERSE_BLOCKS_PER_SM": "1"})
-run("eighth_4ctx_default", 4, eighth, {})
+run("full_1ctx", 1, full)
+run("full_2ctx", 2, full)
+run("full_3ctx", 3, full)
+run("eighth_1ctx", 1, eighth)
+run("eighth_2ctx", 2, eighth)
+run("eighth_4ctx", 4, eighth)
 json.dump(out, open("gpurun_out/overlap_probe.json", "w"), indent=1)

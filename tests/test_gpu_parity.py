@@ -169,9 +169,8 @@ def test_tlas_traversal(multi_blas):
 
 
 def test_tlas_walk_in_the_production_kernel():
-    """28 instances -> 55 TLAS nodes. The phase-scheduled kernel (TLAS = 4th phase, default) and the one-ray-per-lane kernel
-    (IDKPT_TRAVERSE_VARIANT=1) both equal the oracle: images, wavefront state and S/T/I counters; so do 4 samples in flight."""
-    import os
+    """28 instances -> 55 TLAS nodes. The one-ray-per-lane kernel (primary rays) and the phase-scheduled kernel (every later
+    bounce, TLAS = 4th phase) together equal the oracle: images, wavefront state and S/T/I counters; so do 4 samples in flight."""
     scene, cam = scenes.instance_grid(3, threads=1)
     assert scene.use_tlas == 1 and len(scene.tlas_nodes) == 2 * len(scene.blas_instances) - 1 == 55
     s = capi.default_settings()
@@ -181,12 +180,6 @@ def test_tlas_walk_in_the_production_kernel():
     g, o = run_both(scene, cam, w, h, s, calls=2)
     assert_same(g, o)
     assert g["stats"][0].InstanceVisits > g["stats"][0].Rays // 2    # the walk reaches BLASes for most rays (28 instances, culled by the TLAS)
-    os.environ["IDKPT_TRAVERSE_VARIANT"] = "1"
-    try:
-        g1, _ = run_both(scene, cam, w, h, s, calls=2)
-    finally:
-        del os.environ["IDKPT_TRAVERSE_VARIANT"]
-    assert_same(g1, o)
     frame = scenes.camera_frame(cam, w, h)
     with PathTracer(w, h, s, lanes=4) as pt:
         pt.SetScene(scene); pt.SetSky((0.6, 0.7, 0.9)); pt.SetFrame(frame)
@@ -312,34 +305,6 @@ def test_large_config_properties():
     band = (8, 33, 67)   # stripe 8, tile 33 of 67 -> rows 264..271, 800..807 (2 stripes)
     g, o = run_both(scene, cam, w, h, s, tile=band)
     assert_same(g, o)
-
-
-def test_treelet_and_kernel_variants_agree(atrium_small):
-    """Developer knobs select other code paths (plain loop everywhere, phase-scheduled everywhere, TMA-staged treelet with
-    the BFS-first node re-layout): every one of them must reproduce the oracle bit for bit."""
-    import os
-    scene, cam = atrium_small
-    s = capi.default_settings()
-    s.RayDepth = 5
-    rays = random_rays(6000, -6.0, 6.0, 31)
-    ref = ol.trace_rays(scene, rays)
-    for env in ({"IDKPT_TRAVERSE_VARIANT": "1"}, {"IDKPT_TRAVERSE_VARIANT": "2"},
-                {"IDKPT_TRAVERSE_VARIANT": "2", "IDKPT_TREELET_PAIRS": "192"}, {"IDKPT_TREELET_PAIRS": "5"},
-                {"IDKPT_TRAVERSE_VARIANT": "2", "IDKPT_TREELET_PAIRS": "100000"}):
-        old = {k: os.environ.get(k) for k in env}
-        os.environ.update(env)
-        try:
-            assert_same(*run_both(scene, cam, 160, 96, s))
-            with PathTracer(32, 32) as pt:
-                pt.SetScene(scene)
-                g, _ = pt.TraceRays(rays)
-            assert_hits_equal(g, ref)
-        finally:
-            for k, v in old.items():
-                if v is None:
-                    os.environ.pop(k, None)
-                else:
-                    os.environ[k] = v
 
 
 def test_errors(cornell):
