@@ -21,11 +21,24 @@
 #define IDKPT_ABI_VERSION 4u   // 2: IdkPtSceneDesc gained Textures / TextureCount; 3: IdkPtStats gained CompactMs / AccumulateMs, host-buffer registration;
                                // 4: gather handle blob is 5 IPC handles (320 bytes), IDKPT_CREATE_GLOBAL_SLOTS, idkpt_gather_connect
 
-static thread_local std::string g_createError;
-
 struct DevBuf {
     void* p = nullptr;
     size_t bytes = 0;
+};
+
+// What the path tracer (IdkPtCtx) and the voxeliser (IdkVxCtx) contexts share: device, stream, last error, and the events
+// run_timed brackets synchronous work with.
+struct IdkCtxBase {
+    int device = 0;
+    int smCount = 132;
+    cudaStream_t stream = nullptr;
+    std::string lastError;
+    cudaEvent_t timing[4] = {};    // [0], [1]: start and end of run_timed's work; [2], [3]: marks inside it (idkvx_voxelize's spans)
+};
+
+// Material textures: all base levels in one allocation, their records, the sRGB decode table.
+struct TextureTable {
+    DevBuf pixels, recs, srgbLut;
 };
 
 #define IDK_MAX_LANES 16
@@ -47,11 +60,8 @@ struct Lane {
     uint32_t slotEpoch = 0;        // exchanges issued on this lane since the peers were connected (identical on every rank)
 };
 
-struct IdkPtCtx {
-    int device = 0;
-    int smCount = 132;
-    cudaStream_t stream = nullptr;
-    std::string lastError;
+struct IdkPtCtx : IdkCtxBase {
+    static inline thread_local std::string createError;   // last failed idkpt_create (idkpt_last_error(NULL))
 
     // image / tile geometry
     int width = 0, height = 0;
@@ -68,7 +78,7 @@ struct IdkPtCtx {
     float sky[3] = {0.0f, 0.0f, 0.0f};
     DevBuf skyFaces;
     int skyFaceSize = 0;
-    DevBuf texPixels, texRecs, srgbLut;   // material textures (RGBA8 base levels), their records, sRGB decode table
+    TextureTable tex;
     std::vector<uint64_t> hostMaterialMaxHandle;   // per material: largest texture handle it uses (validation of later edits)
 
     // host-array entry points (trace_rays, shadows): device staging buffers, kept between calls
@@ -146,8 +156,14 @@ struct IdkPtCtx {
         }                                                                                          \
     } while (0)
 
-static int fail(IdkPtCtx* ctx, int code, const char* msg) {
-    if (ctx) ctx->lastError = msg; else g_createError = msg;
+// Without a context the message goes to the last create error of that context type.
+template <class Ctx> static int fail(Ctx* ctx, int code, const char* msg) {
+    (ctx ? ctx->lastError : Ctx::createError) = msg;
+    return code;
+}
+
+static int fail(IdkCtxBase* ctx, const char* who, int code, const char* what) {
+    ctx->lastError = std::string(who) + ": " + what;
     return code;
 }
 
@@ -168,9 +184,38 @@ static void release(DevBuf& b) {
     b.bytes = 0;
 }
 
-static int upload(IdkPtCtx* ctx, DevBuf& b, const void* src, size_t bytes) {
+static int upload(IdkCtxBase* ctx, DevBuf& b, const void* src, size_t bytes) {
     CK(ensure(b, std::max<size_t>(bytes, 16)));
     if (bytes) CK(cudaMemcpyAsync(b.p, src, bytes, cudaMemcpyHostToDevice, ctx->stream));
+    return IDKPT_OK;
+}
+
+static int create_stream(IdkCtxBase* ctx) {
+    CK(cudaStreamCreateWithFlags(&ctx->stream, cudaStreamNonBlocking));
+    for (cudaEvent_t& e : ctx->timing) CK(cudaEventCreate(&e));
+    return IDKPT_OK;
+}
+
+static void destroy_stream(IdkCtxBase* ctx) {
+    for (cudaEvent_t e : ctx->timing) if (e) cudaEventDestroy(e);
+    if (ctx->stream) cudaStreamDestroy(ctx->stream);
+}
+
+// Synchronous, timed work on the context's stream: `work` enqueues it between the start and end events and returns IDKPT_OK
+// or an error code. The result's copy to the host (dst, if given) follows the end event, outside the timing. Waits for the
+// stream, reports a launch or execution error as "<who>: <CUDA error>", and writes the elapsed time to *ms only on success.
+template <class Work>
+static int run_timed(IdkCtxBase* ctx, const char* who, float* ms, Work&& work, void* dst = nullptr, const void* src = nullptr, size_t bytes = 0) {
+    CK(cudaEventRecord(ctx->timing[0], ctx->stream));
+    if (int rc = work()) return rc;
+    cudaError_t e = cudaGetLastError();
+    if (e == cudaSuccess) {
+        CK(cudaEventRecord(ctx->timing[1], ctx->stream));
+        if (dst) CK(cudaMemcpyAsync(dst, src, bytes, cudaMemcpyDeviceToHost, ctx->stream));
+        e = cudaStreamSynchronize(ctx->stream);
+    }
+    if (e != cudaSuccess) return fail(ctx, who, IDKPT_ERR_CUDA, cudaGetErrorString(e));
+    if (ms) CK(cudaEventElapsedTime(ms, ctx->timing[0], ctx->timing[1]));
     return IDKPT_OK;
 }
 
@@ -328,10 +373,6 @@ static int allocate_wavefront(IdkPtCtx* ctx) {
     return IDKPT_OK;
 }
 
-// Structural validation of one BLAS before its arrays reach the kernels (a malformed host array must become an error
-// code, never a device fault): child pairs in range, even, and behind their parent (the builder emits DFS order, which
-// also rules out cycles); leaf ranges inside the BLAS's triangle range; and the traversal stack the kernels will need
-// (BLAS.ComputeRequiredStackSize, Bvh/BLAS.cs:672-702) must fit BlasStackSize. Returns nullptr or an error text.
 static const char* validate_material_textures(const GpuMaterial& m, uint64_t textureCount, const char* msg) {
     const uint64_t h[5] = {m.BaseColorTexture, m.MetallicRoughnessTexture, m.NormalTexture, m.EmissiveTexture, m.TransmissionTexture};
     for (int i = 0; i < 5; i++) if (h[i] > textureCount) return msg;
@@ -343,25 +384,69 @@ static uint64_t material_max_handle(const GpuMaterial& m) {
 }
 
 // Material textures: all base levels in one allocation, 256-byte aligned; 32-byte records point into it.
-static int upload_textures(IdkPtCtx* ctx, const IdkPtTextureDesc* textures, uint64_t count) {
+static int upload_textures(IdkCtxBase* ctx, TextureTable& t, const IdkPtTextureDesc* textures, uint64_t count) {
     IdkPtSceneDesc tmp = {};
     tmp.Textures = textures; tmp.TextureCount = count;
     const std::vector<size_t> off = idk_texture_offsets(&tmp);
-    CK(ensure(ctx->texPixels, std::max<size_t>(off[count], 16)));
+    CK(ensure(t.pixels, std::max<size_t>(off[count], 16)));
     std::vector<TexRec> recs;
-    CK(idk_upload_texture_table(textures, count, off, ctx->texPixels.p, ctx->stream, recs));
+    CK(idk_upload_texture_table(textures, count, off, t.pixels.p, ctx->stream, recs));
     int rc;
-    if ((rc = upload(ctx, ctx->texRecs, recs.data(), recs.size() * sizeof(TexRec)))) return rc;
+    if ((rc = upload(ctx, t.recs, recs.data(), recs.size() * sizeof(TexRec)))) return rc;
     float lut[256];
     idk_srgb_lut(lut);
-    if ((rc = upload(ctx, ctx->srgbLut, lut, sizeof(lut)))) return rc;
+    if ((rc = upload(ctx, t.srgbLut, lut, sizeof(lut)))) return rc;
     CK(cudaStreamSynchronize(ctx->stream));   // recs / lut are locals
-    ctx->sc.textures = (const TexRec*)ctx->texRecs.p;
-    ctx->sc.textureCount = (uint32_t)count;
-    ctx->sc.srgbLut = (const float*)ctx->srgbLut.p;
     return IDKPT_OK;
 }
 
+// idk_validate_textures's verdict: formats the decoder lacks are unsupported, anything else is an invalid argument.
+static int texture_error(IdkCtxBase* ctx, const char* who, const char* terr) {
+    return fail(ctx, who, strstr(terr, "not supported") ? IDKPT_ERR_UNSUPPORTED : IDKPT_ERR_INVALID_ARGUMENT, terr);
+}
+
+// Checks idkpt_set_scene and idkvx_set_scene share: every index the kernels chase must be in range (a malformed host array
+// must become an error code, never a device fault).
+static int validate_scene(IdkCtxBase* ctx, const char* who, const IdkPtSceneDesc* s) {
+    if (!s->BlasTriangles || !s->BlasDescs || !s->BlasInstances || !s->MeshTransforms || !s->Meshes || !s->Materials || !s->Vertices || !s->VertexPositions)
+        return fail(ctx, who, IDKPT_ERR_INVALID_ARGUMENT, "a required array is null");
+    if (s->LightCount > IDK_GPU_MAX_UBO_LIGHT_COUNT) return fail(ctx, who, IDKPT_ERR_INVALID_ARGUMENT, "more than 256 lights");
+    for (uint64_t i = 0; i < s->BlasInstanceCount; i++)
+        if (s->BlasInstances[i].BlasId >= s->BlasDescCount || s->BlasInstances[i].MeshTransformId >= s->MeshTransformCount)
+            return fail(ctx, who, IDKPT_ERR_INVALID_ARGUMENT, "BlasInstance references a missing BLAS or transform");
+    for (uint64_t i = 0; i < s->BlasDescCount; i++) {
+        const GpuBlasDesc& d = s->BlasDescs[i];
+        if (d.TriangleOffset < 0 || d.TriangleCount < 0 || (uint64_t)d.TriangleOffset + d.TriangleCount > s->BlasTriangleCount)
+            return fail(ctx, who, IDKPT_ERR_INVALID_ARGUMENT, "GpuBlasDesc triangle range outside the array");
+    }
+    // triangle vertex ids must index the position / vertex arrays (checked on the host copy: cheap relative to the BVH build
+    // that produced it)
+    const uint64_t lim = std::min(s->VertexPositionCount, s->VertexCount);
+    for (uint64_t i = 0; i < s->BlasTriangleCount; i++) {
+        const GpuBlasTriangle& t = s->BlasTriangles[i];
+        if ((uint64_t)(uint32_t)t.X >= lim || (uint64_t)(uint32_t)t.Y >= lim || (uint64_t)(uint32_t)t.Z >= lim || t.MeshId < 0 || (uint64_t)t.MeshId >= s->MeshCount)
+            return fail(ctx, who, IDKPT_ERR_INVALID_ARGUMENT, "GpuBlasTriangle index out of range");
+    }
+    for (uint64_t i = 0; i < s->MeshCount; i++)
+        if (s->Meshes[i].MaterialId < 0 || (uint64_t)s->Meshes[i].MaterialId >= s->MaterialCount) return fail(ctx, who, IDKPT_ERR_INVALID_ARGUMENT, "GpuMesh.MaterialId out of range");
+    if (const char* terr = idk_validate_textures(s)) return texture_error(ctx, who, terr);
+    return IDKPT_OK;
+}
+
+// TLAS.AllocateRequiredNodes (TLAS.cs:266-269): children adjacent and behind their parent, leaves name an existing instance.
+// `t` holds nodes [first, first + count) of a TLAS with nodeCount nodes.
+static bool tlas_nodes_valid(const GpuTlasNode* t, uint64_t first, uint64_t count, uint64_t nodeCount, uint64_t instanceCount) {
+    for (uint64_t i = 0; i < count; i++) {
+        const uint32_t w = t[i].IsLeafAndChildOrInstanceId, id = w & 0x7FFFFFFFu;
+        if ((w >> 31) ? (id >= instanceCount) : (id <= first + i || (uint64_t)id + 1 >= nodeCount)) return false;
+    }
+    return true;
+}
+
+// Structural validation of one BLAS before its arrays reach the kernels: child pairs in range, even, and behind their parent
+// (the builder emits DFS order, which also rules out cycles); leaf ranges inside the BLAS's triangle range; and the
+// traversal stack the kernels will need (BLAS.ComputeRequiredStackSize, Bvh/BLAS.cs:672-702) must fit BlasStackSize.
+// Returns nullptr or an error text.
 static const char* validate_blas(const GpuBlasNode* nodes, const GpuBlasDesc& d, int blasStackSize) {
     const int n = d.NodeCount;
     if (n < 4 || (n & 1)) return "idkpt_set_scene: BLAS node count must be even and >= 4";
@@ -427,32 +512,32 @@ extern "C" {
 
 IDKPT_API uint32_t idkpt_abi_version(void) { return IDKPT_ABI_VERSION; }
 
-IDKPT_API const char* idkpt_last_error(IdkPtCtx* ctx) { return ctx ? ctx->lastError.c_str() : g_createError.c_str(); }
+IDKPT_API const char* idkpt_last_error(IdkPtCtx* ctx) { return ctx ? ctx->lastError.c_str() : IdkPtCtx::createError.c_str(); }
 
 IDKPT_API int idkpt_create(const IdkPtCreateInfo* ci, IdkPtCtx** out) {
-    if (!ci || !out) return fail(nullptr, IDKPT_ERR_INVALID_ARGUMENT, "idkpt_create: null argument");
+    if (!ci || !out) return fail<IdkPtCtx>(nullptr, IDKPT_ERR_INVALID_ARGUMENT, "idkpt_create: null argument");
     *out = nullptr;
     if (ci->Width <= 0 || ci->Height <= 0 || ci->Width > 4096 * 4 || ci->Height > 4096 * 4)
-        return fail(nullptr, IDKPT_ERR_INVALID_ARGUMENT, "idkpt_create: invalid image size");
+        return fail<IdkPtCtx>(nullptr, IDKPT_ERR_INVALID_ARGUMENT, "idkpt_create: invalid image size");
     int stripe = ci->TileStripeHeight > 0 ? ci->TileStripeHeight : 8;
     int tcount = ci->TileCount > 1 ? ci->TileCount : 1;
     if ((ci->Flags & IDKPT_CREATE_GLOBAL_SLOTS) && tcount > 1 && (ci->Height + stripe - 1) / stripe > IDK_MAX_STRIPES)
-        return fail(nullptr, IDKPT_ERR_UNSUPPORTED, "idkpt_create: IDKPT_CREATE_GLOBAL_SLOTS supports at most 4096 stripes (raise TileStripeHeight)");
+        return fail<IdkPtCtx>(nullptr, IDKPT_ERR_UNSUPPORTED, "idkpt_create: IDKPT_CREATE_GLOBAL_SLOTS supports at most 4096 stripes (raise TileStripeHeight)");
     if (tcount > 1 && (ci->TileIndex < 0 || ci->TileIndex >= tcount))
-        return fail(nullptr, IDKPT_ERR_INVALID_ARGUMENT, "idkpt_create: TileIndex out of range");
+        return fail<IdkPtCtx>(nullptr, IDKPT_ERR_INVALID_ARGUMENT, "idkpt_create: TileIndex out of range");
     int deviceCount = 0;
     cudaError_t e = cudaGetDeviceCount(&deviceCount);
     if (e != cudaSuccess || deviceCount == 0)
-        return fail(nullptr, IDKPT_ERR_NO_DEVICE, "idkpt_create: no CUDA device (libidkpt has no CPU fallback)");
+        return fail<IdkPtCtx>(nullptr, IDKPT_ERR_NO_DEVICE, "idkpt_create: no CUDA device (libidkpt has no CPU fallback)");
     if (ci->Device < 0 || ci->Device >= deviceCount)
-        return fail(nullptr, IDKPT_ERR_INVALID_ARGUMENT, "idkpt_create: device ordinal out of range");
-    if (cudaSetDevice(ci->Device) != cudaSuccess) return fail(nullptr, IDKPT_ERR_CUDA, "idkpt_create: cudaSetDevice failed");
+        return fail<IdkPtCtx>(nullptr, IDKPT_ERR_INVALID_ARGUMENT, "idkpt_create: device ordinal out of range");
+    if (cudaSetDevice(ci->Device) != cudaSuccess) return fail<IdkPtCtx>(nullptr, IDKPT_ERR_CUDA, "idkpt_create: cudaSetDevice failed");
     cudaDeviceProp prop;
-    if (cudaGetDeviceProperties(&prop, ci->Device) != cudaSuccess) return fail(nullptr, IDKPT_ERR_CUDA, "idkpt_create: cudaGetDeviceProperties failed");
+    if (cudaGetDeviceProperties(&prop, ci->Device) != cudaSuccess) return fail<IdkPtCtx>(nullptr, IDKPT_ERR_CUDA, "idkpt_create: cudaGetDeviceProperties failed");
     if (prop.major != 9 || prop.minor != 0) {
         char buf[512];
         snprintf(buf, sizeof(buf), "idkpt_create: device '%s' is sm_%d%d; libidkpt is built for sm_90a only", prop.name, prop.major, prop.minor);
-        return fail(nullptr, IDKPT_ERR_NO_DEVICE, buf);
+        return fail<IdkPtCtx>(nullptr, IDKPT_ERR_NO_DEVICE, buf);
     }
     IdkPtCtx* ctx = new IdkPtCtx();
     ctx->device = ci->Device;
@@ -462,10 +547,6 @@ IDKPT_API int idkpt_create(const IdkPtCreateInfo* ci, IdkPtCtx** out) {
     ctx->stripeH = stripe;
     ctx->tileIndex = tcount > 1 ? ci->TileIndex : 0;
     ctx->tileCount = tcount;
-    if (cudaStreamCreateWithFlags(&ctx->stream, cudaStreamNonBlocking) != cudaSuccess) {
-        delete ctx;
-        return fail(nullptr, IDKPT_ERR_CUDA, "idkpt_create: cudaStreamCreate failed");
-    }
     if (const int fl = (ci->Flags >> 8) & 15) ctx->laneCount = std::min(IDK_MAX_LANES, fl);   // IDKPT_CREATE_LANES(n)
     ctx->globalSlots = (ci->Flags & IDKPT_CREATE_GLOBAL_SLOTS) != 0;
     if (const char* v = getenv("IDKPT_LANES")) ctx->laneCount = std::max(1, std::min(IDK_MAX_LANES, atoi(v)));
@@ -474,9 +555,10 @@ IDKPT_API int idkpt_create(const IdkPtCreateInfo* ci, IdkPtCtx** out) {
     if (const char* v = getenv("IDKPT_GATHER_TIMEOUT_MS")) ctx->gatherTimeoutMs = std::max(1.0, atof(v));
     ctx->clockKHz = prop.clockRate;
     compute_tile_rows(ctx);
-    int rc = allocate_wavefront(ctx);
+    int rc = create_stream(ctx);
+    if (rc == IDKPT_OK) rc = allocate_wavefront(ctx);
     if (rc != IDKPT_OK) {
-        g_createError = ctx->lastError;
+        IdkPtCtx::createError = ctx->lastError;
         idkpt_destroy(ctx);
         return rc;
     }
@@ -492,7 +574,7 @@ IDKPT_API void idkpt_destroy(IdkPtCtx* ctx) {
     DevBuf* all[] = {&ctx->nodes, &ctx->triRec, &ctx->blasTris, &ctx->positions, &ctx->descs, &ctx->instances, &ctx->xforms,
                      &ctx->meshes, &ctx->materials, &ctx->vertices, &ctx->lights, &ctx->tlas, &ctx->vtxFrame, &ctx->surfRec,
                      &ctx->images[0], &ctx->images[1], &ctx->images[2], &ctx->counters, &ctx->countLog, &ctx->skyFaces,
-                     &ctx->texPixels, &ctx->texRecs, &ctx->srgbLut, &ctx->bloomDown, &ctx->bloomUp, &ctx->postConsts, &ctx->ldr,
+                     &ctx->tex.pixels, &ctx->tex.recs, &ctx->tex.srgbLut, &ctx->bloomDown, &ctx->bloomUp, &ctx->postConsts, &ctx->ldr,
                      &ctx->unskinned, &ctx->joints, &ctx->refitParents, &ctx->refitLocks, &ctx->scratch[0], &ctx->scratch[1], &ctx->scratch[2],
                      &ctx->tlasScratch, &ctx->oidn[0], &ctx->oidn[1], &ctx->oidn[2], &ctx->oidn[3], &ctx->denoiseWork[0], &ctx->denoiseWork[1], &ctx->denoised};
     for (DevBuf* b : all) release(*b);
@@ -503,7 +585,7 @@ IDKPT_API void idkpt_destroy(IdkPtCtx* ctx) {
     if (ctx->snapDone) cudaEventDestroy(ctx->snapDone);
     if (ctx->copyDone) cudaEventDestroy(ctx->copyDone);
     release(ctx->presentSnap);
-    if (ctx->stream) cudaStreamDestroy(ctx->stream);
+    destroy_stream(ctx);
     delete ctx;
 }
 
@@ -511,52 +593,25 @@ IDKPT_API int idkpt_set_scene(IdkPtCtx* ctx, const IdkPtSceneDesc* s) {
     if (!ctx || !s) return fail(ctx, IDKPT_ERR_INVALID_ARGUMENT, "idkpt_set_scene: null argument");
     DRAIN_PENDING("idkpt_set_scene");
     CK(cudaSetDevice(ctx->device));
-    if (!s->BlasNodes || !s->BlasTriangles || !s->BlasDescs || !s->BlasInstances || !s->MeshTransforms || !s->Meshes ||
-        !s->Materials || !s->Vertices || !s->VertexPositions)
-        return fail(ctx, IDKPT_ERR_INVALID_ARGUMENT, "idkpt_set_scene: a required array is null");
-    if (s->LightCount > IDK_GPU_MAX_UBO_LIGHT_COUNT) return fail(ctx, IDKPT_ERR_INVALID_ARGUMENT, "idkpt_set_scene: more than 256 lights");
+    if (!s->BlasNodes) return fail(ctx, IDKPT_ERR_INVALID_ARGUMENT, "idkpt_set_scene: a required array is null");
+    if (int rc = validate_scene(ctx, "idkpt_set_scene", s)) return rc;
     if (s->UseTlas) {
-        // TLAS.AllocateRequiredNodes: 2n-1 nodes, root at 0, children adjacent (TLAS.cs:266-269)
+        // TLAS.AllocateRequiredNodes: 2n-1 nodes, root at 0 (TLAS.cs:266-269)
         if (!s->TlasNodes || s->BlasInstanceCount == 0 || s->TlasNodeCount != 2 * s->BlasInstanceCount - 1)
             return fail(ctx, IDKPT_ERR_INVALID_ARGUMENT, "idkpt_set_scene: UseTlas needs 2*instances-1 TLAS nodes");
-        for (uint64_t i = 0; i < s->TlasNodeCount; i++) {
-            const uint32_t w = s->TlasNodes[i].IsLeafAndChildOrInstanceId, id = w & 0x7FFFFFFFu;
-            if ((w >> 31) ? (id >= s->BlasInstanceCount) : (id <= i || (uint64_t)id + 1 >= s->TlasNodeCount))
-                return fail(ctx, IDKPT_ERR_INVALID_ARGUMENT, "idkpt_set_scene: malformed TLAS node (child / instance id out of range)");
-        }
+        if (!tlas_nodes_valid(s->TlasNodes, 0, s->TlasNodeCount, s->TlasNodeCount, s->BlasInstanceCount))
+            return fail(ctx, IDKPT_ERR_INVALID_ARGUMENT, "idkpt_set_scene: malformed TLAS node (child / instance id out of range)");
         if (tlas_height(s->TlasNodes, s->TlasNodeCount) > IDK_TLAS_STACK_SIZE)
             return fail(ctx, IDKPT_ERR_UNSUPPORTED, "idkpt_set_scene: TLAS deeper than the 24-entry traversal stack of the TLAS walk (BVHIntersect.glsl:4)");
     }
     if (s->BlasTriangleCount >= (1ull << 31) || s->BlasNodeCount >= (1ull << 31)) return fail(ctx, IDKPT_ERR_INVALID_ARGUMENT, "idkpt_set_scene: scene too large");
-    // validate indices the kernels will chase (a bad host array must not become a device fault)
-    for (uint64_t i = 0; i < s->BlasInstanceCount; i++) {
-        if (s->BlasInstances[i].BlasId >= s->BlasDescCount || s->BlasInstances[i].MeshTransformId >= s->MeshTransformCount)
-            return fail(ctx, IDKPT_ERR_INVALID_ARGUMENT, "idkpt_set_scene: BlasInstance references a missing BLAS or transform");
-    }
     for (uint64_t i = 0; i < s->BlasDescCount; i++) {
         const GpuBlasDesc& d = s->BlasDescs[i];
-        if (d.NodeOffset < 0 || d.NodeCount < 4 || (uint64_t)d.NodeOffset + d.NodeCount > s->BlasNodeCount || d.TriangleOffset < 0 ||
-            (uint64_t)d.TriangleOffset + d.TriangleCount > s->BlasTriangleCount)
-            return fail(ctx, IDKPT_ERR_INVALID_ARGUMENT, "idkpt_set_scene: GpuBlasDesc range outside the node/triangle arrays");
+        if (d.NodeOffset < 0 || d.NodeCount < 4 || (uint64_t)d.NodeOffset + d.NodeCount > s->BlasNodeCount)
+            return fail(ctx, IDKPT_ERR_INVALID_ARGUMENT, "idkpt_set_scene: GpuBlasDesc range outside the node array");
         if (d.RequiredStackSize > s->BlasStackSize)
             return fail(ctx, IDKPT_ERR_INVALID_ARGUMENT, "idkpt_set_scene: BlasStackSize smaller than a BLAS's RequiredStackSize");
         if (const char* err = validate_blas(s->BlasNodes + d.NodeOffset, d, s->BlasStackSize)) return fail(ctx, IDKPT_ERR_INVALID_ARGUMENT, err);
-    }
-    for (uint64_t i = 0; i < s->MeshCount; i++)
-        if (s->Meshes[i].MaterialId < 0 || (uint64_t)s->Meshes[i].MaterialId >= s->MaterialCount)
-            return fail(ctx, IDKPT_ERR_INVALID_ARGUMENT, "idkpt_set_scene: GpuMesh.MaterialId out of range");
-    if (const char* terr = idk_validate_textures(s)) {
-        ctx->lastError = std::string("idkpt_set_scene: ") + terr;
-        return strstr(terr, "not supported") ? IDKPT_ERR_UNSUPPORTED : IDKPT_ERR_INVALID_ARGUMENT;
-    }
-
-    // triangle vertex ids must index the position / vertex arrays
-    // (checked on the host copy: cheap relative to the BVH build that produced it)
-    for (uint64_t i = 0; i < s->BlasTriangleCount; i++) {
-        const GpuBlasTriangle& t = s->BlasTriangles[i];
-        const uint64_t lim = std::min(s->VertexPositionCount, s->VertexCount);
-        if ((uint64_t)(uint32_t)t.X >= lim || (uint64_t)(uint32_t)t.Y >= lim || (uint64_t)(uint32_t)t.Z >= lim || t.MeshId < 0 || (uint64_t)t.MeshId >= s->MeshCount)
-            return fail(ctx, IDKPT_ERR_INVALID_ARGUMENT, "idkpt_set_scene: GpuBlasTriangle index out of range");
     }
     if ((size_t)std::max(1, s->BlasStackSize) * IDK_BLOCK * sizeof(uint32_t) > 200 * 1024)
         return fail(ctx, IDKPT_ERR_UNSUPPORTED, "BlasStackSize too large for the shared-memory traversal stack");
@@ -581,7 +636,7 @@ IDKPT_API int idkpt_set_scene(IdkPtCtx* ctx, const IdkPtSceneDesc* s) {
     if ((rc = upload(ctx, ctx->vertices, s->Vertices, s->VertexCount * sizeof(GpuVertex)))) return rc;
     if ((rc = upload(ctx, ctx->lights, s->Lights, s->LightCount * sizeof(GpuLight)))) return rc;
     if ((rc = upload(ctx, ctx->tlas, s->TlasNodes, s->UseTlas ? s->TlasNodeCount * sizeof(GpuTlasNode) : 0))) return rc;
-    if ((rc = upload_textures(ctx, s->Textures, s->TextureCount))) return rc;
+    if ((rc = upload_textures(ctx, ctx->tex, s->Textures, s->TextureCount))) return rc;
     ctx->hostMaterialMaxHandle.assign(s->MaterialCount, 0);
     for (uint64_t i = 0; i < s->MaterialCount; i++) ctx->hostMaterialMaxHandle[i] = material_max_handle(s->Materials[i]);
 
@@ -623,9 +678,9 @@ IDKPT_API int idkpt_set_scene(IdkPtCtx* ctx, const IdkPtSceneDesc* s) {
     sc.useTlas = s->UseTlas ? 1 : 0;
     sc.vtxFrame = (const float4*)ctx->vtxFrame.p;
     sc.surfRec = (const float4*)ctx->surfRec.p;
-    sc.textures = (const TexRec*)ctx->texRecs.p;
+    sc.textures = (const TexRec*)ctx->tex.recs.p;
     sc.textureCount = (uint32_t)s->TextureCount;
-    sc.srgbLut = (const float*)ctx->srgbLut.p;
+    sc.srgbLut = (const float*)ctx->tex.srgbLut.p;
     ctx->counts = *s;
     ctx->hostDescs.assign(s->BlasDescs, s->BlasDescs + s->BlasDescCount);
     ctx->nodeBytes = nodeBytes;
@@ -685,11 +740,8 @@ IDKPT_API int idkpt_update_range(IdkPtCtx* ctx, IdkPtArrayId which, uint64_t fir
     }
     if (which == IDKPT_ARRAY_TLAS_NODES) {
         const GpuTlasNode* t = (const GpuTlasNode*)data;
-        for (uint64_t i = 0; i < count; i++) {
-            const uint32_t w = t[i].IsLeafAndChildOrInstanceId, id = w & 0x7FFFFFFFu;
-            if ((w >> 31) ? (id >= ctx->counts.BlasInstanceCount) : (id <= first + i || (uint64_t)id + 1 >= ctx->counts.TlasNodeCount))
-                return fail(ctx, IDKPT_ERR_INVALID_ARGUMENT, "idkpt_update_range: malformed TLAS node (child / instance id out of range)");
-        }
+        if (!tlas_nodes_valid(t, first, count, ctx->counts.TlasNodeCount, ctx->counts.BlasInstanceCount))
+            return fail(ctx, IDKPT_ERR_INVALID_ARGUMENT, "idkpt_update_range: malformed TLAS node (child / instance id out of range)");
         if (first == 0 && count == ctx->counts.TlasNodeCount && tlas_height(t, count) > IDK_TLAS_STACK_SIZE)
             return fail(ctx, IDKPT_ERR_UNSUPPORTED, "idkpt_update_range: TLAS deeper than the 24-entry traversal stack of the TLAS walk (BVHIntersect.glsl:4)");
     }
@@ -740,16 +792,16 @@ IDKPT_API int idkpt_set_textures(IdkPtCtx* ctx, const IdkPtTextureDesc* textures
     if (!ctx->haveScene) return fail(ctx, IDKPT_ERR_NO_SCENE, "idkpt_set_textures: no scene");
     IdkPtSceneDesc tmp = {};
     tmp.Textures = textures; tmp.TextureCount = count;
-    if (const char* terr = idk_validate_textures(&tmp)) {
-        ctx->lastError = std::string("idkpt_set_textures: ") + terr;
-        return strstr(terr, "not supported") ? IDKPT_ERR_UNSUPPORTED : IDKPT_ERR_INVALID_ARGUMENT;
-    }
+    if (const char* terr = idk_validate_textures(&tmp)) return texture_error(ctx, "idkpt_set_textures", terr);
     for (uint64_t h : ctx->hostMaterialMaxHandle)
         if (h > count) return fail(ctx, IDKPT_ERR_INVALID_ARGUMENT, "idkpt_set_textures: a material references a texture beyond the new table");
     CK(cudaSetDevice(ctx->device));
     CK(cudaStreamSynchronize(ctx->stream));
-    int rc = upload_textures(ctx, textures, count);
+    int rc = upload_textures(ctx, ctx->tex, textures, count);
     if (rc) return rc;
+    ctx->sc.textures = (const TexRec*)ctx->tex.recs.p;
+    ctx->sc.textureCount = (uint32_t)count;
+    ctx->sc.srgbLut = (const float*)ctx->tex.srgbLut.p;
     ctx->counts.TextureCount = count;
     ctx->accumulatedSamples = 0;
     return IDKPT_OK;
@@ -1160,36 +1212,20 @@ IDKPT_API int idkpt_present_async(IdkPtCtx* ctx, IdkPtImage which, void* dstHost
     if ((int)which < 0 || (int)which > 3) return fail(ctx, IDKPT_ERR_INVALID_ARGUMENT, "idkpt_present_async: unknown image");
     if (bytes < (uint64_t)ctx->width * ctx->height * 16) return fail(ctx, IDKPT_ERR_INVALID_ARGUMENT, "idkpt_present_async: buffer smaller than width*height*16");
     CK(cudaSetDevice(ctx->device));
-    if ((int)which == 3) {
-        // IDKPT_IMAGE_GATHERED: the full multi-GPU frame. Snapshot it on the main stream first: with several frames in flight
-        // a peer may start scattering frame k+2 into this buffer as soon as every rank has finished frame k+1, and that is
-        // ordered after this snapshot (main stream: wait(k) -> snapshot(k) -> scatter(k+1)) but not after a slow D2H copy.
-        if (ctx->gatherWorld < 2 || ctx->gatherCurrent < 0) return fail(ctx, IDKPT_ERR_INVALID_ARGUMENT, "idkpt_present_async: no gathered frame yet");
-        if (!ctx->copyStream) {
-            CK(cudaStreamCreateWithFlags(&ctx->copyStream, cudaStreamNonBlocking));
-            CK(cudaEventCreateWithFlags(&ctx->snapDone, cudaEventDisableTiming));
-            CK(cudaEventCreateWithFlags(&ctx->copyDone, cudaEventDisableTiming));
-        }
-        const size_t full = (size_t)ctx->width * ctx->height * 16;
-        CK(ensure(ctx->presentSnap, full));
-        if (ctx->copyPending) CK(cudaStreamWaitEvent(ctx->stream, ctx->copyDone, 0));   // previous transfer still reads the snapshot
-        CK(cudaMemcpyAsync(ctx->presentSnap.p, ctx->gatherImage[ctx->gatherCurrent].p, full, cudaMemcpyDeviceToDevice, ctx->stream));
-        CK(cudaEventRecord(ctx->snapDone, ctx->stream));
-        CK(cudaStreamWaitEvent(ctx->copyStream, ctx->snapDone, 0));
-        CK(cudaMemcpyAsync(dstHost, ctx->presentSnap.p, full, cudaMemcpyDeviceToHost, ctx->copyStream));
-        CK(cudaEventRecord(ctx->copyDone, ctx->copyStream));
-        ctx->copyPending = true;
-        return IDKPT_OK;
-    }
+    // IDKPT_IMAGE_GATHERED is the full multi-GPU frame. It is snapshot on the main stream too: with several frames in flight a
+    // peer may start scattering frame k+2 into this buffer as soon as every rank has finished frame k+1, and that is ordered
+    // after this snapshot (main stream: wait(k) -> snapshot(k) -> scatter(k+1)) but not after a slow D2H copy.
+    const bool gathered = (int)which == 3;
+    if (gathered && (ctx->gatherWorld < 2 || ctx->gatherCurrent < 0)) return fail(ctx, IDKPT_ERR_INVALID_ARGUMENT, "idkpt_present_async: no gathered frame yet");
     if (!ctx->copyStream) {
         CK(cudaStreamCreateWithFlags(&ctx->copyStream, cudaStreamNonBlocking));
         CK(cudaEventCreateWithFlags(&ctx->snapDone, cudaEventDisableTiming));
         CK(cudaEventCreateWithFlags(&ctx->copyDone, cudaEventDisableTiming));
     }
-    const size_t n = (size_t)ctx->nLocal * 16;
+    const size_t n = gathered ? (size_t)ctx->width * ctx->height * 16 : (size_t)ctx->nLocal * 16;
     CK(ensure(ctx->presentSnap, std::max<size_t>(n, 16)));
     if (ctx->copyPending) CK(cudaStreamWaitEvent(ctx->stream, ctx->copyDone, 0));   // previous transfer still reads the snapshot
-    CK(cudaMemcpyAsync(ctx->presentSnap.p, ctx->images[which].p, n, cudaMemcpyDeviceToDevice, ctx->stream));
+    CK(cudaMemcpyAsync(ctx->presentSnap.p, gathered ? ctx->gatherImage[ctx->gatherCurrent].p : ctx->images[which].p, n, cudaMemcpyDeviceToDevice, ctx->stream));
     CK(cudaEventRecord(ctx->snapDone, ctx->stream));
     CK(cudaStreamWaitEvent(ctx->copyStream, ctx->snapDone, 0));
     // The tile's rows are stored compactly, stripe after stripe; in the full-frame host layout its stripes are tileCount stripes
@@ -1197,7 +1233,9 @@ IDKPT_API int idkpt_present_async(IdkPtCtx* ctx, IdkPtImage which, void* dstHost
     // With a host frame shared by all ranks (idkpt_register_host_buffer on the same mapping in every process) each GPU
     // delivers its own 1/N of the frame over its own PCIe link -- no rank has to download the whole gathered image.
     const size_t rowBytes = (size_t)ctx->width * 16;
-    if (!ctx->rows.empty()) {
+    if (gathered) {
+        CK(cudaMemcpyAsync(dstHost, ctx->presentSnap.p, n, cudaMemcpyDeviceToHost, ctx->copyStream));
+    } else if (!ctx->rows.empty()) {
         const size_t stripeBytes = (size_t)ctx->stripeH * rowBytes;
         const size_t fullStripes = ctx->rows.size() / (size_t)ctx->stripeH, tailRows = ctx->rows.size() % (size_t)ctx->stripeH;
         char* h0 = (char*)dstHost + (size_t)ctx->rows[0] * rowBytes;
@@ -1463,59 +1501,51 @@ IDKPT_API int idkpt_post_process(IdkPtCtx* ctx, const IdkPtPostSettings* s, IdkP
     CK(cudaSetDevice(ctx->device));
     CK(ensure(ctx->ldr, (size_t)w * h * 4));
     CK(ensure(ctx->postConsts, sizeof(PostTonemapConsts)));
-    cudaEvent_t e0, e1;
-    CK(cudaEventCreate(&e0)); CK(cudaEventCreate(&e1));
-    cudaEventRecord(e0, ctx->stream);
     const dim3 blk(256);
     auto grid = [](int gw, int gh) { return dim3((unsigned)((gw + 31) / 32), (unsigned)((gh + 7) / 8)); };
-    PostImage bloomResult = {nullptr, nullptr, 0, 0};
-    if (s->IsBloom) {
-        // Bloom.SetSize (Bloom.cs:132-150): half resolution, levels = max(MaxMipmapLevel - MinusLods, 2); the upsample chain has one level less
-        const int w2 = w / 2, h2 = h / 2;
-        const int levels = std::max(ilogb_int(std::max(w2, h2)) + 1 - s->BloomMinusLods, 2);
-        std::vector<size_t> off(levels + 1, 0);
-        std::vector<int> lw(levels), lh(levels);
-        for (int l = 0; l < levels; l++) {
-            lw[l] = std::max(1, w2 / (1 << std::min(l, 30))); lh[l] = std::max(1, h2 / (1 << std::min(l, 30)));
-            off[l + 1] = off[l] + (size_t)lw[l] * lh[l];
+    return run_timed(ctx, "idkpt_post_process", kernelMs, [&]() -> int {
+        PostImage bloomResult = {nullptr, nullptr, 0, 0};
+        if (s->IsBloom) {
+            // Bloom.SetSize (Bloom.cs:132-150): half resolution, levels = max(MaxMipmapLevel - MinusLods, 2); the upsample chain has one level less
+            const int w2 = w / 2, h2 = h / 2;
+            const int levels = std::max(ilogb_int(std::max(w2, h2)) + 1 - s->BloomMinusLods, 2);
+            std::vector<size_t> off(levels + 1, 0);
+            std::vector<int> lw(levels), lh(levels);
+            for (int l = 0; l < levels; l++) {
+                lw[l] = std::max(1, w2 / (1 << std::min(l, 30))); lh[l] = std::max(1, h2 / (1 << std::min(l, 30)));
+                off[l + 1] = off[l] + (size_t)lw[l] * lh[l];
+            }
+            cudaError_t ce = ensure(ctx->bloomDown, off[levels] * 8);
+            if (ce == cudaSuccess) ce = ensure(ctx->bloomUp, off[levels - 1] * 8);
+            if (ce != cudaSuccess) return fail(ctx, IDKPT_ERR_OUT_OF_MEMORY, "idkpt_post_process: bloom allocation failed");
+            uint2* down = (uint2*)ctx->bloomDown.p;
+            uint2* up = (uint2*)ctx->bloomUp.p;
+            for (int l = 0; l < levels; l++) {
+                BloomDownArgs a;
+                a.src = l == 0 ? PostImage{src, nullptr, w, h} : PostImage{nullptr, down + off[l - 1], lw[l - 1], lh[l - 1]};
+                a.dst = down + off[l]; a.dw = lw[l]; a.dh = lh[l];
+                a.prefilter = l == 0; a.maxColor = s->BloomMaxColor; a.threshold = s->BloomThreshold;
+                k_bloom_down<<<grid(a.dw, a.dh), blk, 0, ctx->stream>>>(a);
+            }
+            for (int l = levels - 2; l >= 0; l--) {
+                BloomUpArgs a;
+                a.up = l == levels - 2 ? PostImage{nullptr, down + off[l + 1], lw[l + 1], lh[l + 1]} : PostImage{nullptr, up + off[l + 1], lw[l + 1], lh[l + 1]};
+                a.down = PostImage{nullptr, down + off[l + 1], lw[l + 1], lh[l + 1]};
+                a.dst = up + off[l]; a.dw = lw[l]; a.dh = lh[l];
+                k_bloom_up<<<grid(a.dw, a.dh), blk, 0, ctx->stream>>>(a);
+            }
+            bloomResult = PostImage{nullptr, up, lw[0], lh[0]};
         }
-        cudaError_t ce = ensure(ctx->bloomDown, off[levels] * 8);
-        if (ce == cudaSuccess) ce = ensure(ctx->bloomUp, off[levels - 1] * 8);
-        if (ce != cudaSuccess) { cudaEventDestroy(e0); cudaEventDestroy(e1); return fail(ctx, IDKPT_ERR_OUT_OF_MEMORY, "idkpt_post_process: bloom allocation failed"); }
-        uint2* down = (uint2*)ctx->bloomDown.p;
-        uint2* up = (uint2*)ctx->bloomUp.p;
-        for (int l = 0; l < levels; l++) {
-            BloomDownArgs a;
-            a.src = l == 0 ? PostImage{src, nullptr, w, h} : PostImage{nullptr, down + off[l - 1], lw[l - 1], lh[l - 1]};
-            a.dst = down + off[l]; a.dw = lw[l]; a.dh = lh[l];
-            a.prefilter = l == 0; a.maxColor = s->BloomMaxColor; a.threshold = s->BloomThreshold;
-            k_bloom_down<<<grid(a.dw, a.dh), blk, 0, ctx->stream>>>(a);
-        }
-        for (int l = levels - 2; l >= 0; l--) {
-            BloomUpArgs a;
-            a.up = l == levels - 2 ? PostImage{nullptr, down + off[l + 1], lw[l + 1], lh[l + 1]} : PostImage{nullptr, up + off[l + 1], lw[l + 1], lh[l + 1]};
-            a.down = PostImage{nullptr, down + off[l + 1], lw[l + 1], lh[l + 1]};
-            a.dst = up + off[l]; a.dw = lw[l]; a.dh = lh[l];
-            k_bloom_up<<<grid(a.dw, a.dh), blk, 0, ctx->stream>>>(a);
-        }
-        bloomResult = PostImage{nullptr, up, lw[0], lh[0]};
-    }
-    k_agx_matrices<<<1, 1, 0, ctx->stream>>>(s->Exposure, s->Compression, (PostTonemapConsts*)ctx->postConsts.p);
-    TonemapArgs t;
-    t.src0 = PostImage{src, nullptr, w, h};
-    t.src1 = bloomResult;
-    t.dst = (uchar4*)ctx->ldr.p; t.w = w; t.h = h;
-    t.saturation = s->Saturation; t.linear = s->Linear; t.peak = s->Peak; t.doTonemap = s->DoTonemapAndSrgbTransform ? 1 : 0;
-    t.consts = (const PostTonemapConsts*)ctx->postConsts.p;
-    k_tonemap<<<grid(w, h), blk, 0, ctx->stream>>>(t);
-    cudaEventRecord(e1, ctx->stream);
-    if (rgba8Out) cudaMemcpyAsync(rgba8Out, ctx->ldr.p, (size_t)w * h * 4, cudaMemcpyDeviceToHost, ctx->stream);
-    cudaError_t e = cudaStreamSynchronize(ctx->stream);
-    if (e == cudaSuccess) e = cudaGetLastError();
-    if (e == cudaSuccess && kernelMs) cudaEventElapsedTime(kernelMs, e0, e1);
-    cudaEventDestroy(e0); cudaEventDestroy(e1);
-    if (e != cudaSuccess) { ctx->lastError = std::string("idkpt_post_process: ") + cudaGetErrorString(e); return IDKPT_ERR_CUDA; }
-    return IDKPT_OK;
+        k_agx_matrices<<<1, 1, 0, ctx->stream>>>(s->Exposure, s->Compression, (PostTonemapConsts*)ctx->postConsts.p);
+        TonemapArgs t;
+        t.src0 = PostImage{src, nullptr, w, h};
+        t.src1 = bloomResult;
+        t.dst = (uchar4*)ctx->ldr.p; t.w = w; t.h = h;
+        t.saturation = s->Saturation; t.linear = s->Linear; t.peak = s->Peak; t.doTonemap = s->DoTonemapAndSrgbTransform ? 1 : 0;
+        t.consts = (const PostTonemapConsts*)ctx->postConsts.p;
+        k_tonemap<<<grid(w, h), blk, 0, ctx->stream>>>(t);
+        return IDKPT_OK;
+    }, rgba8Out, ctx->ldr.p, (size_t)w * h * 4);
 }
 
 IDKPT_API int idkpt_ldr_device_ptr(IdkPtCtx* ctx, void** devPtr, uint64_t* bytes) {
@@ -1547,40 +1577,34 @@ IDKPT_API int idkpt_denoise(IdkPtCtx* ctx, const IdkPtDenoiseSettings* s, float*
     int rc = denoise_alloc(ctx);
     if (rc) return rc;
     const int w = ctx->width, h = ctx->height, n = w * h;
-    cudaEvent_t e0, e1;
-    CK(cudaEventCreate(&e0)); CK(cudaEventCreate(&e1));
-    cudaEventRecord(e0, ctx->stream);
-    DenoisePrepareArgs pa;
-    pa.result = (const float4*)ctx->images[0].p; pa.albedo = (const float4*)ctx->images[1].p; pa.normal = (const float4*)ctx->images[2].p;
-    pa.oidnBeauty = (float*)ctx->oidn[0].p; pa.oidnAlbedo = (float*)ctx->oidn[1].p; pa.oidnNormal = (float*)ctx->oidn[2].p;
-    pa.work = (float4*)ctx->denoiseWork[0].p; pa.count = n; pa.demodulate = s->Demodulate ? 1 : 0;
-    k_denoise_prepare<<<(n + 255) / 256, 256, 0, ctx->stream>>>(pa);
-    int cur = 0;
-    for (int it = 0; it < s->Iterations; it++) {
-        const int step = 1 << it;
-        const float sc = s->SigmaColor / (float)step;
-        DenoiseAtrousArgs a;
-        a.in = (const float4*)ctx->denoiseWork[cur].p; a.out = (float4*)ctx->denoiseWork[cur ^ 1].p;
-        a.albedo = pa.albedo; a.normal = pa.normal; a.w = w; a.h = h; a.step = step;
-        a.invSigmaColor2 = 1.0f / (sc * sc); a.invSigmaNormal2 = 1.0f / (s->SigmaNormal * s->SigmaNormal);
-        a.invSigmaAlbedo2 = 1.0f / (s->SigmaAlbedo * s->SigmaAlbedo); a.invStep2 = 1.0f / ((float)step * (float)step);
-        k_denoise_atrous<<<dim3((unsigned)((w + 31) / 32), (unsigned)((h + 7) / 8)), 256, 0, ctx->stream>>>(a);
-        cur ^= 1;
-    }
-    if (s->Iterations > 0) {
-        DenoiseFinishArgs fa;
-        fa.filtered = (const float4*)ctx->denoiseWork[cur].p; fa.albedo = pa.albedo; fa.denoised = (float4*)ctx->denoised.p;
-        fa.oidnOutput = (float*)ctx->oidn[3].p; fa.count = n; fa.demodulate = pa.demodulate;
-        k_denoise_finish<<<(n + 255) / 256, 256, 0, ctx->stream>>>(fa);
-    }
-    cudaEventRecord(e1, ctx->stream);
-    cudaError_t e = cudaStreamSynchronize(ctx->stream);
-    if (e == cudaSuccess) e = cudaGetLastError();
-    if (e == cudaSuccess && kernelMs) cudaEventElapsedTime(kernelMs, e0, e1);
-    cudaEventDestroy(e0); cudaEventDestroy(e1);
-    if (e != cudaSuccess) { ctx->lastError = std::string("idkpt_denoise: ") + cudaGetErrorString(e); return IDKPT_ERR_CUDA; }
-    if (s->Iterations > 0) ctx->haveDenoised = true;
-    return IDKPT_OK;
+    rc = run_timed(ctx, "idkpt_denoise", kernelMs, [&]() -> int {
+        DenoisePrepareArgs pa;
+        pa.result = (const float4*)ctx->images[0].p; pa.albedo = (const float4*)ctx->images[1].p; pa.normal = (const float4*)ctx->images[2].p;
+        pa.oidnBeauty = (float*)ctx->oidn[0].p; pa.oidnAlbedo = (float*)ctx->oidn[1].p; pa.oidnNormal = (float*)ctx->oidn[2].p;
+        pa.work = (float4*)ctx->denoiseWork[0].p; pa.count = n; pa.demodulate = s->Demodulate ? 1 : 0;
+        k_denoise_prepare<<<(n + 255) / 256, 256, 0, ctx->stream>>>(pa);
+        int cur = 0;
+        for (int it = 0; it < s->Iterations; it++) {
+            const int step = 1 << it;
+            const float sc = s->SigmaColor / (float)step;
+            DenoiseAtrousArgs a;
+            a.in = (const float4*)ctx->denoiseWork[cur].p; a.out = (float4*)ctx->denoiseWork[cur ^ 1].p;
+            a.albedo = pa.albedo; a.normal = pa.normal; a.w = w; a.h = h; a.step = step;
+            a.invSigmaColor2 = 1.0f / (sc * sc); a.invSigmaNormal2 = 1.0f / (s->SigmaNormal * s->SigmaNormal);
+            a.invSigmaAlbedo2 = 1.0f / (s->SigmaAlbedo * s->SigmaAlbedo); a.invStep2 = 1.0f / ((float)step * (float)step);
+            k_denoise_atrous<<<dim3((unsigned)((w + 31) / 32), (unsigned)((h + 7) / 8)), 256, 0, ctx->stream>>>(a);
+            cur ^= 1;
+        }
+        if (s->Iterations > 0) {
+            DenoiseFinishArgs fa;
+            fa.filtered = (const float4*)ctx->denoiseWork[cur].p; fa.albedo = pa.albedo; fa.denoised = (float4*)ctx->denoised.p;
+            fa.oidnOutput = (float*)ctx->oidn[3].p; fa.count = n; fa.demodulate = pa.demodulate;
+            k_denoise_finish<<<(n + 255) / 256, 256, 0, ctx->stream>>>(fa);
+        }
+        return IDKPT_OK;
+    });
+    if (rc == IDKPT_OK && s->Iterations > 0) ctx->haveDenoised = true;
+    return rc;
 }
 
 IDKPT_API int idkpt_denoise_device_ptrs(IdkPtCtx* ctx, void** beauty, void** albedo, void** normal, void** output, uint64_t* bytesEach) {
@@ -1651,25 +1675,19 @@ IDKPT_API int idkpt_skin_vertices(IdkPtCtx* ctx, const float* jointMatrices, uin
     CK(cudaSetDevice(ctx->device));
     int rc;
     if ((rc = upload(ctx, ctx->joints, jointMatrices, jointCount * 48))) return rc;   // jointMatricesBuffer.UploadElements (ModelManager.cs:277)
-    cudaEvent_t e0, e1;
-    CK(cudaEventCreate(&e0)); CK(cudaEventCreate(&e1));
-    cudaEventRecord(e0, ctx->stream);
-    for (uint32_t c = 0; c < cmdCount; c++) {
-        if (!cmds[c].VertexCount) continue;
-        SkinArgs a;
-        a.unskinned = (const uint32_t*)ctx->unskinned.p; a.joints = (const float4*)ctx->joints.p;
-        a.positions = (float*)ctx->positions.p; a.vertices = (uint4*)ctx->vertices.p; a.vtxFrame = (float4*)ctx->vtxFrame.p;
-        a.inOffset = cmds[c].InputVertexOffset; a.outOffset = cmds[c].OutputVertexOffset; a.jointOffset = cmds[c].JointMatricesOffset; a.count = cmds[c].VertexCount;
-        k_skin_vertices<<<(a.count + 255) / 256, 256, 0, ctx->stream>>>(a);
-    }
-    cudaEventRecord(e1, ctx->stream);
-    cudaError_t e = cudaStreamSynchronize(ctx->stream);
-    if (e == cudaSuccess) e = cudaGetLastError();
-    if (e == cudaSuccess && kernelMs) cudaEventElapsedTime(kernelMs, e0, e1);
-    cudaEventDestroy(e0); cudaEventDestroy(e1);
-    if (e != cudaSuccess) { ctx->lastError = std::string("idkpt_skin_vertices: ") + cudaGetErrorString(e); return IDKPT_ERR_CUDA; }
-    ctx->accumulatedSamples = 0;
-    return IDKPT_OK;
+    rc = run_timed(ctx, "idkpt_skin_vertices", kernelMs, [&]() -> int {
+        for (uint32_t c = 0; c < cmdCount; c++) {
+            if (!cmds[c].VertexCount) continue;
+            SkinArgs a;
+            a.unskinned = (const uint32_t*)ctx->unskinned.p; a.joints = (const float4*)ctx->joints.p;
+            a.positions = (float*)ctx->positions.p; a.vertices = (uint4*)ctx->vertices.p; a.vtxFrame = (float4*)ctx->vtxFrame.p;
+            a.inOffset = cmds[c].InputVertexOffset; a.outOffset = cmds[c].OutputVertexOffset; a.jointOffset = cmds[c].JointMatricesOffset; a.count = cmds[c].VertexCount;
+            k_skin_vertices<<<(a.count + 255) / 256, 256, 0, ctx->stream>>>(a);
+        }
+        return IDKPT_OK;
+    });
+    if (rc == IDKPT_OK) ctx->accumulatedSamples = 0;
+    return rc;
 }
 
 IDKPT_API int idkpt_blas_refit(IdkPtCtx* ctx, uint32_t first, uint32_t count, float* kernelMs) {
@@ -1683,28 +1701,22 @@ IDKPT_API int idkpt_blas_refit(IdkPtCtx* ctx, uint32_t first, uint32_t count, fl
     for (uint32_t b = first; b < first + count; b++) maxNodes = std::max(maxNodes, ctx->hostDescs[b].NodeCount);
     CK(ensure(ctx->refitParents, std::max<size_t>((size_t)maxNodes, 4) * 4));   // blasRefitLockBuffer sizing, BVH.cs:451
     CK(ensure(ctx->refitLocks, std::max<size_t>((size_t)maxNodes, 4) * 4));
-    cudaEvent_t e0, e1;
-    CK(cudaEventCreate(&e0)); CK(cudaEventCreate(&e1));
-    cudaEventRecord(e0, ctx->stream);
-    for (uint32_t b = first; b < first + count; b++) {
-        const GpuBlasDesc& d = ctx->hostDescs[b];
-        RefitArgs a;
-        a.nodes = (float4*)ctx->nodes.p + 2 * (size_t)d.NodeOffset;
-        a.blasTris = (const int4*)ctx->blasTris.p; a.positions = (const float*)ctx->positions.p;
-        a.triRec = (float4*)((char*)ctx->nodes.p + ctx->nodeBytes);
-        a.parents = (int32_t*)ctx->refitParents.p; a.locks = (uint32_t*)ctx->refitLocks.p;
-        a.nodeCount = (uint32_t)d.NodeCount; a.triOffset = (uint32_t)d.TriangleOffset; a.triCount = (uint32_t)d.TriangleCount;
-        k_refit_prepare<<<(a.nodeCount + 255) / 256, 256, 0, ctx->stream>>>(a);
-        k_refit_climb<<<(a.nodeCount + 255) / 256, 256, 0, ctx->stream>>>(a);
-    }
-    cudaEventRecord(e1, ctx->stream);
-    cudaError_t e = cudaStreamSynchronize(ctx->stream);
-    if (e == cudaSuccess) e = cudaGetLastError();
-    if (e == cudaSuccess && kernelMs) cudaEventElapsedTime(kernelMs, e0, e1);
-    cudaEventDestroy(e0); cudaEventDestroy(e1);
-    if (e != cudaSuccess) { ctx->lastError = std::string("idkpt_blas_refit: ") + cudaGetErrorString(e); return IDKPT_ERR_CUDA; }
-    ctx->accumulatedSamples = 0;
-    return IDKPT_OK;
+    const int rc = run_timed(ctx, "idkpt_blas_refit", kernelMs, [&]() -> int {
+        for (uint32_t b = first; b < first + count; b++) {
+            const GpuBlasDesc& d = ctx->hostDescs[b];
+            RefitArgs a;
+            a.nodes = (float4*)ctx->nodes.p + 2 * (size_t)d.NodeOffset;
+            a.blasTris = (const int4*)ctx->blasTris.p; a.positions = (const float*)ctx->positions.p;
+            a.triRec = (float4*)((char*)ctx->nodes.p + ctx->nodeBytes);
+            a.parents = (int32_t*)ctx->refitParents.p; a.locks = (uint32_t*)ctx->refitLocks.p;
+            a.nodeCount = (uint32_t)d.NodeCount; a.triOffset = (uint32_t)d.TriangleOffset; a.triCount = (uint32_t)d.TriangleCount;
+            k_refit_prepare<<<(a.nodeCount + 255) / 256, 256, 0, ctx->stream>>>(a);
+            k_refit_climb<<<(a.nodeCount + 255) / 256, 256, 0, ctx->stream>>>(a);
+        }
+        return IDKPT_OK;
+    });
+    if (rc == IDKPT_OK) ctx->accumulatedSamples = 0;
+    return rc;
 }
 
 // BVH.TlasBuild on the device (BVH.cs:278-298, TLAS.cs:28-141): see k_tlas_build.
@@ -1728,16 +1740,11 @@ IDKPT_API int idkpt_tlas_build(IdkPtCtx* ctx, int32_t searchRadius, float* kerne
     a.keys = (uint32_t*)((char*)ctx->tlasScratch.p + keysOff); a.pref = (int*)((char*)ctx->tlasScratch.p + prefOff);
     a.need = (int*)((char*)ctx->tlasScratch.p + needOff);
     a.n = (int)n; a.searchRadius = searchRadius;
-    cudaEvent_t e0, e1;
-    CK(cudaEventCreate(&e0)); CK(cudaEventCreate(&e1));
-    cudaEventRecord(e0, ctx->stream);
-    k_tlas_build<<<1, 1024, 0, ctx->stream>>>(a);
-    cudaEventRecord(e1, ctx->stream);
-    cudaError_t e = cudaStreamSynchronize(ctx->stream);
-    if (e == cudaSuccess) e = cudaGetLastError();
-    if (e == cudaSuccess && kernelMs) cudaEventElapsedTime(kernelMs, e0, e1);
-    cudaEventDestroy(e0); cudaEventDestroy(e1);
-    if (e != cudaSuccess) { ctx->lastError = std::string("idkpt_tlas_build: ") + cudaGetErrorString(e); return IDKPT_ERR_CUDA; }
+    const int rc = run_timed(ctx, "idkpt_tlas_build", kernelMs, [&]() -> int {
+        k_tlas_build<<<1, 1024, 0, ctx->stream>>>(a);
+        return IDKPT_OK;
+    });
+    if (rc) return rc;
     ctx->accumulatedSamples = 0;
     int need = 0;
     CK(cudaMemcpy(&need, a.need, 4, cudaMemcpyDeviceToHost));
@@ -1768,16 +1775,6 @@ IDKPT_API int idkpt_read_range(IdkPtCtx* ctx, IdkPtArrayId which, uint64_t first
     return IDKPT_OK;
 }
 
-static int trace_rays_impl(IdkPtCtx* ctx, const IdkPtRay* rays, uint64_t count, int32_t traceLights, IdkPtHit* hitsOut, float* kernelMs, bool anyHit);
-
-IDKPT_API int idkpt_trace_rays(IdkPtCtx* ctx, const IdkPtRay* rays, uint64_t count, int32_t traceLights, IdkPtHit* hitsOut, float* kernelMs) {
-    return trace_rays_impl(ctx, rays, count, traceLights, hitsOut, kernelMs, false);
-}
-
-IDKPT_API int idkpt_trace_rays_any(IdkPtCtx* ctx, const IdkPtRay* rays, uint64_t count, int32_t traceLights, IdkPtHit* hitsOut, float* kernelMs) {
-    return trace_rays_impl(ctx, rays, count, traceLights, hitsOut, kernelMs, true);
-}
-
 IDKPT_API int idkpt_shadows_ray_traced(IdkPtCtx* ctx, const GpuPerFrameData* frame, const float* depth, const float* normalRG, int32_t width,
                                        int32_t height, int32_t lightIndex, int32_t samples, uint32_t noiseIndex, const float* taaJitter,
                                        float* visibilityOut, float* kernelMs) {
@@ -1789,31 +1786,21 @@ IDKPT_API int idkpt_shadows_ray_traced(IdkPtCtx* ctx, const GpuPerFrameData* fra
     if (kernelMs) *kernelMs = 0.0f;
     const size_t n = (size_t)width * height;
     DevBuf &dDepth = ctx->scratch[0], &dN = ctx->scratch[1], &dVis = ctx->scratch[2];
-    int rc = IDKPT_OK;
-    cudaEvent_t e0 = nullptr, e1 = nullptr;
-    do {
-        if (ensure(dDepth, n * 4) != cudaSuccess || ensure(dN, n * 8) != cudaSuccess || ensure(dVis, n * 4) != cudaSuccess) { rc = fail(ctx, IDKPT_ERR_OUT_OF_MEMORY, "idkpt_shadows_ray_traced: device allocation failed"); break; }
-        cudaMemcpyAsync(dDepth.p, depth, n * 4, cudaMemcpyHostToDevice, ctx->stream);
-        cudaMemcpyAsync(dN.p, normalRG, n * 8, cudaMemcpyHostToDevice, ctx->stream);
-        cudaMemcpyAsync(dVis.p, visibilityOut, n * 4, cudaMemcpyHostToDevice, ctx->stream);   // pixels with depth == 1 keep the caller's value
-        ShadowArgs a;
-        a.sc = ctx->sc;
-        memcpy(a.invProjView, frame->InvProjView, sizeof(a.invProjView));
-        a.jitter[0] = taaJitter ? taaJitter[0] : 0.0f; a.jitter[1] = taaJitter ? taaJitter[1] : 0.0f;
-        a.depth = (const float*)dDepth.p; a.normalRG = (const float2*)dN.p; a.visibility = (float*)dVis.p;
-        a.width = width; a.height = height; a.lightIndex = lightIndex; a.samples = samples; a.noiseIndex = noiseIndex;
-        cudaEventCreate(&e0); cudaEventCreate(&e1);
-        cudaEventRecord(e0, ctx->stream);
+    if (ensure(dDepth, n * 4) != cudaSuccess || ensure(dN, n * 8) != cudaSuccess || ensure(dVis, n * 4) != cudaSuccess)
+        return fail(ctx, IDKPT_ERR_OUT_OF_MEMORY, "idkpt_shadows_ray_traced: device allocation failed");
+    CK(cudaMemcpyAsync(dDepth.p, depth, n * 4, cudaMemcpyHostToDevice, ctx->stream));
+    CK(cudaMemcpyAsync(dN.p, normalRG, n * 8, cudaMemcpyHostToDevice, ctx->stream));
+    CK(cudaMemcpyAsync(dVis.p, visibilityOut, n * 4, cudaMemcpyHostToDevice, ctx->stream));   // pixels with depth == 1 keep the caller's value
+    ShadowArgs a;
+    a.sc = ctx->sc;
+    memcpy(a.invProjView, frame->InvProjView, sizeof(a.invProjView));
+    a.jitter[0] = taaJitter ? taaJitter[0] : 0.0f; a.jitter[1] = taaJitter ? taaJitter[1] : 0.0f;
+    a.depth = (const float*)dDepth.p; a.normalRG = (const float2*)dN.p; a.visibility = (float*)dVis.p;
+    a.width = width; a.height = height; a.lightIndex = lightIndex; a.samples = samples; a.noiseIndex = noiseIndex;
+    return run_timed(ctx, "idkpt_shadows_ray_traced", kernelMs, [&]() -> int {
         k_shadows_ray_traced<<<ctx->traceRaysBlocks, IDK_BLOCK, ctx->stackBytes, ctx->stream>>>(a);
-        cudaEventRecord(e1, ctx->stream);
-        cudaMemcpyAsync(visibilityOut, dVis.p, n * 4, cudaMemcpyDeviceToHost, ctx->stream);
-        cudaError_t e = cudaStreamSynchronize(ctx->stream);
-        if (e != cudaSuccess) { ctx->lastError = std::string("idkpt_shadows_ray_traced: ") + cudaGetErrorString(e); rc = IDKPT_ERR_CUDA; break; }
-        if (kernelMs) cudaEventElapsedTime(kernelMs, e0, e1);
-    } while (0);
-    if (e0) cudaEventDestroy(e0);
-    if (e1) cudaEventDestroy(e1);
-    return rc;
+        return IDKPT_OK;
+    }, visibilityOut, dVis.p, n * 4);
 }
 
 static int trace_rays_impl(IdkPtCtx* ctx, const IdkPtRay* rays, uint64_t count, int32_t traceLights, IdkPtHit* hitsOut, float* kernelMs, bool anyHit) {
@@ -1824,33 +1811,30 @@ static int trace_rays_impl(IdkPtCtx* ctx, const IdkPtRay* rays, uint64_t count, 
     if (count == 0) return IDKPT_OK;
     CK(cudaSetDevice(ctx->device));
     DevBuf &dr = ctx->scratch[0], &dh = ctx->scratch[1], &dt = ctx->scratch[2];
-    int rc = IDKPT_OK;
-    cudaEvent_t e0 = nullptr, e1 = nullptr;
-    do {
-        if (ensure(dr, count * 32) != cudaSuccess || ensure(dh, count * 32) != cudaSuccess || ensure(dt, 16) != cudaSuccess) { rc = fail(ctx, IDKPT_ERR_OUT_OF_MEMORY, "idkpt_trace_rays: device allocation failed"); break; }
-        cudaMemcpyAsync(dr.p, rays, count * 32, cudaMemcpyHostToDevice, ctx->stream);
-        cudaMemsetAsync(dt.p, 0, 16, ctx->stream);
-        TraceRaysArgs a;
-        a.sc = ctx->sc;
-        a.rays = (const float4*)dr.p;
-        a.hits = (uint4*)dh.p;
-        a.count = (uint32_t)count;
-        a.ticket = (uint32_t*)dt.p;
-        a.traceLights = traceLights;
-        cudaEventCreate(&e0);
-        cudaEventCreate(&e1);
-        cudaEventRecord(e0, ctx->stream);
+    if (ensure(dr, count * 32) != cudaSuccess || ensure(dh, count * 32) != cudaSuccess || ensure(dt, 16) != cudaSuccess)
+        return fail(ctx, IDKPT_ERR_OUT_OF_MEMORY, "idkpt_trace_rays: device allocation failed");
+    CK(cudaMemcpyAsync(dr.p, rays, count * 32, cudaMemcpyHostToDevice, ctx->stream));
+    CK(cudaMemsetAsync(dt.p, 0, 16, ctx->stream));
+    TraceRaysArgs a;
+    a.sc = ctx->sc;
+    a.rays = (const float4*)dr.p;
+    a.hits = (uint4*)dh.p;
+    a.count = (uint32_t)count;
+    a.ticket = (uint32_t*)dt.p;
+    a.traceLights = traceLights;
+    return run_timed(ctx, "idkpt_trace_rays", kernelMs, [&]() -> int {
         if (anyHit) k_trace_rays_any<<<ctx->traceRaysBlocks, IDK_BLOCK, ctx->stackBytes, ctx->stream>>>(a);
         else k_trace_rays<<<ctx->traceRaysBlocks, IDK_BLOCK, ctx->stackBytes, ctx->stream>>>(a);
-        cudaEventRecord(e1, ctx->stream);
-        cudaMemcpyAsync(hitsOut, dh.p, count * 32, cudaMemcpyDeviceToHost, ctx->stream);
-        cudaError_t e = cudaStreamSynchronize(ctx->stream);
-        if (e != cudaSuccess) { ctx->lastError = std::string("idkpt_trace_rays: ") + cudaGetErrorString(e); rc = IDKPT_ERR_CUDA; break; }
-        if (kernelMs) cudaEventElapsedTime(kernelMs, e0, e1);
-    } while (0);
-    if (e0) cudaEventDestroy(e0);
-    if (e1) cudaEventDestroy(e1);
-    return rc;
+        return IDKPT_OK;
+    }, hitsOut, dh.p, count * 32);
+}
+
+IDKPT_API int idkpt_trace_rays(IdkPtCtx* ctx, const IdkPtRay* rays, uint64_t count, int32_t traceLights, IdkPtHit* hitsOut, float* kernelMs) {
+    return trace_rays_impl(ctx, rays, count, traceLights, hitsOut, kernelMs, false);
+}
+
+IDKPT_API int idkpt_trace_rays_any(IdkPtCtx* ctx, const IdkPtRay* rays, uint64_t count, int32_t traceLights, IdkPtHit* hitsOut, float* kernelMs) {
+    return trace_rays_impl(ctx, rays, count, traceLights, hitsOut, kernelMs, true);
 }
 
 } // extern "C"
