@@ -307,6 +307,55 @@ def multi_blas(threads=None):
     return scene, cam
 
 
+# --------------------------------------------------------------------------- wavefront-count scenes
+def closed_box(subdiv=1, half=1.0, height=2.0, threads=None):
+    """A closed box [-half, half] x [0, height] x [-half, half] of inward-facing diffuse walls, each face a subdiv x subdiv
+    grid (12 * subdiv^2 triangles). The ceiling cells within the middle third are emissive (the whole ceiling for subdiv 1).
+    The camera sits inside. With Russian roulette off a path ends only on a miss, so every bounce keeps nearly all rays alive
+    (short of the few that slip through an edge)."""
+    meshes, mats = _materials([dict(color=(0.75, 0.72, 0.68)), dict(color=(1, 1, 1), emissive=(6, 6, 6))])
+    h, H, n = float(half), float(height), int(subdiv)
+    faces = [  # origin, du, dv with cross(du, dv) pointing into the box
+        ([-h, 0, -h], [0, 0, 2 * h], [2 * h, 0, 0]),          # floor, +Y
+        ([-h, H, -h], [2 * h, 0, 0], [0, 0, 2 * h]),          # ceiling, -Y
+        ([-h, 0, -h], [2 * h, 0, 0], [0, H, 0]),              # back, +Z
+        ([-h, 0, h], [0, H, 0], [2 * h, 0, 0]),               # front, -Z
+        ([-h, 0, -h], [0, H, 0], [0, 0, 2 * h]),              # left, +X
+        ([h, 0, -h], [0, 0, 2 * h], [0, H, 0]),               # right, -X
+    ]
+    a = _Assembler()
+    for k, (o, du, dv) in enumerate(faces):
+        p, idx = grid(o, du, dv, n, n)
+        if k == 1:
+            c = p[idx].mean(1)
+            lit = (np.abs(c[:, 0]) <= h / 3 + 1e-6) & (np.abs(c[:, 2]) <= h / 3 + 1e-6) if n > 1 else np.ones(len(idx), bool)
+            a.add((p, idx[~lit]), 0)
+            a.add((p, idx[lit]), 1)
+        else:
+            a.add((p, idx), 0)
+    scene = Scene().add(a.model(meshes, mats, name="closed_box"), threads=threads)
+    cam = dict(position=(0.0, 0.45 * H, 0.8 * h), view_dir=(0.1, 0.05, -1.0), fov_y_deg=70.0)
+    return scene, cam
+
+
+def open_floor(size=4.0, threads=None):
+    """One diffuse floor quad and a camera looking down at it from 1 unit: every primary ray hits the floor and every
+    bounce ray leaves the scene, so the alive count drops to zero after the first bounce."""
+    meshes, mats = _materials([dict(color=(0.6, 0.6, 0.6))])
+    a = _Assembler()
+    s = float(size)
+    a.add(quad([-s, 0, -s], [-s, 0, s], [s, 0, s], [s, 0, -s]), 0)
+    scene = Scene().add(a.model(meshes, mats, name="open_floor"), threads=threads)
+    cam = dict(position=(0.0, 1.0, 0.0), view_dir=(0.0, -1.0, -0.05), fov_y_deg=60.0)
+    return scene, cam
+
+
+def camera_away(cam):
+    """The same camera turned around (e.g. out of the Cornell box's open side: nothing but sky in view)."""
+    out = dict(cam)
+    out["view_dir"] = tuple(-np.asarray(cam["view_dir"], np.float64))
+    return out
+
 
 def instance_grid(n=3, threads=None):
     """n^3 small models (spheres, boxes, cylinders; rotated / non-uniformly scaled instances) over a floor: a TLAS with
