@@ -4,12 +4,12 @@
 //   k_prepare_triangles/vertices/surfaces  scene upload: 64-byte triangle records, decoded vertex frames, per-mesh surfaces
 //   k_init_sample        per sample: zero alive counts and work tickets
 //   k_raygen             FirstHit/compute.glsl:44-81   ray generation (camera, jitter, thin lens)
-//   k_traverse           BVHIntersect.glsl:27-105,183-291  closest hit, one ray per lane (primary rays, TLAS walk)
+//   k_traverse           BVHIntersect.glsl:27-105,183-291  closest hit, one ray per lane (primary rays, TLAS walk): trace_ray<STATS, false>
 //   k_traverse2          same per-ray operation sequence, warp-level SETUP/BOX/LEAF phase scheduling with lane refill
 //   k_shade              FirstHit/compute.glsl:100-234, NHit/compute.glsl:91-215 (barrier-free, state in place)
 //   k_compact            the ordered (canonical) outcome of the alive-list atomics, decoupled look-back scan
 //   k_accumulate         FinalDraw/compute.glsl:24-62; k_accumulate_scatter: fused with the NVLink peer gather
-//   k_trace_rays         stand-alone closest-hit batch (BVH.Intersect analogue)
+//   k_trace_rays         stand-alone closest-hit batch (BVH.Intersect analogue): trace_ray<true, false>
 #pragma once
 #include "idk_device.cuh"
 #include "../../include/idk_gpu_types.h"
@@ -131,9 +131,11 @@ __global__ void k_prepare_surfaces(const GpuMesh* __restrict__ meshes, const Gpu
 }
 
 // ------------------------------------------------------------------------------------------------
-// IntersectBlas (BVHIntersect.glsl:27-105) for one local-space ray. `stack` points at this thread's column of the
-// shared stack (stride IDK_BLOCK), exactly the reference's `shared uint BlasTraversalStack[SIZE][LOCAL_SIZE]`.
-template <bool STATS>
+// The serial BVH walk (one ray per thread) for closest hit and, with ANY, any hit. The any-hit walk descends a BLAS left
+// first instead of closer first, returns at the first accepted triangle or light, and keeps no counters (STATS = false).
+// IntersectBlas / IntersectBlasAny (BVHIntersect.glsl:27-181) for one local-space ray. `stack` points at this thread's
+// column of the shared stack (stride IDK_BLOCK), exactly the reference's `shared uint BlasTraversalStack[SIZE][LOCAL_SIZE]`.
+template <bool STATS, bool ANY>
 __device__ __forceinline__ bool intersect_blas(const DeviceScene& sc, const float4* nodes, uint32_t triOffset, f3 lo, f3 ld, f3 inv,
                                                bool rootTest, uint32_t* stack, HitRec& hit, uint32_t& S, uint32_t& T, float& cost) {
     float tMinLeft, tMinRight;
@@ -172,6 +174,7 @@ __device__ __forceinline__ bool intersect_blas(const DeviceScene& sc, const floa
                     hit.bx = bx;
                     hit.by = by;
                     hit.t = t;
+                    if (ANY) return true;
                 }
             }
         }
@@ -180,9 +183,9 @@ __device__ __forceinline__ bool intersect_blas(const DeviceScene& sc, const floa
         const bool traverseRight = hitRight && rCount == 0;
         if (traverseLeft || traverseRight) {
             if (traverseLeft && traverseRight) {
-                const bool leftCloser = tMinLeft < tMinRight;
-                top = leftCloser ? (uint32_t)lChild : (uint32_t)rChild;
-                stack[(sp++) * IDK_BLOCK] = leftCloser ? (uint32_t)rChild : (uint32_t)lChild;
+                const bool leftFirst = ANY || tMinLeft < tMinRight;
+                top = leftFirst ? (uint32_t)lChild : (uint32_t)rChild;
+                stack[(sp++) * IDK_BLOCK] = leftFirst ? (uint32_t)rChild : (uint32_t)lChild;
             } else {
                 top = traverseLeft ? (uint32_t)lChild : (uint32_t)rChild;
             }
@@ -194,9 +197,9 @@ __device__ __forceinline__ bool intersect_blas(const DeviceScene& sc, const floa
     return blasHit;
 }
 
-// One BLAS instance: local ray (Ray.glsl:7-12) + IntersectBlas.
-template <bool STATS>
-__device__ __forceinline__ void trace_instance(const DeviceScene& sc, uint32_t inst, f3 o, f3 d, bool rootTest, uint32_t* stack,
+// One BLAS instance: local ray (Ray.glsl:7-12) + IntersectBlas. Returns whether the BLAS took the hit.
+template <bool STATS, bool ANY>
+__device__ __forceinline__ bool trace_instance(const DeviceScene& sc, uint32_t inst, f3 o, f3 d, bool rootTest, uint32_t* stack,
                                                HitRec& hit, uint32_t& hitXform, uint32_t& S, uint32_t& T, uint32_t& I, float& cost) {
     const GpuBlasInstance bi = sc.instances[inst];
     const int nodeOffset = sc.descs[bi.BlasId].NodeOffset;
@@ -207,14 +210,16 @@ __device__ __forceinline__ void trace_instance(const DeviceScene& sc, uint32_t i
     const f3 ld = xform_vector(r0, r1, r2, d);
     const f3 inv = mk3(1.0f / ld.x, 1.0f / ld.y, 1.0f / ld.z);
     if (STATS) I++;
-    if (intersect_blas<STATS>(sc, sc.nodes + 2 * (size_t)nodeOffset, triOffset, lo, ld, inv, rootTest, stack, hit, S, T, cost)) hitXform = bi.MeshTransformId;
+    if (!intersect_blas<STATS, ANY>(sc, sc.nodes + 2 * (size_t)nodeOffset, triOffset, lo, ld, inv, rootTest, stack, hit, S, T, cost)) return false;
+    hitXform = bi.MeshTransformId;
+    return true;
 }
 
-// TraceRay (BVHIntersect.glsl:183-291): lights, then the instance loop (default) or the TLAS walk.
-template <bool STATS>
-__device__ __forceinline__ void trace_closest(const DeviceScene& sc, f3 o, f3 d, float tMax, bool traceLights,
-                                              uint32_t* stack, HitRec& hit, uint32_t& hitXform,
-                                              uint32_t& S, uint32_t& T, uint32_t& I, float& cost) {
+// TraceRay / TraceRayAny (BVHIntersect.glsl:183-291,299-411): lights, then the instance loop (default) or the TLAS walk.
+// Returns what the reference returns: closest hit, hit.t != tMax; any hit, whether a light or triangle was accepted.
+template <bool STATS, bool ANY>
+__device__ __forceinline__ bool trace_ray(const DeviceScene& sc, f3 o, f3 d, float tMax, bool traceLights,
+                                          uint32_t* stack, HitRec& hit, uint32_t& hitXform, uint32_t& S, uint32_t& T, uint32_t& I, float& cost) {
     hit.t = tMax;
     hit.tri = ~0u;
     hit.bx = 0.0f;
@@ -229,6 +234,7 @@ __device__ __forceinline__ void trace_closest(const DeviceScene& sc, f3 o, f3 d,
                 hit.t = tMin < 0.0f ? tMx : tMin;
                 hitXform = i;
                 hit.tri = ~0u;
+                if (ANY) return true;
             }
         }
     }
@@ -242,7 +248,8 @@ __device__ __forceinline__ void trace_closest(const DeviceScene& sc, f3 o, f3 d,
             const uint32_t word = __float_as_uint(pA.w);
             const uint32_t id = word & 0x7FFFFFFFu;
             if (word >> 31) {
-                trace_instance<STATS>(sc, id, o, d, false, stack, hit, hitXform, S, T, I, cost);
+                const bool instHit = trace_instance<STATS, ANY>(sc, id, o, d, false, stack, hit, hitXform, S, T, I, cost);
+                if (ANY && instHit) return true;
                 if (sp == 0) break;
                 top = tstack[--sp];
                 continue;
@@ -266,8 +273,12 @@ __device__ __forceinline__ void trace_closest(const DeviceScene& sc, f3 o, f3 d,
             }
         }
     } else {
-        for (uint32_t inst = 0; inst < sc.instanceCount; inst++) trace_instance<STATS>(sc, inst, o, d, true, stack, hit, hitXform, S, T, I, cost);
+        for (uint32_t inst = 0; inst < sc.instanceCount; inst++) {
+            const bool instHit = trace_instance<STATS, ANY>(sc, inst, o, d, true, stack, hit, hitXform, S, T, I, cost);
+            if (ANY && instHit) return true;
+        }
     }
+    return !ANY && hit.t != tMax;
 }
 
 struct TraverseArgs {
@@ -308,7 +319,7 @@ __global__ void __launch_bounds__(IDK_BLOCK) k_traverse(TraverseArgs a) {
             uint32_t xf;
             float cost = 0.0f;
             const uint32_t stepsBefore = S;
-            trace_closest<STATS>(a.sc, o, d, IDK_FLOAT_MAX, a.traceLights != 0, stack, hit, xf, S, T, I, cost);
+            trace_ray<STATS, false>(a.sc, o, d, IDK_FLOAT_MAX, a.traceLights != 0, stack, hit, xf, S, T, I, cost);
             if (STATS) atomicMax(&a.counters->maxSteps[a.bounce & 63], S - stepsBefore);
             reinterpret_cast<float4*>(a.hits)[gid] = make_float4(hit.bx, hit.by, hit.t, __uint_as_float(hit.tri));
             a.hitXform[gid] = xf;
@@ -336,8 +347,8 @@ __global__ void __launch_bounds__(IDK_BLOCK) k_traverse(TraverseArgs a) {
 
 
 // ------------------------------------------------------------------------------------------------
-// k_traverse2: the production traversal kernel. Same per-ray operation sequence as trace_closest (hence the same
-// bits and the same S/T/I counters), but the warp is scheduled as a small state machine so that divergent work is
+// k_traverse2: the production traversal kernel. Same per-ray operation sequence as trace_ray<STATS, false> (hence the
+// same bits and the same S/T/I counters), but the warp is scheduled as a small state machine so that divergent work is
 // batched instead of serialised:
 //   SETUP  lanes whose ray is finished write their hit, claim a new slot (one atomicAdd per warp for all needy
 //          lanes -- persistent threads with lane refill) and set up the next BLAS instance (local ray, root test);
@@ -346,6 +357,8 @@ __global__ void __launch_bounds__(IDK_BLOCK) k_traverse(TraverseArgs a) {
 //   LEAF   lanes with a pending range test ONE triangle.
 // Each iteration the warp votes (ballots) which phase to run: a phase runs when enough lanes wait for it or nothing
 // else can run. Traversal stacks live in shared memory, one column per thread (the reference's layout).
+// Its phases restate the serial walk (trace_ray, trace_instance, intersect_blas) step for step, written out in place:
+// a change to a traversal rule must be made in both.
 struct TraverseTuning { int setupThreshold; int leafThreshold; int packRays; };   // packRays: 32 rays per warp whatever the count (throughput mode: several samples share the SMs)
 #define IDK_T2_SETUP_THRESHOLD 12   // SETUP runs when this many lanes wait in it (capped at 3/8 of the rays a warp carries)
 #define IDK_T2_LEAF_THRESHOLD 4     // LEAF runs when this many lanes wait in it (capped at 1/8 of the rays a warp carries)
@@ -631,7 +644,7 @@ __global__ void __launch_bounds__(IDK_BLOCK) k_trace_rays(TraceRaysArgs a) {
             HitRec hit;
             uint32_t xf, S = 0, T = 0, I = 0;
             float cost = 0.0f;
-            trace_closest<true>(a.sc, mk3(r0.x, r0.y, r0.z), mk3(r1.x, r1.y, r1.z), r0.w, a.traceLights != 0, stack, hit, xf, S, T, I, cost);
+            trace_ray<true, false>(a.sc, mk3(r0.x, r0.y, r0.z), mk3(r1.x, r1.y, r1.z), r0.w, a.traceLights != 0, stack, hit, xf, S, T, I, cost);
             a.hits[2 * (size_t)gid] = make_uint4(__float_as_uint(hit.bx), __float_as_uint(hit.by), __float_as_uint(hit.t), hit.tri);
             a.hits[2 * (size_t)gid + 1] = make_uint4(xf, S, T, 0u);
         }

@@ -1,120 +1,9 @@
 // "Next" rows of the scope table (SURVEY.md 8f.1): any-hit traversal and the ray-traced point-light shadow pass, both on
-// top of the path tracer's traversal code.
-//   k_trace_rays_any        TraceRayAny / IntersectBlasAny, include/BVHIntersect.glsl:107-181,299-411
+// top of the path tracer's serial walk (trace_ray, idk_kernels.cuh).
+//   k_trace_rays_any        TraceRayAny / IntersectBlasAny, include/BVHIntersect.glsl:107-181,299-411: trace_ray<false, true>
 //   k_shadows_ray_traced    ShadowsRayTraced/compute.glsl (PointShadowManager.ComputeRayTracedShadowMaps, PointShadowManager.cs:53-75)
 #pragma once
 #include "idk_kernels.cuh"
-
-// IntersectBlasAny: left-first descent, returns at the first accepted triangle.
-__device__ __forceinline__ bool intersect_blas_any(const DeviceScene& sc, const float4* nodes, uint32_t triOffset, f3 lo, f3 ld, f3 inv,
-                                                   bool rootTest, uint32_t* stack, HitRec& hit) {
-    float tMinLeft, tMinRight;
-    if (rootTest) {
-        const float4 a = ldg4(nodes + 2), b = ldg4(nodes + 3);
-        if (!(ray_box(lo, inv, a, b, tMinLeft) && tMinLeft < hit.t)) return false;
-    }
-    uint32_t sp = 0, top = 2;
-    while (true) {
-        const NodePair pr = ldg_pair(nodes + 2 * (size_t)top);
-        const float4 lA = pr.lA, lB = pr.lB, rA = pr.rA, rB = pr.rB;
-        const int lChild = __float_as_int(lA.w), lCount = __float_as_int(lB.w);
-        const int rChild = __float_as_int(rA.w), rCount = __float_as_int(rB.w);
-        const bool hitLeft = ray_box(lo, inv, lA, lB, tMinLeft) && tMinLeft <= hit.t;
-        const bool hitRight = ray_box(lo, inv, rA, rB, tMinRight) && tMinRight <= hit.t;
-        const bool intersectLeft = hitLeft && lCount > 0, intersectRight = hitRight && rCount > 0;
-        if (intersectLeft || intersectRight) {
-            uint32_t first = (intersectLeft ? (uint32_t)lChild : (uint32_t)rChild) + triOffset;
-            const uint32_t end = (!intersectRight ? (uint32_t)(lChild + lCount) : (uint32_t)(rChild + rCount)) + triOffset;
-            for (uint32_t i = first; i < end; i++) {
-                float4 a, b, c;
-                ldg_tri(sc.triRec, i, a, b, c);
-                float bx, by, t;
-                if (ray_triangle(lo, ld, mk3(a.x, a.y, a.z), mk3(a.w, b.x, b.y), mk3(b.z, b.w, c.x), mk3(c.y, c.z, c.w), bx, by, t) && t < hit.t) {
-                    hit.tri = i; hit.bx = bx; hit.by = by; hit.t = t;
-                    return true;
-                }
-            }
-        }
-        const bool traverseLeft = hitLeft && lCount == 0, traverseRight = hitRight && rCount == 0;
-        if (traverseLeft || traverseRight) {
-            if (traverseLeft && traverseRight) {
-                top = (uint32_t)lChild;
-                stack[(sp++) * IDK_BLOCK] = (uint32_t)rChild;
-            } else {
-                top = traverseLeft ? (uint32_t)lChild : (uint32_t)rChild;
-            }
-        } else {
-            if (sp == 0) break;
-            top = stack[(--sp) * IDK_BLOCK];
-        }
-    }
-    return false;
-}
-
-__device__ __forceinline__ bool trace_instance_any(const DeviceScene& sc, uint32_t inst, f3 o, f3 d, bool rootTest, uint32_t* stack, HitRec& hit, uint32_t& hitXform) {
-    const GpuBlasInstance bi = sc.instances[inst];
-    const int nodeOffset = sc.descs[bi.BlasId].NodeOffset;
-    const uint32_t triOffset = (uint32_t)sc.descs[bi.BlasId].TriangleOffset;
-    const float4* xf = sc.xforms + 9 * (size_t)bi.MeshTransformId + 3;
-    const float4 r0 = ldg4(xf), r1 = ldg4(xf + 1), r2 = ldg4(xf + 2);
-    const f3 lo = xform_point(r0, r1, r2, o), ld = xform_vector(r0, r1, r2, d);
-    const f3 inv = mk3(1.0f / ld.x, 1.0f / ld.y, 1.0f / ld.z);
-    if (intersect_blas_any(sc, sc.nodes + 2 * (size_t)nodeOffset, triOffset, lo, ld, inv, rootTest, stack, hit)) { hitXform = bi.MeshTransformId; return true; }
-    return false;
-}
-
-// TraceRayAny
-__device__ __forceinline__ bool trace_any(const DeviceScene& sc, f3 o, f3 d, float tMax, bool traceLights, uint32_t* stack, HitRec& hit, uint32_t& hitXform) {
-    hit.t = tMax; hit.tri = ~0u; hit.bx = 0.0f; hit.by = 0.0f;
-    hitXform = 0;
-    if (traceLights) {
-        for (uint32_t i = 0; i < sc.lightCount; i++) {
-            const GpuLight& L = sc.lights[i];
-            float tMin, tMx;
-            if (ray_sphere(o, d, mk3(L.Position[0], L.Position[1], L.Position[2]), L.Radius, tMin, tMx) && tMin < hit.t) {
-                hit.t = tMin < 0.0f ? tMx : tMin;
-                hitXform = i;
-                return true;
-            }
-        }
-    }
-    if (sc.useTlas) {
-        const f3 inv = mk3(1.0f / d.x, 1.0f / d.y, 1.0f / d.z);
-        uint32_t tstack[IDK_TLAS_STACK_SIZE];
-        uint32_t sp = 0, top = 0;
-        while (true) {
-            const float4 pA = ldg4(sc.tlasNodes + 2 * (size_t)top);
-            const uint32_t word = __float_as_uint(pA.w), id = word & 0x7FFFFFFFu;
-            if (word >> 31) {
-                if (trace_instance_any(sc, id, o, d, false, stack, hit, hitXform)) return true;
-                if (sp == 0) break;
-                top = tstack[--sp];
-                continue;
-            }
-            const float4 lA = ldg4(sc.tlasNodes + 2 * (size_t)id), lB = ldg4(sc.tlasNodes + 2 * (size_t)id + 1);
-            const float4 rA = ldg4(sc.tlasNodes + 2 * (size_t)id + 2), rB = ldg4(sc.tlasNodes + 2 * (size_t)id + 3);
-            float tMinLeft, tMinRight;
-            const bool tl = ray_box(o, inv, lA, lB, tMinLeft) && tMinLeft < hit.t;
-            const bool tr = ray_box(o, inv, rA, rB, tMinRight) && tMinRight < hit.t;
-            if (tl || tr) {
-                if (tl && tr) {
-                    const bool leftCloser = tMinLeft < tMinRight;
-                    top = leftCloser ? id : id + 1;
-                    tstack[sp++] = leftCloser ? id + 1 : id;
-                } else {
-                    top = tl ? id : id + 1;
-                }
-            } else {
-                if (sp == 0) break;
-                top = tstack[--sp];
-            }
-        }
-    } else {
-        for (uint32_t inst = 0; inst < sc.instanceCount; inst++)
-            if (trace_instance_any(sc, inst, o, d, true, stack, hit, hitXform)) return true;
-    }
-    return false;
-}
 
 __global__ void __launch_bounds__(IDK_BLOCK) k_trace_rays_any(TraceRaysArgs a) {
     extern __shared__ uint32_t s_stack[];
@@ -128,9 +17,11 @@ __global__ void __launch_bounds__(IDK_BLOCK) k_trace_rays_any(TraceRaysArgs a) {
         const uint32_t gid = base + lane;
         if (gid < a.count) {
             const float4 r0 = a.rays[2 * (size_t)gid], r1 = a.rays[2 * (size_t)gid + 1];
+            uint32_t S = 0, T = 0, I = 0;
+            float cost = 0.0f;
             HitRec hit;
             uint32_t xf;
-            const bool any = trace_any(a.sc, mk3(r0.x, r0.y, r0.z), mk3(r1.x, r1.y, r1.z), r0.w, a.traceLights != 0, stack, hit, xf);
+            const bool any = trace_ray<false, true>(a.sc, mk3(r0.x, r0.y, r0.z), mk3(r1.x, r1.y, r1.z), r0.w, a.traceLights != 0, stack, hit, xf, S, T, I, cost);
             a.hits[2 * (size_t)gid] = make_uint4(__float_as_uint(hit.bx), __float_as_uint(hit.by), __float_as_uint(hit.t), hit.tri);
             a.hits[2 * (size_t)gid + 1] = make_uint4(xf, any ? 1u : 0u, 0u, 0u);
         }
@@ -214,7 +105,7 @@ __global__ void __launch_bounds__(IDK_BLOCK) k_shadows_ray_traced(ShadowArgs a) 
                 uint32_t xf, S = 0, T = 0, I = 0;
                 float cost = 0.0f;
                 const float maxDist = distanceToLight - 0.001f;
-                trace_closest<false>(sc, origin, direction, maxDist, true, stack, hit, xf, S, T, I, cost);
+                trace_ray<false, false>(sc, origin, direction, maxDist, true, stack, hit, xf, S, T, I, cost);
                 if (!(hit.t != maxDist)) break;
                 if (hit.tri == ~0u) {
                     if (xf != (uint32_t)a.lightIndex) thisVisibility = 0.0f;

@@ -150,8 +150,9 @@ __device__ __forceinline__ bool vx_pixel(const VxScene& sc, const VxGridDev& g, 
                 // towards the light; here that point is connected to the light by an any-hit ray instead of the PCF lookup
                 const float bias = 0.02f;
                 HitRec sh;
-                uint32_t sx;
-                const bool occluded = trace_any(sc.occ, fragPos + sampleToLight * bias, lightDir, dist * (1.0f - bias), false, stack, sh, sx);
+                uint32_t sx, S = 0, T = 0, I = 0;
+                float cost = 0.0f;
+                const bool occluded = trace_ray<false, true>(sc.occ, fragPos + sampleToLight * bias, lightDir, dist * (1.0f - bias), false, stack, sh, sx, S, T, I, cost);
                 contrib = contrib * (occluded ? 0.0f : 1.0f);
             }
             direct = direct + contrib;
