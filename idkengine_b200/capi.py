@@ -96,7 +96,10 @@ EXPORTS = [
     "idkpt_read_wavefront_rays", "idkpt_trace_rays", "idkpt_trace_rays_any", "idkpt_shadows_ray_traced",
     "idkpt_set_skinning_data", "idkpt_skin_vertices", "idkpt_blas_refit", "idkpt_read_range", "idkpt_post_process", "idkpt_ldr_device_ptr", "idkpt_abi_version",
     "idkpt_denoise", "idkpt_denoise_device_ptrs", "idkpt_denoise_import_output", "idkpt_tlas_build",
+    "idkpt_set_point_shadows", "idkpt_render_point_shadows", "idkpt_read_point_shadow", "idkpt_point_shadow_device_ptr",
 ]
+
+IDKPT_MAX_POINT_SHADOWS = 128
 
 
 class IdkPtDenoiseSettings(ctypes.Structure):
@@ -297,6 +300,14 @@ def load(path=None):
     L.idkpt_denoise_device_ptrs.argtypes = [c_vp, P(c_vp), P(c_vp), P(c_vp), P(c_vp), P(c_u64)]
     L.idkpt_denoise_import_output.restype = c_i32
     L.idkpt_denoise_import_output.argtypes = [c_vp]
+    L.idkpt_set_point_shadows.restype = c_i32
+    L.idkpt_set_point_shadows.argtypes = [c_vp, c_vp, c_vp, c_u32]
+    L.idkpt_render_point_shadows.restype = c_i32
+    L.idkpt_render_point_shadows.argtypes = [c_vp, c_u32, c_u32, c_vp, P(c_f)]
+    L.idkpt_read_point_shadow.restype = c_i32
+    L.idkpt_read_point_shadow.argtypes = [c_vp, c_i32, c_vp, c_u64]
+    L.idkpt_point_shadow_device_ptr.restype = c_i32
+    L.idkpt_point_shadow_device_ptr.argtypes = [c_vp, c_i32, P(c_vp), P(c_u64)]
     L.idkpt_abi_version.restype = c_u32
     L.idkpt_abi_version.argtypes = []
     if path == _build.LIBIDKPT:

@@ -776,14 +776,12 @@ __device__ __forceinline__ void sky_face_to_cube(int face, int sc, int tc, int s
         default: X = -sc; Y = -tc; Z = -size; break;
     }
 }
-__device__ __forceinline__ f3 sky_texel_in(const DeviceScene& sc, int face, int x, int y) {
-    const float4 t = __ldg(sc.skyFaces + ((size_t)face * sc.skyFaceSize + y) * sc.skyFaceSize + x);
-    return mk3(t.x, t.y, t.z);
-}
-// texel (x, y) of `face` where x or y (not both) may lie one texel outside the face
-__device__ __forceinline__ f3 sky_texel_edge(const DeviceScene& sc, int face, int x, int y) {
-    const int size = sc.skyFaceSize;
-    if (x >= 0 && x < size && y >= 0 && y < size) return sky_texel_in(sc, face, x, y);
+struct CubeTexel { int face, x, y; };
+
+// Texel (x, y) of `face` where x or y (not both) may lie one texel outside the face: a texel beyond an edge is the one across
+// that edge on the neighbouring face.
+__device__ __forceinline__ CubeTexel cube_texel_edge(int face, int x, int y, int size) {
+    if (x >= 0 && x < size && y >= 0 && y < size) return CubeTexel{face, x, y};
     int s2 = 2 * x + 1 - size, t2 = 2 * y + 1 - size;     // |.| == size + 1 for the coordinate that left the face
     int X, Y, Z;
     sky_face_to_cube(face, s2, t2, size, X, Y, Z);
@@ -795,13 +793,15 @@ __device__ __forceinline__ f3 sky_texel_edge(const DeviceScene& sc, int face, in
     if (X == size) { nf = 0; ns = -Z; nt = -Y; } else if (X == -size) { nf = 1; ns = Z; nt = -Y; }
     else if (Y == size) { nf = 2; ns = X; nt = Z; } else if (Y == -size) { nf = 3; ns = X; nt = -Z; }
     else if (Z == size) { nf = 4; ns = X; nt = -Y; } else { nf = 5; ns = -X; nt = -Y; }
-    return sky_texel_in(sc, nf, (ns + size - 1) / 2, (nt + size - 1) / 2);
+    return CubeTexel{nf, (ns + size - 1) / 2, (nt + size - 1) / 2};
 }
 
-// texture(skyBoxUBO.Albedo, dir).rgb: GL cube-map face selection (spec table 8.19), bilinear filtering, seamless across edges.
-__device__ __forceinline__ f3 sample_sky(const DeviceScene& sc, f3 d) {
-    if (sc.skyFaceSize == 0) return mk3(sc.skyR, sc.skyG, sc.skyB);
-    const int size = sc.skyFaceSize;
+// The bilinear footprint of direction d on a cube map of face size `size`: GL face selection (spec table 8.19), the four taps
+// t00, t10, t01, t11 (x fastest), seamless across edges, and the weights fx, fy. At a cube corner exactly one tap lies outside
+// the face in both directions and no face holds it (corner = its index 0..3, else -1); the caller replaces it by the mean of
+// the other three. The sky lookup and the point-shadow PCF lookup (idk_point_shadows.cuh) share this.
+struct CubeFootprint { CubeTexel t00, t10, t01, t11; float fx, fy; int corner; };
+__device__ __forceinline__ CubeFootprint cube_footprint(f3 d, int size) {
     const float ax = fabsf(d.x), ay = fabsf(d.y), az = fabsf(d.z);
     int face;
     float scc, tc, ma;
@@ -811,26 +811,41 @@ __device__ __forceinline__ f3 sample_sky(const DeviceScene& sc, f3 d) {
     const float s = 0.5f * (scc / ma + 1.0f), t = 0.5f * (tc / ma + 1.0f);
     const float px = s * (float)size - 0.5f, py = t * (float)size - 0.5f;
     const float fx0 = floorf(px), fy0 = floorf(py);
-    const float fx = px - fx0, fy = py - fy0;
+    CubeFootprint fp;
+    fp.fx = px - fx0; fp.fy = py - fy0;
     const int x0 = (int)fx0, x1 = (int)fx0 + 1, y0 = (int)fy0, y1 = (int)fy0 + 1;      // each in [-1, size]
     const bool ox0 = x0 < 0, ox1 = x1 >= size, oy0 = y0 < 0, oy1 = y1 >= size;
-    f3 t00, t10, t01, t11;
-    if ((ox0 || ox1) && (oy0 || oy1)) {
-        // cube corner: exactly one of the four texels lies outside in both directions; it is the mean of the other three
-        const bool c00 = ox0 && oy0, c10 = ox1 && oy0, c01 = ox0 && oy1;
-        t00 = c00 ? mk3(0, 0, 0) : sky_texel_edge(sc, face, x0, y0);
-        t10 = c10 ? mk3(0, 0, 0) : sky_texel_edge(sc, face, x1, y0);
-        t01 = c01 ? mk3(0, 0, 0) : sky_texel_edge(sc, face, x0, y1);
-        t11 = (c00 || c10 || c01) ? sky_texel_edge(sc, face, x1, y1) : mk3(0, 0, 0);
+    fp.corner = -1;
+    if ((ox0 || ox1) && (oy0 || oy1)) fp.corner = (ox0 && oy0) ? 0 : (ox1 && oy0) ? 1 : (ox0 && oy1) ? 2 : 3;
+    const CubeTexel none = {face, 0, 0};
+    fp.t00 = fp.corner == 0 ? none : cube_texel_edge(face, x0, y0, size);
+    fp.t10 = fp.corner == 1 ? none : cube_texel_edge(face, x1, y0, size);
+    fp.t01 = fp.corner == 2 ? none : cube_texel_edge(face, x0, y1, size);
+    fp.t11 = fp.corner == 3 ? none : cube_texel_edge(face, x1, y1, size);
+    return fp;
+}
+
+__device__ __forceinline__ f3 sky_texel_in(const DeviceScene& sc, CubeTexel c) {
+    const float4 t = __ldg(sc.skyFaces + ((size_t)c.face * sc.skyFaceSize + c.y) * sc.skyFaceSize + c.x);
+    return mk3(t.x, t.y, t.z);
+}
+
+// texture(skyBoxUBO.Albedo, dir).rgb: GL cube-map face selection (spec table 8.19), bilinear filtering, seamless across edges.
+__device__ __forceinline__ f3 sample_sky(const DeviceScene& sc, f3 d) {
+    if (sc.skyFaceSize == 0) return mk3(sc.skyR, sc.skyG, sc.skyB);
+    const CubeFootprint fp = cube_footprint(d, sc.skyFaceSize);
+    const f3 zero = mk3(0, 0, 0);
+    f3 t00 = fp.corner == 0 ? zero : sky_texel_in(sc, fp.t00);
+    f3 t10 = fp.corner == 1 ? zero : sky_texel_in(sc, fp.t10);
+    f3 t01 = fp.corner == 2 ? zero : sky_texel_in(sc, fp.t01);
+    f3 t11 = fp.corner == 3 ? zero : sky_texel_in(sc, fp.t11);
+    if (fp.corner >= 0) {
         const f3 mean = ((t00 + t10) + (t01 + t11)) / 3.0f;
-        if (c00) t00 = mean; else if (c10) t10 = mean; else if (c01) t01 = mean; else t11 = mean;
-    } else {
-        t00 = sky_texel_edge(sc, face, x0, y0); t10 = sky_texel_edge(sc, face, x1, y0);
-        t01 = sky_texel_edge(sc, face, x0, y1); t11 = sky_texel_edge(sc, face, x1, y1);
+        if (fp.corner == 0) t00 = mean; else if (fp.corner == 1) t10 = mean; else if (fp.corner == 2) t01 = mean; else t11 = mean;
     }
-    const f3 a = mix3(t00, t10, fx);
-    const f3 b = mix3(t01, t11, fx);
-    return mix3(a, b, fy);
+    const f3 a = mix3(t00, t10, fp.fx);
+    const f3 b = mix3(t01, t11, fp.fx);
+    return mix3(a, b, fp.fy);
 }
 
 struct ShadeArgs {

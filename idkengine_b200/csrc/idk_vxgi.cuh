@@ -10,6 +10,7 @@
 #include <cuda_fp16.h>
 #include "idk_device.cuh"
 #include "idk_shadows.cuh"
+#include "idk_point_shadows.cuh"
 #include "../../include/idk_gpu_types.h"
 
 #define IDKVX_MAX_LEVELS 16
@@ -39,6 +40,8 @@ struct VxScene {
     const float* srgbLut;
     DeviceScene occ;               // the path tracer's device scene: occluders of the point-shadowed lights (idkvx_set_shadow_tracer)
     int occValid;
+    PointShadowMapsDev psm;        // the path tracer's point-shadow cube maps (idkvx_set_shadow_maps); takes precedence over occ
+    int psmValid;
 };
 
 __device__ __forceinline__ float det_tan(float x) { float s, c; det_sincos(x, &s, &c); return s / c; }
@@ -116,7 +119,7 @@ __device__ __forceinline__ bool vx_pixel(const VxScene& sc, const VxGridDev& g, 
     if (vx >= g.sx[0] || vy >= g.sy[0] || vz >= g.sz[0]) return false;
     if (vz < g.z0 || vz >= g.z1) return false;                    // another rank's slab
 
-    // fragment.glsl:31-79 (no point shadows). GetSurface(material, TexCoord): the fragment stage samples with implicit
+    // fragment.glsl:31-79. GetSurface(material, TexCoord): the fragment stage samples with implicit
     // derivatives / mip levels; here the base level is sampled bilinearly like everywhere else in this library.
     const GpuMesh& mesh = sc.meshes[t.meshId];
     const GpuMaterial& mat = sc.materials[mesh.MaterialId];
@@ -145,7 +148,10 @@ __device__ __forceinline__ bool vx_pixel(const VxScene& sc, const VxGridDev& g, 
             const float lr = fmaxf(L.Radius, 0.0001f);
             const float dsq = fmaxf(dist * dist, 0.0001f);
             f3 contrib = diffuse * ((lr * lr) / dsq);
-            if (L.PointShadowIndex >= 0 && sc.occValid) {
+            if (L.PointShadowIndex >= 0 && sc.psmValid) {
+                // Visibility(pointShadow, -sampleToLight) (fragment.glsl:55-58,100-117): the PCF lookup into the cube map
+                contrib = contrib * point_shadow_visibility(sc.psm, L.PointShadowIndex, -sampleToLight);
+            } else if (L.PointShadowIndex >= 0 && sc.occValid) {
                 // Visibility(pointShadow, -sampleToLight) (fragment.glsl:100-110): the shadow-map compare point sits 2 % of the way
                 // towards the light; here that point is connected to the light by an any-hit ray instead of the PCF lookup
                 const float bias = 0.02f;

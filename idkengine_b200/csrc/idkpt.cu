@@ -9,6 +9,7 @@
 #include <string>
 #include <vector>
 #include <algorithm>
+#include <cmath>
 
 #include "../../include/idkpt.h"
 #include "idk_kernels.cuh"
@@ -16,10 +17,12 @@
 #include "idk_shadows.cuh"
 #include "idk_dynamic.cuh"
 #include "idk_post.cuh"
+#include "idk_point_shadows.cuh"
 #include "idk_textures_host.h"
 
 #define IDKPT_ABI_VERSION 4u   // 2: IdkPtSceneDesc gained Textures / TextureCount; 3: IdkPtStats gained CompactMs / AccumulateMs, host-buffer registration;
-                               // 4: gather handle blob is 5 IPC handles (320 bytes), IDKPT_CREATE_GLOBAL_SLOTS, idkpt_gather_connect
+                               // 4: gather handle blob is 5 IPC handles (320 bytes), IDKPT_CREATE_GLOBAL_SLOTS, idkpt_gather_connect.
+                               // Entry points added since (point-shadow cube maps, idkvx_set_shadow_maps) are additive and keep 4.
 
 struct DevBuf {
     void* p = nullptr;
@@ -83,6 +86,12 @@ struct IdkPtCtx : IdkCtxBase {
 
     // host-array entry points (trace_rays, shadows): device staging buffers, kept between calls
     DevBuf scratch[3];
+
+    // point-shadow cube maps (idkpt_set_point_shadows): host copies of the records and sizes, device records, one D16 allocation
+    std::vector<GpuPointShadow> pointShadows;
+    std::vector<int32_t> pointShadowSizes;
+    std::vector<PointShadowDev> pointShadowRecs;
+    DevBuf pointShadowDev, pointShadowMaps;
 
     // present chain: bloom mip chains (rgba16f), AgX constants, RGBA8 frame
     DevBuf bloomDown, bloomUp, postConsts, ldr;
@@ -239,6 +248,7 @@ static int configure_launches(IdkPtCtx* ctx) {
     CK(cudaFuncSetAttribute(k_trace_rays, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)ctx->stackBytes));
     CK(cudaFuncSetAttribute(k_trace_rays_any, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)ctx->stackBytes));
     CK(cudaFuncSetAttribute(k_shadows_ray_traced, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)ctx->stackBytes));
+    CK(cudaFuncSetAttribute(k_point_shadow_faces, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)ctx->stackBytes));
     ctx->traverse2Smem = (size_t)stackSize * IDK_T2_BLOCK * sizeof(uint32_t);
     CK(cudaFuncSetAttribute(k_traverse2<false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)ctx->traverse2Smem));
     CK(cudaFuncSetAttribute(k_traverse2<true, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)ctx->traverse2Smem));
@@ -576,7 +586,8 @@ IDKPT_API void idkpt_destroy(IdkPtCtx* ctx) {
                      &ctx->images[0], &ctx->images[1], &ctx->images[2], &ctx->counters, &ctx->countLog, &ctx->skyFaces,
                      &ctx->tex.pixels, &ctx->tex.recs, &ctx->tex.srgbLut, &ctx->bloomDown, &ctx->bloomUp, &ctx->postConsts, &ctx->ldr,
                      &ctx->unskinned, &ctx->joints, &ctx->refitParents, &ctx->refitLocks, &ctx->scratch[0], &ctx->scratch[1], &ctx->scratch[2],
-                     &ctx->tlasScratch, &ctx->oidn[0], &ctx->oidn[1], &ctx->oidn[2], &ctx->oidn[3], &ctx->denoiseWork[0], &ctx->denoiseWork[1], &ctx->denoised};
+                     &ctx->tlasScratch, &ctx->oidn[0], &ctx->oidn[1], &ctx->oidn[2], &ctx->oidn[3], &ctx->denoiseWork[0], &ctx->denoiseWork[1], &ctx->denoised,
+                     &ctx->pointShadowDev, &ctx->pointShadowMaps};
     for (DevBuf* b : all) release(*b);
     for (int i = 0; i < IDK_MAX_LANES; i++) release_lane(ctx->lanes[i], false);
     for (cudaEvent_t ev : ctx->events) cudaEventDestroy(ev);
@@ -620,6 +631,8 @@ IDKPT_API int idkpt_set_scene(IdkPtCtx* ctx, const IdkPtSceneDesc* s) {
     // complete the context has NO scene: a failure below (CUDA error, out of memory) must not leave the previous scene's
     // pointers and counts looking valid.
     ctx->haveScene = false;
+    ctx->pointShadows.clear(); ctx->pointShadowSizes.clear(); ctx->pointShadowRecs.clear();   // the shadows belong to the old scene
+    release(ctx->pointShadowDev); release(ctx->pointShadowMaps);
     int rc;
     // nodes and triangle records share one allocation ("bvh"): [nodes | triRec], so that one L2 access-policy window covers both
     const size_t nodeBytes = ((s->BlasNodeCount * sizeof(GpuBlasNode)) + 255) & ~(size_t)255;
@@ -1301,7 +1314,7 @@ static int preload_kernels(IdkPtCtx* ctx) {
     IDK_PRELOAD(k_skin_vertices); IDK_PRELOAD(k_refit_prepare); IDK_PRELOAD(k_refit_climb); IDK_PRELOAD(k_tlas_build);
     IDK_PRELOAD(k_bloom_down); IDK_PRELOAD(k_bloom_up); IDK_PRELOAD(k_agx_matrices); IDK_PRELOAD(k_tonemap);
     IDK_PRELOAD(k_denoise_prepare); IDK_PRELOAD(k_denoise_atrous); IDK_PRELOAD(k_denoise_finish); IDK_PRELOAD(k_denoise_import);
-    IDK_PRELOAD(k_bcn_decode);
+    IDK_PRELOAD(k_bcn_decode); IDK_PRELOAD(k_point_shadow_faces);
 #undef IDK_PRELOAD
     return IDKPT_OK;
 }
@@ -1835,6 +1848,98 @@ IDKPT_API int idkpt_trace_rays(IdkPtCtx* ctx, const IdkPtRay* rays, uint64_t cou
 
 IDKPT_API int idkpt_trace_rays_any(IdkPtCtx* ctx, const IdkPtRay* rays, uint64_t count, int32_t traceLights, IdkPtHit* hitsOut, float* kernelMs) {
     return trace_rays_impl(ctx, rays, count, traceLights, hitsOut, kernelMs, true);
+}
+
+// ---- point-shadow cube maps (PointShadowManager.UpdateBuffer / RenderShadowMaps) ----------------------------------------------
+IDKPT_API int idkpt_set_point_shadows(IdkPtCtx* ctx, const GpuPointShadow* shadows, const int32_t* sizes, uint32_t count) {
+    if (!ctx || (count && (!shadows || !sizes))) return fail(ctx, IDKPT_ERR_INVALID_ARGUMENT, "idkpt_set_point_shadows: null argument");
+    if (!ctx->haveScene) return fail(ctx, IDKPT_ERR_NO_SCENE, "idkpt_set_point_shadows: no scene");
+    if (count > IDKPT_MAX_POINT_SHADOWS) return fail(ctx, IDKPT_ERR_INVALID_ARGUMENT, "idkpt_set_point_shadows: more than IDKPT_MAX_POINT_SHADOWS shadows");
+    for (uint32_t i = 0; i < count; i++) {
+        if (sizes[i] < 1 || sizes[i] > 16384) return fail(ctx, IDKPT_ERR_INVALID_ARGUMENT, "idkpt_set_point_shadows: size outside 1..16384");
+        if (!(shadows[i].NearPlane > 0.0f) || !std::isfinite(shadows[i].NearPlane))
+            return fail(ctx, IDKPT_ERR_INVALID_ARGUMENT, "idkpt_set_point_shadows: NearPlane must be > 0");
+        if (!(shadows[i].FarPlane > shadows[i].NearPlane) || !std::isfinite(shadows[i].FarPlane))
+            return fail(ctx, IDKPT_ERR_INVALID_ARGUMENT, "idkpt_set_point_shadows: FarPlane must be > NearPlane");
+    }
+    CK(cudaSetDevice(ctx->device));
+    std::vector<PointShadowDev> recs(count);
+    size_t texels = 0;
+    for (uint32_t i = 0; i < count; i++) {
+        PointShadowDev& r = recs[i];
+        for (int k = 0; k < 3; k++) r.pos[k] = shadows[i].Position[k];
+        r.nearPlane = shadows[i].NearPlane; r.farPlane = shadows[i].FarPlane;
+        r.size = sizes[i];
+        r.offset = texels;
+        texels += 6 * (size_t)sizes[i] * (size_t)sizes[i];
+    }
+    if (std::vector<int32_t>(sizes, sizes + count) != ctx->pointShadowSizes) {
+        // new layout: the maps start cleared to 65535 (ShadowMap.Fill(1.0))
+        ctx->pointShadowSizes.clear();
+        ctx->pointShadows.clear();
+        ctx->pointShadowRecs.clear();
+        release(ctx->pointShadowMaps);
+        if (ensure(ctx->pointShadowMaps, std::max<size_t>(texels, 1) * 2) != cudaSuccess)
+            return fail(ctx, IDKPT_ERR_OUT_OF_MEMORY, "idkpt_set_point_shadows: cube-map allocation failed");
+        CK(cudaMemsetAsync(ctx->pointShadowMaps.p, 0xFF, texels * 2, ctx->stream));
+    }
+    if (int rc = upload(ctx, ctx->pointShadowDev, recs.data(), recs.size() * sizeof(PointShadowDev))) return rc;
+    CK(cudaStreamSynchronize(ctx->stream));
+    ctx->pointShadows.assign(shadows, shadows + count);
+    ctx->pointShadowSizes.assign(sizes, sizes + count);
+    ctx->pointShadowRecs = recs;
+    return IDKPT_OK;
+}
+
+IDKPT_API int idkpt_render_point_shadows(IdkPtCtx* ctx, uint32_t first, uint32_t count, const uint32_t* faceMasks, float* kernelMs) {
+    if (!ctx) return IDKPT_ERR_INVALID_ARGUMENT;
+    if (!ctx->haveScene) return fail(ctx, IDKPT_ERR_NO_SCENE, "idkpt_render_point_shadows: no scene");
+    const uint32_t have = (uint32_t)ctx->pointShadowRecs.size();
+    if (first > have || count > have - first) return fail(ctx, IDKPT_ERR_INVALID_ARGUMENT, "idkpt_render_point_shadows: shadow range outside the set shadows");
+    for (uint32_t i = 0; faceMasks && i < count; i++)
+        if (faceMasks[i] > 0x3Fu) return fail(ctx, IDKPT_ERR_INVALID_ARGUMENT, "idkpt_render_point_shadows: face mask has bits above the six faces");
+    if (kernelMs) *kernelMs = 0.0f;
+    if (count == 0) return IDKPT_OK;
+    CK(cudaSetDevice(ctx->device));
+    return run_timed(ctx, "idkpt_render_point_shadows", kernelMs, [&]() -> int {
+        for (uint32_t i = first; i < first + count; i++) {
+            const PointShadowDev& r = ctx->pointShadowRecs[i];
+            const uint32_t mask = faceMasks ? faceMasks[i - first] : 0x3Fu;
+            PointShadowRenderArgs a;
+            a.sc = ctx->sc;
+            for (int k = 0; k < 3; k++) a.pos[k] = r.pos[k];
+            a.nearPlane = r.nearPlane; a.farPlane = r.farPlane; a.size = r.size;
+            a.map = (uint16_t*)ctx->pointShadowMaps.p + r.offset;
+            int faces = 0;
+            for (int f = 0; f < 6; f++) if (mask & (1u << f)) a.faces[faces++] = f;
+            if (faces == 0) continue;
+            const size_t tilesX = ((size_t)r.size + 7) / 8, tiles = tilesX * tilesX;
+            const dim3 grid((unsigned)((tiles + IDK_BLOCK / 64 - 1) / (IDK_BLOCK / 64)), (unsigned)faces);
+            k_point_shadow_faces<<<grid, IDK_BLOCK, ctx->stackBytes, ctx->stream>>>(a);
+        }
+        return IDKPT_OK;
+    });
+}
+
+IDKPT_API int idkpt_point_shadow_device_ptr(IdkPtCtx* ctx, int32_t index, void** devPtr, uint64_t* bytes) {
+    if (!ctx || !devPtr) return fail(ctx, IDKPT_ERR_INVALID_ARGUMENT, "idkpt_point_shadow_device_ptr: null argument");
+    if (index < 0 || (size_t)index >= ctx->pointShadowRecs.size()) return fail(ctx, IDKPT_ERR_INVALID_ARGUMENT, "idkpt_point_shadow_device_ptr: shadow index out of range");
+    const PointShadowDev& r = ctx->pointShadowRecs[index];
+    *devPtr = (uint16_t*)ctx->pointShadowMaps.p + r.offset;
+    if (bytes) *bytes = 6 * (uint64_t)r.size * (uint64_t)r.size * 2;
+    return IDKPT_OK;
+}
+
+IDKPT_API int idkpt_read_point_shadow(IdkPtCtx* ctx, int32_t index, uint16_t* dst, uint64_t bytes) {
+    if (!ctx || !dst) return fail(ctx, IDKPT_ERR_INVALID_ARGUMENT, "idkpt_read_point_shadow: null argument");
+    if (index < 0 || (size_t)index >= ctx->pointShadowRecs.size()) return fail(ctx, IDKPT_ERR_INVALID_ARGUMENT, "idkpt_read_point_shadow: shadow index out of range");
+    const PointShadowDev& r = ctx->pointShadowRecs[index];
+    const uint64_t need = 6 * (uint64_t)r.size * (uint64_t)r.size * 2;
+    if (bytes < need) return fail(ctx, IDKPT_ERR_INVALID_ARGUMENT, "idkpt_read_point_shadow: buffer too small");
+    CK(cudaSetDevice(ctx->device));
+    CK(cudaMemcpyAsync(dst, (const uint16_t*)ctx->pointShadowMaps.p + r.offset, need, cudaMemcpyDeviceToHost, ctx->stream));
+    CK(cudaStreamSynchronize(ctx->stream));
+    return IDKPT_OK;
 }
 
 } // extern "C"

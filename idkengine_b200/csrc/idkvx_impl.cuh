@@ -24,7 +24,9 @@ struct IdkVxCtx : IdkCtxBase {
     DevBuf scratch[4];                    // idkvx_cone_trace_rows: device copies of the G-buffer rows and of the output, kept between calls
     bool slabMode = false;                // idkvx_set_slab: voxelise one z-slab, no mip chain (the host all-gathers the slabs first)
     IdkPtCtx* shadowTracer = nullptr;     // idkvx_set_shadow_tracer: visibility of point-shadowed lights by shadow rays through this scene
+    IdkPtCtx* shadowMaps = nullptr;       // idkvx_set_shadow_maps: visibility by the PCF lookup into this context's point-shadow cube maps
     bool shadowedLights = false;
+    int32_t maxPointShadowIndex = -1;     // largest PointShadowIndex of the scene's lights
 };
 
 static void set_grid_bounds(IdkVxCtx* ctx, const float* mn, const float* mx) {
@@ -126,7 +128,9 @@ IDKPT_API int idkvx_set_scene(IdkVxCtx* ctx, const IdkPtSceneDesc* s) {
     if (int rc = validate_scene(ctx, "idkvx_set_scene", s)) return rc;
     ctx->haveScene = false;   // the device arrays are overwritten from here on: a failure below leaves no scene
     ctx->shadowedLights = false;
-    for (uint64_t i = 0; i < s->LightCount; i++) ctx->shadowedLights = ctx->shadowedLights || s->Lights[i].PointShadowIndex >= 0;
+    ctx->maxPointShadowIndex = -1;
+    for (uint64_t i = 0; i < s->LightCount; i++) ctx->maxPointShadowIndex = std::max(ctx->maxPointShadowIndex, s->Lights[i].PointShadowIndex);
+    ctx->shadowedLights = ctx->maxPointShadowIndex >= 0;
     int rc;
     if ((rc = upload(ctx, ctx->positions, s->VertexPositions, s->VertexPositionCount * sizeof(PackedVec3)))) return rc;
     if ((rc = upload(ctx, ctx->vertices, s->Vertices, s->VertexCount * sizeof(GpuVertex)))) return rc;
@@ -168,11 +172,22 @@ IDKPT_API int idkvx_voxelize(IdkVxCtx* ctx, IdkVxStats* stats) {
     if (!ctx) return IDKPT_ERR_INVALID_ARGUMENT;
     if (!ctx->haveScene) return fail(ctx, IDKPT_ERR_NO_SCENE, "idkvx_voxelize: idkvx_set_scene has not been called");
     // fragment.glsl:55-58: lights with PointShadowIndex >= 0 are multiplied by Visibility(), a PCF lookup into the shadow cube
-    // map the rasteriser renders. Without a rasteriser the same question -- is the (2 % biased) sample point visible from the
-    // light -- is answered by an any-hit shadow ray through the path tracer's BVH (idkvx_set_shadow_tracer).
+    // map. With shadow maps attached that lookup runs on the path tracer's traced cube maps (idkvx_set_shadow_maps); otherwise
+    // the same question -- is the (2 % biased) sample point visible from the light -- is answered by an any-hit shadow ray
+    // through the path tracer's BVH (idkvx_set_shadow_tracer).
     size_t shadowSmem = 0;
     ctx->sc.occValid = 0;
-    if (ctx->shadowedLights) {
+    ctx->sc.psmValid = 0;
+    if (ctx->shadowedLights && ctx->shadowMaps) {
+        IdkPtCtx* pt = ctx->shadowMaps;
+        if (pt->device != ctx->device) return fail(ctx, IDKPT_ERR_UNSUPPORTED, "idkvx_voxelize: the shadow-map context is on another device");
+        if ((size_t)ctx->maxPointShadowIndex >= pt->pointShadowRecs.size())
+            return fail(ctx, IDKPT_ERR_INVALID_ARGUMENT, "idkvx_voxelize: a light's PointShadowIndex is not below the shadow-map context's shadow count (idkpt_set_point_shadows)");
+        ctx->sc.psm.shadows = (const PointShadowDev*)pt->pointShadowDev.p;
+        ctx->sc.psm.texels = (const uint16_t*)pt->pointShadowMaps.p;
+        ctx->sc.psm.count = (uint32_t)pt->pointShadowRecs.size();
+        ctx->sc.psmValid = 1;
+    } else if (ctx->shadowedLights) {
         IdkPtCtx* pt = ctx->shadowTracer;
         if (!pt || !pt->haveScene || pt->device != ctx->device)
             return fail(ctx, IDKPT_ERR_UNSUPPORTED, "idkvx_voxelize: the scene has point-shadowed lights (PointShadowIndex >= 0): give the voxeliser a path-tracer context "
@@ -258,6 +273,12 @@ IDKPT_API int idkvx_mipmap(IdkVxCtx* ctx, IdkVxStats* stats) {
 IDKPT_API int idkvx_set_shadow_tracer(IdkVxCtx* ctx, IdkPtCtx* pathTracer) {
     if (!ctx) return IDKPT_ERR_INVALID_ARGUMENT;
     ctx->shadowTracer = pathTracer;
+    return IDKPT_OK;
+}
+
+IDKPT_API int idkvx_set_shadow_maps(IdkVxCtx* ctx, IdkPtCtx* pathTracer) {
+    if (!ctx) return IDKPT_ERR_INVALID_ARGUMENT;
+    ctx->shadowMaps = pathTracer;
     return IDKPT_OK;
 }
 

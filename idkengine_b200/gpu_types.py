@@ -30,6 +30,8 @@ GpuUnskinnedVertex = np.dtype([("JointIndices", u4, 4), ("JointWeights", f4, 4),
 IdkPtSkinningCmd = np.dtype([("InputVertexOffset", u4), ("OutputVertexOffset", u4), ("JointMatricesOffset", u4), ("VertexCount", u4)])
 GpuLight = np.dtype([("Position", f4, 3), ("Radius", f4), ("Color", f4, 3), ("PointShadowIndex", i4),
                      ("PrevPosition", f4, 3), ("_pad0", f4)])
+GpuPointShadow = np.dtype([("Texture", u8), ("ShadowTexture", u8), ("ProjViewMatrices", f4, (6, 16)), ("Position", f4, 3),
+                           ("NearPlane", f4), ("RayTracedShadowTexture", u8), ("FarPlane", f4), ("LightIndex", i4)])
 GpuPerFrameData = np.dtype([
     ("ProjView", f4, 16), ("View", f4, 16), ("InvView", f4, 16), ("PrevView", f4, 16),
     ("ViewPos", f4, 3), ("Frame", u4),
@@ -47,7 +49,7 @@ IdkPtHit = np.dtype([("BaryX", f4), ("BaryY", f4), ("T", f4), ("TriangleId", u4)
 EXPECTED_SIZES = {
     "GpuBlasNode": 32, "GpuBlasTriangle": 16, "GpuBlasDesc": 40, "GpuBlasInstance": 8, "GpuTlasNode": 32,
     "GpuMeshTransform": 144, "GpuMesh": 96, "GpuMaterial": 96, "GpuVertex": 16, "PackedVec3": 12,
-    "GpuLight": 48, "GpuPerFrameData": 544, "GpuWavefrontRay": 48, "GpuAovRay": 32, "IdkPtGpuSettings": 20,
+    "GpuLight": 48, "GpuPointShadow": 432, "GpuPerFrameData": 544, "GpuWavefrontRay": 48, "GpuAovRay": 32, "IdkPtGpuSettings": 20,
     "IdkPtRay": 32, "IdkPtHit": 32, "GpuUnskinnedVertex": 52, "IdkPtSkinningCmd": 16,
 }
 for _name, _size in EXPECTED_SIZES.items():

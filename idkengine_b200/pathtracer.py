@@ -311,6 +311,42 @@ class PathTracer:
                                                        samples, noise_index, jit.ctypes.data, vis.ctypes.data, ctypes.byref(ms)), "idkpt_shadows_ray_traced")
         return vis, ms.value
 
+    # ---- point-shadow cube maps (PointShadowManager.UpdateBuffer / RenderShadowMaps)
+    def SetPointShadows(self, shadows, sizes):
+        """GpuPointShadow records (gpu_types.GpuPointShadow) and the face size of each cube map. Same sizes as the last call:
+        the maps are kept; otherwise they are reallocated and cleared to 65535."""
+        shadows = np.ascontiguousarray(shadows, gt.GpuPointShadow)
+        sizes = np.ascontiguousarray(sizes, np.int32)
+        assert len(shadows) == len(sizes)
+        self._point_shadow_sizes = [int(n) for n in sizes]
+        self._check(self._lib.idkpt_set_point_shadows(self._ctx, shadows.ctypes.data if len(shadows) else None,
+                                                      sizes.ctypes.data if len(sizes) else None, len(shadows)), "idkpt_set_point_shadows")
+
+    def RenderPointShadows(self, first=0, count=None, face_masks=None):
+        """Renders shadows [first, first + count) (default: all set ones); face_masks: one 6-bit mask per shadow (None = all
+        faces). Returns the kernel time in ms."""
+        if count is None:
+            count = len(getattr(self, "_point_shadow_sizes", [])) - first
+        masks = None if face_masks is None else np.ascontiguousarray(face_masks, np.uint32)
+        if masks is not None:
+            assert len(masks) == count
+        ms = ctypes.c_float()
+        self._check(self._lib.idkpt_render_point_shadows(self._ctx, first, count, masks.ctypes.data if masks is not None else None,
+                                                         ctypes.byref(ms)), "idkpt_render_point_shadows")
+        return ms.value
+
+    def ReadPointShadow(self, index):
+        """One shadow's cube map as uint16 [6, N, N] (face +X,-X,+Y,-Y,+Z,-Z; row y = t; D16, 65535 = nothing)."""
+        n = self._point_shadow_sizes[index] if 0 <= index < len(getattr(self, "_point_shadow_sizes", [])) else 1
+        out = np.zeros((6, n, n), np.uint16)
+        self._check(self._lib.idkpt_read_point_shadow(self._ctx, index, out.ctypes.data, out.nbytes), "idkpt_read_point_shadow")
+        return out
+
+    def PointShadowDevicePtr(self, index):
+        p, n = ctypes.c_void_p(), ctypes.c_uint64()
+        self._check(self._lib.idkpt_point_shadow_device_ptr(self._ctx, index, ctypes.byref(p), ctypes.byref(n)), "idkpt_point_shadow_device_ptr")
+        return p.value, n.value
+
     # ---- properties with the reference's reset-on-set behaviour
     def _reset_prop(name, sub=None):  # noqa: N805
         def get(self):

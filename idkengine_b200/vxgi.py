@@ -26,7 +26,7 @@ class IdkVxStats(ctypes.Structure):
 
 VX_EXPORTS = ["idkvx_create", "idkvx_destroy", "idkvx_last_error", "idkvx_set_scene", "idkvx_set_grid", "idkvx_level_count",
               "idkvx_voxelize", "idkvx_read_level", "idkvx_cone_trace", "idkvx_set_shadow_tracer",
-              "idkvx_set_slab", "idkvx_level_device_ptr", "idkvx_mipmap", "idkvx_cone_trace_rows"]
+              "idkvx_set_shadow_maps", "idkvx_set_slab", "idkvx_level_device_ptr", "idkvx_mipmap", "idkvx_cone_trace_rows"]
 
 DEFAULT_GRID_MIN = (-28.0, -3.0, -17.0)   # RasterPipeline.cs:213
 DEFAULT_GRID_MAX = (28.0, 20.0, 17.0)
@@ -79,6 +79,8 @@ def _declare(L):
     L.idkvx_cone_trace_rows.argtypes = [c_vp, c_vp, P(IdkVxConeSettings), c_vp, c_vp, c_vp, c_i32, c_i32, c_i32, c_i32, P(c_f * 3), c_vp, P(IdkVxStats)]
     L.idkvx_set_shadow_tracer.restype = c_i32
     L.idkvx_set_shadow_tracer.argtypes = [c_vp, c_vp]
+    L.idkvx_set_shadow_maps.restype = c_i32
+    L.idkvx_set_shadow_maps.argtypes = [c_vp, c_vp]
     L.idkvx_read_level.restype = c_i32
     L.idkvx_read_level.argtypes = [c_vp, c_i32, c_vp, c_u64]
     L.idkvx_cone_trace.restype = c_i32
@@ -122,6 +124,11 @@ class Voxelizer:
     def SetShadowTracer(self, path_tracer):
         """Shadow rays for lights with PointShadowIndex >= 0 go through this PathTracer's scene (None detaches)."""
         self._check(self._lib.idkvx_set_shadow_tracer(self._ctx, path_tracer._ctx if path_tracer is not None else None), "idkvx_set_shadow_tracer")
+
+    def SetShadowMaps(self, path_tracer):
+        """Lights with PointShadowIndex >= 0 are filtered through this PathTracer's point-shadow cube maps (PCF lookup;
+        SetPointShadows / RenderPointShadows). Takes precedence over SetShadowTracer; None detaches."""
+        self._check(self._lib.idkvx_set_shadow_maps(self._ctx, path_tracer._ctx if path_tracer is not None else None), "idkvx_set_shadow_maps")
 
     # ---- multi-GPU: z-slab voxelisation, gather, mip chain, screen-tiled cone trace (include/idkvx.h)
     def SetSlab(self, z0, z1):

@@ -165,6 +165,23 @@ typedef struct GpuLight {
 IDK_STATIC_ASSERT(sizeof(GpuLight) == 48, "GpuLight must be 48 bytes");
 #define IDK_GPU_MAX_UBO_LIGHT_COUNT 256 /* StaticUniformBuffers.glsl:6 */
 
+/* SRC/GpuTypes/GpuPointShadow.cs:7-41, GpuTypes.glsl:104-120 (std140, 432 bytes): what CpuPointShadow.GetGpuPointShadow()
+ * returns. libidkpt reads Position, NearPlane and FarPlane; the bindless handles and the six face matrices
+ * (+X,-X,+Y,-Y,+Z,-Z, OpenTK row-vector view * projection) are carried so the engine can pass the struct as it is. */
+typedef struct GpuPointShadow {
+    uint64_t Texture;
+    uint64_t ShadowTexture;
+    float    ProjViewMatrices[6][16];
+    float    Position[3];
+    float    NearPlane;
+    uint64_t RayTracedShadowTexture;
+    float    FarPlane;
+    int32_t  LightIndex;
+} GpuPointShadow;
+IDK_STATIC_ASSERT(sizeof(GpuPointShadow) == 432, "GpuPointShadow must be 432 bytes");
+IDK_STATIC_ASSERT(offsetof(GpuPointShadow, Position) == 400, "GpuPointShadow.Position offset");
+IDK_STATIC_ASSERT(offsetof(GpuPointShadow, FarPlane) == 424, "GpuPointShadow.FarPlane offset");
+
 /* SRC/GpuTypes/GpuPerFrameData.cs:5-21, GpuTypes.glsl:74-90 (UBO 1).
  * Matrices are OpenTK row-vector matrices uploaded raw, i.e. GLSL sees
  * column c = the 4 floats at [c*4 .. c*4+3]:  (M*v)[i] = sum_c M[c*4+i]*v[c]. */

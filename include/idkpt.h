@@ -289,6 +289,26 @@ IDKPT_API int idkpt_shadows_ray_traced(IdkPtCtx* ctx, const GpuPerFrameData* fra
                                        int32_t width, int32_t height, int32_t light_index, int32_t samples, uint32_t noise_index,
                                        const float* taa_jitter, float* visibility_out, float* kernel_ms);
 
+/* ---- point-shadow cube maps (PointShadowManager.UpdateBuffer / RenderShadowMaps, CpuPointShadow.RenderShadowMap) ----
+ * idkpt_set_point_shadows: the engine's GpuPointShadow array (count <= IDKPT_MAX_POINT_SHADOWS) and the face size of each
+ *   shadow's cube map (1..16384). Only Position, NearPlane (> 0) and FarPlane (> NearPlane) are read. The maps are one device
+ *   allocation of 6*size^2 uint16 (D16) per shadow, face-major (+X,-X,+Y,-Y,+Z,-Z), row y = t of GL table 8.19, x fastest.
+ *   A call whose sizes equal the previous call's keeps the maps; otherwise they are reallocated and every texel is 65535.
+ * idkpt_render_point_shadows: shadows [first, first + count). Texel (x, y) of face f stores the D16 depth of the closest
+ *   surface along the ray through its centre (GetLogarithmicDepth, Math.glsl:59-66, near/far clipped; 65535 = nothing),
+ *   which is what the engine's raster pass stores there. face_masks[i] (bit f = face f, NULL = all six) selects the faces
+ *   written for shadow first + i; the other faces keep their texels (the camera-frustum face culling of
+ *   CpuPointShadow.RenderShadowMap:125-145 is the host's). Synchronous; kernel_ms may be NULL.
+ * idkpt_read_point_shadow copies one shadow's 6*size^2*2 bytes to the host; idkpt_point_shadow_device_ptr hands the device
+ *   copy over for interop (valid until the next idkpt_set_point_shadows with other sizes, or idkpt_set_scene).
+ * The scene must be set first, and idkpt_set_scene drops the shadows. The maps show the scene as it was at the last render:
+ * re-render after idkpt_blas_refit / idkpt_tlas_build, as the engine does every frame. */
+#define IDKPT_MAX_POINT_SHADOWS 128   /* GPU_MAX_UBO_POINT_SHADOW_COUNT */
+IDKPT_API int idkpt_set_point_shadows(IdkPtCtx* ctx, const GpuPointShadow* shadows, const int32_t* sizes, uint32_t count);
+IDKPT_API int idkpt_render_point_shadows(IdkPtCtx* ctx, uint32_t first, uint32_t count, const uint32_t* face_masks, float* kernel_ms);
+IDKPT_API int idkpt_read_point_shadow(IdkPtCtx* ctx, int32_t index, uint16_t* dst, uint64_t bytes);
+IDKPT_API int idkpt_point_shadow_device_ptr(IdkPtCtx* ctx, int32_t index, void** dev_ptr, uint64_t* bytes);
+
 /* ---- dynamic geometry (SURVEY.md 8f.2): ModelManager.Update = skin -> refit -> TLAS (ModelManager.cs:236-261) ----
  * idkpt_set_skinning_data: unskinnedVertexSSBO upload (52-byte GpuUnskinnedVertex records).
  * idkpt_skin_vertices: uploads the joint matrices (row-major mat4x3 = 3 x vec4 each, ModelManager.cs:272-277) and runs

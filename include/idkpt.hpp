@@ -166,6 +166,21 @@ public:
                           uint32_t noiseIndex, const float* taaJitter, float* visibilityInOut) {
         check(idkpt_shadows_ray_traced(ctx_, &frame, depth, normalRG, width, height, lightIndex, samples, noiseIndex, taaJitter, visibilityInOut, nullptr), "idkpt_shadows_ray_traced");
     }
+    // PointShadowManager.UpdateBuffer / RenderShadowMaps: traced D16 cube maps, 6 * size^2 uint16 per shadow (idkpt.h)
+    void SetPointShadows(const GpuPointShadow* shadows, const int32_t* sizes, uint32_t count) {
+        check(idkpt_set_point_shadows(ctx_, shadows, sizes, count), "idkpt_set_point_shadows");
+    }
+    float RenderPointShadows(uint32_t first, uint32_t count, const uint32_t* faceMasks = nullptr) {
+        float ms = 0.0f;
+        check(idkpt_render_point_shadows(ctx_, first, count, faceMasks, &ms), "idkpt_render_point_shadows");
+        return ms;
+    }
+    void ReadPointShadow(int32_t index, uint16_t* dst, uint64_t bytes) { check(idkpt_read_point_shadow(ctx_, index, dst, bytes), "idkpt_read_point_shadow"); }
+    void* PointShadowDevicePtr(int32_t index, uint64_t* bytes = nullptr) {
+        void* p = nullptr;
+        check(idkpt_point_shadow_device_ptr(ctx_, index, &p, bytes), "idkpt_point_shadow_device_ptr");
+        return p;
+    }
     void SetSkinningData(const GpuUnskinnedVertex* vertices, uint64_t count) { check(idkpt_set_skinning_data(ctx_, vertices, count), "idkpt_set_skinning_data"); }
     void SkinVertices(const float* jointMatrices3x4, uint64_t jointCount, const IdkPtSkinningCmd* cmds, uint32_t cmdCount) {
         check(idkpt_skin_vertices(ctx_, jointMatrices3x4, jointCount, cmds, cmdCount, nullptr), "idkpt_skin_vertices");
@@ -229,6 +244,9 @@ public:
     void SetGrid(const float gridMin[3], const float gridMax[3]) { check(idkvx_set_grid(ctx_, gridMin, gridMax), "idkvx_set_grid"); }   // GridMin / GridMax setters
     int LevelCount() const { return idkvx_level_count(ctx_); }
     IdkVxStats Render() { IdkVxStats st = {}; check(idkvx_voxelize(ctx_, &st), "idkvx_voxelize"); return st; }
+    // point-shadowed lights: PCF lookup into a path tracer's cube maps, or shadow rays through its BVH (idkvx.h); nullptr detaches
+    void SetShadowMaps(const PathTracer* pt) { check(idkvx_set_shadow_maps(ctx_, pt ? pt->Handle() : nullptr), "idkvx_set_shadow_maps"); }
+    void SetShadowTracer(const PathTracer* pt) { check(idkvx_set_shadow_tracer(ctx_, pt ? pt->Handle() : nullptr), "idkvx_set_shadow_tracer"); }
     // ConeTracer.Compute: G-buffer attachments in, rgba32f indirect light out (width * height * 4 floats)
     std::vector<float> ConeTrace(const GpuPerFrameData& frame, const IdkVxConeSettings& settings, const float* depth, const float* normalRG,
                                  const float* metallicRoughness, int width, int height, const float skyColor[3], IdkVxStats* stats = nullptr) {

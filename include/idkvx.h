@@ -67,13 +67,19 @@ IDKPT_API int32_t idkvx_level_count(IdkVxCtx* ctx);                             
 IDKPT_API int idkvx_voxelize(IdkVxCtx* ctx, IdkVxStats* stats);
 
 /* rgba16f texels of one mip level, x fastest (size = w*h*d*8 bytes). */
-/* Lights with PointShadowIndex >= 0 are attenuated by Visibility() in the fragment stage (Voxelize/fragment.glsl:55-58,100-115),
- * a PCF lookup into the shadow cube map the rasteriser renders (PointShadowManager). Without a rasteriser the voxeliser asks the
- * same question with an any-hit shadow ray from the 2 %-biased sample point to the light through the BVH of a path-tracer
- * context holding the same scene on the same device (hard shadows instead of the PCF-filtered lookup). NULL detaches.
- * A scene with such lights cannot be voxelised without it (IDKPT_ERR_UNSUPPORTED). */
+/* Lights with PointShadowIndex >= 0 are attenuated by Visibility() in the fragment stage (Voxelize/fragment.glsl:55-58,100-117),
+ * a PCF lookup into the shadow cube map the rasteriser renders (PointShadowManager). The voxeliser evaluates it in one of two
+ * modes, each taking a path-tracer context on the same device (NULL detaches):
+ *   shadow maps (idkvx_set_shadow_maps): the PCF lookup itself -- 2 % biased reference depth, seamless bilinear footprint,
+ *     compare LESS -- into the cube maps of that context (idkpt_set_point_shadows / idkpt_render_point_shadows), at the
+ *     light's PointShadowIndex. An index >= the context's shadow count fails with IDKPT_ERR_INVALID_ARGUMENT.
+ *   shadow tracer (idkvx_set_shadow_tracer): an any-hit shadow ray from the 2 %-biased sample point to the light through the
+ *     BVH of a context holding the same scene (hard 0/1 shadows instead of the filtered lookup; needs no cube-map memory).
+ * Shadow maps take precedence when both are attached. A scene with such lights cannot be voxelised with neither
+ * (IDKPT_ERR_UNSUPPORTED). */
 struct IdkPtCtx;
 IDKPT_API int idkvx_set_shadow_tracer(IdkVxCtx* ctx, struct IdkPtCtx* path_tracer);
+IDKPT_API int idkvx_set_shadow_maps(IdkVxCtx* ctx, struct IdkPtCtx* path_tracer);
 IDKPT_API int idkvx_read_level(IdkVxCtx* ctx, int32_t level, void* dst_rgba16f, uint64_t bytes);
 
 /* ConeTracer.Compute(): per pixel of a width x height G-buffer (host arrays: depth [w*h], normal = octahedral rg
