@@ -97,9 +97,20 @@ EXPORTS = [
     "idkpt_set_skinning_data", "idkpt_skin_vertices", "idkpt_blas_refit", "idkpt_read_range", "idkpt_post_process", "idkpt_ldr_device_ptr", "idkpt_abi_version",
     "idkpt_denoise", "idkpt_denoise_device_ptrs", "idkpt_denoise_import_output", "idkpt_tlas_build",
     "idkpt_set_point_shadows", "idkpt_render_point_shadows", "idkpt_read_point_shadow", "idkpt_point_shadow_device_ptr",
+    "idkpt_volumetric_lighting", "idkpt_volumetric_device_ptr",
 ]
 
 IDKPT_MAX_POINT_SHADOWS = 128
+
+
+class IdkPtVolumetricSettings(ctypes.Structure):
+    _fields_ = [("Absorbance", c_f * 3), ("SampleCount", c_i32), ("Scattering", c_f), ("MaxDist", c_f), ("Strength", c_f),
+                ("ResolutionScale", c_f)]
+
+
+def default_volumetric_settings():
+    """VolumetricLighting.GpuSettings defaults (VolumetricLighting.cs:10-21) and its ResolutionScale of 0.6."""
+    return IdkPtVolumetricSettings((c_f * 3)(0.025, 0.025, 0.025), 5, 0.758, 50.0, 0.1, 0.6)
 
 
 class IdkPtDenoiseSettings(ctypes.Structure):
@@ -308,6 +319,10 @@ def load(path=None):
     L.idkpt_read_point_shadow.argtypes = [c_vp, c_i32, c_vp, c_u64]
     L.idkpt_point_shadow_device_ptr.restype = c_i32
     L.idkpt_point_shadow_device_ptr.argtypes = [c_vp, c_i32, P(c_vp), P(c_u64)]
+    L.idkpt_volumetric_lighting.restype = c_i32
+    L.idkpt_volumetric_lighting.argtypes = [c_vp, c_vp, P(IdkPtVolumetricSettings), c_vp, c_i32, c_i32, c_i32, c_i32, c_vp, c_vp, P(c_f)]
+    L.idkpt_volumetric_device_ptr.restype = c_i32
+    L.idkpt_volumetric_device_ptr.argtypes = [c_vp, P(c_vp), P(c_u64)]
     L.idkpt_abi_version.restype = c_u32
     L.idkpt_abi_version.argtypes = []
     if path == _build.LIBIDKPT:

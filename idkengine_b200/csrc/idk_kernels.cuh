@@ -796,19 +796,27 @@ __device__ __forceinline__ CubeTexel cube_texel_edge(int face, int x, int y, int
     return CubeTexel{nf, (ns + size - 1) / 2, (nt + size - 1) / 2};
 }
 
-// The bilinear footprint of direction d on a cube map of face size `size`: GL face selection (spec table 8.19), the four taps
-// t00, t10, t01, t11 (x fastest), seamless across edges, and the weights fx, fy. At a cube corner exactly one tap lies outside
-// the face in both directions and no face holds it (corner = its index 0..3, else -1); the caller replaces it by the mean of
-// the other three. The sky lookup and the point-shadow PCF lookup (idk_point_shadows.cuh) share this.
-struct CubeFootprint { CubeTexel t00, t10, t01, t11; float fx, fy; int corner; };
-__device__ __forceinline__ CubeFootprint cube_footprint(f3 d, int size) {
+// GL cube-map face selection (spec table 8.19, ties x >= y >= z): the face of direction d and its (s, t) in [0, 1]. The
+// bilinear footprint below and the volumetric pass's nearest lookup (idk_volumetric.cuh) share this.
+__device__ __forceinline__ int cube_face_st(f3 d, float& s, float& t) {
     const float ax = fabsf(d.x), ay = fabsf(d.y), az = fabsf(d.z);
     int face;
     float scc, tc, ma;
     if (ax >= ay && ax >= az) { face = d.x >= 0.0f ? 0 : 1; scc = d.x >= 0.0f ? -d.z : d.z; tc = -d.y; ma = ax; }
     else if (ay >= az) { face = d.y >= 0.0f ? 2 : 3; scc = d.x; tc = d.y >= 0.0f ? d.z : -d.z; ma = ay; }
     else { face = d.z >= 0.0f ? 4 : 5; scc = d.z >= 0.0f ? d.x : -d.x; tc = -d.y; ma = az; }
-    const float s = 0.5f * (scc / ma + 1.0f), t = 0.5f * (tc / ma + 1.0f);
+    s = 0.5f * (scc / ma + 1.0f); t = 0.5f * (tc / ma + 1.0f);
+    return face;
+}
+
+// The bilinear footprint of direction d on a cube map of face size `size`: GL face selection (spec table 8.19), the four taps
+// t00, t10, t01, t11 (x fastest), seamless across edges, and the weights fx, fy. At a cube corner exactly one tap lies outside
+// the face in both directions and no face holds it (corner = its index 0..3, else -1); the caller replaces it by the mean of
+// the other three. The sky lookup and the point-shadow PCF lookup (idk_point_shadows.cuh) share this.
+struct CubeFootprint { CubeTexel t00, t10, t01, t11; float fx, fy; int corner; };
+__device__ __forceinline__ CubeFootprint cube_footprint(f3 d, int size) {
+    float s, t;
+    const int face = cube_face_st(d, s, t);
     const float px = s * (float)size - 0.5f, py = t * (float)size - 0.5f;
     const float fx0 = floorf(px), fy0 = floorf(py);
     CubeFootprint fp;

@@ -18,11 +18,13 @@
 #include "idk_dynamic.cuh"
 #include "idk_post.cuh"
 #include "idk_point_shadows.cuh"
+#include "idk_volumetric.cuh"
 #include "idk_textures_host.h"
 
 #define IDKPT_ABI_VERSION 4u   // 2: IdkPtSceneDesc gained Textures / TextureCount; 3: IdkPtStats gained CompactMs / AccumulateMs, host-buffer registration;
                                // 4: gather handle blob is 5 IPC handles (320 bytes), IDKPT_CREATE_GLOBAL_SLOTS, idkpt_gather_connect.
-                               // Entry points added since (point-shadow cube maps, idkvx_set_shadow_maps) are additive and keep 4.
+                               // Entry points added since (point-shadow cube maps, idkvx_set_shadow_maps, volumetric lighting) are
+                               // additive and keep 4.
 
 struct DevBuf {
     void* p = nullptr;
@@ -92,6 +94,11 @@ struct IdkPtCtx : IdkCtxBase {
     std::vector<int32_t> pointShadowSizes;
     std::vector<PointShadowDev> pointShadowRecs;
     DevBuf pointShadowDev, pointShadowMaps;
+    DevBuf pointShadowLights;      // int32 LightIndex per shadow (the volumetric pass's Lights[shadow.LightIndex])
+
+    // volumetric lighting (idkpt_volumetric_lighting): render-size rgba16f + r32f, presentation-size rgba16f
+    DevBuf volMarch, volDepth, volOut;
+    int volW = 0, volH = 0;        // presentation size of the last successful call (0: none since the scene was set)
 
     // present chain: bloom mip chains (rgba16f), AgX constants, RGBA8 frame
     DevBuf bloomDown, bloomUp, postConsts, ldr;
@@ -587,7 +594,7 @@ IDKPT_API void idkpt_destroy(IdkPtCtx* ctx) {
                      &ctx->tex.pixels, &ctx->tex.recs, &ctx->tex.srgbLut, &ctx->bloomDown, &ctx->bloomUp, &ctx->postConsts, &ctx->ldr,
                      &ctx->unskinned, &ctx->joints, &ctx->refitParents, &ctx->refitLocks, &ctx->scratch[0], &ctx->scratch[1], &ctx->scratch[2],
                      &ctx->tlasScratch, &ctx->oidn[0], &ctx->oidn[1], &ctx->oidn[2], &ctx->oidn[3], &ctx->denoiseWork[0], &ctx->denoiseWork[1], &ctx->denoised,
-                     &ctx->pointShadowDev, &ctx->pointShadowMaps};
+                     &ctx->pointShadowDev, &ctx->pointShadowMaps, &ctx->pointShadowLights, &ctx->volMarch, &ctx->volDepth, &ctx->volOut};
     for (DevBuf* b : all) release(*b);
     for (int i = 0; i < IDK_MAX_LANES; i++) release_lane(ctx->lanes[i], false);
     for (cudaEvent_t ev : ctx->events) cudaEventDestroy(ev);
@@ -632,7 +639,9 @@ IDKPT_API int idkpt_set_scene(IdkPtCtx* ctx, const IdkPtSceneDesc* s) {
     // pointers and counts looking valid.
     ctx->haveScene = false;
     ctx->pointShadows.clear(); ctx->pointShadowSizes.clear(); ctx->pointShadowRecs.clear();   // the shadows belong to the old scene
-    release(ctx->pointShadowDev); release(ctx->pointShadowMaps);
+    release(ctx->pointShadowDev); release(ctx->pointShadowMaps); release(ctx->pointShadowLights);
+    release(ctx->volMarch); release(ctx->volDepth); release(ctx->volOut);
+    ctx->volW = ctx->volH = 0;
     int rc;
     // nodes and triangle records share one allocation ("bvh"): [nodes | triRec], so that one L2 access-policy window covers both
     const size_t nodeBytes = ((s->BlasNodeCount * sizeof(GpuBlasNode)) + 255) & ~(size_t)255;
@@ -1314,7 +1323,7 @@ static int preload_kernels(IdkPtCtx* ctx) {
     IDK_PRELOAD(k_skin_vertices); IDK_PRELOAD(k_refit_prepare); IDK_PRELOAD(k_refit_climb); IDK_PRELOAD(k_tlas_build);
     IDK_PRELOAD(k_bloom_down); IDK_PRELOAD(k_bloom_up); IDK_PRELOAD(k_agx_matrices); IDK_PRELOAD(k_tonemap);
     IDK_PRELOAD(k_denoise_prepare); IDK_PRELOAD(k_denoise_atrous); IDK_PRELOAD(k_denoise_finish); IDK_PRELOAD(k_denoise_import);
-    IDK_PRELOAD(k_bcn_decode); IDK_PRELOAD(k_point_shadow_faces);
+    IDK_PRELOAD(k_bcn_decode); IDK_PRELOAD(k_point_shadow_faces); IDK_PRELOAD(k_volumetric_march); IDK_PRELOAD(k_volumetric_upscale);
 #undef IDK_PRELOAD
     return IDKPT_OK;
 }
@@ -1864,8 +1873,10 @@ IDKPT_API int idkpt_set_point_shadows(IdkPtCtx* ctx, const GpuPointShadow* shado
     }
     CK(cudaSetDevice(ctx->device));
     std::vector<PointShadowDev> recs(count);
+    std::vector<int32_t> lightIndex(count);   // checked against the light count where it is read (idkpt_volumetric_lighting)
     size_t texels = 0;
     for (uint32_t i = 0; i < count; i++) {
+        lightIndex[i] = shadows[i].LightIndex;
         PointShadowDev& r = recs[i];
         for (int k = 0; k < 3; k++) r.pos[k] = shadows[i].Position[k];
         r.nearPlane = shadows[i].NearPlane; r.farPlane = shadows[i].FarPlane;
@@ -1884,6 +1895,7 @@ IDKPT_API int idkpt_set_point_shadows(IdkPtCtx* ctx, const GpuPointShadow* shado
         CK(cudaMemsetAsync(ctx->pointShadowMaps.p, 0xFF, texels * 2, ctx->stream));
     }
     if (int rc = upload(ctx, ctx->pointShadowDev, recs.data(), recs.size() * sizeof(PointShadowDev))) return rc;
+    if (int rc = upload(ctx, ctx->pointShadowLights, lightIndex.data(), lightIndex.size() * sizeof(int32_t))) return rc;
     CK(cudaStreamSynchronize(ctx->stream));
     ctx->pointShadows.assign(shadows, shadows + count);
     ctx->pointShadowSizes.assign(sizes, sizes + count);
@@ -1939,6 +1951,63 @@ IDKPT_API int idkpt_read_point_shadow(IdkPtCtx* ctx, int32_t index, uint16_t* ds
     CK(cudaSetDevice(ctx->device));
     CK(cudaMemcpyAsync(dst, (const uint16_t*)ctx->pointShadowMaps.p + r.offset, need, cudaMemcpyDeviceToHost, ctx->stream));
     CK(cudaStreamSynchronize(ctx->stream));
+    return IDKPT_OK;
+}
+
+// ---- volumetric lighting (VolumetricLighting.Compute: march + depth-aware upscale) ---------------------------------------------
+IDKPT_API int idkpt_volumetric_lighting(IdkPtCtx* ctx, const GpuPerFrameData* frame, const IdkPtVolumetricSettings* s, const float* depth,
+                                        int32_t depthWidth, int32_t depthHeight, int32_t width, int32_t height, const float* taaJitter,
+                                        uint16_t* outRgba16f, float* kernelMs) {
+    if (!ctx || !frame || !s || !depth) return fail(ctx, IDKPT_ERR_INVALID_ARGUMENT, "idkpt_volumetric_lighting: null argument");
+    if (!ctx->haveScene) return fail(ctx, IDKPT_ERR_NO_SCENE, "idkpt_volumetric_lighting: no scene");
+    if (depthWidth < 1 || depthHeight < 1 || depthWidth > 16384 || depthHeight > 16384 || width < 1 || height < 1 || width > 16384 || height > 16384)
+        return fail(ctx, IDKPT_ERR_INVALID_ARGUMENT, "idkpt_volumetric_lighting: size outside 1..16384");
+    if (s->SampleCount < 1 || s->SampleCount > 1024) return fail(ctx, IDKPT_ERR_INVALID_ARGUMENT, "idkpt_volumetric_lighting: SampleCount outside 1..1024");
+    if (!(s->ResolutionScale > 0.0f && s->ResolutionScale <= 1.0f)) return fail(ctx, IDKPT_ERR_INVALID_ARGUMENT, "idkpt_volumetric_lighting: ResolutionScale not in (0, 1]");
+    // VolumetricLighting.SetSize: (Vector2i)((Vector2)PresentationResolution * ResolutionScale), truncated
+    const int w = (int)((float)width * s->ResolutionScale), h = (int)((float)height * s->ResolutionScale);
+    if (w < 1 || h < 1) return fail(ctx, IDKPT_ERR_INVALID_ARGUMENT, "idkpt_volumetric_lighting: render size of 0 (ResolutionScale too small for the size)");
+    for (const GpuPointShadow& ps : ctx->pointShadows)
+        if (ps.LightIndex < 0 || (uint64_t)ps.LightIndex >= ctx->counts.LightCount)
+            return fail(ctx, IDKPT_ERR_INVALID_ARGUMENT, "idkpt_volumetric_lighting: a shadow's LightIndex is not below the scene's light count");
+    CK(cudaSetDevice(ctx->device));
+    if (kernelMs) *kernelMs = 0.0f;
+    const size_t nDepth = (size_t)depthWidth * depthHeight, nRender = (size_t)w * h, nOut = (size_t)width * height;
+    DevBuf& dDepth = ctx->scratch[0];
+    if (ensure(dDepth, nDepth * 4) != cudaSuccess || ensure(ctx->volMarch, nRender * 8) != cudaSuccess ||
+        ensure(ctx->volDepth, nRender * 4) != cudaSuccess || ensure(ctx->volOut, nOut * 8) != cudaSuccess)
+        return fail(ctx, IDKPT_ERR_OUT_OF_MEMORY, "idkpt_volumetric_lighting: device allocation failed");
+    CK(cudaMemcpyAsync(dDepth.p, depth, nDepth * 4, cudaMemcpyHostToDevice, ctx->stream));
+    VolumetricMarchArgs a;
+    a.shadows = (const PointShadowDev*)ctx->pointShadowDev.p; a.lightIndex = (const int32_t*)ctx->pointShadowLights.p;
+    a.lights = ctx->sc.lights; a.maps = (const uint16_t*)ctx->pointShadowMaps.p; a.count = (int)ctx->pointShadowRecs.size();
+    a.gdepth = (const float*)dDepth.p; a.gw = depthWidth; a.gh = depthHeight;
+    a.color = (uint2*)ctx->volMarch.p; a.depth = (float*)ctx->volDepth.p; a.w = w; a.h = h;
+    memcpy(a.invProjView, frame->InvProjView, sizeof(a.invProjView));
+    for (int k = 0; k < 3; k++) { a.viewPos[k] = frame->ViewPos[k]; a.absorbance[k] = s->Absorbance[k]; }
+    a.jitter[0] = taaJitter ? taaJitter[0] : 0.0f; a.jitter[1] = taaJitter ? taaJitter[1] : 0.0f;
+    a.sampleCount = s->SampleCount; a.scattering = s->Scattering; a.strength = s->Strength; a.maxDist = s->MaxDist;
+    VolumetricUpscaleArgs b;
+    b.gdepth = a.gdepth; b.gw = depthWidth; b.gh = depthHeight;
+    b.march = PostImage{nullptr, (const uint2*)ctx->volMarch.p, w, h};
+    b.depth = (const float*)ctx->volDepth.p;
+    b.out = (uint2*)ctx->volOut.p; b.W = width; b.H = height;
+    b.nearPlane = frame->NearPlane; b.farPlane = frame->FarPlane;
+    const size_t tiles = (size_t)((w + 7) / 8) * (size_t)((h + 7) / 8);
+    const int rc = run_timed(ctx, "idkpt_volumetric_lighting", kernelMs, [&]() -> int {
+        k_volumetric_march<<<(unsigned)((tiles + 3) / 4), 256, 0, ctx->stream>>>(a);
+        k_volumetric_upscale<<<dim3((unsigned)((width + 31) / 32), (unsigned)((height + 7) / 8)), 256, 0, ctx->stream>>>(b);
+        return IDKPT_OK;
+    }, outRgba16f, ctx->volOut.p, outRgba16f ? nOut * 8 : 0);
+    if (rc == IDKPT_OK) { ctx->volW = width; ctx->volH = height; }
+    return rc;
+}
+
+IDKPT_API int idkpt_volumetric_device_ptr(IdkPtCtx* ctx, void** devPtr, uint64_t* bytes) {
+    if (!ctx || !devPtr) return fail(ctx, IDKPT_ERR_INVALID_ARGUMENT, "idkpt_volumetric_device_ptr: null argument");
+    if (!ctx->volW) return fail(ctx, IDKPT_ERR_INVALID_ARGUMENT, "idkpt_volumetric_device_ptr: call idkpt_volumetric_lighting first");
+    *devPtr = ctx->volOut.p;
+    if (bytes) *bytes = (uint64_t)ctx->volW * ctx->volH * 8;
     return IDKPT_OK;
 }
 

@@ -347,6 +347,30 @@ class PathTracer:
         self._check(self._lib.idkpt_point_shadow_device_ptr(self._ctx, index, ctypes.byref(p), ctypes.byref(n)), "idkpt_point_shadow_device_ptr")
         return p.value, n.value
 
+    # ---- volumetric lighting (VolumetricLighting.Compute)
+    def VolumetricLighting(self, frame, depth, width, height, settings=None, jitter=None, download=True):
+        """Volumetric point-light scattering through the point-shadow cube maps at width x height from the G-buffer depth
+        (float32 [Hg, Wg], any size). settings: capi.IdkPtVolumetricSettings (default: the engine's). Returns float16
+        [height, width, 4], or None with download=False (the image stays on the device: VolumetricDevicePtr). The kernel time
+        in ms is left in last_volumetric_ms."""
+        st = settings if settings is not None else capi.default_volumetric_settings()
+        d = np.ascontiguousarray(depth, np.float32)
+        jit = None if jitter is None else np.ascontiguousarray(jitter, np.float32)
+        frame = np.ascontiguousarray(frame)
+        out = np.zeros((height, width, 4), np.float16) if download else None
+        ms = ctypes.c_float()
+        self._check(self._lib.idkpt_volumetric_lighting(self._ctx, frame.ctypes.data, ctypes.byref(st), d.ctypes.data, d.shape[1], d.shape[0],
+                                                        width, height, jit.ctypes.data if jit is not None else None,
+                                                        out.ctypes.data if download else None, ctypes.byref(ms)), "idkpt_volumetric_lighting")
+        self.last_volumetric_ms = ms.value
+        return out
+
+    def VolumetricDevicePtr(self):
+        """(device pointer, bytes) of the last VolumetricLighting image (rgba16f)."""
+        p, n = ctypes.c_void_p(), ctypes.c_uint64()
+        self._check(self._lib.idkpt_volumetric_device_ptr(self._ctx, ctypes.byref(p), ctypes.byref(n)), "idkpt_volumetric_device_ptr")
+        return p.value, n.value
+
     # ---- properties with the reference's reset-on-set behaviour
     def _reset_prop(name, sub=None):  # noqa: N805
         def get(self):

@@ -166,7 +166,7 @@ IDK_STATIC_ASSERT(sizeof(GpuLight) == 48, "GpuLight must be 48 bytes");
 #define IDK_GPU_MAX_UBO_LIGHT_COUNT 256 /* StaticUniformBuffers.glsl:6 */
 
 /* SRC/GpuTypes/GpuPointShadow.cs:7-41, GpuTypes.glsl:104-120 (std140, 432 bytes): what CpuPointShadow.GetGpuPointShadow()
- * returns. libidkpt reads Position, NearPlane and FarPlane; the bindless handles and the six face matrices
+ * returns. libidkpt reads Position, NearPlane, FarPlane and LightIndex; the bindless handles and the six face matrices
  * (+X,-X,+Y,-Y,+Z,-Z, OpenTK row-vector view * projection) are carried so the engine can pass the struct as it is. */
 typedef struct GpuPointShadow {
     uint64_t Texture;

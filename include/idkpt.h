@@ -291,7 +291,8 @@ IDKPT_API int idkpt_shadows_ray_traced(IdkPtCtx* ctx, const GpuPerFrameData* fra
 
 /* ---- point-shadow cube maps (PointShadowManager.UpdateBuffer / RenderShadowMaps, CpuPointShadow.RenderShadowMap) ----
  * idkpt_set_point_shadows: the engine's GpuPointShadow array (count <= IDKPT_MAX_POINT_SHADOWS) and the face size of each
- *   shadow's cube map (1..16384). Only Position, NearPlane (> 0) and FarPlane (> NearPlane) are read. The maps are one device
+ *   shadow's cube map (1..16384). Position, NearPlane (> 0), FarPlane (> NearPlane) and LightIndex are read; LightIndex is
+ *   used only by idkpt_volumetric_lighting, which checks it against the scene's light count. The maps are one device
  *   allocation of 6*size^2 uint16 (D16) per shadow, face-major (+X,-X,+Y,-Y,+Z,-Z), row y = t of GL table 8.19, x fastest.
  *   A call whose sizes equal the previous call's keeps the maps; otherwise they are reallocated and every texel is 65535.
  * idkpt_render_point_shadows: shadows [first, first + count). Texel (x, y) of face f stores the D16 depth of the closest
@@ -308,6 +309,28 @@ IDKPT_API int idkpt_set_point_shadows(IdkPtCtx* ctx, const GpuPointShadow* shado
 IDKPT_API int idkpt_render_point_shadows(IdkPtCtx* ctx, uint32_t first, uint32_t count, const uint32_t* face_masks, float* kernel_ms);
 IDKPT_API int idkpt_read_point_shadow(IdkPtCtx* ctx, int32_t index, uint16_t* dst, uint64_t bytes);
 IDKPT_API int idkpt_point_shadow_device_ptr(IdkPtCtx* ctx, int32_t index, void** dev_ptr, uint64_t* bytes);
+
+/* ---- volumetric lighting (VolumetricLighting.Compute: VolumetricLight/compute.glsl + VolumetricLight/Upscale/compute.glsl) ----
+ * Ray-marched in-scattering of every point shadow's light through the cube maps of idkpt_set_point_shadows /
+ * idkpt_render_point_shadows (NEAREST lookup, no bias), at the render size w = (int)(width * ResolutionScale),
+ * h = (int)(height * ResolutionScale), then upscaled to width x height with four depth-weighted bilinear taps.
+ * depth: the G-buffer depth [depth_height][depth_width] (host array, sampled NEAREST); taa_jitter may be NULL.
+ * out_rgba16f: width*height*4 halves (rgba16f, alpha 1), or NULL to keep the image on the device
+ * (idkpt_volumetric_device_ptr: valid until the next call with other sizes, idkpt_set_scene or idkpt_destroy).
+ * Synchronous; ordered after the samples idkpt_compute has queued. With no shadows set the image is 0.
+ * Every shadow's LightIndex must be below the scene's light count. */
+typedef struct IdkPtVolumetricSettings {   /* VolumetricLighting.GpuSettings (VolumetricLighting.cs:10-21) + ResolutionScale */
+    float   Absorbance[3];                 /* 0.025, 0.025, 0.025 */
+    int32_t SampleCount;                   /* 5 (1..1024) */
+    float   Scattering;                    /* 0.758: Henyey-Greenstein g */
+    float   MaxDist;                       /* 50 */
+    float   Strength;                      /* 0.1 */
+    float   ResolutionScale;               /* 0.6, in (0, 1] */
+} IdkPtVolumetricSettings;
+IDKPT_API int idkpt_volumetric_lighting(IdkPtCtx* ctx, const GpuPerFrameData* frame, const IdkPtVolumetricSettings* settings, const float* depth,
+                                        int32_t depth_width, int32_t depth_height, int32_t width, int32_t height, const float* taa_jitter,
+                                        uint16_t* out_rgba16f, float* kernel_ms);
+IDKPT_API int idkpt_volumetric_device_ptr(IdkPtCtx* ctx, void** dev_ptr, uint64_t* bytes);
 
 /* ---- dynamic geometry (SURVEY.md 8f.2): ModelManager.Update = skin -> refit -> TLAS (ModelManager.cs:236-261) ----
  * idkpt_set_skinning_data: unskinnedVertexSSBO upload (52-byte GpuUnskinnedVertex records).

@@ -181,6 +181,20 @@ public:
         check(idkpt_point_shadow_device_ptr(ctx_, index, &p, bytes), "idkpt_point_shadow_device_ptr");
         return p;
     }
+    // VolumetricLighting.Compute through the point-shadow cube maps: out = width * height * 4 halves, or nullptr to keep the
+    // image on the device (VolumetricDevicePtr). Returns the kernel time in ms.
+    float VolumetricLighting(const GpuPerFrameData& frame, const IdkPtVolumetricSettings& settings, const float* depth, int depthWidth, int depthHeight,
+                             int width, int height, const float* taaJitter, uint16_t* outRgba16f) {
+        float ms = 0.0f;
+        check(idkpt_volumetric_lighting(ctx_, &frame, &settings, depth, depthWidth, depthHeight, width, height, taaJitter, outRgba16f, &ms),
+              "idkpt_volumetric_lighting");
+        return ms;
+    }
+    void* VolumetricDevicePtr(uint64_t* bytes = nullptr) {
+        void* p = nullptr;
+        check(idkpt_volumetric_device_ptr(ctx_, &p, bytes), "idkpt_volumetric_device_ptr");
+        return p;
+    }
     void SetSkinningData(const GpuUnskinnedVertex* vertices, uint64_t count) { check(idkpt_set_skinning_data(ctx_, vertices, count), "idkpt_set_skinning_data"); }
     void SkinVertices(const float* jointMatrices3x4, uint64_t jointCount, const IdkPtSkinningCmd* cmds, uint32_t cmdCount) {
         check(idkpt_skin_vertices(ctx_, jointMatrices3x4, jointCount, cmds, cmdCount, nullptr), "idkpt_skin_vertices");
