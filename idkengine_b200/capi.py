@@ -98,6 +98,7 @@ EXPORTS = [
     "idkpt_denoise", "idkpt_denoise_device_ptrs", "idkpt_denoise_import_output", "idkpt_tlas_build",
     "idkpt_set_point_shadows", "idkpt_render_point_shadows", "idkpt_read_point_shadow", "idkpt_point_shadow_device_ptr",
     "idkpt_volumetric_lighting", "idkpt_volumetric_device_ptr",
+    "idkpt_ssao", "idkpt_ssao_device_ptr", "idkpt_deferred_lighting", "idkpt_deferred_device_ptr",
 ]
 
 IDKPT_MAX_POINT_SHADOWS = 128
@@ -111,6 +112,32 @@ class IdkPtVolumetricSettings(ctypes.Structure):
 def default_volumetric_settings():
     """VolumetricLighting.GpuSettings defaults (VolumetricLighting.cs:10-21) and its ResolutionScale of 0.6."""
     return IdkPtVolumetricSettings((c_f * 3)(0.025, 0.025, 0.025), 5, 0.758, 50.0, 0.1, 0.6)
+
+
+class IdkPtGBuffer(ctypes.Structure):
+    _fields_ = [("Width", c_i32), ("Height", c_i32), ("OnDevice", c_i32), ("Depth", c_vp), ("NormalRG", c_vp), ("AlbedoRGB", c_vp),
+                ("MetallicRoughness", c_vp), ("EmissiveRGB", c_vp)]
+
+
+class IdkPtSsaoSettings(ctypes.Structure):
+    _fields_ = [("SampleCount", c_i32), ("Radius", c_f), ("Strength", c_f), ("NoiseIndex", c_u32)]
+
+
+def default_ssao_settings():
+    """SSAO.GpuSettings defaults (SSAO.cs:10-15), noise index 0 (no TAA)."""
+    return IdkPtSsaoSettings(10, 0.2, 1.3, 0)
+
+
+class IdkPtDeferredSettings(ctypes.Structure):
+    _fields_ = [("ShadowMode", c_i32), ("IsSSAO", c_i32), ("IsVXGI", c_i32)]
+
+
+SHADOW_MODE_NONE, SHADOW_MODE_PCF, SHADOW_MODE_RAY_TRACED = 0, 1, 2   # RasterPipeline.ShadowMode
+
+
+def default_deferred_settings():
+    """RasterPipeline's defaults (RasterPipeline.cs:247-256): ShadowMode.Pcf, IsSSAO on, IsVXGI off."""
+    return IdkPtDeferredSettings(SHADOW_MODE_PCF, 1, 0)
 
 
 class IdkPtDenoiseSettings(ctypes.Structure):
@@ -323,6 +350,14 @@ def load(path=None):
     L.idkpt_volumetric_lighting.argtypes = [c_vp, c_vp, P(IdkPtVolumetricSettings), c_vp, c_i32, c_i32, c_i32, c_i32, c_vp, c_vp, P(c_f)]
     L.idkpt_volumetric_device_ptr.restype = c_i32
     L.idkpt_volumetric_device_ptr.argtypes = [c_vp, P(c_vp), P(c_u64)]
+    L.idkpt_ssao.restype = c_i32
+    L.idkpt_ssao.argtypes = [c_vp, c_vp, P(IdkPtSsaoSettings), P(IdkPtGBuffer), c_vp, P(c_f)]
+    L.idkpt_ssao_device_ptr.restype = c_i32
+    L.idkpt_ssao_device_ptr.argtypes = [c_vp, P(c_vp), P(c_u64)]
+    L.idkpt_deferred_lighting.restype = c_i32
+    L.idkpt_deferred_lighting.argtypes = [c_vp, c_vp, P(IdkPtDeferredSettings), P(IdkPtGBuffer), c_vp, c_vp, c_vp, c_u32, c_vp, P(c_f)]
+    L.idkpt_deferred_device_ptr.restype = c_i32
+    L.idkpt_deferred_device_ptr.argtypes = [c_vp, P(c_vp), P(c_u64)]
     L.idkpt_abi_version.restype = c_u32
     L.idkpt_abi_version.argtypes = []
     if path == _build.LIBIDKPT:

@@ -19,12 +19,13 @@
 #include "idk_post.cuh"
 #include "idk_point_shadows.cuh"
 #include "idk_volumetric.cuh"
+#include "idk_deferred.cuh"
 #include "idk_textures_host.h"
 
 #define IDKPT_ABI_VERSION 4u   // 2: IdkPtSceneDesc gained Textures / TextureCount; 3: IdkPtStats gained CompactMs / AccumulateMs, host-buffer registration;
                                // 4: gather handle blob is 5 IPC handles (320 bytes), IDKPT_CREATE_GLOBAL_SLOTS, idkpt_gather_connect.
-                               // Entry points added since (point-shadow cube maps, idkvx_set_shadow_maps, volumetric lighting) are
-                               // additive and keep 4.
+                               // Entry points added since (point-shadow cube maps, idkvx_set_shadow_maps, volumetric lighting, SSAO
+                               // and deferred lighting) are additive and keep 4.
 
 struct DevBuf {
     void* p = nullptr;
@@ -80,6 +81,7 @@ struct IdkPtCtx : IdkCtxBase {
     DeviceScene sc = {};
     IdkPtSceneDesc counts = {};    // element counts only (pointers unused)
     DevBuf nodes, triRec, blasTris, positions, descs, instances, xforms, meshes, materials, vertices, lights, tlas, vtxFrame, surfRec;
+    std::vector<GpuLight> hostLights;   // host mirror of `lights` (idkpt_set_scene, idkpt_update_range): shadow-index checks
     float sky[3] = {0.0f, 0.0f, 0.0f};
     DevBuf skyFaces;
     int skyFaceSize = 0;
@@ -99,6 +101,12 @@ struct IdkPtCtx : IdkCtxBase {
     // volumetric lighting (idkpt_volumetric_lighting): render-size rgba16f + r32f, presentation-size rgba16f
     DevBuf volMarch, volDepth, volOut;
     int volW = 0, volH = 0;        // presentation size of the last successful call (0: none since the scene was set)
+
+    // G-buffer lighting (idkpt_ssao, idkpt_deferred_lighting): host G-buffer uploads, the ray-traced visibility uploads and
+    // their device pointer table, the R8Unorm SSAO image and the rgba32f lit image
+    DevBuf gbufStage, rtStage, rtPtrs, ssaoOut, deferredOut;
+    int ssaoW = 0, ssaoH = 0;      // size of the last successful call (0: none since the scene was set)
+    int deferredW = 0, deferredH = 0;
 
     // present chain: bloom mip chains (rgba16f), AgX constants, RGBA8 frame
     DevBuf bloomDown, bloomUp, postConsts, ldr;
@@ -594,7 +602,8 @@ IDKPT_API void idkpt_destroy(IdkPtCtx* ctx) {
                      &ctx->tex.pixels, &ctx->tex.recs, &ctx->tex.srgbLut, &ctx->bloomDown, &ctx->bloomUp, &ctx->postConsts, &ctx->ldr,
                      &ctx->unskinned, &ctx->joints, &ctx->refitParents, &ctx->refitLocks, &ctx->scratch[0], &ctx->scratch[1], &ctx->scratch[2],
                      &ctx->tlasScratch, &ctx->oidn[0], &ctx->oidn[1], &ctx->oidn[2], &ctx->oidn[3], &ctx->denoiseWork[0], &ctx->denoiseWork[1], &ctx->denoised,
-                     &ctx->pointShadowDev, &ctx->pointShadowMaps, &ctx->pointShadowLights, &ctx->volMarch, &ctx->volDepth, &ctx->volOut};
+                     &ctx->pointShadowDev, &ctx->pointShadowMaps, &ctx->pointShadowLights, &ctx->volMarch, &ctx->volDepth, &ctx->volOut,
+                     &ctx->gbufStage, &ctx->rtStage, &ctx->rtPtrs, &ctx->ssaoOut, &ctx->deferredOut};
     for (DevBuf* b : all) release(*b);
     for (int i = 0; i < IDK_MAX_LANES; i++) release_lane(ctx->lanes[i], false);
     for (cudaEvent_t ev : ctx->events) cudaEventDestroy(ev);
@@ -642,6 +651,8 @@ IDKPT_API int idkpt_set_scene(IdkPtCtx* ctx, const IdkPtSceneDesc* s) {
     release(ctx->pointShadowDev); release(ctx->pointShadowMaps); release(ctx->pointShadowLights);
     release(ctx->volMarch); release(ctx->volDepth); release(ctx->volOut);
     ctx->volW = ctx->volH = 0;
+    release(ctx->gbufStage); release(ctx->rtStage); release(ctx->rtPtrs); release(ctx->ssaoOut); release(ctx->deferredOut);
+    ctx->ssaoW = ctx->ssaoH = ctx->deferredW = ctx->deferredH = 0;
     int rc;
     // nodes and triangle records share one allocation ("bvh"): [nodes | triRec], so that one L2 access-policy window covers both
     const size_t nodeBytes = ((s->BlasNodeCount * sizeof(GpuBlasNode)) + 255) & ~(size_t)255;
@@ -704,6 +715,7 @@ IDKPT_API int idkpt_set_scene(IdkPtCtx* ctx, const IdkPtSceneDesc* s) {
     sc.textureCount = (uint32_t)s->TextureCount;
     sc.srgbLut = (const float*)ctx->tex.srgbLut.p;
     ctx->counts = *s;
+    ctx->hostLights.assign(s->Lights, s->Lights + s->LightCount);
     ctx->hostDescs.assign(s->BlasDescs, s->BlasDescs + s->BlasDescCount);
     ctx->nodeBytes = nodeBytes;
     if ((rc = configure_launches(ctx))) return rc;
@@ -775,6 +787,7 @@ IDKPT_API int idkpt_update_range(IdkPtCtx* ctx, IdkPtArrayId which, uint64_t fir
         for (uint64_t i = 0; i < count; i++) ctx->hostMaterialMaxHandle[first + i] = material_max_handle(m[i]);
     }
     CK(cudaMemcpyAsync((char*)b->p + first * elem, data, count * elem, cudaMemcpyHostToDevice, ctx->stream));
+    if (which == IDKPT_ARRAY_LIGHTS) std::copy((const GpuLight*)data, (const GpuLight*)data + count, ctx->hostLights.begin() + first);
     if ((which == IDKPT_ARRAY_MESHES || which == IDKPT_ARRAY_MATERIALS) && ctx->counts.MeshCount) {
         const uint32_t nm = (uint32_t)ctx->counts.MeshCount;   // refresh the per-mesh surface records
         k_prepare_surfaces<<<(nm + 255) / 256, 256, 0, ctx->stream>>>((const GpuMesh*)ctx->meshes.p, (const GpuMaterial*)ctx->materials.p, (float4*)ctx->surfRec.p, nm);
@@ -1324,6 +1337,7 @@ static int preload_kernels(IdkPtCtx* ctx) {
     IDK_PRELOAD(k_bloom_down); IDK_PRELOAD(k_bloom_up); IDK_PRELOAD(k_agx_matrices); IDK_PRELOAD(k_tonemap);
     IDK_PRELOAD(k_denoise_prepare); IDK_PRELOAD(k_denoise_atrous); IDK_PRELOAD(k_denoise_finish); IDK_PRELOAD(k_denoise_import);
     IDK_PRELOAD(k_bcn_decode); IDK_PRELOAD(k_point_shadow_faces); IDK_PRELOAD(k_volumetric_march); IDK_PRELOAD(k_volumetric_upscale);
+    IDK_PRELOAD(k_ssao); IDK_PRELOAD(k_deferred_lighting);
 #undef IDK_PRELOAD
     return IDKPT_OK;
 }
@@ -2008,6 +2022,182 @@ IDKPT_API int idkpt_volumetric_device_ptr(IdkPtCtx* ctx, void** devPtr, uint64_t
     if (!ctx->volW) return fail(ctx, IDKPT_ERR_INVALID_ARGUMENT, "idkpt_volumetric_device_ptr: call idkpt_volumetric_lighting first");
     *devPtr = ctx->volOut.p;
     if (bytes) *bytes = (uint64_t)ctx->volW * ctx->volH * 8;
+    return IDKPT_OK;
+}
+
+// ---- G-buffer lighting (SSAO.Compute, the deferred lighting draw) -------------------------------------------------------------
+// An OnDevice input the kernels read in place: device memory on the context's device, aligned to the width of the kernels'
+// loads of it (`align` bytes: 4 for one float per pixel, 8 for the float2 attachments, 16 for the float4 indirect image).
+// Checked before anything is allocated or launched, so a rejected pointer is never read.
+static int gbuffer_device_check(IdkPtCtx* ctx, const char* who, const float* src, size_t align) {
+    cudaPointerAttributes attr;
+    const cudaError_t e = cudaPointerGetAttributes(&attr, src);
+    if (e != cudaSuccess) cudaGetLastError();   // not a pointer CUDA knows: clear the error, reject below
+    if (e != cudaSuccess || !(attr.type == cudaMemoryTypeDevice || attr.type == cudaMemoryTypeManaged) || attr.device != ctx->device)
+        return fail(ctx, who, IDKPT_ERR_INVALID_ARGUMENT, "OnDevice = 1 with a pointer that is not device memory on the context's device");
+    if ((uintptr_t)src % align != 0)
+        return fail(ctx, who, IDKPT_ERR_INVALID_ARGUMENT, align == 4 ? "OnDevice pointer not 4-byte aligned"
+                                                          : align == 8 ? "OnDevice NormalRG / MetallicRoughness pointer not 8-byte aligned"
+                                                                       : "OnDevice indirect-light pointer not 16-byte aligned");
+    return IDKPT_OK;
+}
+
+// A G-buffer input of `floats` floats per pixel: read in place (OnDevice, already checked by gbuffer_device_check) or uploaded
+// into stage + *offset (256-byte aligned). Returns IDKPT_OK or the failure.
+static int gbuffer_input(IdkPtCtx* ctx, const IdkPtGBuffer* g, const float* src, size_t floats, DevBuf& stage, size_t& offset,
+                         const float*& dst) {
+    const size_t bytes = (size_t)g->Width * g->Height * floats * 4;
+    if (g->OnDevice) {
+        dst = src;
+        return IDKPT_OK;
+    }
+    dst = (const float*)((char*)stage.p + offset);
+    CK(cudaMemcpyAsync((char*)stage.p + offset, src, bytes, cudaMemcpyHostToDevice, ctx->stream));
+    offset += (bytes + 255) & ~(size_t)255;
+    return IDKPT_OK;
+}
+
+static int gbuffer_check(IdkPtCtx* ctx, const char* who, const IdkPtGBuffer* g, bool all) {
+    if (!g->Depth || !g->NormalRG || (all && (!g->AlbedoRGB || !g->MetallicRoughness || !g->EmissiveRGB)))
+        return fail(ctx, who, IDKPT_ERR_INVALID_ARGUMENT, "null argument");
+    if (g->Width < 1 || g->Height < 1 || g->Width > 16384 || g->Height > 16384) return fail(ctx, who, IDKPT_ERR_INVALID_ARGUMENT, "size outside 1..16384");
+    if (g->OnDevice != 0 && g->OnDevice != 1) return fail(ctx, who, IDKPT_ERR_INVALID_ARGUMENT, "OnDevice is neither 0 nor 1");
+    return IDKPT_OK;
+}
+
+// the stage for `floats` floats per pixel of host input, each array 256-byte aligned
+static size_t gbuffer_stage_bytes(const IdkPtGBuffer* g, std::initializer_list<size_t> floats) {
+    size_t n = 0;
+    for (size_t f : floats) n += (((size_t)g->Width * g->Height * f * 4) + 255) & ~(size_t)255;
+    return n;
+}
+
+IDKPT_API int idkpt_ssao(IdkPtCtx* ctx, const GpuPerFrameData* frame, const IdkPtSsaoSettings* s, const IdkPtGBuffer* g, uint8_t* outR8, float* kernelMs) {
+    static const char* who = "idkpt_ssao";
+    if (!ctx || !frame || !s || !g) return fail(ctx, IDKPT_ERR_INVALID_ARGUMENT, "idkpt_ssao: null argument");
+    if (!ctx->haveScene) return fail(ctx, IDKPT_ERR_NO_SCENE, "idkpt_ssao: no scene");
+    if (int rc = gbuffer_check(ctx, who, g, false)) return rc;
+    if (s->SampleCount < 1 || s->SampleCount > 1024) return fail(ctx, IDKPT_ERR_INVALID_ARGUMENT, "idkpt_ssao: SampleCount outside 1..1024");
+    CK(cudaSetDevice(ctx->device));
+    if (g->OnDevice) {
+        if (int rc = gbuffer_device_check(ctx, who, g->Depth, 4)) return rc;
+        if (int rc = gbuffer_device_check(ctx, who, g->NormalRG, 8)) return rc;
+    }
+    if (kernelMs) *kernelMs = 0.0f;
+    const size_t n = (size_t)g->Width * g->Height;
+    ctx->ssaoW = ctx->ssaoH = 0;   // the image may be reallocated and is overwritten: valid again only when the call succeeds
+    if ((!g->OnDevice && ensure(ctx->gbufStage, gbuffer_stage_bytes(g, {1, 2})) != cudaSuccess) || ensure(ctx->ssaoOut, n) != cudaSuccess)
+        return fail(ctx, IDKPT_ERR_OUT_OF_MEMORY, "idkpt_ssao: device allocation failed");
+    SsaoArgs a;
+    size_t off = 0;
+    const float *depth, *nrg;
+    if (int rc = gbuffer_input(ctx, g, g->Depth, 1, ctx->gbufStage, off, depth)) return rc;
+    if (int rc = gbuffer_input(ctx, g, g->NormalRG, 2, ctx->gbufStage, off, nrg)) return rc;
+    a.g = DeferredGBuffer{depth, (const float2*)nrg, nullptr, nullptr, nullptr, g->Width, g->Height};
+    a.out = (uint8_t*)ctx->ssaoOut.p;
+    memcpy(a.invProjView, frame->InvProjView, sizeof(a.invProjView));
+    memcpy(a.projView, frame->ProjView, sizeof(a.projView));
+    a.sampleCount = s->SampleCount; a.radius = s->Radius; a.strength = s->Strength; a.noiseIndex = s->NoiseIndex;
+    const size_t tiles = (size_t)((g->Width + 7) / 8) * (size_t)((g->Height + 7) / 8);
+    const int rc = run_timed(ctx, who, kernelMs, [&]() -> int {
+        k_ssao<<<(unsigned)((tiles + 3) / 4), 256, 0, ctx->stream>>>(a);
+        return IDKPT_OK;
+    }, outR8, ctx->ssaoOut.p, outR8 ? n : 0);
+    if (rc == IDKPT_OK) { ctx->ssaoW = g->Width; ctx->ssaoH = g->Height; }
+    return rc;
+}
+
+IDKPT_API int idkpt_ssao_device_ptr(IdkPtCtx* ctx, void** devPtr, uint64_t* bytes) {
+    if (!ctx || !devPtr) return fail(ctx, IDKPT_ERR_INVALID_ARGUMENT, "idkpt_ssao_device_ptr: null argument");
+    if (!ctx->ssaoW) return fail(ctx, IDKPT_ERR_INVALID_ARGUMENT, "idkpt_ssao_device_ptr: call idkpt_ssao first");
+    *devPtr = ctx->ssaoOut.p;
+    if (bytes) *bytes = (uint64_t)ctx->ssaoW * ctx->ssaoH;
+    return IDKPT_OK;
+}
+
+IDKPT_API int idkpt_deferred_lighting(IdkPtCtx* ctx, const GpuPerFrameData* frame, const IdkPtDeferredSettings* s, const IdkPtGBuffer* g,
+                                      const float* taaJitter, const float* indirect, const float* const* rtVisibility, uint32_t rtCount,
+                                      float* outRgba32f, float* kernelMs) {
+    static const char* who = "idkpt_deferred_lighting";
+    if (!ctx || !frame || !s || !g) return fail(ctx, IDKPT_ERR_INVALID_ARGUMENT, "idkpt_deferred_lighting: null argument");
+    if (!ctx->haveScene) return fail(ctx, IDKPT_ERR_NO_SCENE, "idkpt_deferred_lighting: no scene");
+    if (int rc = gbuffer_check(ctx, who, g, true)) return rc;
+    if (s->ShadowMode < 0 || s->ShadowMode > 2) return fail(ctx, IDKPT_ERR_INVALID_ARGUMENT, "idkpt_deferred_lighting: ShadowMode outside 0..2");
+    if (s->IsVXGI && !indirect) return fail(ctx, IDKPT_ERR_INVALID_ARGUMENT, "idkpt_deferred_lighting: IsVXGI without an indirect-light image");
+    if (s->IsSSAO && (ctx->ssaoW != g->Width || ctx->ssaoH != g->Height))
+        return fail(ctx, IDKPT_ERR_INVALID_ARGUMENT, "idkpt_deferred_lighting: IsSSAO needs an idkpt_ssao image of the G-buffer's size");
+    const uint32_t shadowCount = (uint32_t)ctx->pointShadowRecs.size();
+    if (s->ShadowMode != 0) {
+        for (const GpuLight& L : ctx->hostLights)
+            if (L.PointShadowIndex != -1 && (L.PointShadowIndex < 0 || (uint32_t)L.PointShadowIndex >= shadowCount))
+                return fail(ctx, IDKPT_ERR_INVALID_ARGUMENT, "idkpt_deferred_lighting: a light's PointShadowIndex is neither -1 nor below the point-shadow count");
+    }
+    if (s->ShadowMode == 2) {
+        if (rtCount < shadowCount || (rtCount && !rtVisibility))
+            return fail(ctx, IDKPT_ERR_INVALID_ARGUMENT, "idkpt_deferred_lighting: RayTraced needs a visibility image per point shadow");
+        for (uint32_t i = 0; i < rtCount; i++)
+            if (!rtVisibility[i]) return fail(ctx, IDKPT_ERR_INVALID_ARGUMENT, "idkpt_deferred_lighting: a visibility image is null");
+    }
+    CK(cudaSetDevice(ctx->device));
+    const uint32_t rtUsed = s->ShadowMode == 2 ? shadowCount : 0;
+    if (g->OnDevice) {
+        const float* ptrs[5] = {g->Depth, g->NormalRG, g->AlbedoRGB, g->MetallicRoughness, g->EmissiveRGB};
+        const size_t align[5] = {4, 8, 4, 8, 4};
+        for (int i = 0; i < 5; i++)
+            if (int rc = gbuffer_device_check(ctx, who, ptrs[i], align[i])) return rc;
+        if (s->IsVXGI)
+            if (int rc = gbuffer_device_check(ctx, who, indirect, 16)) return rc;
+        for (uint32_t i = 0; i < rtUsed; i++)
+            if (int rc = gbuffer_device_check(ctx, who, rtVisibility[i], 4)) return rc;
+    }
+    if (kernelMs) *kernelMs = 0.0f;
+    const size_t n = (size_t)g->Width * g->Height;
+    ctx->deferredW = ctx->deferredH = 0;   // the image may be reallocated and is overwritten: valid again only when the call succeeds
+    const size_t stageBytes = g->OnDevice ? 0 : gbuffer_stage_bytes(g, {1, 2, 3, 2, 3, s->IsVXGI ? 4u : 0u});
+    if ((stageBytes && ensure(ctx->gbufStage, stageBytes) != cudaSuccess) || (rtUsed && !g->OnDevice && ensure(ctx->rtStage, rtUsed * ((n * 4 + 255) & ~(size_t)255)) != cudaSuccess) ||
+        ensure(ctx->deferredOut, n * 16) != cudaSuccess)
+        return fail(ctx, IDKPT_ERR_OUT_OF_MEMORY, "idkpt_deferred_lighting: device allocation failed");
+    size_t off = 0;
+    const float *depth, *nrg, *albedo, *mr, *emissive, *gi = nullptr;
+    if (int rc = gbuffer_input(ctx, g, g->Depth, 1, ctx->gbufStage, off, depth)) return rc;
+    if (int rc = gbuffer_input(ctx, g, g->NormalRG, 2, ctx->gbufStage, off, nrg)) return rc;
+    if (int rc = gbuffer_input(ctx, g, g->AlbedoRGB, 3, ctx->gbufStage, off, albedo)) return rc;
+    if (int rc = gbuffer_input(ctx, g, g->MetallicRoughness, 2, ctx->gbufStage, off, mr)) return rc;
+    if (int rc = gbuffer_input(ctx, g, g->EmissiveRGB, 3, ctx->gbufStage, off, emissive)) return rc;
+    if (s->IsVXGI)
+        if (int rc = gbuffer_input(ctx, g, indirect, 4, ctx->gbufStage, off, gi)) return rc;
+    std::vector<const float*> rt(rtUsed);
+    size_t rtOff = 0;
+    for (uint32_t i = 0; i < rtUsed; i++)
+        if (int rc = gbuffer_input(ctx, g, rtVisibility[i], 1, ctx->rtStage, rtOff, rt[i])) return rc;
+    if (rtUsed)
+        if (int rc = upload(ctx, ctx->rtPtrs, rt.data(), rt.size() * sizeof(const float*))) return rc;
+    DeferredArgs a;
+    a.g = DeferredGBuffer{depth, (const float2*)nrg, albedo, (const float2*)mr, emissive, g->Width, g->Height};
+    a.ssao = s->IsSSAO ? (const uint8_t*)ctx->ssaoOut.p : nullptr;
+    a.indirect = (const float4*)gi;
+    a.rtVisibility = rtUsed ? (const float* const*)ctx->rtPtrs.p : nullptr;
+    a.lights = ctx->sc.lights; a.lightCount = (int)ctx->counts.LightCount;
+    a.shadows = PointShadowMapsDev{(const PointShadowDev*)ctx->pointShadowDev.p, (const uint16_t*)ctx->pointShadowMaps.p, shadowCount};
+    a.out = (float4*)ctx->deferredOut.p;
+    memcpy(a.invProjView, frame->InvProjView, sizeof(a.invProjView));
+    for (int k = 0; k < 3; k++) a.viewPos[k] = frame->ViewPos[k];
+    a.jitter[0] = taaJitter ? taaJitter[0] : 0.0f; a.jitter[1] = taaJitter ? taaJitter[1] : 0.0f;
+    a.shadowMode = s->ShadowMode;
+    const size_t tiles = (size_t)((g->Width + 7) / 8) * (size_t)((g->Height + 7) / 8);
+    const int rc = run_timed(ctx, who, kernelMs, [&]() -> int {
+        k_deferred_lighting<<<(unsigned)((tiles + 3) / 4), 256, 0, ctx->stream>>>(a);
+        return IDKPT_OK;
+    }, outRgba32f, ctx->deferredOut.p, outRgba32f ? n * 16 : 0);
+    if (rc == IDKPT_OK) { ctx->deferredW = g->Width; ctx->deferredH = g->Height; }
+    return rc;
+}
+
+IDKPT_API int idkpt_deferred_device_ptr(IdkPtCtx* ctx, void** devPtr, uint64_t* bytes) {
+    if (!ctx || !devPtr) return fail(ctx, IDKPT_ERR_INVALID_ARGUMENT, "idkpt_deferred_device_ptr: null argument");
+    if (!ctx->deferredW) return fail(ctx, IDKPT_ERR_INVALID_ARGUMENT, "idkpt_deferred_device_ptr: call idkpt_deferred_lighting first");
+    *devPtr = ctx->deferredOut.p;
+    if (bytes) *bytes = (uint64_t)ctx->deferredW * ctx->deferredH * 16;
     return IDKPT_OK;
 }
 

@@ -371,6 +371,89 @@ class PathTracer:
         self._check(self._lib.idkpt_volumetric_device_ptr(self._ctx, ctypes.byref(p), ctypes.byref(n)), "idkpt_volumetric_device_ptr")
         return p.value, n.value
 
+    # ---- G-buffer lighting (SSAO.Compute, the deferred lighting draw)
+    @staticmethod
+    def _gbuffer(arrays, channels):
+        """IdkPtGBuffer over G-buffer arrays ([H, W] depth first, then [H, W, c] arrays or None): numpy arrays are passed as host
+        arrays, CUDA torch tensors in place (OnDevice = 1). Returns (struct, the contiguous arrays to keep alive, on_device)."""
+        on_device = type(arrays[0]).__module__.startswith("torch")
+        if on_device and not all(a is None or (type(a).__module__.startswith("torch") and a.is_cuda) for a in arrays):
+            raise TypeError("G-buffer: pass either all numpy arrays or all CUDA tensors")
+        keep = []
+        for a, c in zip(arrays, channels):
+            if a is None:
+                keep.append(None)
+                continue
+            if on_device:
+                import torch
+                t = a.to(torch.float32).contiguous()
+                keep.append(t)
+            else:
+                keep.append(np.ascontiguousarray(a, np.float32))
+            # the library copies or reads W * H * c floats of every array: a smaller one must never reach it
+            want = tuple(keep[0].shape[:2]) + (() if c == 1 else (c,))
+            if tuple(keep[-1].shape) != want or len(keep[0].shape) != 2:
+                raise ValueError(f"G-buffer array of shape {tuple(keep[-1].shape)}: expected {want} (depth [H, W] first)")
+        h, w = keep[0].shape[:2]
+        if on_device:   # the library's stream does not wait for torch's: let the tensors' producers finish
+            import torch
+            torch.cuda.synchronize(keep[0].device)
+
+        def ptr(a):
+            return None if a is None else (a.data_ptr() if on_device else a.ctypes.data)
+        g = capi.IdkPtGBuffer(w, h, int(on_device), *[ptr(a) for a in keep[:5]] + [None] * (5 - len(keep[:5])))
+        return g, keep, on_device
+
+    def Ssao(self, frame, depth, normal_rg, settings=None, download=True):
+        """SSAO.Compute on a G-buffer (depth [H, W], octahedral normal [H, W, 2]; numpy arrays or CUDA tensors). settings:
+        capi.IdkPtSsaoSettings (default: the engine's). Returns uint8 [H, W] (R8Unorm), or None with download=False (the image
+        stays on the device: SsaoDevicePtr, and DeferredLighting's IsSSAO reads it). Kernel ms in last_ssao_ms."""
+        st = settings if settings is not None else capi.default_ssao_settings()
+        g, keep, _ = self._gbuffer([depth, normal_rg], [1, 2])
+        frame = np.ascontiguousarray(frame)
+        out = np.zeros((g.Height, g.Width), np.uint8) if download else None
+        ms = ctypes.c_float()
+        self._check(self._lib.idkpt_ssao(self._ctx, frame.ctypes.data, ctypes.byref(st), ctypes.byref(g), out.ctypes.data if download else None,
+                                         ctypes.byref(ms)), "idkpt_ssao")
+        self.last_ssao_ms = ms.value
+        return out
+
+    def SsaoDevicePtr(self):
+        """(device pointer, bytes) of the last Ssao image (R8Unorm)."""
+        p, n = ctypes.c_void_p(), ctypes.c_uint64()
+        self._check(self._lib.idkpt_ssao_device_ptr(self._ctx, ctypes.byref(p), ctypes.byref(n)), "idkpt_ssao_device_ptr")
+        return p.value, n.value
+
+    def DeferredLighting(self, frame, depth, normal_rg, albedo, metallic_roughness, emissive, settings=None, jitter=None, indirect=None,
+                         rt_visibility=None, download=True):
+        """The deferred lighting pass on a G-buffer (depth [H, W], normal [H, W, 2], albedo [H, W, 3], metallic/roughness [H, W, 2],
+        emissive [H, W, 3]; numpy arrays or CUDA tensors, and indirect ([H, W, 4], IsVXGI) and rt_visibility (one [H, W] image
+        per point shadow, ShadowMode RayTraced) of the same kind). settings: capi.IdkPtDeferredSettings (default: the engine's).
+        Returns float32 [H, W, 4] (alpha 1), or None with download=False (DeferredDevicePtr). Kernel ms in last_deferred_ms."""
+        st = settings if settings is not None else capi.default_deferred_settings()
+        rt = list(rt_visibility) if rt_visibility is not None else []
+        g, keep, on_device = self._gbuffer([depth, normal_rg, albedo, metallic_roughness, emissive, indirect] + rt, [1, 2, 3, 2, 3, 4] + [1] * len(rt))
+
+        def ptr(a):
+            return None if a is None else (a.data_ptr() if on_device else a.ctypes.data)
+        rt_ptrs = (ctypes.c_void_p * max(len(rt), 1))(*[ptr(a) for a in keep[6:]])
+        jit = None if jitter is None else np.ascontiguousarray(jitter, np.float32)
+        frame = np.ascontiguousarray(frame)
+        out = np.zeros((g.Height, g.Width, 4), np.float32) if download else None
+        ms = ctypes.c_float()
+        self._check(self._lib.idkpt_deferred_lighting(self._ctx, frame.ctypes.data, ctypes.byref(st), ctypes.byref(g),
+                                                      jit.ctypes.data if jit is not None else None, ptr(keep[5]),
+                                                      rt_ptrs if rt else None, len(rt), out.ctypes.data if download else None,
+                                                      ctypes.byref(ms)), "idkpt_deferred_lighting")
+        self.last_deferred_ms = ms.value
+        return out
+
+    def DeferredDevicePtr(self):
+        """(device pointer, bytes) of the last DeferredLighting image (rgba32f)."""
+        p, n = ctypes.c_void_p(), ctypes.c_uint64()
+        self._check(self._lib.idkpt_deferred_device_ptr(self._ctx, ctypes.byref(p), ctypes.byref(n)), "idkpt_deferred_device_ptr")
+        return p.value, n.value
+
     # ---- properties with the reference's reset-on-set behaviour
     def _reset_prop(name, sub=None):  # noqa: N805
         def get(self):

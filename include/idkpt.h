@@ -332,6 +332,54 @@ IDKPT_API int idkpt_volumetric_lighting(IdkPtCtx* ctx, const GpuPerFrameData* fr
                                         uint16_t* out_rgba16f, float* kernel_ms);
 IDKPT_API int idkpt_volumetric_device_ptr(IdkPtCtx* ctx, void** dev_ptr, uint64_t* bytes);
 
+/* ---- G-buffer lighting (RasterPipeline.Render: SSAO.Compute, then the "Deferred Lighting" draw) ----
+ * IdkPtGBuffer: the G-buffer attachments as float arrays [Height][Width] in the engine's channel layout. OnDevice = 0: host
+ *   arrays, uploaded per call. OnDevice = 1: every pointer is device memory on the context's device and is read in place
+ *   (checked with cudaPointerGetAttributes), aligned to the kernels' loads: NormalRG and MetallicRoughness to 8 bytes, the
+ *   indirect-light image to 16 bytes, the other arrays to 4 bytes (cudaMalloc'd buffers always are). Any other OnDevice
+ *   value, or a pointer that is not device memory or not so aligned, is IDKPT_ERR_INVALID_ARGUMENT, before anything runs.
+ *   SSAO reads Depth and NormalRG; deferred lighting reads all five.
+ * idkpt_ssao: SSAO/compute.glsl at the G-buffer size into an R8Unorm image (out_r8: Width*Height bytes, or NULL to keep it on
+ *   the device: idkpt_ssao_device_ptr).
+ * idkpt_deferred_lighting: DeferredLighting/fragment.glsl at the G-buffer size into an rgba32f image (alpha 1; the engine's
+ *   beforeTAATexture is R11G11B10F, packing to it is the caller's business). out_rgba32f: Width*Height*4 floats, or NULL to
+ *   keep it on the device (idkpt_deferred_device_ptr). taa_jitter may be NULL (0, 0). IsSSAO reads the image of the last
+ *   idkpt_ssao call, which must have the G-buffer's size. indirect_rgba32f (IsVXGI; the cone trace's image, [Height][Width]
+ *   rgba32f) and the ShadowMode 2 visibility images (rt_visibility[k]: shadow k's float [Height][Width] image, as
+ *   idkpt_shadows_ray_traced writes it; read through the R8Unorm store rule) are host or device arrays as gbuffer->OnDevice
+ *   says. In ShadowMode 1 and 2 every light's PointShadowIndex must be -1 or below the idkpt_set_point_shadows count, and
+ *   ShadowMode 2 needs rt_count >= that count with no NULL entry; ShadowMode 0 ignores the index.
+ * Both calls are synchronous and ordered after the samples idkpt_compute has queued. Their images are context allocations,
+ * reused by calls with the same size, valid until the next call with another size, idkpt_set_scene or idkpt_destroy. */
+typedef struct IdkPtGBuffer {
+    int32_t Width;
+    int32_t Height;
+    int32_t OnDevice;                      /* 0: host arrays, 1: device arrays on the context's device */
+    const float* Depth;                    /* D32F: 1 float per pixel */
+    const float* NormalRG;                 /* octahedral normal (EncodeUnitVec): 2 floats */
+    const float* AlbedoRGB;                /* 3 floats */
+    const float* MetallicRoughness;        /* 2 floats */
+    const float* EmissiveRGB;              /* 3 floats */
+} IdkPtGBuffer;
+typedef struct IdkPtSsaoSettings {         /* SSAO.GpuSettings (SSAO.cs:10-15) + the noise index */
+    int32_t  SampleCount;                  /* 10 (1..1024) */
+    float    Radius;                       /* 0.2 */
+    float    Strength;                     /* 1.3 */
+    uint32_t NoiseIndex;                   /* (Frame % TAASamples) * SampleCount * 3 with TAA, 0 without */
+} IdkPtSsaoSettings;
+typedef struct IdkPtDeferredSettings {     /* the deferred lighting program's uniforms (RasterPipeline.cs:454-458) */
+    int32_t ShadowMode;                    /* 1: 0 None, 1 Pcf, 2 RayTraced (RasterPipeline.ShadowMode) */
+    int32_t IsSSAO;                        /* 1 */
+    int32_t IsVXGI;                        /* 0 */
+} IdkPtDeferredSettings;
+IDKPT_API int idkpt_ssao(IdkPtCtx* ctx, const GpuPerFrameData* frame, const IdkPtSsaoSettings* settings, const IdkPtGBuffer* gbuffer,
+                         uint8_t* out_r8, float* kernel_ms);
+IDKPT_API int idkpt_ssao_device_ptr(IdkPtCtx* ctx, void** dev_ptr, uint64_t* bytes);
+IDKPT_API int idkpt_deferred_lighting(IdkPtCtx* ctx, const GpuPerFrameData* frame, const IdkPtDeferredSettings* settings, const IdkPtGBuffer* gbuffer,
+                                      const float* taa_jitter, const float* indirect_rgba32f, const float* const* rt_visibility, uint32_t rt_count,
+                                      float* out_rgba32f, float* kernel_ms);
+IDKPT_API int idkpt_deferred_device_ptr(IdkPtCtx* ctx, void** dev_ptr, uint64_t* bytes);
+
 /* ---- dynamic geometry (SURVEY.md 8f.2): ModelManager.Update = skin -> refit -> TLAS (ModelManager.cs:236-261) ----
  * idkpt_set_skinning_data: unskinnedVertexSSBO upload (52-byte GpuUnskinnedVertex records).
  * idkpt_skin_vertices: uploads the joint matrices (row-major mat4x3 = 3 x vec4 each, ModelManager.cs:272-277) and runs

@@ -195,6 +195,32 @@ public:
         check(idkpt_volumetric_device_ptr(ctx_, &p, bytes), "idkpt_volumetric_device_ptr");
         return p;
     }
+    // SSAO.Compute on a host or device G-buffer: out = Width * Height bytes (R8Unorm), or nullptr to keep the image on the device
+    // (SsaoDevicePtr; DeferredLighting's IsSSAO reads it). Returns the kernel time in ms.
+    float Ssao(const GpuPerFrameData& frame, const IdkPtSsaoSettings& settings, const IdkPtGBuffer& gbuffer, uint8_t* outR8) {
+        float ms = 0.0f;
+        check(idkpt_ssao(ctx_, &frame, &settings, &gbuffer, outR8, &ms), "idkpt_ssao");
+        return ms;
+    }
+    void* SsaoDevicePtr(uint64_t* bytes = nullptr) {
+        void* p = nullptr;
+        check(idkpt_ssao_device_ptr(ctx_, &p, bytes), "idkpt_ssao_device_ptr");
+        return p;
+    }
+    // The deferred lighting draw: out = Width * Height * 4 floats (rgba32f), or nullptr to keep the image on the device
+    // (DeferredDevicePtr). indirect and rtVisibility follow gbuffer.OnDevice. Returns the kernel time in ms.
+    float DeferredLighting(const GpuPerFrameData& frame, const IdkPtDeferredSettings& settings, const IdkPtGBuffer& gbuffer, const float* taaJitter,
+                           const float* indirectRgba32f, const float* const* rtVisibility, uint32_t rtCount, float* outRgba32f) {
+        float ms = 0.0f;
+        check(idkpt_deferred_lighting(ctx_, &frame, &settings, &gbuffer, taaJitter, indirectRgba32f, rtVisibility, rtCount, outRgba32f, &ms),
+              "idkpt_deferred_lighting");
+        return ms;
+    }
+    void* DeferredDevicePtr(uint64_t* bytes = nullptr) {
+        void* p = nullptr;
+        check(idkpt_deferred_device_ptr(ctx_, &p, bytes), "idkpt_deferred_device_ptr");
+        return p;
+    }
     void SetSkinningData(const GpuUnskinnedVertex* vertices, uint64_t count) { check(idkpt_set_skinning_data(ctx_, vertices, count), "idkpt_set_skinning_data"); }
     void SkinVertices(const float* jointMatrices3x4, uint64_t jointCount, const IdkPtSkinningCmd* cmds, uint32_t cmdCount) {
         check(idkpt_skin_vertices(ctx_, jointMatrices3x4, jointCount, cmds, cmdCount, nullptr), "idkpt_skin_vertices");

@@ -1,4 +1,5 @@
-"""Tiny run of every kernel family for compute-sanitizer (memcheck): no torch, small sizes."""
+"""Tiny run of every kernel family for compute-sanitizer (memcheck): small sizes, torch only for the device-memory G-buffer of
+the last section."""
 import os, sys
 sys.path.insert(0, os.path.join(os.path.dirname(os.path.abspath(__file__)), ".."))
 sys.path.insert(0, os.path.join(os.path.dirname(os.path.abspath(__file__)), "..", "tests"))
@@ -107,3 +108,36 @@ with vxgi.Voxelizer((24, 20, 28), (-3.1, -0.1, -3.1), (3.1, 4.1, 3.1)) as vx:
     f2 = scenes.camera_frame(cam, 48, 32)
     vx.ConeTrace(f2, np.full((32, 48), 0.95, np.float32), np.full((32, 48, 2), 0.5, np.float32), np.full((32, 48, 2), 0.5, np.float32), vxgi.default_cone_settings())
 print("vxgi ok")
+
+# G-buffer lighting: SSAO -> deferred lighting in every ShadowMode (cube maps for Pcf, idkpt_shadows_ray_traced images for
+# RayTraced), host arrays and a device-memory G-buffer (OnDevice = 1), odd sizes so that the last tiles are partial
+scene4, cam4 = scenes.cornell_1k(threads=1)
+scene4.add_light((0.0, 1.6, 0.3), (6.0, 5.5, 5.0), 0.2)
+scene4.add_light((-0.6, 0.5, 0.6), (0.5, 0.8, 3.0), 0.1)
+scene4.add_light((0.5, 1.2, 0.8), (1.0, 0.4, 0.3), 0.15)
+scene4.lights["PointShadowIndex"][:] = [1, 0, -1]
+sh4 = np.zeros(2, gt.GpuPointShadow)
+for i, li in enumerate((1, 0)):
+    sh4[i]["Position"], sh4[i]["NearPlane"], sh4[i]["FarPlane"], sh4[i]["LightIndex"] = scene4.lights[li]["Position"], 0.1, 60.0, li
+gw, gh = 37, 23
+f4 = scenes.camera_frame(cam4, gw, gh)
+with PathTracer(16, 16) as pt:
+    pt.SetScene(scene4)
+    pt.SetPointShadows(sh4, [16, 9])
+    pt.RenderPointShadows()
+    gd, gn, gmr = vxgi.synth_gbuffer(pt, scene4, f4, gw, gh)
+    rng = np.random.default_rng(5)
+    gb = (gd, gn, rng.random((gh, gw, 3), dtype=np.float32), gmr, rng.random((gh, gw, 3), dtype=np.float32))
+    gi = rng.random((gh, gw, 4), dtype=np.float32)
+    rtv = [pt.ShadowsRayTraced(f4, gd, gn, li, samples=1)[0] for li in (1, 0)]
+    pt.Ssao(f4, gd, gn, capi.IdkPtSsaoSettings(64, 0.5, 1.3, 3))
+    for mode in (0, 1, 2):
+        pt.DeferredLighting(f4, *gb, settings=capi.IdkPtDeferredSettings(mode, 1, 1), jitter=(0.01, -0.02), indirect=gi, rt_visibility=rtv)
+    import torch
+    dgb = [torch.from_numpy(a).cuda() for a in gb]
+    pt.Ssao(f4, dgb[0], dgb[1], download=False)
+    for mode in (1, 2):
+        pt.DeferredLighting(f4, *dgb, settings=capi.IdkPtDeferredSettings(mode, 1, 1), indirect=torch.from_numpy(gi).cuda(),
+                            rt_visibility=[torch.from_numpy(v).cuda() for v in rtv], download=False)
+    pt.SsaoDevicePtr(); pt.DeferredDevicePtr()
+print("ssao + deferred lighting ok")
