@@ -99,6 +99,7 @@ EXPORTS = [
     "idkpt_set_point_shadows", "idkpt_render_point_shadows", "idkpt_read_point_shadow", "idkpt_point_shadow_device_ptr",
     "idkpt_volumetric_lighting", "idkpt_volumetric_device_ptr",
     "idkpt_ssao", "idkpt_ssao_device_ptr", "idkpt_deferred_lighting", "idkpt_deferred_device_ptr",
+    "idkpt_ssr", "idkpt_ssr_device_ptrs", "idkpt_taa_resolve", "idkpt_taa_device_ptr",
 ]
 
 IDKPT_MAX_POINT_SHADOWS = 128
@@ -138,6 +139,32 @@ SHADOW_MODE_NONE, SHADOW_MODE_PCF, SHADOW_MODE_RAY_TRACED = 0, 1, 2   # RasterPi
 def default_deferred_settings():
     """RasterPipeline's defaults (RasterPipeline.cs:247-256): ShadowMode.Pcf, IsSSAO on, IsVXGI off."""
     return IdkPtDeferredSettings(SHADOW_MODE_PCF, 1, 0)
+
+
+LIT_SOURCE_ARRAY, LIT_SOURCE_DEFERRED, LIT_SOURCE_MERGED = 0, 1, 2   # IDKPT_LIT_SOURCE_*: the lit image idkpt_ssr / idkpt_taa_resolve read
+
+
+class IdkPtSsrSettings(ctypes.Structure):
+    _fields_ = [("SampleCount", c_i32), ("BinarySearchCount", c_i32), ("MaxDist", c_f)]
+
+
+def default_ssr_settings():
+    """SSR.GpuSettings defaults (SSR.cs:10-19)."""
+    return IdkPtSsrSettings(30, 8, 50.0)
+
+
+class IdkPtTaaSettings(ctypes.Structure):
+    _fields_ = [("IsNaiveTaa", c_i32), ("PreferAliasingOverBlur", c_f), ("SampleCount", c_i32)]
+
+
+def default_taa_settings():
+    """TAAResolve.GpuSettings defaults (TAAResolve.cs:10-18) and the engine's 6 TAA samples."""
+    return IdkPtTaaSettings(0, 0.25, 6)
+
+
+class IdkPtTaaInputs(ctypes.Structure):
+    _fields_ = [("Width", c_i32), ("Height", c_i32), ("OnDevice", c_i32), ("Source", c_i32), ("Depth", c_vp), ("VelocityRG", c_vp),
+                ("ColorRgba32f", c_vp)]
 
 
 class IdkPtDenoiseSettings(ctypes.Structure):
@@ -358,6 +385,14 @@ def load(path=None):
     L.idkpt_deferred_lighting.argtypes = [c_vp, c_vp, P(IdkPtDeferredSettings), P(IdkPtGBuffer), c_vp, c_vp, c_vp, c_u32, c_vp, P(c_f)]
     L.idkpt_deferred_device_ptr.restype = c_i32
     L.idkpt_deferred_device_ptr.argtypes = [c_vp, P(c_vp), P(c_u64)]
+    L.idkpt_ssr.restype = c_i32
+    L.idkpt_ssr.argtypes = [c_vp, c_vp, P(IdkPtSsrSettings), P(IdkPtGBuffer), c_i32, c_vp, c_vp, c_vp, P(c_f)]
+    L.idkpt_ssr_device_ptrs.restype = c_i32
+    L.idkpt_ssr_device_ptrs.argtypes = [c_vp, P(c_vp), P(c_vp), P(c_u64), P(c_u64)]
+    L.idkpt_taa_resolve.restype = c_i32
+    L.idkpt_taa_resolve.argtypes = [c_vp, P(IdkPtTaaSettings), P(IdkPtTaaInputs), c_i32, c_i32, c_vp, P(c_f)]
+    L.idkpt_taa_device_ptr.restype = c_i32
+    L.idkpt_taa_device_ptr.argtypes = [c_vp, P(c_vp), P(c_u64)]
     L.idkpt_abi_version.restype = c_u32
     L.idkpt_abi_version.argtypes = []
     if path == _build.LIBIDKPT:

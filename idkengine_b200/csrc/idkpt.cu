@@ -20,12 +20,13 @@
 #include "idk_point_shadows.cuh"
 #include "idk_volumetric.cuh"
 #include "idk_deferred.cuh"
+#include "idk_ssr_taa.cuh"
 #include "idk_textures_host.h"
 
 #define IDKPT_ABI_VERSION 4u   // 2: IdkPtSceneDesc gained Textures / TextureCount; 3: IdkPtStats gained CompactMs / AccumulateMs, host-buffer registration;
                                // 4: gather handle blob is 5 IPC handles (320 bytes), IDKPT_CREATE_GLOBAL_SLOTS, idkpt_gather_connect.
                                // Entry points added since (point-shadow cube maps, idkvx_set_shadow_maps, volumetric lighting, SSAO
-                               // and deferred lighting) are additive and keep 4.
+                               // and deferred lighting, SSR and the TAA resolve) are additive and keep 4.
 
 struct DevBuf {
     void* p = nullptr;
@@ -107,6 +108,14 @@ struct IdkPtCtx : IdkCtxBase {
     DevBuf gbufStage, rtStage, rtPtrs, ssaoOut, deferredOut;
     int ssaoW = 0, ssaoH = 0;      // size of the last successful call (0: none since the scene was set)
     int deferredW = 0, deferredH = 0;
+
+    // the end of the raster frame (idkpt_ssr, idkpt_taa_resolve): the rgba16f SSR image and the rgba32f merged image at the
+    // G-buffer size; the TAA history, two rgba16f presentation-size images (TAAResolve's ping-pong) and its frame counter
+    DevBuf ssrOut, ssrMerged, taaHist[2];
+    int ssrW = 0, ssrH = 0;        // size of the last successful idkpt_ssr call (0: none since the scene was set)
+    int taaW = 0, taaH = 0;        // presentation size of the history pair (0: none since the scene was set)
+    int taaFrame = 0;              // TAAResolve.frame: Result = taaHist[taaFrame % 2], PrevResult the other one
+    int taaLast = -1;              // the image the last successful call wrote, -1: none
 
     // present chain: bloom mip chains (rgba16f), AgX constants, RGBA8 frame
     DevBuf bloomDown, bloomUp, postConsts, ldr;
@@ -603,7 +612,8 @@ IDKPT_API void idkpt_destroy(IdkPtCtx* ctx) {
                      &ctx->unskinned, &ctx->joints, &ctx->refitParents, &ctx->refitLocks, &ctx->scratch[0], &ctx->scratch[1], &ctx->scratch[2],
                      &ctx->tlasScratch, &ctx->oidn[0], &ctx->oidn[1], &ctx->oidn[2], &ctx->oidn[3], &ctx->denoiseWork[0], &ctx->denoiseWork[1], &ctx->denoised,
                      &ctx->pointShadowDev, &ctx->pointShadowMaps, &ctx->pointShadowLights, &ctx->volMarch, &ctx->volDepth, &ctx->volOut,
-                     &ctx->gbufStage, &ctx->rtStage, &ctx->rtPtrs, &ctx->ssaoOut, &ctx->deferredOut};
+                     &ctx->gbufStage, &ctx->rtStage, &ctx->rtPtrs, &ctx->ssaoOut, &ctx->deferredOut,
+                     &ctx->ssrOut, &ctx->ssrMerged, &ctx->taaHist[0], &ctx->taaHist[1]};
     for (DevBuf* b : all) release(*b);
     for (int i = 0; i < IDK_MAX_LANES; i++) release_lane(ctx->lanes[i], false);
     for (cudaEvent_t ev : ctx->events) cudaEventDestroy(ev);
@@ -653,6 +663,9 @@ IDKPT_API int idkpt_set_scene(IdkPtCtx* ctx, const IdkPtSceneDesc* s) {
     ctx->volW = ctx->volH = 0;
     release(ctx->gbufStage); release(ctx->rtStage); release(ctx->rtPtrs); release(ctx->ssaoOut); release(ctx->deferredOut);
     ctx->ssaoW = ctx->ssaoH = ctx->deferredW = ctx->deferredH = 0;
+    release(ctx->ssrOut); release(ctx->ssrMerged); release(ctx->taaHist[0]); release(ctx->taaHist[1]);
+    ctx->ssrW = ctx->ssrH = ctx->taaW = ctx->taaH = ctx->taaFrame = 0;
+    ctx->taaLast = -1;
     int rc;
     // nodes and triangle records share one allocation ("bvh"): [nodes | triRec], so that one L2 access-policy window covers both
     const size_t nodeBytes = ((s->BlasNodeCount * sizeof(GpuBlasNode)) + 255) & ~(size_t)255;
@@ -1337,7 +1350,7 @@ static int preload_kernels(IdkPtCtx* ctx) {
     IDK_PRELOAD(k_bloom_down); IDK_PRELOAD(k_bloom_up); IDK_PRELOAD(k_agx_matrices); IDK_PRELOAD(k_tonemap);
     IDK_PRELOAD(k_denoise_prepare); IDK_PRELOAD(k_denoise_atrous); IDK_PRELOAD(k_denoise_finish); IDK_PRELOAD(k_denoise_import);
     IDK_PRELOAD(k_bcn_decode); IDK_PRELOAD(k_point_shadow_faces); IDK_PRELOAD(k_volumetric_march); IDK_PRELOAD(k_volumetric_upscale);
-    IDK_PRELOAD(k_ssao); IDK_PRELOAD(k_deferred_lighting);
+    IDK_PRELOAD(k_ssao); IDK_PRELOAD(k_deferred_lighting); IDK_PRELOAD(k_ssr); IDK_PRELOAD(k_taa_resolve);
 #undef IDK_PRELOAD
     return IDKPT_OK;
 }
@@ -2198,6 +2211,167 @@ IDKPT_API int idkpt_deferred_device_ptr(IdkPtCtx* ctx, void** devPtr, uint64_t* 
     if (!ctx->deferredW) return fail(ctx, IDKPT_ERR_INVALID_ARGUMENT, "idkpt_deferred_device_ptr: call idkpt_deferred_lighting first");
     *devPtr = ctx->deferredOut.p;
     if (bytes) *bytes = (uint64_t)ctx->deferredW * ctx->deferredH * 16;
+    return IDKPT_OK;
+}
+
+// ---- the end of the raster frame (SSR.Compute, "Merge Textures", TaaResolve.Compute) --------------------------------------------
+// An OnDevice array that is not a G-buffer attachment: device memory on the context's device (gbuffer_device_check), aligned
+// to `align` bytes, else `what`.
+static int device_array_check(IdkPtCtx* ctx, const char* who, const float* src, size_t align, const char* what) {
+    if (int rc = gbuffer_device_check(ctx, who, src, 1)) return rc;
+    if ((uintptr_t)src % align != 0) return fail(ctx, who, IDKPT_ERR_INVALID_ARGUMENT, what);
+    return IDKPT_OK;
+}
+
+// The lit-image selector of both calls, checked before anything is allocated: a caller array, or a context image of w x h.
+static int lit_source_check(IdkPtCtx* ctx, const char* who, int32_t source, bool allowMerged, const float* color, int w, int h, int onDevice) {
+    if (source != IDKPT_LIT_SOURCE_ARRAY && source != IDKPT_LIT_SOURCE_DEFERRED && (!allowMerged || source != IDKPT_LIT_SOURCE_MERGED))
+        return fail(ctx, who, IDKPT_ERR_INVALID_ARGUMENT, allowMerged ? "source is not ARRAY, DEFERRED or MERGED" : "source is neither ARRAY nor DEFERRED");
+    if (source == IDKPT_LIT_SOURCE_ARRAY && !color) return fail(ctx, who, IDKPT_ERR_INVALID_ARGUMENT, "ARRAY source without a colour array");
+    if (source == IDKPT_LIT_SOURCE_DEFERRED && (ctx->deferredW != w || ctx->deferredH != h))
+        return fail(ctx, who, IDKPT_ERR_INVALID_ARGUMENT, "DEFERRED source needs an idkpt_deferred_lighting image of the render size");
+    if (source == IDKPT_LIT_SOURCE_MERGED && (ctx->ssrW != w || ctx->ssrH != h))
+        return fail(ctx, who, IDKPT_ERR_INVALID_ARGUMENT, "MERGED source needs an idkpt_ssr image of the render size");
+    if (source == IDKPT_LIT_SOURCE_ARRAY && onDevice)
+        return device_array_check(ctx, who, color, 16, "OnDevice colour pointer not 16-byte aligned");
+    return IDKPT_OK;
+}
+
+// The lit image a call reads: the caller array (read in place or uploaded into the stage) or the context image.
+static int lit_source_input(IdkPtCtx* ctx, const IdkPtGBuffer* g, int32_t source, const float* color, size_t& offset, const float*& dst) {
+    if (source == IDKPT_LIT_SOURCE_DEFERRED) dst = (const float*)ctx->deferredOut.p;
+    else if (source == IDKPT_LIT_SOURCE_MERGED) dst = (const float*)ctx->ssrMerged.p;
+    else return gbuffer_input(ctx, g, color, 4, ctx->gbufStage, offset, dst);
+    return IDKPT_OK;
+}
+
+IDKPT_API int idkpt_ssr(IdkPtCtx* ctx, const GpuPerFrameData* frame, const IdkPtSsrSettings* s, const IdkPtGBuffer* g, int32_t source,
+                        const float* color, float* mergedOut, uint16_t* ssrOut, float* kernelMs) {
+    static const char* who = "idkpt_ssr";
+    if (!ctx || !frame || !s || !g) return fail(ctx, IDKPT_ERR_INVALID_ARGUMENT, "idkpt_ssr: null argument");
+    if (!ctx->haveScene) return fail(ctx, IDKPT_ERR_NO_SCENE, "idkpt_ssr: no scene");
+    if (int rc = gbuffer_check(ctx, who, g, false)) return rc;
+    if (!g->AlbedoRGB || !g->MetallicRoughness) return fail(ctx, who, IDKPT_ERR_INVALID_ARGUMENT, "null argument");
+    if (s->SampleCount < 1 || s->SampleCount > 1024) return fail(ctx, who, IDKPT_ERR_INVALID_ARGUMENT, "SampleCount outside 1..1024");
+    if (s->BinarySearchCount < 0 || s->BinarySearchCount > 64) return fail(ctx, who, IDKPT_ERR_INVALID_ARGUMENT, "BinarySearchCount outside 0..64");
+    if (!std::isfinite(s->MaxDist)) return fail(ctx, who, IDKPT_ERR_INVALID_ARGUMENT, "MaxDist not finite");
+    CK(cudaSetDevice(ctx->device));
+    if (int rc = lit_source_check(ctx, who, source, false, color, g->Width, g->Height, g->OnDevice)) return rc;
+    if (g->OnDevice) {
+        const float* ptrs[4] = {g->Depth, g->NormalRG, g->AlbedoRGB, g->MetallicRoughness};
+        const size_t align[4] = {4, 8, 4, 8};
+        for (int i = 0; i < 4; i++)
+            if (int rc = gbuffer_device_check(ctx, who, ptrs[i], align[i])) return rc;
+    }
+    if (kernelMs) *kernelMs = 0.0f;
+    const size_t n = (size_t)g->Width * g->Height;
+    ctx->ssrW = ctx->ssrH = 0;     // the images may be reallocated and are overwritten: valid again only when the call succeeds
+    const size_t stageBytes = g->OnDevice ? 0 : gbuffer_stage_bytes(g, {1, 2, 3, 2, source == IDKPT_LIT_SOURCE_ARRAY ? 4u : 0u});
+    if ((stageBytes && ensure(ctx->gbufStage, stageBytes) != cudaSuccess) || ensure(ctx->ssrOut, n * 8) != cudaSuccess ||
+        ensure(ctx->ssrMerged, n * 16) != cudaSuccess)
+        return fail(ctx, IDKPT_ERR_OUT_OF_MEMORY, "idkpt_ssr: device allocation failed");
+    size_t off = 0;
+    const float *depth, *nrg, *albedo, *mr, *src;
+    if (int rc = gbuffer_input(ctx, g, g->Depth, 1, ctx->gbufStage, off, depth)) return rc;
+    if (int rc = gbuffer_input(ctx, g, g->NormalRG, 2, ctx->gbufStage, off, nrg)) return rc;
+    if (int rc = gbuffer_input(ctx, g, g->AlbedoRGB, 3, ctx->gbufStage, off, albedo)) return rc;
+    if (int rc = gbuffer_input(ctx, g, g->MetallicRoughness, 2, ctx->gbufStage, off, mr)) return rc;
+    if (int rc = lit_source_input(ctx, g, source, color, off, src)) return rc;
+    SsrArgs a;
+    a.g = DeferredGBuffer{depth, (const float2*)nrg, albedo, (const float2*)mr, nullptr, g->Width, g->Height};
+    a.src = (const float4*)src;
+    a.ssr = (uint2*)ctx->ssrOut.p;
+    a.merged = (float4*)ctx->ssrMerged.p;
+    a.sc = ctx->sc;
+    memcpy(a.projection, frame->Projection, sizeof(a.projection));
+    memcpy(a.invProjection, frame->InvProjection, sizeof(a.invProjection));
+    memcpy(a.invView, frame->InvView, sizeof(a.invView));
+    a.sampleCount = s->SampleCount; a.binarySearchCount = s->BinarySearchCount; a.maxDist = s->MaxDist;
+    const size_t tiles = (size_t)((g->Width + 7) / 8) * (size_t)((g->Height + 7) / 8);
+    const int rc = run_timed(ctx, who, kernelMs, [&]() -> int {
+        k_ssr<<<(unsigned)((tiles + 3) / 4), 256, 0, ctx->stream>>>(a);
+        return IDKPT_OK;
+    }, mergedOut, ctx->ssrMerged.p, mergedOut ? n * 16 : 0);
+    if (rc != IDKPT_OK) return rc;
+    if (ssrOut) {
+        CK(cudaMemcpyAsync(ssrOut, ctx->ssrOut.p, n * 8, cudaMemcpyDeviceToHost, ctx->stream));
+        CK(cudaStreamSynchronize(ctx->stream));
+    }
+    ctx->ssrW = g->Width; ctx->ssrH = g->Height;
+    return IDKPT_OK;
+}
+
+IDKPT_API int idkpt_ssr_device_ptrs(IdkPtCtx* ctx, void** mergedDevPtr, void** ssrDevPtr, uint64_t* mergedBytes, uint64_t* ssrBytes) {
+    if (!ctx || (!mergedDevPtr && !ssrDevPtr)) return fail(ctx, IDKPT_ERR_INVALID_ARGUMENT, "idkpt_ssr_device_ptrs: null argument");
+    if (!ctx->ssrW) return fail(ctx, IDKPT_ERR_INVALID_ARGUMENT, "idkpt_ssr_device_ptrs: call idkpt_ssr first");
+    const uint64_t n = (uint64_t)ctx->ssrW * ctx->ssrH;
+    if (mergedDevPtr) *mergedDevPtr = ctx->ssrMerged.p;
+    if (ssrDevPtr) *ssrDevPtr = ctx->ssrOut.p;
+    if (mergedBytes) *mergedBytes = n * 16;
+    if (ssrBytes) *ssrBytes = n * 8;
+    return IDKPT_OK;
+}
+
+IDKPT_API int idkpt_taa_resolve(IdkPtCtx* ctx, const IdkPtTaaSettings* s, const IdkPtTaaInputs* in, int width, int height, uint16_t* out,
+                                float* kernelMs) {
+    static const char* who = "idkpt_taa_resolve";
+    if (!ctx || !s || !in || !in->Depth || !in->VelocityRG) return fail(ctx, IDKPT_ERR_INVALID_ARGUMENT, "idkpt_taa_resolve: null argument");
+    if (in->Width < 1 || in->Height < 1 || in->Width > 16384 || in->Height > 16384 || width < 1 || height < 1 || width > 16384 || height > 16384)
+        return fail(ctx, who, IDKPT_ERR_INVALID_ARGUMENT, "size outside 1..16384");
+    if (in->OnDevice != 0 && in->OnDevice != 1) return fail(ctx, who, IDKPT_ERR_INVALID_ARGUMENT, "OnDevice is neither 0 nor 1");
+    if (s->IsNaiveTaa != 0 && s->IsNaiveTaa != 1) return fail(ctx, who, IDKPT_ERR_INVALID_ARGUMENT, "IsNaiveTaa is neither 0 nor 1");
+    if (s->SampleCount < 1 || s->SampleCount > 1024) return fail(ctx, who, IDKPT_ERR_INVALID_ARGUMENT, "SampleCount outside 1..1024");
+    if (!std::isfinite(s->PreferAliasingOverBlur)) return fail(ctx, who, IDKPT_ERR_INVALID_ARGUMENT, "PreferAliasingOverBlur not finite");
+    CK(cudaSetDevice(ctx->device));
+    if (int rc = lit_source_check(ctx, who, in->Source, true, in->ColorRgba32f, in->Width, in->Height, in->OnDevice)) return rc;
+    if (in->OnDevice) {
+        if (int rc = gbuffer_device_check(ctx, who, in->Depth, 4)) return rc;
+        if (int rc = device_array_check(ctx, who, in->VelocityRG, 8, "OnDevice VelocityRG pointer not 8-byte aligned")) return rc;
+    }
+    if (kernelMs) *kernelMs = 0.0f;
+    ctx->taaLast = -1;             // valid again only when the call succeeds
+    const size_t bytes = (size_t)width * height * 8;
+    if (width != ctx->taaW || height != ctx->taaH) {   // a new presentation size restarts from a zero history
+        ctx->taaW = ctx->taaH = 0;
+        if (ensure(ctx->taaHist[0], bytes) != cudaSuccess || ensure(ctx->taaHist[1], bytes) != cudaSuccess)
+            return fail(ctx, IDKPT_ERR_OUT_OF_MEMORY, "idkpt_taa_resolve: device allocation failed");
+        CK(cudaMemsetAsync(ctx->taaHist[0].p, 0, bytes, ctx->stream));
+        CK(cudaMemsetAsync(ctx->taaHist[1].p, 0, bytes, ctx->stream));
+        ctx->taaW = width; ctx->taaH = height;
+    }
+    const IdkPtGBuffer g = {in->Width, in->Height, in->OnDevice, nullptr, nullptr, nullptr, nullptr, nullptr};
+    const size_t stageBytes = in->OnDevice ? 0 : gbuffer_stage_bytes(&g, {1, 2, in->Source == IDKPT_LIT_SOURCE_ARRAY ? 4u : 0u});
+    if (stageBytes && ensure(ctx->gbufStage, stageBytes) != cudaSuccess)
+        return fail(ctx, IDKPT_ERR_OUT_OF_MEMORY, "idkpt_taa_resolve: device allocation failed");
+    size_t off = 0;
+    const float *depth, *velocity, *color;
+    if (int rc = gbuffer_input(ctx, &g, in->Depth, 1, ctx->gbufStage, off, depth)) return rc;
+    if (int rc = gbuffer_input(ctx, &g, in->VelocityRG, 2, ctx->gbufStage, off, velocity)) return rc;
+    if (int rc = lit_source_input(ctx, &g, in->Source, in->ColorRgba32f, off, color)) return rc;
+    ctx->taaFrame++;
+    const int dst = ctx->taaFrame % 2 == 0 ? 0 : 1;
+    TaaArgs a;
+    a.color = PostImage{(const float4*)color, nullptr, in->Width, in->Height};
+    a.depth = depth;
+    a.velocity = (const float2*)velocity;
+    a.history = PostImage{nullptr, (const uint2*)ctx->taaHist[1 - dst].p, width, height};
+    a.out = (uint2*)ctx->taaHist[dst].p;
+    a.W = width; a.H = height;
+    a.isNaive = s->IsNaiveTaa; a.sampleCount = s->SampleCount; a.preferAliasingOverBlur = s->PreferAliasingOverBlur;
+    const size_t tiles = (size_t)((width + 7) / 8) * (size_t)((height + 7) / 8);
+    const int rc = run_timed(ctx, who, kernelMs, [&]() -> int {
+        k_taa_resolve<<<(unsigned)((tiles + 3) / 4), 256, 0, ctx->stream>>>(a);
+        return IDKPT_OK;
+    }, out, ctx->taaHist[dst].p, out ? bytes : 0);
+    if (rc == IDKPT_OK) ctx->taaLast = dst;
+    return rc;
+}
+
+IDKPT_API int idkpt_taa_device_ptr(IdkPtCtx* ctx, void** devPtr, uint64_t* bytes) {
+    if (!ctx || !devPtr) return fail(ctx, IDKPT_ERR_INVALID_ARGUMENT, "idkpt_taa_device_ptr: null argument");
+    if (ctx->taaLast < 0) return fail(ctx, IDKPT_ERR_INVALID_ARGUMENT, "idkpt_taa_device_ptr: call idkpt_taa_resolve first");
+    *devPtr = ctx->taaHist[ctx->taaLast].p;
+    if (bytes) *bytes = (uint64_t)ctx->taaW * ctx->taaH * 8;
     return IDKPT_OK;
 }
 

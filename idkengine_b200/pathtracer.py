@@ -454,6 +454,70 @@ class PathTracer:
         self._check(self._lib.idkpt_deferred_device_ptr(self._ctx, ctypes.byref(p), ctypes.byref(n)), "idkpt_deferred_device_ptr")
         return p.value, n.value
 
+    # ---- the end of the raster frame (SSR.Compute, "Merge Textures", TaaResolve.Compute)
+    @staticmethod
+    def _lit_source(source, color):
+        """The lit-image selector: ARRAY when a colour array is given, DEFERRED otherwise, unless `source` says."""
+        if source is None:
+            return capi.LIT_SOURCE_ARRAY if color is not None else capi.LIT_SOURCE_DEFERRED
+        if (source == capi.LIT_SOURCE_ARRAY) != (color is not None):
+            raise ValueError("a colour array goes with LIT_SOURCE_ARRAY, and only with it")
+        return source
+
+    def Ssr(self, frame, depth, normal_rg, albedo, metallic_roughness, settings=None, color=None, source=None, download=True):
+        """SSR.Compute and the "Merge Textures" dispatch on a G-buffer (depth [H, W], normal [H, W, 2], albedo [H, W, 3],
+        metallic/roughness [H, W, 2]; numpy arrays or CUDA tensors). The lit image is `color` (rgba32f [H, W, 4] of the same
+        kind; LIT_SOURCE_ARRAY) or the last DeferredLighting image (LIT_SOURCE_DEFERRED). settings: capi.IdkPtSsrSettings
+        (default: the engine's). Returns (merged float32 [H, W, 4], ssr float16 [H, W, 4]), or None with download=False (the
+        images stay on the device: SsrDevicePtrs, and TaaResolve's LIT_SOURCE_MERGED reads the merged one). Kernel ms in
+        last_ssr_ms."""
+        st = settings if settings is not None else capi.default_ssr_settings()
+        src = self._lit_source(source, color)
+        g, keep, on_device = self._gbuffer([depth, normal_rg, albedo, metallic_roughness, None, color], [1, 2, 3, 2, 3, 4])
+        col = None if keep[5] is None else (keep[5].data_ptr() if on_device else keep[5].ctypes.data)
+        frame = np.ascontiguousarray(frame)
+        merged = np.zeros((g.Height, g.Width, 4), np.float32) if download else None
+        ssr = np.zeros((g.Height, g.Width, 4), np.float16) if download else None
+        ms = ctypes.c_float()
+        self._check(self._lib.idkpt_ssr(self._ctx, frame.ctypes.data, ctypes.byref(st), ctypes.byref(g), src, col,
+                                        merged.ctypes.data if download else None, ssr.ctypes.data if download else None,
+                                        ctypes.byref(ms)), "idkpt_ssr")
+        self.last_ssr_ms = ms.value
+        return (merged, ssr) if download else None
+
+    def SsrDevicePtrs(self):
+        """((merged device pointer, bytes), (SSR device pointer, bytes)) of the last Ssr images (rgba32f, rgba16f)."""
+        pm, ps, nm, ns = ctypes.c_void_p(), ctypes.c_void_p(), ctypes.c_uint64(), ctypes.c_uint64()
+        self._check(self._lib.idkpt_ssr_device_ptrs(self._ctx, ctypes.byref(pm), ctypes.byref(ps), ctypes.byref(nm), ctypes.byref(ns)),
+                    "idkpt_ssr_device_ptrs")
+        return (pm.value, nm.value), (ps.value, ns.value)
+
+    def TaaResolve(self, depth, velocity_rg, width, height, settings=None, color=None, source=None, download=True):
+        """TaaResolve.Compute at width x height (the presentation size) over render-size inputs: depth [h, w], velocity [h, w, 2]
+        and the lit image `color` (rgba32f [h, w, 4]; LIT_SOURCE_ARRAY), or the last DeferredLighting (LIT_SOURCE_DEFERRED) or
+        merged Ssr image (LIT_SOURCE_MERGED); numpy arrays or CUDA tensors. settings: capi.IdkPtTaaSettings (default: the
+        engine's). The history is the context's. Returns float16 [height, width, 4], or None with download=False
+        (TaaDevicePtr). Kernel ms in last_taa_ms."""
+        st = settings if settings is not None else capi.default_taa_settings()
+        src = self._lit_source(source, color)
+        g, keep, on_device = self._gbuffer([depth, velocity_rg, color], [1, 2, 4])
+
+        def ptr(a):
+            return None if a is None else (a.data_ptr() if on_device else a.ctypes.data)
+        inputs = capi.IdkPtTaaInputs(g.Width, g.Height, g.OnDevice, src, ptr(keep[0]), ptr(keep[1]), ptr(keep[2]))
+        out = np.zeros((height, width, 4), np.float16) if download else None
+        ms = ctypes.c_float()
+        self._check(self._lib.idkpt_taa_resolve(self._ctx, ctypes.byref(st), ctypes.byref(inputs), width, height,
+                                                out.ctypes.data if download else None, ctypes.byref(ms)), "idkpt_taa_resolve")
+        self.last_taa_ms = ms.value
+        return out
+
+    def TaaDevicePtr(self):
+        """(device pointer, bytes) of the image the last TaaResolve wrote (rgba16f)."""
+        p, n = ctypes.c_void_p(), ctypes.c_uint64()
+        self._check(self._lib.idkpt_taa_device_ptr(self._ctx, ctypes.byref(p), ctypes.byref(n)), "idkpt_taa_device_ptr")
+        return p.value, n.value
+
     # ---- properties with the reference's reset-on-set behaviour
     def _reset_prop(name, sub=None):  # noqa: N805
         def get(self):

@@ -380,6 +380,53 @@ IDKPT_API int idkpt_deferred_lighting(IdkPtCtx* ctx, const GpuPerFrameData* fram
                                       float* out_rgba32f, float* kernel_ms);
 IDKPT_API int idkpt_deferred_device_ptr(IdkPtCtx* ctx, void** dev_ptr, uint64_t* bytes);
 
+/* ---- the end of the raster frame (RasterPipeline.Render: SSR.Compute, "Merge Textures", TaaResolve.Compute) ----
+ * The lit image both calls read (`source`): IDKPT_LIT_SOURCE_ARRAY, a caller rgba32f [Height][Width] array (host or device as
+ *   the call's OnDevice says; a host that keeps the light, skybox and transparency draws in GL passes its composited buffer);
+ *   IDKPT_LIT_SOURCE_DEFERRED, the image of the last idkpt_deferred_lighting call; IDKPT_LIT_SOURCE_MERGED (TAA only), the
+ *   merged image of the last idkpt_ssr call. A context image must exist and have the render size.
+ * idkpt_ssr: SSR/compute.glsl at the G-buffer size (reads Depth, NormalRG, AlbedoRGB and MetallicRoughness; EmissiveRGB may be
+ *   NULL), then MergeTextures/compute.glsl: merged = source.rgb + SSR.rgb (alpha 1). The sky is the context's (idkpt_set_sky).
+ *   merged_out_rgba32f: Width*Height*4 floats; ssr_out_rgba16f: Width*Height*4 halves (alpha 0 where the shader's early out
+ *   stores vec4(0), else 1). Either may be NULL to keep that image on the device (idkpt_ssr_device_ptrs).
+ * idkpt_taa_resolve: TAAResolve/compute.glsl at the presentation size width x height over the render-size inputs (the sizes
+ *   are independent: upscaling TAA). The context keeps two rgba16f presentation-size images and a frame counter (TAAResolve's
+ *   ping-pong): each call increments the counter, writes Result and reads PrevResult. Both images are zero-filled whenever
+ *   the presentation size changes (and on the first call); idkpt_set_scene drops them. out_rgba16f: width*height*4 halves
+ *   (alpha 1), or NULL (idkpt_taa_device_ptr: the image the last call wrote).
+ * OnDevice arrays must be device memory on the context's device, aligned to 4 bytes (depth), 8 bytes (velocity and the float2
+ * G-buffer attachments) and 16 bytes (colour arrays). Both calls are synchronous and ordered after the samples idkpt_compute
+ * has queued. Their images are context allocations, valid until the next call with another size, idkpt_set_scene or
+ * idkpt_destroy. */
+#define IDKPT_LIT_SOURCE_ARRAY    0
+#define IDKPT_LIT_SOURCE_DEFERRED 1
+#define IDKPT_LIT_SOURCE_MERGED   2
+typedef struct IdkPtSsrSettings {          /* SSR.GpuSettings (SSR.cs:10-19) */
+    int32_t SampleCount;                   /* 30 (1..1024) */
+    int32_t BinarySearchCount;             /* 8 (0..64) */
+    float   MaxDist;                       /* 50 (finite) */
+} IdkPtSsrSettings;
+typedef struct IdkPtTaaSettings {          /* TAAResolve.GpuSettings (TAAResolve.cs:10-18) + GpuTaaData.SampleCount */
+    int32_t IsNaiveTaa;                    /* 0 */
+    float   PreferAliasingOverBlur;        /* 0.25 */
+    int32_t SampleCount;                   /* 6 (1..1024) */
+} IdkPtTaaSettings;
+typedef struct IdkPtTaaInputs {            /* the render-size images TAAResolve/compute.glsl samples */
+    int32_t Width;                         /* render size */
+    int32_t Height;
+    int32_t OnDevice;                      /* 0: host arrays, 1: device arrays on the context's device */
+    int32_t Source;                        /* IDKPT_LIT_SOURCE_*: the colour */
+    const float* Depth;                    /* D32F: 1 float per pixel */
+    const float* VelocityRG;               /* 2 floats per pixel (R16G16F in the engine) */
+    const float* ColorRgba32f;             /* Source ARRAY: 4 floats per pixel, else ignored */
+} IdkPtTaaInputs;
+IDKPT_API int idkpt_ssr(IdkPtCtx* ctx, const GpuPerFrameData* frame, const IdkPtSsrSettings* settings, const IdkPtGBuffer* gbuffer,
+                        int32_t source, const float* color_rgba32f, float* merged_out_rgba32f, uint16_t* ssr_out_rgba16f, float* kernel_ms);
+IDKPT_API int idkpt_ssr_device_ptrs(IdkPtCtx* ctx, void** merged_dev_ptr, void** ssr_dev_ptr, uint64_t* merged_bytes, uint64_t* ssr_bytes);
+IDKPT_API int idkpt_taa_resolve(IdkPtCtx* ctx, const IdkPtTaaSettings* settings, const IdkPtTaaInputs* inputs, int width, int height,
+                                uint16_t* out_rgba16f, float* kernel_ms);
+IDKPT_API int idkpt_taa_device_ptr(IdkPtCtx* ctx, void** dev_ptr, uint64_t* bytes);
+
 /* ---- dynamic geometry (SURVEY.md 8f.2): ModelManager.Update = skin -> refit -> TLAS (ModelManager.cs:236-261) ----
  * idkpt_set_skinning_data: unskinnedVertexSSBO upload (52-byte GpuUnskinnedVertex records).
  * idkpt_skin_vertices: uploads the joint matrices (row-major mat4x3 = 3 x vec4 each, ModelManager.cs:272-277) and runs

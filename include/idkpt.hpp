@@ -221,6 +221,30 @@ public:
         check(idkpt_deferred_device_ptr(ctx_, &p, bytes), "idkpt_deferred_device_ptr");
         return p;
     }
+    // SSR.Compute + "Merge Textures": source = IDKPT_LIT_SOURCE_ARRAY (colorRgba32f, host or device as gbuffer.OnDevice says)
+    // or IDKPT_LIT_SOURCE_DEFERRED. mergedOut = Width * Height * 4 floats, ssrOut = Width * Height * 4 halves; either may be
+    // nullptr to keep that image on the device (SsrDevicePtrs). Returns the kernel time in ms.
+    float Ssr(const GpuPerFrameData& frame, const IdkPtSsrSettings& settings, const IdkPtGBuffer& gbuffer, int32_t source,
+              const float* colorRgba32f, float* mergedOutRgba32f, uint16_t* ssrOutRgba16f) {
+        float ms = 0.0f;
+        check(idkpt_ssr(ctx_, &frame, &settings, &gbuffer, source, colorRgba32f, mergedOutRgba32f, ssrOutRgba16f, &ms), "idkpt_ssr");
+        return ms;
+    }
+    void SsrDevicePtrs(void** merged, void** ssr, uint64_t* mergedBytes = nullptr, uint64_t* ssrBytes = nullptr) {
+        check(idkpt_ssr_device_ptrs(ctx_, merged, ssr, mergedBytes, ssrBytes), "idkpt_ssr_device_ptrs");
+    }
+    // TaaResolve.Compute at width x height over the render-size inputs, against the context's history: out = width * height * 4
+    // halves, or nullptr to keep the result on the device (TaaDevicePtr). Returns the kernel time in ms.
+    float TaaResolve(const IdkPtTaaSettings& settings, const IdkPtTaaInputs& inputs, int width, int height, uint16_t* outRgba16f) {
+        float ms = 0.0f;
+        check(idkpt_taa_resolve(ctx_, &settings, &inputs, width, height, outRgba16f, &ms), "idkpt_taa_resolve");
+        return ms;
+    }
+    void* TaaDevicePtr(uint64_t* bytes = nullptr) {
+        void* p = nullptr;
+        check(idkpt_taa_device_ptr(ctx_, &p, bytes), "idkpt_taa_device_ptr");
+        return p;
+    }
     void SetSkinningData(const GpuUnskinnedVertex* vertices, uint64_t count) { check(idkpt_set_skinning_data(ctx_, vertices, count), "idkpt_set_skinning_data"); }
     void SkinVertices(const float* jointMatrices3x4, uint64_t jointCount, const IdkPtSkinningCmd* cmds, uint32_t cmdCount) {
         check(idkpt_skin_vertices(ctx_, jointMatrices3x4, jointCount, cmds, cmdCount, nullptr), "idkpt_skin_vertices");

@@ -141,3 +141,26 @@ with PathTracer(16, 16) as pt:
                             rt_visibility=[torch.from_numpy(v).cuda() for v in rtv], download=False)
     pt.SsaoDevicePtr(); pt.DeferredDevicePtr()
 print("ssao + deferred lighting ok")
+
+# the end of the raster frame: SSR + merge (ARRAY and DEFERRED sources, constant and 6-face sky, host and device G-buffer),
+# then the TAA resolve naive and clamped, upscaling from the render size, from host arrays and on the device from MERGED
+with PathTracer(16, 16) as pt:
+    pt.SetScene(scene4)
+    rng = np.random.default_rng(6)
+    gd, gn, gmr = vxgi.synth_gbuffer(pt, scene4, f4, gw, gh)
+    gmr = gmr.copy()
+    gmr[..., 0] = rng.random((gh, gw), dtype=np.float32)
+    gb = (gd, gn, rng.random((gh, gw, 3), dtype=np.float32), gmr, rng.random((gh, gw, 3), dtype=np.float32))
+    lit = rng.random((gh, gw, 4), dtype=np.float32)
+    vel = ((rng.random((gh, gw, 2)) - 0.5) * 0.1).astype(np.float32)
+    pt.Ssr(f4, *gb[:4], color=lit)
+    pt.SetSky((0.3, 0.4, 0.5), rng.random((6, 8, 8, 4), dtype=np.float32))
+    pt.DeferredLighting(f4, *gb, settings=capi.IdkPtDeferredSettings(0, 0, 0))
+    pt.Ssr(f4, *gb[:4], capi.IdkPtSsrSettings(64, 1, 3.0), source=capi.LIT_SOURCE_DEFERRED)
+    for naive in (0, 1):
+        pt.TaaResolve(gd, vel, 61, 39, capi.IdkPtTaaSettings(naive, 0.25, 6), color=lit)
+    dgb = [torch.from_numpy(a).cuda() for a in gb]
+    pt.Ssr(f4, *dgb[:4], color=torch.from_numpy(lit).cuda(), download=False)
+    pt.TaaResolve(dgb[0], torch.from_numpy(vel).cuda(), 61, 39, source=capi.LIT_SOURCE_MERGED, download=False)
+    pt.SsrDevicePtrs(); pt.TaaDevicePtr()
+print("ssr + taa resolve ok")
