@@ -100,6 +100,7 @@ EXPORTS = [
     "idkpt_volumetric_lighting", "idkpt_volumetric_device_ptr",
     "idkpt_ssao", "idkpt_ssao_device_ptr", "idkpt_deferred_lighting", "idkpt_deferred_device_ptr",
     "idkpt_ssr", "idkpt_ssr_device_ptrs", "idkpt_taa_resolve", "idkpt_taa_device_ptr",
+    "idkpt_shading_rate", "idkpt_shading_rate_device_ptr",
 ]
 
 IDKPT_MAX_POINT_SHADOWS = 128
@@ -130,15 +131,15 @@ def default_ssao_settings():
 
 
 class IdkPtDeferredSettings(ctypes.Structure):
-    _fields_ = [("ShadowMode", c_i32), ("IsSSAO", c_i32), ("IsVXGI", c_i32)]
+    _fields_ = [("ShadowMode", c_i32), ("IsSSAO", c_i32), ("IsVXGI", c_i32), ("IsVariableRateShading", c_i32)]
 
 
 SHADOW_MODE_NONE, SHADOW_MODE_PCF, SHADOW_MODE_RAY_TRACED = 0, 1, 2   # RasterPipeline.ShadowMode
 
 
 def default_deferred_settings():
-    """RasterPipeline's defaults (RasterPipeline.cs:247-256): ShadowMode.Pcf, IsSSAO on, IsVXGI off."""
-    return IdkPtDeferredSettings(SHADOW_MODE_PCF, 1, 0)
+    """RasterPipeline's defaults (RasterPipeline.cs:247-256): ShadowMode.Pcf, IsSSAO on, IsVXGI off, IsVariableRateShading off."""
+    return IdkPtDeferredSettings(SHADOW_MODE_PCF, 1, 0, 0)
 
 
 LIT_SOURCE_ARRAY, LIT_SOURCE_DEFERRED, LIT_SOURCE_MERGED = 0, 1, 2   # IDKPT_LIT_SOURCE_*: the lit image idkpt_ssr / idkpt_taa_resolve read
@@ -165,6 +166,25 @@ def default_taa_settings():
 class IdkPtTaaInputs(ctypes.Structure):
     _fields_ = [("Width", c_i32), ("Height", c_i32), ("OnDevice", c_i32), ("Source", c_i32), ("Depth", c_vp), ("VelocityRG", c_vp),
                 ("ColorRgba32f", c_vp)]
+
+
+class IdkPtShadingRateSettings(ctypes.Structure):
+    _fields_ = [("DebugMode", c_i32), ("SpeedFactor", c_f), ("LumVarianceFactor", c_f)]
+
+
+# LightingShadingRateClassifier.DebugMode
+VRS_DEBUG_NONE, VRS_DEBUG_SHADING_RATE, VRS_DEBUG_SPEED, VRS_DEBUG_LUMINANCE, VRS_DEBUG_LUMINANCE_VARIANCE = 0, 1, 2, 3, 4
+VRS_TILE = 16   # pixels per rate-image texel along each axis
+VRS_PALETTE = ((1, 1), (2, 1), (2, 2), (4, 2), (4, 4))   # palette index -> coarse fragment (width, height)
+
+
+def default_shading_rate_settings():
+    """LightingShadingRateClassifier.GpuSettings defaults: no debug image, SpeedFactor 0.2, LumVarianceFactor 0.04."""
+    return IdkPtShadingRateSettings(VRS_DEBUG_NONE, 0.2, 0.04)
+
+
+class IdkPtShadingRateInputs(ctypes.Structure):
+    _fields_ = [("Width", c_i32), ("Height", c_i32), ("OnDevice", c_i32), ("Source", c_i32), ("VelocityRG", c_vp), ("ColorRgba32f", c_vp)]
 
 
 class IdkPtDenoiseSettings(ctypes.Structure):
@@ -393,6 +413,10 @@ def load(path=None):
     L.idkpt_taa_resolve.argtypes = [c_vp, P(IdkPtTaaSettings), P(IdkPtTaaInputs), c_i32, c_i32, c_vp, P(c_f)]
     L.idkpt_taa_device_ptr.restype = c_i32
     L.idkpt_taa_device_ptr.argtypes = [c_vp, P(c_vp), P(c_u64)]
+    L.idkpt_shading_rate.restype = c_i32
+    L.idkpt_shading_rate.argtypes = [c_vp, c_vp, P(IdkPtShadingRateSettings), P(IdkPtShadingRateInputs), c_vp, c_vp, P(c_f)]
+    L.idkpt_shading_rate_device_ptr.restype = c_i32
+    L.idkpt_shading_rate_device_ptr.argtypes = [c_vp, P(c_vp), P(c_u64)]
     L.idkpt_abi_version.restype = c_u32
     L.idkpt_abi_version.argtypes = []
     if path == _build.LIBIDKPT:

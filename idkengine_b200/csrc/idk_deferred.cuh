@@ -152,17 +152,17 @@ __device__ __forceinline__ float deferred_pcf(const PointShadowMapsDev& m, int s
     return visibility / 21.0f;
 }
 
-__global__ void __launch_bounds__(256) k_deferred_lighting(DeferredArgs a) {
-    __shared__ GpuLight s_lights[IDK_GPU_MAX_UBO_LIGHT_COUNT];
-    for (int i = threadIdx.x; i < a.lightCount; i += blockDim.x) s_lights[i] = a.lights[i];
-    __syncthreads();
-    int x, y;
-    if (!deferred_pixel(a.g.w, a.g.h, x, y)) return;
-    const size_t p = (size_t)y * a.g.w + x;
+// The fragment shader at one sample: every G-buffer read at texel p (imgCoord), the NDC from uv() (a float2, evaluated after
+// the sky test). Hands the lit value (alpha 1; the sky, depth 1, is black) to store(float4). k_deferred_lighting runs it once
+// per pixel, k_deferred_lighting_vrs (idk_vrs.cuh) once per coarse fragment. The callbacks keep k_deferred_lighting's SASS
+// what it was before the body was shared.
+template <class Uv, class Store>
+__device__ __forceinline__ void deferred_shade(const DeferredArgs& a, const GpuLight* s_lights, size_t p, Uv&& uv, Store&& store) {
     const float depth = a.g.depth[p];
-    if (depth == 1.0f) { a.out[p] = make_float4(0.0f, 0.0f, 0.0f, 1.0f); return; }
+    if (depth == 1.0f) { store(make_float4(0.0f, 0.0f, 0.0f, 1.0f)); return; }
 
-    const float u = ((float)x + 0.5f) / (float)a.g.w, v = ((float)y + 0.5f) / (float)a.g.h;
+    const float2 uvs = uv();
+    const float u = uvs.x, v = uvs.y;
     const float nx = u * 2.0f - 1.0f, ny = v * 2.0f - 1.0f;
     const f3 fragPos = deferred_perspective(a.invProjView, nx, ny, depth);
     const f3 unjitteredFragPos = deferred_perspective(a.invProjView, nx - a.jitter[0], ny - a.jitter[1], depth);
@@ -230,5 +230,16 @@ __global__ void __launch_bounds__(256) k_deferred_lighting(DeferredArgs a) {
         indirect = mk3(0.015f, 0.015f, 0.015f) * albedo;
     }
     const f3 c = (direct + indirect) + emissive;
-    a.out[p] = make_float4(c.x, c.y, c.z, 1.0f);
+    store(make_float4(c.x, c.y, c.z, 1.0f));
+}
+
+__global__ void __launch_bounds__(256) k_deferred_lighting(DeferredArgs a) {
+    __shared__ GpuLight s_lights[IDK_GPU_MAX_UBO_LIGHT_COUNT];
+    for (int i = threadIdx.x; i < a.lightCount; i += blockDim.x) s_lights[i] = a.lights[i];
+    __syncthreads();
+    int x, y;
+    if (!deferred_pixel(a.g.w, a.g.h, x, y)) return;
+    const size_t p = (size_t)y * a.g.w + x;
+    deferred_shade(a, s_lights, p, [&]() { return make_float2(((float)x + 0.5f) / (float)a.g.w, ((float)y + 0.5f) / (float)a.g.h); },
+                   [&](float4 c) { a.out[p] = c; });
 }

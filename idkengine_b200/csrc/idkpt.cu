@@ -21,12 +21,14 @@
 #include "idk_volumetric.cuh"
 #include "idk_deferred.cuh"
 #include "idk_ssr_taa.cuh"
+#include "idk_vrs.cuh"
 #include "idk_textures_host.h"
 
 #define IDKPT_ABI_VERSION 4u   // 2: IdkPtSceneDesc gained Textures / TextureCount; 3: IdkPtStats gained CompactMs / AccumulateMs, host-buffer registration;
                                // 4: gather handle blob is 5 IPC handles (320 bytes), IDKPT_CREATE_GLOBAL_SLOTS, idkpt_gather_connect.
                                // Entry points added since (point-shadow cube maps, idkvx_set_shadow_maps, volumetric lighting, SSAO
-                               // and deferred lighting, SSR and the TAA resolve) are additive and keep 4.
+                               // and deferred lighting, SSR and the TAA resolve, the shading-rate classifier) are additive and keep 4;
+                               // IdkPtDeferredSettings grew a trailing IsVariableRateShading.
 
 struct DevBuf {
     void* p = nullptr;
@@ -116,6 +118,11 @@ struct IdkPtCtx : IdkCtxBase {
     int taaW = 0, taaH = 0;        // presentation size of the history pair (0: none since the scene was set)
     int taaFrame = 0;              // TAAResolve.frame: Result = taaHist[taaFrame % 2], PrevResult the other one
     int taaLast = -1;              // the image the last successful call wrote, -1: none
+
+    // variable-rate deferred lighting (idkpt_shading_rate; idkpt_deferred_lighting with IsVariableRateShading): the R8 rate
+    // image and the r32f debug image, one texel per 16x16 tile, and the per-tile coarse-fragment offsets of the lighting pass
+    DevBuf vrsRates, vrsDebug, vrsOffsets;
+    int vrsW = 0, vrsH = 0;        // render size of the last successful idkpt_shading_rate call (0: none since the scene was set)
 
     // present chain: bloom mip chains (rgba16f), AgX constants, RGBA8 frame
     DevBuf bloomDown, bloomUp, postConsts, ldr;
@@ -613,7 +620,7 @@ IDKPT_API void idkpt_destroy(IdkPtCtx* ctx) {
                      &ctx->tlasScratch, &ctx->oidn[0], &ctx->oidn[1], &ctx->oidn[2], &ctx->oidn[3], &ctx->denoiseWork[0], &ctx->denoiseWork[1], &ctx->denoised,
                      &ctx->pointShadowDev, &ctx->pointShadowMaps, &ctx->pointShadowLights, &ctx->volMarch, &ctx->volDepth, &ctx->volOut,
                      &ctx->gbufStage, &ctx->rtStage, &ctx->rtPtrs, &ctx->ssaoOut, &ctx->deferredOut,
-                     &ctx->ssrOut, &ctx->ssrMerged, &ctx->taaHist[0], &ctx->taaHist[1]};
+                     &ctx->ssrOut, &ctx->ssrMerged, &ctx->taaHist[0], &ctx->taaHist[1], &ctx->vrsRates, &ctx->vrsDebug, &ctx->vrsOffsets};
     for (DevBuf* b : all) release(*b);
     for (int i = 0; i < IDK_MAX_LANES; i++) release_lane(ctx->lanes[i], false);
     for (cudaEvent_t ev : ctx->events) cudaEventDestroy(ev);
@@ -666,6 +673,8 @@ IDKPT_API int idkpt_set_scene(IdkPtCtx* ctx, const IdkPtSceneDesc* s) {
     release(ctx->ssrOut); release(ctx->ssrMerged); release(ctx->taaHist[0]); release(ctx->taaHist[1]);
     ctx->ssrW = ctx->ssrH = ctx->taaW = ctx->taaH = ctx->taaFrame = 0;
     ctx->taaLast = -1;
+    release(ctx->vrsRates); release(ctx->vrsDebug); release(ctx->vrsOffsets);
+    ctx->vrsW = ctx->vrsH = 0;
     int rc;
     // nodes and triangle records share one allocation ("bvh"): [nodes | triRec], so that one L2 access-policy window covers both
     const size_t nodeBytes = ((s->BlasNodeCount * sizeof(GpuBlasNode)) + 255) & ~(size_t)255;
@@ -1351,6 +1360,7 @@ static int preload_kernels(IdkPtCtx* ctx) {
     IDK_PRELOAD(k_denoise_prepare); IDK_PRELOAD(k_denoise_atrous); IDK_PRELOAD(k_denoise_finish); IDK_PRELOAD(k_denoise_import);
     IDK_PRELOAD(k_bcn_decode); IDK_PRELOAD(k_point_shadow_faces); IDK_PRELOAD(k_volumetric_march); IDK_PRELOAD(k_volumetric_upscale);
     IDK_PRELOAD(k_ssao); IDK_PRELOAD(k_deferred_lighting); IDK_PRELOAD(k_ssr); IDK_PRELOAD(k_taa_resolve);
+    IDK_PRELOAD(k_shading_rate); IDK_PRELOAD(k_vrs_scan); IDK_PRELOAD(k_deferred_lighting_vrs);
 #undef IDK_PRELOAD
     return IDKPT_OK;
 }
@@ -2136,6 +2146,10 @@ IDKPT_API int idkpt_deferred_lighting(IdkPtCtx* ctx, const GpuPerFrameData* fram
     if (!ctx->haveScene) return fail(ctx, IDKPT_ERR_NO_SCENE, "idkpt_deferred_lighting: no scene");
     if (int rc = gbuffer_check(ctx, who, g, true)) return rc;
     if (s->ShadowMode < 0 || s->ShadowMode > 2) return fail(ctx, IDKPT_ERR_INVALID_ARGUMENT, "idkpt_deferred_lighting: ShadowMode outside 0..2");
+    if (s->IsVariableRateShading != 0 && s->IsVariableRateShading != 1)
+        return fail(ctx, IDKPT_ERR_INVALID_ARGUMENT, "idkpt_deferred_lighting: IsVariableRateShading is neither 0 nor 1");
+    if (s->IsVariableRateShading && (ctx->vrsW != g->Width || ctx->vrsH != g->Height))
+        return fail(ctx, IDKPT_ERR_INVALID_ARGUMENT, "idkpt_deferred_lighting: IsVariableRateShading needs an idkpt_shading_rate image of the G-buffer's size");
     if (s->IsVXGI && !indirect) return fail(ctx, IDKPT_ERR_INVALID_ARGUMENT, "idkpt_deferred_lighting: IsVXGI without an indirect-light image");
     if (s->IsSSAO && (ctx->ssaoW != g->Width || ctx->ssaoH != g->Height))
         return fail(ctx, IDKPT_ERR_INVALID_ARGUMENT, "idkpt_deferred_lighting: IsSSAO needs an idkpt_ssao image of the G-buffer's size");
@@ -2167,8 +2181,9 @@ IDKPT_API int idkpt_deferred_lighting(IdkPtCtx* ctx, const GpuPerFrameData* fram
     const size_t n = (size_t)g->Width * g->Height;
     ctx->deferredW = ctx->deferredH = 0;   // the image may be reallocated and is overwritten: valid again only when the call succeeds
     const size_t stageBytes = g->OnDevice ? 0 : gbuffer_stage_bytes(g, {1, 2, 3, 2, 3, s->IsVXGI ? 4u : 0u});
+    const int tilesX = (g->Width + IDK_VRS_TILE - 1) / IDK_VRS_TILE, vrsTiles = tilesX * ((g->Height + IDK_VRS_TILE - 1) / IDK_VRS_TILE);
     if ((stageBytes && ensure(ctx->gbufStage, stageBytes) != cudaSuccess) || (rtUsed && !g->OnDevice && ensure(ctx->rtStage, rtUsed * ((n * 4 + 255) & ~(size_t)255)) != cudaSuccess) ||
-        ensure(ctx->deferredOut, n * 16) != cudaSuccess)
+        ensure(ctx->deferredOut, n * 16) != cudaSuccess || (s->IsVariableRateShading && ensure(ctx->vrsOffsets, ((size_t)vrsTiles + 1) * 4) != cudaSuccess))
         return fail(ctx, IDKPT_ERR_OUT_OF_MEMORY, "idkpt_deferred_lighting: device allocation failed");
     size_t off = 0;
     const float *depth, *nrg, *albedo, *mr, *emissive, *gi = nullptr;
@@ -2198,8 +2213,14 @@ IDKPT_API int idkpt_deferred_lighting(IdkPtCtx* ctx, const GpuPerFrameData* fram
     a.jitter[0] = taaJitter ? taaJitter[0] : 0.0f; a.jitter[1] = taaJitter ? taaJitter[1] : 0.0f;
     a.shadowMode = s->ShadowMode;
     const size_t tiles = (size_t)((g->Width + 7) / 8) * (size_t)((g->Height + 7) / 8);
+    const VrsTiles v{(const uint8_t*)ctx->vrsRates.p, (uint32_t*)ctx->vrsOffsets.p, g->Width, g->Height, tilesX, vrsTiles};
     const int rc = run_timed(ctx, who, kernelMs, [&]() -> int {
-        k_deferred_lighting<<<(unsigned)((tiles + 3) / 4), 256, 0, ctx->stream>>>(a);
+        if (s->IsVariableRateShading) {   // the fragment list, then one thread per coarse fragment (grid sized for all 1x1)
+            k_vrs_scan<<<1, 1024, 0, ctx->stream>>>(v);
+            k_deferred_lighting_vrs<<<(unsigned)((n + 255) / 256), 256, 0, ctx->stream>>>(a, v);
+        } else {
+            k_deferred_lighting<<<(unsigned)((tiles + 3) / 4), 256, 0, ctx->stream>>>(a);
+        }
         return IDKPT_OK;
     }, outRgba32f, ctx->deferredOut.p, outRgba32f ? n * 16 : 0);
     if (rc == IDKPT_OK) { ctx->deferredW = g->Width; ctx->deferredH = g->Height; }
@@ -2372,6 +2393,64 @@ IDKPT_API int idkpt_taa_device_ptr(IdkPtCtx* ctx, void** devPtr, uint64_t* bytes
     if (ctx->taaLast < 0) return fail(ctx, IDKPT_ERR_INVALID_ARGUMENT, "idkpt_taa_device_ptr: call idkpt_taa_resolve first");
     *devPtr = ctx->taaHist[ctx->taaLast].p;
     if (bytes) *bytes = (uint64_t)ctx->taaW * ctx->taaH * 8;
+    return IDKPT_OK;
+}
+
+// ---- variable-rate deferred lighting (LightingShadingRateClassifier.Compute) ---------------------------------------------------
+IDKPT_API int idkpt_shading_rate(IdkPtCtx* ctx, const GpuPerFrameData* frame, const IdkPtShadingRateSettings* s, const IdkPtShadingRateInputs* in,
+                                 uint8_t* outRates, float* debugOut, float* kernelMs) {
+    static const char* who = "idkpt_shading_rate";
+    if (!ctx || !frame || !s || !in || !in->VelocityRG) return fail(ctx, IDKPT_ERR_INVALID_ARGUMENT, "idkpt_shading_rate: null argument");
+    if (in->Width < 1 || in->Height < 1 || in->Width > 16384 || in->Height > 16384) return fail(ctx, who, IDKPT_ERR_INVALID_ARGUMENT, "size outside 1..16384");
+    if (in->OnDevice != 0 && in->OnDevice != 1) return fail(ctx, who, IDKPT_ERR_INVALID_ARGUMENT, "OnDevice is neither 0 nor 1");
+    if (s->DebugMode < 0 || s->DebugMode > 4) return fail(ctx, who, IDKPT_ERR_INVALID_ARGUMENT, "DebugMode outside 0..4");
+    if (debugOut && s->DebugMode < 2) return fail(ctx, who, IDKPT_ERR_INVALID_ARGUMENT, "a debug image needs DebugMode 2, 3 or 4");
+    if (!std::isfinite(s->SpeedFactor) || !std::isfinite(s->LumVarianceFactor))
+        return fail(ctx, who, IDKPT_ERR_INVALID_ARGUMENT, "SpeedFactor or LumVarianceFactor not finite");
+    CK(cudaSetDevice(ctx->device));
+    if (int rc = lit_source_check(ctx, who, in->Source, false, in->ColorRgba32f, in->Width, in->Height, in->OnDevice)) return rc;
+    if (in->OnDevice)
+        if (int rc = device_array_check(ctx, who, in->VelocityRG, 8, "OnDevice VelocityRG pointer not 8-byte aligned")) return rc;
+    if (kernelMs) *kernelMs = 0.0f;
+    const unsigned tilesX = (unsigned)(in->Width + IDK_VRS_TILE - 1) / IDK_VRS_TILE, tilesY = (unsigned)(in->Height + IDK_VRS_TILE - 1) / IDK_VRS_TILE;
+    const size_t tiles = (size_t)tilesX * tilesY;
+    ctx->vrsW = ctx->vrsH = 0;     // the image may be reallocated and is overwritten: valid again only when the call succeeds
+    const IdkPtGBuffer g = {in->Width, in->Height, in->OnDevice, nullptr, nullptr, nullptr, nullptr, nullptr};
+    const size_t stageBytes = in->OnDevice ? 0 : gbuffer_stage_bytes(&g, {2, in->Source == IDKPT_LIT_SOURCE_ARRAY ? 4u : 0u});
+    const bool debug = s->DebugMode >= 2;
+    if ((stageBytes && ensure(ctx->gbufStage, stageBytes) != cudaSuccess) || ensure(ctx->vrsRates, tiles) != cudaSuccess ||
+        (debug && ensure(ctx->vrsDebug, tiles * 4) != cudaSuccess))
+        return fail(ctx, IDKPT_ERR_OUT_OF_MEMORY, "idkpt_shading_rate: device allocation failed");
+    size_t off = 0;
+    const float *velocity, *color;
+    if (int rc = gbuffer_input(ctx, &g, in->VelocityRG, 2, ctx->gbufStage, off, velocity)) return rc;
+    if (int rc = lit_source_input(ctx, &g, in->Source, in->ColorRgba32f, off, color)) return rc;
+    ShadingRateArgs a;
+    a.color = (const float4*)color;
+    a.velocity = (const float2*)velocity;
+    a.w = in->Width; a.h = in->Height;
+    a.deltaRenderTime = frame->DeltaRenderTime; a.speedFactor = s->SpeedFactor; a.lumVarianceFactor = s->LumVarianceFactor;
+    a.debugMode = s->DebugMode;
+    a.rates = (uint8_t*)ctx->vrsRates.p;
+    a.debug = debug ? (float*)ctx->vrsDebug.p : nullptr;
+    const int rc = run_timed(ctx, who, kernelMs, [&]() -> int {
+        k_shading_rate<<<dim3(tilesX, tilesY), 256, 0, ctx->stream>>>(a);
+        return IDKPT_OK;
+    }, outRates, ctx->vrsRates.p, outRates ? tiles : 0);
+    if (rc != IDKPT_OK) return rc;
+    if (debugOut) {
+        CK(cudaMemcpyAsync(debugOut, ctx->vrsDebug.p, tiles * 4, cudaMemcpyDeviceToHost, ctx->stream));
+        CK(cudaStreamSynchronize(ctx->stream));
+    }
+    ctx->vrsW = in->Width; ctx->vrsH = in->Height;
+    return IDKPT_OK;
+}
+
+IDKPT_API int idkpt_shading_rate_device_ptr(IdkPtCtx* ctx, void** devPtr, uint64_t* bytes) {
+    if (!ctx || !devPtr) return fail(ctx, IDKPT_ERR_INVALID_ARGUMENT, "idkpt_shading_rate_device_ptr: null argument");
+    if (!ctx->vrsW) return fail(ctx, IDKPT_ERR_INVALID_ARGUMENT, "idkpt_shading_rate_device_ptr: call idkpt_shading_rate first");
+    *devPtr = ctx->vrsRates.p;
+    if (bytes) *bytes = (uint64_t)((ctx->vrsW + IDK_VRS_TILE - 1) / IDK_VRS_TILE) * ((ctx->vrsH + IDK_VRS_TILE - 1) / IDK_VRS_TILE);
     return IDKPT_OK;
 }
 

@@ -425,12 +425,17 @@ class PathTracer:
         return p.value, n.value
 
     def DeferredLighting(self, frame, depth, normal_rg, albedo, metallic_roughness, emissive, settings=None, jitter=None, indirect=None,
-                         rt_visibility=None, download=True):
+                         rt_visibility=None, download=True, vrs=False):
         """The deferred lighting pass on a G-buffer (depth [H, W], normal [H, W, 2], albedo [H, W, 3], metallic/roughness [H, W, 2],
         emissive [H, W, 3]; numpy arrays or CUDA tensors, and indirect ([H, W, 4], IsVXGI) and rt_visibility (one [H, W] image
         per point shadow, ShadowMode RayTraced) of the same kind). settings: capi.IdkPtDeferredSettings (default: the engine's).
-        Returns float32 [H, W, 4] (alpha 1), or None with download=False (DeferredDevicePtr). Kernel ms in last_deferred_ms."""
+        vrs=True sets IsVariableRateShading: the pass shades under the rate image of the last ShadingRate call (which must have
+        the G-buffer's size). Returns float32 [H, W, 4] (alpha 1), or None with download=False (DeferredDevicePtr). Kernel ms
+        in last_deferred_ms."""
         st = settings if settings is not None else capi.default_deferred_settings()
+        if vrs:
+            st = capi.IdkPtDeferredSettings.from_buffer_copy(st)
+            st.IsVariableRateShading = 1
         rt = list(rt_visibility) if rt_visibility is not None else []
         g, keep, on_device = self._gbuffer([depth, normal_rg, albedo, metallic_roughness, emissive, indirect] + rt, [1, 2, 3, 2, 3, 4] + [1] * len(rt))
 
@@ -452,6 +457,51 @@ class PathTracer:
         """(device pointer, bytes) of the last DeferredLighting image (rgba32f)."""
         p, n = ctypes.c_void_p(), ctypes.c_uint64()
         self._check(self._lib.idkpt_deferred_device_ptr(self._ctx, ctypes.byref(p), ctypes.byref(n)), "idkpt_deferred_device_ptr")
+        return p.value, n.value
+
+    # ---- variable-rate deferred lighting (LightingShadingRateClassifier.Compute)
+    def ShadingRate(self, frame, velocity_rg, settings=None, color=None, source=None, download=True, debug=False):
+        """LightingShadingRateClassifier.Compute over render-size inputs: velocity [h, w, 2] and the lit image `color` (rgba32f
+        [h, w, 4]; LIT_SOURCE_ARRAY) or the last DeferredLighting image (LIT_SOURCE_DEFERRED); numpy arrays or CUDA tensors.
+        frame's DeltaRenderTime divides the mean speed. settings: capi.IdkPtShadingRateSettings (default: the engine's). Returns
+        the rate image, uint8 [ceil(h/16), ceil(w/16)] palette indices (capi.VRS_PALETTE), or None with download=False (the
+        image stays on the device: ShadingRateDevicePtr, and DeferredLighting(vrs=True) reads it). debug=True (DebugMode 2..4)
+        returns (rates, float32 debug image of the same size) instead. Kernel ms in last_shading_rate_ms."""
+        st = settings if settings is not None else capi.default_shading_rate_settings()
+        src = self._lit_source(source, color)
+        v = velocity_rg
+        on_device = type(v).__module__.startswith("torch")
+        if on_device:
+            import torch
+            if not v.is_cuda or (color is not None and not (type(color).__module__.startswith("torch") and color.is_cuda)):
+                raise TypeError("ShadingRate: pass either all numpy arrays or all CUDA tensors")
+            keep = [v.to(torch.float32).contiguous()] + ([] if color is None else [color.to(torch.float32).contiguous()])
+            torch.cuda.synchronize(keep[0].device)   # the library's stream does not wait for torch's
+        else:
+            keep = [np.ascontiguousarray(v, np.float32)] + ([] if color is None else [np.ascontiguousarray(color, np.float32)])
+        h, w = keep[0].shape[:2]
+        if tuple(keep[0].shape) != (h, w, 2) or (color is not None and tuple(keep[1].shape) != (h, w, 4)):
+            raise ValueError(f"ShadingRate: velocity {tuple(keep[0].shape)} / colour {None if color is None else tuple(keep[1].shape)}: "
+                             "expected [h, w, 2] and [h, w, 4]")
+
+        def ptr(a):
+            return a.data_ptr() if on_device else a.ctypes.data
+        inputs = capi.IdkPtShadingRateInputs(w, h, int(on_device), src, ptr(keep[0]), ptr(keep[1]) if color is not None else None)
+        tiles = ((h + capi.VRS_TILE - 1) // capi.VRS_TILE, (w + capi.VRS_TILE - 1) // capi.VRS_TILE)
+        rates = np.zeros(tiles, np.uint8) if download else None
+        dbg = np.zeros(tiles, np.float32) if debug else None
+        frame = np.ascontiguousarray(frame)
+        ms = ctypes.c_float()
+        self._check(self._lib.idkpt_shading_rate(self._ctx, frame.ctypes.data, ctypes.byref(st), ctypes.byref(inputs),
+                                                 rates.ctypes.data if download else None, dbg.ctypes.data if debug else None,
+                                                 ctypes.byref(ms)), "idkpt_shading_rate")
+        self.last_shading_rate_ms = ms.value
+        return (rates, dbg) if debug else rates
+
+    def ShadingRateDevicePtr(self):
+        """(device pointer, bytes) of the last ShadingRate image (R8 palette indices, [ceil(h/16)][ceil(w/16)])."""
+        p, n = ctypes.c_void_p(), ctypes.c_uint64()
+        self._check(self._lib.idkpt_shading_rate_device_ptr(self._ctx, ctypes.byref(p), ctypes.byref(n)), "idkpt_shading_rate_device_ptr")
         return p.value, n.value
 
     # ---- the end of the raster frame (SSR.Compute, "Merge Textures", TaaResolve.Compute)

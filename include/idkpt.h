@@ -371,6 +371,8 @@ typedef struct IdkPtDeferredSettings {     /* the deferred lighting program's un
     int32_t ShadowMode;                    /* 1: 0 None, 1 Pcf, 2 RayTraced (RasterPipeline.ShadowMode) */
     int32_t IsSSAO;                        /* 1 */
     int32_t IsVXGI;                        /* 0 */
+    int32_t IsVariableRateShading;         /* 0 (RasterPipeline.IsVariableRateShading): 1 shades under the rate image of the last
+                                              idkpt_shading_rate call, which must have the G-buffer's size (see below) */
 } IdkPtDeferredSettings;
 IDKPT_API int idkpt_ssao(IdkPtCtx* ctx, const GpuPerFrameData* frame, const IdkPtSsaoSettings* settings, const IdkPtGBuffer* gbuffer,
                          uint8_t* out_r8, float* kernel_ms);
@@ -426,6 +428,38 @@ IDKPT_API int idkpt_ssr_device_ptrs(IdkPtCtx* ctx, void** merged_dev_ptr, void**
 IDKPT_API int idkpt_taa_resolve(IdkPtCtx* ctx, const IdkPtTaaSettings* settings, const IdkPtTaaInputs* inputs, int width, int height,
                                 uint16_t* out_rgba16f, float* kernel_ms);
 IDKPT_API int idkpt_taa_device_ptr(IdkPtCtx* ctx, void** dev_ptr, uint64_t* bytes);
+
+/* ---- variable-rate deferred lighting (LightingShadingRateClassifier.Compute; the deferred lighting draw under its image) ----
+ * idkpt_shading_rate: ShadingRateClassification/compute.glsl over a render-size lit image (Source ARRAY: a caller rgba32f
+ *   [Height][Width] array; DEFERRED: the image of the last idkpt_deferred_lighting call, which must have the render size;
+ *   MERGED is rejected: the engine classifies the image before SSR) and the velocity (RG float [Height][Width]). Every 16x16
+ *   tile gets a palette index of the engine's palette {1x1, 2x1, 2x2, 4x2, 4x4} from its mean speed (/ frame->DeltaRenderTime)
+ *   and its luminance's coefficient of variation. out_rates: ceil(Height/16) * ceil(Width/16) bytes, or NULL to keep the
+ *   image on the device (idkpt_shading_rate_device_ptr). debug_out_r32f (DebugMode 2 Speed, 3 Luminance, 4 LuminanceVariance):
+ *   the mean speed, mean luminance or coefficient of variation per tile, same size; it must be NULL in DebugMode 0 and 1 and
+ *   may be NULL in the others. The sums are taken in a pinned order and the rate conversion is pinned too (DESIGN.md 8f.1f).
+ * With IdkPtDeferredSettings.IsVariableRateShading = 1, idkpt_deferred_lighting shades each pixel under NV_shading_rate_image's
+ *   rules with the context's rate image: the fragment shader runs once per coarse fragment, at its centre, and its result is
+ *   written to every pixel of the fragment. The image of frame N's classification drives frame N+1's lighting.
+ * OnDevice arrays must be device memory on the context's device, aligned to 8 bytes (velocity) and 16 bytes (colour). The call
+ * is synchronous and ordered after the samples idkpt_compute has queued. Its image is a context allocation, valid until the
+ * next call with another size, a failed call, idkpt_set_scene or idkpt_destroy. */
+typedef struct IdkPtShadingRateSettings {  /* LightingShadingRateClassifier.GpuSettings */
+    int32_t DebugMode;                     /* 0: 0 None, 1 ShadingRate, 2 Speed, 3 Luminance, 4 LuminanceVariance */
+    float   SpeedFactor;                   /* 0.2 (finite) */
+    float   LumVarianceFactor;             /* 0.04 (finite) */
+} IdkPtShadingRateSettings;
+typedef struct IdkPtShadingRateInputs {    /* the render-size images the classifier reads */
+    int32_t Width;
+    int32_t Height;
+    int32_t OnDevice;                      /* 0: host arrays, 1: device arrays on the context's device */
+    int32_t Source;                        /* IDKPT_LIT_SOURCE_ARRAY or _DEFERRED */
+    const float* VelocityRG;               /* 2 floats per pixel (R16G16F in the engine) */
+    const float* ColorRgba32f;             /* Source ARRAY: 4 floats per pixel, else ignored */
+} IdkPtShadingRateInputs;
+IDKPT_API int idkpt_shading_rate(IdkPtCtx* ctx, const GpuPerFrameData* frame, const IdkPtShadingRateSettings* settings,
+                                 const IdkPtShadingRateInputs* inputs, uint8_t* out_rates, float* debug_out_r32f, float* kernel_ms);
+IDKPT_API int idkpt_shading_rate_device_ptr(IdkPtCtx* ctx, void** dev_ptr, uint64_t* bytes);
 
 /* ---- dynamic geometry (SURVEY.md 8f.2): ModelManager.Update = skin -> refit -> TLAS (ModelManager.cs:236-261) ----
  * idkpt_set_skinning_data: unskinnedVertexSSBO upload (52-byte GpuUnskinnedVertex records).

@@ -245,6 +245,20 @@ public:
         check(idkpt_taa_device_ptr(ctx_, &p, bytes), "idkpt_taa_device_ptr");
         return p;
     }
+    // LightingShadingRateClassifier.Compute over the render-size inputs: outRates = ceil(h/16) * ceil(w/16) palette indices, or
+    // nullptr to keep the image on the device (ShadingRateDevicePtr; DeferredLighting with IsVariableRateShading reads it);
+    // debugOutR32f (DebugMode 2..4 only) the same size, or nullptr. Returns the kernel time in ms.
+    float ShadingRate(const GpuPerFrameData& frame, const IdkPtShadingRateSettings& settings, const IdkPtShadingRateInputs& inputs,
+                      uint8_t* outRates, float* debugOutR32f = nullptr) {
+        float ms = 0.0f;
+        check(idkpt_shading_rate(ctx_, &frame, &settings, &inputs, outRates, debugOutR32f, &ms), "idkpt_shading_rate");
+        return ms;
+    }
+    void* ShadingRateDevicePtr(uint64_t* bytes = nullptr) {
+        void* p = nullptr;
+        check(idkpt_shading_rate_device_ptr(ctx_, &p, bytes), "idkpt_shading_rate_device_ptr");
+        return p;
+    }
     void SetSkinningData(const GpuUnskinnedVertex* vertices, uint64_t count) { check(idkpt_set_skinning_data(ctx_, vertices, count), "idkpt_set_skinning_data"); }
     void SkinVertices(const float* jointMatrices3x4, uint64_t jointCount, const IdkPtSkinningCmd* cmds, uint32_t cmdCount) {
         check(idkpt_skin_vertices(ctx_, jointMatrices3x4, jointCount, cmds, cmdCount, nullptr), "idkpt_skin_vertices");

@@ -164,3 +164,34 @@ with PathTracer(16, 16) as pt:
     pt.TaaResolve(dgb[0], torch.from_numpy(vel).cuda(), 61, 39, source=capi.LIT_SOURCE_MERGED, download=False)
     pt.SsrDevicePtrs(); pt.TaaDevicePtr()
 print("ssr + taa resolve ok")
+
+# variable-rate deferred lighting: the classifier in every DebugMode (ARRAY and DEFERRED, host and device inputs), then the
+# coarse pass under rate images with every rate, uniform and mixed, at odd sizes (partial tiles, clamped fragment centres)
+with PathTracer(16, 16) as pt:
+    pt.SetScene(scene4)
+    pt.SetPointShadows(sh4, [16, 9])
+    pt.RenderPointShadows()
+    for vw, vh in ((37, 23), (5, 3), (1, 1), (49, 33)):
+        fv = scenes.camera_frame(cam4, vw, vh).copy()
+        fv["DeltaRenderTime"] = 1.0
+        gd, gn, gmr = vxgi.synth_gbuffer(pt, scene4, fv, vw, vh)
+        rng = np.random.default_rng(vw)
+        gb = (gd, gn, rng.random((vh, vw, 3), dtype=np.float32), gmr, rng.random((vh, vw, 3), dtype=np.float32))
+        pt.Ssao(fv, gd, gn)
+        pt.DeferredLighting(fv, *gb, jitter=(0.01, -0.02))
+        col = (0.2 + rng.random((vh, vw, 4))).astype(np.float32)
+        for mode in range(5):
+            pt.ShadingRate(fv, ((rng.random((vh, vw, 2)) - 0.5) * 0.02).astype(np.float32), capi.IdkPtShadingRateSettings(mode, 0.2, 0.04),
+                           color=col, debug=mode >= 2)
+            pt.ShadingRate(fv, np.zeros((vh, vw, 2), np.float32), capi.IdkPtShadingRateSettings(mode, 0.2, 0.04),
+                           source=capi.LIT_SOURCE_DEFERRED, debug=mode >= 2)
+        for r in range(5):   # LumVarianceFactor 0, SpeedFactor 1: a mean speed of r / 4 gives rate r
+            pt.ShadingRate(fv, np.full((vh, vw, 2), (r / 4.0 + 0.01) / np.sqrt(2), np.float32), capi.IdkPtShadingRateSettings(0, 1.0, 0.0), color=col)
+            pt.DeferredLighting(fv, *gb, settings=capi.IdkPtDeferredSettings(1, 1, 0, 1), jitter=(0.01, -0.02))
+        spd = np.repeat(np.repeat(rng.integers(0, 5, ((vh + 15) // 16, (vw + 15) // 16)) / 4.0 + 0.01, 16, 0), 16, 1)[:vh, :vw]
+        pt.ShadingRate(fv, np.stack([spd, np.zeros_like(spd)], -1).astype(np.float32), capi.IdkPtShadingRateSettings(0, 1.0, 0.0), color=col)
+        dgb = [torch.from_numpy(a).cuda() for a in gb]
+        pt.DeferredLighting(fv, *dgb, settings=capi.IdkPtDeferredSettings(2, 1, 0, 1), rt_visibility=[dgb[0], dgb[0]], download=False)
+        pt.ShadingRate(fv, torch.zeros((vh, vw, 2), device="cuda"), source=capi.LIT_SOURCE_DEFERRED, download=False)
+        pt.ShadingRateDevicePtr()
+print("shading rate + coarse deferred lighting ok")
