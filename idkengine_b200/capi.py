@@ -101,6 +101,7 @@ EXPORTS = [
     "idkpt_ssao", "idkpt_ssao_device_ptr", "idkpt_deferred_lighting", "idkpt_deferred_device_ptr",
     "idkpt_ssr", "idkpt_ssr_device_ptrs", "idkpt_taa_resolve", "idkpt_taa_device_ptr",
     "idkpt_shading_rate", "idkpt_shading_rate_device_ptr",
+    "idkpt_gbuffer", "idkpt_gbuffer_device_ptrs", "idkpt_read_gbuffer",
 ]
 
 IDKPT_MAX_POINT_SHADOWS = 128
@@ -417,6 +418,12 @@ def load(path=None):
     L.idkpt_shading_rate.argtypes = [c_vp, c_vp, P(IdkPtShadingRateSettings), P(IdkPtShadingRateInputs), c_vp, c_vp, P(c_f)]
     L.idkpt_shading_rate_device_ptr.restype = c_i32
     L.idkpt_shading_rate_device_ptr.argtypes = [c_vp, P(c_vp), P(c_u64)]
+    L.idkpt_gbuffer.restype = c_i32
+    L.idkpt_gbuffer.argtypes = [c_vp, c_vp, c_i32, c_i32, c_vp, c_vp, P(c_f)]
+    L.idkpt_gbuffer_device_ptrs.restype = c_i32
+    L.idkpt_gbuffer_device_ptrs.argtypes = [c_vp, P(IdkPtGBuffer), P(c_vp)]
+    L.idkpt_read_gbuffer.restype = c_i32
+    L.idkpt_read_gbuffer.argtypes = [c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp]
     L.idkpt_abi_version.restype = c_u32
     L.idkpt_abi_version.argtypes = []
     if path == _build.LIBIDKPT:

@@ -135,9 +135,17 @@ __global__ void k_prepare_surfaces(const GpuMesh* __restrict__ meshes, const Gpu
 // first instead of closer first, returns at the first accepted triangle or light, and keeps no counters (STATS = false).
 // IntersectBlas / IntersectBlasAny (BVHIntersect.glsl:27-181) for one local-space ray. `stack` points at this thread's
 // column of the shared stack (stride IDK_BLOCK), exactly the reference's `shared uint BlasTraversalStack[SIZE][LOCAL_SIZE]`.
-template <bool STATS, bool ANY>
+// Accept: which triangles may take the hit. A triangle that beats hit.t becomes the hit only if accept(sc, i, bx, by, t) holds;
+// trace_instance hands intersect_blas the instance's predicate, accept.at(sc, MeshTransformId, local direction). The default,
+// AcceptAll, takes every triangle and compiles away (the G-buffer pass's depth-test rules are AcceptGBuffer, idk_gbuffer.cuh).
+struct AcceptAll {
+    __device__ __forceinline__ bool operator()(const DeviceScene&, uint32_t, float, float, float) const { return true; }
+    __device__ __forceinline__ AcceptAll at(const DeviceScene&, uint32_t, f3) const { return *this; }
+};
+template <bool STATS, bool ANY, class Accept = AcceptAll>
 __device__ __forceinline__ bool intersect_blas(const DeviceScene& sc, const float4* nodes, uint32_t triOffset, f3 lo, f3 ld, f3 inv,
-                                               bool rootTest, uint32_t* stack, HitRec& hit, uint32_t& S, uint32_t& T, float& cost) {
+                                               bool rootTest, uint32_t* stack, HitRec& hit, uint32_t& S, uint32_t& T, float& cost,
+                                               const Accept& accept = Accept()) {
     float tMinLeft, tMinRight;
     if (rootTest) {   // #if !USE_TLAS
         const float4 a = ldg4(nodes + 2), b = ldg4(nodes + 3);   // root = node 1
@@ -168,7 +176,7 @@ __device__ __forceinline__ bool intersect_blas(const DeviceScene& sc, const floa
                 float4 a, b, c;
                 ldg_tri(sc.triRec, i, a, b, c);
                 float bx, by, t;
-                if (ray_triangle(lo, ld, mk3(a.x, a.y, a.z), mk3(a.w, b.x, b.y), mk3(b.z, b.w, c.x), mk3(c.y, c.z, c.w), bx, by, t) && t < hit.t) {
+                if (ray_triangle(lo, ld, mk3(a.x, a.y, a.z), mk3(a.w, b.x, b.y), mk3(b.z, b.w, c.x), mk3(c.y, c.z, c.w), bx, by, t) && t < hit.t && accept(sc, i, bx, by, t)) {
                     blasHit = true;
                     hit.tri = i;
                     hit.bx = bx;
@@ -198,9 +206,10 @@ __device__ __forceinline__ bool intersect_blas(const DeviceScene& sc, const floa
 }
 
 // One BLAS instance: local ray (Ray.glsl:7-12) + IntersectBlas. Returns whether the BLAS took the hit.
-template <bool STATS, bool ANY>
+template <bool STATS, bool ANY, class Accept = AcceptAll>
 __device__ __forceinline__ bool trace_instance(const DeviceScene& sc, uint32_t inst, f3 o, f3 d, bool rootTest, uint32_t* stack,
-                                               HitRec& hit, uint32_t& hitXform, uint32_t& S, uint32_t& T, uint32_t& I, float& cost) {
+                                               HitRec& hit, uint32_t& hitXform, uint32_t& S, uint32_t& T, uint32_t& I, float& cost,
+                                               const Accept& accept = Accept()) {
     const GpuBlasInstance bi = sc.instances[inst];
     const int nodeOffset = sc.descs[bi.BlasId].NodeOffset;
     const uint32_t triOffset = (uint32_t)sc.descs[bi.BlasId].TriangleOffset;
@@ -210,16 +219,18 @@ __device__ __forceinline__ bool trace_instance(const DeviceScene& sc, uint32_t i
     const f3 ld = xform_vector(r0, r1, r2, d);
     const f3 inv = mk3(1.0f / ld.x, 1.0f / ld.y, 1.0f / ld.z);
     if (STATS) I++;
-    if (!intersect_blas<STATS, ANY>(sc, sc.nodes + 2 * (size_t)nodeOffset, triOffset, lo, ld, inv, rootTest, stack, hit, S, T, cost)) return false;
+    if (!intersect_blas<STATS, ANY>(sc, sc.nodes + 2 * (size_t)nodeOffset, triOffset, lo, ld, inv, rootTest, stack, hit, S, T, cost,
+                                    accept.at(sc, bi.MeshTransformId, ld))) return false;
     hitXform = bi.MeshTransformId;
     return true;
 }
 
 // TraceRay / TraceRayAny (BVHIntersect.glsl:183-291,299-411): lights, then the instance loop (default) or the TLAS walk.
 // Returns what the reference returns: closest hit, hit.t != tMax; any hit, whether a light or triangle was accepted.
-template <bool STATS, bool ANY>
+template <bool STATS, bool ANY, class Accept = AcceptAll>
 __device__ __forceinline__ bool trace_ray(const DeviceScene& sc, f3 o, f3 d, float tMax, bool traceLights,
-                                          uint32_t* stack, HitRec& hit, uint32_t& hitXform, uint32_t& S, uint32_t& T, uint32_t& I, float& cost) {
+                                          uint32_t* stack, HitRec& hit, uint32_t& hitXform, uint32_t& S, uint32_t& T, uint32_t& I, float& cost,
+                                          const Accept& accept = Accept()) {
     hit.t = tMax;
     hit.tri = ~0u;
     hit.bx = 0.0f;
@@ -248,7 +259,7 @@ __device__ __forceinline__ bool trace_ray(const DeviceScene& sc, f3 o, f3 d, flo
             const uint32_t word = __float_as_uint(pA.w);
             const uint32_t id = word & 0x7FFFFFFFu;
             if (word >> 31) {
-                const bool instHit = trace_instance<STATS, ANY>(sc, id, o, d, false, stack, hit, hitXform, S, T, I, cost);
+                const bool instHit = trace_instance<STATS, ANY>(sc, id, o, d, false, stack, hit, hitXform, S, T, I, cost, accept);
                 if (ANY && instHit) return true;
                 if (sp == 0) break;
                 top = tstack[--sp];
@@ -274,7 +285,7 @@ __device__ __forceinline__ bool trace_ray(const DeviceScene& sc, f3 o, f3 d, flo
         }
     } else {
         for (uint32_t inst = 0; inst < sc.instanceCount; inst++) {
-            const bool instHit = trace_instance<STATS, ANY>(sc, inst, o, d, true, stack, hit, hitXform, S, T, I, cost);
+            const bool instHit = trace_instance<STATS, ANY>(sc, inst, o, d, true, stack, hit, hitXform, S, T, I, cost, accept);
             if (ANY && instHit) return true;
         }
     }

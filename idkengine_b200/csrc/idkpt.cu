@@ -22,12 +22,14 @@
 #include "idk_deferred.cuh"
 #include "idk_ssr_taa.cuh"
 #include "idk_vrs.cuh"
+#include "idk_gbuffer.cuh"
 #include "idk_textures_host.h"
 
 #define IDKPT_ABI_VERSION 4u   // 2: IdkPtSceneDesc gained Textures / TextureCount; 3: IdkPtStats gained CompactMs / AccumulateMs, host-buffer registration;
                                // 4: gather handle blob is 5 IPC handles (320 bytes), IDKPT_CREATE_GLOBAL_SLOTS, idkpt_gather_connect.
                                // Entry points added since (point-shadow cube maps, idkvx_set_shadow_maps, volumetric lighting, SSAO
-                               // and deferred lighting, SSR and the TAA resolve, the shading-rate classifier) are additive and keep 4;
+                               // and deferred lighting, SSR and the TAA resolve, the shading-rate classifier, the G-buffer pass) are
+                               // additive and keep 4;
                                // IdkPtDeferredSettings grew a trailing IsVariableRateShading.
 
 struct DevBuf {
@@ -123,6 +125,10 @@ struct IdkPtCtx : IdkCtxBase {
     // image and the r32f debug image, one texel per 16x16 tile, and the per-tile coarse-fragment offsets of the lighting pass
     DevBuf vrsRates, vrsDebug, vrsOffsets;
     int vrsW = 0, vrsH = 0;        // render size of the last successful idkpt_shading_rate call (0: none since the scene was set)
+
+    // the G-buffer pass (idkpt_gbuffer): the six planar fp32 attachments in one allocation, the previous positions' upload
+    DevBuf gbImages, gbPrev;
+    int gbW = 0, gbH = 0;          // render size of the last successful idkpt_gbuffer call (0: none since the scene was set)
 
     // present chain: bloom mip chains (rgba16f), AgX constants, RGBA8 frame
     DevBuf bloomDown, bloomUp, postConsts, ldr;
@@ -280,6 +286,7 @@ static int configure_launches(IdkPtCtx* ctx) {
     CK(cudaFuncSetAttribute(k_trace_rays_any, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)ctx->stackBytes));
     CK(cudaFuncSetAttribute(k_shadows_ray_traced, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)ctx->stackBytes));
     CK(cudaFuncSetAttribute(k_point_shadow_faces, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)ctx->stackBytes));
+    CK(cudaFuncSetAttribute(k_gbuffer, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)ctx->stackBytes));
     ctx->traverse2Smem = (size_t)stackSize * IDK_T2_BLOCK * sizeof(uint32_t);
     CK(cudaFuncSetAttribute(k_traverse2<false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)ctx->traverse2Smem));
     CK(cudaFuncSetAttribute(k_traverse2<true, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)ctx->traverse2Smem));
@@ -620,7 +627,8 @@ IDKPT_API void idkpt_destroy(IdkPtCtx* ctx) {
                      &ctx->tlasScratch, &ctx->oidn[0], &ctx->oidn[1], &ctx->oidn[2], &ctx->oidn[3], &ctx->denoiseWork[0], &ctx->denoiseWork[1], &ctx->denoised,
                      &ctx->pointShadowDev, &ctx->pointShadowMaps, &ctx->pointShadowLights, &ctx->volMarch, &ctx->volDepth, &ctx->volOut,
                      &ctx->gbufStage, &ctx->rtStage, &ctx->rtPtrs, &ctx->ssaoOut, &ctx->deferredOut,
-                     &ctx->ssrOut, &ctx->ssrMerged, &ctx->taaHist[0], &ctx->taaHist[1], &ctx->vrsRates, &ctx->vrsDebug, &ctx->vrsOffsets};
+                     &ctx->ssrOut, &ctx->ssrMerged, &ctx->taaHist[0], &ctx->taaHist[1], &ctx->vrsRates, &ctx->vrsDebug, &ctx->vrsOffsets,
+                     &ctx->gbImages, &ctx->gbPrev};
     for (DevBuf* b : all) release(*b);
     for (int i = 0; i < IDK_MAX_LANES; i++) release_lane(ctx->lanes[i], false);
     for (cudaEvent_t ev : ctx->events) cudaEventDestroy(ev);
@@ -675,6 +683,8 @@ IDKPT_API int idkpt_set_scene(IdkPtCtx* ctx, const IdkPtSceneDesc* s) {
     ctx->taaLast = -1;
     release(ctx->vrsRates); release(ctx->vrsDebug); release(ctx->vrsOffsets);
     ctx->vrsW = ctx->vrsH = 0;
+    release(ctx->gbImages); release(ctx->gbPrev);
+    ctx->gbW = ctx->gbH = 0;
     int rc;
     // nodes and triangle records share one allocation ("bvh"): [nodes | triRec], so that one L2 access-policy window covers both
     const size_t nodeBytes = ((s->BlasNodeCount * sizeof(GpuBlasNode)) + 255) & ~(size_t)255;
@@ -1360,7 +1370,7 @@ static int preload_kernels(IdkPtCtx* ctx) {
     IDK_PRELOAD(k_denoise_prepare); IDK_PRELOAD(k_denoise_atrous); IDK_PRELOAD(k_denoise_finish); IDK_PRELOAD(k_denoise_import);
     IDK_PRELOAD(k_bcn_decode); IDK_PRELOAD(k_point_shadow_faces); IDK_PRELOAD(k_volumetric_march); IDK_PRELOAD(k_volumetric_upscale);
     IDK_PRELOAD(k_ssao); IDK_PRELOAD(k_deferred_lighting); IDK_PRELOAD(k_ssr); IDK_PRELOAD(k_taa_resolve);
-    IDK_PRELOAD(k_shading_rate); IDK_PRELOAD(k_vrs_scan); IDK_PRELOAD(k_deferred_lighting_vrs);
+    IDK_PRELOAD(k_shading_rate); IDK_PRELOAD(k_vrs_scan); IDK_PRELOAD(k_deferred_lighting_vrs); IDK_PRELOAD(k_gbuffer);
 #undef IDK_PRELOAD
     return IDKPT_OK;
 }
@@ -2451,6 +2461,87 @@ IDKPT_API int idkpt_shading_rate_device_ptr(IdkPtCtx* ctx, void** devPtr, uint64
     if (!ctx->vrsW) return fail(ctx, IDKPT_ERR_INVALID_ARGUMENT, "idkpt_shading_rate_device_ptr: call idkpt_shading_rate first");
     *devPtr = ctx->vrsRates.p;
     if (bytes) *bytes = (uint64_t)((ctx->vrsW + IDK_VRS_TILE - 1) / IDK_VRS_TILE) * ((ctx->vrsH + IDK_VRS_TILE - 1) / IDK_VRS_TILE);
+    return IDKPT_OK;
+}
+
+// ---- the G-buffer pass (RasterPipeline.Render's "Fill G-Buffer" draws) --------------------------------------------------------
+// The six attachments' planes in one allocation, each 256-byte aligned: Depth 1, NormalRG 2, AlbedoRGB 3, MetallicRoughness 2,
+// EmissiveRGB 3, VelocityRG 2 floats per pixel. Returns the total size.
+static size_t gbuffer_planes(int w, int h, size_t offsets[6]) {
+    static const size_t floats[6] = {1, 2, 3, 2, 3, 2};
+    size_t n = 0;
+    for (int i = 0; i < 6; i++) {
+        offsets[i] = n;
+        n += (((size_t)w * h * floats[i] * 4) + 255) & ~(size_t)255;
+    }
+    return n;
+}
+
+IDKPT_API int idkpt_gbuffer(IdkPtCtx* ctx, const GpuPerFrameData* frame, int32_t width, int32_t height, const float* taaJitter,
+                            const PackedVec3* prevPositions, float* kernelMs) {
+    static const char* who = "idkpt_gbuffer";
+    if (!ctx || !frame) return fail(ctx, IDKPT_ERR_INVALID_ARGUMENT, "idkpt_gbuffer: null argument");
+    if (!ctx->haveScene) return fail(ctx, IDKPT_ERR_NO_SCENE, "idkpt_gbuffer: no scene");
+    if (width < 1 || height < 1 || width > 16384 || height > 16384) return fail(ctx, who, IDKPT_ERR_INVALID_ARGUMENT, "size outside 1..16384");
+    if (taaJitter && (!std::isfinite(taaJitter[0]) || !std::isfinite(taaJitter[1])))
+        return fail(ctx, who, IDKPT_ERR_INVALID_ARGUMENT, "jitter not finite");
+    CK(cudaSetDevice(ctx->device));
+    if (kernelMs) *kernelMs = 0.0f;
+    size_t off[6];
+    const size_t bytes = gbuffer_planes(width, height, off);
+    const size_t prevBytes = ctx->counts.VertexPositionCount * sizeof(PackedVec3);
+    ctx->gbW = ctx->gbH = 0;       // the images may be reallocated and are overwritten: valid again only when the call succeeds
+    if (ensure(ctx->gbImages, bytes) != cudaSuccess || (prevPositions && ensure(ctx->gbPrev, std::max<size_t>(prevBytes, 16)) != cudaSuccess))
+        return fail(ctx, IDKPT_ERR_OUT_OF_MEMORY, "idkpt_gbuffer: device allocation failed");
+    if (prevPositions && prevBytes) CK(cudaMemcpyAsync(ctx->gbPrev.p, prevPositions, prevBytes, cudaMemcpyHostToDevice, ctx->stream));
+    char* base = (char*)ctx->gbImages.p;
+    GBufferArgs a;
+    a.sc = ctx->sc;
+    a.positions = (const float*)ctx->positions.p;
+    a.prevPositions = prevPositions ? (const float*)ctx->gbPrev.p : a.positions;
+    memcpy(a.projView, frame->ProjView, sizeof(a.projView));
+    memcpy(a.prevProjView, frame->PrevProjView, sizeof(a.prevProjView));
+    memcpy(a.invProjView, frame->InvProjView, sizeof(a.invProjView));
+    for (int k = 0; k < 3; k++) a.viewPos[k] = frame->ViewPos[k];
+    a.jitter[0] = taaJitter ? taaJitter[0] : 0.0f; a.jitter[1] = taaJitter ? taaJitter[1] : 0.0f;
+    a.w = width; a.h = height;
+    a.depth = (float*)(base + off[0]); a.normalRG = (float2*)(base + off[1]); a.albedo = (float*)(base + off[2]);
+    a.metallicRoughness = (float2*)(base + off[3]); a.emissive = (float*)(base + off[4]); a.velocity = (float2*)(base + off[5]);
+    const size_t tiles = (size_t)((width + 7) / 8) * (size_t)((height + 7) / 8);
+    const int rc = run_timed(ctx, who, kernelMs, [&]() -> int {
+        k_gbuffer<<<(unsigned)((tiles + 3) / 4), IDK_BLOCK, ctx->stackBytes, ctx->stream>>>(a);
+        return IDKPT_OK;
+    });
+    if (rc == IDKPT_OK) { ctx->gbW = width; ctx->gbH = height; }
+    return rc;
+}
+
+IDKPT_API int idkpt_gbuffer_device_ptrs(IdkPtCtx* ctx, IdkPtGBuffer* gbufferOut, const float** velocityOut) {
+    if (!ctx || (!gbufferOut && !velocityOut)) return fail(ctx, IDKPT_ERR_INVALID_ARGUMENT, "idkpt_gbuffer_device_ptrs: null argument");
+    if (!ctx->gbW) return fail(ctx, IDKPT_ERR_INVALID_ARGUMENT, "idkpt_gbuffer_device_ptrs: call idkpt_gbuffer first");
+    size_t off[6];
+    gbuffer_planes(ctx->gbW, ctx->gbH, off);
+    const char* base = (const char*)ctx->gbImages.p;
+    if (gbufferOut)
+        *gbufferOut = IdkPtGBuffer{ctx->gbW, ctx->gbH, 1, (const float*)(base + off[0]), (const float*)(base + off[1]),
+                                   (const float*)(base + off[2]), (const float*)(base + off[3]), (const float*)(base + off[4])};
+    if (velocityOut) *velocityOut = (const float*)(base + off[5]);
+    return IDKPT_OK;
+}
+
+IDKPT_API int idkpt_read_gbuffer(IdkPtCtx* ctx, float* depth, float* normalRG, float* albedoRGB, float* metallicRoughness,
+                                 float* emissiveRGB, float* velocityRG) {
+    if (!ctx) return IDKPT_ERR_INVALID_ARGUMENT;
+    if (!ctx->gbW) return fail(ctx, IDKPT_ERR_INVALID_ARGUMENT, "idkpt_read_gbuffer: call idkpt_gbuffer first");
+    CK(cudaSetDevice(ctx->device));
+    size_t off[6];
+    gbuffer_planes(ctx->gbW, ctx->gbH, off);
+    float* dst[6] = {depth, normalRG, albedoRGB, metallicRoughness, emissiveRGB, velocityRG};
+    static const size_t floats[6] = {1, 2, 3, 2, 3, 2};
+    const size_t n = (size_t)ctx->gbW * ctx->gbH;
+    for (int i = 0; i < 6; i++)
+        if (dst[i]) CK(cudaMemcpyAsync(dst[i], (const char*)ctx->gbImages.p + off[i], n * floats[i] * 4, cudaMemcpyDeviceToHost, ctx->stream));
+    CK(cudaStreamSynchronize(ctx->stream));
     return IDKPT_OK;
 }
 

@@ -34,6 +34,7 @@ class PathTracer:
             raise IdkPtError(f"idkpt_create failed ({rc}): {msg.decode() if msg else ''}")
         self.width, self.height = width, height
         self.tile = tile
+        self._device = device
         self._frame = None
         self._keep = None
         self.last_stats = None
@@ -66,6 +67,7 @@ class PathTracer:
     def SetScene(self, scene):
         d, keep = capi.scene_desc(scene)
         self._check(self._lib.idkpt_set_scene(self._ctx, ctypes.byref(d)), "idkpt_set_scene")
+        self._vertex_position_count = int(d.VertexPositionCount)
 
     def UpdateRange(self, which, first, data):
         data = np.ascontiguousarray(data)
@@ -458,6 +460,48 @@ class PathTracer:
         p, n = ctypes.c_void_p(), ctypes.c_uint64()
         self._check(self._lib.idkpt_deferred_device_ptr(self._ctx, ctypes.byref(p), ctypes.byref(n)), "idkpt_deferred_device_ptr")
         return p.value, n.value
+
+    # ---- the G-buffer pass (RasterPipeline.Render's "Fill G-Buffer" draws)
+    GBUFFER_CHANNELS = (1, 2, 3, 2, 3, 2)   # depth, normal_rg, albedo, metallic_roughness, emissive, velocity_rg
+
+    def GBuffer(self, frame, width, height, jitter=None, prev_positions=None, download=True):
+        """Renders the G-buffer pass at width x height (DESIGN.md 8f.1g). jitter: taaDataUBO.Jitter in NDC units (None = 0);
+        prev_positions: the previous frame's vertex positions, float32 [VertexPositionCount, 3] (None = this frame's). Returns
+        (depth [h, w], normal_rg [h, w, 2], albedo [h, w, 3], metallic_roughness [h, w, 2], emissive [h, w, 3], velocity_rg
+        [h, w, 2]) as float32 numpy arrays, or None with download=False (the images stay on the device: GBufferDevicePtrs).
+        Kernel ms in last_gbuffer_ms."""
+        jit = None if jitter is None else np.ascontiguousarray(jitter, np.float32)
+        prev = None if prev_positions is None else np.ascontiguousarray(prev_positions, np.float32)
+        if jit is not None and jit.size != 2:
+            raise ValueError("GBuffer: jitter has two components")
+        if prev is not None and (prev.ndim != 2 or prev.shape[1] != 3 or prev.shape[0] != self._vertex_position_count):
+            raise ValueError(f"GBuffer: prev_positions {prev.shape}: expected ({self._vertex_position_count}, 3)")
+        frame = np.ascontiguousarray(frame)
+        ms = ctypes.c_float()
+        self._check(self._lib.idkpt_gbuffer(self._ctx, frame.ctypes.data, width, height, jit.ctypes.data if jit is not None else None,
+                                            prev.ctypes.data if prev is not None else None, ctypes.byref(ms)), "idkpt_gbuffer")
+        self.last_gbuffer_ms = ms.value
+        if not download:
+            return None
+        out = [np.zeros((height, width) if c == 1 else (height, width, c), np.float32) for c in self.GBUFFER_CHANNELS]
+        self._check(self._lib.idkpt_read_gbuffer(self._ctx, *[a.ctypes.data for a in out]), "idkpt_read_gbuffer")
+        return tuple(out)
+
+    def GBufferDevicePtrs(self, tensors=False):
+        """The images of the last GBuffer call: (capi.IdkPtGBuffer with OnDevice = 1, velocity device pointer), or with
+        tensors=True zero-copy CUDA tensors (depth, normal_rg, albedo, metallic_roughness, emissive, velocity_rg) over them,
+        valid until the next GBuffer call with another size or SetScene."""
+        g, v = capi.IdkPtGBuffer(), ctypes.c_void_p()
+        self._check(self._lib.idkpt_gbuffer_device_ptrs(self._ctx, ctypes.byref(g), ctypes.byref(v)), "idkpt_gbuffer_device_ptrs")
+        if not tensors:
+            return g, v.value
+        import torch
+        from .multigpu import DeviceArray
+        h, w = g.Height, g.Width
+        ptrs = [g.Depth, g.NormalRG, g.AlbedoRGB, g.MetallicRoughness, g.EmissiveRGB, v.value]
+        dev = torch.device("cuda", self._device)
+        return tuple(torch.as_tensor(DeviceArray(p, (h, w) if c == 1 else (h, w, c)), device=dev)
+                     for p, c in zip(ptrs, self.GBUFFER_CHANNELS))
 
     # ---- variable-rate deferred lighting (LightingShadingRateClassifier.Compute)
     def ShadingRate(self, frame, velocity_rg, settings=None, color=None, source=None, download=True, debug=False):

@@ -461,6 +461,28 @@ IDKPT_API int idkpt_shading_rate(IdkPtCtx* ctx, const GpuPerFrameData* frame, co
                                  const IdkPtShadingRateInputs* inputs, uint8_t* out_rates, float* debug_out_r32f, float* kernel_ms);
 IDKPT_API int idkpt_shading_rate_device_ptr(IdkPtCtx* ctx, void** dev_ptr, uint64_t* bytes);
 
+/* ---- the G-buffer pass (RasterPipeline.Render: the "Fill G-Buffer" draws, GBuffer/VertexPath/vertex.glsl + fragment.glsl) ----
+ * idkpt_gbuffer: renders the pass at the render size width x height into context images, ray-cast at pixel centres: each pixel
+ *   holds the closest surface along the ray through its centre that the pass does not clip (depth outside [0, 1]), cull
+ *   (blended materials; back faces of single-sided materials) or discard (alpha test). Six planar fp32 arrays [Height][Width],
+ *   each 256-byte aligned: Depth 1 float per pixel, NormalRG 2, AlbedoRGB 3, MetallicRoughness 2, EmissiveRGB 3, VelocityRG 2,
+ *   holding exactly what the engine's attachments hold (R11G11B10F albedo and emissive, RG8 normal and metallic/roughness,
+ *   RG16F velocity, D32F depth); pixels without a surface hold the clears (depth 1, everything else 0). The rules are in
+ *   DESIGN.md 8f.1g. taa_jitter: taaDataUBO.Jitter in NDC units, NULL = (0, 0). prev_positions: the previous frame's vertex
+ *   positions (prevVertexPositionSSBO, VertexPositionCount entries), NULL = this frame's (static geometry); idkpt_skin_vertices
+ *   keeps no copy, so a host that animates passes them. Lights and the skybox are separate draws and are not rendered.
+ * idkpt_gbuffer_device_ptrs: the images of the last successful call: an IdkPtGBuffer with OnDevice = 1 that idkpt_ssao,
+ *   idkpt_deferred_lighting and idkpt_ssr take as it is, and the velocity for IdkPtTaaInputs / IdkPtShadingRateInputs.
+ *   Either output may be NULL.
+ * idkpt_read_gbuffer: downloads the images of the last successful call; any argument may be NULL.
+ * The call is synchronous and ordered after the samples idkpt_compute has queued. Its images are context allocations, reused
+ * by calls with the same size, valid until the next call with another size, a failed call, idkpt_set_scene or idkpt_destroy. */
+IDKPT_API int idkpt_gbuffer(IdkPtCtx* ctx, const GpuPerFrameData* frame, int32_t width, int32_t height, const float* taa_jitter,
+                            const PackedVec3* prev_positions, float* kernel_ms);
+IDKPT_API int idkpt_gbuffer_device_ptrs(IdkPtCtx* ctx, IdkPtGBuffer* gbuffer_out, const float** velocity_rg_out);
+IDKPT_API int idkpt_read_gbuffer(IdkPtCtx* ctx, float* depth, float* normal_rg, float* albedo_rgb, float* metallic_roughness,
+                                 float* emissive_rgb, float* velocity_rg);
+
 /* ---- dynamic geometry (SURVEY.md 8f.2): ModelManager.Update = skin -> refit -> TLAS (ModelManager.cs:236-261) ----
  * idkpt_set_skinning_data: unskinnedVertexSSBO upload (52-byte GpuUnskinnedVertex records).
  * idkpt_skin_vertices: uploads the joint matrices (row-major mat4x3 = 3 x vec4 each, ModelManager.cs:272-277) and runs

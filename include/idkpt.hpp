@@ -259,6 +259,23 @@ public:
         check(idkpt_shading_rate_device_ptr(ctx_, &p, bytes), "idkpt_shading_rate_device_ptr");
         return p;
     }
+    // The G-buffer pass at width x height into context images (DESIGN.md 8f.1g); taaJitter and prevPositions may be nullptr.
+    // Returns the kernel time in ms.
+    float GBuffer(const GpuPerFrameData& frame, int32_t width, int32_t height, const float* taaJitter = nullptr,
+                  const PackedVec3* prevPositions = nullptr) {
+        float ms = 0.0f;
+        check(idkpt_gbuffer(ctx_, &frame, width, height, taaJitter, prevPositions, &ms), "idkpt_gbuffer");
+        return ms;
+    }
+    // The images of the last GBuffer call: an OnDevice G-buffer for Ssao / DeferredLighting / Ssr, and the velocity.
+    IdkPtGBuffer GBufferDevicePtrs(const float** velocityRG = nullptr) {
+        IdkPtGBuffer g = {};
+        check(idkpt_gbuffer_device_ptrs(ctx_, &g, velocityRG), "idkpt_gbuffer_device_ptrs");
+        return g;
+    }
+    void ReadGBuffer(float* depth, float* normalRG, float* albedoRGB, float* metallicRoughness, float* emissiveRGB, float* velocityRG) {
+        check(idkpt_read_gbuffer(ctx_, depth, normalRG, albedoRGB, metallicRoughness, emissiveRGB, velocityRG), "idkpt_read_gbuffer");
+    }
     void SetSkinningData(const GpuUnskinnedVertex* vertices, uint64_t count) { check(idkpt_set_skinning_data(ctx_, vertices, count), "idkpt_set_skinning_data"); }
     void SkinVertices(const float* jointMatrices3x4, uint64_t jointCount, const IdkPtSkinningCmd* cmds, uint32_t cmdCount) {
         check(idkpt_skin_vertices(ctx_, jointMatrices3x4, jointCount, cmds, cmdCount, nullptr), "idkpt_skin_vertices");

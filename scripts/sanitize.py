@@ -195,3 +195,18 @@ with PathTracer(16, 16) as pt:
         pt.ShadingRate(fv, torch.zeros((vh, vw, 2), device="cuda"), source=capi.LIT_SOURCE_DEFERRED, download=False)
         pt.ShadingRateDevicePtr()
 print("shading rate + coarse deferred lighting ok")
+
+# the G-buffer pass: the textured room (alpha cut-outs, every texture slot) through the instance loop and the TLAS walk, odd
+# sizes, jitter and previous positions, then the device chain on its images
+for use_tlas in (False, True):
+    scene.build_tlas(use=use_tlas)
+    prev = np.stack([scene.positions["x"], scene.positions["y"], scene.positions["z"]], 1).astype(np.float32) + 0.01
+    with PathTracer(16, 16) as pt:
+        pt.SetScene(scene)
+        for gw, gh in ((37, 23), (1, 1), (96, 64)):
+            fg = scenes.camera_frame(cam, gw, gh)
+            pt.GBuffer(fg, gw, gh, jitter=(0.01, -0.02), prev_positions=prev)
+            d, n, a, mr, e, v = pt.GBufferDevicePtrs(tensors=True)
+            pt.Ssao(fg, d, n, download=False)
+            pt.DeferredLighting(fg, d, n, a, mr, e, settings=capi.IdkPtDeferredSettings(0, 1, 0, 0), download=False)
+print("g-buffer pass ok")
