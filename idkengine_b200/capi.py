@@ -101,7 +101,7 @@ EXPORTS = [
     "idkpt_ssao", "idkpt_ssao_device_ptr", "idkpt_deferred_lighting", "idkpt_deferred_device_ptr",
     "idkpt_ssr", "idkpt_ssr_device_ptrs", "idkpt_taa_resolve", "idkpt_taa_device_ptr",
     "idkpt_shading_rate", "idkpt_shading_rate_device_ptr",
-    "idkpt_gbuffer", "idkpt_gbuffer_device_ptrs", "idkpt_read_gbuffer",
+    "idkpt_gbuffer", "idkpt_gbuffer_device_ptrs", "idkpt_read_gbuffer", "idkpt_transparency",
 ]
 
 IDKPT_MAX_POINT_SHADOWS = 128
@@ -167,6 +167,18 @@ def default_taa_settings():
 class IdkPtTaaInputs(ctypes.Structure):
     _fields_ = [("Width", c_i32), ("Height", c_i32), ("OnDevice", c_i32), ("Source", c_i32), ("Depth", c_vp), ("VelocityRG", c_vp),
                 ("ColorRgba32f", c_vp)]
+
+
+class IdkPtTransparencySettings(ctypes.Structure):
+    _fields_ = [("ShadowMode", c_i32), ("IsVXGI", c_i32)]
+
+
+def default_transparency_settings():
+    """The record program's uniforms at RasterPipeline's defaults: ShadowMode.Pcf, IsVXGI off."""
+    return IdkPtTransparencySettings(SHADOW_MODE_PCF, 0)
+
+
+TRANSPARENT_LAYERS = 10   # RasterPipeline.TRANSPARENT_LAYERS: blended layers kept per pixel
 
 
 class IdkPtShadingRateSettings(ctypes.Structure):
@@ -422,6 +434,8 @@ def load(path=None):
     L.idkpt_gbuffer.argtypes = [c_vp, c_vp, c_i32, c_i32, c_vp, c_vp, P(c_f)]
     L.idkpt_gbuffer_device_ptrs.restype = c_i32
     L.idkpt_gbuffer_device_ptrs.argtypes = [c_vp, P(IdkPtGBuffer), P(c_vp)]
+    L.idkpt_transparency.restype = c_i32
+    L.idkpt_transparency.argtypes = [c_vp, c_vp, P(IdkPtTransparencySettings), P(IdkPtGBuffer), c_vp, c_vp, c_vp, c_i32, c_vp, c_vp, P(c_f)]
     L.idkpt_read_gbuffer.restype = c_i32
     L.idkpt_read_gbuffer.argtypes = [c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp]
     L.idkpt_abi_version.restype = c_u32

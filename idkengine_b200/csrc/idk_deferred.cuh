@@ -152,6 +152,36 @@ __device__ __forceinline__ float deferred_pcf(const PointShadowMapsDev& m, int s
     return visibility / 21.0f;
 }
 
+// EvaluateLighting (Impl.glsl:5-23) of one light, unshadowed: GGXBrdf with the per-surface terms precomputed by the caller
+// (f0 = mix(vec3(r0), albedo, metallic) with r0 of the caller's IOR, diffuseBrdf = albedo * (1 - ao), 1 - metallic, and the
+// squared roughness clamped for DistributionGGX (rD) and SmithGGXCorrelated (rG)); V = normalize(viewPos - fragPos).
+__device__ __forceinline__ f3 deferred_evaluate_light(const GpuLight& light, f3 fragPos, f3 normal, f3 V, f3 f0, f3 diffuseBrdf,
+                                                      float oneMinusMetallic, float rD, float rG) {
+    const f3 lightPos = mk3(light.Position[0], light.Position[1], light.Position[2]);
+    const f3 surfaceToLight = lightPos - fragPos;
+    const f3 L = normalize3(surfaceToLight);
+    const float distSq = dot3(surfaceToLight, surfaceToLight);
+    const float lr = fmaxf(light.Radius, 0.0001f);
+    const float attenuation = (lr * lr) / fmaxf(distSq, 0.0001f);   // GetAttenuationFactor
+    const f3 H = normalize3(V + L);
+    const float NoV = fabsf(dot3(normal, V));
+    const float NoL = clamp1(dot3(normal, L), 0.0f, 1.0f);
+    const float NoH = clamp1(dot3(normal, H), 0.0f, 1.0f);
+    const float LoH = clamp1(dot3(L, H), 0.0f, 1.0f);
+    const float aD = NoH * rD;                                        // DistributionGGX
+    const float k = rD / ((1.0f - NoH * NoH) + aD * aD);
+    const float D = (k * k) / IDK_PI;
+    const float ggxl = NoV * sqrtf((-NoL * rG + NoL) * NoL + rG);     // SmithGGXCorrelated
+    const float ggxv = NoL * sqrtf((-NoV * rG + NoV) * NoV + rG);
+    const float G = 0.5f / (ggxv + ggxl);
+    const float fw = det_exp((det_log2(1.0f - LoH) * 0.69314718f) * 5.0f);   // FresnelSchlick: pow(1 - LoH, 5)
+    const f3 F = mk3(f0.x + (1.0f - f0.x) * fw, f0.y + (1.0f - f0.y) * fw, f0.z + (1.0f - f0.z) * fw);
+    const f3 specular = F * (D * G);
+    const f3 combined = specular + (diffuseBrdf * (mk3(1.0f, 1.0f, 1.0f) - F)) * oneMinusMetallic;
+    const float cosTheta = clamp1(dot3(normal, L), 0.0f, 1.0f);
+    return ((combined * attenuation) * cosTheta) * mk3(light.Color[0], light.Color[1], light.Color[2]);
+}
+
 // The fragment shader at one sample: every G-buffer read at texel p (imgCoord), the NDC from uv() (a float2, evaluated after
 // the sky test). Hands the lit value (alpha 1; the sky, depth 1, is black) to store(float4). k_deferred_lighting runs it once
 // per pixel, k_deferred_lighting_vrs (idk_vrs.cuh) once per coarse fragment. The callbacks keep k_deferred_lighting's SASS
@@ -190,29 +220,7 @@ __device__ __forceinline__ void deferred_shade(const DeferredArgs& a, const GpuL
     for (int i = 0; i < a.lightCount; i++) {
         const GpuLight& light = s_lights[i];
         const f3 lightPos = mk3(light.Position[0], light.Position[1], light.Position[2]);
-        // EvaluateLighting (Impl.glsl:5-23)
-        const f3 surfaceToLight = lightPos - fragPos;
-        const f3 L = normalize3(surfaceToLight);
-        const float distSq = dot3(surfaceToLight, surfaceToLight);
-        const float lr = fmaxf(light.Radius, 0.0001f);
-        const float attenuation = (lr * lr) / fmaxf(distSq, 0.0001f);   // GetAttenuationFactor
-        const f3 H = normalize3(V + L);
-        const float NoV = fabsf(dot3(normal, V));
-        const float NoL = clamp1(dot3(normal, L), 0.0f, 1.0f);
-        const float NoH = clamp1(dot3(normal, H), 0.0f, 1.0f);
-        const float LoH = clamp1(dot3(L, H), 0.0f, 1.0f);
-        const float aD = NoH * rD;                                        // DistributionGGX
-        const float k = rD / ((1.0f - NoH * NoH) + aD * aD);
-        const float D = (k * k) / IDK_PI;
-        const float ggxl = NoV * sqrtf((-NoL * rG + NoL) * NoL + rG);     // SmithGGXCorrelated
-        const float ggxv = NoL * sqrtf((-NoV * rG + NoV) * NoV + rG);
-        const float G = 0.5f / (ggxv + ggxl);
-        const float fw = det_exp((det_log2(1.0f - LoH) * 0.69314718f) * 5.0f);   // FresnelSchlick: pow(1 - LoH, 5)
-        const f3 F = mk3(f0.x + (1.0f - f0.x) * fw, f0.y + (1.0f - f0.y) * fw, f0.z + (1.0f - f0.z) * fw);
-        const f3 specular = F * (D * G);
-        const f3 combined = specular + (diffuseBrdf * (mk3(1.0f, 1.0f, 1.0f) - F)) * oneMinusMetallic;
-        const float cosTheta = clamp1(dot3(normal, L), 0.0f, 1.0f);
-        f3 contribution = ((combined * attenuation) * cosTheta) * mk3(light.Color[0], light.Color[1], light.Color[2]);
+        f3 contribution = deferred_evaluate_light(light, fragPos, normal, V, f0, diffuseBrdf, oneMinusMetallic, rD, rG);
         if ((contribution.x != 0.0f || contribution.y != 0.0f || contribution.z != 0.0f) && light.PointShadowIndex != -1) {
             if (a.shadowMode == 1) {
                 contribution = contribution * deferred_pcf(a.shadows, light.PointShadowIndex, unjitteredFragPos - lightPos);

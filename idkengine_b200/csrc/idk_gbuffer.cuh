@@ -42,6 +42,18 @@ __device__ __forceinline__ float gbuffer_det(const float4* model) {
     return (m0.x * (m1.y * m2.z - m1.z * m2.y) - m0.y * (m1.x * m2.z - m1.z * m2.x)) + m0.z * (m1.x * m2.y - m1.y * m2.x);
 }
 
+// The surface's alpha at barycentrics (b0, b1, b2), sampled as surface_textured samples it.
+__device__ __forceinline__ float gbuffer_alpha(const DeviceScene& sc, const GpuMaterial& mat, int4 tri, float b0, float b1, float b2) {
+    const float4 s0 = ldg4(sc.surfRec + 5 * (size_t)tri.w), s4 = ldg4(sc.surfRec + 5 * (size_t)tri.w + 4);
+    float alpha = s0.w;
+    if (__float_as_uint(s4.x) & 4u) {
+        float u, v;
+        interp_texcoord(sc, tri, b0, b1, b2, u, v);
+        alpha = tex_sample(sc, mat.BaseColorTexture, u, v).w * ((float)((mat.BaseColorFactor >> 24) & 255u) / 255.0f);
+    }
+    return alpha;
+}
+
 // One instance's depth-test rules (rule 2): a triangle that beats the current t takes the hit unless it is clipped (depth
 // outside [0, 1]), blended (AlphaCutoff == 2: culled from the pass), back-facing on a single-sided material (CullFace), or
 // alpha-discarded (Alpha < AlphaCutoff, the base-colour alpha sampled as surface_textured does).
@@ -63,14 +75,7 @@ struct AcceptGBufferInstance {
         const float b2 = 1.0f - bx - by;
         const float depth = gbuffer_depth(projView, positions, model, tri, bx, by, b2);
         if (!(depth >= 0.0f && depth <= 1.0f)) return false;
-        const float4 s0 = ldg4(sc.surfRec + 5 * (size_t)tri.w), s4 = ldg4(sc.surfRec + 5 * (size_t)tri.w + 4);
-        float alpha = s0.w;
-        if (__float_as_uint(s4.x) & 4u) {
-            float u, v;
-            interp_texcoord(sc, tri, bx, by, b2, u, v);
-            alpha = tex_sample(sc, mat.BaseColorTexture, u, v).w * ((float)((mat.BaseColorFactor >> 24) & 255u) / 255.0f);
-        }
-        return !(alpha < alphaCutoff);
+        return !(gbuffer_alpha(sc, mat, tri, bx, by, b2) < alphaCutoff);
     }
 };
 struct AcceptGBuffer {
@@ -81,6 +86,48 @@ struct AcceptGBuffer {
         return AcceptGBufferInstance{projView, positions, model, gbuffer_det(model), ld};
     }
 };
+
+// Rule 4 at barycentrics (b0, b1, b2) of BLAS triangle triIndex (= tri) in transform mt, seen along world direction d: the
+// surface (the per-mesh record, or the textures at level 0) into s, and the world normal: per-vertex world normal and tangent,
+// interpolated, then GetTBN, the normal map mixed in by NormalMapStrength, negated on a back face.
+__device__ __forceinline__ f3 gbuffer_surface(const DeviceScene& sc, uint32_t triIndex, int4 tri, const float4* mt, float b0, float b1,
+                                              float b2, f3 d, Surface& s) {
+    const float4 i0 = ldg4(mt + 3), i1 = ldg4(mt + 4), i2 = ldg4(mt + 5);
+    const float4* vf = sc.vtxFrame;
+    const float4 a0 = ldg4(vf + 2 * (size_t)tri.x), a1 = ldg4(vf + 2 * (size_t)tri.x + 1);
+    const float4 c0 = ldg4(vf + 2 * (size_t)tri.y), c1 = ldg4(vf + 2 * (size_t)tri.y + 1);
+    const float4 e0 = ldg4(vf + 2 * (size_t)tri.z), e1 = ldg4(vf + 2 * (size_t)tri.z + 1);
+    const f3 wn0 = normalize3(xform_normal(i0, i1, i2, mk3(a0.x, a0.y, a0.z)));
+    const f3 wn1 = normalize3(xform_normal(i0, i1, i2, mk3(c0.x, c0.y, c0.z)));
+    const f3 wn2 = normalize3(xform_normal(i0, i1, i2, mk3(e0.x, e0.y, e0.z)));
+    const f3 wt0 = normalize3(xform_normal(i0, i1, i2, mk3(a0.w, a1.x, a1.y)));
+    const f3 wt1 = normalize3(xform_normal(i0, i1, i2, mk3(c0.w, c1.x, c1.y)));
+    const f3 wt2 = normalize3(xform_normal(i0, i1, i2, mk3(e0.w, e1.x, e1.y)));
+    const f3 interpNormal = normalize3((wn0 * b0 + wn1 * b1) + wn2 * b2);
+    const f3 interpTangent = normalize3((wt0 * b0 + wt1 * b1) + wt2 * b2);
+
+    const float4* sr = sc.surfRec + 5 * (size_t)tri.w;
+    const float4 s0 = ldg4(sr), s1 = ldg4(sr + 1), s2 = ldg4(sr + 2), s3 = ldg4(sr + 3), s4 = ldg4(sr + 4);
+    s.Albedo = mk3(s0.x, s0.y, s0.z); s.Alpha = s0.w;
+    s.Normal = mk3(1.0f, 1.0f, 0.0f);
+    s.Emissive = mk3(s1.x, s1.y, s1.z); s.Metallic = s1.w;
+    s.Absorbance = mk3(s2.x, s2.y, s2.z); s.Roughness = s2.w;
+    s.Transmission = s3.x; s.IOR = s3.y; s.AlphaCutoff = s3.z;
+    s.IsVolumetric = false; s.TintOnTransmissive = false;
+    if (__float_as_uint(s4.x) & 4u) {
+        float tu, tv;
+        interp_texcoord(sc, tri, b0, b1, b2, tu, tv);
+        surface_textured(sc, tri.w, tu, tv, s);
+    }
+    const f3 N = normalize3(interpNormal);
+    const f3 Tn = normalize3(interpTangent);
+    const f3 B = normalize3(cross3(N, Tn));
+    const f3 tbnN = (Tn * s.Normal.x + B * s.Normal.y) + N * s.Normal.z;
+    f3 normal = normalize3(mix3(interpNormal, tbnN, s3.w));
+    const float4 nr = ldg4(sc.triRec + 4 * (size_t)triIndex + 2);
+    if (!gbuffer_front(gbuffer_det(mt), mk3(nr.y, nr.z, nr.w), xform_vector(i0, i1, i2, d))) normal = normal * -1.0f;
+    return normal;
+}
 
 // Unsigned 11- / 10-bit float (R11G11B10F, GL core spec 2.3.4.3) with `mbits` mantissa bits, as fp32: nearest, ties to even,
 // denormals below 2^-14; negative values, -0 and -inf store 0; finite values above the largest finite value (`maxv`: 65024
@@ -136,42 +183,8 @@ __global__ void __launch_bounds__(IDK_BLOCK) k_gbuffer(GBufferArgs a) {
         const float b0 = hit.bx, b1 = hit.by, b2 = 1.0f - hit.bx - hit.by;
         depth = gbuffer_depth(a.projView, a.positions, mt, tri, b0, b1, b2);
 
-        // rule 4: per-vertex world normal and tangent, interpolated, then GetTBN and the normal map
-        const float4 i0 = ldg4(mt + 3), i1 = ldg4(mt + 4), i2 = ldg4(mt + 5);
-        const float4* vf = sc.vtxFrame;
-        const float4 a0 = ldg4(vf + 2 * (size_t)tri.x), a1 = ldg4(vf + 2 * (size_t)tri.x + 1);
-        const float4 c0 = ldg4(vf + 2 * (size_t)tri.y), c1 = ldg4(vf + 2 * (size_t)tri.y + 1);
-        const float4 e0 = ldg4(vf + 2 * (size_t)tri.z), e1 = ldg4(vf + 2 * (size_t)tri.z + 1);
-        const f3 wn0 = normalize3(xform_normal(i0, i1, i2, mk3(a0.x, a0.y, a0.z)));
-        const f3 wn1 = normalize3(xform_normal(i0, i1, i2, mk3(c0.x, c0.y, c0.z)));
-        const f3 wn2 = normalize3(xform_normal(i0, i1, i2, mk3(e0.x, e0.y, e0.z)));
-        const f3 wt0 = normalize3(xform_normal(i0, i1, i2, mk3(a0.w, a1.x, a1.y)));
-        const f3 wt1 = normalize3(xform_normal(i0, i1, i2, mk3(c0.w, c1.x, c1.y)));
-        const f3 wt2 = normalize3(xform_normal(i0, i1, i2, mk3(e0.w, e1.x, e1.y)));
-        const f3 interpNormal = normalize3((wn0 * b0 + wn1 * b1) + wn2 * b2);
-        const f3 interpTangent = normalize3((wt0 * b0 + wt1 * b1) + wt2 * b2);
-
-        const float4* sr = sc.surfRec + 5 * (size_t)tri.w;
-        const float4 s0 = ldg4(sr), s1 = ldg4(sr + 1), s2 = ldg4(sr + 2), s3 = ldg4(sr + 3), s4 = ldg4(sr + 4);
         Surface s;
-        s.Albedo = mk3(s0.x, s0.y, s0.z); s.Alpha = s0.w;
-        s.Normal = mk3(1.0f, 1.0f, 0.0f);
-        s.Emissive = mk3(s1.x, s1.y, s1.z); s.Metallic = s1.w;
-        s.Absorbance = mk3(s2.x, s2.y, s2.z); s.Roughness = s2.w;
-        s.Transmission = s3.x; s.IOR = s3.y; s.AlphaCutoff = s3.z;
-        s.IsVolumetric = false; s.TintOnTransmissive = false;
-        if (__float_as_uint(s4.x) & 4u) {
-            float tu, tv;
-            interp_texcoord(sc, tri, b0, b1, b2, tu, tv);
-            surface_textured(sc, tri.w, tu, tv, s);
-        }
-        const f3 N = normalize3(interpNormal);
-        const f3 Tn = normalize3(interpTangent);
-        const f3 B = normalize3(cross3(N, Tn));
-        const f3 tbnN = (Tn * s.Normal.x + B * s.Normal.y) + N * s.Normal.z;
-        f3 normal = normalize3(mix3(interpNormal, tbnN, s3.w));
-        const float4 nr = ldg4(sc.triRec + 4 * (size_t)hit.tri + 2);
-        if (!gbuffer_front(gbuffer_det(mt), mk3(nr.y, nr.z, nr.w), xform_vector(i0, i1, i2, d))) normal = normal * -1.0f;
+        const f3 normal = gbuffer_surface(sc, hit.tri, tri, mt, b0, b1, b2, d, s);
 
         // rule 5: the previous frame's clip position, interpolated
         const float4 p0 = ldg4(mt + 6), p1 = ldg4(mt + 7), p2 = ldg4(mt + 8);

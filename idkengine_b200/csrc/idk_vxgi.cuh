@@ -312,6 +312,13 @@ __global__ void __launch_bounds__(256) k_vx_mipmap(VxGridDev g, int level) {
 }
 
 // ------------------------------------------------------------------------------------------------ cone tracing
+// ConeTraceGISettings (ConeTraceGI/include/Impl.glsl:7-15) and the noise index (the cone settings of idkpt_transparency)
+struct VxConeParams {
+    int maxSamples;
+    float stepMultiplier, giBoost, giSkyBoxBoost, normalRayOffset;
+    uint32_t noiseIndex;
+};
+
 struct VxConeArgs {
     VxGridDev g;
     float invProjView[16];
@@ -363,6 +370,46 @@ __device__ __forceinline__ float4 vx_trace_cone(const VxGridDev& g, f3 origin, f
     return acc;
 }
 
+// IndirectLight (ConeTraceGI/include/Impl.glsl:27-80) without the final GIBoost, as a statement: it declares `out` (an f3)
+// and leaves in it the irradiance averaged over the material's cone count. NOISE(i) is InterleavedGradientNoise(GetPixelCoord(), i) (the integer id
+// in a compute shader, gl_FragCoord.xy in a fragment shader); SKY(dir) is texture(skyBoxUBO.Albedo, dir) * GISkyBoxBoost;
+// `roughnessIn` is the surface's, squared here; `steps` counts the cone samples. It is a macro rather than a function because
+// nvcc optimises a callee on its own before it inlines it, which reschedules k_vx_cone_trace; written out in place, the loop
+// compiles to the instructions it compiled to when it was k_vx_cone_trace's own.
+#define VX_INDIRECT_LIGHT(out, g, maxSamples, noiseIndex0, stepMultiplier, normalRayOffset, fragPos, normal, metallicIn, roughnessIn, \
+                          incomming, NOISE, SKY, steps)                                                                               \
+    f3 out = mk3(0.0f, 0.0f, 0.0f);                                                                                                  \
+    {                                                                                                                                \
+        const float vxMetallic = (metallicIn);                                                                                      \
+        float vxRoughness = (roughnessIn);                                                                                          \
+        vxRoughness *= vxRoughness;                                                                                                  \
+        const float vxDc = 1.0f - vxMetallic - 0.0f;                                                                                 \
+        const float vxMaterialVariance = vxDc + vxMetallic * vxRoughness + 0.0f * vxRoughness;                                       \
+        const uint32_t vxSamples = (uint32_t)mix1(1.0f, (float)(maxSamples), vxMaterialVariance);                                   \
+        uint32_t vxNoiseIndex = (noiseIndex0);                                                                                       \
+        for (uint32_t vxI = 0; vxI < vxSamples; vxI++) {                                                                             \
+            const float vxRnd0 = NOISE(vxNoiseIndex + 0);                                                                              \
+            const float vxRnd1 = NOISE(vxNoiseIndex + 1);                                                                              \
+            const float vxRnd2 = NOISE(vxNoiseIndex + 2);                                                                              \
+            vxNoiseIndex++;                                                                                                          \
+            const f3 vxDiffuseDir = normalize3((normal) + sample_sphere(vxRnd0, vxRnd1));                                                  \
+            f3 vxDir;                                                                                                                  \
+            float vxConeAngle;                                                                                                         \
+            if (vxMetallic > vxRnd2) {                                                                                                 \
+                vxDir = normalize3(mix3(reflect3((incomming), (normal)), vxDiffuseDir, vxRoughness));                                    \
+                vxConeAngle = mix1(0.0f, 0.32f, vxRoughness);                                                                          \
+            } else {                                                                                                                 \
+                vxDir = vxDiffuseDir;                                                                                                    \
+                vxConeAngle = 0.32f;                                                                                                   \
+            }                                                                                                                        \
+            const float4 vxCone = vx_trace_cone((g), (fragPos), vxDir, (normal), vxConeAngle, (stepMultiplier), (normalRayOffset), 0.99f, steps); \
+            const float vxK = 1.0f - vxCone.w;                                                                                              \
+            const f3 vxSky = SKY(vxDir);                                                                                                   \
+            out = out + mk3(vxCone.x + vxK * vxSky.x, vxCone.y + vxK * vxSky.y, vxCone.z + vxK * vxSky.z);                                          \
+        }                                                                                                                            \
+        out = out / (float)vxSamples;                                                                                       \
+    }
+
 __global__ void __launch_bounds__(64) k_vx_cone_trace(VxConeArgs a) {
     const int x = blockIdx.x * 8 + threadIdx.x, yl = blockIdx.y * 8 + threadIdx.y;
     const int y = yl + a.rowFirst;
@@ -383,35 +430,13 @@ __global__ void __launch_bounds__(64) k_vx_cone_trace(VxConeArgs a) {
             const f3 fragPos = mk3(wx / ww, wy / ww, wz / ww);
             const float2 nrg = a.normalRG[p], mr = a.metalRough[p];
             const f3 normal = decode_unit_vec(nrg.x, nrg.y);
-            const float metallic = mr.x;
-            float roughness = mr.y;
             const f3 incomming = fragPos - mk3(a.viewPos[0], a.viewPos[1], a.viewPos[2]);
-            roughness *= roughness;
-            const float dc = 1.0f - metallic - 0.0f;
-            const float materialVariance = dc + metallic * roughness + 0.0f * roughness;
-            const uint32_t samples = (uint32_t)mix1(1.0f, (float)a.maxSamples, materialVariance);
-            uint32_t noiseIndex = a.noiseIndex;
-            f3 irradiance = mk3(0.0f, 0.0f, 0.0f);
-            for (uint32_t i = 0; i < samples; i++) {
-                const float rnd0 = vx_ign((float)x, (float)y, noiseIndex + 0);
-                const float rnd1 = vx_ign((float)x, (float)y, noiseIndex + 1);
-                const float rnd2 = vx_ign((float)x, (float)y, noiseIndex + 2);
-                noiseIndex++;
-                const f3 diffuseDir = normalize3(normal + sample_sphere(rnd0, rnd1));
-                f3 dir;
-                float coneAngle;
-                if (metallic > rnd2) {
-                    dir = normalize3(mix3(reflect3(incomming, normal), diffuseDir, roughness));
-                    coneAngle = mix1(0.0f, 0.32f, roughness);
-                } else {
-                    dir = diffuseDir;
-                    coneAngle = 0.32f;
-                }
-                const float4 c = vx_trace_cone(a.g, fragPos, dir, normal, coneAngle, a.stepMultiplier, a.normalRayOffset, 0.99f, steps);
-                const float k = 1.0f - c.w;
-                irradiance = irradiance + mk3(c.x + k * (a.sky[0] * a.giSkyBoxBoost), c.y + k * (a.sky[1] * a.giSkyBoxBoost), c.z + k * (a.sky[2] * a.giSkyBoxBoost));
-            }
-            irradiance = irradiance / (float)samples;
+#define VX_NOISE(i) vx_ign((float)x, (float)y, i)
+#define VX_SKY(dir) mk3(a.sky[0] * a.giSkyBoxBoost, a.sky[1] * a.giSkyBoxBoost, a.sky[2] * a.giSkyBoxBoost)
+            VX_INDIRECT_LIGHT(irradiance, a.g, a.maxSamples, a.noiseIndex, a.stepMultiplier, a.normalRayOffset, fragPos, normal, mr.x, mr.y,
+                              incomming, VX_NOISE, VX_SKY, steps)
+#undef VX_NOISE
+#undef VX_SKY
             a.out[p] = make_float4(irradiance.x * a.giBoost, irradiance.y * a.giBoost, irradiance.z * a.giBoost, 1.0f);
         }
     }

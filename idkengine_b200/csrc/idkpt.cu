@@ -23,12 +23,14 @@
 #include "idk_ssr_taa.cuh"
 #include "idk_vrs.cuh"
 #include "idk_gbuffer.cuh"
+#include "idk_transparency.cuh"
 #include "idk_textures_host.h"
 
 #define IDKPT_ABI_VERSION 4u   // 2: IdkPtSceneDesc gained Textures / TextureCount; 3: IdkPtStats gained CompactMs / AccumulateMs, host-buffer registration;
                                // 4: gather handle blob is 5 IPC handles (320 bytes), IDKPT_CREATE_GLOBAL_SLOTS, idkpt_gather_connect.
                                // Entry points added since (point-shadow cube maps, idkvx_set_shadow_maps, volumetric lighting, SSAO
-                               // and deferred lighting, SSR and the TAA resolve, the shading-rate classifier, the G-buffer pass) are
+                               // and deferred lighting, SSR and the TAA resolve, the shading-rate classifier, the G-buffer pass,
+                               // transparency) are
                                // additive and keep 4;
                                // IdkPtDeferredSettings grew a trailing IsVariableRateShading.
 
@@ -287,6 +289,8 @@ static int configure_launches(IdkPtCtx* ctx) {
     CK(cudaFuncSetAttribute(k_shadows_ray_traced, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)ctx->stackBytes));
     CK(cudaFuncSetAttribute(k_point_shadow_faces, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)ctx->stackBytes));
     CK(cudaFuncSetAttribute(k_gbuffer, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)ctx->stackBytes));
+    CK(cudaFuncSetAttribute(k_transparency<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)ctx->stackBytes));
+    CK(cudaFuncSetAttribute(k_transparency<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)ctx->stackBytes));
     ctx->traverse2Smem = (size_t)stackSize * IDK_T2_BLOCK * sizeof(uint32_t);
     CK(cudaFuncSetAttribute(k_traverse2<false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)ctx->traverse2Smem));
     CK(cudaFuncSetAttribute(k_traverse2<true, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)ctx->traverse2Smem));
@@ -1371,6 +1375,7 @@ static int preload_kernels(IdkPtCtx* ctx) {
     IDK_PRELOAD(k_bcn_decode); IDK_PRELOAD(k_point_shadow_faces); IDK_PRELOAD(k_volumetric_march); IDK_PRELOAD(k_volumetric_upscale);
     IDK_PRELOAD(k_ssao); IDK_PRELOAD(k_deferred_lighting); IDK_PRELOAD(k_ssr); IDK_PRELOAD(k_taa_resolve);
     IDK_PRELOAD(k_shading_rate); IDK_PRELOAD(k_vrs_scan); IDK_PRELOAD(k_deferred_lighting_vrs); IDK_PRELOAD(k_gbuffer);
+    IDK_PRELOAD(k_transparency<false>); IDK_PRELOAD(k_transparency<true>);
 #undef IDK_PRELOAD
     return IDKPT_OK;
 }
@@ -2548,3 +2553,75 @@ IDKPT_API int idkpt_read_gbuffer(IdkPtCtx* ctx, float* depth, float* normalRG, f
 } // extern "C"
 
 #include "idkvx_impl.cuh"
+
+// ---- transparency (RasterPipeline.Render's "Record transparent fragments" + "Resolve transparent fragments") -------------------
+// After the voxeliser's context (idkvx_impl.cuh): the VXGI path cone-traces that context's grid.
+extern "C" {
+
+IDKPT_API int idkpt_transparency(IdkPtCtx* ctx, const GpuPerFrameData* frame, const IdkPtTransparencySettings* s, const IdkPtGBuffer* g,
+                                 const float* taaJitter, IdkVxCtx* voxels, const IdkVxConeSettings* cone, int32_t source, float* color,
+                                 float* outRgba32f, float* kernelMs) {
+    static const char* who = "idkpt_transparency";
+    if (!ctx || !frame || !s || !g || !g->Depth) return fail(ctx, IDKPT_ERR_INVALID_ARGUMENT, "idkpt_transparency: null argument");
+    if (!ctx->haveScene) return fail(ctx, IDKPT_ERR_NO_SCENE, "idkpt_transparency: no scene");
+    if (g->Width < 1 || g->Height < 1 || g->Width > 16384 || g->Height > 16384) return fail(ctx, who, IDKPT_ERR_INVALID_ARGUMENT, "size outside 1..16384");
+    if (g->OnDevice != 0 && g->OnDevice != 1) return fail(ctx, who, IDKPT_ERR_INVALID_ARGUMENT, "OnDevice is neither 0 nor 1");
+    if (s->ShadowMode < 0 || s->ShadowMode > 2) return fail(ctx, who, IDKPT_ERR_INVALID_ARGUMENT, "ShadowMode outside 0..2");
+    if (s->IsVXGI != 0 && s->IsVXGI != 1) return fail(ctx, who, IDKPT_ERR_INVALID_ARGUMENT, "IsVXGI is neither 0 nor 1");
+    if (s->IsVXGI) {
+        if (!voxels || !cone) return fail(ctx, who, IDKPT_ERR_INVALID_ARGUMENT, "IsVXGI without a voxeliser context or cone settings");
+        if (!voxels->voxelized) return fail(ctx, who, IDKPT_ERR_INVALID_ARGUMENT, "IsVXGI with a voxeliser context that has not voxelised its grid");
+        if (voxels->device != ctx->device) return fail(ctx, who, IDKPT_ERR_INVALID_ARGUMENT, "IsVXGI with a voxeliser context on another device");
+        if (cone->MaxSamples < 1 || cone->MaxSamples > 64) return fail(ctx, who, IDKPT_ERR_INVALID_ARGUMENT, "cone MaxSamples out of range");
+    }
+    if (taaJitter && (!std::isfinite(taaJitter[0]) || !std::isfinite(taaJitter[1])))
+        return fail(ctx, who, IDKPT_ERR_INVALID_ARGUMENT, "jitter not finite");
+    const uint32_t shadowCount = (uint32_t)ctx->pointShadowRecs.size();
+    if (s->ShadowMode == 1) {
+        for (const GpuLight& L : ctx->hostLights)
+            if (L.PointShadowIndex != -1 && (L.PointShadowIndex < 0 || (uint32_t)L.PointShadowIndex >= shadowCount))
+                return fail(ctx, who, IDKPT_ERR_INVALID_ARGUMENT, "a light's PointShadowIndex is neither -1 nor below the point-shadow count");
+    }
+    CK(cudaSetDevice(ctx->device));
+    if (int rc = lit_source_check(ctx, who, source, false, color, g->Width, g->Height, g->OnDevice)) return rc;
+    if (g->OnDevice)
+        if (int rc = gbuffer_device_check(ctx, who, g->Depth, 4)) return rc;
+    if (kernelMs) *kernelMs = 0.0f;
+    const size_t n = (size_t)g->Width * g->Height;
+    const bool hostArray = source == IDKPT_LIT_SOURCE_ARRAY && !g->OnDevice;
+    const size_t stageBytes = g->OnDevice ? 0 : gbuffer_stage_bytes(g, {1, hostArray ? 4u : 0u});
+    if (stageBytes && ensure(ctx->gbufStage, stageBytes) != cudaSuccess)
+        return fail(ctx, IDKPT_ERR_OUT_OF_MEMORY, "idkpt_transparency: device allocation failed");
+    size_t off = 0;
+    const float *depth, *target;
+    if (int rc = gbuffer_input(ctx, g, g->Depth, 1, ctx->gbufStage, off, depth)) return rc;
+    if (int rc = lit_source_input(ctx, g, source, color, off, target)) return rc;
+    TransparencyArgs a;
+    a.sc = ctx->sc;
+    a.positions = (const float*)ctx->positions.p;
+    memcpy(a.projView, frame->ProjView, sizeof(a.projView));
+    memcpy(a.invProjView, frame->InvProjView, sizeof(a.invProjView));
+    for (int k = 0; k < 3; k++) a.viewPos[k] = frame->ViewPos[k];
+    a.jitter[0] = taaJitter ? taaJitter[0] : 0.0f; a.jitter[1] = taaJitter ? taaJitter[1] : 0.0f;
+    a.w = g->Width; a.h = g->Height;
+    a.depth = depth;
+    a.color = (float4*)target;     // the stage copy, the caller's device array or the context's deferred image: written in place
+    a.shadowMode = s->ShadowMode;
+    a.shadows = PointShadowMapsDev{(const PointShadowDev*)ctx->pointShadowDev.p, (const uint16_t*)ctx->pointShadowMaps.p, shadowCount};
+    a.g = s->IsVXGI ? voxels->grid : VxGridDev{};
+    a.cone = s->IsVXGI ? VxConeParams{cone->MaxSamples, cone->StepMultiplier, cone->GIBoost, cone->GISkyBoxBoost, cone->NormalRayOffset, cone->NoiseIndex}
+                       : VxConeParams{1, 0.0f, 0.0f, 0.0f, 0.0f, 0u};
+    const size_t tiles = (size_t)((g->Width + 7) / 8) * (size_t)((g->Height + 7) / 8);
+    const int rc = run_timed(ctx, who, kernelMs, [&]() -> int {
+        if (s->IsVXGI) k_transparency<true><<<(unsigned)((tiles + 3) / 4), IDK_BLOCK, ctx->stackBytes, ctx->stream>>>(a);
+        else k_transparency<false><<<(unsigned)((tiles + 3) / 4), IDK_BLOCK, ctx->stackBytes, ctx->stream>>>(a);
+        return IDKPT_OK;
+    });
+    if (rc != IDKPT_OK) return rc;
+    if (hostArray) CK(cudaMemcpyAsync(color, target, n * 16, cudaMemcpyDeviceToHost, ctx->stream));
+    if (outRgba32f) CK(cudaMemcpyAsync(outRgba32f, target, n * 16, cudaMemcpyDeviceToHost, ctx->stream));
+    if (hostArray || outRgba32f) CK(cudaStreamSynchronize(ctx->stream));
+    return IDKPT_OK;
+}
+
+} // extern "C"

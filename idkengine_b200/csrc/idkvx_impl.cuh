@@ -27,6 +27,11 @@ struct IdkVxCtx : IdkCtxBase {
     IdkPtCtx* shadowMaps = nullptr;       // idkvx_set_shadow_maps: visibility by the PCF lookup into this context's point-shadow cube maps
     bool shadowedLights = false;
     int32_t maxPointShadowIndex = -1;     // largest PointShadowIndex of the scene's lights
+    // the grid holds a whole voxelisation with its mip chain (idkpt_transparency's cone trace reads it): set by a successful
+    // idkvx_voxelize of the whole grid, or by idkvx_mipmap after a slab voxelisation (the multi-GPU flow all-gathers the slabs in
+    // between); cleared by idkvx_set_grid, idkvx_set_scene and idkvx_set_slab
+    bool voxelized = false;
+    bool slabVoxelized = false;           // idkvx_voxelize ran in slab mode since the grid last changed
 };
 
 static void set_grid_bounds(IdkVxCtx* ctx, const float* mn, const float* mx) {
@@ -119,6 +124,7 @@ IDKPT_API int32_t idkvx_level_count(IdkVxCtx* ctx) { return ctx ? ctx->grid.leve
 IDKPT_API int idkvx_set_grid(IdkVxCtx* ctx, const float gridMin[3], const float gridMax[3]) {
     if (!ctx || !gridMin || !gridMax) return fail(ctx, IDKPT_ERR_INVALID_ARGUMENT, "idkvx_set_grid: null argument");
     set_grid_bounds(ctx, gridMin, gridMax);
+    ctx->voxelized = ctx->slabVoxelized = false;
     return IDKPT_OK;
 }
 
@@ -126,6 +132,7 @@ IDKPT_API int idkvx_set_scene(IdkVxCtx* ctx, const IdkPtSceneDesc* s) {
     if (!ctx || !s) return fail(ctx, IDKPT_ERR_INVALID_ARGUMENT, "idkvx_set_scene: null argument");
     CK(cudaSetDevice(ctx->device));
     if (int rc = validate_scene(ctx, "idkvx_set_scene", s)) return rc;
+    ctx->voxelized = ctx->slabVoxelized = false;
     ctx->haveScene = false;   // the device arrays are overwritten from here on: a failure below leaves no scene
     ctx->shadowedLights = false;
     ctx->maxPointShadowIndex = -1;
@@ -227,6 +234,8 @@ IDKPT_API int idkvx_voxelize(IdkVxCtx* ctx, IdkVxStats* stats) {
         return IDKPT_OK;
     });
     if (rc) return rc;
+    ctx->voxelized = !ctx->slabMode;
+    ctx->slabVoxelized = ctx->slabMode;
     if (stats) {
         CK(cudaEventElapsedTime(&stats->ClearMs, ctx->timing[0], ctx->timing[2]));
         CK(cudaEventElapsedTime(&stats->VoxelizeMs, ctx->timing[2], ctx->timing[3]));
@@ -245,6 +254,7 @@ IDKPT_API int idkvx_set_slab(IdkVxCtx* ctx, int32_t z0, int32_t z1) {
     const int d = ctx->grid.sz[0];
     if (z0 < 0 || z1 > d || z0 >= z1) return fail(ctx, IDKPT_ERR_INVALID_ARGUMENT, "idkvx_set_slab: need 0 <= z0 < z1 <= depth");
     ctx->grid.z0 = z0; ctx->grid.z1 = z1;
+    ctx->voxelized = ctx->slabVoxelized = false;
     ctx->slabMode = !(z0 == 0 && z1 == d);
     return IDKPT_OK;
 }
@@ -267,6 +277,7 @@ IDKPT_API int idkvx_mipmap(IdkVxCtx* ctx, IdkVxStats* stats) {
         return IDKPT_OK;
     });
     if (rc == IDKPT_OK && stats) stats->KernelLaunches = launches;
+    if (rc == IDKPT_OK && ctx->slabVoxelized) ctx->voxelized = true;
     return rc;
 }
 

@@ -503,6 +503,43 @@ class PathTracer:
         return tuple(torch.as_tensor(DeviceArray(p, (h, w) if c == 1 else (h, w, c)), device=dev)
                      for p, c in zip(ptrs, self.GBUFFER_CHANNELS))
 
+    # ---- transparency (RasterPipeline.Render's "Record transparent fragments" + "Resolve transparent fragments")
+    def Transparency(self, frame, depth, settings=None, jitter=None, color=None, source=None, voxelizer=None, cone=None,
+                     download=True):
+        """Ray-casts the blended layers along the G-buffer pass's rays, lights them and composites them front to back over the
+        lit image, in place (DESIGN.md 8f.1h). depth: the opaque depth [H, W] (numpy array or CUDA tensor). The lit image is
+        `color` (rgba32f [H, W, 4] of the same kind, LIT_SOURCE_ARRAY: composited in place, a numpy array included) or the
+        last DeferredLighting image (LIT_SOURCE_DEFERRED: later DEFERRED reads see the composite). settings:
+        capi.IdkPtTransparencySettings (default: the engine's); IsVXGI traces `voxelizer` (a voxelised vxgi.Voxelizer on the
+        same device) with `cone` (vxgi.IdkVxConeSettings, default: the engine's). Returns the composited float32 [H, W, 4], or
+        None with download=False. Kernel ms in last_transparency_ms."""
+        st = settings if settings is not None else capi.default_transparency_settings()
+        src = self._lit_source(source, color)
+        g, keep, on_device = self._gbuffer([depth, None, None, None, None, color], [1, 2, 3, 2, 3, 4])
+        col = None if keep[5] is None else (keep[5].data_ptr() if on_device else keep[5].ctypes.data)
+        jit = None if jitter is None else np.ascontiguousarray(jitter, np.float32)
+        if jit is not None and jit.size != 2:
+            raise ValueError("Transparency: jitter has two components")
+        cn = None
+        if st.IsVXGI:
+            from . import vxgi
+            cn = cone if cone is not None else vxgi.default_cone_settings()
+        frame = np.ascontiguousarray(frame)
+        out = np.zeros((g.Height, g.Width, 4), np.float32) if download else None
+        ms = ctypes.c_float()
+        self._check(self._lib.idkpt_transparency(self._ctx, frame.ctypes.data, ctypes.byref(st), ctypes.byref(g),
+                                                 jit.ctypes.data if jit is not None else None,
+                                                 voxelizer._ctx if voxelizer is not None else None,
+                                                 ctypes.byref(cn) if cn is not None else None, src, col,
+                                                 out.ctypes.data if download else None, ctypes.byref(ms)), "idkpt_transparency")
+        self.last_transparency_ms = ms.value
+        if color is not None and keep[5] is not color:
+            if on_device:
+                color.copy_(keep[5])
+            else:
+                np.copyto(color, keep[5], casting="unsafe")
+        return out
+
     # ---- variable-rate deferred lighting (LightingShadingRateClassifier.Compute)
     def ShadingRate(self, frame, velocity_rg, settings=None, color=None, source=None, download=True, debug=False):
         """LightingShadingRateClassifier.Compute over render-size inputs: velocity [h, w, 2] and the lit image `color` (rgba32f

@@ -385,7 +385,8 @@ IDKPT_API int idkpt_deferred_device_ptr(IdkPtCtx* ctx, void** dev_ptr, uint64_t*
 /* ---- the end of the raster frame (RasterPipeline.Render: SSR.Compute, "Merge Textures", TaaResolve.Compute) ----
  * The lit image both calls read (`source`): IDKPT_LIT_SOURCE_ARRAY, a caller rgba32f [Height][Width] array (host or device as
  *   the call's OnDevice says; a host that keeps the light, skybox and transparency draws in GL passes its composited buffer);
- *   IDKPT_LIT_SOURCE_DEFERRED, the image of the last idkpt_deferred_lighting call; IDKPT_LIT_SOURCE_MERGED (TAA only), the
+ *   IDKPT_LIT_SOURCE_DEFERRED, the context's lit image as the last idkpt_deferred_lighting call left it, composited by any
+ *   idkpt_transparency since; IDKPT_LIT_SOURCE_MERGED (TAA only), the
  *   merged image of the last idkpt_ssr call. A context image must exist and have the render size.
  * idkpt_ssr: SSR/compute.glsl at the G-buffer size (reads Depth, NormalRG, AlbedoRGB and MetallicRoughness; EmissiveRGB may be
  *   NULL), then MergeTextures/compute.glsl: merged = source.rgb + SSR.rgb (alpha 1). The sky is the context's (idkpt_set_sky).
@@ -482,6 +483,34 @@ IDKPT_API int idkpt_gbuffer(IdkPtCtx* ctx, const GpuPerFrameData* frame, int32_t
 IDKPT_API int idkpt_gbuffer_device_ptrs(IdkPtCtx* ctx, IdkPtGBuffer* gbuffer_out, const float** velocity_rg_out);
 IDKPT_API int idkpt_read_gbuffer(IdkPtCtx* ctx, float* depth, float* normal_rg, float* albedo_rgb, float* metallic_roughness,
                                  float* emissive_rgb, float* velocity_rg);
+
+/* ---- transparency (RasterPipeline.Render: "Record transparent fragments" + "Resolve transparent fragments") ----
+ * idkpt_transparency: the blended surfaces (AlphaCutoff == 2) the G-buffer pass culls, ray-cast at pixel centres along
+ *   idkpt_gbuffer's rays and composited front to back over the lit image, in place. A fragment is kept where its material is
+ *   blended, it is front-facing or double-sided, its depth is in [0, 1] and below gbuffer->Depth, and its alpha is not 0;
+ *   per pixel the 10 (TRANSPARENT_LAYERS) with the smallest depth are kept, ties broken by BLAS triangle, then
+ *   MeshTransformId. Each is lit as the record shader lights it: every light through GGX with the surface's IOR, shadowed by
+ *   the PCF filter (ShadowMode 1; ShadowMode 2 leaves transparents unshadowed, as the engine does), plus VXGI indirect light
+ *   traced from `voxels` with the context's sky (IsVXGI) or 0.015 * albedo; premultiplied and rounded to rgba16f. The result
+ *   is acc.rgb of ResolveTransparent's blend with alpha 1; a pixel without a layer keeps its bytes. The rules are in DESIGN.md
+ *   8f.1h.
+ * gbuffer: Width, Height, OnDevice and Depth are read; the other attachments may be NULL. source: IDKPT_LIT_SOURCE_DEFERRED
+ *   composites the context's deferred image (later DEFERRED reads see it); IDKPT_LIT_SOURCE_ARRAY composites color_rgba32f
+ *   (host or device as OnDevice says; a host array is uploaded and downloaded back into itself); MERGED is rejected (the engine
+ *   resolves before SSR). out_rgba32f: an optional download of the result (Width*Height*4 floats). taa_jitter: NULL = (0, 0).
+ *   voxels / cone: IsVXGI only; the grid must be voxelised, on the context's device. Every argument is checked before anything
+ *   is uploaded or launched, so a failed call leaves the target unchanged. The call is synchronous and ordered after the
+ *   samples idkpt_compute has queued. */
+struct IdkVxCtx;
+struct IdkVxConeSettings;
+typedef struct IdkPtTransparencySettings { /* the record program's uniforms (RasterPipeline.cs:555-558) */
+    int32_t ShadowMode;                    /* 1: 0 None, 1 Pcf, 2 RayTraced (no shadow on transparents, as in the engine) */
+    int32_t IsVXGI;                        /* 0 */
+} IdkPtTransparencySettings;
+IDKPT_API int idkpt_transparency(IdkPtCtx* ctx, const GpuPerFrameData* frame, const IdkPtTransparencySettings* settings,
+                                 const IdkPtGBuffer* gbuffer, const float* taa_jitter, struct IdkVxCtx* voxels,
+                                 const struct IdkVxConeSettings* cone, int32_t source, float* color_rgba32f, float* out_rgba32f,
+                                 float* kernel_ms);
 
 /* ---- dynamic geometry (SURVEY.md 8f.2): ModelManager.Update = skin -> refit -> TLAS (ModelManager.cs:236-261) ----
  * idkpt_set_skinning_data: unskinnedVertexSSBO upload (52-byte GpuUnskinnedVertex records).

@@ -276,6 +276,16 @@ public:
     void ReadGBuffer(float* depth, float* normalRG, float* albedoRGB, float* metallicRoughness, float* emissiveRGB, float* velocityRG) {
         check(idkpt_read_gbuffer(ctx_, depth, normalRG, albedoRGB, metallicRoughness, emissiveRGB, velocityRG), "idkpt_read_gbuffer");
     }
+    // The blended layers composited over the lit image in place (DESIGN.md 8f.1h): the context's deferred image (source
+    // IDKPT_LIT_SOURCE_DEFERRED) or `color` (IDKPT_LIT_SOURCE_ARRAY); only gbuffer.Depth is read. voxels / cone: IsVXGI only.
+    // Returns the kernel time in ms.
+    float Transparency(const GpuPerFrameData& frame, const IdkPtTransparencySettings& settings, const IdkPtGBuffer& gbuffer,
+                       int32_t source, float* color = nullptr, const float* taaJitter = nullptr, IdkVxCtx* voxels = nullptr,
+                       const IdkVxConeSettings* cone = nullptr, float* outRgba32f = nullptr) {
+        float ms = 0.0f;
+        check(idkpt_transparency(ctx_, &frame, &settings, &gbuffer, taaJitter, voxels, cone, source, color, outRgba32f, &ms), "idkpt_transparency");
+        return ms;
+    }
     void SetSkinningData(const GpuUnskinnedVertex* vertices, uint64_t count) { check(idkpt_set_skinning_data(ctx_, vertices, count), "idkpt_set_skinning_data"); }
     void SkinVertices(const float* jointMatrices3x4, uint64_t jointCount, const IdkPtSkinningCmd* cmds, uint32_t cmdCount) {
         check(idkpt_skin_vertices(ctx_, jointMatrices3x4, jointCount, cmds, cmdCount, nullptr), "idkpt_skin_vertices");

@@ -210,3 +210,22 @@ for use_tlas in (False, True):
             pt.Ssao(fg, d, n, download=False)
             pt.DeferredLighting(fg, d, n, a, mr, e, settings=capi.IdkPtDeferredSettings(0, 1, 0, 0), download=False)
 print("g-buffer pass ok")
+
+# transparency: the textured room's blended card through the instance loop and the TLAS walk, odd sizes, every ShadowMode,
+# IsVXGI, host and device arrays and the deferred image
+with vxgi.Voxelizer(16, (-3.0, -1.0, -3.0), (3.0, 3.0, 3.0)) as tvx:
+    tvx.SetScene(scene); tvx.Render()
+    for use_tlas in (False, True):
+        scene.build_tlas(use=use_tlas)
+        with PathTracer(16, 16) as pt:
+            pt.SetScene(scene)
+            for gw, gh in ((37, 23), (1, 1), (96, 64)):
+                fg = scenes.camera_frame(cam, gw, gh)
+                pt.GBuffer(fg, gw, gh, jitter=(0.01, -0.02))
+                d, n, a, mr, e, v = pt.GBufferDevicePtrs(tensors=True)
+                pt.DeferredLighting(fg, d, n, a, mr, e, settings=capi.IdkPtDeferredSettings(0, 0, 0, 0), download=False)
+                for mode in (0, 2):
+                    pt.Transparency(fg, d, settings=capi.IdkPtTransparencySettings(mode, 0), source=capi.LIT_SOURCE_DEFERRED, download=False)
+                pt.Transparency(fg, d, settings=capi.IdkPtTransparencySettings(0, 1), source=capi.LIT_SOURCE_DEFERRED, voxelizer=tvx)
+                pt.Transparency(fg, d.cpu().numpy(), settings=capi.IdkPtTransparencySettings(0, 0), color=np.ones((gh, gw, 4), np.float32))
+print("transparency ok")
