@@ -101,7 +101,7 @@ EXPORTS = [
     "idkpt_ssao", "idkpt_ssao_device_ptr", "idkpt_deferred_lighting", "idkpt_deferred_device_ptr",
     "idkpt_ssr", "idkpt_ssr_device_ptrs", "idkpt_taa_resolve", "idkpt_taa_device_ptr",
     "idkpt_shading_rate", "idkpt_shading_rate_device_ptr",
-    "idkpt_gbuffer", "idkpt_gbuffer_device_ptrs", "idkpt_read_gbuffer", "idkpt_transparency",
+    "idkpt_gbuffer", "idkpt_gbuffer_device_ptrs", "idkpt_read_gbuffer", "idkpt_transparency", "idkpt_lights_and_skybox",
 ]
 
 IDKPT_MAX_POINT_SHADOWS = 128
@@ -438,6 +438,8 @@ def load(path=None):
     L.idkpt_transparency.argtypes = [c_vp, c_vp, P(IdkPtTransparencySettings), P(IdkPtGBuffer), c_vp, c_vp, c_vp, c_i32, c_vp, c_vp, P(c_f)]
     L.idkpt_read_gbuffer.restype = c_i32
     L.idkpt_read_gbuffer.argtypes = [c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp]
+    L.idkpt_lights_and_skybox.restype = c_i32
+    L.idkpt_lights_and_skybox.argtypes = [c_vp, c_vp, c_vp, c_vp, P(c_f)]
     L.idkpt_abi_version.restype = c_u32
     L.idkpt_abi_version.argtypes = []
     if path == _build.LIBIDKPT:

@@ -24,13 +24,14 @@
 #include "idk_vrs.cuh"
 #include "idk_gbuffer.cuh"
 #include "idk_transparency.cuh"
+#include "idk_lights_skybox.cuh"
 #include "idk_textures_host.h"
 
 #define IDKPT_ABI_VERSION 4u   // 2: IdkPtSceneDesc gained Textures / TextureCount; 3: IdkPtStats gained CompactMs / AccumulateMs, host-buffer registration;
                                // 4: gather handle blob is 5 IPC handles (320 bytes), IDKPT_CREATE_GLOBAL_SLOTS, idkpt_gather_connect.
                                // Entry points added since (point-shadow cube maps, idkvx_set_shadow_maps, volumetric lighting, SSAO
                                // and deferred lighting, SSR and the TAA resolve, the shading-rate classifier, the G-buffer pass,
-                               // transparency) are
+                               // transparency, the light spheres and the skybox) are
                                // additive and keep 4;
                                // IdkPtDeferredSettings grew a trailing IsVariableRateShading.
 
@@ -560,6 +561,17 @@ static void gather_teardown(IdkPtCtx* ctx) {
     ctx->gatherEpoch = 0;
 }
 
+// The light spheres' mesh (k_lights_skybox's constant tables) on the context's device. Every context writes the same bytes.
+static int upload_sphere_mesh(IdkPtCtx* ctx) {
+    float3 vertices[IDK_SPHERE_VERTICES];
+    uint32_t triangles[IDK_SPHERE_TRIANGLES];
+    sphere_mesh_tables(vertices, triangles);
+    CK(cudaMemcpyToSymbolAsync(c_sphere_vertices, vertices, sizeof(vertices), 0, cudaMemcpyHostToDevice, ctx->stream));
+    CK(cudaMemcpyToSymbolAsync(c_sphere_triangles, triangles, sizeof(triangles), 0, cudaMemcpyHostToDevice, ctx->stream));
+    CK(cudaStreamSynchronize(ctx->stream));
+    return IDKPT_OK;
+}
+
 extern "C" {
 
 IDKPT_API uint32_t idkpt_abi_version(void) { return IDKPT_ABI_VERSION; }
@@ -609,6 +621,7 @@ IDKPT_API int idkpt_create(const IdkPtCreateInfo* ci, IdkPtCtx** out) {
     compute_tile_rows(ctx);
     int rc = create_stream(ctx);
     if (rc == IDKPT_OK) rc = allocate_wavefront(ctx);
+    if (rc == IDKPT_OK) rc = upload_sphere_mesh(ctx);
     if (rc != IDKPT_OK) {
         IdkPtCtx::createError = ctx->lastError;
         idkpt_destroy(ctx);
@@ -1375,7 +1388,7 @@ static int preload_kernels(IdkPtCtx* ctx) {
     IDK_PRELOAD(k_bcn_decode); IDK_PRELOAD(k_point_shadow_faces); IDK_PRELOAD(k_volumetric_march); IDK_PRELOAD(k_volumetric_upscale);
     IDK_PRELOAD(k_ssao); IDK_PRELOAD(k_deferred_lighting); IDK_PRELOAD(k_ssr); IDK_PRELOAD(k_taa_resolve);
     IDK_PRELOAD(k_shading_rate); IDK_PRELOAD(k_vrs_scan); IDK_PRELOAD(k_deferred_lighting_vrs); IDK_PRELOAD(k_gbuffer);
-    IDK_PRELOAD(k_transparency<false>); IDK_PRELOAD(k_transparency<true>);
+    IDK_PRELOAD(k_transparency<false>); IDK_PRELOAD(k_transparency<true>); IDK_PRELOAD(k_lights_skybox);
 #undef IDK_PRELOAD
     return IDKPT_OK;
 }
@@ -2622,6 +2635,46 @@ IDKPT_API int idkpt_transparency(IdkPtCtx* ctx, const GpuPerFrameData* frame, co
     if (outRgba32f) CK(cudaMemcpyAsync(outRgba32f, target, n * 16, cudaMemcpyDeviceToHost, ctx->stream));
     if (hostArray || outRgba32f) CK(cudaStreamSynchronize(ctx->stream));
     return IDKPT_OK;
+}
+
+// ---- the light spheres and the skybox (RasterPipeline.Render's "Draw lights" + "Draw skybox") ---------------------------------
+IDKPT_API int idkpt_lights_and_skybox(IdkPtCtx* ctx, const GpuPerFrameData* frame, const float* taaJitter, float* outRgba32f,
+                                      float* kernelMs) {
+    static const char* who = "idkpt_lights_and_skybox";
+    if (!ctx || !frame) return fail(ctx, IDKPT_ERR_INVALID_ARGUMENT, "idkpt_lights_and_skybox: null argument");
+    if (!ctx->haveScene) return fail(ctx, IDKPT_ERR_NO_SCENE, "idkpt_lights_and_skybox: no scene");
+    if (!ctx->gbW) return fail(ctx, who, IDKPT_ERR_INVALID_ARGUMENT, "call idkpt_gbuffer first");
+    if (ctx->deferredW != ctx->gbW || ctx->deferredH != ctx->gbH)
+        return fail(ctx, who, IDKPT_ERR_INVALID_ARGUMENT, "needs an idkpt_deferred_lighting image of the G-buffer's size");
+    if (taaJitter && (!std::isfinite(taaJitter[0]) || !std::isfinite(taaJitter[1])))
+        return fail(ctx, who, IDKPT_ERR_INVALID_ARGUMENT, "jitter not finite");
+    CK(cudaSetDevice(ctx->device));
+    if (kernelMs) *kernelMs = 0.0f;
+    const int w = ctx->gbW, h = ctx->gbH;
+    size_t off[6];
+    gbuffer_planes(w, h, off);
+    char* base = (char*)ctx->gbImages.p;
+    LightsSkyboxArgs a;
+    a.sc = ctx->sc;
+    a.lights = ctx->sc.lights; a.lightCount = (int)ctx->counts.LightCount;
+    memcpy(a.projView, frame->ProjView, sizeof(a.projView));
+    memcpy(a.prevProjView, frame->PrevProjView, sizeof(a.prevProjView));
+    memcpy(a.invProjView, frame->InvProjView, sizeof(a.invProjView));
+    memcpy(a.projection, frame->Projection, sizeof(a.projection));
+    memcpy(a.invProjection, frame->InvProjection, sizeof(a.invProjection));
+    memcpy(a.invView, frame->InvView, sizeof(a.invView));
+    memcpy(a.prevView, frame->PrevView, sizeof(a.prevView));
+    for (int k = 0; k < 3; k++) a.viewPos[k] = frame->ViewPos[k];
+    a.jitter[0] = taaJitter ? taaJitter[0] : 0.0f; a.jitter[1] = taaJitter ? taaJitter[1] : 0.0f;
+    a.w = w; a.h = h;
+    a.depth = (float*)(base + off[0]); a.normalRG = (float2*)(base + off[1]); a.emissive = (float*)(base + off[4]);
+    a.velocity = (float2*)(base + off[5]);
+    a.color = (float4*)ctx->deferredOut.p;
+    const size_t n = (size_t)w * h, tiles = (size_t)((w + 7) / 8) * (size_t)((h + 7) / 8);
+    return run_timed(ctx, who, kernelMs, [&]() -> int {
+        k_lights_skybox<<<(unsigned)((tiles + 3) / 4), 256, 0, ctx->stream>>>(a);
+        return IDKPT_OK;
+    }, outRgba32f, ctx->deferredOut.p, outRgba32f ? n * 16 : 0);
 }
 
 } // extern "C"

@@ -540,6 +540,27 @@ class PathTracer:
                 np.copyto(color, keep[5], casting="unsafe")
         return out
 
+    # ---- the light spheres and the skybox (RasterPipeline.Render's "Draw lights" + "Draw skybox")
+    def LightsAndSkybox(self, frame, jitter=None, download=True):
+        """Draws the light spheres and the skybox into the images of the last GBuffer call and the last DeferredLighting image
+        (which must have the G-buffer's size), in place (DESIGN.md 8f.1i): later DEFERRED reads, GBufferDevicePtrs and
+        GBuffer downloads see them. jitter: taaDataUBO.Jitter in NDC units (None = 0). Returns the lit image, float32 [H, W, 4],
+        or None with download=False. Kernel ms in last_lights_and_skybox_ms."""
+        jit = None if jitter is None else np.ascontiguousarray(jitter, np.float32)
+        if jit is not None and jit.size != 2:
+            raise ValueError("LightsAndSkybox: jitter has two components")
+        frame = np.ascontiguousarray(frame)
+        out = None
+        if download:
+            g, _ = self.GBufferDevicePtrs()
+            out = np.zeros((g.Height, g.Width, 4), np.float32)
+        ms = ctypes.c_float()
+        self._check(self._lib.idkpt_lights_and_skybox(self._ctx, frame.ctypes.data, jit.ctypes.data if jit is not None else None,
+                                                      out.ctypes.data if download else None, ctypes.byref(ms)),
+                    "idkpt_lights_and_skybox")
+        self.last_lights_and_skybox_ms = ms.value
+        return out
+
     # ---- variable-rate deferred lighting (LightingShadingRateClassifier.Compute)
     def ShadingRate(self, frame, velocity_rg, settings=None, color=None, source=None, download=True, debug=False):
         """LightingShadingRateClassifier.Compute over render-size inputs: velocity [h, w, 2] and the lit image `color` (rgba32f

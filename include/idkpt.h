@@ -471,7 +471,8 @@ IDKPT_API int idkpt_shading_rate_device_ptr(IdkPtCtx* ctx, void** dev_ptr, uint6
  *   RG16F velocity, D32F depth); pixels without a surface hold the clears (depth 1, everything else 0). The rules are in
  *   DESIGN.md 8f.1g. taa_jitter: taaDataUBO.Jitter in NDC units, NULL = (0, 0). prev_positions: the previous frame's vertex
  *   positions (prevVertexPositionSSBO, VertexPositionCount entries), NULL = this frame's (static geometry); idkpt_skin_vertices
- *   keeps no copy, so a host that animates passes them. Lights and the skybox are separate draws and are not rendered.
+ *   keeps no copy, so a host that animates passes them. Lights and the skybox are separate draws: idkpt_lights_and_skybox
+ *   draws them into these images afterwards.
  * idkpt_gbuffer_device_ptrs: the images of the last successful call: an IdkPtGBuffer with OnDevice = 1 that idkpt_ssao,
  *   idkpt_deferred_lighting and idkpt_ssr take as it is, and the velocity for IdkPtTaaInputs / IdkPtShadingRateInputs.
  *   Either output may be NULL.
@@ -511,6 +512,24 @@ IDKPT_API int idkpt_transparency(IdkPtCtx* ctx, const GpuPerFrameData* frame, co
                                  const IdkPtGBuffer* gbuffer, const float* taa_jitter, struct IdkVxCtx* voxels,
                                  const struct IdkVxConeSettings* cone, int32_t source, float* color_rgba32f, float* out_rgba32f,
                                  float* kernel_ms);
+
+/* ---- the light spheres and the skybox (RasterPipeline.Render: "Draw lights" + "Draw skybox") ----
+ * idkpt_lights_and_skybox: the two draws the engine runs between deferred lighting and transparency, ray-cast at pixel centres
+ *   along idkpt_gbuffer's rays and written in place into the context's images: the G-buffer of the last successful
+ *   idkpt_gbuffer (Depth, NormalRG, EmissiveRGB, VelocityRG) and the deferred image of idkpt_deferred_lighting, which must have
+ *   the G-buffer's size. So later DEFERRED reads, idkpt_gbuffer_device_ptrs and idkpt_read_gbuffer see the result.
+ *   Lights: each scene light is LightManager's 12 x 12 sphere mesh scaled by Radius at Position, depth-tested LESS against the
+ *   G-buffer depth with back faces culled; the nearest fragment wins, ties keep the first in draw order (light, then triangle).
+ *   It writes the light's Color to the lit image (alpha 1) and to EmissiveRGB, the encoded sphere normal, the velocity
+ *   against PrevPosition and PrevProjView, and its depth. A camera inside a sphere sees none of it.
+ *   Skybox: every pixel whose depth is still 1 gets the context's sky (idkpt_set_sky) seen through the unjittered pixel
+ *   centre (alpha 1) and the rotation-only velocity between View and PrevView; its depth stays 1.
+ *   AlbedoRGB and MetallicRoughness are never written. The rules are in DESIGN.md 8f.1i.
+ * taa_jitter: NULL = (0, 0). out_rgba32f: an optional download of the lit image (Width*Height*4 floats). Every argument is
+ * checked before anything is launched, so a failed call changes no byte. A second call with the same arguments changes nothing.
+ * The call is synchronous and ordered after the samples idkpt_compute has queued. */
+IDKPT_API int idkpt_lights_and_skybox(IdkPtCtx* ctx, const GpuPerFrameData* frame, const float* taa_jitter, float* out_rgba32f,
+                                      float* kernel_ms);
 
 /* ---- dynamic geometry (SURVEY.md 8f.2): ModelManager.Update = skin -> refit -> TLAS (ModelManager.cs:236-261) ----
  * idkpt_set_skinning_data: unskinnedVertexSSBO upload (52-byte GpuUnskinnedVertex records).

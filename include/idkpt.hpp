@@ -286,6 +286,13 @@ public:
         check(idkpt_transparency(ctx_, &frame, &settings, &gbuffer, taaJitter, voxels, cone, source, color, outRgba32f, &ms), "idkpt_transparency");
         return ms;
     }
+    // The light spheres and the skybox, in place into the last GBuffer's images and the deferred image (DESIGN.md 8f.1i);
+    // taaJitter and outRgba32f may be nullptr. Returns the kernel time in ms.
+    float LightsAndSkybox(const GpuPerFrameData& frame, const float* taaJitter = nullptr, float* outRgba32f = nullptr) {
+        float ms = 0.0f;
+        check(idkpt_lights_and_skybox(ctx_, &frame, taaJitter, outRgba32f, &ms), "idkpt_lights_and_skybox");
+        return ms;
+    }
     void SetSkinningData(const GpuUnskinnedVertex* vertices, uint64_t count) { check(idkpt_set_skinning_data(ctx_, vertices, count), "idkpt_set_skinning_data"); }
     void SkinVertices(const float* jointMatrices3x4, uint64_t jointCount, const IdkPtSkinningCmd* cmds, uint32_t cmdCount) {
         check(idkpt_skin_vertices(ctx_, jointMatrices3x4, jointCount, cmds, cmdCount, nullptr), "idkpt_skin_vertices");

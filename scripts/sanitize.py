@@ -229,3 +229,19 @@ with vxgi.Voxelizer(16, (-3.0, -1.0, -3.0), (3.0, 3.0, 3.0)) as tvx:
                 pt.Transparency(fg, d, settings=capi.IdkPtTransparencySettings(0, 1), source=capi.LIT_SOURCE_DEFERRED, voxelizer=tvx)
                 pt.Transparency(fg, d.cpu().numpy(), settings=capi.IdkPtTransparencySettings(0, 0), color=np.ones((gh, gw, 4), np.float32))
 print("transparency ok")
+
+# the light spheres and the skybox: the textured room with its lights, a light in front of the camera and a cube-map sky, odd
+# sizes and jitter, in place into the G-buffer and the deferred image
+lit_scene = scenes.textured_room(threads=1)[0]
+eye, vd = np.asarray(cam["position"], np.float64), np.asarray(cam["view_dir"], np.float64)
+lit_scene.add_light(tuple(eye + vd / np.linalg.norm(vd) * 0.5), (40.0, 50.0, 60.0), 0.3)
+with PathTracer(16, 16) as pt:
+    pt.SetScene(lit_scene)
+    pt.SetSky(np.random.default_rng(2).random((6, 5, 5, 4), dtype=np.float32))
+    for gw, gh in ((37, 23), (1, 1), (96, 64)):
+        fg = scenes.camera_frame(cam, gw, gh)
+        pt.GBuffer(fg, gw, gh, jitter=(0.01, -0.02), download=False)
+        d, n, a, mr, e, v = pt.GBufferDevicePtrs(tensors=True)
+        pt.DeferredLighting(fg, d, n, a, mr, e, settings=capi.IdkPtDeferredSettings(0, 0, 0, 0), download=False)
+        pt.LightsAndSkybox(fg, jitter=(0.01, -0.02))
+print("lights and skybox ok")
