@@ -207,9 +207,36 @@ def _vx_declare():
     L.oracle_vx_voxelize.argtypes = [P(capi.IdkPtSceneDesc), P(vxgi.IdkVxCreateInfo), vp, u64, P(u64), i32]
     L.oracle_vx_cone_trace.restype = i32
     L.oracle_vx_cone_trace.argtypes = [P(vxgi.IdkVxCreateInfo), vp, vp, P(vxgi.IdkVxConeSettings), vp, vp, vp, i32, i32, vp, vp, P(u64), i32]
+    L.oracle_vx_mipmap.restype = i32
+    L.oracle_vx_mipmap.argtypes = [P(vxgi.IdkVxCreateInfo), vp, i32]
     L.oracle_half_roundtrip.argtypes = [vp, u64, vp, vp]
     L.oracle_det_log2.argtypes = [vp, u64, vp]
     return L
+
+
+def _vx_split(raw, sizes):
+    levels, off = [], 0
+    for (w, h, dd) in sizes:
+        k = w * h * dd * 4
+        levels.append(raw[off:off + k].view(np.float16).reshape(dd, h, w, 4))
+        off += k
+    return levels
+
+
+def vx_mipmap(ci, level0, threads=None):
+    """Levels 1 .. n-1 of the mip chain built from a caller-supplied level 0 (float16 [d, h, w, 4]).
+    Returns (list of float16 [d, h, w, 4] arrays per level, concatenated raw uint16 chain)."""
+    from idkengine_b200 import vxgi
+    L = _vx_declare()
+    sizes = vxgi.level_sizes(ci)
+    w, h, d = sizes[0]
+    level0 = np.ascontiguousarray(level0, np.float16)
+    assert level0.shape == (d, h, w, 4), level0.shape
+    raw = np.zeros(sum(a * b * c for a, b, c in sizes) * 4, np.uint16)
+    raw[:level0.size] = level0.reshape(-1).view(np.uint16)
+    n = L.oracle_vx_mipmap(ctypes.byref(ci), raw.ctypes.data, threads or default_threads())
+    assert n == len(sizes), n
+    return _vx_split(raw, sizes), raw
 
 
 def vx_voxelize(scene, ci, threads=None, raster_rule=0):
@@ -231,12 +258,7 @@ def vx_voxelize(scene, ci, threads=None, raster_rule=0):
     finally:
         L.oracle_vx_set_raster_rule(0)
     assert n == len(sizes), n
-    levels, off = [], 0
-    for (w, h, dd) in sizes:
-        k = w * h * dd * 4
-        levels.append(raw[off:off + k].view(np.float16).reshape(dd, h, w, 4))
-        off += k
-    return levels, raw, frags.value
+    return _vx_split(raw, sizes), raw, frags.value
 
 
 def vx_cone_trace(ci, raw_chain, frame, settings, depth, normal_rg, metal_rough, sky=(0.6, 0.7, 0.9), threads=None):
