@@ -3,15 +3,16 @@
 //
 //   k_prepare_triangles/vertices/surfaces  scene upload: 64-byte triangle records, decoded vertex frames, per-mesh surfaces
 //   k_init_sample        per sample: zero alive counts and work tickets
-//   k_raygen             FirstHit/compute.glsl:44-81   ray generation (camera, jitter, thin lens)
-//   k_traverse           BVHIntersect.glsl:27-105,183-291  closest hit, one ray per lane (primary rays, TLAS walk): trace_ray<STATS, false>
-//   k_traverse2          same per-ray operation sequence, warp-level SETUP/BOX/LEAF phase scheduling with lane refill
-//   k_shade              FirstHit/compute.glsl:100-234, NHit/compute.glsl:91-215 (barrier-free, state in place)
+//   k_first_hit          bounce 0 in registers: FirstHit/compute.glsl:44-81 ray generation (camera, jitter, thin lens), the closest
+//                        hit (BVHIntersect.glsl:27-105,183-291, trace_ray<STATS, false>, one ray per lane) and FirstHit:100-234 shading
+//   k_traverse2          same per-ray operation sequence, warp-level SETUP/BOX/LEAF phase scheduling with lane refill (bounces >= 1)
+//   k_shade              NHit/compute.glsl:91-215 (barrier-free, state in place); shade_ray is the per-ray body both shaders share
 //   k_compact            the ordered (canonical) outcome of the alive-list atomics, decoupled look-back scan
 //   k_accumulate         FinalDraw/compute.glsl:24-62; k_accumulate_scatter: fused with the NVLink peer gather
 //   k_trace_rays         stand-alone closest-hit batch (BVH.Intersect analogue): trace_ray<true, false>
 #pragma once
 #include "idk_device.cuh"
+#include "idk_reorder.h"
 #include "../../include/idk_gpu_types.h"
 
 #define IDK_BLOCK 256
@@ -227,7 +228,10 @@ __device__ __forceinline__ bool trace_instance(const DeviceScene& sc, uint32_t i
 
 // TraceRay / TraceRayAny (BVHIntersect.glsl:183-291,299-411): lights, then the instance loop (default) or the TLAS walk.
 // Returns what the reference returns: closest hit, hit.t != tMax; any hit, whether a light or triangle was accepted.
-template <bool STATS, bool ANY, class Accept = AcceptAll>
+// TLAS picks the top level: TLAS_RUNTIME follows sc.useTlas; a kernel instantiated per scene kind passes TLAS_ON or TLAS_OFF,
+// and its instance-loop build then carries no TLAS stack.
+enum TlasMode { TLAS_OFF = 0, TLAS_ON = 1, TLAS_RUNTIME = 2 };
+template <bool STATS, bool ANY, class Accept = AcceptAll, int TLAS = TLAS_RUNTIME>
 __device__ __forceinline__ bool trace_ray(const DeviceScene& sc, f3 o, f3 d, float tMax, bool traceLights,
                                           uint32_t* stack, HitRec& hit, uint32_t& hitXform, uint32_t& S, uint32_t& T, uint32_t& I, float& cost,
                                           const Accept& accept = Accept()) {
@@ -250,7 +254,7 @@ __device__ __forceinline__ bool trace_ray(const DeviceScene& sc, f3 o, f3 d, flo
         }
     }
 
-    if (sc.useTlas) {
+    if (TLAS == TLAS_ON || (TLAS == TLAS_RUNTIME && sc.useTlas)) {
         const f3 inv = mk3(1.0f / d.x, 1.0f / d.y, 1.0f / d.z);
         uint32_t tstack[IDK_TLAS_STACK_SIZE];
         uint32_t sp = 0, top = 0;
@@ -305,57 +309,6 @@ struct TraverseArgs {
     int traceLights;
     int bounce;
 };
-
-// Persistent warps: every warp repeatedly claims 32 consecutive slots of the alive list.
-template <bool STATS>
-__global__ void __launch_bounds__(IDK_BLOCK) k_traverse(TraverseArgs a) {
-    extern __shared__ uint32_t s_stack[];
-    uint32_t* stack = s_stack + threadIdx.x;
-    const uint32_t lane = threadIdx.x & 31;
-    const uint32_t count = *a.count;
-    uint32_t S = 0, T = 0, I = 0, H = 0;
-    for (;;) {
-        uint32_t base = 0;
-        if (lane == 0) base = atomicAdd(a.ticket, 32u);
-        base = __shfl_sync(0xffffffffu, base, 0);
-        if (base >= count) break;
-        const uint32_t gid = base + lane;
-        if (gid < count) {
-            const uint32_t src = a.perm ? a.perm[gid] : gid;
-            const float4* sp = reinterpret_cast<const float4*>(a.state + src);
-            const float4 s0 = sp[0], s1 = sp[1];
-            const f3 o = mk3(s0.x, s0.y, s0.z);
-            const f3 d = decode_unit_vec(s1.x, s1.y);
-            HitRec hit;
-            uint32_t xf;
-            float cost = 0.0f;
-            const uint32_t stepsBefore = S;
-            trace_ray<STATS, false>(a.sc, o, d, IDK_FLOAT_MAX, a.traceLights != 0, stack, hit, xf, S, T, I, cost);
-            if (STATS) atomicMax(&a.counters->maxSteps[a.bounce & 63], S - stepsBefore);
-            reinterpret_cast<float4*>(a.hits)[gid] = make_float4(hit.bx, hit.by, hit.t, __uint_as_float(hit.tri));
-            a.hitXform[gid] = xf;
-            if (STATS) {
-                a.debugCost[gid] = cost;
-                if (hit.tri != ~0u) H++;
-            }
-        }
-    }
-    if (STATS) {
-        for (int off = 16; off > 0; off >>= 1) {
-            S += __shfl_down_sync(0xffffffffu, S, off);
-            T += __shfl_down_sync(0xffffffffu, T, off);
-            I += __shfl_down_sync(0xffffffffu, I, off);
-            H += __shfl_down_sync(0xffffffffu, H, off);
-        }
-        if (lane == 0) {
-            atomicAdd(&a.counters->steps, (unsigned long long)S);
-            atomicAdd(&a.counters->tris, (unsigned long long)T);
-            atomicAdd(&a.counters->instances, (unsigned long long)I);
-            atomicAdd(&a.counters->hits, (unsigned long long)H);
-        }
-    }
-}
-
 
 // ------------------------------------------------------------------------------------------------
 // k_traverse2: the production traversal kernel. Same per-ray operation sequence as trace_ray<STATS, false> (hence the
@@ -674,33 +627,20 @@ struct FrameParams {
     int doDebugTraversal, doTraceLights, doRussianRoulette;
 };
 
-__device__ __forceinline__ bool tile_owns_row(const FrameParams& f, int y, int& localRow) {
-    const int stripe = y / f.stripeH;
-    if (f.tileCount > 1 && (stripe % f.tileCount) != f.tileIndex) return false;
-    localRow = (f.tileCount > 1 ? (stripe / f.tileCount) : stripe) * f.stripeH + (y % f.stripeH);
-    return true;
+// The image row of tile row `localRow`: the tile owns the stripes of stripeH rows whose index is tileIndex modulo tileCount and
+// stores them compactly, in image order.
+__device__ __forceinline__ int tile_row_y(const FrameParams& f, int localRow) {
+    const int localStripe = localRow / f.stripeH;
+    const int stripe = f.tileCount > 1 ? localStripe * f.tileCount + f.tileIndex : localStripe;
+    return stripe * f.stripeH + localRow % f.stripeH;
 }
 
-// One thread per (un-swizzled) invocation of the reference's 8x8 FirstHit dispatch.
-__global__ void __launch_bounds__(64) k_raygen(FrameParams f, PathState* __restrict__ state) {
-    // ReorderInvocations(20), FirstHit/compute.glsl:236-262
-    const uint32_t n = 20;
-    const uint32_t idx = blockIdx.y * gridDim.x + blockIdx.x;
-    const uint32_t columnSize = gridDim.y * n;
-    const uint32_t fullColumnCount = gridDim.x / n;
-    const uint32_t lastColumnWidth = gridDim.x % n;
-    const uint32_t columnIdx = idx / columnSize;
-    const uint32_t idxInColumn = idx % columnSize;
-    uint32_t columnWidth = n;
-    if (columnIdx == fullColumnCount) columnWidth = lastColumnWidth;
-    const uint32_t swy = idxInColumn / columnWidth;
-    const uint32_t swx = idxInColumn % columnWidth + columnIdx * n;
-    const int x = (int)(swx * 8 + threadIdx.x), y = (int)(swy * 8 + threadIdx.y);
-    if (x >= f.width || y >= f.height) return;
-    int localRow;
-    if (!tile_owns_row(f, y, localRow)) return;
-
-    const uint32_t gidX = blockIdx.x * 8 + threadIdx.x, gidY = blockIdx.y * 8 + threadIdx.y;
+// FirstHit/compute.glsl:44-81: the camera ray of pixel (x, y), tile pixel li, as the path state FirstHit starts from. The
+// invocation that the reference's 8x8 dispatch gives this pixel after ReorderInvocations(20) fixes `reseed`.
+__device__ __forceinline__ PathState camera_ray(const FrameParams& f, int x, int y, uint32_t li) {
+    uint32_t bx, by;
+    reorder_invocations_inverse((uint32_t)(f.width + 7) / 8u, (uint32_t)(f.height + 7) / 8u, (uint32_t)x / 8u, (uint32_t)y / 8u, bx, by);
+    const uint32_t gidX = bx * 8 + (uint32_t)x % 8u, gidY = by * 8 + (uint32_t)y % 8u;
     uint32_t seed = (uint32_t)(y * 4096 + x) * (f.accumulatedSamples + 1u);
     const float sx = rnd01(seed), sy = rnd01(seed);
     const float ndcx = ((float)x + sx) / (float)f.width * 2.0f - 1.0f;
@@ -714,14 +654,13 @@ __global__ void __launch_bounds__(64) k_raygen(FrameParams f, PathState* __restr
     const f3 pointOnLense = mat4_mul_xyz(f.invView, f.lenseRadius * dx, f.lenseRadius * dy, 0.0f, 1.0f);
     camDir = normalize3(focalPoint - pointOnLense);
 
-    float pdx, pdy;
-    encode_unit_vec(camDir, pdx, pdy);
-    const uint32_t li = (uint32_t)localRow * (uint32_t)f.width + (uint32_t)x;
-    float4* out = reinterpret_cast<float4*>(state + li);
-    out[0] = make_float4(pointOnLense.x, pointOnLense.y, pointOnLense.z, 1.0f);
-    out[1] = make_float4(pdx, pdy, __uint_as_float(li), __uint_as_float(gidY * 4096u + gidX));
-    out[2] = make_float4(1.0f, 1.0f, 1.0f, __uint_as_float(seed));
-    out[3] = make_float4(0.0f, 0.0f, 0.0f, 0.0f);
+    PathState st;
+    st.ox = pointOnLense.x; st.oy = pointOnLense.y; st.oz = pointOnLense.z; st.prevIor = 1.0f;
+    encode_unit_vec(camDir, st.pdx, st.pdy);
+    st.pix = li; st.reseed = gidY * 4096u + gidX;
+    st.tx = 1.0f; st.ty = 1.0f; st.tz = 1.0f; st.rng = seed;
+    st.rx = 0.0f; st.ry = 0.0f; st.rz = 0.0f; st.pad = 0;
+    return st;
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -872,10 +811,9 @@ struct ShadeArgs {
     FrameParams f;
     PathState* state;              // pixel-indexed, updated in place (the reference's Rays[rayIndex], SSBO 30)
     float4* aov;                   // 2 x float4 per pixel, in place (SSBO 31), AOVs only
-    const uint32_t* alive;         // alive list of this bounce: slot -> tile pixel; null = identity (first hit)
+    const uint32_t* alive;         // alive list of this bounce: slot -> tile pixel
     const HitRec* hits;            // by slot
     const uint32_t* hitXform;
-    const float* debugCost;        // by slot (debug traversal only)
     const uint32_t* count;         // alive count in
     uint32_t* survivors;           // by slot: tile pixel of a surviving ray, ~0u otherwise (input of k_compact)
     uint32_t* keysTmp;             // by slot: sort key of a surviving ray (ray sorting only), may be null
@@ -885,7 +823,6 @@ struct ShadeArgs {
     const uint32_t* slotDelta;     // multi-GPU global slots (k_slot_exchange): per local stripe, global slot - local slot; null = local slots
     uint32_t stripePixels;         // pixels per stripe (stripe height x width)
     int exportState;               // debug export: terminated paths also write their final state back
-    int firstHit;
     int lastBounce;                // survivors are final: no compaction
     int outputAovs;
 };
@@ -899,263 +836,326 @@ __device__ __forceinline__ unsigned long long pack_status(uint32_t epoch, uint32
 }
 __device__ __forceinline__ uint32_t status_epoch(unsigned long long sv) { return (uint32_t)(sv >> 34) & IDK_EPOCH_MASK; }
 
-// One thread per alive ray, no block-level cooperation: every warp runs at its own pace (the ordered compaction of
+// The per-ray body of FirstHit (FIRST, FirstHit/compute.glsl:100-234) and NHit (NHit/compute.glsl:91-215): shade the hit of the
+// path in `st` (slot `gid` of this bounce, tile pixel `src`) and write what the bounce leaves behind: the state of a survivor
+// (in place), the radiance and AOVs of a finished path, survivors[gid] and its sort key. FirstHit takes its random numbers from
+// the camera ray's state, NHit from the ray's slot. debugCost: the primary ray's traversal cost (FirstHit, debug view only).
+template <bool TEX, bool FIRST>
+__device__ __forceinline__ void shade_ray(const ShadeArgs& a, uint32_t gid, uint32_t src, PathState st, const HitRec& hit, uint32_t hitXf,
+                                          float debugCost) {
+    const DeviceScene& sc = a.sc;
+    const FrameParams& f = a.f;
+    bool survive = false;
+    float4 aov0 = make_float4(0.0f, 0.0f, 0.0f, 1.0f), aov1 = make_float4(0.0f, 0.0f, 0.0f, 0.0f);
+    uint32_t sortingKey = 0;
+    if (a.outputAovs && !FIRST) { aov0 = a.aov[2 * (size_t)src]; aov1 = a.aov[2 * (size_t)src + 1]; }
+    // NHit's gl_GlobalInvocationID.x is the ray's slot in the alive list of the WHOLE image; a stripe tile adds the number of
+    // alive rays in the other ranks' stripes above it (k_slot_exchange), so that N GPUs draw the 1-GPU random numbers
+    const uint32_t slot = (a.slotDelta && !FIRST) ? gid + a.slotDelta[src / a.stripePixels] : gid;
+    uint32_t rng = FIRST ? st.rng : (slot * 4096u + f.accumulatedSamples);
+    const uint32_t reseed = FIRST ? st.reseed : slot;   // gl_GlobalInvocationID.y*4096 + .x
+
+    const float hitT = hit.t;
+    const uint32_t hitTri = hit.tri;
+    const bool hitScene = hitT != IDK_FLOAT_MAX;
+    const f3 rayDir = decode_unit_vec(st.pdx, st.pdy);
+    f3 origin = mk3(st.ox, st.oy, st.oz);
+    f3 thr = mk3(st.tx, st.ty, st.tz);
+    f3 rad = mk3(st.rx, st.ry, st.rz);
+
+    if (FIRST && f.doDebugTraversal) {
+        st.prevIor = debugCost;
+        survive = false;
+    } else if (hitScene) {
+        origin = origin + rayDir * hitT;
+        Surface s;
+        s.Albedo = mk3(1.0f, 1.0f, 1.0f); s.Alpha = 1.0f;
+        s.Normal = mk3(0.0f, 0.0f, 0.0f); s.Emissive = mk3(0.0f, 0.0f, 0.0f); s.Absorbance = mk3(0.0f, 0.0f, 0.0f);
+        s.Metallic = 0.0f; s.Roughness = 0.0f; s.Transmission = 0.0f; s.IOR = 1.5f; s.AlphaCutoff = 0.5f;
+        s.IsVolumetric = false; s.TintOnTransmissive = true;
+        f3 geometricNormal = mk3(0.0f, 0.0f, 0.0f);
+        bool passThrough = false;
+        const bool hitLight = hitTri == ~0u;
+        if (!hitLight) {
+            sortingKey = hitTri;
+            const int4 tri = __ldg(sc.blasTris + hitTri);
+            // independent gathers issued together: vertex frames, transform, per-mesh surface record, triangle normal
+            const float4* vf = sc.vtxFrame;
+            const float4 a0 = ldg4(vf + 2 * (size_t)tri.x), a1 = ldg4(vf + 2 * (size_t)tri.x + 1);
+            const float4 c0 = ldg4(vf + 2 * (size_t)tri.y), c1 = ldg4(vf + 2 * (size_t)tri.y + 1);
+            const float4 e0 = ldg4(vf + 2 * (size_t)tri.z), e1 = ldg4(vf + 2 * (size_t)tri.z + 1);
+            const float4* xf = sc.xforms + 9 * (size_t)hitXf + 3;
+            const float4 r0 = ldg4(xf), r1 = ldg4(xf + 1), r2 = ldg4(xf + 2);
+            const float4* sr = sc.surfRec + 5 * (size_t)tri.w;
+            const float4 s0 = ldg4(sr), s1 = ldg4(sr + 1), s2 = ldg4(sr + 2), s3 = ldg4(sr + 3), s4 = ldg4(sr + 4);
+            const float b0 = hit.bx, b1 = hit.by, b2 = 1.0f - hit.bx - hit.by;
+            const f3 interpNormal = normalize3((mk3(a0.x, a0.y, a0.z) * b0 + mk3(c0.x, c0.y, c0.z) * b1) + mk3(e0.x, e0.y, e0.z) * b2);
+            const f3 interpTangent = normalize3((mk3(a0.w, a1.x, a1.y) * b0 + mk3(c0.w, c1.x, c1.y) * b1) + mk3(e0.w, e1.x, e1.y) * b2);
+            const float normalMapStrength = s3.w;
+
+            // GetSurface (1x1 white textures, Surface.glsl:49-77) + SurfaceApplyModificatons (Surface.glsl:85-96),
+            // precomputed per mesh at upload (k_prepare_surfaces)
+            s.Albedo = mk3(s0.x, s0.y, s0.z);
+            s.Alpha = s0.w;
+            s.Normal = mk3(1.0f, 1.0f, 0.0f);
+            s.Emissive = mk3(s1.x, s1.y, s1.z);
+            s.Metallic = s1.w;
+            s.Absorbance = mk3(s2.x, s2.y, s2.z);
+            s.Roughness = s2.w;
+            s.Transmission = s3.x;
+            s.IOR = s3.y;
+            s.AlphaCutoff = s3.z;
+            s.IsVolumetric = (__float_as_uint(s4.x) & 1u) != 0;
+            s.TintOnTransmissive = (__float_as_uint(s4.x) & 2u) != 0;
+            if (TEX && (__float_as_uint(s4.x) & 4u)) {
+                float tu, tv;
+                interp_texcoord(sc, tri, b0, b1, b2, tu, tv);
+                surface_textured(sc, tri.w, tu, tv, s);
+            }
+
+            const float alphaCutoff = (s.AlphaCutoff == 2.0f) ? rnd01(rng) : s.AlphaCutoff;
+            if (s.Alpha < alphaCutoff) {
+                origin = origin + rayDir * 0.001f;
+                passThrough = true;
+            } else {
+                const f3 worldNormal = normalize3(xform_normal(r0, r1, r2, interpNormal));
+                const f3 worldTangent = normalize3(xform_normal(r0, r1, r2, interpTangent));
+                const f3 N = normalize3(worldNormal);
+                const f3 T = normalize3(worldTangent);
+                const f3 B = normalize3(cross3(N, T));
+                const f3 tbnN = (T * s.Normal.x + B * s.Normal.y) + N * s.Normal.z;
+                s.Normal = normalize3(mix3(worldNormal, tbnN, normalMapStrength));
+                const float4 tr = ldg4(sc.triRec + 4 * (size_t)hitTri + 2);
+                geometricNormal = normalize3(mk3(tr.y, tr.z, tr.w));   // GetTriangleNormal
+                geometricNormal = normalize3(xform_normal(r0, r1, r2, geometricNormal));
+            }
+        } else if (f.doTraceLights) {
+            sortingKey = hitXf;
+            const GpuLight& L = sc.lights[hitXf];
+            s.Emissive = mk3(L.Color[0], L.Color[1], L.Color[2]);
+            s.Albedo = s.Emissive;
+            s.Normal = (origin - mk3(L.Position[0], L.Position[1], L.Position[2])) / L.Radius;
+            geometricNormal = s.Normal;
+        }
+
+        if (passThrough) {
+            survive = true;
+        } else {
+            float prevIor = FIRST ? 1.0f : st.prevIor;
+            const bool fromInside = dot3(-rayDir, geometricNormal) < 0.0f;
+            if (fromInside) {
+                if (FIRST) prevIor = s.IOR;
+                geometricNormal = geometricNormal * -1.0f;
+                if (s.IsVolumetric) {
+                    const f3 e = -s.Absorbance * hitT;
+                    thr = thr * mk3(det_exp(e.x), det_exp(e.y), det_exp(e.z));
+                }
+            }
+            float cosTheta = dot3(-rayDir, s.Normal);
+            if (cosTheta < 0.0f) s.Normal = s.Normal * -1.0f;
+
+            rad = rad + s.Emissive * thr;
+
+            // ---- SampleMaterial (Shading.glsl:52-150)
+            Surface m = s;
+            m.Roughness *= m.Roughness;
+            cosTheta = dot3(-rayDir, m.Normal);
+            {
+                const float diffuseChance = 1.0f - m.Metallic - m.Transmission;
+                const float r0f = (prevIor - m.IOR) / (prevIor + m.IOR);
+                const float f0 = r0f * r0f;
+                const float fres = f0 + (1.0f - f0) * pow5f(1.0f - cosTheta);
+                m.Metallic = mix1(m.Metallic, 1.0f, fres);
+                m.Transmission = fmaxf(1.0f - diffuseChance - m.Metallic, 0.0f);
+            }
+            uint32_t bsdfType;
+            {
+                const float rnd = rnd01(rng);
+                if (m.Metallic > rnd) bsdfType = 1u;
+                else if (m.Metallic + m.Transmission > rnd) bsdfType = 2u;
+                else bsdfType = 0u;
+            }
+            f3 diffuseRayDir;
+            {
+                uint32_t tmp = reseed;
+                const float g = 1.32471795724474602596f;
+                const float a1 = 1.0f / g, a2 = 1.0f / (g * g);
+                const float r2u = fract1((float)f.accumulatedSamples * a1), r2v = fract1((float)f.accumulatedSamples * a2);
+                const float po0 = rnd01(tmp), po1 = rnd01(tmp);
+                const float u = fract1(r2u + po0), v = fract1(r2v + po1);
+                diffuseRayDir = normalize3(m.Normal + sample_sphere(u, v));
+            }
+            f3 newDir, bsdf;
+            float newIor;
+            if (bsdfType == 0u) {
+                newDir = diffuseRayDir; newIor = prevIor; bsdf = m.Albedo;
+            } else if (bsdfType == 1u) {
+                newDir = normalize3(mix3(reflect3(rayDir, m.Normal), diffuseRayDir, m.Roughness));
+                bsdf = m.Albedo; newIor = prevIor;
+            } else {
+                newIor = fromInside ? 1.0f : m.IOR;
+                f3 refr;
+                bool tir;
+                if (!m.IsVolumetric) {
+                    refr = rayDir; tir = false; newIor = 1.0f;
+                } else {
+                    refr = refract3(rayDir, m.Normal, prevIor / newIor);
+                    tir = refr.x == 0.0f && refr.y == 0.0f && refr.z == 0.0f;
+                    if (tir) { refr = reflect3(rayDir, m.Normal); newIor = prevIor; }
+                }
+                newDir = normalize3(mix3(refr, !tir ? -diffuseRayDir : diffuseRayDir, m.Roughness));
+                const bool gltfWantsTint = m.IsVolumetric || !fromInside;
+                bsdf = (gltfWantsTint && m.TintOnTransmissive) ? m.Albedo : mk3(1.0f, 1.0f, 1.0f);
+            }
+            // result.Pdf = max(1.0, 0.0001) = 1.0 in every branch; bsdf / 1.0f == bsdf exactly
+            thr = thr * bsdf;
+
+            if (a.outputAovs) {
+                // GetSurfaceVariance uses the un-remapped surface (FirstHit:197-203)
+                const float dc = 1.0f - s.Metallic - s.Transmission;
+                const float weight = dc + s.Metallic * s.Roughness + s.Transmission * s.Roughness;
+                if (FIRST) {
+                    const f3 al = s.Albedo * weight, no = s.Normal * weight;
+                    aov0 = make_float4(al.x, al.y, al.z, 1.0f - weight);
+                    aov1 = make_float4(no.x, no.y, no.z, 0.0f);
+                } else {
+                    const f3 al = mk3(aov0.x, aov0.y, aov0.z) + aov0.w * s.Albedo * weight;
+                    const f3 no = mk3(aov1.x, aov1.y, aov1.z) + aov0.w * s.Normal * weight;
+                    aov0 = make_float4(al.x, al.y, al.z, aov0.w * (1.0f - weight));
+                    aov1 = make_float4(no.x, no.y, no.z, 0.0f);
+                }
+            }
+
+            bool terminate = false;
+            if (!FIRST && f.doRussianRoulette) {
+                const float p = fmaxf(thr.x, fmaxf(thr.y, thr.z));
+                if (rnd01(rng) > p) terminate = true;
+                else thr = thr / p;
+            }
+            if (!terminate) {
+                if (bsdfType == 2u) geometricNormal = geometricNormal * -1.0f;
+                origin = origin + geometricNormal * 0.001f;
+                st.prevIor = newIor;
+                encode_unit_vec(newDir, st.pdx, st.pdy);
+                survive = true;
+            }
+        }
+    } else {
+        const f3 albedo = sample_sky(sc, rayDir);
+        if (a.outputAovs) {
+            const f3 fn = cubemap_face_normal(rayDir);
+            if (FIRST) {
+                aov0 = make_float4(albedo.x, albedo.y, albedo.z, 0.0f);
+                aov1 = make_float4(fn.x, fn.y, fn.z, 0.0f);
+            } else {
+                const f3 al = mk3(aov0.x, aov0.y, aov0.z) + aov0.w * albedo;
+                const f3 no = mk3(aov1.x, aov1.y, aov1.z) + aov0.w * fn;
+                aov0 = make_float4(al.x, al.y, al.z, 0.0f);
+                aov1 = make_float4(no.x, no.y, no.z, 0.0f);
+            }
+        }
+        rad = rad + albedo * thr;
+        survive = false;
+    }
+    st.ox = origin.x; st.oy = origin.y; st.oz = origin.z;
+    st.tx = thr.x; st.ty = thr.y; st.tz = thr.z;
+    st.rx = rad.x; st.ry = rad.y; st.rz = rad.z;
+
+    if (!survive || a.lastBounce) {
+        // path is final for this sample: hand its radiance (and AOVs) to the accumulate kernel
+        a.radiance[src] = make_float4(st.rx, st.ry, st.rz, st.prevIor);
+        if (a.outputAovs) { a.aovAlbedoFinal[src] = aov0; a.aovNormalFinal[src] = aov1; }
+    }
+    if ((survive && !a.lastBounce) || a.exportState) {
+        // wavefrontRaySSBO.Rays[rayIndex] = wavefrontRay (FirstHit:84, NHit:63), in place
+        float4* op = reinterpret_cast<float4*>(a.state + src);
+        op[0] = make_float4(st.ox, st.oy, st.oz, st.prevIor);
+        op[1] = make_float4(st.pdx, st.pdy, __uint_as_float(src), 0.0f);
+        op[2] = make_float4(st.tx, st.ty, st.tz, 0.0f);
+        op[3] = make_float4(st.rx, st.ry, st.rz, 0.0f);
+        if (a.outputAovs) { a.aov[2 * (size_t)src] = aov0; a.aov[2 * (size_t)src + 1] = aov1; }
+    }
+    if (!a.lastBounce) {
+        a.survivors[gid] = survive ? src : ~0u;
+        if (a.keysTmp) a.keysTmp[gid] = sortingKey & 0x1FFFFFu;
+    }
+}
+
+// NHit: one thread per alive ray, no block-level cooperation: every warp runs at its own pace (the ordered compaction of
 // the reference's atomic alive list is a separate, uniform-cost pass over 4-byte entries: k_compact).
 // TEX = the scene has material textures (idkpt_set_scene); the untextured instantiation is the north-star path.
 template <bool TEX>
 __global__ void __launch_bounds__(IDK_BLOCK, 3) k_shade(ShadeArgs a) {
     const uint32_t count = *a.count;
-    const DeviceScene& sc = a.sc;
-    const FrameParams& f = a.f;
-
     for (uint32_t gid = blockIdx.x * blockDim.x + threadIdx.x; gid < count; gid += gridDim.x * blockDim.x) {
-        bool survive = false;
+        const uint32_t src = a.alive[gid];
         PathState st;
-        float4 aov0 = make_float4(0.0f, 0.0f, 0.0f, 1.0f), aov1 = make_float4(0.0f, 0.0f, 0.0f, 0.0f);
-        uint32_t sortingKey = 0;
-        const uint32_t src = a.alive ? a.alive[gid] : gid;
-        {
-            {
-                const float4* sp = reinterpret_cast<const float4*>(a.state + src);
-                float4 v0 = sp[0], v1 = sp[1], v2 = sp[2], v3 = sp[3];
-                st.ox = v0.x; st.oy = v0.y; st.oz = v0.z; st.prevIor = v0.w;
-                st.pdx = v1.x; st.pdy = v1.y; st.pix = __float_as_uint(v1.z); st.reseed = __float_as_uint(v1.w);
-                st.tx = v2.x; st.ty = v2.y; st.tz = v2.z; st.rng = __float_as_uint(v2.w);
-                st.rx = v3.x; st.ry = v3.y; st.rz = v3.z; st.pad = 0;
+        const float4* sp = reinterpret_cast<const float4*>(a.state + src);
+        const float4 v0 = sp[0], v1 = sp[1], v2 = sp[2], v3 = sp[3];
+        st.ox = v0.x; st.oy = v0.y; st.oz = v0.z; st.prevIor = v0.w;
+        st.pdx = v1.x; st.pdy = v1.y; st.pix = __float_as_uint(v1.z); st.reseed = __float_as_uint(v1.w);
+        st.tx = v2.x; st.ty = v2.y; st.tz = v2.z; st.rng = __float_as_uint(v2.w);
+        st.rx = v3.x; st.ry = v3.y; st.rz = v3.z; st.pad = 0;
+        const float4 hv = reinterpret_cast<const float4*>(a.hits)[gid];
+        const HitRec hit = {hv.x, hv.y, hv.z, __float_as_uint(hv.w)};
+        shade_ray<TEX, false>(a, gid, src, st, hit, a.hitXform[gid], 0.0f);
+    }
+}
+
+// Bounce 0 in one pass, in registers: every warp repeatedly claims an 8x4 block of the tile's pixels (a compact footprint for
+// the coherent camera rays), and each lane generates its pixel's camera ray (camera_ray), finds the closest hit with the
+// serial walk (trace_ray, so the counters are those of every other closest-hit walk) and shades it (shade_ray<TEX, true>).
+// The slot of a primary ray is its tile pixel. k_compact follows as after every bounce.
+struct FirstHitArgs {
+    ShadeArgs s;                   // alive, hits, hitXform and slotDelta unused: the slot is the tile pixel
+    uint32_t* ticket;              // 8x4 pixel blocks claimed so far (zeroed per sample)
+    TraceCounters* counters;       // STATS only
+    uint32_t rows;                 // tile rows
+};
+
+template <bool STATS, bool TLAS, bool TEX>
+__global__ void __launch_bounds__(IDK_BLOCK, 3) k_first_hit(FirstHitArgs a) {
+    extern __shared__ uint32_t s_stack[];
+    uint32_t* stack = s_stack + threadIdx.x;
+    const uint32_t lane = threadIdx.x & 31;
+    const FrameParams& f = a.s.f;
+    const uint32_t width = (uint32_t)f.width;
+    const uint32_t blocksX = (width + 7) / 8, blocks = blocksX * ((a.rows + 3) / 4);
+    uint32_t S = 0, T = 0, I = 0, H = 0;
+    for (;;) {
+        uint32_t b = 0;
+        if (lane == 0) b = atomicAdd(a.ticket, 1u);
+        b = __shfl_sync(0xffffffffu, b, 0);
+        if (b >= blocks) break;
+        const uint32_t x = (b % blocksX) * 8 + (lane & 7), row = (b / blocksX) * 4 + (lane >> 3);
+        if (x < width && row < a.rows) {
+            const uint32_t li = row * width + x;
+            const PathState st = camera_ray(f, (int)x, tile_row_y(f, (int)row), li);
+            HitRec hit;
+            uint32_t xf;
+            float cost = 0.0f;
+            const uint32_t stepsBefore = S;
+            trace_ray<STATS, false, AcceptAll, TLAS ? TLAS_ON : TLAS_OFF>(a.s.sc, mk3(st.ox, st.oy, st.oz), decode_unit_vec(st.pdx, st.pdy),
+                                                                         IDK_FLOAT_MAX, f.doTraceLights != 0, stack, hit, xf, S, T, I, cost);
+            if (STATS) {
+                atomicMax(&a.counters->maxSteps[0], S - stepsBefore);
+                if (hit.tri != ~0u) H++;
             }
-            if (a.outputAovs && !a.firstHit) { aov0 = a.aov[2 * (size_t)src]; aov1 = a.aov[2 * (size_t)src + 1]; }
-            // NHit's gl_GlobalInvocationID.x is the ray's slot in the alive list of the WHOLE image; a stripe tile adds the number of
-            // alive rays in the other ranks' stripes above it (k_slot_exchange), so that N GPUs draw the 1-GPU random numbers
-            const uint32_t slot = (a.slotDelta && !a.firstHit) ? gid + a.slotDelta[src / a.stripePixels] : gid;
-            uint32_t rng = a.firstHit ? st.rng : (slot * 4096u + f.accumulatedSamples);
-            const uint32_t reseed = a.firstHit ? st.reseed : slot;   // gl_GlobalInvocationID.y*4096 + .x
-
-            const float4 hv = reinterpret_cast<const float4*>(a.hits)[gid];
-            const float hitT = hv.z;
-            const uint32_t hitTri = __float_as_uint(hv.w);
-            const uint32_t hitXf = a.hitXform[gid];
-            const bool hitScene = hitT != IDK_FLOAT_MAX;
-            const f3 rayDir = decode_unit_vec(st.pdx, st.pdy);
-            f3 origin = mk3(st.ox, st.oy, st.oz);
-            f3 thr = mk3(st.tx, st.ty, st.tz);
-            f3 rad = mk3(st.rx, st.ry, st.rz);
-
-            if (a.firstHit && f.doDebugTraversal) {
-                st.prevIor = a.debugCost[gid];
-                survive = false;
-            } else if (hitScene) {
-                origin = origin + rayDir * hitT;
-                Surface s;
-                s.Albedo = mk3(1.0f, 1.0f, 1.0f); s.Alpha = 1.0f;
-                s.Normal = mk3(0.0f, 0.0f, 0.0f); s.Emissive = mk3(0.0f, 0.0f, 0.0f); s.Absorbance = mk3(0.0f, 0.0f, 0.0f);
-                s.Metallic = 0.0f; s.Roughness = 0.0f; s.Transmission = 0.0f; s.IOR = 1.5f; s.AlphaCutoff = 0.5f;
-                s.IsVolumetric = false; s.TintOnTransmissive = true;
-                f3 geometricNormal = mk3(0.0f, 0.0f, 0.0f);
-                bool passThrough = false;
-                const bool hitLight = hitTri == ~0u;
-                if (!hitLight) {
-                    sortingKey = hitTri;
-                    const int4 tri = __ldg(sc.blasTris + hitTri);
-                    // independent gathers issued together: vertex frames, transform, per-mesh surface record, triangle normal
-                    const float4* vf = sc.vtxFrame;
-                    const float4 a0 = ldg4(vf + 2 * (size_t)tri.x), a1 = ldg4(vf + 2 * (size_t)tri.x + 1);
-                    const float4 c0 = ldg4(vf + 2 * (size_t)tri.y), c1 = ldg4(vf + 2 * (size_t)tri.y + 1);
-                    const float4 e0 = ldg4(vf + 2 * (size_t)tri.z), e1 = ldg4(vf + 2 * (size_t)tri.z + 1);
-                    const float4* xf = sc.xforms + 9 * (size_t)hitXf + 3;
-                    const float4 r0 = ldg4(xf), r1 = ldg4(xf + 1), r2 = ldg4(xf + 2);
-                    const float4* sr = sc.surfRec + 5 * (size_t)tri.w;
-                    const float4 s0 = ldg4(sr), s1 = ldg4(sr + 1), s2 = ldg4(sr + 2), s3 = ldg4(sr + 3), s4 = ldg4(sr + 4);
-                    const float b0 = hv.x, b1 = hv.y, b2 = 1.0f - hv.x - hv.y;
-                    const f3 interpNormal = normalize3((mk3(a0.x, a0.y, a0.z) * b0 + mk3(c0.x, c0.y, c0.z) * b1) + mk3(e0.x, e0.y, e0.z) * b2);
-                    const f3 interpTangent = normalize3((mk3(a0.w, a1.x, a1.y) * b0 + mk3(c0.w, c1.x, c1.y) * b1) + mk3(e0.w, e1.x, e1.y) * b2);
-                    const float normalMapStrength = s3.w;
-
-                    // GetSurface (1x1 white textures, Surface.glsl:49-77) + SurfaceApplyModificatons (Surface.glsl:85-96),
-                    // precomputed per mesh at upload (k_prepare_surfaces)
-                    s.Albedo = mk3(s0.x, s0.y, s0.z);
-                    s.Alpha = s0.w;
-                    s.Normal = mk3(1.0f, 1.0f, 0.0f);
-                    s.Emissive = mk3(s1.x, s1.y, s1.z);
-                    s.Metallic = s1.w;
-                    s.Absorbance = mk3(s2.x, s2.y, s2.z);
-                    s.Roughness = s2.w;
-                    s.Transmission = s3.x;
-                    s.IOR = s3.y;
-                    s.AlphaCutoff = s3.z;
-                    s.IsVolumetric = (__float_as_uint(s4.x) & 1u) != 0;
-                    s.TintOnTransmissive = (__float_as_uint(s4.x) & 2u) != 0;
-                    if (TEX && (__float_as_uint(s4.x) & 4u)) {
-                        float tu, tv;
-                        interp_texcoord(sc, tri, b0, b1, b2, tu, tv);
-                        surface_textured(sc, tri.w, tu, tv, s);
-                    }
-
-                    const float alphaCutoff = (s.AlphaCutoff == 2.0f) ? rnd01(rng) : s.AlphaCutoff;
-                    if (s.Alpha < alphaCutoff) {
-                        origin = origin + rayDir * 0.001f;
-                        passThrough = true;
-                    } else {
-                        const f3 worldNormal = normalize3(xform_normal(r0, r1, r2, interpNormal));
-                        const f3 worldTangent = normalize3(xform_normal(r0, r1, r2, interpTangent));
-                        const f3 N = normalize3(worldNormal);
-                        const f3 T = normalize3(worldTangent);
-                        const f3 B = normalize3(cross3(N, T));
-                        const f3 tbnN = (T * s.Normal.x + B * s.Normal.y) + N * s.Normal.z;
-                        s.Normal = normalize3(mix3(worldNormal, tbnN, normalMapStrength));
-                        const float4 tr = ldg4(sc.triRec + 4 * (size_t)hitTri + 2);
-                        geometricNormal = normalize3(mk3(tr.y, tr.z, tr.w));   // GetTriangleNormal
-                        geometricNormal = normalize3(xform_normal(r0, r1, r2, geometricNormal));
-                    }
-                } else if (f.doTraceLights) {
-                    sortingKey = hitXf;
-                    const GpuLight& L = sc.lights[hitXf];
-                    s.Emissive = mk3(L.Color[0], L.Color[1], L.Color[2]);
-                    s.Albedo = s.Emissive;
-                    s.Normal = (origin - mk3(L.Position[0], L.Position[1], L.Position[2])) / L.Radius;
-                    geometricNormal = s.Normal;
-                }
-
-                if (passThrough) {
-                    survive = true;
-                } else {
-                    float prevIor = a.firstHit ? 1.0f : st.prevIor;
-                    const bool fromInside = dot3(-rayDir, geometricNormal) < 0.0f;
-                    if (fromInside) {
-                        if (a.firstHit) prevIor = s.IOR;
-                        geometricNormal = geometricNormal * -1.0f;
-                        if (s.IsVolumetric) {
-                            const f3 e = -s.Absorbance * hitT;
-                            thr = thr * mk3(det_exp(e.x), det_exp(e.y), det_exp(e.z));
-                        }
-                    }
-                    float cosTheta = dot3(-rayDir, s.Normal);
-                    if (cosTheta < 0.0f) s.Normal = s.Normal * -1.0f;
-
-                    rad = rad + s.Emissive * thr;
-
-                    // ---- SampleMaterial (Shading.glsl:52-150)
-                    Surface m = s;
-                    m.Roughness *= m.Roughness;
-                    cosTheta = dot3(-rayDir, m.Normal);
-                    {
-                        const float diffuseChance = 1.0f - m.Metallic - m.Transmission;
-                        const float r0f = (prevIor - m.IOR) / (prevIor + m.IOR);
-                        const float f0 = r0f * r0f;
-                        const float fres = f0 + (1.0f - f0) * pow5f(1.0f - cosTheta);
-                        m.Metallic = mix1(m.Metallic, 1.0f, fres);
-                        m.Transmission = fmaxf(1.0f - diffuseChance - m.Metallic, 0.0f);
-                    }
-                    uint32_t bsdfType;
-                    {
-                        const float rnd = rnd01(rng);
-                        if (m.Metallic > rnd) bsdfType = 1u;
-                        else if (m.Metallic + m.Transmission > rnd) bsdfType = 2u;
-                        else bsdfType = 0u;
-                    }
-                    f3 diffuseRayDir;
-                    {
-                        uint32_t tmp = reseed;
-                        const float g = 1.32471795724474602596f;
-                        const float a1 = 1.0f / g, a2 = 1.0f / (g * g);
-                        const float r2u = fract1((float)f.accumulatedSamples * a1), r2v = fract1((float)f.accumulatedSamples * a2);
-                        const float po0 = rnd01(tmp), po1 = rnd01(tmp);
-                        const float u = fract1(r2u + po0), v = fract1(r2v + po1);
-                        diffuseRayDir = normalize3(m.Normal + sample_sphere(u, v));
-                    }
-                    f3 newDir, bsdf;
-                    float newIor;
-                    if (bsdfType == 0u) {
-                        newDir = diffuseRayDir; newIor = prevIor; bsdf = m.Albedo;
-                    } else if (bsdfType == 1u) {
-                        newDir = normalize3(mix3(reflect3(rayDir, m.Normal), diffuseRayDir, m.Roughness));
-                        bsdf = m.Albedo; newIor = prevIor;
-                    } else {
-                        newIor = fromInside ? 1.0f : m.IOR;
-                        f3 refr;
-                        bool tir;
-                        if (!m.IsVolumetric) {
-                            refr = rayDir; tir = false; newIor = 1.0f;
-                        } else {
-                            refr = refract3(rayDir, m.Normal, prevIor / newIor);
-                            tir = refr.x == 0.0f && refr.y == 0.0f && refr.z == 0.0f;
-                            if (tir) { refr = reflect3(rayDir, m.Normal); newIor = prevIor; }
-                        }
-                        newDir = normalize3(mix3(refr, !tir ? -diffuseRayDir : diffuseRayDir, m.Roughness));
-                        const bool gltfWantsTint = m.IsVolumetric || !fromInside;
-                        bsdf = (gltfWantsTint && m.TintOnTransmissive) ? m.Albedo : mk3(1.0f, 1.0f, 1.0f);
-                    }
-                    // result.Pdf = max(1.0, 0.0001) = 1.0 in every branch; bsdf / 1.0f == bsdf exactly
-                    thr = thr * bsdf;
-
-                    if (a.outputAovs) {
-                        // GetSurfaceVariance uses the un-remapped surface (FirstHit:197-203)
-                        const float dc = 1.0f - s.Metallic - s.Transmission;
-                        const float weight = dc + s.Metallic * s.Roughness + s.Transmission * s.Roughness;
-                        if (a.firstHit) {
-                            const f3 al = s.Albedo * weight, no = s.Normal * weight;
-                            aov0 = make_float4(al.x, al.y, al.z, 1.0f - weight);
-                            aov1 = make_float4(no.x, no.y, no.z, 0.0f);
-                        } else {
-                            const f3 al = mk3(aov0.x, aov0.y, aov0.z) + aov0.w * s.Albedo * weight;
-                            const f3 no = mk3(aov1.x, aov1.y, aov1.z) + aov0.w * s.Normal * weight;
-                            aov0 = make_float4(al.x, al.y, al.z, aov0.w * (1.0f - weight));
-                            aov1 = make_float4(no.x, no.y, no.z, 0.0f);
-                        }
-                    }
-
-                    bool terminate = false;
-                    if (!a.firstHit && f.doRussianRoulette) {
-                        const float p = fmaxf(thr.x, fmaxf(thr.y, thr.z));
-                        if (rnd01(rng) > p) terminate = true;
-                        else thr = thr / p;
-                    }
-                    if (!terminate) {
-                        if (bsdfType == 2u) geometricNormal = geometricNormal * -1.0f;
-                        origin = origin + geometricNormal * 0.001f;
-                        st.prevIor = newIor;
-                        encode_unit_vec(newDir, st.pdx, st.pdy);
-                        survive = true;
-                    }
-                }
-            } else {
-                const f3 albedo = sample_sky(sc, rayDir);
-                if (a.outputAovs) {
-                    const f3 fn = cubemap_face_normal(rayDir);
-                    if (a.firstHit) {
-                        aov0 = make_float4(albedo.x, albedo.y, albedo.z, 0.0f);
-                        aov1 = make_float4(fn.x, fn.y, fn.z, 0.0f);
-                    } else {
-                        const f3 al = mk3(aov0.x, aov0.y, aov0.z) + aov0.w * albedo;
-                        const f3 no = mk3(aov1.x, aov1.y, aov1.z) + aov0.w * fn;
-                        aov0 = make_float4(al.x, al.y, al.z, 0.0f);
-                        aov1 = make_float4(no.x, no.y, no.z, 0.0f);
-                    }
-                }
-                rad = rad + albedo * thr;
-                survive = false;
-            }
-            st.ox = origin.x; st.oy = origin.y; st.oz = origin.z;
-            st.tx = thr.x; st.ty = thr.y; st.tz = thr.z;
-            st.rx = rad.x; st.ry = rad.y; st.rz = rad.z;
-
-            if (!survive || a.lastBounce) {
-                // path is final for this sample: hand its radiance (and AOVs) to the accumulate kernel
-                a.radiance[src] = make_float4(st.rx, st.ry, st.rz, st.prevIor);
-                if (a.outputAovs) { a.aovAlbedoFinal[src] = aov0; a.aovNormalFinal[src] = aov1; }
-            }
-            if ((survive && !a.lastBounce) || a.exportState) {
-                // wavefrontRaySSBO.Rays[rayIndex] = wavefrontRay (FirstHit:84, NHit:63), in place
-                float4* op = reinterpret_cast<float4*>(a.state + src);
-                op[0] = make_float4(st.ox, st.oy, st.oz, st.prevIor);
-                op[1] = make_float4(st.pdx, st.pdy, __uint_as_float(src), 0.0f);
-                op[2] = make_float4(st.tx, st.ty, st.tz, 0.0f);
-                op[3] = make_float4(st.rx, st.ry, st.rz, 0.0f);
-                if (a.outputAovs) { a.aov[2 * (size_t)src] = aov0; a.aov[2 * (size_t)src + 1] = aov1; }
-            }
-            if (!a.lastBounce) {
-                a.survivors[gid] = survive ? src : ~0u;
-                if (a.keysTmp) a.keysTmp[gid] = sortingKey & 0x1FFFFFu;
-            }
+            shade_ray<TEX, true>(a.s, li, li, st, hit, xf, cost);
+        }
+    }
+    if (STATS) {
+        for (int off = 16; off > 0; off >>= 1) {
+            S += __shfl_down_sync(0xffffffffu, S, off);
+            T += __shfl_down_sync(0xffffffffu, T, off);
+            I += __shfl_down_sync(0xffffffffu, I, off);
+            H += __shfl_down_sync(0xffffffffu, H, off);
+        }
+        if (lane == 0) {
+            atomicAdd(&a.counters->steps, (unsigned long long)S);
+            atomicAdd(&a.counters->tris, (unsigned long long)T);
+            atomicAdd(&a.counters->instances, (unsigned long long)I);
+            atomicAdd(&a.counters->hits, (unsigned long long)H);
         }
     }
 }

@@ -162,8 +162,8 @@ struct IdkPtCtx : IdkCtxBase {
 
     // launch configuration
     int traverseBlocks = 0, traverseBlocksStats = 0, shadeBlocks = 0, traceRaysBlocks = 0, compactBlocks = 0;
-    int traverse1Blocks = 0, traverse1BlocksStats = 0;
-    int traverseBlocksLane = 0, traverse1BlocksLane = 0;   // grids of the asynchronous path: the resident-block budget split between the lanes
+    int firstHitBlocks[2][2] = {};  // k_first_hit grids of this scene's TLAS mode, [STATS][TEX]
+    int traverseBlocksLane = 0, firstHitBlocksLane[2] = {};   // grids of the asynchronous path ([TEX]): the resident-block budget split between the lanes
     size_t stackBytes = 0;
     size_t traverse2Smem = 0;      // k_traverse2 stacks (IDK_T2_BLOCK columns)
 
@@ -279,12 +279,16 @@ static void compute_tile_rows(IdkPtCtx* ctx) {
         if (ctx->tileCount <= 1 || (s % ctx->tileCount) == ctx->tileIndex) ctx->nLocalStripes++;
 }
 
+// k_first_hit<STATS, TLAS, TEX> by [TLAS][STATS][TEX]
+using FirstHitKernel = void (*)(FirstHitArgs);
+static const FirstHitKernel kFirstHit[2][2][2] = {
+    {{k_first_hit<false, false, false>, k_first_hit<false, false, true>}, {k_first_hit<true, false, false>, k_first_hit<true, false, true>}},
+    {{k_first_hit<false, true, false>, k_first_hit<false, true, true>}, {k_first_hit<true, true, false>, k_first_hit<true, true, true>}}};
+
 static int configure_launches(IdkPtCtx* ctx) {
     const int stackSize = std::max(1, ctx->sc.stackSize);
     ctx->stackBytes = (size_t)stackSize * IDK_BLOCK * sizeof(uint32_t);
     if (ctx->stackBytes > 200 * 1024) return fail(ctx, IDKPT_ERR_UNSUPPORTED, "BlasStackSize too large for the shared-memory traversal stack");
-    CK(cudaFuncSetAttribute(k_traverse<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)ctx->stackBytes));
-    CK(cudaFuncSetAttribute(k_traverse<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)ctx->stackBytes));
     CK(cudaFuncSetAttribute(k_trace_rays, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)ctx->stackBytes));
     CK(cudaFuncSetAttribute(k_trace_rays_any, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)ctx->stackBytes));
     CK(cudaFuncSetAttribute(k_shadows_ray_traced, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)ctx->stackBytes));
@@ -298,10 +302,14 @@ static int configure_launches(IdkPtCtx* ctx) {
     CK(cudaFuncSetAttribute(k_traverse2<false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)ctx->traverse2Smem));
     CK(cudaFuncSetAttribute(k_traverse2<true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)ctx->traverse2Smem));
     int n = 0;
-    CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&n, k_traverse<false>, IDK_BLOCK, ctx->stackBytes));
-    ctx->traverse1Blocks = std::max(1, n) * ctx->smCount;
-    CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&n, k_traverse<true>, IDK_BLOCK, ctx->stackBytes));
-    ctx->traverse1BlocksStats = std::max(1, n) * ctx->smCount;
+    // both TEX variants: idkpt_set_textures may switch between them without coming back here
+    for (int stats = 0; stats < 2; stats++)
+        for (int tex = 0; tex < 2; tex++) {
+            const FirstHitKernel k = kFirstHit[ctx->sc.useTlas ? 1 : 0][stats][tex];
+            CK(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)ctx->stackBytes));
+            CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&n, k, IDK_BLOCK, ctx->stackBytes));
+            ctx->firstHitBlocks[stats][tex] = std::max(1, n) * ctx->smCount;
+        }
     if (ctx->sc.useTlas) {
         CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&n, k_traverse2<false, true>, IDK_T2_BLOCK, ctx->traverse2Smem));
         ctx->traverseBlocks = std::max(1, n) * ctx->smCount;
@@ -323,9 +331,10 @@ static int configure_launches(IdkPtCtx* ctx) {
     // the resident-block budget
     {
         const int lanes = std::max(1, ctx->laneCount);
-        const int perSm2 = (ctx->traverseBlocks / ctx->smCount + lanes - 1) / lanes, perSm1 = (ctx->traverse1Blocks / ctx->smCount + lanes - 1) / lanes;
+        const int perSm2 = (ctx->traverseBlocks / ctx->smCount + lanes - 1) / lanes;
         ctx->traverseBlocksLane = std::max(1, perSm2) * ctx->smCount;
-        ctx->traverse1BlocksLane = std::max(1, perSm1) * ctx->smCount;
+        for (int tex = 0; tex < 2; tex++)
+            ctx->firstHitBlocksLane[tex] = std::max(1, (ctx->firstHitBlocks[0][tex] / ctx->smCount + lanes - 1) / lanes) * ctx->smCount;
     }
     return IDKPT_OK;
 }
@@ -1019,7 +1028,6 @@ IDKPT_API int idkpt_compute(IdkPtCtx* ctx, const GpuPerFrameData* frame, const I
     if (stats) CK(ensure(countLog, hostCounts.size() * sizeof(uint32_t)));
     if (wantStats) CK(cudaMemsetAsync(ctx->counters.p, 0, sizeof(TraceCounters), ctx->stream));
 
-    const dim3 rgGrid((ctx->width + 7) / 8, (ctx->height + 7) / 8), rgBlock(8, 8);
     const int accBlocks = std::min<int>((int)((n + IDK_BLOCK - 1) / IDK_BLOCK), ctx->smCount * 8);
 
     for (int s = 0; s < st->SamplesPerPixel; s++) {
@@ -1045,15 +1053,11 @@ IDKPT_API int idkpt_compute(IdkPtCtx* ctx, const GpuPerFrameData* frame, const I
         k_init_sample<<<1, 256, 0, ls>>>(counts, IDKPT_MAX_RAY_DEPTH + 1, tickets, 2 * (IDKPT_MAX_RAY_DEPTH + 1), n);
         launches++;
 
-        size_t e0 = ev.begin();
-        k_raygen<<<rgGrid, rgBlock, 0, ls>>>(f, (PathState*)ln.state.p);
-        ev.end(e0, 3);
-        launches++;
-
+        size_t e0 = 0;
         for (int j = 0; j < st->RayDepth; j++) {
             const bool first = j == 0;
             const bool last = j == st->RayDepth - 1;
-            // alive list of this bounce: slot -> tile pixel (identity for the first hit)
+            // alive list of this bounce: slot -> tile pixel (none for the first hit: its slot is the tile pixel)
             const uint32_t* alive = first ? nullptr : (const uint32_t*)ln.alive[j & 1].p;
             if (sorting && j > 1) {
                 // PathTracer.RaySorting(), PathTracer.cs:273-297: stable sort of the alive list by cached key
@@ -1089,23 +1093,50 @@ IDKPT_API int idkpt_compute(IdkPtCtx* ctx, const GpuPerFrameData* frame, const I
                 launches++;
             }
 
-            TraverseArgs ta;
-            ta.sc = ctx->sc;
-            ta.state = (const PathState*)ln.state.p;
-            ta.perm = alive;
-            ta.count = counts + j;
-            ta.ticket = tickets + 2 * j;
-            ta.hits = (HitRec*)ln.hits.p;
-            ta.hitXform = (uint32_t*)ln.hitXform.p;
-            ta.debugCost = (float*)ln.debugCost.p;
-            ta.counters = (TraceCounters*)ctx->counters.p;
-            ta.traceLights = st->Gpu.DoTraceLights;
-            ta.bounce = j;
+            ShadeArgs sa;
+            sa.sc = ctx->sc;
+            sa.f = f;
+            sa.state = (PathState*)ln.state.p;
+            sa.aov = (float4*)ln.aov.p;
+            sa.alive = alive;
+            sa.hits = (const HitRec*)ln.hits.p;
+            sa.hitXform = (const uint32_t*)ln.hitXform.p;
+            sa.count = counts + j;
+            sa.survivors = (uint32_t*)ln.survivors.p;
+            sa.keysTmp = sorting ? (uint32_t*)ln.keysTmp.p : nullptr;
+            sa.radiance = (float4*)ln.radiance.p;
+            sa.aovAlbedoFinal = (float4*)ln.aovAlbedoFinal.p;
+            sa.aovNormalFinal = (float4*)ln.aovNormalFinal.p;
+            sa.slotDelta = (globalSlots && !first) ? (const uint32_t*)ln.slotDelta.p : nullptr;
+            sa.stripePixels = (uint32_t)ctx->stripeH * (uint32_t)ctx->width;
+            sa.exportState = ctx->exportEnabled ? 1 : 0;
+            sa.lastBounce = last ? 1 : 0;
+            sa.outputAovs = aovs ? 1 : 0;
+            const int tex = ctx->sc.textureCount ? 1 : 0;
+
+            // bounce 0 is one kernel (camera rays, closest hit, FirstHit shading), timed as its traversal
             e0 = ev.begin();
-            if (first) {     // the coherent primary rays: one ray per lane
-                if (wantStats) k_traverse<true><<<ctx->traverse1BlocksStats, IDK_BLOCK, ctx->stackBytes, ls>>>(ta);
-                else k_traverse<false><<<async ? ctx->traverse1BlocksLane : ctx->traverse1Blocks, IDK_BLOCK, ctx->stackBytes, ls>>>(ta);
+            if (first) {
+                FirstHitArgs fa;
+                fa.s = sa;
+                fa.ticket = tickets;
+                fa.counters = (TraceCounters*)ctx->counters.p;
+                fa.rows = n / (uint32_t)ctx->width;
+                const int fb = wantStats ? ctx->firstHitBlocks[1][tex] : async ? ctx->firstHitBlocksLane[tex] : ctx->firstHitBlocks[0][tex];
+                kFirstHit[ctx->sc.useTlas ? 1 : 0][wantStats ? 1 : 0][tex]<<<fb, IDK_BLOCK, ctx->stackBytes, ls>>>(fa);
             } else {         // every later bounce: phase-scheduled warps
+                TraverseArgs ta;
+                ta.sc = ctx->sc;
+                ta.state = (const PathState*)ln.state.p;
+                ta.perm = alive;
+                ta.count = counts + j;
+                ta.ticket = tickets + 2 * j;
+                ta.hits = (HitRec*)ln.hits.p;
+                ta.hitXform = (uint32_t*)ln.hitXform.p;
+                ta.debugCost = (float*)ln.debugCost.p;
+                ta.counters = (TraceCounters*)ctx->counters.p;
+                ta.traceLights = st->Gpu.DoTraceLights;
+                ta.bounce = j;
                 const int tb = async ? ctx->traverseBlocksLane : ctx->traverseBlocks;
                 const TraverseTuning tune = {IDK_T2_SETUP_THRESHOLD, IDK_T2_LEAF_THRESHOLD, async ? 1 : 0};
                 if (ctx->sc.useTlas) {       // the TLAS walk is a fourth phase of the production kernel (BVHIntersect.glsl:205-272)
@@ -1120,31 +1151,12 @@ IDKPT_API int idkpt_compute(IdkPtCtx* ctx, const GpuPerFrameData* frame, const I
             launches++;
             traverseLaunches++;
 
-            ShadeArgs sa;
-            sa.sc = ctx->sc;
-            sa.f = f;
-            sa.state = (PathState*)ln.state.p;
-            sa.aov = (float4*)ln.aov.p;
-            sa.alive = alive;
-            sa.hits = (const HitRec*)ln.hits.p;
-            sa.hitXform = (const uint32_t*)ln.hitXform.p;
-            sa.debugCost = (const float*)ln.debugCost.p;
-            sa.count = counts + j;
-            sa.survivors = (uint32_t*)ln.survivors.p;
-            sa.keysTmp = sorting ? (uint32_t*)ln.keysTmp.p : nullptr;
-            sa.radiance = (float4*)ln.radiance.p;
-            sa.aovAlbedoFinal = (float4*)ln.aovAlbedoFinal.p;
-            sa.aovNormalFinal = (float4*)ln.aovNormalFinal.p;
-            sa.slotDelta = (globalSlots && !first) ? (const uint32_t*)ln.slotDelta.p : nullptr;
-            sa.stripePixels = (uint32_t)ctx->stripeH * (uint32_t)ctx->width;
-            sa.exportState = ctx->exportEnabled ? 1 : 0;
-            sa.firstHit = first ? 1 : 0;
-            sa.lastBounce = last ? 1 : 0;
-            sa.outputAovs = aovs ? 1 : 0;
             e0 = ev.begin();
-            if (ctx->sc.textureCount) k_shade<true><<<ctx->shadeBlocks, IDK_BLOCK, 0, ls>>>(sa);
-            else k_shade<false><<<ctx->shadeBlocks, IDK_BLOCK, 0, ls>>>(sa);
-            launches++;
+            if (!first) {
+                if (tex) k_shade<true><<<ctx->shadeBlocks, IDK_BLOCK, 0, ls>>>(sa);
+                else k_shade<false><<<ctx->shadeBlocks, IDK_BLOCK, 0, ls>>>(sa);
+                launches++;
+            }
             if (!last) {
                 CompactArgs ca;
                 ca.survivors = (const uint32_t*)ln.survivors.p;
@@ -1375,7 +1387,9 @@ static int preload_kernels(IdkPtCtx* ctx) {
     cudaFuncAttributes fa;
 #define IDK_PRELOAD(k) CK(cudaFuncGetAttributes(&fa, k))
     IDK_PRELOAD(k_init_sample); IDK_PRELOAD(k_prepare_triangles); IDK_PRELOAD(k_prepare_vertices); IDK_PRELOAD(k_prepare_surfaces);
-    IDK_PRELOAD(k_raygen); IDK_PRELOAD(k_traverse<false>); IDK_PRELOAD(k_traverse<true>);
+    for (const auto& byStats : kFirstHit)
+        for (const auto& byTex : byStats)
+            for (FirstHitKernel k : byTex) IDK_PRELOAD(k);
     IDK_PRELOAD((k_traverse2<false, false>)); IDK_PRELOAD((k_traverse2<true, false>));
     IDK_PRELOAD((k_traverse2<false, true>)); IDK_PRELOAD((k_traverse2<true, true>));
     IDK_PRELOAD(k_shade<false>); IDK_PRELOAD(k_shade<true>); IDK_PRELOAD(k_compact); IDK_PRELOAD(k_slot_exchange);

@@ -156,10 +156,10 @@ typedef struct IdkPtStats {
     uint64_t InstanceVisits;                     /* I (valid if CollectStats) */
     uint64_t Hits;                               /* rays that hit scene geometry (valid if CollectStats) */
     float    TotalMs;                            /* CUDA-event time of the whole call */
-    float    TraverseMs;                         /* sum over traversal launches */
-    float    ShadeMs;                            /* sum over shade launches */
+    float    TraverseMs;                         /* sum over traversal launches (bounce 0's includes ray-gen and FirstHit shading) */
+    float    ShadeMs;                            /* sum over shade launches (bounces >= 1) + compaction */
     float    SortMs;
-    float    OtherMs;                            /* ray-gen + accumulate */
+    float    OtherMs;                            /* accumulate */
     uint32_t KernelLaunches;
     uint32_t TraverseLaunches;
     float    BounceTraverseMs[IDKPT_MAX_RAY_DEPTH];   /* per bounce, summed over samples */
