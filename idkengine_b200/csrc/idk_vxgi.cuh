@@ -14,7 +14,7 @@
 #include "../../include/idk_gpu_types.h"
 
 #define IDKVX_MAX_LEVELS 16
-#define IDKVX_SMALL_LIMIT 16   // bounding boxes up to this many pixel centres are rasterised by the discovering thread
+#define IDKVX_SMALL_LIMIT 16   // bounding boxes up to this many pixels are rasterised by the discovering thread
 #define IDKVX_TILE 64          // larger boxes are cut into IDKVX_TILE^2 pixel tiles, one CTA each
 
 struct VxGridDev {
@@ -60,7 +60,13 @@ struct VxTri {
 __device__ __forceinline__ float vx_edge(float ax, float ay, float bx, float by, float cx, float cy) { return (bx - ax) * (cy - ay) - (by - ay) * (cx - ax); }
 __device__ __forceinline__ float f3get(f3 v, int i) { return i == 0 ? v.x : (i == 1 ? v.y : v.z); }
 
-__device__ __forceinline__ void vx_setup(const VxScene& sc, const VxGridDev& g, uint32_t inst, uint32_t triIndex, VxTri& t) {
+// Per-triangle state of the conservative coverage rule (DESIGN.md section 7): r[k] = 0.5 (|da_k| + |db_k|) is the most edge
+// function k can gain anywhere in a pixel square around the centre where it is evaluated. The centre rule carries none.
+template <bool Conservative> struct VxCover {};
+template <> struct VxCover<true> { float r[3]; };
+
+template <bool Conservative>
+__device__ __forceinline__ void vx_setup(const VxScene& sc, const VxGridDev& g, uint32_t inst, uint32_t triIndex, VxTri& t, VxCover<Conservative>& cv) {
     const GpuBlasInstance bi = sc.instances[inst];
     const float4* xf = sc.xforms + 9 * (size_t)bi.MeshTransformId;
     const float4 m0 = ldg4(xf), m1 = ldg4(xf + 1), m2 = ldg4(xf + 2), i0 = ldg4(xf + 3), i1 = ldg4(xf + 4), i2 = ldg4(xf + 5);
@@ -94,19 +100,35 @@ __device__ __forceinline__ void vx_setup(const VxScene& sc, const VxGridDev& g, 
     t.valid = !(t.area == 0.0f || !(t.area == t.area));
     const float mina = fminf(t.qa[0], fminf(t.qa[1], t.qa[2])), maxa = fmaxf(t.qa[0], fmaxf(t.qa[1], t.qa[2]));
     const float minb = fminf(t.qb[0], fminf(t.qb[1], t.qb[2])), maxb = fmaxf(t.qb[0], fmaxf(t.qb[1], t.qb[2]));
-    t.i0 = max(0, (int)ceilf(mina - 0.5f)); t.i1 = min(sa - 1, (int)floorf(maxa - 0.5f));
-    t.j0 = max(0, (int)ceilf(minb - 0.5f)); t.j1 = min(sb - 1, (int)floorf(maxb - 0.5f));
+    if constexpr (Conservative) {
+        // every pixel whose closed square [i, i+1] x [j, j+1] meets the closed bounding box
+        t.i0 = max(0, (int)(ceilf(mina) - 1.0f)); t.i1 = min(sa - 1, (int)floorf(maxa));
+        t.j0 = max(0, (int)(ceilf(minb) - 1.0f)); t.j1 = min(sb - 1, (int)floorf(maxb));
+        cv.r[0] = 0.5f * (fabsf(t.qa[2] - t.qa[1]) + fabsf(t.qb[2] - t.qb[1]));
+        cv.r[1] = 0.5f * (fabsf(t.qa[0] - t.qa[2]) + fabsf(t.qb[0] - t.qb[2]));
+        cv.r[2] = 0.5f * (fabsf(t.qa[1] - t.qa[0]) + fabsf(t.qb[1] - t.qb[0]));
+    } else {
+        t.i0 = max(0, (int)ceilf(mina - 0.5f)); t.i1 = min(sa - 1, (int)floorf(maxa - 0.5f));
+        t.j0 = max(0, (int)ceilf(minb - 0.5f)); t.j1 = min(sb - 1, (int)floorf(maxb - 0.5f));
+    }
     t.meshId = tri.w;
     if (t.i1 < t.i0 || t.j1 < t.j0) t.valid = false;
 }
 
-// one pixel centre (i, j) of the projection plane; returns true if a voxel was written
-__device__ __forceinline__ bool vx_pixel(const VxScene& sc, const VxGridDev& g, const VxTri& t, int i, int j, uint32_t* stack) {
+// one pixel (i, j) of the projection plane: covered if its centre is inside the triangle (centre rule) or if its square meets
+// the triangle (conservative rule); attributes at the centre either way. Returns true if a voxel was written.
+template <bool Conservative>
+__device__ __forceinline__ bool vx_pixel(const VxScene& sc, const VxGridDev& g, const VxTri& t, const VxCover<Conservative>& cv, int i, int j, uint32_t* stack) {
     const float cx = (float)i + 0.5f, cy = (float)j + 0.5f;
     const float w0 = vx_edge(t.qa[1], t.qb[1], t.qa[2], t.qb[2], cx, cy);
     const float w1 = vx_edge(t.qa[2], t.qb[2], t.qa[0], t.qb[0], cx, cy);
     const float w2 = vx_edge(t.qa[0], t.qb[0], t.qa[1], t.qb[1], cx, cy);
-    const bool inside = t.area > 0.0f ? (w0 >= 0.0f && w1 >= 0.0f && w2 >= 0.0f) : (w0 <= 0.0f && w1 <= 0.0f && w2 <= 0.0f);
+    bool inside;
+    if constexpr (Conservative)
+        inside = t.area > 0.0f ? (w0 + cv.r[0] >= 0.0f && w1 + cv.r[1] >= 0.0f && w2 + cv.r[2] >= 0.0f)
+                               : (w0 - cv.r[0] <= 0.0f && w1 - cv.r[1] <= 0.0f && w2 - cv.r[2] <= 0.0f);
+    else
+        inside = t.area > 0.0f ? (w0 >= 0.0f && w1 >= 0.0f && w2 >= 0.0f) : (w0 <= 0.0f && w1 <= 0.0f && w2 <= 0.0f);
     if (!inside) return false;
     const float b0 = w0 / t.area, b1 = w1 / t.area, b2 = w2 / t.area;
     const f3 fragPos = (t.P[0] * b0 + t.P[1] * b1) + t.P[2] * b2;
@@ -196,6 +218,7 @@ struct VxVoxelizeArgs {
     unsigned long long* fragments;
 };
 
+template <bool Conservative>
 __global__ void __launch_bounds__(256) k_vx_voxelize_small(VxVoxelizeArgs a) {
     extern __shared__ uint32_t s_vxStack[];          // shadow-ray traversal stacks (only with point-shadowed lights)
     uint32_t* stack = s_vxStack + threadIdx.x;
@@ -203,12 +226,13 @@ __global__ void __launch_bounds__(256) k_vx_voxelize_small(VxVoxelizeArgs a) {
     uint32_t frags = 0;
     if (k < a.triCount) {
         VxTri t;
-        vx_setup(a.sc, a.g, a.instance, a.triFirst + k, t);
+        VxCover<Conservative> cv;
+        vx_setup(a.sc, a.g, a.instance, a.triFirst + k, t, cv);
         if (t.valid) {
             const int area = (t.i1 - t.i0 + 1) * (t.j1 - t.j0 + 1);
             if (area <= IDKVX_SMALL_LIMIT) {
                 for (int j = t.j0; j <= t.j1; j++)
-                    for (int i = t.i0; i <= t.i1; i++) frags += vx_pixel(a.sc, a.g, t, i, j, stack) ? 1u : 0u;
+                    for (int i = t.i0; i <= t.i1; i++) frags += vx_pixel(a.sc, a.g, t, cv, i, j, stack) ? 1u : 0u;
             } else {
                 // cut the bounding box into tiles and queue one work item per tile (a wall-sized triangle becomes
                 // dozens of CTAs instead of one); if the queue is full the thread rasterises the remainder itself
@@ -221,7 +245,7 @@ __global__ void __launch_bounds__(256) k_vx_voxelize_small(VxVoxelizeArgs a) {
                     } else {
                         const int i0 = t.i0 + ox * IDKVX_TILE, j0 = t.j0 + oy * IDKVX_TILE;
                         for (int j = j0; j <= min(t.j1, j0 + IDKVX_TILE - 1); j++)
-                            for (int i = i0; i <= min(t.i1, i0 + IDKVX_TILE - 1); i++) frags += vx_pixel(a.sc, a.g, t, i, j, stack) ? 1u : 0u;
+                            for (int i = i0; i <= min(t.i1, i0 + IDKVX_TILE - 1); i++) frags += vx_pixel(a.sc, a.g, t, cv, i, j, stack) ? 1u : 0u;
                     }
                 }
             }
@@ -231,7 +255,8 @@ __global__ void __launch_bounds__(256) k_vx_voxelize_small(VxVoxelizeArgs a) {
     if ((threadIdx.x & 31) == 0 && frags) atomicAdd(a.fragments, (unsigned long long)frags);
 }
 
-// one CTA per queued (triangle, tile) work item, threads stride over the tile's pixel centres
+// one CTA per queued (triangle, tile) work item, threads stride over the tile's pixels
+template <bool Conservative>
 __global__ void __launch_bounds__(256) k_vx_voxelize_large(VxScene sc, VxGridDev g, const uint4* __restrict__ queue,
                                                            const uint32_t* __restrict__ queueCount, uint32_t queueCapacity,
                                                            unsigned long long* fragments) {
@@ -242,11 +267,12 @@ __global__ void __launch_bounds__(256) k_vx_voxelize_large(VxScene sc, VxGridDev
     for (uint32_t q = blockIdx.x; q < n; q += gridDim.x) {
         const uint4 e = queue[q];
         VxTri t;
-        vx_setup(sc, g, e.x, e.y, t);
+        VxCover<Conservative> cv;
+        vx_setup(sc, g, e.x, e.y, t, cv);
         const int i0 = t.i0 + (int)e.z * IDKVX_TILE, j0 = t.j0 + (int)e.w * IDKVX_TILE;
         const int w = min(t.i1, i0 + IDKVX_TILE - 1) - i0 + 1, h = min(t.j1, j0 + IDKVX_TILE - 1) - j0 + 1;
         for (int p = threadIdx.x; p < w * h; p += blockDim.x)
-            frags += vx_pixel(sc, g, t, i0 + p % w, j0 + p / w, stack) ? 1u : 0u;
+            frags += vx_pixel(sc, g, t, cv, i0 + p % w, j0 + p / w, stack) ? 1u : 0u;
     }
     for (int off = 16; off > 0; off >>= 1) frags += __shfl_down_sync(0xffffffffu, frags, off);
     if ((threadIdx.x & 31) == 0 && frags) atomicAdd(fragments, (unsigned long long)frags);

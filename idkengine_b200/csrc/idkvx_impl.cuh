@@ -32,6 +32,7 @@ struct IdkVxCtx : IdkCtxBase {
     // between); cleared by idkvx_set_grid, idkvx_set_scene and idkvx_set_slab
     bool voxelized = false;
     bool slabVoxelized = false;           // idkvx_voxelize ran in slab mode since the grid last changed
+    bool conservative = false;            // idkvx_set_conservative_rasterization: coverage rule of the next idkvx_voxelize
 };
 
 static void set_grid_bounds(IdkVxCtx* ctx, const float* mn, const float* mx) {
@@ -182,6 +183,10 @@ IDKPT_API int idkvx_voxelize(IdkVxCtx* ctx, IdkVxStats* stats) {
     // map. With shadow maps attached that lookup runs on the path tracer's traced cube maps (idkvx_set_shadow_maps); otherwise
     // the same question -- is the (2 % biased) sample point visible from the light -- is answered by an any-hit shadow ray
     // through the path tracer's BVH (idkvx_set_shadow_tracer).
+    // Voxelizer.IsConservativeRasterization picks the coverage rule: pixel centres, or every pixel the triangle touches
+    void (*const small)(VxVoxelizeArgs) = ctx->conservative ? k_vx_voxelize_small<true> : k_vx_voxelize_small<false>;
+    void (*const large)(VxScene, VxGridDev, const uint4*, const uint32_t*, uint32_t, unsigned long long*) =
+        ctx->conservative ? k_vx_voxelize_large<true> : k_vx_voxelize_large<false>;
     size_t shadowSmem = 0;
     ctx->sc.occValid = 0;
     ctx->sc.psmValid = 0;
@@ -203,8 +208,8 @@ IDKPT_API int idkvx_voxelize(IdkVxCtx* ctx, IdkVxStats* stats) {
         ctx->sc.occ = pt->sc;
         ctx->sc.occValid = 1;
         shadowSmem = pt->stackBytes;
-        CK(cudaFuncSetAttribute(k_vx_voxelize_small, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)shadowSmem));
-        CK(cudaFuncSetAttribute(k_vx_voxelize_large, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)shadowSmem));
+        CK(cudaFuncSetAttribute(small, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)shadowSmem));
+        CK(cudaFuncSetAttribute(large, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)shadowSmem));
     }
     CK(cudaSetDevice(ctx->device));
     if (stats) memset(stats, 0, sizeof(*stats));
@@ -223,11 +228,11 @@ IDKPT_API int idkvx_voxelize(IdkVxCtx* ctx, IdkVxStats* stats) {
             a.triFirst = (uint32_t)d.TriangleOffset; a.triCount = (uint32_t)d.TriangleCount;
             a.queue = (uint4*)ctx->queue.p; a.queueCount = (uint32_t*)ctx->queueCount.p; a.queueCapacity = (uint32_t)ctx->queueCapacity;
             a.fragments = (unsigned long long*)ctx->counters.p;
-            k_vx_voxelize_small<<<(a.triCount + 255) / 256, 256, shadowSmem, ctx->stream>>>(a);
+            small<<<(a.triCount + 255) / 256, 256, shadowSmem, ctx->stream>>>(a);
             launches++;
         }
-        k_vx_voxelize_large<<<ctx->smCount * 8, 256, shadowSmem, ctx->stream>>>(ctx->sc, ctx->grid, (const uint4*)ctx->queue.p, (const uint32_t*)ctx->queueCount.p,
-                                                                         (uint32_t)ctx->queueCapacity, (unsigned long long*)ctx->counters.p);
+        large<<<ctx->smCount * 8, 256, shadowSmem, ctx->stream>>>(ctx->sc, ctx->grid, (const uint4*)ctx->queue.p, (const uint32_t*)ctx->queueCount.p,
+                                                           (uint32_t)ctx->queueCapacity, (unsigned long long*)ctx->counters.p);
         launches++;
         CK(cudaEventRecord(ctx->timing[3], ctx->stream));
         if (!ctx->slabMode) launches += launch_mips(ctx);
@@ -279,6 +284,13 @@ IDKPT_API int idkvx_mipmap(IdkVxCtx* ctx, IdkVxStats* stats) {
     if (rc == IDKPT_OK && stats) stats->KernelLaunches = launches;
     if (rc == IDKPT_OK && ctx->slabVoxelized) ctx->voxelized = true;
     return rc;
+}
+
+IDKPT_API int idkvx_set_conservative_rasterization(IdkVxCtx* ctx, int32_t enable) {
+    if (!ctx) return IDKPT_ERR_INVALID_ARGUMENT;
+    if (enable != 0 && enable != 1) return fail(ctx, IDKPT_ERR_INVALID_ARGUMENT, "idkvx_set_conservative_rasterization: enable must be 0 or 1");
+    ctx->conservative = enable == 1;   // takes effect at the next idkvx_voxelize; the current grid is left as it is
+    return IDKPT_OK;
 }
 
 IDKPT_API int idkvx_set_shadow_tracer(IdkVxCtx* ctx, IdkPtCtx* pathTracer) {

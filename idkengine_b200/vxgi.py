@@ -26,7 +26,8 @@ class IdkVxStats(ctypes.Structure):
 
 VX_EXPORTS = ["idkvx_create", "idkvx_destroy", "idkvx_last_error", "idkvx_set_scene", "idkvx_set_grid", "idkvx_level_count",
               "idkvx_voxelize", "idkvx_read_level", "idkvx_cone_trace", "idkvx_set_shadow_tracer",
-              "idkvx_set_shadow_maps", "idkvx_set_slab", "idkvx_level_device_ptr", "idkvx_mipmap", "idkvx_cone_trace_rows"]
+              "idkvx_set_shadow_maps", "idkvx_set_slab", "idkvx_level_device_ptr", "idkvx_mipmap", "idkvx_cone_trace_rows",
+              "idkvx_set_conservative_rasterization"]
 
 DEFAULT_GRID_MIN = (-28.0, -3.0, -17.0)   # RasterPipeline.cs:213
 DEFAULT_GRID_MAX = (28.0, 20.0, 17.0)
@@ -69,6 +70,8 @@ def _declare(L):
     L.idkvx_level_count.argtypes = [c_vp]
     L.idkvx_voxelize.restype = c_i32
     L.idkvx_voxelize.argtypes = [c_vp, P(IdkVxStats)]
+    L.idkvx_set_conservative_rasterization.restype = c_i32
+    L.idkvx_set_conservative_rasterization.argtypes = [c_vp, c_i32]
     L.idkvx_set_slab.restype = c_i32
     L.idkvx_set_slab.argtypes = [c_vp, c_i32, c_i32]
     L.idkvx_level_device_ptr.restype = c_i32
@@ -101,6 +104,7 @@ class Voxelizer:
         if rc != 0:
             raise IdkVxError(f"idkvx_create failed ({rc}): {(self._lib.idkvx_last_error(None) or b'').decode()}")
         self.sizes = level_sizes(self.ci)
+        self._conservative = False
 
     def _check(self, rc, what):
         if rc != 0:
@@ -121,6 +125,10 @@ class Voxelizer:
         d, keep = capi.scene_desc(scene)
         self._check(self._lib.idkvx_set_scene(self._ctx, ctypes.byref(d)), "idkvx_set_scene")
 
+    def SetGrid(self, grid_min, grid_max):
+        """Voxelizer.GridMin / GridMax setters (Voxelizer.cs:16-33); the next Render voxelises the new bounds."""
+        self._check(self._lib.idkvx_set_grid(self._ctx, ctypes.byref((c_f * 3)(*grid_min)), ctypes.byref((c_f * 3)(*grid_max))), "idkvx_set_grid")
+
     def SetShadowTracer(self, path_tracer):
         """Shadow rays for lights with PointShadowIndex >= 0 go through this PathTracer's scene (None detaches)."""
         self._check(self._lib.idkvx_set_shadow_tracer(self._ctx, path_tracer._ctx if path_tracer is not None else None), "idkvx_set_shadow_tracer")
@@ -129,6 +137,19 @@ class Voxelizer:
         """Lights with PointShadowIndex >= 0 are filtered through this PathTracer's point-shadow cube maps (PCF lookup;
         SetPointShadows / RenderPointShadows). Takes precedence over SetShadowTracer; None detaches."""
         self._check(self._lib.idkvx_set_shadow_maps(self._ctx, path_tracer._ctx if path_tracer is not None else None), "idkvx_set_shadow_maps")
+
+    @property
+    def IsConservativeRasterization(self):
+        """Voxelizer.IsConservativeRasterization (Voxelizer.cs:41-56): False = a triangle writes the voxels of the pixel centres
+        it covers; True = of every pixel it touches (thin geometry without gaps). Applies from the next Render on."""
+        return self._conservative
+
+    @IsConservativeRasterization.setter
+    def IsConservativeRasterization(self, value):
+        if not isinstance(value, (bool, np.bool_)):
+            raise TypeError("IsConservativeRasterization is a bool")
+        self._check(self._lib.idkvx_set_conservative_rasterization(self._ctx, int(bool(value))), "idkvx_set_conservative_rasterization")
+        self._conservative = bool(value)
 
     # ---- multi-GPU: z-slab voxelisation, gather, mip chain, screen-tiled cone trace (include/idkvx.h)
     def SetSlab(self, z0, z1):

@@ -356,6 +356,10 @@ public:
     void SetGrid(const float gridMin[3], const float gridMax[3]) { check(idkvx_set_grid(ctx_, gridMin, gridMax), "idkvx_set_grid"); }   // GridMin / GridMax setters
     int LevelCount() const { return idkvx_level_count(ctx_); }
     IdkVxStats Render() { IdkVxStats st = {}; check(idkvx_voxelize(ctx_, &st), "idkvx_voxelize"); return st; }
+    // IsConservativeRasterization setter: every pixel a triangle touches instead of the pixel centres it covers, from the next Render on
+    void SetConservativeRasterization(bool enable) {
+        check(idkvx_set_conservative_rasterization(ctx_, enable ? 1 : 0), "idkvx_set_conservative_rasterization");
+    }
     // point-shadowed lights: PCF lookup into a path tracer's cube maps, or shadow rays through its BVH (idkvx.h); nullptr detaches
     void SetShadowMaps(const PathTracer* pt) { check(idkvx_set_shadow_maps(ctx_, pt ? pt->Handle() : nullptr), "idkvx_set_shadow_maps"); }
     void SetShadowTracer(const PathTracer* pt) { check(idkvx_set_shadow_tracer(ctx_, pt ? pt->Handle() : nullptr), "idkvx_set_shadow_tracer"); }

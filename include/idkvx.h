@@ -10,7 +10,10 @@
  *
  * The reference voxelises with the GL rasteriser (one draw per dominant axis via NV passthrough geometry shader +
  * viewport swizzle, Voxelize/geometry.glsl); this library rasterises the same projection in a compute kernel
- * (pixel-centre coverage, DESIGN.md section 8), which matches GL to tolerance and its own CPU oracle bit for bit.
+ * (pixel-centre coverage, DESIGN.md section 8), which matches GL to tolerance and its own CPU oracle bit for bit. The engine's
+ * conservative-raster option (Voxelizer.IsConservativeRasterization, GL_NV_conservative_raster) is built too:
+ * idkvx_set_conservative_rasterization switches the kernels to an exact square-against-triangle coverage test (DESIGN.md
+ * section 7).
  * Same conventions as idkpt.h: status codes, idkvx_last_error, borrowed host arrays, no CPU fallback.
  */
 #ifndef IDKVX_H
@@ -65,6 +68,14 @@ IDKPT_API int32_t idkvx_level_count(IdkVxCtx* ctx);                             
 
 /* Voxelizer.Render(): clear + voxelise + mip chain. */
 IDKPT_API int idkvx_voxelize(IdkVxCtx* ctx, IdkVxStats* stats);
+
+/* Voxelizer.IsConservativeRasterization (Voxelizer.cs:41-56,142): 0 (the default after idkvx_create) = a triangle covers the
+ * pixels whose centre it contains; 1 = it covers every pixel whose closed square it touches, with attributes extrapolated to
+ * the pixel centre, so that geometry thinner than a voxel voxelises without gaps (DESIGN.md section 7). `enable` other than
+ * 0 or 1 fails with IDKPT_ERR_INVALID_ARGUMENT and leaves the setting as it was. The setting belongs to the context: it
+ * survives idkvx_set_scene / idkvx_set_grid / idkvx_set_slab, applies from the next idkvx_voxelize on, and does not touch
+ * the current grid. */
+IDKPT_API int idkvx_set_conservative_rasterization(IdkVxCtx* ctx, int32_t enable);
 
 /* rgba16f texels of one mip level, x fastest (size = w*h*d*8 bytes). */
 /* Lights with PointShadowIndex >= 0 are attenuated by Visibility() in the fragment stage (Voxelize/fragment.glsl:55-58,100-117),
