@@ -56,6 +56,15 @@ class IdkPtSkyDesc(ctypes.Structure):
     _fields_ = [("Color", c_f * 3), ("FaceSize", c_i32), ("Faces", c_vp * 6)]
 
 
+class IdkPtAtmosphereSettings(ctypes.Structure):
+    _fields_ = [("ISteps", c_i32), ("JSteps", c_i32), ("LightIntensity", c_f), ("Azimuth", c_f), ("Elevation", c_f)]
+
+
+def default_atmosphere_settings():
+    """AtmosphericScatterer.GpuSettings defaults (AtmosphericScatterer.cs:9-20): 40 x 8 steps, intensity 15, sun at the zenith."""
+    return IdkPtAtmosphereSettings(40, 8, 15.0, 0.0, 0.0)
+
+
 class IdkPtSettings(ctypes.Structure):
     _fields_ = [("Gpu", IdkPtGpuSettings), ("RayDepth", c_i32), ("SamplesPerPixel", c_i32),
                 ("DoRaySorting", c_i32), ("OutputAOVs", c_i32), ("CollectStats", c_i32)]
@@ -102,6 +111,7 @@ EXPORTS = [
     "idkpt_ssr", "idkpt_ssr_device_ptrs", "idkpt_taa_resolve", "idkpt_taa_device_ptr",
     "idkpt_shading_rate", "idkpt_shading_rate_device_ptr",
     "idkpt_gbuffer", "idkpt_gbuffer_device_ptrs", "idkpt_read_gbuffer", "idkpt_transparency", "idkpt_lights_and_skybox",
+    "idkpt_sky_atmosphere", "idkpt_sky_equirectangular", "idkpt_read_sky",
 ]
 
 IDKPT_MAX_POINT_SHADOWS = 128
@@ -330,6 +340,12 @@ def load(path=None):
     L.idkpt_update_range.argtypes = [c_vp, c_i32, c_u64, c_u64, c_vp]
     L.idkpt_set_sky.restype = c_i32
     L.idkpt_set_sky.argtypes = [c_vp, P(IdkPtSkyDesc)]
+    L.idkpt_sky_atmosphere.restype = c_i32
+    L.idkpt_sky_atmosphere.argtypes = [c_vp, P(IdkPtAtmosphereSettings), c_i32, P(c_f)]
+    L.idkpt_sky_equirectangular.restype = c_i32
+    L.idkpt_sky_equirectangular.argtypes = [c_vp, c_vp, c_i32, c_i32, P(c_f)]
+    L.idkpt_read_sky.restype = c_i32
+    L.idkpt_read_sky.argtypes = [c_vp, P(c_i32), c_vp, c_u64]
     L.idkpt_resize.restype = c_i32
     L.idkpt_resize.argtypes = [c_vp, c_i32, c_i32]
     L.idkpt_reset_accumulation.restype = c_i32

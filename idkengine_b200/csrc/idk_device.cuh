@@ -83,6 +83,39 @@ __device__ __forceinline__ float det_log2(float x) {
     return (m + y) * 1.44269504f + (float)e;
 }
 
+// ---- deterministic atan2 / asin (DESIGN.md 8f.1j): Cephes atanf / asinf polynomials, no libm call
+// atan of t in [0, 1]: reduced to |r| <= tan(pi/8) around 0 or pi/4, then the odd degree-9 polynomial.
+__device__ __forceinline__ float det_atan01(float t) {
+    float base = 0.0f;
+    if (t > 0.41421356f) { t = (t - 1.0f) / (t + 1.0f); base = 0.78539816f; }
+    const float z = t * t;
+    return base + ((((8.05374449538e-2f * z - 1.38776856032e-1f) * z + 1.99777106478e-1f) * z - 3.33329491539e-1f) * z * t + t);
+}
+// C's atan2 on the signed zeros: atan2(+-0, +0) = +-0, atan2(+-0, -0) = +-pi, atan2(y != 0, +-0) = +-pi/2; NaN propagates.
+__device__ __forceinline__ float det_atan2(float y, float x) {
+    if (x != x || y != y) return x + y;
+    const float ax = fabsf(x), ay = fabsf(y);
+    float a;
+    if (ay == 0.0f) a = 0.0f;
+    else if (ay <= ax) a = det_atan01(ay / ax);
+    else a = 1.57079637f - det_atan01(ax / ay);
+    if (signbit(x)) a = 3.14159274f - a;
+    return copysignf(a, y);
+}
+// asin on [-1, 1] (NaN outside): x itself below 1e-4; z = x^2 up to 0.5, else pi/2 - 2 asin(sqrt((1 - |x|) / 2)).
+__device__ __forceinline__ float det_asin(float x) {
+    const float a = fabsf(x);
+    if (a > 1.0f) return __int_as_float(0x7fffffff);
+    if (a < 1e-4f) return x;
+    float z, s;
+    const bool big = a > 0.5f;
+    if (big) { z = 0.5f * (1.0f - a); s = sqrtf(z); }
+    else { z = a * a; s = a; }
+    float p = ((((4.2163199048e-2f * z + 2.4181311049e-2f) * z + 4.5470025998e-2f) * z + 7.4953002686e-2f) * z + 1.6666752422e-1f) * z * s + s;
+    if (big) p = 1.57079637f - (p + p);
+    return copysignf(p, x);
+}
+
 // One 2-D RGBA8 texture, base level only: compute shaders sample lod 0 (Surface.glsl:57-60).
 struct TexRec {
     const void* px;               // decoded level 0: uchar4 (kind 0), float2 (1), float (2) or float4 (3) texels

@@ -25,6 +25,7 @@
 #include "idk_gbuffer.cuh"
 #include "idk_transparency.cuh"
 #include "idk_lights_skybox.cuh"
+#include "idk_sky.cuh"
 #include "idk_textures_host.h"
 
 #define IDKPT_ABI_VERSION 4u   // 2: IdkPtSceneDesc gained Textures / TextureCount; 3: IdkPtStats gained CompactMs / AccumulateMs, host-buffer registration;
@@ -877,6 +878,94 @@ IDKPT_API int idkpt_set_sky(IdkPtCtx* ctx, const IdkPtSkyDesc* sky) {
     return IDKPT_OK;
 }
 
+} // extern "C"
+
+// ---- the sky generated on the device (SkyBoxManager: AtmosphericScatterer.Compute, LoadSkyBoxEquirectangular) -----------------
+// Runs `launch(faces)` over the 6 x n x n grid into the sky's allocation when it is large enough, else into a new one that
+// replaces it only once the kernel has succeeded, then leaves the context as idkpt_set_sky would with those faces.
+template <class Launch>
+static int sky_generate(IdkPtCtx* ctx, const char* who, int n, float* kernelMs, Launch&& launch) {
+    const size_t bytes = 6 * (size_t)n * n * 16;
+    DevBuf fresh;
+    if (bytes > ctx->skyFaces.bytes && ensure(fresh, bytes) != cudaSuccess) {
+        release(fresh);
+        return fail(ctx, who, IDKPT_ERR_OUT_OF_MEMORY, "device allocation failed");
+    }
+    float4* faces = (float4*)(fresh.p ? fresh.p : ctx->skyFaces.p);
+    const dim3 grid((unsigned)((n + 7) / 8), (unsigned)((n + 7) / 8), 6), block(8, 8);
+    const int rc = run_timed(ctx, who, kernelMs, [&]() -> int { launch(grid, block, faces); return IDKPT_OK; });
+    if (rc != IDKPT_OK) { release(fresh); return rc; }
+    if (fresh.p) { release(ctx->skyFaces); ctx->skyFaces = fresh; }
+    ctx->skyFaceSize = n;
+    ctx->sc.skyFaces = (const float4*)ctx->skyFaces.p;
+    ctx->sc.skyFaceSize = n;
+    ctx->accumulatedSamples = 0;
+    return IDKPT_OK;
+}
+
+extern "C" {
+
+IDKPT_API int idkpt_sky_atmosphere(IdkPtCtx* ctx, const IdkPtAtmosphereSettings* s, int32_t faceSize, float* kernelMs) {
+    static const char* who = "idkpt_sky_atmosphere";
+    if (!ctx || !s) return fail(ctx, IDKPT_ERR_INVALID_ARGUMENT, "idkpt_sky_atmosphere: null argument");
+    DRAIN_PENDING(who);
+    if (faceSize < 1 || faceSize > 8192) return fail(ctx, who, IDKPT_ERR_INVALID_ARGUMENT, "face size outside 1..8192");
+    if (s->ISteps < 1 || s->ISteps > 1024 || s->JSteps < 1 || s->JSteps > 1024)
+        return fail(ctx, who, IDKPT_ERR_INVALID_ARGUMENT, "ISteps or JSteps outside 1..1024");
+    if (!std::isfinite(s->LightIntensity) || !std::isfinite(s->Azimuth) || !std::isfinite(s->Elevation))
+        return fail(ctx, who, IDKPT_ERR_INVALID_ARGUMENT, "a setting is not finite");
+    CK(cudaSetDevice(ctx->device));
+    if (kernelMs) *kernelMs = 0.0f;
+    SkyAtmosphereArgs a;
+    a.n = faceSize;
+    a.iSteps = s->ISteps; a.jSteps = s->JSteps;
+    a.lightIntensity = std::max(s->LightIntensity, 0.0f);   // AtmosphericScatterer.Compute
+    a.azimuth = s->Azimuth; a.elevation = s->Elevation;
+    return sky_generate(ctx, who, faceSize, kernelMs, [&](dim3 grid, dim3 block, float4* faces) {
+        a.faces = faces;
+        k_sky_atmosphere<<<grid, block, 0, ctx->stream>>>(a);
+    });
+}
+
+IDKPT_API int idkpt_sky_equirectangular(IdkPtCtx* ctx, const float* rgb, int32_t width, int32_t height, float* kernelMs) {
+    static const char* who = "idkpt_sky_equirectangular";
+    if (!ctx || !rgb) return fail(ctx, IDKPT_ERR_INVALID_ARGUMENT, "idkpt_sky_equirectangular: null argument");
+    DRAIN_PENDING(who);
+    if (width < 4 || height < 1 || width / 4 > 8192)
+        return fail(ctx, who, IDKPT_ERR_INVALID_ARGUMENT, "width outside 4..32771 (face size width / 4 in 1..8192) or height below 1");
+    CK(cudaSetDevice(ctx->device));
+    if (kernelMs) *kernelMs = 0.0f;
+    const size_t srcBytes = (size_t)width * height * 12;
+    DevBuf src;                    // the source lives for this call only: an import is a one-off, and it can be large
+    if (ensure(src, srcBytes) != cudaSuccess) { release(src); return fail(ctx, who, IDKPT_ERR_OUT_OF_MEMORY, "device allocation failed"); }
+    cudaError_t e = cudaMemcpyAsync(src.p, rgb, srcBytes, cudaMemcpyHostToDevice, ctx->stream);
+    if (e != cudaSuccess) { release(src); return fail(ctx, who, IDKPT_ERR_CUDA, cudaGetErrorString(e)); }
+    SkyEquirectArgs a;
+    a.rgb = (const float*)src.p;
+    a.w = width; a.h = height;
+    a.n = width / 4;               // SkyBoxManager.cs:124
+    const int rc = sky_generate(ctx, who, a.n, kernelMs, [&](dim3 grid, dim3 block, float4* faces) {
+        a.faces = faces;
+        k_sky_equirect<<<grid, block, 0, ctx->stream>>>(a);
+    });
+    release(src);                  // run_timed synchronised the stream (or the call failed)
+    return rc;
+}
+
+IDKPT_API int idkpt_read_sky(IdkPtCtx* ctx, int32_t* faceSize, float* dst, uint64_t bytes) {
+    if (!ctx || !faceSize) return fail(ctx, IDKPT_ERR_INVALID_ARGUMENT, "idkpt_read_sky: null argument");
+    DRAIN_PENDING("idkpt_read_sky");
+    const uint64_t need = 6 * (uint64_t)ctx->skyFaceSize * (uint64_t)ctx->skyFaceSize * 16;
+    if (dst && bytes < need) return fail(ctx, IDKPT_ERR_INVALID_ARGUMENT, "idkpt_read_sky: buffer smaller than 6 * FaceSize^2 * 16 bytes");
+    *faceSize = ctx->skyFaceSize;
+    if (dst && need) {
+        CK(cudaSetDevice(ctx->device));
+        CK(cudaMemcpyAsync(dst, ctx->skyFaces.p, need, cudaMemcpyDeviceToHost, ctx->stream));
+        CK(cudaStreamSynchronize(ctx->stream));
+    }
+    return IDKPT_OK;
+}
+
 // Replaces the texture table (SURVEY 8b idkpt_set_textures): e.g. streamed-in higher-resolution images. Handles already
 // stored in the materials must stay valid.
 IDKPT_API int idkpt_set_textures(IdkPtCtx* ctx, const IdkPtTextureDesc* textures, uint64_t count) {
@@ -1403,6 +1492,7 @@ static int preload_kernels(IdkPtCtx* ctx) {
     IDK_PRELOAD(k_ssao); IDK_PRELOAD(k_deferred_lighting); IDK_PRELOAD(k_ssr); IDK_PRELOAD(k_taa_resolve);
     IDK_PRELOAD(k_shading_rate); IDK_PRELOAD(k_vrs_scan); IDK_PRELOAD(k_deferred_lighting_vrs); IDK_PRELOAD(k_gbuffer);
     IDK_PRELOAD(k_transparency<false>); IDK_PRELOAD(k_transparency<true>); IDK_PRELOAD(k_lights_skybox);
+    IDK_PRELOAD(k_sky_atmosphere); IDK_PRELOAD(k_sky_equirect);
 #undef IDK_PRELOAD
     return IDKPT_OK;
 }

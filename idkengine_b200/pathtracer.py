@@ -151,6 +151,35 @@ class PathTracer:
         s = capi.sky_desc(color, faces)
         self._check(self._lib.idkpt_set_sky(self._ctx, ctypes.byref(s)), "idkpt_set_sky")
 
+    def SkyAtmosphere(self, settings=None, face_size=128):
+        """AtmosphericScatterer.Compute on the device into the context's sky (DESIGN.md 8f.1j). settings:
+        capi.IdkPtAtmosphereSettings (default: the engine's); face_size 128 is the engine's. Returns kernel ms."""
+        st = settings if settings is not None else capi.default_atmosphere_settings()
+        ms = ctypes.c_float()
+        self._check(self._lib.idkpt_sky_atmosphere(self._ctx, ctypes.byref(st), int(face_size), ctypes.byref(ms)), "idkpt_sky_atmosphere")
+        return ms.value
+
+    def SkyEquirectangular(self, rgb):
+        """SkyBoxManager.LoadSkyBoxEquirectangular's unprojection on the device: rgb float32 [H, W, 3], row 0 first (what
+        ImageLoader.Load(path, RGB, true) returns) -> faces of size W // 4 in the context's sky. Returns kernel ms."""
+        img = np.ascontiguousarray(rgb, np.float32)
+        if img.ndim != 3 or img.shape[2] != 3:
+            raise ValueError("SkyEquirectangular: rgb must be [H, W, 3]")
+        ms = ctypes.c_float()
+        self._check(self._lib.idkpt_sky_equirectangular(self._ctx, img.ctypes.data, img.shape[1], img.shape[0], ctypes.byref(ms)),
+                    "idkpt_sky_equirectangular")
+        return ms.value
+
+    def read_sky(self):
+        """The context's sky faces, float32 [6, n, n, 4] (+X,-X,+Y,-Y,+Z,-Z), or None for a constant sky."""
+        n = ctypes.c_int32()
+        self._check(self._lib.idkpt_read_sky(self._ctx, ctypes.byref(n), None, 0), "idkpt_read_sky")
+        if n.value == 0:
+            return None
+        faces = np.empty((6, n.value, n.value, 4), np.float32)
+        self._check(self._lib.idkpt_read_sky(self._ctx, ctypes.byref(n), faces.ctypes.data, faces.nbytes), "idkpt_read_sky")
+        return faces
+
     def SetFrame(self, per_frame_data):
         """GpuPerFrameData (UBO 1). A changed camera resets the accumulation like Application.OnRender does
         (SRC/Application.cs:209-213)."""

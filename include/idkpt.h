@@ -206,6 +206,28 @@ IDKPT_API const char* idkpt_last_error(IdkPtCtx* ctx);                        /*
 IDKPT_API int idkpt_set_scene(IdkPtCtx* ctx, const IdkPtSceneDesc* scene);    /* ModelManager.Add -> UpdateBuffers + BVH.BlasesBuild uploads (ModelManager.cs:207-213, BVH.cs:445-451) */
 IDKPT_API int idkpt_update_range(IdkPtCtx* ctx, IdkPtArrayId which, uint64_t first, uint64_t count, const void* data); /* dirty-range uploads, ModelManager.cs:236-261; LightManager.cs:363-380 */
 IDKPT_API int idkpt_set_sky(IdkPtCtx* ctx, const IdkPtSkyDesc* sky);
+
+/* ---- the sky generated on the device (SkyBoxManager's two compute passes; DESIGN.md 8f.1j) ----
+ * Both write the context's sky in place, in the layout idkpt_set_sky fills, and leave the context as idkpt_set_sky would with
+ * those faces: the face size changes, Color is kept, the accumulation is reset. No scene is needed. Every argument is checked
+ * before anything is launched, so a failed call changes no byte of the sky. They are synchronous and ordered after the samples
+ * idkpt_compute has queued. kernel_ms (may be NULL): the kernel's CUDA-event time.
+ * idkpt_sky_atmosphere: AtmosphericScattering/compute.glsl (the engine's default sky, 128^2) at face_size 1..8192; ISteps and
+ *   JSteps 1..1024, every setting finite; LightIntensity is clamped to >= 0 as AtmosphericScatterer.Compute does.
+ * idkpt_sky_equirectangular: UnprojectEquirectangular/compute.glsl over a host image of width*height*3 floats, row 0 first
+ *   (ImageLoader.Load(path, RGB, true)), uploaded as RGB16F; face size width / 4 (integer division), width 4..32771, height >= 1.
+ *   The faces hold RGBA16F values (alpha 1).
+ * idkpt_read_sky: the face size (0 for a constant sky) and, when dst is not NULL, the 6 * n^2 * 16 bytes of the faces. */
+typedef struct IdkPtAtmosphereSettings {   /* AtmosphericScatterer.GpuSettings (AtmosphericScatterer.cs:9-20) */
+    int32_t ISteps;          /* 40 */
+    int32_t JSteps;          /* 8 */
+    float   LightIntensity;  /* 15 */
+    float   Azimuth;         /* 0 */
+    float   Elevation;       /* 0 = sun at the zenith (PolarToCartesian, Math.glsl:139-153) */
+} IdkPtAtmosphereSettings;
+IDKPT_API int idkpt_sky_atmosphere(IdkPtCtx* ctx, const IdkPtAtmosphereSettings* settings, int32_t face_size, float* kernel_ms);
+IDKPT_API int idkpt_sky_equirectangular(IdkPtCtx* ctx, const float* rgb, int32_t width, int32_t height, float* kernel_ms);
+IDKPT_API int idkpt_read_sky(IdkPtCtx* ctx, int32_t* face_size, float* dst_rgba32f, uint64_t bytes);
 /* Replace the material texture table of the current scene (same rules as IdkPtSceneDesc.Textures); every handle stored in
  * a material must remain inside the new table. Resets the accumulation. */
 IDKPT_API int idkpt_set_textures(IdkPtCtx* ctx, const IdkPtTextureDesc* textures, uint64_t count);

@@ -126,6 +126,28 @@ public:
     void UpdateRange(IdkPtArrayId which, uint64_t first, uint64_t count, const void* data) { check(idkpt_update_range(ctx_, which, first, count, data), "idkpt_update_range"); }
     void SetTextures(const IdkPtTextureDesc* textures, uint64_t count) { check(idkpt_set_textures(ctx_, textures, count), "idkpt_set_textures"); }
     void SetSky(const IdkPtSkyDesc& sky) { check(idkpt_set_sky(ctx_, &sky), "idkpt_set_sky"); }
+    // The sky generated on the device (DESIGN.md 8f.1j): AtmosphericScatterer.Compute at faceSize (the engine's is 128), or the
+    // unprojection of an equirectangular RGB float image (width * height * 3, row 0 first) at face size width / 4.
+    // Each returns the kernel time in ms.
+    float SkyAtmosphere(const IdkPtAtmosphereSettings& settings, int32_t faceSize = 128) {
+        float ms = 0.0f;
+        check(idkpt_sky_atmosphere(ctx_, &settings, faceSize, &ms), "idkpt_sky_atmosphere");
+        return ms;
+    }
+    float SkyEquirectangular(const float* rgb, int32_t width, int32_t height) {
+        float ms = 0.0f;
+        check(idkpt_sky_equirectangular(ctx_, rgb, width, height, &ms), "idkpt_sky_equirectangular");
+        return ms;
+    }
+    // The sky's faces, 6 * n * n rgba32f (+X,-X,+Y,-Y,+Z,-Z); empty for a constant sky.
+    std::vector<float> ReadSky(int32_t* faceSize = nullptr) const {
+        int32_t n = 0;
+        check(idkpt_read_sky(ctx_, &n, nullptr, 0), "idkpt_read_sky");
+        std::vector<float> faces((size_t)6 * n * n * 4);
+        if (n) check(idkpt_read_sky(ctx_, &n, faces.data(), faces.size() * sizeof(float)), "idkpt_read_sky");
+        if (faceSize) *faceSize = n;
+        return faces;
+    }
 
     // ---- presentation / interop -------------------------------------------------------------------------------------------
     void PresentAsync(void* pinnedHostRgba32f, uint64_t bytes, IdkPtImage which = IDKPT_IMAGE_RESULT) { check(idkpt_present_async(ctx_, which, pinnedHostRgba32f, bytes), "idkpt_present_async"); }
