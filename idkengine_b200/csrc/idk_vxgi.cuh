@@ -3,6 +3,7 @@
 //   k_vx_voxelize_small / k_vx_voxelize_large   Voxelize/{vertex,geometry,fragment}.glsl + MergeIntermediates
 //   k_vx_mipmap                                 Voxelize/Mipmap/compute.glsl
 //   k_vx_cone_trace                             VXGI/ConeTraceGI/** + include/TraceCone.glsl
+//   k_vx_debug_bricks / _dilate / _render       VXGI/Voxelize/DebugVisualization/compute.glsl (Voxelizer.DebugRender)
 //
 // Rasterisation rule, filtering rule and float semantics are spelled out in DESIGN.md section 8 and implemented
 // independently by the CPU oracle (oracle/oracle_vxgi.inc); the two agree bit for bit.
@@ -465,6 +466,162 @@ __global__ void __launch_bounds__(64) k_vx_cone_trace(VxConeArgs a) {
 #undef VX_SKY
             a.out[p] = make_float4(irradiance.x * a.giBoost, irradiance.y * a.giBoost, irradiance.z * a.giBoost, 1.0f);
         }
+    }
+    for (int off = 16; off > 0; off >>= 1) steps += __shfl_down_sync(0xffffffffu, steps, off);
+    if (((threadIdx.y * 8 + threadIdx.x) & 31) == 0 && steps) atomicAdd(a.steps, (unsigned long long)steps);
+}
+
+// ------------------------------------------------------------------------------------------------ grid visualisation
+// Voxelizer.DebugRender (VXGI/Voxelize/DebugVisualization/compute.glsl), DESIGN.md 8f.1k: a cone marched through the grid
+// from where the pixel's camera ray enters it, blended over the sky.
+//
+// Empty-space skipping: a level-0 sample whose eight clamped taps are all zero bytes filters to exactly (+0, +0, +0, +0),
+// so the march takes that value without fetching the taps. The march still runs every step. One bit per 4^3 brick of level 0
+// marks the bricks holding a non-zero texel (k_vx_debug_bricks); the dilated mask (k_vx_debug_dilate) ORs each brick with
+// its +x, +y and +z neighbours, so that the bit of the brick holding the lowest tap covers all eight taps. The call uses the
+// skip at cone angle 0 only: a wider cone reads level 0 for at most its first few samples, too few to pay for the masks.
+// IDKVX_DEBUG_SKIP is 1 in the library; scripts/time_vxgi_debug.py builds a second copy with 0 to time the march without it.
+#ifndef IDKVX_DEBUG_SKIP
+#define IDKVX_DEBUG_SKIP 1
+#endif
+#define IDKVX_BRICK_SHIFT 2   // 4^3 texels per brick
+
+struct VxBrickGrid {
+    int nx, ny, nz;            // bricks per axis: ceil(level-0 size / 4)
+    uint32_t words;            // ceil(nx * ny * nz / 32): one bit per brick, x fastest
+};
+
+// one thread per brick: a warp owns one 32-brick word of the occupancy mask
+__global__ void __launch_bounds__(256) k_vx_debug_bricks(VxGridDev g, VxBrickGrid bg, uint32_t* occupancy) {
+    const uint32_t b = blockIdx.x * blockDim.x + threadIdx.x;
+    bool any = false;
+    if (b < (uint32_t)bg.nx * bg.ny * bg.nz) {
+        const int bx = (int)(b % bg.nx), by = (int)((b / bg.nx) % bg.ny), bz = (int)(b / ((uint32_t)bg.nx * bg.ny));
+        const int x0 = bx << IDKVX_BRICK_SHIFT, y0 = by << IDKVX_BRICK_SHIFT, z0 = bz << IDKVX_BRICK_SHIFT;
+        const int x1 = min(x0 + 4, g.sx[0]), y1 = min(y0 + 4, g.sy[0]), z1 = min(z0 + 4, g.sz[0]);
+        for (int z = z0; z < z1; z++)
+            for (int y = y0; y < y1; y++)
+                for (int x = x0; x < x1; x++) any |= __ldg(g.level[0] + (((size_t)z * g.sy[0] + y) * g.sx[0] + x)) != 0ull;
+    }
+    const uint32_t word = __ballot_sync(0xffffffffu, any);
+    if ((threadIdx.x & 31) == 0 && (b >> 5) < bg.words) occupancy[b >> 5] = word;
+}
+
+__device__ __forceinline__ bool vx_brick_bit(const uint32_t* mask, const VxBrickGrid& bg, int bx, int by, int bz) {
+    const uint32_t b = ((uint32_t)bz * bg.ny + by) * bg.nx + bx;
+    return (__ldg(mask + (b >> 5)) >> (b & 31u)) & 1u;
+}
+
+__global__ void __launch_bounds__(256) k_vx_debug_dilate(VxBrickGrid bg, const uint32_t* __restrict__ occupancy, uint32_t* __restrict__ dilated) {
+    const uint32_t b = blockIdx.x * blockDim.x + threadIdx.x;
+    bool any = false;
+    if (b < (uint32_t)bg.nx * bg.ny * bg.nz) {
+        const int bx = (int)(b % bg.nx), by = (int)((b / bg.nx) % bg.ny), bz = (int)(b / ((uint32_t)bg.nx * bg.ny));
+        for (int z = bz; z <= min(bz + 1, bg.nz - 1); z++)
+            for (int y = by; y <= min(by + 1, bg.ny - 1); y++)
+                for (int x = bx; x <= min(bx + 1, bg.nx - 1); x++) any |= vx_brick_bit(occupancy, bg, x, y, z);
+    }
+    const uint32_t word = __ballot_sync(0xffffffffu, any);
+    if ((threadIdx.x & 31) == 0 && (b >> 5) < bg.words) dilated[b >> 5] = word;
+}
+
+// RayBoxIntersect(ray, box, t1, t2) (IntersectionRoutines.glsl:25-40) with both distances. invDir = 1 / dir, so a zero
+// component gives +-inf; min and max are fminf / fmaxf as in ray_box, so a NaN from 0 * inf (origin on a face plane of a
+// parallel axis) drops out of the comparisons.
+__device__ __forceinline__ bool vx_ray_box_t2(f3 o, f3 dir, const float* bmin, const float* bmax, float& t1, float& t2) {
+    const f3 inv = mk3(1.0f / dir.x, 1.0f / dir.y, 1.0f / dir.z);
+    const float t0x = (bmin[0] - o.x) * inv.x, t0y = (bmin[1] - o.y) * inv.y, t0z = (bmin[2] - o.z) * inv.z;
+    const float t1x = (bmax[0] - o.x) * inv.x, t1y = (bmax[1] - o.y) * inv.y, t1z = (bmax[2] - o.z) * inv.z;
+    const float sx = fminf(t0x, t1x), sy = fminf(t0y, t1y), sz = fminf(t0z, t1z);
+    const float bx = fmaxf(t0x, t1x), by = fmaxf(t0y, t1y), bz = fmaxf(t0z, t1z);
+    t1 = fmaxf(sx, fmaxf(sy, fmaxf(sz, 0.0f)));
+    t2 = fminf(bx, fminf(by, bz));
+    return t1 <= t2;
+}
+
+// vx_trace_cone with normal = 0 and normalRayOffset = 0 (TraceCone's four-argument overload, TraceCone.glsl:41-46). With Skip,
+// a level-0 sample inside a brick the dilated mask marks empty takes the value its taps filter to, +0 in every channel.
+// Everything else (the steps, the exit test, the accumulation) is vx_trace_cone's.
+template <bool Skip>
+__device__ __forceinline__ float4 vx_trace_cone_skip(const VxGridDev& g, const uint32_t* mask, const VxBrickGrid& bg, f3 origin, f3 dir,
+                                                     float coneAngle, float stepMultiplier, float alphaThreshold, uint32_t& steps) {
+    const float vsx = (g.gmax[0] - g.gmin[0]) / (float)g.sx[0], vsy = (g.gmax[1] - g.gmin[1]) / (float)g.sy[0], vsz = (g.gmax[2] - g.gmin[2]) / (float)g.sz[0];
+    const float voxelMaxLength = fmaxf(vsx, fmaxf(vsy, vsz));
+    const float voxelMinLength = fminf(vsx, fminf(vsy, vsz));
+    const float maxLevel = (float)(g.levels - 1);
+    float4 acc = make_float4(0.0f, 0.0f, 0.0f, 0.0f);
+    const f3 normal = mk3(0.0f, 0.0f, 0.0f);
+    origin = origin + normal * voxelMaxLength * 0.0f;
+    float distFromStart = voxelMaxLength;
+    const float tanA = det_tan(coneAngle);
+    while (acc.w < alphaThreshold) {
+        const float coneDiameter = 2.0f * tanA * distFromStart;
+        const float sampleDiameter = fmaxf(voxelMinLength, coneDiameter);
+        const float sampleLod = det_log2(sampleDiameter / voxelMinLength);
+        const f3 worldPos = origin + dir * distFromStart;
+        const float u = (worldPos.x - g.gmin[0]) / (g.gmax[0] - g.gmin[0]);
+        const float v = (worldPos.y - g.gmin[1]) / (g.gmax[1] - g.gmin[1]);
+        const float w = (worldPos.z - g.gmin[2]) / (g.gmax[2] - g.gmin[2]);
+        if (u < 0.0f || v < 0.0f || w < 0.0f || u >= 1.0f || v >= 1.0f || w >= 1.0f || sampleLod > maxLevel || !(u == u) || !(v == v) || !(w == w)) break;
+        float4 s;
+        bool empty = false;
+        if (Skip && sampleLod == 0.0f) {
+            // the lowest tap of vx_trilinear(level 0); the other seven lie at +0 or +1 texel on each axis
+            const int x0 = clampi((int)floorf(u * (float)g.sx[0] - 0.5f), 0, g.sx[0] - 1);
+            const int y0 = clampi((int)floorf(v * (float)g.sy[0] - 0.5f), 0, g.sy[0] - 1);
+            const int z0 = clampi((int)floorf(w * (float)g.sz[0] - 0.5f), 0, g.sz[0] - 1);
+            empty = !vx_brick_bit(mask, bg, x0 >> IDKVX_BRICK_SHIFT, y0 >> IDKVX_BRICK_SHIFT, z0 >> IDKVX_BRICK_SHIFT);
+        }
+        if (empty) s = make_float4(0.0f, 0.0f, 0.0f, 0.0f);
+        else s = vx_texture_lod(g, u, v, w, sampleLod);
+        const float weight = 1.0f - acc.w;
+        acc = make_float4(acc.x + s.x * weight, acc.y + s.y * weight, acc.z + s.z * weight, acc.w + s.w * weight);
+        distFromStart += sampleDiameter * stepMultiplier;
+        steps++;
+    }
+    return acc;
+}
+
+struct VxDebugArgs {
+    VxGridDev g;
+    VxBrickGrid bg;
+    const uint32_t* mask;         // dilated brick mask of level 0 (Skip only)
+    DeviceScene sky;              // the sky of the path-tracer context (sample_sky)
+    float invProjection[4];       // mat2(InvProjection): [0], [1], [4], [5]
+    float invView[16];
+    float viewPos[3];
+    float coneAngle, stepMultiplier;
+    float4* out;
+    int width, height;
+    unsigned long long* steps;
+};
+
+// Skip: the march skips empty level-0 samples (cone angle 0, where every sample reads level 0 only; DESIGN.md 8f.1k)
+template <bool Skip>
+__global__ void __launch_bounds__(64) k_vx_debug_render(VxDebugArgs a) {
+    const int x = blockIdx.x * 8 + threadIdx.x, y = blockIdx.y * 8 + threadIdx.y;
+    uint32_t steps = 0;
+    if (x < a.width && y < a.height) {
+        const float nx = ((float)x + 0.5f) / (float)a.width * 2.0f - 1.0f;
+        const float ny = ((float)y + 0.5f) / (float)a.height * 2.0f - 1.0f;
+        // GetWorldSpaceDirection (Math.glsl:6-15)
+        const float rvx = a.invProjection[0] * nx + a.invProjection[2] * ny;
+        const float rvy = a.invProjection[1] * nx + a.invProjection[3] * ny;
+        const f3 dir = normalize3(mat4_mul_xyz(a.invView, rvx, rvy, -1.0f, 0.0f));
+        const f3 viewPos = mk3(a.viewPos[0], a.viewPos[1], a.viewPos[2]);
+        const f3 sky = sample_sky(a.sky, dir);
+        float t1, t2;
+        float4 c;
+        if (!(vx_ray_box_t2(viewPos, dir, a.g.gmin, a.g.gmax, t1, t2) && t2 > 0.0f)) {
+            c = make_float4(sky.x, sky.y, sky.z, 1.0f);
+        } else {
+            // t1 >= 0, so the shader's isInsideGrid (t1 < 0) never holds: the march starts where the ray enters the grid
+            const f3 origin = viewPos + dir * t1;
+            const float4 cone = vx_trace_cone_skip<Skip>(a.g, a.mask, a.bg, origin, dir, a.coneAngle, a.stepMultiplier, 1.0f, steps);
+            const float k = 1.0f - cone.w;
+            c = make_float4(cone.x + k * sky.x, cone.y + k * sky.y, cone.z + k * sky.z, cone.w + k * 1.0f);
+        }
+        a.out[(size_t)y * a.width + x] = c;
     }
     for (int off = 16; off > 0; off >>= 1) steps += __shfl_down_sync(0xffffffffu, steps, off);
     if (((threadIdx.y * 8 + threadIdx.x) & 31) == 0 && steps) atomicAdd(a.steps, (unsigned long long)steps);

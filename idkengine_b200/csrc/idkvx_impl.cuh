@@ -33,6 +33,8 @@ struct IdkVxCtx : IdkCtxBase {
     bool voxelized = false;
     bool slabVoxelized = false;           // idkvx_voxelize ran in slab mode since the grid last changed
     bool conservative = false;            // idkvx_set_conservative_rasterization: coverage rule of the next idkvx_voxelize
+    DevBuf debugImage, debugMask;         // idkvx_debug_render: the rgba32f image and the level-0 brick masks
+    size_t debugBytes = 0;                // bytes of the last successful idkvx_debug_render's image (0: none yet)
 };
 
 static void set_grid_bounds(IdkVxCtx* ctx, const float* mn, const float* mx) {
@@ -114,7 +116,7 @@ IDKPT_API void idkvx_destroy(IdkVxCtx* ctx) {
     if (ctx->stream) cudaStreamSynchronize(ctx->stream);
     DevBuf* all[] = {&ctx->gridMem, &ctx->positions, &ctx->vertices, &ctx->tris, &ctx->descs, &ctx->instances, &ctx->xforms, &ctx->meshes,
                      &ctx->materials, &ctx->lights, &ctx->tex.pixels, &ctx->tex.recs, &ctx->tex.srgbLut, &ctx->queue, &ctx->queueCount,
-                     &ctx->counters, &ctx->scratch[0], &ctx->scratch[1], &ctx->scratch[2], &ctx->scratch[3]};
+                     &ctx->counters, &ctx->scratch[0], &ctx->scratch[1], &ctx->scratch[2], &ctx->scratch[3], &ctx->debugImage, &ctx->debugMask};
     for (DevBuf* b : all) release(*b);
     destroy_stream(ctx);
     delete ctx;
@@ -359,6 +361,91 @@ IDKPT_API int idkvx_cone_trace_rows(IdkVxCtx* ctx, const GpuPerFrameData* frame,
         stats->ConeSteps = s;
         stats->KernelLaunches = 1;
     }
+    return IDKPT_OK;
+}
+
+// Voxelizer.DebugRender (Voxelizer.cs:230-244): the grid as it is now, marched per pixel and blended over the sky of `sky`.
+IDKPT_API int idkvx_debug_render(IdkVxCtx* ctx, IdkPtCtx* sky, const GpuPerFrameData* frame, float stepMultiplier, float coneAngle,
+                                 int32_t width, int32_t height, float* out, IdkVxStats* stats) {
+    static const char* who = "idkvx_debug_render";
+    if (!ctx) return IDKPT_ERR_INVALID_ARGUMENT;
+    if (!sky || !frame) return fail(ctx, who, IDKPT_ERR_INVALID_ARGUMENT, "null argument");
+    if (sky->device != ctx->device) return fail(ctx, who, IDKPT_ERR_INVALID_ARGUMENT, "the sky's path-tracer context is on another device");
+    if (width < 1 || height < 1 || width > 16384 || height > 16384) return fail(ctx, who, IDKPT_ERR_INVALID_ARGUMENT, "width or height outside 1..16384");
+    if (!std::isfinite(coneAngle) || coneAngle < 0.0f || coneAngle > 1.5f) return fail(ctx, who, IDKPT_ERR_INVALID_ARGUMENT, "cone angle not finite or outside [0, 1.5]");
+    if (!std::isfinite(stepMultiplier) || !(stepMultiplier > 0.0f)) return fail(ctx, who, IDKPT_ERR_INVALID_ARGUMENT, "step multiplier not finite or not > 0");
+    // every march ends within (|GridMax - GridMin| + voxelMaxLength) / (voxelMinLength * stepMultiplier) steps (DESIGN.md 8f.1k)
+    const VxGridDev& g = ctx->grid;
+    double diag2 = 0.0, vmin = 0.0, vmax = 0.0;
+    for (int i = 0; i < 3; i++) {
+        const float e = g.gmax[i] - g.gmin[i];
+        const double vs = (double)(e / (float)(i == 0 ? g.sx[0] : (i == 1 ? g.sy[0] : g.sz[0])));
+        diag2 += (double)e * (double)e;
+        vmin = i == 0 ? vs : std::min(vmin, vs);
+        vmax = i == 0 ? vs : std::max(vmax, vs);
+    }
+    const double bound = (std::sqrt(diag2) + vmax) / (vmin * (double)stepMultiplier);
+    if (!(bound <= 65536.0)) return fail(ctx, who, IDKPT_ERR_INVALID_ARGUMENT, "step multiplier too small for the grid: the march would take more than 65536 steps");
+    CK(cudaSetDevice(ctx->device));
+    if (stats) memset(stats, 0, sizeof(*stats));
+
+    // the skip pays for its mask only where the march reads level 0 alone: at cone angle 0 (DESIGN.md 8f.1k)
+    const bool skip = IDKVX_DEBUG_SKIP && coneAngle == 0.0f;
+    VxBrickGrid bg;
+    bg.nx = (g.sx[0] + 3) >> IDKVX_BRICK_SHIFT; bg.ny = (g.sy[0] + 3) >> IDKVX_BRICK_SHIFT; bg.nz = (g.sz[0] + 3) >> IDKVX_BRICK_SHIFT;
+    const uint32_t bricks = (uint32_t)bg.nx * bg.ny * bg.nz;
+    bg.words = (bricks + 31) / 32;
+    if (skip && ensure(ctx->debugMask, 2 * (size_t)bg.words * 4) != cudaSuccess) return fail(ctx, who, IDKPT_ERR_OUT_OF_MEMORY, "device allocation failed");
+    // a larger image goes into a fresh allocation that replaces the old one only once the kernel has succeeded
+    const size_t n = (size_t)width * height, bytes = n * 16;
+    DevBuf fresh;
+    if (bytes > ctx->debugImage.bytes && ensure(fresh, bytes) != cudaSuccess) {
+        release(fresh);
+        return fail(ctx, who, IDKPT_ERR_OUT_OF_MEMORY, "device allocation failed");
+    }
+    float4* image = (float4*)(fresh.p ? fresh.p : ctx->debugImage.p);
+    VxDebugArgs a;
+    a.g = g;
+    a.bg = bg;
+    a.mask = (const uint32_t*)ctx->debugMask.p + bg.words;
+    a.sky = sky->sc;
+    a.invProjection[0] = frame->InvProjection[0]; a.invProjection[1] = frame->InvProjection[1];
+    a.invProjection[2] = frame->InvProjection[4]; a.invProjection[3] = frame->InvProjection[5];
+    memcpy(a.invView, frame->InvView, sizeof(a.invView));
+    memcpy(a.viewPos, frame->ViewPos, sizeof(a.viewPos));
+    a.coneAngle = coneAngle; a.stepMultiplier = stepMultiplier;
+    a.out = image;
+    a.width = width; a.height = height;
+    a.steps = (unsigned long long*)ctx->counters.p;
+    uint32_t launches = 0;
+    const int rc = run_timed(ctx, who, stats ? &stats->ConeTraceMs : nullptr, [&]() -> int {
+        CK(cudaMemsetAsync(ctx->counters.p, 0, 16, ctx->stream));
+        if (skip) {
+            const unsigned blocks = (unsigned)(((size_t)bg.words * 32 + 255) / 256);
+            k_vx_debug_bricks<<<blocks, 256, 0, ctx->stream>>>(g, bg, (uint32_t*)ctx->debugMask.p);
+            k_vx_debug_dilate<<<blocks, 256, 0, ctx->stream>>>(bg, (const uint32_t*)ctx->debugMask.p, (uint32_t*)ctx->debugMask.p + bg.words);
+            launches += 2;
+        }
+        (skip ? k_vx_debug_render<true> : k_vx_debug_render<false>)<<<dim3((width + 7) / 8, (height + 7) / 8), dim3(8, 8), 0, ctx->stream>>>(a);
+        launches++;
+        return IDKPT_OK;
+    }, out, image, out ? bytes : 0);
+    if (rc) { release(fresh); return rc; }
+    if (fresh.p) { release(ctx->debugImage); ctx->debugImage = fresh; }
+    ctx->debugBytes = bytes;
+    if (stats) {
+        unsigned long long s = 0;
+        CK(cudaMemcpy(&s, ctx->counters.p, 8, cudaMemcpyDeviceToHost));
+        stats->ConeSteps = s;
+        stats->KernelLaunches = launches;
+    }
+    return IDKPT_OK;
+}
+
+IDKPT_API int idkvx_debug_device_ptr(IdkVxCtx* ctx, void** devPtr, uint64_t* bytes) {
+    if (!ctx || !devPtr) return fail(ctx, IDKPT_ERR_INVALID_ARGUMENT, "idkvx_debug_device_ptr: null argument");
+    *devPtr = ctx->debugBytes ? ctx->debugImage.p : nullptr;
+    if (bytes) *bytes = ctx->debugBytes;
     return IDKPT_OK;
 }
 

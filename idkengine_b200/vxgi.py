@@ -27,7 +27,7 @@ class IdkVxStats(ctypes.Structure):
 VX_EXPORTS = ["idkvx_create", "idkvx_destroy", "idkvx_last_error", "idkvx_set_scene", "idkvx_set_grid", "idkvx_level_count",
               "idkvx_voxelize", "idkvx_read_level", "idkvx_cone_trace", "idkvx_set_shadow_tracer",
               "idkvx_set_shadow_maps", "idkvx_set_slab", "idkvx_level_device_ptr", "idkvx_mipmap", "idkvx_cone_trace_rows",
-              "idkvx_set_conservative_rasterization"]
+              "idkvx_set_conservative_rasterization", "idkvx_debug_render", "idkvx_debug_device_ptr"]
 
 DEFAULT_GRID_MIN = (-28.0, -3.0, -17.0)   # RasterPipeline.cs:213
 DEFAULT_GRID_MAX = (28.0, 20.0, 17.0)
@@ -88,6 +88,10 @@ def _declare(L):
     L.idkvx_read_level.argtypes = [c_vp, c_i32, c_vp, c_u64]
     L.idkvx_cone_trace.restype = c_i32
     L.idkvx_cone_trace.argtypes = [c_vp, c_vp, P(IdkVxConeSettings), c_vp, c_vp, c_vp, c_i32, c_i32, P(c_f * 3), c_vp, P(IdkVxStats)]
+    L.idkvx_debug_render.restype = c_i32
+    L.idkvx_debug_render.argtypes = [c_vp, c_vp, c_vp, c_f, c_f, c_i32, c_i32, c_vp, P(IdkVxStats)]
+    L.idkvx_debug_device_ptr.restype = c_i32
+    L.idkvx_debug_device_ptr.argtypes = [c_vp, P(c_vp), P(c_u64)]
     return L
 
 
@@ -96,8 +100,8 @@ class IdkVxError(RuntimeError):
 
 
 class Voxelizer:
-    def __init__(self, size=256, grid_min=DEFAULT_GRID_MIN, grid_max=DEFAULT_GRID_MAX, device=0):
-        self._lib = _declare(capi.load())
+    def __init__(self, size=256, grid_min=DEFAULT_GRID_MIN, grid_max=DEFAULT_GRID_MAX, device=0, lib_path=None):
+        self._lib = _declare(capi.load(lib_path))
         self.ci = create_info(size, grid_min, grid_max, device)
         self._ctx = c_vp()
         rc = self._lib.idkvx_create(ctypes.byref(self.ci), ctypes.byref(self._ctx))
@@ -105,6 +109,8 @@ class Voxelizer:
             raise IdkVxError(f"idkvx_create failed ({rc}): {(self._lib.idkvx_last_error(None) or b'').decode()}")
         self.sizes = level_sizes(self.ci)
         self._conservative = False
+        self.DebugStepMultiplier = 0.4     # the constructor defaults of Voxelizer.cs:68 (DebugRender)
+        self.DebugConeAngle = 0.0
 
     def _check(self, rc, what):
         if rc != 0:
@@ -179,6 +185,25 @@ class Voxelizer:
         self._check(self._lib.idkvx_cone_trace_rows(self._ctx, frame.ctypes.data, ctypes.byref(settings), depth.ctypes.data, nrg.ctypes.data,
                                                     mr.ctypes.data, w, full_height, row_first, h, ctypes.byref(skyc), out.ctypes.data, ctypes.byref(st)), "idkvx_cone_trace_rows")
         return out, st
+
+    def DebugRender(self, path_tracer, frame, width, height, out=True):
+        """Voxelizer.DebugRender (Voxelizer.cs:230-244): the grid as it is now, marched per pixel with DebugConeAngle and
+        DebugStepMultiplier and blended over path_tracer's sky (idkvx_debug_render). Returns (image float32 [h, w, 4] or None
+        with out=False, when the image stays on the device: DebugDevicePtr), stats)."""
+        frame = np.ascontiguousarray(frame)
+        assert frame.dtype == gt.GpuPerFrameData
+        img = np.empty((height, width, 4), np.float32) if out else None
+        st = IdkVxStats()
+        self._check(self._lib.idkvx_debug_render(self._ctx, path_tracer._ctx if path_tracer is not None else None, frame.ctypes.data,
+                                                 float(self.DebugStepMultiplier), float(self.DebugConeAngle), int(width), int(height),
+                                                 img.ctypes.data if out else None, ctypes.byref(st)), "idkvx_debug_render")
+        return img, st
+
+    def DebugDevicePtr(self):
+        """(device pointer, bytes) of the last DebugRender's rgba32f image; (None, 0) before the first."""
+        p, n = c_vp(), c_u64()
+        self._check(self._lib.idkvx_debug_device_ptr(self._ctx, ctypes.byref(p), ctypes.byref(n)), "idkvx_debug_device_ptr")
+        return p.value, n.value
 
     def Render(self):
         """Voxelizer.Render(modelManager): clear + voxelise + mipmap."""

@@ -398,6 +398,21 @@ public:
         c.MaxSamples = 4; c.StepMultiplier = 0.16f; c.GIBoost = 1.3f; c.GISkyBoxBoost = 1.0f / 1.3f; c.NormalRayOffset = 1.0f; c.NoiseIndex = 0;
         return c;
     }
+    // DebugRender's settings, with the constructor defaults of Voxelizer.cs:68
+    float DebugStepMultiplier = 0.4f;
+    float DebugConeAngle = 0.0f;
+    // Voxelizer.DebugRender: the grid marched per pixel over the sky of `sky`, rgba32f out (width * height * 4 floats)
+    std::vector<float> DebugRender(const PathTracer& sky, const GpuPerFrameData& frame, int width, int height, IdkVxStats* stats = nullptr) {
+        std::vector<float> out((size_t)width * height * 4);
+        check(idkvx_debug_render(ctx_, sky.Handle(), &frame, DebugStepMultiplier, DebugConeAngle, width, height, out.data(), stats), "idkvx_debug_render");
+        return out;
+    }
+    // the last DebugRender's image on the device (nullptr before the first)
+    void* DebugDevicePtr(uint64_t* bytes = nullptr) const {
+        void* p = nullptr;
+        check(idkvx_debug_device_ptr(ctx_, &p, bytes), "idkvx_debug_device_ptr");
+        return p;
+    }
 
 private:
     void check(int rc, const char* what) const {

@@ -99,6 +99,30 @@ IDKPT_API int idkvx_cone_trace(IdkVxCtx* ctx, const GpuPerFrameData* frame, cons
                                const float* depth, const float* normalRG, const float* metallicRoughness,
                                int32_t width, int32_t height, const float skyColor[3], float* out_rgba32f, IdkVxStats* stats);
 
+/* Voxelizer.DebugRender (Voxelizer.cs:230-244, VXGI/Voxelize/DebugVisualization/compute.glsl): the grid-configuration view
+ * (RasterPipeline.Render's IsConfigureGridMode branch). Per pixel of a width x height image, the camera ray of `frame`
+ * (InvProjection, InvView, ViewPos; pixel centres, no jitter) is clipped to [GridMin, GridMax]; a ray that misses the box, or
+ * has it behind the camera, stores the sky (rgb, 1). Otherwise a cone of `cone_angle` is marched through the context's
+ * current grid (every level, whatever it holds; a fresh context's cleared grid renders as sky) from where the ray enters the
+ * grid, or from ViewPos inside it, with steps of step_multiplier x the sample diameter, until alpha reaches 1 or the cone
+ * leaves the grid; the result c is blended over the sky: (c.rgb + (1 - c.a) * sky.rgb, c.a + (1 - c.a)). The sky is that of
+ * the path-tracer context `sky` on the same device (idkpt_set_sky, idkpt_sky_atmosphere, idkpt_sky_equirectangular; a
+ * constant sky works the same way); every sky the library holds is opaque, so the blend takes its alpha as 1.
+ * out_rgba32f: width*height*4 floats, row 0 first, not rounded (the engine's target is rgba16f or R11G11B10F: the host rounds
+ * when it copies into its texture). out_rgba32f may be NULL: the image then stays on the device only, where
+ * idkvx_debug_device_ptr finds it; either way the context keeps the image of the last successful call, in an allocation that
+ * calls of the same or a smaller size reuse. stats (may be NULL): ConeTraceMs = CUDA-event time of the kernels, ConeSteps =
+ * samples the marches took, KernelLaunches. Synchronous. Fails with IDKPT_ERR_INVALID_ARGUMENT, before anything is launched
+ * (the previous image keeps every byte), on a NULL ctx, sky or frame; a sky context on another device; width or height
+ * outside 1..16384; cone_angle not finite or outside [0, 1.5]; step_multiplier not finite or not > 0; and a grid and
+ * step_multiplier for which (|GridMax - GridMin| + voxelMaxLength) / (voxelMinLength * step_multiplier) > 65536, the most
+ * steps a march may take (DESIGN.md 8f.1k). */
+IDKPT_API int idkvx_debug_render(IdkVxCtx* ctx, struct IdkPtCtx* sky, const GpuPerFrameData* frame, float step_multiplier,
+                                 float cone_angle, int32_t width, int32_t height, float* out_rgba32f, IdkVxStats* stats);
+/* The device image of the last successful idkvx_debug_render (rgba32f, width*height*16 bytes); NULL and 0 bytes before the
+ * first. The pointer stays valid until the next idkvx_debug_render with a larger image, or idkvx_destroy. */
+IDKPT_API int idkvx_debug_device_ptr(IdkVxCtx* ctx, void** dev_ptr, uint64_t* bytes);
+
 /* ---- multi-GPU (SURVEY.md 8e): voxelise by z-slab, all-gather, cone-trace screen tiles ----
  * Rank r of N: idkvx_set_slab(r * D / N, (r + 1) * D / N), idkvx_voxelize (writes only that slab of level 0, no mip chain),
  * one all-gather of the slabs straight into the grid (a z-slab of the linear x-fastest level is one contiguous range:

@@ -245,3 +245,20 @@ with PathTracer(16, 16) as pt:
         pt.DeferredLighting(fg, d, n, a, mr, e, settings=capi.IdkPtDeferredSettings(0, 0, 0, 0), download=False)
         pt.LightsAndSkybox(fg, jitter=(0.01, -0.02))
 print("lights and skybox ok")
+
+# the grid visualisation: the brick masks and the march, a constant and a cube-map sky, odd sizes and grid shapes (partial
+# bricks and 8x8 blocks), cone angles 0 and 0.25, from outside and inside the grid
+with PathTracer(16, 16) as pt, vxgi.Voxelizer((23, 9, 14), (-3.1, -0.1, -3.1), (3.1, 4.1, 3.1)) as vx:
+    vx.SetScene(scene); vx.Render()
+    for sky in ((0.6, 0.7, 0.9), None):
+        if sky is None:
+            pt.SkyAtmosphere(face_size=5)
+        else:
+            pt.SetSky(sky)
+        for gw, gh in ((37, 23), (1, 1)):
+            for cone in (0.0, 0.25):
+                vx.DebugConeAngle = cone
+                vx.DebugRender(pt, scenes.camera_frame(cam, gw, gh), gw, gh)
+                vx.DebugRender(pt, scenes.camera_frame(dict(position=(6.0, 5.0, -7.0), view_dir=(-0.6, -0.4, 0.7)), gw, gh), gw, gh, out=False)
+    vx.DebugDevicePtr()
+print("grid visualisation ok")
