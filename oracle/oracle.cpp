@@ -38,6 +38,10 @@
 // normalize(v) = v * (1/sqrt(dot(v,v))); pow(x,5) = ((x*x)*(x*x))*x; sin/cos/exp
 // are the polynomial routines below (glibc's and CUDA's libm differ in the last
 // ulp, so both sides implement the same documented algorithm instead).
+//
+// The pass oracles (oracle_*.cpp) include this file and each other; oracle/liboracle.cpp includes them all, so the whole
+// checker is one translation unit and one library, oracle/liboracle.so (oracle/build.py).
+#pragma once
 
 #include <cstdint>
 #include <cstring>
@@ -54,29 +58,33 @@
 
 #include "../include/idkpt.h"
 
+// The small helpers below are inlined whatever the size of the translation unit, so the traversal and shading loops that
+// bench.py times do not change speed as pass oracles are added to the library.
+#define ORACLE_INLINE inline __attribute__((always_inline))
+
 namespace {
 
 // ------------------------------------------------------------------ vec3
 struct vec3 { float x, y, z; };
-static inline vec3 V(float x, float y, float z) { return {x, y, z}; }
-static inline vec3 V(const float* p) { return {p[0], p[1], p[2]}; }
-static inline vec3 operator+(vec3 a, vec3 b) { return {a.x + b.x, a.y + b.y, a.z + b.z}; }
-static inline vec3 operator-(vec3 a, vec3 b) { return {a.x - b.x, a.y - b.y, a.z - b.z}; }
-static inline vec3 operator-(vec3 a) { return {-a.x, -a.y, -a.z}; }
-static inline vec3 operator*(vec3 a, vec3 b) { return {a.x * b.x, a.y * b.y, a.z * b.z}; }
-static inline vec3 operator*(vec3 a, float s) { return {a.x * s, a.y * s, a.z * s}; }
-static inline vec3 operator*(float s, vec3 a) { return {s * a.x, s * a.y, s * a.z}; }
-static inline vec3 operator/(vec3 a, float s) { return {a.x / s, a.y / s, a.z / s}; }
-static inline vec3 operator/(vec3 a, vec3 b) { return {a.x / b.x, a.y / b.y, a.z / b.z}; }
-static inline float dot(vec3 a, vec3 b) { return (a.x * b.x + a.y * b.y) + a.z * b.z; }
-static inline vec3 cross(vec3 a, vec3 b) { return {a.y * b.z - b.y * a.z, a.z * b.x - b.z * a.x, a.x * b.y - b.x * a.y}; }
-static inline vec3 normalize(vec3 v) { float inv = 1.0f / sqrtf(dot(v, v)); return v * inv; }
-static inline float mixf(float x, float y, float a) { return x * (1.0f - a) + y * a; }
-static inline vec3 mix(vec3 x, vec3 y, float a) { return {mixf(x.x, y.x, a), mixf(x.y, y.y, a), mixf(x.z, y.z, a)}; }
-static inline float clampf(float x, float lo, float hi) { return fminf(fmaxf(x, lo), hi); }
-static inline float fractf(float x) { return x - floorf(x); }
-static inline vec3 reflect(vec3 I, vec3 N) { return I - (2.0f * dot(N, I)) * N; }
-static inline vec3 refract(vec3 I, vec3 N, float eta) {
+static ORACLE_INLINE vec3 V(float x, float y, float z) { return {x, y, z}; }
+static ORACLE_INLINE vec3 V(const float* p) { return {p[0], p[1], p[2]}; }
+static ORACLE_INLINE vec3 operator+(vec3 a, vec3 b) { return {a.x + b.x, a.y + b.y, a.z + b.z}; }
+static ORACLE_INLINE vec3 operator-(vec3 a, vec3 b) { return {a.x - b.x, a.y - b.y, a.z - b.z}; }
+static ORACLE_INLINE vec3 operator-(vec3 a) { return {-a.x, -a.y, -a.z}; }
+static ORACLE_INLINE vec3 operator*(vec3 a, vec3 b) { return {a.x * b.x, a.y * b.y, a.z * b.z}; }
+static ORACLE_INLINE vec3 operator*(vec3 a, float s) { return {a.x * s, a.y * s, a.z * s}; }
+static ORACLE_INLINE vec3 operator*(float s, vec3 a) { return {s * a.x, s * a.y, s * a.z}; }
+static ORACLE_INLINE vec3 operator/(vec3 a, float s) { return {a.x / s, a.y / s, a.z / s}; }
+static ORACLE_INLINE vec3 operator/(vec3 a, vec3 b) { return {a.x / b.x, a.y / b.y, a.z / b.z}; }
+static ORACLE_INLINE float dot(vec3 a, vec3 b) { return (a.x * b.x + a.y * b.y) + a.z * b.z; }
+static ORACLE_INLINE vec3 cross(vec3 a, vec3 b) { return {a.y * b.z - b.y * a.z, a.z * b.x - b.z * a.x, a.x * b.y - b.x * a.y}; }
+static ORACLE_INLINE vec3 normalize(vec3 v) { float inv = 1.0f / sqrtf(dot(v, v)); return v * inv; }
+static ORACLE_INLINE float mixf(float x, float y, float a) { return x * (1.0f - a) + y * a; }
+static ORACLE_INLINE vec3 mix(vec3 x, vec3 y, float a) { return {mixf(x.x, y.x, a), mixf(x.y, y.y, a), mixf(x.z, y.z, a)}; }
+static ORACLE_INLINE float clampf(float x, float lo, float hi) { return fminf(fmaxf(x, lo), hi); }
+static ORACLE_INLINE float fractf(float x) { return x - floorf(x); }
+static ORACLE_INLINE vec3 reflect(vec3 I, vec3 N) { return I - (2.0f * dot(N, I)) * N; }
+static ORACLE_INLINE vec3 refract(vec3 I, vec3 N, float eta) {
     float d = dot(N, I);
     float k = 1.0f - eta * eta * (1.0f - d * d);
     if (k < 0.0f) return V(0.0f, 0.0f, 0.0f);
@@ -89,7 +97,7 @@ static inline vec3 refract(vec3 I, vec3 N, float eta) {
 // ------------------------------------------------------------------ deterministic sin/cos/exp
 // sincos for x in [0, 2*pi]: quadrant reduction with a two-term pi/2 (Cody-Waite), then the
 // classic single-precision minimax polynomials on [-pi/4, pi/4] (Cephes sinf/cosf coefficients).
-static inline void det_sincos(float x, float* s, float* c) {
+static ORACLE_INLINE void det_sincos(float x, float* s, float* c) {
     float q = floorf(x * 0.63661977236758134f + 0.5f); // nearest multiple of pi/2
     int n = (int)q;
     float r = (x - q * 1.5703125f) - q * 4.83826794897e-4f; // pi/2 = 1.5703125 + 4.83826794897e-4
@@ -105,7 +113,7 @@ static inline void det_sincos(float x, float* s, float* c) {
 }
 
 // exp(x): n = round(x*log2e), r = x - n*ln2 (two-term), degree-5 polynomial (Cephes expf), scale by 2^n.
-static inline float det_exp(float x) {
+static ORACLE_INLINE float det_exp(float x) {
     if (x < -87.0f) return 0.0f;
     if (x > 88.0f) return INFINITY;
     float fn = floorf(x * 1.44269504088896341f + 0.5f);
@@ -140,7 +148,7 @@ struct HitInfo {
 struct Counters { uint32_t steps, tris, instances; float debugCost; };
 
 // IntersectionRoutines.glsl:6-23
-static inline bool RayTriangleIntersect(const Ray& ray, vec3 p0, vec3 p1, vec3 p2, vec3& bary, float& t) {
+static ORACLE_INLINE bool RayTriangleIntersect(const Ray& ray, vec3 p0, vec3 p1, vec3 p2, vec3& bary, float& t) {
     vec3 p1p0 = p1 - p0;
     vec3 p2p0 = p2 - p0;
     vec3 rop0 = ray.o - p0;
@@ -155,7 +163,7 @@ static inline bool RayTriangleIntersect(const Ray& ray, vec3 p0, vec3 p1, vec3 p
 }
 
 // IntersectionRoutines.glsl:25-46 (invDir hoisted by the caller: 1.0 / ray.Direction)
-static inline bool RayBoxIntersect(const Ray& ray, vec3 invDir, const float* bmin, const float* bmax, float& t1) {
+static ORACLE_INLINE bool RayBoxIntersect(const Ray& ray, vec3 invDir, const float* bmin, const float* bmax, float& t1) {
     vec3 t0s = (V(bmin) - ray.o) * invDir;
     vec3 t1s = (V(bmax) - ray.o) * invDir;
     vec3 ts = {fminf(t0s.x, t1s.x), fminf(t0s.y, t1s.y), fminf(t0s.z, t1s.z)};
@@ -166,7 +174,7 @@ static inline bool RayBoxIntersect(const Ray& ray, vec3 invDir, const float* bmi
 }
 
 // IntersectionRoutines.glsl:48-69
-static inline bool RaySphereIntersect(const Ray& ray, vec3 position, float radius, float& t1, float& t2) {
+static ORACLE_INLINE bool RaySphereIntersect(const Ray& ray, vec3 position, float radius, float& t1, float& t2) {
     t1 = FLOAT_MAX;
     t2 = FLOAT_MAX;
     vec3 sphereToRay = ray.o - position;
@@ -180,7 +188,7 @@ static inline bool RaySphereIntersect(const Ray& ray, vec3 position, float radiu
     return t1 <= t2 && t2 > 0.0f;
 }
 
-static inline vec3 pos(const Scene& s, int32_t i) { const PackedVec3& p = s.d.VertexPositions[i]; return {p.x, p.y, p.z}; }
+static ORACLE_INLINE vec3 pos(const Scene& s, int32_t i) { const PackedVec3& p = s.d.VertexPositions[i]; return {p.x, p.y, p.z}; }
 
 // BVHIntersect.glsl:27-105
 static bool IntersectBlas(const Scene& s, const Ray& ray, const GpuBlasDesc& blasDesc, HitInfo& hitInfo, Counters& cnt, bool useTlas) {
@@ -248,7 +256,7 @@ static bool IntersectBlas(const Scene& s, const Ray& ray, const GpuBlasDesc& bla
 }
 
 // Ray.glsl:7-12 with mat4(mat4x3): rows of the stored 3x4.
-static inline Ray RayTransform(const Ray& ray, const float m[3][4]) {
+static ORACLE_INLINE Ray RayTransform(const Ray& ray, const float m[3][4]) {
     Ray r;
     r.o.x = ((m[0][0] * ray.o.x + m[0][1] * ray.o.y) + m[0][2] * ray.o.z) + m[0][3];
     r.o.y = ((m[1][0] * ray.o.x + m[1][1] * ray.o.y) + m[1][2] * ray.o.z) + m[1][3];
@@ -359,9 +367,9 @@ static bool BruteForce(const Scene& s, const Ray& ray, HitInfo& hitInfo, float m
 
 // ------------------------------------------------------------------ CPU (C#) traversal = baseline
 // Intersections.RayVsBox (Intersections.cs:363-377): division based, MaxNative/MinNative.
-static inline float minN(float a, float b) { return a < b ? a : b; }
-static inline float maxN(float a, float b) { return a > b ? a : b; }
-static inline bool CsRayVsBox(const Ray& ray, const float* bmin, const float* bmax, float& t1) {
+static ORACLE_INLINE float minN(float a, float b) { return a < b ? a : b; }
+static ORACLE_INLINE float maxN(float a, float b) { return a > b ? a : b; }
+static ORACLE_INLINE bool CsRayVsBox(const Ray& ray, const float* bmin, const float* bmax, float& t1) {
     vec3 t0s = (V(bmin) - ray.o) / ray.d;
     vec3 t1s = (V(bmax) - ray.o) / ray.d;
     vec3 ts = {minN(t0s.x, t1s.x), minN(t0s.y, t1s.y), minN(t0s.z, t1s.z)};
@@ -371,9 +379,9 @@ static inline bool CsRayVsBox(const Ray& ray, const float* bmin, const float* bm
     return t1 <= t2;
 }
 // Intersections.RayVsTriangle (Intersections.cs:379-396): divisions by x, t > 0. OpenTK Vector3.Cross/Dot.
-static inline vec3 csCross(vec3 l, vec3 r) { return {l.y * r.z - l.z * r.y, l.z * r.x - l.x * r.z, l.x * r.y - l.y * r.x}; }
-static inline float csDot(vec3 a, vec3 b) { return a.x * b.x + a.y * b.y + a.z * b.z; }
-static inline bool CsRayVsTriangle(const Ray& ray, vec3 p0, vec3 p1, vec3 p2, vec3& bary, float& t) {
+static ORACLE_INLINE vec3 csCross(vec3 l, vec3 r) { return {l.y * r.z - l.z * r.y, l.z * r.x - l.x * r.z, l.x * r.y - l.y * r.x}; }
+static ORACLE_INLINE float csDot(vec3 a, vec3 b) { return a.x * b.x + a.y * b.y + a.z * b.z; }
+static ORACLE_INLINE bool CsRayVsTriangle(const Ray& ray, vec3 p0, vec3 p1, vec3 p2, vec3& bary, float& t) {
     vec3 v1v0 = p1 - p0, v2v0 = p2 - p0, rov0 = ray.o - p0;
     vec3 normal = csCross(v1v0, v2v0);
     vec3 q = csCross(rov0, ray.d);
@@ -429,8 +437,8 @@ static bool CsBlasIntersect(const Scene& s, const GpuBlasDesc& desc, const Ray& 
     }
     return hit.T != tMaxDist;
 }
-// BVH.Intersect (BVH.cs:162-193), no TLAS
-static bool CsBvhIntersect(const Scene& s, const Ray& ray, HitInfo& hitInfo, float tMax, Counters& cnt) {
+// BVH.Intersect (BVH.cs:162-193), no TLAS. Inlined into oracle_cpu_intersect's worker, the cpu_baseline loop bench.py times.
+static ORACLE_INLINE bool CsBvhIntersect(const Scene& s, const Ray& ray, HitInfo& hitInfo, float tMax, Counters& cnt) {
     hitInfo.T = tMax;
     hitInfo.TriangleId = ~0u;
     hitInfo.MeshTransformId = 0;
@@ -452,14 +460,14 @@ static bool CsBvhIntersect(const Scene& s, const Ray& ray, HitInfo& hitInfo, flo
 
 // ------------------------------------------------------------------ RNG / sampling / compression
 struct Rng { uint32_t seed; };
-static inline uint32_t GetPCGHash(uint32_t& seed) {
+static ORACLE_INLINE uint32_t GetPCGHash(uint32_t& seed) {
     seed = seed * 747796405u + 2891336453u;
     uint32_t word = ((seed >> ((seed >> 28u) + 4u)) ^ seed) * 277803737u;
     return (word >> 22u) ^ word;
 }
-static inline float GetRandomFloat01(Rng& r) { return (float)GetPCGHash(r.seed) / 4294967296.0f; }
+static ORACLE_INLINE float GetRandomFloat01(Rng& r) { return (float)GetPCGHash(r.seed) / 4294967296.0f; }
 
-static inline void R2Sequence(uint32_t id, float& u, float& v) {
+static ORACLE_INLINE void R2Sequence(uint32_t id, float& u, float& v) {
     const float g = 1.32471795724474602596f;
     const float a1 = 1.0f / g;
     const float a2 = 1.0f / (g * g);
@@ -467,7 +475,7 @@ static inline void R2Sequence(uint32_t id, float& u, float& v) {
     v = fractf((float)id * a2);
 }
 
-static inline vec3 SampleSphere(float rnd0, float rnd1) {
+static ORACLE_INLINE vec3 SampleSphere(float rnd0, float rnd1) {
     float cosTheta = rnd0 * 2.0f - 1.0f;
     float phi = rnd1 * 2.0f * PI_F;
     float sinTheta = sqrtf(1.0f - cosTheta * cosTheta);
@@ -475,9 +483,9 @@ static inline vec3 SampleSphere(float rnd0, float rnd1) {
     det_sincos(phi, &sinPhi, &cosPhi);
     return {sinTheta * cosPhi, sinTheta * sinPhi, cosTheta};
 }
-static inline vec3 CosineSampleHemisphere(vec3 normal, float u, float v) { return normalize(normal + SampleSphere(u, v)); }
+static ORACLE_INLINE vec3 CosineSampleHemisphere(vec3 normal, float u, float v) { return normalize(normal + SampleSphere(u, v)); }
 
-static inline void SampleDisk(Rng& rng, float& px, float& py) {
+static ORACLE_INLINE void SampleDisk(Rng& rng, float& px, float& py) {
     float dist;
     float lastRnd = GetRandomFloat01(rng);
     do {
@@ -491,7 +499,7 @@ static inline void SampleDisk(Rng& rng, float& px, float& py) {
     py = py * 2.0f - 1.0f;
 }
 
-static inline vec3 DecompressSR11G11B10(uint32_t data) {
+static ORACLE_INLINE vec3 DecompressSR11G11B10(uint32_t data) {
     float r = (float)((data >> 0) & ((1u << 11) - 1));
     float g = (float)((data >> 11) & ((1u << 11) - 1));
     float b = (float)((data >> 22) & ((1u << 10) - 1));
@@ -501,7 +509,7 @@ static inline vec3 DecompressSR11G11B10(uint32_t data) {
     return {r * 2.0f - 1.0f, g * 2.0f - 1.0f, b * 2.0f - 1.0f};
 }
 
-static inline void EncodeUnitVec(vec3 n, float& ex, float& ey) {
+static ORACLE_INLINE void EncodeUnitVec(vec3 n, float& ex, float& ey) {
     float l1 = (fabsf(n.x) + fabsf(n.y)) + fabsf(n.z);
     n = n / l1;
     float nx = n.x, ny = n.y;
@@ -517,7 +525,7 @@ static inline void EncodeUnitVec(vec3 n, float& ex, float& ey) {
     ex = nx * 0.5f + 0.5f;
     ey = ny * 0.5f + 0.5f;
 }
-static inline vec3 DecodeUnitVec(float fx, float fy) {
+static ORACLE_INLINE vec3 DecodeUnitVec(float fx, float fy) {
     fx = fx * 2.0f - 1.0f;
     fy = fy * 2.0f - 1.0f;
     vec3 n = {fx, fy, 1.0f - fabsf(fx) - fabsf(fy)};
@@ -527,7 +535,7 @@ static inline vec3 DecodeUnitVec(float fx, float fy) {
     return normalize(n);
 }
 
-static inline vec3 CubemapFaceNormal(vec3 dir) {
+static ORACLE_INLINE vec3 CubemapFaceNormal(vec3 dir) {
     vec3 a = {fabsf(dir.x), fabsf(dir.y), fabsf(dir.z)};
     float mx = a.x >= fmaxf(a.y, a.z) ? 1.0f : 0.0f;
     float my = a.y >= fmaxf(a.z, a.x) ? 1.0f : 0.0f;
@@ -537,7 +545,8 @@ static inline vec3 CubemapFaceNormal(vec3 dir) {
 }
 
 // texture(skyBoxUBO.Albedo, dir).rgb (FirstHit:227, NHit:208). Face selection and (s,t) per the OpenGL 4.6 spec table
-// 8.19 (major axis; ties x >= y >= z), then bilinear filtering inside the face with clamp-to-edge texel indices.
+// 8.19 (major axis; ties x >= y >= z), then bilinear filtering inside the face with clamp-to-edge texel indices. Not forced
+// inline: it runs once per ray that leaves the scene, and out of line it keeps its texel lambdas inlined.
 struct Scene;
 static inline vec3 SampleSky(const float* const faces[6], int size, const float* constant, vec3 d) {
     if (size == 0) return V(constant);
@@ -614,7 +623,7 @@ static Surface GetDefaultSurface() {
 // texture(sampler2D, uv) at lod 0 (compute shaders have no derivatives, Surface.glsl:57-60): explicit fp32 bilinear on the base
 // level, glTF wrap modes, sRGB decode before filtering. Handle 0 = 1x1 white, k = Textures[k-1] (include/idkpt.h).
 struct Vec4 { float x, y, z, w; };
-static inline int TexWrap(int i, int n, int mode) {
+static ORACLE_INLINE int TexWrap(int i, int n, int mode) {
     if (mode == 33071) return i < 0 ? 0 : (i > n - 1 ? n - 1 : i);
     if (mode == 33648) { int m = i % (2 * n); if (m < 0) m += 2 * n; return m < n ? m : 2 * n - 1 - m; }
     int m = i % n;
@@ -635,7 +644,7 @@ static const float* SrgbLut() {
 // The oracle samples UNCOMPRESSED texels only (RGBA8 unorm / sRGB, R / RG / RGBA 32F; GL channel defaults (R,G,0,1) for missing
 // channels). Block-compressed textures reach it already decoded by tests/bcn_ref.py, an implementation that shares no code
 // with the CUDA decoders (csrc/idk_bcn.cuh) -- the two are then compared through the rendered images.
-static inline Vec4 TexFetch(const IdkPtTextureDesc& t, int x, int y) {
+static ORACLE_INLINE Vec4 TexFetch(const IdkPtTextureDesc& t, int x, int y) {
     const size_t i = (size_t)y * t.Width + x;
     Vec4 r;
     if (t.Format == IDKPT_TEX_RG32F) { const float* c = (const float*)t.Pixels + 2 * i; r = {c[0], c[1], 0.0f, 1.0f}; }
@@ -649,7 +658,7 @@ static inline Vec4 TexFetch(const IdkPtTextureDesc& t, int x, int y) {
     if (t.Flags & IDKPT_TEX_FLAG_R_FROM_B) r.x = r.z;      // texture.SetSwizzleR(Swizzle.B), ModelLoader.cs:989-994
     return r;
 }
-static inline Vec4 TexLerp(Vec4 a, Vec4 b, float t) {
+static ORACLE_INLINE Vec4 TexLerp(Vec4 a, Vec4 b, float t) {
     const float s = 1.0f - t;
     return {a.x * s + b.x * t, a.y * s + b.y * t, a.z * s + b.z * t, a.w * s + b.w * t};
 }
@@ -669,7 +678,7 @@ static Vec4 TexSample(const IdkPtSceneDesc& d, uint64_t handle, float u, float v
     const Vec4 b = TexLerp(TexFetch(t, x0, y1), TexFetch(t, x1, y1), fx);
     return TexLerp(a, b, fy);
 }
-static inline bool MaterialHasTextures(const GpuMaterial& m) {
+static ORACLE_INLINE bool MaterialHasTextures(const GpuMaterial& m) {
     return (m.BaseColorTexture | m.MetallicRoughnessTexture | m.NormalTexture | m.EmissiveTexture | m.TransmissionTexture) != 0;
 }
 
@@ -697,7 +706,7 @@ static Surface GetSurface(const IdkPtSceneDesc& d, const GpuMaterial& m, float u
     s.TintOnTransmissive = true;
     return s;
 }
-static inline void InterpTexCoord(const IdkPtSceneDesc& d, const GpuBlasTriangle& tri, float b0, float b1, float b2, float& u, float& v) {
+static ORACLE_INLINE void InterpTexCoord(const IdkPtSceneDesc& d, const GpuBlasTriangle& tri, float b0, float b1, float b2, float& u, float& v) {
     const GpuVertex& v0 = d.Vertices[tri.X]; const GpuVertex& v1 = d.Vertices[tri.Y]; const GpuVertex& v2 = d.Vertices[tri.Z];
     u = (v0.TexCoord[0] * b0 + v1.TexCoord[0] * b1) + v2.TexCoord[0] * b2;   // Interpolate(), Math.glsl:54-57
     v = (v0.TexCoord[1] * b0 + v1.TexCoord[1] * b1) + v2.TexCoord[1] * b2;
@@ -730,11 +739,11 @@ static void SurfaceApplyModificatons(Surface& s, const GpuMesh& mesh) {
     s.IOR = fmaxf(s.IOR + mesh.IORBias, 1.0f);
     s.TintOnTransmissive = mesh.TintOnTransmissive != 0;
 }
-static inline float GetSurfaceVariance(float specularChance, float transmissionChance, float roughness) {
+static ORACLE_INLINE float GetSurfaceVariance(float specularChance, float transmissionChance, float roughness) {
     float diffuseChance = 1.0f - specularChance - transmissionChance;
     return diffuseChance + specularChance * roughness + transmissionChance * roughness;
 }
-static inline float pow5(float x) { float x2 = x * x; return (x2 * x2) * x; }
+static ORACLE_INLINE float pow5(float x) { float x2 = x * x; return (x2 * x2) * x; }
 
 enum { BSDF_DIFFUSE = 0, BSDF_SPECULAR = 1, BSDF_TRANSMISSIVE = 2 };
 struct SampleMaterialResult { vec3 RayDirection; uint32_t BsdfType; vec3 Bsdf; float Pdf; float NewIor; };
@@ -1004,7 +1013,8 @@ static vec3 TurboColormap(float x) {
 // Persistent worker pool with dynamic chunking (round-1 verdict: spawning `threads` fresh std::threads per phase per bounce
 // made the CPU arm noisy by 2x between boxes). Workers are created once and parked on a condition variable; a job is a
 // range cut into chunks that the workers (and the calling thread, as worker 0) claim with an atomic counter, so uneven
-// rows / rays balance themselves. f(begin, end, workerId) may be called several times per worker.
+// rows / rays balance themselves. f(begin, end, workerId) may be called several times per worker. Every entry point of
+// liboracle.so shares the one pool, and it runs one job at a time.
 class WorkerPool {
 public:
     static WorkerPool& get() { static WorkerPool p; return p; }
@@ -1550,7 +1560,7 @@ ORACLE_API int oracle_shadows_ray_traced(const IdkPtSceneDesc* scene, const GpuP
 // ---- dynamic geometry (SURVEY.md 8f.2) --------------------------------------------------------------------------------------
 // Test infrastructure like the rest of this file: CPU restatement of Skinning/compute.glsl and of BLAS.Refit.
 
-static inline uint32_t CompressSR11G11B10(vec3 v) {
+static ORACLE_INLINE uint32_t CompressSR11G11B10(vec3 v) {
     // Compression.glsl:1-28; round() half-way case: floor(x + 0.5) (GLSL leaves it to the implementation)
     const float x = v.x * 0.5f + 0.5f, y = v.y * 0.5f + 0.5f, z = v.z * 0.5f + 0.5f;
     const uint32_t r = (uint32_t)floorf(x * 2047.0f + 0.5f);

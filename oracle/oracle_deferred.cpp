@@ -1,8 +1,8 @@
 // ORACLE (TEST INFRASTRUCTURE ONLY) -- the raster mode's G-buffer lighting: SSAO and the deferred lighting pass with its
 // PCF / ray-traced point shadows and VXGI indirect light.
 //
-// Built as its own library (tests/deferred_oracle.py -> oracle/liboracle_deferred.so). It compiles oracle_point_shadows.cpp
-// (and with it oracle.cpp) into the same translation unit and reuses its cube-map footprint (CubeFootprint),
+// Part of liboracle.so (wrapped by tests/deferred_oracle.py). It includes oracle_point_shadows.cpp (and with it oracle.cpp)
+// and reuses its cube-map footprint (CubeFootprint),
 // GetLogarithmicDepth, DecodeUnitVec, SampleSphere, InterleavedGradientNoise and the det_exp / det_log2 polynomials
 // unchanged; what it adds is restated here from the shaders.
 //
@@ -14,6 +14,7 @@
 //                                                                SmithGGXCorrelated, FresnelSchlick, GGXBrdf
 //   Resource/Shaders/include/Math.glsl:75-87                    PerspectiveTransform, PerspectiveTransformUvDepth
 //   Source/Render/CpuPointShadow.cs:211-218, 242                 the shadow sampler (LINEAR, compare LESS); R8Unorm RT images
+#pragma once
 #include "oracle_point_shadows.cpp"
 
 namespace {

@@ -1,7 +1,7 @@
 // ORACLE (TEST INFRASTRUCTURE ONLY) -- the G-buffer pass, ray-cast at pixel centres.
 //
-// Built as its own library (tests/gbuffer_oracle.py -> oracle/liboracle_gbuffer.so). It compiles oracle.cpp into the same
-// translation unit and reuses its scene access, RayTriangleIntersect, RayBoxIntersect, RayTransform, GetSurface,
+// Part of liboracle.so (wrapped by tests/gbuffer_oracle.py). It includes oracle.cpp and reuses its scene access,
+// RayTriangleIntersect, RayBoxIntersect, RayTransform, GetSurface,
 // SurfaceApplyModificatons, TexSample, InterpTexCoord, DecompressSR11G11B10, EncodeUnitVec and the half conversion unchanged;
 // the serial walk with the depth test's acceptance rules and the fragment stage are restated here.
 //
@@ -17,6 +17,7 @@
 // clipped (screen-linear depth outside [0, 1]), blended, back-facing on a single-sided material (det(Model) * dot(n, d) sign)
 // or alpha-discarded; depth = (sum b_i clip_i.z) / (sum b_i clip_i.w); the vertex shader's order (transform, then interpolate);
 // R11G11B10F nearest-even, RG8 through the R8 rule, RG16F nearest-even.
+#pragma once
 #include "oracle.cpp"
 
 #include <cmath>

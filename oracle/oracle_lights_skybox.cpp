@@ -1,7 +1,7 @@
 // ORACLE (TEST INFRASTRUCTURE ONLY) -- the light spheres and the skybox, ray-cast at pixel centres.
 //
-// Built as its own library (tests/lights_skybox_oracle.py -> oracle/liboracle_lights_skybox.so). It compiles the G-buffer
-// oracle (and with it oracle.cpp) into the same translation unit and reuses its clip transform, front-face rule and attachment
+// Part of liboracle.so (wrapped by tests/lights_skybox_oracle.py). It includes the G-buffer oracle (and with it oracle.cpp)
+// and reuses its clip transform, front-face rule and attachment
 // conversions, and oracle.cpp's RayTriangleIntersect, EncodeUnitVec, SampleSky and half conversion unchanged. The sphere mesh,
 // the brute-force light draw (every triangle of every light, no rejection) and the skybox draw are restated here.
 //
@@ -13,6 +13,7 @@
 //   Source/Render/RasterPipeline.cs:465-516                    the two draws: LESS + CullFace, then LEQUAL without culling
 //
 // DESIGN.md 8f.1i pins the rules.
+#pragma once
 #include "oracle_gbuffer.cpp"
 
 namespace {

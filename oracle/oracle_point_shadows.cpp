@@ -1,8 +1,7 @@
 // ORACLE (TEST INFRASTRUCTURE ONLY) -- point-shadow cube maps and the voxeliser's PCF lookup into them.
 //
-// Built as its own library (tests/point_shadow_oracle.py -> oracle/liboracle_point_shadows.so). It compiles oracle.cpp into
-// the same translation unit and reuses its scene access, TraceRay, GetSurface and VXGI helpers unchanged; what it adds is
-// restated here.
+// Part of liboracle.so (wrapped by tests/point_shadow_oracle.py). It includes oracle.cpp and reuses its scene access, TraceRay,
+// GetSurface and VXGI helpers unchanged; what it adds is restated here.
 //
 // Restated sources (relative to the reference repository's IDKEngine):
 //   Source/Render/CpuPointShadow.cs:116-232                 the raster pass (depth test only, no culling, D16Unorm, Fill(1.0)),
@@ -10,6 +9,7 @@
 //   Resource/Shaders/include/Math.glsl:59-66                GetLogarithmicDepth
 //   Resource/Shaders/VXGI/Voxelize/Voxelize/fragment.glsl:31-117   fragment stage incl. Visibility() / GetLightSpaceDepth
 //   OpenGL 4.6 spec 8.13 (table 8.19), 8.14.2, 8.17 (seamless cube maps), 8.23.1 (depth compare)
+#pragma once
 #include "oracle.cpp"
 
 namespace {

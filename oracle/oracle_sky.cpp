@@ -1,8 +1,8 @@
 // ORACLE (TEST INFRASTRUCTURE ONLY) -- the sky cube map generated on the device: atmospheric scattering and the
 // equirectangular import.
 //
-// Built as its own library (tests/sky_oracle.py -> oracle/liboracle_sky.so). It compiles oracle.cpp into the same translation
-// unit and reuses its normalize, det_sincos / det_exp / det_log2 polynomials and the half conversion unchanged; the two
+// Part of liboracle.so (wrapped by tests/sky_oracle.py). It includes oracle.cpp and reuses its normalize, det_sincos / det_exp
+// / det_log2 polynomials and the half conversion unchanged; the two
 // shaders, GetWorldSpaceDirection and the atan2 / asin polynomials are restated here.
 //
 // Restated sources (relative to the reference repository's IDKEngine):
@@ -14,6 +14,7 @@
 //   OpenGL 4.6 spec 8.14.2                                     LINEAR filtering with REPEAT on the texel indices
 //
 // DESIGN.md 8f.1j pins the rules.
+#pragma once
 #include "oracle.cpp"
 
 namespace {

@@ -1,8 +1,8 @@
 // ORACLE (TEST INFRASTRUCTURE ONLY) -- the end of the raster frame: screen-space reflections, the lighting merge and one TAA
 // resolve step.
 //
-// Built as its own library (tests/ssr_taa_oracle.py -> oracle/liboracle_ssr_taa.so). It compiles oracle_deferred.cpp (and
-// with it oracle_point_shadows.cpp and oracle.cpp) into the same translation unit and reuses SampleSky, PostBilinear /
+// Part of liboracle.so (wrapped by tests/ssr_taa_oracle.py). It includes oracle_deferred.cpp (and with it
+// oracle_point_shadows.cpp and oracle.cpp) and reuses SampleSky, PostBilinear /
 // PostTex, the rgba16f conversions, DfPerspective, DfNearest, DecodeUnitVec, normalize, reflect, mixf and fractf unchanged;
 // what it adds is restated here from the shaders. The TAA history is the caller's: each call is one resolve step.
 //
@@ -12,6 +12,7 @@
 //   Resource/Shaders/TAAResolve/compute.glsl          the resolve, GetResolveData, SampleTextureCatmullRom;
 //                                                      Source/Render/TAAResolve.cs (rgba16f ping-pong, LINEAR, clamp to edge)
 //   Source/Render/RasterPipeline.cs:672-676            the velocity texture (R16G16F, NEAREST)
+#pragma once
 #include "oracle_deferred.cpp"
 
 namespace {

@@ -1,13 +1,12 @@
 // ORACLE (TEST INFRASTRUCTURE ONLY) -- transparency: the record pass's blended fragments, ray-cast at pixel centres, lit, and
 // resolved front to back over the lit image.
 //
-// Built as its own library (tests/transparency_oracle.py -> oracle/liboracle_transparency.so). It compiles
-// oracle_deferred.cpp (and with it oracle_point_shadows.cpp and oracle.cpp) into the same translation unit and reuses its
-// EvaluateLighting / GGXBrdf (DfSurface carries the IOR), the 21-tap PCF filter (DfVisibility), DfPerspective, and oracle.cpp's
-// RayTriangleIntersect, RayBoxIntersect, RayTransform, GetSurface, SurfaceApplyModificatons, InterpTexCoord,
-// DecompressSR11G11B10, SampleSky, InterleavedGradientNoise, vx_trace_cone and the half conversion unchanged. oracle.cpp has no
-// include guard, so oracle_gbuffer.cpp (which includes it too) cannot join the same translation unit: the G-buffer pass's
-// geometric rules it needs (clip position, depth, front face, the per-vertex world normal) are the few lines restated below.
+// Part of liboracle.so (wrapped by tests/transparency_oracle.py). It includes oracle_deferred.cpp (and with it
+// oracle_point_shadows.cpp and oracle.cpp) and oracle_gbuffer.cpp, and reuses EvaluateLighting / GGXBrdf (DfSurface carries
+// the IOR), the 21-tap PCF filter (DfVisibility), DfPerspective, the G-buffer pass's geometric rules (GbDepth, GbDet,
+// GbFrontFacing, GbUnitVecToWorld), and oracle.cpp's RayTriangleIntersect, RayBoxIntersect, RayTransform, GetSurface,
+// SurfaceApplyModificatons, InterpTexCoord, DecompressSR11G11B10, SampleSky, InterleavedGradientNoise, vx_trace_cone and the
+// half conversion unchanged.
 //
 // Restated sources (relative to the reference repository's IDKEngine):
 //   Resource/Shaders/RecordTransparent/fragment.glsl            the record fragment shader (lighting, premultiplied rgba16f)
@@ -19,7 +18,9 @@
 // DESIGN.md 8f.1h pins the rules: the G-buffer pass's ray; a candidate is kept if blended, front-facing or double-sided, depth
 // in [0, 1] and below the opaque depth, alpha != 0; the 10 smallest (depth, BLAS triangle, MeshTransformId) are kept, in that
 // order; the walk's bound is the reconstructed opaque distance times 1.125 (unbounded where the depth is not below 1).
+#pragma once
 #include "oracle_deferred.cpp"
+#include "oracle_gbuffer.cpp"
 
 namespace {
 
@@ -30,34 +31,6 @@ struct TrLayer { float depth; uint32_t tri, xf; float bx, by; };
 
 static inline bool TrBefore(const TrLayer& a, const TrLayer& b) {
     return a.depth < b.depth || (a.depth == b.depth && (a.tri < b.tri || (a.tri == b.tri && a.xf < b.xf)));
-}
-
-// The G-buffer pass's geometric rules (DESIGN.md 8f.1g rules 2-4), as oracle_gbuffer.cpp states them.
-static inline vec3 TrXformPoint(const float m[3][4], vec3 p) {
-    return {((m[0][0] * p.x + m[0][1] * p.y) + m[0][2] * p.z) + m[0][3], ((m[1][0] * p.x + m[1][1] * p.y) + m[1][2] * p.z) + m[1][3],
-            ((m[2][0] * p.x + m[2][1] * p.y) + m[2][2] * p.z) + m[2][3]};
-}
-static inline vec3 TrUnitVecToWorld(const float im[3][4], vec3 v) {
-    return {(im[0][0] * v.x + im[1][0] * v.y) + im[2][0] * v.z, (im[0][1] * v.x + im[1][1] * v.y) + im[2][1] * v.z,
-            (im[0][2] * v.x + im[1][2] * v.y) + im[2][2] * v.z};
-}
-static inline float TrDet(const float m[3][4]) {
-    return (m[0][0] * (m[1][1] * m[2][2] - m[1][2] * m[2][1]) - m[0][1] * (m[1][0] * m[2][2] - m[1][2] * m[2][0])) +
-           m[0][2] * (m[1][0] * m[2][1] - m[1][1] * m[2][0]);
-}
-static inline bool TrFrontFacing(float det, vec3 nLocal, vec3 ld) {
-    const float dn = dot(nLocal, ld);
-    return (det > 0.0f && dn < 0.0f) || (det < 0.0f && dn > 0.0f);
-}
-static float TrDepth(const float* pv, const Scene& s, const float model[3][4], const GpuBlasTriangle& tri, float b0, float b1, float b2) {
-    float cz[3], cw[3];
-    const int32_t ids[3] = {tri.X, tri.Y, tri.Z};
-    for (int i = 0; i < 3; i++) {
-        const vec3 p = TrXformPoint(model, pos(s, ids[i]));
-        cz[i] = ((pv[2] * p.x + pv[6] * p.y) + pv[10] * p.z) + pv[14];
-        cw[i] = ((pv[3] * p.x + pv[7] * p.y) + pv[11] * p.z) + pv[15];
-    }
-    return ((cz[0] * b0 + cz[1] * b1) + cz[2] * b2) / ((cw[0] * b0 + cw[1] * b1) + cw[2] * b2);
 }
 
 struct TrWalk {
@@ -81,10 +54,10 @@ struct TrWalk {
         if (material.AlphaCutoff != 2.0f) return;
         if (!material.IsDoubleSided) {
             const vec3 p0 = pos(s, tri.X), p1 = pos(s, tri.Y), p2 = pos(s, tri.Z);
-            if (!TrFrontFacing(det, cross(p1 - p0, p2 - p0), localRay.d)) return;
+            if (!GbFrontFacing(det, cross(p1 - p0, p2 - p0), localRay.d)) return;
         }
         const float b2 = 1.0f - b0 - b1;
-        const float depth = TrDepth(f.ProjView, s, mt.ModelMatrix, tri, b0, b1, b2);
+        const float depth = GbDepth(f.ProjView, s.d.VertexPositions, mt.ModelMatrix, tri, b0, b1, b2);
         if (!(depth >= 0.0f && depth <= 1.0f && depth < opaqueDepth)) return;
         float u, v;
         InterpTexCoord(s.d, tri, b0, b1, b2, u, v);
@@ -98,7 +71,7 @@ struct TrWalk {
         float tMinLeft, tMinRight;
         const GpuBlasNode* nodes = s.d.BlasNodes + blasDesc.NodeOffset;
         const vec3 invDir = {1.0f / ray.d.x, 1.0f / ray.d.y, 1.0f / ray.d.z};
-        const float det = TrDet(mt.ModelMatrix);
+        const float det = GbDet(mt.ModelMatrix);
         if (!useTlas) {
             const GpuBlasNode& rootNode = nodes[1];
             if (!(RayBoxIntersect(ray, invDir, rootNode.Min, rootNode.Max, tMinLeft) && tMinLeft < tMax)) return;
@@ -228,8 +201,8 @@ static bool TrPixel(const Scene& s, const GpuPerFrameData& f, const TrInputs& in
         const GpuVertex* vs[3] = {&s.d.Vertices[tri.X], &s.d.Vertices[tri.Y], &s.d.Vertices[tri.Z]};
         vec3 wn[3], wt[3];
         for (int i = 0; i < 3; i++) {
-            wn[i] = normalize(TrUnitVecToWorld(mt.InvModelMatrix, DecompressSR11G11B10(vs[i]->Normal)));
-            wt[i] = normalize(TrUnitVecToWorld(mt.InvModelMatrix, DecompressSR11G11B10(vs[i]->Tangent)));
+            wn[i] = normalize(GbUnitVecToWorld(mt.InvModelMatrix, DecompressSR11G11B10(vs[i]->Normal)));
+            wt[i] = normalize(GbUnitVecToWorld(mt.InvModelMatrix, DecompressSR11G11B10(vs[i]->Tangent)));
         }
         const vec3 interpNormal = normalize((wn[0] * b0 + wn[1] * b1) + wn[2] * b2);
         const vec3 interpTangent = normalize((wt[0] * b0 + wt[1] * b1) + wt[2] * b2);
@@ -241,7 +214,7 @@ static bool TrPixel(const Scene& s, const GpuPerFrameData& f, const TrInputs& in
         const vec3 sn = surface.Normal;
         vec3 normal = normalize(mix(interpNormal, (T * sn.x + B * sn.y) + N * sn.z, mesh.NormalMapStrength));
         const vec3 p0 = pos(s, tri.X), p1 = pos(s, tri.Y), p2 = pos(s, tri.Z);
-        if (!TrFrontFacing(TrDet(mt.ModelMatrix), cross(p1 - p0, p2 - p0), RayTransform(Ray{viewPos, dir}, mt.InvModelMatrix).d)) normal = normal * -1.0f;
+        if (!GbFrontFacing(GbDet(mt.ModelMatrix), cross(p1 - p0, p2 - p0), RayTransform(Ray{viewPos, dir}, mt.InvModelMatrix).d)) normal = normal * -1.0f;
 
         const vec3 fragPos = DfPerspective(f.InvProjView, nx, ny, l.depth);
         const vec3 unjitteredFragPos = DfPerspective(f.InvProjView, nx - jitter[0], ny - jitter[1], l.depth);

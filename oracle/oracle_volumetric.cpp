@@ -1,8 +1,8 @@
 // ORACLE (TEST INFRASTRUCTURE ONLY) -- the volumetric lighting pass: a ray march through the point-shadow cube maps and its
 // depth-aware upscale.
 //
-// Built as its own library (tests/volumetric_oracle.py -> oracle/liboracle_volumetric.so). It compiles
-// oracle_point_shadows.cpp (and with it oracle.cpp) into the same translation unit and reuses its GetLogarithmicDepth, the
+// Part of liboracle.so (wrapped by tests/volumetric_oracle.py). It includes oracle_point_shadows.cpp (and with it
+// oracle.cpp) and reuses its GetLogarithmicDepth, the
 // det_exp / det_log2 polynomials and the present chain's PostTex / PostBilinear / half conversions unchanged; what it adds
 // is restated here, including its own NEAREST cube-map lookup.
 //
@@ -14,6 +14,7 @@
 //   Resource/Shaders/include/Math.glsl:68-73, Pbr.glsl:9-17    LogarithmicDepthToLinearViewDepth, GetAttenuationFactor
 //   Source/Render/CpuPointShadow.cs:220-230                    the shadow map's plain sampler (NEAREST, no compare)
 //   OpenGL 4.6 spec 8.13 (table 8.19)                          cube-map face selection
+#pragma once
 #include "oracle_point_shadows.cpp"
 
 namespace {

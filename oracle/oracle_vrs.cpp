@@ -1,8 +1,8 @@
 // ORACLE (TEST INFRASTRUCTURE ONLY) -- variable-rate deferred lighting: the lighting shading-rate classifier and the deferred
 // lighting draw under its rate image.
 //
-// Built as its own library (tests/vrs_oracle.py -> oracle/liboracle_vrs.so). It compiles oracle_deferred.cpp (and with it
-// oracle_point_shadows.cpp and oracle.cpp) into the same translation unit and reuses EvaluateLighting, DfVisibility,
+// Part of liboracle.so (wrapped by tests/vrs_oracle.py). It includes oracle_deferred.cpp (and with it oracle_point_shadows.cpp
+// and oracle.cpp) and reuses EvaluateLighting, DfVisibility,
 // DfPerspective, DfStoreR8, DecodeUnitVec and mixf unchanged; what it adds is restated here from the shaders and from
 // NV_shading_rate_image.
 //
@@ -16,6 +16,7 @@
 // The rules DESIGN.md 8f.1f pins: the per-warp xor butterfly (16, 8, 4, 2, 1) and the in-order sum of the eight warp sums;
 // round() half to even; uint() as cvt.rzi.sat.u32 (NaN and negatives 0, overflow UINT_MAX); edge lanes read colour 0 and
 // velocity 0 and still count in the 256; a coarse fragment's sample at the centre of its area with imgCoord clamped to the image.
+#pragma once
 #include "oracle_deferred.cpp"
 
 #include <cfenv>

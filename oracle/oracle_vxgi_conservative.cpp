@@ -1,13 +1,14 @@
 // ORACLE (TEST INFRASTRUCTURE ONLY) -- the voxeliser under Voxelizer.IsConservativeRasterization.
 //
-// Built as its own library (tests/vxgi_conservative_oracle.py -> oracle/liboracle_vxgi_conservative.so). It compiles
-// oracle_point_shadows.cpp (and with it oracle.cpp and oracle_vxgi.inc) into the same translation unit and reuses the
+// Part of liboracle.so (wrapped by tests/vxgi_conservative_oracle.py). It includes oracle_point_shadows.cpp (and with it
+// oracle.cpp and oracle_vxgi.inc) and reuses the
 // projection, both fragment stages (vx_fragment: shadow rays; vx_fragment_pcf: the PCF lookup), the merge and the mip chain
 // unchanged; what it adds is the coverage rule, stated in DESIGN.md section 7 and restated here.
 //
 // Restated sources (relative to the reference repository's IDKEngine):
 //   Source/Render/VXGI/Voxelizer/Voxelizer.cs:41-56,142     IsConservativeRasterization -> GL_NV_conservative_raster
 //   Resource/Shaders/VXGI/Voxelize/Voxelize/{vertex,geometry,fragment}.glsl   as in oracle_vxgi.inc
+#pragma once
 #include "oracle_point_shadows.cpp"
 
 #include <climits>

@@ -1,7 +1,7 @@
 // ORACLE (TEST INFRASTRUCTURE ONLY) -- the VXGI grid visualisation, Voxelizer.DebugRender.
 //
-// Built as its own library (tests/vxgi_debug_oracle.py -> oracle/liboracle_vxgi_debug.so). It compiles oracle.cpp (and with it
-// oracle_vxgi.inc) into the same translation unit and reuses its SampleSky, vx_trace_cone and the half conversion unchanged.
+// Part of liboracle.so (wrapped by tests/vxgi_debug_oracle.py). It includes oracle.cpp (and with it oracle_vxgi.inc) and
+// reuses its SampleSky, vx_trace_cone and the half conversion unchanged.
 // The march here fetches every sample: the device kernel's empty-space skipping is exact (DESIGN.md 8f.1k), so it has no
 // counterpart in the oracle.
 //
@@ -11,6 +11,7 @@
 //   Resource/Shaders/include/IntersectionRoutines.glsl:25-40         RayBoxIntersect with t1 and t2
 //   Resource/Shaders/include/TraceCone.glsl:41-46                    the four-argument TraceCone
 //   Source/Render/VXGI/Voxelizer/Voxelizer.cs:230-244                DebugRender
+#pragma once
 #include "oracle.cpp"
 
 namespace {

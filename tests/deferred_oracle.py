@@ -1,54 +1,11 @@
-"""ctypes wrapper of the G-buffer lighting oracle (oracle/oracle_deferred.cpp -> oracle/liboracle_deferred.so), which
-tests/test_deferred*.py use. The library is compiled on first use with the flags of oracle/build.py."""
+"""ctypes wrapper of the G-buffer lighting oracle (oracle/oracle_deferred.cpp in oracle/liboracle.so), which tests/test_deferred*.py
+use."""
 import ctypes
-import os
-import subprocess
 
 import numpy as np
 
-from idkengine_b200 import capi, gpu_types as gt
-
-REPO = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-ORACLE_DIR = os.path.join(REPO, "oracle")
-SRC = os.path.join(ORACLE_DIR, "oracle_deferred.cpp")
-LIB = os.path.join(ORACLE_DIR, "liboracle_deferred.so")
-
-_lib = None
-
-
-def build(force=False):
-    deps = [SRC] + [os.path.join(ORACLE_DIR, f) for f in ("oracle_point_shadows.cpp", "oracle.cpp", "oracle_vxgi.inc", "oracle_post.inc")] + \
-        [os.path.join(REPO, "include", f) for f in ("idkpt.h", "idkvx.h", "idk_gpu_types.h")]
-    if not force and os.path.exists(LIB) and all(os.path.getmtime(d) <= os.path.getmtime(LIB) for d in deps):
-        return LIB
-    tmp = LIB + ".%d.tmp" % os.getpid()
-    subprocess.run(["g++", "-O2", "-std=c++17", "-ffp-contract=off", "-fno-fast-math", "-fPIC", "-shared", "-pthread",
-                    "-fvisibility=hidden", "-o", tmp, SRC], check=True)
-    os.replace(tmp, LIB)
-    return LIB
-
-
-def lib():
-    global _lib
-    if _lib is None:
-        L = ctypes.CDLL(build())
-        vp, i32, u64 = ctypes.c_void_p, ctypes.c_int32, ctypes.c_uint64
-        L.oracle_ssao.restype = i32
-        L.oracle_ssao.argtypes = [vp, ctypes.POINTER(capi.IdkPtSsaoSettings), vp, vp, i32, i32, vp]
-        L.oracle_deferred_lighting.restype = i32
-        L.oracle_deferred_lighting.argtypes = [vp, u64, vp, i32, vp, vp, vp, i32, vp, vp, vp, vp, vp, i32, i32, vp, vp, vp, vp, i32, vp]
-        L.oracle_deferred_visibility.restype = None
-        L.oracle_deferred_visibility.argtypes = [vp, i32, vp, vp, u64, vp]
-        L.oracle_ggx_brdf.restype = None
-        L.oracle_ggx_brdf.argtypes = [vp, u64, vp]
-        L.oracle_store_r8.restype = None
-        L.oracle_store_r8.argtypes = [vp, u64, vp]
-        _lib = L
-    return _lib
-
-
-def _f32(a):
-    return np.ascontiguousarray(a, np.float32)
+from idkengine_b200 import gpu_types as gt
+from oracle_lib import _f32, lib, pack_shadow_maps
 
 
 def ssao(frame, settings, depth, normal_rg):
@@ -61,15 +18,11 @@ def ssao(frame, settings, depth, normal_rg):
     return out
 
 
-def deferred_lighting(lights, frame, shadow_mode, shadows, maps, gbuffer, jitter=None, ssao=None, indirect=None, rt=None):
-    """The deferred lighting draw: gbuffer = (depth [H, W], normal [H, W, 2], albedo [H, W, 3], metallic/roughness [H, W, 2],
-    emissive [H, W, 3]); shadows (GpuPointShadow) with one uint16 [6, N, N] map each; ssao uint8 [H, W] (IsSSAO) or None;
-    indirect float32 [H, W, 4] (IsVXGI) or None; rt: one float32 [H, W] image per shadow (ShadowMode 2). -> float32 [H, W, 4]."""
+def deferred_args(lights, frame, shadow_mode, shadows, maps, gbuffer, jitter, ssao, indirect, rt):
+    """oracle_deferred_lighting's arguments before its output, the arrays to keep alive while they are used, and (h, w)."""
     lt = np.ascontiguousarray(lights, gt.GpuLight)
-    sh = np.ascontiguousarray(shadows, gt.GpuPointShadow).reshape(-1)
+    sh, sizes, texels = pack_shadow_maps(shadows, maps)
     assert len(sh) == len(maps)
-    sizes = np.array([m.shape[1] for m in maps] or [0], np.int32)
-    texels = np.ascontiguousarray(np.concatenate([np.ascontiguousarray(m, np.uint16).ravel() for m in maps]) if maps else np.zeros(1, np.uint16))
     d, n, a, mr, e = [_f32(x) for x in gbuffer]
     h, w = d.shape
     fr = np.ascontiguousarray(frame)
@@ -78,12 +31,21 @@ def deferred_lighting(lights, frame, shadow_mode, shadows, maps, gbuffer, jitter
     gi = None if indirect is None else _f32(indirect)
     rts = [_f32(x) for x in (rt or [])]
     rt_ptrs = (ctypes.c_void_p * max(len(rts), 1))(*[x.ctypes.data for x in rts])
+    keep = (lt, sh, sizes, texels, d, n, a, mr, e, fr, jit, ao, gi, rts, rt_ptrs)
+    args = [lt.ctypes.data if len(lt) else None, len(lt), fr.ctypes.data, shadow_mode, sh.ctypes.data if len(sh) else None,
+            sizes.ctypes.data, texels.ctypes.data, len(sh), d.ctypes.data, n.ctypes.data, a.ctypes.data, mr.ctypes.data, e.ctypes.data,
+            w, h, jit.ctypes.data if jit is not None else None, ao.ctypes.data if ao is not None else None,
+            gi.ctypes.data if gi is not None else None, rt_ptrs, len(rts)]
+    return args, keep, (h, w)
+
+
+def deferred_lighting(lights, frame, shadow_mode, shadows, maps, gbuffer, jitter=None, ssao=None, indirect=None, rt=None):
+    """The deferred lighting draw: gbuffer = (depth [H, W], normal [H, W, 2], albedo [H, W, 3], metallic/roughness [H, W, 2],
+    emissive [H, W, 3]); shadows (GpuPointShadow) with one uint16 [6, N, N] map each; ssao uint8 [H, W] (IsSSAO) or None;
+    indirect float32 [H, W, 4] (IsVXGI) or None; rt: one float32 [H, W] image per shadow (ShadowMode 2). -> float32 [H, W, 4]."""
+    args, keep, (h, w) = deferred_args(lights, frame, shadow_mode, shadows, maps, gbuffer, jitter, ssao, indirect, rt)
     out = np.zeros((h, w, 4), np.float32)
-    rc = lib().oracle_deferred_lighting(lt.ctypes.data if len(lt) else None, len(lt), fr.ctypes.data, shadow_mode,
-                                        sh.ctypes.data if len(sh) else None, sizes.ctypes.data, texels.ctypes.data, len(sh),
-                                        d.ctypes.data, n.ctypes.data, a.ctypes.data, mr.ctypes.data, e.ctypes.data, w, h,
-                                        jit.ctypes.data if jit is not None else None, ao.ctypes.data if ao is not None else None,
-                                        gi.ctypes.data if gi is not None else None, rt_ptrs, len(rts), out.ctypes.data)
+    rc = lib().oracle_deferred_lighting(*args, out.ctypes.data)
     assert rc == 0, rc
     return out
 

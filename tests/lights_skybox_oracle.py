@@ -1,50 +1,16 @@
-"""ctypes wrapper of the light-sphere and skybox oracle (oracle/oracle_lights_skybox.cpp -> oracle/liboracle_lights_skybox.so),
-which tests/test_lights_skybox*.py use. The library is compiled on first use with the flags of oracle/build.py."""
+"""ctypes wrapper of the light-sphere and skybox oracle (oracle/oracle_lights_skybox.cpp in oracle/liboracle.so), which
+tests/test_lights_skybox*.py use."""
 import ctypes
-import os
-import subprocess
 
 import numpy as np
 
 import oracle_lib as ol
 from idkengine_b200 import capi
-
-REPO = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-ORACLE_DIR = os.path.join(REPO, "oracle")
-SRC = os.path.join(ORACLE_DIR, "oracle_lights_skybox.cpp")
-LIB = os.path.join(ORACLE_DIR, "liboracle_lights_skybox.so")
+from oracle_lib import lib
 
 SPHERE_VERTICES, SPHERE_TRIANGLES = 169, 264
 SKY = -2       # winner codes besides light * SPHERE_TRIANGLES + triangle
 UNTOUCHED = -1
-
-_lib = None
-
-
-def build(force=False):
-    deps = [SRC] + [os.path.join(ORACLE_DIR, f) for f in ("oracle_gbuffer.cpp", "oracle.cpp", "oracle_vxgi.inc", "oracle_post.inc")] + \
-        [os.path.join(REPO, "include", f) for f in ("idkpt.h", "idkvx.h", "idk_gpu_types.h")]
-    if not force and os.path.exists(LIB) and all(os.path.getmtime(d) <= os.path.getmtime(LIB) for d in deps):
-        return LIB
-    tmp = LIB + ".%d.tmp" % os.getpid()
-    subprocess.run(["g++", "-O2", "-std=c++17", "-ffp-contract=off", "-fno-fast-math", "-fPIC", "-shared", "-pthread",
-                    "-fvisibility=hidden", "-o", tmp, SRC], check=True)
-    os.replace(tmp, LIB)
-    return LIB
-
-
-def lib():
-    global _lib
-    if _lib is None:
-        L = ctypes.CDLL(build())
-        vp, i32 = ctypes.c_void_p, ctypes.c_int32
-        L.oracle_lights_skybox.restype = i32
-        L.oracle_lights_skybox.argtypes = [ctypes.POINTER(capi.IdkPtSceneDesc), vp, vp, i32, i32, vp, vp, vp, vp, vp, vp, vp, i32]
-        L.oracle_sphere_mesh.restype = None
-        L.oracle_sphere_mesh.argtypes = [vp, vp]
-        _lib = L
-    return _lib
-
 
 def sphere_mesh():
     """(vertices float32 [169, 3], indices uint32 [264, 3]) of the unit sphere."""

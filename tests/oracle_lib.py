@@ -1,5 +1,7 @@
-"""ctypes wrapper of oracle/liboracle.so -- imported by tests/, __graft_entry__.smoke() and bench.py's CPU legs only."""
+"""ctypes wrapper of oracle/liboracle.so -- imported by tests/, __graft_entry__.smoke() and bench.py's CPU legs only.
+The per-pass wrappers (tests/*_oracle.py) call the same library through lib()."""
 import ctypes
+import importlib.util
 import os
 import sys
 
@@ -9,45 +11,131 @@ REPO = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, REPO)
 sys.path.insert(0, os.path.join(REPO, "oracle"))
 
-from idkengine_b200 import capi, gpu_types as gt  # noqa: E402
+from idkengine_b200 import capi, gpu_types as gt, vxgi  # noqa: E402
+
+
+def _signatures():
+    """Every export of the library: name -> (restype, argtypes). tests/test_oracle_library.py checks it against the sources."""
+    P = ctypes.POINTER
+    vp, f32, i32, u32, u64 = ctypes.c_void_p, ctypes.c_float, ctypes.c_int32, ctypes.c_uint32, ctypes.c_uint64
+    SCENE, SKY, CI = P(capi.IdkPtSceneDesc), P(capi.IdkPtSkyDesc), P(vxgi.IdkVxCreateInfo)
+    # oracle_deferred_lighting's arguments up to the output; the variable-rate entry points take the same ones first
+    deferred = [vp, u64, vp, i32, vp, vp, vp, i32, vp, vp, vp, vp, vp, i32, i32, vp, vp, vp, vp, i32]
+    return {
+        # oracle.cpp
+        "oracle_trace_rays": (i32, [SCENE, vp, u64, i32, vp, i32]),
+        "oracle_trace_rays_any": (i32, [SCENE, vp, u64, i32, vp, i32]),
+        "oracle_brute_force": (i32, [SCENE, vp, u64, vp, i32]),
+        "oracle_cpu_intersect": (ctypes.c_double, [SCENE, vp, u64, vp, i32]),
+        "oracle_gui_test_rays": (None, [vp, i32, i32, i32, i32, vp]),
+        "oracle_path_trace": (i32, [SCENE, SKY, vp, P(capi.IdkPtSettings), i32, i32, i32, i32, i32, P(u32), vp, vp, vp, vp,
+                                    P(capi.IdkPtStats), i32]),
+        "oracle_sample_sky": (None, [vp, vp, u64, vp]),
+        "oracle_det_sincos": (None, [vp, u64, vp, vp]),
+        "oracle_det_exp": (None, [vp, u64, vp]),
+        "oracle_encode_decode": (None, [vp, u64, vp, vp]),
+        "oracle_pcg": (u32, [u32, P(u32)]),
+        "oracle_shadows_ray_traced": (i32, [SCENE, vp, vp, vp, i32, i32, i32, i32, u32, vp, vp, i32]),
+        "oracle_skin_vertices": (None, [vp] * 4 + [u32] * 4),
+        "oracle_blas_refit": (None, [vp] * 4),
+        "oracle_tex_sample": (None, [P(capi.IdkPtTextureDesc), vp, u64, vp]),
+        # oracle_post.inc
+        "oracle_post_process": (i32, [vp, i32, i32, P(capi.IdkPtPostSettings), vp, vp, i32]),
+        "oracle_denoise": (i32, [vp, vp, vp, i32, i32, P(capi.IdkPtDenoiseSettings), vp, i32]),
+        # oracle_vxgi.inc
+        "oracle_vx_set_raster_rule": (None, [i32]),
+        "oracle_vx_voxelize": (i32, [SCENE, CI, vp, u64, P(u64), i32]),
+        "oracle_vx_mipmap": (i32, [CI, vp, i32]),
+        "oracle_vx_cone_trace": (i32, [CI, vp, vp, P(vxgi.IdkVxConeSettings), vp, vp, vp, i32, i32, vp, vp, P(u64), i32]),
+        "oracle_half_roundtrip": (None, [vp, u64, vp, vp]),
+        "oracle_det_log2": (None, [vp, u64, vp]),
+        # oracle_point_shadows.cpp
+        "oracle_point_shadow_render": (None, [SCENE, vp, i32, u32, vp]),
+        "oracle_point_shadow_visibility": (None, [vp, i32, vp, vp, u64, vp]),
+        "oracle_vx_voxelize_shadow_maps": (i32, [SCENE, CI, vp, vp, vp, i32, vp, u64, P(u64), i32]),
+        # oracle_deferred.cpp
+        "oracle_ssao": (i32, [vp, P(capi.IdkPtSsaoSettings), vp, vp, i32, i32, vp]),
+        "oracle_deferred_lighting": (i32, deferred + [vp]),
+        "oracle_deferred_visibility": (None, [vp, i32, vp, vp, u64, vp]),
+        "oracle_ggx_brdf": (None, [vp, u64, vp]),
+        "oracle_store_r8": (None, [vp, u64, vp]),
+        # oracle_vrs.cpp
+        "oracle_shading_rate": (i32, [vp, P(capi.IdkPtShadingRateSettings), vp, vp, i32, i32, vp, vp]),
+        "oracle_deferred_lighting_vrs": (i32, deferred + [vp, vp]),
+        "oracle_deferred_samples": (i32, deferred + [vp, vp, u64, vp]),
+        # oracle_ssr_taa.cpp
+        "oracle_ssr": (i32, [vp, P(capi.IdkPtSsrSettings), SKY, vp, vp, vp, vp, vp, i32, i32, vp, vp]),
+        "oracle_taa_resolve": (i32, [P(capi.IdkPtTaaSettings), vp, vp, vp, i32, i32, vp, i32, i32, vp]),
+        # oracle_gbuffer.cpp
+        "oracle_gbuffer": (i32, [SCENE, vp, i32, i32, vp, vp, vp, vp, vp, vp, vp, vp, i32]),
+        "oracle_gbuffer_store": (None, [i32, vp, u64, vp]),
+        # oracle_transparency.cpp
+        "oracle_transparency": (i32, [SCENE, SKY, vp, i32, i32, vp, vp, vp, i32, vp, vp, vp, vp, i32, i32, vp, i32, vp, vp, vp,
+                                      vp, i32]),
+        # oracle_lights_skybox.cpp
+        "oracle_lights_skybox": (i32, [SCENE, vp, vp, i32, i32, vp, vp, vp, vp, vp, vp, vp, i32]),
+        "oracle_sphere_mesh": (None, [vp, vp]),
+        # oracle_volumetric.cpp
+        "oracle_volumetric_lighting": (i32, [vp, u64, vp, P(capi.IdkPtVolumetricSettings), vp, vp, vp, i32, vp, i32, i32, i32, i32,
+                                             vp, vp, vp, vp]),
+        "oracle_volumetric_upscale": (None, [vp, vp, i32, i32, vp, vp, i32, i32, i32, i32, vp]),
+        "oracle_cube_nearest": (None, [vp, i32, vp, u64, vp]),
+        # oracle_sky.cpp
+        "oracle_sky_atmosphere": (i32, [P(capi.IdkPtAtmosphereSettings), i32, vp, i32]),
+        "oracle_sky_equirect": (i32, [vp, i32, i32, vp, i32]),
+        "oracle_sky_directions": (None, [i32, vp]),
+        "oracle_det_atan2": (None, [vp, vp, u64, vp]),
+        "oracle_det_asin": (None, [vp, u64, vp]),
+        # oracle_vxgi_conservative.cpp
+        "oracle_vx_voxelize_conservative": (i32, [SCENE, CI, vp, u64, P(u64), i32]),
+        "oracle_vx_voxelize_conservative_shadow_maps": (i32, [SCENE, CI, vp, vp, vp, i32, vp, u64, P(u64), i32]),
+        # oracle_vxgi_debug.cpp
+        "oracle_vx_debug_render": (i32, [vp, vp, vp, vp, f32, f32, i32, i32, vp, P(u64), i32]),
+    }
+
+
+SIGNATURES = _signatures()
 
 _lib = None
 
 
 def lib():
+    """oracle/liboracle.so, rebuilt first if an oracle source is newer than it, with every export's signature declared."""
     global _lib
     if _lib is None:
-        import importlib.util
         spec = importlib.util.spec_from_file_location("oracle_build", os.path.join(REPO, "oracle", "build.py"))
         ob = importlib.util.module_from_spec(spec)
         spec.loader.exec_module(ob)
-        path = ob.LIBORACLE if os.path.exists(ob.LIBORACLE) else ob.build()
-        try:
-            path = ob.build()
-        except Exception:
-            pass
-        L = ctypes.CDLL(path)
-        P = ctypes.POINTER
-        vp, u64, i32 = ctypes.c_void_p, ctypes.c_uint64, ctypes.c_int32
-        L.oracle_trace_rays.restype = i32
-        L.oracle_trace_rays.argtypes = [P(capi.IdkPtSceneDesc), vp, u64, i32, vp, i32]
-        L.oracle_brute_force.restype = i32
-        L.oracle_brute_force.argtypes = [P(capi.IdkPtSceneDesc), vp, u64, vp, i32]
-        L.oracle_cpu_intersect.restype = ctypes.c_double
-        L.oracle_cpu_intersect.argtypes = [P(capi.IdkPtSceneDesc), vp, u64, vp, i32]
-        L.oracle_gui_test_rays.restype = None
-        L.oracle_gui_test_rays.argtypes = [vp, i32, i32, i32, i32, vp]
-        L.oracle_path_trace.restype = i32
-        L.oracle_path_trace.argtypes = [P(capi.IdkPtSceneDesc), P(capi.IdkPtSkyDesc), vp, P(capi.IdkPtSettings),
-                                        i32, i32, i32, i32, i32, P(ctypes.c_uint32), vp, vp, vp, vp,
-                                        P(capi.IdkPtStats), i32]
-        L.oracle_det_sincos.argtypes = [vp, u64, vp, vp]
-        L.oracle_det_exp.argtypes = [vp, u64, vp]
-        L.oracle_encode_decode.argtypes = [vp, u64, vp, vp]
-        L.oracle_pcg.restype = ctypes.c_uint32
-        L.oracle_pcg.argtypes = [ctypes.c_uint32, P(ctypes.c_uint32)]
+        L = ctypes.CDLL(ob.build())
+        for name, (restype, argtypes) in SIGNATURES.items():
+            fn = getattr(L, name)
+            fn.restype, fn.argtypes = restype, argtypes
         _lib = L
     return _lib
+
+
+def _f32(a):
+    return np.ascontiguousarray(a, np.float32)
+
+
+def pack_shadow_maps(shadows, maps):
+    """GpuPointShadow records with one uint16 [6, N, N] cube map each -> (records, int32 sizes N, the maps' texels back to
+    back), as the oracle takes them; without maps, sizes and texels are one-element placeholders."""
+    records = np.ascontiguousarray(shadows, gt.GpuPointShadow).reshape(-1)
+    sizes = np.array([m.shape[1] for m in maps] or [0], np.int32)
+    texels = np.ascontiguousarray(np.concatenate([np.ascontiguousarray(m, np.uint16).ravel() for m in maps]) if len(maps) else
+                                  np.zeros(1, np.uint16))
+    return records, sizes, texels
+
+
+def split_levels(raw, ci):
+    """A grid's raw uint16 mip chain -> the float16 [d, h, w, 4] view of each level."""
+    levels, off = [], 0
+    for (w, h, d) in vxgi.level_sizes(ci):
+        k = w * h * d * 4
+        levels.append(raw[off:off + k].view(np.float16).reshape(d, h, w, 4))
+        off += k
+    return levels
 
 
 def default_threads():
@@ -73,9 +161,7 @@ def trace_rays(scene, rays, trace_lights=False, threads=None):
 def trace_rays_any(scene, rays, trace_lights=False, threads=None):
     d, keep = capi.scene_desc(scene)
     out = np.zeros(len(rays), gt.IdkPtHit)
-    L = lib()
-    L.oracle_trace_rays_any.argtypes = [ctypes.POINTER(capi.IdkPtSceneDesc), ctypes.c_void_p, ctypes.c_uint64, ctypes.c_int32, ctypes.c_void_p, ctypes.c_int32]
-    L.oracle_trace_rays_any(ctypes.byref(d), rays.ctypes.data, len(rays), int(trace_lights), out.ctypes.data, threads or default_threads())
+    lib().oracle_trace_rays_any(ctypes.byref(d), rays.ctypes.data, len(rays), int(trace_lights), out.ctypes.data, threads or default_threads())
     return out
 
 
@@ -86,33 +172,23 @@ def shadows_ray_traced(scene, frame, depth, normal_rg, light_index, samples=1, n
     nrg = np.ascontiguousarray(normal_rg, np.float32)
     vis = np.zeros((h, w), np.float32) if visibility is None else np.ascontiguousarray(visibility, np.float32)
     jit = np.array(jitter, np.float32)
-    L = lib()
-    L.oracle_shadows_ray_traced.restype = ctypes.c_int32
-    L.oracle_shadows_ray_traced.argtypes = [ctypes.POINTER(capi.IdkPtSceneDesc), ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int32,
-                                            ctypes.c_int32, ctypes.c_int32, ctypes.c_int32, ctypes.c_uint32, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int32]
-    rc = L.oracle_shadows_ray_traced(ctypes.byref(d), frame.ctypes.data, depth.ctypes.data, nrg.ctypes.data, w, h, light_index, samples, noise_index,
-                                     jit.ctypes.data, vis.ctypes.data, threads or default_threads())
+    rc = lib().oracle_shadows_ray_traced(ctypes.byref(d), frame.ctypes.data, depth.ctypes.data, nrg.ctypes.data, w, h, light_index, samples,
+                                         noise_index, jit.ctypes.data, vis.ctypes.data, threads or default_threads())
     assert rc == 0
     return vis
 
 
 def skin_vertices(unskinned, joint_matrices, positions, vertices, cmd):
     """In-place oracle_skin_vertices on numpy arrays (positions: PackedVec3, vertices: GpuVertex)."""
-    L = lib()
-    L.oracle_skin_vertices.restype = None
-    L.oracle_skin_vertices.argtypes = [ctypes.c_void_p] * 4 + [ctypes.c_uint32] * 4
     jm = np.ascontiguousarray(joint_matrices, np.float32)
-    L.oracle_skin_vertices(unskinned.ctypes.data, jm.ctypes.data, positions.ctypes.data, vertices.ctypes.data, int(cmd["InputVertexOffset"]),
-                           int(cmd["OutputVertexOffset"]), int(cmd["JointMatricesOffset"]), int(cmd["VertexCount"]))
+    lib().oracle_skin_vertices(unskinned.ctypes.data, jm.ctypes.data, positions.ctypes.data, vertices.ctypes.data, int(cmd["InputVertexOffset"]),
+                               int(cmd["OutputVertexOffset"]), int(cmd["JointMatricesOffset"]), int(cmd["VertexCount"]))
 
 
 def blas_refit(scene, blas_id):
     """In-place BLAS.Refit of scene.blas_nodes for one BLAS from scene.positions."""
-    L = lib()
-    L.oracle_blas_refit.restype = None
-    L.oracle_blas_refit.argtypes = [ctypes.c_void_p] * 4
     desc = np.ascontiguousarray(scene.blas_descs[blas_id:blas_id + 1])
-    L.oracle_blas_refit(scene.blas_nodes.ctypes.data, desc.ctypes.data, scene.blas_triangles.ctypes.data, scene.positions.ctypes.data)
+    lib().oracle_blas_refit(scene.blas_nodes.ctypes.data, desc.ctypes.data, scene.blas_triangles.ctypes.data, scene.positions.ctypes.data)
 
 
 def post_process(result, settings=None, want_bloom=False, threads=None):
@@ -122,12 +198,8 @@ def post_process(result, settings=None, want_bloom=False, threads=None):
     result = np.ascontiguousarray(result, np.float32)
     out = np.zeros((h, w, 4), np.uint8)
     bloom = np.zeros((max(h // 2, 1), max(w // 2, 1), 3), np.float32)
-    L = lib()
-    L.oracle_post_process.restype = ctypes.c_int32
-    L.oracle_post_process.argtypes = [ctypes.c_void_p, ctypes.c_int32, ctypes.c_int32, ctypes.POINTER(capi.IdkPtPostSettings), ctypes.c_void_p,
-                                      ctypes.c_void_p, ctypes.c_int32]
-    rc = L.oracle_post_process(result.ctypes.data, w, h, ctypes.byref(st), out.ctypes.data, bloom.ctypes.data if want_bloom else None,
-                               threads or default_threads())
+    rc = lib().oracle_post_process(result.ctypes.data, w, h, ctypes.byref(st), out.ctypes.data, bloom.ctypes.data if want_bloom else None,
+                                   threads or default_threads())
     assert rc == 0
     return (out, bloom) if want_bloom else out
 
@@ -137,10 +209,7 @@ def tex_sample(pixels, uv, srgb=False, wrap_s=10497, wrap_t=10497, flags=0):
     uv = np.ascontiguousarray(uv, np.float32)
     t = capi.IdkPtTextureDesc(px.ctypes.data, px.shape[1], px.shape[0], 1 if srgb else 0, wrap_s, wrap_t, flags)
     out = np.zeros((len(uv), 4), np.float32)
-    L = lib()
-    L.oracle_tex_sample.restype = None
-    L.oracle_tex_sample.argtypes = [ctypes.POINTER(capi.IdkPtTextureDesc), ctypes.c_void_p, ctypes.c_uint64, ctypes.c_void_p]
-    L.oracle_tex_sample(ctypes.byref(t), uv.ctypes.data, len(uv), out.ctypes.data)
+    lib().oracle_tex_sample(ctypes.byref(t), uv.ctypes.data, len(uv), out.ctypes.data)
     return out
 
 
@@ -198,71 +267,40 @@ def path_trace(scene, frame, settings, width, height, sky=(0.6, 0.7, 0.9), tile=
 
 
 # ----------------------------------------------------------------------------------------------- VXGI
-def _vx_declare():
-    L = lib()
-    from idkengine_b200 import vxgi
-    P = ctypes.POINTER
-    vp, u64, i32 = ctypes.c_void_p, ctypes.c_uint64, ctypes.c_int32
-    L.oracle_vx_voxelize.restype = i32
-    L.oracle_vx_voxelize.argtypes = [P(capi.IdkPtSceneDesc), P(vxgi.IdkVxCreateInfo), vp, u64, P(u64), i32]
-    L.oracle_vx_cone_trace.restype = i32
-    L.oracle_vx_cone_trace.argtypes = [P(vxgi.IdkVxCreateInfo), vp, vp, P(vxgi.IdkVxConeSettings), vp, vp, vp, i32, i32, vp, vp, P(u64), i32]
-    L.oracle_vx_mipmap.restype = i32
-    L.oracle_vx_mipmap.argtypes = [P(vxgi.IdkVxCreateInfo), vp, i32]
-    L.oracle_half_roundtrip.argtypes = [vp, u64, vp, vp]
-    L.oracle_det_log2.argtypes = [vp, u64, vp]
-    return L
-
-
-def _vx_split(raw, sizes):
-    levels, off = [], 0
-    for (w, h, dd) in sizes:
-        k = w * h * dd * 4
-        levels.append(raw[off:off + k].view(np.float16).reshape(dd, h, w, 4))
-        off += k
-    return levels
-
-
 def vx_mipmap(ci, level0, threads=None):
     """Levels 1 .. n-1 of the mip chain built from a caller-supplied level 0 (float16 [d, h, w, 4]).
     Returns (list of float16 [d, h, w, 4] arrays per level, concatenated raw uint16 chain)."""
-    from idkengine_b200 import vxgi
-    L = _vx_declare()
     sizes = vxgi.level_sizes(ci)
     w, h, d = sizes[0]
     level0 = np.ascontiguousarray(level0, np.float16)
     assert level0.shape == (d, h, w, 4), level0.shape
     raw = np.zeros(sum(a * b * c for a, b, c in sizes) * 4, np.uint16)
     raw[:level0.size] = level0.reshape(-1).view(np.uint16)
-    n = L.oracle_vx_mipmap(ctypes.byref(ci), raw.ctypes.data, threads or default_threads())
+    n = lib().oracle_vx_mipmap(ctypes.byref(ci), raw.ctypes.data, threads or default_threads())
     assert n == len(sizes), n
-    return _vx_split(raw, sizes), raw
+    return split_levels(raw, ci), raw
 
 
 def vx_voxelize(scene, ci, threads=None, raster_rule=0):
     """Returns (list of float16 [d,h,w,4] arrays per level, concatenated raw uint16 chain, fragment count).
     raster_rule: 0 = the product's coverage rule (what the GPU kernels implement), 1 = the GL model (1/256-pixel snapping +
     top-left fill rule) used only to measure the distance between the two."""
-    from idkengine_b200 import vxgi
-    L = _vx_declare()
-    L.oracle_vx_set_raster_rule.restype = None
-    L.oracle_vx_set_raster_rule.argtypes = [ctypes.c_int]
-    L.oracle_vx_set_raster_rule(int(raster_rule))
+    L = lib()
     sizes = vxgi.level_sizes(ci)
     total = sum(w * h * d for w, h, d in sizes)
     raw = np.zeros(total * 4, np.uint16)
     d, keep = capi.scene_desc(scene)
     frags = ctypes.c_uint64()
     try:
+        L.oracle_vx_set_raster_rule(int(raster_rule))   # process-wide: every other voxeliser entry point runs under rule 0
         n = L.oracle_vx_voxelize(ctypes.byref(d), ctypes.byref(ci), raw.ctypes.data, total, ctypes.byref(frags), threads or default_threads())
     finally:
         L.oracle_vx_set_raster_rule(0)
     assert n == len(sizes), n
-    return _vx_split(raw, sizes), raw, frags.value
+    return split_levels(raw, ci), raw, frags.value
 
 
 def vx_cone_trace(ci, raw_chain, frame, settings, depth, normal_rg, metal_rough, sky=(0.6, 0.7, 0.9), threads=None):
-    L = _vx_declare()
     h, w = depth.shape
     out = np.zeros((h, w, 4), np.float32)
     skyc = np.array(sky, np.float32)
@@ -270,9 +308,9 @@ def vx_cone_trace(ci, raw_chain, frame, settings, depth, normal_rg, metal_rough,
     depth = np.ascontiguousarray(depth, np.float32)
     nrg = np.ascontiguousarray(normal_rg, np.float32)
     mr = np.ascontiguousarray(metal_rough, np.float32)
-    rc = L.oracle_vx_cone_trace(ctypes.byref(ci), raw_chain.ctypes.data, frame.ctypes.data, ctypes.byref(settings), depth.ctypes.data,
-                                nrg.ctypes.data, mr.ctypes.data, w, h, skyc.ctypes.data, out.ctypes.data, ctypes.byref(steps),
-                                threads or default_threads())
+    rc = lib().oracle_vx_cone_trace(ctypes.byref(ci), raw_chain.ctypes.data, frame.ctypes.data, ctypes.byref(settings), depth.ctypes.data,
+                                    nrg.ctypes.data, mr.ctypes.data, w, h, skyc.ctypes.data, out.ctypes.data, ctypes.byref(steps),
+                                    threads or default_threads())
     assert rc == 0
     return out, steps.value
 
@@ -319,11 +357,7 @@ def denoise(result, albedo, normal, settings=None, threads=None):
     h, w = result.shape[:2]
     r, a, n = (np.ascontiguousarray(x, np.float32) for x in (result, albedo, normal))
     out = np.zeros((h, w, 4), np.float32)
-    L = lib()
-    L.oracle_denoise.restype = ctypes.c_int32
-    L.oracle_denoise.argtypes = [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int32, ctypes.c_int32, ctypes.POINTER(capi.IdkPtDenoiseSettings),
-                                 ctypes.c_void_p, ctypes.c_int32]
-    rc = L.oracle_denoise(r.ctypes.data, a.ctypes.data, n.ctypes.data, w, h, ctypes.byref(st), out.ctypes.data, threads or default_threads())
+    rc = lib().oracle_denoise(r.ctypes.data, a.ctypes.data, n.ctypes.data, w, h, ctypes.byref(st), out.ctypes.data, threads or default_threads())
     assert rc == 0
     return out
 
@@ -333,8 +367,5 @@ def sample_sky(faces, dirs):
     sk = capi.sky_desc((0.0, 0.0, 0.0), faces)
     d = np.ascontiguousarray(dirs, np.float32)
     out = np.zeros((len(d), 3), np.float32)
-    L = lib()
-    L.oracle_sample_sky.restype = None
-    L.oracle_sample_sky.argtypes = [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_uint64, ctypes.c_void_p]
-    L.oracle_sample_sky(ctypes.byref(sk), d.ctypes.data, len(d), out.ctypes.data)
+    lib().oracle_sample_sky(ctypes.byref(sk), d.ctypes.data, len(d), out.ctypes.data)
     return out

@@ -1,51 +1,10 @@
-"""ctypes wrapper of the sky oracle (oracle/oracle_sky.cpp -> oracle/liboracle_sky.so), which tests/test_sky*.py use. The
-library is compiled on first use with the flags of oracle/build.py."""
+"""ctypes wrapper of the sky oracle (oracle/oracle_sky.cpp in oracle/liboracle.so), which tests/test_sky*.py use."""
 import ctypes
-import os
-import subprocess
 
 import numpy as np
 
 import oracle_lib as ol
-from idkengine_b200 import capi
-
-REPO = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-ORACLE_DIR = os.path.join(REPO, "oracle")
-SRC = os.path.join(ORACLE_DIR, "oracle_sky.cpp")
-LIB = os.path.join(ORACLE_DIR, "liboracle_sky.so")
-
-_lib = None
-
-
-def build(force=False):
-    deps = [SRC] + [os.path.join(ORACLE_DIR, f) for f in ("oracle.cpp", "oracle_vxgi.inc", "oracle_post.inc")] + \
-        [os.path.join(REPO, "include", f) for f in ("idkpt.h", "idkvx.h", "idk_gpu_types.h")]
-    if not force and os.path.exists(LIB) and all(os.path.getmtime(d) <= os.path.getmtime(LIB) for d in deps):
-        return LIB
-    tmp = LIB + ".%d.tmp" % os.getpid()
-    subprocess.run(["g++", "-O2", "-std=c++17", "-ffp-contract=off", "-fno-fast-math", "-fPIC", "-shared", "-pthread",
-                    "-fvisibility=hidden", "-o", tmp, SRC], check=True)
-    os.replace(tmp, LIB)
-    return LIB
-
-
-def lib():
-    global _lib
-    if _lib is None:
-        L = ctypes.CDLL(build())
-        vp, i32, u64 = ctypes.c_void_p, ctypes.c_int32, ctypes.c_uint64
-        L.oracle_sky_atmosphere.restype = i32
-        L.oracle_sky_atmosphere.argtypes = [ctypes.POINTER(capi.IdkPtAtmosphereSettings), i32, vp, i32]
-        L.oracle_sky_equirect.restype = i32
-        L.oracle_sky_equirect.argtypes = [vp, i32, i32, vp, i32]
-        L.oracle_sky_directions.restype = None
-        L.oracle_sky_directions.argtypes = [i32, vp]
-        L.oracle_det_atan2.restype = None
-        L.oracle_det_atan2.argtypes = [vp, vp, u64, vp]
-        L.oracle_det_asin.restype = None
-        L.oracle_det_asin.argtypes = [vp, u64, vp]
-        _lib = L
-    return _lib
+from oracle_lib import lib
 
 
 def atmosphere(settings, n, threads=None):

@@ -1,49 +1,10 @@
-"""ctypes wrapper of the SSR / TAA oracle (oracle/oracle_ssr_taa.cpp -> oracle/liboracle_ssr_taa.so), which tests/test_ssr_taa*.py
-use. The library is compiled on first use with the flags of oracle/build.py."""
+"""ctypes wrapper of the SSR / TAA oracle (oracle/oracle_ssr_taa.cpp in oracle/liboracle.so), which tests/test_ssr_taa*.py
+use."""
 import ctypes
-import os
-import subprocess
 
 import numpy as np
 
-from idkengine_b200 import capi
-
-REPO = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-ORACLE_DIR = os.path.join(REPO, "oracle")
-SRC = os.path.join(ORACLE_DIR, "oracle_ssr_taa.cpp")
-LIB = os.path.join(ORACLE_DIR, "liboracle_ssr_taa.so")
-
-_lib = None
-
-
-def build(force=False):
-    deps = [SRC] + [os.path.join(ORACLE_DIR, f) for f in ("oracle_deferred.cpp", "oracle_point_shadows.cpp", "oracle.cpp", "oracle_vxgi.inc",
-                                                          "oracle_post.inc")] + \
-        [os.path.join(REPO, "include", f) for f in ("idkpt.h", "idkvx.h", "idk_gpu_types.h")]
-    if not force and os.path.exists(LIB) and all(os.path.getmtime(d) <= os.path.getmtime(LIB) for d in deps):
-        return LIB
-    tmp = LIB + ".%d.tmp" % os.getpid()
-    subprocess.run(["g++", "-O2", "-std=c++17", "-ffp-contract=off", "-fno-fast-math", "-fPIC", "-shared", "-pthread",
-                    "-fvisibility=hidden", "-o", tmp, SRC], check=True)
-    os.replace(tmp, LIB)
-    return LIB
-
-
-def lib():
-    global _lib
-    if _lib is None:
-        L = ctypes.CDLL(build())
-        vp, i32 = ctypes.c_void_p, ctypes.c_int32
-        L.oracle_ssr.restype = i32
-        L.oracle_ssr.argtypes = [vp, ctypes.POINTER(capi.IdkPtSsrSettings), ctypes.POINTER(capi.IdkPtSkyDesc), vp, vp, vp, vp, vp, i32, i32, vp, vp]
-        L.oracle_taa_resolve.restype = i32
-        L.oracle_taa_resolve.argtypes = [ctypes.POINTER(capi.IdkPtTaaSettings), vp, vp, vp, i32, i32, vp, i32, i32, vp]
-        _lib = L
-    return _lib
-
-
-def _f32(a):
-    return np.ascontiguousarray(a, np.float32)
+from oracle_lib import _f32, lib
 
 
 def ssr(frame, settings, sky, depth, normal_rg, albedo, metallic_roughness, src):

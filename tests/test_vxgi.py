@@ -16,7 +16,7 @@ def lit_cornell():
 
 
 def test_half_conversion_and_log2():
-    L = ol._vx_declare()
+    L = ol.lib()
     x = np.concatenate([np.linspace(0, 70000, 20001), 10.0 ** np.linspace(-9, 5, 3001), [65504, 65519.9, 65520, 1e-8, 6e-8, 5.96e-8, 2.98e-8]]).astype(np.float32)
     h, back = np.zeros(len(x), np.uint16), np.zeros(len(x), np.float32)
     L.oracle_half_roundtrip(x.ctypes.data, len(x), h.ctypes.data, back.ctypes.data)

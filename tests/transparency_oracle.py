@@ -1,46 +1,14 @@
-"""ctypes wrapper of the transparency oracle (oracle/oracle_transparency.cpp -> oracle/liboracle_transparency.so), which
-tests/test_transparency*.py use. The library is compiled on first use with the flags of oracle/build.py."""
+"""ctypes wrapper of the transparency oracle (oracle/oracle_transparency.cpp in oracle/liboracle.so), which
+tests/test_transparency*.py use."""
 import ctypes
-import os
-import subprocess
 
 import numpy as np
 
 import oracle_lib as ol
 from idkengine_b200 import capi, gpu_types as gt
+from oracle_lib import lib
 
-REPO = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-ORACLE_DIR = os.path.join(REPO, "oracle")
-SRC = os.path.join(ORACLE_DIR, "oracle_transparency.cpp")
-LIB = os.path.join(ORACLE_DIR, "liboracle_transparency.so")
 LAYERS = 10
-
-_lib = None
-
-
-def build(force=False):
-    deps = [SRC] + [os.path.join(ORACLE_DIR, f) for f in ("oracle_deferred.cpp", "oracle_point_shadows.cpp", "oracle.cpp",
-                                                           "oracle_vxgi.inc", "oracle_post.inc")] + \
-        [os.path.join(REPO, "include", f) for f in ("idkpt.h", "idkvx.h", "idk_gpu_types.h")]
-    if not force and os.path.exists(LIB) and all(os.path.getmtime(d) <= os.path.getmtime(LIB) for d in deps):
-        return LIB
-    tmp = LIB + ".%d.tmp" % os.getpid()
-    subprocess.run(["g++", "-O2", "-std=c++17", "-ffp-contract=off", "-fno-fast-math", "-fPIC", "-shared", "-pthread",
-                    "-fvisibility=hidden", "-o", tmp, SRC], check=True)
-    os.replace(tmp, LIB)
-    return LIB
-
-
-def lib():
-    global _lib
-    if _lib is None:
-        L = ctypes.CDLL(build())
-        vp, i32 = ctypes.c_void_p, ctypes.c_int32
-        L.oracle_transparency.restype = i32
-        L.oracle_transparency.argtypes = [ctypes.POINTER(capi.IdkPtSceneDesc), ctypes.POINTER(capi.IdkPtSkyDesc), vp, i32, i32,
-                                          vp, vp, vp, i32, vp, vp, vp, vp, i32, i32, vp, i32, vp, vp, vp, vp, i32]
-        _lib = L
-    return _lib
 
 
 def transparency(scene, frame, depth, color, shadow_mode=0, shadows=None, maps=(), jitter=None, sky=None, voxels=None,
@@ -56,9 +24,7 @@ def transparency(scene, frame, depth, color, shadow_mode=0, shadows=None, maps=(
     h, w = dep.shape
     out = np.array(color, np.float32, copy=True, order="C")
     assert out.shape == (h, w, 4)
-    sh = np.ascontiguousarray(shadows if shadows is not None else np.zeros(0, gt.GpuPointShadow), gt.GpuPointShadow).reshape(-1)
-    sizes = np.array([m.shape[1] for m in maps] or [0], np.int32)
-    texels = np.ascontiguousarray(np.concatenate([np.ascontiguousarray(m, np.uint16).ravel() for m in maps]) if maps else np.zeros(1, np.uint16))
+    sh, sizes, texels = ol.pack_shadow_maps(shadows if shadows is not None else np.zeros(0, gt.GpuPointShadow), maps)
     jit = None if jitter is None else np.ascontiguousarray(jitter, np.float32)
     sky_keep = sky
     sky_struct = sky[0] if isinstance(sky, tuple) else sky
