@@ -112,9 +112,21 @@ EXPORTS = [
     "idkpt_shading_rate", "idkpt_shading_rate_device_ptr",
     "idkpt_gbuffer", "idkpt_gbuffer_device_ptrs", "idkpt_read_gbuffer", "idkpt_transparency", "idkpt_lights_and_skybox",
     "idkpt_sky_atmosphere", "idkpt_sky_equirectangular", "idkpt_read_sky",
+    "idkpt_blas_build", "idkpt_blas_build_info", "idkpt_blas_build_copy", "idkpt_blas_build_free",
 ]
 
 IDKPT_MAX_POINT_SHADOWS = 128
+
+
+class IdkPtBlasBuildSettings(ctypes.Structure):
+    """BLAS.BuildSettings + PreSplitting.Settings: host.IdkBlasBuildSettings without Threads."""
+    _fields_ = [("StopSplittingThreshold", c_i32), ("MaxLeafTriangleCount", c_i32), ("TriangleCost", c_f),
+                ("StackOptThreshold", c_i32), ("StackOptSahIncreaseAcceptance", c_f), ("SplitFactor", c_f), ("DoPreSplit", c_i32)]
+
+
+def default_blas_build_settings():
+    """BLAS.BuildSettings / PreSplitting.Settings defaults (the host build's idkhost_default_build_settings)."""
+    return IdkPtBlasBuildSettings(1, 2, 1.1, 16, 0.0009745, 0.3, 1)
 
 
 class IdkPtVolumetricSettings(ctypes.Structure):
@@ -408,6 +420,14 @@ def load(path=None):
     L.idkpt_sync.argtypes = [c_vp]
     L.idkpt_tlas_build.restype = c_i32
     L.idkpt_tlas_build.argtypes = [c_vp, c_i32, P(c_f)]
+    L.idkpt_blas_build.restype = c_i32
+    L.idkpt_blas_build.argtypes = [c_vp, c_vp, c_u64, c_vp, c_u64, P(IdkPtBlasBuildSettings), P(c_vp), P(c_f)]
+    L.idkpt_blas_build_info.restype = c_i32
+    L.idkpt_blas_build_info.argtypes = [c_vp, P(c_u64), P(c_u64), P(c_i32), P(c_i32), P(ctypes.c_double)]
+    L.idkpt_blas_build_copy.restype = c_i32
+    L.idkpt_blas_build_copy.argtypes = [c_vp, c_vp, c_vp]
+    L.idkpt_blas_build_free.restype = None
+    L.idkpt_blas_build_free.argtypes = [c_vp]
     L.idkpt_denoise.restype = c_i32
     L.idkpt_denoise.argtypes = [c_vp, P(IdkPtDenoiseSettings), P(c_f)]
     L.idkpt_denoise_device_ptrs.restype = c_i32

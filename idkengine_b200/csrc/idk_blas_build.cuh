@@ -1,0 +1,1240 @@
+// BLAS.Build + PreSplitting.PreSplit on the device (idkpt_blas_build): the engine's SweepSAH builder with pre-splitting,
+// node for node equal to the host mirror (host_mirror/bvh_build.cpp) under libidkpt's flags (-fmad=false, IEEE div and
+// sqrt; fmaf only in HalfArea, where the mirror uses it). DESIGN §8f.5 gives the stages and why each one is exact.
+//
+// Stages (the mirror's function in brackets):
+//   1. pre-split [preSplit]: priorities per triangle; their float sum in triangle order by one thread; split counts and
+//      their exclusive scan; each triangle splits into its own output range, using the range's tail as its stack.
+//   2. sorts [radixSortFragments]: three stable sorts of fragment ids by floatToKey(min + max) (CUB radix sort).
+//   3. tree [processSubtree, trySplit]: level by level, one block per node above SMALL_NODE fragments (full prefix and
+//      suffix box scans, first strict minimum of L[i] + R[i+1]), then one thread per remaining subtree (the mirror's serial
+//      trySplit). Node ids do not depend on the order nodes are split in.
+//   4. post passes [computeRequiredStackSize, optimizeStackSize, removeEmptySubtrees, unindex*, computeGlobalSAH]: parallel
+//      except for the double sums, which one thread adds in the mirror's DFS order.
+#pragma once
+#include <cfloat>
+#include <climits>
+#include <cstdint>
+#include <cstdio>
+#include <cstdlib>
+#include <string>
+#include <vector>
+#include <cub/cub.cuh>
+
+#include "../../include/idk_gpu_types.h"
+#include "idk_cbrt.h"
+
+namespace idkbb {
+
+constexpr int SMALL_NODE = 64;          // subtrees of at most this many fragments are finished by one thread
+constexpr int BIG_THREADS = 512;
+constexpr int BIG_ITEMS = 4;
+constexpr int BIG_TILE = BIG_THREADS * BIG_ITEMS;
+constexpr int MAX_FRAGMENTS = 1 << 24;  // float counters are exact up to here
+constexpr int DEPTH_NONE = 0x7F7F7F7F;  // memset byte 0x7F: larger than any depth
+
+struct Params {
+    int stopSplittingThreshold, maxLeafTriangleCount;
+    float triangleCost;
+    int stackOptThreshold;
+    float stackOptSahIncreaseAcceptance, splitFactor;
+    int doPreSplit;
+};
+
+struct FBox { float mn[3], mx[3]; };
+
+// Vector128.MinNative / MaxNative: (a < b) ? a : b. Folding a sequence with them keeps, among equal values, the last one
+// (which matters for +-0), and the operation is associative, so a scan that combines (earlier, later) in order is exact.
+__device__ __forceinline__ float minN(float a, float b) { return a < b ? a : b; }
+__device__ __forceinline__ float maxN(float a, float b) { return a > b ? a : b; }
+__device__ __forceinline__ FBox boxEmpty() { return {{FLT_MAX, FLT_MAX, FLT_MAX}, {-FLT_MAX, -FLT_MAX, -FLT_MAX}}; }
+// exact identity of the ordered combine (for padding partial tiles); the mirror's Box::empty() is a real first element
+__device__ __forceinline__ FBox boxIdentity() { return {{INFINITY, INFINITY, INFINITY}, {-INFINITY, -INFINITY, -INFINITY}}; }
+__device__ __forceinline__ FBox combine(const FBox& a, const FBox& b) {
+    FBox r;
+#pragma unroll
+    for (int i = 0; i < 3; i++) { r.mn[i] = minN(a.mn[i], b.mn[i]); r.mx[i] = maxN(a.mx[i], b.mx[i]); }
+    return r;
+}
+__device__ __forceinline__ float halfArea(const FBox& b) {   // MyMath.HalfArea
+    const float sx = b.mx[0] - b.mn[0], sy = b.mx[1] - b.mn[1], sz = b.mx[2] - b.mn[2];
+    return fmaf(sx + sy, sz, sx * sy);
+}
+__device__ __forceinline__ float nodeHalfArea(const GpuBlasNode& n) {
+    const float sx = n.Max[0] - n.Min[0], sy = n.Max[1] - n.Min[1], sz = n.Max[2] - n.Min[2];
+    return fmaf(sx + sy, sz, sx * sy);
+}
+__device__ __forceinline__ FBox loadBox(const FBox* b, int i) {
+    const float2* p = reinterpret_cast<const float2*>(b + i);
+    const float2 a = p[0], c = p[1], d = p[2];
+    return {{a.x, a.y, c.x}, {c.y, d.x, d.y}};
+}
+__device__ __forceinline__ void storeBox(FBox* b, size_t i, const FBox& v) {
+    float2* p = reinterpret_cast<float2*>(b + i);
+    p[0] = make_float2(v.mn[0], v.mn[1]); p[1] = make_float2(v.mn[2], v.mx[0]); p[2] = make_float2(v.mx[1], v.mx[2]);
+}
+__device__ __forceinline__ void setBounds(GpuBlasNode& n, const FBox& b) {
+    for (int i = 0; i < 3; i++) { n.Min[i] = b.mn[i]; n.Max[i] = b.mx[i]; }
+}
+__device__ __forceinline__ uint32_t floatToKey(float v) {
+    const uint32_t f = __float_as_uint(v);
+    return f ^ (uint32_t)(((int32_t)f >> 31) | (int32_t)0x80000000);
+}
+__device__ __forceinline__ int csFloatToInt(float f) {   // (int)float in C# on x86-64: NaN / out of range -> INT_MIN
+    if (!(f > -2147483904.0f && f < 2147483648.0f)) return INT_MIN;
+    return (int)f;
+}
+
+// ---------------------------------------------------------------------------------------------------------------- pre-split
+struct V3 { float v[3]; };
+struct Tri { V3 p[3]; };
+__device__ __forceinline__ Tri loadTri(const PackedVec3* pos, const GpuBlasTriangle* tris, int i) {
+    const GpuBlasTriangle t = tris[i];
+    const int id[3] = {t.X, t.Y, t.Z};
+    Tri r;
+    for (int k = 0; k < 3; k++) { const PackedVec3 q = pos[(uint32_t)id[k]]; r.p[k] = {{q.x, q.y, q.z}}; }
+    return r;
+}
+__device__ __forceinline__ void grow(FBox& b, const V3& p) {
+    for (int i = 0; i < 3; i++) { b.mn[i] = minN(b.mn[i], p.v[i]); b.mx[i] = maxN(b.mx[i], p.v[i]); }
+}
+__device__ __forceinline__ FBox boxFromTri(const Tri& t) {
+    FBox b = {{t.p[0].v[0], t.p[0].v[1], t.p[0].v[2]}, {t.p[0].v[0], t.p[0].v[1], t.p[0].v[2]}};
+    grow(b, t.p[1]);
+    grow(b, t.p[2]);
+    return b;
+}
+__device__ __forceinline__ float boxSize(const FBox& b, int i) { return b.mx[i] - b.mn[i]; }
+__device__ __forceinline__ float largestExtent(const FBox& b) { return maxN(boxSize(b, 0), maxN(boxSize(b, 1), boxSize(b, 2))); }
+__device__ __forceinline__ int largestAxis(const FBox& b) {
+    int axis = 0;
+    if (boxSize(b, 0) < boxSize(b, 1)) axis = 1;
+    if (boxSize(b, axis) < boxSize(b, 2)) axis = 2;
+    return axis;
+}
+
+__device__ float priority(const Tri& t) {   // PreSplitting.GetPriority
+    const FBox b = boxFromTri(t);
+    const float le = largestExtent(b);
+    const float extentPrio = le * le;
+    float e1[3], e2[3];
+    for (int i = 0; i < 3; i++) { e1[i] = t.p[1].v[i] - t.p[0].v[i]; e2[i] = t.p[2].v[i] - t.p[0].v[i]; }
+    const float cx = e1[1] * e2[2] - e1[2] * e2[1], cy = e1[2] * e2[0] - e1[0] * e2[2], cz = e1[0] * e2[1] - e1[1] * e2[0];
+    const float triArea = sqrtf(cx * cx + cy * cy + cz * cz) * 0.5f;
+    const float emptyAreaPrio = halfArea(b) * 2.0f - triArea;
+    return idk_cbrtf(extentPrio * emptyAreaPrio);
+}
+
+__global__ void k_priorities(const PackedVec3* pos, const GpuBlasTriangle* tris, int n, float* prio) {
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i < n) prio[i] = priority(loadTri(pos, tris, i));
+}
+
+// Ordered sums: one thread adds the values in index order, as the mirror does (float addition is not associative).
+// The block stages tiles through shared memory so that the one adding thread reads nothing from HBM itself.
+constexpr int SUM_THREADS = 1024;
+template <class T, int TILE>
+__global__ void __launch_bounds__(SUM_THREADS) k_ordered_sum(const T* v, int n, const int* nDev, T* acc) {
+    __shared__ T tile[TILE];
+    if (nDev) n = *nDev;
+    T s = threadIdx.x == 0 ? *acc : T(0);
+    for (int base = 0; base < n; base += TILE) {
+        const int m = min(TILE, n - base);
+        for (int k = threadIdx.x; k < m; k += SUM_THREADS) tile[k] = v[base + k];
+        __syncthreads();
+        if (threadIdx.x == 0) {
+#pragma unroll 8
+            for (int k = 0; k < m; k++) s += tile[k];
+        }
+        __syncthreads();
+    }
+    if (threadIdx.x == 0) *acc = s;
+}
+
+__global__ void k_split_counts(const float* prio, const float* total, int n, float splitFactor, unsigned long long* counts) {
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i > n) return;
+    if (i == n) { counts[n] = 0; return; }
+    const float shareOfTris = prio[i] / *total * (float)n;
+    int c = csFloatToInt(shareOfTris * splitFactor);
+    if (c == INT_MIN || c < 0) c = 0;    // the mirror's guard for degenerate input
+    counts[i] = 1ull + (unsigned long long)c;
+}
+
+// Box of every vertex in triangle order (p0, p1, p2 of each): per-thread chunks folded in order, chunks combined in order.
+__global__ void __launch_bounds__(1024) k_global_box(const PackedVec3* pos, const GpuBlasTriangle* tris, int n, FBox* out) {
+    __shared__ FBox part[1024];
+    __shared__ int has[1024];
+    const int per = (n + 1023) / 1024;
+    const int b0 = min(n, threadIdx.x * per), e0 = min(n, b0 + per);
+    FBox acc = boxIdentity();
+    for (int i = b0; i < e0; i++) {
+        const Tri t = loadTri(pos, tris, i);
+        for (int k = 0; k < 3; k++) { FBox p = {{t.p[k].v[0], t.p[k].v[1], t.p[k].v[2]}, {t.p[k].v[0], t.p[k].v[1], t.p[k].v[2]}}; acc = combine(acc, p); }
+    }
+    part[threadIdx.x] = acc;
+    has[threadIdx.x] = e0 > b0;
+    __syncthreads();
+    if (threadIdx.x == 0) {
+        FBox g = boxEmpty();
+        for (int t = 0; t < 1024; t++) if (has[t]) g = combine(g, part[t]);
+        *out = g;
+    }
+}
+
+__device__ __forceinline__ void triSplit(const Tri& t, int axis, float position, FBox& l, FBox& r) {   // Triangle.Split
+    l = boxEmpty();
+    r = boxEmpty();
+    const bool q[3] = {t.p[0].v[axis] <= position, t.p[1].v[axis] <= position, t.p[2].v[axis] <= position};
+    for (int k = 0; k < 3; k++) { if (q[k]) grow(l, t.p[k]); else grow(r, t.p[k]); }
+    for (int k = 0; k < 3; k++) {
+        const int k1 = (k + 1) % 3;
+        if (q[k] ^ q[k1]) {
+            const V3 a = t.p[k], b = t.p[k1];
+            const float tt = (position - a.v[axis]) / (b.v[axis] - a.v[axis]);
+            V3 m;
+            for (int i = 0; i < 3; i++) m.v[i] = a.v[i] + tt * (b.v[i] - a.v[i]);
+            grow(l, m);
+            grow(r, m);
+        }
+    }
+}
+
+// One thread per triangle, writing its fragments to [off[i], off[i+1]). The split stack lives in the same range, growing
+// down from its end: the stack's items hold at least one fragment each and together exactly the ones not yet written, so
+// they never reach the slot the next fragment goes to. Item j: box in bounds[end-1-j], split count in ids[end-1-j].
+__global__ void k_presplit(const PackedVec3* pos, const GpuBlasTriangle* tris, int n, const unsigned long long* off,
+                           const FBox* globalBox, FBox* bounds, int* origIds) {
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    const FBox g = *globalBox;
+    const Tri tri = loadTri(pos, tris, i);
+    const size_t begin = (size_t)off[i], end = (size_t)off[i + 1];
+    size_t counter = begin;
+    int sp = 0;
+    storeBox(bounds, end - 1, boxFromTri(tri));
+    origIds[end - 1] = (int)(end - begin);
+    sp = 1;
+    while (sp > 0) {
+        sp--;
+        const FBox box = loadBox(bounds, (int)(end - 1 - sp));
+        const int splits = origIds[end - 1 - sp];
+        if (splits == 1) {
+            storeBox(bounds, counter, box);
+            origIds[counter] = i;
+            counter++;
+            continue;
+        }
+        const int axis = largestAxis(box);
+        const float le = largestExtent(box);
+        const float globalSize = g.mx[axis] - g.mn[axis];
+        const float alpha = le / globalSize;   // getNodeSize: the power of two below alpha, times globalSize
+        float nodeSize = __uint_as_float(__float_as_uint(alpha) & (255u << 23)) * globalSize;
+        if (nodeSize >= le - 0.0001f) nodeSize *= 0.5f;
+        const float midPos = (box.mn[axis] + box.mx[axis]) * 0.5f;
+        const float index = rintf((midPos - g.mn[axis]) / nodeSize);   // MathF.Round: half to even
+        const float splitPos = g.mn[axis] + index * nodeSize;
+        FBox l, r;
+        triSplit(tri, axis, splitPos, l, r);
+        for (int k = 0; k < 3; k++) {   // clip to the item's box
+            l.mn[k] = maxN(l.mn[k], box.mn[k]); l.mx[k] = minN(l.mx[k], box.mx[k]);
+            r.mn[k] = maxN(r.mn[k], box.mn[k]); r.mx[k] = minN(r.mx[k], box.mx[k]);
+        }
+        const float leftExtent = largestExtent(l), rightExtent = largestExtent(r);
+        int leftCount = csFloatToInt((float)splits * (leftExtent / (leftExtent + rightExtent)));
+        leftCount = min(max(leftCount, 1), splits - 1);
+        storeBox(bounds, end - 1 - sp, r);
+        origIds[end - 1 - sp] = splits - leftCount;
+        sp++;
+        storeBox(bounds, end - 1 - sp, l);
+        origIds[end - 1 - sp] = leftCount;
+        sp++;
+    }
+}
+
+__global__ void k_tri_bounds(const PackedVec3* pos, const GpuBlasTriangle* tris, int n, FBox* bounds) {
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i < n) storeBox(bounds, i, boxFromTri(loadTri(pos, tris, i)));
+}
+
+__global__ void k_sort_keys(const FBox* bounds, int n, int axis, uint32_t* keys, int* vals) {
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    const FBox b = loadBox(bounds, i);
+    keys[i] = floatToKey(b.mn[axis] + b.mx[axis]);
+    vals[i] = i;
+}
+
+// ---------------------------------------------------------------------------------------------------------------- tree
+struct TreeArgs {
+    const FBox* bounds;
+    int* ids[3];
+    int* aux;
+    uint8_t* table;
+    float* rcost;               // right costs by fragment position (the mirror's rightCostsAccum)
+    GpuBlasNode* nodes;
+    int* parent;                // per node id: its parent, the root's is 0
+    int* depth;                 // per node id: depth below the root (-1: id not used)
+    int* ostart;                // per node id: first fragment of its range (also for nodes later split)
+    int* ocount;                // per node id: fragments in its range
+    const int2* tasks;          // (parentNodeId, newNodesId) of this level's large nodes
+    int2* nextTasks;
+    int* nextCount;
+    int2* small;                // subtrees left to one thread each
+    int* smallCount;
+    Params p;
+};
+
+__device__ __forceinline__ void pushTask(const TreeArgs& a, int2 t, int count) {
+    if (count > SMALL_NODE) a.nextTasks[atomicAdd(a.nextCount, 1)] = t;
+    else a.small[atomicAdd(a.smallCount, 1)] = t;
+}
+
+__device__ __forceinline__ void writeChildren(const TreeArgs& a, int pid, int2 task, int start, int count, int split) {
+    GpuBlasNode& parent = a.nodes[pid];
+    const int leftId = task.y, rightId = leftId + 1;
+    const int lc = split - start, rc = count - lc;
+    GpuBlasNode l = {}, r = {};
+    l.TriStartOrChild = start; l.TriCount = lc;
+    r.TriStartOrChild = split; r.TriCount = rc;
+    a.nodes[leftId] = l;
+    a.nodes[rightId] = r;
+    const int d = a.depth[pid] + 1;
+    a.parent[leftId] = pid; a.parent[rightId] = pid;
+    a.depth[leftId] = d; a.depth[rightId] = d;
+    a.ostart[leftId] = start; a.ocount[leftId] = lc;
+    a.ostart[rightId] = split; a.ocount[rightId] = rc;
+    parent.TriStartOrChild = leftId;
+    parent.TriCount = 0;
+}
+
+// ---- block-wide ordered scans
+__device__ __forceinline__ FBox shflUpBox(const FBox& v, int o) {
+    FBox r;
+    for (int i = 0; i < 3; i++) { r.mn[i] = __shfl_up_sync(0xffffffffu, v.mn[i], o); r.mx[i] = __shfl_up_sync(0xffffffffu, v.mx[i], o); }
+    return r;
+}
+
+// Exclusive ordered scan of one box per thread over the block; `total` is the fold of all of them.
+__device__ FBox blockScanBox(FBox v, FBox& total) {
+    __shared__ FBox warpTot[BIG_THREADS / 32];
+    __shared__ FBox warpPre[BIG_THREADS / 32];
+    __shared__ FBox all;
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    FBox inc = v;
+#pragma unroll
+    for (int o = 1; o < 32; o <<= 1) {
+        const FBox other = shflUpBox(inc, o);
+        if (lane >= o) inc = combine(other, inc);
+    }
+    FBox exc = shflUpBox(inc, 1);
+    if (lane == 0) exc = boxIdentity();
+    if (lane == 31) warpTot[warp] = inc;
+    __syncthreads();
+    if (threadIdx.x == 0) {
+        FBox acc = boxIdentity();
+        for (int w = 0; w < BIG_THREADS / 32; w++) { warpPre[w] = acc; acc = combine(acc, warpTot[w]); }
+        all = acc;
+    }
+    __syncthreads();
+    total = all;
+    const FBox r = combine(warpPre[warp], exc);
+    __syncthreads();   // the shared words are reused by the next call
+    return r;
+}
+
+__device__ int blockScanInt(int v, int& total) {
+    __shared__ int warpTot[BIG_THREADS / 32];
+    __shared__ int warpPre[BIG_THREADS / 32 + 1];
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    int inc = v;
+#pragma unroll
+    for (int o = 1; o < 32; o <<= 1) {
+        const int other = __shfl_up_sync(0xffffffffu, inc, o);
+        if (lane >= o) inc += other;
+    }
+    if (lane == 31) warpTot[warp] = inc;
+    __syncthreads();
+    if (threadIdx.x == 0) {
+        int acc = 0;
+        for (int w = 0; w < BIG_THREADS / 32; w++) { warpPre[w] = acc; acc += warpTot[w]; }
+        warpPre[BIG_THREADS / 32] = acc;
+    }
+    __syncthreads();
+    total = warpPre[BIG_THREADS / 32];
+    const int r = warpPre[warp] + inc - v;
+    __syncthreads();
+    return r;
+}
+
+__device__ unsigned long long blockMinU64(unsigned long long v) {
+    __shared__ unsigned long long s;
+    if (threadIdx.x == 0) s = ~0ull;
+    __syncthreads();
+    for (int o = 16; o > 0; o >>= 1) v = min(v, __shfl_down_sync(0xffffffffu, v, o));
+    if ((threadIdx.x & 31) == 0) atomicMin(&s, v);
+    __syncthreads();
+    const unsigned long long r = s;
+    __syncthreads();
+    return r;
+}
+
+// computeBoundingBox: Box::empty() grown by the fragments [lo, hi) of `ids` in order.
+__device__ FBox blockRangeBox(const FBox* bounds, const int* ids, int lo, int hi) {
+    FBox carry = boxEmpty();
+    for (int base = lo; base < hi; base += BIG_TILE) {
+        FBox loc = boxIdentity();
+        for (int k = 0; k < BIG_ITEMS; k++) {
+            const int i = base + threadIdx.x * BIG_ITEMS + k;
+            if (i < hi) loc = combine(loc, loadBox(bounds, ids[i]));
+        }
+        FBox total;
+        blockScanBox(loc, total);
+        carry = combine(carry, total);
+    }
+    return carry;
+}
+
+// Stable partition of ids[start, end) by table[id] (ones first), through aux; `ones` is the number of ones.
+__device__ void blockPartition(int* ids, int* aux, const uint8_t* table, int start, int end, int ones) {
+    int carryOnes = 0;
+    for (int base = start; base < end; base += BIG_TILE) {
+        int id[BIG_ITEMS];
+        int f = 0;
+        for (int k = 0; k < BIG_ITEMS; k++) {
+            const int i = base + threadIdx.x * BIG_ITEMS + k;
+            id[k] = i < end ? ids[i] : -1;
+            f += (id[k] >= 0 && table[id[k]]) ? 1 : 0;
+        }
+        int total;
+        int before = carryOnes + blockScanInt(f, total);
+        for (int k = 0; k < BIG_ITEMS; k++) {
+            const int i = base + threadIdx.x * BIG_ITEMS + k;
+            if (i >= end) break;
+            if (table[id[k]]) aux[start + before++] = id[k];
+            else aux[start + ones + (i - start) - before] = id[k];
+        }
+        carryOnes += total;
+    }
+    __syncthreads();
+    for (int i = start + threadIdx.x; i < end; i += BIG_THREADS) ids[i] = aux[i];
+    __syncthreads();
+}
+
+// One block per node: BLAS.TrySplit over full scans (DESIGN §8f.5), then the split.
+__global__ void __launch_bounds__(BIG_THREADS) k_split_large(TreeArgs a) {
+    const int2 task = a.tasks[blockIdx.x];
+    const int pid = task.x;
+    const int start = a.nodes[pid].TriStartOrChild, count = a.nodes[pid].TriCount, end = start + count;
+    const FBox pbox = blockRangeBox(a.bounds, a.ids[0], start, end);
+    if (threadIdx.x == 0) setBounds(a.nodes[pid], pbox);
+    if (count <= a.p.stopSplittingThreshold) return;
+
+    float bestCost = FLT_MAX;
+    int bestAxis = 0, bestSplit = 0;
+    for (int axis = 0; axis < 3; axis++) {
+        const int* ids = a.ids[axis];
+        // suffix: R[i] = HalfArea(box of [i, end)) * (end - i), i in [start + 1, end)
+        FBox carry = boxEmpty();
+        for (int jb = 0; jb < count - 1; jb += BIG_TILE) {
+            FBox b[BIG_ITEMS];
+            FBox loc = boxIdentity();
+            for (int k = 0; k < BIG_ITEMS; k++) {
+                const int j = jb + threadIdx.x * BIG_ITEMS + k;
+                b[k] = j < count - 1 ? loadBox(a.bounds, ids[end - 1 - j]) : boxIdentity();
+                loc = combine(loc, b[k]);
+            }
+            FBox total;
+            FBox acc = combine(carry, blockScanBox(loc, total));
+            for (int k = 0; k < BIG_ITEMS; k++) {
+                const int j = jb + threadIdx.x * BIG_ITEMS + k;
+                acc = combine(acc, b[k]);
+                if (j < count - 1) a.rcost[end - 1 - j] = halfArea(acc) * (float)(j + 1);
+            }
+            carry = combine(carry, total);
+        }
+        __syncthreads();
+        // prefix: L[i] = HalfArea(box of [start, i]) * (i - start + 1); candidate split i + 1 costs L[i] + R[i + 1]
+        unsigned long long best = ~0ull;
+        carry = boxEmpty();
+        for (int base = start; base < end - 1; base += BIG_TILE) {
+            FBox b[BIG_ITEMS];
+            FBox loc = boxIdentity();
+            for (int k = 0; k < BIG_ITEMS; k++) {
+                const int i = base + threadIdx.x * BIG_ITEMS + k;
+                b[k] = i < end - 1 ? loadBox(a.bounds, ids[i]) : boxIdentity();
+                loc = combine(loc, b[k]);
+            }
+            FBox total;
+            FBox acc = combine(carry, blockScanBox(loc, total));
+            for (int k = 0; k < BIG_ITEMS; k++) {
+                const int i = base + threadIdx.x * BIG_ITEMS + k;
+                acc = combine(acc, b[k]);
+                if (i < end - 1) {
+                    const float cost = halfArea(acc) * (float)(i - start + 1) + a.rcost[i + 1];
+                    if (cost < FLT_MAX) best = min(best, ((unsigned long long)__float_as_uint(cost) << 32) | (uint32_t)(i + 1));
+                }
+            }
+            carry = combine(carry, total);
+        }
+        best = blockMinU64(best);
+        if (best != ~0ull) {
+            const float c = __uint_as_float((uint32_t)(best >> 32));
+            if (c < bestCost) { bestCost = c; bestAxis = axis; bestSplit = (int)(uint32_t)best; }
+        }
+    }
+    if (bestCost == FLT_MAX) { bestAxis = 0; bestSplit = start + count / 2; }   // the mirror's guard for non-finite costs
+    if (count <= a.p.maxLeafTriangleCount) {
+        const float notSplitCost = a.p.triangleCost * (float)count;
+        const float newCost = 1.0f + (a.p.triangleCost * bestCost / halfArea(pbox));
+        if (newCost >= notSplitCost) return;
+    }
+    int* ids = a.ids[bestAxis];
+    const FBox lbox = blockRangeBox(a.bounds, ids, start, bestSplit);
+    const FBox rbox = blockRangeBox(a.bounds, ids, bestSplit, end);
+    const bool swapSides = halfArea(lbox) < halfArea(rbox);   // the larger child goes left
+    for (int i = start + threadIdx.x; i < end; i += BIG_THREADS) a.table[ids[i]] = i < bestSplit ? !swapSides : swapSides;
+    __syncthreads();
+    const int ones = swapSides ? end - bestSplit : bestSplit - start;
+    if (swapSides) blockPartition(ids, a.aux, a.table, start, end, ones);
+    blockPartition(a.ids[(bestAxis + 1) % 3], a.aux, a.table, start, end, ones);
+    blockPartition(a.ids[(bestAxis + 2) % 3], a.aux, a.table, start, end, ones);
+    if (threadIdx.x == 0) {
+        const int split = start + ones;
+        writeChildren(a, pid, task, start, count, split);
+        const int lc = split - start;
+        pushTask(a, make_int2(task.y, task.y + 2), lc);
+        pushTask(a, make_int2(task.y + 1, task.y + 1 + (2 * lc - 1)), count - lc);
+    }
+}
+
+// ---- one thread per subtree: the mirror's processSubtree and trySplit, line for line
+__device__ FBox rangeBox(const FBox* bounds, const int* ids, int lo, int hi) {
+    FBox b = boxEmpty();
+    for (int i = lo; i < hi; i++) b = combine(b, loadBox(bounds, ids[i]));
+    return b;
+}
+
+__device__ int stablePartition(int* source, int count, int* aux, const uint8_t* table) {
+    int l = 0, r = 0;
+    for (int i = 0; i < count; i++) {
+        const int id = source[i];
+        if (table[id]) source[l++] = id; else aux[r++] = id;
+    }
+    for (int i = 0; i < r; i++) source[l + i] = aux[i];
+    return l;
+}
+
+// returns the split index, or -1 for a leaf
+__device__ int trySplitSerial(const TreeArgs& a, const FBox& parentBox, int start, int count) {
+    if (count <= a.p.stopSplittingThreshold) return -1;
+    const int end = start + count;
+    float bestCost = FLT_MAX;
+    int bestAxis = 0, bestSplit = 0;
+    for (int axis = 0; axis < 3; axis++) {
+        const int* ids = a.ids[axis];
+        int firstRight = start + 1;
+        FBox rightAcc = boxEmpty();
+        float rightCounter = 0.0f;
+        for (int i = end - 1; i >= firstRight; i--) {
+            rightCounter++;
+            rightAcc = combine(rightAcc, loadBox(a.bounds, ids[i]));
+            const float rightCost = halfArea(rightAcc) * rightCounter;
+            a.rcost[i] = rightCost;
+            if (rightCost >= bestCost) { firstRight = i + 1; break; }
+        }
+        FBox leftAcc = boxEmpty();
+        float leftCounter = (float)(firstRight - start) - 1.0f;
+        for (int i = start; i < firstRight - 1; i++) leftAcc = combine(leftAcc, loadBox(a.bounds, ids[i]));
+        for (int i = firstRight - 1; i < end - 1; i++) {
+            leftCounter++;
+            leftAcc = combine(leftAcc, loadBox(a.bounds, ids[i]));
+            const float leftCost = halfArea(leftAcc) * leftCounter;
+            const float cost = leftCost + a.rcost[i + 1];
+            if (cost < bestCost) { bestSplit = i + 1; bestAxis = axis; bestCost = cost; }
+            else if (leftCost >= bestCost) break;
+        }
+    }
+    if (bestCost == FLT_MAX) { bestAxis = 0; bestSplit = start + count / 2; }
+    if (count <= a.p.maxLeafTriangleCount) {
+        const float notSplitCost = a.p.triangleCost * (float)count;
+        const float newCost = 1.0f + (a.p.triangleCost * bestCost / halfArea(parentBox));
+        if (newCost >= notSplitCost) return -1;
+    }
+    int* ids = a.ids[bestAxis];
+    const bool swapSides = halfArea(rangeBox(a.bounds, ids, start, bestSplit)) < halfArea(rangeBox(a.bounds, ids, bestSplit, end));
+    for (int i = start; i < bestSplit; i++) a.table[ids[i]] = !swapSides;
+    for (int i = bestSplit; i < end; i++) a.table[ids[i]] = swapSides;
+    int* aux = a.aux + start;
+    if (swapSides) bestSplit = start + stablePartition(ids + start, count, aux, a.table);
+    stablePartition(a.ids[(bestAxis + 1) % 3] + start, count, aux, a.table);
+    stablePartition(a.ids[(bestAxis + 2) % 3] + start, count, aux, a.table);
+    return bestSplit;
+}
+
+__global__ void k_split_small(TreeArgs a, int n) {
+    const int t = blockIdx.x * blockDim.x + threadIdx.x;
+    if (t >= n) return;
+    int2 stack[SMALL_NODE + 1];   // a subtree of c fragments is at most c - 1 deep
+    int sp = 0;
+    stack[sp++] = a.small[t];
+    while (sp > 0) {
+        const int2 task = stack[--sp];
+        GpuBlasNode& parent = a.nodes[task.x];
+        const int start = parent.TriStartOrChild, count = parent.TriCount;
+        const FBox box = rangeBox(a.bounds, a.ids[0], start, start + count);
+        setBounds(parent, box);
+        const int split = trySplitSerial(a, box, start, count);
+        if (split < 0) continue;
+        writeChildren(a, task.x, task, start, count, split);
+        const int lc = split - start;
+        stack[sp++] = make_int2(task.y + 1, task.y + 1 + (2 * lc - 1));
+        stack[sp++] = make_int2(task.y, task.y + 2);
+    }
+}
+
+// ---------------------------------------------------------------------------------------------------------------- post passes
+__global__ void k_root_duplicate(GpuBlasNode* nodes, int* parent, int* depth, int* ostart, int* ocount, int n) {
+    GpuBlasNode root = nodes[1];
+    nodes[2] = root;
+    nodes[3] = root;
+    root.TriStartOrChild = 2;
+    root.TriCount = 0;
+    nodes[1] = root;
+    for (int k = 2; k < 4; k++) { parent[k] = 1; depth[k] = 1; ostart[k] = 0; ocount[k] = n; }
+}
+
+// computeRequiredStackSize, bottom up: g(v) = 0 if both children of v are leaves, g(inner child) if one is, and
+// max(g(l), g(r)) + 1 if both are. Each climb starts at a node with two leaf children; at a node with two inner children
+// the second arrival continues.
+__global__ void k_stack_size(const GpuBlasNode* nodes, const int* parent, const int* depth, int cap, int* g, int* arrive) {
+    int v = blockIdx.x * blockDim.x + threadIdx.x;
+    if (v < 1 || v >= cap || depth[v] < 0 || nodes[v].TriCount > 0) return;
+    const int c0 = nodes[v].TriStartOrChild;
+    if (!(nodes[c0].TriCount > 0 && nodes[c0 + 1].TriCount > 0)) return;
+    int gv = 0;
+    g[v] = 0;
+    for (;;) {
+        const int p = parent[v];
+        if (p <= 0) return;
+        const int c = nodes[p].TriStartOrChild;
+        const bool li = !(nodes[c].TriCount > 0), ri = !(nodes[c + 1].TriCount > 0);
+        if (li && ri) {
+            __threadfence();
+            if (atomicAdd(&arrive[p], 1) == 0) return;
+            __threadfence();
+            const int gl = ((volatile int*)g)[c], gr = ((volatile int*)g)[c + 1];
+            gv = max(gl, gr) + 1;
+        }
+        ((volatile int*)g)[p] = gv;
+        v = p;
+    }
+}
+
+// Pre-order ranks: the nodes whose range starts at fragment s are a chain of left children, one per depth from the
+// highest one (dmin) down to a leaf (dleaf); pre-order lists the chains by s. rank = base[s] + depth - dmin[s].
+__global__ void k_chain_ends(const GpuBlasNode* nodes, const int* depth, const int* ostart, int cap, int* dmin, int* dleaf) {
+    const int v = blockIdx.x * blockDim.x + threadIdx.x;
+    if (v < 1 || v >= cap || depth[v] < 0) return;
+    atomicMin(&dmin[ostart[v]], depth[v]);
+    if (nodes[v].TriCount > 0) dleaf[ostart[v]] = depth[v];
+}
+__global__ void k_chain_len(const int* dmin, const int* dleaf, int n, int* len) {
+    const int s = blockIdx.x * blockDim.x + threadIdx.x;
+    if (s < n) len[s] = dmin[s] == DEPTH_NONE ? 0 : dleaf[s] - dmin[s] + 1;
+}
+__global__ void k_preorder(const int* depth, const int* ostart, int cap, const int* dmin, const int* base, int* order) {
+    const int v = blockIdx.x * blockDim.x + threadIdx.x;
+    if (v < 1 || v >= cap || depth[v] < 0) return;
+    const int s = ostart[v];
+    order[base[s] + depth[v] - dmin[s]] = v;
+}
+__global__ void k_preorder_root_duplicate(int* order) { order[0] = 1; order[1] = 2; order[2] = 3; }
+
+// computeGlobalSAH terms in pre-order; leaf counts from `counts` (by node id) or, for the compacted tree, `final`.
+__global__ void k_sah_terms(const int* order, int m, const GpuBlasNode* nodes, const GpuBlasNode* final, const int* fidx,
+                            float triangleCost, double* terms) {
+    const int j = blockIdx.x * blockDim.x + threadIdx.x;
+    if (j >= m) return;
+    const int v = order[j];
+    const GpuBlasNode n = final ? final[fidx[v]] : nodes[v];
+    const GpuBlasNode root = final ? final[1] : nodes[1];
+    const double rootArea = 1.0 / (double)nodeHalfArea(root);
+    const double prob = (double)nodeHalfArea(n) * rootArea;
+    terms[j] = n.TriCount > 0 ? (double)(triangleCost * (float)n.TriCount) * prob : 1.0 * prob;
+}
+
+// collapseDeepestLevel's cost terms, in pre-order (the nodes that add one never contain each other, so this is also the
+// mirror's post-order among them). First pass: inner nodes deeper than `level` whose children are both leaves. Later passes:
+// inner nodes at depth `level`, whose children are leaves after the pass's collapse and hold their whole subtrees.
+__global__ void k_collapse_terms(const int* order, int m, const GpuBlasNode* nodes, const int* depth, const int* ocount,
+                                 int level, int firstPass, float triangleCost, double* terms, uint8_t* flags) {
+    const int j = blockIdx.x * blockDim.x + threadIdx.x;
+    if (j >= m) return;
+    const int v = order[j];
+    const GpuBlasNode n = nodes[v];
+    bool q = false;
+    if (!(n.TriCount > 0)) {
+        const int c = n.TriStartOrChild;
+        q = firstPass ? (depth[v] > level && nodes[c].TriCount > 0 && nodes[c + 1].TriCount > 0) : depth[v] == level;
+        if (q) {
+            const int lc = ocount[c], rc = ocount[c + 1];
+            const double leavesCost = (double)triangleCost * ((double)lc * (double)nodeHalfArea(nodes[c]) + (double)rc * (double)nodeHalfArea(nodes[c + 1]));
+            const double newParentLeafCost = (double)triangleCost * (double)(lc + rc);
+            terms[j] = ((double)nodeHalfArea(n) * (newParentLeafCost - 1.0) - leavesCost) / (double)nodeHalfArea(nodes[1]);
+        }
+    }
+    flags[j] = q;
+}
+
+__global__ void k_reachable(const int* order, int m, const int* depth, int maxDepth, uint8_t* flags) {
+    const int j = blockIdx.x * blockDim.x + threadIdx.x;
+    if (j < m) flags[j] = depth[order[j]] <= maxDepth;
+}
+
+// After the collapse passes a node is inner if it was split and is shallower than the collapsed level.
+__device__ __forceinline__ bool finalInner(const GpuBlasNode* nodes, const int* depth, int v, int maxDepth) {
+    return !(nodes[v].TriCount > 0) && depth[v] < maxDepth;
+}
+__global__ void k_inner_flags(const int* order, int m, const GpuBlasNode* nodes, const int* depth, int maxDepth, int* flags) {
+    const int j = blockIdx.x * blockDim.x + threadIdx.x;
+    if (j < m) flags[j] = finalInner(nodes, depth, order[j], maxDepth);
+}
+__global__ void k_inner_ranks(const int* order, int m, const int* scan, int* rankOf) {
+    const int j = blockIdx.x * blockDim.x + threadIdx.x;
+    if (j < m) rankOf[order[j]] = scan[j];
+}
+
+// removeEmptySubtrees: the children of the inner node of pre-order rank k land at 2 + 2k.
+__global__ void k_final_nodes(const int* order, int m, const GpuBlasNode* nodes, const int* parent, const int* depth,
+                              const int* ostart, const int* ocount, const int* rankOf, int maxDepth, GpuBlasNode* final, int* fidx) {
+    const int j = blockIdx.x * blockDim.x + threadIdx.x;
+    if (j >= m) return;
+    const int v = order[j];
+    int fi = 1;
+    if (v != 1) {
+        const int p = parent[v];
+        fi = 2 + 2 * rankOf[p] + (v == nodes[p].TriStartOrChild + 1 ? 1 : 0);
+    }
+    fidx[v] = fi;
+    GpuBlasNode out = nodes[v];
+    if (finalInner(nodes, depth, v, maxDepth)) { out.TriStartOrChild = 2 + 2 * rankOf[v]; out.TriCount = 0; }
+    else { out.TriStartOrChild = ostart[v]; out.TriCount = ocount[v]; }
+    final[fi] = out;
+}
+
+// BLAS.GetUnindexedTriangles: leaves in node order, fragment = triangle. The array holds n triangles; when the root is a
+// leaf, its two copies list all n each, and the second one's triangles would land past the end: the mirror writes them
+// beyond its n-element array (heap overflow), so what it returns is the first copy's n triangles and the second leaf's
+// offset n. The writes past n are dropped here.
+__global__ void k_leaf_counts(const GpuBlasNode* final, int f, int* counts) {
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i < f) counts[i] = (i >= 2 && final[i].TriCount > 0) ? final[i].TriCount : 0;
+}
+__global__ void k_unindex_plain(GpuBlasNode* final, int f, const int* offsets, const int* ids0, const GpuBlasTriangle* in,
+                                GpuBlasTriangle* out, int n) {
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i < 2 || i >= f || !(final[i].TriCount > 0)) return;
+    const int s = final[i].TriStartOrChild, c = final[i].TriCount, o = offsets[i];
+    for (int k = 0; k < c && o + k < n; k++) out[o + k] = in[ids0[s + k]];
+    final[i].TriStartOrChild = o;
+}
+
+// PreSplitting.GetUnindexedTriangles: per leaf the sorted unique triangle ids, from one sort of (leaf start, triangle id)
+__global__ void k_leaf_marks(const GpuBlasNode* final, int f, int* marks) {
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= 2 && i < f && final[i].TriCount > 0) marks[final[i].TriStartOrChild] = final[i].TriStartOrChild;
+}
+__global__ void k_leaf_keys(const int* segStart, const int* ids0, const int* origIds, int n, unsigned long long* keys) {
+    const int q = blockIdx.x * blockDim.x + threadIdx.x;
+    if (q < n) keys[q] = ((unsigned long long)(uint32_t)segStart[q] << 32) | (uint32_t)origIds[ids0[q]];
+}
+
+struct MaxOp { __device__ int operator()(int x, int y) const { return x > y ? x : y; } };
+
+struct Uniq {   // walks the sorted ids of one leaf, skipping repeats
+    const unsigned long long* k;
+    int i, end;
+    __device__ Uniq(const unsigned long long* keys, const GpuBlasNode& leaf) : k(keys), i(leaf.TriStartOrChild), end(leaf.TriStartOrChild + leaf.TriCount) {}
+    __device__ bool done() const { return i >= end; }
+    __device__ int cur() const { return (int)(uint32_t)k[i]; }
+    __device__ void next() { const int c = cur(); while (i < end && cur() == c) i++; }
+};
+__device__ int uniqueCount(const unsigned long long* keys, const GpuBlasNode& leaf) {
+    int c = 0;
+    for (Uniq u(keys, leaf); !u.done(); u.next()) c++;
+    return c;
+}
+__device__ int sharedCount(const unsigned long long* keys, const GpuBlasNode& l, const GpuBlasNode& r) {
+    int c = 0;
+    Uniq a(keys, l), b(keys, r);
+    while (!a.done() && !b.done()) {
+        if (a.cur() < b.cur()) a.next();
+        else if (b.cur() < a.cur()) b.next();
+        else { c++; a.next(); b.next(); }
+    }
+    return c;
+}
+
+__global__ void k_pair_sizes(const GpuBlasNode* final, int pairs, const unsigned long long* keys, int* sizes) {
+    const int p = blockIdx.x * blockDim.x + threadIdx.x;
+    if (p > pairs) return;
+    if (p == pairs) { sizes[p] = 0; return; }
+    const GpuBlasNode l = final[2 + 2 * p], r = final[3 + 2 * p];
+    const bool ll = l.TriCount > 0, rl = r.TriCount > 0;
+    int s = 0;
+    if (ll && rl) s = uniqueCount(keys, l) + uniqueCount(keys, r) - sharedCount(keys, l, r);
+    else if (ll) s = uniqueCount(keys, l);
+    else if (rl) s = uniqueCount(keys, r);
+    sizes[p] = s;
+}
+
+__global__ void k_pair_write(GpuBlasNode* final, int pairs, const unsigned long long* keys, const int* offsets,
+                             const GpuBlasTriangle* in, GpuBlasTriangle* out) {
+    const int p = blockIdx.x * blockDim.x + threadIdx.x;
+    if (p >= pairs) return;
+    GpuBlasNode& l = final[2 + 2 * p];
+    GpuBlasNode& r = final[3 + 2 * p];
+    const bool ll = l.TriCount > 0, rl = r.TriCount > 0;
+    const int counter = offsets[p];
+    if (ll && rl) {
+        const GpuBlasNode L = l, R = r;
+        const int lu = uniqueCount(keys, L), ru = uniqueCount(keys, R);
+        int onlyLeft = 0, backwards = 0;
+        {   // left ids ascending: the ones also in the right leaf fill the end of the left range backwards
+            Uniq a(keys, L), b(keys, R);
+            for (; !a.done(); a.next()) {
+                const int id = a.cur();
+                while (!b.done() && b.cur() < id) b.next();
+                if (!b.done() && b.cur() == id) out[counter + lu - backwards++ - 1] = in[id];
+                else out[counter + onlyLeft++] = in[id];
+            }
+        }
+        int onlyRight = 0;
+        {
+            Uniq a(keys, R), b(keys, L);
+            for (; !a.done(); a.next()) {
+                const int id = a.cur();
+                while (!b.done() && b.cur() < id) b.next();
+                if (!(!b.done() && b.cur() == id)) out[counter + lu + onlyRight++] = in[id];
+            }
+        }
+        l.TriStartOrChild = counter; l.TriCount = lu;
+        r.TriStartOrChild = counter + onlyLeft; r.TriCount = ru;
+    } else if (ll || rl) {
+        GpuBlasNode& leaf = ll ? l : r;
+        const GpuBlasNode Lf = leaf;
+        int c = 0;
+        for (Uniq u(keys, Lf); !u.done(); u.next()) out[counter + c++] = in[u.cur()];
+        leaf.TriStartOrChild = counter;
+        leaf.TriCount = c;
+    }
+}
+
+}  // namespace idkbb
+
+// ---------------------------------------------------------------------------------------------------------------- host driver
+struct IdkPtBlasBuild {
+    std::vector<GpuBlasNode> nodes;
+    std::vector<GpuBlasTriangle> tris;
+    int32_t requiredStackSize = 0;
+    int32_t fragmentCount = 0;
+    double sah = 0.0;
+};
+
+namespace idkbb {
+
+// Device allocations of one build, freed together.
+struct Arena {
+    std::vector<void*> ptrs;
+    ~Arena() { for (void* p : ptrs) cudaFree(p); }
+    template <class T> cudaError_t get(T*& out, size_t count) {
+        void* p = nullptr;
+        cudaError_t e = cudaMalloc(&p, std::max<size_t>(count, 1) * sizeof(T));
+        if (e == cudaSuccess) ptrs.push_back(p);
+        out = (T*)p;
+        return e;
+    }
+};
+
+// Per-stage device times (IDKPT_BLAS_TIMING=1 prints them to stderr, like the host mirror's IDKHOST_TIMING).
+struct StageTimer {
+    cudaStream_t s;
+    std::vector<std::pair<const char*, cudaEvent_t>> marks;
+    explicit StageTimer(cudaStream_t st) : s(st) {}
+    ~StageTimer() { for (auto& m : marks) cudaEventDestroy(m.second); }
+    void mark(const char* what) {
+        cudaEvent_t e;
+        if (cudaEventCreate(&e) != cudaSuccess) return;
+        cudaEventRecord(e, s);
+        marks.push_back({what, e});
+    }
+    float total() {
+        float ms = 0.0f;
+        if (marks.size() >= 2) cudaEventElapsedTime(&ms, marks.front().second, marks.back().second);
+        return ms;
+    }
+    void print(int fragments) {
+        if (!getenv("IDKPT_BLAS_TIMING")) return;
+        for (size_t i = 1; i < marks.size(); i++) {
+            float ms = 0.0f;
+            cudaEventElapsedTime(&ms, marks[i - 1].second, marks[i].second);
+            fprintf(stderr, "[idkpt_blas_build] %-14s %8.2f ms\n", marks[i].first, ms);
+        }
+        fprintf(stderr, "[idkpt_blas_build] %-14s %8.2f ms (%d fragments)\n", "total", total(), fragments);
+    }
+};
+
+template <class F> static inline int blocksFor(F n, int t) { return (int)((n + t - 1) / t); }
+
+enum { BB_OK = 0, BB_CUDA = 1, BB_TOO_MANY_FRAGMENTS = 2 };
+
+#define BB_CK(call)                                                                                     \
+    do {                                                                                                \
+        cudaError_t e_ = (call);                                                                        \
+        if (e_ != cudaSuccess) { err = std::string(#call) + ": " + cudaGetErrorString(e_); return BB_CUDA; } \
+    } while (0)
+
+// Runs the whole build on `stream`; the arguments have been validated. Fills `out` and the total device time.
+static int build(cudaStream_t stream, const PackedVec3* hPos, uint64_t vertexCount, const GpuBlasTriangle* hTris, int triCount,
+                 const Params& p, IdkPtBlasBuild& out, float& totalMs, std::string& err) {
+    Arena ar;
+    StageTimer tm(stream);
+    tm.mark("start");
+    PackedVec3* pos;
+    GpuBlasTriangle* tris;
+    BB_CK(ar.get(pos, vertexCount));
+    BB_CK(ar.get(tris, triCount));
+    BB_CK(cudaMemcpyAsync(pos, hPos, vertexCount * sizeof(PackedVec3), cudaMemcpyHostToDevice, stream));
+    BB_CK(cudaMemcpyAsync(tris, hTris, (size_t)triCount * sizeof(GpuBlasTriangle), cudaMemcpyHostToDevice, stream));
+    tm.mark("upload");
+
+    // ---- 1. fragments
+    int n = triCount;
+    FBox* bounds = nullptr;
+    int* origIds = nullptr;
+    void* cubTemp = nullptr;
+    size_t cubBytes = 0;
+    auto cubScratch = [&](size_t need) -> cudaError_t {
+        if (need <= cubBytes) return cudaSuccess;
+        uint8_t* q;
+        cudaError_t e = ar.get(q, need);
+        if (e == cudaSuccess) { cubTemp = q; cubBytes = need; }
+        return e;
+    };
+    if (p.doPreSplit) {
+        float* prio;
+        float* total;
+        unsigned long long *counts, *offsets;
+        FBox* gbox;
+        BB_CK(ar.get(prio, triCount));
+        BB_CK(ar.get(total, 1));
+        BB_CK(ar.get(counts, (size_t)triCount + 1));
+        BB_CK(ar.get(offsets, (size_t)triCount + 1));
+        BB_CK(ar.get(gbox, 1));
+        k_priorities<<<blocksFor(triCount, 256), 256, 0, stream>>>(pos, tris, triCount, prio);
+        tm.mark("priorities");
+        BB_CK(cudaMemsetAsync(total, 0, sizeof(float), stream));
+        k_ordered_sum<float, 8192><<<1, SUM_THREADS, 0, stream>>>(prio, triCount, nullptr, total);
+        tm.mark("priority sum");
+        k_split_counts<<<blocksFor(triCount + 1, 256), 256, 0, stream>>>(prio, total, triCount, p.splitFactor, counts);
+        size_t need = 0;
+        BB_CK(cub::DeviceScan::ExclusiveSum(nullptr, need, counts, offsets, triCount + 1, stream));
+        BB_CK(cubScratch(need));
+        BB_CK(cub::DeviceScan::ExclusiveSum(cubTemp, need, counts, offsets, triCount + 1, stream));
+        unsigned long long fragments = 0;
+        BB_CK(cudaMemcpyAsync(&fragments, offsets + triCount, sizeof(fragments), cudaMemcpyDeviceToHost, stream));
+        BB_CK(cudaStreamSynchronize(stream));
+        if (fragments > (unsigned long long)MAX_FRAGMENTS) {
+            err = "pre-splitting makes " + std::to_string(fragments) + " fragments, more than 2^24";
+            return BB_TOO_MANY_FRAGMENTS;
+        }
+        n = (int)fragments;
+        BB_CK(ar.get(bounds, n));
+        BB_CK(ar.get(origIds, n));
+        k_global_box<<<1, 1024, 0, stream>>>(pos, tris, triCount, gbox);
+        k_presplit<<<blocksFor(triCount, 128), 128, 0, stream>>>(pos, tris, triCount, offsets, gbox, bounds, origIds);
+        tm.mark("split");
+    } else {
+        BB_CK(ar.get(bounds, n));
+        k_tri_bounds<<<blocksFor(n, 256), 256, 0, stream>>>(pos, tris, n, bounds);
+        tm.mark("bounds");
+    }
+
+    // ---- 2. three stable sorts by centroid key
+    TreeArgs a = {};
+    {
+        uint32_t *keys, *keysOut;
+        int* vals;
+        BB_CK(ar.get(keys, n));
+        BB_CK(ar.get(keysOut, n));
+        BB_CK(ar.get(vals, n));
+        for (int axis = 0; axis < 3; axis++) {
+            BB_CK(ar.get(a.ids[axis], n));
+            k_sort_keys<<<blocksFor(n, 256), 256, 0, stream>>>(bounds, n, axis, keys, vals);
+            size_t need = 0;
+            BB_CK(cub::DeviceRadixSort::SortPairs(nullptr, need, keys, keysOut, vals, a.ids[axis], n, 0, 32, stream));
+            BB_CK(cubScratch(need));
+            BB_CK(cub::DeviceRadixSort::SortPairs(cubTemp, need, keys, keysOut, vals, a.ids[axis], n, 0, 32, stream));
+        }
+    }
+    tm.mark("sort");
+
+    // ---- 3. tree
+    const int cap = std::max(2 * n, 4);
+    a.bounds = bounds;
+    a.p = p;
+    BB_CK(ar.get(a.aux, n));
+    BB_CK(ar.get(a.table, n));
+    BB_CK(ar.get(a.rcost, n));
+    BB_CK(ar.get(a.nodes, cap));
+    BB_CK(ar.get(a.parent, cap));
+    BB_CK(ar.get(a.depth, cap));
+    BB_CK(ar.get(a.ostart, cap));
+    BB_CK(ar.get(a.ocount, cap));
+    const int bigCap = n / (SMALL_NODE + 1) + 2;
+    int2 *big[2], *small;
+    int* counters;   // [0]: next level's large nodes, [1]: small subtrees
+    BB_CK(ar.get(big[0], bigCap));
+    BB_CK(ar.get(big[1], bigCap));
+    BB_CK(ar.get(small, n + 1));
+    BB_CK(ar.get(counters, 2));
+    BB_CK(cudaMemsetAsync(a.nodes, 0, (size_t)cap * sizeof(GpuBlasNode), stream));
+    BB_CK(cudaMemsetAsync(a.depth, 0xFF, (size_t)cap * sizeof(int), stream));
+    BB_CK(cudaMemsetAsync(counters, 0, 2 * sizeof(int), stream));
+    {
+        GpuBlasNode root = {};
+        root.TriStartOrChild = 0;
+        root.TriCount = n;
+        const int zero = 0;
+        const int2 task = make_int2(1, 2);
+        BB_CK(cudaMemcpyAsync(a.nodes + 1, &root, sizeof(root), cudaMemcpyHostToDevice, stream));
+        BB_CK(cudaMemcpyAsync(a.parent + 1, &zero, 4, cudaMemcpyHostToDevice, stream));
+        BB_CK(cudaMemcpyAsync(a.depth + 1, &zero, 4, cudaMemcpyHostToDevice, stream));
+        BB_CK(cudaMemcpyAsync(a.ostart + 1, &zero, 4, cudaMemcpyHostToDevice, stream));
+        BB_CK(cudaMemcpyAsync(a.ocount + 1, &n, 4, cudaMemcpyHostToDevice, stream));
+        if (n > SMALL_NODE) BB_CK(cudaMemcpyAsync(big[0], &task, sizeof(task), cudaMemcpyHostToDevice, stream));
+        else {
+            const int one = 1;
+            BB_CK(cudaMemcpyAsync(small, &task, sizeof(task), cudaMemcpyHostToDevice, stream));
+            BB_CK(cudaMemcpyAsync(counters + 1, &one, 4, cudaMemcpyHostToDevice, stream));
+        }
+        BB_CK(cudaStreamSynchronize(stream));   // the host values above go out of scope
+    }
+    a.nextCount = counters;
+    a.small = small;
+    a.smallCount = counters + 1;
+    int levelCount = n > SMALL_NODE ? 1 : 0, cur = 0;
+    int hostCounters[2] = {0, 0};
+    while (levelCount > 0) {
+        a.tasks = big[cur];
+        a.nextTasks = big[cur ^ 1];
+        BB_CK(cudaMemsetAsync(counters, 0, sizeof(int), stream));
+        k_split_large<<<levelCount, BIG_THREADS, 0, stream>>>(a);
+        BB_CK(cudaMemcpyAsync(hostCounters, counters, 2 * sizeof(int), cudaMemcpyDeviceToHost, stream));
+        BB_CK(cudaStreamSynchronize(stream));
+        levelCount = hostCounters[0];
+        cur ^= 1;
+    }
+    tm.mark("tree (large)");
+    BB_CK(cudaMemcpyAsync(hostCounters, counters, 2 * sizeof(int), cudaMemcpyDeviceToHost, stream));
+    BB_CK(cudaStreamSynchronize(stream));
+    if (hostCounters[1] > 0) k_split_small<<<blocksFor(hostCounters[1], 64), 64, 0, stream>>>(a, hostCounters[1]);
+    BB_CK(cudaGetLastError());
+    tm.mark("tree (small)");
+
+    // ---- 4. post passes
+    GpuBlasNode hRoot;
+    BB_CK(cudaMemcpyAsync(&hRoot, a.nodes + 1, sizeof(hRoot), cudaMemcpyDeviceToHost, stream));
+    BB_CK(cudaStreamSynchronize(stream));
+    const bool rootLeaf = hRoot.TriCount > 0;
+    if (rootLeaf) k_root_duplicate<<<1, 1, 0, stream>>>(a.nodes, a.parent, a.depth, a.ostart, a.ocount, n);
+
+    int *g, *arrive;
+    BB_CK(ar.get(g, cap));
+    BB_CK(ar.get(arrive, cap));
+    BB_CK(cudaMemsetAsync(arrive, 0, (size_t)cap * sizeof(int), stream));
+    k_stack_size<<<blocksFor(cap, 256), 256, 0, stream>>>(a.nodes, a.parent, a.depth, cap, g, arrive);
+    int requiredStackSize = 0;
+    BB_CK(cudaMemcpyAsync(&requiredStackSize, g + 1, 4, cudaMemcpyDeviceToHost, stream));
+
+    // pre-order of every node of the built tree
+    int* order;
+    int m = 0;
+    BB_CK(ar.get(order, cap));
+    if (rootLeaf) {
+        k_preorder_root_duplicate<<<1, 1, 0, stream>>>(order);
+        m = 3;
+    } else {
+        int *dmin, *dleaf, *len, *base;
+        BB_CK(ar.get(dmin, n));
+        BB_CK(ar.get(dleaf, n));
+        BB_CK(ar.get(len, n + 1));
+        BB_CK(ar.get(base, n + 1));
+        BB_CK(cudaMemsetAsync(dmin, 0x7F, (size_t)n * sizeof(int), stream));   // DEPTH_NONE
+        k_chain_ends<<<blocksFor(cap, 256), 256, 0, stream>>>(a.nodes, a.depth, a.ostart, cap, dmin, dleaf);
+        k_chain_len<<<blocksFor(n, 256), 256, 0, stream>>>(dmin, dleaf, n, len);
+        BB_CK(cudaMemsetAsync(len + n, 0, sizeof(int), stream));
+        size_t need = 0;
+        BB_CK(cub::DeviceScan::ExclusiveSum(nullptr, need, len, base, n + 1, stream));
+        BB_CK(cubScratch(need));
+        BB_CK(cub::DeviceScan::ExclusiveSum(cubTemp, need, len, base, n + 1, stream));
+        k_preorder<<<blocksFor(cap, 256), 256, 0, stream>>>(a.depth, a.ostart, cap, dmin, base, order);
+        BB_CK(cudaMemcpyAsync(&m, base + n, 4, cudaMemcpyDeviceToHost, stream));
+    }
+    BB_CK(cudaStreamSynchronize(stream));
+    tm.mark("stack size");
+
+    double* terms;
+    double* acc;   // [0]: SAH of the built tree, [1]: added collapse cost, [2]: final SAH
+    double* packed;
+    uint8_t* flags;
+    int* selCount;
+    BB_CK(ar.get(terms, cap));
+    BB_CK(ar.get(packed, cap));
+    BB_CK(ar.get(acc, 3));
+    BB_CK(ar.get(flags, cap));
+    BB_CK(ar.get(selCount, 1));
+    BB_CK(cudaMemsetAsync(acc, 0, 3 * sizeof(double), stream));
+    auto flaggedSum = [&](double* dst) -> int {   // dst += the flagged terms, in order
+        size_t need = 0;
+        BB_CK(cub::DeviceSelect::Flagged(nullptr, need, terms, flags, packed, selCount, m, stream));
+        BB_CK(cubScratch(need));
+        BB_CK(cub::DeviceSelect::Flagged(cubTemp, need, terms, flags, packed, selCount, m, stream));
+        k_ordered_sum<double, 4096><<<1, SUM_THREADS, 0, stream>>>(packed, 0, selCount, dst);
+        return BB_OK;
+    };
+
+    // OptimizeStackSize
+    int maxDepth = INT_MAX;   // nodes deeper than this are gone after the collapse passes
+    if (requiredStackSize >= p.stackOptThreshold) {
+        k_sah_terms<<<blocksFor(m, 256), 256, 0, stream>>>(order, m, a.nodes, nullptr, nullptr, p.triangleCost, terms);
+        k_ordered_sum<double, 4096><<<1, SUM_THREADS, 0, stream>>>(terms, m, nullptr, acc + 0);
+        k_collapse_terms<<<blocksFor(m, 256), 256, 0, stream>>>(order, m, a.nodes, a.depth, a.ocount, requiredStackSize - 1, 1,
+                                                                 p.triangleCost, terms, flags);
+        if (int rc = flaggedSum(acc + 1)) return rc;
+        double h[2];
+        BB_CK(cudaMemcpyAsync(h, acc, sizeof(h), cudaMemcpyDeviceToHost, stream));
+        BB_CK(cudaStreamSynchronize(stream));
+        // (the mirror's stackOptMaxLeafTriangleCount is INT_MAX: no collapse of at most 2^24 fragments exceeds it)
+        double increasePercent = h[1] / h[0];
+        while (increasePercent <= (double)p.stackOptSahIncreaseAcceptance && requiredStackSize > 0) {
+            const int level = --requiredStackSize;
+            maxDepth = level + 1;
+            k_collapse_terms<<<blocksFor(m, 256), 256, 0, stream>>>(order, m, a.nodes, a.depth, a.ocount, level, 0,
+                                                                     p.triangleCost, terms, flags);
+            if (int rc = flaggedSum(acc + 1)) return rc;
+            BB_CK(cudaMemcpyAsync(h, acc, sizeof(h), cudaMemcpyDeviceToHost, stream));
+            BB_CK(cudaStreamSynchronize(stream));
+            increasePercent = h[1] / h[0];
+        }
+    }
+    tm.mark("stack opt");
+
+    // removeEmptySubtrees: the nodes left after the collapse, in pre-order
+    int* order2 = order;
+    int m2 = m;
+    if (maxDepth != INT_MAX) {
+        BB_CK(ar.get(order2, m));
+        k_reachable<<<blocksFor(m, 256), 256, 0, stream>>>(order, m, a.depth, maxDepth, flags);
+        size_t need = 0;
+        BB_CK(cub::DeviceSelect::Flagged(nullptr, need, order, flags, order2, selCount, m, stream));
+        BB_CK(cubScratch(need));
+        BB_CK(cub::DeviceSelect::Flagged(cubTemp, need, order, flags, order2, selCount, m, stream));
+        BB_CK(cudaMemcpyAsync(&m2, selCount, 4, cudaMemcpyDeviceToHost, stream));
+        BB_CK(cudaStreamSynchronize(stream));
+    }
+    int *innerFlag, *innerScan, *rankOf, *fidx;
+    BB_CK(ar.get(innerFlag, m2 + 1));
+    BB_CK(ar.get(innerScan, m2 + 1));
+    BB_CK(ar.get(rankOf, cap));
+    BB_CK(ar.get(fidx, cap));
+    k_inner_flags<<<blocksFor(m2, 256), 256, 0, stream>>>(order2, m2, a.nodes, a.depth, maxDepth, innerFlag);
+    BB_CK(cudaMemsetAsync(innerFlag + m2, 0, sizeof(int), stream));
+    {
+        size_t need = 0;
+        BB_CK(cub::DeviceScan::ExclusiveSum(nullptr, need, innerFlag, innerScan, m2 + 1, stream));
+        BB_CK(cubScratch(need));
+        BB_CK(cub::DeviceScan::ExclusiveSum(cubTemp, need, innerFlag, innerScan, m2 + 1, stream));
+    }
+    int inner = 0;
+    BB_CK(cudaMemcpyAsync(&inner, innerScan + m2, 4, cudaMemcpyDeviceToHost, stream));
+    BB_CK(cudaStreamSynchronize(stream));
+    k_inner_ranks<<<blocksFor(m2, 256), 256, 0, stream>>>(order2, m2, innerScan, rankOf);
+    const int f = 2 + 2 * inner;
+    GpuBlasNode* final;
+    BB_CK(ar.get(final, f));
+    BB_CK(cudaMemsetAsync(final, 0, sizeof(GpuBlasNode) * 2, stream));
+    k_final_nodes<<<blocksFor(m2, 256), 256, 0, stream>>>(order2, m2, a.nodes, a.parent, a.depth, a.ostart, a.ocount, rankOf,
+                                                          maxDepth, final, fidx);
+    tm.mark("compact");
+
+    // unindexing
+    GpuBlasTriangle* outTris;
+    BB_CK(ar.get(outTris, n));
+    int triOut = n;
+    if (!p.doPreSplit) {
+        int *cnt, *off;
+        BB_CK(ar.get(cnt, f));
+        BB_CK(ar.get(off, f));
+        k_leaf_counts<<<blocksFor(f, 256), 256, 0, stream>>>(final, f, cnt);
+        size_t need = 0;
+        BB_CK(cub::DeviceScan::ExclusiveSum(nullptr, need, cnt, off, f, stream));
+        BB_CK(cubScratch(need));
+        BB_CK(cub::DeviceScan::ExclusiveSum(cubTemp, need, cnt, off, f, stream));
+        k_unindex_plain<<<blocksFor(f, 256), 256, 0, stream>>>(final, f, off, a.ids[0], tris, outTris, n);
+    } else {
+        int *marks, *segStart, *sizes, *off;
+        unsigned long long *keys, *keysSorted;
+        BB_CK(ar.get(marks, n));
+        BB_CK(ar.get(segStart, n));
+        BB_CK(ar.get(keys, n));
+        BB_CK(ar.get(keysSorted, n));
+        BB_CK(ar.get(sizes, inner + 1));
+        BB_CK(ar.get(off, inner + 1));
+        BB_CK(cudaMemsetAsync(marks, 0, (size_t)n * sizeof(int), stream));
+        k_leaf_marks<<<blocksFor(f, 256), 256, 0, stream>>>(final, f, marks);
+        size_t need = 0;
+        BB_CK(cub::DeviceScan::InclusiveScan(nullptr, need, marks, segStart, MaxOp(), n, stream));
+        BB_CK(cubScratch(need));
+        BB_CK(cub::DeviceScan::InclusiveScan(cubTemp, need, marks, segStart, MaxOp(), n, stream));
+        k_leaf_keys<<<blocksFor(n, 256), 256, 0, stream>>>(segStart, a.ids[0], origIds, n, keys);
+        int endBit = 32;
+        while ((1 << (endBit - 32)) < n && endBit < 64) endBit++;
+        need = 0;
+        BB_CK(cub::DeviceRadixSort::SortKeys(nullptr, need, keys, keysSorted, n, 0, endBit, stream));
+        BB_CK(cubScratch(need));
+        BB_CK(cub::DeviceRadixSort::SortKeys(cubTemp, need, keys, keysSorted, n, 0, endBit, stream));
+        k_pair_sizes<<<blocksFor(inner + 1, 256), 256, 0, stream>>>(final, inner, keysSorted, sizes);
+        need = 0;
+        BB_CK(cub::DeviceScan::ExclusiveSum(nullptr, need, sizes, off, inner + 1, stream));
+        BB_CK(cubScratch(need));
+        BB_CK(cub::DeviceScan::ExclusiveSum(cubTemp, need, sizes, off, inner + 1, stream));
+        k_pair_write<<<blocksFor(inner, 256), 256, 0, stream>>>(final, inner, keysSorted, off, tris, outTris);
+        BB_CK(cudaMemcpyAsync(&triOut, off + inner, 4, cudaMemcpyDeviceToHost, stream));
+    }
+    tm.mark("unindex");
+
+    k_sah_terms<<<blocksFor(m2, 256), 256, 0, stream>>>(order2, m2, nullptr, final, fidx, p.triangleCost, terms);
+    k_ordered_sum<double, 4096><<<1, SUM_THREADS, 0, stream>>>(terms, m2, nullptr, acc + 2);
+    tm.mark("sah");
+    BB_CK(cudaGetLastError());
+    BB_CK(cudaStreamSynchronize(stream));
+
+    out.nodes.resize(f);
+    out.tris.resize(triOut);
+    BB_CK(cudaMemcpyAsync(out.nodes.data(), final, (size_t)f * sizeof(GpuBlasNode), cudaMemcpyDeviceToHost, stream));
+    if (triOut) BB_CK(cudaMemcpyAsync(out.tris.data(), outTris, (size_t)triOut * sizeof(GpuBlasTriangle), cudaMemcpyDeviceToHost, stream));
+    BB_CK(cudaMemcpyAsync(&out.sah, acc + 2, sizeof(double), cudaMemcpyDeviceToHost, stream));
+    tm.mark("download");
+    BB_CK(cudaStreamSynchronize(stream));
+    out.requiredStackSize = requiredStackSize;
+    out.fragmentCount = n;
+    totalMs = tm.total();
+    tm.print(n);
+    return BB_OK;
+}
+
+#undef BB_CK
+
+}  // namespace idkbb

@@ -26,6 +26,7 @@
 #include "idk_transparency.cuh"
 #include "idk_lights_skybox.cuh"
 #include "idk_sky.cuh"
+#include "idk_blas_build.cuh"
 #include "idk_textures_host.h"
 
 #define IDKPT_ABI_VERSION 4u   // 2: IdkPtSceneDesc gained Textures / TextureCount; 3: IdkPtStats gained CompactMs / AccumulateMs, host-buffer registration;
@@ -1945,6 +1946,66 @@ IDKPT_API int idkpt_tlas_build(IdkPtCtx* ctx, int32_t searchRadius, float* kerne
     }
     return IDKPT_OK;
 }
+
+// BLAS.Build + PreSplitting.PreSplit on the device (BVH.BlasesBuild's loop body, BVH.cs:315-377): see idk_blas_build.cuh.
+IDKPT_API int idkpt_blas_build(IdkPtCtx* ctx, const PackedVec3* positions, uint64_t vertexCount, const GpuBlasTriangle* triangles,
+                               uint64_t triangleCount, const IdkPtBlasBuildSettings* settings, IdkPtBlasBuild** out, float* kernelMs) {
+    if (!ctx) return IDKPT_ERR_INVALID_ARGUMENT;
+    if (out) *out = nullptr;
+    if (kernelMs) *kernelMs = 0.0f;
+    if (!positions || !triangles || !out) return fail(ctx, IDKPT_ERR_INVALID_ARGUMENT, "idkpt_blas_build: null argument");
+    if (triangleCount == 0) return fail(ctx, IDKPT_ERR_INVALID_ARGUMENT, "idkpt_blas_build: no triangles");
+    IdkPtBlasBuildSettings s;
+    if (settings) s = *settings;
+    else s = {1, 2, 1.1f, 16, 0.0009745f, 0.3f, 1};
+    if (!std::isfinite(s.TriangleCost) || !std::isfinite(s.StackOptSahIncreaseAcceptance) || !std::isfinite(s.SplitFactor))
+        return fail(ctx, IDKPT_ERR_INVALID_ARGUMENT, "idkpt_blas_build: non-finite setting");
+    if (s.StopSplittingThreshold < 1)   // a node of 0 fragments would read as an interior node (GpuBlasNode.TriCount == 0)
+        return fail(ctx, IDKPT_ERR_INVALID_ARGUMENT, "idkpt_blas_build: StopSplittingThreshold must be at least 1");
+    if (triangleCount > (uint64_t)idkbb::MAX_FRAGMENTS)
+        return fail(ctx, IDKPT_ERR_UNSUPPORTED, "idkpt_blas_build: more than 2^24 triangles");
+    for (uint64_t i = 0; i < triangleCount; i++) {
+        const GpuBlasTriangle& t = triangles[i];
+        if ((uint64_t)(uint32_t)t.X >= vertexCount || (uint64_t)(uint32_t)t.Y >= vertexCount || (uint64_t)(uint32_t)t.Z >= vertexCount)
+            return fail(ctx, IDKPT_ERR_INVALID_ARGUMENT, "idkpt_blas_build: vertex id out of range");
+    }
+    DRAIN_PENDING("idkpt_blas_build");
+    CK(cudaSetDevice(ctx->device));
+    idkbb::Params p = {s.StopSplittingThreshold, s.MaxLeafTriangleCount, s.TriangleCost, s.StackOptThreshold,
+                       s.StackOptSahIncreaseAcceptance, s.SplitFactor, s.DoPreSplit ? 1 : 0};
+    IdkPtBlasBuild* b = new IdkPtBlasBuild();
+    std::string err;
+    float ms = 0.0f;
+    const int rc = idkbb::build(ctx->stream, positions, vertexCount, triangles, (int)triangleCount, p, *b, ms, err);
+    if (rc != idkbb::BB_OK) {
+        delete b;
+        if (rc == idkbb::BB_CUDA) cudaStreamSynchronize(ctx->stream);
+        return fail(ctx, "idkpt_blas_build", rc == idkbb::BB_TOO_MANY_FRAGMENTS ? IDKPT_ERR_UNSUPPORTED : IDKPT_ERR_CUDA, err.c_str());
+    }
+    *out = b;
+    if (kernelMs) *kernelMs = ms;
+    return IDKPT_OK;
+}
+
+IDKPT_API int idkpt_blas_build_info(const IdkPtBlasBuild* b, uint64_t* nodeCount, uint64_t* triangleCount, int32_t* requiredStackSize,
+                                    int32_t* fragmentCount, double* sah) {
+    if (!b) return IDKPT_ERR_INVALID_ARGUMENT;
+    if (nodeCount) *nodeCount = b->nodes.size();
+    if (triangleCount) *triangleCount = b->tris.size();
+    if (requiredStackSize) *requiredStackSize = b->requiredStackSize;
+    if (fragmentCount) *fragmentCount = b->fragmentCount;
+    if (sah) *sah = b->sah;
+    return IDKPT_OK;
+}
+
+IDKPT_API int idkpt_blas_build_copy(const IdkPtBlasBuild* b, GpuBlasNode* nodes, GpuBlasTriangle* triangles) {
+    if (!b || !nodes || !triangles) return IDKPT_ERR_INVALID_ARGUMENT;
+    memcpy(nodes, b->nodes.data(), b->nodes.size() * sizeof(GpuBlasNode));
+    memcpy(triangles, b->tris.data(), b->tris.size() * sizeof(GpuBlasTriangle));
+    return IDKPT_OK;
+}
+
+IDKPT_API void idkpt_blas_build_free(IdkPtBlasBuild* b) { delete b; }
 
 IDKPT_API int idkpt_read_range(IdkPtCtx* ctx, IdkPtArrayId which, uint64_t first, uint64_t count, void* out) {
     if (!ctx || (!out && count)) return fail(ctx, IDKPT_ERR_INVALID_ARGUMENT, "idkpt_read_range: null argument");

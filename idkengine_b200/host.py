@@ -252,9 +252,11 @@ class Scene:
         self.source_triangle_count = 0
         self.build_info = []
 
-    def add(self, *models, threads=None, cache_dir=None):
+    def add(self, *models, threads=None, cache_dir=None, blas_builder=None):
         """ModelManager.Add (SRC/ModelManager.cs:128-213) + BVH.Add/BlasesBuild (SRC/Bvh/BVH.cs:236-276,300-451):
-        one BLAS + one instance per model. cache_dir (or $IDKHOST_BVH_CACHE): directory of the on-disk BLAS cache."""
+        one BLAS + one instance per model. cache_dir (or $IDKHOST_BVH_CACHE): directory of the on-disk BLAS cache.
+        blas_builder: a function with build_blas's (positions, triangles, presplit=...) signature and result, e.g. the device
+        build PathTracer.BuildBlas; default the host build (with `threads`). Both build the same BLAS, so the cache is shared."""
         cache_dir = cache_dir or os.environ.get("IDKHOST_BVH_CACHE") or None
         for m in models:
             v_off = len(self.positions)
@@ -299,7 +301,10 @@ class Scene:
                     b["triangles"]["MeshId"] += mesh_off
                     b["from_cache"] = True
             if b is None:
-                b = build_blas(self.positions, src, presplit=not m.refittable, threads=threads)
+                if blas_builder is None:
+                    b = build_blas(self.positions, src, presplit=not m.refittable, threads=threads)
+                else:
+                    b = blas_builder(self.positions, src, presplit=not m.refittable)
                 if cache_path is not None:
                     rel = dict(b)
                     rel["triangles"] = b["triangles"].copy()

@@ -38,6 +38,7 @@ class PathTracer:
         self._frame = None
         self._keep = None
         self.last_stats = None
+        self.last_blas_build_ms = None   # device time of the last BuildBlas
         self._export = False
 
     # ------------------------------------------------------------------ plumbing
@@ -140,6 +141,36 @@ class PathTracer:
         ms = ctypes.c_float()
         self._check(self._lib.idkpt_tlas_build(self._ctx, search_radius, ctypes.byref(ms)), "idkpt_tlas_build")
         return ms.value
+
+    def BuildBlas(self, positions, triangles, presplit=True, settings=None):
+        """BLAS.Build + PreSplitting.PreSplit on the device (idkpt_blas_build), with host.build_blas's signature and result:
+        dict(nodes, triangles, required_stack_size, fragment_count, sah), equal to the host build. settings: an
+        IdkPtBlasBuildSettings or host.IdkBlasBuildSettings (its Threads is ignored); DoPreSplit comes from `presplit`.
+        The device time of the build (kernel_ms) is left in `last_blas_build_ms`."""
+        positions = np.ascontiguousarray(positions)
+        triangles = np.ascontiguousarray(triangles)
+        assert positions.dtype == gt.PackedVec3 and triangles.dtype == gt.GpuBlasTriangle
+        s = capi.default_blas_build_settings()
+        if settings is not None:
+            for name, _ in capi.IdkPtBlasBuildSettings._fields_:
+                setattr(s, name, getattr(settings, name))
+        s.DoPreSplit = 1 if presplit else 0
+        h = ctypes.c_void_p()
+        ms = ctypes.c_float()
+        self._check(self._lib.idkpt_blas_build(self._ctx, positions.ctypes.data, len(positions), triangles.ctypes.data, len(triangles),
+                                               ctypes.byref(s), ctypes.byref(h), ctypes.byref(ms)), "idkpt_blas_build")
+        try:
+            nn, nt = ctypes.c_uint64(), ctypes.c_uint64()
+            stack, frags, sah = ctypes.c_int32(), ctypes.c_int32(), ctypes.c_double()
+            self._check(self._lib.idkpt_blas_build_info(h, ctypes.byref(nn), ctypes.byref(nt), ctypes.byref(stack), ctypes.byref(frags),
+                                                        ctypes.byref(sah)), "idkpt_blas_build_info")
+            nodes = np.zeros(nn.value, gt.GpuBlasNode)
+            tris = np.zeros(nt.value, gt.GpuBlasTriangle)
+            self._check(self._lib.idkpt_blas_build_copy(h, nodes.ctypes.data, tris.ctypes.data), "idkpt_blas_build_copy")
+        finally:
+            self._lib.idkpt_blas_build_free(h)
+        self.last_blas_build_ms = float(ms.value)
+        return dict(nodes=nodes, triangles=tris, required_stack_size=int(stack.value), fragment_count=int(frags.value), sah=float(sah.value))
 
     def SetTextures(self, textures):
         """Replace the material texture table (list of dict(pixels, srgb, wrap_s, wrap_t), as host.Scene.textures)."""

@@ -577,6 +577,34 @@ IDKPT_API int idkpt_read_range(IdkPtCtx* ctx, IdkPtArrayId which, uint64_t first
  * scene's TLAS node array (UseTlas scenes) with exactly the nodes the host build produces -- a moving scene reads nothing back. */
 IDKPT_API int idkpt_tlas_build(IdkPtCtx* ctx, int32_t search_radius, float* kernel_ms);
 
+/* BLAS.Build + PreSplitting.PreSplit on the device (the loop body of BVH.BlasesBuild, BVH.cs:315-377): the SweepSAH build of
+ * one BLAS with early split clipping, node for node and triangle for triangle equal to the host build (idkhost_blas_build),
+ * with the same required stack size, fragment count and SAH bits. Host arrays in and out, like the host build: the engine
+ * keeps a CPU copy of every BLAS for BVH.Intersect and hands the arrays to idkpt_set_scene. Needs no scene and leaves the
+ * context's scene, sky and accumulation alone; synchronous, ordered after queued idkpt_compute samples.
+ * IDKPT_ERR_INVALID_ARGUMENT: a NULL pointer, no triangles, a vertex id >= vertex_count, a non-finite setting, or
+ * StopSplittingThreshold < 1. IDKPT_ERR_UNSUPPORTED: more than 2^24 fragments after pre-splitting (the host's float
+ * counters saturate there). kernel_ms (may be NULL): device time of the whole build, copies included. */
+typedef struct IdkPtBlasBuildSettings {      /* BLAS.BuildSettings + PreSplitting.Settings; = IdkBlasBuildSettings without Threads */
+    int32_t StopSplittingThreshold;          /* 1 */
+    int32_t MaxLeafTriangleCount;            /* 2 */
+    float   TriangleCost;                    /* 1.1 */
+    int32_t StackOptThreshold;               /* 16 */
+    float   StackOptSahIncreaseAcceptance;   /* 0.0009745 */
+    float   SplitFactor;                     /* 0.3 */
+    int32_t DoPreSplit;                      /* 1 (= !IsRefittable) */
+} IdkPtBlasBuildSettings;
+typedef struct IdkPtBlasBuild IdkPtBlasBuild;
+IDKPT_API int idkpt_blas_build(IdkPtCtx* ctx, const PackedVec3* positions, uint64_t vertex_count,
+                               const GpuBlasTriangle* triangles, uint64_t triangle_count,
+                               const IdkPtBlasBuildSettings* settings /* NULL = defaults */,
+                               IdkPtBlasBuild** out, float* kernel_ms);
+IDKPT_API int  idkpt_blas_build_info(const IdkPtBlasBuild* b, uint64_t* node_count, uint64_t* triangle_count,
+                                     int32_t* required_stack_size, int32_t* fragment_count, double* sah);
+/* nodes: node_count GpuBlasNode (node 0 the pad, node 1 the root); triangles: triangle_count GpuBlasTriangle */
+IDKPT_API int  idkpt_blas_build_copy(const IdkPtBlasBuild* b, GpuBlasNode* nodes, GpuBlasTriangle* triangles);
+IDKPT_API void idkpt_blas_build_free(IdkPtBlasBuild* b);
+
 /* ---- present chain (SURVEY.md 8f.3): Bloom.Compute(Result) + TonemapAndGamma.Compute(Result, Bloom.Result)
  * (Application.cs:217-223) -> the RGBA8 frame the reference copies to the swapchain, produced on the device. ---- */
 typedef struct IdkPtPostSettings {

@@ -153,6 +153,27 @@ public:
     void PresentAsync(void* pinnedHostRgba32f, uint64_t bytes, IdkPtImage which = IDKPT_IMAGE_RESULT) { check(idkpt_present_async(ctx_, which, pinnedHostRgba32f, bytes), "idkpt_present_async"); }
     void PresentWait() { check(idkpt_present_wait(ctx_), "idkpt_present_wait"); }
     float TlasBuild(int searchRadius = 15) { float ms = 0.0f; check(idkpt_tlas_build(ctx_, searchRadius, &ms), "idkpt_tlas_build"); return ms; }   // BVH.TlasBuild on the device
+    // BLAS.Build + PreSplitting.PreSplit on the device (one BLAS of BVH.BlasesBuild); equal to the host build
+    struct BlasBuildResult {
+        std::vector<GpuBlasNode> nodes;
+        std::vector<GpuBlasTriangle> triangles;
+        int32_t requiredStackSize = 0, fragmentCount = 0;
+        double sah = 0.0;
+        float kernelMs = 0.0f;
+    };
+    BlasBuildResult BuildBlas(const PackedVec3* positions, uint64_t vertexCount, const GpuBlasTriangle* triangles, uint64_t triangleCount,
+                              const IdkPtBlasBuildSettings* settings = nullptr) {
+        BlasBuildResult r;
+        IdkPtBlasBuild* b = nullptr;
+        check(idkpt_blas_build(ctx_, positions, vertexCount, triangles, triangleCount, settings, &b, &r.kernelMs), "idkpt_blas_build");
+        uint64_t nodeCount = 0, triCount = 0;
+        idkpt_blas_build_info(b, &nodeCount, &triCount, &r.requiredStackSize, &r.fragmentCount, &r.sah);
+        r.nodes.resize(nodeCount);
+        r.triangles.resize(triCount);
+        idkpt_blas_build_copy(b, r.nodes.data(), r.triangles.data());
+        idkpt_blas_build_free(b);
+        return r;
+    }
     float Denoise(const IdkPtDenoiseSettings& s) { float ms = 0.0f; check(idkpt_denoise(ctx_, &s, &ms), "idkpt_denoise"); return ms; }   // PathTracerPipeline.Denoise
     std::vector<float> Denoised() const { return read(IDKPT_IMAGE_DENOISED); }
     void RegisterHostBuffer(void* hostPtr, uint64_t bytes) { check(idkpt_register_host_buffer(ctx_, hostPtr, bytes), "idkpt_register_host_buffer"); }
