@@ -57,6 +57,36 @@ struct TextureTable {
     DevBuf pixels, recs, srgbLut;
 };
 
+// An output of a raster pass: its device buffer(s) and the size of the image they hold. A call invalidates the record before
+// it may reallocate or overwrite the buffers and publishes it only when it succeeds, so the *_device_ptr exports and the passes
+// that read the image never see a stale or half-written one.
+struct RasterImage {
+    DevBuf buf[2];
+    int w = 0, h = 0;
+    int last = -1;                 // the buffer the last successful call wrote; -1: none since the scene was set, or a later call failed
+    void invalidate() { last = -1; }
+    void publish(int width, int height, int written = 0) { w = width; h = height; last = written; }
+    bool valid() const { return last >= 0; }
+    bool valid_at(int width, int height) const { return valid() && w == width && h == height; }
+};
+
+// What the raster passes keep between calls; idkpt_set_scene drops all of it (release_raster).
+struct RasterState {
+    DevBuf stage;                  // the host inputs of a call (stage_inputs)
+    DevBuf rtPtrs;                 // deferred lighting: the device pointer table of the ray-traced visibility images
+    DevBuf volMarch, volDepth;     // volumetric lighting: the render-size march (rgba16f) and its depth (r32f)
+    DevBuf vrsOffsets;             // variable-rate deferred lighting: the per-tile coarse-fragment offsets
+    DevBuf gbPrev;                 // the G-buffer pass: the previous vertex positions' upload
+    RasterImage vol;               // rgba16f at the presentation size
+    RasterImage ssao;              // R8Unorm
+    RasterImage deferred;          // rgba32f lit image
+    RasterImage ssr;               // [0] the rgba32f merged image, [1] the rgba16f SSR image
+    RasterImage vrs;               // [0] R8 rates, [1] r32f debug image, one texel per 16x16 tile; w x h is the render size
+    RasterImage gb;                // the six planar fp32 attachments in one allocation (gbuffer_planes)
+    RasterImage taa;               // the two rgba16f presentation-size history images (TAAResolve's ping-pong); w x h: their size
+    int taaFrame = 0;              // TAAResolve.frame: Result = taa.buf[taaFrame % 2], PrevResult the other one
+};
+
 #define IDK_MAX_LANES 16
 
 struct Lane {
@@ -98,7 +128,7 @@ struct IdkPtCtx : IdkCtxBase {
     TextureTable tex;
     std::vector<uint64_t> hostMaterialMaxHandle;   // per material: largest texture handle it uses (validation of later edits)
 
-    // host-array entry points (trace_rays, shadows): device staging buffers, kept between calls
+    // idkpt_trace_rays / idkpt_trace_rays_any: device staging buffers, kept between calls
     DevBuf scratch[3];
 
     // point-shadow cube maps (idkpt_set_point_shadows): host copies of the records and sizes, device records, one D16 allocation
@@ -108,32 +138,7 @@ struct IdkPtCtx : IdkCtxBase {
     DevBuf pointShadowDev, pointShadowMaps;
     DevBuf pointShadowLights;      // int32 LightIndex per shadow (the volumetric pass's Lights[shadow.LightIndex])
 
-    // volumetric lighting (idkpt_volumetric_lighting): render-size rgba16f + r32f, presentation-size rgba16f
-    DevBuf volMarch, volDepth, volOut;
-    int volW = 0, volH = 0;        // presentation size of the last successful call (0: none since the scene was set)
-
-    // G-buffer lighting (idkpt_ssao, idkpt_deferred_lighting): host G-buffer uploads, the ray-traced visibility uploads and
-    // their device pointer table, the R8Unorm SSAO image and the rgba32f lit image
-    DevBuf gbufStage, rtStage, rtPtrs, ssaoOut, deferredOut;
-    int ssaoW = 0, ssaoH = 0;      // size of the last successful call (0: none since the scene was set)
-    int deferredW = 0, deferredH = 0;
-
-    // the end of the raster frame (idkpt_ssr, idkpt_taa_resolve): the rgba16f SSR image and the rgba32f merged image at the
-    // G-buffer size; the TAA history, two rgba16f presentation-size images (TAAResolve's ping-pong) and its frame counter
-    DevBuf ssrOut, ssrMerged, taaHist[2];
-    int ssrW = 0, ssrH = 0;        // size of the last successful idkpt_ssr call (0: none since the scene was set)
-    int taaW = 0, taaH = 0;        // presentation size of the history pair (0: none since the scene was set)
-    int taaFrame = 0;              // TAAResolve.frame: Result = taaHist[taaFrame % 2], PrevResult the other one
-    int taaLast = -1;              // the image the last successful call wrote, -1: none
-
-    // variable-rate deferred lighting (idkpt_shading_rate; idkpt_deferred_lighting with IsVariableRateShading): the R8 rate
-    // image and the r32f debug image, one texel per 16x16 tile, and the per-tile coarse-fragment offsets of the lighting pass
-    DevBuf vrsRates, vrsDebug, vrsOffsets;
-    int vrsW = 0, vrsH = 0;        // render size of the last successful idkpt_shading_rate call (0: none since the scene was set)
-
-    // the G-buffer pass (idkpt_gbuffer): the six planar fp32 attachments in one allocation, the previous positions' upload
-    DevBuf gbImages, gbPrev;
-    int gbW = 0, gbH = 0;          // render size of the last successful idkpt_gbuffer call (0: none since the scene was set)
+    RasterState raster;            // the raster passes (volumetric lighting .. the light spheres and the skybox)
 
     // present chain: bloom mip chains (rgba16f), AgX constants, RGBA8 frame
     DevBuf bloomDown, bloomUp, postConsts, ldr;
@@ -233,6 +238,13 @@ static void release(DevBuf& b) {
     if (b.p) cudaFree(b.p);
     b.p = nullptr;
     b.bytes = 0;
+}
+
+static void release_raster(RasterState& r) {
+    for (DevBuf* b : {&r.stage, &r.rtPtrs, &r.volMarch, &r.volDepth, &r.vrsOffsets, &r.gbPrev}) release(*b);
+    for (RasterImage* img : {&r.vol, &r.ssao, &r.deferred, &r.ssr, &r.vrs, &r.gb, &r.taa})
+        for (DevBuf& b : img->buf) release(b);
+    r = RasterState{};
 }
 
 static int upload(IdkCtxBase* ctx, DevBuf& b, const void* src, size_t bytes) {
@@ -653,11 +665,9 @@ IDKPT_API void idkpt_destroy(IdkPtCtx* ctx) {
                      &ctx->tex.pixels, &ctx->tex.recs, &ctx->tex.srgbLut, &ctx->bloomDown, &ctx->bloomUp, &ctx->postConsts, &ctx->ldr,
                      &ctx->unskinned, &ctx->joints, &ctx->refitParents, &ctx->refitLocks, &ctx->scratch[0], &ctx->scratch[1], &ctx->scratch[2],
                      &ctx->tlasScratch, &ctx->oidn[0], &ctx->oidn[1], &ctx->oidn[2], &ctx->oidn[3], &ctx->denoiseWork[0], &ctx->denoiseWork[1], &ctx->denoised,
-                     &ctx->pointShadowDev, &ctx->pointShadowMaps, &ctx->pointShadowLights, &ctx->volMarch, &ctx->volDepth, &ctx->volOut,
-                     &ctx->gbufStage, &ctx->rtStage, &ctx->rtPtrs, &ctx->ssaoOut, &ctx->deferredOut,
-                     &ctx->ssrOut, &ctx->ssrMerged, &ctx->taaHist[0], &ctx->taaHist[1], &ctx->vrsRates, &ctx->vrsDebug, &ctx->vrsOffsets,
-                     &ctx->gbImages, &ctx->gbPrev};
+                     &ctx->pointShadowDev, &ctx->pointShadowMaps, &ctx->pointShadowLights};
     for (DevBuf* b : all) release(*b);
+    release_raster(ctx->raster);
     for (int i = 0; i < IDK_MAX_LANES; i++) release_lane(ctx->lanes[i], false);
     for (cudaEvent_t ev : ctx->events) cudaEventDestroy(ev);
     gather_teardown(ctx);
@@ -702,17 +712,7 @@ IDKPT_API int idkpt_set_scene(IdkPtCtx* ctx, const IdkPtSceneDesc* s) {
     ctx->haveScene = false;
     ctx->pointShadows.clear(); ctx->pointShadowSizes.clear(); ctx->pointShadowRecs.clear();   // the shadows belong to the old scene
     release(ctx->pointShadowDev); release(ctx->pointShadowMaps); release(ctx->pointShadowLights);
-    release(ctx->volMarch); release(ctx->volDepth); release(ctx->volOut);
-    ctx->volW = ctx->volH = 0;
-    release(ctx->gbufStage); release(ctx->rtStage); release(ctx->rtPtrs); release(ctx->ssaoOut); release(ctx->deferredOut);
-    ctx->ssaoW = ctx->ssaoH = ctx->deferredW = ctx->deferredH = 0;
-    release(ctx->ssrOut); release(ctx->ssrMerged); release(ctx->taaHist[0]); release(ctx->taaHist[1]);
-    ctx->ssrW = ctx->ssrH = ctx->taaW = ctx->taaH = ctx->taaFrame = 0;
-    ctx->taaLast = -1;
-    release(ctx->vrsRates); release(ctx->vrsDebug); release(ctx->vrsOffsets);
-    ctx->vrsW = ctx->vrsH = 0;
-    release(ctx->gbImages); release(ctx->gbPrev);
-    ctx->gbW = ctx->gbH = 0;
+    release_raster(ctx->raster);   // the raster images belong to the old scene too
     int rc;
     // nodes and triangle records share one allocation ("bvh"): [nodes | triRec], so that one L2 access-policy window covers both
     const size_t nodeBytes = ((s->BlasNodeCount * sizeof(GpuBlasNode)) + 255) & ~(size_t)255;
@@ -2027,34 +2027,6 @@ IDKPT_API int idkpt_read_range(IdkPtCtx* ctx, IdkPtArrayId which, uint64_t first
     return IDKPT_OK;
 }
 
-IDKPT_API int idkpt_shadows_ray_traced(IdkPtCtx* ctx, const GpuPerFrameData* frame, const float* depth, const float* normalRG, int32_t width,
-                                       int32_t height, int32_t lightIndex, int32_t samples, uint32_t noiseIndex, const float* taaJitter,
-                                       float* visibilityOut, float* kernelMs) {
-    if (!ctx || !frame || !depth || !normalRG || !visibilityOut) return fail(ctx, IDKPT_ERR_INVALID_ARGUMENT, "idkpt_shadows_ray_traced: null argument");
-    if (!ctx->haveScene) return fail(ctx, IDKPT_ERR_NO_SCENE, "idkpt_shadows_ray_traced: no scene");
-    if (width < 1 || height < 1 || width > 16384 || height > 16384 || samples < 1 || samples > 1024) return fail(ctx, IDKPT_ERR_INVALID_ARGUMENT, "idkpt_shadows_ray_traced: invalid size / sample count");
-    if (lightIndex < 0 || (uint64_t)lightIndex >= ctx->counts.LightCount) return fail(ctx, IDKPT_ERR_INVALID_ARGUMENT, "idkpt_shadows_ray_traced: light index out of range");
-    CK(cudaSetDevice(ctx->device));
-    if (kernelMs) *kernelMs = 0.0f;
-    const size_t n = (size_t)width * height;
-    DevBuf &dDepth = ctx->scratch[0], &dN = ctx->scratch[1], &dVis = ctx->scratch[2];
-    if (ensure(dDepth, n * 4) != cudaSuccess || ensure(dN, n * 8) != cudaSuccess || ensure(dVis, n * 4) != cudaSuccess)
-        return fail(ctx, IDKPT_ERR_OUT_OF_MEMORY, "idkpt_shadows_ray_traced: device allocation failed");
-    CK(cudaMemcpyAsync(dDepth.p, depth, n * 4, cudaMemcpyHostToDevice, ctx->stream));
-    CK(cudaMemcpyAsync(dN.p, normalRG, n * 8, cudaMemcpyHostToDevice, ctx->stream));
-    CK(cudaMemcpyAsync(dVis.p, visibilityOut, n * 4, cudaMemcpyHostToDevice, ctx->stream));   // pixels with depth == 1 keep the caller's value
-    ShadowArgs a;
-    a.sc = ctx->sc;
-    memcpy(a.invProjView, frame->InvProjView, sizeof(a.invProjView));
-    a.jitter[0] = taaJitter ? taaJitter[0] : 0.0f; a.jitter[1] = taaJitter ? taaJitter[1] : 0.0f;
-    a.depth = (const float*)dDepth.p; a.normalRG = (const float2*)dN.p; a.visibility = (float*)dVis.p;
-    a.width = width; a.height = height; a.lightIndex = lightIndex; a.samples = samples; a.noiseIndex = noiseIndex;
-    return run_timed(ctx, "idkpt_shadows_ray_traced", kernelMs, [&]() -> int {
-        k_shadows_ray_traced<<<ctx->traceRaysBlocks, IDK_BLOCK, ctx->stackBytes, ctx->stream>>>(a);
-        return IDKPT_OK;
-    }, visibilityOut, dVis.p, n * 4);
-}
-
 static int trace_rays_impl(IdkPtCtx* ctx, const IdkPtRay* rays, uint64_t count, int32_t traceLights, IdkPtHit* hitsOut, float* kernelMs, bool anyHit) {
     if (!ctx || (!rays && count) || (!hitsOut && count)) return fail(ctx, IDKPT_ERR_INVALID_ARGUMENT, "idkpt_trace_rays: null argument");
     if (!ctx->haveScene) return fail(ctx, IDKPT_ERR_NO_SCENE, "idkpt_trace_rays: no scene");
@@ -2184,151 +2156,250 @@ IDKPT_API int idkpt_read_point_shadow(IdkPtCtx* ctx, int32_t index, uint16_t* ds
     return IDKPT_OK;
 }
 
-// ---- volumetric lighting (VolumetricLighting.Compute: march + depth-aware upscale) ---------------------------------------------
-IDKPT_API int idkpt_volumetric_lighting(IdkPtCtx* ctx, const GpuPerFrameData* frame, const IdkPtVolumetricSettings* s, const float* depth,
-                                        int32_t depthWidth, int32_t depthHeight, int32_t width, int32_t height, const float* taaJitter,
-                                        uint16_t* outRgba16f, float* kernelMs) {
-    if (!ctx || !frame || !s || !depth) return fail(ctx, IDKPT_ERR_INVALID_ARGUMENT, "idkpt_volumetric_lighting: null argument");
-    if (!ctx->haveScene) return fail(ctx, IDKPT_ERR_NO_SCENE, "idkpt_volumetric_lighting: no scene");
-    if (depthWidth < 1 || depthHeight < 1 || depthWidth > 16384 || depthHeight > 16384 || width < 1 || height < 1 || width > 16384 || height > 16384)
-        return fail(ctx, IDKPT_ERR_INVALID_ARGUMENT, "idkpt_volumetric_lighting: size outside 1..16384");
-    if (s->SampleCount < 1 || s->SampleCount > 1024) return fail(ctx, IDKPT_ERR_INVALID_ARGUMENT, "idkpt_volumetric_lighting: SampleCount outside 1..1024");
-    if (!(s->ResolutionScale > 0.0f && s->ResolutionScale <= 1.0f)) return fail(ctx, IDKPT_ERR_INVALID_ARGUMENT, "idkpt_volumetric_lighting: ResolutionScale not in (0, 1]");
-    // VolumetricLighting.SetSize: (Vector2i)((Vector2)PresentationResolution * ResolutionScale), truncated
-    const int w = (int)((float)width * s->ResolutionScale), h = (int)((float)height * s->ResolutionScale);
-    if (w < 1 || h < 1) return fail(ctx, IDKPT_ERR_INVALID_ARGUMENT, "idkpt_volumetric_lighting: render size of 0 (ResolutionScale too small for the size)");
-    for (const GpuPointShadow& ps : ctx->pointShadows)
-        if (ps.LightIndex < 0 || (uint64_t)ps.LightIndex >= ctx->counts.LightCount)
-            return fail(ctx, IDKPT_ERR_INVALID_ARGUMENT, "idkpt_volumetric_lighting: a shadow's LightIndex is not below the scene's light count");
-    CK(cudaSetDevice(ctx->device));
-    if (kernelMs) *kernelMs = 0.0f;
-    const size_t nDepth = (size_t)depthWidth * depthHeight, nRender = (size_t)w * h, nOut = (size_t)width * height;
-    DevBuf& dDepth = ctx->scratch[0];
-    if (ensure(dDepth, nDepth * 4) != cudaSuccess || ensure(ctx->volMarch, nRender * 8) != cudaSuccess ||
-        ensure(ctx->volDepth, nRender * 4) != cudaSuccess || ensure(ctx->volOut, nOut * 8) != cudaSuccess)
-        return fail(ctx, IDKPT_ERR_OUT_OF_MEMORY, "idkpt_volumetric_lighting: device allocation failed");
-    CK(cudaMemcpyAsync(dDepth.p, depth, nDepth * 4, cudaMemcpyHostToDevice, ctx->stream));
-    VolumetricMarchArgs a;
-    a.shadows = (const PointShadowDev*)ctx->pointShadowDev.p; a.lightIndex = (const int32_t*)ctx->pointShadowLights.p;
-    a.lights = ctx->sc.lights; a.maps = (const uint16_t*)ctx->pointShadowMaps.p; a.count = (int)ctx->pointShadowRecs.size();
-    a.gdepth = (const float*)dDepth.p; a.gw = depthWidth; a.gh = depthHeight;
-    a.color = (uint2*)ctx->volMarch.p; a.depth = (float*)ctx->volDepth.p; a.w = w; a.h = h;
-    memcpy(a.invProjView, frame->InvProjView, sizeof(a.invProjView));
-    for (int k = 0; k < 3; k++) { a.viewPos[k] = frame->ViewPos[k]; a.absorbance[k] = s->Absorbance[k]; }
-    a.jitter[0] = taaJitter ? taaJitter[0] : 0.0f; a.jitter[1] = taaJitter ? taaJitter[1] : 0.0f;
-    a.sampleCount = s->SampleCount; a.scattering = s->Scattering; a.strength = s->Strength; a.maxDist = s->MaxDist;
-    VolumetricUpscaleArgs b;
-    b.gdepth = a.gdepth; b.gw = depthWidth; b.gh = depthHeight;
-    b.march = PostImage{nullptr, (const uint2*)ctx->volMarch.p, w, h};
-    b.depth = (const float*)ctx->volDepth.p;
-    b.out = (uint2*)ctx->volOut.p; b.W = width; b.H = height;
-    b.nearPlane = frame->NearPlane; b.farPlane = frame->FarPlane;
+// ---- the raster passes: their shared checks, input stage and output images ----------------------------------------------------
+// Their messages read "<entry point>: <what>" (fail(ctx, who, ...)); a null context goes through the template fail, so that
+// idkpt_last_error(NULL) reports it.
+
+static int size_check(IdkPtCtx* ctx, const char* who, int w, int h) {
+    if (w < 1 || h < 1 || w > 16384 || h > 16384) return fail(ctx, who, IDKPT_ERR_INVALID_ARGUMENT, "size outside 1..16384");
+    return IDKPT_OK;
+}
+
+// The shadowed lighting modes read the point shadow of every light whose PointShadowIndex is not -1.
+static int shadow_index_check(IdkPtCtx* ctx, const char* who) {
+    for (const GpuLight& L : ctx->hostLights)
+        if (L.PointShadowIndex != -1 && (L.PointShadowIndex < 0 || (size_t)L.PointShadowIndex >= ctx->pointShadowRecs.size()))
+            return fail(ctx, who, IDKPT_ERR_INVALID_ARGUMENT, "a light's PointShadowIndex is neither -1 nor below the point-shadow count");
+    return IDKPT_OK;
+}
+
+// The TAA jitter of a call in NDC units: taaJitter[0..1], or none without the array. Returns whether both are finite.
+static bool read_jitter(const float* taaJitter, float jitter[2]) {
+    jitter[0] = taaJitter ? taaJitter[0] : 0.0f;
+    jitter[1] = taaJitter ? taaJitter[1] : 0.0f;
+    return std::isfinite(jitter[0]) && std::isfinite(jitter[1]);
+}
+
+// The grid of a raster kernel over 8x8-pixel tiles, four tiles per block.
+static unsigned tile_blocks(int w, int h) {
     const size_t tiles = (size_t)((w + 7) / 8) * (size_t)((h + 7) / 8);
-    const int rc = run_timed(ctx, "idkpt_volumetric_lighting", kernelMs, [&]() -> int {
-        k_volumetric_march<<<(unsigned)((tiles + 3) / 4), 256, 0, ctx->stream>>>(a);
-        k_volumetric_upscale<<<dim3((unsigned)((width + 31) / 32), (unsigned)((height + 7) / 8)), 256, 0, ctx->stream>>>(b);
-        return IDKPT_OK;
-    }, outRgba16f, ctx->volOut.p, outRgba16f ? nOut * 8 : 0);
-    if (rc == IDKPT_OK) { ctx->volW = width; ctx->volH = height; }
-    return rc;
+    return (unsigned)((tiles + 3) / 4);
 }
 
-IDKPT_API int idkpt_volumetric_device_ptr(IdkPtCtx* ctx, void** devPtr, uint64_t* bytes) {
-    if (!ctx || !devPtr) return fail(ctx, IDKPT_ERR_INVALID_ARGUMENT, "idkpt_volumetric_device_ptr: null argument");
-    if (!ctx->volW) return fail(ctx, IDKPT_ERR_INVALID_ARGUMENT, "idkpt_volumetric_device_ptr: call idkpt_volumetric_lighting first");
-    *devPtr = ctx->volOut.p;
-    if (bytes) *bytes = (uint64_t)ctx->volW * ctx->volH * 8;
-    return IDKPT_OK;
+// One input image of a raster call: the caller's array of `floats` floats per pixel, or (floats 0) an image of the context,
+// read in place. The caller's arrays are read in place when the call's OnDevice is 1: each must then be device memory on the
+// context's device, aligned to the width of the kernels' loads of it (`align` bytes), else the call fails with `misaligned`.
+struct StageInput {
+    const float* src;
+    size_t floats;
+    size_t align;
+    const char* misaligned;
+};
+
+// A G-buffer attachment: loaded as float2 when it has two floats per pixel, as floats otherwise.
+static StageInput attachment(const float* src, size_t floats) {
+    return floats == 2 ? StageInput{src, 2, 8, "OnDevice NormalRG / MetallicRoughness pointer not 8-byte aligned"}
+                       : StageInput{src, floats, 4, "OnDevice pointer not 4-byte aligned"};
 }
 
-// ---- G-buffer lighting (SSAO.Compute, the deferred lighting draw) -------------------------------------------------------------
-// An OnDevice input the kernels read in place: device memory on the context's device, aligned to the width of the kernels'
-// loads of it (`align` bytes: 4 for one float per pixel, 8 for the float2 attachments, 16 for the float4 indirect image).
-// Checked before anything is allocated or launched, so a rejected pointer is never read.
-static int gbuffer_device_check(IdkPtCtx* ctx, const char* who, const float* src, size_t align) {
-    cudaPointerAttributes attr;
-    const cudaError_t e = cudaPointerGetAttributes(&attr, src);
-    if (e != cudaSuccess) cudaGetLastError();   // not a pointer CUDA knows: clear the error, reject below
-    if (e != cudaSuccess || !(attr.type == cudaMemoryTypeDevice || attr.type == cudaMemoryTypeManaged) || attr.device != ctx->device)
-        return fail(ctx, who, IDKPT_ERR_INVALID_ARGUMENT, "OnDevice = 1 with a pointer that is not device memory on the context's device");
-    if ((uintptr_t)src % align != 0)
-        return fail(ctx, who, IDKPT_ERR_INVALID_ARGUMENT, align == 4 ? "OnDevice pointer not 4-byte aligned"
-                                                          : align == 8 ? "OnDevice NormalRG / MetallicRoughness pointer not 8-byte aligned"
-                                                                       : "OnDevice indirect-light pointer not 16-byte aligned");
-    return IDKPT_OK;
-}
+static StageInput velocity_input(const float* src) { return {src, 2, 8, "OnDevice VelocityRG pointer not 8-byte aligned"}; }
 
-// A G-buffer input of `floats` floats per pixel: read in place (OnDevice, already checked by gbuffer_device_check) or uploaded
-// into stage + *offset (256-byte aligned). Returns IDKPT_OK or the failure.
-static int gbuffer_input(IdkPtCtx* ctx, const IdkPtGBuffer* g, const float* src, size_t floats, DevBuf& stage, size_t& offset,
-                         const float*& dst) {
-    const size_t bytes = (size_t)g->Width * g->Height * floats * 4;
-    if (g->OnDevice) {
-        dst = src;
-        return IDKPT_OK;
+// The input stage of a raster call over w x h pixels. Checks every OnDevice array first, so that a rejected pointer is never
+// read and nothing has been allocated or invalidated; then uploads the host arrays into the stage, each at a 256-byte aligned
+// offset. Writes the device pointer of every input to dev[], in order (null for a null src: an input the call does not use).
+static int stage_inputs(IdkPtCtx* ctx, const char* who, int w, int h, int onDevice, const std::vector<StageInput>& in, const float** dev) {
+    const size_t pixels = (size_t)w * h;
+    size_t bytes = 0;
+    for (const StageInput& i : in) {
+        if (!i.src || !i.floats) continue;
+        if (!onDevice) {
+            bytes += (pixels * i.floats * 4 + 255) & ~(size_t)255;
+            continue;
+        }
+        cudaPointerAttributes attr;
+        const cudaError_t e = cudaPointerGetAttributes(&attr, i.src);
+        if (e != cudaSuccess) cudaGetLastError();   // not a pointer CUDA knows: clear the error, reject below
+        if (e != cudaSuccess || !(attr.type == cudaMemoryTypeDevice || attr.type == cudaMemoryTypeManaged) || attr.device != ctx->device)
+            return fail(ctx, who, IDKPT_ERR_INVALID_ARGUMENT, "OnDevice = 1 with a pointer that is not device memory on the context's device");
+        if ((uintptr_t)i.src % i.align != 0) return fail(ctx, who, IDKPT_ERR_INVALID_ARGUMENT, i.misaligned);
     }
-    dst = (const float*)((char*)stage.p + offset);
-    CK(cudaMemcpyAsync((char*)stage.p + offset, src, bytes, cudaMemcpyHostToDevice, ctx->stream));
-    offset += (bytes + 255) & ~(size_t)255;
+    if (bytes && ensure(ctx->raster.stage, bytes) != cudaSuccess) return fail(ctx, who, IDKPT_ERR_OUT_OF_MEMORY, "device allocation failed");
+    char* stage = (char*)ctx->raster.stage.p;
+    for (const StageInput& i : in) {
+        *dev = i.src;
+        if (i.src && i.floats && !onDevice) {
+            CK(cudaMemcpyAsync(stage, i.src, pixels * i.floats * 4, cudaMemcpyHostToDevice, ctx->stream));
+            *dev = (const float*)stage;
+            stage += (pixels * i.floats * 4 + 255) & ~(size_t)255;
+        }
+        dev++;
+    }
     return IDKPT_OK;
 }
 
 static int gbuffer_check(IdkPtCtx* ctx, const char* who, const IdkPtGBuffer* g, bool all) {
     if (!g->Depth || !g->NormalRG || (all && (!g->AlbedoRGB || !g->MetallicRoughness || !g->EmissiveRGB)))
         return fail(ctx, who, IDKPT_ERR_INVALID_ARGUMENT, "null argument");
-    if (g->Width < 1 || g->Height < 1 || g->Width > 16384 || g->Height > 16384) return fail(ctx, who, IDKPT_ERR_INVALID_ARGUMENT, "size outside 1..16384");
+    if (int rc = size_check(ctx, who, g->Width, g->Height)) return rc;
     if (g->OnDevice != 0 && g->OnDevice != 1) return fail(ctx, who, IDKPT_ERR_INVALID_ARGUMENT, "OnDevice is neither 0 nor 1");
     return IDKPT_OK;
 }
 
-// the stage for `floats` floats per pixel of host input, each array 256-byte aligned
-static size_t gbuffer_stage_bytes(const IdkPtGBuffer* g, std::initializer_list<size_t> floats) {
-    size_t n = 0;
-    for (size_t f : floats) n += (((size_t)g->Width * g->Height * f * 4) + 255) & ~(size_t)255;
-    return n;
+// The lit-image selector (IdkPtLitSource), checked before anything is allocated: a caller array, or a context image of w x h.
+static int lit_source_check(IdkPtCtx* ctx, const char* who, int32_t source, bool allowMerged, const float* color, int w, int h) {
+    if (source != IDKPT_LIT_SOURCE_ARRAY && source != IDKPT_LIT_SOURCE_DEFERRED && (!allowMerged || source != IDKPT_LIT_SOURCE_MERGED))
+        return fail(ctx, who, IDKPT_ERR_INVALID_ARGUMENT, allowMerged ? "source is not ARRAY, DEFERRED or MERGED" : "source is neither ARRAY nor DEFERRED");
+    if (source == IDKPT_LIT_SOURCE_ARRAY && !color) return fail(ctx, who, IDKPT_ERR_INVALID_ARGUMENT, "ARRAY source without a colour array");
+    if (source == IDKPT_LIT_SOURCE_DEFERRED && !ctx->raster.deferred.valid_at(w, h))
+        return fail(ctx, who, IDKPT_ERR_INVALID_ARGUMENT, "DEFERRED source needs an idkpt_deferred_lighting image of the render size");
+    if (source == IDKPT_LIT_SOURCE_MERGED && !ctx->raster.ssr.valid_at(w, h))
+        return fail(ctx, who, IDKPT_ERR_INVALID_ARGUMENT, "MERGED source needs an idkpt_ssr image of the render size");
+    return IDKPT_OK;
 }
 
+// The input entry of that lit image: the caller's rgba32f array, or the context's deferred or merged image.
+static StageInput lit_input(IdkPtCtx* ctx, int32_t source, const float* color) {
+    if (source == IDKPT_LIT_SOURCE_DEFERRED) return {(const float*)ctx->raster.deferred.buf[0].p, 0, 0, nullptr};
+    if (source == IDKPT_LIT_SOURCE_MERGED) return {(const float*)ctx->raster.ssr.buf[0].p, 0, 0, nullptr};
+    return {color, 4, 16, "OnDevice colour pointer not 16-byte aligned"};
+}
+
+// The checks of the *_device_ptr exports: a context, somewhere to write, and the image `img` as its pass (`producer`) left it
+// after a successful call. Returns the image, or null with the error (IDKPT_ERR_INVALID_ARGUMENT) set.
+static const RasterImage* published_image(IdkPtCtx* ctx, const char* who, bool haveOut, RasterImage RasterState::*img, const char* producer) {
+    if (!ctx || !haveOut) {
+        fail(ctx, IDKPT_ERR_INVALID_ARGUMENT, (std::string(who) + ": null argument").c_str());
+        return nullptr;
+    }
+    const RasterImage& r = ctx->raster.*img;
+    if (!r.valid()) {
+        fail(ctx, who, IDKPT_ERR_INVALID_ARGUMENT, (std::string("call ") + producer + " first").c_str());
+        return nullptr;
+    }
+    return &r;
+}
+
+// A one-image *_device_ptr export: the image's device pointer and its size in bytes, `texelBytes` per texel, one texel per
+// tile x tile pixels.
+static int image_device_ptr(IdkPtCtx* ctx, const char* who, RasterImage RasterState::*img, const char* producer, uint64_t texelBytes,
+                            int tile, void** devPtr, uint64_t* bytes) {
+    const RasterImage* r = published_image(ctx, who, devPtr != nullptr, img, producer);
+    if (!r) return IDKPT_ERR_INVALID_ARGUMENT;
+    *devPtr = r->buf[r->last].p;
+    if (bytes) *bytes = (uint64_t)((r->w + tile - 1) / tile) * ((r->h + tile - 1) / tile) * texelBytes;
+    return IDKPT_OK;
+}
+
+// ---- volumetric lighting (VolumetricLighting.Compute: march + depth-aware upscale) ---------------------------------------------
+IDKPT_API int idkpt_volumetric_lighting(IdkPtCtx* ctx, const GpuPerFrameData* frame, const IdkPtVolumetricSettings* s, const float* depth,
+                                        int32_t depthWidth, int32_t depthHeight, int32_t width, int32_t height, const float* taaJitter,
+                                        uint16_t* outRgba16f, float* kernelMs) {
+    static const char* who = "idkpt_volumetric_lighting";
+    if (!ctx || !frame || !s || !depth) return fail(ctx, IDKPT_ERR_INVALID_ARGUMENT, "idkpt_volumetric_lighting: null argument");
+    if (!ctx->haveScene) return fail(ctx, who, IDKPT_ERR_NO_SCENE, "no scene");
+    if (int rc = size_check(ctx, who, depthWidth, depthHeight)) return rc;
+    if (int rc = size_check(ctx, who, width, height)) return rc;
+    if (s->SampleCount < 1 || s->SampleCount > 1024) return fail(ctx, who, IDKPT_ERR_INVALID_ARGUMENT, "SampleCount outside 1..1024");
+    if (!(s->ResolutionScale > 0.0f && s->ResolutionScale <= 1.0f)) return fail(ctx, who, IDKPT_ERR_INVALID_ARGUMENT, "ResolutionScale not in (0, 1]");
+    // VolumetricLighting.SetSize: (Vector2i)((Vector2)PresentationResolution * ResolutionScale), truncated
+    const int w = (int)((float)width * s->ResolutionScale), h = (int)((float)height * s->ResolutionScale);
+    if (w < 1 || h < 1) return fail(ctx, who, IDKPT_ERR_INVALID_ARGUMENT, "render size of 0 (ResolutionScale too small for the size)");
+    for (const GpuPointShadow& ps : ctx->pointShadows)
+        if (ps.LightIndex < 0 || (uint64_t)ps.LightIndex >= ctx->counts.LightCount)
+            return fail(ctx, who, IDKPT_ERR_INVALID_ARGUMENT, "a shadow's LightIndex is not below the scene's light count");
+    CK(cudaSetDevice(ctx->device));
+    const float* gdepth;
+    if (int rc = stage_inputs(ctx, who, depthWidth, depthHeight, 0, {attachment(depth, 1)}, &gdepth)) return rc;
+    if (kernelMs) *kernelMs = 0.0f;
+    RasterState& r = ctx->raster;
+    const size_t nRender = (size_t)w * h, nOut = (size_t)width * height;
+    r.vol.invalidate();            // the image may be reallocated and is overwritten: valid again only when the call succeeds
+    if (ensure(r.volMarch, nRender * 8) != cudaSuccess || ensure(r.volDepth, nRender * 4) != cudaSuccess || ensure(r.vol.buf[0], nOut * 8) != cudaSuccess)
+        return fail(ctx, who, IDKPT_ERR_OUT_OF_MEMORY, "device allocation failed");
+    VolumetricMarchArgs a;
+    a.shadows = (const PointShadowDev*)ctx->pointShadowDev.p; a.lightIndex = (const int32_t*)ctx->pointShadowLights.p;
+    a.lights = ctx->sc.lights; a.maps = (const uint16_t*)ctx->pointShadowMaps.p; a.count = (int)ctx->pointShadowRecs.size();
+    a.gdepth = gdepth; a.gw = depthWidth; a.gh = depthHeight;
+    a.color = (uint2*)r.volMarch.p; a.depth = (float*)r.volDepth.p; a.w = w; a.h = h;
+    memcpy(a.invProjView, frame->InvProjView, sizeof(a.invProjView));
+    for (int k = 0; k < 3; k++) { a.viewPos[k] = frame->ViewPos[k]; a.absorbance[k] = s->Absorbance[k]; }
+    read_jitter(taaJitter, a.jitter);
+    a.sampleCount = s->SampleCount; a.scattering = s->Scattering; a.strength = s->Strength; a.maxDist = s->MaxDist;
+    VolumetricUpscaleArgs b;
+    b.gdepth = a.gdepth; b.gw = depthWidth; b.gh = depthHeight;
+    b.march = PostImage{nullptr, (const uint2*)r.volMarch.p, w, h};
+    b.depth = (const float*)r.volDepth.p;
+    b.out = (uint2*)r.vol.buf[0].p; b.W = width; b.H = height;
+    b.nearPlane = frame->NearPlane; b.farPlane = frame->FarPlane;
+    const int rc = run_timed(ctx, who, kernelMs, [&]() -> int {
+        k_volumetric_march<<<tile_blocks(w, h), 256, 0, ctx->stream>>>(a);
+        k_volumetric_upscale<<<dim3((unsigned)((width + 31) / 32), (unsigned)((height + 7) / 8)), 256, 0, ctx->stream>>>(b);
+        return IDKPT_OK;
+    }, outRgba16f, r.vol.buf[0].p, outRgba16f ? nOut * 8 : 0);
+    if (rc == IDKPT_OK) r.vol.publish(width, height);
+    return rc;
+}
+
+IDKPT_API int idkpt_volumetric_device_ptr(IdkPtCtx* ctx, void** devPtr, uint64_t* bytes) {
+    return image_device_ptr(ctx, "idkpt_volumetric_device_ptr", &RasterState::vol, "idkpt_volumetric_lighting", 8, 1, devPtr, bytes);
+}
+
+// ---- G-buffer lighting (SSAO.Compute, the deferred lighting draw) -------------------------------------------------------------
 IDKPT_API int idkpt_ssao(IdkPtCtx* ctx, const GpuPerFrameData* frame, const IdkPtSsaoSettings* s, const IdkPtGBuffer* g, uint8_t* outR8, float* kernelMs) {
     static const char* who = "idkpt_ssao";
     if (!ctx || !frame || !s || !g) return fail(ctx, IDKPT_ERR_INVALID_ARGUMENT, "idkpt_ssao: null argument");
-    if (!ctx->haveScene) return fail(ctx, IDKPT_ERR_NO_SCENE, "idkpt_ssao: no scene");
+    if (!ctx->haveScene) return fail(ctx, who, IDKPT_ERR_NO_SCENE, "no scene");
     if (int rc = gbuffer_check(ctx, who, g, false)) return rc;
-    if (s->SampleCount < 1 || s->SampleCount > 1024) return fail(ctx, IDKPT_ERR_INVALID_ARGUMENT, "idkpt_ssao: SampleCount outside 1..1024");
+    if (s->SampleCount < 1 || s->SampleCount > 1024) return fail(ctx, who, IDKPT_ERR_INVALID_ARGUMENT, "SampleCount outside 1..1024");
     CK(cudaSetDevice(ctx->device));
-    if (g->OnDevice) {
-        if (int rc = gbuffer_device_check(ctx, who, g->Depth, 4)) return rc;
-        if (int rc = gbuffer_device_check(ctx, who, g->NormalRG, 8)) return rc;
-    }
+    const float* in[2];
+    if (int rc = stage_inputs(ctx, who, g->Width, g->Height, g->OnDevice, {attachment(g->Depth, 1), attachment(g->NormalRG, 2)}, in)) return rc;
     if (kernelMs) *kernelMs = 0.0f;
+    RasterImage& out = ctx->raster.ssao;
     const size_t n = (size_t)g->Width * g->Height;
-    ctx->ssaoW = ctx->ssaoH = 0;   // the image may be reallocated and is overwritten: valid again only when the call succeeds
-    if ((!g->OnDevice && ensure(ctx->gbufStage, gbuffer_stage_bytes(g, {1, 2})) != cudaSuccess) || ensure(ctx->ssaoOut, n) != cudaSuccess)
-        return fail(ctx, IDKPT_ERR_OUT_OF_MEMORY, "idkpt_ssao: device allocation failed");
+    out.invalidate();              // the image may be reallocated and is overwritten: valid again only when the call succeeds
+    if (ensure(out.buf[0], n) != cudaSuccess) return fail(ctx, who, IDKPT_ERR_OUT_OF_MEMORY, "device allocation failed");
     SsaoArgs a;
-    size_t off = 0;
-    const float *depth, *nrg;
-    if (int rc = gbuffer_input(ctx, g, g->Depth, 1, ctx->gbufStage, off, depth)) return rc;
-    if (int rc = gbuffer_input(ctx, g, g->NormalRG, 2, ctx->gbufStage, off, nrg)) return rc;
-    a.g = DeferredGBuffer{depth, (const float2*)nrg, nullptr, nullptr, nullptr, g->Width, g->Height};
-    a.out = (uint8_t*)ctx->ssaoOut.p;
+    a.g = DeferredGBuffer{in[0], (const float2*)in[1], nullptr, nullptr, nullptr, g->Width, g->Height};
+    a.out = (uint8_t*)out.buf[0].p;
     memcpy(a.invProjView, frame->InvProjView, sizeof(a.invProjView));
     memcpy(a.projView, frame->ProjView, sizeof(a.projView));
     a.sampleCount = s->SampleCount; a.radius = s->Radius; a.strength = s->Strength; a.noiseIndex = s->NoiseIndex;
-    const size_t tiles = (size_t)((g->Width + 7) / 8) * (size_t)((g->Height + 7) / 8);
     const int rc = run_timed(ctx, who, kernelMs, [&]() -> int {
-        k_ssao<<<(unsigned)((tiles + 3) / 4), 256, 0, ctx->stream>>>(a);
+        k_ssao<<<tile_blocks(g->Width, g->Height), 256, 0, ctx->stream>>>(a);
         return IDKPT_OK;
-    }, outR8, ctx->ssaoOut.p, outR8 ? n : 0);
-    if (rc == IDKPT_OK) { ctx->ssaoW = g->Width; ctx->ssaoH = g->Height; }
+    }, outR8, out.buf[0].p, outR8 ? n : 0);
+    if (rc == IDKPT_OK) out.publish(g->Width, g->Height);
     return rc;
 }
 
 IDKPT_API int idkpt_ssao_device_ptr(IdkPtCtx* ctx, void** devPtr, uint64_t* bytes) {
-    if (!ctx || !devPtr) return fail(ctx, IDKPT_ERR_INVALID_ARGUMENT, "idkpt_ssao_device_ptr: null argument");
-    if (!ctx->ssaoW) return fail(ctx, IDKPT_ERR_INVALID_ARGUMENT, "idkpt_ssao_device_ptr: call idkpt_ssao first");
-    *devPtr = ctx->ssaoOut.p;
-    if (bytes) *bytes = (uint64_t)ctx->ssaoW * ctx->ssaoH;
-    return IDKPT_OK;
+    return image_device_ptr(ctx, "idkpt_ssao_device_ptr", &RasterState::ssao, "idkpt_ssao", 1, 1, devPtr, bytes);
+}
+
+// The RayTraced mode's visibility images (PointShadowManager.ComputeRayTracedShadowMaps for one light), from host arrays.
+IDKPT_API int idkpt_shadows_ray_traced(IdkPtCtx* ctx, const GpuPerFrameData* frame, const float* depth, const float* normalRG, int32_t width,
+                                       int32_t height, int32_t lightIndex, int32_t samples, uint32_t noiseIndex, const float* taaJitter,
+                                       float* visibilityOut, float* kernelMs) {
+    static const char* who = "idkpt_shadows_ray_traced";
+    if (!ctx || !frame || !depth || !normalRG || !visibilityOut) return fail(ctx, IDKPT_ERR_INVALID_ARGUMENT, "idkpt_shadows_ray_traced: null argument");
+    if (!ctx->haveScene) return fail(ctx, who, IDKPT_ERR_NO_SCENE, "no scene");
+    if (width < 1 || height < 1 || width > 16384 || height > 16384 || samples < 1 || samples > 1024) return fail(ctx, who, IDKPT_ERR_INVALID_ARGUMENT, "invalid size / sample count");
+    if (lightIndex < 0 || (uint64_t)lightIndex >= ctx->counts.LightCount) return fail(ctx, who, IDKPT_ERR_INVALID_ARGUMENT, "light index out of range");
+    CK(cudaSetDevice(ctx->device));
+    if (kernelMs) *kernelMs = 0.0f;
+    const float* in[3];            // depth, normal and the visibility: pixels with depth == 1 keep the caller's value
+    if (int rc = stage_inputs(ctx, who, width, height, 0, {attachment(depth, 1), attachment(normalRG, 2), attachment(visibilityOut, 1)}, in)) return rc;
+    ShadowArgs a;
+    a.sc = ctx->sc;
+    memcpy(a.invProjView, frame->InvProjView, sizeof(a.invProjView));
+    read_jitter(taaJitter, a.jitter);
+    a.depth = in[0]; a.normalRG = (const float2*)in[1]; a.visibility = (float*)in[2];
+    a.width = width; a.height = height; a.lightIndex = lightIndex; a.samples = samples; a.noiseIndex = noiseIndex;
+    return run_timed(ctx, who, kernelMs, [&]() -> int {
+        k_shadows_ray_traced<<<ctx->traceRaysBlocks, IDK_BLOCK, ctx->stackBytes, ctx->stream>>>(a);
+        return IDKPT_OK;
+    }, visibilityOut, in[2], (size_t)width * height * 4);
 }
 
 IDKPT_API int idkpt_deferred_lighting(IdkPtCtx* ctx, const GpuPerFrameData* frame, const IdkPtDeferredSettings* s, const IdkPtGBuffer* g,
@@ -2336,191 +2407,123 @@ IDKPT_API int idkpt_deferred_lighting(IdkPtCtx* ctx, const GpuPerFrameData* fram
                                       float* outRgba32f, float* kernelMs) {
     static const char* who = "idkpt_deferred_lighting";
     if (!ctx || !frame || !s || !g) return fail(ctx, IDKPT_ERR_INVALID_ARGUMENT, "idkpt_deferred_lighting: null argument");
-    if (!ctx->haveScene) return fail(ctx, IDKPT_ERR_NO_SCENE, "idkpt_deferred_lighting: no scene");
+    if (!ctx->haveScene) return fail(ctx, who, IDKPT_ERR_NO_SCENE, "no scene");
     if (int rc = gbuffer_check(ctx, who, g, true)) return rc;
-    if (s->ShadowMode < 0 || s->ShadowMode > 2) return fail(ctx, IDKPT_ERR_INVALID_ARGUMENT, "idkpt_deferred_lighting: ShadowMode outside 0..2");
+    if (s->ShadowMode < 0 || s->ShadowMode > 2) return fail(ctx, who, IDKPT_ERR_INVALID_ARGUMENT, "ShadowMode outside 0..2");
     if (s->IsVariableRateShading != 0 && s->IsVariableRateShading != 1)
-        return fail(ctx, IDKPT_ERR_INVALID_ARGUMENT, "idkpt_deferred_lighting: IsVariableRateShading is neither 0 nor 1");
-    if (s->IsVariableRateShading && (ctx->vrsW != g->Width || ctx->vrsH != g->Height))
-        return fail(ctx, IDKPT_ERR_INVALID_ARGUMENT, "idkpt_deferred_lighting: IsVariableRateShading needs an idkpt_shading_rate image of the G-buffer's size");
-    if (s->IsVXGI && !indirect) return fail(ctx, IDKPT_ERR_INVALID_ARGUMENT, "idkpt_deferred_lighting: IsVXGI without an indirect-light image");
-    if (s->IsSSAO && (ctx->ssaoW != g->Width || ctx->ssaoH != g->Height))
-        return fail(ctx, IDKPT_ERR_INVALID_ARGUMENT, "idkpt_deferred_lighting: IsSSAO needs an idkpt_ssao image of the G-buffer's size");
+        return fail(ctx, who, IDKPT_ERR_INVALID_ARGUMENT, "IsVariableRateShading is neither 0 nor 1");
+    RasterState& r = ctx->raster;
+    if (s->IsVariableRateShading && !r.vrs.valid_at(g->Width, g->Height))
+        return fail(ctx, who, IDKPT_ERR_INVALID_ARGUMENT, "IsVariableRateShading needs an idkpt_shading_rate image of the G-buffer's size");
+    if (s->IsVXGI && !indirect) return fail(ctx, who, IDKPT_ERR_INVALID_ARGUMENT, "IsVXGI without an indirect-light image");
+    if (s->IsSSAO && !r.ssao.valid_at(g->Width, g->Height))
+        return fail(ctx, who, IDKPT_ERR_INVALID_ARGUMENT, "IsSSAO needs an idkpt_ssao image of the G-buffer's size");
+    if (s->ShadowMode != 0)
+        if (int rc = shadow_index_check(ctx, who)) return rc;
     const uint32_t shadowCount = (uint32_t)ctx->pointShadowRecs.size();
-    if (s->ShadowMode != 0) {
-        for (const GpuLight& L : ctx->hostLights)
-            if (L.PointShadowIndex != -1 && (L.PointShadowIndex < 0 || (uint32_t)L.PointShadowIndex >= shadowCount))
-                return fail(ctx, IDKPT_ERR_INVALID_ARGUMENT, "idkpt_deferred_lighting: a light's PointShadowIndex is neither -1 nor below the point-shadow count");
-    }
     if (s->ShadowMode == 2) {
         if (rtCount < shadowCount || (rtCount && !rtVisibility))
-            return fail(ctx, IDKPT_ERR_INVALID_ARGUMENT, "idkpt_deferred_lighting: RayTraced needs a visibility image per point shadow");
+            return fail(ctx, who, IDKPT_ERR_INVALID_ARGUMENT, "RayTraced needs a visibility image per point shadow");
         for (uint32_t i = 0; i < rtCount; i++)
-            if (!rtVisibility[i]) return fail(ctx, IDKPT_ERR_INVALID_ARGUMENT, "idkpt_deferred_lighting: a visibility image is null");
+            if (!rtVisibility[i]) return fail(ctx, who, IDKPT_ERR_INVALID_ARGUMENT, "a visibility image is null");
     }
     CK(cudaSetDevice(ctx->device));
     const uint32_t rtUsed = s->ShadowMode == 2 ? shadowCount : 0;
-    if (g->OnDevice) {
-        const float* ptrs[5] = {g->Depth, g->NormalRG, g->AlbedoRGB, g->MetallicRoughness, g->EmissiveRGB};
-        const size_t align[5] = {4, 8, 4, 8, 4};
-        for (int i = 0; i < 5; i++)
-            if (int rc = gbuffer_device_check(ctx, who, ptrs[i], align[i])) return rc;
-        if (s->IsVXGI)
-            if (int rc = gbuffer_device_check(ctx, who, indirect, 16)) return rc;
-        for (uint32_t i = 0; i < rtUsed; i++)
-            if (int rc = gbuffer_device_check(ctx, who, rtVisibility[i], 4)) return rc;
-    }
+    std::vector<StageInput> inputs = {attachment(g->Depth, 1), attachment(g->NormalRG, 2), attachment(g->AlbedoRGB, 3),
+                                      attachment(g->MetallicRoughness, 2), attachment(g->EmissiveRGB, 3),
+                                      {s->IsVXGI ? indirect : nullptr, 4, 16, "OnDevice indirect-light pointer not 16-byte aligned"}};
+    for (uint32_t i = 0; i < rtUsed; i++) inputs.push_back(attachment(rtVisibility[i], 1));
+    std::vector<const float*> in(inputs.size());   // the G-buffer, the indirect light, the visibility images
+    if (int rc = stage_inputs(ctx, who, g->Width, g->Height, g->OnDevice, inputs, in.data())) return rc;
     if (kernelMs) *kernelMs = 0.0f;
     const size_t n = (size_t)g->Width * g->Height;
-    ctx->deferredW = ctx->deferredH = 0;   // the image may be reallocated and is overwritten: valid again only when the call succeeds
-    const size_t stageBytes = g->OnDevice ? 0 : gbuffer_stage_bytes(g, {1, 2, 3, 2, 3, s->IsVXGI ? 4u : 0u});
     const int tilesX = (g->Width + IDK_VRS_TILE - 1) / IDK_VRS_TILE, vrsTiles = tilesX * ((g->Height + IDK_VRS_TILE - 1) / IDK_VRS_TILE);
-    if ((stageBytes && ensure(ctx->gbufStage, stageBytes) != cudaSuccess) || (rtUsed && !g->OnDevice && ensure(ctx->rtStage, rtUsed * ((n * 4 + 255) & ~(size_t)255)) != cudaSuccess) ||
-        ensure(ctx->deferredOut, n * 16) != cudaSuccess || (s->IsVariableRateShading && ensure(ctx->vrsOffsets, ((size_t)vrsTiles + 1) * 4) != cudaSuccess))
-        return fail(ctx, IDKPT_ERR_OUT_OF_MEMORY, "idkpt_deferred_lighting: device allocation failed");
-    size_t off = 0;
-    const float *depth, *nrg, *albedo, *mr, *emissive, *gi = nullptr;
-    if (int rc = gbuffer_input(ctx, g, g->Depth, 1, ctx->gbufStage, off, depth)) return rc;
-    if (int rc = gbuffer_input(ctx, g, g->NormalRG, 2, ctx->gbufStage, off, nrg)) return rc;
-    if (int rc = gbuffer_input(ctx, g, g->AlbedoRGB, 3, ctx->gbufStage, off, albedo)) return rc;
-    if (int rc = gbuffer_input(ctx, g, g->MetallicRoughness, 2, ctx->gbufStage, off, mr)) return rc;
-    if (int rc = gbuffer_input(ctx, g, g->EmissiveRGB, 3, ctx->gbufStage, off, emissive)) return rc;
-    if (s->IsVXGI)
-        if (int rc = gbuffer_input(ctx, g, indirect, 4, ctx->gbufStage, off, gi)) return rc;
-    std::vector<const float*> rt(rtUsed);
-    size_t rtOff = 0;
-    for (uint32_t i = 0; i < rtUsed; i++)
-        if (int rc = gbuffer_input(ctx, g, rtVisibility[i], 1, ctx->rtStage, rtOff, rt[i])) return rc;
+    r.deferred.invalidate();       // the image may be reallocated and is overwritten: valid again only when the call succeeds
+    if (ensure(r.deferred.buf[0], n * 16) != cudaSuccess || (s->IsVariableRateShading && ensure(r.vrsOffsets, ((size_t)vrsTiles + 1) * 4) != cudaSuccess))
+        return fail(ctx, who, IDKPT_ERR_OUT_OF_MEMORY, "device allocation failed");
     if (rtUsed)
-        if (int rc = upload(ctx, ctx->rtPtrs, rt.data(), rt.size() * sizeof(const float*))) return rc;
+        if (int rc = upload(ctx, r.rtPtrs, in.data() + 6, rtUsed * sizeof(const float*))) return rc;
     DeferredArgs a;
-    a.g = DeferredGBuffer{depth, (const float2*)nrg, albedo, (const float2*)mr, emissive, g->Width, g->Height};
-    a.ssao = s->IsSSAO ? (const uint8_t*)ctx->ssaoOut.p : nullptr;
-    a.indirect = (const float4*)gi;
-    a.rtVisibility = rtUsed ? (const float* const*)ctx->rtPtrs.p : nullptr;
+    a.g = DeferredGBuffer{in[0], (const float2*)in[1], in[2], (const float2*)in[3], in[4], g->Width, g->Height};
+    a.ssao = s->IsSSAO ? (const uint8_t*)r.ssao.buf[0].p : nullptr;
+    a.indirect = (const float4*)in[5];
+    a.rtVisibility = rtUsed ? (const float* const*)r.rtPtrs.p : nullptr;
     a.lights = ctx->sc.lights; a.lightCount = (int)ctx->counts.LightCount;
     a.shadows = PointShadowMapsDev{(const PointShadowDev*)ctx->pointShadowDev.p, (const uint16_t*)ctx->pointShadowMaps.p, shadowCount};
-    a.out = (float4*)ctx->deferredOut.p;
+    a.out = (float4*)r.deferred.buf[0].p;
     memcpy(a.invProjView, frame->InvProjView, sizeof(a.invProjView));
     for (int k = 0; k < 3; k++) a.viewPos[k] = frame->ViewPos[k];
-    a.jitter[0] = taaJitter ? taaJitter[0] : 0.0f; a.jitter[1] = taaJitter ? taaJitter[1] : 0.0f;
+    read_jitter(taaJitter, a.jitter);
     a.shadowMode = s->ShadowMode;
-    const size_t tiles = (size_t)((g->Width + 7) / 8) * (size_t)((g->Height + 7) / 8);
-    const VrsTiles v{(const uint8_t*)ctx->vrsRates.p, (uint32_t*)ctx->vrsOffsets.p, g->Width, g->Height, tilesX, vrsTiles};
+    const VrsTiles v{(const uint8_t*)r.vrs.buf[0].p, (uint32_t*)r.vrsOffsets.p, g->Width, g->Height, tilesX, vrsTiles};
     const int rc = run_timed(ctx, who, kernelMs, [&]() -> int {
         if (s->IsVariableRateShading) {   // the fragment list, then one thread per coarse fragment (grid sized for all 1x1)
             k_vrs_scan<<<1, 1024, 0, ctx->stream>>>(v);
             k_deferred_lighting_vrs<<<(unsigned)((n + 255) / 256), 256, 0, ctx->stream>>>(a, v);
         } else {
-            k_deferred_lighting<<<(unsigned)((tiles + 3) / 4), 256, 0, ctx->stream>>>(a);
+            k_deferred_lighting<<<tile_blocks(g->Width, g->Height), 256, 0, ctx->stream>>>(a);
         }
         return IDKPT_OK;
-    }, outRgba32f, ctx->deferredOut.p, outRgba32f ? n * 16 : 0);
-    if (rc == IDKPT_OK) { ctx->deferredW = g->Width; ctx->deferredH = g->Height; }
+    }, outRgba32f, r.deferred.buf[0].p, outRgba32f ? n * 16 : 0);
+    if (rc == IDKPT_OK) r.deferred.publish(g->Width, g->Height);
     return rc;
 }
 
 IDKPT_API int idkpt_deferred_device_ptr(IdkPtCtx* ctx, void** devPtr, uint64_t* bytes) {
-    if (!ctx || !devPtr) return fail(ctx, IDKPT_ERR_INVALID_ARGUMENT, "idkpt_deferred_device_ptr: null argument");
-    if (!ctx->deferredW) return fail(ctx, IDKPT_ERR_INVALID_ARGUMENT, "idkpt_deferred_device_ptr: call idkpt_deferred_lighting first");
-    *devPtr = ctx->deferredOut.p;
-    if (bytes) *bytes = (uint64_t)ctx->deferredW * ctx->deferredH * 16;
-    return IDKPT_OK;
+    return image_device_ptr(ctx, "idkpt_deferred_device_ptr", &RasterState::deferred, "idkpt_deferred_lighting", 16, 1, devPtr, bytes);
 }
 
 // ---- the end of the raster frame (SSR.Compute, "Merge Textures", TaaResolve.Compute) --------------------------------------------
-// An OnDevice array that is not a G-buffer attachment: device memory on the context's device (gbuffer_device_check), aligned
-// to `align` bytes, else `what`.
-static int device_array_check(IdkPtCtx* ctx, const char* who, const float* src, size_t align, const char* what) {
-    if (int rc = gbuffer_device_check(ctx, who, src, 1)) return rc;
-    if ((uintptr_t)src % align != 0) return fail(ctx, who, IDKPT_ERR_INVALID_ARGUMENT, what);
-    return IDKPT_OK;
-}
-
-// The lit-image selector of both calls, checked before anything is allocated: a caller array, or a context image of w x h.
-static int lit_source_check(IdkPtCtx* ctx, const char* who, int32_t source, bool allowMerged, const float* color, int w, int h, int onDevice) {
-    if (source != IDKPT_LIT_SOURCE_ARRAY && source != IDKPT_LIT_SOURCE_DEFERRED && (!allowMerged || source != IDKPT_LIT_SOURCE_MERGED))
-        return fail(ctx, who, IDKPT_ERR_INVALID_ARGUMENT, allowMerged ? "source is not ARRAY, DEFERRED or MERGED" : "source is neither ARRAY nor DEFERRED");
-    if (source == IDKPT_LIT_SOURCE_ARRAY && !color) return fail(ctx, who, IDKPT_ERR_INVALID_ARGUMENT, "ARRAY source without a colour array");
-    if (source == IDKPT_LIT_SOURCE_DEFERRED && (ctx->deferredW != w || ctx->deferredH != h))
-        return fail(ctx, who, IDKPT_ERR_INVALID_ARGUMENT, "DEFERRED source needs an idkpt_deferred_lighting image of the render size");
-    if (source == IDKPT_LIT_SOURCE_MERGED && (ctx->ssrW != w || ctx->ssrH != h))
-        return fail(ctx, who, IDKPT_ERR_INVALID_ARGUMENT, "MERGED source needs an idkpt_ssr image of the render size");
-    if (source == IDKPT_LIT_SOURCE_ARRAY && onDevice)
-        return device_array_check(ctx, who, color, 16, "OnDevice colour pointer not 16-byte aligned");
-    return IDKPT_OK;
-}
-
-// The lit image a call reads: the caller array (read in place or uploaded into the stage) or the context image.
-static int lit_source_input(IdkPtCtx* ctx, const IdkPtGBuffer* g, int32_t source, const float* color, size_t& offset, const float*& dst) {
-    if (source == IDKPT_LIT_SOURCE_DEFERRED) dst = (const float*)ctx->deferredOut.p;
-    else if (source == IDKPT_LIT_SOURCE_MERGED) dst = (const float*)ctx->ssrMerged.p;
-    else return gbuffer_input(ctx, g, color, 4, ctx->gbufStage, offset, dst);
-    return IDKPT_OK;
-}
-
 IDKPT_API int idkpt_ssr(IdkPtCtx* ctx, const GpuPerFrameData* frame, const IdkPtSsrSettings* s, const IdkPtGBuffer* g, int32_t source,
                         const float* color, float* mergedOut, uint16_t* ssrOut, float* kernelMs) {
     static const char* who = "idkpt_ssr";
     if (!ctx || !frame || !s || !g) return fail(ctx, IDKPT_ERR_INVALID_ARGUMENT, "idkpt_ssr: null argument");
-    if (!ctx->haveScene) return fail(ctx, IDKPT_ERR_NO_SCENE, "idkpt_ssr: no scene");
+    if (!ctx->haveScene) return fail(ctx, who, IDKPT_ERR_NO_SCENE, "no scene");
     if (int rc = gbuffer_check(ctx, who, g, false)) return rc;
     if (!g->AlbedoRGB || !g->MetallicRoughness) return fail(ctx, who, IDKPT_ERR_INVALID_ARGUMENT, "null argument");
     if (s->SampleCount < 1 || s->SampleCount > 1024) return fail(ctx, who, IDKPT_ERR_INVALID_ARGUMENT, "SampleCount outside 1..1024");
     if (s->BinarySearchCount < 0 || s->BinarySearchCount > 64) return fail(ctx, who, IDKPT_ERR_INVALID_ARGUMENT, "BinarySearchCount outside 0..64");
     if (!std::isfinite(s->MaxDist)) return fail(ctx, who, IDKPT_ERR_INVALID_ARGUMENT, "MaxDist not finite");
     CK(cudaSetDevice(ctx->device));
-    if (int rc = lit_source_check(ctx, who, source, false, color, g->Width, g->Height, g->OnDevice)) return rc;
-    if (g->OnDevice) {
-        const float* ptrs[4] = {g->Depth, g->NormalRG, g->AlbedoRGB, g->MetallicRoughness};
-        const size_t align[4] = {4, 8, 4, 8};
-        for (int i = 0; i < 4; i++)
-            if (int rc = gbuffer_device_check(ctx, who, ptrs[i], align[i])) return rc;
-    }
+    if (int rc = lit_source_check(ctx, who, source, false, color, g->Width, g->Height)) return rc;
+    const float* in[5];            // the lit image, the G-buffer
+    if (int rc = stage_inputs(ctx, who, g->Width, g->Height, g->OnDevice, {lit_input(ctx, source, color), attachment(g->Depth, 1),
+                              attachment(g->NormalRG, 2), attachment(g->AlbedoRGB, 3), attachment(g->MetallicRoughness, 2)}, in)) return rc;
     if (kernelMs) *kernelMs = 0.0f;
+    RasterImage& out = ctx->raster.ssr;
     const size_t n = (size_t)g->Width * g->Height;
-    ctx->ssrW = ctx->ssrH = 0;     // the images may be reallocated and are overwritten: valid again only when the call succeeds
-    const size_t stageBytes = g->OnDevice ? 0 : gbuffer_stage_bytes(g, {1, 2, 3, 2, source == IDKPT_LIT_SOURCE_ARRAY ? 4u : 0u});
-    if ((stageBytes && ensure(ctx->gbufStage, stageBytes) != cudaSuccess) || ensure(ctx->ssrOut, n * 8) != cudaSuccess ||
-        ensure(ctx->ssrMerged, n * 16) != cudaSuccess)
-        return fail(ctx, IDKPT_ERR_OUT_OF_MEMORY, "idkpt_ssr: device allocation failed");
-    size_t off = 0;
-    const float *depth, *nrg, *albedo, *mr, *src;
-    if (int rc = gbuffer_input(ctx, g, g->Depth, 1, ctx->gbufStage, off, depth)) return rc;
-    if (int rc = gbuffer_input(ctx, g, g->NormalRG, 2, ctx->gbufStage, off, nrg)) return rc;
-    if (int rc = gbuffer_input(ctx, g, g->AlbedoRGB, 3, ctx->gbufStage, off, albedo)) return rc;
-    if (int rc = gbuffer_input(ctx, g, g->MetallicRoughness, 2, ctx->gbufStage, off, mr)) return rc;
-    if (int rc = lit_source_input(ctx, g, source, color, off, src)) return rc;
+    out.invalidate();              // the images may be reallocated and are overwritten: valid again only when the call succeeds
+    if (ensure(out.buf[0], n * 16) != cudaSuccess || ensure(out.buf[1], n * 8) != cudaSuccess)
+        return fail(ctx, who, IDKPT_ERR_OUT_OF_MEMORY, "device allocation failed");
     SsrArgs a;
-    a.g = DeferredGBuffer{depth, (const float2*)nrg, albedo, (const float2*)mr, nullptr, g->Width, g->Height};
-    a.src = (const float4*)src;
-    a.ssr = (uint2*)ctx->ssrOut.p;
-    a.merged = (float4*)ctx->ssrMerged.p;
+    a.g = DeferredGBuffer{in[1], (const float2*)in[2], in[3], (const float2*)in[4], nullptr, g->Width, g->Height};
+    a.src = (const float4*)in[0];
+    a.ssr = (uint2*)out.buf[1].p;
+    a.merged = (float4*)out.buf[0].p;
     a.sc = ctx->sc;
     memcpy(a.projection, frame->Projection, sizeof(a.projection));
     memcpy(a.invProjection, frame->InvProjection, sizeof(a.invProjection));
     memcpy(a.invView, frame->InvView, sizeof(a.invView));
     a.sampleCount = s->SampleCount; a.binarySearchCount = s->BinarySearchCount; a.maxDist = s->MaxDist;
-    const size_t tiles = (size_t)((g->Width + 7) / 8) * (size_t)((g->Height + 7) / 8);
     const int rc = run_timed(ctx, who, kernelMs, [&]() -> int {
-        k_ssr<<<(unsigned)((tiles + 3) / 4), 256, 0, ctx->stream>>>(a);
+        k_ssr<<<tile_blocks(g->Width, g->Height), 256, 0, ctx->stream>>>(a);
         return IDKPT_OK;
-    }, mergedOut, ctx->ssrMerged.p, mergedOut ? n * 16 : 0);
+    }, mergedOut, out.buf[0].p, mergedOut ? n * 16 : 0);
     if (rc != IDKPT_OK) return rc;
     if (ssrOut) {
-        CK(cudaMemcpyAsync(ssrOut, ctx->ssrOut.p, n * 8, cudaMemcpyDeviceToHost, ctx->stream));
+        CK(cudaMemcpyAsync(ssrOut, out.buf[1].p, n * 8, cudaMemcpyDeviceToHost, ctx->stream));
         CK(cudaStreamSynchronize(ctx->stream));
     }
-    ctx->ssrW = g->Width; ctx->ssrH = g->Height;
+    out.publish(g->Width, g->Height);
     return IDKPT_OK;
 }
 
 IDKPT_API int idkpt_ssr_device_ptrs(IdkPtCtx* ctx, void** mergedDevPtr, void** ssrDevPtr, uint64_t* mergedBytes, uint64_t* ssrBytes) {
-    if (!ctx || (!mergedDevPtr && !ssrDevPtr)) return fail(ctx, IDKPT_ERR_INVALID_ARGUMENT, "idkpt_ssr_device_ptrs: null argument");
-    if (!ctx->ssrW) return fail(ctx, IDKPT_ERR_INVALID_ARGUMENT, "idkpt_ssr_device_ptrs: call idkpt_ssr first");
-    const uint64_t n = (uint64_t)ctx->ssrW * ctx->ssrH;
-    if (mergedDevPtr) *mergedDevPtr = ctx->ssrMerged.p;
-    if (ssrDevPtr) *ssrDevPtr = ctx->ssrOut.p;
+    const RasterImage* r = published_image(ctx, "idkpt_ssr_device_ptrs", mergedDevPtr || ssrDevPtr, &RasterState::ssr, "idkpt_ssr");
+    if (!r) return IDKPT_ERR_INVALID_ARGUMENT;
+    const uint64_t n = (uint64_t)r->w * r->h;
+    if (mergedDevPtr) *mergedDevPtr = r->buf[0].p;
+    if (ssrDevPtr) *ssrDevPtr = r->buf[1].p;
     if (mergedBytes) *mergedBytes = n * 16;
     if (ssrBytes) *ssrBytes = n * 8;
     return IDKPT_OK;
@@ -2530,63 +2533,49 @@ IDKPT_API int idkpt_taa_resolve(IdkPtCtx* ctx, const IdkPtTaaSettings* s, const 
                                 float* kernelMs) {
     static const char* who = "idkpt_taa_resolve";
     if (!ctx || !s || !in || !in->Depth || !in->VelocityRG) return fail(ctx, IDKPT_ERR_INVALID_ARGUMENT, "idkpt_taa_resolve: null argument");
-    if (in->Width < 1 || in->Height < 1 || in->Width > 16384 || in->Height > 16384 || width < 1 || height < 1 || width > 16384 || height > 16384)
-        return fail(ctx, who, IDKPT_ERR_INVALID_ARGUMENT, "size outside 1..16384");
+    if (int rc = size_check(ctx, who, in->Width, in->Height)) return rc;
+    if (int rc = size_check(ctx, who, width, height)) return rc;
     if (in->OnDevice != 0 && in->OnDevice != 1) return fail(ctx, who, IDKPT_ERR_INVALID_ARGUMENT, "OnDevice is neither 0 nor 1");
     if (s->IsNaiveTaa != 0 && s->IsNaiveTaa != 1) return fail(ctx, who, IDKPT_ERR_INVALID_ARGUMENT, "IsNaiveTaa is neither 0 nor 1");
     if (s->SampleCount < 1 || s->SampleCount > 1024) return fail(ctx, who, IDKPT_ERR_INVALID_ARGUMENT, "SampleCount outside 1..1024");
     if (!std::isfinite(s->PreferAliasingOverBlur)) return fail(ctx, who, IDKPT_ERR_INVALID_ARGUMENT, "PreferAliasingOverBlur not finite");
     CK(cudaSetDevice(ctx->device));
-    if (int rc = lit_source_check(ctx, who, in->Source, true, in->ColorRgba32f, in->Width, in->Height, in->OnDevice)) return rc;
-    if (in->OnDevice) {
-        if (int rc = gbuffer_device_check(ctx, who, in->Depth, 4)) return rc;
-        if (int rc = device_array_check(ctx, who, in->VelocityRG, 8, "OnDevice VelocityRG pointer not 8-byte aligned")) return rc;
-    }
+    if (int rc = lit_source_check(ctx, who, in->Source, true, in->ColorRgba32f, in->Width, in->Height)) return rc;
+    const float* src[3];           // the lit image, depth, velocity
+    if (int rc = stage_inputs(ctx, who, in->Width, in->Height, in->OnDevice, {lit_input(ctx, in->Source, in->ColorRgba32f),
+                              attachment(in->Depth, 1), velocity_input(in->VelocityRG)}, src)) return rc;
     if (kernelMs) *kernelMs = 0.0f;
-    ctx->taaLast = -1;             // valid again only when the call succeeds
+    RasterState& r = ctx->raster;
+    r.taa.invalidate();            // valid again only when the call succeeds
     const size_t bytes = (size_t)width * height * 8;
-    if (width != ctx->taaW || height != ctx->taaH) {   // a new presentation size restarts from a zero history
-        ctx->taaW = ctx->taaH = 0;
-        if (ensure(ctx->taaHist[0], bytes) != cudaSuccess || ensure(ctx->taaHist[1], bytes) != cudaSuccess)
-            return fail(ctx, IDKPT_ERR_OUT_OF_MEMORY, "idkpt_taa_resolve: device allocation failed");
-        CK(cudaMemsetAsync(ctx->taaHist[0].p, 0, bytes, ctx->stream));
-        CK(cudaMemsetAsync(ctx->taaHist[1].p, 0, bytes, ctx->stream));
-        ctx->taaW = width; ctx->taaH = height;
+    if (width != r.taa.w || height != r.taa.h) {   // a new presentation size restarts from a zero history
+        r.taa.w = r.taa.h = 0;
+        if (ensure(r.taa.buf[0], bytes) != cudaSuccess || ensure(r.taa.buf[1], bytes) != cudaSuccess)
+            return fail(ctx, who, IDKPT_ERR_OUT_OF_MEMORY, "device allocation failed");
+        CK(cudaMemsetAsync(r.taa.buf[0].p, 0, bytes, ctx->stream));
+        CK(cudaMemsetAsync(r.taa.buf[1].p, 0, bytes, ctx->stream));
+        r.taa.w = width; r.taa.h = height;
     }
-    const IdkPtGBuffer g = {in->Width, in->Height, in->OnDevice, nullptr, nullptr, nullptr, nullptr, nullptr};
-    const size_t stageBytes = in->OnDevice ? 0 : gbuffer_stage_bytes(&g, {1, 2, in->Source == IDKPT_LIT_SOURCE_ARRAY ? 4u : 0u});
-    if (stageBytes && ensure(ctx->gbufStage, stageBytes) != cudaSuccess)
-        return fail(ctx, IDKPT_ERR_OUT_OF_MEMORY, "idkpt_taa_resolve: device allocation failed");
-    size_t off = 0;
-    const float *depth, *velocity, *color;
-    if (int rc = gbuffer_input(ctx, &g, in->Depth, 1, ctx->gbufStage, off, depth)) return rc;
-    if (int rc = gbuffer_input(ctx, &g, in->VelocityRG, 2, ctx->gbufStage, off, velocity)) return rc;
-    if (int rc = lit_source_input(ctx, &g, in->Source, in->ColorRgba32f, off, color)) return rc;
-    ctx->taaFrame++;
-    const int dst = ctx->taaFrame % 2 == 0 ? 0 : 1;
+    r.taaFrame++;
+    const int dst = r.taaFrame % 2 == 0 ? 0 : 1;
     TaaArgs a;
-    a.color = PostImage{(const float4*)color, nullptr, in->Width, in->Height};
-    a.depth = depth;
-    a.velocity = (const float2*)velocity;
-    a.history = PostImage{nullptr, (const uint2*)ctx->taaHist[1 - dst].p, width, height};
-    a.out = (uint2*)ctx->taaHist[dst].p;
+    a.color = PostImage{(const float4*)src[0], nullptr, in->Width, in->Height};
+    a.depth = src[1];
+    a.velocity = (const float2*)src[2];
+    a.history = PostImage{nullptr, (const uint2*)r.taa.buf[1 - dst].p, width, height};
+    a.out = (uint2*)r.taa.buf[dst].p;
     a.W = width; a.H = height;
     a.isNaive = s->IsNaiveTaa; a.sampleCount = s->SampleCount; a.preferAliasingOverBlur = s->PreferAliasingOverBlur;
-    const size_t tiles = (size_t)((width + 7) / 8) * (size_t)((height + 7) / 8);
     const int rc = run_timed(ctx, who, kernelMs, [&]() -> int {
-        k_taa_resolve<<<(unsigned)((tiles + 3) / 4), 256, 0, ctx->stream>>>(a);
+        k_taa_resolve<<<tile_blocks(width, height), 256, 0, ctx->stream>>>(a);
         return IDKPT_OK;
-    }, out, ctx->taaHist[dst].p, out ? bytes : 0);
-    if (rc == IDKPT_OK) ctx->taaLast = dst;
+    }, out, r.taa.buf[dst].p, out ? bytes : 0);
+    if (rc == IDKPT_OK) r.taa.publish(width, height, dst);
     return rc;
 }
 
 IDKPT_API int idkpt_taa_device_ptr(IdkPtCtx* ctx, void** devPtr, uint64_t* bytes) {
-    if (!ctx || !devPtr) return fail(ctx, IDKPT_ERR_INVALID_ARGUMENT, "idkpt_taa_device_ptr: null argument");
-    if (ctx->taaLast < 0) return fail(ctx, IDKPT_ERR_INVALID_ARGUMENT, "idkpt_taa_device_ptr: call idkpt_taa_resolve first");
-    *devPtr = ctx->taaHist[ctx->taaLast].p;
-    if (bytes) *bytes = (uint64_t)ctx->taaW * ctx->taaH * 8;
-    return IDKPT_OK;
+    return image_device_ptr(ctx, "idkpt_taa_device_ptr", &RasterState::taa, "idkpt_taa_resolve", 8, 1, devPtr, bytes);
 }
 
 // ---- variable-rate deferred lighting (LightingShadingRateClassifier.Compute) ---------------------------------------------------
@@ -2594,57 +2583,48 @@ IDKPT_API int idkpt_shading_rate(IdkPtCtx* ctx, const GpuPerFrameData* frame, co
                                  uint8_t* outRates, float* debugOut, float* kernelMs) {
     static const char* who = "idkpt_shading_rate";
     if (!ctx || !frame || !s || !in || !in->VelocityRG) return fail(ctx, IDKPT_ERR_INVALID_ARGUMENT, "idkpt_shading_rate: null argument");
-    if (in->Width < 1 || in->Height < 1 || in->Width > 16384 || in->Height > 16384) return fail(ctx, who, IDKPT_ERR_INVALID_ARGUMENT, "size outside 1..16384");
+    if (int rc = size_check(ctx, who, in->Width, in->Height)) return rc;
     if (in->OnDevice != 0 && in->OnDevice != 1) return fail(ctx, who, IDKPT_ERR_INVALID_ARGUMENT, "OnDevice is neither 0 nor 1");
     if (s->DebugMode < 0 || s->DebugMode > 4) return fail(ctx, who, IDKPT_ERR_INVALID_ARGUMENT, "DebugMode outside 0..4");
     if (debugOut && s->DebugMode < 2) return fail(ctx, who, IDKPT_ERR_INVALID_ARGUMENT, "a debug image needs DebugMode 2, 3 or 4");
     if (!std::isfinite(s->SpeedFactor) || !std::isfinite(s->LumVarianceFactor))
         return fail(ctx, who, IDKPT_ERR_INVALID_ARGUMENT, "SpeedFactor or LumVarianceFactor not finite");
     CK(cudaSetDevice(ctx->device));
-    if (int rc = lit_source_check(ctx, who, in->Source, false, in->ColorRgba32f, in->Width, in->Height, in->OnDevice)) return rc;
-    if (in->OnDevice)
-        if (int rc = device_array_check(ctx, who, in->VelocityRG, 8, "OnDevice VelocityRG pointer not 8-byte aligned")) return rc;
+    if (int rc = lit_source_check(ctx, who, in->Source, false, in->ColorRgba32f, in->Width, in->Height)) return rc;
+    const float* src[2];           // the lit image, velocity
+    if (int rc = stage_inputs(ctx, who, in->Width, in->Height, in->OnDevice, {lit_input(ctx, in->Source, in->ColorRgba32f),
+                              velocity_input(in->VelocityRG)}, src)) return rc;
     if (kernelMs) *kernelMs = 0.0f;
     const unsigned tilesX = (unsigned)(in->Width + IDK_VRS_TILE - 1) / IDK_VRS_TILE, tilesY = (unsigned)(in->Height + IDK_VRS_TILE - 1) / IDK_VRS_TILE;
     const size_t tiles = (size_t)tilesX * tilesY;
-    ctx->vrsW = ctx->vrsH = 0;     // the image may be reallocated and is overwritten: valid again only when the call succeeds
-    const IdkPtGBuffer g = {in->Width, in->Height, in->OnDevice, nullptr, nullptr, nullptr, nullptr, nullptr};
-    const size_t stageBytes = in->OnDevice ? 0 : gbuffer_stage_bytes(&g, {2, in->Source == IDKPT_LIT_SOURCE_ARRAY ? 4u : 0u});
+    RasterImage& out = ctx->raster.vrs;
+    out.invalidate();              // the images may be reallocated and are overwritten: valid again only when the call succeeds
     const bool debug = s->DebugMode >= 2;
-    if ((stageBytes && ensure(ctx->gbufStage, stageBytes) != cudaSuccess) || ensure(ctx->vrsRates, tiles) != cudaSuccess ||
-        (debug && ensure(ctx->vrsDebug, tiles * 4) != cudaSuccess))
-        return fail(ctx, IDKPT_ERR_OUT_OF_MEMORY, "idkpt_shading_rate: device allocation failed");
-    size_t off = 0;
-    const float *velocity, *color;
-    if (int rc = gbuffer_input(ctx, &g, in->VelocityRG, 2, ctx->gbufStage, off, velocity)) return rc;
-    if (int rc = lit_source_input(ctx, &g, in->Source, in->ColorRgba32f, off, color)) return rc;
+    if (ensure(out.buf[0], tiles) != cudaSuccess || (debug && ensure(out.buf[1], tiles * 4) != cudaSuccess))
+        return fail(ctx, who, IDKPT_ERR_OUT_OF_MEMORY, "device allocation failed");
     ShadingRateArgs a;
-    a.color = (const float4*)color;
-    a.velocity = (const float2*)velocity;
+    a.color = (const float4*)src[0];
+    a.velocity = (const float2*)src[1];
     a.w = in->Width; a.h = in->Height;
     a.deltaRenderTime = frame->DeltaRenderTime; a.speedFactor = s->SpeedFactor; a.lumVarianceFactor = s->LumVarianceFactor;
     a.debugMode = s->DebugMode;
-    a.rates = (uint8_t*)ctx->vrsRates.p;
-    a.debug = debug ? (float*)ctx->vrsDebug.p : nullptr;
+    a.rates = (uint8_t*)out.buf[0].p;
+    a.debug = debug ? (float*)out.buf[1].p : nullptr;
     const int rc = run_timed(ctx, who, kernelMs, [&]() -> int {
         k_shading_rate<<<dim3(tilesX, tilesY), 256, 0, ctx->stream>>>(a);
         return IDKPT_OK;
-    }, outRates, ctx->vrsRates.p, outRates ? tiles : 0);
+    }, outRates, out.buf[0].p, outRates ? tiles : 0);
     if (rc != IDKPT_OK) return rc;
     if (debugOut) {
-        CK(cudaMemcpyAsync(debugOut, ctx->vrsDebug.p, tiles * 4, cudaMemcpyDeviceToHost, ctx->stream));
+        CK(cudaMemcpyAsync(debugOut, out.buf[1].p, tiles * 4, cudaMemcpyDeviceToHost, ctx->stream));
         CK(cudaStreamSynchronize(ctx->stream));
     }
-    ctx->vrsW = in->Width; ctx->vrsH = in->Height;
+    out.publish(in->Width, in->Height);
     return IDKPT_OK;
 }
 
 IDKPT_API int idkpt_shading_rate_device_ptr(IdkPtCtx* ctx, void** devPtr, uint64_t* bytes) {
-    if (!ctx || !devPtr) return fail(ctx, IDKPT_ERR_INVALID_ARGUMENT, "idkpt_shading_rate_device_ptr: null argument");
-    if (!ctx->vrsW) return fail(ctx, IDKPT_ERR_INVALID_ARGUMENT, "idkpt_shading_rate_device_ptr: call idkpt_shading_rate first");
-    *devPtr = ctx->vrsRates.p;
-    if (bytes) *bytes = (uint64_t)((ctx->vrsW + IDK_VRS_TILE - 1) / IDK_VRS_TILE) * ((ctx->vrsH + IDK_VRS_TILE - 1) / IDK_VRS_TILE);
-    return IDKPT_OK;
+    return image_device_ptr(ctx, "idkpt_shading_rate_device_ptr", &RasterState::vrs, "idkpt_shading_rate", 1, IDK_VRS_TILE, devPtr, bytes);
 }
 
 // ---- the G-buffer pass (RasterPipeline.Render's "Fill G-Buffer" draws) --------------------------------------------------------
@@ -2664,49 +2644,47 @@ IDKPT_API int idkpt_gbuffer(IdkPtCtx* ctx, const GpuPerFrameData* frame, int32_t
                             const PackedVec3* prevPositions, float* kernelMs) {
     static const char* who = "idkpt_gbuffer";
     if (!ctx || !frame) return fail(ctx, IDKPT_ERR_INVALID_ARGUMENT, "idkpt_gbuffer: null argument");
-    if (!ctx->haveScene) return fail(ctx, IDKPT_ERR_NO_SCENE, "idkpt_gbuffer: no scene");
-    if (width < 1 || height < 1 || width > 16384 || height > 16384) return fail(ctx, who, IDKPT_ERR_INVALID_ARGUMENT, "size outside 1..16384");
-    if (taaJitter && (!std::isfinite(taaJitter[0]) || !std::isfinite(taaJitter[1])))
-        return fail(ctx, who, IDKPT_ERR_INVALID_ARGUMENT, "jitter not finite");
+    if (!ctx->haveScene) return fail(ctx, who, IDKPT_ERR_NO_SCENE, "no scene");
+    if (int rc = size_check(ctx, who, width, height)) return rc;
+    GBufferArgs a;
+    if (!read_jitter(taaJitter, a.jitter)) return fail(ctx, who, IDKPT_ERR_INVALID_ARGUMENT, "jitter not finite");
     CK(cudaSetDevice(ctx->device));
     if (kernelMs) *kernelMs = 0.0f;
+    RasterState& r = ctx->raster;
     size_t off[6];
     const size_t bytes = gbuffer_planes(width, height, off);
     const size_t prevBytes = ctx->counts.VertexPositionCount * sizeof(PackedVec3);
-    ctx->gbW = ctx->gbH = 0;       // the images may be reallocated and are overwritten: valid again only when the call succeeds
-    if (ensure(ctx->gbImages, bytes) != cudaSuccess || (prevPositions && ensure(ctx->gbPrev, std::max<size_t>(prevBytes, 16)) != cudaSuccess))
-        return fail(ctx, IDKPT_ERR_OUT_OF_MEMORY, "idkpt_gbuffer: device allocation failed");
-    if (prevPositions && prevBytes) CK(cudaMemcpyAsync(ctx->gbPrev.p, prevPositions, prevBytes, cudaMemcpyHostToDevice, ctx->stream));
-    char* base = (char*)ctx->gbImages.p;
-    GBufferArgs a;
+    r.gb.invalidate();             // the images may be reallocated and are overwritten: valid again only when the call succeeds
+    if (ensure(r.gb.buf[0], bytes) != cudaSuccess || (prevPositions && ensure(r.gbPrev, std::max<size_t>(prevBytes, 16)) != cudaSuccess))
+        return fail(ctx, who, IDKPT_ERR_OUT_OF_MEMORY, "device allocation failed");
+    if (prevPositions && prevBytes) CK(cudaMemcpyAsync(r.gbPrev.p, prevPositions, prevBytes, cudaMemcpyHostToDevice, ctx->stream));
+    char* base = (char*)r.gb.buf[0].p;
     a.sc = ctx->sc;
     a.positions = (const float*)ctx->positions.p;
-    a.prevPositions = prevPositions ? (const float*)ctx->gbPrev.p : a.positions;
+    a.prevPositions = prevPositions ? (const float*)r.gbPrev.p : a.positions;
     memcpy(a.projView, frame->ProjView, sizeof(a.projView));
     memcpy(a.prevProjView, frame->PrevProjView, sizeof(a.prevProjView));
     memcpy(a.invProjView, frame->InvProjView, sizeof(a.invProjView));
     for (int k = 0; k < 3; k++) a.viewPos[k] = frame->ViewPos[k];
-    a.jitter[0] = taaJitter ? taaJitter[0] : 0.0f; a.jitter[1] = taaJitter ? taaJitter[1] : 0.0f;
     a.w = width; a.h = height;
     a.depth = (float*)(base + off[0]); a.normalRG = (float2*)(base + off[1]); a.albedo = (float*)(base + off[2]);
     a.metallicRoughness = (float2*)(base + off[3]); a.emissive = (float*)(base + off[4]); a.velocity = (float2*)(base + off[5]);
-    const size_t tiles = (size_t)((width + 7) / 8) * (size_t)((height + 7) / 8);
     const int rc = run_timed(ctx, who, kernelMs, [&]() -> int {
-        k_gbuffer<<<(unsigned)((tiles + 3) / 4), IDK_BLOCK, ctx->stackBytes, ctx->stream>>>(a);
+        k_gbuffer<<<tile_blocks(width, height), IDK_BLOCK, ctx->stackBytes, ctx->stream>>>(a);
         return IDKPT_OK;
     });
-    if (rc == IDKPT_OK) { ctx->gbW = width; ctx->gbH = height; }
+    if (rc == IDKPT_OK) r.gb.publish(width, height);
     return rc;
 }
 
 IDKPT_API int idkpt_gbuffer_device_ptrs(IdkPtCtx* ctx, IdkPtGBuffer* gbufferOut, const float** velocityOut) {
-    if (!ctx || (!gbufferOut && !velocityOut)) return fail(ctx, IDKPT_ERR_INVALID_ARGUMENT, "idkpt_gbuffer_device_ptrs: null argument");
-    if (!ctx->gbW) return fail(ctx, IDKPT_ERR_INVALID_ARGUMENT, "idkpt_gbuffer_device_ptrs: call idkpt_gbuffer first");
+    const RasterImage* r = published_image(ctx, "idkpt_gbuffer_device_ptrs", gbufferOut || velocityOut, &RasterState::gb, "idkpt_gbuffer");
+    if (!r) return IDKPT_ERR_INVALID_ARGUMENT;
     size_t off[6];
-    gbuffer_planes(ctx->gbW, ctx->gbH, off);
-    const char* base = (const char*)ctx->gbImages.p;
+    gbuffer_planes(r->w, r->h, off);
+    const char* base = (const char*)r->buf[0].p;
     if (gbufferOut)
-        *gbufferOut = IdkPtGBuffer{ctx->gbW, ctx->gbH, 1, (const float*)(base + off[0]), (const float*)(base + off[1]),
+        *gbufferOut = IdkPtGBuffer{r->w, r->h, 1, (const float*)(base + off[0]), (const float*)(base + off[1]),
                                    (const float*)(base + off[2]), (const float*)(base + off[3]), (const float*)(base + off[4])};
     if (velocityOut) *velocityOut = (const float*)(base + off[5]);
     return IDKPT_OK;
@@ -2715,15 +2693,16 @@ IDKPT_API int idkpt_gbuffer_device_ptrs(IdkPtCtx* ctx, IdkPtGBuffer* gbufferOut,
 IDKPT_API int idkpt_read_gbuffer(IdkPtCtx* ctx, float* depth, float* normalRG, float* albedoRGB, float* metallicRoughness,
                                  float* emissiveRGB, float* velocityRG) {
     if (!ctx) return IDKPT_ERR_INVALID_ARGUMENT;
-    if (!ctx->gbW) return fail(ctx, IDKPT_ERR_INVALID_ARGUMENT, "idkpt_read_gbuffer: call idkpt_gbuffer first");
+    const RasterImage& gb = ctx->raster.gb;
+    if (!gb.valid()) return fail(ctx, "idkpt_read_gbuffer", IDKPT_ERR_INVALID_ARGUMENT, "call idkpt_gbuffer first");
     CK(cudaSetDevice(ctx->device));
     size_t off[6];
-    gbuffer_planes(ctx->gbW, ctx->gbH, off);
+    gbuffer_planes(gb.w, gb.h, off);
     float* dst[6] = {depth, normalRG, albedoRGB, metallicRoughness, emissiveRGB, velocityRG};
     static const size_t floats[6] = {1, 2, 3, 2, 3, 2};
-    const size_t n = (size_t)ctx->gbW * ctx->gbH;
+    const size_t n = (size_t)gb.w * gb.h;
     for (int i = 0; i < 6; i++)
-        if (dst[i]) CK(cudaMemcpyAsync(dst[i], (const char*)ctx->gbImages.p + off[i], n * floats[i] * 4, cudaMemcpyDeviceToHost, ctx->stream));
+        if (dst[i]) CK(cudaMemcpyAsync(dst[i], (const char*)gb.buf[0].p + off[i], n * floats[i] * 4, cudaMemcpyDeviceToHost, ctx->stream));
     CK(cudaStreamSynchronize(ctx->stream));
     return IDKPT_OK;
 }
@@ -2741,8 +2720,8 @@ IDKPT_API int idkpt_transparency(IdkPtCtx* ctx, const GpuPerFrameData* frame, co
                                  float* outRgba32f, float* kernelMs) {
     static const char* who = "idkpt_transparency";
     if (!ctx || !frame || !s || !g || !g->Depth) return fail(ctx, IDKPT_ERR_INVALID_ARGUMENT, "idkpt_transparency: null argument");
-    if (!ctx->haveScene) return fail(ctx, IDKPT_ERR_NO_SCENE, "idkpt_transparency: no scene");
-    if (g->Width < 1 || g->Height < 1 || g->Width > 16384 || g->Height > 16384) return fail(ctx, who, IDKPT_ERR_INVALID_ARGUMENT, "size outside 1..16384");
+    if (!ctx->haveScene) return fail(ctx, who, IDKPT_ERR_NO_SCENE, "no scene");
+    if (int rc = size_check(ctx, who, g->Width, g->Height)) return rc;
     if (g->OnDevice != 0 && g->OnDevice != 1) return fail(ctx, who, IDKPT_ERR_INVALID_ARGUMENT, "OnDevice is neither 0 nor 1");
     if (s->ShadowMode < 0 || s->ShadowMode > 2) return fail(ctx, who, IDKPT_ERR_INVALID_ARGUMENT, "ShadowMode outside 0..2");
     if (s->IsVXGI != 0 && s->IsVXGI != 1) return fail(ctx, who, IDKPT_ERR_INVALID_ARGUMENT, "IsVXGI is neither 0 nor 1");
@@ -2752,52 +2731,39 @@ IDKPT_API int idkpt_transparency(IdkPtCtx* ctx, const GpuPerFrameData* frame, co
         if (voxels->device != ctx->device) return fail(ctx, who, IDKPT_ERR_INVALID_ARGUMENT, "IsVXGI with a voxeliser context on another device");
         if (cone->MaxSamples < 1 || cone->MaxSamples > 64) return fail(ctx, who, IDKPT_ERR_INVALID_ARGUMENT, "cone MaxSamples out of range");
     }
-    if (taaJitter && (!std::isfinite(taaJitter[0]) || !std::isfinite(taaJitter[1])))
-        return fail(ctx, who, IDKPT_ERR_INVALID_ARGUMENT, "jitter not finite");
-    const uint32_t shadowCount = (uint32_t)ctx->pointShadowRecs.size();
-    if (s->ShadowMode == 1) {
-        for (const GpuLight& L : ctx->hostLights)
-            if (L.PointShadowIndex != -1 && (L.PointShadowIndex < 0 || (uint32_t)L.PointShadowIndex >= shadowCount))
-                return fail(ctx, who, IDKPT_ERR_INVALID_ARGUMENT, "a light's PointShadowIndex is neither -1 nor below the point-shadow count");
-    }
+    TransparencyArgs a;
+    if (!read_jitter(taaJitter, a.jitter)) return fail(ctx, who, IDKPT_ERR_INVALID_ARGUMENT, "jitter not finite");
+    if (s->ShadowMode == 1)
+        if (int rc = shadow_index_check(ctx, who)) return rc;
     CK(cudaSetDevice(ctx->device));
-    if (int rc = lit_source_check(ctx, who, source, false, color, g->Width, g->Height, g->OnDevice)) return rc;
-    if (g->OnDevice)
-        if (int rc = gbuffer_device_check(ctx, who, g->Depth, 4)) return rc;
+    if (int rc = lit_source_check(ctx, who, source, false, color, g->Width, g->Height)) return rc;
+    const float* in[2];            // the lit image (the stage copy, the caller's device array or the context's deferred image), depth
+    if (int rc = stage_inputs(ctx, who, g->Width, g->Height, g->OnDevice, {lit_input(ctx, source, color), attachment(g->Depth, 1)}, in)) return rc;
     if (kernelMs) *kernelMs = 0.0f;
     const size_t n = (size_t)g->Width * g->Height;
     const bool hostArray = source == IDKPT_LIT_SOURCE_ARRAY && !g->OnDevice;
-    const size_t stageBytes = g->OnDevice ? 0 : gbuffer_stage_bytes(g, {1, hostArray ? 4u : 0u});
-    if (stageBytes && ensure(ctx->gbufStage, stageBytes) != cudaSuccess)
-        return fail(ctx, IDKPT_ERR_OUT_OF_MEMORY, "idkpt_transparency: device allocation failed");
-    size_t off = 0;
-    const float *depth, *target;
-    if (int rc = gbuffer_input(ctx, g, g->Depth, 1, ctx->gbufStage, off, depth)) return rc;
-    if (int rc = lit_source_input(ctx, g, source, color, off, target)) return rc;
-    TransparencyArgs a;
     a.sc = ctx->sc;
     a.positions = (const float*)ctx->positions.p;
     memcpy(a.projView, frame->ProjView, sizeof(a.projView));
     memcpy(a.invProjView, frame->InvProjView, sizeof(a.invProjView));
     for (int k = 0; k < 3; k++) a.viewPos[k] = frame->ViewPos[k];
-    a.jitter[0] = taaJitter ? taaJitter[0] : 0.0f; a.jitter[1] = taaJitter ? taaJitter[1] : 0.0f;
     a.w = g->Width; a.h = g->Height;
-    a.depth = depth;
-    a.color = (float4*)target;     // the stage copy, the caller's device array or the context's deferred image: written in place
+    a.depth = in[1];
+    a.color = (float4*)in[0];      // written in place
     a.shadowMode = s->ShadowMode;
-    a.shadows = PointShadowMapsDev{(const PointShadowDev*)ctx->pointShadowDev.p, (const uint16_t*)ctx->pointShadowMaps.p, shadowCount};
+    a.shadows = PointShadowMapsDev{(const PointShadowDev*)ctx->pointShadowDev.p, (const uint16_t*)ctx->pointShadowMaps.p,
+                                   (uint32_t)ctx->pointShadowRecs.size()};
     a.g = s->IsVXGI ? voxels->grid : VxGridDev{};
     a.cone = s->IsVXGI ? VxConeParams{cone->MaxSamples, cone->StepMultiplier, cone->GIBoost, cone->GISkyBoxBoost, cone->NormalRayOffset, cone->NoiseIndex}
                        : VxConeParams{1, 0.0f, 0.0f, 0.0f, 0.0f, 0u};
-    const size_t tiles = (size_t)((g->Width + 7) / 8) * (size_t)((g->Height + 7) / 8);
     const int rc = run_timed(ctx, who, kernelMs, [&]() -> int {
-        if (s->IsVXGI) k_transparency<true><<<(unsigned)((tiles + 3) / 4), IDK_BLOCK, ctx->stackBytes, ctx->stream>>>(a);
-        else k_transparency<false><<<(unsigned)((tiles + 3) / 4), IDK_BLOCK, ctx->stackBytes, ctx->stream>>>(a);
+        if (s->IsVXGI) k_transparency<true><<<tile_blocks(g->Width, g->Height), IDK_BLOCK, ctx->stackBytes, ctx->stream>>>(a);
+        else k_transparency<false><<<tile_blocks(g->Width, g->Height), IDK_BLOCK, ctx->stackBytes, ctx->stream>>>(a);
         return IDKPT_OK;
     });
     if (rc != IDKPT_OK) return rc;
-    if (hostArray) CK(cudaMemcpyAsync(color, target, n * 16, cudaMemcpyDeviceToHost, ctx->stream));
-    if (outRgba32f) CK(cudaMemcpyAsync(outRgba32f, target, n * 16, cudaMemcpyDeviceToHost, ctx->stream));
+    if (hostArray) CK(cudaMemcpyAsync(color, in[0], n * 16, cudaMemcpyDeviceToHost, ctx->stream));
+    if (outRgba32f) CK(cudaMemcpyAsync(outRgba32f, in[0], n * 16, cudaMemcpyDeviceToHost, ctx->stream));
     if (hostArray || outRgba32f) CK(cudaStreamSynchronize(ctx->stream));
     return IDKPT_OK;
 }
@@ -2807,19 +2773,19 @@ IDKPT_API int idkpt_lights_and_skybox(IdkPtCtx* ctx, const GpuPerFrameData* fram
                                       float* kernelMs) {
     static const char* who = "idkpt_lights_and_skybox";
     if (!ctx || !frame) return fail(ctx, IDKPT_ERR_INVALID_ARGUMENT, "idkpt_lights_and_skybox: null argument");
-    if (!ctx->haveScene) return fail(ctx, IDKPT_ERR_NO_SCENE, "idkpt_lights_and_skybox: no scene");
-    if (!ctx->gbW) return fail(ctx, who, IDKPT_ERR_INVALID_ARGUMENT, "call idkpt_gbuffer first");
-    if (ctx->deferredW != ctx->gbW || ctx->deferredH != ctx->gbH)
+    if (!ctx->haveScene) return fail(ctx, who, IDKPT_ERR_NO_SCENE, "no scene");
+    const RasterState& r = ctx->raster;
+    if (!r.gb.valid()) return fail(ctx, who, IDKPT_ERR_INVALID_ARGUMENT, "call idkpt_gbuffer first");
+    if (!r.deferred.valid_at(r.gb.w, r.gb.h))
         return fail(ctx, who, IDKPT_ERR_INVALID_ARGUMENT, "needs an idkpt_deferred_lighting image of the G-buffer's size");
-    if (taaJitter && (!std::isfinite(taaJitter[0]) || !std::isfinite(taaJitter[1])))
-        return fail(ctx, who, IDKPT_ERR_INVALID_ARGUMENT, "jitter not finite");
+    LightsSkyboxArgs a;
+    if (!read_jitter(taaJitter, a.jitter)) return fail(ctx, who, IDKPT_ERR_INVALID_ARGUMENT, "jitter not finite");
     CK(cudaSetDevice(ctx->device));
     if (kernelMs) *kernelMs = 0.0f;
-    const int w = ctx->gbW, h = ctx->gbH;
+    const int w = r.gb.w, h = r.gb.h;
     size_t off[6];
     gbuffer_planes(w, h, off);
-    char* base = (char*)ctx->gbImages.p;
-    LightsSkyboxArgs a;
+    char* base = (char*)r.gb.buf[0].p;
     a.sc = ctx->sc;
     a.lights = ctx->sc.lights; a.lightCount = (int)ctx->counts.LightCount;
     memcpy(a.projView, frame->ProjView, sizeof(a.projView));
@@ -2830,16 +2796,14 @@ IDKPT_API int idkpt_lights_and_skybox(IdkPtCtx* ctx, const GpuPerFrameData* fram
     memcpy(a.invView, frame->InvView, sizeof(a.invView));
     memcpy(a.prevView, frame->PrevView, sizeof(a.prevView));
     for (int k = 0; k < 3; k++) a.viewPos[k] = frame->ViewPos[k];
-    a.jitter[0] = taaJitter ? taaJitter[0] : 0.0f; a.jitter[1] = taaJitter ? taaJitter[1] : 0.0f;
     a.w = w; a.h = h;
     a.depth = (float*)(base + off[0]); a.normalRG = (float2*)(base + off[1]); a.emissive = (float*)(base + off[4]);
     a.velocity = (float2*)(base + off[5]);
-    a.color = (float4*)ctx->deferredOut.p;
-    const size_t n = (size_t)w * h, tiles = (size_t)((w + 7) / 8) * (size_t)((h + 7) / 8);
+    a.color = (float4*)r.deferred.buf[0].p;
     return run_timed(ctx, who, kernelMs, [&]() -> int {
-        k_lights_skybox<<<(unsigned)((tiles + 3) / 4), 256, 0, ctx->stream>>>(a);
+        k_lights_skybox<<<tile_blocks(w, h), 256, 0, ctx->stream>>>(a);
         return IDKPT_OK;
-    }, outRgba32f, ctx->deferredOut.p, outRgba32f ? n * 16 : 0);
+    }, outRgba32f, r.deferred.buf[0].p, outRgba32f ? (size_t)w * h * 16 : 0);
 }
 
 } // extern "C"

@@ -47,6 +47,12 @@ class PathTracer:
             msg = self._lib.idkpt_last_error(self._ctx)
             raise IdkPtError(f"{what} failed ({rc}): {msg.decode() if msg else ''}")
 
+    def _device_ptr(self, name, *args):
+        """(device pointer, bytes) from the library's export `name` (an idkpt_*_device_ptr)."""
+        p, n = ctypes.c_void_p(), ctypes.c_uint64()
+        self._check(getattr(self._lib, name)(self._ctx, *args, ctypes.byref(p), ctypes.byref(n)), name)
+        return p.value, n.value
+
     def Dispose(self):
         if self._ctx:
             self._lib.idkpt_destroy(self._ctx)
@@ -315,14 +321,10 @@ class PathTracer:
             raise IdkPtError("idkpt_gather_connect failed (%d): %s" % (rc, "; ".join(m.decode() for m in msgs if m)))
 
     def GatheredDevicePtr(self):
-        p, n = ctypes.c_void_p(), ctypes.c_uint64()
-        self._check(self._lib.idkpt_gather_device_ptr(self._ctx, ctypes.byref(p), ctypes.byref(n)), "idkpt_gather_device_ptr")
-        return p.value, n.value
+        return self._device_ptr("idkpt_gather_device_ptr")
 
     def ResultDevicePtr(self, which=capi.IDKPT_IMAGE_RESULT):
-        p, n = ctypes.c_void_p(), ctypes.c_uint64()
-        self._check(self._lib.idkpt_result_device_ptr(self._ctx, which, ctypes.byref(p), ctypes.byref(n)), "idkpt_result_device_ptr")
-        return p.value, n.value
+        return self._device_ptr("idkpt_result_device_ptr", which)
 
     def TileRows(self):
         n = ctypes.c_int32()
@@ -366,11 +368,11 @@ class PathTracer:
         depth = np.ascontiguousarray(depth, np.float32)
         nrg = np.ascontiguousarray(normal_rg, np.float32)
         vis = np.zeros((h, w), np.float32) if visibility is None else np.ascontiguousarray(visibility, np.float32)
-        jit = np.array(jitter, np.float32)
         frame = np.ascontiguousarray(frame)
         ms = ctypes.c_float()
         self._check(self._lib.idkpt_shadows_ray_traced(self._ctx, frame.ctypes.data, depth.ctypes.data, nrg.ctypes.data, w, h, light_index,
-                                                       samples, noise_index, jit.ctypes.data, vis.ctypes.data, ctypes.byref(ms)), "idkpt_shadows_ray_traced")
+                                                       samples, noise_index, self._jitter(jitter), vis.ctypes.data, ctypes.byref(ms)),
+                    "idkpt_shadows_ray_traced")
         return vis, ms.value
 
     # ---- point-shadow cube maps (PointShadowManager.UpdateBuffer / RenderShadowMaps)
@@ -405,9 +407,7 @@ class PathTracer:
         return out
 
     def PointShadowDevicePtr(self, index):
-        p, n = ctypes.c_void_p(), ctypes.c_uint64()
-        self._check(self._lib.idkpt_point_shadow_device_ptr(self._ctx, index, ctypes.byref(p), ctypes.byref(n)), "idkpt_point_shadow_device_ptr")
-        return p.value, n.value
+        return self._device_ptr("idkpt_point_shadow_device_ptr", index)
 
     # ---- volumetric lighting (VolumetricLighting.Compute)
     def VolumetricLighting(self, frame, depth, width, height, settings=None, jitter=None, download=True):
@@ -417,61 +417,63 @@ class PathTracer:
         in ms is left in last_volumetric_ms."""
         st = settings if settings is not None else capi.default_volumetric_settings()
         d = np.ascontiguousarray(depth, np.float32)
-        jit = None if jitter is None else np.ascontiguousarray(jitter, np.float32)
         frame = np.ascontiguousarray(frame)
         out = np.zeros((height, width, 4), np.float16) if download else None
         ms = ctypes.c_float()
         self._check(self._lib.idkpt_volumetric_lighting(self._ctx, frame.ctypes.data, ctypes.byref(st), d.ctypes.data, d.shape[1], d.shape[0],
-                                                        width, height, jit.ctypes.data if jit is not None else None,
-                                                        out.ctypes.data if download else None, ctypes.byref(ms)), "idkpt_volumetric_lighting")
+                                                        width, height, self._jitter(jitter), out.ctypes.data if download else None,
+                                                        ctypes.byref(ms)), "idkpt_volumetric_lighting")
         self.last_volumetric_ms = ms.value
         return out
 
     def VolumetricDevicePtr(self):
         """(device pointer, bytes) of the last VolumetricLighting image (rgba16f)."""
-        p, n = ctypes.c_void_p(), ctypes.c_uint64()
-        self._check(self._lib.idkpt_volumetric_device_ptr(self._ctx, ctypes.byref(p), ctypes.byref(n)), "idkpt_volumetric_device_ptr")
-        return p.value, n.value
+        return self._device_ptr("idkpt_volumetric_device_ptr")
 
-    # ---- G-buffer lighting (SSAO.Compute, the deferred lighting draw)
+    # ---- the raster passes' marshalling
     @staticmethod
     def _gbuffer(arrays, channels):
-        """IdkPtGBuffer over G-buffer arrays ([H, W] depth first, then [H, W, c] arrays or None): numpy arrays are passed as host
-        arrays, CUDA torch tensors in place (OnDevice = 1). Returns (struct, the contiguous arrays to keep alive, on_device)."""
+        """The input images of a raster call: [H, W] (channels 1) or [H, W, c] arrays, or None; the first one sets H and W. numpy
+        arrays are passed as host arrays, CUDA torch tensors in place (OnDevice = 1). Returns (IdkPtGBuffer over the first five,
+        every array's pointer (None for None), the contiguous arrays to keep alive)."""
         on_device = type(arrays[0]).__module__.startswith("torch")
         if on_device and not all(a is None or (type(a).__module__.startswith("torch") and a.is_cuda) for a in arrays):
             raise TypeError("G-buffer: pass either all numpy arrays or all CUDA tensors")
+        if on_device:
+            import torch
         keep = []
         for a, c in zip(arrays, channels):
             if a is None:
                 keep.append(None)
                 continue
-            if on_device:
-                import torch
-                t = a.to(torch.float32).contiguous()
-                keep.append(t)
-            else:
-                keep.append(np.ascontiguousarray(a, np.float32))
+            keep.append(a.to(torch.float32).contiguous() if on_device else np.ascontiguousarray(a, np.float32))
             # the library copies or reads W * H * c floats of every array: a smaller one must never reach it
             want = tuple(keep[0].shape[:2]) + (() if c == 1 else (c,))
-            if tuple(keep[-1].shape) != want or len(keep[0].shape) != 2:
-                raise ValueError(f"G-buffer array of shape {tuple(keep[-1].shape)}: expected {want} (depth [H, W] first)")
+            if tuple(keep[-1].shape) != want or keep[0].ndim < 2:
+                raise ValueError(f"G-buffer array of shape {tuple(keep[-1].shape)}: expected {want} (H and W from the first array)")
         h, w = keep[0].shape[:2]
         if on_device:   # the library's stream does not wait for torch's: let the tensors' producers finish
-            import torch
             torch.cuda.synchronize(keep[0].device)
+        ptrs = [None if a is None else (a.data_ptr() if on_device else a.ctypes.data) for a in keep]
+        return capi.IdkPtGBuffer(w, h, int(on_device), *ptrs[:5]), ptrs, keep
 
-        def ptr(a):
-            return None if a is None else (a.data_ptr() if on_device else a.ctypes.data)
-        g = capi.IdkPtGBuffer(w, h, int(on_device), *[ptr(a) for a in keep[:5]] + [None] * (5 - len(keep[:5])))
-        return g, keep, on_device
+    @staticmethod
+    def _jitter(jitter):
+        """taaDataUBO.Jitter in NDC units as the two floats the library reads, or None (no jitter)."""
+        if jitter is None:
+            return None
+        jit = np.ascontiguousarray(jitter, np.float32)
+        if jit.size != 2:
+            raise ValueError(f"jitter has two components, not {jit.size}")
+        return (ctypes.c_float * 2)(*jit.ravel())
 
+    # ---- G-buffer lighting (SSAO.Compute, the deferred lighting draw)
     def Ssao(self, frame, depth, normal_rg, settings=None, download=True):
         """SSAO.Compute on a G-buffer (depth [H, W], octahedral normal [H, W, 2]; numpy arrays or CUDA tensors). settings:
         capi.IdkPtSsaoSettings (default: the engine's). Returns uint8 [H, W] (R8Unorm), or None with download=False (the image
         stays on the device: SsaoDevicePtr, and DeferredLighting's IsSSAO reads it). Kernel ms in last_ssao_ms."""
         st = settings if settings is not None else capi.default_ssao_settings()
-        g, keep, _ = self._gbuffer([depth, normal_rg], [1, 2])
+        g, _, keep = self._gbuffer([depth, normal_rg], [1, 2])
         frame = np.ascontiguousarray(frame)
         out = np.zeros((g.Height, g.Width), np.uint8) if download else None
         ms = ctypes.c_float()
@@ -482,9 +484,7 @@ class PathTracer:
 
     def SsaoDevicePtr(self):
         """(device pointer, bytes) of the last Ssao image (R8Unorm)."""
-        p, n = ctypes.c_void_p(), ctypes.c_uint64()
-        self._check(self._lib.idkpt_ssao_device_ptr(self._ctx, ctypes.byref(p), ctypes.byref(n)), "idkpt_ssao_device_ptr")
-        return p.value, n.value
+        return self._device_ptr("idkpt_ssao_device_ptr")
 
     def DeferredLighting(self, frame, depth, normal_rg, albedo, metallic_roughness, emissive, settings=None, jitter=None, indirect=None,
                          rt_visibility=None, download=True, vrs=False):
@@ -499,27 +499,20 @@ class PathTracer:
             st = capi.IdkPtDeferredSettings.from_buffer_copy(st)
             st.IsVariableRateShading = 1
         rt = list(rt_visibility) if rt_visibility is not None else []
-        g, keep, on_device = self._gbuffer([depth, normal_rg, albedo, metallic_roughness, emissive, indirect] + rt, [1, 2, 3, 2, 3, 4] + [1] * len(rt))
-
-        def ptr(a):
-            return None if a is None else (a.data_ptr() if on_device else a.ctypes.data)
-        rt_ptrs = (ctypes.c_void_p * max(len(rt), 1))(*[ptr(a) for a in keep[6:]])
-        jit = None if jitter is None else np.ascontiguousarray(jitter, np.float32)
+        g, ptrs, keep = self._gbuffer([depth, normal_rg, albedo, metallic_roughness, emissive, indirect] + rt, [1, 2, 3, 2, 3, 4] + [1] * len(rt))
+        rt_ptrs = (ctypes.c_void_p * max(len(rt), 1))(*ptrs[6:])
         frame = np.ascontiguousarray(frame)
         out = np.zeros((g.Height, g.Width, 4), np.float32) if download else None
         ms = ctypes.c_float()
-        self._check(self._lib.idkpt_deferred_lighting(self._ctx, frame.ctypes.data, ctypes.byref(st), ctypes.byref(g),
-                                                      jit.ctypes.data if jit is not None else None, ptr(keep[5]),
-                                                      rt_ptrs if rt else None, len(rt), out.ctypes.data if download else None,
+        self._check(self._lib.idkpt_deferred_lighting(self._ctx, frame.ctypes.data, ctypes.byref(st), ctypes.byref(g), self._jitter(jitter),
+                                                      ptrs[5], rt_ptrs if rt else None, len(rt), out.ctypes.data if download else None,
                                                       ctypes.byref(ms)), "idkpt_deferred_lighting")
         self.last_deferred_ms = ms.value
         return out
 
     def DeferredDevicePtr(self):
         """(device pointer, bytes) of the last DeferredLighting image (rgba32f)."""
-        p, n = ctypes.c_void_p(), ctypes.c_uint64()
-        self._check(self._lib.idkpt_deferred_device_ptr(self._ctx, ctypes.byref(p), ctypes.byref(n)), "idkpt_deferred_device_ptr")
-        return p.value, n.value
+        return self._device_ptr("idkpt_deferred_device_ptr")
 
     # ---- the G-buffer pass (RasterPipeline.Render's "Fill G-Buffer" draws)
     GBUFFER_CHANNELS = (1, 2, 3, 2, 3, 2)   # depth, normal_rg, albedo, metallic_roughness, emissive, velocity_rg
@@ -530,15 +523,13 @@ class PathTracer:
         (depth [h, w], normal_rg [h, w, 2], albedo [h, w, 3], metallic_roughness [h, w, 2], emissive [h, w, 3], velocity_rg
         [h, w, 2]) as float32 numpy arrays, or None with download=False (the images stay on the device: GBufferDevicePtrs).
         Kernel ms in last_gbuffer_ms."""
-        jit = None if jitter is None else np.ascontiguousarray(jitter, np.float32)
+        jit = self._jitter(jitter)
         prev = None if prev_positions is None else np.ascontiguousarray(prev_positions, np.float32)
-        if jit is not None and jit.size != 2:
-            raise ValueError("GBuffer: jitter has two components")
         if prev is not None and (prev.ndim != 2 or prev.shape[1] != 3 or prev.shape[0] != self._vertex_position_count):
             raise ValueError(f"GBuffer: prev_positions {prev.shape}: expected ({self._vertex_position_count}, 3)")
         frame = np.ascontiguousarray(frame)
         ms = ctypes.c_float()
-        self._check(self._lib.idkpt_gbuffer(self._ctx, frame.ctypes.data, width, height, jit.ctypes.data if jit is not None else None,
+        self._check(self._lib.idkpt_gbuffer(self._ctx, frame.ctypes.data, width, height, jit,
                                             prev.ctypes.data if prev is not None else None, ctypes.byref(ms)), "idkpt_gbuffer")
         self.last_gbuffer_ms = ms.value
         if not download:
@@ -575,11 +566,8 @@ class PathTracer:
         None with download=False. Kernel ms in last_transparency_ms."""
         st = settings if settings is not None else capi.default_transparency_settings()
         src = self._lit_source(source, color)
-        g, keep, on_device = self._gbuffer([depth, None, None, None, None, color], [1, 2, 3, 2, 3, 4])
-        col = None if keep[5] is None else (keep[5].data_ptr() if on_device else keep[5].ctypes.data)
-        jit = None if jitter is None else np.ascontiguousarray(jitter, np.float32)
-        if jit is not None and jit.size != 2:
-            raise ValueError("Transparency: jitter has two components")
+        g, ptrs, keep = self._gbuffer([depth, None, None, None, None, color], [1, 2, 3, 2, 3, 4])
+        jit = self._jitter(jitter)
         cn = None
         if st.IsVXGI:
             from . import vxgi
@@ -587,14 +575,13 @@ class PathTracer:
         frame = np.ascontiguousarray(frame)
         out = np.zeros((g.Height, g.Width, 4), np.float32) if download else None
         ms = ctypes.c_float()
-        self._check(self._lib.idkpt_transparency(self._ctx, frame.ctypes.data, ctypes.byref(st), ctypes.byref(g),
-                                                 jit.ctypes.data if jit is not None else None,
+        self._check(self._lib.idkpt_transparency(self._ctx, frame.ctypes.data, ctypes.byref(st), ctypes.byref(g), jit,
                                                  voxelizer._ctx if voxelizer is not None else None,
-                                                 ctypes.byref(cn) if cn is not None else None, src, col,
+                                                 ctypes.byref(cn) if cn is not None else None, src, ptrs[5],
                                                  out.ctypes.data if download else None, ctypes.byref(ms)), "idkpt_transparency")
         self.last_transparency_ms = ms.value
         if color is not None and keep[5] is not color:
-            if on_device:
+            if g.OnDevice:
                 color.copy_(keep[5])
             else:
                 np.copyto(color, keep[5], casting="unsafe")
@@ -606,18 +593,15 @@ class PathTracer:
         (which must have the G-buffer's size), in place (DESIGN.md 8f.1i): later DEFERRED reads, GBufferDevicePtrs and
         GBuffer downloads see them. jitter: taaDataUBO.Jitter in NDC units (None = 0). Returns the lit image, float32 [H, W, 4],
         or None with download=False. Kernel ms in last_lights_and_skybox_ms."""
-        jit = None if jitter is None else np.ascontiguousarray(jitter, np.float32)
-        if jit is not None and jit.size != 2:
-            raise ValueError("LightsAndSkybox: jitter has two components")
+        jit = self._jitter(jitter)
         frame = np.ascontiguousarray(frame)
         out = None
         if download:
             g, _ = self.GBufferDevicePtrs()
             out = np.zeros((g.Height, g.Width, 4), np.float32)
         ms = ctypes.c_float()
-        self._check(self._lib.idkpt_lights_and_skybox(self._ctx, frame.ctypes.data, jit.ctypes.data if jit is not None else None,
-                                                      out.ctypes.data if download else None, ctypes.byref(ms)),
-                    "idkpt_lights_and_skybox")
+        self._check(self._lib.idkpt_lights_and_skybox(self._ctx, frame.ctypes.data, jit, out.ctypes.data if download else None,
+                                                      ctypes.byref(ms)), "idkpt_lights_and_skybox")
         self.last_lights_and_skybox_ms = ms.value
         return out
 
@@ -631,24 +615,9 @@ class PathTracer:
         returns (rates, float32 debug image of the same size) instead. Kernel ms in last_shading_rate_ms."""
         st = settings if settings is not None else capi.default_shading_rate_settings()
         src = self._lit_source(source, color)
-        v = velocity_rg
-        on_device = type(v).__module__.startswith("torch")
-        if on_device:
-            import torch
-            if not v.is_cuda or (color is not None and not (type(color).__module__.startswith("torch") and color.is_cuda)):
-                raise TypeError("ShadingRate: pass either all numpy arrays or all CUDA tensors")
-            keep = [v.to(torch.float32).contiguous()] + ([] if color is None else [color.to(torch.float32).contiguous()])
-            torch.cuda.synchronize(keep[0].device)   # the library's stream does not wait for torch's
-        else:
-            keep = [np.ascontiguousarray(v, np.float32)] + ([] if color is None else [np.ascontiguousarray(color, np.float32)])
-        h, w = keep[0].shape[:2]
-        if tuple(keep[0].shape) != (h, w, 2) or (color is not None and tuple(keep[1].shape) != (h, w, 4)):
-            raise ValueError(f"ShadingRate: velocity {tuple(keep[0].shape)} / colour {None if color is None else tuple(keep[1].shape)}: "
-                             "expected [h, w, 2] and [h, w, 4]")
-
-        def ptr(a):
-            return a.data_ptr() if on_device else a.ctypes.data
-        inputs = capi.IdkPtShadingRateInputs(w, h, int(on_device), src, ptr(keep[0]), ptr(keep[1]) if color is not None else None)
+        g, ptrs, keep = self._gbuffer([velocity_rg, color], [2, 4])
+        h, w = g.Height, g.Width
+        inputs = capi.IdkPtShadingRateInputs(w, h, g.OnDevice, src, *ptrs)
         tiles = ((h + capi.VRS_TILE - 1) // capi.VRS_TILE, (w + capi.VRS_TILE - 1) // capi.VRS_TILE)
         rates = np.zeros(tiles, np.uint8) if download else None
         dbg = np.zeros(tiles, np.float32) if debug else None
@@ -662,9 +631,7 @@ class PathTracer:
 
     def ShadingRateDevicePtr(self):
         """(device pointer, bytes) of the last ShadingRate image (R8 palette indices, [ceil(h/16)][ceil(w/16)])."""
-        p, n = ctypes.c_void_p(), ctypes.c_uint64()
-        self._check(self._lib.idkpt_shading_rate_device_ptr(self._ctx, ctypes.byref(p), ctypes.byref(n)), "idkpt_shading_rate_device_ptr")
-        return p.value, n.value
+        return self._device_ptr("idkpt_shading_rate_device_ptr")
 
     # ---- the end of the raster frame (SSR.Compute, "Merge Textures", TaaResolve.Compute)
     @staticmethod
@@ -685,13 +652,12 @@ class PathTracer:
         last_ssr_ms."""
         st = settings if settings is not None else capi.default_ssr_settings()
         src = self._lit_source(source, color)
-        g, keep, on_device = self._gbuffer([depth, normal_rg, albedo, metallic_roughness, None, color], [1, 2, 3, 2, 3, 4])
-        col = None if keep[5] is None else (keep[5].data_ptr() if on_device else keep[5].ctypes.data)
+        g, ptrs, keep = self._gbuffer([depth, normal_rg, albedo, metallic_roughness, None, color], [1, 2, 3, 2, 3, 4])
         frame = np.ascontiguousarray(frame)
         merged = np.zeros((g.Height, g.Width, 4), np.float32) if download else None
         ssr = np.zeros((g.Height, g.Width, 4), np.float16) if download else None
         ms = ctypes.c_float()
-        self._check(self._lib.idkpt_ssr(self._ctx, frame.ctypes.data, ctypes.byref(st), ctypes.byref(g), src, col,
+        self._check(self._lib.idkpt_ssr(self._ctx, frame.ctypes.data, ctypes.byref(st), ctypes.byref(g), src, ptrs[5],
                                         merged.ctypes.data if download else None, ssr.ctypes.data if download else None,
                                         ctypes.byref(ms)), "idkpt_ssr")
         self.last_ssr_ms = ms.value
@@ -712,11 +678,8 @@ class PathTracer:
         (TaaDevicePtr). Kernel ms in last_taa_ms."""
         st = settings if settings is not None else capi.default_taa_settings()
         src = self._lit_source(source, color)
-        g, keep, on_device = self._gbuffer([depth, velocity_rg, color], [1, 2, 4])
-
-        def ptr(a):
-            return None if a is None else (a.data_ptr() if on_device else a.ctypes.data)
-        inputs = capi.IdkPtTaaInputs(g.Width, g.Height, g.OnDevice, src, ptr(keep[0]), ptr(keep[1]), ptr(keep[2]))
+        g, ptrs, keep = self._gbuffer([depth, velocity_rg, color], [1, 2, 4])
+        inputs = capi.IdkPtTaaInputs(g.Width, g.Height, g.OnDevice, src, *ptrs)
         out = np.zeros((height, width, 4), np.float16) if download else None
         ms = ctypes.c_float()
         self._check(self._lib.idkpt_taa_resolve(self._ctx, ctypes.byref(st), ctypes.byref(inputs), width, height,
@@ -726,9 +689,7 @@ class PathTracer:
 
     def TaaDevicePtr(self):
         """(device pointer, bytes) of the image the last TaaResolve wrote (rgba16f)."""
-        p, n = ctypes.c_void_p(), ctypes.c_uint64()
-        self._check(self._lib.idkpt_taa_device_ptr(self._ctx, ctypes.byref(p), ctypes.byref(n)), "idkpt_taa_device_ptr")
-        return p.value, n.value
+        return self._device_ptr("idkpt_taa_device_ptr")
 
     # ---- properties with the reference's reset-on-set behaviour
     def _reset_prop(name, sub=None):  # noqa: N805

@@ -251,12 +251,15 @@ def test_wrapper_rejects_mismatched_gbuffer_shapes():
     import pytest
     from idkengine_b200.pathtracer import PathTracer
     d, n = np.zeros((H, W), np.float32), np.zeros((H, W, 2), np.float32)
-    g, _, on_device = PathTracer._gbuffer([d, n], [1, 2])
-    assert (g.Width, g.Height, g.OnDevice, on_device) == (W, H, 0, False)
+    g, ptrs, _ = PathTracer._gbuffer([d, n, None], [1, 2, 3])
+    assert (g.Width, g.Height, g.OnDevice) == (W, H, 0) and ptrs == [d.ctypes.data, n.ctypes.data, None]
+    assert (g.Depth, g.NormalRG, g.AlbedoRGB) == (d.ctypes.data, n.ctypes.data, None)
     for arrays, channels in (([d, n[:-1]], [1, 2]),                      # fewer rows
                              ([d, n[..., :1]], [1, 2]),                   # one channel where two are read
                              ([d[..., None], n], [1, 2]),                 # depth not 2-D
                              ([d.ravel(), n], [1, 2]),
-                             ([d, n, np.zeros((H, W // 2, 3), np.float32)], [1, 2, 3])):
+                             ([d, n, np.zeros((H, W // 2, 3), np.float32)], [1, 2, 3]),
+                             ([n, np.zeros((H, W - 1, 4), np.float32)], [2, 4]),   # ShadingRate: velocity first
+                             ([n[..., 0], np.zeros((H, W, 4), np.float32)], [2, 4])):
         with pytest.raises(ValueError, match="G-buffer array of shape"):
             PathTracer._gbuffer(arrays, channels)

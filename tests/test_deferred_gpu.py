@@ -298,7 +298,7 @@ def test_gpu_deferred_errors_leave_the_context_working():
         g = gbuffer(pt, scene, frame, W, H)
         pt.Ssao(frame, g[0], g[1])
         good = pt.DeferredLighting(frame, *g, jitter=JITTER)
-        gb, keep, _ = PathTracer._gbuffer(list(g), [1, 2, 3, 2, 3])
+        gb, _, keep = PathTracer._gbuffer(list(g), [1, 2, 3, 2, 3])
         sst, dst = ssao_settings(), deferred_settings(1, 1, 0)
 
         def ssao_rc(f=fr, s=sst, gg=None):
@@ -439,7 +439,7 @@ def test_gpu_misaligned_device_pointers_are_rejected_before_anything_runs():
         gi = torch.zeros((H, W, 4), dtype=torch.float32, device="cuda")
         with pytest.raises(IdkPtError, match="indirect-light pointer not 16-byte aligned"):
             pt.DeferredLighting(frame, *dg, settings=deferred_settings(0, 0, 1), indirect=shifted(gi, 2))
-        gb, keep, _ = PathTracer._gbuffer(dg, [1, 2, 3, 2, 3])
+        gb, _, keep = PathTracer._gbuffer(dg, [1, 2, 3, 2, 3])
         bad = capi.IdkPtGBuffer.from_buffer_copy(gb)
         bad.Depth = gb.Depth + 2                                                     # not even float-aligned
         with pytest.raises(IdkPtError, match="OnDevice pointer not 4-byte aligned"):
@@ -458,3 +458,36 @@ def test_gpu_misaligned_device_pointers_are_rejected_before_anything_runs():
         dev = torch.as_tensor(multigpu.DeviceArray(p, (nbytes // 4,), "<f4"), device="cuda").cpu().numpy()
         assert np.array_equal(canon(dev.reshape(8, 8, 4)), canon(lit))
         assert np.array_equal(pt.Ssao(frame, dg[0], dg[1]), pt.Ssao(frame, g[0], g[1]))   # aligned device arrays still work
+
+
+@pytest.mark.gpu
+@pytest.mark.parametrize("wrapper", ["ShadowsRayTraced", "VolumetricLighting", "DeferredLighting", "GBuffer", "Transparency", "LightsAndSkybox"])
+def test_gpu_wrappers_reject_a_jitter_without_two_components(wrapper):
+    """The library reads taaJitter[0] and [1]: a one-element jitter is a ValueError before it reaches the library, and the
+    context renders the same image afterwards."""
+    scene, cam, shadows = setup("cornell")
+    W, H = 24, 16
+    frame = scenes.camera_frame(cam, W, H)
+    with PathTracer(16, 16) as pt:
+        pt.SetScene(scene)
+        pt.SetPointShadows(shadows, [16, 16])
+        pt.RenderPointShadows()
+        gb = pt.GBuffer(frame, W, H)
+        lit = pt.DeferredLighting(frame, *gb[:5], settings=deferred_settings(1, 0, 0))
+
+        def lights_and_skybox(jitter):   # draws into the G-buffer pass's images and the lit image: render both again first
+            pt.GBuffer(frame, W, H, download=False)
+            pt.DeferredLighting(frame, *gb[:5], settings=deferred_settings(1, 0, 0), download=False)
+            return pt.LightsAndSkybox(frame, jitter=jitter)
+        call = {
+            "ShadowsRayTraced": lambda j: pt.ShadowsRayTraced(frame, gb[0], gb[1], 0, samples=2, jitter=j)[0],
+            "VolumetricLighting": lambda j: pt.VolumetricLighting(frame, gb[0], W, H, jitter=j),
+            "DeferredLighting": lambda j: pt.DeferredLighting(frame, *gb[:5], settings=deferred_settings(1, 0, 0), jitter=j),
+            "GBuffer": lambda j: np.concatenate([a.reshape(H, W, -1) for a in pt.GBuffer(frame, W, H, jitter=j)], -1),
+            "Transparency": lambda j: pt.Transparency(frame, gb[0], jitter=j, color=lit.copy()),
+            "LightsAndSkybox": lights_and_skybox,
+        }[wrapper]
+        want = call(JITTER)
+        with pytest.raises(ValueError, match="jitter has two components"):
+            call((0.01,))
+        assert np.array_equal(canon(call(JITTER)), canon(want))

@@ -287,7 +287,7 @@ def test_gpu_errors_leave_the_context_working():
         pt.SetScene(scene)
         g, lit = ssr_gbuffer(pt, scene, frame, W, H)
         good = pt.Ssr(frame, *g[:4], color=lit)
-        gb, keep, _ = PathTracer._gbuffer([g[0], g[1], g[2], g[3], None, lit], [1, 2, 3, 2, 3, 4])
+        gb, _, keep = PathTracer._gbuffer([g[0], g[1], g[2], g[3], None, lit], [1, 2, 3, 2, 3, 4])
         sst = capi.default_ssr_settings()
 
         def ssr_rc(f=fr, s=sst, gg=None, source=capi.LIT_SOURCE_ARRAY, color=lit.ctypes.data):
