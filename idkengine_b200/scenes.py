@@ -525,3 +525,18 @@ def load_gltf_geometry(path):
 
 def camera_frame(cam, width, height):
     return make_per_frame_data(cam["position"], cam["view_dir"], width, height, cam.get("fov_y_deg", 102.0))
+
+
+# --------------------------------------------------------------------------- lights and point shadows
+# The engine's three startup lights (SRC/Application.cs:487-498): (position, colour, radius).
+STARTUP_LIGHTS = [((-4.5, 5.7, -2.0), (429.8974, 22.459948, 28.425867), 0.3),
+                  ((-0.5, 5.7, -2.0), (8.773416, 506.7525, 28.425867), 0.3),
+                  ((4.5, 5.7, -2.0), (8.773416, 22.459948, 533.77466), 0.3)]
+
+
+def point_shadows(specs):
+    """[(position, near, far, light index)] -> GpuPointShadow array (every other field zero)."""
+    s = np.zeros(len(specs), gt.GpuPointShadow)
+    for i, (p, n, f, li) in enumerate(specs):
+        s[i]["Position"], s[i]["NearPlane"], s[i]["FarPlane"], s[i]["LightIndex"] = p, n, f, li
+    return s

@@ -253,11 +253,17 @@ def camera_rays(frame, width, height):
     return rays
 
 
-def synth_gbuffer(pt, scene, frame, width, height):
-    """The G-buffer attachments ConeTracer.Compute reads (depth, octahedral normal, metallic/roughness), synthesised from the
-    path tracer's first hit on the GPU (`pt.TraceRays`) for scenes that have no rasteriser behind them (SURVEY 8d config 5)."""
-    rays = camera_rays(frame, width, height)
-    hits, _ = pt.TraceRays(rays)
+def encode_unit_vec(n):
+    """EncodeUnitVec (Compression.glsl:54-61): unit vectors [..., 3] -> octahedral (x, y) in [0, 1], computed in n's precision
+    and returned as float32."""
+    m = n / np.sum(np.abs(n), -1, keepdims=True)
+    wrap = (1.0 - np.abs(m[..., [1, 0]])) * np.where(m[..., :2] < 0, -1.0, 1.0)
+    return (np.where((m[..., 2] > 0)[..., None], m[..., :2], wrap) * 0.5 + 0.5).astype(np.float32)
+
+
+def gbuffer_from_hits(scene, frame, rays, hits, width, height):
+    """The G-buffer attachments ConeTracer.Compute reads, from first hits of camera rays: depth = ProjView-projected hit point
+    (1.0 = sky), normal = octahedral geometric normal facing the camera, metallic/roughness from the hit material."""
     hit = hits["TriangleId"] != 0xFFFFFFFF
     o = rays["Origin"].astype(np.float64)
     d = rays["Direction"].astype(np.float64)
@@ -276,14 +282,19 @@ def synth_gbuffer(pt, scene, frame, width, height):
     p0, p1, p2 = pnt("X"), pnt("Y"), pnt("Z")
     n = np.cross(p1 - p0, p2 - p0)
     inv = scene.mesh_transforms["InvModelMatrix"][hits["MeshTransformId"]][:, :, :3].astype(np.float64)
-    n = np.einsum("nji,nj->ni", inv, n)
+    n = np.einsum("nji,nj->ni", inv, n)                                # transpose(inv) * n
     n /= np.maximum(np.linalg.norm(n, axis=1, keepdims=True), 1e-30)
     n = np.where((np.sum(n * d, 1) > 0)[:, None], -n, n)
-    m = n / np.sum(np.abs(n), 1, keepdims=True)                        # EncodeUnitVec (Compression.glsl:54-61)
-    wrap = (1.0 - np.abs(m[:, [1, 0]])) * np.where(m[:, :2] < 0, -1.0, 1.0)
-    xy = np.where((m[:, 2] > 0)[:, None], m[:, :2], wrap)
-    nrg = (xy * 0.5 + 0.5).astype(np.float32)
+    nrg = encode_unit_vec(n)
     mesh = scene.meshes[tri["MeshId"]]
     mat = scene.materials[mesh["MaterialId"]]
     mr = np.stack([np.clip(mat["MetallicFactor"] + mesh["SpecularBias"], 0, 1), np.clip(mat["RoughnessFactor"] + mesh["RoughnessBias"], 0, 1)], 1).astype(np.float32)
     return depth.reshape(height, width), nrg.reshape(height, width, 2), mr.reshape(height, width, 2)
+
+
+def synth_gbuffer(pt, scene, frame, width, height):
+    """gbuffer_from_hits for the path tracer's first hit on the GPU (`pt.TraceRays`), for scenes that have no rasteriser behind
+    them (SURVEY 8d config 5)."""
+    rays = camera_rays(frame, width, height)
+    hits, _ = pt.TraceRays(rays)
+    return gbuffer_from_hits(scene, frame, rays, hits, width, height)

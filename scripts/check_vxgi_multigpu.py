@@ -27,9 +27,8 @@ frame = scenes.camera_frame(cam, w, h)
 with PathTracer(64, 64, device=local) as pt:
     pt.SetScene(scene)
     depth, nrg, mr = vxgi.synth_gbuffer(pt, scene, frame, w, h)
-scene.add_light((-4.5, 5.7, -2.0), (429.8974, 22.459948, 28.425867), 0.3)
-scene.add_light((-0.5, 5.7, -2.0), (8.773416, 506.7525, 28.425867), 0.3)
-scene.add_light((4.5, 5.7, -2.0), (8.773416, 22.459948, 533.77466), 0.3)
+for light in scenes.STARTUP_LIGHTS:
+    scene.add_light(*light)
 with vxgi.Voxelizer(size, device=local) as vx:
     vx.SetScene(scene)
     multigpu.voxelize_multi_gpu(vx, rank, world, dev)          # warm-up (allocations, NCCL channels)

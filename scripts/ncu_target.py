@@ -5,7 +5,7 @@ import sys
 
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import bench  # noqa: E402
-from idkengine_b200 import capi, vxgi  # noqa: E402
+from idkengine_b200 import capi, scenes, vxgi  # noqa: E402
 from idkengine_b200.pathtracer import PathTracer  # noqa: E402
 
 what = sys.argv[1] if len(sys.argv) > 1 else "pt"
@@ -21,9 +21,8 @@ with PathTracer(args.width, args.height, s) as pt:
         pt.Compute()
     else:
         depth, nrg, mr = vxgi.synth_gbuffer(pt, scene, frame, args.width, args.height)
-        scene.add_light((-4.5, 5.7, -2.0), (429.8974, 22.459948, 28.425867), 0.3)
-        scene.add_light((-0.5, 5.7, -2.0), (8.773416, 506.7525, 28.425867), 0.3)
-        scene.add_light((4.5, 5.7, -2.0), (8.773416, 22.459948, 533.77466), 0.3)
+        for light in scenes.STARTUP_LIGHTS:
+            scene.add_light(*light)
         with vxgi.Voxelizer(384) as vx:
             vx.SetScene(scene)
             vx.Render()

@@ -85,9 +85,8 @@ def sort_ab():
 
 def config5():
     scene, cam = scenes.atrium(262144)
-    scene.add_light((-4.5, 5.7, -2.0), (429.8974, 22.459948, 28.425867), 0.3)    # Application.cs:488-490
-    scene.add_light((-0.5, 5.7, -2.0), (8.773416, 506.7525, 28.425867), 0.3)
-    scene.add_light((4.5, 5.7, -2.0), (8.773416, 22.459948, 533.77466), 0.3)
+    for light in scenes.STARTUP_LIGHTS:
+        scene.add_light(*light)
     w, h = 1920, 1080
     frame = scenes.camera_frame(cam, w, h)
     depth, nrg, mr = ol.synth_gbuffer(scene, frame, w, h)

@@ -116,9 +116,7 @@ scene4.add_light((0.0, 1.6, 0.3), (6.0, 5.5, 5.0), 0.2)
 scene4.add_light((-0.6, 0.5, 0.6), (0.5, 0.8, 3.0), 0.1)
 scene4.add_light((0.5, 1.2, 0.8), (1.0, 0.4, 0.3), 0.15)
 scene4.lights["PointShadowIndex"][:] = [1, 0, -1]
-sh4 = np.zeros(2, gt.GpuPointShadow)
-for i, li in enumerate((1, 0)):
-    sh4[i]["Position"], sh4[i]["NearPlane"], sh4[i]["FarPlane"], sh4[i]["LightIndex"] = scene4.lights[li]["Position"], 0.1, 60.0, li
+sh4 = scenes.point_shadows([(scene4.lights[li]["Position"], 0.1, 60.0, li) for li in (1, 0)])
 gw, gh = 37, 23
 f4 = scenes.camera_frame(cam4, gw, gh)
 with PathTracer(16, 16) as pt:

@@ -20,7 +20,7 @@ import numpy as np  # noqa: E402
 
 from idkengine_b200 import host, scenes  # noqa: E402
 from idkengine_b200.pathtracer import PathTracer  # noqa: E402
-from time_gbuffer import card  # noqa: E402
+from timing_lib import card, write_out  # noqa: E402
 
 
 def atrium_model(n):
@@ -78,9 +78,7 @@ def main():
             result["runs"].append(run)
             print(json.dumps(run), flush=True)
     print(json.dumps(result))
-    if a.out:
-        with open(a.out, "w") as f:
-            json.dump(result, f, indent=1)
+    write_out(a.out, result)
 
 
 if __name__ == "__main__":

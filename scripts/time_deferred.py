@@ -14,27 +14,17 @@ algorithmic bytes / kernel time, against the 3.35 TB/s HBM3 bound of the H100 SX
 import argparse
 import json
 import os
-import subprocess
 import sys
 import time
 
 sys.path.insert(0, os.path.join(os.path.dirname(os.path.abspath(__file__)), ".."))
 import numpy as np  # noqa: E402
 
-from idkengine_b200 import capi, gpu_types as gt, scenes, vxgi  # noqa: E402
+from idkengine_b200 import capi, scenes, vxgi  # noqa: E402
 from idkengine_b200.pathtracer import PathTracer  # noqa: E402
+from timing_lib import card, shadowed_atrium, write_out  # noqa: E402
 
-LIGHTS = [((-4.5, 5.7, -2.0), (429.8974, 22.459948, 28.425867), 0.3),
-          ((-0.5, 5.7, -2.0), (8.773416, 506.7525, 28.425867), 0.3),
-          ((4.5, 5.7, -2.0), (8.773416, 22.459948, 533.77466), 0.3)]
 HBM_BYTES_PER_S = 3.35e12
-
-
-def card():
-    q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"],
-                       capture_output=True, text=True, check=True).stdout.strip().splitlines()[0]
-    name, power, clock = (s.strip() for s in q.split(","))
-    return dict(name=name, power_limit=power, max_sm_clock=clock)
 
 
 def algorithmic_bytes(pas, w, h, lights=0, shadow_sizes=(), vxgi_on=False):
@@ -67,20 +57,13 @@ def main():
     ap.add_argument("--out", default=None, help="also write the JSON result to this file")
     a = ap.parse_args()
 
-    scene, cam = scenes.atrium(a.tris)
-    scene.lights = scene.lights[:0]
-    for p, c, r in LIGHTS:
-        scene.add_light(p, c, r)
-    scene.lights["PointShadowIndex"][:] = np.arange(len(LIGHTS))
-    shadows = np.zeros(len(LIGHTS), gt.GpuPointShadow)
-    for i, (p, c, r) in enumerate(LIGHTS):
-        shadows[i]["Position"], shadows[i]["NearPlane"], shadows[i]["FarPlane"], shadows[i]["LightIndex"] = p, r, 60.0, i
+    scene, cam, shadows = shadowed_atrium(a.tris)
     size, W, H = 512, 1920, 1080
 
-    out = dict(card=card(), triangles=int(len(scene.blas_triangles)), shadows=len(LIGHTS), shadow_map_size=size, size=[W, H])
+    out = dict(card=card(), triangles=int(len(scene.blas_triangles)), shadows=len(scenes.STARTUP_LIGHTS), shadow_map_size=size, size=[W, H])
     with PathTracer(64, 64) as pt:
         pt.SetScene(scene)
-        pt.SetPointShadows(shadows, [size] * len(LIGHTS))
+        pt.SetPointShadows(shadows, [size] * len(scenes.STARTUP_LIGHTS))
         pt.RenderPointShadows()
         frame = scenes.camera_frame(cam, W, H)
         depth, nrg, mr = vxgi.synth_gbuffer(pt, scene, frame, W, H)
@@ -104,14 +87,11 @@ def main():
                               lambda: pt.last_deferred_ms, a.reps)
             _, c_dev = timed(lambda: pt.DeferredLighting(frame, *dev, settings=st, jitter=jitter, indirect=gi_dev if vx else None,
                                                          download=False), lambda: pt.last_deferred_ms, a.reps)
-            nb = algorithmic_bytes("deferred", W, H, len(LIGHTS), [size] * len(LIGHTS), bool(vx))
+            nb = algorithmic_bytes("deferred", W, H, len(scenes.STARTUP_LIGHTS), [size] * len(scenes.STARTUP_LIGHTS), bool(vx))
             out[f"deferred pcf vxgi={vx}"] = dict(kernel_ms=k, call_ms_host_arrays=c_host, call_ms_on_device=c_dev, algorithmic_bytes=nb,
                                                   gb_per_s=nb / (k * 1e-3) / 1e9, share_of_hbm_bound=nb / HBM_BYTES_PER_S / (k * 1e-3))
     print("DEFERRED", json.dumps(out))
-    if a.out:
-        os.makedirs(os.path.dirname(a.out) or ".", exist_ok=True)
-        with open(a.out, "w") as f:
-            json.dump(out, f, indent=1)
+    write_out(a.out, out)
 
 
 if __name__ == "__main__":

@@ -13,7 +13,6 @@ in the same run.
 import argparse
 import json
 import os
-import subprocess
 import sys
 
 sys.path.insert(0, os.path.join(os.path.dirname(os.path.abspath(__file__)), ".."))
@@ -21,18 +20,7 @@ import numpy as np  # noqa: E402
 
 from idkengine_b200 import capi, gpu_types as gt, scenes  # noqa: E402
 from idkengine_b200.pathtracer import PathTracer  # noqa: E402
-
-LIGHTS = [((-4.5, 5.7, -2.0), (429.8974, 22.459948, 28.425867), 0.3),
-          ((-0.5, 5.7, -2.0), (8.773416, 506.7525, 28.425867), 0.3),
-          ((4.5, 5.7, -2.0), (8.773416, 22.459948, 533.77466), 0.3)]
-JITTER = (0.0003, -0.0002)
-
-
-def card():
-    q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"],
-                       capture_output=True, text=True, check=True).stdout.strip().splitlines()[0]
-    name, power, clock = (s.strip() for s in q.split(","))
-    return dict(name=name, power_limit=power, max_sm_clock=clock)
+from timing_lib import JITTER, card, median_ms, shadowed_atrium, write_out  # noqa: E402
 
 
 def primary_rays(frame, w, h):
@@ -50,11 +38,6 @@ def primary_rays(frame, w, h):
     return r
 
 
-def median_ms(fn, reps):
-    t = [fn() for _ in range(reps + 2)]
-    return float(np.median(t[2:]))
-
-
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--tris", type=int, default=262144)
@@ -62,20 +45,13 @@ def main():
     ap.add_argument("--out", default=None, help="also write the JSON result to this file")
     a = ap.parse_args()
 
-    scene, cam = scenes.atrium(a.tris)
-    scene.lights = scene.lights[:0]
-    for p, c, r in LIGHTS:
-        scene.add_light(p, c, r)
-    scene.lights["PointShadowIndex"][:] = np.arange(len(LIGHTS))
-    shadows = np.zeros(len(LIGHTS), gt.GpuPointShadow)
-    for i, (p, c, r) in enumerate(LIGHTS):
-        shadows[i]["Position"], shadows[i]["NearPlane"], shadows[i]["FarPlane"], shadows[i]["LightIndex"] = p, r, 60.0, i
+    scene, cam, shadows = shadowed_atrium(a.tris)
 
     out = dict(card=card(), triangles=int(len(scene.blas_triangles)), reps=a.reps)
     with PathTracer(64, 64) as pt:
         pt.SetScene(scene)
         pt.SetSky((0.6, 0.7, 0.9))
-        pt.SetPointShadows(shadows, [512] * len(LIGHTS))
+        pt.SetPointShadows(shadows, [512] * len(scenes.STARTUP_LIGHTS))
         pt.RenderPointShadows()
         for W, H in ((1920, 1080), (1152, 648)):
             frame = scenes.camera_frame(cam, W, H)
@@ -113,10 +89,7 @@ def main():
             row["raster_frame_kernel_ms"] = frame_ms
             out[f"{W}x{H}"] = row
     print("GBUFFER", json.dumps(out))
-    if a.out:
-        os.makedirs(os.path.dirname(a.out) or ".", exist_ok=True)
-        with open(a.out, "w") as f:
-            json.dump(out, f, indent=1)
+    write_out(a.out, out)
 
 
 if __name__ == "__main__":

@@ -21,7 +21,7 @@ import numpy as np  # noqa: E402
 
 from idkengine_b200 import capi, scenes  # noqa: E402
 from idkengine_b200.pathtracer import PathTracer  # noqa: E402
-from time_gbuffer import JITTER, LIGHTS, card, median_ms  # noqa: E402
+from timing_lib import JITTER, card, median_ms, write_out  # noqa: E402
 
 
 def light_sets(scene, cam):
@@ -33,7 +33,7 @@ def light_sets(scene, cam):
     many = [near] + [(tuple(eye + vd * rng.uniform(0.5, 12.0) + rng.uniform(-3.0, 3.0, 3)), tuple(rng.uniform(0.5, 60.0, 3)),
                       float(rng.uniform(0.02, 0.6))) for _ in range(255)]
     out = {}
-    for name, lights in (("startup", LIGHTS), ("startup_near", LIGHTS + [near]), ("256", many)):
+    for name, lights in (("startup", scenes.STARTUP_LIGHTS), ("startup_near", scenes.STARTUP_LIGHTS + [near]), ("256", many)):
         s = copy.deepcopy(scene)
         s.lights = s.lights[:0]
         for p, c, r in lights:
@@ -88,9 +88,7 @@ def main():
         cov[name] = dict(light=round(float((winner >= 0).mean()), 4), sky=round(float((winner == lo.SKY).mean()), 4))
     result["coverage_480x270"] = cov
     print(json.dumps(dict(card=result["card"], coverage_480x270=cov)), flush=True)
-    if a.out:
-        with open(a.out, "w") as f:
-            json.dump(result, f, indent=1)
+    write_out(a.out, result)
 
 
 if __name__ == "__main__":

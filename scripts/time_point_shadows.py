@@ -9,25 +9,14 @@ warm-up calls); Grays/s = traced texels / kernel time.
 import argparse
 import json
 import os
-import subprocess
 import sys
 
 sys.path.insert(0, os.path.join(os.path.dirname(os.path.abspath(__file__)), ".."))
 import numpy as np  # noqa: E402
 
-from idkengine_b200 import gpu_types as gt, scenes, vxgi  # noqa: E402
+from idkengine_b200 import scenes, vxgi  # noqa: E402
 from idkengine_b200.pathtracer import PathTracer  # noqa: E402
-
-LIGHTS = [((-4.5, 5.7, -2.0), (429.8974, 22.459948, 28.425867), 0.3),
-          ((-0.5, 5.7, -2.0), (8.773416, 506.7525, 28.425867), 0.3),
-          ((4.5, 5.7, -2.0), (8.773416, 22.459948, 533.77466), 0.3)]
-
-
-def card():
-    q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"],
-                       capture_output=True, text=True, check=True).stdout.strip().splitlines()[0]
-    name, power, clock = (s.strip() for s in q.split(","))
-    return dict(name=name, power_limit=power, max_sm_clock=clock)
+from timing_lib import card, shadowed_atrium, write_out  # noqa: E402
 
 
 def main():
@@ -38,21 +27,14 @@ def main():
     ap.add_argument("--out", default=None, help="also write the JSON result to this file")
     a = ap.parse_args()
 
-    scene, cam = scenes.atrium(a.tris)
-    scene.lights = scene.lights[:0]
-    for p, c, r in LIGHTS:
-        scene.add_light(p, c, r)
-    scene.lights["PointShadowIndex"][:] = np.arange(len(LIGHTS))
-    shadows = np.zeros(len(LIGHTS), gt.GpuPointShadow)
-    for i, (p, c, r) in enumerate(LIGHTS):
-        shadows[i]["Position"], shadows[i]["NearPlane"], shadows[i]["FarPlane"] = p, r, 60.0
+    scene, cam, shadows = shadowed_atrium(a.tris)
 
-    out = dict(card=card(), triangles=int(len(scene.blas_triangles)), lights=len(LIGHTS))
+    out = dict(card=card(), triangles=int(len(scene.blas_triangles)), lights=len(scenes.STARTUP_LIGHTS))
     med = lambda xs: float(np.median(xs))  # noqa: E731
     with PathTracer(64, 64) as pt:
         pt.SetScene(scene)
         for n in (512, 1024):
-            pt.SetPointShadows(shadows, [n] * len(LIGHTS))
+            pt.SetPointShadows(shadows, [n] * len(scenes.STARTUP_LIGHTS))
             for count in (1, 3):
                 for label, mask, faces in (("all faces", None, 6), ("3-face mask", 0b010101, 3)):
                     masks = None if mask is None else [mask] * count
@@ -60,7 +42,7 @@ def main():
                     texels = faces * n * n * count
                     out[f"render N={n} shadows={count} {label}"] = dict(kernel_ms=med(ms), grays_per_s=texels / (med(ms) * 1e-3) / 1e9)
         # the engine's maps for the voxeliser comparison
-        pt.SetPointShadows(shadows, [512] * len(LIGHTS))
+        pt.SetPointShadows(shadows, [512] * len(scenes.STARTUP_LIGHTS))
         render_ms = med([pt.RenderPointShadows() for _ in range(a.reps + 2)][2:])
         with vxgi.Voxelizer(a.grid) as vx:
             vx.SetScene(scene)
@@ -73,10 +55,7 @@ def main():
             res["shadow maps"]["render_ms_3x512"] = render_ms
             out[f"voxelize {a.grid}^3"] = res
     print("POINT_SHADOWS", json.dumps(out))
-    if a.out:
-        os.makedirs(os.path.dirname(a.out) or ".", exist_ok=True)
-        with open(a.out, "w") as f:
-            json.dump(out, f, indent=1)
+    write_out(a.out, out)
 
 
 if __name__ == "__main__":

@@ -19,7 +19,7 @@ import numpy as np  # noqa: E402
 
 from idkengine_b200 import capi  # noqa: E402
 from idkengine_b200.pathtracer import PathTracer  # noqa: E402
-from time_gbuffer import card, median_ms  # noqa: E402
+from timing_lib import card, median_ms, write_out  # noqa: E402
 
 
 def main():
@@ -52,9 +52,7 @@ def main():
             result["equirect"].append(run)
             print(json.dumps(run), flush=True)
     print(json.dumps(dict(card=result["card"])), flush=True)
-    if a.out:
-        with open(a.out, "w") as f:
-            json.dump(result, f, indent=1)
+    write_out(a.out, result)
 
 
 if __name__ == "__main__":

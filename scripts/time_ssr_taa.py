@@ -14,7 +14,6 @@ bytes / kernel time, against the 3.35 TB/s HBM3 bound of the H100 SXM data sheet
 import argparse
 import json
 import os
-import subprocess
 import sys
 import time
 
@@ -23,15 +22,9 @@ import numpy as np  # noqa: E402
 
 from idkengine_b200 import capi, scenes, vxgi  # noqa: E402
 from idkengine_b200.pathtracer import PathTracer  # noqa: E402
+from timing_lib import card, write_out  # noqa: E402
 
 HBM_BYTES_PER_S = 3.35e12
-
-
-def card():
-    q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"],
-                       capture_output=True, text=True, check=True).stdout.strip().splitlines()[0]
-    name, power, clock = (s.strip() for s in q.split(","))
-    return dict(name=name, power_limit=power, max_sm_clock=clock)
 
 
 def algorithmic_bytes(pas, rw, rh, W=0, H=0):
@@ -89,10 +82,7 @@ def main():
             out[f"taa {rw}x{rh} -> {W}x{H}"] = dict(kernel_ms=k, call_ms=c, algorithmic_bytes=nb, gb_per_s=nb / (k * 1e-3) / 1e9,
                                                     share_of_hbm_bound=nb / HBM_BYTES_PER_S / (k * 1e-3))
     print("SSR_TAA", json.dumps(out))
-    if a.out:
-        os.makedirs(os.path.dirname(a.out) or ".", exist_ok=True)
-        with open(a.out, "w") as f:
-            json.dump(out, f, indent=1)
+    write_out(a.out, out)
 
 
 if __name__ == "__main__":

@@ -21,9 +21,9 @@ sys.path.insert(0, os.path.join(os.path.dirname(os.path.abspath(__file__)), ".."
 sys.path.insert(0, os.path.join(os.path.dirname(os.path.abspath(__file__)), "..", "tests"))
 import numpy as np  # noqa: E402
 
-from idkengine_b200 import capi, gpu_types as gt, scenes, vxgi  # noqa: E402
+from idkengine_b200 import capi, scenes, vxgi  # noqa: E402
 from idkengine_b200.pathtracer import PathTracer  # noqa: E402
-from time_gbuffer import JITTER, LIGHTS, card, median_ms  # noqa: E402
+from timing_lib import JITTER, card, median_ms, shadowed_atrium, write_out  # noqa: E402
 
 
 def main():
@@ -33,14 +33,7 @@ def main():
     ap.add_argument("--out", default=None, help="also write the JSON result to this file")
     a = ap.parse_args()
 
-    scene, cam = scenes.atrium(a.tris)
-    scene.lights = scene.lights[:0]
-    for p, c, r in LIGHTS:
-        scene.add_light(p, c, r)
-    scene.lights["PointShadowIndex"][:] = np.arange(len(LIGHTS))
-    shadows = np.zeros(len(LIGHTS), gt.GpuPointShadow)
-    for i, (p, c, r) in enumerate(LIGHTS):
-        shadows[i]["Position"], shadows[i]["NearPlane"], shadows[i]["FarPlane"], shadows[i]["LightIndex"] = p, r, 60.0, i
+    scene, cam, shadows = shadowed_atrium(a.tris)
     blended = int((scene.materials["AlphaCutoff"] == 2.0).sum())
 
     out = dict(card=card(), triangles=int(len(scene.blas_triangles)), blended_materials=blended, reps=a.reps)
@@ -51,7 +44,7 @@ def main():
     with PathTracer(64, 64) as pt, vxgi.Voxelizer(256, tuple(lo), tuple(hi)) as vx:
         pt.SetScene(scene)
         pt.SetSky((0.6, 0.7, 0.9))
-        pt.SetPointShadows(shadows, [512] * len(LIGHTS))
+        pt.SetPointShadows(shadows, [512] * len(scenes.STARTUP_LIGHTS))
         pt.RenderPointShadows()
         vx.SetScene(unshadowed)
         vx.Render()
@@ -108,10 +101,7 @@ def main():
                                        mean_layers_where_any=float(counts[counts > 0].mean()) if (counts > 0).any() else 0.0,
                                        max_layers=int(counts.max()))
     print("TRANSPARENCY", json.dumps(out))
-    if a.out:
-        os.makedirs(os.path.dirname(a.out) or ".", exist_ok=True)
-        with open(a.out, "w") as f:
-            json.dump(out, f, indent=1)
+    write_out(a.out, out)
 
 
 if __name__ == "__main__":

@@ -13,27 +13,17 @@ depth (written, then read), the presentation image and the cube maps; GB/s = alg
 import argparse
 import json
 import os
-import subprocess
 import sys
 import time
 
 sys.path.insert(0, os.path.join(os.path.dirname(os.path.abspath(__file__)), ".."))
 import numpy as np  # noqa: E402
 
-from idkengine_b200 import capi, gpu_types as gt, scenes, vxgi  # noqa: E402
+from idkengine_b200 import capi, scenes, vxgi  # noqa: E402
 from idkengine_b200.pathtracer import PathTracer  # noqa: E402
+from timing_lib import card, shadowed_atrium, write_out  # noqa: E402
 
-LIGHTS = [((-4.5, 5.7, -2.0), (429.8974, 22.459948, 28.425867), 0.3),
-          ((-0.5, 5.7, -2.0), (8.773416, 506.7525, 28.425867), 0.3),
-          ((4.5, 5.7, -2.0), (8.773416, 22.459948, 533.77466), 0.3)]
 HBM_BYTES_PER_S = 3.35e12
-
-
-def card():
-    q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"],
-                       capture_output=True, text=True, check=True).stdout.strip().splitlines()[0]
-    name, power, clock = (s.strip() for s in q.split(","))
-    return dict(name=name, power_limit=power, max_sm_clock=clock)
 
 
 def main():
@@ -43,21 +33,14 @@ def main():
     ap.add_argument("--out", default=None, help="also write the JSON result to this file")
     a = ap.parse_args()
 
-    scene, cam = scenes.atrium(a.tris)
-    scene.lights = scene.lights[:0]
-    for p, c, r in LIGHTS:
-        scene.add_light(p, c, r)
-    scene.lights["PointShadowIndex"][:] = np.arange(len(LIGHTS))
-    shadows = np.zeros(len(LIGHTS), gt.GpuPointShadow)
-    for i, (p, c, r) in enumerate(LIGHTS):
-        shadows[i]["Position"], shadows[i]["NearPlane"], shadows[i]["FarPlane"], shadows[i]["LightIndex"] = p, r, 60.0, i
+    scene, cam, shadows = shadowed_atrium(a.tris)
     size = 512
 
-    out = dict(card=card(), triangles=int(len(scene.blas_triangles)), shadows=len(LIGHTS), shadow_map_size=size)
+    out = dict(card=card(), triangles=int(len(scene.blas_triangles)), shadows=len(scenes.STARTUP_LIGHTS), shadow_map_size=size)
     med = lambda xs: float(np.median(xs))  # noqa: E731
     with PathTracer(64, 64) as pt:
         pt.SetScene(scene)
-        pt.SetPointShadows(shadows, [size] * len(LIGHTS))
+        pt.SetPointShadows(shadows, [size] * len(scenes.STARTUP_LIGHTS))
         pt.RenderPointShadows()
         for W, H in ((1920, 1080), (3840, 2160)):
             frame = scenes.camera_frame(cam, W, H)
@@ -74,15 +57,12 @@ def main():
                         kernel.append(pt.last_volumetric_ms)
                     kernel, call = kernel[2:], call[2:]
                     w, h = int(np.float32(W) * np.float32(scale)), int(np.float32(H) * np.float32(scale))
-                    nbytes = 2 * W * H * 4 + 2 * w * h * 12 + W * H * 8 + len(LIGHTS) * 6 * size * size * 2
+                    nbytes = 2 * W * H * 4 + 2 * w * h * 12 + W * H * 8 + len(scenes.STARTUP_LIGHTS) * 6 * size * size * 2
                     out[f"{W}x{H} scale={scale} samples={samples}"] = dict(
                         render_size=[w, h], kernel_ms=med(kernel), call_ms=med(call), algorithmic_bytes=nbytes,
                         gb_per_s=nbytes / (med(kernel) * 1e-3) / 1e9, share_of_hbm_bound=nbytes / HBM_BYTES_PER_S / (med(kernel) * 1e-3))
     print("VOLUMETRIC", json.dumps(out))
-    if a.out:
-        os.makedirs(os.path.dirname(a.out) or ".", exist_ok=True)
-        with open(a.out, "w") as f:
-            json.dump(out, f, indent=1)
+    write_out(a.out, out)
 
 
 if __name__ == "__main__":

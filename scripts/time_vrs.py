@@ -14,25 +14,14 @@ card name and power limit are read in the same run.
 import argparse
 import json
 import os
-import subprocess
 import sys
 
 sys.path.insert(0, os.path.join(os.path.dirname(os.path.abspath(__file__)), ".."))
 import numpy as np  # noqa: E402
 
-from idkengine_b200 import capi, gpu_types as gt, scenes, vxgi  # noqa: E402
+from idkengine_b200 import capi, scenes, vxgi  # noqa: E402
 from idkengine_b200.pathtracer import PathTracer  # noqa: E402
-
-LIGHTS = [((-4.5, 5.7, -2.0), (429.8974, 22.459948, 28.425867), 0.3),
-          ((-0.5, 5.7, -2.0), (8.773416, 506.7525, 28.425867), 0.3),
-          ((4.5, 5.7, -2.0), (8.773416, 22.459948, 533.77466), 0.3)]
-
-
-def card():
-    q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"],
-                       capture_output=True, text=True, check=True).stdout.strip().splitlines()[0]
-    name, power, clock = (s.strip() for s in q.split(","))
-    return dict(name=name, power_limit=power, max_sm_clock=clock)
+from timing_lib import card, shadowed_atrium, write_out  # noqa: E402
 
 
 def main():
@@ -43,20 +32,13 @@ def main():
     ap.add_argument("--out", default=None, help="also write the JSON result to this file")
     a = ap.parse_args()
 
-    scene, cam = scenes.atrium(a.tris)
-    scene.lights = scene.lights[:0]
-    for p, c, r in LIGHTS:
-        scene.add_light(p, c, r)
-    scene.lights["PointShadowIndex"][:] = np.arange(len(LIGHTS))
-    shadows = np.zeros(len(LIGHTS), gt.GpuPointShadow)
-    for i, (p, c, r) in enumerate(LIGHTS):
-        shadows[i]["Position"], shadows[i]["NearPlane"], shadows[i]["FarPlane"], shadows[i]["LightIndex"] = p, r, 60.0, i
+    scene, cam, shadows = shadowed_atrium(a.tris)
     size, W, H = 512, 1920, 1080
 
-    out = dict(card=card(), triangles=int(len(scene.blas_triangles)), shadows=len(LIGHTS), shadow_map_size=size, size=[W, H])
+    out = dict(card=card(), triangles=int(len(scene.blas_triangles)), shadows=len(scenes.STARTUP_LIGHTS), shadow_map_size=size, size=[W, H])
     with PathTracer(64, 64) as pt:
         pt.SetScene(scene)
-        pt.SetPointShadows(shadows, [size] * len(LIGHTS))
+        pt.SetPointShadows(shadows, [size] * len(scenes.STARTUP_LIGHTS))
         pt.RenderPointShadows()
         frame = scenes.camera_frame(cam, W, H).copy()
         frame["DeltaRenderTime"] = 1.0 / 60.0
@@ -109,10 +91,7 @@ def main():
                                                       tile_share=share, invocations_over_pixels=frags / (W * H))
         out["classifier rates"] = {f"{capi.VRS_PALETTE[r][0]}x{capi.VRS_PALETTE[r][1]}": float(np.mean(rates == r)) for r in range(5)}
     print("VRS", json.dumps(out))
-    if a.out:
-        os.makedirs(os.path.dirname(a.out) or ".", exist_ok=True)
-        with open(a.out, "w") as f:
-            json.dump(out, f, indent=1)
+    write_out(a.out, out)
 
 
 if __name__ == "__main__":

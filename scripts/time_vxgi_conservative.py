@@ -13,7 +13,6 @@ import argparse
 import copy
 import json
 import os
-import subprocess
 import sys
 
 REPO = os.path.join(os.path.dirname(os.path.abspath(__file__)), "..")
@@ -22,17 +21,9 @@ sys.path.insert(0, os.path.join(REPO, "tests"))
 import numpy as np  # noqa: E402
 
 from idkengine_b200 import scenes, vxgi  # noqa: E402
+from timing_lib import card, write_out  # noqa: E402
 
-LIGHTS = [((-4.5, 5.7, -2.0), (429.8974, 22.459948, 28.425867)), ((-0.5, 5.7, -2.0), (8.773416, 506.7525, 28.425867)),
-          ((4.5, 5.7, -2.0), (8.773416, 22.459948, 533.77466))]
 RULES = {"centre": False, "conservative": True}
-
-
-def card():
-    q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"],
-                       capture_output=True, text=True, check=True).stdout.strip().splitlines()[0]
-    name, power, clock = (s.strip() for s in q.split(","))
-    return dict(name=name, power_limit=power, max_sm_clock=clock)
 
 
 def bench_scene(tris):
@@ -40,8 +31,8 @@ def bench_scene(tris):
     scene, _ = scenes.atrium(tris)
     sc = copy.copy(scene)
     sc.lights = scene.lights.copy()
-    for pos, col in LIGHTS:
-        sc.add_light(pos, col, 0.3)
+    for light in scenes.STARTUP_LIGHTS:
+        sc.add_light(*light)
     return sc
 
 
@@ -81,10 +72,7 @@ def main():
         out["ratio_ms"] = out["conservative"]["voxelize_ms_median"] / out["centre"]["voxelize_ms_median"]
     out["ratio_fragments"] = out["oracle_fragments"]["conservative"] / out["oracle_fragments"]["centre"]
     print("VXGI_CONSERVATIVE", json.dumps(out))
-    if a.out:
-        os.makedirs(os.path.dirname(a.out) or ".", exist_ok=True)
-        with open(a.out, "w") as f:
-            json.dump(out, f, indent=1)
+    write_out(a.out, out)
 
 
 if __name__ == "__main__":

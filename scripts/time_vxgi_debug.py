@@ -27,17 +27,9 @@ import numpy as np  # noqa: E402
 
 from idkengine_b200 import build, scenes, vxgi  # noqa: E402
 from idkengine_b200.pathtracer import PathTracer  # noqa: E402
+from timing_lib import card, write_out  # noqa: E402
 
-LIGHTS = [((-4.5, 5.7, -2.0), (429.8974, 22.459948, 28.425867)), ((-0.5, 5.7, -2.0), (8.773416, 506.7525, 28.425867)),
-          ((4.5, 5.7, -2.0), (8.773416, 22.459948, 533.77466))]
 OUTSIDE = dict(position=(34.0, 24.0, -30.0), view_dir=(-0.7, -0.35, 0.6))   # beyond the +x, +y, -z corner, looking across
-
-
-def card():
-    q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"],
-                       capture_output=True, text=True, check=True).stdout.strip().splitlines()[0]
-    name, power, clock = (s.strip() for s in q.split(","))
-    return dict(name=name, power_limit=power, max_sm_clock=clock)
 
 
 def build_variant(tmp):
@@ -64,8 +56,8 @@ def main():
     scene, cam = scenes.atrium(a.tris)
     sc = copy.copy(scene)
     sc.lights = scene.lights.copy()
-    for pos, col in LIGHTS:
-        sc.add_light(pos, col, 0.3)
+    for light in scenes.STARTUP_LIGHTS:
+        sc.add_light(*light)
     w, h = a.width, a.height
     views = {"bench_camera_inside": scenes.camera_frame(cam, w, h), "outside_across": scenes.camera_frame(OUTSIDE, w, h)}
     out = dict(card=card(), triangles=int(len(sc.blas_triangles)), resolution=f"{w}x{h}", reps=a.reps, warmup=a.warmup, cases=[])
@@ -111,10 +103,7 @@ def main():
                     vx.Dispose()
                     pt.Dispose()
     print("VXGI_DEBUG", json.dumps(out))
-    if a.out:
-        os.makedirs(os.path.dirname(a.out) or ".", exist_ok=True)
-        with open(a.out, "w") as f:
-            json.dump(out, f, indent=1)
+    write_out(a.out, out)
 
 
 if __name__ == "__main__":

@@ -316,39 +316,9 @@ def vx_cone_trace(ci, raw_chain, frame, settings, depth, normal_rg, metal_rough,
 
 
 def synth_gbuffer(scene, frame, width, height):
-    """G-buffer for the cone tracer synthesised from the path tracer's first hit (SURVEY 8d config 5):
-    depth = ProjView-projected hit point (1.0 = sky), normal = octahedral geometric normal facing the camera,
-    metallic/roughness from the hit material."""
+    """vxgi.gbuffer_from_hits for the oracle's first hit through pixel centres (instead of Gui.Test's pixel corners)."""
     rays = gui_test_rays(frame, width, height)
-    # pixel centres instead of Gui.Test's pixel corners
-    hits = trace_rays(scene, rays)
-    hit = hits["TriangleId"] != 0xFFFFFFFF
-    o = rays["Origin"].astype(np.float64)
-    d = rays["Direction"].astype(np.float64)
-    pos = o + d * hits["T"][:, None].astype(np.float64)
-    pv = frame["ProjView"][0].astype(np.float64).reshape(4, 4)      # OpenTK rows: clip = [p,1] @ pv
-    clip = np.concatenate([pos, np.ones((len(pos), 1))], 1) @ pv
-    depth = np.where(hit, clip[:, 2] / clip[:, 3], 1.0).astype(np.float32)
-    depth = np.where(hit & (depth >= 1.0), np.float32(0.999999), depth)
-    tri = scene.blas_triangles[np.where(hit, hits["TriangleId"], 0)]
-    P = scene.positions
-    p0 = np.stack([P["x"][tri["X"]], P["y"][tri["X"]], P["z"][tri["X"]]], 1).astype(np.float64)
-    p1 = np.stack([P["x"][tri["Y"]], P["y"][tri["Y"]], P["z"][tri["Y"]]], 1).astype(np.float64)
-    p2 = np.stack([P["x"][tri["Z"]], P["y"][tri["Z"]], P["z"][tri["Z"]]], 1).astype(np.float64)
-    n = np.cross(p1 - p0, p2 - p0)
-    inv = scene.mesh_transforms["InvModelMatrix"][hits["MeshTransformId"]][:, :, :3].astype(np.float64)   # [N,3,3]
-    n = np.einsum("nji,nj->ni", inv, n)                                # transpose(inv) * n
-    n /= np.maximum(np.linalg.norm(n, axis=1, keepdims=True), 1e-30)
-    n = np.where((np.sum(n * d, 1) > 0)[:, None], -n, n)
-    # EncodeUnitVec (Compression.glsl:54-61)
-    m = n / np.sum(np.abs(n), 1, keepdims=True)
-    wrap = (1.0 - np.abs(m[:, [1, 0]])) * np.where(m[:, :2] < 0, -1.0, 1.0)
-    xy = np.where((m[:, 2] > 0)[:, None], m[:, :2], wrap)
-    nrg = (xy * 0.5 + 0.5).astype(np.float32)
-    mesh = scene.meshes[tri["MeshId"]]
-    mat = scene.materials[mesh["MaterialId"]]
-    mr = np.stack([np.clip(mat["MetallicFactor"] + mesh["SpecularBias"], 0, 1), np.clip(mat["RoughnessFactor"] + mesh["RoughnessBias"], 0, 1)], 1).astype(np.float32)
-    return depth.reshape(height, width), nrg.reshape(height, width, 2), mr.reshape(height, width, 2)
+    return vxgi.gbuffer_from_hits(scene, frame, rays, trace_rays(scene, rays), width, height)
 
 
 def denoise(result, albedo, normal, settings=None, threads=None):

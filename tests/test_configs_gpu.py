@@ -113,9 +113,8 @@ def test_config5_vxgi_384_cubed(atrium_262k):
     """configs[4]: 384^3 rgba16f voxelise + mip chain (9 levels) + cone trace over the 262k atrium with the reference's three
     lights (Application.cs:488-490): fragment count, EVERY level and the 1080p cone-trace image equal the oracle's."""
     scene, cam = scenes.atrium(262144)
-    scene.add_light((-4.5, 5.7, -2.0), (429.8974, 22.459948, 28.425867), 0.3)
-    scene.add_light((-0.5, 5.7, -2.0), (8.773416, 506.7525, 28.425867), 0.3)
-    scene.add_light((4.5, 5.7, -2.0), (8.773416, 22.459948, 533.77466), 0.3)
+    for light in scenes.STARTUP_LIGHTS:
+        scene.add_light(*light)
     ci = vxgi.create_info(384)
     levels, raw, frags = ol.vx_voxelize(scene, ci)
     assert [lv.shape[0] for lv in levels] == [384, 192, 96, 48, 24, 12, 6, 3, 1]

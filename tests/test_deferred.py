@@ -12,23 +12,16 @@ exact properties of both passes (no GPU).
 import numpy as np
 
 import deferred_oracle as do
-from idkengine_b200 import capi, gpu_types as gt, scenes
+import raster_lib as rl
+from idkengine_b200 import capi, scenes, vxgi
 
 W, H = 48, 32
 
 
 def lit_cornell():
     """Three lights; lights 0 and 1 shadowed (crossed indices), light 2 not."""
-    scene, cam = scenes.cornell_1k(threads=1)
-    scene.add_light((0.0, 1.6, 0.3), (6.0, 5.5, 5.0), 0.2)
-    scene.add_light((-0.6, 0.5, 0.6), (0.5, 0.8, 3.0), 0.1)
-    scene.add_light((0.5, 1.2, 0.8), (1.0, 0.4, 0.3), 0.15)
-    scene.lights["PointShadowIndex"][:] = [1, 0, -1]
-    shadows = np.zeros(2, gt.GpuPointShadow)
-    for i, li in enumerate((1, 0)):
-        shadows[i]["Position"], shadows[i]["NearPlane"], shadows[i]["FarPlane"] = scene.lights[li]["Position"], 0.1, 60.0
-        shadows[i]["LightIndex"] = li
-    return scene, cam, shadows
+    scene, cam = rl.lit_cornell(3)
+    return scene, cam, rl.crossed_shadows(scene, 0.1, 0.1)
 
 
 def frame_of(cam):
@@ -54,12 +47,6 @@ def depth_at(f, p):
     return np.float32(clip[2] / clip[3])
 
 
-def encode_unit_vec(n):
-    m = n / np.sum(np.abs(n), -1, keepdims=True)
-    wrap = (1.0 - np.abs(m[..., [1, 0]])) * np.where(m[..., :2] < 0, -1.0, 1.0)
-    return (np.where((m[..., 2] > 0)[..., None], m[..., :2], wrap) * 0.5 + 0.5).astype(np.float32)
-
-
 def decode_unit_vec64(e):
     e = e.astype(np.float64) * 2 - 1
     n = np.stack([e[..., 0], e[..., 1], 1 - np.abs(e[..., 0]) - np.abs(e[..., 1])], -1)
@@ -76,7 +63,7 @@ def walls(f, dist_left, dist_right):
     depth = np.empty((H, W), np.float32)
     depth[:, : W // 2] = depth_at(f, pos + fwd * dist_left)
     depth[:, W // 2:] = depth_at(f, pos + fwd * dist_right)
-    nrg = np.broadcast_to(encode_unit_vec(-fwd), (H, W, 2)).copy()
+    nrg = np.broadcast_to(vxgi.encode_unit_vec(-fwd), (H, W, 2)).copy()
     return depth, nrg
 
 
@@ -148,7 +135,7 @@ def gbuffer_corner(f):
     rng = np.random.default_rng(3)
     _, fwd = camera_basis(f)
     n = -fwd + rng.normal(scale=0.3, size=(H, W, 3))                           # normals around the camera direction
-    nrg = encode_unit_vec(n / np.linalg.norm(n, axis=-1, keepdims=True))
+    nrg = vxgi.encode_unit_vec(n / np.linalg.norm(n, axis=-1, keepdims=True))
     depth[0, 0] = 1.0
     return (depth, nrg) + surfaces()
 

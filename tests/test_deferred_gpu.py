@@ -1,101 +1,19 @@
 """SSAO (k_ssao) and deferred lighting (k_deferred_lighting) on the GPU, bit for bit against the oracle.
 
 float32 images are compared as bytes with every NaN canonicalised (the device and x86 produce different NaN payloads)."""
-import copy
 import ctypes
-import functools
 
 import numpy as np
 import pytest
 
 import deferred_oracle as do
-from idkengine_b200 import capi, multigpu, scenes, vxgi
-from idkengine_b200 import gpu_types as gt
+from idkengine_b200 import capi, multigpu, scenes
 from idkengine_b200.pathtracer import IdkPtError, PathTracer
-
-JITTER = (0.0123, -0.0311)
-GRID_MIN, GRID_MAX = (-1.2, -0.2, -1.2), (1.2, 2.2, 1.2)
-
-
-def make_shadows(specs):
-    """[(position, near, far, light index)] -> GpuPointShadow array."""
-    s = np.zeros(len(specs), gt.GpuPointShadow)
-    for i, (p, n, f, li) in enumerate(specs):
-        s[i]["Position"], s[i]["NearPlane"], s[i]["FarPlane"], s[i]["LightIndex"] = p, n, f, li
-    return s
-
-
-@functools.lru_cache(maxsize=None)
-def setup(which):
-    """(scene, camera, shadows): two shadowed lights (the second shadow belongs to an earlier light) and one without a shadow."""
-    if which == "cornell":
-        scene, cam = scenes.cornell_1k(threads=1)
-        scene.add_light((0.0, 1.6, 0.3), (6.0, 5.5, 5.0), 0.2)
-        scene.add_light((-0.6, 0.5, 0.6), (0.5, 0.8, 3.0), 0.1)
-        scene.add_light((0.5, 1.2, 0.8), (1.0, 0.4, 0.3), 0.15)
-        scene.lights["PointShadowIndex"][:] = [1, 0, -1]                     # light 0 uses shadow 1 and the other way round
-        return scene, cam, make_shadows([(scene.lights[1]["Position"], 0.1, 60.0, 1), (scene.lights[0]["Position"], 0.2, 60.0, 0)])
-    if which == "multi_blas_tlas":
-        scene, cam = scenes.multi_blas(threads=1)
-        scene.build_tlas()
-        p = (0.2, 1.9, 0.8)
-    else:
-        scene, cam = scenes.atrium(20000, threads=1)
-        p = (0.0, 3.0, 0.5)
-    if len(scene.lights) == 0:
-        scene.add_light((1.0, 2.0, -0.5), (3.0, 3.0, 3.0), 0.2)
-    scene.add_light(p, (20.0, 18.0, 15.0), 0.3)
-    scene.add_light((-0.5, 1.0, 1.0), (2.0, 1.0, 0.5), 0.1)
-    n = len(scene.lights)
-    scene.lights["PointShadowIndex"][:] = -1
-    scene.lights["PointShadowIndex"][n - 2] = 0
-    scene.lights["PointShadowIndex"][0] = 1
-    return scene, cam, make_shadows([(p, 0.3, 60.0, n - 2), (scene.lights[0]["Position"], 0.3, 60.0, 0)])
-
-
-def canon(a):
-    u = np.ascontiguousarray(a, np.float32).view(np.uint32).copy()
-    u[((u & 0x7F800000) == 0x7F800000) & ((u & 0x007FFFFF) != 0)] = 0x7FC00000
-    return u
-
-
-def encode_unit_vec(n):
-    m = n / np.sum(np.abs(n), -1, keepdims=True)
-    wrap = (1.0 - np.abs(m[..., [1, 0]])) * np.where(m[..., :2] < 0, -1.0, 1.0)
-    return (np.where((m[..., 2] > 0)[..., None], m[..., :2], wrap) * 0.5 + 0.5).astype(np.float32)
-
-
-def gbuffer(pt, scene, frame, w, h, seed=1):
-    """(depth, normal, albedo, metallic/roughness, emissive) from the first hit, seeded albedo / emissive, and hand-made pixels
-    in row 0: sky (depth 1), roughness 0, metallic 0, metallic 1, a normal facing away from every light."""
-    depth, nrg, mr = vxgi.synth_gbuffer(pt, scene, frame, w, h)
-    rng = np.random.default_rng(seed)
-    albedo = rng.random((h, w, 3), dtype=np.float32)
-    emissive = np.where(rng.random((h, w, 1)) < 0.2, rng.random((h, w, 3)) * 0.5, 0.0).astype(np.float32)
-    depth, nrg, mr = depth.copy(), nrg.copy(), mr.copy()
-    if w >= 5 and h >= 1:
-        depth[0, 0] = 1.0
-        mr[0, 1, 1] = 0.0
-        mr[0, 2, 0] = 0.0
-        mr[0, 3, 0] = 1.0
-        f = frame[0] if frame.ndim else frame
-        M = np.asarray(f["InvProjView"], np.float64).reshape(4, 4)
-        d = depth[0, 4] if depth[0, 4] != 1.0 else 0.99
-        depth[0, 4] = d
-        wp = np.array([(4.5 / w) * 2 - 1, (0.5 / h) * 2 - 1, d, 1.0]) @ M
-        frag = wp[:3] / wp[3]
-        to_lights = np.asarray(scene.lights["Position"], np.float64) - frag
-        away = -np.sum(to_lights / np.linalg.norm(to_lights, axis=1, keepdims=True), 0)
-        nrg[0, 4] = encode_unit_vec(away / np.linalg.norm(away))
-    return depth, nrg, albedo, mr, emissive
+from raster_lib import JITTER, canon, cone_trace_gi, deferred_settings, deferred_setup, gbuffer, rt_images
 
 
 def ssao_settings(samples=10, radius=0.2, noise=0, strength=1.3):
     return capi.IdkPtSsaoSettings(samples, radius, strength, noise)
-
-
-def deferred_settings(mode, is_ssao, is_vxgi):
-    return capi.IdkPtDeferredSettings(mode, int(is_ssao), int(is_vxgi))
 
 
 SSAO_CASES = {   # name: (W, H, SampleCount, Radius, NoiseIndex)
@@ -111,7 +29,7 @@ SSAO_RUNS = [("cornell", c) for c in SSAO_CASES] + [(w, c) for w in ("multi_blas
 @pytest.mark.gpu
 @pytest.mark.parametrize("which, case", SSAO_RUNS)
 def test_gpu_ssao_matches_oracle(which, case):
-    scene, cam, _ = setup(which)
+    scene, cam, _ = deferred_setup(which)
     W, H, samples, radius, noise = SSAO_CASES[case]
     st = ssao_settings(samples, radius, noise)
     frame = scenes.camera_frame(cam, W, H)
@@ -126,15 +44,6 @@ def test_gpu_ssao_matches_oracle(which, case):
         assert got.any()
 
 
-def rt_images(pt, scene, frame, g, shadows):
-    """Shadow k's visibility image from idkpt_shadows_ray_traced for the light whose PointShadowIndex is k."""
-    out = []
-    for k in range(len(shadows)):
-        li = int(np.nonzero(scene.lights["PointShadowIndex"] == k)[0][0])
-        out.append(pt.ShadowsRayTraced(frame, g[0], g[1], li, samples=2, jitter=JITTER)[0])
-    return out
-
-
 def run_deferred(pt, scene, frame, shadows, maps, g, st, jitter=JITTER, ssao=None, indirect=None, rt=None):
     got = pt.DeferredLighting(frame, *g, settings=st, jitter=jitter, indirect=indirect if st.IsVXGI else None,
                               rt_visibility=rt if st.ShadowMode == 2 else None)
@@ -145,25 +54,10 @@ def run_deferred(pt, scene, frame, shadows, maps, g, st, jitter=JITTER, ssao=Non
     return got
 
 
-@functools.lru_cache(maxsize=None)
-def cone_trace_gi(W, H):
-    scene, cam, _ = setup("cornell")
-    frame = scenes.camera_frame(cam, W, H)
-    with PathTracer(16, 16) as pt:
-        pt.SetScene(scene)
-        g = gbuffer(pt, scene, frame, W, H)
-    unshadowed = copy.deepcopy(scene)                                           # the voxeliser's lights without shadow maps
-    unshadowed.lights["PointShadowIndex"][:] = -1
-    with vxgi.Voxelizer(32, GRID_MIN, GRID_MAX) as vx:
-        vx.SetScene(unshadowed)
-        vx.Render()
-        return vx.ConeTrace(frame, g[0], g[1], g[3])[0]
-
-
 @pytest.mark.gpu
 def test_gpu_deferred_every_mode_matches_oracle():
     """Every ShadowMode x IsSSAO x IsVXGI on the Cornell box: RT visibility from idkpt_shadows_ray_traced, GI from the cone trace."""
-    scene, cam, shadows = setup("cornell")
+    scene, cam, shadows = deferred_setup("cornell")
     W, H = 37, 23
     frame = scenes.camera_frame(cam, W, H)
     gi = cone_trace_gi(W, H)
@@ -193,7 +87,7 @@ def test_gpu_deferred_every_mode_matches_oracle():
 def test_gpu_deferred_maps_cleared_masked_rendered_and_seeded_inputs(which):
     """PCF on maps cleared, partly rendered through face masks and fully rendered; jitter NULL and non-zero; RayTraced from a
     seeded float image (values outside [0, 1] and NaN included); GI from a seeded image."""
-    scene, cam, shadows = setup(which)
+    scene, cam, shadows = deferred_setup(which)
     W, H = 40, 24
     frame = scenes.camera_frame(cam, W, H)
     rng = np.random.default_rng(7)
@@ -224,7 +118,7 @@ def test_gpu_deferred_maps_cleared_masked_rendered_and_seeded_inputs(which):
 @pytest.mark.gpu
 def test_gpu_device_tensor_gbuffer_gives_identical_bytes():
     import torch
-    scene, cam, shadows = setup("cornell")
+    scene, cam, shadows = deferred_setup("cornell")
     W, H = 37, 23
     frame = scenes.camera_frame(cam, W, H)
     gi = cone_trace_gi(W, H)
@@ -251,7 +145,7 @@ def test_gpu_device_tensor_gbuffer_gives_identical_bytes():
 @pytest.mark.gpu
 def test_gpu_device_ptrs_match_download():
     import torch
-    scene, cam, shadows = setup("cornell")
+    scene, cam, shadows = deferred_setup("cornell")
     W, H = 53, 31
     frame = scenes.camera_frame(cam, W, H)
     with PathTracer(16, 16) as pt:
@@ -280,7 +174,7 @@ def test_gpu_device_ptrs_match_download():
 
 @pytest.mark.gpu
 def test_gpu_deferred_errors_leave_the_context_working():
-    scene, cam, shadows = setup("cornell")
+    scene, cam, shadows = deferred_setup("cornell")
     W, H = 24, 16
     frame = scenes.camera_frame(cam, W, H)
     fr = np.ascontiguousarray(frame)
@@ -378,7 +272,7 @@ def test_gpu_deferred_errors_leave_the_context_working():
 
 @pytest.mark.gpu
 def test_gpu_deferred_between_async_computes():
-    scene, cam, shadows = setup("cornell")
+    scene, cam, shadows = deferred_setup("cornell")
     w, h = 160, 120
     frame = scenes.camera_frame(cam, w, h)
 
@@ -413,7 +307,7 @@ def test_gpu_misaligned_device_pointers_are_rejected_before_anything_runs():
     4 B otherwise). Only the rejection is checked: no misaligned pointer is ever launched. A rejected call leaves the previous
     images valid."""
     import torch
-    scene, cam, shadows = setup("cornell")
+    scene, cam, shadows = deferred_setup("cornell")
     W, H = 24, 16
     frame = scenes.camera_frame(cam, W, H)
     fr = np.ascontiguousarray(frame)
@@ -465,7 +359,7 @@ def test_gpu_misaligned_device_pointers_are_rejected_before_anything_runs():
 def test_gpu_wrappers_reject_a_jitter_without_two_components(wrapper):
     """The library reads taaJitter[0] and [1]: a one-element jitter is a ValueError before it reaches the library, and the
     context renders the same image afterwards."""
-    scene, cam, shadows = setup("cornell")
+    scene, cam, shadows = deferred_setup("cornell")
     W, H = 24, 16
     frame = scenes.camera_frame(cam, W, H)
     with PathTracer(16, 16) as pt:

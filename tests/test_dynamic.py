@@ -7,34 +7,7 @@ import pytest
 import oracle_lib as ol
 from idkengine_b200 import capi, scenes
 from idkengine_b200 import gpu_types as gt
-
-
-def skinning_setup(scene, blas_id, joints=6, seed=3):
-    """Unskinned vertices for the vertex range of one BLAS (random joints / weights) + joint matrices of a gentle deformation."""
-    rng = np.random.default_rng(seed)
-    d = scene.blas_descs[blas_id]
-    tris = scene.blas_triangles[d["TriangleOffset"]:d["TriangleOffset"] + d["TriangleCount"]]
-    idx = np.concatenate([tris["X"], tris["Y"], tris["Z"]])
-    v0, v1 = int(idx.min()), int(idx.max()) + 1
-    n = v1 - v0
-    u = np.zeros(n, gt.GpuUnskinnedVertex)
-    u["JointIndices"] = rng.integers(0, joints, (n, 4))
-    w = rng.uniform(0.0, 1.0, (n, 4)).astype(np.float32)
-    u["JointWeights"] = w / w.sum(1, keepdims=True)
-    u["Position"][:, 0] = scene.positions["x"][v0:v1]
-    u["Position"][:, 1] = scene.positions["y"][v0:v1]
-    u["Position"][:, 2] = scene.positions["z"][v0:v1]
-    u["Normal"] = scene.vertices["Normal"][v0:v1]
-    u["Tangent"] = scene.vertices["Tangent"][v0:v1]
-    jm = np.zeros((joints + 2, 3, 4), np.float32)          # two unused leading matrices: exercises JointMatricesOffset
-    for j in range(joints):
-        a = rng.uniform(-0.25, 0.25)
-        c, s = np.cos(a), np.sin(a)
-        jm[2 + j, :, :3] = np.array([[c, 0, s], [0, 1, 0], [-s, 0, c]], np.float32) * rng.uniform(0.9, 1.2)
-        jm[2 + j, :, 3] = rng.uniform(-0.15, 0.15, 3)
-    cmd = np.zeros(1, gt.IdkPtSkinningCmd)
-    cmd["InputVertexOffset"], cmd["OutputVertexOffset"], cmd["JointMatricesOffset"], cmd["VertexCount"] = 0, v0, 2, n
-    return u, jm, cmd
+from raster_lib import skinning_setup
 
 
 def test_oracle_refit_bounds_triangles(multi_blas):

@@ -10,18 +10,12 @@ import pytest
 import gbuffer_oracle as go
 from idkengine_b200 import capi, scenes
 from idkengine_b200.pathtracer import IdkPtError, PathTracer
+from raster_lib import JITTER, assert_bits
 from test_gbuffer import small_scene
 
 pytestmark = pytest.mark.gpu
 
-JITTER = (0.0123, -0.0311)
 ERR_INVALID_ARGUMENT, ERR_NO_SCENE = -1, -4   # IdkPtStatus
-
-
-def canon(a):
-    u = np.ascontiguousarray(a, np.float32).view(np.uint32).copy()
-    u[((u & 0x7F800000) == 0x7F800000) & ((u & 0x007FFFFF) != 0)] = 0x7FC00000
-    return u
 
 
 @functools.lru_cache(maxsize=None)
@@ -48,10 +42,9 @@ def prev_of(scene):
 
 
 def assert_same(got, want):
-    for k, (a, b) in enumerate(zip(got, want)):
+    for a, b in zip(got, want):
         assert a.shape == b.shape
-        bad = canon(a) != canon(b)
-        assert not bad.any(), f"attachment {k}: {int(bad.sum())} values differ"
+        assert_bits(a, b)
 
 
 @pytest.mark.parametrize("which", ["cornell", "multi_blas", "multi_blas_tlas", "atrium", "textured_room", "small"])

@@ -13,21 +13,11 @@ import lights_skybox_oracle as lo
 from idkengine_b200 import capi, scenes
 from idkengine_b200 import gpu_types as gt
 from idkengine_b200.pathtracer import IdkPtError, PathTracer
-from test_transparency import rule_scene
+from raster_lib import JITTER, canon, rule_scene
 
 pytestmark = pytest.mark.gpu
 
-JITTER = (0.0123, -0.0311)
 ERR_INVALID_ARGUMENT, ERR_NO_SCENE = -1, -4
-STARTUP_LIGHTS = [((-4.5, 5.7, -2.0), (429.8974, 22.459948, 28.425867), 0.3),   # Application.cs's three startup lights
-                  ((-0.5, 5.7, -2.0), (8.773416, 506.7525, 28.425867), 0.3),
-                  ((4.5, 5.7, -2.0), (8.773416, 22.459948, 533.77466), 0.3)]
-
-
-def canon(a):
-    u = np.ascontiguousarray(a, np.float32).view(np.uint32).copy()
-    u[((u & 0x7F800000) == 0x7F800000) & ((u & 0x007FFFFF) != 0)] = 0x7FC00000
-    return u
 
 
 def cube_sky(n=5):
@@ -63,7 +53,7 @@ def setup(which, lights, moving=False):
     vd = vd / np.linalg.norm(vd)
     near = (tuple(eye + vd * 0.5), (61.0, 42.0, 55.0), 0.3)
     if lights == "startup":
-        for L in STARTUP_LIGHTS + [near]:
+        for L in scenes.STARTUP_LIGHTS + [near]:
             scene.add_light(*L)
     elif lights == "many":
         scene.add_light(*near)

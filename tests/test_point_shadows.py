@@ -11,17 +11,8 @@ import numpy as np
 
 import oracle_lib as ol
 import point_shadow_oracle as pso
-from idkengine_b200 import gpu_types as gt, host, scenes, vxgi
-
-GRID_MIN, GRID_MAX = (-1.2, -0.2, -1.2), (1.2, 2.2, 1.2)
-
-
-def make_shadow(position, near, far):
-    s = np.zeros(1, gt.GpuPointShadow)
-    s["Position"] = position
-    s["NearPlane"] = near
-    s["FarPlane"] = far
-    return s
+from idkengine_b200 import host, scenes, vxgi
+from raster_lib import GRID_MAX, GRID_MIN, lit_cornell
 
 
 def face_dirs64(n):
@@ -81,7 +72,7 @@ def test_cube_map_matches_float64_ray_cast():
     shows; far = 1.25 puts the red wall (1.3 away along -X) beyond the far plane while the floor and ceiling of that face stay."""
     scene, cam = scenes.cornell_1k(threads=1)
     pos, near, far, n = (0.3, 1.1, 0.2), 0.35, 1.25, 32
-    m = pso.point_shadow_render(scene, make_shadow(pos, near, far), n)
+    m = pso.point_shadow_render(scene, scenes.point_shadows([(pos, near, far, 0)]), n)
     dirs = face_dirs64(n).reshape(-1, 3)
     origins = np.asarray(pos, np.float64) + dirs * near
     t, flagged = cast64(world_triangles(scene), origins, dirs, far - near, 1e-5)
@@ -147,7 +138,7 @@ def test_pcf_lookup_matches_gl_rules():
     n = 8
     m = rng.integers(20000, 60000, (6, n, n)).astype(np.uint16)
     near, far = 0.1, 10.0
-    sh = make_shadow((0.0, 0.0, 0.0), near, far)
+    sh = scenes.point_shadows([((0.0, 0.0, 0.0), near, far, 0)])
     dirs = [rng.normal(size=(400, 3))]
     # aimed at face edges and cube corners, and exactly on them
     e = rng.uniform(-1, 1, (300, 3))
@@ -199,11 +190,9 @@ def test_face_layout_matches_engine_face_matrices():
 
 
 def lit_cornell_shadowed():
-    scene, cam = scenes.cornell_1k(threads=1)
-    scene.add_light((0.0, 1.6, 0.3), (6.0, 5.5, 5.0), 0.2)
-    scene.add_light((-0.6, 0.5, 0.6), (0.5, 0.8, 3.0), 0.1)
+    scene, _ = lit_cornell()
     scene.lights["PointShadowIndex"][:] = [0, 1]
-    shadows = np.concatenate([make_shadow(l["Position"], l["Radius"], 60.0) for l in scene.lights])
+    shadows = scenes.point_shadows([(l["Position"], l["Radius"], 60.0, 0) for l in scene.lights])
     return scene, shadows
 
 

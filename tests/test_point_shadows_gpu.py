@@ -7,18 +7,8 @@ import pytest
 import oracle_lib as ol
 import point_shadow_oracle as pso
 from idkengine_b200 import multigpu, scenes, vxgi
-from idkengine_b200 import gpu_types as gt
 from idkengine_b200.pathtracer import IdkPtError, PathTracer
-
-GRID_MIN, GRID_MAX = (-1.2, -0.2, -1.2), (1.2, 2.2, 1.2)
-
-
-def make_shadows(specs):
-    """[(position, near, far)] -> GpuPointShadow array."""
-    s = np.zeros(len(specs), gt.GpuPointShadow)
-    for i, (p, n, f) in enumerate(specs):
-        s[i]["Position"], s[i]["NearPlane"], s[i]["FarPlane"] = p, n, f
-    return s
+from raster_lib import GRID_MAX, GRID_MIN, lit_cornell_shadowed, skinning_setup
 
 
 def scene_and_light(which):
@@ -38,7 +28,7 @@ def scene_and_light(which):
 @pytest.mark.parametrize("which", ["cornell", "multi_blas", "multi_blas_tlas", "atrium"])
 def test_gpu_cube_maps_match_oracle(which, size):
     scene, light = scene_and_light(which)
-    sh = make_shadows([light])
+    sh = scenes.point_shadows([(*light, 0)])
     want = pso.point_shadow_render(scene, sh[0], size)
     with PathTracer(16, 16) as pt:
         pt.SetScene(scene)
@@ -55,7 +45,7 @@ def test_gpu_cube_maps_match_oracle(which, size):
 @pytest.mark.gpu
 def test_gpu_several_shadows_face_mask_and_device_ptr():
     scene, cam = scenes.cornell_1k(threads=1)
-    sh = make_shadows([((0.3, 1.1, 0.2), 0.35, 1.25), ((-0.5, 0.6, 0.5), 0.1, 60.0), ((0.0, 1.9, 0.0), 0.05, 3.0)])
+    sh = scenes.point_shadows([((0.3, 1.1, 0.2), 0.35, 1.25, 0), ((-0.5, 0.6, 0.5), 0.1, 60.0, 0), ((0.0, 1.9, 0.0), 0.05, 3.0, 0)])
     sizes = [33, 64, 8]
     with PathTracer(16, 16) as pt:
         pt.SetScene(scene)
@@ -89,7 +79,7 @@ def test_gpu_several_shadows_face_mask_and_device_ptr():
 @pytest.mark.gpu
 def test_gpu_point_shadow_errors():
     scene, cam = scenes.cornell_1k(threads=1)
-    sh = make_shadows([((0.0, 1.0, 0.0), 0.1, 60.0)])
+    sh = scenes.point_shadows([((0.0, 1.0, 0.0), 0.1, 60.0, 0)])
     with PathTracer(16, 16) as pt:
         with pytest.raises(IdkPtError, match="idkpt_set_point_shadows: no scene"):
             pt.SetPointShadows(sh, [16])
@@ -141,15 +131,6 @@ def test_gpu_point_shadow_errors():
             assert vx._lib.idkvx_voxelize(vx._ctx, None) == -1                 # IDKPT_ERR_INVALID_ARGUMENT
 
 
-def lit_cornell_shadowed():
-    scene, cam = scenes.cornell_1k(threads=1)
-    scene.add_light((0.0, 1.6, 0.3), (6.0, 5.5, 5.0), 0.2)
-    scene.add_light((-0.6, 0.5, 0.6), (0.5, 0.8, 3.0), 0.1)
-    scene.lights["PointShadowIndex"][:] = [1, 0]                           # light 0 uses shadow 1 and the other way round
-    shadows = make_shadows([(scene.lights[1]["Position"], 0.1, 60.0), (scene.lights[0]["Position"], 0.2, 60.0)])
-    return scene, shadows
-
-
 @pytest.mark.gpu
 def test_gpu_voxelize_with_shadow_maps_matches_oracle():
     scene, shadows = lit_cornell_shadowed()
@@ -196,7 +177,6 @@ def test_gpu_voxelize_with_shadow_maps_matches_oracle():
 
 @pytest.mark.gpu
 def test_gpu_maps_after_skin_refit_tlas_build():
-    from test_dynamic import skinning_setup
     scene, cam = scenes.multi_blas(threads=1)
     scene.build_tlas()
     expect = copy.deepcopy(scene)
@@ -204,7 +184,7 @@ def test_gpu_maps_after_skin_refit_tlas_build():
     ol.skin_vertices(u, jm, expect.positions, expect.vertices, cmd[0])
     ol.blas_refit(expect, 2)
     expect.build_tlas()
-    sh = make_shadows([((0.2, 1.9, 0.8), 0.3, 60.0), ((1.8, 0.6, 1.5), 0.1, 20.0)])
+    sh = scenes.point_shadows([((0.2, 1.9, 0.8), 0.3, 60.0, 0), ((1.8, 0.6, 1.5), 0.1, 20.0, 0)])
     with PathTracer(16, 16) as pt:
         pt.SetScene(scene)
         pt.SetPointShadows(sh, [64, 48])
@@ -226,7 +206,7 @@ def test_gpu_render_between_async_computes_leaves_image_unchanged():
     scene, cam = scenes.cornell_1k(threads=1)
     w, h = 160, 120
     frame = scenes.camera_frame(cam, w, h)
-    sh = make_shadows([((0.0, 1.6, 0.3), 0.2, 60.0)])
+    sh = scenes.point_shadows([((0.0, 1.6, 0.3), 0.2, 60.0, 0)])
 
     def run(with_render):
         with PathTracer(w, h, lanes=4) as pt:

@@ -12,22 +12,12 @@ import oracle_lib as ol
 import sky_oracle as so
 from idkengine_b200 import capi, scenes
 from idkengine_b200.pathtracer import PathTracer
+from raster_lib import assert_bits
 from test_sky import synthetic_equirect
 
 pytestmark = pytest.mark.gpu
 
 ERR_INVALID_ARGUMENT = -1
-
-
-def canon(a):
-    u = np.ascontiguousarray(a, np.float32).view(np.uint32).copy()
-    u[((u & 0x7F800000) == 0x7F800000) & ((u & 0x007FFFFF) != 0)] = 0x7FC00000
-    return u
-
-
-def assert_bits(got, want):
-    bad = canon(got) != canon(want)
-    assert not bad.any(), f"{int(bad.sum())} of {bad.size} values differ"
 
 
 def atmo(i_steps=40, j_steps=8, intensity=15.0, azimuth=0.0, elevation=0.0):

@@ -4,7 +4,7 @@ import numpy as np
 import pytest
 
 import ssr_taa_oracle as so
-from idkengine_b200 import capi, scenes
+from idkengine_b200 import capi, scenes, vxgi
 
 W, H = 23, 17
 
@@ -18,12 +18,6 @@ def mat(frame, name):
     """GpuPerFrameData matrix as M with GLSL's M * v == v @ M."""
     f = frame[0] if frame.ndim else frame
     return np.asarray(f[name], np.float64).reshape(4, 4)
-
-
-def encode_unit_vec(n):
-    m = n / np.sum(np.abs(n), -1, keepdims=True)
-    wrap = (1.0 - np.abs(m[..., [1, 0]])) * np.where(m[..., :2] < 0, -1.0, 1.0)
-    return (np.where((m[..., 2] > 0)[..., None], m[..., :2], wrap) * 0.5 + 0.5).astype(np.float32)
 
 
 def decode_unit_vec(e):
@@ -44,7 +38,7 @@ def synthetic_gbuffer(seed, w=W, h=H):
     depth[0, 0] = 1.0
     n = rng.normal(size=(h, w, 3))
     n[..., 2] = np.abs(n[..., 2]) + 0.5
-    nrg = encode_unit_vec(n / np.linalg.norm(n, axis=-1, keepdims=True))
+    nrg = vxgi.encode_unit_vec(n / np.linalg.norm(n, axis=-1, keepdims=True))
     albedo = rng.random((h, w, 3), dtype=np.float32)
     mr = rng.random((h, w, 2), dtype=np.float32)
     mr[rng.random((h, w)) < 0.15, 0] = 0.0005
@@ -212,7 +206,7 @@ def mirror_gbuffer(frame, r_view, metallic=0.75, w=W, h=H):
     nv = (r - i) / np.linalg.norm(r - i)
     nw = np.linalg.solve(IV[:3, :3], nv)
     nrg = np.zeros((h, w, 2), np.float32)
-    nrg[y, x] = encode_unit_vec(nw / np.linalg.norm(nw))
+    nrg[y, x] = vxgi.encode_unit_vec(nw / np.linalg.norm(nw))
     albedo = np.full((h, w, 3), 0.5, np.float32)
     albedo[y, x] = (0.9, 0.6, 0.3)
     mr = np.zeros((h, w, 2), np.float32)

@@ -9,15 +9,9 @@ import pytest
 import ssr_taa_oracle as so
 from idkengine_b200 import capi, multigpu, scenes
 from idkengine_b200.pathtracer import IdkPtError, PathTracer
-from test_deferred_gpu import JITTER, canon, gbuffer, setup
+from raster_lib import JITTER, canon, deferred_setup, gbuffer
 
 SKY = (0.35, 0.55, 0.9)
-
-
-def canon16(a):
-    u = np.ascontiguousarray(a, np.float16).view(np.uint16).copy()
-    u[((u & 0x7C00) == 0x7C00) & ((u & 0x03FF) != 0)] = 0x7E00
-    return u
 
 
 def sky_faces(n=8, seed=2):
@@ -25,7 +19,7 @@ def sky_faces(n=8, seed=2):
 
 
 def ssr_gbuffer(pt, scene, frame, w, h, seed=1):
-    """test_deferred_gpu.gbuffer with seeded metallic values (a tenth of them below SSR's 0.001 threshold) and a seeded
+    """raster_lib.gbuffer with seeded metallic values (a tenth of them below SSR's 0.001 threshold) and a seeded
     rgba32f lit image."""
     d, n, a, mr, e = gbuffer(pt, scene, frame, w, h, seed)
     rng = np.random.default_rng(seed + 100)
@@ -43,7 +37,7 @@ def check_ssr(pt, frame, g, st, sky, lit, source=None):
         got = pt.Ssr(frame, g[0], g[1], g[2], g[3], st, color=lit)
     want = so.ssr(frame, st, sky, g[0], g[1], g[2], g[3], lit)
     assert np.array_equal(canon(got[0]), canon(want[0]))
-    assert np.array_equal(canon16(got[1]), canon16(want[1]))
+    assert np.array_equal(canon(got[1]), canon(want[1]))
     return got
 
 
@@ -64,7 +58,7 @@ SSR_RUNS = [("cornell", c) for c in SSR_CASES] + [(w, c) for w in ("multi_blas_t
 @pytest.mark.parametrize("which, case", SSR_RUNS)
 @pytest.mark.parametrize("faces", [False, True], ids=["constant_sky", "cube_sky"])
 def test_gpu_ssr_matches_oracle(which, case, faces):
-    scene, cam, _ = setup(which)
+    scene, cam, _ = deferred_setup(which)
     W, H, samples, bsc, max_dist = SSR_CASES[case]
     st = capi.IdkPtSsrSettings(samples, bsc, max_dist)
     frame = scenes.camera_frame(cam, W, H)
@@ -85,7 +79,7 @@ def test_gpu_ssr_matches_oracle(which, case, faces):
 def test_gpu_ssr_every_source_and_device_tensors():
     """ARRAY (host and device) and DEFERRED sources, host and device G-buffers: identical bytes, equal to the oracle."""
     import torch
-    scene, cam, shadows = setup("cornell")
+    scene, cam, shadows = deferred_setup("cornell")
     W, H = 37, 23
     frame = scenes.camera_frame(cam, W, H)
     st = capi.default_ssr_settings()
@@ -99,13 +93,13 @@ def test_gpu_ssr_every_source_and_device_tensors():
         host = check_ssr(pt, frame, g, st, sky, lit)
         dg = [torch.from_numpy(a).cuda() for a in g]
         dev = pt.Ssr(frame, dg[0], dg[1], dg[2], dg[3], st, color=torch.from_numpy(lit).cuda())
-        assert np.array_equal(canon(host[0]), canon(dev[0])) and np.array_equal(canon16(host[1]), canon16(dev[1]))
+        assert np.array_equal(canon(host[0]), canon(dev[0])) and np.array_equal(canon(host[1]), canon(dev[1]))
         pt.Ssao(frame, g[0], g[1])
         deferred = pt.DeferredLighting(frame, *g, jitter=JITTER)
         from_deferred = check_ssr(pt, frame, g, st, sky, deferred, source=capi.LIT_SOURCE_DEFERRED)
         pt.DeferredLighting(frame, *dg, jitter=JITTER, download=False)
         dev = pt.Ssr(frame, dg[0], dg[1], dg[2], dg[3], st, source=capi.LIT_SOURCE_DEFERRED)
-        assert np.array_equal(canon(from_deferred[0]), canon(dev[0])) and np.array_equal(canon16(from_deferred[1]), canon16(dev[1]))
+        assert np.array_equal(canon(from_deferred[0]), canon(dev[0])) and np.array_equal(canon(from_deferred[1]), canon(dev[1]))
         with pytest.raises(TypeError):
             pt.Ssr(frame, dg[0], dg[1], dg[2], dg[3], st, color=lit)
 
@@ -169,7 +163,7 @@ TAA_SETTINGS = [(0, 0.25, 6), (0, 0.0, 6), (0, 1.0, 1), (0, 0.25, 1), (1, 0.25, 
 def test_gpu_taa_sequence_matches_oracle(scale, naive, prefer, samples):
     """Six frames of a moving camera: the deferred image of each frame (with its jitter) resolved against the history, frame by
     frame, at render = presentation size and at render scales 0.6 and 0.5."""
-    scene, cam, _ = setup("cornell")
+    scene, cam, _ = deferred_setup("cornell")
     W, H = 37, 23
     rw, rh = max(1, int(W * scale)), max(1, int(H * scale))
     st = capi.IdkPtTaaSettings(naive, prefer, samples)
@@ -183,7 +177,7 @@ def test_gpu_taa_sequence_matches_oracle(scale, naive, prefer, samples):
             lit = pt.DeferredLighting(frame, *g, settings=capi.IdkPtDeferredSettings(0, 0, 0), jitter=jit)
             got = pt.TaaResolve(depth, vel, W, H, st, source=capi.LIT_SOURCE_DEFERRED)
             want = so.taa_resolve(st, lit, depth, vel, history)
-            assert np.array_equal(canon16(got), canon16(want)), k
+            assert np.array_equal(canon(got), canon(want)), k
             assert np.all(got[..., 3] == 1)
             history = want
 
@@ -202,14 +196,14 @@ def test_gpu_taa_tiny_sizes(size):
             vel = ((rng.random((H, W, 2)) - 0.5) * 0.2).astype(np.float32)
             got = pt.TaaResolve(depth, vel, W, H, st, color=color)
             want = so.taa_resolve(st, color, depth, vel, history)
-            assert np.array_equal(canon16(got), canon16(want))
+            assert np.array_equal(canon(got), canon(want))
             history = want
 
 
 @pytest.mark.gpu
 def test_gpu_taa_restarts_from_zero_history_on_resize_and_new_scene():
     import torch
-    scene, cam, _ = setup("cornell")
+    scene, cam, _ = deferred_setup("cornell")
     rng = np.random.default_rng(9)
     st = capi.default_taa_settings()
     with PathTracer(16, 16) as pt:
@@ -223,11 +217,11 @@ def test_gpu_taa_restarts_from_zero_history_on_resize_and_new_scene():
             vel = ((rng.random((rh, rw, 2)) - 0.5) * 0.05).astype(np.float32)
             got = pt.TaaResolve(depth, vel, W, H, st, color=color)
             want = so.taa_resolve(st, color, depth, vel, history if history is not None else np.zeros((H, W, 4), np.float16))
-            assert np.array_equal(canon16(got), canon16(want))
+            assert np.array_equal(canon(got), canon(want))
             p, nbytes = pt.TaaDevicePtr()
             assert nbytes == W * H * 8
             dev = torch.as_tensor(multigpu.DeviceArray(p, (nbytes // 2,), "<f2"), device="cuda").cpu().numpy()
-            assert np.array_equal(canon16(dev.reshape(H, W, 4)), canon16(got))
+            assert np.array_equal(canon(dev.reshape(H, W, 4)), canon(got))
             return got
         h = step(20, 12, 12, 8, None)
         h = step(20, 12, 12, 8, h)
@@ -243,7 +237,7 @@ def test_gpu_taa_restarts_from_zero_history_on_resize_and_new_scene():
 @pytest.mark.gpu
 def test_gpu_device_ptrs_and_the_merged_source():
     import torch
-    scene, cam, _ = setup("cornell")
+    scene, cam, _ = deferred_setup("cornell")
     W, H = 53, 31
     frame = scenes.camera_frame(cam, W, H)
     with PathTracer(16, 16) as pt:
@@ -258,19 +252,19 @@ def test_gpu_device_ptrs_and_the_merged_source():
         assert nm == W * H * 16 and ns == W * H * 8
         dm = torch.as_tensor(multigpu.DeviceArray(pm, (nm // 4,), "<f4"), device="cuda").cpu().numpy().reshape(H, W, 4)
         ds = torch.as_tensor(multigpu.DeviceArray(ps, (ns // 2,), "<f2"), device="cuda").cpu().numpy().reshape(H, W, 4)
-        assert np.array_equal(canon(dm), canon(merged)) and np.array_equal(canon16(ds), canon16(ssr))
+        assert np.array_equal(canon(dm), canon(merged)) and np.array_equal(canon(ds), canon(ssr))
         depth, vel = g[0], np.zeros((H, W, 2), np.float32)
         a = pt.TaaResolve(depth, vel, W, H, source=capi.LIT_SOURCE_MERGED)
         with PathTracer(16, 16) as other:                                      # the same image as an ARRAY
             b = other.TaaResolve(depth, vel, W, H, color=merged)
-        assert np.array_equal(canon16(a), canon16(b))
+        assert np.array_equal(canon(a), canon(b))
         assert pt.last_ssr_ms > 0 and pt.last_taa_ms > 0
 
 
 @pytest.mark.gpu
 def test_gpu_errors_leave_the_context_working():
     import torch
-    scene, cam, _ = setup("cornell")
+    scene, cam, _ = deferred_setup("cornell")
     W, H = 24, 16
     frame = scenes.camera_frame(cam, W, H)
     fr = np.ascontiguousarray(frame)
@@ -386,7 +380,7 @@ def test_gpu_errors_leave_the_context_working():
 
 @pytest.mark.gpu
 def test_gpu_ssr_taa_between_async_computes():
-    scene, cam, _ = setup("cornell")
+    scene, cam, _ = deferred_setup("cornell")
     w, h = 160, 120
     frame = scenes.camera_frame(cam, w, h)
 
@@ -413,8 +407,8 @@ def test_gpu_ssr_taa_between_async_computes():
     img1, (want, want_taa), got = go(True)
     assert np.array_equal(img0.view(np.uint32), img1.view(np.uint32))
     for k, ((merged, ssr), taa) in enumerate(got):
-        assert np.array_equal(canon(merged), canon(want[0])) and np.array_equal(canon16(ssr), canon16(want[1]))
-        assert np.array_equal(canon16(taa), canon16(want_taa[k]))
+        assert np.array_equal(canon(merged), canon(want[0])) and np.array_equal(canon(ssr), canon(want[1]))
+        assert np.array_equal(canon(taa), canon(want_taa[k]))
 
 
 @pytest.mark.gpu
@@ -422,7 +416,7 @@ def test_gpu_whole_chain_on_the_device_equals_host_arrays():
     """G-buffer -> SSAO -> deferred lighting -> SSR + merge -> TAA with every image on the device, against the same chain fed
     with host arrays and downloads in between, over three frames at render scale 0.6."""
     import torch
-    scene, cam, shadows = setup("cornell")
+    scene, cam, shadows = deferred_setup("cornell")
     W, H = 61, 37
     rw, rh = int(W * 0.6), int(H * 0.6)
     frames, jitters = frame_sequence(cam, rw, rh, 3)
@@ -454,12 +448,12 @@ def test_gpu_whole_chain_on_the_device_equals_host_arrays():
 
     dev, host = run(True), run(False)
     for a, b in zip(dev, host):
-        assert np.array_equal(canon16(a), canon16(b))
+        assert np.array_equal(canon(a), canon(b))
 
 
 @pytest.mark.gpu
 def test_gpu_full_size_atrium_1152x648_to_1080p():
-    scene, cam, _ = setup("atrium")
+    scene, cam, _ = deferred_setup("atrium")
     rw, rh, W, H = 1152, 648, 1920, 1080
     frames, jitters = frame_sequence(cam, rw, rh, 3)
     st, tst = capi.default_ssr_settings(), capi.default_taa_settings()
@@ -474,5 +468,5 @@ def test_gpu_full_size_atrium_1152x648_to_1080p():
             depth, vel = reprojected_velocity(frame, g[0])
             got = pt.TaaResolve(depth, vel, W, H, tst, source=capi.LIT_SOURCE_MERGED)
             want = so.taa_resolve(tst, merged, depth, vel, history)
-            assert np.array_equal(canon16(got), canon16(want)), k
+            assert np.array_equal(canon(got), canon(want)), k
             history = want

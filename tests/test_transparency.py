@@ -8,57 +8,7 @@ import pytest
 
 import transparency_oracle as to
 from idkengine_b200 import scenes
-from idkengine_b200.host import Model, Scene
-
-CAM = dict(position=(0.0, 1.0, 3.0), view_dir=(0.0, 0.0, -1.0), fov_y_deg=60.0)
-
-
-def rule_scene():
-    """Every rule in view: an opaque back wall with a blended pane behind it (fails depth); a single-sided blended quad seen from
-    behind (culled) and a double-sided one (kept, normal flipped); a textured blended card with alpha-0 and partial-alpha texels;
-    a blended quad crossing the near plane; blended panes over the background; a mirrored blended instance; two coplanar
-    duplicated quads with different materials (an exact depth tie); and a stack of 13 panes (the 10-layer cap)."""
-    specs = [dict(color=(0.7, 0.7, 0.7), roughness=0.6),                               # 0 opaque back wall
-             dict(color=(0.9, 0.2, 0.2, 0.5), cutoff=2.0),                             # 1 blended, behind the wall
-             dict(color=(0.9, 0.1, 0.1, 0.6), cutoff=2.0),                             # 2 single-sided, seen from behind
-             dict(color=(0.1, 0.9, 0.1, 0.4), cutoff=2.0, metallic=0.5, emissive=(0.5, 0.25, 0.0)),  # 3 double-sided, from behind
-             dict(color=(1.0, 1.0, 1.0, 1.0), cutoff=2.0),                             # 4 textured card (alpha 0 / partial texels)
-             dict(color=(0.3, 0.8, 0.8, 0.5), cutoff=2.0),                             # 5 crosses the near plane
-             dict(color=(0.2, 0.4, 0.9, 0.3), cutoff=2.0, ior=1.5, roughness=0.1),     # 6 glass over the background
-             dict(color=(0.6, 0.3, 0.8, 0.5), cutoff=2.0),                             # 7 mirrored instance
-             dict(color=(0.9, 0.9, 0.1, 0.5), cutoff=2.0),                             # 8 coplanar tie, material A
-             dict(color=(0.1, 0.9, 0.9, 0.5), cutoff=2.0),                             # 9 coplanar tie, material B
-             dict(color=(0.8, 0.5, 0.2, 0.2), cutoff=2.0, ior=1.33)]                   # 10 the 13-pane stack
-    scene = Scene()
-    t_card = scene.add_texture(scenes._checker(32, 2, (200, 120, 60), (60, 120, 200), alpha_a=0, alpha_b=128, seed=5), srgb=True)
-    meshes, mats = scenes._materials(specs)
-    mats["IsDoubleSided"][3] = mats["IsDoubleSided"][5] = 1
-    mats["BaseColorTexture"][4] = t_card
-
-    def model(quads, mesh, matrix=None, uv=None):
-        a = scenes._Assembler()
-        for q in quads:
-            a.add(scenes.quad(*q), 0)
-        m, t = meshes[mesh:mesh + 1].copy(), mats[mesh:mesh + 1].copy()
-        m["MaterialId"] = 0
-        return Model(np.concatenate(a.pos), np.concatenate(a.idx), np.concatenate(a.mesh), texcoords=uv, meshes=m, materials=t,
-                     model_matrix=matrix)
-    ccw = lambda x0, x1, y0, y1, z: ([x0, y0, z], [x1, y0, z], [x1, y1, z], [x0, y1, z])   # front-facing from +z
-    cw = lambda x0, x1, y0, y1, z: ([x0, y0, z], [x0, y1, z], [x1, y1, z], [x1, y0, z])    # back-facing from +z
-    uv = np.array([[0, 0], [2, 0], [2, 2], [0, 2]], np.float32)
-    scene.add(model([ccw(-1.5, 0.5, -1, 1.6, -2)], 0),
-              model([ccw(-1.2, 0.0, 0.0, 1.0, -2.5)], 1),
-              model([cw(-1.4, -0.6, 0.2, 0.9, -1)], 2),
-              model([cw(0.6, 1.4, 0.2, 0.9, -1)], 3),
-              model([ccw(-1.4, -0.6, 1.2, 1.8, -1.2)], 4, uv=uv),
-              model([([0.05, 0.85, 2.95], [0.35, 0.85, 2.4], [0.35, 1.15, 2.4], [0.05, 1.15, 2.95])], 5),
-              model([ccw(0.7, 1.9, 1.2, 2.2, -3.0)], 6),
-              model([cw(0.6, 1.4, -0.7, -0.1, -1)], 7, matrix=np.diag([-1.0, 1.0, 1.0, 1.0])),
-              model([ccw(-0.4, 0.4, 1.9, 2.3, -0.8)], 8),
-              model([ccw(-0.4, 0.4, 1.9, 2.3, -0.8)], 9),
-              model([ccw(-0.3, 0.3, 0.3, 0.9, -0.3 - 0.1 * k) for k in range(13)], 10), threads=1)
-    scene.add_light((0.5, 2.0, 0.5), (4.0, 3.5, 3.0), 0.2)
-    return scene, CAM
+from raster_lib import rule_scene
 
 
 def opaque_inputs(scene, frame, w, h):

@@ -11,28 +11,13 @@ import pytest
 import gbuffer_oracle as go
 import transparency_oracle as to
 from idkengine_b200 import capi, scenes, vxgi
-from idkengine_b200 import gpu_types as gt
 from idkengine_b200.pathtracer import IdkPtError, PathTracer
-from test_transparency import rule_scene
+from raster_lib import JITTER, canon, rule_scene
 
 pytestmark = pytest.mark.gpu
 
-JITTER = (0.0123, -0.0311)
 GRID_MIN, GRID_MAX = (-2.0, -1.2, -3.2), (2.0, 3.2, 3.2)
 ERR_INVALID_ARGUMENT, ERR_NO_SCENE = -1, -4
-
-
-def canon(a):
-    u = np.ascontiguousarray(a, np.float32).view(np.uint32).copy()
-    u[((u & 0x7F800000) == 0x7F800000) & ((u & 0x007FFFFF) != 0)] = 0x7FC00000
-    return u
-
-
-def make_shadows(specs):
-    s = np.zeros(len(specs), gt.GpuPointShadow)
-    for i, (p, n, f, li) in enumerate(specs):
-        s[i]["Position"], s[i]["NearPlane"], s[i]["FarPlane"], s[i]["LightIndex"] = p, n, f, li
-    return s
 
 
 @functools.lru_cache(maxsize=None)
@@ -58,7 +43,7 @@ def setup(which):
     n = len(scene.lights)
     scene.lights["PointShadowIndex"][:] = -1
     scene.lights["PointShadowIndex"][n - 2] = 0
-    return scene, cam, make_shadows([(scene.lights[n - 2]["Position"], 0.1, 60.0, n - 2)])
+    return scene, cam, scenes.point_shadows([(scene.lights[n - 2]["Position"], 0.1, 60.0, n - 2)])
 
 
 def lit_image(h, w, seed=4):

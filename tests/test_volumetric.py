@@ -9,23 +9,17 @@ restatement of both dispatches (no GPU).
 import numpy as np
 
 import oracle_lib as ol
+import raster_lib as rl
 import volumetric_oracle as vo
-from idkengine_b200 import capi, gpu_types as gt, scenes
+from idkengine_b200 import capi, scenes
 
 DITHER = np.array([[0.0, 0.5, 0.125, 0.625], [0.75, 0.22, 0.875, 0.375], [0.1875, 0.6875, 0.0625, 0.5625], [0.9375, 0.4375, 0.8125, 0.3125]])
 
 
 def lit_cornell():
     """Two lights, each with a point shadow; shadow 0 belongs to light 1 and shadow 1 to light 0."""
-    scene, cam = scenes.cornell_1k(threads=1)
-    scene.add_light((0.0, 1.6, 0.3), (6.0, 5.5, 5.0), 0.2)
-    scene.add_light((-0.6, 0.5, 0.6), (0.5, 0.8, 3.0), 0.1)
-    scene.lights["PointShadowIndex"][:] = [1, 0]
-    shadows = np.zeros(2, gt.GpuPointShadow)
-    for i, li in enumerate((1, 0)):
-        shadows[i]["Position"], shadows[i]["NearPlane"], shadows[i]["FarPlane"] = scene.lights[li]["Position"], 0.1, 60.0
-        shadows[i]["LightIndex"] = li
-    return scene, cam, shadows
+    scene, cam = rl.lit_cornell(2)
+    return scene, cam, rl.crossed_shadows(scene, 0.1, 0.1)
 
 
 def nearest64(u, n):

@@ -9,29 +9,16 @@ import pytest
 
 import volumetric_oracle as vo
 from idkengine_b200 import capi, multigpu, scenes, vxgi
-from idkengine_b200 import gpu_types as gt
 from idkengine_b200.pathtracer import IdkPtError, PathTracer
-
-JITTER = (0.0123, -0.0311)
-
-
-def make_shadows(specs):
-    """[(position, near, far, light index)] -> GpuPointShadow array."""
-    s = np.zeros(len(specs), gt.GpuPointShadow)
-    for i, (p, n, f, li) in enumerate(specs):
-        s[i]["Position"], s[i]["NearPlane"], s[i]["FarPlane"], s[i]["LightIndex"] = p, n, f, li
-    return s
+from raster_lib import JITTER, canon, crossed_shadows, lit_cornell
 
 
 @functools.lru_cache(maxsize=None)
 def setup(which):
     """(scene, camera, shadows): two shadows per scene, the second one's LightIndex pointing at an earlier light."""
     if which == "cornell":
-        scene, cam = scenes.cornell_1k(threads=1)
-        scene.add_light((0.0, 1.6, 0.3), (6.0, 5.5, 5.0), 0.2)
-        scene.add_light((-0.6, 0.5, 0.6), (0.5, 0.8, 3.0), 0.1)
-        scene.lights["PointShadowIndex"][:] = [1, 0]                     # light 0 uses shadow 1 and the other way round
-        return scene, cam, make_shadows([(scene.lights[1]["Position"], 0.1, 60.0, 1), (scene.lights[0]["Position"], 0.2, 60.0, 0)])
+        scene, cam = lit_cornell(2)
+        return scene, cam, crossed_shadows(scene, 0.1, 0.2)
     if which == "multi_blas_tlas":
         scene, cam = scenes.multi_blas(threads=1)
         scene.build_tlas()
@@ -41,13 +28,7 @@ def setup(which):
         p = (0.0, 3.0, 0.5)
     scene.add_light(p, (20.0, 18.0, 15.0), 0.3)
     n = len(scene.lights)
-    return scene, cam, make_shadows([(p, 0.3, 60.0, n - 1), (scene.lights[0]["Position"], 0.3, 60.0, 0)])
-
-
-def canon(a):
-    u = np.ascontiguousarray(a).view(np.uint16).copy()
-    u[((u & 0x7C00) == 0x7C00) & ((u & 0x03FF) != 0)] = 0x7E00
-    return u
+    return scene, cam, scenes.point_shadows([(p, 0.3, 60.0, n - 1), (scene.lights[0]["Position"], 0.3, 60.0, 0)])
 
 
 def settings(scale=0.6, samples=5, max_dist=50.0):

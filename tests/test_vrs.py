@@ -13,8 +13,9 @@ import numpy as np
 import pytest
 
 import deferred_oracle as do
+import raster_lib as rl
 import vrs_oracle as vo
-from idkengine_b200 import capi, gpu_types as gt, scenes
+from idkengine_b200 import capi, scenes
 
 SPEED, LUM, COV = capi.VRS_DEBUG_SPEED, capi.VRS_DEBUG_LUMINANCE, capi.VRS_DEBUG_LUMINANCE_VARIANCE
 
@@ -196,16 +197,8 @@ def test_rejected_settings():
 
 # ---- coarse deferred lighting
 def lit_cornell():
-    scene, cam = scenes.cornell_1k(threads=1)
-    scene.add_light((0.0, 1.6, 0.3), (6.0, 5.5, 5.0), 0.2)
-    scene.add_light((-0.6, 0.5, 0.6), (0.5, 0.8, 3.0), 0.1)
-    scene.add_light((0.5, 1.2, 0.8), (1.0, 0.4, 0.3), 0.15)
-    scene.lights["PointShadowIndex"][:] = [1, 0, -1]
-    shadows = np.zeros(2, gt.GpuPointShadow)
-    for i, li in enumerate((1, 0)):
-        shadows[i]["Position"], shadows[i]["NearPlane"], shadows[i]["FarPlane"] = scene.lights[li]["Position"], 0.1, 60.0
-        shadows[i]["LightIndex"] = li
-    return scene, cam, shadows
+    scene, cam = rl.lit_cornell(3)
+    return scene, cam, rl.crossed_shadows(scene, 0.1, 0.1)
 
 
 def synthetic_inputs(w, h, seed):

@@ -8,7 +8,7 @@ import pytest
 import vrs_oracle as vo
 from idkengine_b200 import capi, multigpu, scenes
 from idkengine_b200.pathtracer import IdkPtError, PathTracer
-from test_deferred_gpu import JITTER, canon, cone_trace_gi, deferred_settings, gbuffer, rt_images, setup
+from raster_lib import JITTER, canon, cone_trace_gi, deferred_settings, deferred_setup, gbuffer, rt_images
 
 
 def frame_dt(cam, w, h, dt=1.0 / 60.0):
@@ -58,7 +58,7 @@ SIZES = [(1, 1), (16, 16), (17, 9), (37, 23), (1920, 1080)]
 @pytest.mark.parametrize("w, h", SIZES)
 def test_gpu_shading_rate_matches_oracle(w, h):
     import torch
-    scene, cam, _ = setup("cornell")
+    scene, cam, _ = deferred_setup("cornell")
     frame = frame_dt(cam, w, h)
     color, velocity = classifier_inputs(w, h, w + h)
     dcolor, dvel = torch.from_numpy(color).cuda(), torch.from_numpy(velocity).cuda()
@@ -104,7 +104,7 @@ def run_vrs(pt, scene, frame, shadows, maps, g, st, rates, ssao=None, indirect=N
 @pytest.mark.gpu
 def test_gpu_coarse_deferred_every_mode_matches_oracle():
     """Every ShadowMode x IsSSAO x IsVXGI on the Cornell box under a rate image with all five rates and partial edge tiles."""
-    scene, cam, shadows = setup("cornell")
+    scene, cam, shadows = deferred_setup("cornell")
     W, H = 37, 23
     frame = frame_dt(cam, W, H, 1.0)
     gi = cone_trace_gi(W, H)
@@ -128,7 +128,7 @@ def test_gpu_coarse_deferred_every_mode_matches_oracle():
 @pytest.mark.gpu
 @pytest.mark.parametrize("W, H", [(53, 37), (96, 64), (1, 1), (5, 3)])
 def test_gpu_coarse_deferred_atrium_all_rates(W, H):
-    scene, cam, shadows = setup("atrium")
+    scene, cam, shadows = deferred_setup("atrium")
     frame = frame_dt(cam, W, H, 1.0)
     color, velocity = five_rate_inputs(W, H, W)
     with PathTracer(16, 16) as pt:
@@ -156,7 +156,7 @@ def test_gpu_coarse_deferred_atrium_all_rates(W, H):
 @pytest.mark.gpu
 def test_gpu_vrs_at_full_rate_equals_the_per_pixel_pass():
     """A flat lit image gives cov 0 -> NaN -> rate 0 in every tile; IsVariableRateShading then returns exactly the bytes of 0."""
-    scene, cam, shadows = setup("cornell")
+    scene, cam, shadows = deferred_setup("cornell")
     W, H = 61, 35
     frame = frame_dt(cam, W, H)
     with PathTracer(16, 16) as pt:
@@ -184,7 +184,7 @@ def test_gpu_device_only_chain():
     """Frame N: deferred; classify its image (DEFERRED); frame N+1: deferred under the rates. CUDA tensors in, nothing
     downloaded; the device pointers equal the downloads of the same calls and the host-array chain."""
     import torch
-    scene, cam, shadows = setup("cornell")
+    scene, cam, shadows = deferred_setup("cornell")
     W, H = 83, 45
     frame = frame_dt(cam, W, H)
     with PathTracer(16, 16) as pt:
@@ -219,7 +219,7 @@ def test_gpu_device_only_chain():
 @pytest.mark.gpu
 def test_gpu_shading_rate_errors_leave_the_context_working():
     import torch
-    scene, cam, shadows = setup("cornell")
+    scene, cam, shadows = deferred_setup("cornell")
     W, H = 40, 24
     frame = frame_dt(cam, W, H)
     fr = np.ascontiguousarray(frame)
@@ -309,7 +309,7 @@ def test_gpu_shading_rate_errors_leave_the_context_working():
 
 @pytest.mark.gpu
 def test_gpu_vrs_between_async_computes():
-    scene, cam, shadows = setup("cornell")
+    scene, cam, shadows = deferred_setup("cornell")
     w, h = 160, 120
     frame = frame_dt(cam, w, h)
     color, velocity = classifier_inputs(w, h, 5)

@@ -4,15 +4,7 @@ import pytest
 
 import oracle_lib as ol
 from idkengine_b200 import scenes, vxgi
-
-GRID_MIN, GRID_MAX = (-1.2, -0.2, -1.2), (1.2, 2.2, 1.2)
-
-
-def lit_cornell():
-    scene, cam = scenes.cornell_1k(threads=1)
-    scene.add_light((0.0, 1.6, 0.3), (6.0, 5.5, 5.0), 0.2)
-    scene.add_light((-0.6, 0.5, 0.6), (0.5, 0.8, 3.0), 0.1)
-    return scene, cam
+from raster_lib import GRID_MAX, GRID_MIN, TEX_GRID_MAX, TEX_GRID_MIN, lit_cornell
 
 
 def test_half_conversion_and_log2():
@@ -184,9 +176,6 @@ def test_gpu_point_shadowed_lights_match_oracle():
 
 
 # ---- material textures in the voxeliser (BaseColor / Emissive slots, base level, same sampler rules as the path tracer)
-TEX_GRID_MIN, TEX_GRID_MAX = (-3.1, -0.1, -3.1), (3.1, 4.1, 3.1)
-
-
 def test_oracle_voxelize_textured_differs_from_factor_only():
     import copy
     scene, cam = scenes.textured_room(threads=1)

@@ -16,7 +16,7 @@ import oracle_lib as ol
 import vxgi_conservative_oracle as vco
 import vxgi_conservative_ref64 as r64c
 from idkengine_b200 import host, scenes, vxgi
-from test_vxgi_ref import GRID_MAX, GRID_MIN, check_voxelized, lit_cornell
+from raster_lib import GRID_MAX, GRID_MIN, check_voxelized, lit_cornell
 
 # a 32^3 grid over [0, 4]^3: window coordinates are 8 * world, so dyadic world coordinates are exact in fp32
 KNOWN_MIN, KNOWN_MAX, KNOWN_SIZE = (0.0, 0.0, 0.0), (4.0, 4.0, 4.0), 32

@@ -9,10 +9,8 @@ import point_shadow_oracle as pso
 import vxgi_conservative_oracle as vco
 from idkengine_b200 import multigpu, scenes, vxgi
 from idkengine_b200.pathtracer import PathTracer
-from test_point_shadows_gpu import lit_cornell_shadowed
-from test_vxgi import TEX_GRID_MAX, TEX_GRID_MIN
+from raster_lib import GRID_MAX, GRID_MIN, TEX_GRID_MAX, TEX_GRID_MIN, lit_cornell, lit_cornell_shadowed
 from test_vxgi_conservative import THIN_MAX, THIN_MIN, THIN_SIZE, atrium_lit, thin_scene
-from test_vxgi_ref import GRID_MAX, GRID_MIN, lit_cornell
 
 pytestmark = pytest.mark.gpu
 

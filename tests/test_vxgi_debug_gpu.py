@@ -13,9 +13,8 @@ import oracle_lib as ol
 import vxgi_debug_oracle as vdo
 from idkengine_b200 import capi, scenes, vxgi
 from idkengine_b200.pathtracer import PathTracer
+from raster_lib import GRID_MAX, GRID_MIN, lit_cornell, synthetic_chain, write_level
 from test_vxgi_debug import hand_frame
-from test_vxgi_ref import GRID_MAX, GRID_MIN, lit_cornell, synthetic_chain
-from test_vxgi_ref_gpu import write_level
 
 pytestmark = pytest.mark.gpu
 
@@ -164,10 +163,6 @@ def test_gpu_debug_render_inf_texels_hit():
     assert np.isnan(img[0, 0]).any()
 
 
-ATRIUM_LIGHTS = [((-4.5, 5.7, -2.0), (429.8974, 22.459948, 28.425867)), ((-0.5, 5.7, -2.0), (8.773416, 506.7525, 28.425867)),
-                 ((4.5, 5.7, -2.0), (8.773416, 22.459948, 533.77466))]
-
-
 def test_gpu_debug_render_atrium_full_size():
     """bench.py's atrium with the reference's startup lights, voxelised at 256^3 over the default bounds and rendered at
     1920x1080 with the engine's defaults (cone angle 0, step multiplier 0.4) from the bench camera, inside the grid, and
@@ -176,8 +171,8 @@ def test_gpu_debug_render_atrium_full_size():
     scene, cam = scenes.atrium(262144)
     sc = copy.copy(scene)
     sc.lights = scene.lights.copy()
-    for pos, col in ATRIUM_LIGHTS:
-        sc.add_light(pos, col, 0.3)
+    for light in scenes.STARTUP_LIGHTS:
+        sc.add_light(*light)
     w, h = 1920, 1080
     set_sky, sky_desc = sky_case("atmosphere128")
     frames = [scenes.camera_frame(cam, w, h), scenes.camera_frame(dict(position=(34.0, 24.0, -30.0), view_dir=(-0.7, -0.35, 0.6)), w, h)]

@@ -17,48 +17,12 @@ import pytest
 import oracle_lib as ol
 import vxgi_ref64 as r
 from idkengine_b200 import gpu_types as gt, host, scenes, vxgi
+from raster_lib import FILLS, GRID_MAX, GRID_MIN, check_voxelized, level0_fill, lit_cornell, synthetic_chain
 
-GRID_MIN, GRID_MAX = (-1.2, -0.2, -1.2), (1.2, 2.2, 1.2)
 SKY = (0.6, 0.7, 0.9)
 
 SHAPES = [(1, 1, 1), (1, 1, 2), (3, 1, 7), (5, 33, 2), (40, 56, 30), (384, 384, 384), (2048, 1, 1)]
 MIP_SHAPES = [s for s in SHAPES if s != (384, 384, 384)] + [(7, 3, 129), (1, 64, 3)]
-FILLS = ["random", "sparse", "zeros", "subnormal", "near_max", "inf"]
-
-
-def lit_cornell():
-    scene, cam = scenes.cornell_1k(threads=1)
-    scene.add_light((0.0, 1.6, 0.3), (6.0, 5.5, 5.0), 0.2)
-    scene.add_light((-0.6, 0.5, 0.6), (0.5, 0.8, 3.0), 0.1)
-    return scene, cam
-
-
-def level0_fill(shape, fill, seed=0):
-    """A synthetic level 0 (float16 [d, h, w, 4]) of one of FILLS."""
-    w, h, d = shape
-    rng = np.random.default_rng(seed + 7919 * FILLS.index(fill))
-    n = (d, h, w, 4)
-    if fill == "random":
-        return rng.uniform(0.0, 4.0, n).astype(np.float16)
-    if fill == "sparse":                     # voxeliser-like: alpha 0 or 1, rgb only where occupied
-        occ = rng.random((d, h, w)) < 0.15
-        out = np.zeros(n, np.float16)
-        out[occ, :3] = rng.uniform(0.0, 20.0, (int(occ.sum()), 3)).astype(np.float16)
-        out[occ, 3] = 1.0
-        return out
-    if fill == "zeros":
-        return np.zeros(n, np.float16)
-    if fill == "subnormal":                  # every float16 subnormal is a bit pattern 1 .. 1023
-        return rng.integers(0, 1024, n).astype(np.uint16).view(np.float16)
-    if fill == "near_max":
-        return rng.uniform(60000.0, 65504.0, n).astype(np.float16)
-    if fill == "inf":
-        out = rng.uniform(0.0, 8.0, n).astype(np.float16)
-        out[rng.random(n) < 0.02] = np.inf
-        return out
-    raise ValueError(fill)
-
-
 def check_chain(levels, shape):
     """Every level of an oracle (or kernel) chain against mip64 of the chain's own level below: within 1 ulp, and at most
     0.1 % of the texels differing at all (at least 4: fp32 rounding moves a texel by one ulp where the exact value lies next
@@ -169,18 +133,6 @@ def cornell_gbuffer(w, h, metal_rough=None, seed=0):
 
 def cone_settings(max_samples=4, step_multiplier=0.16, normal_ray_offset=1.0, noise_index=0, gi_boost=1.3, sky_boost=1.0 / 1.3):
     return vxgi.IdkVxConeSettings(max_samples, step_multiplier, gi_boost, sky_boost, normal_ray_offset, noise_index)
-
-
-def synthetic_chain(ci, kind, seed=0):
-    """A mip chain (levels, raw) from a synthetic level 0: 'sparse' (voxeliser-like occupancy), 'dense' (random alpha)."""
-    w, h, d = ci.Width, ci.Height, ci.Depth
-    if kind == "sparse":
-        level0 = level0_fill((w, h, d), "sparse", seed)
-        level0[..., :3] = (level0[..., :3].astype(np.float32) * 0.1).astype(np.float16)
-    else:
-        rng = np.random.default_rng(seed)
-        level0 = np.concatenate([rng.uniform(0, 0.3, (d, h, w, 3)), rng.uniform(0, 0.2, (d, h, w, 1))], -1).astype(np.float16)
-    return ol.vx_mipmap(ci, level0)
 
 
 def compare_cone_trace(ci, levels, raw, frame, st, depth, nrg, mr, eps=1e-6, rtol=1e-3, min_fraction=0.9):
@@ -334,22 +286,6 @@ def test_cone_trace_exact_decisions(name):
 
 
 # ---------------------------------------------------------------------------------------------------------- voxelisation
-def check_voxelized(level0, frags, v, max_ambiguous_fraction):
-    """A voxelised level 0 and its fragment count against voxelize64's result v: occupancy equal on every unambiguous voxel,
-    rgb there within 1 ulp, at most max_ambiguous_fraction of the occupied voxels ambiguous, and the fragment counts apart
-    by no more than the ambiguous samples."""
-    occ = level0[..., 3] != 0
-    assert np.all(level0[occ][:, 3] == 1.0)
-    clear = ~v["ambiguous"]
-    assert np.array_equal(occ & clear, v["written"] & clear)
-    both = occ & v["written"] & clear
-    u = r.half_ulp_distance(level0[both][:, :3], v["level0"][both][:, :3])
-    assert u.max() <= 1.0, u.max()
-    amb = int((v["ambiguous"] & occ).sum())
-    assert amb <= max_ambiguous_fraction * occ.sum(), (amb, int(occ.sum()))
-    assert abs(frags - v["fragments"]) <= v["ambiguous_samples"], (frags, v["fragments"], v["ambiguous_samples"])
-
-
 def compare_voxelize(scene, ci, max_ambiguous_fraction):
     levels, _, frags = ol.vx_voxelize(scene, ci)
     v = r.voxelize64(scene, ci)

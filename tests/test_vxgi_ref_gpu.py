@@ -7,22 +7,10 @@ import pytest
 import oracle_lib as ol
 import vxgi_ref64 as r
 from idkengine_b200 import vxgi
-from test_vxgi_ref import (EXACT, GRID_MAX, GRID_MIN, MIP_SHAPES, PROBES, SKY, check_chain, check_voxelized, compare_cone_trace,
-                           cone_settings, cornell_gbuffer, level0_fill, lit_cornell, probe_case, synthetic_chain)
+from raster_lib import GRID_MAX, GRID_MIN, check_voxelized, level0_fill, lit_cornell, synthetic_chain, write_level
+from test_vxgi_ref import EXACT, MIP_SHAPES, PROBES, SKY, check_chain, compare_cone_trace, cone_settings, cornell_gbuffer, probe_case
 
 pytestmark = pytest.mark.gpu
-
-
-def write_level(vx, level, data):
-    """Copies a float16 [d, h, w, 4] level into the context's grid with torch."""
-    import torch
-    from idkengine_b200 import multigpu
-    ptr, nbytes = vx.LevelDevicePtr(level)
-    data = np.ascontiguousarray(data, np.float16).reshape(-1).view(np.int16)
-    assert nbytes == data.nbytes
-    vx.ReadLevel(len(vx.sizes) - 1)          # synchronises the context's stream (the grid's initial clear runs on it)
-    torch.as_tensor(multigpu.DeviceArray(ptr, (data.size,), "<i2"), device="cuda").copy_(torch.from_numpy(data))
-    torch.cuda.synchronize()
 
 
 def gpu_chain(vx, level0):
