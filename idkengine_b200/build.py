@@ -54,11 +54,12 @@ def find_nvcc():
 
 def build_host(force=False, verbose=False):
     srcs = _sources(HOST_DIR, (".cpp",))
-    deps = srcs + _sources(INCLUDE_DIR, (".h",))
+    # the builder's arithmetic is shared with libidkpt: an edit to it must rebuild both libraries
+    deps = srcs + _sources(INCLUDE_DIR, (".h",)) + [os.path.join(CSRC_DIR, "idk_bvh_math.h"), os.path.join(CSRC_DIR, "idk_cbrt.h")]
     if not force and _newer(LIBIDKHOST, deps):
         return LIBIDKHOST
     cmd = ["g++", "-O2", "-std=c++17", "-ffp-contract=off", "-fPIC", "-shared", "-pthread",
-           "-fvisibility=hidden", "-I", INCLUDE_DIR, "-o", LIBIDKHOST] + srcs
+           "-fvisibility=hidden", "-I", INCLUDE_DIR, "-I", CSRC_DIR, "-o", LIBIDKHOST] + srcs
     if verbose:
         print(" ".join(cmd))
     subprocess.run(cmd, check=True)

@@ -11,6 +11,11 @@
 //      trySplit). Node ids do not depend on the order nodes are split in.
 //   4. post passes [computeRequiredStackSize, optimizeStackSize, removeEmptySubtrees, unindex*, computeGlobalSAH]: parallel
 //      except for the double sums, which one thread adds in the mirror's DFS order.
+//
+// The scalar arithmetic comes from idk_bvh_math.h, which the mirror compiles too: boxes, Triangle.Split, the priority, the
+// split count, one pre-split step, the serial trySplit (stage 3's one-thread subtrees), the leaf-cost test and side swap that
+// end k_split_large, and the SAH and collapse terms. This file keeps the kernels, the block scans and partitions, the
+// post-pass kernels and the driver.
 #pragma once
 #include <cfloat>
 #include <climits>
@@ -22,7 +27,7 @@
 #include <cub/cub.cuh>
 
 #include "../../include/idk_gpu_types.h"
-#include "idk_cbrt.h"
+#include "idk_bvh_math.h"
 
 namespace idkbb {
 
@@ -33,96 +38,22 @@ constexpr int BIG_TILE = BIG_THREADS * BIG_ITEMS;
 constexpr int MAX_FRAGMENTS = 1 << 24;  // float counters are exact up to here
 constexpr int DEPTH_NONE = 0x7F7F7F7F;  // memset byte 0x7F: larger than any depth
 
-struct Params {
-    int stopSplittingThreshold, maxLeafTriangleCount;
-    float triangleCost;
-    int stackOptThreshold;
-    float stackOptSahIncreaseAcceptance, splitFactor;
-    int doPreSplit;
-};
+using namespace idkbvh;
 
-struct FBox { float mn[3], mx[3]; };
-
-// Vector128.MinNative / MaxNative: (a < b) ? a : b. Folding a sequence with them keeps, among equal values, the last one
-// (which matters for +-0), and the operation is associative, so a scan that combines (earlier, later) in order is exact.
-__device__ __forceinline__ float minN(float a, float b) { return a < b ? a : b; }
-__device__ __forceinline__ float maxN(float a, float b) { return a > b ? a : b; }
-__device__ __forceinline__ FBox boxEmpty() { return {{FLT_MAX, FLT_MAX, FLT_MAX}, {-FLT_MAX, -FLT_MAX, -FLT_MAX}}; }
-// exact identity of the ordered combine (for padding partial tiles); the mirror's Box::empty() is a real first element
-__device__ __forceinline__ FBox boxIdentity() { return {{INFINITY, INFINITY, INFINITY}, {-INFINITY, -INFINITY, -INFINITY}}; }
-__device__ __forceinline__ FBox combine(const FBox& a, const FBox& b) {
-    FBox r;
-#pragma unroll
-    for (int i = 0; i < 3; i++) { r.mn[i] = minN(a.mn[i], b.mn[i]); r.mx[i] = maxN(a.mx[i], b.mx[i]); }
-    return r;
-}
-__device__ __forceinline__ float halfArea(const FBox& b) {   // MyMath.HalfArea
-    const float sx = b.mx[0] - b.mn[0], sy = b.mx[1] - b.mn[1], sz = b.mx[2] - b.mn[2];
-    return fmaf(sx + sy, sz, sx * sy);
-}
-__device__ __forceinline__ float nodeHalfArea(const GpuBlasNode& n) {
-    const float sx = n.Max[0] - n.Min[0], sy = n.Max[1] - n.Min[1], sz = n.Max[2] - n.Min[2];
-    return fmaf(sx + sy, sz, sx * sy);
-}
-__device__ __forceinline__ FBox loadBox(const FBox* b, int i) {
-    const float2* p = reinterpret_cast<const float2*>(b + i);
-    const float2 a = p[0], c = p[1], d = p[2];
-    return {{a.x, a.y, c.x}, {c.y, d.x, d.y}};
-}
-__device__ __forceinline__ void storeBox(FBox* b, size_t i, const FBox& v) {
+// exact identity of the ordered combine (for padding partial tiles); boxEmpty() is a real first element
+__device__ __forceinline__ Box boxIdentity() { return {{INFINITY, INFINITY, INFINITY}, {-INFINITY, -INFINITY, -INFINITY}}; }
+__device__ __forceinline__ void storeBox(Box* b, size_t i, const Box& v) {
     float2* p = reinterpret_cast<float2*>(b + i);
     p[0] = make_float2(v.mn[0], v.mn[1]); p[1] = make_float2(v.mn[2], v.mx[0]); p[2] = make_float2(v.mx[1], v.mx[2]);
 }
-__device__ __forceinline__ void setBounds(GpuBlasNode& n, const FBox& b) {
-    for (int i = 0; i < 3; i++) { n.Min[i] = b.mn[i]; n.Max[i] = b.mx[i]; }
-}
-__device__ __forceinline__ uint32_t floatToKey(float v) {
-    const uint32_t f = __float_as_uint(v);
-    return f ^ (uint32_t)(((int32_t)f >> 31) | (int32_t)0x80000000);
-}
-__device__ __forceinline__ int csFloatToInt(float f) {   // (int)float in C# on x86-64: NaN / out of range -> INT_MIN
-    if (!(f > -2147483904.0f && f < 2147483648.0f)) return INT_MIN;
-    return (int)f;
-}
 
 // ---------------------------------------------------------------------------------------------------------------- pre-split
-struct V3 { float v[3]; };
-struct Tri { V3 p[3]; };
 __device__ __forceinline__ Tri loadTri(const PackedVec3* pos, const GpuBlasTriangle* tris, int i) {
     const GpuBlasTriangle t = tris[i];
     const int id[3] = {t.X, t.Y, t.Z};
     Tri r;
     for (int k = 0; k < 3; k++) { const PackedVec3 q = pos[(uint32_t)id[k]]; r.p[k] = {{q.x, q.y, q.z}}; }
     return r;
-}
-__device__ __forceinline__ void grow(FBox& b, const V3& p) {
-    for (int i = 0; i < 3; i++) { b.mn[i] = minN(b.mn[i], p.v[i]); b.mx[i] = maxN(b.mx[i], p.v[i]); }
-}
-__device__ __forceinline__ FBox boxFromTri(const Tri& t) {
-    FBox b = {{t.p[0].v[0], t.p[0].v[1], t.p[0].v[2]}, {t.p[0].v[0], t.p[0].v[1], t.p[0].v[2]}};
-    grow(b, t.p[1]);
-    grow(b, t.p[2]);
-    return b;
-}
-__device__ __forceinline__ float boxSize(const FBox& b, int i) { return b.mx[i] - b.mn[i]; }
-__device__ __forceinline__ float largestExtent(const FBox& b) { return maxN(boxSize(b, 0), maxN(boxSize(b, 1), boxSize(b, 2))); }
-__device__ __forceinline__ int largestAxis(const FBox& b) {
-    int axis = 0;
-    if (boxSize(b, 0) < boxSize(b, 1)) axis = 1;
-    if (boxSize(b, axis) < boxSize(b, 2)) axis = 2;
-    return axis;
-}
-
-__device__ float priority(const Tri& t) {   // PreSplitting.GetPriority
-    const FBox b = boxFromTri(t);
-    const float le = largestExtent(b);
-    const float extentPrio = le * le;
-    float e1[3], e2[3];
-    for (int i = 0; i < 3; i++) { e1[i] = t.p[1].v[i] - t.p[0].v[i]; e2[i] = t.p[2].v[i] - t.p[0].v[i]; }
-    const float cx = e1[1] * e2[2] - e1[2] * e2[1], cy = e1[2] * e2[0] - e1[0] * e2[2], cz = e1[0] * e2[1] - e1[1] * e2[0];
-    const float triArea = sqrtf(cx * cx + cy * cy + cz * cz) * 0.5f;
-    const float emptyAreaPrio = halfArea(b) * 2.0f - triArea;
-    return idk_cbrtf(extentPrio * emptyAreaPrio);
 }
 
 __global__ void k_priorities(const PackedVec3* pos, const GpuBlasTriangle* tris, int n, float* prio) {
@@ -155,48 +86,27 @@ __global__ void k_split_counts(const float* prio, const float* total, int n, flo
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i > n) return;
     if (i == n) { counts[n] = 0; return; }
-    const float shareOfTris = prio[i] / *total * (float)n;
-    int c = csFloatToInt(shareOfTris * splitFactor);
-    if (c == INT_MIN || c < 0) c = 0;    // the mirror's guard for degenerate input
-    counts[i] = 1ull + (unsigned long long)c;
+    counts[i] = splitCount(prio[i], *total, n, splitFactor);
 }
 
 // Box of every vertex in triangle order (p0, p1, p2 of each): per-thread chunks folded in order, chunks combined in order.
-__global__ void __launch_bounds__(1024) k_global_box(const PackedVec3* pos, const GpuBlasTriangle* tris, int n, FBox* out) {
-    __shared__ FBox part[1024];
+__global__ void __launch_bounds__(1024) k_global_box(const PackedVec3* pos, const GpuBlasTriangle* tris, int n, Box* out) {
+    __shared__ Box part[1024];
     __shared__ int has[1024];
     const int per = (n + 1023) / 1024;
     const int b0 = min(n, threadIdx.x * per), e0 = min(n, b0 + per);
-    FBox acc = boxIdentity();
+    Box acc = boxIdentity();
     for (int i = b0; i < e0; i++) {
         const Tri t = loadTri(pos, tris, i);
-        for (int k = 0; k < 3; k++) { FBox p = {{t.p[k].v[0], t.p[k].v[1], t.p[k].v[2]}, {t.p[k].v[0], t.p[k].v[1], t.p[k].v[2]}}; acc = combine(acc, p); }
+        for (int k = 0; k < 3; k++) { Box p = {{t.p[k].v[0], t.p[k].v[1], t.p[k].v[2]}, {t.p[k].v[0], t.p[k].v[1], t.p[k].v[2]}}; acc = combine(acc, p); }
     }
     part[threadIdx.x] = acc;
     has[threadIdx.x] = e0 > b0;
     __syncthreads();
     if (threadIdx.x == 0) {
-        FBox g = boxEmpty();
+        Box g = boxEmpty();
         for (int t = 0; t < 1024; t++) if (has[t]) g = combine(g, part[t]);
         *out = g;
-    }
-}
-
-__device__ __forceinline__ void triSplit(const Tri& t, int axis, float position, FBox& l, FBox& r) {   // Triangle.Split
-    l = boxEmpty();
-    r = boxEmpty();
-    const bool q[3] = {t.p[0].v[axis] <= position, t.p[1].v[axis] <= position, t.p[2].v[axis] <= position};
-    for (int k = 0; k < 3; k++) { if (q[k]) grow(l, t.p[k]); else grow(r, t.p[k]); }
-    for (int k = 0; k < 3; k++) {
-        const int k1 = (k + 1) % 3;
-        if (q[k] ^ q[k1]) {
-            const V3 a = t.p[k], b = t.p[k1];
-            const float tt = (position - a.v[axis]) / (b.v[axis] - a.v[axis]);
-            V3 m;
-            for (int i = 0; i < 3; i++) m.v[i] = a.v[i] + tt * (b.v[i] - a.v[i]);
-            grow(l, m);
-            grow(r, m);
-        }
     }
 }
 
@@ -204,10 +114,10 @@ __device__ __forceinline__ void triSplit(const Tri& t, int axis, float position,
 // down from its end: the stack's items hold at least one fragment each and together exactly the ones not yet written, so
 // they never reach the slot the next fragment goes to. Item j: box in bounds[end-1-j], split count in ids[end-1-j].
 __global__ void k_presplit(const PackedVec3* pos, const GpuBlasTriangle* tris, int n, const unsigned long long* off,
-                           const FBox* globalBox, FBox* bounds, int* origIds) {
+                           const Box* globalBox, Box* bounds, int* origIds) {
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= n) return;
-    const FBox g = *globalBox;
+    const Box g = *globalBox;
     const Tri tri = loadTri(pos, tris, i);
     const size_t begin = (size_t)off[i], end = (size_t)off[i + 1];
     size_t counter = begin;
@@ -217,7 +127,7 @@ __global__ void k_presplit(const PackedVec3* pos, const GpuBlasTriangle* tris, i
     sp = 1;
     while (sp > 0) {
         sp--;
-        const FBox box = loadBox(bounds, (int)(end - 1 - sp));
+        const Box box = loadBox(bounds, (int)(end - 1 - sp));
         const int splits = origIds[end - 1 - sp];
         if (splits == 1) {
             storeBox(bounds, counter, box);
@@ -225,24 +135,8 @@ __global__ void k_presplit(const PackedVec3* pos, const GpuBlasTriangle* tris, i
             counter++;
             continue;
         }
-        const int axis = largestAxis(box);
-        const float le = largestExtent(box);
-        const float globalSize = g.mx[axis] - g.mn[axis];
-        const float alpha = le / globalSize;   // getNodeSize: the power of two below alpha, times globalSize
-        float nodeSize = __uint_as_float(__float_as_uint(alpha) & (255u << 23)) * globalSize;
-        if (nodeSize >= le - 0.0001f) nodeSize *= 0.5f;
-        const float midPos = (box.mn[axis] + box.mx[axis]) * 0.5f;
-        const float index = rintf((midPos - g.mn[axis]) / nodeSize);   // MathF.Round: half to even
-        const float splitPos = g.mn[axis] + index * nodeSize;
-        FBox l, r;
-        triSplit(tri, axis, splitPos, l, r);
-        for (int k = 0; k < 3; k++) {   // clip to the item's box
-            l.mn[k] = maxN(l.mn[k], box.mn[k]); l.mx[k] = minN(l.mx[k], box.mx[k]);
-            r.mn[k] = maxN(r.mn[k], box.mn[k]); r.mx[k] = minN(r.mx[k], box.mx[k]);
-        }
-        const float leftExtent = largestExtent(l), rightExtent = largestExtent(r);
-        int leftCount = csFloatToInt((float)splits * (leftExtent / (leftExtent + rightExtent)));
-        leftCount = min(max(leftCount, 1), splits - 1);
+        Box l, r;
+        const int leftCount = presplitStep(tri, box, splits, g, l, r);
         storeBox(bounds, end - 1 - sp, r);
         origIds[end - 1 - sp] = splits - leftCount;
         sp++;
@@ -252,22 +146,22 @@ __global__ void k_presplit(const PackedVec3* pos, const GpuBlasTriangle* tris, i
     }
 }
 
-__global__ void k_tri_bounds(const PackedVec3* pos, const GpuBlasTriangle* tris, int n, FBox* bounds) {
+__global__ void k_tri_bounds(const PackedVec3* pos, const GpuBlasTriangle* tris, int n, Box* bounds) {
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i < n) storeBox(bounds, i, boxFromTri(loadTri(pos, tris, i)));
 }
 
-__global__ void k_sort_keys(const FBox* bounds, int n, int axis, uint32_t* keys, int* vals) {
+__global__ void k_sort_keys(const Box* bounds, int n, int axis, uint32_t* keys, int* vals) {
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= n) return;
-    const FBox b = loadBox(bounds, i);
+    const Box b = loadBox(bounds, i);
     keys[i] = floatToKey(b.mn[axis] + b.mx[axis]);
     vals[i] = i;
 }
 
 // ---------------------------------------------------------------------------------------------------------------- tree
 struct TreeArgs {
-    const FBox* bounds;
+    const Box* bounds;
     int* ids[3];
     int* aux;
     uint8_t* table;
@@ -309,36 +203,36 @@ __device__ __forceinline__ void writeChildren(const TreeArgs& a, int pid, int2 t
 }
 
 // ---- block-wide ordered scans
-__device__ __forceinline__ FBox shflUpBox(const FBox& v, int o) {
-    FBox r;
+__device__ __forceinline__ Box shflUpBox(const Box& v, int o) {
+    Box r;
     for (int i = 0; i < 3; i++) { r.mn[i] = __shfl_up_sync(0xffffffffu, v.mn[i], o); r.mx[i] = __shfl_up_sync(0xffffffffu, v.mx[i], o); }
     return r;
 }
 
 // Exclusive ordered scan of one box per thread over the block; `total` is the fold of all of them.
-__device__ FBox blockScanBox(FBox v, FBox& total) {
-    __shared__ FBox warpTot[BIG_THREADS / 32];
-    __shared__ FBox warpPre[BIG_THREADS / 32];
-    __shared__ FBox all;
+__device__ Box blockScanBox(Box v, Box& total) {
+    __shared__ Box warpTot[BIG_THREADS / 32];
+    __shared__ Box warpPre[BIG_THREADS / 32];
+    __shared__ Box all;
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-    FBox inc = v;
+    Box inc = v;
 #pragma unroll
     for (int o = 1; o < 32; o <<= 1) {
-        const FBox other = shflUpBox(inc, o);
+        const Box other = shflUpBox(inc, o);
         if (lane >= o) inc = combine(other, inc);
     }
-    FBox exc = shflUpBox(inc, 1);
+    Box exc = shflUpBox(inc, 1);
     if (lane == 0) exc = boxIdentity();
     if (lane == 31) warpTot[warp] = inc;
     __syncthreads();
     if (threadIdx.x == 0) {
-        FBox acc = boxIdentity();
+        Box acc = boxIdentity();
         for (int w = 0; w < BIG_THREADS / 32; w++) { warpPre[w] = acc; acc = combine(acc, warpTot[w]); }
         all = acc;
     }
     __syncthreads();
     total = all;
-    const FBox r = combine(warpPre[warp], exc);
+    const Box r = combine(warpPre[warp], exc);
     __syncthreads();   // the shared words are reused by the next call
     return r;
 }
@@ -380,15 +274,15 @@ __device__ unsigned long long blockMinU64(unsigned long long v) {
 }
 
 // computeBoundingBox: Box::empty() grown by the fragments [lo, hi) of `ids` in order.
-__device__ FBox blockRangeBox(const FBox* bounds, const int* ids, int lo, int hi) {
-    FBox carry = boxEmpty();
+__device__ Box blockRangeBox(const Box* bounds, const int* ids, int lo, int hi) {
+    Box carry = boxEmpty();
     for (int base = lo; base < hi; base += BIG_TILE) {
-        FBox loc = boxIdentity();
+        Box loc = boxIdentity();
         for (int k = 0; k < BIG_ITEMS; k++) {
             const int i = base + threadIdx.x * BIG_ITEMS + k;
             if (i < hi) loc = combine(loc, loadBox(bounds, ids[i]));
         }
-        FBox total;
+        Box total;
         blockScanBox(loc, total);
         carry = combine(carry, total);
     }
@@ -426,7 +320,7 @@ __global__ void __launch_bounds__(BIG_THREADS) k_split_large(TreeArgs a) {
     const int2 task = a.tasks[blockIdx.x];
     const int pid = task.x;
     const int start = a.nodes[pid].TriStartOrChild, count = a.nodes[pid].TriCount, end = start + count;
-    const FBox pbox = blockRangeBox(a.bounds, a.ids[0], start, end);
+    const Box pbox = blockRangeBox(a.bounds, a.ids[0], start, end);
     if (threadIdx.x == 0) setBounds(a.nodes[pid], pbox);
     if (count <= a.p.stopSplittingThreshold) return;
 
@@ -435,17 +329,17 @@ __global__ void __launch_bounds__(BIG_THREADS) k_split_large(TreeArgs a) {
     for (int axis = 0; axis < 3; axis++) {
         const int* ids = a.ids[axis];
         // suffix: R[i] = HalfArea(box of [i, end)) * (end - i), i in [start + 1, end)
-        FBox carry = boxEmpty();
+        Box carry = boxEmpty();
         for (int jb = 0; jb < count - 1; jb += BIG_TILE) {
-            FBox b[BIG_ITEMS];
-            FBox loc = boxIdentity();
+            Box b[BIG_ITEMS];
+            Box loc = boxIdentity();
             for (int k = 0; k < BIG_ITEMS; k++) {
                 const int j = jb + threadIdx.x * BIG_ITEMS + k;
                 b[k] = j < count - 1 ? loadBox(a.bounds, ids[end - 1 - j]) : boxIdentity();
                 loc = combine(loc, b[k]);
             }
-            FBox total;
-            FBox acc = combine(carry, blockScanBox(loc, total));
+            Box total;
+            Box acc = combine(carry, blockScanBox(loc, total));
             for (int k = 0; k < BIG_ITEMS; k++) {
                 const int j = jb + threadIdx.x * BIG_ITEMS + k;
                 acc = combine(acc, b[k]);
@@ -458,15 +352,15 @@ __global__ void __launch_bounds__(BIG_THREADS) k_split_large(TreeArgs a) {
         unsigned long long best = ~0ull;
         carry = boxEmpty();
         for (int base = start; base < end - 1; base += BIG_TILE) {
-            FBox b[BIG_ITEMS];
-            FBox loc = boxIdentity();
+            Box b[BIG_ITEMS];
+            Box loc = boxIdentity();
             for (int k = 0; k < BIG_ITEMS; k++) {
                 const int i = base + threadIdx.x * BIG_ITEMS + k;
                 b[k] = i < end - 1 ? loadBox(a.bounds, ids[i]) : boxIdentity();
                 loc = combine(loc, b[k]);
             }
-            FBox total;
-            FBox acc = combine(carry, blockScanBox(loc, total));
+            Box total;
+            Box acc = combine(carry, blockScanBox(loc, total));
             for (int k = 0; k < BIG_ITEMS; k++) {
                 const int i = base + threadIdx.x * BIG_ITEMS + k;
                 acc = combine(acc, b[k]);
@@ -483,20 +377,15 @@ __global__ void __launch_bounds__(BIG_THREADS) k_split_large(TreeArgs a) {
             if (c < bestCost) { bestCost = c; bestAxis = axis; bestSplit = (int)(uint32_t)best; }
         }
     }
-    if (bestCost == FLT_MAX) { bestAxis = 0; bestSplit = start + count / 2; }   // the mirror's guard for non-finite costs
-    if (count <= a.p.maxLeafTriangleCount) {
-        const float notSplitCost = a.p.triangleCost * (float)count;
-        const float newCost = 1.0f + (a.p.triangleCost * bestCost / halfArea(pbox));
-        if (newCost >= notSplitCost) return;
-    }
+    if (!keepSplit(a.p, pbox, start, count, bestCost, bestAxis, bestSplit)) return;
     int* ids = a.ids[bestAxis];
-    const FBox lbox = blockRangeBox(a.bounds, ids, start, bestSplit);
-    const FBox rbox = blockRangeBox(a.bounds, ids, bestSplit, end);
-    const bool swapSides = halfArea(lbox) < halfArea(rbox);   // the larger child goes left
-    for (int i = start + threadIdx.x; i < end; i += BIG_THREADS) a.table[ids[i]] = i < bestSplit ? !swapSides : swapSides;
+    const Box lbox = blockRangeBox(a.bounds, ids, start, bestSplit);
+    const Box rbox = blockRangeBox(a.bounds, ids, bestSplit, end);
+    const bool swap = swapSides(lbox, rbox);
+    for (int i = start + threadIdx.x; i < end; i += BIG_THREADS) a.table[ids[i]] = i < bestSplit ? !swap : swap;
     __syncthreads();
-    const int ones = swapSides ? end - bestSplit : bestSplit - start;
-    if (swapSides) blockPartition(ids, a.aux, a.table, start, end, ones);
+    const int ones = swap ? end - bestSplit : bestSplit - start;
+    if (swap) blockPartition(ids, a.aux, a.table, start, end, ones);
     blockPartition(a.ids[(bestAxis + 1) % 3], a.aux, a.table, start, end, ones);
     blockPartition(a.ids[(bestAxis + 2) % 3], a.aux, a.table, start, end, ones);
     if (threadIdx.x == 0) {
@@ -508,70 +397,7 @@ __global__ void __launch_bounds__(BIG_THREADS) k_split_large(TreeArgs a) {
     }
 }
 
-// ---- one thread per subtree: the mirror's processSubtree and trySplit, line for line
-__device__ FBox rangeBox(const FBox* bounds, const int* ids, int lo, int hi) {
-    FBox b = boxEmpty();
-    for (int i = lo; i < hi; i++) b = combine(b, loadBox(bounds, ids[i]));
-    return b;
-}
-
-__device__ int stablePartition(int* source, int count, int* aux, const uint8_t* table) {
-    int l = 0, r = 0;
-    for (int i = 0; i < count; i++) {
-        const int id = source[i];
-        if (table[id]) source[l++] = id; else aux[r++] = id;
-    }
-    for (int i = 0; i < r; i++) source[l + i] = aux[i];
-    return l;
-}
-
-// returns the split index, or -1 for a leaf
-__device__ int trySplitSerial(const TreeArgs& a, const FBox& parentBox, int start, int count) {
-    if (count <= a.p.stopSplittingThreshold) return -1;
-    const int end = start + count;
-    float bestCost = FLT_MAX;
-    int bestAxis = 0, bestSplit = 0;
-    for (int axis = 0; axis < 3; axis++) {
-        const int* ids = a.ids[axis];
-        int firstRight = start + 1;
-        FBox rightAcc = boxEmpty();
-        float rightCounter = 0.0f;
-        for (int i = end - 1; i >= firstRight; i--) {
-            rightCounter++;
-            rightAcc = combine(rightAcc, loadBox(a.bounds, ids[i]));
-            const float rightCost = halfArea(rightAcc) * rightCounter;
-            a.rcost[i] = rightCost;
-            if (rightCost >= bestCost) { firstRight = i + 1; break; }
-        }
-        FBox leftAcc = boxEmpty();
-        float leftCounter = (float)(firstRight - start) - 1.0f;
-        for (int i = start; i < firstRight - 1; i++) leftAcc = combine(leftAcc, loadBox(a.bounds, ids[i]));
-        for (int i = firstRight - 1; i < end - 1; i++) {
-            leftCounter++;
-            leftAcc = combine(leftAcc, loadBox(a.bounds, ids[i]));
-            const float leftCost = halfArea(leftAcc) * leftCounter;
-            const float cost = leftCost + a.rcost[i + 1];
-            if (cost < bestCost) { bestSplit = i + 1; bestAxis = axis; bestCost = cost; }
-            else if (leftCost >= bestCost) break;
-        }
-    }
-    if (bestCost == FLT_MAX) { bestAxis = 0; bestSplit = start + count / 2; }
-    if (count <= a.p.maxLeafTriangleCount) {
-        const float notSplitCost = a.p.triangleCost * (float)count;
-        const float newCost = 1.0f + (a.p.triangleCost * bestCost / halfArea(parentBox));
-        if (newCost >= notSplitCost) return -1;
-    }
-    int* ids = a.ids[bestAxis];
-    const bool swapSides = halfArea(rangeBox(a.bounds, ids, start, bestSplit)) < halfArea(rangeBox(a.bounds, ids, bestSplit, end));
-    for (int i = start; i < bestSplit; i++) a.table[ids[i]] = !swapSides;
-    for (int i = bestSplit; i < end; i++) a.table[ids[i]] = swapSides;
-    int* aux = a.aux + start;
-    if (swapSides) bestSplit = start + stablePartition(ids + start, count, aux, a.table);
-    stablePartition(a.ids[(bestAxis + 1) % 3] + start, count, aux, a.table);
-    stablePartition(a.ids[(bestAxis + 2) % 3] + start, count, aux, a.table);
-    return bestSplit;
-}
-
+// ---- one thread per subtree: the mirror's processSubtree around the shared serial trySplit
 __global__ void k_split_small(TreeArgs a, int n) {
     const int t = blockIdx.x * blockDim.x + threadIdx.x;
     if (t >= n) return;
@@ -582,9 +408,9 @@ __global__ void k_split_small(TreeArgs a, int n) {
         const int2 task = stack[--sp];
         GpuBlasNode& parent = a.nodes[task.x];
         const int start = parent.TriStartOrChild, count = parent.TriCount;
-        const FBox box = rangeBox(a.bounds, a.ids[0], start, start + count);
+        const Box box = rangeBox(a.bounds, a.ids[0], start, start + count);
         setBounds(parent, box);
-        const int split = trySplitSerial(a, box, start, count);
+        const int split = trySplitSerial(a.bounds, a.ids, a.rcost, a.table, a.aux, a.p, box, start, count);
         if (split < 0) continue;
         writeChildren(a, task.x, task, start, count, split);
         const int lc = split - start;
@@ -659,9 +485,7 @@ __global__ void k_sah_terms(const int* order, int m, const GpuBlasNode* nodes, c
     const int v = order[j];
     const GpuBlasNode n = final ? final[fidx[v]] : nodes[v];
     const GpuBlasNode root = final ? final[1] : nodes[1];
-    const double rootArea = 1.0 / (double)nodeHalfArea(root);
-    const double prob = (double)nodeHalfArea(n) * rootArea;
-    terms[j] = n.TriCount > 0 ? (double)(triangleCost * (float)n.TriCount) * prob : 1.0 * prob;
+    terms[j] = sahTerm(n, 1.0 / (double)nodeHalfArea(root), triangleCost);
 }
 
 // collapseDeepestLevel's cost terms, in pre-order (the nodes that add one never contain each other, so this is also the
@@ -678,10 +502,7 @@ __global__ void k_collapse_terms(const int* order, int m, const GpuBlasNode* nod
         const int c = n.TriStartOrChild;
         q = firstPass ? (depth[v] > level && nodes[c].TriCount > 0 && nodes[c + 1].TriCount > 0) : depth[v] == level;
         if (q) {
-            const int lc = ocount[c], rc = ocount[c + 1];
-            const double leavesCost = (double)triangleCost * ((double)lc * (double)nodeHalfArea(nodes[c]) + (double)rc * (double)nodeHalfArea(nodes[c + 1]));
-            const double newParentLeafCost = (double)triangleCost * (double)(lc + rc);
-            terms[j] = ((double)nodeHalfArea(n) * (newParentLeafCost - 1.0) - leavesCost) / (double)nodeHalfArea(nodes[1]);
+            terms[j] = collapseTerm(n, nodes[c], nodes[c + 1], ocount[c], ocount[c + 1], nodes[1], triangleCost);
         }
     }
     flags[j] = q;
@@ -911,7 +732,7 @@ static int build(cudaStream_t stream, const PackedVec3* hPos, uint64_t vertexCou
 
     // ---- 1. fragments
     int n = triCount;
-    FBox* bounds = nullptr;
+    Box* bounds = nullptr;
     int* origIds = nullptr;
     void* cubTemp = nullptr;
     size_t cubBytes = 0;
@@ -926,7 +747,7 @@ static int build(cudaStream_t stream, const PackedVec3* hPos, uint64_t vertexCou
         float* prio;
         float* total;
         unsigned long long *counts, *offsets;
-        FBox* gbox;
+        Box* gbox;
         BB_CK(ar.get(prio, triCount));
         BB_CK(ar.get(total, 1));
         BB_CK(ar.get(counts, (size_t)triCount + 1));
@@ -1116,7 +937,7 @@ static int build(cudaStream_t stream, const PackedVec3* hPos, uint64_t vertexCou
         double h[2];
         BB_CK(cudaMemcpyAsync(h, acc, sizeof(h), cudaMemcpyDeviceToHost, stream));
         BB_CK(cudaStreamSynchronize(stream));
-        // (the mirror's stackOptMaxLeafTriangleCount is INT_MAX: no collapse of at most 2^24 fragments exceeds it)
+        // (no collapse of at most 2^24 fragments exceeds STACK_OPT_MAX_LEAF_TRIANGLE_COUNT, so that test is not made here)
         double increasePercent = h[1] / h[0];
         while (increasePercent <= (double)p.stackOptSahIncreaseAcceptance && requiredStackSize > 0) {
             const int level = --requiredStackSize;

@@ -6,6 +6,7 @@
 // "one thread per node, leaves start the climb": no host pre-pass, no extra upload.
 #pragma once
 #include "idk_kernels.cuh"
+#include "idk_bvh_math.h"
 
 __device__ __forceinline__ uint32_t compress_sr11g11b10(f3 v) {
     // CompressSR11G11B10 (Compression.glsl:1-28). GLSL leaves round()'s half-way case to the implementation; this and the
@@ -142,7 +143,7 @@ __global__ void __launch_bounds__(256) k_refit_climb(RefitArgs a) {
 // scene never reads its roots back to the host. One CTA (instance counts are tens to thousands): the parallel parts are the
 // box transform, the Morton keys, the stable rank sort and the O(n * radius) neighbour search; the ordered placement of merged /
 // unmerged nodes runs on one thread, exactly as the reference's loop does, so the node array equals the host build bit for bit
-// (idkhost_tlas_build, tests/test_dynamic.py). HalfArea = fma(x + y, z, x * y) like MyMath.HalfArea.
+// (idkhost_tlas_build, tests/test_dynamic.py): both take the box, key and half-area arithmetic from idk_bvh_math.h.
 struct TlasBuildArgs {
     const float4* blasNodes;         // global GpuBlasNode array (2 x float4 each)
     const GpuBlasDesc* descs;
@@ -157,25 +158,11 @@ struct TlasBuildArgs {
     int n, searchRadius;
 };
 
-__device__ __forceinline__ float tlas_min(float a, float b) { return a < b ? a : b; }   // Box.GrowToFit semantics of the host mirror
-__device__ __forceinline__ float tlas_max(float a, float b) { return a > b ? a : b; }
-__device__ __forceinline__ uint32_t tlas_insert_two_zeros(uint32_t v) {
-    v = (v * 0x00010001u) & 0xFF0000FFu;
-    v = (v * 0x00000101u) & 0x0F00F00Fu;
-    v = (v * 0x00000011u) & 0xC30C30C3u;
-    v = (v * 0x00000005u) & 0x49249249u;
-    return v;
-}
-__device__ __forceinline__ uint32_t tlas_quant(float f) {
-    const float s = f * 1024.0f;
-    const uint32_t u = s <= 0.0f ? 0u : (s >= 4294967040.0f ? 0xFFFFFFFFu : (uint32_t)s);
-    return u < 1023u ? u : 1023u;
-}
-
 __global__ void __launch_bounds__(1024) k_tlas_build(TlasBuildArgs a) {
     __shared__ float s_min[3][32], s_max[3][32];
     __shared__ float s_gmin[3], s_gmax[3];
     __shared__ int s_range[2];
+    using namespace idkbvh;
     const int n = a.n, nodeCount = 2 * n - 1, tid = threadIdx.x, nt = blockDim.x;
     for (int i = tid; i < nodeCount; i += nt) { a.nodes[2 * i] = make_float4(0, 0, 0, 0); a.nodes[2 * i + 1] = make_float4(0, 0, 0, 0); }
     // ---- world-space box of every instance: Box.Transformed(BLAS root, ModelMatrix) = the 8 corners through the 3x4 matrix
@@ -186,16 +173,11 @@ __global__ void __launch_bounds__(1024) k_tlas_build(TlasBuildArgs a) {
         const float4 rA = root[0], rB = root[1];
         const float4* m = a.xforms + 9 * (size_t)bi.MeshTransformId;
         const float4 m0 = m[0], m1 = m[1], m2 = m[2];
-        float bmn[3] = {3.4028235e38f, 3.4028235e38f, 3.4028235e38f}, bmx[3] = {-3.4028235e38f, -3.4028235e38f, -3.4028235e38f};
-        for (int c = 0; c < 8; c++) {
-            const float x = (c & 1) ? rB.x : rA.x, y = (c & 2) ? rB.y : rA.y, z = (c & 4) ? rB.z : rA.z;
-            const float p[3] = {((x * m0.x + y * m0.y) + z * m0.z) + 1.0f * m0.w, ((x * m1.x + y * m1.y) + z * m1.z) + 1.0f * m1.w,
-                                ((x * m2.x + y * m2.y) + z * m2.z) + 1.0f * m2.w};
-            for (int k = 0; k < 3; k++) { bmn[k] = tlas_min(bmn[k], p[k]); bmx[k] = tlas_max(bmx[k], p[k]); }
-        }
-        a.leaves[2 * i] = make_float4(bmn[0], bmn[1], bmn[2], __uint_as_float(0x80000000u | (uint32_t)i));
-        a.leaves[2 * i + 1] = make_float4(bmx[0], bmx[1], bmx[2], 0.0f);
-        for (int k = 0; k < 3; k++) { lmn[k] = tlas_min(lmn[k], bmn[k]); lmx[k] = tlas_max(lmx[k], bmx[k]); }
+        const float m12[12] = {m0.x, m0.y, m0.z, m0.w, m1.x, m1.y, m1.z, m1.w, m2.x, m2.y, m2.z, m2.w};
+        const Box b = transformedBox({{rA.x, rA.y, rA.z}, {rB.x, rB.y, rB.z}}, m12);
+        a.leaves[2 * i] = make_float4(b.mn[0], b.mn[1], b.mn[2], __uint_as_float(0x80000000u | (uint32_t)i));
+        a.leaves[2 * i + 1] = make_float4(b.mx[0], b.mx[1], b.mx[2], 0.0f);
+        for (int k = 0; k < 3; k++) { lmn[k] = minN(lmn[k], b.mn[k]); lmx[k] = maxN(lmx[k], b.mx[k]); }
     }
     // global box: min / max are exact, so the reduction order does not matter
     for (int k = 0; k < 3; k++) {
@@ -213,15 +195,7 @@ __global__ void __launch_bounds__(1024) k_tlas_build(TlasBuildArgs a) {
     // ---- Morton code of the box centre mapped to [0, 1] by the global box (MyMath.GetMortonCode30 / MapToZeroOne)
     for (int i = tid; i < n; i += nt) {
         const float4 A = a.leaves[2 * i], B = a.leaves[2 * i + 1];
-        const float cA[3] = {A.x, A.y, A.z}, cB[3] = {B.x, B.y, B.z};
-        float mm[3];
-        for (int k = 0; k < 3; k++) {
-            const float c = (cB[k] + cA[k]) * 0.5f;
-            const float t = s_gmax[k] - s_gmin[k];
-            mm[k] = (c - s_gmin[k]) / t * (1.0f - 0.0f) + 0.0f;
-            if (t == 0.0f) mm[k] = 0.0f;
-        }
-        a.keys[i] = (tlas_insert_two_zeros(tlas_quant(mm[0])) << 2) | (tlas_insert_two_zeros(tlas_quant(mm[1])) << 1) | tlas_insert_two_zeros(tlas_quant(mm[2]));
+        a.keys[i] = centreKey({{A.x, A.y, A.z}, {B.x, B.y, B.z}}, {{s_gmin[0], s_gmin[1], s_gmin[2]}, {s_gmax[0], s_gmax[1], s_gmax[2]}});
     }
     __syncthreads();
     // ---- stable sort by key (rank sort): the leaf with rank r goes to nodes[nodeCount - n + r]
@@ -246,9 +220,7 @@ __global__ void __launch_bounds__(1024) k_tlas_build(TlasBuildArgs a) {
             for (int j = s; j < e; j++) {
                 if (j == node) continue;
                 const float4 oA = a.nodes[2 * j], oB = a.nodes[2 * j + 1];
-                const float sx = tlas_max(nB.x, oB.x) - tlas_min(nA.x, oA.x), sy = tlas_max(nB.y, oB.y) - tlas_min(nA.y, oA.y),
-                            sz = tlas_max(nB.z, oB.z) - tlas_min(nA.z, oA.z);
-                const float area = __fmaf_rn(sx + sy, sz, sx * sy);
+                const float area = halfArea(combine({{nA.x, nA.y, nA.z}, {nB.x, nB.y, nB.z}}, {{oA.x, oA.y, oA.z}, {oB.x, oB.y, oB.z}}));
                 if (area < smallest) { smallest = area; best = j; }
             }
             a.pref[i] = best - start;
@@ -270,8 +242,8 @@ __global__ void __launch_bounds__(1024) k_tlas_build(TlasBuildArgs a) {
                         const float4 cA0 = a.nodes[2 * aId], cB0 = a.nodes[2 * aId + 1], cA1 = a.nodes[2 * bId], cB1 = a.nodes[2 * bId + 1];
                         a.temp[2 * mergedHead] = cA0; a.temp[2 * mergedHead + 1] = cB0;
                         a.temp[2 * (mergedHead + 1)] = cA1; a.temp[2 * (mergedHead + 1) + 1] = cB1;
-                        a.temp[2 * unmergedHead] = make_float4(tlas_min(cA0.x, cA1.x), tlas_min(cA0.y, cA1.y), tlas_min(cA0.z, cA1.z), __uint_as_float((uint32_t)mergedHead));
-                        a.temp[2 * unmergedHead + 1] = make_float4(tlas_max(cB0.x, cB1.x), tlas_max(cB0.y, cB1.y), tlas_max(cB0.z, cB1.z), 0.0f);
+                        a.temp[2 * unmergedHead] = make_float4(minN(cA0.x, cA1.x), minN(cA0.y, cA1.y), minN(cA0.z, cA1.z), __uint_as_float((uint32_t)mergedHead));
+                        a.temp[2 * unmergedHead + 1] = make_float4(maxN(cB0.x, cB1.x), maxN(cB0.y, cB1.y), maxN(cB0.z, cB1.z), 0.0f);
                         unmergedHead++;
                         mergedHead += 2;
                     }

@@ -1955,9 +1955,9 @@ IDKPT_API int idkpt_blas_build(IdkPtCtx* ctx, const PackedVec3* positions, uint6
     if (kernelMs) *kernelMs = 0.0f;
     if (!positions || !triangles || !out) return fail(ctx, IDKPT_ERR_INVALID_ARGUMENT, "idkpt_blas_build: null argument");
     if (triangleCount == 0) return fail(ctx, IDKPT_ERR_INVALID_ARGUMENT, "idkpt_blas_build: no triangles");
-    IdkPtBlasBuildSettings s;
-    if (settings) s = *settings;
-    else s = {1, 2, 1.1f, 16, 0.0009745f, 0.3f, 1};
+    const idkbvh::Params d;
+    const IdkPtBlasBuildSettings s = settings ? *settings : IdkPtBlasBuildSettings{d.stopSplittingThreshold, d.maxLeafTriangleCount,
+        d.triangleCost, d.stackOptThreshold, d.stackOptSahIncreaseAcceptance, d.splitFactor, d.doPreSplit};
     if (!std::isfinite(s.TriangleCost) || !std::isfinite(s.StackOptSahIncreaseAcceptance) || !std::isfinite(s.SplitFactor))
         return fail(ctx, IDKPT_ERR_INVALID_ARGUMENT, "idkpt_blas_build: non-finite setting");
     if (s.StopSplittingThreshold < 1)   // a node of 0 fragments would read as an interior node (GpuBlasNode.TriCount == 0)
@@ -1971,8 +1971,8 @@ IDKPT_API int idkpt_blas_build(IdkPtCtx* ctx, const PackedVec3* positions, uint6
     }
     DRAIN_PENDING("idkpt_blas_build");
     CK(cudaSetDevice(ctx->device));
-    idkbb::Params p = {s.StopSplittingThreshold, s.MaxLeafTriangleCount, s.TriangleCost, s.StackOptThreshold,
-                       s.StackOptSahIncreaseAcceptance, s.SplitFactor, s.DoPreSplit ? 1 : 0};
+    const idkbvh::Params p = {s.StopSplittingThreshold, s.MaxLeafTriangleCount, s.TriangleCost, s.StackOptThreshold,
+                             s.StackOptSahIncreaseAcceptance, s.SplitFactor, s.DoPreSplit ? 1 : 0};
     IdkPtBlasBuild* b = new IdkPtBlasBuild();
     std::string err;
     float ms = 0.0f;

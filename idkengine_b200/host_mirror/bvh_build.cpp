@@ -12,11 +12,15 @@
 //   Bvh/BLAS.cs:441-466          GetUnindexedTriangles (refittable path)
 //   Bvh/PreSplitting.cs:169-273  GetUnindexedTriangles (dedup + straddling)
 //   Utils/Algorithms.cs:15-112,276-297  FloatToKey, RadixSort, StablePartition
-//   Shapes/Box.cs, Shapes/Triangle.cs:47-92, Utils/MyMath.cs:222-230
 //
-// Float semantics: C# does not contract a*b+c; only MyMath.HalfArea uses an
-// explicit fused multiply-add (float.MultiplyAddEstimate). Compile with
-// -ffp-contract=off; fmaf() is used where the reference fuses.
+// The scalar arithmetic (boxes, Triangle.Split, GetPriority, one pre-split step, the
+// serial TrySplit, the SAH and collapse terms, the TLAS keys, the settings' defaults)
+// lives in csrc/idk_bvh_math.h, which the device build (csrc/idk_blas_build.cuh)
+// compiles too. This file keeps what only the host does: the thread pool, the wide
+// split's six concurrent scans, the radix sort, processSubtree, the recursive
+// collapse, both unindexings and the serial PLOC of the TLAS.
+//
+// Float semantics: compile with -ffp-contract=off (see idk_bvh_math.h).
 
 #include <cstdint>
 #include <cstring>
@@ -32,111 +36,14 @@
 #include <condition_variable>
 #include <string>
 
-#include "../../include/idk_gpu_types.h"
+#include "idk_bvh_math.h"
 
 namespace {
 
-struct V3 {
-    float x, y, z;
-    float operator[](int i) const { return i == 0 ? x : (i == 1 ? y : z); }
-};
-static inline V3 operator-(V3 a, V3 b) { return {a.x - b.x, a.y - b.y, a.z - b.z}; }
-static inline V3 operator+(V3 a, V3 b) { return {a.x + b.x, a.y + b.y, a.z + b.z}; }
-static inline V3 operator*(float s, V3 a) { return {s * a.x, s * a.y, s * a.z}; }
-static inline V3 cross(V3 l, V3 r) {
-    // OpenTK Vector3.Cross
-    return {l.y * r.z - l.z * r.y, l.z * r.x - l.x * r.z, l.x * r.y - l.y * r.x};
-}
+using namespace idkbvh;
 
-// Vector128.MinNative/MaxNative on x86 = minps/maxps: (a < b) ? a : b.
-static inline float minN(float a, float b) { return a < b ? a : b; }
-static inline float maxN(float a, float b) { return a > b ? a : b; }
-
-struct Box {
-    float mn[3], mx[3];
-    static Box empty() { return {{FLT_MAX, FLT_MAX, FLT_MAX}, {-FLT_MAX, -FLT_MAX, -FLT_MAX}}; }
-    void grow(V3 p) {
-        mn[0] = minN(mn[0], p.x); mn[1] = minN(mn[1], p.y); mn[2] = minN(mn[2], p.z);
-        mx[0] = maxN(mx[0], p.x); mx[1] = maxN(mx[1], p.y); mx[2] = maxN(mx[2], p.z);
-    }
-    void grow(const Box& b) {
-        for (int i = 0; i < 3; i++) { mn[i] = minN(mn[i], b.mn[i]); mx[i] = maxN(mx[i], b.mx[i]); }
-    }
-    void clip(const Box& b) {
-        for (int i = 0; i < 3; i++) { mn[i] = maxN(mn[i], b.mn[i]); mx[i] = minN(mx[i], b.mx[i]); }
-    }
-    float size(int i) const { return mx[i] - mn[i]; }
-    int largestAxis() const {
-        int axis = 0;
-        if (size(0) < size(1)) axis = 1;
-        if (size(axis) < size(2)) axis = 2;
-        return axis;
-    }
-    float largestExtent() const { return maxN(size(0), maxN(size(1), size(2))); }
-    // MyMath.HalfArea: fma(x + y, z, x * y)
-    float halfArea() const {
-        float sx = size(0), sy = size(1), sz = size(2);
-        return fmaf(sx + sy, sz, sx * sy);
-    }
-    float area() const { return halfArea() * 2.0f; }
-};
-
-static inline float nodeHalfArea(const GpuBlasNode& n) {
-    float sx = n.Max[0] - n.Min[0], sy = n.Max[1] - n.Min[1], sz = n.Max[2] - n.Min[2];
-    return fmaf(sx + sy, sz, sx * sy);
-}
-
-struct Tri { V3 p0, p1, p2; };
-
-static Box boxFromTri(const Tri& t) {
-    Box b = {{t.p0.x, t.p0.y, t.p0.z}, {t.p0.x, t.p0.y, t.p0.z}};
-    b.grow(t.p1);
-    b.grow(t.p2);
-    return b;
-}
-
-// Triangle.Split, Shapes/Triangle.cs:47-92
-static void triSplit(const Tri& t, int axis, float position, Box& lBox, Box& rBox) {
-    lBox = Box::empty();
-    rBox = Box::empty();
-    bool q0 = t.p0[axis] <= position;
-    bool q1 = t.p1[axis] <= position;
-    bool q2 = t.p2[axis] <= position;
-    if (q0) lBox.grow(t.p0); else rBox.grow(t.p0);
-    if (q1) lBox.grow(t.p1); else rBox.grow(t.p1);
-    if (q2) lBox.grow(t.p2); else rBox.grow(t.p2);
-    auto splitEdge = [&](V3 a, V3 b) {
-        float tt = (position - a[axis]) / (b[axis] - a[axis]);
-        return a + tt * (b - a);
-    };
-    if (q0 ^ q1) { V3 m = splitEdge(t.p0, t.p1); lBox.grow(m); rBox.grow(m); }
-    if (q1 ^ q2) { V3 m = splitEdge(t.p1, t.p2); lBox.grow(m); rBox.grow(m); }
-    if (q2 ^ q0) { V3 m = splitEdge(t.p2, t.p0); lBox.grow(m); rBox.grow(m); }
-}
-
-static inline uint32_t floatToKey(float v) {
-    uint32_t f;
-    memcpy(&f, &v, 4);
-    uint32_t mask = (uint32_t)(((int32_t)f >> 31) | (1 << 31));
-    return f ^ mask;
-}
-
-// C# (int)float on x86-64 (cvttss2si): NaN / out of range -> INT_MIN.
-static inline int csFloatToInt(float f) {
-    if (!(f > -2147483904.0f && f < 2147483648.0f)) return INT_MIN;
-    return (int)f;
-}
-
-struct Settings {
-    int   stopSplittingThreshold = 1;
-    int   maxLeafTriangleCount = 2;
-    float triangleCost = 1.1f;
-    int   stackOptThreshold = 16;
-    float stackOptSahIncreaseAcceptance = 0.0009745f;
-    float stackOptMaxLeafTriangleCount = (float)INT_MAX;
-    float splitFactor = 0.3f;
-    int   doPreSplit = 1;
-    int   threads = 1;
+struct Settings : Params {
+    int threads = 1;
 };
 
 struct Geometry {
@@ -145,7 +52,7 @@ struct Geometry {
     int triCount;
     Tri tri(int i) const {
         const GpuBlasTriangle& t = tris[i];
-        return {{pos[t.X].x, pos[t.X].y, pos[t.X].z}, {pos[t.Y].x, pos[t.Y].y, pos[t.Y].z}, {pos[t.Z].x, pos[t.Z].y, pos[t.Z].z}};
+        return {{{{pos[t.X].x, pos[t.X].y, pos[t.X].z}}, {{pos[t.Y].x, pos[t.Y].y, pos[t.Y].z}}, {{pos[t.Z].x, pos[t.Z].y, pos[t.Z].z}}}};
     }
 };
 
@@ -155,33 +62,6 @@ struct Fragments {
 };
 
 // ---------------------------------------------------------------- PreSplitting.PreSplit
-static float priority(const Tri& t) {
-    Box b = boxFromTri(t);
-    float le = b.largestExtent();
-    float extentPrio = le * le;
-    V3 c = cross(t.p1 - t.p0, t.p2 - t.p0);
-    float triArea = sqrtf(c.x * c.x + c.y * c.y + c.z * c.z) * 0.5f;
-    float emptyAreaPrio = b.area() - triArea;
-    return cbrtf(extentPrio * emptyAreaPrio);
-}
-
-static int getSplitCount(float prio, float totalPrio, int triCount, float splitFactor) {
-    float shareOfTris = prio / totalPrio * (float)triCount;
-    int c = csFloatToInt(shareOfTris * splitFactor);
-    if (c == INT_MIN || c < 0) c = 0; // robustness guard (degenerate input); reference would overflow
-    return 1 + c;
-}
-
-static float getNodeSize(float extent, float globalSize) {
-    float alpha = extent / globalSize;
-    uint32_t bits;
-    memcpy(&bits, &alpha, 4);
-    bits &= (255u << 23);
-    float p2;
-    memcpy(&p2, &bits, 4);
-    return p2 * globalSize;
-}
-
 static void preSplit(const Geometry& g, const Settings& s, Fragments& out) {
     // Priorities once (the reference evaluates GetPriority three times per triangle); the total is summed in triangle order
     // on one thread, exactly as PreSplitting.cs:33-37 does, because float addition order matters.
@@ -200,16 +80,15 @@ static void preSplit(const Geometry& g, const Settings& s, Fragments& out) {
 
     // every triangle emits exactly its split count (left + right counts always add up), so the output offsets are a prefix sum
     std::vector<size_t> offset((size_t)g.triCount + 1, 0);
-    for (int i = 0; i < g.triCount; i++) offset[i + 1] = offset[i] + (size_t)getSplitCount(prio[i], totalPriority, g.triCount, s.splitFactor);
+    for (int i = 0; i < g.triCount; i++) offset[i + 1] = offset[i] + (size_t)splitCount(prio[i], totalPriority, g.triCount, s.splitFactor);
     out.bounds.resize(offset[g.triCount]);
     out.originalTriIds.resize(offset[g.triCount]);
 
-    Box globalBox = Box::empty();
+    Box globalBox = boxEmpty();
     for (int i = 0; i < g.triCount; i++) {
         Tri t = g.tri(i);
-        globalBox.grow(t.p0); globalBox.grow(t.p1); globalBox.grow(t.p2);
+        for (int k = 0; k < 3; k++) grow(globalBox, t.p[k]);
     }
-    float globalSize[3] = {globalBox.size(0), globalBox.size(1), globalBox.size(2)};
 
     struct Item { Box box; int splits; };
     chunked([&](int b0, int e0) {
@@ -217,9 +96,8 @@ static void preSplit(const Geometry& g, const Settings& s, Fragments& out) {
     for (int i = b0; i < e0; i++) {
         Tri tri = g.tri(i);
         size_t counter = offset[i];
-        int splitCount = (int)(offset[i + 1] - offset[i]);
         int sp = 0;
-        stack[sp++] = {boxFromTri(tri), splitCount};
+        stack[sp++] = {boxFromTri(tri), (int)(offset[i + 1] - offset[i])};
         while (sp > 0) {
             Item it = stack[--sp];
             if (it.splits == 1) {
@@ -228,28 +106,10 @@ static void preSplit(const Geometry& g, const Settings& s, Fragments& out) {
                 counter++;
                 continue;
             }
-            int axis = it.box.largestAxis();
-            float largestExtent = it.box.largestExtent();
-            float nodeSize = getNodeSize(largestExtent, globalSize[axis]);
-            if (nodeSize >= largestExtent - 0.0001f) nodeSize *= 0.5f;
-
-            float midPos = (it.box.mn[axis] + it.box.mx[axis]) * 0.5f;
-            float index = nearbyintf((midPos - globalBox.mn[axis]) / nodeSize); // MathF.Round: half to even
-            float splitPos = globalBox.mn[axis] + index * nodeSize;
-
             Box lBox, rBox;
-            triSplit(tri, axis, splitPos, lBox, rBox);
-            lBox.clip(it.box);
-            rBox.clip(it.box);
-
-            float leftExtent = lBox.largestExtent();
-            float rightExtent = rBox.largestExtent();
-            int leftCount = csFloatToInt((float)it.splits * (leftExtent / (leftExtent + rightExtent)));
-            leftCount = std::min(std::max(leftCount, 1), it.splits - 1);
-            int rightCount = it.splits - leftCount;
-
+            const int leftCount = presplitStep(tri, it.box, it.splits, globalBox, lBox, rBox);
             if (sp + 2 > (int)stack.size()) stack.resize(stack.size() * 2);
-            stack[sp++] = {rBox, rightCount};
+            stack[sp++] = {rBox, it.splits - leftCount};
             stack[sp++] = {lBox, leftCount};
         }
     }
@@ -298,100 +158,15 @@ static void radixSortFragments(const Fragments& f, int axis, std::vector<int>& o
 }
 
 static Box computeBoundingBox(int start, int count, const BuildData& bd, int axis) {
-    Box box = Box::empty();
-    const int* ids = bd.sorted[axis].data() + start;
-    for (int i = 0; i < count; i++) box.grow(bd.frags.bounds[ids[i]]);
-    return box;
+    return rangeBox(bd.frags.bounds.data(), bd.sorted[axis].data(), start, start + count);
 }
 
-// Algorithms.StablePartition(source, auxiliary, bitArray)
-static int stablePartition(int* source, int count, int* aux, const uint8_t* table) {
-    int l = 0, r = 0;
-    for (int i = 0; i < count; i++) {
-        int id = source[i];
-        if (table[id]) source[l++] = id; else aux[r++] = id;
-    }
-    memcpy(source + l, aux, sizeof(int) * (size_t)r);
-    return l;
-}
-
-struct ObjectSplit { int axis; int splitIndex; float newCost; bool valid; };
-
-// BLAS.TrySplit, Bvh/BLAS.cs:730-873
-static ObjectSplit trySplit(const GpuBlasNode& parent, BuildData& bd, const Settings& s) {
-    ObjectSplit none = {0, 0, 0.0f, false};
-    Box parentBox = {{parent.Min[0], parent.Min[1], parent.Min[2]}, {parent.Max[0], parent.Max[1], parent.Max[2]}};
-    if (parent.TriCount <= s.stopSplittingThreshold) return none;
-
-    const int start = parent.TriStartOrChild;
-    const int end = parent.TriStartOrChild + parent.TriCount;
-
-    ObjectSplit best = {0, 0, FLT_MAX, true};
-    float* rightCostsAccum = bd.rightCostsAccum.data();
-    const Box* fragBounds = bd.frags.bounds.data();
-
-    for (int axis = 0; axis < 3; axis++) {
-        const int* ids = bd.sorted[axis].data();
-        int firstRight = start + 1;
-
-        Box rightBoxAccum = Box::empty();
-        float rightCounter = 0.0f;
-        for (int i = end - 1; i >= firstRight; i--) {
-            rightCounter++;
-            rightBoxAccum.grow(fragBounds[ids[i]]);
-            float rightCost = rightBoxAccum.halfArea() * rightCounter;
-            rightCostsAccum[i] = rightCost;
-            if (rightCost >= best.newCost) { firstRight = i + 1; break; }
-        }
-
-        Box leftBoxAccum = Box::empty();
-        float leftCounter = (float)(firstRight - start) - 1.0f;
-        for (int i = start; i < firstRight - 1; i++) leftBoxAccum.grow(fragBounds[ids[i]]);
-        for (int i = firstRight - 1; i < end - 1; i++) {
-            int splitIndex = i + 1;
-            leftCounter++;
-            leftBoxAccum.grow(fragBounds[ids[i]]);
-            float leftCost = leftBoxAccum.halfArea() * leftCounter;
-            float rightCost = rightCostsAccum[splitIndex];
-            float cost = leftCost + rightCost;
-            if (cost < best.newCost) {
-                best.splitIndex = splitIndex;
-                best.axis = axis;
-                best.newCost = cost;
-            } else if (leftCost >= best.newCost) {
-                break;
-            }
-        }
-    }
-
-    if (best.newCost == FLT_MAX) {
-        // Degenerate input (non-finite costs): the reference would index out of range.
-        // Robustness guard: median split on axis 0.
-        best.axis = 0;
-        best.splitIndex = start + parent.TriCount / 2;
-    }
-
-    if (parent.TriCount <= s.maxLeafTriangleCount) {
-        float notSplitCost = s.triangleCost * (float)parent.TriCount;
-        best.newCost = 1.0f /*TRAVERSAL_COST*/ + (s.triangleCost * best.newCost / parentBox.halfArea());
-        if (best.newCost >= notSplitCost) return none;
-    }
-
-    Box leftBox = computeBoundingBox(start, best.splitIndex - start, bd, best.axis);
-    Box rightBox = computeBoundingBox(best.splitIndex, end - best.splitIndex, bd, best.axis);
-    bool leftSmaller = leftBox.halfArea() < rightBox.halfArea();
-    bool swapSides = leftSmaller; // larger child goes left
-
-    uint8_t* table = bd.fragLeftTable.data();
-    int* ids = bd.sorted[best.axis].data();
-    for (int i = start; i < best.splitIndex; i++) table[ids[i]] = !swapSides;
-    for (int i = best.splitIndex; i < end; i++) table[ids[i]] = swapSides;
-
-    int* aux = bd.partitionAux.data() + start;
-    if (swapSides) best.splitIndex = start + stablePartition(ids + start, parent.TriCount, aux, table);
-    stablePartition(bd.sorted[(best.axis + 1) % 3].data() + start, parent.TriCount, aux, table);
-    stablePartition(bd.sorted[(best.axis + 2) % 3].data() + start, parent.TriCount, aux, table);
-    return best;
+// BLAS.TrySplit, serial; returns the split index, or -1 for a leaf
+static int trySplit(const GpuBlasNode& parent, BuildData& bd, const Settings& s) {
+    const Box parentBox = {{parent.Min[0], parent.Min[1], parent.Min[2]}, {parent.Max[0], parent.Max[1], parent.Max[2]}};
+    int* const ids[3] = {bd.sorted[0].data(), bd.sorted[1].data(), bd.sorted[2].data()};
+    return trySplitSerial(bd.frags.bounds.data(), ids, bd.rightCostsAccum.data(), bd.fragLeftTable.data(), bd.partitionAux.data(),
+                          s, parentBox, parent.TriStartOrChild, parent.TriCount);
 }
 
 
@@ -416,10 +191,9 @@ static void runTasks(int taskCount, int threads, F&& f) {
     for (auto& th : pool) th.join();
 }
 
-static ObjectSplit trySplitWide(const GpuBlasNode& parent, BuildData& bd, const Settings& s, WideScratch& ws) {
-    ObjectSplit none = {0, 0, 0.0f, false};
-    Box parentBox = {{parent.Min[0], parent.Min[1], parent.Min[2]}, {parent.Max[0], parent.Max[1], parent.Max[2]}};
-    if (parent.TriCount <= s.stopSplittingThreshold) return none;
+static int trySplitWide(const GpuBlasNode& parent, BuildData& bd, const Settings& s, WideScratch& ws) {
+    const Box parentBox = {{parent.Min[0], parent.Min[1], parent.Min[2]}, {parent.Max[0], parent.Max[1], parent.Max[2]}};
+    if (parent.TriCount <= s.stopSplittingThreshold) return -1;
     const int start = parent.TriStartOrChild;
     const int end = parent.TriStartOrChild + parent.TriCount;
     const Box* fragBounds = bd.frags.bounds.data();
@@ -429,73 +203,58 @@ static ObjectSplit trySplitWide(const GpuBlasNode& parent, BuildData& bd, const 
         const int axis = task >> 1;
         const int* ids = bd.sorted[axis].data();
         if (task & 1) {           // suffix: R[i] = halfArea(box of [i, end)) * (end - i)
-            Box acc = Box::empty();
+            Box acc = boxEmpty();
             float counter = 0.0f;
             float* R = ws.R[axis].data();
-            for (int i = end - 1; i >= start + 1; i--) { counter++; acc.grow(fragBounds[ids[i]]); R[i] = acc.halfArea() * counter; }
+            for (int i = end - 1; i >= start + 1; i--) { counter++; acc = combine(acc, fragBounds[ids[i]]); R[i] = halfArea(acc) * counter; }
         } else {                  // prefix: L[i] = halfArea(box of [start, i]) * (i - start + 1)
-            Box acc = Box::empty();
+            Box acc = boxEmpty();
             float counter = 0.0f;
             float* L = ws.L[axis].data();
-            for (int i = start; i < end - 1; i++) { counter++; acc.grow(fragBounds[ids[i]]); L[i] = acc.halfArea() * counter; }
+            for (int i = start; i < end - 1; i++) { counter++; acc = combine(acc, fragBounds[ids[i]]); L[i] = halfArea(acc) * counter; }
         }
     });
 
-    ObjectSplit best = {0, 0, FLT_MAX, true};
+    float bestCost = FLT_MAX;
+    int bestAxis = 0, bestSplit = 0;
     for (int axis = 0; axis < 3; axis++) {   // BLAS.TrySplit's sweep, reading the precomputed costs
         const float* L = ws.L[axis].data();
         const float* R = ws.R[axis].data();
         int firstRight = start + 1;
         for (int i = end - 1; i >= firstRight; i--)
-            if (R[i] >= best.newCost) { firstRight = i + 1; break; }
+            if (R[i] >= bestCost) { firstRight = i + 1; break; }
         for (int i = firstRight - 1; i < end - 1; i++) {
-            const int splitIndex = i + 1;
             const float leftCost = L[i];
-            const float cost = leftCost + R[splitIndex];
-            if (cost < best.newCost) {
-                best.splitIndex = splitIndex;
-                best.axis = axis;
-                best.newCost = cost;
-            } else if (leftCost >= best.newCost) {
-                break;
-            }
+            const float cost = leftCost + R[i + 1];
+            if (cost < bestCost) { bestSplit = i + 1; bestAxis = axis; bestCost = cost; }
+            else if (leftCost >= bestCost) break;
         }
     }
-    if (best.newCost == FLT_MAX) {
-        best.axis = 0;
-        best.splitIndex = start + parent.TriCount / 2;
-    }
-    if (parent.TriCount <= s.maxLeafTriangleCount) {
-        float notSplitCost = s.triangleCost * (float)parent.TriCount;
-        best.newCost = 1.0f + (s.triangleCost * best.newCost / parentBox.halfArea());
-        if (best.newCost >= notSplitCost) return none;
-    }
+    if (!keepSplit(s, parentBox, start, parent.TriCount, bestCost, bestAxis, bestSplit)) return -1;
 
     Box childBox[2];
     runTasks(2, s.threads, [&](int t) {
-        childBox[t] = t == 0 ? computeBoundingBox(start, best.splitIndex - start, bd, best.axis)
-                             : computeBoundingBox(best.splitIndex, end - best.splitIndex, bd, best.axis);
+        childBox[t] = t == 0 ? computeBoundingBox(start, bestSplit - start, bd, bestAxis)
+                             : computeBoundingBox(bestSplit, end - bestSplit, bd, bestAxis);
     });
-    const bool swapSides = childBox[0].halfArea() < childBox[1].halfArea();   // larger child goes left
+    const bool swap = swapSides(childBox[0], childBox[1]);
 
     uint8_t* table = bd.fragLeftTable.data();
-    int* ids = bd.sorted[best.axis].data();
-    const int split0 = best.splitIndex;
+    int* ids = bd.sorted[bestAxis].data();
     runTasks(2, s.threads, [&](int t) {
-        if (t == 0) for (int i = start; i < split0; i++) table[ids[i]] = !swapSides;
-        else for (int i = split0; i < end; i++) table[ids[i]] = swapSides;
+        if (t == 0) for (int i = start; i < bestSplit; i++) table[ids[i]] = !swap;
+        else for (int i = bestSplit; i < end; i++) table[ids[i]] = swap;
     });
 
     // three independent id arrays: each needs its own auxiliary range
     std::vector<int> auxB(parent.TriCount), auxC(parent.TriCount);
-    int newSplit = best.splitIndex;
+    int newSplit = bestSplit;
     runTasks(3, s.threads, [&](int t) {
-        if (t == 0) { if (swapSides) newSplit = start + stablePartition(ids + start, parent.TriCount, bd.partitionAux.data() + start, table); }
-        else if (t == 1) stablePartition(bd.sorted[(best.axis + 1) % 3].data() + start, parent.TriCount, auxB.data(), table);
-        else stablePartition(bd.sorted[(best.axis + 2) % 3].data() + start, parent.TriCount, auxC.data(), table);
+        if (t == 0) { if (swap) newSplit = start + stablePartition(ids + start, parent.TriCount, bd.partitionAux.data() + start, table); }
+        else if (t == 1) stablePartition(bd.sorted[(bestAxis + 1) % 3].data() + start, parent.TriCount, auxB.data(), table);
+        else stablePartition(bd.sorted[(bestAxis + 2) % 3].data() + start, parent.TriCount, auxC.data(), table);
     });
-    best.splitIndex = newSplit;
-    return best;
+    return newSplit;
 }
 
 // ---------------------------------------------------------------- BLAS.Build
@@ -503,10 +262,6 @@ struct BuildResult {
     std::vector<GpuBlasNode> nodes;
     int requiredStackSize = 0;
 };
-
-static void setBounds(GpuBlasNode& n, const Box& b) {
-    for (int i = 0; i < 3; i++) { n.Min[i] = b.mn[i]; n.Max[i] = b.mx[i]; }
-}
 
 struct BuildTask { int parentNodeId; int newNodesId; };
 
@@ -519,14 +274,14 @@ static void processSubtree(BuildResult& blas, BuildData& bd, const Settings& s, 
         stack.pop_back();
         GpuBlasNode& parent = blas.nodes[t.parentNodeId];
         setBounds(parent, computeBoundingBox(parent.TriStartOrChild, parent.TriCount, bd, 0));
-        ObjectSplit split = trySplit(parent, bd, s);
-        if (!split.valid) continue;
+        const int split = trySplit(parent, bd, s);
+        if (split < 0) continue;
 
         GpuBlasNode left = {};
         left.TriStartOrChild = parent.TriStartOrChild;
-        left.TriCount = split.splitIndex - left.TriStartOrChild;
+        left.TriCount = split - left.TriStartOrChild;
         GpuBlasNode right = {};
-        right.TriStartOrChild = split.splitIndex;
+        right.TriStartOrChild = split;
         right.TriCount = parent.TriCount - left.TriCount;
 
         int leftId = t.newNodesId, rightId = leftId + 1;
@@ -572,11 +327,8 @@ static double computeGlobalSAH(const BuildResult& blas, const Settings& s) {
     while (!stack.empty()) {
         const GpuBlasNode& n = blas.nodes[stack.back()];
         stack.pop_back();
-        double prob = (double)nodeHalfArea(n) * rootArea;
-        if (n.TriCount > 0) {
-            cost += (double)(s.triangleCost * (float)n.TriCount) * prob; // float*int in C# = float, then * double
-        } else {
-            cost += 1.0 * prob;
+        cost += sahTerm(n, rootArea, s.triangleCost);
+        if (!(n.TriCount > 0)) {
             stack.push_back(n.TriStartOrChild + 1);
             stack.push_back(n.TriStartOrChild);
         }
@@ -600,13 +352,11 @@ static void collapseDeepestLevel(BuildResult& blas, const Settings& s, int newSt
             parent.TriCount = l.TriCount + r.TriCount;
         }
         if ((stackSize == newStackSize && !firstPass) || (stackSize > newStackSize && firstPass)) {
-            if ((float)(l.TriCount + r.TriCount) > s.stackOptMaxLeafTriangleCount) {
+            if ((float)(l.TriCount + r.TriCount) > STACK_OPT_MAX_LEAF_TRIANGLE_COUNT) {
                 nextCollapseCost = (double)FLT_MAX;
                 return;
             }
-            double leavesCost = (double)s.triangleCost * ((double)l.TriCount * (double)nodeHalfArea(l) + (double)r.TriCount * (double)nodeHalfArea(r));
-            double newParentLeafCost = (double)s.triangleCost * (double)(l.TriCount + r.TriCount);
-            nextCollapseCost += ((double)nodeHalfArea(parent) * (newParentLeafCost - 1.0) - leavesCost) / (double)nodeHalfArea(blas.nodes[1]);
+            nextCollapseCost += collapseTerm(parent, l, r, l.TriCount, r.TriCount, blas.nodes[1], s.triangleCost);
         }
     }
 }
@@ -671,10 +421,10 @@ static int buildBlas(BuildResult& blas, BuildData& bd, const Settings& s) {
         auto splitOnce = [&](BuildTask t, WideScratch* wide) {
             GpuBlasNode& parent = blas.nodes[t.parentNodeId];
             setBounds(parent, computeBoundingBox(parent.TriStartOrChild, parent.TriCount, bd, 0));
-            ObjectSplit split = wide ? trySplitWide(parent, bd, s, *wide) : trySplit(parent, bd, s);
-            if (!split.valid) return;
-            GpuBlasNode left = {}; left.TriStartOrChild = parent.TriStartOrChild; left.TriCount = split.splitIndex - left.TriStartOrChild;
-            GpuBlasNode right = {}; right.TriStartOrChild = split.splitIndex; right.TriCount = parent.TriCount - left.TriCount;
+            const int split = wide ? trySplitWide(parent, bd, s, *wide) : trySplit(parent, bd, s);
+            if (split < 0) return;
+            GpuBlasNode left = {}; left.TriStartOrChild = parent.TriStartOrChild; left.TriCount = split - left.TriStartOrChild;
+            GpuBlasNode right = {}; right.TriStartOrChild = split; right.TriCount = parent.TriCount - left.TriCount;
             int leftId = t.newNodesId, rightId = leftId + 1;
             blas.nodes[leftId] = left; blas.nodes[rightId] = right;
             parent.TriStartOrChild = leftId; parent.TriCount = 0;
@@ -789,16 +539,19 @@ static void unindexPreSplit(BuildResult& blas, const BuildData& bd, const Geomet
     tris.resize(counter);
 }
 
-// BLAS.GetUnindexedTriangles, Bvh/BLAS.cs:441-466
+// BLAS.GetUnindexedTriangles, Bvh/BLAS.cs:441-466. The array holds n triangles; when the root stays a leaf, its two copies
+// list all n each, and the reference writes the second copy's past the end of its array. Those writes are dropped: the
+// result is the first copy's n triangles and the offset n for the second copy.
 static void unindexPlain(BuildResult& blas, const BuildData& bd, const Geometry& g, std::vector<GpuBlasTriangle>& tris) {
-    tris.assign(bd.n(), GpuBlasTriangle{});
+    const int n = bd.n();
+    tris.assign(n, GpuBlasTriangle{});
     int counter = 0;
     for (size_t i = 2; i < blas.nodes.size(); i++) {
-        GpuBlasNode& n = blas.nodes[i];
-        if (n.TriCount > 0) {
-            for (int j = 0; j < n.TriCount; j++) tris[counter + j] = g.tris[bd.sorted[0][n.TriStartOrChild + j]];
-            n.TriStartOrChild = counter;
-            counter += n.TriCount;
+        GpuBlasNode& node = blas.nodes[i];
+        if (node.TriCount > 0) {
+            for (int j = 0; j < node.TriCount && counter + j < n; j++) tris[counter + j] = g.tris[bd.sorted[0][node.TriStartOrChild + j]];
+            node.TriStartOrChild = counter;
+            counter += node.TriCount;
         }
     }
 }
@@ -829,14 +582,9 @@ struct IdkBlasBuildSettings {
 
 __attribute__((visibility("default")))
 void idkhost_default_build_settings(IdkBlasBuildSettings* s) {
-    s->StopSplittingThreshold = 1;
-    s->MaxLeafTriangleCount = 2;
-    s->TriangleCost = 1.1f;
-    s->StackOptThreshold = 16;
-    s->StackOptSahIncreaseAcceptance = 0.0009745f;
-    s->SplitFactor = 0.3f;
-    s->DoPreSplit = 1;
-    s->Threads = 1;
+    const Settings d;
+    *s = {d.stopSplittingThreshold, d.maxLeafTriangleCount, d.triangleCost, d.stackOptThreshold,
+          d.stackOptSahIncreaseAcceptance, d.splitFactor, d.doPreSplit, d.threads};
 }
 
 // One BLAS: BVH.BlasesBuild loop body, Bvh/BVH.cs:315-377.
@@ -917,17 +665,6 @@ __attribute__((visibility("default"))) void idkhost_blas_free(IdkBlasBuild* b) {
 // ---------------------------------------------------------------- TLAS (Bvh/TLAS.cs:28-141, serial PLOC)
 namespace {
 
-static inline uint32_t insertTwoZeros(uint32_t v) {   // MyMath.InsertTwoZerosAfterEachBit
-    v = (v * 0x00010001u) & 0xFF0000FFu;
-    v = (v * 0x00000101u) & 0x0F00F00Fu;
-    v = (v * 0x00000011u) & 0xC30C30C3u;
-    v = (v * 0x00000005u) & 0x49249249u;
-    return v;
-}
-static inline uint32_t morton30(float x, float y, float z) {   // MyMath.GetMortonCode30
-    auto q = [](float f) { float s = f * 1024.0f; uint32_t u = s <= 0.0f ? 0u : (s >= 4294967040.0f ? 0xFFFFFFFFu : (uint32_t)s); return std::min(u, 1023u); };
-    return (insertTwoZeros(q(x)) << 2) | (insertTwoZeros(q(y)) << 1) | insertTwoZeros(q(z));
-}
 static inline Box tlasBox(const GpuTlasNode& n) { return {{n.Min[0], n.Min[1], n.Min[2]}, {n.Max[0], n.Max[1], n.Max[2]}}; }
 static inline void tlasSetBounds(GpuTlasNode& n, const Box& b) { for (int i = 0; i < 3; i++) { n.Min[i] = b.mn[i]; n.Max[i] = b.mx[i]; } }
 
@@ -937,9 +674,7 @@ static int findBestMatch(const GpuTlasNode* nodes, int start, int end, int nodeI
     Box nodeBox = tlasBox(nodes[nodeIndex]);
     for (int i = start; i < end; i++) {
         if (i == nodeIndex) continue;
-        Box merged = nodeBox;
-        merged.grow(tlasBox(nodes[i]));
-        float area = merged.halfArea();
+        float area = halfArea(combine(nodeBox, tlasBox(nodes[i])));
         if (area < smallestArea) { smallestArea = area; best = i; }
     }
     return best;
@@ -952,16 +687,7 @@ extern "C" {
 // Box.Transformed(localBounds, modelMatrix) (Shapes/Box.cs:166-175): 8 corners through the (column-vector) 3x4 model matrix.
 __attribute__((visibility("default")))
 void idkhost_transform_box(const float mn[3], const float mx[3], const float model3x4[12], float outMin[3], float outMax[3]) {
-    Box b = Box::empty();
-    for (int i = 0; i < 8; i++) {
-        float x = (i & 1) ? mx[0] : mn[0], y = (i & 2) ? mx[1] : mn[1], z = (i & 4) ? mx[2] : mn[2];
-        // OpenTK Vector4 * Matrix4 (row vector): x*Row0 + y*Row1 + z*Row2 + w*Row3; Row_k.c = model3x4[c][k]
-        V3 p;
-        p.x = x * model3x4[0] + y * model3x4[1] + z * model3x4[2] + 1.0f * model3x4[3];
-        p.y = x * model3x4[4] + y * model3x4[5] + z * model3x4[6] + 1.0f * model3x4[7];
-        p.z = x * model3x4[8] + y * model3x4[9] + z * model3x4[10] + 1.0f * model3x4[11];
-        b.grow(p);
-    }
+    const Box b = transformedBox({{mn[0], mn[1], mn[2]}, {mx[0], mx[1], mx[2]}}, model3x4);
     for (int i = 0; i < 3; i++) { outMin[i] = b.mn[i]; outMax[i] = b.mx[i]; }
 }
 
@@ -974,27 +700,17 @@ void idkhost_tlas_build(const float* boxes, int32_t primitiveCount, GpuTlasNode*
     memset(nodes, 0, sizeof(GpuTlasNode) * (size_t)nodeCount);
     {
         GpuTlasNode* leaves = temp.data() + (nodeCount - primitiveCount);
-        Box global = Box::empty();
+        Box global = boxEmpty();
         for (int i = 0; i < primitiveCount; i++) {
             Box b = {{boxes[6 * i], boxes[6 * i + 1], boxes[6 * i + 2]}, {boxes[6 * i + 3], boxes[6 * i + 4], boxes[6 * i + 5]}};
-            global.grow(b);
+            global = combine(global, b);
             GpuTlasNode n = {};
             tlasSetBounds(n, b);
             n.IsLeafAndChildOrInstanceId = (1u << 31) | (uint32_t)i;
             leaves[i] = n;
         }
         std::vector<std::pair<uint32_t, int>> keyed(primitiveCount);
-        for (int i = 0; i < primitiveCount; i++) {
-            const GpuTlasNode& n = leaves[i];
-            float c[3], m[3];
-            for (int a = 0; a < 3; a++) {
-                c[a] = (n.Max[a] + n.Min[a]) * 0.5f;
-                float t = global.mx[a] - global.mn[a];
-                m[a] = (c[a] - global.mn[a]) / t * (1.0f - 0.0f) + 0.0f;   // MyMath.MapToZeroOne / Remap
-                if (t == 0.0f) m[a] = 0.0f;
-            }
-            keyed[i] = {morton30(m[0], m[1], m[2]), i};
-        }
+        for (int i = 0; i < primitiveCount; i++) keyed[i] = {centreKey(tlasBox(leaves[i]), global), i};
         std::stable_sort(keyed.begin(), keyed.end(), [](const std::pair<uint32_t, int>& a, const std::pair<uint32_t, int>& b) { return a.first < b.first; });
         for (int i = 0; i < primitiveCount; i++) nodes[nodeCount - primitiveCount + i] = leaves[keyed[i].second];
     }
@@ -1021,10 +737,8 @@ void idkhost_tlas_build(const float* boxes, int32_t primitiveCount, GpuTlasNode*
                     int bId = b + activeRangeStart;
                     temp[mergedHead] = nodes[aId];
                     temp[mergedHead + 1] = nodes[bId];
-                    Box mb = tlasBox(temp[mergedHead]);
-                    mb.grow(tlasBox(temp[mergedHead + 1]));
                     GpuTlasNode nn = {};
-                    tlasSetBounds(nn, mb);
+                    tlasSetBounds(nn, combine(tlasBox(temp[mergedHead]), tlasBox(temp[mergedHead + 1])));
                     nn.IsLeafAndChildOrInstanceId = (uint32_t)mergedHead;
                     temp[unmergedHead++] = nn;
                     mergedHead += 2;
