@@ -48,7 +48,7 @@ struct BloomDownArgs {
     PostImage src;
     uint2* dst;
     int dw, dh;
-    int prefilter;          // Lod == 0
+    int prefilter;          // the shader's Lod uniform is 0: down levels 0 and 1
     float maxColor, threshold;
 };
 

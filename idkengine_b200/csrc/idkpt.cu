@@ -1712,11 +1712,13 @@ IDKPT_API int idkpt_post_process(IdkPtCtx* ctx, const IdkPtPostSettings* s, IdkP
             if (ce != cudaSuccess) return fail(ctx, IDKPT_ERR_OUT_OF_MEMORY, "idkpt_post_process: bloom allocation failed");
             uint2* down = (uint2*)ctx->bloomDown.p;
             uint2* up = (uint2*)ctx->bloomUp.p;
+            // Bloom.cs:62-93. The shader prefilters when its Lod uniform is 0, and Lod is 0 for the dispatch that writes level 0
+            // and again for the one that writes level 1 (that one uploads currentWriteLod - 1): both levels are prefiltered.
             for (int l = 0; l < levels; l++) {
                 BloomDownArgs a;
                 a.src = l == 0 ? PostImage{src, nullptr, w, h} : PostImage{nullptr, down + off[l - 1], lw[l - 1], lh[l - 1]};
                 a.dst = down + off[l]; a.dw = lw[l]; a.dh = lh[l];
-                a.prefilter = l == 0; a.maxColor = s->BloomMaxColor; a.threshold = s->BloomThreshold;
+                a.prefilter = l <= 1; a.maxColor = s->BloomMaxColor; a.threshold = s->BloomThreshold;
                 k_bloom_down<<<grid(a.dw, a.dh), blk, 0, ctx->stream>>>(a);
             }
             for (int l = levels - 2; l >= 0; l--) {

@@ -39,15 +39,17 @@ def test_gpu_reproduces_golden(name):
         assert st.NodePairFetches == exp["node_pair_fetches"] and st.TriangleTests == exp["triangle_tests"]
 
 
+# next_rows_golden.json pins the present chain ("ldr", "ldr_mean") with Prefilter on bloom down levels 0 and 1, the two
+# dispatches of Bloom.cs that upload Lod 0.
 NEXT = json.load(open(os.path.join(HERE, "golden", "next_rows_golden.json")))
 
 
-def test_oracle_reproduces_next_rows_golden():
+def test_oracle_reproduces_next_rows_golden_two_prefiltered_bloom_levels():
     assert mg.next_rows_expect() == NEXT
 
 
 @pytest.mark.gpu
-def test_gpu_reproduces_next_rows_golden():
+def test_gpu_reproduces_next_rows_golden_two_prefiltered_bloom_levels():
     from idkengine_b200 import capi
     from idkengine_b200.pathtracer import PathTracer
     x = mg.next_rows_inputs()

@@ -3,6 +3,7 @@ import numpy as np
 import pytest
 
 import oracle_lib as ol
+import post_ref64
 from idkengine_b200 import capi, scenes
 
 
@@ -35,14 +36,18 @@ def test_oracle_tonemap_properties():
     assert vals.min() >= 125 and vals.max() <= 130 and len(vals) >= 3      # 0.5 * 255 = 127.5 +- Bayer dither of +-2 LSB
 
 
-def test_oracle_bloom_properties():
+def test_oracle_bloom_properties_two_prefiltered_levels():
+    """No bloom below the threshold; around a hot spot, bloom that falls off and peaks where the float64 chain of
+    tests/post_ref64.py peaks (0.147 here: Prefilter runs on down levels 0 and 1, as the engine's Lod-0 dispatches do)."""
     st = capi.default_post_settings()
     img = np.full((96, 128, 4), 0.3, np.float32)
     _, bloom = ol.post_process(img, st, want_bloom=True)
     assert bloom.shape == (48, 64, 3) and np.abs(bloom).max() == 0.0            # nothing above the threshold: no bloom
     img[40:44, 60:64, :3] = 50.0
     out, bloom = ol.post_process(img, st, want_bloom=True)
-    assert bloom.max() > 0.5 and bloom[22, 31].sum() > bloom[2, 2].sum()         # energy around the hot spot, falling off
+    peak = post_ref64.bloom64(img, st.BloomThreshold, st.BloomMaxColor, st.BloomMinusLods)[1][0].max()
+    assert 0.1 < peak < 0.2 and abs(bloom.max() - peak) <= 2.0 ** -10 * peak
+    assert bloom[22, 31].sum() > bloom[2, 2].sum()                                # energy around the hot spot, falling off
     st.IsBloom = 0
     plain = ol.post_process(img, st)
     assert (out.astype(int) >= plain.astype(int) - 1).all() and (out.astype(int) > plain.astype(int) + 3).any()
