@@ -103,6 +103,7 @@ EXPORTS = [
     "idkpt_gather_export", "idkpt_gather_import", "idkpt_gather_connect", "idkpt_gather_device_ptr",
     "idkpt_result_device_ptr", "idkpt_tile_rows",
     "idkpt_read_wavefront_rays", "idkpt_trace_rays", "idkpt_trace_rays_any", "idkpt_shadows_ray_traced",
+    "idkpt_shadows_ray_traced_gbuffer", "idkpt_shadows_device_ptr", "idkpt_volumetric_lighting_gbuffer",
     "idkpt_set_skinning_data", "idkpt_skin_vertices", "idkpt_blas_refit", "idkpt_read_range", "idkpt_post_process", "idkpt_ldr_device_ptr", "idkpt_abi_version",
     "idkpt_denoise", "idkpt_denoise_device_ptrs", "idkpt_denoise_import_output", "idkpt_tlas_build",
     "idkpt_set_point_shadows", "idkpt_render_point_shadows", "idkpt_read_point_shadow", "idkpt_point_shadow_device_ptr",
@@ -400,6 +401,10 @@ def load(path=None):
     L.idkpt_trace_rays_any.argtypes = [c_vp, c_vp, c_u64, c_i32, c_vp, P(c_f)]
     L.idkpt_shadows_ray_traced.restype = c_i32
     L.idkpt_shadows_ray_traced.argtypes = [c_vp, c_vp, c_vp, c_vp, c_i32, c_i32, c_i32, c_i32, c_u32, c_vp, c_vp, P(c_f)]
+    L.idkpt_shadows_ray_traced_gbuffer.restype = c_i32
+    L.idkpt_shadows_ray_traced_gbuffer.argtypes = [c_vp, c_vp, P(IdkPtGBuffer), c_i32, c_i32, c_u32, c_vp, c_i32, c_vp, P(c_f)]
+    L.idkpt_shadows_device_ptr.restype = c_i32
+    L.idkpt_shadows_device_ptr.argtypes = [c_vp, c_i32, P(c_vp), P(c_u64)]
     L.idkpt_set_skinning_data.restype = c_i32
     L.idkpt_set_skinning_data.argtypes = [c_vp, c_vp, c_u64]
     L.idkpt_skin_vertices.restype = c_i32
@@ -444,6 +449,8 @@ def load(path=None):
     L.idkpt_point_shadow_device_ptr.argtypes = [c_vp, c_i32, P(c_vp), P(c_u64)]
     L.idkpt_volumetric_lighting.restype = c_i32
     L.idkpt_volumetric_lighting.argtypes = [c_vp, c_vp, P(IdkPtVolumetricSettings), c_vp, c_i32, c_i32, c_i32, c_i32, c_vp, c_vp, P(c_f)]
+    L.idkpt_volumetric_lighting_gbuffer.restype = c_i32
+    L.idkpt_volumetric_lighting_gbuffer.argtypes = [c_vp, c_vp, P(IdkPtVolumetricSettings), P(IdkPtGBuffer), c_i32, c_i32, c_vp, c_vp, P(c_f)]
     L.idkpt_volumetric_device_ptr.restype = c_i32
     L.idkpt_volumetric_device_ptr.argtypes = [c_vp, P(c_vp), P(c_u64)]
     L.idkpt_ssao.restype = c_i32

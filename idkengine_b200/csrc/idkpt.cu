@@ -85,6 +85,9 @@ struct RasterState {
     RasterImage gb;                // the six planar fp32 attachments in one allocation (gbuffer_planes)
     RasterImage taa;               // the two rgba16f presentation-size history images (TAAResolve's ping-pong); w x h: their size
     int taaFrame = 0;              // TAAResolve.frame: Result = taa.buf[taaFrame % 2], PrevResult the other one
+    // the ray-traced visibility (r32f) of each idkpt_shadows_ray_traced_gbuffer slot; the extra last one is the image the
+    // host-array idkpt_shadows_ray_traced seeds with the caller's array
+    RasterImage rtShadow[IDKPT_MAX_POINT_SHADOWS + 1];
 };
 
 #define IDK_MAX_LANES 16
@@ -244,6 +247,7 @@ static void release_raster(RasterState& r) {
     for (DevBuf* b : {&r.stage, &r.rtPtrs, &r.volMarch, &r.volDepth, &r.vrsOffsets, &r.gbPrev}) release(*b);
     for (RasterImage* img : {&r.vol, &r.ssao, &r.deferred, &r.ssr, &r.vrs, &r.gb, &r.taa})
         for (DevBuf& b : img->buf) release(b);
+    for (RasterImage& img : r.rtShadow) release(img.buf[0]);
     r = RasterState{};
 }
 
@@ -2162,7 +2166,7 @@ IDKPT_API int idkpt_read_point_shadow(IdkPtCtx* ctx, int32_t index, uint16_t* ds
 // Their messages read "<entry point>: <what>" (fail(ctx, who, ...)); a null context goes through the template fail, so that
 // idkpt_last_error(NULL) reports it.
 
-static int size_check(IdkPtCtx* ctx, const char* who, int w, int h) {
+static int size_check(IdkCtxBase* ctx, const char* who, int w, int h) {
     if (w < 1 || h < 1 || w > 16384 || h > 16384) return fail(ctx, who, IDKPT_ERR_INVALID_ARGUMENT, "size outside 1..16384");
     return IDKPT_OK;
 }
@@ -2207,9 +2211,10 @@ static StageInput attachment(const float* src, size_t floats) {
 static StageInput velocity_input(const float* src) { return {src, 2, 8, "OnDevice VelocityRG pointer not 8-byte aligned"}; }
 
 // The input stage of a raster call over w x h pixels. Checks every OnDevice array first, so that a rejected pointer is never
-// read and nothing has been allocated or invalidated; then uploads the host arrays into the stage, each at a 256-byte aligned
+// read and nothing has been allocated or invalidated; then uploads the host arrays into `stage`, each at a 256-byte aligned
 // offset. Writes the device pointer of every input to dev[], in order (null for a null src: an input the call does not use).
-static int stage_inputs(IdkPtCtx* ctx, const char* who, int w, int h, int onDevice, const std::vector<StageInput>& in, const float** dev) {
+static int stage_inputs_into(IdkCtxBase* ctx, DevBuf& stageBuf, const char* who, int w, int h, int onDevice, const std::vector<StageInput>& in,
+                             const float** dev) {
     const size_t pixels = (size_t)w * h;
     size_t bytes = 0;
     for (const StageInput& i : in) {
@@ -2225,8 +2230,8 @@ static int stage_inputs(IdkPtCtx* ctx, const char* who, int w, int h, int onDevi
             return fail(ctx, who, IDKPT_ERR_INVALID_ARGUMENT, "OnDevice = 1 with a pointer that is not device memory on the context's device");
         if ((uintptr_t)i.src % i.align != 0) return fail(ctx, who, IDKPT_ERR_INVALID_ARGUMENT, i.misaligned);
     }
-    if (bytes && ensure(ctx->raster.stage, bytes) != cudaSuccess) return fail(ctx, who, IDKPT_ERR_OUT_OF_MEMORY, "device allocation failed");
-    char* stage = (char*)ctx->raster.stage.p;
+    if (bytes && ensure(stageBuf, bytes) != cudaSuccess) return fail(ctx, who, IDKPT_ERR_OUT_OF_MEMORY, "device allocation failed");
+    char* stage = (char*)stageBuf.p;
     for (const StageInput& i : in) {
         *dev = i.src;
         if (i.src && i.floats && !onDevice) {
@@ -2239,12 +2244,22 @@ static int stage_inputs(IdkPtCtx* ctx, const char* who, int w, int h, int onDevi
     return IDKPT_OK;
 }
 
-static int gbuffer_check(IdkPtCtx* ctx, const char* who, const IdkPtGBuffer* g, bool all) {
-    if (!g->Depth || !g->NormalRG || (all && (!g->AlbedoRGB || !g->MetallicRoughness || !g->EmissiveRGB)))
-        return fail(ctx, who, IDKPT_ERR_INVALID_ARGUMENT, "null argument");
+// The raster passes of the path-tracer context stage into its raster stage.
+static int stage_inputs(IdkPtCtx* ctx, const char* who, int w, int h, int onDevice, const std::vector<StageInput>& in, const float** dev) {
+    return stage_inputs_into(ctx, ctx->raster.stage, who, w, h, onDevice, in, dev);
+}
+
+// A G-buffer's size and OnDevice; the callers check the attachments they read.
+static int gbuffer_shape_check(IdkCtxBase* ctx, const char* who, const IdkPtGBuffer* g) {
     if (int rc = size_check(ctx, who, g->Width, g->Height)) return rc;
     if (g->OnDevice != 0 && g->OnDevice != 1) return fail(ctx, who, IDKPT_ERR_INVALID_ARGUMENT, "OnDevice is neither 0 nor 1");
     return IDKPT_OK;
+}
+
+static int gbuffer_check(IdkCtxBase* ctx, const char* who, const IdkPtGBuffer* g, bool all) {
+    if (!g->Depth || !g->NormalRG || (all && (!g->AlbedoRGB || !g->MetallicRoughness || !g->EmissiveRGB)))
+        return fail(ctx, who, IDKPT_ERR_INVALID_ARGUMENT, "null argument");
+    return gbuffer_shape_check(ctx, who, g);
 }
 
 // The lit-image selector (IdkPtLitSource), checked before anything is allocated: a caller array, or a context image of w x h.
@@ -2293,13 +2308,13 @@ static int image_device_ptr(IdkPtCtx* ctx, const char* who, RasterImage RasterSt
 }
 
 // ---- volumetric lighting (VolumetricLighting.Compute: march + depth-aware upscale) ---------------------------------------------
-IDKPT_API int idkpt_volumetric_lighting(IdkPtCtx* ctx, const GpuPerFrameData* frame, const IdkPtVolumetricSettings* s, const float* depth,
-                                        int32_t depthWidth, int32_t depthHeight, int32_t width, int32_t height, const float* taaJitter,
-                                        uint16_t* outRgba16f, float* kernelMs) {
-    static const char* who = "idkpt_volumetric_lighting";
-    if (!ctx || !frame || !s || !depth) return fail(ctx, IDKPT_ERR_INVALID_ARGUMENT, "idkpt_volumetric_lighting: null argument");
+// Both entry points: g's Depth (g->Width x g->Height, the other attachments unused), read in place when g->OnDevice is 1.
+static int volumetric_lighting(IdkPtCtx* ctx, const char* who, const GpuPerFrameData* frame, const IdkPtVolumetricSettings* s,
+                               const IdkPtGBuffer* g, int32_t width, int32_t height, const float* taaJitter, uint16_t* outRgba16f,
+                               float* kernelMs) {
+    const int depthWidth = g->Width, depthHeight = g->Height;
     if (!ctx->haveScene) return fail(ctx, who, IDKPT_ERR_NO_SCENE, "no scene");
-    if (int rc = size_check(ctx, who, depthWidth, depthHeight)) return rc;
+    if (int rc = gbuffer_shape_check(ctx, who, g)) return rc;
     if (int rc = size_check(ctx, who, width, height)) return rc;
     if (s->SampleCount < 1 || s->SampleCount > 1024) return fail(ctx, who, IDKPT_ERR_INVALID_ARGUMENT, "SampleCount outside 1..1024");
     if (!(s->ResolutionScale > 0.0f && s->ResolutionScale <= 1.0f)) return fail(ctx, who, IDKPT_ERR_INVALID_ARGUMENT, "ResolutionScale not in (0, 1]");
@@ -2311,7 +2326,7 @@ IDKPT_API int idkpt_volumetric_lighting(IdkPtCtx* ctx, const GpuPerFrameData* fr
             return fail(ctx, who, IDKPT_ERR_INVALID_ARGUMENT, "a shadow's LightIndex is not below the scene's light count");
     CK(cudaSetDevice(ctx->device));
     const float* gdepth;
-    if (int rc = stage_inputs(ctx, who, depthWidth, depthHeight, 0, {attachment(depth, 1)}, &gdepth)) return rc;
+    if (int rc = stage_inputs(ctx, who, depthWidth, depthHeight, g->OnDevice, {attachment(g->Depth, 1)}, &gdepth)) return rc;
     if (kernelMs) *kernelMs = 0.0f;
     RasterState& r = ctx->raster;
     const size_t nRender = (size_t)w * h, nOut = (size_t)width * height;
@@ -2340,6 +2355,20 @@ IDKPT_API int idkpt_volumetric_lighting(IdkPtCtx* ctx, const GpuPerFrameData* fr
     }, outRgba16f, r.vol.buf[0].p, outRgba16f ? nOut * 8 : 0);
     if (rc == IDKPT_OK) r.vol.publish(width, height);
     return rc;
+}
+
+IDKPT_API int idkpt_volumetric_lighting(IdkPtCtx* ctx, const GpuPerFrameData* frame, const IdkPtVolumetricSettings* s, const float* depth,
+                                        int32_t depthWidth, int32_t depthHeight, int32_t width, int32_t height, const float* taaJitter,
+                                        uint16_t* outRgba16f, float* kernelMs) {
+    if (!ctx || !frame || !s || !depth) return fail(ctx, IDKPT_ERR_INVALID_ARGUMENT, "idkpt_volumetric_lighting: null argument");
+    const IdkPtGBuffer g{depthWidth, depthHeight, 0, depth, nullptr, nullptr, nullptr, nullptr};
+    return volumetric_lighting(ctx, "idkpt_volumetric_lighting", frame, s, &g, width, height, taaJitter, outRgba16f, kernelMs);
+}
+
+IDKPT_API int idkpt_volumetric_lighting_gbuffer(IdkPtCtx* ctx, const GpuPerFrameData* frame, const IdkPtVolumetricSettings* s, const IdkPtGBuffer* g,
+                                                int32_t width, int32_t height, const float* taaJitter, uint16_t* outRgba16f, float* kernelMs) {
+    if (!ctx || !frame || !s || !g || !g->Depth) return fail(ctx, IDKPT_ERR_INVALID_ARGUMENT, "idkpt_volumetric_lighting_gbuffer: null argument");
+    return volumetric_lighting(ctx, "idkpt_volumetric_lighting_gbuffer", frame, s, g, width, height, taaJitter, outRgba16f, kernelMs);
 }
 
 IDKPT_API int idkpt_volumetric_device_ptr(IdkPtCtx* ctx, void** devPtr, uint64_t* bytes) {
@@ -2379,7 +2408,43 @@ IDKPT_API int idkpt_ssao_device_ptr(IdkPtCtx* ctx, void** devPtr, uint64_t* byte
     return image_device_ptr(ctx, "idkpt_ssao_device_ptr", &RasterState::ssao, "idkpt_ssao", 1, 1, devPtr, bytes);
 }
 
-// The RayTraced mode's visibility images (PointShadowManager.ComputeRayTracedShadowMaps for one light), from host arrays.
+// The RayTraced mode's visibility images (PointShadowManager.ComputeRayTracedShadowMaps for one light) into the image of `slot`
+// (ctx->raster.rtShadow). Pixels with depth == 1 keep what the image held, as the shader returns early there: the caller's
+// array with `seed` (uploaded first), else the last successful call's values when the image has the G-buffer's size, else 0.
+// The deferred pass never reads those pixels (DeferredLighting/fragment.glsl returns early on them too).
+static int shadows_ray_traced(IdkPtCtx* ctx, const char* who, const GpuPerFrameData* frame, const IdkPtGBuffer* g, int32_t lightIndex,
+                              int32_t samples, uint32_t noiseIndex, const float* taaJitter, int slot, const float* seed,
+                              float* visibilityOut, float* kernelMs) {
+    if (!ctx->haveScene) return fail(ctx, who, IDKPT_ERR_NO_SCENE, "no scene");
+    if (int rc = gbuffer_check(ctx, who, g, false)) return rc;
+    if (samples < 1 || samples > 1024) return fail(ctx, who, IDKPT_ERR_INVALID_ARGUMENT, "samples outside 1..1024");
+    if (lightIndex < 0 || (uint64_t)lightIndex >= ctx->counts.LightCount) return fail(ctx, who, IDKPT_ERR_INVALID_ARGUMENT, "light index out of range");
+    CK(cudaSetDevice(ctx->device));
+    const float* in[2];
+    if (int rc = stage_inputs(ctx, who, g->Width, g->Height, g->OnDevice, {attachment(g->Depth, 1), attachment(g->NormalRG, 2)}, in)) return rc;
+    if (kernelMs) *kernelMs = 0.0f;
+    RasterImage& out = ctx->raster.rtShadow[slot];
+    const size_t bytes = (size_t)g->Width * g->Height * 4;
+    const bool keep = out.valid_at(g->Width, g->Height);
+    out.invalidate();              // the image may be reallocated and is overwritten: valid again only when the call succeeds
+    if (ensure(out.buf[0], bytes) != cudaSuccess) return fail(ctx, who, IDKPT_ERR_OUT_OF_MEMORY, "device allocation failed");
+    if (seed) CK(cudaMemcpyAsync(out.buf[0].p, seed, bytes, cudaMemcpyHostToDevice, ctx->stream));
+    else if (!keep) CK(cudaMemsetAsync(out.buf[0].p, 0, bytes, ctx->stream));
+    ShadowArgs a;
+    a.sc = ctx->sc;
+    memcpy(a.invProjView, frame->InvProjView, sizeof(a.invProjView));
+    read_jitter(taaJitter, a.jitter);
+    a.depth = in[0]; a.normalRG = (const float2*)in[1]; a.visibility = (float*)out.buf[0].p;
+    a.width = g->Width; a.height = g->Height; a.lightIndex = lightIndex; a.samples = samples; a.noiseIndex = noiseIndex;
+    const int rc = run_timed(ctx, who, kernelMs, [&]() -> int {
+        k_shadows_ray_traced<<<ctx->traceRaysBlocks, IDK_BLOCK, ctx->stackBytes, ctx->stream>>>(a);
+        return IDKPT_OK;
+    }, visibilityOut, out.buf[0].p, visibilityOut ? bytes : 0);
+    if (rc == IDKPT_OK) out.publish(g->Width, g->Height);
+    return rc;
+}
+
+// From host arrays: visibility_out is read-modify-write, through the context's own image (the slot after the last public one).
 IDKPT_API int idkpt_shadows_ray_traced(IdkPtCtx* ctx, const GpuPerFrameData* frame, const float* depth, const float* normalRG, int32_t width,
                                        int32_t height, int32_t lightIndex, int32_t samples, uint32_t noiseIndex, const float* taaJitter,
                                        float* visibilityOut, float* kernelMs) {
@@ -2387,21 +2452,29 @@ IDKPT_API int idkpt_shadows_ray_traced(IdkPtCtx* ctx, const GpuPerFrameData* fra
     if (!ctx || !frame || !depth || !normalRG || !visibilityOut) return fail(ctx, IDKPT_ERR_INVALID_ARGUMENT, "idkpt_shadows_ray_traced: null argument");
     if (!ctx->haveScene) return fail(ctx, who, IDKPT_ERR_NO_SCENE, "no scene");
     if (width < 1 || height < 1 || width > 16384 || height > 16384 || samples < 1 || samples > 1024) return fail(ctx, who, IDKPT_ERR_INVALID_ARGUMENT, "invalid size / sample count");
-    if (lightIndex < 0 || (uint64_t)lightIndex >= ctx->counts.LightCount) return fail(ctx, who, IDKPT_ERR_INVALID_ARGUMENT, "light index out of range");
-    CK(cudaSetDevice(ctx->device));
-    if (kernelMs) *kernelMs = 0.0f;
-    const float* in[3];            // depth, normal and the visibility: pixels with depth == 1 keep the caller's value
-    if (int rc = stage_inputs(ctx, who, width, height, 0, {attachment(depth, 1), attachment(normalRG, 2), attachment(visibilityOut, 1)}, in)) return rc;
-    ShadowArgs a;
-    a.sc = ctx->sc;
-    memcpy(a.invProjView, frame->InvProjView, sizeof(a.invProjView));
-    read_jitter(taaJitter, a.jitter);
-    a.depth = in[0]; a.normalRG = (const float2*)in[1]; a.visibility = (float*)in[2];
-    a.width = width; a.height = height; a.lightIndex = lightIndex; a.samples = samples; a.noiseIndex = noiseIndex;
-    return run_timed(ctx, who, kernelMs, [&]() -> int {
-        k_shadows_ray_traced<<<ctx->traceRaysBlocks, IDK_BLOCK, ctx->stackBytes, ctx->stream>>>(a);
-        return IDKPT_OK;
-    }, visibilityOut, in[2], (size_t)width * height * 4);
+    const IdkPtGBuffer g{width, height, 0, depth, normalRG, nullptr, nullptr, nullptr};
+    return shadows_ray_traced(ctx, who, frame, &g, lightIndex, samples, noiseIndex, taaJitter, IDKPT_MAX_POINT_SHADOWS, visibilityOut,
+                              visibilityOut, kernelMs);
+}
+
+IDKPT_API int idkpt_shadows_ray_traced_gbuffer(IdkPtCtx* ctx, const GpuPerFrameData* frame, const IdkPtGBuffer* g, int32_t lightIndex,
+                                               int32_t samples, uint32_t noiseIndex, const float* taaJitter, int32_t slot, float* visibilityOut,
+                                               float* kernelMs) {
+    static const char* who = "idkpt_shadows_ray_traced_gbuffer";
+    if (!ctx || !frame || !g) return fail(ctx, IDKPT_ERR_INVALID_ARGUMENT, "idkpt_shadows_ray_traced_gbuffer: null argument");
+    if (slot < 0 || slot >= IDKPT_MAX_POINT_SHADOWS) return fail(ctx, who, IDKPT_ERR_INVALID_ARGUMENT, "slot outside 0..IDKPT_MAX_POINT_SHADOWS - 1");
+    return shadows_ray_traced(ctx, who, frame, g, lightIndex, samples, noiseIndex, taaJitter, slot, nullptr, visibilityOut, kernelMs);
+}
+
+IDKPT_API int idkpt_shadows_device_ptr(IdkPtCtx* ctx, int32_t slot, void** devPtr, uint64_t* bytes) {
+    static const char* who = "idkpt_shadows_device_ptr";
+    if (!ctx || !devPtr) return fail(ctx, IDKPT_ERR_INVALID_ARGUMENT, "idkpt_shadows_device_ptr: null argument");
+    if (slot < 0 || slot >= IDKPT_MAX_POINT_SHADOWS) return fail(ctx, who, IDKPT_ERR_INVALID_ARGUMENT, "slot outside 0..IDKPT_MAX_POINT_SHADOWS - 1");
+    const RasterImage& r = ctx->raster.rtShadow[slot];
+    if (!r.valid()) return fail(ctx, who, IDKPT_ERR_INVALID_ARGUMENT, "call idkpt_shadows_ray_traced_gbuffer for the slot first");
+    *devPtr = r.buf[0].p;
+    if (bytes) *bytes = (uint64_t)r.w * r.h * 4;
+    return IDKPT_OK;
 }
 
 IDKPT_API int idkpt_deferred_lighting(IdkPtCtx* ctx, const GpuPerFrameData* frame, const IdkPtDeferredSettings* s, const IdkPtGBuffer* g,

@@ -21,7 +21,8 @@ struct IdkVxCtx : IdkCtxBase {
     TextureTable tex;
     DevBuf queue, queueCount, counters;
     size_t queueCapacity = 0;
-    DevBuf scratch[4];                    // idkvx_cone_trace_rows: device copies of the G-buffer rows and of the output, kept between calls
+    DevBuf stage;                         // the cone trace's host G-buffer arrays (stage_inputs_into), kept between calls
+    RasterImage cone;                     // the rgba32f image of the last successful cone trace (width x rows traced)
     bool slabMode = false;                // idkvx_set_slab: voxelise one z-slab, no mip chain (the host all-gathers the slabs first)
     IdkPtCtx* shadowTracer = nullptr;     // idkvx_set_shadow_tracer: visibility of point-shadowed lights by shadow rays through this scene
     IdkPtCtx* shadowMaps = nullptr;       // idkvx_set_shadow_maps: visibility by the PCF lookup into this context's point-shadow cube maps
@@ -116,7 +117,7 @@ IDKPT_API void idkvx_destroy(IdkVxCtx* ctx) {
     if (ctx->stream) cudaStreamSynchronize(ctx->stream);
     DevBuf* all[] = {&ctx->gridMem, &ctx->positions, &ctx->vertices, &ctx->tris, &ctx->descs, &ctx->instances, &ctx->xforms, &ctx->meshes,
                      &ctx->materials, &ctx->lights, &ctx->tex.pixels, &ctx->tex.recs, &ctx->tex.srgbLut, &ctx->queue, &ctx->queueCount,
-                     &ctx->counters, &ctx->scratch[0], &ctx->scratch[1], &ctx->scratch[2], &ctx->scratch[3], &ctx->debugImage, &ctx->debugMask};
+                     &ctx->counters, &ctx->stage, &ctx->cone.buf[0], &ctx->debugImage, &ctx->debugMask};
     for (DevBuf* b : all) release(*b);
     destroy_stream(ctx);
     delete ctx;
@@ -317,29 +318,20 @@ IDKPT_API int idkvx_read_level(IdkVxCtx* ctx, int32_t level, void* dst, uint64_t
     return IDKPT_OK;
 }
 
-IDKPT_API int idkvx_cone_trace(IdkVxCtx* ctx, const GpuPerFrameData* frame, const IdkVxConeSettings* st, const float* depth,
-                               const float* normalRG, const float* metallicRoughness, int32_t width, int32_t height,
-                               const float skyColor[3], float* out, IdkVxStats* stats) {
-    return idkvx_cone_trace_rows(ctx, frame, st, depth, normalRG, metallicRoughness, width, height, 0, height, skyColor, out, stats);
-}
-
-// Screen-tiled cone tracing (multi-GPU: the grid is replicated, every rank traces its rows): the arrays hold `height` rows starting
-// at row `rowFirst` of a G-buffer that is `fullHeight` rows tall; pixel coordinates (noise, NDC) are those of the full image.
-IDKPT_API int idkvx_cone_trace_rows(IdkVxCtx* ctx, const GpuPerFrameData* frame, const IdkVxConeSettings* st, const float* depth,
-                                    const float* normalRG, const float* metallicRoughness, int32_t width, int32_t fullHeight,
-                                    int32_t rowFirst, int32_t height, const float skyColor[3], float* out, IdkVxStats* stats) {
-    if (!ctx || !frame || !st || !depth || !normalRG || !metallicRoughness || !skyColor || !out) return fail(ctx, IDKPT_ERR_INVALID_ARGUMENT, "idkvx_cone_trace: null argument");
-    if (width < 1 || height < 1 || width > 16384 || fullHeight > 16384 || rowFirst < 0 || rowFirst + height > fullHeight) return fail(ctx, IDKPT_ERR_INVALID_ARGUMENT, "idkvx_cone_trace: invalid image size / row range");
-    if (st->MaxSamples < 1 || st->MaxSamples > 64) return fail(ctx, IDKPT_ERR_INVALID_ARGUMENT, "idkvx_cone_trace: MaxSamples out of range");
+// ConeTracer.Compute for every entry point, into ctx->cone: g (Depth, NormalRG and MetallicRoughness, read in place when
+// g->OnDevice is 1; its arguments checked by the caller) holds g->Height rows starting at row `rowFirst` of a G-buffer that is
+// `fullHeight` rows tall; pixel coordinates (noise, NDC) are those of the full image. out (may be null) gets a copy.
+static int cone_trace(IdkVxCtx* ctx, const char* who, const GpuPerFrameData* frame, const IdkVxConeSettings* st, const IdkPtGBuffer* g,
+                      int32_t fullHeight, int32_t rowFirst, const float skyColor[3], float* out, IdkVxStats* stats) {
+    const int width = g->Width, height = g->Height;
     CK(cudaSetDevice(ctx->device));
+    const float* in[3];
+    if (int rc = stage_inputs_into(ctx, ctx->stage, who, width, height, g->OnDevice,
+                              {attachment(g->Depth, 1), attachment(g->NormalRG, 2), attachment(g->MetallicRoughness, 2)}, in)) return rc;
     if (stats) memset(stats, 0, sizeof(*stats));
     const size_t n = (size_t)width * height;
-    DevBuf &dDepth = ctx->scratch[0], &dN = ctx->scratch[1], &dMR = ctx->scratch[2], &dOut = ctx->scratch[3];
-    if (ensure(dDepth, n * 4) != cudaSuccess || ensure(dN, n * 8) != cudaSuccess || ensure(dMR, n * 8) != cudaSuccess || ensure(dOut, n * 16) != cudaSuccess)
-        return fail(ctx, IDKPT_ERR_OUT_OF_MEMORY, "idkvx_cone_trace: device allocation failed");
-    CK(cudaMemcpyAsync(dDepth.p, depth, n * 4, cudaMemcpyHostToDevice, ctx->stream));
-    CK(cudaMemcpyAsync(dN.p, normalRG, n * 8, cudaMemcpyHostToDevice, ctx->stream));
-    CK(cudaMemcpyAsync(dMR.p, metallicRoughness, n * 8, cudaMemcpyHostToDevice, ctx->stream));
+    ctx->cone.invalidate();        // the image may be reallocated and is overwritten: valid again only when the call succeeds
+    if (ensure(ctx->cone.buf[0], n * 16) != cudaSuccess) return fail(ctx, who, IDKPT_ERR_OUT_OF_MEMORY, "device allocation failed");
     CK(cudaMemsetAsync(ctx->counters.p, 0, 16, ctx->stream));
     VxConeArgs a;
     a.g = ctx->grid;
@@ -348,19 +340,55 @@ IDKPT_API int idkvx_cone_trace_rows(IdkVxCtx* ctx, const GpuPerFrameData* frame,
     a.maxSamples = st->MaxSamples; a.stepMultiplier = st->StepMultiplier; a.giBoost = st->GIBoost; a.giSkyBoxBoost = st->GISkyBoxBoost;
     a.normalRayOffset = st->NormalRayOffset; a.noiseIndex = st->NoiseIndex;
     for (int i = 0; i < 3; i++) a.sky[i] = skyColor[i];
-    a.depth = (const float*)dDepth.p; a.normalRG = (const float2*)dN.p; a.metalRough = (const float2*)dMR.p; a.out = (float4*)dOut.p;
+    a.depth = in[0]; a.normalRG = (const float2*)in[1]; a.metalRough = (const float2*)in[2]; a.out = (float4*)ctx->cone.buf[0].p;
     a.width = width; a.height = height; a.fullHeight = fullHeight; a.rowFirst = rowFirst; a.steps = (unsigned long long*)ctx->counters.p;
-    const int rc = run_timed(ctx, "idkvx_cone_trace", stats ? &stats->ConeTraceMs : nullptr, [&]() -> int {
+    const int rc = run_timed(ctx, who, stats ? &stats->ConeTraceMs : nullptr, [&]() -> int {
         k_vx_cone_trace<<<dim3((width + 7) / 8, (height + 7) / 8), dim3(8, 8), 0, ctx->stream>>>(a);
         return IDKPT_OK;
-    }, out, dOut.p, n * 16);
+    }, out, ctx->cone.buf[0].p, out ? n * 16 : 0);
     if (rc) return rc;
+    ctx->cone.publish(width, height);
     if (stats) {
         unsigned long long s = 0;
         CK(cudaMemcpy(&s, ctx->counters.p, 8, cudaMemcpyDeviceToHost));
         stats->ConeSteps = s;
         stats->KernelLaunches = 1;
     }
+    return IDKPT_OK;
+}
+
+IDKPT_API int idkvx_cone_trace(IdkVxCtx* ctx, const GpuPerFrameData* frame, const IdkVxConeSettings* st, const float* depth,
+                               const float* normalRG, const float* metallicRoughness, int32_t width, int32_t height,
+                               const float skyColor[3], float* out, IdkVxStats* stats) {
+    return idkvx_cone_trace_rows(ctx, frame, st, depth, normalRG, metallicRoughness, width, height, 0, height, skyColor, out, stats);
+}
+
+// Screen-tiled cone tracing (multi-GPU: the grid is replicated, every rank traces its rows) from host arrays of `height` rows.
+IDKPT_API int idkvx_cone_trace_rows(IdkVxCtx* ctx, const GpuPerFrameData* frame, const IdkVxConeSettings* st, const float* depth,
+                                    const float* normalRG, const float* metallicRoughness, int32_t width, int32_t fullHeight,
+                                    int32_t rowFirst, int32_t height, const float skyColor[3], float* out, IdkVxStats* stats) {
+    if (!ctx || !frame || !st || !depth || !normalRG || !metallicRoughness || !skyColor || !out) return fail(ctx, IDKPT_ERR_INVALID_ARGUMENT, "idkvx_cone_trace: null argument");
+    if (width < 1 || height < 1 || width > 16384 || fullHeight > 16384 || rowFirst < 0 || rowFirst + height > fullHeight) return fail(ctx, IDKPT_ERR_INVALID_ARGUMENT, "idkvx_cone_trace: invalid image size / row range");
+    if (st->MaxSamples < 1 || st->MaxSamples > 64) return fail(ctx, IDKPT_ERR_INVALID_ARGUMENT, "idkvx_cone_trace: MaxSamples out of range");
+    const IdkPtGBuffer g{width, height, 0, depth, normalRG, nullptr, metallicRoughness, nullptr};
+    return cone_trace(ctx, "idkvx_cone_trace", frame, st, &g, fullHeight, rowFirst, skyColor, out, stats);
+}
+
+IDKPT_API int idkvx_cone_trace_gbuffer(IdkVxCtx* ctx, const GpuPerFrameData* frame, const IdkVxConeSettings* st, const IdkPtGBuffer* g,
+                                       const float skyColor[3], float* out, IdkVxStats* stats) {
+    static const char* who = "idkvx_cone_trace_gbuffer";
+    if (!ctx || !frame || !st || !g || !skyColor) return fail(ctx, IDKPT_ERR_INVALID_ARGUMENT, "idkvx_cone_trace_gbuffer: null argument");
+    if (!g->Depth || !g->NormalRG || !g->MetallicRoughness) return fail(ctx, who, IDKPT_ERR_INVALID_ARGUMENT, "null argument");
+    if (int rc = gbuffer_shape_check(ctx, who, g)) return rc;
+    if (st->MaxSamples < 1 || st->MaxSamples > 64) return fail(ctx, who, IDKPT_ERR_INVALID_ARGUMENT, "MaxSamples outside 1..64");
+    return cone_trace(ctx, who, frame, st, g, g->Height, 0, skyColor, out, stats);
+}
+
+IDKPT_API int idkvx_cone_trace_device_ptr(IdkVxCtx* ctx, void** devPtr, uint64_t* bytes) {
+    if (!ctx || !devPtr) return fail(ctx, IDKPT_ERR_INVALID_ARGUMENT, "idkvx_cone_trace_device_ptr: null argument");
+    if (!ctx->cone.valid()) return fail(ctx, "idkvx_cone_trace_device_ptr", IDKPT_ERR_INVALID_ARGUMENT, "call idkvx_cone_trace_gbuffer first");
+    *devPtr = ctx->cone.buf[0].p;
+    if (bytes) *bytes = (uint64_t)ctx->cone.w * ctx->cone.h * 16;
     return IDKPT_OK;
 }
 

@@ -430,6 +430,53 @@ class PathTracer:
         """(device pointer, bytes) of the last VolumetricLighting image (rgba16f)."""
         return self._device_ptr("idkpt_volumetric_device_ptr")
 
+    # ---- the ray-traced shadows and the volumetric light on a G-buffer (host or device)
+    @classmethod
+    def gbuffer_arg(cls, gbuffer):
+        """A G-buffer argument: a capi.IdkPtGBuffer as it is, or GBufferDevicePtrs()'s (IdkPtGBuffer, velocity) pair, or the
+        arrays (depth, normal_rg, albedo, metallic_roughness, emissive; trailing ones may be left out, None for one the call
+        does not read) marshalled like the raster calls' arrays. Returns (IdkPtGBuffer, the arrays to keep alive)."""
+        if isinstance(gbuffer, capi.IdkPtGBuffer):
+            return gbuffer, None
+        if isinstance(gbuffer, (tuple, list)) and gbuffer and isinstance(gbuffer[0], capi.IdkPtGBuffer):
+            return gbuffer[0], None
+        arrays = list(gbuffer) + [None] * (5 - len(gbuffer))
+        g, _, keep = cls._gbuffer(arrays, [1, 2, 3, 2, 3])
+        return g, keep
+
+    def ShadowsRayTracedGBuffer(self, frame, gbuffer, light_index, slot, samples=1, noise_index=0, jitter=None, download=True):
+        """ShadowsRayTraced on a G-buffer (gbuffer_arg: Depth and NormalRG are read) into the context's visibility image of
+        `slot` (0 .. capi.IDKPT_MAX_POINT_SHADOWS - 1), which DeferredLighting takes as rt_visibility through ShadowsDevicePtr.
+        Pixels with depth 1 keep the slot image's values (0 in a new image). Returns float32 [H, W], or None with
+        download=False. Kernel ms in last_shadows_ms."""
+        g, keep = self.gbuffer_arg(gbuffer)
+        frame = np.ascontiguousarray(frame)
+        out = np.zeros((g.Height, g.Width), np.float32) if download else None
+        ms = ctypes.c_float()
+        self._check(self._lib.idkpt_shadows_ray_traced_gbuffer(self._ctx, frame.ctypes.data, ctypes.byref(g), light_index, samples, noise_index,
+                                                               self._jitter(jitter), slot, out.ctypes.data if download else None,
+                                                               ctypes.byref(ms)), "idkpt_shadows_ray_traced_gbuffer")
+        self.last_shadows_ms = ms.value
+        return out
+
+    def ShadowsDevicePtr(self, slot):
+        """(device pointer, bytes) of the last ShadowsRayTracedGBuffer image of `slot` (float32 [H, W])."""
+        return self._device_ptr("idkpt_shadows_device_ptr", slot)
+
+    def VolumetricLightingGBuffer(self, frame, gbuffer, width, height, settings=None, jitter=None, download=True):
+        """VolumetricLighting with the depth of a G-buffer (gbuffer_arg: only Depth is read, at the G-buffer's size). Returns
+        float16 [height, width, 4], or None with download=False (VolumetricDevicePtr). Kernel ms in last_volumetric_ms."""
+        st = settings if settings is not None else capi.default_volumetric_settings()
+        g, keep = self.gbuffer_arg(gbuffer)
+        frame = np.ascontiguousarray(frame)
+        out = np.zeros((height, width, 4), np.float16) if download else None
+        ms = ctypes.c_float()
+        self._check(self._lib.idkpt_volumetric_lighting_gbuffer(self._ctx, frame.ctypes.data, ctypes.byref(st), ctypes.byref(g), width, height,
+                                                                self._jitter(jitter), out.ctypes.data if download else None,
+                                                                ctypes.byref(ms)), "idkpt_volumetric_lighting_gbuffer")
+        self.last_volumetric_ms = ms.value
+        return out
+
     # ---- the raster passes' marshalling
     @staticmethod
     def _gbuffer(arrays, channels):

@@ -27,7 +27,8 @@ class IdkVxStats(ctypes.Structure):
 VX_EXPORTS = ["idkvx_create", "idkvx_destroy", "idkvx_last_error", "idkvx_set_scene", "idkvx_set_grid", "idkvx_level_count",
               "idkvx_voxelize", "idkvx_read_level", "idkvx_cone_trace", "idkvx_set_shadow_tracer",
               "idkvx_set_shadow_maps", "idkvx_set_slab", "idkvx_level_device_ptr", "idkvx_mipmap", "idkvx_cone_trace_rows",
-              "idkvx_set_conservative_rasterization", "idkvx_debug_render", "idkvx_debug_device_ptr"]
+              "idkvx_set_conservative_rasterization", "idkvx_debug_render", "idkvx_debug_device_ptr",
+              "idkvx_cone_trace_gbuffer", "idkvx_cone_trace_device_ptr"]
 
 DEFAULT_GRID_MIN = (-28.0, -3.0, -17.0)   # RasterPipeline.cs:213
 DEFAULT_GRID_MAX = (28.0, 20.0, 17.0)
@@ -88,6 +89,10 @@ def _declare(L):
     L.idkvx_read_level.argtypes = [c_vp, c_i32, c_vp, c_u64]
     L.idkvx_cone_trace.restype = c_i32
     L.idkvx_cone_trace.argtypes = [c_vp, c_vp, P(IdkVxConeSettings), c_vp, c_vp, c_vp, c_i32, c_i32, P(c_f * 3), c_vp, P(IdkVxStats)]
+    L.idkvx_cone_trace_gbuffer.restype = c_i32
+    L.idkvx_cone_trace_gbuffer.argtypes = [c_vp, c_vp, P(IdkVxConeSettings), P(capi.IdkPtGBuffer), P(c_f * 3), c_vp, P(IdkVxStats)]
+    L.idkvx_cone_trace_device_ptr.restype = c_i32
+    L.idkvx_cone_trace_device_ptr.argtypes = [c_vp, P(c_vp), P(c_u64)]
     L.idkvx_debug_render.restype = c_i32
     L.idkvx_debug_render.argtypes = [c_vp, c_vp, c_vp, c_f, c_f, c_i32, c_i32, c_vp, P(IdkVxStats)]
     L.idkvx_debug_device_ptr.restype = c_i32
@@ -232,6 +237,28 @@ class Voxelizer:
         self._check(self._lib.idkvx_cone_trace(self._ctx, frame.ctypes.data, ctypes.byref(settings), depth.ctypes.data, nrg.ctypes.data,
                                                mr.ctypes.data, w, h, ctypes.byref(skyc), out.ctypes.data, ctypes.byref(st)), "idkvx_cone_trace")
         return out, st
+
+    def ConeTraceGBuffer(self, frame, gbuffer, settings=None, sky=(0.6, 0.7, 0.9), download=True):
+        """ConeTracer.Compute(voxels) on a G-buffer: a capi.IdkPtGBuffer (e.g. PathTracer.GBufferDevicePtrs()'s, read in place)
+        or arrays as PathTracer.gbuffer_arg takes them; Depth, NormalRG and MetallicRoughness are read. Returns (float32
+        [H, W, 4] or None with download=False, when the image stays on the device: ConeTraceDevicePtr, stats)."""
+        from .pathtracer import PathTracer
+        g, keep = PathTracer.gbuffer_arg(gbuffer)
+        settings = settings or default_cone_settings()
+        out = np.zeros((g.Height, g.Width, 4), np.float32) if download else None
+        st = IdkVxStats()
+        skyc = (c_f * 3)(*sky)
+        frame = np.ascontiguousarray(frame)
+        assert frame.dtype == gt.GpuPerFrameData
+        self._check(self._lib.idkvx_cone_trace_gbuffer(self._ctx, frame.ctypes.data, ctypes.byref(settings), ctypes.byref(g), ctypes.byref(skyc),
+                                                       out.ctypes.data if download else None, ctypes.byref(st)), "idkvx_cone_trace_gbuffer")
+        return out, st
+
+    def ConeTraceDevicePtr(self):
+        """(device pointer, bytes) of the last cone trace's rgba32f image: DeferredLighting's indirect light on the device."""
+        p, n = c_vp(), c_u64()
+        self._check(self._lib.idkvx_cone_trace_device_ptr(self._ctx, ctypes.byref(p), ctypes.byref(n)), "idkvx_cone_trace_device_ptr")
+        return p.value, n.value
 
 
 def camera_rays(frame, width, height):

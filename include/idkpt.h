@@ -306,7 +306,8 @@ IDKPT_API int idkpt_trace_rays_any(IdkPtCtx* ctx, const IdkPtRay* rays, uint64_t
 /* Ray-traced point-light shadows: ShadowsRayTraced/compute.glsl for one light (PointShadowManager.ComputeRayTracedShadowMaps,
  * Source/Render/PointShadowManager.cs:53-75). Host arrays: depth [w*h], octahedral normal rg [w*h*2]; visibility_out [w*h] is
  * read-modify-write (pixels with depth == 1 are left untouched, as the shader returns early). noise_index = the
- * (Frame % SampleCount) * samples term (0 without TAA); taa_jitter may be NULL. */
+ * (Frame % SampleCount) * samples term (0 without TAA); taa_jitter may be NULL. idkpt_shadows_ray_traced_gbuffer (below, with
+ * the G-buffer passes) runs the same pass on an IdkPtGBuffer into a context image. */
 IDKPT_API int idkpt_shadows_ray_traced(IdkPtCtx* ctx, const GpuPerFrameData* frame, const float* depth, const float* normalRG,
                                        int32_t width, int32_t height, int32_t light_index, int32_t samples, uint32_t noise_index,
                                        const float* taa_jitter, float* visibility_out, float* kernel_ms);
@@ -336,7 +337,8 @@ IDKPT_API int idkpt_point_shadow_device_ptr(IdkPtCtx* ctx, int32_t index, void**
  * Ray-marched in-scattering of every point shadow's light through the cube maps of idkpt_set_point_shadows /
  * idkpt_render_point_shadows (NEAREST lookup, no bias), at the render size w = (int)(width * ResolutionScale),
  * h = (int)(height * ResolutionScale), then upscaled to width x height with four depth-weighted bilinear taps.
- * depth: the G-buffer depth [depth_height][depth_width] (host array, sampled NEAREST); taa_jitter may be NULL.
+ * depth: the G-buffer depth [depth_height][depth_width] (host array, sampled NEAREST; idkpt_volumetric_lighting_gbuffer, below
+ * with the G-buffer passes, takes it from an IdkPtGBuffer); taa_jitter may be NULL.
  * out_rgba16f: width*height*4 halves (rgba16f, alpha 1), or NULL to keep the image on the device
  * (idkpt_volumetric_device_ptr: valid until the next call with other sizes, idkpt_set_scene or idkpt_destroy).
  * Synchronous; ordered after the samples idkpt_compute has queued. With no shadows set the image is 0.
@@ -368,7 +370,8 @@ IDKPT_API int idkpt_volumetric_device_ptr(IdkPtCtx* ctx, void** dev_ptr, uint64_
  *   keep it on the device (idkpt_deferred_device_ptr). taa_jitter may be NULL (0, 0). IsSSAO reads the image of the last
  *   idkpt_ssao call, which must have the G-buffer's size. indirect_rgba32f (IsVXGI; the cone trace's image, [Height][Width]
  *   rgba32f) and the ShadowMode 2 visibility images (rt_visibility[k]: shadow k's float [Height][Width] image, as
- *   idkpt_shadows_ray_traced writes it; read through the R8Unorm store rule) are host or device arrays as gbuffer->OnDevice
+ *   idkpt_shadows_ray_traced writes it or idkpt_shadows_device_ptr hands it over; read through the R8Unorm store rule;
+ *   idkvx_cone_trace_device_ptr hands over the indirect light) are host or device arrays as gbuffer->OnDevice
  *   says. In ShadowMode 1 and 2 every light's PointShadowIndex must be -1 or below the idkpt_set_point_shadows count, and
  *   ShadowMode 2 needs rt_count >= that count with no NULL entry; ShadowMode 0 ignores the index.
  * Both calls are synchronous and ordered after the samples idkpt_compute has queued. Their images are context allocations,
@@ -403,6 +406,30 @@ IDKPT_API int idkpt_deferred_lighting(IdkPtCtx* ctx, const GpuPerFrameData* fram
                                       const float* taa_jitter, const float* indirect_rgba32f, const float* const* rt_visibility, uint32_t rt_count,
                                       float* out_rgba32f, float* kernel_ms);
 IDKPT_API int idkpt_deferred_device_ptr(IdkPtCtx* ctx, void** dev_ptr, uint64_t* bytes);
+
+/* ---- the deferred pass's other inputs from an IdkPtGBuffer: ray-traced shadows and volumetric light ----
+ * Read the G-buffer as idkpt_ssao does (OnDevice 0: host arrays uploaded per call; 1: device arrays read in place, checked and
+ * aligned alike), so that a frame whose G-buffer comes from idkpt_gbuffer_device_ptrs never leaves the device. Every argument
+ * is checked before anything is uploaded or launched: a rejected call (IDKPT_ERR_INVALID_ARGUMENT) leaves every image as it
+ * was. Both calls are synchronous and ordered after the samples idkpt_compute has queued.
+ * idkpt_shadows_ray_traced_gbuffer: idkpt_shadows_ray_traced's pass for light light_index (samples 1..1024) over Depth and
+ *   NormalRG (the other attachments may be NULL), into the context's float [Height][Width] visibility image of `slot`
+ *   (0 <= slot < IDKPT_MAX_POINT_SHADOWS; one per point shadow). Pixels with depth == 1 keep what the image held, as the
+ *   shader returns early there: the last successful call's values for the slot if it had the G-buffer's size, else 0 (the
+ *   slot's first call, a new size, after a failed call or idkpt_set_scene). The deferred pass returns early on those pixels
+ *   too, so it never reads them. visibility_out: Width*Height floats, or NULL to keep the image on the device only.
+ * idkpt_shadows_device_ptr: that image of `slot` (Width*Height*4 bytes, 256-byte aligned) for idkpt_deferred_lighting's
+ *   rt_visibility[k] with OnDevice = 1; valid until the slot's next call with another size, a failed call for the slot,
+ *   idkpt_set_scene or idkpt_destroy. Fails before the slot's first successful call.
+ * idkpt_volumetric_lighting_gbuffer: idkpt_volumetric_lighting with the depth gbuffer->Depth [Height][Width] (the other
+ *   attachments are not read and may be NULL); same image, same idkpt_volumetric_device_ptr. */
+IDKPT_API int idkpt_shadows_ray_traced_gbuffer(IdkPtCtx* ctx, const GpuPerFrameData* frame, const IdkPtGBuffer* gbuffer, int32_t light_index,
+                                               int32_t samples, uint32_t noise_index, const float* taa_jitter, int32_t slot,
+                                               float* visibility_out, float* kernel_ms);
+IDKPT_API int idkpt_shadows_device_ptr(IdkPtCtx* ctx, int32_t slot, void** dev_ptr, uint64_t* bytes);
+IDKPT_API int idkpt_volumetric_lighting_gbuffer(IdkPtCtx* ctx, const GpuPerFrameData* frame, const IdkPtVolumetricSettings* settings,
+                                                const IdkPtGBuffer* gbuffer, int32_t width, int32_t height, const float* taa_jitter,
+                                                uint16_t* out_rgba16f, float* kernel_ms);
 
 /* ---- the end of the raster frame (RasterPipeline.Render: SSR.Compute, "Merge Textures", TaaResolve.Compute) ----
  * The lit image both calls read (`source`): IDKPT_LIT_SOURCE_ARRAY, a caller rgba32f [Height][Width] array (host or device as

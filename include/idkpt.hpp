@@ -238,6 +238,27 @@ public:
         check(idkpt_volumetric_device_ptr(ctx_, &p, bytes), "idkpt_volumetric_device_ptr");
         return p;
     }
+    // The two passes above on a host or device G-buffer (GBufferDevicePtrs' as it is). ShadowsRayTracedGBuffer writes the
+    // context's visibility image of `slot` (ShadowsDevicePtr: DeferredLighting's rtVisibility[k]); visibilityOut may be nullptr.
+    float ShadowsRayTracedGBuffer(const GpuPerFrameData& frame, const IdkPtGBuffer& gbuffer, int lightIndex, int samples, uint32_t noiseIndex,
+                                  const float* taaJitter, int32_t slot, float* visibilityOut) {
+        float ms = 0.0f;
+        check(idkpt_shadows_ray_traced_gbuffer(ctx_, &frame, &gbuffer, lightIndex, samples, noiseIndex, taaJitter, slot, visibilityOut, &ms),
+              "idkpt_shadows_ray_traced_gbuffer");
+        return ms;
+    }
+    void* ShadowsDevicePtr(int32_t slot, uint64_t* bytes = nullptr) {
+        void* p = nullptr;
+        check(idkpt_shadows_device_ptr(ctx_, slot, &p, bytes), "idkpt_shadows_device_ptr");
+        return p;
+    }
+    float VolumetricLightingGBuffer(const GpuPerFrameData& frame, const IdkPtVolumetricSettings& settings, const IdkPtGBuffer& gbuffer,
+                                    int width, int height, const float* taaJitter, uint16_t* outRgba16f) {
+        float ms = 0.0f;
+        check(idkpt_volumetric_lighting_gbuffer(ctx_, &frame, &settings, &gbuffer, width, height, taaJitter, outRgba16f, &ms),
+              "idkpt_volumetric_lighting_gbuffer");
+        return ms;
+    }
     // SSAO.Compute on a host or device G-buffer: out = Width * Height bytes (R8Unorm), or nullptr to keep the image on the device
     // (SsaoDevicePtr; DeferredLighting's IsSSAO reads it). Returns the kernel time in ms.
     float Ssao(const GpuPerFrameData& frame, const IdkPtSsaoSettings& settings, const IdkPtGBuffer& gbuffer, uint8_t* outR8) {
@@ -412,6 +433,17 @@ public:
         std::vector<float> out((size_t)width * height * 4);
         check(idkvx_cone_trace(ctx_, &frame, &settings, depth, normalRG, metallicRoughness, width, height, skyColor, out.data(), stats), "idkvx_cone_trace");
         return out;
+    }
+    // ConeTracer.Compute on a host or device G-buffer (PathTracer::GBufferDevicePtrs' as it is): out may be nullptr to keep the
+    // image on the device (ConeTraceDevicePtr: DeferredLighting's indirect light)
+    void ConeTraceGBuffer(const GpuPerFrameData& frame, const IdkVxConeSettings& settings, const IdkPtGBuffer& gbuffer, const float skyColor[3],
+                          float* outRgba32f, IdkVxStats* stats = nullptr) {
+        check(idkvx_cone_trace_gbuffer(ctx_, &frame, &settings, &gbuffer, skyColor, outRgba32f, stats), "idkvx_cone_trace_gbuffer");
+    }
+    void* ConeTraceDevicePtr(uint64_t* bytes = nullptr) const {
+        void* p = nullptr;
+        check(idkvx_cone_trace_device_ptr(ctx_, &p, bytes), "idkvx_cone_trace_device_ptr");
+        return p;
     }
     // ConeTracer.GpuSettings defaults (ConeTracer.cs:10-22)
     static IdkVxConeSettings DefaultConeSettings() {

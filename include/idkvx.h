@@ -99,6 +99,18 @@ IDKPT_API int idkvx_cone_trace(IdkVxCtx* ctx, const GpuPerFrameData* frame, cons
                                const float* depth, const float* normalRG, const float* metallicRoughness,
                                int32_t width, int32_t height, const float skyColor[3], float* out_rgba32f, IdkVxStats* stats);
 
+/* The same trace on an IdkPtGBuffer: Depth, NormalRG and MetallicRoughness (the other attachments may be NULL), host arrays with
+ * OnDevice = 0, device arrays on the context's device read in place with OnDevice = 1 (aligned to 4 bytes for Depth, 8 for the
+ * other two; as idkpt.h's G-buffer passes check them), e.g. idkpt_gbuffer_device_ptrs' G-buffer. out_rgba32f: Width*Height*4
+ * floats, or NULL to keep the image on the device only. Every argument is checked before anything is uploaded or launched:
+ * a rejected call (IDKPT_ERR_INVALID_ARGUMENT) leaves the image as it was.
+ * idkvx_cone_trace_device_ptr: the rgba32f image of the last successful idkvx_cone_trace* call (width * rows traced * 16 bytes,
+ * 256-byte aligned: idkpt_deferred_lighting's indirect_rgba32f with OnDevice = 1); valid until the next cone trace or
+ * idkvx_destroy. Fails before the first successful trace and after a failed one. */
+IDKPT_API int idkvx_cone_trace_gbuffer(IdkVxCtx* ctx, const GpuPerFrameData* frame, const IdkVxConeSettings* settings,
+                                       const IdkPtGBuffer* gbuffer, const float skyColor[3], float* out_rgba32f, IdkVxStats* stats);
+IDKPT_API int idkvx_cone_trace_device_ptr(IdkVxCtx* ctx, void** dev_ptr, uint64_t* bytes);
+
 /* Voxelizer.DebugRender (Voxelizer.cs:230-244, VXGI/Voxelize/DebugVisualization/compute.glsl): the grid-configuration view
  * (RasterPipeline.Render's IsConfigureGridMode branch). Per pixel of a width x height image, the camera ray of `frame`
  * (InvProjection, InvView, ViewPos; pixel centres, no jitter) is clipped to [GridMin, GridMax]; a ray that misses the box, or
