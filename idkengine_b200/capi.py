@@ -111,7 +111,7 @@ EXPORTS = [
     "idkpt_ssao", "idkpt_ssao_device_ptr", "idkpt_deferred_lighting", "idkpt_deferred_device_ptr",
     "idkpt_ssr", "idkpt_ssr_device_ptrs", "idkpt_taa_resolve", "idkpt_taa_device_ptr",
     "idkpt_shading_rate", "idkpt_shading_rate_device_ptr",
-    "idkpt_gbuffer", "idkpt_gbuffer_device_ptrs", "idkpt_read_gbuffer", "idkpt_transparency", "idkpt_lights_and_skybox",
+    "idkpt_gbuffer", "idkpt_gbuffer_device_ptrs", "idkpt_read_gbuffer", "idkpt_prev_positions_device_ptr", "idkpt_transparency", "idkpt_lights_and_skybox",
     "idkpt_sky_atmosphere", "idkpt_sky_equirectangular", "idkpt_read_sky",
     "idkpt_blas_build", "idkpt_blas_build_info", "idkpt_blas_build_copy", "idkpt_blas_build_free",
 ]
@@ -477,6 +477,8 @@ def load(path=None):
     L.idkpt_gbuffer.argtypes = [c_vp, c_vp, c_i32, c_i32, c_vp, c_vp, P(c_f)]
     L.idkpt_gbuffer_device_ptrs.restype = c_i32
     L.idkpt_gbuffer_device_ptrs.argtypes = [c_vp, P(IdkPtGBuffer), P(c_vp)]
+    L.idkpt_prev_positions_device_ptr.restype = c_i32
+    L.idkpt_prev_positions_device_ptr.argtypes = [c_vp, P(c_vp), P(c_u64)]
     L.idkpt_transparency.restype = c_i32
     L.idkpt_transparency.argtypes = [c_vp, c_vp, P(IdkPtTransparencySettings), P(IdkPtGBuffer), c_vp, c_vp, c_vp, c_i32, c_vp, c_vp, P(c_f)]
     L.idkpt_read_gbuffer.restype = c_i32

@@ -154,7 +154,16 @@ struct IdkPtCtx : IdkCtxBase {
     uint64_t unskinnedCount = 0;
     std::vector<uint32_t> unskinnedMaxJoint;   // per vertex max(JointIndices), host copy for range validation
     std::vector<GpuBlasDesc> hostDescs;
+    std::vector<GpuBlasInstance> hostInstances;   // host mirror of `instances` (idkpt_set_scene): a bound voxeliser's draw list
     size_t nodeBytes = 0;
+    // prevVertexPositionSSBO (ModelManager.cs:620): the positions before the last skin of each range. Created from the
+    // positions at the first idkpt_skin_vertices or idkpt_prev_positions_device_ptr after idkpt_set_scene, which releases it.
+    DevBuf prevPositions;
+
+    // voxelisers reading this scene (idkvx_set_scene_from); idkpt_destroy unbinds them. sceneGeneration counts idkpt_set_scene
+    // calls, so that a bound voxeliser knows when the instance list, and with it its work-queue size, may have changed.
+    std::vector<IdkVxCtx*> boundVoxelizers;
+    uint64_t sceneGeneration = 0;
 
     // wavefront buffers: one set per lane. A lane is one sample in flight (ray-gen .. last shade) on its own stream; with
     // several lanes the latency-bound tail bounces of one sample overlap the throughput-bound head of the next
@@ -599,6 +608,21 @@ static int upload_sphere_mesh(IdkPtCtx* ctx) {
     return IDKPT_OK;
 }
 
+// The kept previous positions, created on first need as a copy of the positions (ModelManager.cs:620 creates
+// prevVertexPositionSSBO from the uploaded positions; only skinning moves them afterwards). Ordered on the context stream.
+static int keep_prev_positions(IdkPtCtx* ctx) {
+    if (ctx->prevPositions.p) return IDKPT_OK;
+    const size_t bytes = ctx->counts.VertexPositionCount * sizeof(PackedVec3);
+    CK(ensure(ctx->prevPositions, std::max<size_t>(bytes, 16)));
+    const cudaError_t e = bytes ? cudaMemcpyAsync(ctx->prevPositions.p, ctx->positions.p, bytes, cudaMemcpyDeviceToDevice, ctx->stream) : cudaSuccess;
+    if (e != cudaSuccess) release(ctx->prevPositions);
+    CK(e);
+    return IDKPT_OK;
+}
+
+// idkvx_impl.cuh: forgets this context in every voxeliser bound to it (idkvx_set_scene_from), before it goes away.
+static void unbind_voxelizers(IdkPtCtx* ctx);
+
 extern "C" {
 
 IDKPT_API uint32_t idkpt_abi_version(void) { return IDKPT_ABI_VERSION; }
@@ -663,13 +687,14 @@ IDKPT_API void idkpt_destroy(IdkPtCtx* ctx) {
     if (!ctx) return;
     cudaSetDevice(ctx->device);
     drain(ctx);
+    unbind_voxelizers(ctx);
     DevBuf* all[] = {&ctx->nodes, &ctx->triRec, &ctx->blasTris, &ctx->positions, &ctx->descs, &ctx->instances, &ctx->xforms,
                      &ctx->meshes, &ctx->materials, &ctx->vertices, &ctx->lights, &ctx->tlas, &ctx->vtxFrame, &ctx->surfRec,
                      &ctx->images[0], &ctx->images[1], &ctx->images[2], &ctx->counters, &ctx->countLog, &ctx->skyFaces,
                      &ctx->tex.pixels, &ctx->tex.recs, &ctx->tex.srgbLut, &ctx->bloomDown, &ctx->bloomUp, &ctx->postConsts, &ctx->ldr,
                      &ctx->unskinned, &ctx->joints, &ctx->refitParents, &ctx->refitLocks, &ctx->scratch[0], &ctx->scratch[1], &ctx->scratch[2],
                      &ctx->tlasScratch, &ctx->oidn[0], &ctx->oidn[1], &ctx->oidn[2], &ctx->oidn[3], &ctx->denoiseWork[0], &ctx->denoiseWork[1], &ctx->denoised,
-                     &ctx->pointShadowDev, &ctx->pointShadowMaps, &ctx->pointShadowLights};
+                     &ctx->pointShadowDev, &ctx->pointShadowMaps, &ctx->pointShadowLights, &ctx->prevPositions};
     for (DevBuf* b : all) release(*b);
     release_raster(ctx->raster);
     for (int i = 0; i < IDK_MAX_LANES; i++) release_lane(ctx->lanes[i], false);
@@ -714,8 +739,10 @@ IDKPT_API int idkpt_set_scene(IdkPtCtx* ctx, const IdkPtSceneDesc* s) {
     // complete the context has NO scene: a failure below (CUDA error, out of memory) must not leave the previous scene's
     // pointers and counts looking valid.
     ctx->haveScene = false;
+    ctx->sceneGeneration++;
     ctx->pointShadows.clear(); ctx->pointShadowSizes.clear(); ctx->pointShadowRecs.clear();   // the shadows belong to the old scene
     release(ctx->pointShadowDev); release(ctx->pointShadowMaps); release(ctx->pointShadowLights);
+    release(ctx->prevPositions);
     release_raster(ctx->raster);   // the raster images belong to the old scene too
     int rc;
     // nodes and triangle records share one allocation ("bvh"): [nodes | triRec], so that one L2 access-policy window covers both
@@ -781,6 +808,7 @@ IDKPT_API int idkpt_set_scene(IdkPtCtx* ctx, const IdkPtSceneDesc* s) {
     ctx->counts = *s;
     ctx->hostLights.assign(s->Lights, s->Lights + s->LightCount);
     ctx->hostDescs.assign(s->BlasDescs, s->BlasDescs + s->BlasDescCount);
+    ctx->hostInstances.assign(s->BlasInstances, s->BlasInstances + s->BlasInstanceCount);
     ctx->nodeBytes = nodeBytes;
     if ((rc = configure_launches(ctx))) return rc;
     // Keep the BVH resident in the 50 MB L2: persisting access-policy window over [nodes | triRec] on the render stream.
@@ -1873,9 +1901,14 @@ IDKPT_API int idkpt_skin_vertices(IdkPtCtx* ctx, const float* jointMatrices, uin
     CK(cudaSetDevice(ctx->device));
     int rc;
     if ((rc = upload(ctx, ctx->joints, jointMatrices, jointCount * 48))) return rc;   // jointMatricesBuffer.UploadElements (ModelManager.cs:277)
+    if ((rc = keep_prev_positions(ctx))) return rc;
     rc = run_timed(ctx, "idkpt_skin_vertices", kernelMs, [&]() -> int {
         for (uint32_t c = 0; c < cmdCount; c++) {
             if (!cmds[c].VertexCount) continue;
+            // Skinning/compute.glsl:42, prevVertexPositionSSBO = vertexPositionSSBO over the command's output range, dispatch by
+            // dispatch: with overlapping commands the kept positions are those the previous command left, as in the engine
+            const size_t off = (size_t)cmds[c].OutputVertexOffset * sizeof(PackedVec3), n = (size_t)cmds[c].VertexCount * sizeof(PackedVec3);
+            CK(cudaMemcpyAsync((char*)ctx->prevPositions.p + off, (const char*)ctx->positions.p + off, n, cudaMemcpyDeviceToDevice, ctx->stream));
             SkinArgs a;
             a.unskinned = (const uint32_t*)ctx->unskinned.p; a.joints = (const float4*)ctx->joints.p;
             a.positions = (float*)ctx->positions.p; a.vertices = (uint4*)ctx->vertices.p; a.vtxFrame = (float4*)ctx->vtxFrame.p;
@@ -2729,14 +2762,17 @@ IDKPT_API int idkpt_gbuffer(IdkPtCtx* ctx, const GpuPerFrameData* frame, int32_t
     size_t off[6];
     const size_t bytes = gbuffer_planes(width, height, off);
     const size_t prevBytes = ctx->counts.VertexPositionCount * sizeof(PackedVec3);
+    // idkpt_prev_positions_device_ptr's buffer is read in place; any other pointer is a host array
+    const bool kept = prevPositions && (const void*)prevPositions == ctx->prevPositions.p;
+    const bool hostPrev = prevPositions && !kept;
     r.gb.invalidate();             // the images may be reallocated and are overwritten: valid again only when the call succeeds
-    if (ensure(r.gb.buf[0], bytes) != cudaSuccess || (prevPositions && ensure(r.gbPrev, std::max<size_t>(prevBytes, 16)) != cudaSuccess))
+    if (ensure(r.gb.buf[0], bytes) != cudaSuccess || (hostPrev && ensure(r.gbPrev, std::max<size_t>(prevBytes, 16)) != cudaSuccess))
         return fail(ctx, who, IDKPT_ERR_OUT_OF_MEMORY, "device allocation failed");
-    if (prevPositions && prevBytes) CK(cudaMemcpyAsync(r.gbPrev.p, prevPositions, prevBytes, cudaMemcpyHostToDevice, ctx->stream));
+    if (hostPrev && prevBytes) CK(cudaMemcpyAsync(r.gbPrev.p, prevPositions, prevBytes, cudaMemcpyHostToDevice, ctx->stream));
     char* base = (char*)r.gb.buf[0].p;
     a.sc = ctx->sc;
     a.positions = (const float*)ctx->positions.p;
-    a.prevPositions = prevPositions ? (const float*)r.gbPrev.p : a.positions;
+    a.prevPositions = kept ? (const float*)ctx->prevPositions.p : hostPrev ? (const float*)r.gbPrev.p : a.positions;
     memcpy(a.projView, frame->ProjView, sizeof(a.projView));
     memcpy(a.prevProjView, frame->PrevProjView, sizeof(a.prevProjView));
     memcpy(a.invProjView, frame->InvProjView, sizeof(a.invProjView));
@@ -2762,6 +2798,20 @@ IDKPT_API int idkpt_gbuffer_device_ptrs(IdkPtCtx* ctx, IdkPtGBuffer* gbufferOut,
         *gbufferOut = IdkPtGBuffer{r->w, r->h, 1, (const float*)(base + off[0]), (const float*)(base + off[1]),
                                    (const float*)(base + off[2]), (const float*)(base + off[3]), (const float*)(base + off[4])};
     if (velocityOut) *velocityOut = (const float*)(base + off[5]);
+    return IDKPT_OK;
+}
+
+IDKPT_API int idkpt_prev_positions_device_ptr(IdkPtCtx* ctx, void** devPtr, uint64_t* bytes) {
+    static const char* who = "idkpt_prev_positions_device_ptr";
+    if (!ctx || !devPtr) return fail(ctx, IDKPT_ERR_INVALID_ARGUMENT, "idkpt_prev_positions_device_ptr: null argument");
+    if (!ctx->haveScene) return fail(ctx, who, IDKPT_ERR_NO_SCENE, "no scene");
+    CK(cudaSetDevice(ctx->device));
+    if (!ctx->prevPositions.p) {
+        if (int rc = keep_prev_positions(ctx)) return rc;
+        CK(cudaStreamSynchronize(ctx->stream));    // the copy is complete before the pointer is handed out
+    }
+    *devPtr = ctx->prevPositions.p;
+    if (bytes) *bytes = ctx->counts.VertexPositionCount * sizeof(PackedVec3);
     return IDKPT_OK;
 }
 

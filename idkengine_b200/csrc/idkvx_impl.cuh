@@ -12,7 +12,10 @@ struct IdkVxCtx : IdkCtxBase {
     VxGridDev grid = {};
     DevBuf gridMem;
     size_t levelTexels[IDKVX_MAX_LEVELS] = {};
-    bool haveScene = false;
+    bool haveScene = false;               // idkvx_set_scene: the context holds its own copy of a scene
+    // idkvx_set_scene_from: no copy; each idkvx_voxelize reads this path tracer's device scene as it stands (bind_source)
+    IdkPtCtx* source = nullptr;
+    uint64_t sourceGeneration = 0;        // source->sceneGeneration that queueCapacity was sized for
     VxScene sc = {};
     IdkPtSceneDesc counts = {};
     std::vector<GpuBlasDesc> hostDescs;
@@ -30,7 +33,7 @@ struct IdkVxCtx : IdkCtxBase {
     int32_t maxPointShadowIndex = -1;     // largest PointShadowIndex of the scene's lights
     // the grid holds a whole voxelisation with its mip chain (idkpt_transparency's cone trace reads it): set by a successful
     // idkvx_voxelize of the whole grid, or by idkvx_mipmap after a slab voxelisation (the multi-GPU flow all-gathers the slabs in
-    // between); cleared by idkvx_set_grid, idkvx_set_scene and idkvx_set_slab
+    // between); cleared by idkvx_set_grid, idkvx_set_scene, idkvx_set_scene_from and idkvx_set_slab
     bool voxelized = false;
     bool slabVoxelized = false;           // idkvx_voxelize ran in slab mode since the grid last changed
     bool conservative = false;            // idkvx_set_conservative_rasterization: coverage rule of the next idkvx_voxelize
@@ -51,6 +54,68 @@ static int allocate_grid(IdkVxCtx* ctx, size_t bytes) {
     CK(cudaMemsetAsync(ctx->gridMem.p, 0, bytes, ctx->stream));   // ResultVoxels.Fill(0), Voxelizer.cs:258
     CK(ensure(ctx->queueCount, 16));
     CK(ensure(ctx->counters, 16));
+    return IDKPT_OK;
+}
+
+// Removes the voxeliser from its path tracer's list of bound voxelisers (idkvx_set_scene_from).
+static void unbind_source(IdkVxCtx* ctx) {
+    if (!ctx->source) return;
+    std::vector<IdkVxCtx*>& v = ctx->source->boundVoxelizers;
+    v.erase(std::remove(v.begin(), v.end(), ctx), v.end());
+    ctx->source = nullptr;
+}
+
+static void unbind_voxelizers(IdkPtCtx* pt) {
+    for (IdkVxCtx* vx : pt->boundVoxelizers) vx->source = nullptr;
+    pt->boundVoxelizers.clear();
+}
+
+// The scene arrays idkvx_set_scene copies, the texture table included.
+static void release_scene(IdkVxCtx* ctx) {
+    for (DevBuf* b : {&ctx->positions, &ctx->vertices, &ctx->tris, &ctx->descs, &ctx->instances, &ctx->xforms, &ctx->meshes,
+                      &ctx->materials, &ctx->lights, &ctx->tex.pixels, &ctx->tex.recs, &ctx->tex.srgbLut})
+        release(*b);
+}
+
+// Work items of the large-triangle queue for a draw list: (triangle, tile) items of large triangles.
+static int size_queue(IdkVxCtx* ctx, const std::vector<GpuBlasDesc>& descs, const std::vector<GpuBlasInstance>& instances) {
+    size_t maxTris = 0;
+    for (const GpuBlasInstance& bi : instances) maxTris += (size_t)descs[bi.BlasId].TriangleCount;
+    ctx->queueCapacity = maxTris * 2 + (1u << 20);
+    CK(ensure(ctx->queue, ctx->queueCapacity * sizeof(uint4)));
+    return IDKPT_OK;
+}
+
+// idkvx_voxelize of a bound voxeliser: VxScene's pointers, the light count and the shadowed-light bound from the path tracer's
+// scene as it stands now. Every path-tracer call that writes these arrays (idkpt_set_scene, idkpt_update_range,
+// idkpt_set_textures, idkpt_skin_vertices, idkpt_blas_refit, idkpt_tlas_build) ends in a synchronise of its stream, and so
+// does idkvx_voxelize; samples idkpt_compute has queued only read them. So the voxelisation reads a finished scene without
+// waiting for the path tracer, and a pointer is never kept past the call that could reallocate it.
+static int bind_source(IdkVxCtx* ctx) {
+    IdkPtCtx* pt = ctx->source;
+    if (!pt->haveScene)
+        return fail(ctx, IDKPT_ERR_NO_SCENE, "idkvx_voxelize: the path-tracer context bound with idkvx_set_scene_from has no scene (idkpt_set_scene)");
+    VxScene& sc = ctx->sc;
+    sc.positions = (const float*)pt->positions.p;
+    sc.vertices = (const uint4*)pt->vertices.p;
+    sc.blasTris = (const int4*)pt->blasTris.p;
+    sc.descs = (const GpuBlasDesc*)pt->descs.p;
+    sc.instances = (const GpuBlasInstance*)pt->instances.p;
+    sc.xforms = (const float4*)pt->xforms.p;
+    sc.meshes = (const GpuMesh*)pt->meshes.p;
+    sc.materials = (const GpuMaterial*)pt->materials.p;
+    sc.lights = (const GpuLight*)pt->lights.p;
+    sc.textures = (const TexRec*)pt->tex.recs.p;
+    sc.srgbLut = (const float*)pt->tex.srgbLut.p;
+    sc.lightCount = (uint32_t)pt->counts.LightCount;
+    ctx->maxPointShadowIndex = -1;   // idkpt_update_range(LIGHTS) may have changed it
+    for (const GpuLight& L : pt->hostLights) ctx->maxPointShadowIndex = std::max(ctx->maxPointShadowIndex, L.PointShadowIndex);
+    ctx->shadowedLights = ctx->maxPointShadowIndex >= 0;
+    if (ctx->sourceGeneration != pt->sceneGeneration) {
+        CK(cudaSetDevice(ctx->device));
+        if (int rc = size_queue(ctx, pt->hostDescs, pt->hostInstances)) return rc;
+        ctx->sourceGeneration = pt->sceneGeneration;
+    }
     return IDKPT_OK;
 }
 
@@ -115,9 +180,9 @@ IDKPT_API void idkvx_destroy(IdkVxCtx* ctx) {
     if (!ctx) return;
     cudaSetDevice(ctx->device);
     if (ctx->stream) cudaStreamSynchronize(ctx->stream);
-    DevBuf* all[] = {&ctx->gridMem, &ctx->positions, &ctx->vertices, &ctx->tris, &ctx->descs, &ctx->instances, &ctx->xforms, &ctx->meshes,
-                     &ctx->materials, &ctx->lights, &ctx->tex.pixels, &ctx->tex.recs, &ctx->tex.srgbLut, &ctx->queue, &ctx->queueCount,
-                     &ctx->counters, &ctx->stage, &ctx->cone.buf[0], &ctx->debugImage, &ctx->debugMask};
+    unbind_source(ctx);
+    release_scene(ctx);
+    DevBuf* all[] = {&ctx->gridMem, &ctx->queue, &ctx->queueCount, &ctx->counters, &ctx->stage, &ctx->cone.buf[0], &ctx->debugImage, &ctx->debugMask};
     for (DevBuf* b : all) release(*b);
     destroy_stream(ctx);
     delete ctx;
@@ -136,6 +201,7 @@ IDKPT_API int idkvx_set_scene(IdkVxCtx* ctx, const IdkPtSceneDesc* s) {
     if (!ctx || !s) return fail(ctx, IDKPT_ERR_INVALID_ARGUMENT, "idkvx_set_scene: null argument");
     CK(cudaSetDevice(ctx->device));
     if (int rc = validate_scene(ctx, "idkvx_set_scene", s)) return rc;
+    unbind_source(ctx);
     ctx->voxelized = ctx->slabVoxelized = false;
     ctx->haveScene = false;   // the device arrays are overwritten from here on: a failure below leaves no scene
     ctx->shadowedLights = false;
@@ -154,12 +220,9 @@ IDKPT_API int idkvx_set_scene(IdkVxCtx* ctx, const IdkPtSceneDesc* s) {
     if ((rc = upload(ctx, ctx->lights, s->Lights, s->LightCount * sizeof(GpuLight)))) return rc;
     // material textures (BaseColor / Emissive are the slots the voxeliser's fragment stage uses)
     if ((rc = upload_textures(ctx, ctx->tex, s->Textures, s->TextureCount))) return rc;
-    size_t maxTris = 0;
     ctx->hostDescs.assign(s->BlasDescs, s->BlasDescs + s->BlasDescCount);
     ctx->hostInstances.assign(s->BlasInstances, s->BlasInstances + s->BlasInstanceCount);
-    for (const GpuBlasInstance& bi : ctx->hostInstances) maxTris += (size_t)ctx->hostDescs[bi.BlasId].TriangleCount;
-    ctx->queueCapacity = maxTris * 2 + (1u << 20);   // (triangle, tile) work items of large triangles
-    CK(ensure(ctx->queue, ctx->queueCapacity * sizeof(uint4)));
+    if ((rc = size_queue(ctx, ctx->hostDescs, ctx->hostInstances))) return rc;
     VxScene& sc = ctx->sc;
     sc.positions = (const float*)ctx->positions.p;
     sc.vertices = (const uint4*)ctx->vertices.p;
@@ -179,9 +242,38 @@ IDKPT_API int idkvx_set_scene(IdkVxCtx* ctx, const IdkPtSceneDesc* s) {
     return IDKPT_OK;
 }
 
+IDKPT_API int idkvx_set_scene_from(IdkVxCtx* ctx, IdkPtCtx* pathTracer) {
+    if (!ctx) return IDKPT_ERR_INVALID_ARGUMENT;
+    if (pathTracer && pathTracer->device != ctx->device)
+        return fail(ctx, IDKPT_ERR_UNSUPPORTED, "idkvx_set_scene_from: the path-tracer context is on another device");
+    CK(cudaSetDevice(ctx->device));
+    unbind_source(ctx);
+    release_scene(ctx);
+    ctx->haveScene = false;
+    ctx->hostDescs.clear();
+    ctx->hostInstances.clear();
+    ctx->counts = {};
+    ctx->shadowedLights = false;
+    ctx->maxPointShadowIndex = -1;
+    ctx->voxelized = ctx->slabVoxelized = false;
+    if (pathTracer) {
+        ctx->source = pathTracer;
+        ctx->sourceGeneration = pathTracer->sceneGeneration - 1;   // sizes the work queue at the first voxelisation
+        pathTracer->boundVoxelizers.push_back(ctx);
+    }
+    return IDKPT_OK;
+}
+
 IDKPT_API int idkvx_voxelize(IdkVxCtx* ctx, IdkVxStats* stats) {
     if (!ctx) return IDKPT_ERR_INVALID_ARGUMENT;
-    if (!ctx->haveScene) return fail(ctx, IDKPT_ERR_NO_SCENE, "idkvx_voxelize: idkvx_set_scene has not been called");
+    if (ctx->source) {
+        if (int rc = bind_source(ctx)) return rc;
+    } else if (!ctx->haveScene) {
+        return fail(ctx, IDKPT_ERR_NO_SCENE, "idkvx_voxelize: idkvx_set_scene has not been called (or idkvx_set_scene_from's path-tracer "
+                                             "context was unbound or destroyed)");
+    }
+    const std::vector<GpuBlasDesc>& descs = ctx->source ? ctx->source->hostDescs : ctx->hostDescs;
+    const std::vector<GpuBlasInstance>& instances = ctx->source ? ctx->source->hostInstances : ctx->hostInstances;
     // fragment.glsl:55-58: lights with PointShadowIndex >= 0 are multiplied by Visibility(), a PCF lookup into the shadow cube
     // map. With shadow maps attached that lookup runs on the path tracer's traced cube maps (idkvx_set_shadow_maps); otherwise
     // the same question -- is the (2 % biased) sample point visible from the light -- is answered by an any-hit shadow ray
@@ -223,8 +315,8 @@ IDKPT_API int idkvx_voxelize(IdkVxCtx* ctx, IdkVxStats* stats) {
         CK(cudaMemsetAsync(ctx->queueCount.p, 0, 16, ctx->stream));
         CK(cudaMemsetAsync(ctx->counters.p, 0, 16, ctx->stream));
         CK(cudaEventRecord(ctx->timing[2], ctx->stream));
-        for (size_t i = 0; i < ctx->hostInstances.size(); i++) {
-            const GpuBlasDesc& d = ctx->hostDescs[ctx->hostInstances[i].BlasId];
+        for (size_t i = 0; i < instances.size(); i++) {
+            const GpuBlasDesc& d = descs[instances[i].BlasId];
             if (d.TriangleCount <= 0) continue;
             VxVoxelizeArgs a;
             a.sc = ctx->sc; a.g = ctx->grid; a.instance = (uint32_t)i;

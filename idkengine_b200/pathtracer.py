@@ -566,24 +566,35 @@ class PathTracer:
 
     def GBuffer(self, frame, width, height, jitter=None, prev_positions=None, download=True):
         """Renders the G-buffer pass at width x height (DESIGN.md 8f.1g). jitter: taaDataUBO.Jitter in NDC units (None = 0);
-        prev_positions: the previous frame's vertex positions, float32 [VertexPositionCount, 3] (None = this frame's). Returns
+        prev_positions: the previous frame's vertex positions, float32 [VertexPositionCount, 3], "kept" for the positions
+        SkinVertices keeps on the device (PrevPositionsDevicePtr, read in place), or None for this frame's. Returns
         (depth [h, w], normal_rg [h, w, 2], albedo [h, w, 3], metallic_roughness [h, w, 2], emissive [h, w, 3], velocity_rg
         [h, w, 2]) as float32 numpy arrays, or None with download=False (the images stay on the device: GBufferDevicePtrs).
         Kernel ms in last_gbuffer_ms."""
         jit = self._jitter(jitter)
-        prev = None if prev_positions is None else np.ascontiguousarray(prev_positions, np.float32)
-        if prev is not None and (prev.ndim != 2 or prev.shape[1] != 3 or prev.shape[0] != self._vertex_position_count):
-            raise ValueError(f"GBuffer: prev_positions {prev.shape}: expected ({self._vertex_position_count}, 3)")
+        if isinstance(prev_positions, str):
+            if prev_positions != "kept":
+                raise ValueError(f"GBuffer: prev_positions {prev_positions!r}: expected an array, 'kept' or None")
+            prev_ptr = self.PrevPositionsDevicePtr()[0]
+        else:
+            prev = None if prev_positions is None else np.ascontiguousarray(prev_positions, np.float32)
+            if prev is not None and (prev.ndim != 2 or prev.shape[1] != 3 or prev.shape[0] != self._vertex_position_count):
+                raise ValueError(f"GBuffer: prev_positions {prev.shape}: expected ({self._vertex_position_count}, 3)")
+            prev_ptr = prev.ctypes.data if prev is not None else None
         frame = np.ascontiguousarray(frame)
         ms = ctypes.c_float()
-        self._check(self._lib.idkpt_gbuffer(self._ctx, frame.ctypes.data, width, height, jit,
-                                            prev.ctypes.data if prev is not None else None, ctypes.byref(ms)), "idkpt_gbuffer")
+        self._check(self._lib.idkpt_gbuffer(self._ctx, frame.ctypes.data, width, height, jit, prev_ptr, ctypes.byref(ms)), "idkpt_gbuffer")
         self.last_gbuffer_ms = ms.value
         if not download:
             return None
         out = [np.zeros((height, width) if c == 1 else (height, width, c), np.float32) for c in self.GBUFFER_CHANNELS]
         self._check(self._lib.idkpt_read_gbuffer(self._ctx, *[a.ctypes.data for a in out]), "idkpt_read_gbuffer")
         return tuple(out)
+
+    def PrevPositionsDevicePtr(self):
+        """(device pointer, bytes) of the previous vertex positions SkinVertices keeps (prevVertexPositionSSBO: PackedVec3 per
+        vertex position), valid until SetScene or Dispose."""
+        return self._device_ptr("idkpt_prev_positions_device_ptr")
 
     def GBufferDevicePtrs(self, tensors=False):
         """The images of the last GBuffer call: (capi.IdkPtGBuffer with OnDevice = 1, velocity device pointer), or with

@@ -24,7 +24,7 @@ class IdkVxStats(ctypes.Structure):
                 ("ConeSteps", c_u64), ("KernelLaunches", c_u32), ("_pad0", c_u32)]
 
 
-VX_EXPORTS = ["idkvx_create", "idkvx_destroy", "idkvx_last_error", "idkvx_set_scene", "idkvx_set_grid", "idkvx_level_count",
+VX_EXPORTS = ["idkvx_create", "idkvx_destroy", "idkvx_last_error", "idkvx_set_scene", "idkvx_set_scene_from", "idkvx_set_grid", "idkvx_level_count",
               "idkvx_voxelize", "idkvx_read_level", "idkvx_cone_trace", "idkvx_set_shadow_tracer",
               "idkvx_set_shadow_maps", "idkvx_set_slab", "idkvx_level_device_ptr", "idkvx_mipmap", "idkvx_cone_trace_rows",
               "idkvx_set_conservative_rasterization", "idkvx_debug_render", "idkvx_debug_device_ptr",
@@ -65,6 +65,8 @@ def _declare(L):
     L.idkvx_last_error.argtypes = [c_vp]
     L.idkvx_set_scene.restype = c_i32
     L.idkvx_set_scene.argtypes = [c_vp, P(capi.IdkPtSceneDesc)]
+    L.idkvx_set_scene_from.restype = c_i32
+    L.idkvx_set_scene_from.argtypes = [c_vp, c_vp]
     L.idkvx_set_grid.restype = c_i32
     L.idkvx_set_grid.argtypes = [c_vp, P(c_f * 3), P(c_f * 3)]
     L.idkvx_level_count.restype = c_i32
@@ -114,6 +116,7 @@ class Voxelizer:
             raise IdkVxError(f"idkvx_create failed ({rc}): {(self._lib.idkvx_last_error(None) or b'').decode()}")
         self.sizes = level_sizes(self.ci)
         self._conservative = False
+        self._source = None                # the PathTracer bound with SetSceneFrom, kept alive while bound
         self.DebugStepMultiplier = 0.4     # the constructor defaults of Voxelizer.cs:68 (DebugRender)
         self.DebugConeAngle = 0.0
 
@@ -125,6 +128,7 @@ class Voxelizer:
         if self._ctx:
             self._lib.idkvx_destroy(self._ctx)
             self._ctx = c_vp()
+            self._source = None
 
     def __enter__(self):
         return self
@@ -135,6 +139,13 @@ class Voxelizer:
     def SetScene(self, scene):
         d, keep = capi.scene_desc(scene)
         self._check(self._lib.idkvx_set_scene(self._ctx, ctypes.byref(d)), "idkvx_set_scene")
+        self._source = None
+
+    def SetSceneFrom(self, path_tracer):
+        """Voxelise path_tracer's device scene as it stands at each Render, with no copy of it (idkvx_set_scene_from): skinning,
+        UpdateRange and a new SetScene on the path tracer reach the next Render. None unbinds and leaves no scene."""
+        self._check(self._lib.idkvx_set_scene_from(self._ctx, path_tracer._ctx if path_tracer is not None else None), "idkvx_set_scene_from")
+        self._source = path_tracer
 
     def SetGrid(self, grid_min, grid_max):
         """Voxelizer.GridMin / GridMax setters (Voxelizer.cs:16-33); the next Render voxelises the new bounds."""

@@ -519,13 +519,17 @@ IDKPT_API int idkpt_shading_rate_device_ptr(IdkPtCtx* ctx, void** dev_ptr, uint6
  *   holding exactly what the engine's attachments hold (R11G11B10F albedo and emissive, RG8 normal and metallic/roughness,
  *   RG16F velocity, D32F depth); pixels without a surface hold the clears (depth 1, everything else 0). The rules are in
  *   DESIGN.md 8f.1g. taa_jitter: taaDataUBO.Jitter in NDC units, NULL = (0, 0). prev_positions: the previous frame's vertex
- *   positions (prevVertexPositionSSBO, VertexPositionCount entries), NULL = this frame's (static geometry); idkpt_skin_vertices
- *   keeps no copy, so a host that animates passes them. Lights and the skybox are separate draws: idkpt_lights_and_skybox
- *   draws them into these images afterwards.
+ *   positions (prevVertexPositionSSBO, VertexPositionCount entries): idkpt_prev_positions_device_ptr's pointer, read in place
+ *   (what idkpt_skin_vertices keeps, so an animated frame uploads nothing), any other pointer a host array, NULL = this
+ *   frame's (static geometry). Lights and the skybox are separate draws: idkpt_lights_and_skybox draws them into these
+ *   images afterwards.
  * idkpt_gbuffer_device_ptrs: the images of the last successful call: an IdkPtGBuffer with OnDevice = 1 that idkpt_ssao,
  *   idkpt_deferred_lighting and idkpt_ssr take as it is, and the velocity for IdkPtTaaInputs / IdkPtShadingRateInputs.
  *   Either output may be NULL.
  * idkpt_read_gbuffer: downloads the images of the last successful call; any argument may be NULL.
+ * idkpt_prev_positions_device_ptr: the context's previous positions (PackedVec3 [VertexPositionCount], *bytes their size), as
+ *   idkpt_skin_vertices keeps them. Created at the first idkpt_skin_vertices or idkpt_prev_positions_device_ptr after
+ *   idkpt_set_scene as a copy of the positions at that moment; valid until idkpt_set_scene or idkpt_destroy. Needs a scene.
  * The call is synchronous and ordered after the samples idkpt_compute has queued. Its images are context allocations, reused
  * by calls with the same size, valid until the next call with another size, a failed call, idkpt_set_scene or idkpt_destroy. */
 IDKPT_API int idkpt_gbuffer(IdkPtCtx* ctx, const GpuPerFrameData* frame, int32_t width, int32_t height, const float* taa_jitter,
@@ -533,6 +537,7 @@ IDKPT_API int idkpt_gbuffer(IdkPtCtx* ctx, const GpuPerFrameData* frame, int32_t
 IDKPT_API int idkpt_gbuffer_device_ptrs(IdkPtCtx* ctx, IdkPtGBuffer* gbuffer_out, const float** velocity_rg_out);
 IDKPT_API int idkpt_read_gbuffer(IdkPtCtx* ctx, float* depth, float* normal_rg, float* albedo_rgb, float* metallic_roughness,
                                  float* emissive_rgb, float* velocity_rg);
+IDKPT_API int idkpt_prev_positions_device_ptr(IdkPtCtx* ctx, void** dev_ptr, uint64_t* bytes);
 
 /* ---- transparency (RasterPipeline.Render: "Record transparent fragments" + "Resolve transparent fragments") ----
  * idkpt_transparency: the blended surfaces (AlphaCutoff == 2) the G-buffer pass culls, ray-cast at pixel centres along
@@ -583,7 +588,10 @@ IDKPT_API int idkpt_lights_and_skybox(IdkPtCtx* ctx, const GpuPerFrameData* fram
 /* ---- dynamic geometry (SURVEY.md 8f.2): ModelManager.Update = skin -> refit -> TLAS (ModelManager.cs:236-261) ----
  * idkpt_set_skinning_data: unskinnedVertexSSBO upload (52-byte GpuUnskinnedVertex records).
  * idkpt_skin_vertices: uploads the joint matrices (row-major mat4x3 = 3 x vec4 each, ModelManager.cs:272-277) and runs
- *   Skinning/compute.glsl once per command; positions, normals and tangents are rewritten in place on the device.
+ *   Skinning/compute.glsl once per command; positions, normals and tangents are rewritten in place on the device. Before
+ *   each command skins its output range, the call copies that range of the positions into the context's previous positions
+ *   (Skinning/compute.glsl:42, idkpt_prev_positions_device_ptr), so overlapping commands keep what the earlier command
+ *   left. Every argument is checked first: a rejected call changes neither. kernel_ms covers the copies and the kernels.
  * idkpt_blas_refit: BVH.GpuBlasesRefit(first, count) (BVH.cs:472-489, BLASRefit/compute.glsl); also refreshes the derived
  *   triangle records of the refitted BLASes. Call it for every BLAS whose vertices moved.
  * idkpt_read_range: device -> host read-back (refitted BLAS nodes for the host TLAS build, skinned vertices).

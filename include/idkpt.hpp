@@ -324,7 +324,7 @@ public:
         return p;
     }
     // The G-buffer pass at width x height into context images (DESIGN.md 8f.1g); taaJitter and prevPositions may be nullptr.
-    // Returns the kernel time in ms.
+    // prevPositions may be PrevPositionsDevicePtr(), read in place. Returns the kernel time in ms.
     float GBuffer(const GpuPerFrameData& frame, int32_t width, int32_t height, const float* taaJitter = nullptr,
                   const PackedVec3* prevPositions = nullptr) {
         float ms = 0.0f;
@@ -339,6 +339,12 @@ public:
     }
     void ReadGBuffer(float* depth, float* normalRG, float* albedoRGB, float* metallicRoughness, float* emissiveRGB, float* velocityRG) {
         check(idkpt_read_gbuffer(ctx_, depth, normalRG, albedoRGB, metallicRoughness, emissiveRGB, velocityRG), "idkpt_read_gbuffer");
+    }
+    // prevVertexPositionSSBO: the positions SkinVertices keeps from before each skin, valid until SetScene or Dispose
+    const PackedVec3* PrevPositionsDevicePtr(uint64_t* bytes = nullptr) {
+        void* p = nullptr;
+        check(idkpt_prev_positions_device_ptr(ctx_, &p, bytes), "idkpt_prev_positions_device_ptr");
+        return (const PackedVec3*)p;
     }
     // The blended layers composited over the lit image in place (DESIGN.md 8f.1h): the context's deferred image (source
     // IDKPT_LIT_SOURCE_DEFERRED) or `color` (IDKPT_LIT_SOURCE_ARRAY); only gbuffer.Depth is read. voxels / cone: IsVXGI only.
@@ -417,6 +423,8 @@ public:
     void Dispose() { if (ctx_) { idkvx_destroy(ctx_); ctx_ = nullptr; } }
 
     void SetScene(const IdkPtSceneDesc& scene) { check(idkvx_set_scene(ctx_, &scene), "idkvx_set_scene"); }
+    // Voxelise pt's device scene as it stands at each Render, with no copy (idkvx_set_scene_from); SetScene ends the binding
+    void SetSceneFrom(PathTracer& pt) { check(idkvx_set_scene_from(ctx_, pt.Handle()), "idkvx_set_scene_from"); }
     void SetGrid(const float gridMin[3], const float gridMax[3]) { check(idkvx_set_grid(ctx_, gridMin, gridMax), "idkvx_set_grid"); }   // GridMin / GridMax setters
     int LevelCount() const { return idkvx_level_count(ctx_); }
     IdkVxStats Render() { IdkVxStats st = {}; check(idkvx_voxelize(ctx_, &st), "idkvx_voxelize"); return st; }

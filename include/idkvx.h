@@ -63,6 +63,21 @@ IDKPT_API const char* idkvx_last_error(IdkVxCtx* ctx);
 /* Geometry + materials + lights of the scene (same arrays as idkpt_set_scene; the BVH members are used only for the
  * triangle list and the instance -> transform map). */
 IDKPT_API int idkvx_set_scene(IdkVxCtx* ctx, const IdkPtSceneDesc* scene);
+
+/* Voxelizer.Render(modelManager) reads the scene the engine binds globally; this is that binding. After the call the voxeliser
+ * holds no scene of its own (idkvx_set_scene's copies are released) and every idkvx_voxelize reads path_tracer's device arrays
+ * as they stand at that moment: positions, normals and tangents after idkpt_skin_vertices, MESH_TRANSFORMS, MESHES,
+ * MATERIALS and LIGHTS after idkpt_update_range, textures after idkpt_set_textures, and a new idkpt_set_scene all reach the
+ * next voxelisation with no copy. The kernels, their launches, slab mode, both coverage rules and the point-shadow rules
+ * (idkvx_set_shadow_maps / idkvx_set_shadow_tracer) are those of a voxeliser with its own scene.
+ * path_tracer must be on the voxeliser's device (else IDKPT_ERR_UNSUPPORTED); it may have no scene yet: idkvx_voxelize then
+ * fails with IDKPT_ERR_NO_SCENE until it has one. NULL unbinds and leaves no scene. The grid's voxelised state is cleared, as
+ * idkvx_set_scene clears it. A later idkvx_set_scene returns to an owned copy.
+ * Lifetime: idkpt_destroy unbinds every voxeliser bound to the path tracer (their next idkvx_voxelize fails with
+ * IDKPT_ERR_NO_SCENE); idkvx_destroy, a rebind, idkvx_set_scene or an unbind ends the binding from the voxeliser's side.
+ * Ordering: every path-tracer call that writes scene arrays, and idkvx_voxelize, is synchronous, and samples idkpt_compute has
+ * queued only read the scene; so idkvx_voxelize needs no idkpt_sync. */
+IDKPT_API int idkvx_set_scene_from(IdkVxCtx* ctx, struct IdkPtCtx* path_tracer);
 IDKPT_API int idkvx_set_grid(IdkVxCtx* ctx, const float gridMin[3], const float gridMax[3]);   /* Voxelizer.GridMin/GridMax, Voxelizer.cs:16-33 */
 IDKPT_API int32_t idkvx_level_count(IdkVxCtx* ctx);                                           /* Texture.GetMaxMipmapLevel */
 
