@@ -93,6 +93,7 @@ IDKPT_GATHER_HANDLE_BYTES = 320
 IDKPT_CREATE_GLOBAL_SLOTS = 1 << 12
 IDKPT_ARRAY_MESH_TRANSFORMS, IDKPT_ARRAY_MESHES, IDKPT_ARRAY_MATERIALS, IDKPT_ARRAY_LIGHTS = 0, 1, 2, 3
 IDKPT_ARRAY_TLAS_NODES, IDKPT_ARRAY_BLAS_NODES, IDKPT_ARRAY_VERTEX_POSITIONS, IDKPT_ARRAY_VERTICES = 4, 5, 6, 7
+IDKPT_ARRAY_BLAS_TRIANGLES, IDKPT_ARRAY_BLAS_DESCS = 8, 9
 
 # every symbol include/idkpt.h declares
 EXPORTS = [
@@ -113,7 +114,7 @@ EXPORTS = [
     "idkpt_shading_rate", "idkpt_shading_rate_device_ptr",
     "idkpt_gbuffer", "idkpt_gbuffer_device_ptrs", "idkpt_read_gbuffer", "idkpt_prev_positions_device_ptr", "idkpt_transparency", "idkpt_lights_and_skybox",
     "idkpt_sky_atmosphere", "idkpt_sky_equirectangular", "idkpt_read_sky",
-    "idkpt_blas_build", "idkpt_blas_build_info", "idkpt_blas_build_copy", "idkpt_blas_build_free",
+    "idkpt_blas_build", "idkpt_blas_build_info", "idkpt_blas_build_copy", "idkpt_blas_build_free", "idkpt_blas_rebuild", "idkpt_blas_sah",
 ]
 
 IDKPT_MAX_POINT_SHADOWS = 128
@@ -433,6 +434,10 @@ def load(path=None):
     L.idkpt_blas_build_copy.argtypes = [c_vp, c_vp, c_vp]
     L.idkpt_blas_build_free.restype = None
     L.idkpt_blas_build_free.argtypes = [c_vp]
+    L.idkpt_blas_rebuild.restype = c_i32
+    L.idkpt_blas_rebuild.argtypes = [c_vp, c_u32, c_u32, P(IdkPtBlasBuildSettings), P(c_f)]
+    L.idkpt_blas_sah.restype = c_i32
+    L.idkpt_blas_sah.argtypes = [c_vp, c_u32, c_u32, P(IdkPtBlasBuildSettings), c_vp]
     L.idkpt_denoise.restype = c_i32
     L.idkpt_denoise.argtypes = [c_vp, P(IdkPtDenoiseSettings), P(c_f)]
     L.idkpt_denoise_device_ptrs.restype = c_i32

@@ -652,6 +652,28 @@ __global__ void k_pair_write(GpuBlasNode* final, int pairs, const unsigned long 
     }
 }
 
+// BLAS.ComputeGlobalSAH (BLAS.cs:629-656) of one BLAS as the device holds it (built, refitted or rebuilt): one thread walks
+// the tree in the engine's pre-order, left child first, and adds the terms in that order. `stack` holds the pending right
+// children: at most one per level, so the node count bounds it.
+__global__ void k_global_sah(const GpuBlasNode* nodes, int* stack, float triangleCost, double* out) {
+    const double rootArea = 1.0 / (double)nodeHalfArea(nodes[1]);
+    double cost = 0.0;
+    int sp = 0, v = 1;
+    for (;;) {
+        const GpuBlasNode n = nodes[v];
+        cost += sahTerm(n, rootArea, triangleCost);
+        if (!(n.TriCount > 0)) {
+            stack[sp++] = n.TriStartOrChild + 1;
+            v = n.TriStartOrChild;
+        } else if (sp > 0) {
+            v = stack[--sp];
+        } else {
+            break;
+        }
+    }
+    *out = cost;
+}
+
 }  // namespace idkbb
 
 // ---------------------------------------------------------------------------------------------------------------- host driver
@@ -716,19 +738,22 @@ enum { BB_OK = 0, BB_CUDA = 1, BB_TOO_MANY_FRAGMENTS = 2 };
         if (e_ != cudaSuccess) { err = std::string(#call) + ": " + cudaGetErrorString(e_); return BB_CUDA; } \
     } while (0)
 
-// Runs the whole build on `stream`; the arguments have been validated. Fills `out` and the total device time.
-static int build(cudaStream_t stream, const PackedVec3* hPos, uint64_t vertexCount, const GpuBlasTriangle* hTris, int triCount,
-                 const Params& p, IdkPtBlasBuild& out, float& totalMs, std::string& err) {
+// One build's result on the device: the nodes, the triangles and the SAH live in allocations of the caller's arena.
+struct DeviceResult {
+    GpuBlasNode* nodes = nullptr;
+    int nodeCount = 0;
+    GpuBlasTriangle* tris = nullptr;
+    int triCount = 0;
+    int requiredStackSize = 0;
+    int fragmentCount = 0;
+    double* sah = nullptr;
+};
+
+// Runs the whole build on `stream` from device arrays (global vertex ids into `pos`); the arguments have been validated.
+// The result goes to `out`, in allocations of `keep`; the scratch is freed on return, after the stream has been waited for.
+static int build_device(cudaStream_t stream, const PackedVec3* pos, const GpuBlasTriangle* tris, int triCount, const Params& p,
+                        Arena& keep, DeviceResult& out, StageTimer& tm, std::string& err) {
     Arena ar;
-    StageTimer tm(stream);
-    tm.mark("start");
-    PackedVec3* pos;
-    GpuBlasTriangle* tris;
-    BB_CK(ar.get(pos, vertexCount));
-    BB_CK(ar.get(tris, triCount));
-    BB_CK(cudaMemcpyAsync(pos, hPos, vertexCount * sizeof(PackedVec3), cudaMemcpyHostToDevice, stream));
-    BB_CK(cudaMemcpyAsync(tris, hTris, (size_t)triCount * sizeof(GpuBlasTriangle), cudaMemcpyHostToDevice, stream));
-    tm.mark("upload");
 
     // ---- 1. fragments
     int n = triCount;
@@ -913,7 +938,7 @@ static int build(cudaStream_t stream, const PackedVec3* hPos, uint64_t vertexCou
     int* selCount;
     BB_CK(ar.get(terms, cap));
     BB_CK(ar.get(packed, cap));
-    BB_CK(ar.get(acc, 3));
+    BB_CK(keep.get(acc, 3));
     BB_CK(ar.get(flags, cap));
     BB_CK(ar.get(selCount, 1));
     BB_CK(cudaMemsetAsync(acc, 0, 3 * sizeof(double), stream));
@@ -984,7 +1009,7 @@ static int build(cudaStream_t stream, const PackedVec3* hPos, uint64_t vertexCou
     k_inner_ranks<<<blocksFor(m2, 256), 256, 0, stream>>>(order2, m2, innerScan, rankOf);
     const int f = 2 + 2 * inner;
     GpuBlasNode* final;
-    BB_CK(ar.get(final, f));
+    BB_CK(keep.get(final, f));
     BB_CK(cudaMemsetAsync(final, 0, sizeof(GpuBlasNode) * 2, stream));
     k_final_nodes<<<blocksFor(m2, 256), 256, 0, stream>>>(order2, m2, a.nodes, a.parent, a.depth, a.ostart, a.ocount, rankOf,
                                                           maxDepth, final, fidx);
@@ -992,7 +1017,7 @@ static int build(cudaStream_t stream, const PackedVec3* hPos, uint64_t vertexCou
 
     // unindexing
     GpuBlasTriangle* outTris;
-    BB_CK(ar.get(outTris, n));
+    BB_CK(keep.get(outTris, n));
     int triOut = n;
     if (!p.doPreSplit) {
         int *cnt, *off;
@@ -1041,18 +1066,44 @@ static int build(cudaStream_t stream, const PackedVec3* hPos, uint64_t vertexCou
     tm.mark("sah");
     BB_CK(cudaGetLastError());
     BB_CK(cudaStreamSynchronize(stream));
-
-    out.nodes.resize(f);
-    out.tris.resize(triOut);
-    BB_CK(cudaMemcpyAsync(out.nodes.data(), final, (size_t)f * sizeof(GpuBlasNode), cudaMemcpyDeviceToHost, stream));
-    if (triOut) BB_CK(cudaMemcpyAsync(out.tris.data(), outTris, (size_t)triOut * sizeof(GpuBlasTriangle), cudaMemcpyDeviceToHost, stream));
-    BB_CK(cudaMemcpyAsync(&out.sah, acc + 2, sizeof(double), cudaMemcpyDeviceToHost, stream));
-    tm.mark("download");
-    BB_CK(cudaStreamSynchronize(stream));
+    out.nodes = final;
+    out.nodeCount = f;
+    out.tris = outTris;
+    out.triCount = triOut;
     out.requiredStackSize = requiredStackSize;
     out.fragmentCount = n;
+    out.sah = acc + 2;
+    return BB_OK;
+}
+
+// idkpt_blas_build: build_device between an upload of the host arrays and a download of its result. Fills `out` and the
+// total device time.
+static int build(cudaStream_t stream, const PackedVec3* hPos, uint64_t vertexCount, const GpuBlasTriangle* hTris, int triCount,
+                 const Params& p, IdkPtBlasBuild& out, float& totalMs, std::string& err) {
+    Arena ar;
+    StageTimer tm(stream);
+    tm.mark("start");
+    PackedVec3* pos;
+    GpuBlasTriangle* tris;
+    BB_CK(ar.get(pos, vertexCount));
+    BB_CK(ar.get(tris, triCount));
+    BB_CK(cudaMemcpyAsync(pos, hPos, vertexCount * sizeof(PackedVec3), cudaMemcpyHostToDevice, stream));
+    BB_CK(cudaMemcpyAsync(tris, hTris, (size_t)triCount * sizeof(GpuBlasTriangle), cudaMemcpyHostToDevice, stream));
+    tm.mark("upload");
+    DeviceResult r;
+    if (int rc = build_device(stream, pos, tris, triCount, p, ar, r, tm, err)) return rc;
+
+    out.nodes.resize(r.nodeCount);
+    out.tris.resize(r.triCount);
+    BB_CK(cudaMemcpyAsync(out.nodes.data(), r.nodes, (size_t)r.nodeCount * sizeof(GpuBlasNode), cudaMemcpyDeviceToHost, stream));
+    if (r.triCount) BB_CK(cudaMemcpyAsync(out.tris.data(), r.tris, (size_t)r.triCount * sizeof(GpuBlasTriangle), cudaMemcpyDeviceToHost, stream));
+    BB_CK(cudaMemcpyAsync(&out.sah, r.sah, sizeof(double), cudaMemcpyDeviceToHost, stream));
+    tm.mark("download");
+    BB_CK(cudaStreamSynchronize(stream));
+    out.requiredStackSize = r.requiredStackSize;
+    out.fragmentCount = r.fragmentCount;
     totalMs = tm.total();
-    tm.print(n);
+    tm.print(r.fragmentCount);
     return BB_OK;
 }
 

@@ -151,6 +151,7 @@ struct IdkPtCtx : IdkCtxBase {
 
     // dynamic geometry: unskinned vertices, joint matrices, refit scratch (parents + locks of the largest BLAS)
     DevBuf unskinned, joints, refitParents, refitLocks, tlasScratch;
+    DevBuf sahScratch;             // idkpt_blas_sah: the walk's stack and the per-BLAS results
     uint64_t unskinnedCount = 0;
     std::vector<uint32_t> unskinnedMaxJoint;   // per vertex max(JointIndices), host copy for range validation
     std::vector<GpuBlasDesc> hostDescs;
@@ -161,7 +162,8 @@ struct IdkPtCtx : IdkCtxBase {
     DevBuf prevPositions;
 
     // voxelisers reading this scene (idkvx_set_scene_from); idkpt_destroy unbinds them. sceneGeneration counts idkpt_set_scene
-    // calls, so that a bound voxeliser knows when the instance list, and with it its work-queue size, may have changed.
+    // and idkpt_blas_rebuild calls, so that a bound voxeliser knows when the instance list or the BLAS triangle counts, and
+    // with them its work-queue size, may have changed.
     std::vector<IdkVxCtx*> boundVoxelizers;
     uint64_t sceneGeneration = 0;
 
@@ -620,6 +622,46 @@ static int keep_prev_positions(IdkPtCtx* ctx) {
     return IDKPT_OK;
 }
 
+// Keep the BVH resident in the 50 MB L2: persisting access-policy window over [nodes | triRec] (bvhBytes from `base`) on the
+// render stream and every lane stream. The wavefront buffers (hundreds of MB per frame) stream through the rest of the cache
+// without evicting the tree.
+static int set_l2_window(IdkPtCtx* ctx, void* base, size_t bvhBytes) {
+    cudaDeviceProp prop;
+    CK(cudaGetDeviceProperties(&prop, ctx->device));
+    cudaStreamAttrValue& attr = ctx->l2Window;
+    memset(&attr, 0, sizeof(attr));
+    if (prop.persistingL2CacheMaxSize > 0 && prop.accessPolicyMaxWindowSize > 0) {
+        const size_t setAside = std::min<size_t>((size_t)prop.persistingL2CacheMaxSize, std::max<size_t>(bvhBytes, 1 << 20));
+        CK(cudaDeviceSetLimit(cudaLimitPersistingL2CacheSize, setAside));
+        const size_t window = std::min<size_t>(bvhBytes, (size_t)prop.accessPolicyMaxWindowSize);
+        attr.accessPolicyWindow.base_ptr = base;
+        attr.accessPolicyWindow.num_bytes = window;
+        attr.accessPolicyWindow.hitRatio = window <= setAside ? 1.0f : (float)((double)setAside / (double)window);
+        attr.accessPolicyWindow.hitProp = cudaAccessPropertyPersisting;
+        attr.accessPolicyWindow.missProp = cudaAccessPropertyNormal;
+    } else {
+        attr.accessPolicyWindow.num_bytes = 0;
+    }
+    CK(cudaStreamSetAttribute(ctx->stream, cudaStreamAttributeAccessPolicyWindow, &attr));
+    for (int i = 0; i < IDK_MAX_LANES; i++)    // the asynchronous path launches traverse / shade on the lane streams
+        if (ctx->lanes[i].stream) CK(cudaStreamSetAttribute(ctx->lanes[i].stream, cudaStreamAttributeAccessPolicyWindow, &attr));
+    return IDKPT_OK;
+}
+
+// IdkPtBlasBuildSettings (NULL: the engine's defaults) as the builder's parameters. Rejects non-finite values and
+// StopSplittingThreshold < 1 (a node of 0 fragments would read as an interior node, GpuBlasNode.TriCount == 0).
+static int blas_build_params(IdkPtCtx* ctx, const char* who, const IdkPtBlasBuildSettings* settings, idkbvh::Params& p) {
+    const idkbvh::Params d;
+    const IdkPtBlasBuildSettings s = settings ? *settings : IdkPtBlasBuildSettings{d.stopSplittingThreshold, d.maxLeafTriangleCount,
+        d.triangleCost, d.stackOptThreshold, d.stackOptSahIncreaseAcceptance, d.splitFactor, d.doPreSplit};
+    if (!std::isfinite(s.TriangleCost) || !std::isfinite(s.StackOptSahIncreaseAcceptance) || !std::isfinite(s.SplitFactor))
+        return fail(ctx, who, IDKPT_ERR_INVALID_ARGUMENT, "non-finite setting");
+    if (s.StopSplittingThreshold < 1) return fail(ctx, who, IDKPT_ERR_INVALID_ARGUMENT, "StopSplittingThreshold must be at least 1");
+    p = {s.StopSplittingThreshold, s.MaxLeafTriangleCount, s.TriangleCost, s.StackOptThreshold, s.StackOptSahIncreaseAcceptance,
+         s.SplitFactor, s.DoPreSplit ? 1 : 0};
+    return IDKPT_OK;
+}
+
 // idkvx_impl.cuh: forgets this context in every voxeliser bound to it (idkvx_set_scene_from), before it goes away.
 static void unbind_voxelizers(IdkPtCtx* ctx);
 
@@ -693,7 +735,7 @@ IDKPT_API void idkpt_destroy(IdkPtCtx* ctx) {
                      &ctx->images[0], &ctx->images[1], &ctx->images[2], &ctx->counters, &ctx->countLog, &ctx->skyFaces,
                      &ctx->tex.pixels, &ctx->tex.recs, &ctx->tex.srgbLut, &ctx->bloomDown, &ctx->bloomUp, &ctx->postConsts, &ctx->ldr,
                      &ctx->unskinned, &ctx->joints, &ctx->refitParents, &ctx->refitLocks, &ctx->scratch[0], &ctx->scratch[1], &ctx->scratch[2],
-                     &ctx->tlasScratch, &ctx->oidn[0], &ctx->oidn[1], &ctx->oidn[2], &ctx->oidn[3], &ctx->denoiseWork[0], &ctx->denoiseWork[1], &ctx->denoised,
+                     &ctx->tlasScratch, &ctx->sahScratch, &ctx->oidn[0], &ctx->oidn[1], &ctx->oidn[2], &ctx->oidn[3], &ctx->denoiseWork[0], &ctx->denoiseWork[1], &ctx->denoised,
                      &ctx->pointShadowDev, &ctx->pointShadowMaps, &ctx->pointShadowLights, &ctx->prevPositions};
     for (DevBuf* b : all) release(*b);
     release_raster(ctx->raster);
@@ -811,30 +853,7 @@ IDKPT_API int idkpt_set_scene(IdkPtCtx* ctx, const IdkPtSceneDesc* s) {
     ctx->hostInstances.assign(s->BlasInstances, s->BlasInstances + s->BlasInstanceCount);
     ctx->nodeBytes = nodeBytes;
     if ((rc = configure_launches(ctx))) return rc;
-    // Keep the BVH resident in the 50 MB L2: persisting access-policy window over [nodes | triRec] on the render stream.
-    // The wavefront buffers (hundreds of MB per frame) stream through the rest of the cache without evicting the tree.
-    {
-        cudaDeviceProp prop;
-        CK(cudaGetDeviceProperties(&prop, ctx->device));
-        cudaStreamAttrValue& attr = ctx->l2Window;
-        memset(&attr, 0, sizeof(attr));
-        if (prop.persistingL2CacheMaxSize > 0 && prop.accessPolicyMaxWindowSize > 0) {
-            const size_t bvhBytes = nodeBytes + triRecBytes;
-            const size_t setAside = std::min<size_t>((size_t)prop.persistingL2CacheMaxSize, std::max<size_t>(bvhBytes, 1 << 20));
-            CK(cudaDeviceSetLimit(cudaLimitPersistingL2CacheSize, setAside));
-            const size_t window = std::min<size_t>(bvhBytes, (size_t)prop.accessPolicyMaxWindowSize);
-            attr.accessPolicyWindow.base_ptr = ctx->nodes.p;
-            attr.accessPolicyWindow.num_bytes = window;
-            attr.accessPolicyWindow.hitRatio = window <= setAside ? 1.0f : (float)((double)setAside / (double)window);
-            attr.accessPolicyWindow.hitProp = cudaAccessPropertyPersisting;
-            attr.accessPolicyWindow.missProp = cudaAccessPropertyNormal;
-        } else {
-            attr.accessPolicyWindow.num_bytes = 0;
-        }
-        CK(cudaStreamSetAttribute(ctx->stream, cudaStreamAttributeAccessPolicyWindow, &attr));
-        for (int i = 0; i < IDK_MAX_LANES; i++)    // the asynchronous path launches traverse / shade on the lane streams
-            if (ctx->lanes[i].stream) CK(cudaStreamSetAttribute(ctx->lanes[i].stream, cudaStreamAttributeAccessPolicyWindow, &attr));
-    }
+    if ((rc = set_l2_window(ctx, ctx->nodes.p, nodeBytes + triRecBytes))) return rc;
     CK(cudaStreamSynchronize(ctx->stream));
     ctx->haveScene = true;
     ctx->accumulatedSamples = 0;
@@ -1994,13 +2013,8 @@ IDKPT_API int idkpt_blas_build(IdkPtCtx* ctx, const PackedVec3* positions, uint6
     if (kernelMs) *kernelMs = 0.0f;
     if (!positions || !triangles || !out) return fail(ctx, IDKPT_ERR_INVALID_ARGUMENT, "idkpt_blas_build: null argument");
     if (triangleCount == 0) return fail(ctx, IDKPT_ERR_INVALID_ARGUMENT, "idkpt_blas_build: no triangles");
-    const idkbvh::Params d;
-    const IdkPtBlasBuildSettings s = settings ? *settings : IdkPtBlasBuildSettings{d.stopSplittingThreshold, d.maxLeafTriangleCount,
-        d.triangleCost, d.stackOptThreshold, d.stackOptSahIncreaseAcceptance, d.splitFactor, d.doPreSplit};
-    if (!std::isfinite(s.TriangleCost) || !std::isfinite(s.StackOptSahIncreaseAcceptance) || !std::isfinite(s.SplitFactor))
-        return fail(ctx, IDKPT_ERR_INVALID_ARGUMENT, "idkpt_blas_build: non-finite setting");
-    if (s.StopSplittingThreshold < 1)   // a node of 0 fragments would read as an interior node (GpuBlasNode.TriCount == 0)
-        return fail(ctx, IDKPT_ERR_INVALID_ARGUMENT, "idkpt_blas_build: StopSplittingThreshold must be at least 1");
+    idkbvh::Params p;
+    if (int rc = blas_build_params(ctx, "idkpt_blas_build", settings, p)) return rc;
     if (triangleCount > (uint64_t)idkbb::MAX_FRAGMENTS)
         return fail(ctx, IDKPT_ERR_UNSUPPORTED, "idkpt_blas_build: more than 2^24 triangles");
     for (uint64_t i = 0; i < triangleCount; i++) {
@@ -2010,8 +2024,6 @@ IDKPT_API int idkpt_blas_build(IdkPtCtx* ctx, const PackedVec3* positions, uint6
     }
     DRAIN_PENDING("idkpt_blas_build");
     CK(cudaSetDevice(ctx->device));
-    const idkbvh::Params p = {s.StopSplittingThreshold, s.MaxLeafTriangleCount, s.TriangleCost, s.StackOptThreshold,
-                             s.StackOptSahIncreaseAcceptance, s.SplitFactor, s.DoPreSplit ? 1 : 0};
     IdkPtBlasBuild* b = new IdkPtBlasBuild();
     std::string err;
     float ms = 0.0f;
@@ -2046,6 +2058,163 @@ IDKPT_API int idkpt_blas_build_copy(const IdkPtBlasBuild* b, GpuBlasNode* nodes,
 
 IDKPT_API void idkpt_blas_build_free(IdkPtBlasBuild* b) { delete b; }
 
+static int64_t nodes_end(const GpuBlasDesc& d) { return (int64_t)d.NodeOffset + d.NodeCount; }
+static int64_t triangles_end(const GpuBlasDesc& d) { return (int64_t)d.TriangleOffset + d.TriangleCount; }
+
+// BVH.BlasesBuild(first, count) (BVH.cs:300-470) on the scene in place: each BLAS of the range is built by idkbb::build_device
+// from its current triangle records and the device positions, into staging memory. When every build succeeded, the new nodes
+// and triangles replace the old ones in new allocations: the data before the range (up to the end of desc first - 1) and the
+// data after it move unchanged, and the descs from `first` on are repacked behind each other (BVH.cs:378-441).
+IDKPT_API int idkpt_blas_rebuild(IdkPtCtx* ctx, uint32_t first, uint32_t count, const IdkPtBlasBuildSettings* settings, float* kernelMs) {
+    if (!ctx) return IDKPT_ERR_INVALID_ARGUMENT;
+    if (kernelMs) *kernelMs = 0.0f;
+    DRAIN_PENDING("idkpt_blas_rebuild");
+    if (!ctx->haveScene) return fail(ctx, IDKPT_ERR_NO_SCENE, "idkpt_blas_rebuild: no scene");
+    const std::vector<GpuBlasDesc>& old = ctx->hostDescs;
+    const size_t nd = old.size();
+    if ((uint64_t)first + count > nd) return fail(ctx, IDKPT_ERR_INVALID_ARGUMENT, "idkpt_blas_rebuild: BLAS range outside BlasDescs");
+    idkbvh::Params p;
+    if (int rc = blas_build_params(ctx, "idkpt_blas_rebuild", settings, p)) return rc;
+    if (count == 0) return IDKPT_OK;   // BVH.cs:302
+    // The layout BlasesBuild and host.Scene.add produce: from `first` on, each BLAS starts where the previous one ends, and the
+    // last one ends the arrays. The BLASes before the range keep their data, so none may reach past the end of desc first - 1.
+    const int64_t keepNodes = first ? nodes_end(old[first - 1]) : 0, keepTris = first ? triangles_end(old[first - 1]) : 0;
+    for (size_t i = 0; i < nd; i++) {
+        const bool ok = i < first ? nodes_end(old[i]) <= keepNodes && triangles_end(old[i]) <= keepTris
+                                  : i == first || (old[i].NodeOffset == nodes_end(old[i - 1]) && old[i].TriangleOffset == triangles_end(old[i - 1]));
+        if (!ok) return fail(ctx, IDKPT_ERR_INVALID_ARGUMENT, "idkpt_blas_rebuild: the BLASes are not packed behind each other from the first one rebuilt");
+    }
+    if (nodes_end(old[nd - 1]) != (int64_t)ctx->counts.BlasNodeCount || triangles_end(old[nd - 1]) != (int64_t)ctx->counts.BlasTriangleCount)
+        return fail(ctx, IDKPT_ERR_INVALID_ARGUMENT, "idkpt_blas_rebuild: the last BLAS does not end the node and triangle arrays");
+    for (uint32_t b = first; b < first + count; b++)
+        if (old[b].TriangleCount > idkbb::MAX_FRAGMENTS) return fail(ctx, IDKPT_ERR_UNSUPPORTED, "idkpt_blas_rebuild: a BLAS of more than 2^24 triangles");
+    CK(cudaSetDevice(ctx->device));
+
+    std::vector<GpuBlasDesc> descs = old;
+    idkbb::Arena staged;                                  // the rebuilt BLASes, until they are committed
+    std::vector<idkbb::DeviceResult> built(count);
+    DevBuf bvh, tris, descBuf;                            // the new [nodes | triRec], triangles and descs
+    struct Drop { DevBuf* b[3]; ~Drop() { for (DevBuf* x : b) release(*x); } } drop = {{&bvh, &tris, &descBuf}};
+    size_t nodeBytes = 0, triRecBytes = 0;
+    int stackSize = 0;
+    int rc = run_timed(ctx, "idkpt_blas_rebuild", kernelMs, [&]() -> int {
+        for (uint32_t k = 0; k < count; k++) {
+            GpuBlasDesc& d = descs[first + k];
+            idkbvh::Params bp = p;
+            bp.doPreSplit = d.IsRefittable ? 0 : 1;        // BVH.cs:325
+            idkbb::StageTimer tm(ctx->stream);
+            tm.mark("start");
+            std::string err;
+            const int brc = idkbb::build_device(ctx->stream, (const PackedVec3*)ctx->positions.p, (const GpuBlasTriangle*)ctx->blasTris.p + d.TriangleOffset,
+                                                d.TriangleCount, bp, staged, built[k], tm, err);
+            if (brc != idkbb::BB_OK) {
+                if (brc == idkbb::BB_CUDA) cudaStreamSynchronize(ctx->stream);
+                return fail(ctx, "idkpt_blas_rebuild", brc == idkbb::BB_TOO_MANY_FRAGMENTS ? IDKPT_ERR_UNSUPPORTED : IDKPT_ERR_CUDA, err.c_str());
+            }
+            tm.print(built[k].fragmentCount);
+            d.NodeCount = built[k].nodeCount;
+            d.TriangleCount = built[k].triCount;
+            d.RequiredStackSize = built[k].requiredStackSize;
+        }
+        int64_t nodeEnd = 0, triEnd = 0;
+        for (size_t i = first; i < nd; i++) {
+            const int64_t no = i ? nodes_end(descs[i - 1]) : 0, to = i ? triangles_end(descs[i - 1]) : 0;
+            nodeEnd = no + descs[i].NodeCount;
+            triEnd = to + descs[i].TriangleCount;
+            if (nodeEnd >= (1ll << 31) || triEnd >= (1ll << 31)) return fail(ctx, IDKPT_ERR_INVALID_ARGUMENT, "idkpt_blas_rebuild: scene too large");
+            descs[i].NodeOffset = (int32_t)no;
+            descs[i].TriangleOffset = (int32_t)to;
+        }
+        for (const GpuBlasDesc& d : descs) stackSize = std::max(stackSize, d.RequiredStackSize);   // BVH.UpdateBlasStackSize
+        if ((size_t)std::max(1, stackSize) * IDK_BLOCK * sizeof(uint32_t) > 200 * 1024)
+            return fail(ctx, IDKPT_ERR_UNSUPPORTED, "idkpt_blas_rebuild: BlasStackSize too large for the shared-memory traversal stack");
+
+        // the new arrays: the kept prefix, the rebuilt BLASes, the moved tail
+        const GpuBlasDesc &r0 = descs[first], &rl = descs[first + count - 1];
+        const int64_t oldEndN = nodes_end(old[first + count - 1]), oldEndT = triangles_end(old[first + count - 1]);
+        const int64_t tailN = (int64_t)ctx->counts.BlasNodeCount - oldEndN, tailT = (int64_t)ctx->counts.BlasTriangleCount - oldEndT;
+        nodeBytes = (((size_t)nodeEnd * sizeof(GpuBlasNode)) + 255) & ~(size_t)255;
+        triRecBytes = std::max<size_t>((size_t)triEnd, 1) * 64;
+        if (ensure(bvh, nodeBytes + triRecBytes) != cudaSuccess || ensure(tris, std::max<size_t>((size_t)triEnd * sizeof(GpuBlasTriangle), 16)) != cudaSuccess ||
+            ensure(descBuf, std::max<size_t>(nd * sizeof(GpuBlasDesc), 16)) != cudaSuccess)
+            return fail(ctx, IDKPT_ERR_OUT_OF_MEMORY, "idkpt_blas_rebuild: device allocation failed");
+        GpuBlasNode* nodesNew = (GpuBlasNode*)bvh.p;
+        const GpuBlasNode* nodesOld = (const GpuBlasNode*)ctx->nodes.p;
+        float4* recNew = (float4*)((char*)bvh.p + nodeBytes);
+        const float4* recOld = (const float4*)((const char*)ctx->nodes.p + ctx->nodeBytes);
+        GpuBlasTriangle* trisNew = (GpuBlasTriangle*)tris.p;
+        const GpuBlasTriangle* trisOld = (const GpuBlasTriangle*)ctx->blasTris.p;
+        auto d2d = [&](void* dst, const void* src, size_t bytes) { return bytes ? cudaMemcpyAsync(dst, src, bytes, cudaMemcpyDeviceToDevice, ctx->stream) : cudaSuccess; };
+        CK(d2d(nodesNew, nodesOld, (size_t)keepNodes * sizeof(GpuBlasNode)));
+        CK(d2d(trisNew, trisOld, (size_t)keepTris * sizeof(GpuBlasTriangle)));
+        CK(d2d(recNew, recOld, (size_t)keepTris * 64));
+        for (uint32_t k = 0; k < count; k++) {
+            const GpuBlasDesc& d = descs[first + k];
+            CK(d2d(nodesNew + d.NodeOffset, built[k].nodes, (size_t)d.NodeCount * sizeof(GpuBlasNode)));
+            CK(d2d(trisNew + d.TriangleOffset, built[k].tris, (size_t)d.TriangleCount * sizeof(GpuBlasTriangle)));
+        }
+        CK(d2d(nodesNew + nodes_end(rl), nodesOld + oldEndN, (size_t)tailN * sizeof(GpuBlasNode)));
+        CK(d2d(trisNew + triangles_end(rl), trisOld + oldEndT, (size_t)tailT * sizeof(GpuBlasTriangle)));
+        CK(d2d(recNew + 4 * triangles_end(rl), recOld + 4 * oldEndT, (size_t)tailT * 64));
+        if (const uint32_t n = (uint32_t)(triangles_end(rl) - r0.TriangleOffset))   // the rebuilt BLASes' triangle records
+            k_prepare_triangles<<<(n + 255) / 256, 256, 0, ctx->stream>>>((const int4*)(trisNew + r0.TriangleOffset), (const float*)ctx->positions.p,
+                                                                          recNew + 4 * (size_t)r0.TriangleOffset, n);
+        CK(cudaMemcpyAsync(descBuf.p, descs.data(), nd * sizeof(GpuBlasDesc), cudaMemcpyHostToDevice, ctx->stream));
+        return IDKPT_OK;
+    });
+    if (rc) return rc;
+
+    // commit: launch configuration and L2 window for the new arrays first (restored if either fails), then the swap
+    const int oldStack = ctx->sc.stackSize;
+    ctx->sc.stackSize = std::max(1, stackSize);
+    if ((rc = configure_launches(ctx)) || (rc = set_l2_window(ctx, bvh.p, nodeBytes + triRecBytes))) {
+        const std::string err = ctx->lastError;
+        ctx->sc.stackSize = oldStack;
+        configure_launches(ctx);
+        set_l2_window(ctx, ctx->nodes.p, ctx->nodeBytes + std::max<size_t>(ctx->counts.BlasTriangleCount, 1) * 64);
+        ctx->lastError = err;
+        return rc;
+    }
+    std::swap(ctx->nodes, bvh);
+    std::swap(ctx->blasTris, tris);
+    std::swap(ctx->descs, descBuf);                      // `drop` frees the old arrays
+    ctx->nodeBytes = nodeBytes;
+    ctx->sc.nodes = (const float4*)ctx->nodes.p;
+    ctx->sc.triRec = (const float4*)((char*)ctx->nodes.p + nodeBytes);
+    ctx->sc.blasTris = (const int4*)ctx->blasTris.p;
+    ctx->sc.descs = (const GpuBlasDesc*)ctx->descs.p;
+    ctx->counts.BlasNodeCount = (uint64_t)nodes_end(descs[nd - 1]);
+    ctx->counts.BlasTriangleCount = (uint64_t)triangles_end(descs[nd - 1]);
+    ctx->counts.BlasStackSize = stackSize;
+    ctx->hostDescs = std::move(descs);
+    ctx->sceneGeneration++;                              // a bound voxeliser re-sizes its work queue for the new triangle counts
+    ctx->accumulatedSamples = 0;
+    return IDKPT_OK;
+}
+
+// BLAS.ComputeGlobalSAH (BLAS.cs:629-656) of each BLAS in [first, first + count) as the device holds it now: k_global_sah.
+IDKPT_API int idkpt_blas_sah(IdkPtCtx* ctx, uint32_t first, uint32_t count, const IdkPtBlasBuildSettings* settings, double* sahOut) {
+    if (!ctx) return IDKPT_ERR_INVALID_ARGUMENT;
+    if (!sahOut && count) return fail(ctx, IDKPT_ERR_INVALID_ARGUMENT, "idkpt_blas_sah: null argument");
+    DRAIN_PENDING("idkpt_blas_sah");
+    if (!ctx->haveScene) return fail(ctx, IDKPT_ERR_NO_SCENE, "idkpt_blas_sah: no scene");
+    if ((uint64_t)first + count > ctx->hostDescs.size()) return fail(ctx, IDKPT_ERR_INVALID_ARGUMENT, "idkpt_blas_sah: BLAS range outside BlasDescs");
+    const float triangleCost = settings ? settings->TriangleCost : idkbvh::Params().triangleCost;
+    if (!std::isfinite(triangleCost)) return fail(ctx, IDKPT_ERR_INVALID_ARGUMENT, "idkpt_blas_sah: non-finite TriangleCost");
+    if (count == 0) return IDKPT_OK;
+    CK(cudaSetDevice(ctx->device));
+    int maxNodes = 0;
+    for (uint32_t b = first; b < first + count; b++) maxNodes = std::max(maxNodes, ctx->hostDescs[b].NodeCount);
+    CK(ensure(ctx->sahScratch, (size_t)count * sizeof(double) + (size_t)maxNodes * sizeof(int)));
+    double* out = (double*)ctx->sahScratch.p;
+    int* stack = (int*)(out + count);
+    return run_timed(ctx, "idkpt_blas_sah", nullptr, [&]() -> int {
+        for (uint32_t k = 0; k < count; k++)
+            idkbb::k_global_sah<<<1, 1, 0, ctx->stream>>>((const GpuBlasNode*)ctx->nodes.p + ctx->hostDescs[first + k].NodeOffset, stack, triangleCost, out + k);
+        return IDKPT_OK;
+    }, sahOut, out, (size_t)count * sizeof(double));
+}
+
 IDKPT_API int idkpt_read_range(IdkPtCtx* ctx, IdkPtArrayId which, uint64_t first, uint64_t count, void* out) {
     if (!ctx || (!out && count)) return fail(ctx, IDKPT_ERR_INVALID_ARGUMENT, "idkpt_read_range: null argument");
     if (!ctx->haveScene) return fail(ctx, IDKPT_ERR_NO_SCENE, "idkpt_read_range: no scene");
@@ -2057,6 +2226,8 @@ IDKPT_API int idkpt_read_range(IdkPtCtx* ctx, IdkPtArrayId which, uint64_t first
         case IDKPT_ARRAY_VERTEX_POSITIONS: b = &ctx->positions; elem = sizeof(PackedVec3); limit = ctx->counts.VertexPositionCount; break;
         case IDKPT_ARRAY_VERTICES: b = &ctx->vertices; elem = sizeof(GpuVertex); limit = ctx->counts.VertexCount; break;
         case IDKPT_ARRAY_TLAS_NODES: b = &ctx->tlas; elem = sizeof(GpuTlasNode); limit = ctx->counts.UseTlas ? ctx->counts.TlasNodeCount : 0; break;
+        case IDKPT_ARRAY_BLAS_TRIANGLES: b = &ctx->blasTris; elem = sizeof(GpuBlasTriangle); limit = ctx->counts.BlasTriangleCount; break;
+        case IDKPT_ARRAY_BLAS_DESCS: b = &ctx->descs; elem = sizeof(GpuBlasDesc); limit = ctx->counts.BlasDescCount; break;
         default: return fail(ctx, IDKPT_ERR_INVALID_ARGUMENT, "idkpt_read_range: array id not readable");
     }
     if (first > limit || count > limit - first) return fail(ctx, IDKPT_ERR_INVALID_ARGUMENT, "idkpt_read_range: range outside the array");

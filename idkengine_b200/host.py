@@ -70,6 +70,8 @@ def lib():
         L.idkhost_transform_box.argtypes = [ctypes.c_void_p] * 5
         L.idkhost_tlas_build.restype = None
         L.idkhost_tlas_build.argtypes = [ctypes.c_void_p, ctypes.c_int32, ctypes.c_void_p, ctypes.c_int32]
+        L.idkhost_blas_global_sah.restype = ctypes.c_double
+        L.idkhost_blas_global_sah.argtypes = [ctypes.c_void_p, ctypes.c_uint64, ctypes.c_float]
         L.idkhost_default_build_settings.restype = None
         L.idkhost_default_build_settings.argtypes = [ctypes.POINTER(IdkBlasBuildSettings)]
         _lib = L
@@ -103,6 +105,15 @@ def build_blas(positions, triangles, presplit=True, threads=None, settings=None)
                     sah=float(L.idkhost_blas_sah(h)))
     finally:
         L.idkhost_blas_free(h)
+
+
+def blas_global_sah(nodes, triangle_cost=None):
+    """BLAS.ComputeGlobalSAH (SRC/Bvh/BLAS.cs:629-656) of one BLAS's nodes (GpuBlasNode[N], node 1 the root): the pre-order
+    walk, left child first, summed in that order. triangle_cost: BuildSettings.TriangleCost (default 1.1)."""
+    nodes = np.ascontiguousarray(nodes)
+    assert nodes.dtype == gt.GpuBlasNode and len(nodes) >= 4
+    cost = default_build_settings().TriangleCost if triangle_cost is None else triangle_cost
+    return float(lib().idkhost_blas_global_sah(nodes.ctypes.data, len(nodes), cost))
 
 
 # --------------------------------------------------------------------------- on-disk BLAS cache (include/idkhost_cache.h)
@@ -333,6 +344,45 @@ class Scene:
                                         required_stack_size=b["required_stack_size"], sah=b["sah"], from_cache=bool(b.get("from_cache", False))))
         # BVH.UpdateBlasStackSize (BVH.cs:559-567)
         self.blas_stack_size = max(1, int(self.blas_descs["RequiredStackSize"].max())) if len(self.blas_descs) else 1
+        return self
+
+    def rebuild_blases(self, first, count, settings=None, threads=None, blas_builder=None):
+        """BVH.BlasesBuild(first, count) (SRC/Bvh/BVH.cs:300-470) over this Scene's arrays: each BLAS of the range is built again
+        from its current triangle records and positions, pre-split when it is not refittable (settings.DoPreSplit is ignored);
+        the descs from `first` on are repacked behind the previous desc's end, the data behind them moves along, and
+        blas_stack_size becomes the largest RequiredStackSize. The host mirror of idkpt_blas_rebuild.
+        blas_builder: build_blas's signature and result (default the host build with `threads`)."""
+        if count == 0:
+            return self
+        descs = self.blas_descs.copy()
+        built = []
+        for b in range(first, first + count):
+            d = descs[b]
+            tris = self.blas_triangles[d["TriangleOffset"]:d["TriangleOffset"] + d["TriangleCount"]]
+            presplit = not d["IsRefittable"]
+            if blas_builder is None:
+                r = build_blas(self.positions, tris, presplit=presplit, threads=threads, settings=settings)
+            else:
+                r = blas_builder(self.positions, tris, presplit=presplit, settings=settings)
+            d["NodeCount"], d["TriangleCount"], d["RequiredStackSize"] = len(r["nodes"]), len(r["triangles"]), r["required_stack_size"]
+            built.append(r)
+        old_end = self.blas_descs[first + count - 1]
+        old_nodes_end = int(old_end["NodeOffset"] + old_end["NodeCount"])
+        old_tris_end = int(old_end["TriangleOffset"] + old_end["TriangleCount"])
+        for i in range(first, len(descs)):     # BVH.cs:378-386
+            prev = descs[i - 1] if i > 0 else None
+            descs[i]["NodeOffset"] = int(prev["NodeOffset"] + prev["NodeCount"]) if prev is not None else 0
+            descs[i]["TriangleOffset"] = int(prev["TriangleOffset"] + prev["TriangleCount"]) if prev is not None else 0
+        start = descs[first]
+        self.blas_nodes = np.concatenate([self.blas_nodes[:start["NodeOffset"]]] + [r["nodes"] for r in built] +
+                                         [self.blas_nodes[old_nodes_end:]])
+        self.blas_triangles = np.concatenate([self.blas_triangles[:start["TriangleOffset"]]] + [r["triangles"] for r in built] +
+                                             [self.blas_triangles[old_tris_end:]])
+        self.blas_descs = descs
+        for k, r in enumerate(built):
+            self.build_info[first + k].update(fragments=r["fragment_count"], triangles=len(r["triangles"]), nodes=len(r["nodes"]),
+                        required_stack_size=r["required_stack_size"], sah=r["sah"], from_cache=False)
+        self.blas_stack_size = max(1, int(self.blas_descs["RequiredStackSize"].max()))   # BVH.UpdateBlasStackSize
         return self
 
     def build_tlas(self, use=True, search_radius=15):

@@ -660,6 +660,16 @@ void idkhost_blas_copy(const IdkBlasBuild* b, GpuBlasNode* nodes, GpuBlasTriangl
 }
 __attribute__((visibility("default"))) void idkhost_blas_free(IdkBlasBuild* b) { delete b; }
 
+// BLAS.ComputeGlobalSAH (BLAS.cs:629-656) of any BLAS's nodes (node 1 the root): built, refitted or read back from the device.
+__attribute__((visibility("default")))
+double idkhost_blas_global_sah(const GpuBlasNode* nodes, uint64_t nodeCount, float triangleCost) {
+    BuildResult blas;
+    blas.nodes.assign(nodes, nodes + nodeCount);
+    Settings s;
+    s.triangleCost = triangleCost;
+    return computeGlobalSAH(blas, s);
+}
+
 } // extern "C"
 
 // ---------------------------------------------------------------- TLAS (Bvh/TLAS.cs:28-141, serial PLOC)

@@ -81,7 +81,8 @@ class PathTracer:
         self._check(self._lib.idkpt_update_range(self._ctx, which, first, len(data), data.ctypes.data), "idkpt_update_range")
 
     _READ_DTYPES = {capi.IDKPT_ARRAY_TLAS_NODES: gt.GpuTlasNode, capi.IDKPT_ARRAY_BLAS_NODES: gt.GpuBlasNode,
-                    capi.IDKPT_ARRAY_VERTEX_POSITIONS: gt.PackedVec3, capi.IDKPT_ARRAY_VERTICES: gt.GpuVertex}
+                    capi.IDKPT_ARRAY_VERTEX_POSITIONS: gt.PackedVec3, capi.IDKPT_ARRAY_VERTICES: gt.GpuVertex,
+                    capi.IDKPT_ARRAY_BLAS_TRIANGLES: gt.GpuBlasTriangle, capi.IDKPT_ARRAY_BLAS_DESCS: gt.GpuBlasDesc}
 
     def ReadRange(self, which, first, count):
         out = np.zeros(count, self._READ_DTYPES[which])
@@ -148,6 +149,31 @@ class PathTracer:
         self._check(self._lib.idkpt_tlas_build(self._ctx, search_radius, ctypes.byref(ms)), "idkpt_tlas_build")
         return ms.value
 
+    @staticmethod
+    def _blas_settings(settings):
+        """An IdkPtBlasBuildSettings from None (the defaults), an IdkPtBlasBuildSettings or a host.IdkBlasBuildSettings."""
+        s = capi.default_blas_build_settings()
+        if settings is not None:
+            for name, _ in capi.IdkPtBlasBuildSettings._fields_:
+                setattr(s, name, getattr(settings, name))
+        return s
+
+    def RebuildBlases(self, first, count=1, settings=None):
+        """BVH.BlasesBuild(first, count) (BVH.cs:300-470) on the device scene in place, from its current positions
+        (idkpt_blas_rebuild); a BLAS is pre-split when it is not refittable. Call TlasBuild afterwards. Returns kernel ms."""
+        ms = ctypes.c_float()
+        self._check(self._lib.idkpt_blas_rebuild(self._ctx, first, count, ctypes.byref(self._blas_settings(settings)), ctypes.byref(ms)),
+                    "idkpt_blas_rebuild")
+        return ms.value
+
+    def BlasSah(self, first, count=1, settings=None):
+        """BLAS.ComputeGlobalSAH (BLAS.cs:629-656) of BLASes [first, first + count) as the device holds them now; float64 array.
+        Only settings.TriangleCost is read."""
+        out = np.zeros(count, np.float64)
+        self._check(self._lib.idkpt_blas_sah(self._ctx, first, count, ctypes.byref(self._blas_settings(settings)), out.ctypes.data),
+                    "idkpt_blas_sah")
+        return out
+
     def BuildBlas(self, positions, triangles, presplit=True, settings=None):
         """BLAS.Build + PreSplitting.PreSplit on the device (idkpt_blas_build), with host.build_blas's signature and result:
         dict(nodes, triangles, required_stack_size, fragment_count, sah), equal to the host build. settings: an
@@ -156,10 +182,7 @@ class PathTracer:
         positions = np.ascontiguousarray(positions)
         triangles = np.ascontiguousarray(triangles)
         assert positions.dtype == gt.PackedVec3 and triangles.dtype == gt.GpuBlasTriangle
-        s = capi.default_blas_build_settings()
-        if settings is not None:
-            for name, _ in capi.IdkPtBlasBuildSettings._fields_:
-                setattr(s, name, getattr(settings, name))
+        s = self._blas_settings(settings)
         s.DoPreSplit = 1 if presplit else 0
         h = ctypes.c_void_p()
         ms = ctypes.c_float()

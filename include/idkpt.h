@@ -125,7 +125,9 @@ typedef enum IdkPtArrayId {
     IDKPT_ARRAY_TLAS_NODES = 4,        /* update + read: BVH.TlasBuild re-upload (BVH.cs:278-283); needs a scene set with UseTlas */
     IDKPT_ARRAY_BLAS_NODES = 5,        /* read only (idkpt_read_range): refitted boxes for the host-side TLAS build */
     IDKPT_ARRAY_VERTEX_POSITIONS = 6,  /* read only: skinned positions (the download behind fenceCopiedSkinnedVerticesToHost, ModelManager.cs:282) */
-    IDKPT_ARRAY_VERTICES = 7           /* read only: skinned normals / tangents */
+    IDKPT_ARRAY_VERTICES = 7,          /* read only: skinned normals / tangents */
+    IDKPT_ARRAY_BLAS_TRIANGLES = 8,    /* read only: GpuBlasTriangle records (the CPU copy for BVH.Intersect after idkpt_blas_rebuild) */
+    IDKPT_ARRAY_BLAS_DESCS = 9         /* read only: GpuBlasDesc records; the last one's ends are the node and triangle totals */
 } IdkPtArrayId;
 
 /* Replaces SkyBoxManager's bindless samplerCube in UBO 5 (SkyBoxManager.cs:87):
@@ -594,7 +596,8 @@ IDKPT_API int idkpt_lights_and_skybox(IdkPtCtx* ctx, const GpuPerFrameData* fram
  *   left. Every argument is checked first: a rejected call changes neither. kernel_ms covers the copies and the kernels.
  * idkpt_blas_refit: BVH.GpuBlasesRefit(first, count) (BVH.cs:472-489, BLASRefit/compute.glsl); also refreshes the derived
  *   triangle records of the refitted BLASes. Call it for every BLAS whose vertices moved.
- * idkpt_read_range: device -> host read-back (refitted BLAS nodes for the host TLAS build, skinned vertices).
+ * idkpt_read_range: device -> host read-back (refitted BLAS nodes for the host TLAS build, skinned vertices, and after
+ *   idkpt_blas_rebuild the BLAS nodes, triangles and descs for the host's CPU copy).
  * All of them reset the accumulation like any other scene edit. */
 typedef struct IdkPtSkinningCmd {     /* ModelManager.SkinningCmd, Skinning/compute.glsl:9-12 uniforms */
     uint32_t InputVertexOffset;
@@ -639,6 +642,34 @@ IDKPT_API int  idkpt_blas_build_info(const IdkPtBlasBuild* b, uint64_t* node_cou
 /* nodes: node_count GpuBlasNode (node 0 the pad, node 1 the root); triangles: triangle_count GpuBlasTriangle */
 IDKPT_API int  idkpt_blas_build_copy(const IdkPtBlasBuild* b, GpuBlasNode* nodes, GpuBlasTriangle* triangles);
 IDKPT_API void idkpt_blas_build_free(IdkPtBlasBuild* b);
+
+/* BVH.BlasesBuild(first, count) (BVH.cs:300-470) on the scene in place: rebuilds BLASes [first, first + count) from the scene's
+ * current device arrays -- each BLAS's triangle records BlasTriangles[TriangleOffset, +TriangleCount) and the device vertex
+ * positions, including whatever idkpt_skin_vertices last wrote -- with the same builder as idkpt_blas_build. Nothing is uploaded.
+ * A BLAS is pre-split exactly when !IsRefittable (BVH.cs:325); the settings' DoPreSplit is ignored, the other fields mean what
+ * they mean for idkpt_blas_build. A pre-split BLAS is pre-split again from its current, already duplicated triangle list, as
+ * the engine does, so its triangle count can grow with every rebuild.
+ * The new nodes and triangles replace the old ones: NodeOffset and TriangleOffset of every desc from `first` to the end become
+ * the previous desc's end and the data behind them moves along; the rebuilt descs get the new NodeCount, TriangleCount and
+ * RequiredStackSize, and keep IsRefittable and the LeafIndices / ParentIndices fields the host handed over. BlasStackSize
+ * becomes the largest RequiredStackSize (BVH.UpdateBlasStackSize). Everything else -- instances, transforms, meshes,
+ * materials, textures, lights, sky, point-shadow maps, kept previous positions, raster images, TAA history -- stays. The TLAS
+ * is not rebuilt, as after idkpt_blas_refit: call idkpt_tlas_build (or upload TLAS nodes) next. Resets the accumulation.
+ * All or nothing: every BLAS is built into staging memory and committed only when all builds succeeded; a failed call leaves
+ * every scene array, desc, the stack size and the image as they were. Synchronous, ordered after queued idkpt_compute samples.
+ * IDKPT_ERR_INVALID_ARGUMENT: a NULL context, first + count past the descs, a non-finite setting, StopSplittingThreshold < 1,
+ * or a layout other than the one BlasesBuild and host.Scene.add produce (from `first` on each desc's nodes and triangles
+ * start where the previous desc's end and the last desc ends both arrays; the descs before `first` end at or before the end
+ * of desc first - 1). IDKPT_ERR_UNSUPPORTED: more than 2^24 fragments in one build, or a new BlasStackSize beyond the
+ * shared-memory traversal stack (the limit idkpt_set_scene applies). count == 0 does nothing. kernel_ms (may be NULL): device
+ * time of the builds and the commit's copies. */
+IDKPT_API int idkpt_blas_rebuild(IdkPtCtx* ctx, uint32_t first, uint32_t count, const IdkPtBlasBuildSettings* settings /* NULL = defaults */,
+                                 float* kernel_ms);
+/* BLAS.ComputeGlobalSAH (BLAS.cs:629-656) of BLASes [first, first + count) as the device holds them now (built, refitted or
+ * rebuilt): the engine's pre-order walk, left child first, with the double sum in that order. Equals the build's sah for a
+ * BLAS the builder just produced. Only settings->TriangleCost is read (NULL = 1.1). sah_out: count doubles. A host refits most
+ * frames and rebuilds (idkpt_blas_rebuild) when the SAH has drifted far enough from the built one. */
+IDKPT_API int idkpt_blas_sah(IdkPtCtx* ctx, uint32_t first, uint32_t count, const IdkPtBlasBuildSettings* settings, double* sah_out);
 
 /* ---- present chain (SURVEY.md 8f.3): Bloom.Compute(Result) + TonemapAndGamma.Compute(Result, Bloom.Result)
  * (Application.cs:217-223) -> the RGBA8 frame the reference copies to the swapchain, produced on the device. ---- */

@@ -368,6 +368,18 @@ public:
         check(idkpt_skin_vertices(ctx_, jointMatrices3x4, jointCount, cmds, cmdCount, nullptr), "idkpt_skin_vertices");
     }
     void BlasRefit(uint32_t firstBlas, uint32_t count = 1) { check(idkpt_blas_refit(ctx_, firstBlas, count, nullptr), "idkpt_blas_refit"); }
+    // BVH.BlasesBuild(first, count) on the scene in place, from the current device positions; returns the device ms
+    float RebuildBlases(uint32_t firstBlas, uint32_t count = 1, const IdkPtBlasBuildSettings* settings = nullptr) {
+        float ms = 0.0f;
+        check(idkpt_blas_rebuild(ctx_, firstBlas, count, settings, &ms), "idkpt_blas_rebuild");
+        return ms;
+    }
+    // BLAS.ComputeGlobalSAH of each BLAS in [first, first + count) as the device holds it now
+    std::vector<double> BlasSah(uint32_t firstBlas, uint32_t count = 1, const IdkPtBlasBuildSettings* settings = nullptr) const {
+        std::vector<double> sah(count);
+        check(idkpt_blas_sah(ctx_, firstBlas, count, settings, sah.data()), "idkpt_blas_sah");
+        return sah;
+    }
     void ReadRange(IdkPtArrayId which, uint64_t first, uint64_t count, void* out) const { check(idkpt_read_range(ctx_, which, first, count, out), "idkpt_read_range"); }
 
     IdkPtCtx* Handle() const { return ctx_; }
