@@ -115,6 +115,7 @@ EXPORTS = [
     "idkpt_gbuffer", "idkpt_gbuffer_device_ptrs", "idkpt_read_gbuffer", "idkpt_prev_positions_device_ptr", "idkpt_transparency", "idkpt_lights_and_skybox",
     "idkpt_sky_atmosphere", "idkpt_sky_equirectangular", "idkpt_read_sky",
     "idkpt_blas_build", "idkpt_blas_build_info", "idkpt_blas_build_copy", "idkpt_blas_build_free", "idkpt_blas_rebuild", "idkpt_blas_sah",
+    "idkpt_blas_build_batch", "idkpt_blas_build_batch_copy",
 ]
 
 IDKPT_MAX_POINT_SHADOWS = 128
@@ -434,6 +435,10 @@ def load(path=None):
     L.idkpt_blas_build_copy.argtypes = [c_vp, c_vp, c_vp]
     L.idkpt_blas_build_free.restype = None
     L.idkpt_blas_build_free.argtypes = [c_vp]
+    L.idkpt_blas_build_batch.restype = c_i32
+    L.idkpt_blas_build_batch.argtypes = [c_vp, c_vp, c_u64, c_vp, c_u64, c_vp, c_u32, P(IdkPtBlasBuildSettings), P(c_vp), P(c_f)]
+    L.idkpt_blas_build_batch_copy.restype = c_i32
+    L.idkpt_blas_build_batch_copy.argtypes = [c_vp, c_vp, c_vp, c_vp, c_vp, c_vp]
     L.idkpt_blas_rebuild.restype = c_i32
     L.idkpt_blas_rebuild.argtypes = [c_vp, c_u32, c_u32, P(IdkPtBlasBuildSettings), P(c_f)]
     L.idkpt_blas_sah.restype = c_i32

@@ -2,15 +2,18 @@
 // node for node equal to the host mirror (host_mirror/bvh_build.cpp) under libidkpt's flags (-fmad=false, IEEE div and
 // sqrt; fmaf only in HalfArea, where the mirror uses it). DESIGN §8f.5 gives the stages and why each one is exact.
 //
+// The driver builds a batch of BLASes at once (idkpt_blas_build is a batch of one): each BLAS owns its own ranges of
+// fragment positions and node ids, and every stage runs over the whole batch; each BLAS comes out as it would alone.
+//
 // Stages (the mirror's function in brackets):
 //   1. pre-split [preSplit]: priorities per triangle; their float sum in triangle order by one thread; split counts and
 //      their exclusive scan; each triangle splits into its own output range, using the range's tail as its stack.
-//   2. sorts [radixSortFragments]: three stable sorts of fragment ids by floatToKey(min + max) (CUB radix sort).
+//   2. sorts [radixSortFragments]: three stable sorts of fragment ids by (BLAS, floatToKey(min + max)) (CUB radix sort).
 //   3. tree [processSubtree, trySplit]: level by level, one block per node above SMALL_NODE fragments (full prefix and
 //      suffix box scans, first strict minimum of L[i] + R[i+1]), then one thread per remaining subtree (the mirror's serial
 //      trySplit). Node ids do not depend on the order nodes are split in.
 //   4. post passes [computeRequiredStackSize, optimizeStackSize, removeEmptySubtrees, unindex*, computeGlobalSAH]: parallel
-//      except for the double sums, which one thread adds in the mirror's DFS order.
+//      except for the double sums, which one thread per BLAS adds in the mirror's DFS order.
 //
 // The scalar arithmetic comes from idk_bvh_math.h, which the mirror compiles too: boxes, Triangle.Split, the priority, the
 // split count, one pre-split step, the serial trySplit (stage 3's one-thread subtrees), the leaf-cost test and side swap that
@@ -47,6 +50,48 @@ __device__ __forceinline__ void storeBox(Box* b, size_t i, const Box& v) {
     p[0] = make_float2(v.mn[0], v.mn[1]); p[1] = make_float2(v.mn[2], v.mx[0]); p[2] = make_float2(v.mx[1], v.mx[2]);
 }
 
+// ---------------------------------------------------------------------------------------------------------------- batch
+// A batch of B BLASes shares one set of arrays. BLAS s owns the concatenated input triangles [tri[s], tri[s + 1]) (its range
+// of the caller's array starts at in[s]), the fragment positions [frag[s], frag[s + 1]), the node ids [node[s], node[s + 1])
+// with its root at node[s] + 1, the pre-order positions [order[s], order[s + 1]) and the output nodes [final[s],
+// final[s + 1]). Every range is non-empty, so each table is strictly ascending.
+struct Segs {
+    int B;
+    const int* tri;
+    const long long* in;
+    const int* pre;        // DoPreSplit
+    const int* frag;
+    const int* node;
+    const int* order;
+    const int* final;
+    const int* maxDepth;   // nodes deeper than this are gone after the collapse passes (INT_MAX: no pass collapsed)
+    const int* level;      // the collapse round's level
+    const int* pass;       // the collapse round: 0 retired, 1 first pass, 2 a later pass
+};
+
+// The segment holding x: the last s with starts[s] <= x.
+__device__ __forceinline__ int segOf(const int* starts, int B, int x) {
+    int lo = 0, hi = B;
+    while (hi - lo > 1) {
+        const int mid = (lo + hi) >> 1;
+        if (starts[mid] <= x) lo = mid; else hi = mid;
+    }
+    return lo;
+}
+
+template <class T>
+__global__ void k_gather(const T* v, const int* idx, int n, T* out) {
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i < n) out[i] = v[idx[i]];
+}
+
+// out[scan[j]] = v[j] for the flagged j (scan: the exclusive sum of the flags)
+template <class T>
+__global__ void k_pack(const T* v, const int* flags, const int* scan, int m, T* out) {
+    const int j = blockIdx.x * blockDim.x + threadIdx.x;
+    if (j < m && flags[j]) out[scan[j]] = v[j];
+}
+
 // ---------------------------------------------------------------------------------------------------------------- pre-split
 __device__ __forceinline__ Tri loadTri(const PackedVec3* pos, const GpuBlasTriangle* tris, int i) {
     const GpuBlasTriangle t = tris[i];
@@ -56,21 +101,27 @@ __device__ __forceinline__ Tri loadTri(const PackedVec3* pos, const GpuBlasTrian
     return r;
 }
 
-__global__ void k_priorities(const PackedVec3* pos, const GpuBlasTriangle* tris, int n, float* prio) {
+__global__ void k_priorities(const PackedVec3* pos, const GpuBlasTriangle* tris, Segs sg, int n, float* prio) {
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
-    if (i < n) prio[i] = priority(loadTri(pos, tris, i));
+    if (i >= n) return;
+    const int s = segOf(sg.tri, sg.B, i);
+    if (sg.pre[s]) prio[i] = priority(loadTri(pos, tris + sg.in[s], i - sg.tri[s]));
 }
 
-// Ordered sums: one thread adds the values in index order, as the mirror does (float addition is not associative).
-// The block stages tiles through shared memory so that the one adding thread reads nothing from HBM itself.
+// Ordered sums, one block per segment [begin[b], begin[b + 1]) (through `remap` when given): one thread adds the values
+// in index order onto acc[b], as the mirror does (float addition is not associative). Blocks whose `active` entry is 0 do
+// nothing. The block stages tiles through shared memory so that the one adding thread reads nothing from HBM itself.
 constexpr int SUM_THREADS = 1024;
 template <class T, int TILE>
-__global__ void __launch_bounds__(SUM_THREADS) k_ordered_sum(const T* v, int n, const int* nDev, T* acc) {
+__global__ void __launch_bounds__(SUM_THREADS) k_ordered_sum(const T* v, const int* begin, const int* remap, const int* active, T* acc) {
     __shared__ T tile[TILE];
-    if (nDev) n = *nDev;
-    T s = threadIdx.x == 0 ? *acc : T(0);
-    for (int base = 0; base < n; base += TILE) {
-        const int m = min(TILE, n - base);
+    const int b = blockIdx.x;
+    if (active && !active[b]) return;
+    int lo = begin[b], hi = begin[b + 1];
+    if (remap) { lo = remap[lo]; hi = remap[hi]; }
+    T s = threadIdx.x == 0 ? acc[b] : T(0);
+    for (int base = lo; base < hi; base += TILE) {
+        const int m = min(TILE, hi - base);
         for (int k = threadIdx.x; k < m; k += SUM_THREADS) tile[k] = v[base + k];
         __syncthreads();
         if (threadIdx.x == 0) {
@@ -79,25 +130,32 @@ __global__ void __launch_bounds__(SUM_THREADS) k_ordered_sum(const T* v, int n, 
         }
         __syncthreads();
     }
-    if (threadIdx.x == 0) *acc = s;
+    if (threadIdx.x == 0) acc[b] = s;
 }
 
-__global__ void k_split_counts(const float* prio, const float* total, int n, float splitFactor, unsigned long long* counts) {
+// Fragments per triangle: its split count in a pre-split BLAS, 1 in the others. counts[n] = 0 ends the scan.
+__global__ void k_split_counts(const float* prio, const float* total, Segs sg, int n, float splitFactor, unsigned long long* counts) {
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i > n) return;
     if (i == n) { counts[n] = 0; return; }
-    counts[i] = splitCount(prio[i], *total, n, splitFactor);
+    const int s = segOf(sg.tri, sg.B, i);
+    counts[i] = sg.pre[s] ? splitCount(prio[i], total[s], sg.tri[s + 1] - sg.tri[s], splitFactor) : 1ull;
 }
 
-// Box of every vertex in triangle order (p0, p1, p2 of each): per-thread chunks folded in order, chunks combined in order.
-__global__ void __launch_bounds__(1024) k_global_box(const PackedVec3* pos, const GpuBlasTriangle* tris, int n, Box* out) {
+// Box of every vertex of a pre-split BLAS in triangle order (p0, p1, p2 of each), one block per BLAS: per-thread chunks
+// folded in order, chunks combined in order.
+__global__ void __launch_bounds__(1024) k_global_box(const PackedVec3* pos, const GpuBlasTriangle* tris, Segs sg, Box* out) {
     __shared__ Box part[1024];
     __shared__ int has[1024];
+    const int s = blockIdx.x;
+    if (!sg.pre[s]) return;
+    const GpuBlasTriangle* t0 = tris + sg.in[s];
+    const int n = sg.tri[s + 1] - sg.tri[s];
     const int per = (n + 1023) / 1024;
     const int b0 = min(n, threadIdx.x * per), e0 = min(n, b0 + per);
     Box acc = boxIdentity();
     for (int i = b0; i < e0; i++) {
-        const Tri t = loadTri(pos, tris, i);
+        const Tri t = loadTri(pos, t0, i);
         for (int k = 0; k < 3; k++) { Box p = {{t.p[k].v[0], t.p[k].v[1], t.p[k].v[2]}, {t.p[k].v[0], t.p[k].v[1], t.p[k].v[2]}}; acc = combine(acc, p); }
     }
     part[threadIdx.x] = acc;
@@ -106,20 +164,28 @@ __global__ void __launch_bounds__(1024) k_global_box(const PackedVec3* pos, cons
     if (threadIdx.x == 0) {
         Box g = boxEmpty();
         for (int t = 0; t < 1024; t++) if (has[t]) g = combine(g, part[t]);
-        *out = g;
+        out[s] = g;
     }
 }
 
 // One thread per triangle, writing its fragments to [off[i], off[i+1]). The split stack lives in the same range, growing
 // down from its end: the stack's items hold at least one fragment each and together exactly the ones not yet written, so
 // they never reach the slot the next fragment goes to. Item j: box in bounds[end-1-j], split count in ids[end-1-j].
-__global__ void k_presplit(const PackedVec3* pos, const GpuBlasTriangle* tris, int n, const unsigned long long* off,
+// A triangle of one fragment (every triangle of a BLAS that is not pre-split) writes its own box. origIds are BLAS-local.
+__global__ void k_presplit(const PackedVec3* pos, const GpuBlasTriangle* tris, Segs sg, int n, const unsigned long long* off,
                            const Box* globalBox, Box* bounds, int* origIds) {
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= n) return;
-    const Box g = *globalBox;
-    const Tri tri = loadTri(pos, tris, i);
+    const int s = segOf(sg.tri, sg.B, i);
+    const int local = i - sg.tri[s];
+    const Tri tri = loadTri(pos, tris + sg.in[s], local);
     const size_t begin = (size_t)off[i], end = (size_t)off[i + 1];
+    if (end - begin == 1) {
+        storeBox(bounds, begin, boxFromTri(tri));
+        origIds[begin] = local;
+        return;
+    }
+    const Box g = globalBox[s];
     size_t counter = begin;
     int sp = 0;
     storeBox(bounds, end - 1, boxFromTri(tri));
@@ -131,7 +197,7 @@ __global__ void k_presplit(const PackedVec3* pos, const GpuBlasTriangle* tris, i
         const int splits = origIds[end - 1 - sp];
         if (splits == 1) {
             storeBox(bounds, counter, box);
-            origIds[counter] = i;
+            origIds[counter] = local;
             counter++;
             continue;
         }
@@ -146,17 +212,17 @@ __global__ void k_presplit(const PackedVec3* pos, const GpuBlasTriangle* tris, i
     }
 }
 
-__global__ void k_tri_bounds(const PackedVec3* pos, const GpuBlasTriangle* tris, int n, Box* bounds) {
-    const int i = blockIdx.x * blockDim.x + threadIdx.x;
-    if (i < n) storeBox(bounds, i, boxFromTri(loadTri(pos, tris, i)));
-}
-
 __global__ void k_sort_keys(const Box* bounds, int n, int axis, uint32_t* keys, int* vals) {
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= n) return;
     const Box b = loadBox(bounds, i);
     keys[i] = floatToKey(b.mn[axis] + b.mx[axis]);
     vals[i] = i;
+}
+// the BLAS of each fragment id, for the second (stable) sort pass
+__global__ void k_seg_keys(const int* ids, int n, Segs sg, uint32_t* keys) {
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i < n) keys[i] = (uint32_t)segOf(sg.frag, sg.B, ids[i]);
 }
 
 // ---------------------------------------------------------------------------------------------------------------- tree
@@ -420,14 +486,41 @@ __global__ void k_split_small(TreeArgs a, int n) {
 }
 
 // ---------------------------------------------------------------------------------------------------------------- post passes
-__global__ void k_root_duplicate(GpuBlasNode* nodes, int* parent, int* depth, int* ostart, int* ocount, int n) {
-    GpuBlasNode root = nodes[1];
-    nodes[2] = root;
-    nodes[3] = root;
-    root.TriStartOrChild = 2;
+// One thread per BLAS: seeds its root (node[s] + 1 over its fragments) as a task of the first level or as a small subtree.
+// A root's parent is -1.
+__global__ void k_seed_roots(TreeArgs a, Segs sg) {
+    const int s = blockIdx.x * blockDim.x + threadIdx.x;
+    if (s >= sg.B) return;
+    const int r = sg.node[s] + 1, start = sg.frag[s], count = sg.frag[s + 1] - start;
+    GpuBlasNode root = {};
+    root.TriStartOrChild = start;
+    root.TriCount = count;
+    a.nodes[r] = root;
+    a.parent[r] = -1;
+    a.depth[r] = 0;
+    a.ostart[r] = start;
+    a.ocount[r] = count;
+    pushTask(a, make_int2(r, r + 1), count);
+}
+
+// A root that stayed a leaf becomes an inner node over two copies of itself (BLAS.Build's leaf-root case).
+__global__ void k_root_duplicate(GpuBlasNode* nodes, int* parent, int* depth, int* ostart, int* ocount, Segs sg) {
+    const int s = blockIdx.x * blockDim.x + threadIdx.x;
+    if (s >= sg.B) return;
+    const int r = sg.node[s] + 1;
+    GpuBlasNode root = nodes[r];
+    if (!(root.TriCount > 0)) return;
+    nodes[r + 1] = root;
+    nodes[r + 2] = root;
+    root.TriStartOrChild = r + 1;
     root.TriCount = 0;
-    nodes[1] = root;
-    for (int k = 2; k < 4; k++) { parent[k] = 1; depth[k] = 1; ostart[k] = 0; ocount[k] = n; }
+    nodes[r] = root;
+    for (int k = r + 1; k < r + 3; k++) { parent[k] = r; depth[k] = 1; ostart[k] = sg.frag[s]; ocount[k] = sg.frag[s + 1] - sg.frag[s]; }
+}
+// The second copy of a duplicated leaf root: the only right child that starts where its parent starts.
+__device__ __forceinline__ bool rootCopy(const GpuBlasNode* nodes, const int* parent, const int* ostart, int v) {
+    const int p = parent[v];
+    return p >= 0 && v == nodes[p].TriStartOrChild + 1 && ostart[v] == ostart[p];
 }
 
 // computeRequiredStackSize, bottom up: g(v) = 0 if both children of v are leaves, g(inner child) if one is, and
@@ -435,14 +528,14 @@ __global__ void k_root_duplicate(GpuBlasNode* nodes, int* parent, int* depth, in
 // the second arrival continues.
 __global__ void k_stack_size(const GpuBlasNode* nodes, const int* parent, const int* depth, int cap, int* g, int* arrive) {
     int v = blockIdx.x * blockDim.x + threadIdx.x;
-    if (v < 1 || v >= cap || depth[v] < 0 || nodes[v].TriCount > 0) return;
+    if (v >= cap || depth[v] < 0 || nodes[v].TriCount > 0) return;
     const int c0 = nodes[v].TriStartOrChild;
     if (!(nodes[c0].TriCount > 0 && nodes[c0 + 1].TriCount > 0)) return;
     int gv = 0;
     g[v] = 0;
     for (;;) {
         const int p = parent[v];
-        if (p <= 0) return;
+        if (p < 0) return;
         const int c = nodes[p].TriStartOrChild;
         const bool li = !(nodes[c].TriCount > 0), ri = !(nodes[c + 1].TriCount > 0);
         if (li && ri) {
@@ -458,113 +551,111 @@ __global__ void k_stack_size(const GpuBlasNode* nodes, const int* parent, const 
 }
 
 // Pre-order ranks: the nodes whose range starts at fragment s are a chain of left children, one per depth from the
-// highest one (dmin) down to a leaf (dleaf); pre-order lists the chains by s. rank = base[s] + depth - dmin[s].
-__global__ void k_chain_ends(const GpuBlasNode* nodes, const int* depth, const int* ostart, int cap, int* dmin, int* dleaf) {
+// highest one (dmin) down to a leaf (dleaf); pre-order lists the chains by s, and so the BLASes of a batch one after
+// another. rank = base[s] + depth - dmin[s]. A duplicated leaf root's second copy comes after the first: one more rank.
+__global__ void k_chain_ends(const GpuBlasNode* nodes, const int* parent, const int* depth, const int* ostart, int cap, int* dmin, int* dleaf) {
     const int v = blockIdx.x * blockDim.x + threadIdx.x;
-    if (v < 1 || v >= cap || depth[v] < 0) return;
+    if (v >= cap || depth[v] < 0) return;
     atomicMin(&dmin[ostart[v]], depth[v]);
-    if (nodes[v].TriCount > 0) dleaf[ostart[v]] = depth[v];
+    if (nodes[v].TriCount > 0) atomicMax(&dleaf[ostart[v]], depth[v] + (rootCopy(nodes, parent, ostart, v) ? 1 : 0));
 }
 __global__ void k_chain_len(const int* dmin, const int* dleaf, int n, int* len) {
     const int s = blockIdx.x * blockDim.x + threadIdx.x;
     if (s < n) len[s] = dmin[s] == DEPTH_NONE ? 0 : dleaf[s] - dmin[s] + 1;
 }
-__global__ void k_preorder(const int* depth, const int* ostart, int cap, const int* dmin, const int* base, int* order) {
+__global__ void k_preorder(const GpuBlasNode* nodes, const int* parent, const int* depth, const int* ostart, int cap, const int* dmin,
+                           const int* base, int* order) {
     const int v = blockIdx.x * blockDim.x + threadIdx.x;
-    if (v < 1 || v >= cap || depth[v] < 0) return;
+    if (v >= cap || depth[v] < 0) return;
     const int s = ostart[v];
-    order[base[s] + depth[v] - dmin[s]] = v;
+    order[base[s] + depth[v] - dmin[s] + (rootCopy(nodes, parent, ostart, v) ? 1 : 0)] = v;
 }
-__global__ void k_preorder_root_duplicate(int* order) { order[0] = 1; order[1] = 2; order[2] = 3; }
 
-// computeGlobalSAH terms in pre-order; leaf counts from `counts` (by node id) or, for the compacted tree, `final`.
-__global__ void k_sah_terms(const int* order, int m, const GpuBlasNode* nodes, const GpuBlasNode* final, const int* fidx,
+// Per BLAS: its first pre-order position (s <= B) and its RequiredStackSize (s < B).
+__global__ void k_order_info(const int* base, const int* g, Segs sg, int* orderStart, int* stackSize) {
+    const int s = blockIdx.x * blockDim.x + threadIdx.x;
+    if (s > sg.B) return;
+    orderStart[s] = base[sg.frag[s]];
+    if (s < sg.B) stackSize[s] = g[sg.node[s] + 1];
+}
+
+// computeGlobalSAH terms in pre-order: of the built tree (final == nullptr) or of the compacted one.
+__global__ void k_sah_terms(const int* order, int m, Segs sg, const GpuBlasNode* nodes, const GpuBlasNode* final, const int* fidx,
                             float triangleCost, double* terms) {
     const int j = blockIdx.x * blockDim.x + threadIdx.x;
     if (j >= m) return;
+    const int s = segOf(sg.order, sg.B, j);
     const int v = order[j];
     const GpuBlasNode n = final ? final[fidx[v]] : nodes[v];
-    const GpuBlasNode root = final ? final[1] : nodes[1];
+    const GpuBlasNode root = final ? final[sg.final[s] + 1] : nodes[sg.node[s] + 1];
     terms[j] = sahTerm(n, 1.0 / (double)nodeHalfArea(root), triangleCost);
 }
 
 // collapseDeepestLevel's cost terms, in pre-order (the nodes that add one never contain each other, so this is also the
-// mirror's post-order among them). First pass: inner nodes deeper than `level` whose children are both leaves. Later passes:
-// inner nodes at depth `level`, whose children are leaves after the pass's collapse and hold their whole subtrees.
-__global__ void k_collapse_terms(const int* order, int m, const GpuBlasNode* nodes, const int* depth, const int* ocount,
-                                 int level, int firstPass, float triangleCost, double* terms, uint8_t* flags) {
+// mirror's post-order among them), for the BLASes still in the collapse rounds. First pass: inner nodes deeper than
+// `level` whose children are both leaves. Later passes: inner nodes at depth `level`, whose children are leaves after the
+// pass's collapse and hold their whole subtrees.
+__global__ void k_collapse_terms(const int* order, int m, Segs sg, const GpuBlasNode* nodes, const int* depth, const int* ocount,
+                                 float triangleCost, double* terms, int* flags) {
     const int j = blockIdx.x * blockDim.x + threadIdx.x;
-    if (j >= m) return;
+    if (j > m) return;
+    if (j == m) { flags[m] = 0; return; }
+    const int s = segOf(sg.order, sg.B, j);
+    const int pass = sg.pass[s], level = sg.level[s];
     const int v = order[j];
     const GpuBlasNode n = nodes[v];
     bool q = false;
-    if (!(n.TriCount > 0)) {
+    if (pass && !(n.TriCount > 0)) {
         const int c = n.TriStartOrChild;
-        q = firstPass ? (depth[v] > level && nodes[c].TriCount > 0 && nodes[c + 1].TriCount > 0) : depth[v] == level;
-        if (q) {
-            terms[j] = collapseTerm(n, nodes[c], nodes[c + 1], ocount[c], ocount[c + 1], nodes[1], triangleCost);
-        }
+        q = pass == 1 ? (depth[v] > level && nodes[c].TriCount > 0 && nodes[c + 1].TriCount > 0) : depth[v] == level;
+        if (q) terms[j] = collapseTerm(n, nodes[c], nodes[c + 1], ocount[c], ocount[c + 1], nodes[sg.node[s] + 1], triangleCost);
     }
     flags[j] = q;
 }
 
-__global__ void k_reachable(const int* order, int m, const int* depth, int maxDepth, uint8_t* flags) {
+__global__ void k_reachable(const int* order, int m, Segs sg, const int* depth, int* flags) {
     const int j = blockIdx.x * blockDim.x + threadIdx.x;
-    if (j < m) flags[j] = depth[order[j]] <= maxDepth;
+    if (j < m) flags[j] = depth[order[j]] <= sg.maxDepth[segOf(sg.order, sg.B, j)];
+    if (j == m) flags[m] = 0;
 }
 
 // After the collapse passes a node is inner if it was split and is shallower than the collapsed level.
-__device__ __forceinline__ bool finalInner(const GpuBlasNode* nodes, const int* depth, int v, int maxDepth) {
-    return !(nodes[v].TriCount > 0) && depth[v] < maxDepth;
-}
-__global__ void k_inner_flags(const int* order, int m, const GpuBlasNode* nodes, const int* depth, int maxDepth, int* flags) {
+__global__ void k_inner_flags(const int* order, int m, Segs sg, const GpuBlasNode* nodes, const int* depth, int* flags) {
     const int j = blockIdx.x * blockDim.x + threadIdx.x;
-    if (j < m) flags[j] = finalInner(nodes, depth, order[j], maxDepth);
-}
-__global__ void k_inner_ranks(const int* order, int m, const int* scan, int* rankOf) {
-    const int j = blockIdx.x * blockDim.x + threadIdx.x;
-    if (j < m) rankOf[order[j]] = scan[j];
-}
-
-// removeEmptySubtrees: the children of the inner node of pre-order rank k land at 2 + 2k.
-__global__ void k_final_nodes(const int* order, int m, const GpuBlasNode* nodes, const int* parent, const int* depth,
-                              const int* ostart, const int* ocount, const int* rankOf, int maxDepth, GpuBlasNode* final, int* fidx) {
-    const int j = blockIdx.x * blockDim.x + threadIdx.x;
+    if (j == m) flags[m] = 0;
     if (j >= m) return;
     const int v = order[j];
-    int fi = 1;
-    if (v != 1) {
-        const int p = parent[v];
-        fi = 2 + 2 * rankOf[p] + (v == nodes[p].TriStartOrChild + 1 ? 1 : 0);
-    }
-    fidx[v] = fi;
-    GpuBlasNode out = nodes[v];
-    if (finalInner(nodes, depth, v, maxDepth)) { out.TriStartOrChild = 2 + 2 * rankOf[v]; out.TriCount = 0; }
-    else { out.TriStartOrChild = ostart[v]; out.TriCount = ocount[v]; }
-    final[fi] = out;
+    flags[j] = !(nodes[v].TriCount > 0) && depth[v] < sg.maxDepth[segOf(sg.order, sg.B, j)];
+}
+// BLAS-local pre-order ranks of the inner nodes
+__global__ void k_inner_ranks(const int* order, int m, Segs sg, const int* scan, int* rankOf) {
+    const int j = blockIdx.x * blockDim.x + threadIdx.x;
+    if (j < m) rankOf[order[j]] = scan[j] - scan[sg.order[segOf(sg.order, sg.B, j)]];
 }
 
-// BLAS.GetUnindexedTriangles: leaves in node order, fragment = triangle. The array holds n triangles; when the root is a
-// leaf, its two copies list all n each, and the second one's triangles would land past the end: the mirror writes them
-// beyond its n-element array (heap overflow), so what it returns is the first copy's n triangles and the second leaf's
-// offset n. The writes past n are dropped here.
-__global__ void k_leaf_counts(const GpuBlasNode* final, int f, int* counts) {
-    const int i = blockIdx.x * blockDim.x + threadIdx.x;
-    if (i < f) counts[i] = (i >= 2 && final[i].TriCount > 0) ? final[i].TriCount : 0;
-}
-__global__ void k_unindex_plain(GpuBlasNode* final, int f, const int* offsets, const int* ids0, const GpuBlasTriangle* in,
-                                GpuBlasTriangle* out, int n) {
-    const int i = blockIdx.x * blockDim.x + threadIdx.x;
-    if (i < 2 || i >= f || !(final[i].TriCount > 0)) return;
-    const int s = final[i].TriStartOrChild, c = final[i].TriCount, o = offsets[i];
-    for (int k = 0; k < c && o + k < n; k++) out[o + k] = in[ids0[s + k]];
-    final[i].TriStartOrChild = o;
+// removeEmptySubtrees: the children of the inner node of pre-order rank k land at 2 + 2k of the BLAS's output range, whose
+// node 0 is zero. Leaves keep their absolute fragment range until the unindexing.
+__global__ void k_final_nodes(const int* order, int m, Segs sg, const GpuBlasNode* nodes, const int* parent, const int* depth,
+                              const int* ostart, const int* ocount, const int* rankOf, GpuBlasNode* final, int* fidx) {
+    const int j = blockIdx.x * blockDim.x + threadIdx.x;
+    if (j >= m) return;
+    const int s = segOf(sg.order, sg.B, j);
+    const int v = order[j], o = sg.final[s];
+    int fi = 1;
+    const int p = parent[v];
+    if (p >= 0) fi = 2 + 2 * rankOf[p] + (v == nodes[p].TriStartOrChild + 1 ? 1 : 0);
+    else final[o] = GpuBlasNode{};
+    fidx[v] = o + fi;
+    GpuBlasNode out = nodes[v];
+    if (!(nodes[v].TriCount > 0) && depth[v] < sg.maxDepth[s]) { out.TriStartOrChild = 2 + 2 * rankOf[v]; out.TriCount = 0; }
+    else { out.TriStartOrChild = ostart[v]; out.TriCount = ocount[v]; }
+    final[o + fi] = out;
 }
 
 // PreSplitting.GetUnindexedTriangles: per leaf the sorted unique triangle ids, from one sort of (leaf start, triangle id)
-__global__ void k_leaf_marks(const GpuBlasNode* final, int f, int* marks) {
+__global__ void k_leaf_marks(const GpuBlasNode* final, int f, Segs sg, int* marks) {
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= 2 && i < f && final[i].TriCount > 0) marks[final[i].TriStartOrChild] = final[i].TriStartOrChild;
+    if (i < f && i - sg.final[segOf(sg.final, sg.B, i)] >= 2 && final[i].TriCount > 0) marks[final[i].TriStartOrChild] = final[i].TriStartOrChild;
 }
 __global__ void k_leaf_keys(const int* segStart, const int* ids0, const int* origIds, int n, unsigned long long* keys) {
     const int q = blockIdx.x * blockDim.x + threadIdx.x;
@@ -597,27 +688,52 @@ __device__ int sharedCount(const unsigned long long* keys, const GpuBlasNode& l,
     return c;
 }
 
-__global__ void k_pair_sizes(const GpuBlasNode* final, int pairs, const unsigned long long* keys, int* sizes) {
-    const int p = blockIdx.x * blockDim.x + threadIdx.x;
-    if (p > pairs) return;
-    if (p == pairs) { sizes[p] = 0; return; }
-    const GpuBlasNode l = final[2 + 2 * p], r = final[3 + 2 * p];
-    const bool ll = l.TriCount > 0, rl = r.TriCount > 0;
-    int s = 0;
-    if (ll && rl) s = uniqueCount(keys, l) + uniqueCount(keys, r) - sharedCount(keys, l, r);
-    else if (ll) s = uniqueCount(keys, l);
-    else if (rl) s = uniqueCount(keys, r);
-    sizes[p] = s;
+// Output triangles per output node (counts[f] = 0 ends the scan). BLAS.GetUnindexedTriangles (not pre-split): each leaf's
+// fragments, which are its triangles. When the root is a leaf, its two copies list all n each, and the second one's
+// triangles would land past the end: the mirror writes them beyond its n-element array (heap overflow), so what it returns
+// is the first copy's n triangles and the second leaf's offset n; the second copy counts none here. Pre-split: the left
+// node of each sibling pair counts the pair's unique triangles.
+__global__ void k_tri_counts(const GpuBlasNode* final, int f, Segs sg, const unsigned long long* keys, int* counts) {
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i > f) return;
+    if (i == f) { counts[f] = 0; return; }
+    const int s = segOf(sg.final, sg.B, i), li = i - sg.final[s];
+    int c = 0;
+    if (li >= 2 && !sg.pre[s]) {
+        const GpuBlasNode n = final[i];
+        if (n.TriCount > 0 && !(li == 3 && final[i - 1].TriCount > 0 && final[i - 1].TriStartOrChild == n.TriStartOrChild)) c = n.TriCount;
+    } else if (li >= 2 && !(li & 1)) {
+        const GpuBlasNode l = final[i], r = final[i + 1];
+        const bool ll = l.TriCount > 0, rl = r.TriCount > 0;
+        if (ll && rl) c = uniqueCount(keys, l) + uniqueCount(keys, r) - sharedCount(keys, l, r);
+        else if (ll) c = uniqueCount(keys, l);
+        else if (rl) c = uniqueCount(keys, r);
+    }
+    counts[i] = c;
 }
 
-__global__ void k_pair_write(GpuBlasNode* final, int pairs, const unsigned long long* keys, const int* offsets,
-                             const GpuBlasTriangle* in, GpuBlasTriangle* out) {
-    const int p = blockIdx.x * blockDim.x + threadIdx.x;
-    if (p >= pairs) return;
-    GpuBlasNode& l = final[2 + 2 * p];
-    GpuBlasNode& r = final[3 + 2 * p];
+// Writes each output node's triangles at offsets[i] and makes leaf ranges BLAS-local (offsets[final[s]] is the BLAS's first
+// output triangle). `in` is the input array; a BLAS's fragments and origIds index its own range of it.
+__global__ void k_unindex(GpuBlasNode* final, int f, Segs sg, const int* offsets, const int* ids0, const int* origIds,
+                          const unsigned long long* keys, const GpuBlasTriangle* tris, GpuBlasTriangle* out) {
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= f) return;
+    const int s = segOf(sg.final, sg.B, i), li = i - sg.final[s];
+    if (li < 2) return;
+    const GpuBlasTriangle* in = tris + sg.in[s];
+    const int first = offsets[sg.final[s]];
+    const int counter = offsets[i];
+    if (!sg.pre[s]) {
+        if (!(final[i].TriCount > 0)) return;
+        const int st = final[i].TriStartOrChild, c = final[i].TriCount, o = counter - first, n = sg.frag[s + 1] - sg.frag[s];
+        for (int k = 0; k < c && o + k < n; k++) out[counter + k] = in[origIds[ids0[st + k]]];
+        final[i].TriStartOrChild = o;
+        return;
+    }
+    if (li & 1) return;
+    GpuBlasNode& l = final[i];
+    GpuBlasNode& r = final[i + 1];
     const bool ll = l.TriCount > 0, rl = r.TriCount > 0;
-    const int counter = offsets[p];
     if (ll && rl) {
         const GpuBlasNode L = l, R = r;
         const int lu = uniqueCount(keys, L), ru = uniqueCount(keys, R);
@@ -640,14 +756,14 @@ __global__ void k_pair_write(GpuBlasNode* final, int pairs, const unsigned long 
                 if (!(!b.done() && b.cur() == id)) out[counter + lu + onlyRight++] = in[id];
             }
         }
-        l.TriStartOrChild = counter; l.TriCount = lu;
-        r.TriStartOrChild = counter + onlyLeft; r.TriCount = ru;
+        l.TriStartOrChild = counter - first; l.TriCount = lu;
+        r.TriStartOrChild = counter - first + onlyLeft; r.TriCount = ru;
     } else if (ll || rl) {
         GpuBlasNode& leaf = ll ? l : r;
         const GpuBlasNode Lf = leaf;
         int c = 0;
         for (Uniq u(keys, Lf); !u.done(); u.next()) out[counter + c++] = in[u.cur()];
-        leaf.TriStartOrChild = counter;
+        leaf.TriStartOrChild = counter - first;
         leaf.TriCount = c;
     }
 }
@@ -677,12 +793,14 @@ __global__ void k_global_sah(const GpuBlasNode* nodes, int* stack, float triangl
 }  // namespace idkbb
 
 // ---------------------------------------------------------------------------------------------------------------- host driver
+// A finished build on the host: the BLASes' nodes and triangles one after another, and per BLAS its desc (NodeOffset,
+// NodeCount, TriangleOffset, TriangleCount, RequiredStackSize; the rest as the caller's), fragment count and SAH.
 struct IdkPtBlasBuild {
     std::vector<GpuBlasNode> nodes;
     std::vector<GpuBlasTriangle> tris;
-    int32_t requiredStackSize = 0;
-    int32_t fragmentCount = 0;
-    double sah = 0.0;
+    std::vector<GpuBlasDesc> descs;
+    std::vector<int32_t> fragmentCounts;
+    std::vector<double> sahs;
 };
 
 namespace idkbb {
@@ -717,20 +835,20 @@ struct StageTimer {
         if (marks.size() >= 2) cudaEventElapsedTime(&ms, marks.front().second, marks.back().second);
         return ms;
     }
-    void print(int fragments) {
+    void print(int blases, long long fragments) {
         if (!getenv("IDKPT_BLAS_TIMING")) return;
         for (size_t i = 1; i < marks.size(); i++) {
             float ms = 0.0f;
             cudaEventElapsedTime(&ms, marks[i - 1].second, marks[i].second);
             fprintf(stderr, "[idkpt_blas_build] %-14s %8.2f ms\n", marks[i].first, ms);
         }
-        fprintf(stderr, "[idkpt_blas_build] %-14s %8.2f ms (%d fragments)\n", "total", total(), fragments);
+        fprintf(stderr, "[idkpt_blas_build] %-14s %8.2f ms (%d BLASes, %lld fragments)\n", "total", total(), blases, fragments);
     }
 };
 
 template <class F> static inline int blocksFor(F n, int t) { return (int)((n + t - 1) / t); }
 
-enum { BB_OK = 0, BB_CUDA = 1, BB_TOO_MANY_FRAGMENTS = 2 };
+enum { BB_OK = 0, BB_CUDA = 1, BB_TOO_MANY_FRAGMENTS = 2, BB_TOO_MANY_NODES = 3 };
 
 #define BB_CK(call)                                                                                     \
     do {                                                                                                \
@@ -738,27 +856,41 @@ enum { BB_OK = 0, BB_CUDA = 1, BB_TOO_MANY_FRAGMENTS = 2 };
         if (e_ != cudaSuccess) { err = std::string(#call) + ": " + cudaGetErrorString(e_); return BB_CUDA; } \
     } while (0)
 
-// One build's result on the device: the nodes, the triangles and the SAH live in allocations of the caller's arena.
-struct DeviceResult {
-    GpuBlasNode* nodes = nullptr;
-    int nodeCount = 0;
-    GpuBlasTriangle* tris = nullptr;
-    int triCount = 0;
-    int requiredStackSize = 0;
-    int fragmentCount = 0;
-    double* sah = nullptr;
+// One BLAS of a batch: its triangles tris[offset, offset + count) of the caller's array, and whether it is pre-split.
+struct Input {
+    long long offset;
+    int count;
+    int preSplit;
 };
 
-// Runs the whole build on `stream` from device arrays (global vertex ids into `pos`); the arguments have been validated.
-// The result goes to `out`, in allocations of `keep`; the scratch is freed on return, after the stream has been waited for.
-static int build_device(cudaStream_t stream, const PackedVec3* pos, const GpuBlasTriangle* tris, int triCount, const Params& p,
-                        Arena& keep, DeviceResult& out, StageTimer& tm, std::string& err) {
-    Arena ar;
+// A batch's result on the device: the nodes and triangles of all BLASes one after another, in allocations of the caller's
+// arena, and per BLAS its ranges and values.
+struct DeviceResult {
+    GpuBlasNode* nodes = nullptr;
+    GpuBlasTriangle* tris = nullptr;
+    std::vector<int> nodeStart, triStart;   // B + 1 each
+    std::vector<int> requiredStackSize, fragmentCount;
+    std::vector<double> sah;
+};
 
-    // ---- 1. fragments
-    int n = triCount;
-    Box* bounds = nullptr;
-    int* origIds = nullptr;
+// The node ids a batch of BLASes of these fragment counts needs, or -1 when they do not fit in int32.
+template <class C> static long long nodeIdCount(const C& fragments, size_t B) {
+    long long total = 0;
+    for (size_t s = 0; s < B; s++) {
+        total += std::max<long long>(2 * (long long)fragments[s], 4);
+        if (total >= (1ll << 31)) return -1;
+    }
+    return total;
+}
+
+// Builds the BLASes `in` together on `stream` from device arrays (global vertex ids into `pos`); the arguments have been
+// validated, except for the fragment limits that pre-splitting decides. Every BLAS comes out as it would alone: the stages
+// run over the whole batch, with the per-BLAS tables of Segs. The result goes to `out`, in allocations of `keep`; the
+// scratch is freed on return, after the stream has been waited for.
+static int build_device(cudaStream_t stream, const PackedVec3* pos, const GpuBlasTriangle* tris, const std::vector<Input>& in,
+                        const Params& p, Arena& keep, DeviceResult& out, StageTimer& tm, std::string& err) {
+    Arena ar;
+    const int B = (int)in.size();
     void* cubTemp = nullptr;
     size_t cubBytes = 0;
     auto cubScratch = [&](size_t need) -> cudaError_t {
@@ -768,66 +900,129 @@ static int build_device(cudaStream_t stream, const PackedVec3* pos, const GpuBla
         if (e == cudaSuccess) { cubTemp = q; cubBytes = need; }
         return e;
     };
-    if (p.doPreSplit) {
-        float* prio;
-        float* total;
-        unsigned long long *counts, *offsets;
-        Box* gbox;
-        BB_CK(ar.get(prio, triCount));
-        BB_CK(ar.get(total, 1));
-        BB_CK(ar.get(counts, (size_t)triCount + 1));
-        BB_CK(ar.get(offsets, (size_t)triCount + 1));
-        BB_CK(ar.get(gbox, 1));
-        k_priorities<<<blocksFor(triCount, 256), 256, 0, stream>>>(pos, tris, triCount, prio);
-        tm.mark("priorities");
-        BB_CK(cudaMemsetAsync(total, 0, sizeof(float), stream));
-        k_ordered_sum<float, 8192><<<1, SUM_THREADS, 0, stream>>>(prio, triCount, nullptr, total);
-        tm.mark("priority sum");
-        k_split_counts<<<blocksFor(triCount + 1, 256), 256, 0, stream>>>(prio, total, triCount, p.splitFactor, counts);
+    auto exclusiveSum = [&](auto* src, auto* dst, int count) -> cudaError_t {
         size_t need = 0;
-        BB_CK(cub::DeviceScan::ExclusiveSum(nullptr, need, counts, offsets, triCount + 1, stream));
-        BB_CK(cubScratch(need));
-        BB_CK(cub::DeviceScan::ExclusiveSum(cubTemp, need, counts, offsets, triCount + 1, stream));
-        unsigned long long fragments = 0;
-        BB_CK(cudaMemcpyAsync(&fragments, offsets + triCount, sizeof(fragments), cudaMemcpyDeviceToHost, stream));
-        BB_CK(cudaStreamSynchronize(stream));
-        if (fragments > (unsigned long long)MAX_FRAGMENTS) {
-            err = "pre-splitting makes " + std::to_string(fragments) + " fragments, more than 2^24";
+        cudaError_t e = cub::DeviceScan::ExclusiveSum(nullptr, need, src, dst, count, stream);
+        if (e == cudaSuccess) e = cubScratch(need);
+        if (e == cudaSuccess) e = cub::DeviceScan::ExclusiveSum(cubTemp, need, src, dst, count, stream);
+        return e;
+    };
+
+    // ---- the per-BLAS tables (host copies, uploaded as they become known)
+    std::vector<int> hTri(B + 1), hPre(B), hFrag(B + 1), hNode(B + 1), hOrder(B + 1), hFinal(B + 1), hMaxDepth(B, INT_MAX),
+        hLevel(B, 0), hPass(B, 0), hStack(B);
+    std::vector<long long> hIn(B);
+    bool anyPre = false;
+    for (int s = 0; s < B; s++) {
+        hTri[s + 1] = hTri[s] + in[s].count;
+        hIn[s] = in[s].offset;
+        hPre[s] = in[s].preSplit;
+        anyPre |= in[s].preSplit != 0;
+    }
+    const int M = hTri[B];
+    int *dTri, *dPre, *dFrag, *dNode, *dOrder, *dFinal, *dMaxDepth, *dLevel, *dPass;
+    long long* dIn;
+    BB_CK(ar.get(dTri, B + 1));
+    BB_CK(ar.get(dPre, B));
+    BB_CK(ar.get(dFrag, B + 1));
+    BB_CK(ar.get(dNode, B + 1));
+    BB_CK(ar.get(dOrder, B + 1));
+    BB_CK(ar.get(dFinal, B + 1));
+    BB_CK(ar.get(dMaxDepth, B));
+    BB_CK(ar.get(dLevel, B));
+    BB_CK(ar.get(dPass, B));
+    BB_CK(ar.get(dIn, B));
+    const Segs sg = {B, dTri, dIn, dPre, dFrag, dNode, dOrder, dFinal, dMaxDepth, dLevel, dPass};
+    auto up = [&](int* d, const std::vector<int>& h) { return cudaMemcpyAsync(d, h.data(), h.size() * sizeof(int), cudaMemcpyHostToDevice, stream); };
+    BB_CK(up(dTri, hTri));
+    BB_CK(up(dPre, hPre));
+    BB_CK(cudaMemcpyAsync(dIn, hIn.data(), B * sizeof(long long), cudaMemcpyHostToDevice, stream));
+
+    // ---- 1. fragments: split counts (1 for a BLAS that is not pre-split), their scan, then the fragments themselves
+    float *prio, *total;
+    unsigned long long *counts, *offsets, *fragStart;
+    Box* gbox;
+    BB_CK(ar.get(counts, (size_t)M + 1));
+    BB_CK(ar.get(offsets, (size_t)M + 1));
+    BB_CK(ar.get(fragStart, B + 1));
+    BB_CK(ar.get(total, B));
+    BB_CK(ar.get(gbox, B));
+    if (anyPre) {
+        BB_CK(ar.get(prio, M));
+        k_priorities<<<blocksFor(M, 256), 256, 0, stream>>>(pos, tris, sg, M, prio);
+        tm.mark("priorities");
+        BB_CK(cudaMemsetAsync(total, 0, B * sizeof(float), stream));
+        k_ordered_sum<float, 8192><<<B, SUM_THREADS, 0, stream>>>(prio, dTri, nullptr, dPre, total);
+        tm.mark("priority sum");
+    } else {
+        prio = nullptr;
+    }
+    k_split_counts<<<blocksFor(M + 1, 256), 256, 0, stream>>>(prio, total, sg, M, p.splitFactor, counts);
+    BB_CK(exclusiveSum(counts, offsets, M + 1));
+    k_gather<<<blocksFor(B + 1, 256), 256, 0, stream>>>(offsets, dTri, B + 1, fragStart);
+    std::vector<unsigned long long> hFrag64(B + 1);
+    BB_CK(cudaMemcpyAsync(hFrag64.data(), fragStart, (B + 1) * sizeof(unsigned long long), cudaMemcpyDeviceToHost, stream));
+    BB_CK(cudaStreamSynchronize(stream));
+    std::vector<unsigned long long> fragCount(B);
+    for (int s = 0; s < B; s++) {
+        fragCount[s] = hFrag64[s + 1] - hFrag64[s];
+        if (fragCount[s] > (unsigned long long)MAX_FRAGMENTS) {
+            err = "pre-splitting makes " + std::to_string(fragCount[s]) + " fragments of BLAS " + std::to_string(s) + ", more than 2^24";
             return BB_TOO_MANY_FRAGMENTS;
         }
-        n = (int)fragments;
-        BB_CK(ar.get(bounds, n));
-        BB_CK(ar.get(origIds, n));
-        k_global_box<<<1, 1024, 0, stream>>>(pos, tris, triCount, gbox);
-        k_presplit<<<blocksFor(triCount, 128), 128, 0, stream>>>(pos, tris, triCount, offsets, gbox, bounds, origIds);
-        tm.mark("split");
-    } else {
-        BB_CK(ar.get(bounds, n));
-        k_tri_bounds<<<blocksFor(n, 256), 256, 0, stream>>>(pos, tris, n, bounds);
-        tm.mark("bounds");
     }
+    const long long capTotal = nodeIdCount(fragCount, B);
+    if (capTotal < 0) {
+        err = "the batch's " + std::to_string(hFrag64[B]) + " fragments need 2^31 or more node ids";
+        return BB_TOO_MANY_NODES;
+    }
+    const int n = (int)hFrag64[B];   // fragments of the whole batch
+    const int cap = (int)capTotal;
+    for (int s = 0; s < B; s++) {
+        hFrag[s + 1] = (int)hFrag64[s + 1];
+        hNode[s + 1] = hNode[s] + std::max(2 * (int)fragCount[s], 4);
+    }
+    BB_CK(up(dFrag, hFrag));
+    BB_CK(up(dNode, hNode));
+    Box* bounds;
+    int* origIds;
+    BB_CK(ar.get(bounds, n));
+    BB_CK(ar.get(origIds, n));
+    if (anyPre) k_global_box<<<B, 1024, 0, stream>>>(pos, tris, sg, gbox);
+    k_presplit<<<blocksFor(M, 128), 128, 0, stream>>>(pos, tris, sg, M, offsets, gbox, bounds, origIds);
+    tm.mark("split");
 
-    // ---- 2. three stable sorts by centroid key
+    // ---- 2. three stable sorts by (BLAS, centroid key): by the key, then (in a batch) stably by the BLAS
     TreeArgs a = {};
     {
         uint32_t *keys, *keysOut;
-        int* vals;
+        int *vals, *byKey = nullptr;
         BB_CK(ar.get(keys, n));
         BB_CK(ar.get(keysOut, n));
         BB_CK(ar.get(vals, n));
+        if (B > 1) BB_CK(ar.get(byKey, n));
+        int segBits = 0;
+        while ((1 << segBits) < B) segBits++;
         for (int axis = 0; axis < 3; axis++) {
             BB_CK(ar.get(a.ids[axis], n));
+            int* first = B > 1 ? byKey : a.ids[axis];
             k_sort_keys<<<blocksFor(n, 256), 256, 0, stream>>>(bounds, n, axis, keys, vals);
             size_t need = 0;
-            BB_CK(cub::DeviceRadixSort::SortPairs(nullptr, need, keys, keysOut, vals, a.ids[axis], n, 0, 32, stream));
+            BB_CK(cub::DeviceRadixSort::SortPairs(nullptr, need, keys, keysOut, vals, first, n, 0, 32, stream));
             BB_CK(cubScratch(need));
-            BB_CK(cub::DeviceRadixSort::SortPairs(cubTemp, need, keys, keysOut, vals, a.ids[axis], n, 0, 32, stream));
+            BB_CK(cub::DeviceRadixSort::SortPairs(cubTemp, need, keys, keysOut, vals, first, n, 0, 32, stream));
+            if (B > 1) {
+                k_seg_keys<<<blocksFor(n, 256), 256, 0, stream>>>(byKey, n, sg, keys);
+                need = 0;
+                BB_CK(cub::DeviceRadixSort::SortPairs(nullptr, need, keys, keysOut, byKey, a.ids[axis], n, 0, segBits, stream));
+                BB_CK(cubScratch(need));
+                BB_CK(cub::DeviceRadixSort::SortPairs(cubTemp, need, keys, keysOut, byKey, a.ids[axis], n, 0, segBits, stream));
+            }
         }
     }
     tm.mark("sort");
 
-    // ---- 3. tree
-    const int cap = std::max(2 * n, 4);
+    // ---- 3. tree: every BLAS's root is a task of the first level; the levels of all BLASes advance together
     a.bounds = bounds;
     a.p = p;
     BB_CK(ar.get(a.aux, n));
@@ -848,29 +1043,13 @@ static int build_device(cudaStream_t stream, const PackedVec3* pos, const GpuBla
     BB_CK(cudaMemsetAsync(a.nodes, 0, (size_t)cap * sizeof(GpuBlasNode), stream));
     BB_CK(cudaMemsetAsync(a.depth, 0xFF, (size_t)cap * sizeof(int), stream));
     BB_CK(cudaMemsetAsync(counters, 0, 2 * sizeof(int), stream));
-    {
-        GpuBlasNode root = {};
-        root.TriStartOrChild = 0;
-        root.TriCount = n;
-        const int zero = 0;
-        const int2 task = make_int2(1, 2);
-        BB_CK(cudaMemcpyAsync(a.nodes + 1, &root, sizeof(root), cudaMemcpyHostToDevice, stream));
-        BB_CK(cudaMemcpyAsync(a.parent + 1, &zero, 4, cudaMemcpyHostToDevice, stream));
-        BB_CK(cudaMemcpyAsync(a.depth + 1, &zero, 4, cudaMemcpyHostToDevice, stream));
-        BB_CK(cudaMemcpyAsync(a.ostart + 1, &zero, 4, cudaMemcpyHostToDevice, stream));
-        BB_CK(cudaMemcpyAsync(a.ocount + 1, &n, 4, cudaMemcpyHostToDevice, stream));
-        if (n > SMALL_NODE) BB_CK(cudaMemcpyAsync(big[0], &task, sizeof(task), cudaMemcpyHostToDevice, stream));
-        else {
-            const int one = 1;
-            BB_CK(cudaMemcpyAsync(small, &task, sizeof(task), cudaMemcpyHostToDevice, stream));
-            BB_CK(cudaMemcpyAsync(counters + 1, &one, 4, cudaMemcpyHostToDevice, stream));
-        }
-        BB_CK(cudaStreamSynchronize(stream));   // the host values above go out of scope
-    }
     a.nextCount = counters;
     a.small = small;
     a.smallCount = counters + 1;
-    int levelCount = n > SMALL_NODE ? 1 : 0, cur = 0;
+    a.nextTasks = big[0];
+    k_seed_roots<<<blocksFor(B, 128), 128, 0, stream>>>(a, sg);
+    int levelCount = 0, cur = 0;
+    for (int s = 0; s < B; s++) levelCount += fragCount[s] > (unsigned long long)SMALL_NODE;
     int hostCounters[2] = {0, 0};
     while (levelCount > 0) {
         a.tasks = big[cur];
@@ -890,156 +1069,133 @@ static int build_device(cudaStream_t stream, const PackedVec3* pos, const GpuBla
     tm.mark("tree (small)");
 
     // ---- 4. post passes
-    GpuBlasNode hRoot;
-    BB_CK(cudaMemcpyAsync(&hRoot, a.nodes + 1, sizeof(hRoot), cudaMemcpyDeviceToHost, stream));
-    BB_CK(cudaStreamSynchronize(stream));
-    const bool rootLeaf = hRoot.TriCount > 0;
-    if (rootLeaf) k_root_duplicate<<<1, 1, 0, stream>>>(a.nodes, a.parent, a.depth, a.ostart, a.ocount, n);
-
+    k_root_duplicate<<<blocksFor(B, 128), 128, 0, stream>>>(a.nodes, a.parent, a.depth, a.ostart, a.ocount, sg);
     int *g, *arrive;
     BB_CK(ar.get(g, cap));
     BB_CK(ar.get(arrive, cap));
     BB_CK(cudaMemsetAsync(arrive, 0, (size_t)cap * sizeof(int), stream));
     k_stack_size<<<blocksFor(cap, 256), 256, 0, stream>>>(a.nodes, a.parent, a.depth, cap, g, arrive);
-    int requiredStackSize = 0;
-    BB_CK(cudaMemcpyAsync(&requiredStackSize, g + 1, 4, cudaMemcpyDeviceToHost, stream));
 
-    // pre-order of every node of the built tree
-    int* order;
-    int m = 0;
+    // pre-order of every node of the built trees, BLAS after BLAS
+    int *order, *dmin, *dleaf, *len, *base, *dStack;
     BB_CK(ar.get(order, cap));
-    if (rootLeaf) {
-        k_preorder_root_duplicate<<<1, 1, 0, stream>>>(order);
-        m = 3;
-    } else {
-        int *dmin, *dleaf, *len, *base;
-        BB_CK(ar.get(dmin, n));
-        BB_CK(ar.get(dleaf, n));
-        BB_CK(ar.get(len, n + 1));
-        BB_CK(ar.get(base, n + 1));
-        BB_CK(cudaMemsetAsync(dmin, 0x7F, (size_t)n * sizeof(int), stream));   // DEPTH_NONE
-        k_chain_ends<<<blocksFor(cap, 256), 256, 0, stream>>>(a.nodes, a.depth, a.ostart, cap, dmin, dleaf);
-        k_chain_len<<<blocksFor(n, 256), 256, 0, stream>>>(dmin, dleaf, n, len);
-        BB_CK(cudaMemsetAsync(len + n, 0, sizeof(int), stream));
-        size_t need = 0;
-        BB_CK(cub::DeviceScan::ExclusiveSum(nullptr, need, len, base, n + 1, stream));
-        BB_CK(cubScratch(need));
-        BB_CK(cub::DeviceScan::ExclusiveSum(cubTemp, need, len, base, n + 1, stream));
-        k_preorder<<<blocksFor(cap, 256), 256, 0, stream>>>(a.depth, a.ostart, cap, dmin, base, order);
-        BB_CK(cudaMemcpyAsync(&m, base + n, 4, cudaMemcpyDeviceToHost, stream));
-    }
+    BB_CK(ar.get(dmin, n));
+    BB_CK(ar.get(dleaf, n));
+    BB_CK(ar.get(len, n + 1));
+    BB_CK(ar.get(base, n + 1));
+    BB_CK(ar.get(dStack, B));
+    BB_CK(cudaMemsetAsync(dmin, 0x7F, (size_t)n * sizeof(int), stream));   // DEPTH_NONE
+    BB_CK(cudaMemsetAsync(dleaf, 0, (size_t)n * sizeof(int), stream));
+    k_chain_ends<<<blocksFor(cap, 256), 256, 0, stream>>>(a.nodes, a.parent, a.depth, a.ostart, cap, dmin, dleaf);
+    k_chain_len<<<blocksFor(n, 256), 256, 0, stream>>>(dmin, dleaf, n, len);
+    BB_CK(cudaMemsetAsync(len + n, 0, sizeof(int), stream));
+    BB_CK(exclusiveSum(len, base, n + 1));
+    k_preorder<<<blocksFor(cap, 256), 256, 0, stream>>>(a.nodes, a.parent, a.depth, a.ostart, cap, dmin, base, order);
+    k_order_info<<<blocksFor(B + 1, 256), 256, 0, stream>>>(base, g, sg, dOrder, dStack);
+    BB_CK(cudaMemcpyAsync(hOrder.data(), dOrder, (B + 1) * sizeof(int), cudaMemcpyDeviceToHost, stream));
+    BB_CK(cudaMemcpyAsync(hStack.data(), dStack, B * sizeof(int), cudaMemcpyDeviceToHost, stream));
     BB_CK(cudaStreamSynchronize(stream));
+    const int m = hOrder[B];
     tm.mark("stack size");
 
     double* terms;
-    double* acc;   // [0]: SAH of the built tree, [1]: added collapse cost, [2]: final SAH
+    double* acc;   // per BLAS: [0, B) SAH of the built tree, [B, 2B) added collapse cost, [2B, 3B) final SAH
     double* packed;
-    uint8_t* flags;
-    int* selCount;
+    int *flags, *scan;
     BB_CK(ar.get(terms, cap));
     BB_CK(ar.get(packed, cap));
-    BB_CK(keep.get(acc, 3));
-    BB_CK(ar.get(flags, cap));
-    BB_CK(ar.get(selCount, 1));
-    BB_CK(cudaMemsetAsync(acc, 0, 3 * sizeof(double), stream));
-    auto flaggedSum = [&](double* dst) -> int {   // dst += the flagged terms, in order
-        size_t need = 0;
-        BB_CK(cub::DeviceSelect::Flagged(nullptr, need, terms, flags, packed, selCount, m, stream));
-        BB_CK(cubScratch(need));
-        BB_CK(cub::DeviceSelect::Flagged(cubTemp, need, terms, flags, packed, selCount, m, stream));
-        k_ordered_sum<double, 4096><<<1, SUM_THREADS, 0, stream>>>(packed, 0, selCount, dst);
-        return BB_OK;
-    };
+    BB_CK(ar.get(acc, 3 * (size_t)B));
+    BB_CK(ar.get(flags, cap + 1));
+    BB_CK(ar.get(scan, cap + 1));
+    BB_CK(cudaMemsetAsync(acc, 0, 3 * (size_t)B * sizeof(double), stream));
 
-    // OptimizeStackSize
-    int maxDepth = INT_MAX;   // nodes deeper than this are gone after the collapse passes
-    if (requiredStackSize >= p.stackOptThreshold) {
-        k_sah_terms<<<blocksFor(m, 256), 256, 0, stream>>>(order, m, a.nodes, nullptr, nullptr, p.triangleCost, terms);
-        k_ordered_sum<double, 4096><<<1, SUM_THREADS, 0, stream>>>(terms, m, nullptr, acc + 0);
-        k_collapse_terms<<<blocksFor(m, 256), 256, 0, stream>>>(order, m, a.nodes, a.depth, a.ocount, requiredStackSize - 1, 1,
-                                                                 p.triangleCost, terms, flags);
-        if (int rc = flaggedSum(acc + 1)) return rc;
-        double h[2];
-        BB_CK(cudaMemcpyAsync(h, acc, sizeof(h), cudaMemcpyDeviceToHost, stream));
+    // OptimizeStackSize, in rounds: a BLAS whose RequiredStackSize reaches the threshold takes part from the first round,
+    // which adds the first pass's collapse cost, and leaves the rounds when its next pass is not accepted. One host read
+    // per round for the whole batch. (No collapse of at most 2^24 fragments exceeds STACK_OPT_MAX_LEAF_TRIANGLE_COUNT, so
+    // that test is not made here.)
+    bool collapsing = false, collapsed = false;
+    for (int s = 0; s < B; s++) {
+        if (hStack[s] >= p.stackOptThreshold) { hPass[s] = 1; hLevel[s] = hStack[s] - 1; collapsing = true; }
+    }
+    if (collapsing) {
+        BB_CK(up(dPass, hPass));
+        k_sah_terms<<<blocksFor(m, 256), 256, 0, stream>>>(order, m, sg, a.nodes, nullptr, nullptr, p.triangleCost, terms);
+        k_ordered_sum<double, 4096><<<B, SUM_THREADS, 0, stream>>>(terms, dOrder, nullptr, dPass, acc);
+    }
+    std::vector<double> hAcc(2 * (size_t)B);
+    while (collapsing) {
+        BB_CK(up(dPass, hPass));
+        BB_CK(up(dLevel, hLevel));
+        k_collapse_terms<<<blocksFor(m + 1, 256), 256, 0, stream>>>(order, m, sg, a.nodes, a.depth, a.ocount, p.triangleCost, terms, flags);
+        BB_CK(exclusiveSum(flags, scan, m + 1));
+        k_pack<<<blocksFor(m, 256), 256, 0, stream>>>(terms, flags, scan, m, packed);
+        k_ordered_sum<double, 4096><<<B, SUM_THREADS, 0, stream>>>(packed, dOrder, scan, dPass, acc + B);
+        BB_CK(cudaMemcpyAsync(hAcc.data(), acc, hAcc.size() * sizeof(double), cudaMemcpyDeviceToHost, stream));
         BB_CK(cudaStreamSynchronize(stream));
-        // (no collapse of at most 2^24 fragments exceeds STACK_OPT_MAX_LEAF_TRIANGLE_COUNT, so that test is not made here)
-        double increasePercent = h[1] / h[0];
-        while (increasePercent <= (double)p.stackOptSahIncreaseAcceptance && requiredStackSize > 0) {
-            const int level = --requiredStackSize;
-            maxDepth = level + 1;
-            k_collapse_terms<<<blocksFor(m, 256), 256, 0, stream>>>(order, m, a.nodes, a.depth, a.ocount, level, 0,
-                                                                     p.triangleCost, terms, flags);
-            if (int rc = flaggedSum(acc + 1)) return rc;
-            BB_CK(cudaMemcpyAsync(h, acc, sizeof(h), cudaMemcpyDeviceToHost, stream));
-            BB_CK(cudaStreamSynchronize(stream));
-            increasePercent = h[1] / h[0];
+        collapsing = false;
+        for (int s = 0; s < B; s++) {
+            if (!hPass[s]) continue;
+            const double increasePercent = hAcc[B + s] / hAcc[s];
+            if (increasePercent <= (double)p.stackOptSahIncreaseAcceptance && hStack[s] > 0) {
+                hLevel[s] = --hStack[s];
+                hMaxDepth[s] = hLevel[s] + 1;
+                hPass[s] = 2;
+                collapsing = collapsed = true;
+            } else {
+                hPass[s] = 0;
+            }
         }
     }
+    BB_CK(up(dMaxDepth, hMaxDepth));
     tm.mark("stack opt");
 
     // removeEmptySubtrees: the nodes left after the collapse, in pre-order
     int* order2 = order;
-    int m2 = m;
-    if (maxDepth != INT_MAX) {
+    int* dOrder2 = dOrder;
+    std::vector<int> hOrder2 = hOrder;
+    if (collapsed) {
         BB_CK(ar.get(order2, m));
-        k_reachable<<<blocksFor(m, 256), 256, 0, stream>>>(order, m, a.depth, maxDepth, flags);
-        size_t need = 0;
-        BB_CK(cub::DeviceSelect::Flagged(nullptr, need, order, flags, order2, selCount, m, stream));
-        BB_CK(cubScratch(need));
-        BB_CK(cub::DeviceSelect::Flagged(cubTemp, need, order, flags, order2, selCount, m, stream));
-        BB_CK(cudaMemcpyAsync(&m2, selCount, 4, cudaMemcpyDeviceToHost, stream));
+        BB_CK(ar.get(dOrder2, B + 1));
+        k_reachable<<<blocksFor(m + 1, 256), 256, 0, stream>>>(order, m, sg, a.depth, flags);
+        BB_CK(exclusiveSum(flags, scan, m + 1));
+        k_pack<<<blocksFor(m, 256), 256, 0, stream>>>(order, flags, scan, m, order2);
+        k_gather<<<blocksFor(B + 1, 256), 256, 0, stream>>>(scan, dOrder, B + 1, dOrder2);
+        BB_CK(cudaMemcpyAsync(hOrder2.data(), dOrder2, (B + 1) * sizeof(int), cudaMemcpyDeviceToHost, stream));
         BB_CK(cudaStreamSynchronize(stream));
     }
-    int *innerFlag, *innerScan, *rankOf, *fidx;
-    BB_CK(ar.get(innerFlag, m2 + 1));
-    BB_CK(ar.get(innerScan, m2 + 1));
+    const int m2 = hOrder2[B];
+    Segs sg2 = sg;
+    sg2.order = dOrder2;
+    int *rankOf, *fidx, *innerStart;
     BB_CK(ar.get(rankOf, cap));
     BB_CK(ar.get(fidx, cap));
-    k_inner_flags<<<blocksFor(m2, 256), 256, 0, stream>>>(order2, m2, a.nodes, a.depth, maxDepth, innerFlag);
-    BB_CK(cudaMemsetAsync(innerFlag + m2, 0, sizeof(int), stream));
-    {
-        size_t need = 0;
-        BB_CK(cub::DeviceScan::ExclusiveSum(nullptr, need, innerFlag, innerScan, m2 + 1, stream));
-        BB_CK(cubScratch(need));
-        BB_CK(cub::DeviceScan::ExclusiveSum(cubTemp, need, innerFlag, innerScan, m2 + 1, stream));
-    }
-    int inner = 0;
-    BB_CK(cudaMemcpyAsync(&inner, innerScan + m2, 4, cudaMemcpyDeviceToHost, stream));
+    BB_CK(ar.get(innerStart, B + 1));
+    k_inner_flags<<<blocksFor(m2 + 1, 256), 256, 0, stream>>>(order2, m2, sg2, a.nodes, a.depth, flags);
+    BB_CK(exclusiveSum(flags, scan, m2 + 1));
+    k_gather<<<blocksFor(B + 1, 256), 256, 0, stream>>>(scan, dOrder2, B + 1, innerStart);
+    std::vector<int> hInner(B + 1);
+    BB_CK(cudaMemcpyAsync(hInner.data(), innerStart, (B + 1) * sizeof(int), cudaMemcpyDeviceToHost, stream));
     BB_CK(cudaStreamSynchronize(stream));
-    k_inner_ranks<<<blocksFor(m2, 256), 256, 0, stream>>>(order2, m2, innerScan, rankOf);
-    const int f = 2 + 2 * inner;
+    k_inner_ranks<<<blocksFor(m2, 256), 256, 0, stream>>>(order2, m2, sg2, scan, rankOf);
+    for (int s = 0; s < B; s++) hFinal[s + 1] = hFinal[s] + 2 + 2 * (hInner[s + 1] - hInner[s]);
+    BB_CK(up(dFinal, hFinal));
+    const int f = hFinal[B];
     GpuBlasNode* final;
     BB_CK(keep.get(final, f));
-    BB_CK(cudaMemsetAsync(final, 0, sizeof(GpuBlasNode) * 2, stream));
-    k_final_nodes<<<blocksFor(m2, 256), 256, 0, stream>>>(order2, m2, a.nodes, a.parent, a.depth, a.ostart, a.ocount, rankOf,
-                                                          maxDepth, final, fidx);
+    k_final_nodes<<<blocksFor(m2, 256), 256, 0, stream>>>(order2, m2, sg2, a.nodes, a.parent, a.depth, a.ostart, a.ocount, rankOf, final, fidx);
     tm.mark("compact");
 
-    // unindexing
-    GpuBlasTriangle* outTris;
-    BB_CK(keep.get(outTris, n));
-    int triOut = n;
-    if (!p.doPreSplit) {
-        int *cnt, *off;
-        BB_CK(ar.get(cnt, f));
-        BB_CK(ar.get(off, f));
-        k_leaf_counts<<<blocksFor(f, 256), 256, 0, stream>>>(final, f, cnt);
-        size_t need = 0;
-        BB_CK(cub::DeviceScan::ExclusiveSum(nullptr, need, cnt, off, f, stream));
-        BB_CK(cubScratch(need));
-        BB_CK(cub::DeviceScan::ExclusiveSum(cubTemp, need, cnt, off, f, stream));
-        k_unindex_plain<<<blocksFor(f, 256), 256, 0, stream>>>(final, f, off, a.ids[0], tris, outTris, n);
-    } else {
-        int *marks, *segStart, *sizes, *off;
-        unsigned long long *keys, *keysSorted;
+    // unindexing: per output node its triangle count, one scan, then the triangles
+    unsigned long long* keysSorted = nullptr;
+    if (anyPre) {
+        int *marks, *segStart;
+        unsigned long long* keys;
         BB_CK(ar.get(marks, n));
         BB_CK(ar.get(segStart, n));
         BB_CK(ar.get(keys, n));
         BB_CK(ar.get(keysSorted, n));
-        BB_CK(ar.get(sizes, inner + 1));
-        BB_CK(ar.get(off, inner + 1));
         BB_CK(cudaMemsetAsync(marks, 0, (size_t)n * sizeof(int), stream));
-        k_leaf_marks<<<blocksFor(f, 256), 256, 0, stream>>>(final, f, marks);
+        k_leaf_marks<<<blocksFor(f, 256), 256, 0, stream>>>(final, f, sg2, marks);
         size_t need = 0;
         BB_CK(cub::DeviceScan::InclusiveScan(nullptr, need, marks, segStart, MaxOp(), n, stream));
         BB_CK(cubScratch(need));
@@ -1051,35 +1207,43 @@ static int build_device(cudaStream_t stream, const PackedVec3* pos, const GpuBla
         BB_CK(cub::DeviceRadixSort::SortKeys(nullptr, need, keys, keysSorted, n, 0, endBit, stream));
         BB_CK(cubScratch(need));
         BB_CK(cub::DeviceRadixSort::SortKeys(cubTemp, need, keys, keysSorted, n, 0, endBit, stream));
-        k_pair_sizes<<<blocksFor(inner + 1, 256), 256, 0, stream>>>(final, inner, keysSorted, sizes);
-        need = 0;
-        BB_CK(cub::DeviceScan::ExclusiveSum(nullptr, need, sizes, off, inner + 1, stream));
-        BB_CK(cubScratch(need));
-        BB_CK(cub::DeviceScan::ExclusiveSum(cubTemp, need, sizes, off, inner + 1, stream));
-        k_pair_write<<<blocksFor(inner, 256), 256, 0, stream>>>(final, inner, keysSorted, off, tris, outTris);
-        BB_CK(cudaMemcpyAsync(&triOut, off + inner, 4, cudaMemcpyDeviceToHost, stream));
     }
+    int *cnt, *off, *triStart;
+    BB_CK(ar.get(cnt, (size_t)f + 1));
+    BB_CK(ar.get(off, (size_t)f + 1));
+    BB_CK(ar.get(triStart, B + 1));
+    k_tri_counts<<<blocksFor(f + 1, 256), 256, 0, stream>>>(final, f, sg2, keysSorted, cnt);
+    BB_CK(exclusiveSum(cnt, off, f + 1));
+    k_gather<<<blocksFor(B + 1, 256), 256, 0, stream>>>(off, dFinal, B + 1, triStart);
+    out.triStart.assign(B + 1, 0);
+    BB_CK(cudaMemcpyAsync(out.triStart.data(), triStart, (B + 1) * sizeof(int), cudaMemcpyDeviceToHost, stream));
+    BB_CK(cudaStreamSynchronize(stream));
+    GpuBlasTriangle* outTris;
+    BB_CK(keep.get(outTris, out.triStart[B]));
+    k_unindex<<<blocksFor(f, 256), 256, 0, stream>>>(final, f, sg2, off, a.ids[0], origIds, keysSorted, tris, outTris);
     tm.mark("unindex");
 
-    k_sah_terms<<<blocksFor(m2, 256), 256, 0, stream>>>(order2, m2, nullptr, final, fidx, p.triangleCost, terms);
-    k_ordered_sum<double, 4096><<<1, SUM_THREADS, 0, stream>>>(terms, m2, nullptr, acc + 2);
+    k_sah_terms<<<blocksFor(m2, 256), 256, 0, stream>>>(order2, m2, sg2, nullptr, final, fidx, p.triangleCost, terms);
+    k_ordered_sum<double, 4096><<<B, SUM_THREADS, 0, stream>>>(terms, dOrder2, nullptr, nullptr, acc + 2 * B);
+    out.sah.assign(B, 0.0);
+    BB_CK(cudaMemcpyAsync(out.sah.data(), acc + 2 * B, B * sizeof(double), cudaMemcpyDeviceToHost, stream));
     tm.mark("sah");
     BB_CK(cudaGetLastError());
     BB_CK(cudaStreamSynchronize(stream));
     out.nodes = final;
-    out.nodeCount = f;
     out.tris = outTris;
-    out.triCount = triOut;
-    out.requiredStackSize = requiredStackSize;
-    out.fragmentCount = n;
-    out.sah = acc + 2;
+    out.nodeStart = hFinal;
+    out.requiredStackSize = hStack;
+    out.fragmentCount.resize(B);
+    for (int s = 0; s < B; s++) out.fragmentCount[s] = (int)fragCount[s];
     return BB_OK;
 }
 
-// idkpt_blas_build: build_device between an upload of the host arrays and a download of its result. Fills `out` and the
-// total device time.
-static int build(cudaStream_t stream, const PackedVec3* hPos, uint64_t vertexCount, const GpuBlasTriangle* hTris, int triCount,
-                 const Params& p, IdkPtBlasBuild& out, float& totalMs, std::string& err) {
+// idkpt_blas_build and idkpt_blas_build_batch: build_device between an upload of the host arrays and a download of its
+// result. Fills `out` (descs from `descs`, whose other fields are kept) and the total device time.
+static int build(cudaStream_t stream, const PackedVec3* hPos, uint64_t vertexCount, const GpuBlasTriangle* hTris, uint64_t triCount,
+                 const std::vector<Input>& in, const std::vector<GpuBlasDesc>& descs, const Params& p, IdkPtBlasBuild& out,
+                 float& totalMs, std::string& err) {
     Arena ar;
     StageTimer tm(stream);
     tm.mark("start");
@@ -1088,22 +1252,33 @@ static int build(cudaStream_t stream, const PackedVec3* hPos, uint64_t vertexCou
     BB_CK(ar.get(pos, vertexCount));
     BB_CK(ar.get(tris, triCount));
     BB_CK(cudaMemcpyAsync(pos, hPos, vertexCount * sizeof(PackedVec3), cudaMemcpyHostToDevice, stream));
-    BB_CK(cudaMemcpyAsync(tris, hTris, (size_t)triCount * sizeof(GpuBlasTriangle), cudaMemcpyHostToDevice, stream));
+    BB_CK(cudaMemcpyAsync(tris, hTris, triCount * sizeof(GpuBlasTriangle), cudaMemcpyHostToDevice, stream));
     tm.mark("upload");
     DeviceResult r;
-    if (int rc = build_device(stream, pos, tris, triCount, p, ar, r, tm, err)) return rc;
+    if (int rc = build_device(stream, pos, tris, in, p, ar, r, tm, err)) return rc;
 
-    out.nodes.resize(r.nodeCount);
-    out.tris.resize(r.triCount);
-    BB_CK(cudaMemcpyAsync(out.nodes.data(), r.nodes, (size_t)r.nodeCount * sizeof(GpuBlasNode), cudaMemcpyDeviceToHost, stream));
-    if (r.triCount) BB_CK(cudaMemcpyAsync(out.tris.data(), r.tris, (size_t)r.triCount * sizeof(GpuBlasTriangle), cudaMemcpyDeviceToHost, stream));
-    BB_CK(cudaMemcpyAsync(&out.sah, r.sah, sizeof(double), cudaMemcpyDeviceToHost, stream));
+    const size_t B = in.size();
+    out.nodes.resize(r.nodeStart[B]);
+    out.tris.resize(r.triStart[B]);
+    BB_CK(cudaMemcpyAsync(out.nodes.data(), r.nodes, out.nodes.size() * sizeof(GpuBlasNode), cudaMemcpyDeviceToHost, stream));
+    if (!out.tris.empty()) BB_CK(cudaMemcpyAsync(out.tris.data(), r.tris, out.tris.size() * sizeof(GpuBlasTriangle), cudaMemcpyDeviceToHost, stream));
     tm.mark("download");
     BB_CK(cudaStreamSynchronize(stream));
-    out.requiredStackSize = r.requiredStackSize;
-    out.fragmentCount = r.fragmentCount;
+    out.descs = descs;
+    for (size_t s = 0; s < B; s++) {
+        GpuBlasDesc& d = out.descs[s];
+        d.NodeOffset = r.nodeStart[s];
+        d.NodeCount = r.nodeStart[s + 1] - r.nodeStart[s];
+        d.TriangleOffset = r.triStart[s];
+        d.TriangleCount = r.triStart[s + 1] - r.triStart[s];
+        d.RequiredStackSize = r.requiredStackSize[s];
+    }
+    out.fragmentCounts = r.fragmentCount;
+    out.sahs = r.sah;
     totalMs = tm.total();
-    tm.print(r.fragmentCount);
+    long long fragments = 0;
+    for (int c : r.fragmentCount) fragments += c;
+    tm.print((int)B, fragments);
     return BB_OK;
 }
 

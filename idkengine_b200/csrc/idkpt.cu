@@ -2005,7 +2005,14 @@ IDKPT_API int idkpt_tlas_build(IdkPtCtx* ctx, int32_t searchRadius, float* kerne
     return IDKPT_OK;
 }
 
-// BLAS.Build + PreSplitting.PreSplit on the device (BVH.BlasesBuild's loop body, BVH.cs:315-377): see idk_blas_build.cuh.
+// idkbb::build's status as the library's
+static int blas_build_fail(IdkPtCtx* ctx, const char* who, int rc, const std::string& err) {
+    if (rc == idkbb::BB_CUDA) cudaStreamSynchronize(ctx->stream);
+    return fail(ctx, who, rc == idkbb::BB_CUDA ? IDKPT_ERR_CUDA : IDKPT_ERR_UNSUPPORTED, err.c_str());
+}
+
+// BLAS.Build + PreSplitting.PreSplit on the device (BVH.BlasesBuild's loop body, BVH.cs:315-377): a batch of one, see
+// idk_blas_build.cuh.
 IDKPT_API int idkpt_blas_build(IdkPtCtx* ctx, const PackedVec3* positions, uint64_t vertexCount, const GpuBlasTriangle* triangles,
                                uint64_t triangleCount, const IdkPtBlasBuildSettings* settings, IdkPtBlasBuild** out, float* kernelMs) {
     if (!ctx) return IDKPT_ERR_INVALID_ARGUMENT;
@@ -2027,25 +2034,80 @@ IDKPT_API int idkpt_blas_build(IdkPtCtx* ctx, const PackedVec3* positions, uint6
     IdkPtBlasBuild* b = new IdkPtBlasBuild();
     std::string err;
     float ms = 0.0f;
-    const int rc = idkbb::build(ctx->stream, positions, vertexCount, triangles, (int)triangleCount, p, *b, ms, err);
+    const std::vector<idkbb::Input> in = {{0, (int)triangleCount, p.doPreSplit}};
+    const int rc = idkbb::build(ctx->stream, positions, vertexCount, triangles, triangleCount, in, std::vector<GpuBlasDesc>(1), p, *b, ms, err);
     if (rc != idkbb::BB_OK) {
         delete b;
-        if (rc == idkbb::BB_CUDA) cudaStreamSynchronize(ctx->stream);
-        return fail(ctx, "idkpt_blas_build", rc == idkbb::BB_TOO_MANY_FRAGMENTS ? IDKPT_ERR_UNSUPPORTED : IDKPT_ERR_CUDA, err.c_str());
+        return blas_build_fail(ctx, "idkpt_blas_build", rc, err);
     }
     *out = b;
     if (kernelMs) *kernelMs = ms;
     return IDKPT_OK;
 }
 
+// BVH.BlasesBuild's parallel loop (BVH.cs:315-377) as one batch: see idk_blas_build.cuh.
+IDKPT_API int idkpt_blas_build_batch(IdkPtCtx* ctx, const PackedVec3* positions, uint64_t vertexCount, const GpuBlasTriangle* triangles,
+                                     uint64_t triangleCount, const GpuBlasDesc* descs, uint32_t descCount,
+                                     const IdkPtBlasBuildSettings* settings, IdkPtBlasBuild** out, float* kernelMs) {
+    const char* who = "idkpt_blas_build_batch";
+    if (!ctx) return IDKPT_ERR_INVALID_ARGUMENT;
+    if (out) *out = nullptr;
+    if (kernelMs) *kernelMs = 0.0f;
+    if (!positions || !triangles || !descs || !out) return fail(ctx, who, IDKPT_ERR_INVALID_ARGUMENT, "null argument");
+    if (descCount == 0) return fail(ctx, who, IDKPT_ERR_INVALID_ARGUMENT, "no BLASes");
+    idkbvh::Params p;
+    if (int rc = blas_build_params(ctx, who, settings, p)) return rc;
+    std::vector<idkbb::Input> in(descCount);
+    std::vector<int> counts(descCount);
+    for (uint32_t s = 0; s < descCount; s++) {
+        const GpuBlasDesc& d = descs[s];
+        if (d.TriangleCount <= 0) return fail(ctx, who, IDKPT_ERR_INVALID_ARGUMENT, "a BLAS without triangles");
+        if (d.TriangleOffset < 0 || (uint64_t)d.TriangleOffset + (uint64_t)d.TriangleCount > triangleCount)
+            return fail(ctx, who, IDKPT_ERR_INVALID_ARGUMENT, "GpuBlasDesc triangle range outside the array");
+        if (d.TriangleCount > idkbb::MAX_FRAGMENTS) return fail(ctx, who, IDKPT_ERR_UNSUPPORTED, "a BLAS of more than 2^24 triangles");
+        in[s] = {d.TriangleOffset, d.TriangleCount, d.IsRefittable ? 0 : 1};   // BVH.cs:325
+        counts[s] = d.TriangleCount;
+    }
+    if (idkbb::nodeIdCount(counts, descCount) < 0) return fail(ctx, who, IDKPT_ERR_UNSUPPORTED, "the batch needs 2^31 or more node ids");
+    for (uint32_t s = 0; s < descCount; s++) {
+        for (int i = 0; i < descs[s].TriangleCount; i++) {
+            const GpuBlasTriangle& t = triangles[(size_t)descs[s].TriangleOffset + i];
+            if ((uint64_t)(uint32_t)t.X >= vertexCount || (uint64_t)(uint32_t)t.Y >= vertexCount || (uint64_t)(uint32_t)t.Z >= vertexCount)
+                return fail(ctx, who, IDKPT_ERR_INVALID_ARGUMENT, "vertex id out of range");
+        }
+    }
+    DRAIN_PENDING("idkpt_blas_build_batch");
+    CK(cudaSetDevice(ctx->device));
+    IdkPtBlasBuild* b = new IdkPtBlasBuild();
+    std::string err;
+    float ms = 0.0f;
+    const int rc = idkbb::build(ctx->stream, positions, vertexCount, triangles, triangleCount, in,
+                                std::vector<GpuBlasDesc>(descs, descs + descCount), p, *b, ms, err);
+    if (rc != idkbb::BB_OK) {
+        delete b;
+        return blas_build_fail(ctx, who, rc, err);
+    }
+    *out = b;
+    if (kernelMs) *kernelMs = ms;
+    return IDKPT_OK;
+}
+
+// Totals over the batch: the largest RequiredStackSize (BVH.UpdateBlasStackSize) and the SAHs added in BLAS order.
 IDKPT_API int idkpt_blas_build_info(const IdkPtBlasBuild* b, uint64_t* nodeCount, uint64_t* triangleCount, int32_t* requiredStackSize,
                                     int32_t* fragmentCount, double* sah) {
     if (!b) return IDKPT_ERR_INVALID_ARGUMENT;
+    int32_t stack = 0, fragments = 0;
+    double total = 0.0;
+    for (size_t s = 0; s < b->descs.size(); s++) {
+        stack = std::max(stack, b->descs[s].RequiredStackSize);
+        fragments += b->fragmentCounts[s];
+        total += b->sahs[s];
+    }
     if (nodeCount) *nodeCount = b->nodes.size();
     if (triangleCount) *triangleCount = b->tris.size();
-    if (requiredStackSize) *requiredStackSize = b->requiredStackSize;
-    if (fragmentCount) *fragmentCount = b->fragmentCount;
-    if (sah) *sah = b->sah;
+    if (requiredStackSize) *requiredStackSize = stack;
+    if (fragmentCount) *fragmentCount = fragments;
+    if (sah) *sah = total;
     return IDKPT_OK;
 }
 
@@ -2056,13 +2118,25 @@ IDKPT_API int idkpt_blas_build_copy(const IdkPtBlasBuild* b, GpuBlasNode* nodes,
     return IDKPT_OK;
 }
 
+IDKPT_API int idkpt_blas_build_batch_copy(const IdkPtBlasBuild* b, GpuBlasDesc* descs, GpuBlasNode* nodes, GpuBlasTriangle* triangles,
+                                          int32_t* fragmentCounts, double* sahs) {
+    if (!b) return IDKPT_ERR_INVALID_ARGUMENT;
+    const size_t B = b->descs.size();
+    if (descs) memcpy(descs, b->descs.data(), B * sizeof(GpuBlasDesc));
+    if (nodes) memcpy(nodes, b->nodes.data(), b->nodes.size() * sizeof(GpuBlasNode));
+    if (triangles) memcpy(triangles, b->tris.data(), b->tris.size() * sizeof(GpuBlasTriangle));
+    if (fragmentCounts) memcpy(fragmentCounts, b->fragmentCounts.data(), B * sizeof(int32_t));
+    if (sahs) memcpy(sahs, b->sahs.data(), B * sizeof(double));
+    return IDKPT_OK;
+}
+
 IDKPT_API void idkpt_blas_build_free(IdkPtBlasBuild* b) { delete b; }
 
 static int64_t nodes_end(const GpuBlasDesc& d) { return (int64_t)d.NodeOffset + d.NodeCount; }
 static int64_t triangles_end(const GpuBlasDesc& d) { return (int64_t)d.TriangleOffset + d.TriangleCount; }
 
-// BVH.BlasesBuild(first, count) (BVH.cs:300-470) on the scene in place: each BLAS of the range is built by idkbb::build_device
-// from its current triangle records and the device positions, into staging memory. When every build succeeded, the new nodes
+// BVH.BlasesBuild(first, count) (BVH.cs:300-470) on the scene in place: the BLASes of the range are built by one batched
+// idkbb::build_device from their current triangle records and the device positions, into staging memory. When it succeeded, the new nodes
 // and triangles replace the old ones in new allocations: the data before the range (up to the end of desc first - 1) and the
 // data after it move unchanged, and the descs from `first` on are repacked behind each other (BVH.cs:378-441).
 IDKPT_API int idkpt_blas_rebuild(IdkPtCtx* ctx, uint32_t first, uint32_t count, const IdkPtBlasBuildSettings* settings, float* kernelMs) {
@@ -2086,35 +2160,36 @@ IDKPT_API int idkpt_blas_rebuild(IdkPtCtx* ctx, uint32_t first, uint32_t count, 
     }
     if (nodes_end(old[nd - 1]) != (int64_t)ctx->counts.BlasNodeCount || triangles_end(old[nd - 1]) != (int64_t)ctx->counts.BlasTriangleCount)
         return fail(ctx, IDKPT_ERR_INVALID_ARGUMENT, "idkpt_blas_rebuild: the last BLAS does not end the node and triangle arrays");
-    for (uint32_t b = first; b < first + count; b++)
-        if (old[b].TriangleCount > idkbb::MAX_FRAGMENTS) return fail(ctx, IDKPT_ERR_UNSUPPORTED, "idkpt_blas_rebuild: a BLAS of more than 2^24 triangles");
+    std::vector<idkbb::Input> in(count);
+    for (uint32_t k = 0; k < count; k++) {
+        const GpuBlasDesc& d = old[first + k];
+        if (d.TriangleCount > idkbb::MAX_FRAGMENTS) return fail(ctx, IDKPT_ERR_UNSUPPORTED, "idkpt_blas_rebuild: a BLAS of more than 2^24 triangles");
+        in[k] = {d.TriangleOffset, d.TriangleCount, d.IsRefittable ? 0 : 1};   // BVH.cs:325
+    }
     CK(cudaSetDevice(ctx->device));
 
     std::vector<GpuBlasDesc> descs = old;
     idkbb::Arena staged;                                  // the rebuilt BLASes, until they are committed
-    std::vector<idkbb::DeviceResult> built(count);
+    idkbb::DeviceResult built;
     DevBuf bvh, tris, descBuf;                            // the new [nodes | triRec], triangles and descs
     struct Drop { DevBuf* b[3]; ~Drop() { for (DevBuf* x : b) release(*x); } } drop = {{&bvh, &tris, &descBuf}};
     size_t nodeBytes = 0, triRecBytes = 0;
     int stackSize = 0;
     int rc = run_timed(ctx, "idkpt_blas_rebuild", kernelMs, [&]() -> int {
+        idkbb::StageTimer tm(ctx->stream);
+        tm.mark("start");
+        std::string err;
+        const int brc = idkbb::build_device(ctx->stream, (const PackedVec3*)ctx->positions.p, (const GpuBlasTriangle*)ctx->blasTris.p,
+                                            in, p, staged, built, tm, err);
+        if (brc != idkbb::BB_OK) return blas_build_fail(ctx, "idkpt_blas_rebuild", brc, err);
+        long long fragments = 0;
+        for (int c : built.fragmentCount) fragments += c;
+        tm.print((int)count, fragments);
         for (uint32_t k = 0; k < count; k++) {
             GpuBlasDesc& d = descs[first + k];
-            idkbvh::Params bp = p;
-            bp.doPreSplit = d.IsRefittable ? 0 : 1;        // BVH.cs:325
-            idkbb::StageTimer tm(ctx->stream);
-            tm.mark("start");
-            std::string err;
-            const int brc = idkbb::build_device(ctx->stream, (const PackedVec3*)ctx->positions.p, (const GpuBlasTriangle*)ctx->blasTris.p + d.TriangleOffset,
-                                                d.TriangleCount, bp, staged, built[k], tm, err);
-            if (brc != idkbb::BB_OK) {
-                if (brc == idkbb::BB_CUDA) cudaStreamSynchronize(ctx->stream);
-                return fail(ctx, "idkpt_blas_rebuild", brc == idkbb::BB_TOO_MANY_FRAGMENTS ? IDKPT_ERR_UNSUPPORTED : IDKPT_ERR_CUDA, err.c_str());
-            }
-            tm.print(built[k].fragmentCount);
-            d.NodeCount = built[k].nodeCount;
-            d.TriangleCount = built[k].triCount;
-            d.RequiredStackSize = built[k].requiredStackSize;
+            d.NodeCount = built.nodeStart[k + 1] - built.nodeStart[k];
+            d.TriangleCount = built.triStart[k + 1] - built.triStart[k];
+            d.RequiredStackSize = built.requiredStackSize[k];
         }
         int64_t nodeEnd = 0, triEnd = 0;
         for (size_t i = first; i < nd; i++) {
@@ -2148,11 +2223,8 @@ IDKPT_API int idkpt_blas_rebuild(IdkPtCtx* ctx, uint32_t first, uint32_t count, 
         CK(d2d(nodesNew, nodesOld, (size_t)keepNodes * sizeof(GpuBlasNode)));
         CK(d2d(trisNew, trisOld, (size_t)keepTris * sizeof(GpuBlasTriangle)));
         CK(d2d(recNew, recOld, (size_t)keepTris * 64));
-        for (uint32_t k = 0; k < count; k++) {
-            const GpuBlasDesc& d = descs[first + k];
-            CK(d2d(nodesNew + d.NodeOffset, built[k].nodes, (size_t)d.NodeCount * sizeof(GpuBlasNode)));
-            CK(d2d(trisNew + d.TriangleOffset, built[k].tris, (size_t)d.TriangleCount * sizeof(GpuBlasTriangle)));
-        }
+        CK(d2d(nodesNew + r0.NodeOffset, built.nodes, (size_t)built.nodeStart[count] * sizeof(GpuBlasNode)));   // the batch's ranges
+        CK(d2d(trisNew + r0.TriangleOffset, built.tris, (size_t)built.triStart[count] * sizeof(GpuBlasTriangle)));  // are packed already
         CK(d2d(nodesNew + nodes_end(rl), nodesOld + oldEndN, (size_t)tailN * sizeof(GpuBlasNode)));
         CK(d2d(trisNew + triangles_end(rl), trisOld + oldEndT, (size_t)tailT * sizeof(GpuBlasTriangle)));
         CK(d2d(recNew + 4 * triangles_end(rl), recOld + 4 * oldEndT, (size_t)tailT * 64));

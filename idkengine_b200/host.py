@@ -263,12 +263,15 @@ class Scene:
         self.source_triangle_count = 0
         self.build_info = []
 
-    def add(self, *models, threads=None, cache_dir=None, blas_builder=None):
+    def add(self, *models, threads=None, cache_dir=None, blas_builder=None, blas_batch_builder=None):
         """ModelManager.Add (SRC/ModelManager.cs:128-213) + BVH.Add/BlasesBuild (SRC/Bvh/BVH.cs:236-276,300-451):
         one BLAS + one instance per model. cache_dir (or $IDKHOST_BVH_CACHE): directory of the on-disk BLAS cache.
         blas_builder: a function with build_blas's (positions, triangles, presplit=...) signature and result, e.g. the device
-        build PathTracer.BuildBlas; default the host build (with `threads`). Both build the same BLAS, so the cache is shared."""
+        build PathTracer.BuildBlas; default the host build (with `threads`). Both build the same BLAS, so the cache is shared.
+        blas_batch_builder: a function with PathTracer.BuildBlases's (positions, triangles, descs) signature and result; when
+        given, every model not found in the cache is built in one call of it, as BlasesBuild builds a load in one parallel loop."""
         cache_dir = cache_dir or os.environ.get("IDKHOST_BVH_CACHE") or None
+        pending = []   # per model: [source triangles, vertex / mesh / transform offsets, cache key and path, its BLAS or None]
         for m in models:
             v_off = len(self.positions)
             mesh_off = len(self.meshes)
@@ -301,7 +304,7 @@ class Scene:
             self.source_triangle_count += len(src)
 
             b = None
-            cache_path = None
+            key = cache_path = None
             if cache_dir is not None:     # skip the SweepSAH build when this exact model was built before
                 key = blas_source_key(m.positions, m.indices, m.tri_mesh, not m.refittable)
                 cache_path = os.path.join(cache_dir, f"{key:016x}.idkbvh")
@@ -311,19 +314,36 @@ class Scene:
                         b["triangles"][f] += v_off
                     b["triangles"]["MeshId"] += mesh_off
                     b["from_cache"] = True
-            if b is None:
+            if b is None and blas_batch_builder is None:
                 if blas_builder is None:
                     b = build_blas(self.positions, src, presplit=not m.refittable, threads=threads)
                 else:
                     b = blas_builder(self.positions, src, presplit=not m.refittable)
-                if cache_path is not None:
-                    rel = dict(b)
-                    rel["triangles"] = b["triangles"].copy()
-                    for f in ("X", "Y", "Z"):
-                        rel["triangles"][f] -= v_off
-                    rel["triangles"]["MeshId"] -= mesh_off
-                    os.makedirs(cache_dir, exist_ok=True)
-                    cache_save(cache_path, key, rel)
+            pending.append([src, v_off, mesh_off, transform_id, key, cache_path, b])
+
+        todo = [p for p in pending if p[-1] is None]
+        if todo:                          # one batch of every model the cache did not have
+            descs = np.zeros(len(todo), gt.GpuBlasDesc)
+            descs["TriangleCount"] = [len(p[0]) for p in todo]
+            descs["TriangleOffset"] = np.concatenate([[0], np.cumsum(descs["TriangleCount"])[:-1]])
+            descs["IsRefittable"] = [1 if m.refittable else 0 for m, p in zip(models, pending) if p[-1] is None]
+            r = blas_batch_builder(self.positions, np.concatenate([p[0] for p in todo]), descs)
+            for k, p in enumerate(todo):
+                d = r["descs"][k]
+                p[-1] = dict(nodes=r["nodes"][d["NodeOffset"]:d["NodeOffset"] + d["NodeCount"]],
+                            triangles=r["triangles"][d["TriangleOffset"]:d["TriangleOffset"] + d["TriangleCount"]],
+                            required_stack_size=int(d["RequiredStackSize"]), fragment_count=int(r["fragment_counts"][k]),
+                            sah=float(r["sahs"][k]))
+
+        for m, (src, v_off, mesh_off, transform_id, key, cache_path, b) in zip(models, pending):
+            if cache_path is not None and not b.get("from_cache", False):
+                rel = dict(b)
+                rel["triangles"] = b["triangles"].copy()
+                for f in ("X", "Y", "Z"):
+                    rel["triangles"][f] -= v_off
+                rel["triangles"]["MeshId"] -= mesh_off
+                os.makedirs(cache_dir, exist_ok=True)
+                cache_save(cache_path, key, rel)
             desc = np.zeros(1, gt.GpuBlasDesc)
             desc["NodeOffset"] = len(self.blas_nodes)
             desc["NodeCount"] = len(b["nodes"])

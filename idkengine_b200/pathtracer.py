@@ -201,6 +201,37 @@ class PathTracer:
         self.last_blas_build_ms = float(ms.value)
         return dict(nodes=nodes, triangles=tris, required_stack_size=int(stack.value), fragment_count=int(frags.value), sah=float(sah.value))
 
+    def BuildBlases(self, positions, triangles, descs, settings=None):
+        """BVH.BlasesBuild's loop (BVH.cs:315-377) over the BLASes of `descs` in one device call (idkpt_blas_build_batch): BLAS s
+        is built from triangles[TriangleOffset, +TriangleCount) and pre-split when not IsRefittable; only those desc fields
+        are read. settings as BuildBlas (DoPreSplit is ignored). Returns dict(descs, nodes, triangles, fragment_counts, sahs):
+        the descs as BVH.cs:363-386 fills them, with offsets into the concatenated nodes and triangles; each BLAS equal to
+        BuildBlas (and the host build) of it. The device time of the batch is left in `last_blas_build_ms`."""
+        positions = np.ascontiguousarray(positions)
+        triangles = np.ascontiguousarray(triangles)
+        descs = np.ascontiguousarray(descs)
+        assert positions.dtype == gt.PackedVec3 and triangles.dtype == gt.GpuBlasTriangle and descs.dtype == gt.GpuBlasDesc
+        s = self._blas_settings(settings)
+        h = ctypes.c_void_p()
+        ms = ctypes.c_float()
+        self._check(self._lib.idkpt_blas_build_batch(self._ctx, positions.ctypes.data, len(positions), triangles.ctypes.data, len(triangles),
+                                                     descs.ctypes.data, len(descs), ctypes.byref(s), ctypes.byref(h), ctypes.byref(ms)),
+                    "idkpt_blas_build_batch")
+        try:
+            nn, nt = ctypes.c_uint64(), ctypes.c_uint64()
+            self._check(self._lib.idkpt_blas_build_info(h, ctypes.byref(nn), ctypes.byref(nt), None, None, None), "idkpt_blas_build_info")
+            out_descs = np.zeros(len(descs), gt.GpuBlasDesc)
+            nodes = np.zeros(nn.value, gt.GpuBlasNode)
+            tris = np.zeros(nt.value, gt.GpuBlasTriangle)
+            frags = np.zeros(len(descs), np.int32)
+            sahs = np.zeros(len(descs), np.float64)
+            self._check(self._lib.idkpt_blas_build_batch_copy(h, out_descs.ctypes.data, nodes.ctypes.data, tris.ctypes.data,
+                                                              frags.ctypes.data, sahs.ctypes.data), "idkpt_blas_build_batch_copy")
+        finally:
+            self._lib.idkpt_blas_build_free(h)
+        self.last_blas_build_ms = float(ms.value)
+        return dict(descs=out_descs, nodes=nodes, triangles=tris, fragment_counts=frags, sahs=sahs)
+
     def SetTextures(self, textures):
         """Replace the material texture table (list of dict(pixels, srgb, wrap_s, wrap_t), as host.Scene.textures)."""
         arr, keep = capi.texture_descs(textures)

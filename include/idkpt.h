@@ -643,6 +643,33 @@ IDKPT_API int  idkpt_blas_build_info(const IdkPtBlasBuild* b, uint64_t* node_cou
 IDKPT_API int  idkpt_blas_build_copy(const IdkPtBlasBuild* b, GpuBlasNode* nodes, GpuBlasTriangle* triangles);
 IDKPT_API void idkpt_blas_build_free(IdkPtBlasBuild* b);
 
+/* BVH.BlasesBuild's parallel loop (BVH.cs:315-377) in one call: builds every BLAS of `descs` -- a model load's or a rebuild's --
+ * together on the device, each node for node and triangle for triangle equal to building it alone with idkpt_blas_build (and
+ * so to the host build), with the same required stack size, fragment count and SAH bits. Per desc only TriangleOffset,
+ * TriangleCount and IsRefittable are read: the BLAS's triangles are triangles[TriangleOffset, +TriangleCount), anywhere in
+ * the array, and it is pre-split exactly when !IsRefittable (BVH.cs:325); the settings' DoPreSplit is ignored. The batch
+ * pays for its launches and host synchronisations once, not once per BLAS, which is what makes a load of many small BLASes
+ * fast. Needs no scene and leaves the context's scene, sky and accumulation alone; synchronous, ordered after queued
+ * idkpt_compute samples.
+ * The handle works with idkpt_blas_build_info (totals: nodes, triangles, the largest RequiredStackSize as
+ * BVH.UpdateBlasStackSize takes it, fragments, and the BLASes' SAHs added in desc order as BVH.cs:460-468 logs them),
+ * idkpt_blas_build_copy (the BLASes' nodes and triangles one after another) and idkpt_blas_build_batch_copy.
+ * IDKPT_ERR_INVALID_ARGUMENT, before anything runs and with *out NULL: a NULL pointer, desc_count == 0, a desc without
+ * triangles or with a range outside `triangles`, a vertex id >= vertex_count in any BLAS, a non-finite setting, or
+ * StopSplittingThreshold < 1. IDKPT_ERR_UNSUPPORTED: more than 2^24 fragments in one BLAS after pre-splitting, or a batch
+ * whose node ids (the sum of max(2 * fragments, 4) over its BLASes) reach 2^31; both are found before any fragment is
+ * written. kernel_ms (may be NULL): device time of the whole batch, copies included. */
+IDKPT_API int idkpt_blas_build_batch(IdkPtCtx* ctx, const PackedVec3* positions, uint64_t vertex_count,
+                                     const GpuBlasTriangle* triangles, uint64_t triangle_count,
+                                     const GpuBlasDesc* descs, uint32_t desc_count,
+                                     const IdkPtBlasBuildSettings* settings /* NULL = defaults; DoPreSplit ignored */,
+                                     IdkPtBlasBuild** out, float* kernel_ms);
+/* Per BLAS of a batch (desc_count entries each): its desc as BVH.cs:363-386 fills it (NodeOffset and TriangleOffset from 0
+ * over the copied arrays, NodeCount, TriangleCount and RequiredStackSize from the build, the other fields as handed in), its
+ * fragment count and its SAH. nodes and triangles as idkpt_blas_build_copy. Any output pointer may be NULL. */
+IDKPT_API int idkpt_blas_build_batch_copy(const IdkPtBlasBuild* b, GpuBlasDesc* descs, GpuBlasNode* nodes,
+                                          GpuBlasTriangle* triangles, int32_t* fragment_counts, double* sahs);
+
 /* BVH.BlasesBuild(first, count) (BVH.cs:300-470) on the scene in place: rebuilds BLASes [first, first + count) from the scene's
  * current device arrays -- each BLAS's triangle records BlasTriangles[TriangleOffset, +TriangleCount) and the device vertex
  * positions, including whatever idkpt_skin_vertices last wrote -- with the same builder as idkpt_blas_build. Nothing is uploaded.
@@ -655,8 +682,8 @@ IDKPT_API void idkpt_blas_build_free(IdkPtBlasBuild* b);
  * becomes the largest RequiredStackSize (BVH.UpdateBlasStackSize). Everything else -- instances, transforms, meshes,
  * materials, textures, lights, sky, point-shadow maps, kept previous positions, raster images, TAA history -- stays. The TLAS
  * is not rebuilt, as after idkpt_blas_refit: call idkpt_tlas_build (or upload TLAS nodes) next. Resets the accumulation.
- * All or nothing: every BLAS is built into staging memory and committed only when all builds succeeded; a failed call leaves
- * every scene array, desc, the stack size and the image as they were. Synchronous, ordered after queued idkpt_compute samples.
+ * All or nothing: the BLASes are built as one batch (as idkpt_blas_build_batch builds them) into staging memory and committed
+ * only when the whole batch succeeded; a failed call leaves every scene array, desc, the stack size and the image as they were. Synchronous, ordered after queued idkpt_compute samples.
  * IDKPT_ERR_INVALID_ARGUMENT: a NULL context, first + count past the descs, a non-finite setting, StopSplittingThreshold < 1,
  * or a layout other than the one BlasesBuild and host.Scene.add produce (from `first` on each desc's nodes and triangles
  * start where the previous desc's end and the last desc ends both arrays; the descs before `first` end at or before the end

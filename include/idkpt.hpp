@@ -174,6 +174,32 @@ public:
         idkpt_blas_build_free(b);
         return r;
     }
+    // BVH.BlasesBuild's loop over `descs` in one device call (idkpt_blas_build_batch): each BLAS equal to BuildBlas of it
+    struct BlasBatchResult {
+        std::vector<GpuBlasDesc> descs;   // offsets into nodes / triangles, as BVH.cs:363-386 fills them
+        std::vector<GpuBlasNode> nodes;
+        std::vector<GpuBlasTriangle> triangles;
+        std::vector<int32_t> fragmentCounts;
+        std::vector<double> sahs;
+        float kernelMs = 0.0f;
+    };
+    BlasBatchResult BuildBlases(const PackedVec3* positions, uint64_t vertexCount, const GpuBlasTriangle* triangles, uint64_t triangleCount,
+                                const GpuBlasDesc* descs, uint32_t descCount, const IdkPtBlasBuildSettings* settings = nullptr) {
+        BlasBatchResult r;
+        IdkPtBlasBuild* b = nullptr;
+        check(idkpt_blas_build_batch(ctx_, positions, vertexCount, triangles, triangleCount, descs, descCount, settings, &b, &r.kernelMs),
+              "idkpt_blas_build_batch");
+        uint64_t nodeCount = 0, triCount = 0;
+        idkpt_blas_build_info(b, &nodeCount, &triCount, nullptr, nullptr, nullptr);
+        r.descs.resize(descCount);
+        r.nodes.resize(nodeCount);
+        r.triangles.resize(triCount);
+        r.fragmentCounts.resize(descCount);
+        r.sahs.resize(descCount);
+        idkpt_blas_build_batch_copy(b, r.descs.data(), r.nodes.data(), r.triangles.data(), r.fragmentCounts.data(), r.sahs.data());
+        idkpt_blas_build_free(b);
+        return r;
+    }
     float Denoise(const IdkPtDenoiseSettings& s) { float ms = 0.0f; check(idkpt_denoise(ctx_, &s, &ms), "idkpt_denoise"); return ms; }   // PathTracerPipeline.Denoise
     std::vector<float> Denoised() const { return read(IDKPT_IMAGE_DENOISED); }
     void RegisterHostBuffer(void* hostPtr, uint64_t bytes) { check(idkpt_register_host_buffer(ctx_, hostPtr, bytes), "idkpt_register_host_buffer"); }
