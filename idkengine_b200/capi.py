@@ -115,7 +115,7 @@ EXPORTS = [
     "idkpt_gbuffer", "idkpt_gbuffer_device_ptrs", "idkpt_read_gbuffer", "idkpt_prev_positions_device_ptr", "idkpt_transparency", "idkpt_lights_and_skybox",
     "idkpt_sky_atmosphere", "idkpt_sky_equirectangular", "idkpt_read_sky",
     "idkpt_blas_build", "idkpt_blas_build_info", "idkpt_blas_build_copy", "idkpt_blas_build_free", "idkpt_blas_rebuild", "idkpt_blas_sah",
-    "idkpt_blas_build_batch", "idkpt_blas_build_batch_copy",
+    "idkpt_blas_build_batch", "idkpt_blas_build_batch_copy", "idkpt_add_models",
 ]
 
 IDKPT_MAX_POINT_SHADOWS = 128
@@ -291,6 +291,50 @@ def scene_desc(scene):
     return d, keep
 
 
+class IdkPtAddModelsDesc(ctypes.Structure):
+    """idkpt_add_models's arrays (ModelManager.Add on the scene in place); every id is local to them."""
+    _fields_ = [
+        ("Triangles", c_vp), ("TriangleCount", c_u64),
+        ("BlasDescs", c_vp), ("BlasDescCount", c_u64),
+        ("BlasInstances", c_vp), ("BlasInstanceCount", c_u64),
+        ("MeshTransforms", c_vp), ("MeshTransformCount", c_u64),
+        ("Meshes", c_vp), ("MeshCount", c_u64),
+        ("Materials", c_vp), ("MaterialCount", c_u64),
+        ("Vertices", c_vp),
+        ("VertexPositions", c_vp), ("VertexCount", c_u64),
+        ("Textures", c_vp), ("TextureCount", c_u64),
+        ("UnskinnedVertices", c_vp), ("UnskinnedVertexCount", c_u64),
+    ]
+
+
+def add_models_desc(records, textures=(), unskinned=None):
+    """IdkPtAddModelsDesc borrowing host.model_records' call-local arrays, a list of texture dicts (as host.Scene.textures)
+    and an optional GpuUnskinnedVertex array. Returns (desc, keepalive)."""
+    keep = []
+
+    def ptr(a):
+        a = np.ascontiguousarray(a)
+        keep.append(a)
+        return (a.ctypes.data if len(a) else None), len(a)
+
+    d = IdkPtAddModelsDesc()
+    d.Triangles, d.TriangleCount = ptr(records["triangles"])
+    d.BlasDescs, d.BlasDescCount = ptr(records["blas_descs"])
+    d.BlasInstances, d.BlasInstanceCount = ptr(records["blas_instances"])
+    d.MeshTransforms, d.MeshTransformCount = ptr(records["mesh_transforms"])
+    d.Meshes, d.MeshCount = ptr(records["meshes"])
+    d.Materials, d.MaterialCount = ptr(records["materials"])
+    d.Vertices, _ = ptr(records["vertices"])
+    d.VertexPositions, d.VertexCount = ptr(records["positions"])
+    if textures:
+        arr, tkeep = texture_descs(list(textures))
+        keep.extend(tkeep)
+        d.Textures, d.TextureCount = ctypes.addressof(arr), len(textures)
+    if unskinned is not None:
+        d.UnskinnedVertices, d.UnskinnedVertexCount = ptr(unskinned)
+    return d, keep
+
+
 def texture_descs(textures):
     """IdkPtTextureDesc array for a list of texture dicts (host.Scene.textures). Returns (array, keepalive).
       uncompressed RGBA8:  dict(pixels [H, W, 4] uint8, srgb, wrap_s, wrap_t)
@@ -441,6 +485,8 @@ def load(path=None):
     L.idkpt_blas_build_batch_copy.argtypes = [c_vp, c_vp, c_vp, c_vp, c_vp, c_vp]
     L.idkpt_blas_rebuild.restype = c_i32
     L.idkpt_blas_rebuild.argtypes = [c_vp, c_u32, c_u32, P(IdkPtBlasBuildSettings), P(c_f)]
+    L.idkpt_add_models.restype = c_i32
+    L.idkpt_add_models.argtypes = [c_vp, P(IdkPtAddModelsDesc), P(IdkPtBlasBuildSettings), P(c_f)]
     L.idkpt_blas_sah.restype = c_i32
     L.idkpt_blas_sah.argtypes = [c_vp, c_u32, c_u32, P(IdkPtBlasBuildSettings), c_vp]
     L.idkpt_denoise.restype = c_i32

@@ -27,6 +27,7 @@
 #include "idk_lights_skybox.cuh"
 #include "idk_sky.cuh"
 #include "idk_blas_build.cuh"
+#include "idk_scene_add.cuh"
 #include "idk_textures_host.h"
 
 #define IDKPT_ABI_VERSION 4u   // 2: IdkPtSceneDesc gained Textures / TextureCount; 3: IdkPtStats gained CompactMs / AccumulateMs, host-buffer registration;
@@ -52,9 +53,12 @@ struct IdkCtxBase {
     cudaEvent_t timing[4] = {};    // [0], [1]: start and end of run_timed's work; [2], [3]: marks inside it (idkvx_voxelize's spans)
 };
 
-// Material textures: all base levels in one allocation, their records, the sRGB decode table.
+// Material textures: their base levels, their records, the sRGB decode table. pools[0] holds every image of the last
+// idkpt_set_scene / idkpt_set_textures; each idkpt_add_models with textures appends a pool of its own, which the records of
+// its textures point into.
 struct TextureTable {
-    DevBuf pixels, recs, srgbLut;
+    std::vector<DevBuf> pools;
+    DevBuf recs, srgbLut;
 };
 
 // An output of a raster pass: its device buffer(s) and the size of the image they hold. A call invalidates the record before
@@ -158,11 +162,12 @@ struct IdkPtCtx : IdkCtxBase {
     std::vector<GpuBlasInstance> hostInstances;   // host mirror of `instances` (idkpt_set_scene): a bound voxeliser's draw list
     size_t nodeBytes = 0;
     // prevVertexPositionSSBO (ModelManager.cs:620): the positions before the last skin of each range. Created from the
-    // positions at the first idkpt_skin_vertices or idkpt_prev_positions_device_ptr after idkpt_set_scene, which releases it.
+    // positions at the first idkpt_skin_vertices or idkpt_prev_positions_device_ptr after idkpt_set_scene or idkpt_add_models,
+    // which release it.
     DevBuf prevPositions;
 
-    // voxelisers reading this scene (idkvx_set_scene_from); idkpt_destroy unbinds them. sceneGeneration counts idkpt_set_scene
-    // and idkpt_blas_rebuild calls, so that a bound voxeliser knows when the instance list or the BLAS triangle counts, and
+    // voxelisers reading this scene (idkvx_set_scene_from); idkpt_destroy unbinds them. sceneGeneration counts idkpt_set_scene,
+    // idkpt_blas_rebuild and idkpt_add_models calls, so that a bound voxeliser knows when the instance list or the BLAS triangle counts, and
     // with them its work-queue size, may have changed.
     std::vector<IdkVxCtx*> boundVoxelizers;
     uint64_t sceneGeneration = 0;
@@ -252,6 +257,13 @@ static void release(DevBuf& b) {
     if (b.p) cudaFree(b.p);
     b.p = nullptr;
     b.bytes = 0;
+}
+
+static void release_textures(TextureTable& t) {
+    for (DevBuf& b : t.pools) release(b);
+    t.pools.clear();
+    release(t.recs);
+    release(t.srgbLut);
 }
 
 static void release_raster(RasterState& r) {
@@ -479,9 +491,12 @@ static int upload_textures(IdkCtxBase* ctx, TextureTable& t, const IdkPtTextureD
     IdkPtSceneDesc tmp = {};
     tmp.Textures = textures; tmp.TextureCount = count;
     const std::vector<size_t> off = idk_texture_offsets(&tmp);
-    CK(ensure(t.pixels, std::max<size_t>(off[count], 16)));
+    if (t.pools.empty()) t.pools.emplace_back();
+    for (size_t i = 1; i < t.pools.size(); i++) release(t.pools[i]);   // the pools idkpt_add_models appended
+    t.pools.resize(1);
+    CK(ensure(t.pools[0], std::max<size_t>(off[count], 16)));
     std::vector<TexRec> recs;
-    CK(idk_upload_texture_table(textures, count, off, t.pixels.p, ctx->stream, recs));
+    CK(idk_upload_texture_table(textures, count, off, t.pools[0].p, ctx->stream, recs));
     int rc;
     if ((rc = upload(ctx, t.recs, recs.data(), recs.size() * sizeof(TexRec)))) return rc;
     float lut[256];
@@ -733,11 +748,12 @@ IDKPT_API void idkpt_destroy(IdkPtCtx* ctx) {
     DevBuf* all[] = {&ctx->nodes, &ctx->triRec, &ctx->blasTris, &ctx->positions, &ctx->descs, &ctx->instances, &ctx->xforms,
                      &ctx->meshes, &ctx->materials, &ctx->vertices, &ctx->lights, &ctx->tlas, &ctx->vtxFrame, &ctx->surfRec,
                      &ctx->images[0], &ctx->images[1], &ctx->images[2], &ctx->counters, &ctx->countLog, &ctx->skyFaces,
-                     &ctx->tex.pixels, &ctx->tex.recs, &ctx->tex.srgbLut, &ctx->bloomDown, &ctx->bloomUp, &ctx->postConsts, &ctx->ldr,
+                     &ctx->bloomDown, &ctx->bloomUp, &ctx->postConsts, &ctx->ldr,
                      &ctx->unskinned, &ctx->joints, &ctx->refitParents, &ctx->refitLocks, &ctx->scratch[0], &ctx->scratch[1], &ctx->scratch[2],
                      &ctx->tlasScratch, &ctx->sahScratch, &ctx->oidn[0], &ctx->oidn[1], &ctx->oidn[2], &ctx->oidn[3], &ctx->denoiseWork[0], &ctx->denoiseWork[1], &ctx->denoised,
                      &ctx->pointShadowDev, &ctx->pointShadowMaps, &ctx->pointShadowLights, &ctx->prevPositions};
     for (DevBuf* b : all) release(*b);
+    release_textures(ctx->tex);
     release_raster(ctx->raster);
     for (int i = 0; i < IDK_MAX_LANES; i++) release_lane(ctx->lanes[i], false);
     for (cudaEvent_t ev : ctx->events) cudaEventDestroy(ev);
@@ -1969,6 +1985,25 @@ IDKPT_API int idkpt_blas_refit(IdkPtCtx* ctx, uint32_t first, uint32_t count, fl
     return rc;
 }
 
+// k_tlas_build of n >= 1 instances over the given device arrays into `out` (2n - 1 nodes), with its scratch in the context's
+// tlasScratch. On return *need is the device address of the built tree's height (valid once the stream has finished).
+static int enqueue_tlas_build(IdkPtCtx* ctx, const void* blasNodes, const void* descs, const void* instances, const void* xforms,
+                              void* out, uint64_t n, int searchRadius, int** need) {
+    const size_t nodeCount = 2 * n - 1;
+    const size_t tempOff = 0, leavesOff = nodeCount * 32, keysOff = leavesOff + n * 32, prefOff = keysOff + n * 4, needOff = prefOff + n * 4;
+    CK(ensure(ctx->tlasScratch, needOff + nodeCount * 4 + 64));
+    TlasBuildArgs a;
+    a.blasNodes = (const float4*)blasNodes; a.descs = (const GpuBlasDesc*)descs; a.instances = (const GpuBlasInstance*)instances;
+    a.xforms = (const float4*)xforms; a.nodes = (float4*)out;
+    a.temp = (float4*)((char*)ctx->tlasScratch.p + tempOff); a.leaves = (float4*)((char*)ctx->tlasScratch.p + leavesOff);
+    a.keys = (uint32_t*)((char*)ctx->tlasScratch.p + keysOff); a.pref = (int*)((char*)ctx->tlasScratch.p + prefOff);
+    a.need = (int*)((char*)ctx->tlasScratch.p + needOff);
+    a.n = (int)n; a.searchRadius = searchRadius;
+    k_tlas_build<<<1, 1024, 0, ctx->stream>>>(a);
+    *need = a.need;
+    return IDKPT_OK;
+}
+
 // BVH.TlasBuild on the device (BVH.cs:278-298, TLAS.cs:28-141): see k_tlas_build.
 IDKPT_API int idkpt_tlas_build(IdkPtCtx* ctx, int32_t searchRadius, float* kernelMs) {
     if (!ctx) return IDKPT_ERR_INVALID_ARGUMENT;
@@ -1980,24 +2015,14 @@ IDKPT_API int idkpt_tlas_build(IdkPtCtx* ctx, int32_t searchRadius, float* kerne
     const uint64_t n = ctx->counts.BlasInstanceCount;
     if (n > 16384) return fail(ctx, IDKPT_ERR_UNSUPPORTED, "idkpt_tlas_build: more than 16384 instances (single-CTA build); build on the host and idkpt_update_range");
     CK(cudaSetDevice(ctx->device));
-    const size_t nodeCount = 2 * n - 1;
-    const size_t tempOff = 0, leavesOff = nodeCount * 32, keysOff = leavesOff + n * 32, prefOff = keysOff + n * 4, needOff = prefOff + n * 4;
-    CK(ensure(ctx->tlasScratch, needOff + nodeCount * 4 + 64));
-    TlasBuildArgs a;
-    a.blasNodes = (const float4*)ctx->nodes.p; a.descs = (const GpuBlasDesc*)ctx->descs.p; a.instances = (const GpuBlasInstance*)ctx->instances.p;
-    a.xforms = (const float4*)ctx->xforms.p; a.nodes = (float4*)ctx->tlas.p;
-    a.temp = (float4*)((char*)ctx->tlasScratch.p + tempOff); a.leaves = (float4*)((char*)ctx->tlasScratch.p + leavesOff);
-    a.keys = (uint32_t*)((char*)ctx->tlasScratch.p + keysOff); a.pref = (int*)((char*)ctx->tlasScratch.p + prefOff);
-    a.need = (int*)((char*)ctx->tlasScratch.p + needOff);
-    a.n = (int)n; a.searchRadius = searchRadius;
+    int* needDev = nullptr;
     const int rc = run_timed(ctx, "idkpt_tlas_build", kernelMs, [&]() -> int {
-        k_tlas_build<<<1, 1024, 0, ctx->stream>>>(a);
-        return IDKPT_OK;
+        return enqueue_tlas_build(ctx, ctx->nodes.p, ctx->descs.p, ctx->instances.p, ctx->xforms.p, ctx->tlas.p, n, searchRadius, &needDev);
     });
     if (rc) return rc;
     ctx->accumulatedSamples = 0;
     int need = 0;
-    CK(cudaMemcpy(&need, a.need, 4, cudaMemcpyDeviceToHost));
+    CK(cudaMemcpy(&need, needDev, 4, cudaMemcpyDeviceToHost));
     if (need > IDK_TLAS_STACK_SIZE) {     // the walk's stack is fixed (BVHIntersect.glsl:4): refuse to trace through a TLAS it cannot hold
         ctx->haveScene = false;
         return fail(ctx, IDKPT_ERR_UNSUPPORTED, "idkpt_tlas_build: the built TLAS is deeper than the 24-entry traversal stack of the TLAS walk (scene invalidated; set it again)");
@@ -2260,6 +2285,286 @@ IDKPT_API int idkpt_blas_rebuild(IdkPtCtx* ctx, uint32_t first, uint32_t count, 
     ctx->counts.BlasStackSize = stackSize;
     ctx->hostDescs = std::move(descs);
     ctx->sceneGeneration++;                              // a bound voxeliser re-sizes its work queue for the new triangle counts
+    ctx->accumulatedSamples = 0;
+    return IDKPT_OK;
+}
+
+// validate_scene's checks for idkpt_add_models's own arrays, every id local to them: O(model), never O(scene).
+static int validate_add_models(IdkPtCtx* ctx, const char* who, const IdkPtAddModelsDesc* m) {
+    auto invalid = [&](const char* what) { return fail(ctx, who, IDKPT_ERR_INVALID_ARGUMENT, what); };
+    if ((!m->Triangles && m->TriangleCount) || (!m->BlasDescs && m->BlasDescCount) || (!m->BlasInstances && m->BlasInstanceCount) ||
+        (!m->MeshTransforms && m->MeshTransformCount) || (!m->Meshes && m->MeshCount) || (!m->Materials && m->MaterialCount) ||
+        ((!m->Vertices || !m->VertexPositions) && m->VertexCount) || (!m->UnskinnedVertices && m->UnskinnedVertexCount))
+        return invalid("a required array is null");
+    const IdkPtSceneDesc& c = ctx->counts;
+    if (c.VertexCount != c.VertexPositionCount) return invalid("the scene's vertex and position counts differ");
+    const uint64_t lim = 1ull << 31;
+    if (m->TriangleCount >= lim || c.BlasTriangleCount + m->TriangleCount >= lim || m->VertexCount >= lim || c.VertexCount + m->VertexCount >= lim ||
+        m->MeshCount >= lim || c.MeshCount + m->MeshCount >= lim || m->MaterialCount >= lim || c.MaterialCount + m->MaterialCount >= lim ||
+        m->BlasDescCount >= lim || c.BlasDescCount + m->BlasDescCount >= lim || m->MeshTransformCount >= lim ||
+        c.MeshTransformCount + m->MeshTransformCount >= lim || m->BlasInstanceCount >= lim || c.BlasInstanceCount + m->BlasInstanceCount >= lim)
+        return invalid("scene too large");
+    for (uint64_t i = 0; i < m->BlasInstanceCount; i++)
+        if (m->BlasInstances[i].BlasId >= m->BlasDescCount || m->BlasInstances[i].MeshTransformId >= m->MeshTransformCount)
+            return invalid("BlasInstance references a BLAS or transform outside the call's arrays");
+    for (uint64_t i = 0; i < m->BlasDescCount; i++) {
+        const GpuBlasDesc& d = m->BlasDescs[i];
+        if (d.TriangleCount <= 0) return invalid("a BLAS without triangles");
+        if (d.TriangleOffset < 0 || (uint64_t)d.TriangleOffset + (uint64_t)d.TriangleCount > m->TriangleCount)
+            return invalid("GpuBlasDesc triangle range outside the call's triangles");
+        if (d.TriangleCount > idkbb::MAX_FRAGMENTS) return fail(ctx, who, IDKPT_ERR_UNSUPPORTED, "a BLAS of more than 2^24 triangles");
+    }
+    for (uint64_t i = 0; i < m->TriangleCount; i++) {
+        const GpuBlasTriangle& t = m->Triangles[i];
+        if ((uint64_t)(uint32_t)t.X >= m->VertexCount || (uint64_t)(uint32_t)t.Y >= m->VertexCount || (uint64_t)(uint32_t)t.Z >= m->VertexCount ||
+            t.MeshId < 0 || (uint64_t)t.MeshId >= m->MeshCount)
+            return invalid("GpuBlasTriangle index outside the call's vertices or meshes");
+    }
+    for (uint64_t i = 0; i < m->MeshCount; i++)
+        if (m->Meshes[i].MaterialId < 0 || (uint64_t)m->Meshes[i].MaterialId >= m->MaterialCount)
+            return invalid("GpuMesh.MaterialId outside the call's materials");
+    IdkPtSceneDesc tex = {};                             // idk_validate_textures over the call's table and materials
+    tex.Textures = m->Textures; tex.TextureCount = m->TextureCount;
+    tex.Materials = m->Materials; tex.MaterialCount = m->MaterialCount;
+    if (const char* terr = idk_validate_textures(&tex)) return texture_error(ctx, who, terr);
+    if (c.UseTlas && c.BlasInstanceCount + m->BlasInstanceCount > 16384)
+        return fail(ctx, who, IDKPT_ERR_UNSUPPORTED, "more than 16384 instances under UseTlas (single-CTA TLAS build)");
+    return IDKPT_OK;
+}
+
+// ModelManager.Add(models) (ModelManager.cs:128-216) on the scene in place: see idkpt.h and DESIGN.md 8f.5 "Adding models".
+// Everything is built into staging allocations first -- the grown arrays, the new BLASes, the new TLAS -- and swapped in only
+// when all of it succeeded; until then the context's arrays are only read.
+IDKPT_API int idkpt_add_models(IdkPtCtx* ctx, const IdkPtAddModelsDesc* m, const IdkPtBlasBuildSettings* settings, float* kernelMs) {
+    static const char* who = "idkpt_add_models";
+    if (!ctx) return IDKPT_ERR_INVALID_ARGUMENT;
+    if (kernelMs) *kernelMs = 0.0f;
+    if (!m) return fail(ctx, who, IDKPT_ERR_INVALID_ARGUMENT, "null argument");
+    DRAIN_PENDING(who);
+    if (!ctx->haveScene) return fail(ctx, who, IDKPT_ERR_NO_SCENE, "no scene");
+    idkbvh::Params p;
+    if (int rc = blas_build_params(ctx, who, settings, p)) return rc;
+    if (int rc = validate_add_models(ctx, who, m)) return rc;
+    if (!m->TriangleCount && !m->BlasDescCount && !m->BlasInstanceCount && !m->MeshTransformCount && !m->MeshCount && !m->MaterialCount &&
+        !m->VertexCount && !m->TextureCount && !m->UnskinnedVertexCount)
+        return IDKPT_OK;
+    CK(cudaSetDevice(ctx->device));
+
+    const IdkPtSceneDesc old = ctx->counts;
+    const uint64_t nV = old.VertexCount + m->VertexCount, nX = old.MeshTransformCount + m->MeshTransformCount;
+    const uint64_t nM = old.MeshCount + m->MeshCount, nMat = old.MaterialCount + m->MaterialCount;
+    const uint64_t nI = old.BlasInstanceCount + m->BlasInstanceCount, nB = old.BlasDescCount + m->BlasDescCount;
+    const uint64_t nTex = old.TextureCount + m->TextureCount, nU = ctx->unskinnedCount + m->UnskinnedVertexCount;
+    const uint32_t B = (uint32_t)m->BlasDescCount;
+    std::vector<idkbb::Input> in(B);
+    for (uint32_t k = 0; k < B; k++) {
+        const GpuBlasDesc& d = m->BlasDescs[k];
+        in[k] = {d.TriangleOffset, d.TriangleCount, d.IsRefittable ? 0 : 1};   // BVH.cs:325
+    }
+
+    // the grown arrays ([nodes | triRec] in `bvh`), the new texture pool and records, and the staged records with ids
+    DevBuf positions, vertices, xforms, meshes, materials, instances, vtxFrame, surfRec, descBuf, tris, bvh, tlas, recs, pool, unskinned, stage;
+    struct Drop {
+        DevBuf* b[16];
+        ~Drop() { for (DevBuf* x : b) release(*x); }
+    } drop = {{&positions, &vertices, &xforms, &meshes, &materials, &instances, &vtxFrame, &surfRec, &descBuf, &tris, &bvh, &tlas, &recs,
+               &pool, &unskinned, &stage}};
+    std::vector<GpuBlasDesc> descs = ctx->hostDescs;
+    std::vector<TexRec> newRecs;
+    idkbb::Arena staged;                                  // the new BLASes, until they are copied into `bvh`
+    idkbb::DeviceResult built;
+    size_t nodeBytes = 0, triRecBytes = 0;
+    uint64_t nN = old.BlasNodeCount, nT = old.BlasTriangleCount;
+    int stackSize = 0;
+    int* needDev = nullptr;
+    int rc = run_timed(ctx, who, kernelMs, [&]() -> int {
+        auto alloc = [](DevBuf& b, size_t bytes) { return ensure(b, std::max<size_t>(bytes, 16)) == cudaSuccess; };
+        auto d2d = [&](void* dst, const void* src, size_t bytes) { return bytes ? cudaMemcpyAsync(dst, src, bytes, cudaMemcpyDeviceToDevice, ctx->stream) : cudaSuccess; };
+        auto h2d = [&](void* dst, const void* src, size_t bytes) { return bytes ? cudaMemcpyAsync(dst, src, bytes, cudaMemcpyHostToDevice, ctx->stream) : cudaSuccess; };
+        auto at = [](const DevBuf& b, size_t off) { return (void*)((char*)b.p + off); };
+        auto a256 = [](size_t x) { return (x + 255) & ~(size_t)255; };
+        const size_t stTris = 0, stMeshes = a256(m->TriangleCount * sizeof(GpuBlasTriangle)), stMaterials = stMeshes + a256(m->MeshCount * sizeof(GpuMesh));
+        const size_t stInstances = stMaterials + a256(m->MaterialCount * sizeof(GpuMaterial)), stEnd = stInstances + m->BlasInstanceCount * sizeof(GpuBlasInstance);
+        if (!alloc(stage, stEnd) || !alloc(positions, nV * sizeof(PackedVec3)) || !alloc(vertices, nV * sizeof(GpuVertex)) ||
+            !alloc(xforms, nX * sizeof(GpuMeshTransform)) || !alloc(meshes, nM * sizeof(GpuMesh)) || !alloc(materials, nMat * sizeof(GpuMaterial)) ||
+            !alloc(instances, nI * sizeof(GpuBlasInstance)) || !alloc(vtxFrame, std::max<uint64_t>(nV, 1) * 32) || !alloc(surfRec, std::max<uint64_t>(nM, 1) * 80) ||
+            !alloc(descBuf, nB * sizeof(GpuBlasDesc)) || (m->UnskinnedVertexCount && !alloc(unskinned, nU * sizeof(GpuUnskinnedVertex))))
+            return fail(ctx, who, IDKPT_ERR_OUT_OF_MEMORY, "device allocation failed");
+
+        // the scene's arrays move device to device; the call's arrays come over once, those with ids into the staging buffer
+        CK(d2d(positions.p, ctx->positions.p, old.VertexCount * sizeof(PackedVec3)));
+        CK(d2d(vertices.p, ctx->vertices.p, old.VertexCount * sizeof(GpuVertex)));
+        CK(d2d(vtxFrame.p, ctx->vtxFrame.p, old.VertexCount * 32));
+        CK(d2d(xforms.p, ctx->xforms.p, old.MeshTransformCount * sizeof(GpuMeshTransform)));
+        CK(d2d(meshes.p, ctx->meshes.p, old.MeshCount * sizeof(GpuMesh)));
+        CK(d2d(surfRec.p, ctx->surfRec.p, old.MeshCount * 80));
+        CK(d2d(materials.p, ctx->materials.p, old.MaterialCount * sizeof(GpuMaterial)));
+        CK(d2d(instances.p, ctx->instances.p, old.BlasInstanceCount * sizeof(GpuBlasInstance)));
+        CK(h2d(at(positions, old.VertexCount * sizeof(PackedVec3)), m->VertexPositions, m->VertexCount * sizeof(PackedVec3)));
+        CK(h2d(at(vertices, old.VertexCount * sizeof(GpuVertex)), m->Vertices, m->VertexCount * sizeof(GpuVertex)));
+        CK(h2d(at(xforms, old.MeshTransformCount * sizeof(GpuMeshTransform)), m->MeshTransforms, m->MeshTransformCount * sizeof(GpuMeshTransform)));
+        CK(h2d(at(stage, stTris), m->Triangles, m->TriangleCount * sizeof(GpuBlasTriangle)));
+        CK(h2d(at(stage, stMeshes), m->Meshes, m->MeshCount * sizeof(GpuMesh)));
+        CK(h2d(at(stage, stMaterials), m->Materials, m->MaterialCount * sizeof(GpuMaterial)));
+        CK(h2d(at(stage, stInstances), m->BlasInstances, m->BlasInstanceCount * sizeof(GpuBlasInstance)));
+        if (m->UnskinnedVertexCount) {
+            CK(d2d(unskinned.p, ctx->unskinned.p, ctx->unskinnedCount * sizeof(GpuUnskinnedVertex)));
+            CK(h2d(at(unskinned, ctx->unskinnedCount * sizeof(GpuUnskinnedVertex)), m->UnskinnedVertices, m->UnskinnedVertexCount * sizeof(GpuUnskinnedVertex)));
+        }
+        SceneAddArgs a;
+        a.tris = (GpuBlasTriangle*)at(stage, stTris);
+        a.meshesIn = (const GpuMesh*)at(stage, stMeshes); a.meshesOut = (GpuMesh*)meshes.p + old.MeshCount;
+        a.materialsIn = (const GpuMaterial*)at(stage, stMaterials); a.materialsOut = (GpuMaterial*)materials.p + old.MaterialCount;
+        a.instancesIn = (const GpuBlasInstance*)at(stage, stInstances); a.instancesOut = (GpuBlasInstance*)instances.p + old.BlasInstanceCount;
+        a.triCount = m->TriangleCount; a.meshCount = m->MeshCount; a.materialCount = m->MaterialCount; a.instanceCount = m->BlasInstanceCount;
+        a.vertexOffset = (int32_t)old.VertexCount; a.meshOffset = (int32_t)old.MeshCount; a.materialOffset = (int32_t)old.MaterialCount;
+        a.blasOffset = (uint32_t)old.BlasDescCount; a.transformOffset = (uint32_t)old.MeshTransformCount; a.textureOffset = old.TextureCount;
+        if (const uint64_t total = a.triCount + a.meshCount + a.materialCount + a.instanceCount)
+            k_scene_add_rebase<<<(unsigned)((total + 255) / 256), 256, 0, ctx->stream>>>(a);
+        if (const uint32_t n = (uint32_t)m->VertexCount)      // per element: a launch over the appended range equals the full one
+            k_prepare_vertices<<<(n + 255) / 256, 256, 0, ctx->stream>>>((const uint4*)vertices.p + old.VertexCount, (float4*)vtxFrame.p + 2 * old.VertexCount, n);
+        if (const uint32_t n = (uint32_t)m->MeshCount)
+            k_prepare_surfaces<<<(n + 255) / 256, 256, 0, ctx->stream>>>((const GpuMesh*)meshes.p + old.MeshCount, (const GpuMaterial*)materials.p,
+                                                                         (float4*)surfRec.p + 5 * old.MeshCount, n);
+        CK(cudaGetLastError());
+
+        if (m->TextureCount) {                            // decoded once, into a pool of their own; the old records keep theirs
+            IdkPtSceneDesc tmp = {};
+            tmp.Textures = m->Textures; tmp.TextureCount = m->TextureCount;
+            const std::vector<size_t> off = idk_texture_offsets(&tmp);
+            if (!alloc(pool, off[m->TextureCount]) || !alloc(recs, nTex * sizeof(TexRec)))
+                return fail(ctx, who, IDKPT_ERR_OUT_OF_MEMORY, "device allocation failed");
+            CK(idk_upload_texture_table(m->Textures, m->TextureCount, off, pool.p, ctx->stream, newRecs));
+            CK(d2d(recs.p, ctx->tex.recs.p, old.TextureCount * sizeof(TexRec)));
+            CK(h2d(at(recs, old.TextureCount * sizeof(TexRec)), newRecs.data(), m->TextureCount * sizeof(TexRec)));
+        }
+
+        // the new BLASes: one batch over the staged, rebased triangles and the grown positions
+        if (B) {
+            idkbb::StageTimer tm(ctx->stream);
+            tm.mark("start");
+            std::string err;
+            const int brc = idkbb::build_device(ctx->stream, (const PackedVec3*)positions.p, (const GpuBlasTriangle*)at(stage, stTris), in, p,
+                                                staged, built, tm, err);
+            if (brc != idkbb::BB_OK) return blas_build_fail(ctx, who, brc, err);
+            long long fragments = 0;
+            for (int c : built.fragmentCount) fragments += c;
+            tm.print((int)B, fragments);
+            nN += (uint64_t)built.nodeStart[B];
+            nT += (uint64_t)built.triStart[B];
+            if (nN >= (1ull << 31) || nT >= (1ull << 31)) return fail(ctx, who, IDKPT_ERR_INVALID_ARGUMENT, "scene too large");
+            for (uint32_t k = 0; k < B; k++) {            // BVH.cs:363-386
+                GpuBlasDesc d = m->BlasDescs[k];
+                d.NodeOffset = (int32_t)(old.BlasNodeCount + built.nodeStart[k]);
+                d.NodeCount = built.nodeStart[k + 1] - built.nodeStart[k];
+                d.TriangleOffset = (int32_t)(old.BlasTriangleCount + built.triStart[k]);
+                d.TriangleCount = built.triStart[k + 1] - built.triStart[k];
+                d.RequiredStackSize = built.requiredStackSize[k];
+                descs.push_back(d);
+            }
+        }
+        for (const GpuBlasDesc& d : descs) stackSize = std::max(stackSize, d.RequiredStackSize);   // BVH.UpdateBlasStackSize
+        if ((size_t)std::max(1, stackSize) * IDK_BLOCK * sizeof(uint32_t) > 200 * 1024)
+            return fail(ctx, who, IDKPT_ERR_UNSUPPORTED, "BlasStackSize too large for the shared-memory traversal stack");
+        nodeBytes = ((nN * sizeof(GpuBlasNode)) + 255) & ~(size_t)255;
+        triRecBytes = std::max<size_t>(nT, 1) * 64;
+        if (!alloc(bvh, nodeBytes + triRecBytes) || !alloc(tris, nT * sizeof(GpuBlasTriangle)))
+            return fail(ctx, who, IDKPT_ERR_OUT_OF_MEMORY, "device allocation failed");
+        float4* recNew = (float4*)at(bvh, nodeBytes);
+        CK(d2d(bvh.p, ctx->nodes.p, old.BlasNodeCount * sizeof(GpuBlasNode)));
+        CK(d2d(recNew, (const char*)ctx->nodes.p + ctx->nodeBytes, old.BlasTriangleCount * 64));
+        CK(d2d(tris.p, ctx->blasTris.p, old.BlasTriangleCount * sizeof(GpuBlasTriangle)));
+        CK(d2d(descBuf.p, ctx->descs.p, old.BlasDescCount * sizeof(GpuBlasDesc)));
+        if (B) {
+            CK(d2d((GpuBlasNode*)bvh.p + old.BlasNodeCount, built.nodes, (size_t)built.nodeStart[B] * sizeof(GpuBlasNode)));
+            CK(d2d((GpuBlasTriangle*)tris.p + old.BlasTriangleCount, built.tris, (size_t)built.triStart[B] * sizeof(GpuBlasTriangle)));
+            if (const uint32_t n = (uint32_t)built.triStart[B])
+                k_prepare_triangles<<<(n + 255) / 256, 256, 0, ctx->stream>>>((const int4*)tris.p + old.BlasTriangleCount, (const float*)positions.p,
+                                                                              recNew + 4 * old.BlasTriangleCount, n);
+            CK(h2d(at(descBuf, old.BlasDescCount * sizeof(GpuBlasDesc)), descs.data() + old.BlasDescCount, B * sizeof(GpuBlasDesc)));
+        }
+
+        // BVH.TlasBuild(true) in ModelManager.Add: the device PLOC build over every instance, TLAS.BuildSettings.SearchRadius 15
+        if (old.UseTlas) {
+            if (!alloc(tlas, (2 * nI - 1) * sizeof(GpuTlasNode))) return fail(ctx, who, IDKPT_ERR_OUT_OF_MEMORY, "device allocation failed");
+            if (int trc = enqueue_tlas_build(ctx, bvh.p, descBuf.p, instances.p, xforms.p, tlas.p, nI, 15, &needDev)) return trc;
+        }
+        return IDKPT_OK;
+    });
+    if (rc) return rc;
+    if (needDev) {
+        int need = 0;
+        CK(cudaMemcpy(&need, needDev, 4, cudaMemcpyDeviceToHost));
+        if (need > IDK_TLAS_STACK_SIZE)
+            return fail(ctx, who, IDKPT_ERR_UNSUPPORTED, "the TLAS is deeper than the 24-entry traversal stack of the TLAS walk (BVHIntersect.glsl:4)");
+    }
+
+    // commit: launch configuration and L2 window for the new arrays first (restored if either fails), then the swap
+    const int oldStack = ctx->sc.stackSize;
+    ctx->sc.stackSize = std::max(1, stackSize);
+    if ((rc = configure_launches(ctx)) || (rc = set_l2_window(ctx, bvh.p, nodeBytes + triRecBytes))) {
+        const std::string err = ctx->lastError;
+        ctx->sc.stackSize = oldStack;
+        configure_launches(ctx);
+        set_l2_window(ctx, ctx->nodes.p, ctx->nodeBytes + std::max<size_t>(ctx->counts.BlasTriangleCount, 1) * 64);
+        ctx->lastError = err;
+        return rc;
+    }
+    std::swap(ctx->positions, positions);                // `drop` frees the old arrays
+    std::swap(ctx->vertices, vertices);
+    std::swap(ctx->xforms, xforms);
+    std::swap(ctx->meshes, meshes);
+    std::swap(ctx->materials, materials);
+    std::swap(ctx->instances, instances);
+    std::swap(ctx->vtxFrame, vtxFrame);
+    std::swap(ctx->surfRec, surfRec);
+    std::swap(ctx->descs, descBuf);
+    std::swap(ctx->blasTris, tris);
+    std::swap(ctx->nodes, bvh);
+    if (old.UseTlas) std::swap(ctx->tlas, tlas);
+    if (m->TextureCount) {
+        std::swap(ctx->tex.recs, recs);
+        ctx->tex.pools.push_back(pool);
+        pool = DevBuf{};
+    }
+    if (m->UnskinnedVertexCount) std::swap(ctx->unskinned, unskinned);
+    release(ctx->prevPositions);                         // re-created from the positions at its next use (ModelManager.cs:620)
+
+    DeviceScene& sc = ctx->sc;
+    sc.nodes = (const float4*)ctx->nodes.p;
+    sc.triRec = (const float4*)((char*)ctx->nodes.p + nodeBytes);
+    sc.blasTris = (const int4*)ctx->blasTris.p;
+    sc.descs = (const GpuBlasDesc*)ctx->descs.p;
+    sc.instances = (const GpuBlasInstance*)ctx->instances.p;
+    sc.xforms = (const float4*)ctx->xforms.p;
+    sc.meshes = (const GpuMesh*)ctx->meshes.p;
+    sc.materials = (const GpuMaterial*)ctx->materials.p;
+    sc.vertices = (const uint4*)ctx->vertices.p;
+    sc.instanceCount = (uint32_t)nI;
+    sc.tlasNodes = (const float4*)ctx->tlas.p;
+    sc.vtxFrame = (const float4*)ctx->vtxFrame.p;
+    sc.surfRec = (const float4*)ctx->surfRec.p;
+    sc.textures = (const TexRec*)ctx->tex.recs.p;
+    sc.textureCount = (uint32_t)nTex;
+    IdkPtSceneDesc& c = ctx->counts;
+    c.BlasNodeCount = nN; c.BlasTriangleCount = nT; c.BlasDescCount = nB; c.BlasInstanceCount = nI;
+    if (old.UseTlas) c.TlasNodeCount = 2 * nI - 1;
+    c.MeshTransformCount = nX; c.MeshCount = nM; c.MaterialCount = nMat; c.VertexCount = nV; c.VertexPositionCount = nV;
+    c.BlasStackSize = stackSize; c.TextureCount = nTex;
+    ctx->nodeBytes = nodeBytes;
+    ctx->hostDescs = std::move(descs);
+    for (uint64_t i = 0; i < m->BlasInstanceCount; i++)
+        ctx->hostInstances.push_back({m->BlasInstances[i].BlasId + (uint32_t)old.BlasDescCount, m->BlasInstances[i].MeshTransformId + (uint32_t)old.MeshTransformCount});
+    for (uint64_t i = 0; i < m->MaterialCount; i++) {
+        const uint64_t h = material_max_handle(m->Materials[i]);
+        ctx->hostMaterialMaxHandle.push_back(h ? h + old.TextureCount : 0);
+    }
+    for (uint64_t i = 0; i < m->UnskinnedVertexCount; i++) {
+        const uint32_t* j = m->UnskinnedVertices[i].JointIndices;
+        ctx->unskinnedMaxJoint.push_back(std::max(std::max(j[0], j[1]), std::max(j[2], j[3])));
+    }
+    ctx->unskinnedCount = nU;
+    ctx->sceneGeneration++;                              // a bound voxeliser re-sizes its work queue for the new draw list
     ctx->accumulatedSamples = 0;
     return IDKPT_OK;
 }

@@ -73,8 +73,9 @@ static void unbind_voxelizers(IdkPtCtx* pt) {
 // The scene arrays idkvx_set_scene copies, the texture table included.
 static void release_scene(IdkVxCtx* ctx) {
     for (DevBuf* b : {&ctx->positions, &ctx->vertices, &ctx->tris, &ctx->descs, &ctx->instances, &ctx->xforms, &ctx->meshes,
-                      &ctx->materials, &ctx->lights, &ctx->tex.pixels, &ctx->tex.recs, &ctx->tex.srgbLut})
+                      &ctx->materials, &ctx->lights})
         release(*b);
+    release_textures(ctx->tex);
 }
 
 // Work items of the large-triangle queue for a draw list: (triangle, tile) items of large triangles.

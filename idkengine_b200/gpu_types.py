@@ -45,12 +45,18 @@ IdkPtGpuSettings = np.dtype([("FocalLength", f4), ("LenseRadius", f4), ("DoDebug
 IdkPtRay = np.dtype([("Origin", f4, 3), ("TMax", f4), ("Direction", f4, 3), ("_pad0", f4)])
 IdkPtHit = np.dtype([("BaryX", f4), ("BaryY", f4), ("T", f4), ("TriangleId", u4), ("MeshTransformId", u4),
                      ("NodePairFetches", u4), ("TriangleTests", u4), ("_pad0", u4)])
+# idkpt_add_models's argument record: its pointers as u8 (capi.IdkPtAddModelsDesc is the ctypes twin the calls pass)
+IdkPtAddModelsDesc = np.dtype([(n, u8) for n in (
+    "Triangles", "TriangleCount", "BlasDescs", "BlasDescCount", "BlasInstances", "BlasInstanceCount", "MeshTransforms",
+    "MeshTransformCount", "Meshes", "MeshCount", "Materials", "MaterialCount", "Vertices", "VertexPositions", "VertexCount",
+    "Textures", "TextureCount", "UnskinnedVertices", "UnskinnedVertexCount")])
 
 EXPECTED_SIZES = {
     "GpuBlasNode": 32, "GpuBlasTriangle": 16, "GpuBlasDesc": 40, "GpuBlasInstance": 8, "GpuTlasNode": 32,
     "GpuMeshTransform": 144, "GpuMesh": 96, "GpuMaterial": 96, "GpuVertex": 16, "PackedVec3": 12,
     "GpuLight": 48, "GpuPointShadow": 432, "GpuPerFrameData": 544, "GpuWavefrontRay": 48, "GpuAovRay": 32, "IdkPtGpuSettings": 20,
     "IdkPtRay": 32, "IdkPtHit": 32, "GpuUnskinnedVertex": 52, "IdkPtSkinningCmd": 16,
+    "IdkPtAddModelsDesc": 152,
 }
 for _name, _size in EXPECTED_SIZES.items():
     assert globals()[_name].itemsize == _size, (_name, globals()[_name].itemsize, _size)

@@ -202,6 +202,64 @@ def mesh_transform(model4x4):
 
 
 # --------------------------------------------------------------------------- Scene
+TEXTURE_SLOTS = ("BaseColorTexture", "MetallicRoughnessTexture", "NormalTexture", "EmissiveTexture", "TransmissionTexture")
+
+
+def model_records(models):
+    """ModelManager.Add's per-model records (SRC/ModelManager.cs:128-213, BVH.Add SRC/Bvh/BVH.cs:255-272) for `models` in
+    order, every id local to these arrays: the layout idkpt_add_models takes (PathTracer.AddModels). One BLAS and one
+    instance per model: blas_descs[k] covers model k's source triangles (TriangleOffset / TriangleCount into `triangles`,
+    IsRefittable), and blas_instances[k] puts BLAS k under mesh_transforms[k]. Material texture handles are copied as given.
+    Returns dict(positions, vertices, meshes, materials, mesh_transforms, triangles, blas_descs, blas_instances)."""
+    out = {f: [np.zeros(0, t)] for f, t in (("positions", gt.PackedVec3), ("vertices", gt.GpuVertex), ("meshes", gt.GpuMesh),
+                                             ("materials", gt.GpuMaterial), ("mesh_transforms", gt.GpuMeshTransform),
+                                             ("triangles", gt.GpuBlasTriangle))}
+    descs = np.zeros(len(models), gt.GpuBlasDesc)
+    instances = np.zeros(len(models), gt.GpuBlasInstance)
+    v_off = mesh_off = mat_off = tri_off = 0
+    for k, m in enumerate(models):
+        pos = np.zeros(len(m.positions), gt.PackedVec3)
+        pos["x"], pos["y"], pos["z"] = m.positions[:, 0], m.positions[:, 1], m.positions[:, 2]
+        vtx = np.zeros(len(m.positions), gt.GpuVertex)
+        vtx["TexCoord"] = m.texcoords
+        vtx["Normal"] = gt.compress_sr11g11b10(m.normals)
+        vtx["Tangent"] = gt.compress_sr11g11b10(m.tangents)
+        meshes = m.meshes.copy()
+        meshes["MaterialId"] += mat_off
+        src = np.zeros(len(m.indices), gt.GpuBlasTriangle)     # BVH.Add: vertex-offset rebased indices + MeshId
+        src["X"] = m.indices[:, 0].astype(np.int64) + v_off
+        src["Y"] = m.indices[:, 1].astype(np.int64) + v_off
+        src["Z"] = m.indices[:, 2].astype(np.int64) + v_off
+        src["MeshId"] = m.tri_mesh + mesh_off
+        for f, a in (("positions", pos), ("vertices", vtx), ("meshes", meshes), ("materials", m.materials),
+                     ("mesh_transforms", mesh_transform(m.model_matrix)), ("triangles", src)):
+            out[f].append(a)
+        descs[k]["TriangleOffset"], descs[k]["TriangleCount"] = tri_off, len(src)
+        descs[k]["IsRefittable"] = 1 if m.refittable else 0
+        instances[k]["BlasId"], instances[k]["MeshTransformId"] = k, k
+        v_off, mesh_off, mat_off, tri_off = v_off + len(pos), mesh_off + len(meshes), mat_off + len(m.materials), tri_off + len(src)
+    out = {f: np.concatenate(a) for f, a in out.items()}
+    out["blas_descs"], out["blas_instances"] = descs, instances
+    return out
+
+
+def rebase_records(rec, vertices=0, meshes=0, materials=0, textures=0, blases=0, transforms=0):
+    """idkpt_add_models's rebase (include/idkpt.h) of model_records' call-local ids onto a scene that holds these counts:
+    triangle X/Y/Z + vertices and MeshId + meshes, GpuMesh.MaterialId + materials, a texture handle k > 0 + textures (0
+    stays 0), BlasId + blases, MeshTransformId + transforms. The descs keep their call-local triangle ranges. Returns a copy."""
+    out = {f: a.copy() for f, a in rec.items()}
+    for f in ("X", "Y", "Z"):
+        out["triangles"][f] += vertices
+    out["triangles"]["MeshId"] += meshes
+    out["meshes"]["MaterialId"] += materials
+    for f in TEXTURE_SLOTS:
+        h = out["materials"][f]
+        out["materials"][f] = np.where(h > 0, h + np.uint64(textures), np.uint64(0))
+    out["blas_instances"]["BlasId"] += blases
+    out["blas_instances"]["MeshTransformId"] += transforms
+    return out
+
+
 class Model:
     """One glTF-like model after ModelLoader + HoistMeshPrimitives: local-space vertex data, an index
     buffer, a per-triangle local mesh id, per-mesh GpuMesh records, materials and one model matrix."""
@@ -271,36 +329,17 @@ class Scene:
         blas_batch_builder: a function with PathTracer.BuildBlases's (positions, triangles, descs) signature and result; when
         given, every model not found in the cache is built in one call of it, as BlasesBuild builds a load in one parallel loop."""
         cache_dir = cache_dir or os.environ.get("IDKHOST_BVH_CACHE") or None
-        pending = []   # per model: [source triangles, vertex / mesh / transform offsets, cache key and path, its BLAS or None]
-        for m in models:
-            v_off = len(self.positions)
-            mesh_off = len(self.meshes)
-            mat_off = len(self.materials)
-
-            pos = np.zeros(len(m.positions), gt.PackedVec3)
-            pos["x"], pos["y"], pos["z"] = m.positions[:, 0], m.positions[:, 1], m.positions[:, 2]
-            self.positions = np.concatenate([self.positions, pos])
-
-            vtx = np.zeros(len(m.positions), gt.GpuVertex)
-            vtx["TexCoord"] = m.texcoords
-            vtx["Normal"] = gt.compress_sr11g11b10(m.normals)
-            vtx["Tangent"] = gt.compress_sr11g11b10(m.tangents)
-            self.vertices = np.concatenate([self.vertices, vtx])
-
-            meshes = m.meshes.copy()
-            meshes["MaterialId"] += mat_off
-            self.meshes = np.concatenate([self.meshes, meshes])
-            self.materials = np.concatenate([self.materials, m.materials])
-
-            transform_id = len(self.mesh_transforms)
-            self.mesh_transforms = np.concatenate([self.mesh_transforms, mesh_transform(m.model_matrix)])
-
-            # BVH.Add: vertex-offset rebased indices + MeshId (BVH.cs:255-272)
-            src = np.zeros(len(m.indices), gt.GpuBlasTriangle)
-            src["X"] = m.indices[:, 0].astype(np.int64) + v_off
-            src["Y"] = m.indices[:, 1].astype(np.int64) + v_off
-            src["Z"] = m.indices[:, 2].astype(np.int64) + v_off
-            src["MeshId"] = m.tri_mesh + mesh_off
+        rec = rebase_records(model_records(models), vertices=len(self.positions), meshes=len(self.meshes), materials=len(self.materials),
+                             blases=len(self.blas_descs), transforms=len(self.mesh_transforms))
+        v_offs = len(self.positions) + np.concatenate([[0], np.cumsum([len(m.positions) for m in models])]).astype(np.int64)
+        mesh_offs = len(self.meshes) + np.concatenate([[0], np.cumsum([len(m.meshes) for m in models])]).astype(np.int64)
+        for f in ("positions", "vertices", "meshes", "materials", "mesh_transforms"):
+            setattr(self, f, np.concatenate([getattr(self, f), rec[f]]))
+        pending = []   # per model: [source triangles, vertex / mesh offsets, cache key and path, its BLAS or None]
+        for k, m in enumerate(models):
+            v_off, mesh_off = int(v_offs[k]), int(mesh_offs[k])
+            d = rec["blas_descs"][k]
+            src = rec["triangles"][d["TriangleOffset"]:d["TriangleOffset"] + d["TriangleCount"]]
             self.source_triangle_count += len(src)
 
             b = None
@@ -319,7 +358,7 @@ class Scene:
                     b = build_blas(self.positions, src, presplit=not m.refittable, threads=threads)
                 else:
                     b = blas_builder(self.positions, src, presplit=not m.refittable)
-            pending.append([src, v_off, mesh_off, transform_id, key, cache_path, b])
+            pending.append([src, v_off, mesh_off, key, cache_path, b])
 
         todo = [p for p in pending if p[-1] is None]
         if todo:                          # one batch of every model the cache did not have
@@ -335,7 +374,7 @@ class Scene:
                             required_stack_size=int(d["RequiredStackSize"]), fragment_count=int(r["fragment_counts"][k]),
                             sah=float(r["sahs"][k]))
 
-        for m, (src, v_off, mesh_off, transform_id, key, cache_path, b) in zip(models, pending):
+        for k, (m, (src, v_off, mesh_off, key, cache_path, b)) in enumerate(zip(models, pending)):
             if cache_path is not None and not b.get("from_cache", False):
                 rel = dict(b)
                 rel["triangles"] = b["triangles"].copy()
@@ -355,10 +394,7 @@ class Scene:
             self.blas_descs = np.concatenate([self.blas_descs, desc])
             self.blas_nodes = np.concatenate([self.blas_nodes, b["nodes"]])
             self.blas_triangles = np.concatenate([self.blas_triangles, b["triangles"]])
-            inst = np.zeros(1, gt.GpuBlasInstance)
-            inst["BlasId"] = blas_id
-            inst["MeshTransformId"] = transform_id
-            self.blas_instances = np.concatenate([self.blas_instances, inst])
+            self.blas_instances = np.concatenate([self.blas_instances, rec["blas_instances"][k:k + 1]])
             self.build_info.append(dict(name=m.name, source_triangles=len(src), fragments=b["fragment_count"],
                                         triangles=len(b["triangles"]), nodes=len(b["nodes"]),
                                         required_stack_size=b["required_stack_size"], sah=b["sah"], from_cache=bool(b.get("from_cache", False))))

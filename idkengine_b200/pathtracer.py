@@ -13,6 +13,7 @@ import numpy as np
 
 from . import capi
 from . import gpu_types as gt
+from . import host
 
 
 class IdkPtError(RuntimeError):
@@ -231,6 +232,21 @@ class PathTracer:
             self._lib.idkpt_blas_build_free(h)
         self.last_blas_build_ms = float(ms.value)
         return dict(descs=out_descs, nodes=nodes, triangles=tris, fragment_counts=frags, sahs=sahs)
+
+    def AddModels(self, *models, textures=(), unskinned=None, settings=None):
+        """ModelManager.Add(models) (ModelManager.cs:128-216) on the device scene in place (idkpt_add_models): host.Model objects
+        appended with host.model_records' call-local ids -- their material texture handles index `textures` (list of texture
+        dicts as host.Scene.textures, 1-based, 0 = white) -- one BLAS and one instance per model, the BLASes built on the
+        device, the TLAS rebuilt when the scene uses one. unskinned: GpuUnskinnedVertex records appended behind
+        SetSkinningData's. settings as BuildBlas (DoPreSplit is ignored). Returns kernel ms."""
+        if unskinned is not None:
+            unskinned = np.ascontiguousarray(unskinned)
+            assert unskinned.dtype == gt.GpuUnskinnedVertex
+        d, keep = capi.add_models_desc(host.model_records(models), textures, unskinned)
+        ms = ctypes.c_float()
+        self._check(self._lib.idkpt_add_models(self._ctx, ctypes.byref(d), ctypes.byref(self._blas_settings(settings)), ctypes.byref(ms)),
+                    "idkpt_add_models")
+        return ms.value
 
     def SetTextures(self, textures):
         """Replace the material texture table (list of dict(pixels, srgb, wrap_s, wrap_t), as host.Scene.textures)."""

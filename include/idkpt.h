@@ -531,7 +531,8 @@ IDKPT_API int idkpt_shading_rate_device_ptr(IdkPtCtx* ctx, void** dev_ptr, uint6
  * idkpt_read_gbuffer: downloads the images of the last successful call; any argument may be NULL.
  * idkpt_prev_positions_device_ptr: the context's previous positions (PackedVec3 [VertexPositionCount], *bytes their size), as
  *   idkpt_skin_vertices keeps them. Created at the first idkpt_skin_vertices or idkpt_prev_positions_device_ptr after
- *   idkpt_set_scene as a copy of the positions at that moment; valid until idkpt_set_scene or idkpt_destroy. Needs a scene.
+ *   idkpt_set_scene or idkpt_add_models as a copy of the positions at that moment; valid until idkpt_set_scene,
+ *   idkpt_add_models or idkpt_destroy. Needs a scene.
  * The call is synchronous and ordered after the samples idkpt_compute has queued. Its images are context allocations, reused
  * by calls with the same size, valid until the next call with another size, a failed call, idkpt_set_scene or idkpt_destroy. */
 IDKPT_API int idkpt_gbuffer(IdkPtCtx* ctx, const GpuPerFrameData* frame, int32_t width, int32_t height, const float* taa_jitter,
@@ -697,6 +698,55 @@ IDKPT_API int idkpt_blas_rebuild(IdkPtCtx* ctx, uint32_t first, uint32_t count, 
  * BLAS the builder just produced. Only settings->TriangleCost is read (NULL = 1.1). sah_out: count doubles. A host refits most
  * frames and rebuilds (idkpt_blas_rebuild) when the SAH has drifted far enough from the built one. */
 IDKPT_API int idkpt_blas_sah(IdkPtCtx* ctx, uint32_t first, uint32_t count, const IdkPtBlasBuildSettings* settings, double* sah_out);
+
+/* ModelManager.Add(models) (ModelManager.cs:128-216) on the scene in place: appends the call's arrays behind the scene's,
+ * builds the new BLASes on the device and, for a scene set with UseTlas, rebuilds the TLAS. Loading a model costs what the
+ * model costs: nothing already on the device crosses PCIe again, no texture is decoded again, and nothing the renderer keeps
+ * between frames is dropped. Every id is local to this call's arrays; several models are concatenated by the caller, as
+ * ModelManager.Add(params models) does.
+ * Append order and offsets: the call's arrays go behind the scene's, in order, with the scene's old counts added:
+ *   GpuBlasTriangle X/Y/Z + old VertexCount, MeshId + old MeshCount; GpuMesh.MaterialId + old MaterialCount; a material
+ *   texture handle k > 0 + old TextureCount (0, the white fallback, stays 0); GpuBlasInstance.BlasId + old BlasDescCount,
+ *   MeshTransformId + old MeshTransformCount. Every other field (GpuMesh.MeshletsOffset and the like) is copied as given.
+ * BLASes: built as one idkpt_blas_build_batch batch over the rebased triangles, each pre-split exactly when !IsRefittable
+ *   (settings->DoPreSplit is ignored), so each equals idkpt_blas_build_batch's and the host build's node for node. Their
+ *   descs are filled as BVH.cs:363-386 fills them: NodeOffset and TriangleOffset behind the scene's current ends, NodeCount,
+ *   TriangleCount and RequiredStackSize from the build, every other field as handed in. BlasStackSize becomes the largest
+ *   RequiredStackSize of all descs (BVH.UpdateBlasStackSize).
+ * TLAS: with UseTlas the node array grows to 2n - 1 nodes and is rebuilt over every instance by idkpt_tlas_build's PLOC build
+ *   with search radius 15 (BVH.TlasBuild(true) in ModelManager.Add). A scene without UseTlas stays without it.
+ * Kept as they are: lights, sky, point-shadow maps and records, every raster image (G-buffer, SSAO, deferred, shadow
+ *   visibility slots, volumetric, SSR, shading rate), the TAA history and its frame counter, the existing texture records;
+ *   their *_device_ptr exports stay valid. The kept previous positions are released, so that they equal the current
+ *   positions of every vertex, old and new (ModelManager.cs:620); a pointer idkpt_prev_positions_device_ptr returned before is
+ *   no longer valid. UnskinnedVertices are appended behind idkpt_set_skinning_data's; the skinning commands stay the host's.
+ * The call bumps the scene generation (a voxeliser bound with idkvx_set_scene_from re-sizes its work queue at its next
+ * voxelisation), resets the accumulation, and is synchronous and ordered after queued idkpt_compute samples.
+ * All or nothing: every check runs on the host over the call's arrays only, before anything runs on the device. The grown
+ * arrays, the BLASes and the TLAS are built into staging memory (old and new arrays exist together until the commit) and
+ * swapped in only when all of it succeeded; a failed call leaves every array, count, desc, image, exported pointer and the
+ * accumulation as they were. A call whose counts are all 0 does nothing and returns IDKPT_OK.
+ * IDKPT_ERR_NO_SCENE: no scene. IDKPT_ERR_INVALID_ARGUMENT: a NULL pointer with a count, an id outside its call-local range,
+ * a desc without triangles or with a range outside Triangles, a non-finite setting, StopSplittingThreshold < 1, a scene whose
+ * VertexCount and VertexPositionCount differ, or 2^31 or more nodes, triangles, vertices, meshes, materials, descs,
+ * transforms or instances in total. IDKPT_ERR_UNSUPPORTED: a texture format the decoder lacks, more than 2^24 fragments in
+ * one BLAS, a BlasStackSize beyond the shared-memory traversal stack, or with UseTlas more than 16384 instances (the
+ * single-CTA TLAS build) or a TLAS deeper than 24 entries. kernel_ms (may be NULL): device time of the whole call. */
+typedef struct IdkPtAddModelsDesc {
+    const GpuBlasTriangle*    Triangles;         uint64_t TriangleCount;        /* BVH.Add's source triangles: X/Y/Z index this call's vertices, MeshId its meshes */
+    const GpuBlasDesc*        BlasDescs;         uint64_t BlasDescCount;        /* per new BLAS: TriangleOffset/TriangleCount into Triangles, IsRefittable */
+    const GpuBlasInstance*    BlasInstances;     uint64_t BlasInstanceCount;    /* BlasId into BlasDescs, MeshTransformId into MeshTransforms */
+    const GpuMeshTransform*   MeshTransforms;    uint64_t MeshTransformCount;
+    const GpuMesh*            Meshes;            uint64_t MeshCount;            /* MaterialId into Materials */
+    const GpuMaterial*        Materials;         uint64_t MaterialCount;        /* texture handle 0 = white fallback, k > 0 = Textures[k-1] */
+    const GpuVertex*          Vertices;
+    const PackedVec3*         VertexPositions;   uint64_t VertexCount;          /* both arrays VertexCount long */
+    const IdkPtTextureDesc*   Textures;          uint64_t TextureCount;         /* may be NULL/0 */
+    const GpuUnskinnedVertex* UnskinnedVertices; uint64_t UnskinnedVertexCount; /* may be NULL/0 */
+} IdkPtAddModelsDesc;
+IDK_STATIC_ASSERT(sizeof(IdkPtAddModelsDesc) == 152, "IdkPtAddModelsDesc must be 152 bytes");
+IDKPT_API int idkpt_add_models(IdkPtCtx* ctx, const IdkPtAddModelsDesc* models,
+                               const IdkPtBlasBuildSettings* settings /* NULL = defaults; DoPreSplit ignored */, float* kernel_ms);
 
 /* ---- present chain (SURVEY.md 8f.3): Bloom.Compute(Result) + TonemapAndGamma.Compute(Result, Bloom.Result)
  * (Application.cs:217-223) -> the RGBA8 frame the reference copies to the swapchain, produced on the device. ---- */

@@ -200,6 +200,13 @@ public:
         idkpt_blas_build_free(b);
         return r;
     }
+    // ModelManager.Add(models) on the device scene in place (idkpt_add_models): every id of `models` local to its arrays.
+    // Returns the device time of the call.
+    float AddModels(const IdkPtAddModelsDesc& models, const IdkPtBlasBuildSettings* settings = nullptr) {
+        float ms = 0.0f;
+        check(idkpt_add_models(ctx_, &models, settings, &ms), "idkpt_add_models");
+        return ms;
+    }
     float Denoise(const IdkPtDenoiseSettings& s) { float ms = 0.0f; check(idkpt_denoise(ctx_, &s, &ms), "idkpt_denoise"); return ms; }   // PathTracerPipeline.Denoise
     std::vector<float> Denoised() const { return read(IDKPT_IMAGE_DENOISED); }
     void RegisterHostBuffer(void* hostPtr, uint64_t bytes) { check(idkpt_register_host_buffer(ctx_, hostPtr, bytes), "idkpt_register_host_buffer"); }
