@@ -5,6 +5,7 @@
 // derived on the device from the node array itself (children always follow their parent) and the leaf list is replaced by
 // "one thread per node, leaves start the climb": no host pre-pass, no extra upload.
 #pragma once
+#include <cooperative_groups.h>
 #include "idk_kernels.cuh"
 #include "idk_bvh_math.h"
 
@@ -140,8 +141,8 @@ __global__ void __launch_bounds__(256) k_refit_climb(RefitArgs a) {
 // BVH.TlasBuild (BVH.cs:278-298) + TLAS.Build (TLAS.cs:28-141, the serial PLOC variant: Morton-ordered leaves, every node
 // picks the neighbour within `searchRadius` that gives the smallest merged half area, mutual picks merge) for animated scenes:
 // the world-space bounds come from the (refitted) BLAS roots and the current mesh transforms, both already in HBM, so a moving
-// scene never reads its roots back to the host. One CTA (instance counts are tens to thousands): the parallel parts are the
-// box transform, the Morton keys, the stable rank sort and the O(n * radius) neighbour search; the ordered placement of merged /
+// scene never reads its roots back to the host. One CTA, used up to IDK_TLAS_SINGLE_CTA_MAX instances (the grid build below
+// takes the rest): the parallel parts are the box transform, the Morton keys, the stable rank sort and the O(n * radius) neighbour search; the ordered placement of merged /
 // unmerged nodes runs on one thread, exactly as the reference's loop does, so the node array equals the host build bit for bit
 // (idkhost_tlas_build, tests/test_dynamic.py): both take the box, key and half-area arithmetic from idk_bvh_math.h.
 struct TlasBuildArgs {
@@ -154,14 +155,15 @@ struct TlasBuildArgs {
     float4* leaves;                  // scratch: n nodes
     uint32_t* keys;                  // scratch: n
     int* pref;                       // scratch: n
-    int* need;                       // scratch: 2n-1; need[0] on exit = traversal stack entries the TLAS walk needs (tree height)
+    int* need;                       // scratch: 2n-1; need[0] on exit = traversal stack entries the TLAS walk needs (tree height),
+                                     //   or -1 when an iteration merged nothing (a non-finite box: no area is < FLT_MAX)
     int n, searchRadius;
 };
 
 __global__ void __launch_bounds__(1024) k_tlas_build(TlasBuildArgs a) {
     __shared__ float s_min[3][32], s_max[3][32];
     __shared__ float s_gmin[3], s_gmax[3];
-    __shared__ int s_range[2];
+    __shared__ int s_range[2], s_stalled;
     using namespace idkbvh;
     const int n = a.n, nodeCount = 2 * n - 1, tid = threadIdx.x, nt = blockDim.x;
     for (int i = tid; i < nodeCount; i += nt) { a.nodes[2 * i] = make_float4(0, 0, 0, 0); a.nodes[2 * i + 1] = make_float4(0, 0, 0, 0); }
@@ -206,9 +208,9 @@ __global__ void __launch_bounds__(1024) k_tlas_build(TlasBuildArgs a) {
         a.nodes[2 * (nodeCount - n + rank)] = a.leaves[2 * i];
         a.nodes[2 * (nodeCount - n + rank) + 1] = a.leaves[2 * i + 1];
     }
-    if (tid == 0) { s_range[0] = n; s_range[1] = nodeCount; }
+    if (tid == 0) { s_range[0] = n; s_range[1] = nodeCount; s_stalled = 0; }
     __syncthreads();
-    // ---- PLOC iterations
+    // ---- PLOC iterations (best = -1, a node that found no area below FLT_MAX, counts as not mutual)
     while (s_range[0] > 1) {
         const int count = s_range[0], end = s_range[1], start = end - count;
         for (int i = tid; i < count; i += nt) {
@@ -228,15 +230,16 @@ __global__ void __launch_bounds__(1024) k_tlas_build(TlasBuildArgs a) {
         __syncthreads();
         if (tid == 0) {
             int merged = 0;
-            for (int i = 0; i < count; i++) { const int b = a.pref[i], c = a.pref[b]; if (i == c && i < b) merged += 2; }
+            for (int i = 0; i < count; i++) { const int b = a.pref[i]; if (b >= 0 && a.pref[b] == i && i < b) merged += 2; }
+            if (merged == 0) { s_stalled = 1; s_range[0] = 1; }   // nothing would ever merge again: stop, report -1
             const int unmerged = count - merged, newNodes = merged / 2;
             int mergedHead = end - merged;
             const int newBegin = mergedHead - unmerged - newNodes;
             int unmergedHead = newBegin;
             for (int i = 0; i < count; i++) {
-                const int b = a.pref[i], c = a.pref[b];
+                const int b = a.pref[i];
                 const int aId = i + start;
-                if (i == c) {
+                if (b >= 0 && a.pref[b] == i) {
                     if (i < b) {
                         const int bId = b + start;
                         const float4 cA0 = a.nodes[2 * aId], cB0 = a.nodes[2 * aId + 1], cA1 = a.nodes[2 * bId], cB1 = a.nodes[2 * bId + 1];
@@ -252,7 +255,7 @@ __global__ void __launch_bounds__(1024) k_tlas_build(TlasBuildArgs a) {
                     unmergedHead++;
                 }
             }
-            s_range[0] = count - merged / 2;
+            if (!s_stalled) s_range[0] = count - merged / 2;
             s_range[1] = end - merged;
             a.pref[0] = newBegin;        // hand the copy range to the other threads
         }
@@ -265,11 +268,300 @@ __global__ void __launch_bounds__(1024) k_tlas_build(TlasBuildArgs a) {
     }
     // stack entries the TLAS walk (BVHIntersect.glsl:205-272, fixed 24-entry stack) needs = the height of the tree; children
     // always follow their parent in the array, so one backward sweep suffices. The host rejects a TLAS that is too deep.
-    if (tid == 0) {
+    if (tid == 0 && s_stalled) a.need[0] = -1;
+    if (tid == 0 && !s_stalled) {
         for (int i = nodeCount - 1; i >= 0; i--) {
             const uint32_t w = __float_as_uint(a.nodes[2 * i].w);
             const int c = (int)(w & 0x7FFFFFFFu);
             a.need[i] = (w >> 31) ? 0 : 1 + max(a.need[c], a.need[c + 1]);
+        }
+    }
+}
+
+// ------------------------------------------------------------------------------------------------ TLAS build over the grid
+// The same tree as idkhost_tlas_build (TLAS.cs:28-141), node for node, for any instance count the node format holds
+// (2n - 1 < 2^31), with the work spread over the GPU:
+//   k_tlas_leaves  one thread per instance: Box.Transformed of its BLAS root, its instance index, a partial global box per block
+//   k_tlas_bounds  one block: the global box from the partials (min / max are exact, so any order gives the same box)
+//   k_tlas_keys    one thread per leaf: centreKey
+//   cub::DeviceRadixSort::SortPairs of (key, instance) over 30 bits: stable, so equal keys keep their instance order, as
+//                  TLAS.Build's sort does
+//   k_tlas_ploc    one cooperative launch runs every PLOC iteration; grid-wide barriers separate its three phases:
+//     search  one thread per active node tests [max(i - r, 0), min(i + r + 1, count)) in increasing j from a tile of boxes and
+//             its 2r halo in shared memory; a strict < keeps the first smallest area, as TLAS.cs:65-74
+//     count   with b = pref[i], mutual = pref[b] == i and lo = mutual && i < b, node i emits into the new / unmerged region
+//             exactly when !mutual || lo; each block sums emit and lo over its chunk
+//     place   node i's slot there is newBegin + excl_sum(emit)[i]; when lo holds its two children go to
+//             end - merged + 2 excl_sum(lo)[i], with merged = 2 sum(lo), unmerged = count - merged and
+//             newBegin = end - merged - unmerged - merged / 2: the positions TLAS.cs:76-139 hands out one by one
+// The active nodes ping-pong between two scratch arrays. A merged pair is final once placed (no later iteration reaches
+// behind the new active range), so it goes straight into the output. Every active node carries its height (0 for a leaf,
+// 1 + max of its children): the root's is the stack the TLAS walk needs. Heights only grow, so the build stops as soon as a
+// parent exceeds IDK_TLAS_STACK_SIZE; that tree would be refused anyway, and identical boxes (one merge per iteration) stop
+// after IDK_TLAS_STACK_SIZE + 1 iterations instead of n. An iteration that merges nothing also stops the build. While some
+// pair has a half area below FLT_MAX, the smallest node of a cycle of first-smallest picks and its pick choose each other, so
+// only nodes that find no area below FLT_MAX (best = -1: a NaN or infinite box, or one whose half area overflows) get
+// there, and without the stop the loop would never end. Both kernels then report a need of -1; the caller refuses the tree.
+#define IDK_TLAS_BLOCK 256
+// Instance counts up to this build in k_tlas_build instead (DESIGN 8f.2: scripts/time_tlas_build.py times both builds at
+// n = 3 ... 16384 on libraries compiled with this overridden). The default is the largest measured n at which the single
+// CTA was faster.
+#ifndef IDK_TLAS_SINGLE_CTA_MAX
+#define IDK_TLAS_SINGLE_CTA_MAX 64
+#endif
+
+struct TlasGridArgs {
+    const float4* blasNodes;         // global GpuBlasNode array (2 x float4 each)
+    const GpuBlasDesc* descs;
+    const GpuBlasInstance* instances;
+    const float4* xforms;            // 9 x float4 per GpuMeshTransform, rows 0..2 = ModelMatrix
+    float4* nodes;                   // out: 2n-1 GpuTlasNode (2 x float4 each), root at 0
+    float4* bufA;                    // scratch: 2n-1 nodes each, the active range ping-pongs between them; the unsorted
+    float4* bufB;                    //   leaves sit in bufB[0, n) until k_tlas_ploc has gathered them
+    int* hA;                         // scratch: the height of every node of bufA / bufB
+    int* hB;
+    uint32_t* keys;                  // scratch: n each
+    uint32_t* keysSorted;
+    int* order;
+    int* orderSorted;
+    int* pref;                       // scratch: n
+    float* partial;                  // scratch: 6 per k_tlas_leaves block (min xyz, max xyz)
+    float* global;                   // scratch: 6
+    int* blockSums;                  // scratch: 2 per k_tlas_ploc block
+    int* status;                     // [0]: a parent exceeded IDK_TLAS_STACK_SIZE; [1] on exit: the stack entries the walk needs,
+                                     //   or -1 when an iteration merged nothing (see k_tlas_ploc)
+    int n, searchRadius, partialCount;
+};
+
+__device__ __forceinline__ void tlas_load_box(const float4* b, size_t i, float4& A, float4& B) {
+    A = __ldcg(b + 2 * i);           // written by other blocks of the same launch: read through L2
+    B = __ldcg(b + 2 * i + 1);
+}
+
+// block-wide exclusive scan of two counts, with the block's totals
+__device__ __forceinline__ void tlas_block_scan2(int x, int y, int& ex, int& ey, int& tx, int& ty, int (*s)[IDK_TLAS_BLOCK / 32]) {
+    const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
+    int ix = x, iy = y;
+#pragma unroll
+    for (int o = 1; o < 32; o <<= 1) {
+        const int px = __shfl_up_sync(0xffffffffu, ix, o), py = __shfl_up_sync(0xffffffffu, iy, o);
+        if (lane >= o) { ix += px; iy += py; }
+    }
+    if (lane == 31) { s[0][w] = ix; s[1][w] = iy; }
+    __syncthreads();
+    int bx = 0, by = 0;
+    tx = 0; ty = 0;
+#pragma unroll
+    for (int k = 0; k < IDK_TLAS_BLOCK / 32; k++) {
+        const int sx = s[0][k], sy = s[1][k];
+        if (k < w) { bx += sx; by += sy; }
+        tx += sx; ty += sy;
+    }
+    ex = bx + ix - x; ey = by + iy - y;
+    __syncthreads();
+}
+
+__global__ void __launch_bounds__(IDK_TLAS_BLOCK) k_tlas_leaves(TlasGridArgs a) {
+    using namespace idkbvh;
+    __shared__ float s_red[6][IDK_TLAS_BLOCK / 32];
+    const int i = blockIdx.x * IDK_TLAS_BLOCK + threadIdx.x;
+    float v[6] = {3.4028235e38f, 3.4028235e38f, 3.4028235e38f, -3.4028235e38f, -3.4028235e38f, -3.4028235e38f};
+    if (i < a.n) {
+        const GpuBlasInstance bi = a.instances[i];
+        const float4* root = a.blasNodes + 2 * ((size_t)a.descs[bi.BlasId].NodeOffset + 1);
+        const float4 rA = root[0], rB = root[1];
+        const float4* m = a.xforms + 9 * (size_t)bi.MeshTransformId;
+        const float4 m0 = m[0], m1 = m[1], m2 = m[2];
+        const float m12[12] = {m0.x, m0.y, m0.z, m0.w, m1.x, m1.y, m1.z, m1.w, m2.x, m2.y, m2.z, m2.w};
+        const Box b = transformedBox({{rA.x, rA.y, rA.z}, {rB.x, rB.y, rB.z}}, m12);
+        a.bufB[2 * (size_t)i] = make_float4(b.mn[0], b.mn[1], b.mn[2], __uint_as_float(0x80000000u | (uint32_t)i));
+        a.bufB[2 * (size_t)i + 1] = make_float4(b.mx[0], b.mx[1], b.mx[2], 0.0f);
+        a.order[i] = i;
+        for (int k = 0; k < 3; k++) { v[k] = b.mn[k]; v[3 + k] = b.mx[k]; }
+    }
+    if (i == 0) a.status[0] = 0;
+    for (int k = 0; k < 6; k++) {
+        float x = v[k];
+        for (int off = 16; off > 0; off >>= 1) {
+            const float o = __shfl_down_sync(0xffffffffu, x, off);
+            x = k < 3 ? fminf(x, o) : fmaxf(x, o);
+        }
+        if ((threadIdx.x & 31) == 0) s_red[k][threadIdx.x >> 5] = x;
+    }
+    __syncthreads();
+    if (threadIdx.x < 6) {
+        const int k = threadIdx.x;
+        float x = s_red[k][0];
+        for (int w = 1; w < IDK_TLAS_BLOCK / 32; w++) x = k < 3 ? fminf(x, s_red[k][w]) : fmaxf(x, s_red[k][w]);
+        a.partial[6 * (size_t)blockIdx.x + k] = x;
+    }
+}
+
+__global__ void __launch_bounds__(1024) k_tlas_bounds(TlasGridArgs a) {
+    __shared__ float s_red[6][32];
+    float v[6] = {3.4028235e38f, 3.4028235e38f, 3.4028235e38f, -3.4028235e38f, -3.4028235e38f, -3.4028235e38f};
+    for (int p = threadIdx.x; p < a.partialCount; p += blockDim.x)
+        for (int k = 0; k < 6; k++) v[k] = k < 3 ? fminf(v[k], a.partial[6 * (size_t)p + k]) : fmaxf(v[k], a.partial[6 * (size_t)p + k]);
+    for (int k = 0; k < 6; k++) {
+        float x = v[k];
+        for (int off = 16; off > 0; off >>= 1) {
+            const float o = __shfl_down_sync(0xffffffffu, x, off);
+            x = k < 3 ? fminf(x, o) : fmaxf(x, o);
+        }
+        if ((threadIdx.x & 31) == 0) s_red[k][threadIdx.x >> 5] = x;
+    }
+    __syncthreads();
+    if (threadIdx.x < 6) {
+        const int k = threadIdx.x;
+        float x = s_red[k][0];
+        for (int w = 1; w < (int)(blockDim.x + 31) / 32; w++) x = k < 3 ? fminf(x, s_red[k][w]) : fmaxf(x, s_red[k][w]);
+        a.global[k] = x;
+    }
+}
+
+// Morton code of the box centre mapped to [0, 1] by the global box (MyMath.GetMortonCode30 / MapToZeroOne)
+__global__ void __launch_bounds__(IDK_TLAS_BLOCK) k_tlas_keys(TlasGridArgs a) {
+    using namespace idkbvh;
+    const int i = blockIdx.x * IDK_TLAS_BLOCK + threadIdx.x;
+    if (i >= a.n) return;
+    const float4 A = a.bufB[2 * (size_t)i], B = a.bufB[2 * (size_t)i + 1];
+    a.keys[i] = centreKey({{A.x, A.y, A.z}, {B.x, B.y, B.z}}, {{a.global[0], a.global[1], a.global[2]}, {a.global[3], a.global[4], a.global[5]}});
+}
+
+// Launched cooperatively (grid.sync) with (IDK_TLAS_BLOCK + 2 searchRadius) * 6 floats of dynamic shared memory.
+__global__ void __launch_bounds__(IDK_TLAS_BLOCK) k_tlas_ploc(TlasGridArgs a) {
+    using namespace idkbvh;
+    namespace cg = cooperative_groups;
+    extern __shared__ float s_box[];                  // 6 planes (min xyz, max xyz) of span boxes
+    __shared__ int s_scan[2][IDK_TLAS_BLOCK / 32];
+    cg::grid_group grid = cg::this_grid();
+    const int T = IDK_TLAS_BLOCK, tid = threadIdx.x, G = gridDim.x, r = a.searchRadius, n = a.n, span = T + 2 * r;
+    int count = n, end = 2 * n - 1;
+    // the Morton-ordered leaves into the back of the array, height 0
+    for (int k = blockIdx.x * T + tid; k < n; k += G * T) {
+        const size_t src = (size_t)a.orderSorted[k], dst = (size_t)(end - n + k);
+        a.bufA[2 * dst] = a.bufB[2 * src];
+        a.bufA[2 * dst + 1] = a.bufB[2 * src + 1];
+        a.hA[dst] = 0;
+    }
+    float4* cur = a.bufA;
+    float4* nxt = a.bufB;
+    int* hc = a.hA;
+    int* hn = a.hB;
+    bool deep = false, stalled = false;
+    grid.sync();
+    while (count > 1) {
+        const int start = end - count;
+        const int per = (count + G - 1) / G, chunk = (per + T - 1) / T * T;
+        const int c0 = (int)min((long long)blockIdx.x * chunk, (long long)count), c1 = min(c0 + chunk, count);
+        // ---- search: the best partner of every node of this block's chunk, as a local index
+        for (int t0 = c0; t0 < c1; t0 += T) {
+            const int base = t0 - r, lo = max(base, 0), hi = min(t0 + T + r, count);
+            for (int j = lo + tid; j < hi; j += T) {
+                float4 A, B;
+                tlas_load_box(cur, (size_t)(start + j), A, B);
+                const int s = j - base;
+                s_box[s] = A.x; s_box[span + s] = A.y; s_box[2 * span + s] = A.z;
+                s_box[3 * span + s] = B.x; s_box[4 * span + s] = B.y; s_box[5 * span + s] = B.z;
+            }
+            __syncthreads();
+            const int i = t0 + tid;
+            if (i < c1) {
+                const int si = i - base;
+                const Box bi = {{s_box[si], s_box[span + si], s_box[2 * span + si]}, {s_box[3 * span + si], s_box[4 * span + si], s_box[5 * span + si]}};
+                const int s = max(i - r, 0), e = min(i + r + 1, count);
+                float smallest = 3.4028235e38f;
+                int best = -1;
+                for (int j = s; j < e; j++) {
+                    if (j == i) continue;
+                    const int sj = j - base;
+                    const Box bj = {{s_box[sj], s_box[span + sj], s_box[2 * span + sj]}, {s_box[3 * span + sj], s_box[4 * span + sj], s_box[5 * span + sj]}};
+                    const float area = halfArea(combine(bi, bj));
+                    if (area < smallest) { smallest = area; best = j; }
+                }
+                a.pref[i] = best;
+            }
+            __syncthreads();
+        }
+        grid.sync();
+        // ---- count: emit and lo over this block's chunk
+        auto flags = [&](int i, int& b, int& emit, int& lo) {
+            b = __ldcg(a.pref + i);
+            const bool mutual = b >= 0 && __ldcg(a.pref + b) == i;   // b < 0 only when every area is >= FLT_MAX
+            lo = mutual && i < b;
+            emit = !mutual || lo;
+        };
+        {
+            int ne = 0, nl = 0;
+            for (int i = c0 + tid; i < c1; i += T) {
+                int b, e, l;
+                flags(i, b, e, l);
+                ne += e; nl += l;
+            }
+            int ex, ey, tx, ty;
+            tlas_block_scan2(ne, nl, ex, ey, tx, ty, s_scan);
+            if (tid == 0) { a.blockSums[2 * blockIdx.x] = tx; a.blockSums[2 * blockIdx.x + 1] = ty; }
+        }
+        grid.sync();
+        // ---- place: the blocks before this one give its first slots; a block scan per tile gives each node's
+        int merged, runE, runL;
+        {
+            int pe = 0, pl = 0, te = 0, tl = 0;
+            for (int k = tid; k < G; k += T) {
+                const int e = __ldcg(a.blockSums + 2 * k), l = __ldcg(a.blockSums + 2 * k + 1);
+                if (k < (int)blockIdx.x) { pe += e; pl += l; }
+                te += e; tl += l;
+            }
+            int ex, ey, emits, los;
+            tlas_block_scan2(pe, pl, ex, ey, runE, runL, s_scan);
+            tlas_block_scan2(te, tl, ex, ey, emits, los, s_scan);
+            merged = 2 * los;
+        }
+        if (merged == 0) { stalled = true; break; }      // every block has the same sums: nothing would ever merge again
+        const int unmerged = count - merged, newBegin = end - merged - unmerged - merged / 2, mergedBegin = end - merged;
+        for (int t0 = c0; t0 < c1; t0 += T) {
+            const int i = t0 + tid;
+            int b = -1, emit = 0, lo = 0;
+            if (i < c1) flags(i, b, emit, lo);
+            int ee, el, te, tl;
+            tlas_block_scan2(emit, lo, ee, el, te, tl, s_scan);
+            if (emit) {
+                const size_t slot = (size_t)(newBegin + runE + ee);
+                float4 nA, nB;
+                tlas_load_box(cur, (size_t)(start + i), nA, nB);
+                if (lo) {
+                    const size_t head = (size_t)(mergedBegin + 2 * (runL + el));
+                    float4 oA, oB;
+                    tlas_load_box(cur, (size_t)(start + b), oA, oB);
+                    a.nodes[2 * head] = nA; a.nodes[2 * head + 1] = nB;
+                    a.nodes[2 * head + 2] = oA; a.nodes[2 * head + 3] = oB;
+                    nxt[2 * slot] = make_float4(minN(nA.x, oA.x), minN(nA.y, oA.y), minN(nA.z, oA.z), __uint_as_float((uint32_t)head));
+                    nxt[2 * slot + 1] = make_float4(maxN(nB.x, oB.x), maxN(nB.y, oB.y), maxN(nB.z, oB.z), 0.0f);
+                    const int h = 1 + max(__ldcg(hc + start + i), __ldcg(hc + start + b));
+                    hn[slot] = h;
+                    if (h > IDK_TLAS_STACK_SIZE) a.status[0] = 1;
+                } else {
+                    nxt[2 * slot] = nA; nxt[2 * slot + 1] = nB;
+                    hn[slot] = __ldcg(hc + start + i);
+                }
+            }
+            runE += te; runL += tl;
+        }
+        grid.sync();
+        if (__ldcg(a.status)) { deep = true; break; }   // every block reads the same flag behind the same barrier
+        count -= merged / 2;
+        end -= merged;
+        float4* tb = cur; cur = nxt; nxt = tb;
+        int* th = hc; hc = hn; hn = th;
+    }
+    if (blockIdx.x == 0 && tid == 0) {
+        if (stalled) {
+            a.status[1] = -1;
+        } else if (deep) {
+            a.status[1] = IDK_TLAS_STACK_SIZE + 1;
+        } else {
+            a.nodes[0] = __ldcg(cur); a.nodes[1] = __ldcg(cur + 1);
+            a.status[1] = __ldcg(hc);
         }
     }
 }

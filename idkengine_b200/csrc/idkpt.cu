@@ -1554,6 +1554,7 @@ static int preload_kernels(IdkPtCtx* ctx) {
     IDK_PRELOAD(k_sort_histogram); IDK_PRELOAD(k_sort_scan); IDK_PRELOAD(k_sort_scatter);
     IDK_PRELOAD(k_trace_rays); IDK_PRELOAD(k_trace_rays_any); IDK_PRELOAD(k_shadows_ray_traced);
     IDK_PRELOAD(k_skin_vertices); IDK_PRELOAD(k_refit_prepare); IDK_PRELOAD(k_refit_climb); IDK_PRELOAD(k_tlas_build);
+    IDK_PRELOAD(k_tlas_leaves); IDK_PRELOAD(k_tlas_bounds); IDK_PRELOAD(k_tlas_keys); IDK_PRELOAD(k_tlas_ploc);
     IDK_PRELOAD(k_bloom_down); IDK_PRELOAD(k_bloom_up); IDK_PRELOAD(k_agx_matrices); IDK_PRELOAD(k_tonemap);
     IDK_PRELOAD(k_denoise_prepare); IDK_PRELOAD(k_denoise_atrous); IDK_PRELOAD(k_denoise_finish); IDK_PRELOAD(k_denoise_import);
     IDK_PRELOAD(k_bcn_decode); IDK_PRELOAD(k_point_shadow_faces); IDK_PRELOAD(k_volumetric_march); IDK_PRELOAD(k_volumetric_upscale);
@@ -1985,26 +1986,66 @@ IDKPT_API int idkpt_blas_refit(IdkPtCtx* ctx, uint32_t first, uint32_t count, fl
     return rc;
 }
 
-// k_tlas_build of n >= 1 instances over the given device arrays into `out` (2n - 1 nodes), with its scratch in the context's
-// tlasScratch. On return *need is the device address of the built tree's height (valid once the stream has finished).
+// The TLAS build of n >= 1 instances over the given device arrays into `out` (2n - 1 nodes), with its scratch in the context's
+// tlasScratch. Up to IDK_TLAS_SINGLE_CTA_MAX instances k_tlas_build, above it the grid build (k_tlas_ploc): four kernels, the
+// radix sort and one cooperative launch. Neither synchronises with the host. On return
+// *need is the device address of the built tree's height (valid once the stream has finished); a value above
+// IDK_TLAS_STACK_SIZE means the build stopped at the first parent deeper than the walk's stack, and -1 that an iteration
+// merged nothing (a box that is not finite); in both cases `out` is not a tree.
 static int enqueue_tlas_build(IdkPtCtx* ctx, const void* blasNodes, const void* descs, const void* instances, const void* xforms,
                               void* out, uint64_t n, int searchRadius, int** need) {
-    const size_t nodeCount = 2 * n - 1;
-    const size_t tempOff = 0, leavesOff = nodeCount * 32, keysOff = leavesOff + n * 32, prefOff = keysOff + n * 4, needOff = prefOff + n * 4;
-    CK(ensure(ctx->tlasScratch, needOff + nodeCount * 4 + 64));
-    TlasBuildArgs a;
+    if (n <= IDK_TLAS_SINGLE_CTA_MAX) {                   // one launch beats the grid build's nine at a few dozen instances
+        const size_t nodeCount = 2 * n - 1;
+        const size_t tempOff = 0, leavesOff = nodeCount * 32, keysOff = leavesOff + n * 32, prefOff = keysOff + n * 4, needOff = prefOff + n * 4;
+        CK(ensure(ctx->tlasScratch, needOff + nodeCount * 4 + 64));
+        TlasBuildArgs a;
+        a.blasNodes = (const float4*)blasNodes; a.descs = (const GpuBlasDesc*)descs; a.instances = (const GpuBlasInstance*)instances;
+        a.xforms = (const float4*)xforms; a.nodes = (float4*)out;
+        a.temp = (float4*)((char*)ctx->tlasScratch.p + tempOff); a.leaves = (float4*)((char*)ctx->tlasScratch.p + leavesOff);
+        a.keys = (uint32_t*)((char*)ctx->tlasScratch.p + keysOff); a.pref = (int*)((char*)ctx->tlasScratch.p + prefOff);
+        a.need = (int*)((char*)ctx->tlasScratch.p + needOff);
+        a.n = (int)n; a.searchRadius = searchRadius;
+        k_tlas_build<<<1, 1024, 0, ctx->stream>>>(a);
+        *need = a.need;
+        return IDKPT_OK;
+    }
+    const int T = IDK_TLAS_BLOCK;
+    const size_t nodeCount = 2 * n - 1, leafBlocks = (n + T - 1) / T;
+    const int smem = (T + 2 * searchRadius) * 6 * (int)sizeof(float);
+    CK(cudaFuncSetAttribute(k_tlas_ploc, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+    int perSm = 0;
+    CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&perSm, k_tlas_ploc, T, smem));
+    if (perSm < 1) return fail(ctx, IDKPT_ERR_CUDA, "TLAS build: k_tlas_ploc does not fit on an SM");
+    const int G = (int)std::min<size_t>((size_t)perSm * ctx->smCount, leafBlocks);   // co-resident, as grid.sync needs
+    size_t sortBytes = 0;
+    CK(cub::DeviceRadixSort::SortPairs(nullptr, sortBytes, (const uint32_t*)nullptr, (uint32_t*)nullptr, (const int*)nullptr,
+                                       (int*)nullptr, (int)n, 0, 30, ctx->stream));
+    size_t off = 0;
+    auto take = [&](size_t bytes) { const size_t o = off; off += (bytes + 255) & ~(size_t)255; return o; };
+    const size_t oA = take(nodeCount * 32), oB = take(nodeCount * 32), ohA = take(nodeCount * 4), ohB = take(nodeCount * 4);
+    const size_t oKeys = take(n * 4), oKeysSorted = take(n * 4), oOrder = take(n * 4), oOrderSorted = take(n * 4), oPref = take(n * 4);
+    const size_t oPartial = take(leafBlocks * 24), oGlobal = take(24), oSums = take((size_t)G * 8), oStatus = take(8), oSort = take(sortBytes);
+    CK(ensure(ctx->tlasScratch, off));
+    char* s = (char*)ctx->tlasScratch.p;
+    TlasGridArgs a;
     a.blasNodes = (const float4*)blasNodes; a.descs = (const GpuBlasDesc*)descs; a.instances = (const GpuBlasInstance*)instances;
     a.xforms = (const float4*)xforms; a.nodes = (float4*)out;
-    a.temp = (float4*)((char*)ctx->tlasScratch.p + tempOff); a.leaves = (float4*)((char*)ctx->tlasScratch.p + leavesOff);
-    a.keys = (uint32_t*)((char*)ctx->tlasScratch.p + keysOff); a.pref = (int*)((char*)ctx->tlasScratch.p + prefOff);
-    a.need = (int*)((char*)ctx->tlasScratch.p + needOff);
-    a.n = (int)n; a.searchRadius = searchRadius;
-    k_tlas_build<<<1, 1024, 0, ctx->stream>>>(a);
-    *need = a.need;
+    a.bufA = (float4*)(s + oA); a.bufB = (float4*)(s + oB); a.hA = (int*)(s + ohA); a.hB = (int*)(s + ohB);
+    a.keys = (uint32_t*)(s + oKeys); a.keysSorted = (uint32_t*)(s + oKeysSorted);
+    a.order = (int*)(s + oOrder); a.orderSorted = (int*)(s + oOrderSorted); a.pref = (int*)(s + oPref);
+    a.partial = (float*)(s + oPartial); a.global = (float*)(s + oGlobal); a.blockSums = (int*)(s + oSums); a.status = (int*)(s + oStatus);
+    a.n = (int)n; a.searchRadius = searchRadius; a.partialCount = (int)leafBlocks;
+    k_tlas_leaves<<<(unsigned)leafBlocks, T, 0, ctx->stream>>>(a);
+    k_tlas_bounds<<<1, 1024, 0, ctx->stream>>>(a);
+    k_tlas_keys<<<(unsigned)leafBlocks, T, 0, ctx->stream>>>(a);
+    CK(cub::DeviceRadixSort::SortPairs(s + oSort, sortBytes, a.keys, a.keysSorted, a.order, a.orderSorted, (int)n, 0, 30, ctx->stream));
+    void* args[] = {&a};
+    CK(cudaLaunchCooperativeKernel((const void*)k_tlas_ploc, dim3(G), dim3(T), args, (size_t)smem, ctx->stream));
+    *need = a.status + 1;
     return IDKPT_OK;
 }
 
-// BVH.TlasBuild on the device (BVH.cs:278-298, TLAS.cs:28-141): see k_tlas_build.
+// BVH.TlasBuild on the device (BVH.cs:278-298, TLAS.cs:28-141): see k_tlas_ploc.
 IDKPT_API int idkpt_tlas_build(IdkPtCtx* ctx, int32_t searchRadius, float* kernelMs) {
     if (!ctx) return IDKPT_ERR_INVALID_ARGUMENT;
     DRAIN_PENDING("idkpt_tlas_build");
@@ -2013,7 +2054,7 @@ IDKPT_API int idkpt_tlas_build(IdkPtCtx* ctx, int32_t searchRadius, float* kerne
     if (!ctx->counts.UseTlas) return fail(ctx, IDKPT_ERR_INVALID_ARGUMENT, "idkpt_tlas_build: the scene was set without UseTlas (no TLAS node array to fill)");
     if (searchRadius < 1 || searchRadius > 1024) return fail(ctx, IDKPT_ERR_INVALID_ARGUMENT, "idkpt_tlas_build: search radius out of range (TLAS.BuildSettings.SearchRadius, default 15)");
     const uint64_t n = ctx->counts.BlasInstanceCount;
-    if (n > 16384) return fail(ctx, IDKPT_ERR_UNSUPPORTED, "idkpt_tlas_build: more than 16384 instances (single-CTA build); build on the host and idkpt_update_range");
+    if (2 * n - 1 >= (1ull << 31)) return fail(ctx, IDKPT_ERR_UNSUPPORTED, "idkpt_tlas_build: more than 2^30 instances (TLAS child and instance ids are 31 bits)");
     CK(cudaSetDevice(ctx->device));
     int* needDev = nullptr;
     const int rc = run_timed(ctx, "idkpt_tlas_build", kernelMs, [&]() -> int {
@@ -2023,6 +2064,10 @@ IDKPT_API int idkpt_tlas_build(IdkPtCtx* ctx, int32_t searchRadius, float* kerne
     ctx->accumulatedSamples = 0;
     int need = 0;
     CK(cudaMemcpy(&need, needDev, 4, cudaMemcpyDeviceToHost));
+    if (need < 0) {                       // the PLOC loop merged nothing: the node array is not a tree
+        ctx->haveScene = false;
+        return fail(ctx, IDKPT_ERR_INVALID_ARGUMENT, "idkpt_tlas_build: an instance's world box is not finite or its half area overflows (ModelMatrix or BLAS root); scene invalidated; set it again");
+    }
     if (need > IDK_TLAS_STACK_SIZE) {     // the walk's stack is fixed (BVHIntersect.glsl:4): refuse to trace through a TLAS it cannot hold
         ctx->haveScene = false;
         return fail(ctx, IDKPT_ERR_UNSUPPORTED, "idkpt_tlas_build: the built TLAS is deeper than the 24-entry traversal stack of the TLAS walk (scene invalidated; set it again)");
@@ -2327,8 +2372,8 @@ static int validate_add_models(IdkPtCtx* ctx, const char* who, const IdkPtAddMod
     tex.Textures = m->Textures; tex.TextureCount = m->TextureCount;
     tex.Materials = m->Materials; tex.MaterialCount = m->MaterialCount;
     if (const char* terr = idk_validate_textures(&tex)) return texture_error(ctx, who, terr);
-    if (c.UseTlas && c.BlasInstanceCount + m->BlasInstanceCount > 16384)
-        return fail(ctx, who, IDKPT_ERR_UNSUPPORTED, "more than 16384 instances under UseTlas (single-CTA TLAS build)");
+    if (c.UseTlas && 2 * (c.BlasInstanceCount + m->BlasInstanceCount) - 1 >= (1ull << 31))
+        return fail(ctx, who, IDKPT_ERR_UNSUPPORTED, "more than 2^30 instances under UseTlas (TLAS child and instance ids are 31 bits)");
     return IDKPT_OK;
 }
 
@@ -2495,6 +2540,8 @@ IDKPT_API int idkpt_add_models(IdkPtCtx* ctx, const IdkPtAddModelsDesc* m, const
     if (needDev) {
         int need = 0;
         CK(cudaMemcpy(&need, needDev, 4, cudaMemcpyDeviceToHost));
+        if (need < 0)
+            return fail(ctx, who, IDKPT_ERR_INVALID_ARGUMENT, "an instance's world box is not finite or its half area overflows (ModelMatrix or BLAS root)");
         if (need > IDK_TLAS_STACK_SIZE)
             return fail(ctx, who, IDKPT_ERR_UNSUPPORTED, "the TLAS is deeper than the 24-entry traversal stack of the TLAS walk (BVHIntersect.glsl:4)");
     }

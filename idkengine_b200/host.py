@@ -68,6 +68,8 @@ def lib():
         L.idkhost_cache_close.argtypes = [ctypes.c_void_p]
         L.idkhost_transform_box.restype = None
         L.idkhost_transform_box.argtypes = [ctypes.c_void_p] * 5
+        L.idkhost_transform_boxes.restype = None
+        L.idkhost_transform_boxes.argtypes = [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int64, ctypes.c_void_p]
         L.idkhost_tlas_build.restype = None
         L.idkhost_tlas_build.argtypes = [ctypes.c_void_p, ctypes.c_int32, ctypes.c_void_p, ctypes.c_int32]
         L.idkhost_blas_global_sah.restype = ctypes.c_double
@@ -76,6 +78,19 @@ def lib():
         L.idkhost_default_build_settings.argtypes = [ctypes.POINTER(IdkBlasBuildSettings)]
         _lib = L
     return _lib
+
+
+def instance_boxes(scene):
+    """World-space box of every BLAS instance of `scene`, n x {min[3], max[3]} float32: Box.Transformed of its BLAS root by its
+    ModelMatrix (SRC/Shapes/Box.cs:166-175), all instances in one host call."""
+    inst = scene.blas_instances
+    roots = scene.blas_nodes[scene.blas_descs["NodeOffset"][inst["BlasId"]] + 1]
+    r = np.ascontiguousarray(np.concatenate([roots["Min"], roots["Max"]], axis=1), np.float32)
+    m = np.ascontiguousarray(scene.mesh_transforms["ModelMatrix"][inst["MeshTransformId"]], np.float32)
+    boxes = np.zeros((len(inst), 6), np.float32)
+    if len(inst):
+        lib().idkhost_transform_boxes(r.ctypes.data, m.ctypes.data, len(inst), boxes.ctypes.data)
+    return boxes
 
 
 def default_build_settings():
@@ -445,14 +460,8 @@ class Scene:
         """BVH.TlasBuild (SRC/Bvh/BVH.cs:278-298) + TLAS.Build (SRC/Bvh/TLAS.cs:28-141): world-space bounds of every BLAS
         instance (Box.Transformed of the BLAS root by its ModelMatrix), serial PLOC; sets BVH.GpuUseTlas."""
         n = len(self.blas_instances)
-        boxes = np.zeros((n, 6), np.float32)
+        boxes = instance_boxes(self)
         L = lib()
-        for i, inst in enumerate(self.blas_instances):
-            root = self.blas_nodes[self.blas_descs[inst["BlasId"]]["NodeOffset"] + 1]
-            mn = np.ascontiguousarray(root["Min"], np.float32)
-            mx = np.ascontiguousarray(root["Max"], np.float32)
-            m = np.ascontiguousarray(self.mesh_transforms[inst["MeshTransformId"]]["ModelMatrix"], np.float32)
-            L.idkhost_transform_box(mn.ctypes.data, mx.ctypes.data, m.ctypes.data, boxes[i, :3].ctypes.data, boxes[i, 3:].ctypes.data)
         self.tlas_nodes = np.zeros(max(2 * n - 1, 0), gt.GpuTlasNode)
         if n:
             L.idkhost_tlas_build(boxes.ctypes.data, n, self.tlas_nodes.ctypes.data, search_radius)

@@ -701,6 +701,17 @@ void idkhost_transform_box(const float mn[3], const float mx[3], const float mod
     for (int i = 0; i < 3; i++) { outMin[i] = b.mn[i]; outMax[i] = b.mx[i]; }
 }
 
+// idkhost_transform_box over n instances in one call: out[6 i ...] = Box.Transformed(roots[i], models[i]); roots = n x {min[3],
+// max[3]}, models = n x 12 floats (the rows of each 3x4 model matrix).
+__attribute__((visibility("default")))
+void idkhost_transform_boxes(const float* roots, const float* models, int64_t n, float* out) {
+    for (int64_t i = 0; i < n; i++) {
+        const float* r = roots + 6 * i;
+        const Box b = transformedBox({{r[0], r[1], r[2]}, {r[3], r[4], r[5]}}, models + 12 * i);
+        for (int k = 0; k < 3; k++) { out[6 * i + k] = b.mn[k]; out[6 * i + 3 + k] = b.mx[k]; }
+    }
+}
+
 // TLAS.Build: boxes = primitiveCount x {min[3], max[3]} (world space), nodes = 2*primitiveCount-1 GpuTlasNode, root at 0.
 __attribute__((visibility("default")))
 void idkhost_tlas_build(const float* boxes, int32_t primitiveCount, GpuTlasNode* nodes, int32_t searchRadius) {
@@ -733,16 +744,17 @@ void idkhost_tlas_build(const float* boxes, int32_t primitiveCount, GpuTlasNode*
             int s = std::max(a - searchRadius, activeRangeStart), e = std::min(a + searchRadius + 1, activeRangeEnd);
             pref[i] = findBestMatch(nodes, s, e, a) - activeRangeStart;
         }
-        int merged = 0;
-        for (int i = 0; i < activeRangeCount; i++) { int b = pref[i], c = pref[b]; if (i == c && i < b) merged += 2; }
+        int merged = 0;       // b < 0: the node found no half area below FLT_MAX (a box that is not finite)
+        for (int i = 0; i < activeRangeCount; i++) { int b = pref[i]; if (b >= 0 && pref[b] == i && i < b) merged += 2; }
+        if (merged == 0) return;   // nothing would ever merge again: the nodes are not a tree (the device build reports it)
         const int unmerged = activeRangeCount - merged, newNodes = merged / 2;
         int mergedHead = activeRangeEnd - merged;
         const int newBegin = mergedHead - unmerged - newNodes;
         int unmergedHead = newBegin;
         for (int i = 0; i < activeRangeCount; i++) {
-            int b = pref[i], c = pref[b];
+            int b = pref[i];
             int aId = i + activeRangeStart;
-            if (i == c) {
+            if (b >= 0 && pref[b] == i) {
                 if (i < b) {
                     int bId = b + activeRangeStart;
                     temp[mergedHead] = nodes[aId];

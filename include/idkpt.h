@@ -613,7 +613,14 @@ IDKPT_API int idkpt_blas_refit(IdkPtCtx* ctx, uint32_t first_blas, uint32_t coun
 IDKPT_API int idkpt_read_range(IdkPtCtx* ctx, IdkPtArrayId which, uint64_t first, uint64_t count, void* out);
 /* BVH.TlasBuild() on the device (BVH.cs:278-298 + TLAS.Build, TLAS.cs:28-141, serial PLOC with TLAS.BuildSettings.SearchRadius = 15):
  * world bounds of every instance from the (refitted) BLAS roots and the current mesh transforms, both already in HBM; fills the
- * scene's TLAS node array (UseTlas scenes) with exactly the nodes the host build produces -- a moving scene reads nothing back. */
+ * scene's TLAS node array (UseTlas scenes) with exactly the nodes the host build produces -- a moving scene reads nothing back.
+ * Any instance count the node format holds (31-bit child and instance ids: 2n - 1 < 2^31; above, IDKPT_ERR_UNSUPPORTED). Up
+ * to 64 instances one CTA builds the tree; above, the build is spread over the GPU. search_radius: 1..1024.
+ * The TLAS walk's stack has 24 entries (BVHIntersect.glsl:4), so a tree deeper than 24 is refused with IDKPT_ERR_UNSUPPORTED
+ * and invalidates the scene (set it again). Large scenes can reach that depth: the radius-15 tree of 262144 uniformly
+ * scattered boxes is 25 deep, of 1 M boxes in 64 clusters 35. Identical boxes make a chain and are refused after 25 PLOC
+ * iterations, not after n. An instance box that is not finite (a NaN or infinite ModelMatrix or BLAS root) stops the build
+ * with IDKPT_ERR_INVALID_ARGUMENT and also invalidates the scene. */
 IDKPT_API int idkpt_tlas_build(IdkPtCtx* ctx, int32_t search_radius, float* kernel_ms);
 
 /* BLAS.Build + PreSplitting.PreSplit on the device (the loop body of BVH.BlasesBuild, BVH.cs:315-377): the SweepSAH build of
@@ -727,11 +734,12 @@ IDKPT_API int idkpt_blas_sah(IdkPtCtx* ctx, uint32_t first, uint32_t count, cons
  * swapped in only when all of it succeeded; a failed call leaves every array, count, desc, image, exported pointer and the
  * accumulation as they were. A call whose counts are all 0 does nothing and returns IDKPT_OK.
  * IDKPT_ERR_NO_SCENE: no scene. IDKPT_ERR_INVALID_ARGUMENT: a NULL pointer with a count, an id outside its call-local range,
+ * an instance world box under UseTlas that is not finite (see idkpt_tlas_build),
  * a desc without triangles or with a range outside Triangles, a non-finite setting, StopSplittingThreshold < 1, a scene whose
  * VertexCount and VertexPositionCount differ, or 2^31 or more nodes, triangles, vertices, meshes, materials, descs,
  * transforms or instances in total. IDKPT_ERR_UNSUPPORTED: a texture format the decoder lacks, more than 2^24 fragments in
- * one BLAS, a BlasStackSize beyond the shared-memory traversal stack, or with UseTlas more than 16384 instances (the
- * single-CTA TLAS build) or a TLAS deeper than 24 entries. kernel_ms (may be NULL): device time of the whole call. */
+ * one BLAS, a BlasStackSize beyond the shared-memory traversal stack, or with UseTlas more than 2^30 instances (31-bit TLAS
+ * node ids) or a TLAS deeper than 24 entries (see idkpt_tlas_build). kernel_ms (may be NULL): device time of the whole call. */
 typedef struct IdkPtAddModelsDesc {
     const GpuBlasTriangle*    Triangles;         uint64_t TriangleCount;        /* BVH.Add's source triangles: X/Y/Z index this call's vertices, MeshId its meshes */
     const GpuBlasDesc*        BlasDescs;         uint64_t BlasDescCount;        /* per new BLAS: TriangleOffset/TriangleCount into Triangles, IsRefittable */
