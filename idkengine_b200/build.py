@@ -55,7 +55,7 @@ def find_nvcc():
 def build_host(force=False, verbose=False):
     srcs = _sources(HOST_DIR, (".cpp",))
     # the builder's arithmetic is shared with libidkpt: an edit to it must rebuild both libraries
-    deps = srcs + _sources(INCLUDE_DIR, (".h",)) + [os.path.join(CSRC_DIR, "idk_bvh_math.h"), os.path.join(CSRC_DIR, "idk_cbrt.h")]
+    deps = srcs + _sources(INCLUDE_DIR, (".h",)) + [os.path.join(CSRC_DIR, f) for f in ("idk_bvh_math.h", "idk_cbrt.h", "idk_anim_math.h")]
     if not force and _newer(LIBIDKHOST, deps):
         return LIBIDKHOST
     cmd = ["g++", "-O2", "-std=c++17", "-ffp-contract=off", "-fPIC", "-shared", "-pthread",

@@ -6,6 +6,7 @@ import os
 import numpy as np
 
 from . import build as _build
+from . import gpu_types as gt
 
 c_i32, c_u32, c_u64, c_f = ctypes.c_int32, ctypes.c_uint32, ctypes.c_uint64, ctypes.c_float
 c_vp = ctypes.c_void_p
@@ -94,6 +95,9 @@ IDKPT_CREATE_GLOBAL_SLOTS = 1 << 12
 IDKPT_ARRAY_MESH_TRANSFORMS, IDKPT_ARRAY_MESHES, IDKPT_ARRAY_MATERIALS, IDKPT_ARRAY_LIGHTS = 0, 1, 2, 3
 IDKPT_ARRAY_TLAS_NODES, IDKPT_ARRAY_BLAS_NODES, IDKPT_ARRAY_VERTEX_POSITIONS, IDKPT_ARRAY_VERTICES = 4, 5, 6, 7
 IDKPT_ARRAY_BLAS_TRIANGLES, IDKPT_ARRAY_BLAS_DESCS = 8, 9
+IDKPT_ARRAY_NODE_LOCAL_TRANSFORMS, IDKPT_ARRAY_NODE_GLOBAL_TRANSFORMS, IDKPT_ARRAY_JOINT_MATRICES = 10, 11, 12
+IDKPT_ANIM_SCALE, IDKPT_ANIM_ROTATION, IDKPT_ANIM_TRANSLATION = 0, 1, 2
+IDKPT_ANIM_STEP, IDKPT_ANIM_LINEAR = 0, 1
 
 # every symbol include/idkpt.h declares
 EXPORTS = [
@@ -105,6 +109,7 @@ EXPORTS = [
     "idkpt_result_device_ptr", "idkpt_tile_rows",
     "idkpt_read_wavefront_rays", "idkpt_trace_rays", "idkpt_trace_rays_any", "idkpt_shadows_ray_traced",
     "idkpt_shadows_ray_traced_gbuffer", "idkpt_shadows_device_ptr", "idkpt_volumetric_lighting_gbuffer",
+    "idkpt_set_animations", "idkpt_enable_animations", "idkpt_set_node_transforms", "idkpt_update_models",
     "idkpt_set_skinning_data", "idkpt_skin_vertices", "idkpt_blas_refit", "idkpt_read_range", "idkpt_post_process", "idkpt_ldr_device_ptr", "idkpt_abi_version",
     "idkpt_denoise", "idkpt_denoise_device_ptrs", "idkpt_denoise_import_output", "idkpt_tlas_build",
     "idkpt_set_point_shadows", "idkpt_render_point_shadows", "idkpt_read_point_shadow", "idkpt_point_shadow_device_ptr",
@@ -335,6 +340,44 @@ def add_models_desc(records, textures=(), unskinned=None):
     return d, keep
 
 
+class IdkPtAnimationDesc(ctypes.Structure):
+    """idkpt_set_animations' flat arrays (ModelManager's CPU model state)."""
+    _fields_ = [
+        ("Nodes", c_vp), ("NodeCount", c_u64),
+        ("Channels", c_vp), ("ChannelCount", c_u64),
+        ("Animations", c_vp), ("AnimationCount", c_u64),
+        ("Skins", c_vp), ("SkinCount", c_u64),
+        ("JointNodes", c_vp), ("JointCount", c_u64),
+        ("InverseJointMatrices", c_vp),
+        ("KeyFrameTimes", c_vp), ("KeyFrameTimeCount", c_u64),
+        ("KeyFrameData", c_vp), ("KeyFrameDataCount", c_u64),
+    ]
+
+
+assert ctypes.sizeof(IdkPtAnimationDesc) == 120
+
+
+def animation_desc(anim):
+    """IdkPtAnimationDesc borrowing the arrays of a host.Animations. Returns (desc, keepalive)."""
+    keep = []
+
+    def ptr(a, dtype=None):
+        a = np.ascontiguousarray(a, dtype)
+        keep.append(a)
+        return (a.ctypes.data if a.size else None), len(a)
+
+    d = IdkPtAnimationDesc()
+    d.Nodes, d.NodeCount = ptr(anim.nodes, gt.IdkPtNode)
+    d.Channels, d.ChannelCount = ptr(anim.channels, gt.IdkPtNodeAnimation)
+    d.Animations, d.AnimationCount = ptr(anim.animations, gt.IdkPtModelAnimation)
+    d.Skins, d.SkinCount = ptr(anim.skins, gt.IdkPtSkin)
+    d.JointNodes, d.JointCount = ptr(anim.joint_nodes, np.uint32)
+    d.InverseJointMatrices, _ = ptr(np.asarray(anim.inverse_joints, np.float32).reshape(-1, 16), np.float32)
+    d.KeyFrameTimes, d.KeyFrameTimeCount = ptr(anim.times, np.float32)
+    d.KeyFrameData, d.KeyFrameDataCount = ptr(anim.data, np.float32)
+    return d, keep
+
+
 def texture_descs(textures):
     """IdkPtTextureDesc array for a list of texture dicts (host.Scene.textures). Returns (array, keepalive).
       uncompressed RGBA8:  dict(pixels [H, W, 4] uint8, srgb, wrap_s, wrap_t)
@@ -487,6 +530,14 @@ def load(path=None):
     L.idkpt_blas_rebuild.argtypes = [c_vp, c_u32, c_u32, P(IdkPtBlasBuildSettings), P(c_f)]
     L.idkpt_add_models.restype = c_i32
     L.idkpt_add_models.argtypes = [c_vp, P(IdkPtAddModelsDesc), P(IdkPtBlasBuildSettings), P(c_f)]
+    L.idkpt_set_animations.restype = c_i32
+    L.idkpt_set_animations.argtypes = [c_vp, P(IdkPtAnimationDesc)]
+    L.idkpt_enable_animations.restype = c_i32
+    L.idkpt_enable_animations.argtypes = [c_vp, c_u32, c_u32, c_vp]
+    L.idkpt_set_node_transforms.restype = c_i32
+    L.idkpt_set_node_transforms.argtypes = [c_vp, c_u32, c_u32, c_vp]
+    L.idkpt_update_models.restype = c_i32
+    L.idkpt_update_models.argtypes = [c_vp, c_f, c_i32, P(c_u32), P(c_f)]
     L.idkpt_blas_sah.restype = c_i32
     L.idkpt_blas_sah.argtypes = [c_vp, c_u32, c_u32, P(IdkPtBlasBuildSettings), c_vp]
     L.idkpt_denoise.restype = c_i32

@@ -10,6 +10,7 @@
 #include <vector>
 #include <algorithm>
 #include <cmath>
+#include <functional>
 
 #include "../../include/idkpt.h"
 #include "idk_kernels.cuh"
@@ -28,6 +29,7 @@
 #include "idk_sky.cuh"
 #include "idk_blas_build.cuh"
 #include "idk_scene_add.cuh"
+#include "idk_animation.cuh"
 #include "idk_textures_host.h"
 
 #define IDKPT_ABI_VERSION 4u   // 2: IdkPtSceneDesc gained Textures / TextureCount; 3: IdkPtStats gained CompactMs / AccumulateMs, host-buffer registration;
@@ -94,6 +96,19 @@ struct RasterState {
     RasterImage rtShadow[IDKPT_MAX_POINT_SHADOWS + 1];
 };
 
+// idkpt_set_animations' set: the plan's arrays on the device, the node state and this call's scratch (see k_anim_nodes)
+struct AnimState {
+    bool have = false;
+    idkanim::Plan plan;
+    std::vector<IdkPtSkinningCmd> cmds;                  // per skin, GetSkinningCommands
+    DevBuf channels, animations, enabled, groups, pairs, times, data, nodes, levelNodes, levelStart, skins, jointNodes,
+           inverseJoints, jointSlotSkin, jointSlotJoint, owner;
+    DevBuf locals, scratchLocals, globals, newGlobals, diffs, invSkin, pendingDirty, dirty, inSet, movedBits, joints, flags;
+    float prevTime = -FLT_MAX;                           // float.MinValue
+    uint64_t skinCheckedVersion = ~0ull, skinCheckedCount = 0;   // the skinning data the skins last passed check_skin_cmds on
+    bool runSkinning = false;
+};
+
 #define IDK_MAX_LANES 16
 
 struct Lane {
@@ -157,6 +172,7 @@ struct IdkPtCtx : IdkCtxBase {
     DevBuf unskinned, joints, refitParents, refitLocks, tlasScratch;
     DevBuf sahScratch;             // idkpt_blas_sah: the walk's stack and the per-BLAS results
     uint64_t unskinnedCount = 0;
+    uint64_t skinningDataVersion = 0;          // counts idkpt_set_skinning_data calls (idkpt_update_models' cached skin check)
     std::vector<uint32_t> unskinnedMaxJoint;   // per vertex max(JointIndices), host copy for range validation
     std::vector<GpuBlasDesc> hostDescs;
     std::vector<GpuBlasInstance> hostInstances;   // host mirror of `instances` (idkpt_set_scene): a bound voxeliser's draw list
@@ -165,6 +181,7 @@ struct IdkPtCtx : IdkCtxBase {
     // positions at the first idkpt_skin_vertices or idkpt_prev_positions_device_ptr after idkpt_set_scene or idkpt_add_models,
     // which release it.
     DevBuf prevPositions;
+    AnimState anim;                // idkpt_set_animations; idkpt_set_scene releases it
 
     // voxelisers reading this scene (idkvx_set_scene_from); idkpt_destroy unbinds them. sceneGeneration counts idkpt_set_scene,
     // idkpt_blas_rebuild and idkpt_add_models calls, so that a bound voxeliser knows when the instance list or the BLAS triangle counts, and
@@ -272,6 +289,15 @@ static void release_raster(RasterState& r) {
         for (DevBuf& b : img->buf) release(b);
     for (RasterImage& img : r.rtShadow) release(img.buf[0]);
     r = RasterState{};
+}
+
+static void release_anim(AnimState& a) {
+    for (DevBuf* b : {&a.channels, &a.animations, &a.enabled, &a.groups, &a.pairs, &a.times, &a.data, &a.nodes, &a.levelNodes,
+                      &a.levelStart, &a.skins, &a.jointNodes, &a.inverseJoints, &a.jointSlotSkin, &a.jointSlotJoint, &a.owner,
+                      &a.locals, &a.scratchLocals, &a.globals, &a.newGlobals, &a.diffs, &a.invSkin, &a.pendingDirty, &a.dirty,
+                      &a.inSet, &a.movedBits, &a.joints, &a.flags})
+        release(*b);
+    a = AnimState();
 }
 
 static int upload(IdkCtxBase* ctx, DevBuf& b, const void* src, size_t bytes) {
@@ -755,6 +781,7 @@ IDKPT_API void idkpt_destroy(IdkPtCtx* ctx) {
     for (DevBuf* b : all) release(*b);
     release_textures(ctx->tex);
     release_raster(ctx->raster);
+    release_anim(ctx->anim);
     for (int i = 0; i < IDK_MAX_LANES; i++) release_lane(ctx->lanes[i], false);
     for (cudaEvent_t ev : ctx->events) cudaEventDestroy(ev);
     gather_teardown(ctx);
@@ -802,6 +829,7 @@ IDKPT_API int idkpt_set_scene(IdkPtCtx* ctx, const IdkPtSceneDesc* s) {
     release(ctx->pointShadowDev); release(ctx->pointShadowMaps); release(ctx->pointShadowLights);
     release(ctx->prevPositions);
     release_raster(ctx->raster);   // the raster images belong to the old scene too
+    release_anim(ctx->anim);       // and the animation set
     int rc;
     // nodes and triangle records share one allocation ("bvh"): [nodes | triRec], so that one L2 access-policy window covers both
     const size_t nodeBytes = ((s->BlasNodeCount * sizeof(GpuBlasNode)) + 255) & ~(size_t)255;
@@ -1917,6 +1945,38 @@ IDKPT_API int idkpt_set_skinning_data(IdkPtCtx* ctx, const GpuUnskinnedVertex* v
     }
     CK(cudaStreamSynchronize(ctx->stream));
     ctx->unskinnedCount = count;
+    ctx->skinningDataVersion++;
+    return IDKPT_OK;
+}
+
+// idkpt_skin_vertices' checks of the commands against the skinning data, the vertex arrays and `jointCount` joint matrices
+static int check_skin_cmds(IdkPtCtx* ctx, const char* who, const IdkPtSkinningCmd* cmds, uint32_t cmdCount, uint64_t jointCount) {
+    const uint64_t vtxLimit = std::min(ctx->counts.VertexPositionCount, ctx->counts.VertexCount);
+    for (uint32_t c = 0; c < cmdCount; c++) {
+        const IdkPtSkinningCmd& k = cmds[c];
+        if ((uint64_t)k.InputVertexOffset + k.VertexCount > ctx->unskinnedCount) return fail(ctx, who, IDKPT_ERR_INVALID_ARGUMENT, "input range outside the unskinned vertices (idkpt_set_skinning_data)");
+        if ((uint64_t)k.OutputVertexOffset + k.VertexCount > vtxLimit) return fail(ctx, who, IDKPT_ERR_INVALID_ARGUMENT, "output range outside the vertex arrays");
+        uint32_t maxJoint = 0;
+        for (uint64_t i = k.InputVertexOffset; i < (uint64_t)k.InputVertexOffset + k.VertexCount; i++) maxJoint = std::max(maxJoint, ctx->unskinnedMaxJoint[i]);
+        if (k.VertexCount && (uint64_t)k.JointMatricesOffset + maxJoint >= jointCount) return fail(ctx, who, IDKPT_ERR_INVALID_ARGUMENT, "a joint index points past the joint matrices");
+    }
+    return IDKPT_OK;
+}
+
+// The skinning dispatches of checked commands over device joint matrices (keep_prev_positions must have run)
+static int enqueue_skin(IdkPtCtx* ctx, const void* joints, const IdkPtSkinningCmd* cmds, uint32_t cmdCount) {
+    for (uint32_t c = 0; c < cmdCount; c++) {
+        if (!cmds[c].VertexCount) continue;
+        // Skinning/compute.glsl:42, prevVertexPositionSSBO = vertexPositionSSBO over the command's output range, dispatch by
+        // dispatch: with overlapping commands the kept positions are those the previous command left, as in the engine
+        const size_t off = (size_t)cmds[c].OutputVertexOffset * sizeof(PackedVec3), n = (size_t)cmds[c].VertexCount * sizeof(PackedVec3);
+        CK(cudaMemcpyAsync((char*)ctx->prevPositions.p + off, (const char*)ctx->positions.p + off, n, cudaMemcpyDeviceToDevice, ctx->stream));
+        SkinArgs a;
+        a.unskinned = (const uint32_t*)ctx->unskinned.p; a.joints = (const float4*)joints;
+        a.positions = (float*)ctx->positions.p; a.vertices = (uint4*)ctx->vertices.p; a.vtxFrame = (float4*)ctx->vtxFrame.p;
+        a.inOffset = cmds[c].InputVertexOffset; a.outOffset = cmds[c].OutputVertexOffset; a.jointOffset = cmds[c].JointMatricesOffset; a.count = cmds[c].VertexCount;
+        k_skin_vertices<<<(a.count + 255) / 256, 256, 0, ctx->stream>>>(a);
+    }
     return IDKPT_OK;
 }
 
@@ -1925,36 +1985,34 @@ IDKPT_API int idkpt_skin_vertices(IdkPtCtx* ctx, const float* jointMatrices, uin
     DRAIN_PENDING("idkpt_skin_vertices");
     if (!ctx->haveScene) return fail(ctx, IDKPT_ERR_NO_SCENE, "idkpt_skin_vertices: no scene");
     if (kernelMs) *kernelMs = 0.0f;
-    const uint64_t vtxLimit = std::min(ctx->counts.VertexPositionCount, ctx->counts.VertexCount);
-    for (uint32_t c = 0; c < cmdCount; c++) {
-        const IdkPtSkinningCmd& k = cmds[c];
-        if ((uint64_t)k.InputVertexOffset + k.VertexCount > ctx->unskinnedCount) return fail(ctx, IDKPT_ERR_INVALID_ARGUMENT, "idkpt_skin_vertices: input range outside the unskinned vertices (idkpt_set_skinning_data)");
-        if ((uint64_t)k.OutputVertexOffset + k.VertexCount > vtxLimit) return fail(ctx, IDKPT_ERR_INVALID_ARGUMENT, "idkpt_skin_vertices: output range outside the vertex arrays");
-        uint32_t maxJoint = 0;
-        for (uint64_t i = k.InputVertexOffset; i < (uint64_t)k.InputVertexOffset + k.VertexCount; i++) maxJoint = std::max(maxJoint, ctx->unskinnedMaxJoint[i]);
-        if (k.VertexCount && (uint64_t)k.JointMatricesOffset + maxJoint >= jointCount) return fail(ctx, IDKPT_ERR_INVALID_ARGUMENT, "idkpt_skin_vertices: a joint index points past the joint matrices");
-    }
+    if (int rc = check_skin_cmds(ctx, "idkpt_skin_vertices", cmds, cmdCount, jointCount)) return rc;
     CK(cudaSetDevice(ctx->device));
     int rc;
     if ((rc = upload(ctx, ctx->joints, jointMatrices, jointCount * 48))) return rc;   // jointMatricesBuffer.UploadElements (ModelManager.cs:277)
     if ((rc = keep_prev_positions(ctx))) return rc;
-    rc = run_timed(ctx, "idkpt_skin_vertices", kernelMs, [&]() -> int {
-        for (uint32_t c = 0; c < cmdCount; c++) {
-            if (!cmds[c].VertexCount) continue;
-            // Skinning/compute.glsl:42, prevVertexPositionSSBO = vertexPositionSSBO over the command's output range, dispatch by
-            // dispatch: with overlapping commands the kept positions are those the previous command left, as in the engine
-            const size_t off = (size_t)cmds[c].OutputVertexOffset * sizeof(PackedVec3), n = (size_t)cmds[c].VertexCount * sizeof(PackedVec3);
-            CK(cudaMemcpyAsync((char*)ctx->prevPositions.p + off, (const char*)ctx->positions.p + off, n, cudaMemcpyDeviceToDevice, ctx->stream));
-            SkinArgs a;
-            a.unskinned = (const uint32_t*)ctx->unskinned.p; a.joints = (const float4*)ctx->joints.p;
-            a.positions = (float*)ctx->positions.p; a.vertices = (uint4*)ctx->vertices.p; a.vtxFrame = (float4*)ctx->vtxFrame.p;
-            a.inOffset = cmds[c].InputVertexOffset; a.outOffset = cmds[c].OutputVertexOffset; a.jointOffset = cmds[c].JointMatricesOffset; a.count = cmds[c].VertexCount;
-            k_skin_vertices<<<(a.count + 255) / 256, 256, 0, ctx->stream>>>(a);
-        }
-        return IDKPT_OK;
-    });
+    rc = run_timed(ctx, "idkpt_skin_vertices", kernelMs, [&]() -> int { return enqueue_skin(ctx, ctx->joints.p, cmds, cmdCount); });
     if (rc == IDKPT_OK) ctx->accumulatedSamples = 0;
     return rc;
+}
+
+// BVH.GpuBlasesRefit of BLASes [first, first + count), enqueued
+static int enqueue_refit(IdkPtCtx* ctx, uint32_t first, uint32_t count) {
+    int maxNodes = 0;
+    for (uint32_t b = first; b < first + count; b++) maxNodes = std::max(maxNodes, ctx->hostDescs[b].NodeCount);
+    CK(ensure(ctx->refitParents, std::max<size_t>((size_t)maxNodes, 4) * 4));   // blasRefitLockBuffer sizing, BVH.cs:451
+    CK(ensure(ctx->refitLocks, std::max<size_t>((size_t)maxNodes, 4) * 4));
+    for (uint32_t b = first; b < first + count; b++) {
+        const GpuBlasDesc& d = ctx->hostDescs[b];
+        RefitArgs a;
+        a.nodes = (float4*)ctx->nodes.p + 2 * (size_t)d.NodeOffset;
+        a.blasTris = (const int4*)ctx->blasTris.p; a.positions = (const float*)ctx->positions.p;
+        a.triRec = (float4*)((char*)ctx->nodes.p + ctx->nodeBytes);
+        a.parents = (int32_t*)ctx->refitParents.p; a.locks = (uint32_t*)ctx->refitLocks.p;
+        a.nodeCount = (uint32_t)d.NodeCount; a.triOffset = (uint32_t)d.TriangleOffset; a.triCount = (uint32_t)d.TriangleCount;
+        k_refit_prepare<<<(a.nodeCount + 255) / 256, 256, 0, ctx->stream>>>(a);
+        k_refit_climb<<<(a.nodeCount + 255) / 256, 256, 0, ctx->stream>>>(a);
+    }
+    return IDKPT_OK;
 }
 
 IDKPT_API int idkpt_blas_refit(IdkPtCtx* ctx, uint32_t first, uint32_t count, float* kernelMs) {
@@ -1964,24 +2022,7 @@ IDKPT_API int idkpt_blas_refit(IdkPtCtx* ctx, uint32_t first, uint32_t count, fl
     if ((uint64_t)first + count > ctx->hostDescs.size()) return fail(ctx, IDKPT_ERR_INVALID_ARGUMENT, "idkpt_blas_refit: BLAS range outside BlasDescs");
     if (kernelMs) *kernelMs = 0.0f;
     CK(cudaSetDevice(ctx->device));
-    int maxNodes = 0;
-    for (uint32_t b = first; b < first + count; b++) maxNodes = std::max(maxNodes, ctx->hostDescs[b].NodeCount);
-    CK(ensure(ctx->refitParents, std::max<size_t>((size_t)maxNodes, 4) * 4));   // blasRefitLockBuffer sizing, BVH.cs:451
-    CK(ensure(ctx->refitLocks, std::max<size_t>((size_t)maxNodes, 4) * 4));
-    const int rc = run_timed(ctx, "idkpt_blas_refit", kernelMs, [&]() -> int {
-        for (uint32_t b = first; b < first + count; b++) {
-            const GpuBlasDesc& d = ctx->hostDescs[b];
-            RefitArgs a;
-            a.nodes = (float4*)ctx->nodes.p + 2 * (size_t)d.NodeOffset;
-            a.blasTris = (const int4*)ctx->blasTris.p; a.positions = (const float*)ctx->positions.p;
-            a.triRec = (float4*)((char*)ctx->nodes.p + ctx->nodeBytes);
-            a.parents = (int32_t*)ctx->refitParents.p; a.locks = (uint32_t*)ctx->refitLocks.p;
-            a.nodeCount = (uint32_t)d.NodeCount; a.triOffset = (uint32_t)d.TriangleOffset; a.triCount = (uint32_t)d.TriangleCount;
-            k_refit_prepare<<<(a.nodeCount + 255) / 256, 256, 0, ctx->stream>>>(a);
-            k_refit_climb<<<(a.nodeCount + 255) / 256, 256, 0, ctx->stream>>>(a);
-        }
-        return IDKPT_OK;
-    });
+    const int rc = run_timed(ctx, "idkpt_blas_refit", kernelMs, [&]() -> int { return enqueue_refit(ctx, first, count); });
     if (rc == IDKPT_OK) ctx->accumulatedSamples = 0;
     return rc;
 }
@@ -2045,19 +2086,20 @@ static int enqueue_tlas_build(IdkPtCtx* ctx, const void* blasNodes, const void* 
     return IDKPT_OK;
 }
 
-// BVH.TlasBuild on the device (BVH.cs:278-298, TLAS.cs:28-141): see k_tlas_ploc.
-IDKPT_API int idkpt_tlas_build(IdkPtCtx* ctx, int32_t searchRadius, float* kernelMs) {
-    if (!ctx) return IDKPT_ERR_INVALID_ARGUMENT;
-    DRAIN_PENDING("idkpt_tlas_build");
-    if (kernelMs) *kernelMs = 0.0f;
-    if (!ctx->haveScene) return fail(ctx, IDKPT_ERR_NO_SCENE, "idkpt_tlas_build: no scene");
-    if (!ctx->counts.UseTlas) return fail(ctx, IDKPT_ERR_INVALID_ARGUMENT, "idkpt_tlas_build: the scene was set without UseTlas (no TLAS node array to fill)");
-    if (searchRadius < 1 || searchRadius > 1024) return fail(ctx, IDKPT_ERR_INVALID_ARGUMENT, "idkpt_tlas_build: search radius out of range (TLAS.BuildSettings.SearchRadius, default 15)");
+// BVH.TlasBuild on the device (BVH.cs:278-298, TLAS.cs:28-141): see k_tlas_ploc. Shared by idkpt_tlas_build and
+// idkpt_update_models, whose refusals are the same.
+// `pre` enqueues work that must come before the build (idkpt_update_models' skin and refit) inside the same timed, synchronised
+// region, so that it costs no host synchronisation of its own.
+static int tlas_build_scene(IdkPtCtx* ctx, const char* who, int32_t searchRadius, float* kernelMs, const std::function<int()>& pre = nullptr) {
+    if (!ctx->counts.UseTlas) return fail(ctx, who, IDKPT_ERR_INVALID_ARGUMENT, "the scene was set without UseTlas (no TLAS node array to fill)");
+    if (searchRadius < 1 || searchRadius > 1024) return fail(ctx, who, IDKPT_ERR_INVALID_ARGUMENT, "search radius out of range (TLAS.BuildSettings.SearchRadius, default 15)");
     const uint64_t n = ctx->counts.BlasInstanceCount;
-    if (2 * n - 1 >= (1ull << 31)) return fail(ctx, IDKPT_ERR_UNSUPPORTED, "idkpt_tlas_build: more than 2^30 instances (TLAS child and instance ids are 31 bits)");
+    if (2 * n - 1 >= (1ull << 31)) return fail(ctx, who, IDKPT_ERR_UNSUPPORTED, "more than 2^30 instances (TLAS child and instance ids are 31 bits)");
     CK(cudaSetDevice(ctx->device));
     int* needDev = nullptr;
-    const int rc = run_timed(ctx, "idkpt_tlas_build", kernelMs, [&]() -> int {
+    const int rc = run_timed(ctx, who, kernelMs, [&]() -> int {
+        if (pre)
+            if (int r = pre()) return r;
         return enqueue_tlas_build(ctx, ctx->nodes.p, ctx->descs.p, ctx->instances.p, ctx->xforms.p, ctx->tlas.p, n, searchRadius, &needDev);
     });
     if (rc) return rc;
@@ -2066,13 +2108,21 @@ IDKPT_API int idkpt_tlas_build(IdkPtCtx* ctx, int32_t searchRadius, float* kerne
     CK(cudaMemcpy(&need, needDev, 4, cudaMemcpyDeviceToHost));
     if (need < 0) {                       // the PLOC loop merged nothing: the node array is not a tree
         ctx->haveScene = false;
-        return fail(ctx, IDKPT_ERR_INVALID_ARGUMENT, "idkpt_tlas_build: an instance's world box is not finite or its half area overflows (ModelMatrix or BLAS root); scene invalidated; set it again");
+        return fail(ctx, who, IDKPT_ERR_INVALID_ARGUMENT, "an instance's world box is not finite or its half area overflows (ModelMatrix or BLAS root); scene invalidated; set it again");
     }
     if (need > IDK_TLAS_STACK_SIZE) {     // the walk's stack is fixed (BVHIntersect.glsl:4): refuse to trace through a TLAS it cannot hold
         ctx->haveScene = false;
-        return fail(ctx, IDKPT_ERR_UNSUPPORTED, "idkpt_tlas_build: the built TLAS is deeper than the 24-entry traversal stack of the TLAS walk (scene invalidated; set it again)");
+        return fail(ctx, who, IDKPT_ERR_UNSUPPORTED, "the built TLAS is deeper than the 24-entry traversal stack of the TLAS walk (scene invalidated; set it again)");
     }
     return IDKPT_OK;
+}
+
+IDKPT_API int idkpt_tlas_build(IdkPtCtx* ctx, int32_t searchRadius, float* kernelMs) {
+    if (!ctx) return IDKPT_ERR_INVALID_ARGUMENT;
+    DRAIN_PENDING("idkpt_tlas_build");
+    if (kernelMs) *kernelMs = 0.0f;
+    if (!ctx->haveScene) return fail(ctx, IDKPT_ERR_NO_SCENE, "idkpt_tlas_build: no scene");
+    return tlas_build_scene(ctx, "idkpt_tlas_build", searchRadius, kernelMs);
 }
 
 // idkbb::build's status as the library's
@@ -2652,6 +2702,10 @@ IDKPT_API int idkpt_read_range(IdkPtCtx* ctx, IdkPtArrayId which, uint64_t first
         case IDKPT_ARRAY_TLAS_NODES: b = &ctx->tlas; elem = sizeof(GpuTlasNode); limit = ctx->counts.UseTlas ? ctx->counts.TlasNodeCount : 0; break;
         case IDKPT_ARRAY_BLAS_TRIANGLES: b = &ctx->blasTris; elem = sizeof(GpuBlasTriangle); limit = ctx->counts.BlasTriangleCount; break;
         case IDKPT_ARRAY_BLAS_DESCS: b = &ctx->descs; elem = sizeof(GpuBlasDesc); limit = ctx->counts.BlasDescCount; break;
+        case IDKPT_ARRAY_MESH_TRANSFORMS: b = &ctx->xforms; elem = sizeof(GpuMeshTransform); limit = ctx->counts.MeshTransformCount; break;
+        case IDKPT_ARRAY_NODE_LOCAL_TRANSFORMS: b = &ctx->anim.locals; elem = sizeof(IdkPtNodeLocal); limit = ctx->anim.plan.nodes.size(); break;
+        case IDKPT_ARRAY_NODE_GLOBAL_TRANSFORMS: b = &ctx->anim.globals; elem = 64; limit = ctx->anim.plan.nodes.size(); break;
+        case IDKPT_ARRAY_JOINT_MATRICES: b = &ctx->anim.joints; elem = 48; limit = ctx->anim.plan.jointMatrixCount; break;
         default: return fail(ctx, IDKPT_ERR_INVALID_ARGUMENT, "idkpt_read_range: array id not readable");
     }
     if (first > limit || count > limit - first) return fail(ctx, IDKPT_ERR_INVALID_ARGUMENT, "idkpt_read_range: range outside the array");
@@ -3527,3 +3581,168 @@ IDKPT_API int idkpt_lights_and_skybox(IdkPtCtx* ctx, const GpuPerFrameData* fram
 }
 
 } // extern "C"
+
+// ---- ModelManager.Update on the device (idk_animation.cuh) ------------------------------------------------------------------
+
+template <class T> static int upload_vec(IdkCtxBase* ctx, DevBuf& b, const std::vector<T>& v) { return upload(ctx, b, v.data(), v.size() * sizeof(T)); }
+
+IDKPT_API int idkpt_set_animations(IdkPtCtx* ctx, const IdkPtAnimationDesc* d) {
+    if (!ctx || !d) return fail(ctx, IDKPT_ERR_INVALID_ARGUMENT, "idkpt_set_animations: null argument");
+    DRAIN_PENDING("idkpt_set_animations");
+    if (!ctx->haveScene) return fail(ctx, IDKPT_ERR_NO_SCENE, "idkpt_set_animations: no scene");
+    idkanim::Plan plan;
+    const std::string err = idkanim::buildPlan(d, ctx->counts.MeshTransformCount, ctx->hostDescs.size(), plan);
+    if (!err.empty()) return fail(ctx, "idkpt_set_animations", IDKPT_ERR_INVALID_ARGUMENT, err.c_str());
+    CK(cudaSetDevice(ctx->device));
+    release_anim(ctx->anim);
+    AnimState& a = ctx->anim;
+    a.plan = std::move(plan);
+    const idkanim::Plan& p = a.plan;
+    const size_t N = p.nodes.size(), T = p.owner.size();
+    std::vector<uint32_t> enabled(p.animations.size());
+    for (size_t i = 0; i < enabled.size(); i++) enabled[i] = p.animations[i].Enabled ? 1u : 0u;
+    std::vector<IdkPtNodeLocal> locals(N);
+    std::vector<idkanim::M4> globals(N);
+    for (size_t i = 0; i < N; i++) { locals[i] = idkanim::nodeLocal(p.nodes[i]); memcpy(globals[i].m, p.nodes[i].GlobalTransform, 64); }
+    int rc;
+    if ((rc = upload_vec(ctx, a.channels, p.channels)) || (rc = upload_vec(ctx, a.animations, p.animations)) ||
+        (rc = upload_vec(ctx, a.enabled, enabled)) || (rc = upload_vec(ctx, a.groups, p.groups)) || (rc = upload_vec(ctx, a.pairs, p.pairs)) ||
+        (rc = upload_vec(ctx, a.times, p.times)) || (rc = upload_vec(ctx, a.data, p.data)) || (rc = upload_vec(ctx, a.nodes, p.nodes)) ||
+        (rc = upload_vec(ctx, a.levelNodes, p.levelNodes)) || (rc = upload_vec(ctx, a.levelStart, p.levelStart)) ||
+        (rc = upload_vec(ctx, a.skins, p.skins)) || (rc = upload_vec(ctx, a.jointNodes, p.jointNodes)) ||
+        (rc = upload_vec(ctx, a.inverseJoints, p.inverseJoints)) || (rc = upload_vec(ctx, a.jointSlotSkin, p.jointSlotSkin)) ||
+        (rc = upload_vec(ctx, a.jointSlotJoint, p.jointSlotJoint)) || (rc = upload_vec(ctx, a.owner, p.owner)) ||
+        (rc = upload_vec(ctx, a.locals, locals)) || (rc = upload_vec(ctx, a.globals, globals))) {
+        release_anim(ctx->anim);
+        return rc;
+    }
+    for (auto [b, bytes] : {std::pair<DevBuf*, size_t>{&a.scratchLocals, N * sizeof(IdkPtNodeLocal)}, {&a.newGlobals, N * 64},
+                            {&a.diffs, N * 64}, {&a.invSkin, p.skins.size() * 64}, {&a.pendingDirty, N}, {&a.dirty, N}, {&a.inSet, N},
+                            {&a.movedBits, T}, {&a.joints, (size_t)p.jointMatrixCount * 48}, {&a.flags, 4}}) {
+        cudaError_t e = ensure(*b, std::max<size_t>(bytes, 16));
+        if (e == cudaSuccess) e = cudaMemsetAsync(b->p, 0, std::max<size_t>(bytes, 16), ctx->stream);
+        if (e != cudaSuccess) { release_anim(ctx->anim); return fail(ctx, "idkpt_set_animations", IDKPT_ERR_CUDA, cudaGetErrorString(e)); }
+    }
+    for (const IdkPtSkin& k : p.skins) a.cmds.push_back({k.InputVertexOffset, k.OutputVertexOffset, k.JointMatricesOffset, k.VertexCount});
+    const cudaError_t e = cudaStreamSynchronize(ctx->stream);
+    if (e != cudaSuccess) { release_anim(ctx->anim); return fail(ctx, "idkpt_set_animations", IDKPT_ERR_CUDA, cudaGetErrorString(e)); }
+    a.have = true;
+    return IDKPT_OK;
+}
+
+IDKPT_API int idkpt_enable_animations(IdkPtCtx* ctx, uint32_t first, uint32_t count, const uint8_t* enabled) {
+    if (!ctx || (!enabled && count)) return fail(ctx, IDKPT_ERR_INVALID_ARGUMENT, "idkpt_enable_animations: null argument");
+    DRAIN_PENDING("idkpt_enable_animations");
+    AnimState& a = ctx->anim;
+    if (!a.have) return fail(ctx, IDKPT_ERR_NO_SCENE, "idkpt_enable_animations: no animation set");
+    if ((uint64_t)first + count > a.plan.animations.size()) return fail(ctx, IDKPT_ERR_INVALID_ARGUMENT, "idkpt_enable_animations: range outside the animations");
+    CK(cudaSetDevice(ctx->device));
+    std::vector<uint32_t> v(count);
+    for (uint32_t i = 0; i < count; i++) { v[i] = enabled[i] ? 1u : 0u; a.plan.animations[first + i].Enabled = v[i]; }
+    if (count) CK(cudaMemcpyAsync((uint32_t*)a.enabled.p + first, v.data(), count * 4, cudaMemcpyHostToDevice, ctx->stream));
+    CK(cudaStreamSynchronize(ctx->stream));
+    return IDKPT_OK;
+}
+
+IDKPT_API int idkpt_set_node_transforms(IdkPtCtx* ctx, uint32_t first, uint32_t count, const IdkPtNode* nodes) {
+    if (!ctx || (!nodes && count)) return fail(ctx, IDKPT_ERR_INVALID_ARGUMENT, "idkpt_set_node_transforms: null argument");
+    DRAIN_PENDING("idkpt_set_node_transforms");
+    AnimState& a = ctx->anim;
+    if (!a.have) return fail(ctx, IDKPT_ERR_NO_SCENE, "idkpt_set_node_transforms: no animation set");
+    if ((uint64_t)first + count > a.plan.nodes.size()) return fail(ctx, IDKPT_ERR_INVALID_ARGUMENT, "idkpt_set_node_transforms: range outside the nodes");
+    if (!count) return IDKPT_OK;
+    CK(cudaSetDevice(ctx->device));
+    DevBuf& stage = ctx->scratch[0];
+    if (int rc = upload(ctx, stage, nodes, (size_t)count * sizeof(IdkPtNode))) return rc;
+    k_anim_set_locals<<<(count + 255) / 256, 256, 0, ctx->stream>>>((const IdkPtNode*)stage.p, (IdkPtNodeLocal*)a.locals.p,
+                                                                     (uint8_t*)a.pendingDirty.p, first, count);
+    CK(cudaGetLastError());
+    CK(cudaStreamSynchronize(ctx->stream));
+    return IDKPT_OK;
+}
+
+IDKPT_API int idkpt_update_models(IdkPtCtx* ctx, float time, int32_t searchRadius, uint32_t* movedOut, float* kernelMs) {
+    if (!ctx) return IDKPT_ERR_INVALID_ARGUMENT;
+    DRAIN_PENDING("idkpt_update_models");
+    if (kernelMs) *kernelMs = 0.0f;
+    if (movedOut) *movedOut = 0;
+    AnimState& a = ctx->anim;
+    if (!ctx->haveScene || !a.have) return fail(ctx, IDKPT_ERR_NO_SCENE, "idkpt_update_models: no animation set (idkpt_set_animations)");
+    const idkanim::Plan& p = a.plan;
+    const uint32_t cmdCount = (uint32_t)a.cmds.size();
+    // the check walks every skinned vertex: run it only when the skinning data changed since it last passed
+    if (a.skinCheckedVersion != ctx->skinningDataVersion || a.skinCheckedCount != ctx->unskinnedCount) {
+        if (int rc = check_skin_cmds(ctx, "idkpt_update_models", a.cmds.data(), cmdCount, p.jointMatrixCount)) return rc;
+        a.skinCheckedVersion = ctx->skinningDataVersion;
+        a.skinCheckedCount = ctx->unskinnedCount;
+    }
+    CK(cudaSetDevice(ctx->device));
+    const size_t N = p.nodes.size();
+    AnimArgs g;
+    g.channels = (const IdkPtNodeAnimation*)a.channels.p; g.animations = (const IdkPtModelAnimation*)a.animations.p;
+    g.enabled = (const uint32_t*)a.enabled.p; g.groups = (const idkanim::Group*)a.groups.p; g.pairs = (const uint32_t*)a.pairs.p;
+    g.times = (const float*)a.times.p; g.data = (const float*)a.data.p; g.nodes = (const IdkPtNode*)a.nodes.p;
+    g.levelNodes = (const uint32_t*)a.levelNodes.p; g.levelStart = (const uint32_t*)a.levelStart.p; g.skins = (const IdkPtSkin*)a.skins.p;
+    g.jointNodes = (const uint32_t*)a.jointNodes.p; g.inverseJoints = (const float*)a.inverseJoints.p;
+    g.jointSlotSkin = (const uint32_t*)a.jointSlotSkin.p; g.jointSlotJoint = (const uint32_t*)a.jointSlotJoint.p; g.owner = (const int32_t*)a.owner.p;
+    g.locals = (IdkPtNodeLocal*)a.scratchLocals.p; g.globals = (const idkanim::M4*)a.globals.p; g.newGlobals = (idkanim::M4*)a.newGlobals.p;
+    g.diffs = (idkanim::M4*)a.diffs.p; g.invSkin = (idkanim::M4*)a.invSkin.p; g.dirty = (uint8_t*)a.dirty.p; g.inSet = (uint8_t*)a.inSet.p;
+    g.movedBits = (uint8_t*)a.movedBits.p; g.xforms = (GpuMeshTransform*)ctx->xforms.p; g.joints = (float*)a.joints.p; g.flags = (uint32_t*)a.flags.p;
+    g.time = time;
+    g.groupCount = (uint32_t)p.groups.size(); g.levelCount = (uint32_t)p.levelStart.size() - 1; g.skinCount = (uint32_t)p.skins.size();
+    g.transformCount = (uint32_t)p.owner.size(); g.jointMatrixCount = p.jointMatrixCount;
+    const bool sample = !(time == a.prevTime);
+    uint32_t flags = 0;
+    float ms0 = 0.0f, ms1 = 0.0f;
+    // steps 1-4 (UpdateNodeAnimations .. the joint matrices) into scratch, then one read of the flag word
+    int rc = run_timed(ctx, "idkpt_update_models", &ms0, [&]() -> int {
+        if (N) {
+            CK(cudaMemcpyAsync(a.scratchLocals.p, a.locals.p, N * sizeof(IdkPtNodeLocal), cudaMemcpyDeviceToDevice, ctx->stream));
+            CK(cudaMemcpyAsync(a.dirty.p, a.pendingDirty.p, N, cudaMemcpyDeviceToDevice, ctx->stream));
+        }
+        if (sample && g.groupCount) k_anim_sample<<<(g.groupCount + 127) / 128, 128, 0, ctx->stream>>>(g);
+        k_anim_nodes<<<1, IDK_ANIM_NODES_BLOCK, 0, ctx->stream>>>(g);
+        if (g.transformCount) k_anim_transforms<<<(g.transformCount + 255) / 256, 256, 0, ctx->stream>>>(g);
+        if (g.jointMatrixCount) k_anim_joints<<<(g.jointMatrixCount + 127) / 128, 128, 0, ctx->stream>>>(g);
+        return IDKPT_OK;
+    }, &flags, a.flags.p, 4);
+    if (rc) return rc;
+    if (flags & IDK_ANIM_FLAG_SINGULAR)
+        return fail(ctx, "idkpt_update_models", IDKPT_ERR_INVALID_ARGUMENT, "a singular matrix: a moving node's previous global transform or a skinned node's global transform cannot be inverted (Matrix4.Invert); nothing changed");
+    std::swap(a.locals, a.scratchLocals);
+    std::swap(a.globals, a.newGlobals);
+    if (N) CK(cudaMemsetAsync(a.pendingDirty.p, 0, N, ctx->stream));
+    if (sample) a.prevTime = time;
+    const bool anyNode = flags & IDK_ANIM_FLAG_NODE_MOVED, anyInstance = flags & IDK_ANIM_FLAG_INSTANCE_MOVED;
+    const bool runSkin = anyNode || a.runSkinning;
+    a.runSkinning = anyNode;
+    if (movedOut) *movedOut = (anyNode ? 1u : 0u) | (anyInstance ? 2u : 0u);
+    // step 5: skinning (runSkinningShader), the refit of every skin's BLAS and the TLAS, through the existing paths
+    if (runSkin && cmdCount) {
+        if ((rc = keep_prev_positions(ctx))) return rc;
+    }
+    const bool skin = runSkin && cmdCount, refit = anyNode && !p.skins.empty(), tlas = anyNode || anyInstance;
+    auto skinAndRefit = [&]() -> int {
+        if (skin)
+            if (int r = enqueue_skin(ctx, a.joints.p, a.cmds.data(), cmdCount)) return r;
+        if (refit)
+            for (const IdkPtSkin& k : p.skins)
+                if (int r = enqueue_refit(ctx, k.BlasId, 1)) return r;
+        return IDKPT_OK;
+    };
+    // With a TLAS build to follow, the skin and the refit run inside its timed region: no host synchronisation of their own.
+    // A scene the build would refuse (no UseTlas, a bad radius) still gets them first, as the per-stage calls would.
+    const bool tlasRuns = tlas && ctx->counts.UseTlas && searchRadius >= 1 && searchRadius <= 1024;
+    if ((skin || refit) && !tlasRuns)
+        if ((rc = run_timed(ctx, "idkpt_update_models", &ms1, skinAndRefit))) return rc;
+    if (tlas) {
+        ctx->accumulatedSamples = 0;                  // Application.cs:210-213
+        float ms2 = 0.0f;
+        if (tlasRuns) rc = tlas_build_scene(ctx, "idkpt_update_models", searchRadius, &ms2, skinAndRefit);
+        else rc = tlas_build_scene(ctx, "idkpt_update_models", searchRadius, &ms2);
+        if (rc) return rc;
+        ms1 += ms2;
+    }
+    if (kernelMs) *kernelMs = ms0 + ms1;
+    return IDKPT_OK;
+}

@@ -28,6 +28,14 @@ GpuVertex = np.dtype([("TexCoord", f4, 2), ("Tangent", u4), ("Normal", u4)])
 PackedVec3 = np.dtype([("x", f4), ("y", f4), ("z", f4)])
 GpuUnskinnedVertex = np.dtype([("JointIndices", u4, 4), ("JointWeights", f4, 4), ("Position", f4, 3), ("Tangent", u4), ("Normal", u4)])
 IdkPtSkinningCmd = np.dtype([("InputVertexOffset", u4), ("OutputVertexOffset", u4), ("JointMatricesOffset", u4), ("VertexCount", u4)])
+IdkPtNodeLocal = np.dtype([("Translation", f4, 3), ("Rotation", f4, 4), ("Scale", f4, 3)])
+IdkPtNode = np.dtype([("Parent", i4), ("MeshTransformsStart", u4), ("MeshTransformsCount", u4), ("Translation", f4, 3),
+                      ("Rotation", f4, 4), ("Scale", f4, 3), ("GlobalTransform", f4, (4, 4))])
+IdkPtNodeAnimation = np.dtype([("TargetNode", u4), ("Type", i4), ("Mode", i4), ("KeyFrameOffset", u4), ("KeyFrameCount", u4),
+                               ("DataOffset", u4)])
+IdkPtModelAnimation = np.dtype([("TMin", f4), ("TMax", f4), ("FirstChannel", u4), ("ChannelCount", u4), ("Enabled", u4)])
+IdkPtSkin = np.dtype([("SkinnedNode", u4), ("FirstJoint", u4), ("JointCount", u4), ("JointMatricesOffset", u4),
+                      ("InputVertexOffset", u4), ("OutputVertexOffset", u4), ("VertexCount", u4), ("BlasId", u4)])
 GpuLight = np.dtype([("Position", f4, 3), ("Radius", f4), ("Color", f4, 3), ("PointShadowIndex", i4),
                      ("PrevPosition", f4, 3), ("_pad0", f4)])
 GpuPointShadow = np.dtype([("Texture", u8), ("ShadowTexture", u8), ("ProjViewMatrices", f4, (6, 16)), ("Position", f4, 3),
@@ -50,6 +58,9 @@ IdkPtAddModelsDesc = np.dtype([(n, u8) for n in (
     "Triangles", "TriangleCount", "BlasDescs", "BlasDescCount", "BlasInstances", "BlasInstanceCount", "MeshTransforms",
     "MeshTransformCount", "Meshes", "MeshCount", "Materials", "MaterialCount", "Vertices", "VertexPositions", "VertexCount",
     "Textures", "TextureCount", "UnskinnedVertices", "UnskinnedVertexCount")])
+IdkPtAnimationDesc = np.dtype([(n, u8) for n in (
+    "Nodes", "NodeCount", "Channels", "ChannelCount", "Animations", "AnimationCount", "Skins", "SkinCount", "JointNodes",
+    "JointCount", "InverseJointMatrices", "KeyFrameTimes", "KeyFrameTimeCount", "KeyFrameData", "KeyFrameDataCount")])
 
 EXPECTED_SIZES = {
     "GpuBlasNode": 32, "GpuBlasTriangle": 16, "GpuBlasDesc": 40, "GpuBlasInstance": 8, "GpuTlasNode": 32,
@@ -57,6 +68,8 @@ EXPECTED_SIZES = {
     "GpuLight": 48, "GpuPointShadow": 432, "GpuPerFrameData": 544, "GpuWavefrontRay": 48, "GpuAovRay": 32, "IdkPtGpuSettings": 20,
     "IdkPtRay": 32, "IdkPtHit": 32, "GpuUnskinnedVertex": 52, "IdkPtSkinningCmd": 16,
     "IdkPtAddModelsDesc": 152,
+    "IdkPtNodeLocal": 40, "IdkPtNode": 116, "IdkPtNodeAnimation": 24, "IdkPtModelAnimation": 20, "IdkPtSkin": 32,
+    "IdkPtAnimationDesc": 120,
 }
 for _name, _size in EXPECTED_SIZES.items():
     assert globals()[_name].itemsize == _size, (_name, globals()[_name].itemsize, _size)

@@ -74,6 +74,26 @@ def lib():
         L.idkhost_tlas_build.argtypes = [ctypes.c_void_p, ctypes.c_int32, ctypes.c_void_p, ctypes.c_int32]
         L.idkhost_blas_global_sah.restype = ctypes.c_double
         L.idkhost_blas_global_sah.argtypes = [ctypes.c_void_p, ctypes.c_uint64, ctypes.c_float]
+        L.idkhost_anim_create.restype = ctypes.c_void_p
+        L.idkhost_anim_create.argtypes = [ctypes.c_void_p, ctypes.c_uint64, ctypes.c_uint64, ctypes.c_char_p, ctypes.c_uint32]
+        L.idkhost_anim_free.restype = None
+        L.idkhost_anim_free.argtypes = [ctypes.c_void_p]
+        L.idkhost_anim_enable.restype = ctypes.c_int32
+        L.idkhost_anim_enable.argtypes = [ctypes.c_void_p, ctypes.c_uint32, ctypes.c_uint32, ctypes.c_void_p]
+        L.idkhost_anim_set_node_transforms.restype = ctypes.c_int32
+        L.idkhost_anim_set_node_transforms.argtypes = [ctypes.c_void_p, ctypes.c_uint32, ctypes.c_uint32, ctypes.c_void_p]
+        L.idkhost_anim_update.restype = ctypes.c_int32
+        L.idkhost_anim_update.argtypes = [ctypes.c_void_p, ctypes.c_float, ctypes.c_void_p, ctypes.POINTER(ctypes.c_uint32),
+                                          ctypes.POINTER(ctypes.c_int32)]
+        L.idkhost_anim_read.restype = ctypes.c_uint64
+        L.idkhost_anim_read.argtypes = [ctypes.c_void_p, ctypes.c_int32, ctypes.c_void_p]
+        for f in ("idkhost_anim_sin", "idkhost_anim_acos"):
+            getattr(L, f).restype = None
+            getattr(L, f).argtypes = [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_uint64]
+        L.idkhost_anim_lower_bound.restype = ctypes.c_int32
+        L.idkhost_anim_lower_bound.argtypes = [ctypes.c_void_p, ctypes.c_int32, ctypes.c_float]
+        L.idkhost_anim_slerp.restype = None
+        L.idkhost_anim_slerp.argtypes = [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_float, ctypes.c_void_p]
         L.idkhost_default_build_settings.restype = None
         L.idkhost_default_build_settings.argtypes = [ctypes.POINTER(IdkBlasBuildSettings)]
         _lib = L
@@ -214,6 +234,117 @@ def mesh_transform(model4x4):
     out["InvModelMatrix"][0] = np.linalg.inv(m32.astype(np.float64)).astype(np.float32)[:3, :]
     out["PrevModelMatrix"][0] = m32[:3, :]
     return out
+
+
+# --------------------------------------------------------------------------- animation (ModelManager.Update's host half)
+class Animations:
+    """ModelManager's CPU model state as idkpt_set_animations takes it: nodes in pre-order (IdkPtNode), channels
+    (IdkPtNodeAnimation), animations (IdkPtModelAnimation), skins (IdkPtSkin), joint_nodes (uint32), inverse_joints
+    (n x 4 x 4 float32, OpenTK rows), key times and key data (float32)."""
+
+    def __init__(self):
+        self.nodes = np.zeros(0, gt.IdkPtNode)
+        self.channels = np.zeros(0, gt.IdkPtNodeAnimation)
+        self.animations = np.zeros(0, gt.IdkPtModelAnimation)
+        self.skins = np.zeros(0, gt.IdkPtSkin)
+        self.joint_nodes = np.zeros(0, np.uint32)
+        self.inverse_joints = np.zeros((0, 4, 4), np.float32)
+        self.times = np.zeros(0, np.float32)
+        self.data = np.zeros(0, np.float32)
+
+    def add_node(self, parent=-1, translation=(0, 0, 0), rotation=(0, 0, 0, 1), scale=(1, 1, 1), transforms=(0, 0)):
+        """Appends a node (its global is filled in by init_globals). Returns its index."""
+        n = np.zeros(1, gt.IdkPtNode)
+        n["Parent"], n["MeshTransformsStart"], n["MeshTransformsCount"] = parent, transforms[0], transforms[1]
+        n["Translation"], n["Rotation"], n["Scale"] = translation, rotation, scale
+        n["GlobalTransform"] = np.eye(4, dtype=np.float32)
+        self.nodes = np.concatenate([self.nodes, n])
+        return len(self.nodes) - 1
+
+    def add_channel(self, node, kind, mode, times, values):
+        """Appends a channel over keys (times, values: n x 3 or n x 4). Returns its index."""
+        c = np.zeros(1, gt.IdkPtNodeAnimation)
+        c["TargetNode"], c["Type"], c["Mode"] = node, kind, mode
+        c["KeyFrameOffset"], c["KeyFrameCount"], c["DataOffset"] = len(self.times), len(times), len(self.data)
+        self.times = np.concatenate([self.times, np.asarray(times, np.float32)])
+        self.data = np.concatenate([self.data, np.asarray(values, np.float32).ravel()])
+        self.channels = np.concatenate([self.channels, c])
+        return len(self.channels) - 1
+
+    def add_animation(self, first, count, tmin, tmax, enabled=1):
+        a = np.zeros(1, gt.IdkPtModelAnimation)
+        a["TMin"], a["TMax"], a["FirstChannel"], a["ChannelCount"], a["Enabled"] = tmin, tmax, first, count, enabled
+        self.animations = np.concatenate([self.animations, a])
+        return len(self.animations) - 1
+
+    def init_globals(self):
+        """GlobalTransform of every node from its local chain, as the engine computes it at load (float32, OpenTK rows)."""
+        m = AnimationMirror.node_matrix
+        for i, n in enumerate(self.nodes):
+            g = m(n)
+            if n["Parent"] >= 0:
+                g = (g.astype(np.float64) @ self.nodes[n["Parent"]]["GlobalTransform"].astype(np.float64)).astype(np.float32)
+            self.nodes[i]["GlobalTransform"] = g
+
+
+class AnimationMirror:
+    """libidkhost's idkhost_update_models state: the same plan and arithmetic as the device's idkpt_update_models."""
+
+    def __init__(self, anim, transform_count, blas_count):
+        from . import capi
+        d, self._keep = capi.animation_desc(anim)
+        err = ctypes.create_string_buffer(512)
+        self._h = lib().idkhost_anim_create(ctypes.byref(d), transform_count, blas_count, err, 512)
+        if not self._h:
+            raise ValueError(err.value.decode())
+        self.skins = np.array(anim.skins)
+
+    def __del__(self):
+        if getattr(self, "_h", None):
+            lib().idkhost_anim_free(self._h)
+            self._h = None
+
+    @staticmethod
+    def node_matrix(local):
+        """Transformation.GetMatrix in float64 (OpenTK rows): a reference, not the mirror's arithmetic."""
+        x, y, z, w = [float(v) for v in local["Rotation"]]
+        s2 = 2.0 / (x * x + y * y + z * z + w * w)
+        r = np.array([[1 - s2 * (y * y + z * z), s2 * (x * y + z * w), s2 * (x * z - y * w), 0],
+                      [s2 * (x * y - z * w), 1 - s2 * (x * x + z * z), s2 * (y * z + x * w), 0],
+                      [s2 * (x * z + y * w), s2 * (y * z - x * w), 1 - s2 * (x * x + y * y), 0], [0, 0, 0, 1]])
+        m = np.diag([*[float(v) for v in local["Scale"]], 1.0]) @ r
+        m[3, :3] = local["Translation"]
+        return m
+
+    def enable(self, first, enabled):
+        e = np.ascontiguousarray(enabled, np.uint8)
+        assert lib().idkhost_anim_enable(self._h, first, len(e), e.ctypes.data) == 0
+
+    def set_node_transforms(self, first, nodes):
+        nodes = np.ascontiguousarray(nodes, gt.IdkPtNode)
+        assert lib().idkhost_anim_set_node_transforms(self._h, first, len(nodes), nodes.ctypes.data) == 0
+
+    def update(self, time, transforms):
+        """One idkpt_update_models on `transforms` (GpuMeshTransform array, changed in place). Returns (moved bits, skin ran)
+        or None for a singular matrix (nothing changed)."""
+        assert transforms.flags.c_contiguous and transforms.dtype == gt.GpuMeshTransform
+        moved, skin = ctypes.c_uint32(), ctypes.c_int32()
+        if lib().idkhost_anim_update(self._h, time, transforms.ctypes.data, ctypes.byref(moved), ctypes.byref(skin)) != 0:
+            return None
+        return moved.value, bool(skin.value)
+
+    def read(self, which):
+        """0: node locals (IdkPtNodeLocal), 1: node globals (n x 4 x 4), 2: joint matrices (n x 3 x 4)."""
+        n = lib().idkhost_anim_read(self._h, which, None)
+        out = np.zeros(n, gt.IdkPtNodeLocal) if which == 0 else np.zeros((n, 4, 4) if which == 1 else (n, 3, 4), np.float32)
+        lib().idkhost_anim_read(self._h, which, out.ctypes.data)
+        return out
+
+    def skinning_cmds(self):
+        c = np.zeros(len(self.skins), gt.IdkPtSkinningCmd)
+        for f in ("InputVertexOffset", "OutputVertexOffset", "JointMatricesOffset", "VertexCount"):
+            c[f] = self.skins[f]
+        return c
 
 
 # --------------------------------------------------------------------------- Scene

@@ -81,12 +81,15 @@ class PathTracer:
         data = np.ascontiguousarray(data)
         self._check(self._lib.idkpt_update_range(self._ctx, which, first, len(data), data.ctypes.data), "idkpt_update_range")
 
-    _READ_DTYPES = {capi.IDKPT_ARRAY_TLAS_NODES: gt.GpuTlasNode, capi.IDKPT_ARRAY_BLAS_NODES: gt.GpuBlasNode,
+    _READ_DTYPES = {capi.IDKPT_ARRAY_NODE_LOCAL_TRANSFORMS: gt.IdkPtNodeLocal, capi.IDKPT_ARRAY_NODE_GLOBAL_TRANSFORMS: (np.float32, (4, 4)),
+                    capi.IDKPT_ARRAY_JOINT_MATRICES: (np.float32, (3, 4)), capi.IDKPT_ARRAY_MESH_TRANSFORMS: gt.GpuMeshTransform,
+                    capi.IDKPT_ARRAY_TLAS_NODES: gt.GpuTlasNode, capi.IDKPT_ARRAY_BLAS_NODES: gt.GpuBlasNode,
                     capi.IDKPT_ARRAY_VERTEX_POSITIONS: gt.PackedVec3, capi.IDKPT_ARRAY_VERTICES: gt.GpuVertex,
                     capi.IDKPT_ARRAY_BLAS_TRIANGLES: gt.GpuBlasTriangle, capi.IDKPT_ARRAY_BLAS_DESCS: gt.GpuBlasDesc}
 
     def ReadRange(self, which, first, count):
-        out = np.zeros(count, self._READ_DTYPES[which])
+        t = self._READ_DTYPES[which]
+        out = np.zeros((count,) + t[1], t[0]) if isinstance(t, tuple) else np.zeros(count, t)
         self._check(self._lib.idkpt_read_range(self._ctx, which, first, count, out.ctypes.data), "idkpt_read_range")
         return out
 
@@ -149,6 +152,27 @@ class PathTracer:
         ms = ctypes.c_float()
         self._check(self._lib.idkpt_tlas_build(self._ctx, search_radius, ctypes.byref(ms)), "idkpt_tlas_build")
         return ms.value
+
+    # ------------------------------------------------------------------ ModelManager.Update on the device (ModelManager.cs:236-261)
+    def SetAnimations(self, anim):
+        """idkpt_set_animations from a host.Animations."""
+        d, keep = capi.animation_desc(anim)
+        self._check(self._lib.idkpt_set_animations(self._ctx, ctypes.byref(d)), "idkpt_set_animations")
+
+    def EnableAnimations(self, first, enabled):
+        e = np.ascontiguousarray(enabled, np.uint8)
+        self._check(self._lib.idkpt_enable_animations(self._ctx, first, len(e), e.ctypes.data), "idkpt_enable_animations")
+
+    def SetNodeTransforms(self, first, nodes):
+        """Node.LocalTransform setter for nodes [first, first + len(nodes)) (IdkPtNode records; only Translation, Rotation and Scale are read)."""
+        nodes = np.ascontiguousarray(nodes, gt.IdkPtNode)
+        self._check(self._lib.idkpt_set_node_transforms(self._ctx, first, len(nodes), nodes.ctypes.data), "idkpt_set_node_transforms")
+
+    def UpdateModels(self, time, search_radius=15):
+        """ModelManager.Update(time) on the device. Returns (moved bits: 1 anyNodeMoved | 2 anyMeshInstanceMoved, kernel ms)."""
+        moved, ms = ctypes.c_uint32(), ctypes.c_float()
+        self._check(self._lib.idkpt_update_models(self._ctx, time, search_radius, ctypes.byref(moved), ctypes.byref(ms)), "idkpt_update_models")
+        return moved.value, ms.value
 
     @staticmethod
     def _blas_settings(settings):

@@ -540,3 +540,210 @@ def point_shadows(specs):
     for i, (p, n, f, li) in enumerate(specs):
         s[i]["Position"], s[i]["NearPlane"], s[i]["FarPlane"], s[i]["LightIndex"] = p, n, f, li
     return s
+
+
+# --------------------------------------------------------------------------- animated rigs (idkpt_update_models)
+# No animated glTF is at hand, so node hierarchies, channels and skins are built here over synthetic geometry.
+def quat(axis, deg):
+    """Unit quaternion (x, y, z, w) of a turn by `deg` degrees about `axis`, float32."""
+    axis = np.asarray(axis, np.float64) / np.linalg.norm(axis)
+    h = np.radians(deg) / 2
+    return np.array([*(axis * np.sin(h)), np.cos(h)], np.float32)
+
+
+def _joint_inverses(anim, ids):
+    return np.stack([np.linalg.inv(anim.nodes[i]["GlobalTransform"].astype(np.float64)) for i in ids]).astype(np.float32)
+
+
+def _unskinned(scene, v0, v1, joint_indices, joint_weights):
+    n = v1 - v0
+    u = np.zeros(n, gt.GpuUnskinnedVertex)
+    u["JointIndices"], u["JointWeights"] = joint_indices, joint_weights
+    u["Position"][:, 0], u["Position"][:, 1], u["Position"][:, 2] = (scene.positions[c][v0:v1] for c in "xyz")
+    u["Normal"] = scene.vertices["Normal"][v0:v1]
+    u["Tangent"] = scene.vertices["Tangent"][v0:v1]
+    return u
+
+
+def _skin(anim, skinned, ids, offset, v0, n, blas):
+    anim.joint_nodes = np.array(ids, np.uint32)
+    anim.inverse_joints = _joint_inverses(anim, ids)
+    sk = np.zeros(1, gt.IdkPtSkin)
+    sk["SkinnedNode"], sk["FirstJoint"], sk["JointCount"], sk["JointMatricesOffset"] = skinned, 0, len(ids), offset
+    sk["InputVertexOffset"], sk["OutputVertexOffset"], sk["VertexCount"], sk["BlasId"] = 0, v0, n, blas
+    anim.skins = sk
+
+
+def animated_skinned_rig(joints=6, seed=3):
+    """multi_blas with a TLAS; BLAS 2 skinned (random joints and weights) by a chain of `joints` joint nodes. Node 0 is the root
+    and owns every mesh transform (translation + scale channels); the joints turn through both Slerp branches (cos < 0.99 and
+    >= 0.99), a negative dot, equal keys (cos == 1), a STEP channel and two channels on one property (two animations, the
+    later wins). Joint matrices start at offset 2. Returns (scene, host.Animations, unskinned vertices)."""
+    from .host import Animations
+    from . import capi as A
+    sc, _ = multi_blas(threads=1)
+    sc.build_tlas()
+    d = sc.blas_descs[2]
+    tris = sc.blas_triangles[d["TriangleOffset"]:d["TriangleOffset"] + d["TriangleCount"]]
+    idx = np.concatenate([tris["X"], tris["Y"], tris["Z"]])
+    v0, v1 = int(idx.min()), int(idx.max()) + 1
+    rng = np.random.default_rng(seed)
+    w = rng.uniform(0.0, 1.0, (v1 - v0, 4)).astype(np.float32)
+    u = _unskinned(sc, v0, v1, rng.integers(0, joints, (v1 - v0, 4)), w / w.sum(1, keepdims=True))
+    an = Animations()
+    root = an.add_node(transforms=(0, len(sc.mesh_transforms)))
+    ids, parent = [], root
+    for _ in range(joints):
+        parent = an.add_node(parent=parent, translation=(0.0, 0.2, 0.0))
+        ids.append(parent)
+    skinned = an.add_node(parent=root)
+    an.init_globals()
+    L, R, S, T = A.IDKPT_ANIM_LINEAR, A.IDKPT_ANIM_ROTATION, A.IDKPT_ANIM_SCALE, A.IDKPT_ANIM_TRANSLATION
+    an.add_channel(root, T, L, [0.0, 1.0, 2.0], [[0, 0, 0], [0.3, 0.0, -0.2], [0.1, 0.1, 0]])
+    an.add_channel(root, S, L, [0.5, 1.5], [[1, 1, 1], [1.2, 0.9, 1.0]])
+    an.add_channel(ids[0], R, L, [0.0, 1.0, 2.0], [quat((0, 0, 1), 0), quat((0, 0, 1), 50), quat((1, 0, 1), -40)])
+    an.add_channel(ids[1], R, L, [0.0, 2.0], [quat((1, 0, 0), 0), quat((1, 0, 0), 8)])
+    an.add_channel(ids[2], R, L, [0.0, 2.0], [quat((0, 1, 0), 20), -quat((0, 1, 0), 60)])
+    an.add_channel(ids[3], R, A.IDKPT_ANIM_STEP, [0.0, 0.7, 1.4], [quat((0, 0, 1), 0), quat((0, 0, 1), 15), quat((0, 0, 1), 30)])
+    an.add_channel(ids[4], R, L, [0.0, 2.0], [quat((0, 0, 1), 10), quat((0, 0, 1), 10)])
+    n0 = len(an.channels)
+    an.add_animation(0, n0, 0.0, 2.0)
+    an.add_channel(ids[5 % joints], R, L, [0.0, 3.0], [quat((1, 0, 0), 0), quat((1, 0, 0), 70)])
+    an.add_channel(ids[5 % joints], R, L, [1.0, 3.0], [quat((0, 1, 0), 5), quat((0, 1, 0), 45)])
+    an.add_animation(n0, 2, 0.0, 3.0)
+    _skin(an, skinned, ids, 2, v0, v1 - v0, 2)
+    return sc, an, u
+
+
+def _instanced(m):
+    """instance_grid(2)'s nine BLASes with one instance per model matrix (n x 3 x 4), instance i using BLAS 1 + i % 8, and a
+    placeholder TLAS (a heap of height ceil(log2 n)) for the device build to replace."""
+    import copy
+    global _INSTANCED_BASE
+    if _INSTANCED_BASE is None:
+        _INSTANCED_BASE, _ = instance_grid(2, threads=1)
+    sc = copy.deepcopy(_INSTANCED_BASE)
+    n = len(m)
+    xf = np.zeros(n, gt.GpuMeshTransform)
+    full = np.zeros((n, 4, 4))
+    full[:, :3, :] = m.astype(np.float32)
+    full[:, 3, 3] = 1.0
+    xf["ModelMatrix"] = xf["PrevModelMatrix"] = full[:, :3, :]
+    xf["InvModelMatrix"] = np.linalg.inv(full)[:, :3, :]
+    sc.mesh_transforms = xf
+    sc.blas_instances = np.zeros(n, gt.GpuBlasInstance)
+    sc.blas_instances["BlasId"] = 1 + np.arange(n) % 8
+    sc.blas_instances["MeshTransformId"] = np.arange(n)
+    t = np.zeros(2 * n - 1, gt.GpuTlasNode)
+    t["IsLeafAndChildOrInstanceId"][:n - 1] = 2 * np.arange(n - 1) + 1
+    t["IsLeafAndChildOrInstanceId"][n - 1:] = np.uint32(0x80000000) | np.arange(n, dtype=np.uint32)
+    sc.tlas_nodes = t
+    sc.use_tlas = 1
+    return sc
+
+
+_INSTANCED_BASE = None
+
+
+def _grid_matrices(n, scale=0.4):
+    k = int(np.ceil(np.sqrt(n)))
+    i = np.arange(n)
+    m = np.zeros((n, 3, 4))
+    m[:, :, :3] = np.eye(3) * scale
+    m[:, :, 3] = np.stack([(i % k) * 1.25, np.zeros(n), (i // k) * 1.25], 1)
+    return m
+
+
+def animated_crowd(n):
+    """An EXT_mesh_gpu_instancing crowd: n instances in a 2-D grid whose n mesh transforms one node owns, under a parent that
+    moves (translation keys at 0, 0.5 and 1 s, a 1 s animation). Returns (scene, host.Animations)."""
+    from .host import Animations
+    from . import capi as A
+    sc = _instanced(_grid_matrices(n))
+    an = Animations()
+    root = an.add_node()
+    an.add_node(parent=root, transforms=(0, n))
+    an.init_globals()
+    an.add_channel(root, A.IDKPT_ANIM_TRANSLATION, A.IDKPT_ANIM_LINEAR, [0.0, 0.5, 1.0], [[0, 0, 0], [0.5, 0.25, 0], [0, 0, 0]])
+    an.add_animation(0, 1, 0.0, 1.0)
+    return sc, an
+
+
+def animated_nodes(n):
+    """n root nodes, each owning one instance's mesh transform and each with a translation channel of its own."""
+    from .host import Animations
+    from . import capi as A
+    sc = _instanced(_grid_matrices(n))
+    an = Animations()
+    an.nodes = np.zeros(n, gt.IdkPtNode)
+    an.nodes["Parent"] = -1
+    an.nodes["MeshTransformsStart"], an.nodes["MeshTransformsCount"] = np.arange(n), 1
+    an.nodes["Rotation"][:, 3] = 1.0
+    an.nodes["Scale"] = 1.0
+    an.nodes["GlobalTransform"] = np.eye(4, dtype=np.float32)
+    an.channels = np.zeros(n, gt.IdkPtNodeAnimation)
+    an.channels["TargetNode"] = np.arange(n)
+    an.channels["Type"], an.channels["Mode"] = A.IDKPT_ANIM_TRANSLATION, A.IDKPT_ANIM_LINEAR
+    an.channels["KeyFrameOffset"], an.channels["KeyFrameCount"], an.channels["DataOffset"] = 3 * np.arange(n), 3, 9 * np.arange(n)
+    an.times = np.tile(np.array([0.0, 0.5, 1.0], np.float32), n)
+    data = np.zeros((n, 3, 3), np.float32)
+    data[:, 1, 1] = 0.3 + np.arange(n, dtype=np.float32) * 0.001
+    an.data = data.ravel()
+    an.add_animation(0, n, 0.0, 1.0)
+    return sc, an
+
+
+def animated_chain(n):
+    """n nodes in one chain (each the parent of the next), each owning one mesh transform, the root turning."""
+    from .host import Animations
+    from . import capi as A
+    sc = _instanced(_grid_matrices(n))
+    an = Animations()
+    parent = -1
+    for i in range(n):
+        parent = an.add_node(parent=parent, translation=(0.0, 0.0, 0.0) if i == 0 else (0.001, 0.0, 0.0), transforms=(i, 1))
+    an.init_globals()
+    an.add_channel(0, A.IDKPT_ANIM_ROTATION, A.IDKPT_ANIM_LINEAR, [0.0, 1.0], [quat((0, 1, 0), 0), quat((0, 1, 0), 30)])
+    an.add_animation(0, 1, 0.0, 1.0)
+    return sc, an
+
+
+def animated_tentacle(joints=64, seg=64, rings=1600, threads=None):
+    """A skinned cylinder ("tentacle", (rings + 1) * seg vertices) over a floor, bent by a chain of `joints` joint nodes that
+    turn with LINEAR rotation channels; each vertex is weighted between the two joints of its height. The floor and the
+    tentacle are instances 0 and 1 (BLAS 1 is skinned). Returns (scene, host.Animations, unskinned vertices)."""
+    from .host import Animations
+    from . import capi as A
+    meshes, mats = _materials([dict(color=(0.7, 0.7, 0.7))])
+    a = _Assembler()
+    a.add(quad([-6, 0, -6], [-6, 0, 6], [6, 0, 6], [6, 0, -6]), 0)
+    floor = a.model(meshes, mats, name="floor")
+    b = _Assembler()
+    height = 4.0
+    b.add(cylinder([0, 0, 0], 0.3, height, seg, rings, taper=0.6), 0)
+    body = b.model(meshes, mats, name="tentacle")
+    sc = Scene().add(floor, body, threads=threads)
+    sc.build_tlas()
+    nv = (rings + 1) * seg
+    v0 = len(sc.positions) - nv
+    h = np.clip(np.asarray(sc.positions["y"][v0:], np.float64) / height * (joints - 1), 0, joints - 1)
+    j0 = np.minimum(np.floor(h).astype(np.int64), joints - 2)
+    f = (h - j0).astype(np.float32)
+    ji = np.stack([j0, j0 + 1, j0, j0], 1)
+    jw = np.stack([1 - f, f, np.zeros_like(f), np.zeros_like(f)], 1)
+    u = _unskinned(sc, v0, v0 + nv, ji, jw)
+    an = Animations()
+    root = an.add_node(transforms=(0, len(sc.mesh_transforms)))
+    ids, parent = [], root
+    for k in range(joints):
+        parent = an.add_node(parent=parent, translation=(0.0, 0.0 if k == 0 else height / (joints - 1), 0.0))
+        ids.append(parent)
+    skinned = an.add_node(parent=root)
+    an.init_globals()
+    for k, j in enumerate(ids):
+        ax = (1, 0, 0) if k % 2 else (0, 0, 1)
+        an.add_channel(j, A.IDKPT_ANIM_ROTATION, A.IDKPT_ANIM_LINEAR, [0.0, 1.0, 2.0],
+                       [quat(ax, 0), quat(ax, 2.5 + 0.01 * k), quat(ax, -2.0)])
+    an.add_animation(0, joints, 0.0, 2.0)
+    _skin(an, skinned, ids, 0, v0, nv, 1)
+    return sc, an, u

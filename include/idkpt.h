@@ -118,7 +118,7 @@ typedef struct IdkPtSceneDesc {
 } IdkPtSceneDesc;
 
 typedef enum IdkPtArrayId {
-    IDKPT_ARRAY_MESH_TRANSFORMS = 0,
+    IDKPT_ARRAY_MESH_TRANSFORMS = 0,   /* update + read (the transforms idkpt_update_models writes) */
     IDKPT_ARRAY_MESHES = 1,
     IDKPT_ARRAY_MATERIALS = 2,
     IDKPT_ARRAY_LIGHTS = 3,
@@ -127,7 +127,10 @@ typedef enum IdkPtArrayId {
     IDKPT_ARRAY_VERTEX_POSITIONS = 6,  /* read only: skinned positions (the download behind fenceCopiedSkinnedVerticesToHost, ModelManager.cs:282) */
     IDKPT_ARRAY_VERTICES = 7,          /* read only: skinned normals / tangents */
     IDKPT_ARRAY_BLAS_TRIANGLES = 8,    /* read only: GpuBlasTriangle records (the CPU copy for BVH.Intersect after idkpt_blas_rebuild) */
-    IDKPT_ARRAY_BLAS_DESCS = 9         /* read only: GpuBlasDesc records; the last one's ends are the node and triangle totals */
+    IDKPT_ARRAY_BLAS_DESCS = 9,        /* read only: GpuBlasDesc records; the last one's ends are the node and triangle totals */
+    IDKPT_ARRAY_NODE_LOCAL_TRANSFORMS = 10,  /* read only: IdkPtNodeLocal per node of idkpt_set_animations (Node.LocalTransform) */
+    IDKPT_ARRAY_NODE_GLOBAL_TRANSFORMS = 11, /* read only: float[4][4] per node (Node.GlobalTransform, OpenTK rows) */
+    IDKPT_ARRAY_JOINT_MATRICES = 12          /* read only: float[3][4] per joint matrix idkpt_update_models computed */
 } IdkPtArrayId;
 
 /* Replaces SkyBoxManager's bindless samplerCube in UBO 5 (SkyBoxManager.cs:87):
@@ -622,6 +625,92 @@ IDKPT_API int idkpt_read_range(IdkPtCtx* ctx, IdkPtArrayId which, uint64_t first
  * iterations, not after n. An instance box that is not finite (a NaN or infinite ModelMatrix or BLAS root) stops the build
  * with IDKPT_ERR_INVALID_ARGUMENT and also invalidates the scene. */
 IDKPT_API int idkpt_tlas_build(IdkPtCtx* ctx, int32_t search_radius, float* kernel_ms);
+
+/* ---- ModelManager.Update on the device (ModelManager.cs:236-261): keyframes, node hierarchy, mesh transforms, joint
+ * matrices, then skin, refit and TLAS, from one float per frame. ModelManager's CPU model state (ModelLoader.Node /
+ * ModelAnimation / NodeAnimation / Skin and the SkinningCmds) is handed over once as flat arrays.
+ * Nodes are in pre-order (Node.HierarchyToArray), several models one after another: Parent < own index, -1 for a root.
+ * Arithmetic: one copy (idk_anim_math.h) runs on the device and in the host mirror, which agree byte for byte; OpenTK's own
+ * rounding is not reproduced (DESIGN §8f.2). A host that needs it keeps computing the transforms and joint matrices itself
+ * and calls idkpt_update_range, idkpt_skin_vertices, idkpt_blas_refit and idkpt_tlas_build. */
+#define IDKPT_ANIM_SCALE        0
+#define IDKPT_ANIM_ROTATION     1
+#define IDKPT_ANIM_TRANSLATION  2
+#define IDKPT_ANIM_STEP         0
+#define IDKPT_ANIM_LINEAR       1
+typedef struct IdkPtNodeLocal {        /* Transformation (Transformation.cs) */
+    float Translation[3];
+    float Rotation[4];                 /* x y z w */
+    float Scale[3];
+} IdkPtNodeLocal;
+typedef struct IdkPtNode {
+    int32_t  Parent;
+    uint32_t MeshTransformsStart, MeshTransformsCount;   /* Node.MeshTransformsRange; ranges pairwise disjoint */
+    float    Translation[3], Rotation[4], Scale[3];      /* Node.LocalTransform, as IdkPtNodeLocal */
+    float    GlobalTransform[16];                        /* Node.GlobalTransform as the engine holds it, OpenTK rows */
+} IdkPtNode;
+typedef struct IdkPtNodeAnimation {    /* ModelLoader.NodeAnimation */
+    uint32_t TargetNode;
+    int32_t  Type;                     /* IDKPT_ANIM_SCALE / _ROTATION / _TRANSLATION */
+    int32_t  Mode;                     /* IDKPT_ANIM_STEP / _LINEAR */
+    uint32_t KeyFrameOffset, KeyFrameCount;   /* into KeyFrameTimes; count >= 2 */
+    uint32_t DataOffset;                      /* in floats into KeyFrameData: 3 (scale, translation) or 4 (rotation) per key */
+} IdkPtNodeAnimation;
+typedef struct IdkPtModelAnimation {   /* ModelLoader.ModelAnimation: channels [FirstChannel, +ChannelCount) */
+    float    TMin, TMax;
+    uint32_t FirstChannel, ChannelCount;
+    uint32_t Enabled;                  /* CpuModel.EnabledAnimations */
+} IdkPtModelAnimation;
+typedef struct IdkPtSkin {             /* ModelLoader.Skin + ModelManager.SkinningCmd, in GetSkinningCommands order */
+    uint32_t SkinnedNode, FirstJoint, JointCount, JointMatricesOffset;   /* FirstJoint into JointNodes / InverseJointMatrices */
+    uint32_t InputVertexOffset, OutputVertexOffset, VertexCount, BlasId;
+} IdkPtSkin;
+typedef struct IdkPtAnimationDesc {
+    const IdkPtNode*           Nodes;        uint64_t NodeCount;
+    const IdkPtNodeAnimation*  Channels;     uint64_t ChannelCount;
+    const IdkPtModelAnimation* Animations;   uint64_t AnimationCount;
+    const IdkPtSkin*           Skins;        uint64_t SkinCount;
+    const uint32_t*            JointNodes;   uint64_t JointCount;
+    const float*               InverseJointMatrices;                     /* JointCount x float[4][4], OpenTK rows */
+    const float*               KeyFrameTimes; uint64_t KeyFrameTimeCount;
+    const float*               KeyFrameData;  uint64_t KeyFrameDataCount;
+} IdkPtAnimationDesc;
+IDK_STATIC_ASSERT(sizeof(IdkPtNodeLocal) == 40, "IdkPtNodeLocal must be 40 bytes");
+IDK_STATIC_ASSERT(sizeof(IdkPtNode) == 116, "IdkPtNode must be 116 bytes");
+IDK_STATIC_ASSERT(sizeof(IdkPtNodeAnimation) == 24, "IdkPtNodeAnimation must be 24 bytes");
+IDK_STATIC_ASSERT(sizeof(IdkPtModelAnimation) == 20, "IdkPtModelAnimation must be 20 bytes");
+IDK_STATIC_ASSERT(sizeof(IdkPtSkin) == 32, "IdkPtSkin must be 32 bytes");
+IDK_STATIC_ASSERT(sizeof(IdkPtAnimationDesc) == 120, "IdkPtAnimationDesc must be 120 bytes");
+/* idkpt_set_animations: replaces the context's animation set (needs a scene). Every array is copied and checked first;
+ *   IDKPT_ERR_INVALID_ARGUMENT, with the old set kept, for: a NULL pointer with a count, Parent >= own index or < -1, a
+ *   transform range outside the scene's mesh transforms or overlapping another, a node / channel / joint / BLAS id out of
+ *   range, a key range or key data past its array, fewer than 2 keys, an unknown Type or Mode, or joint offsets that
+ *   overflow. Every mesh transform starts with its "moved in the previous call" bit clear; the previous animation time is
+ *   float.MinValue. idkpt_set_scene releases the set; idkpt_add_models keeps it (it only appends).
+ * idkpt_enable_animations: CpuModel.EnabledAnimations[first, +count) = enabled[i] != 0.
+ * idkpt_set_node_transforms: the Node.LocalTransform setter for nodes [first, +count) (only Translation, Rotation and Scale are read): a node
+ *   whose Transformation differs (float.Equals per field: +0 == -0, NaN == NaN) takes it and becomes dirty.
+ * idkpt_update_models: ModelManager.Update(animation_time) in its order. Sampling (skipped when the time equals the last
+ *   call's), the dirty hierarchy (every dirty node and its descendants: Global = Local.GetMatrix() * Parent.Global, and the
+ *   node's mesh transforms Model = (Global * Invert(before)) * Model with InvModel recomputed), then PrevModelMatrix: a
+ *   transform the hierarchy touched, or one that moved in the previous call, gets Prev = its Model before this call and
+ *   keeps "moved" = (Prev != Model) for the next call. Transforms the host writes with idkpt_update_range stay the host's:
+ *   their Prev is its to set. When a node moved, the joint matrices are recomputed (InverseJointMatrices[j] *
+ *   Joints[j].Global * Invert(SkinnedNode.Global), transposed to 3x4) and every skin's BLAS refitted; skinning runs when a
+ *   node moved and once more after the motion stops, keeping the previous positions as idkpt_skin_vertices does; when a
+ *   node or a mesh instance moved the TLAS is rebuilt with search_radius (as idkpt_tlas_build, including its refusals and,
+ *   on a scene set without UseTlas, its error) and the accumulation reset -- and only then.
+ *   moved_out (may be NULL): bit 0 anyNodeMoved, bit 1 anyMeshInstanceMoved. The node-level work runs first; the call
+ *   then reads one flag word. Host synchronisations: that read, plus the TLAS build's two when a flag is set (the skin and
+ *   refit run inside the build's region); the one skinning call after the motion stops, which builds no TLAS, waits once more. A singular `before` of a node
+ *   with mesh transforms or a singular skinned-node global (Matrix4.Invert throws) makes the call return
+ *   IDKPT_ERR_INVALID_ARGUMENT with nothing changed. Skin vertex ranges are checked against the current skinning data
+ *   first (IDKPT_ERR_INVALID_ARGUMENT, nothing changed). IDKPT_ERR_NO_SCENE without an animation set.
+ *   kernel_ms (may be NULL): device time of the whole call. */
+IDKPT_API int idkpt_set_animations(IdkPtCtx* ctx, const IdkPtAnimationDesc* desc);
+IDKPT_API int idkpt_enable_animations(IdkPtCtx* ctx, uint32_t first, uint32_t count, const uint8_t* enabled);
+IDKPT_API int idkpt_set_node_transforms(IdkPtCtx* ctx, uint32_t first, uint32_t count, const IdkPtNode* nodes);
+IDKPT_API int idkpt_update_models(IdkPtCtx* ctx, float animation_time, int32_t search_radius, uint32_t* moved_out, float* kernel_ms);
 
 /* BLAS.Build + PreSplitting.PreSplit on the device (the loop body of BVH.BlasesBuild, BVH.cs:315-377): the SweepSAH build of
  * one BLAS with early split clipping, node for node and triangle for triangle equal to the host build (idkhost_blas_build),

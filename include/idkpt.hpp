@@ -207,6 +207,20 @@ public:
         check(idkpt_add_models(ctx_, &models, settings, &ms), "idkpt_add_models");
         return ms;
     }
+    // ModelManager.Update on the device (idkpt_set_animations .. idkpt_update_models)
+    void SetAnimations(const IdkPtAnimationDesc& desc) { check(idkpt_set_animations(ctx_, &desc), "idkpt_set_animations"); }
+    void EnableAnimations(uint32_t first, uint32_t count, const uint8_t* enabled) {
+        check(idkpt_enable_animations(ctx_, first, count, enabled), "idkpt_enable_animations");
+    }
+    void SetNodeTransforms(uint32_t first, uint32_t count, const IdkPtNode* nodes) {
+        check(idkpt_set_node_transforms(ctx_, first, count, nodes), "idkpt_set_node_transforms");
+    }
+    // Returns the moved bits (1 anyNodeMoved, 2 anyMeshInstanceMoved); *kernelMs (may be null) the device time
+    uint32_t UpdateModels(float animationTime, int32_t searchRadius = 15, float* kernelMs = nullptr) {
+        uint32_t moved = 0;
+        check(idkpt_update_models(ctx_, animationTime, searchRadius, &moved, kernelMs), "idkpt_update_models");
+        return moved;
+    }
     float Denoise(const IdkPtDenoiseSettings& s) { float ms = 0.0f; check(idkpt_denoise(ctx_, &s, &ms), "idkpt_denoise"); return ms; }   // PathTracerPipeline.Denoise
     std::vector<float> Denoised() const { return read(IDKPT_IMAGE_DENOISED); }
     void RegisterHostBuffer(void* hostPtr, uint64_t bytes) { check(idkpt_register_host_buffer(ctx_, hostPtr, bytes), "idkpt_register_host_buffer"); }
