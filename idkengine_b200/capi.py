@@ -118,6 +118,7 @@ EXPORTS = [
     "idkpt_ssr", "idkpt_ssr_device_ptrs", "idkpt_taa_resolve", "idkpt_taa_device_ptr",
     "idkpt_shading_rate", "idkpt_shading_rate_device_ptr",
     "idkpt_gbuffer", "idkpt_gbuffer_device_ptrs", "idkpt_read_gbuffer", "idkpt_prev_positions_device_ptr", "idkpt_transparency", "idkpt_lights_and_skybox",
+    "idkpt_lights_and_skybox_vrs",
     "idkpt_sky_atmosphere", "idkpt_sky_equirectangular", "idkpt_read_sky",
     "idkpt_blas_build", "idkpt_blas_build_info", "idkpt_blas_build_copy", "idkpt_blas_build_free", "idkpt_blas_rebuild", "idkpt_blas_sah",
     "idkpt_blas_build_batch", "idkpt_blas_build_batch_copy", "idkpt_add_models",
@@ -592,6 +593,8 @@ def load(path=None):
     L.idkpt_read_gbuffer.argtypes = [c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp]
     L.idkpt_lights_and_skybox.restype = c_i32
     L.idkpt_lights_and_skybox.argtypes = [c_vp, c_vp, c_vp, c_vp, P(c_f)]
+    L.idkpt_lights_and_skybox_vrs.restype = c_i32
+    L.idkpt_lights_and_skybox_vrs.argtypes = [c_vp, c_vp, c_vp, c_vp, P(c_f)]
     L.idkpt_abi_version.restype = c_u32
     L.idkpt_abi_version.argtypes = []
     if path == _build.LIBIDKPT:

@@ -8,10 +8,14 @@
 //                     constant memory), with the light draw's depth test (LESS, back faces culled) against the G-buffer depth;
 //                     the winning fragment's colour, normal, emissive, velocity and depth; then the skybox (LEQUAL against the
 //                     window depth 1) where the depth is still 1: the cube-map colour and the rotation-only velocity
+//   k_lights_skybox_vrs the same draws under the shading-rate image (VariableRateShadingNV on both draws): the same kernel
+//                     body (lights_skybox_pixel<true>), with coverage and depth per pixel and the fragment shaders' values at
+//                     the centre of the pixel's coarse fragment
 //
 // The rules are spelled out in DESIGN.md 8f.1i and restated independently by the CPU oracle; the two agree bit for bit.
 #pragma once
 #include "idk_gbuffer.cuh"
+#include "idk_vrs.cuh"
 
 // LightManager's sphere: GeometricPrimitives.Sphere with 12 latitudes and 12 longitudes at radius 1.
 #define IDK_SPHERE_SEGMENTS 12
@@ -83,10 +87,20 @@ struct LightsSkyboxArgs {
     float4* color;                 // the deferred image [h][w], written in place
 };
 
-__global__ void __launch_bounds__(256) k_lights_skybox(LightsSkyboxArgs a) {
-    __shared__ GpuLight s_lights[IDK_GPU_MAX_UBO_LIGHT_COUNT];
-    for (int i = threadIdx.x; i < a.lightCount; i += blockDim.x) s_lights[i] = a.lights[i];
-    __syncthreads();
+// Rule 5's direction at NDC (sx, sy): (InvView * vec4(PerspectiveTransform((s, 1), InvProjection), 0)).xyz, as k_ssr's miss
+// direction.
+__device__ __forceinline__ f3 sky_direction(const LightsSkyboxArgs& a, float sx, float sy) {
+    const f3 v = deferred_perspective(a.invProjection, sx, sy, 1.0f);
+    const float* m = a.invView;
+    return mk3(((m[0] * v.x + m[4] * v.y) + m[8] * v.z) + m[12] * 0.0f, ((m[1] * v.x + m[5] * v.y) + m[9] * v.z) + m[13] * 0.0f,
+               ((m[2] * v.x + m[6] * v.y) + m[10] * v.z) + m[14] * 0.0f);
+}
+
+// One pixel of the two draws. kVrs: the draws under the rate image `rates` ([ceil(h/16)][ceil(w/16)] palette indices, 8f.1i's
+// VRS paragraph): coverage, the depth test and the written depth stay the pixel's own; what the fragment shaders compute
+// (FragPos, the normal, the velocity, the sky's TexCoord) is evaluated at the centre of the pixel's coarse fragment.
+template <bool kVrs>
+__device__ __forceinline__ void lights_skybox_pixel(const LightsSkyboxArgs& a, const GpuLight* s_lights, const uint8_t* rates) {
     int x, y;
     if (!deferred_pixel(a.w, a.h, x, y)) return;
     const size_t p = (size_t)y * a.w + x;
@@ -124,6 +138,15 @@ __global__ void __launch_bounds__(256) k_lights_skybox(LightsSkyboxArgs a) {
         }
     }
 
+    // VRS: the pixel's coarse fragment, cw x ch at (x - x mod cw, y - y mod ch) inside its 16x16 tile, and its centre in pixels
+    float xc = 0.0f, yc = 0.0f;
+    if constexpr (kVrs) {
+        int cw, ch;
+        vrs_fragment_size(rates[(size_t)(y / IDK_VRS_TILE) * ((a.w + IDK_VRS_TILE - 1) / IDK_VRS_TILE) + x / IDK_VRS_TILE], cw, ch);
+        xc = (float)(x - x % cw) + 0.5f * (float)cw;
+        yc = (float)(y - y % ch) + 0.5f * (float)ch;
+    }
+
     if (best >= 0) {
         // rule 4: the light fragment's outputs
         const GpuLight& light = s_lights[best];
@@ -132,6 +155,17 @@ __global__ void __launch_bounds__(256) k_lights_skybox(LightsSkyboxArgs a) {
         const float radius = light.Radius;
         const uint32_t k = c_sphere_triangles[bestTri];
         const uint32_t i0 = k & 255u, i1 = (k >> 8) & 255u, i2 = k >> 16;
+        float thisX = ndcX, thisY = ndcY;
+        if constexpr (kVrs) {
+            // the centre's ray against the winning triangle's plane: ray_triangle's arithmetic, its inside and t tests ignored
+            thisX = xc / (float)a.w * 2.0f - 1.0f - a.jitter[0];
+            thisY = yc / (float)a.h * 2.0f - 1.0f - a.jitter[1];
+            const f3 dc = normalize3(deferred_perspective(a.invProjView, thisX, thisY, 1.0f) - o);
+            const f3 w0 = light_vertex(radius, position, i0), w1 = light_vertex(radius, position, i1), w2 = light_vertex(radius, position, i2);
+            const f3 e1 = w1 - w0, e2 = w2 - w0;
+            float tHit;
+            (void)ray_triangle(o, dc, w0, e1, e2, cross3(e1, e2), b0, b1, tHit);
+        }
         const float b2 = 1.0f - b0 - b1;
         const f3 fragPos = (light_vertex(radius, position, i0) * b0 + light_vertex(radius, position, i1) * b1) + light_vertex(radius, position, i2) * b2;
         float ex, ey;
@@ -147,16 +181,24 @@ __global__ void __launch_bounds__(256) k_lights_skybox(LightsSkyboxArgs a) {
         a.emissive[3 * p] = gbuffer_ufloat(light.Color[0], 6, 65024.0f);
         a.emissive[3 * p + 1] = gbuffer_ufloat(light.Color[1], 6, 65024.0f);
         a.emissive[3 * p + 2] = gbuffer_ufloat(light.Color[2], 5, 64512.0f);
-        a.velocity[p] = make_float2(gbuffer_half((ndcX - pcx / pcw) * 0.5f), gbuffer_half((ndcY - pcy / pcw) * 0.5f));
+        a.velocity[p] = make_float2(gbuffer_half((thisX - pcx / pcw) * 0.5f), gbuffer_half((thisY - pcy / pcw) * 0.5f));
         a.color[p] = make_float4(light.Color[0], light.Color[1], light.Color[2], 1.0f);
     } else if (1.0f <= depth) {
         // rule 5: the skybox at the unjittered pixel centre, on the cube around the camera
-        const float sx = ((float)x + 0.5f) / (float)a.w * 2.0f - 1.0f, sy = ((float)y + 0.5f) / (float)a.h * 2.0f - 1.0f;
-        const f3 v = deferred_perspective(a.invProjection, sx, sy, 1.0f);
-        const float* m = a.invView;                                  // (InvView * vec4(v, 0)).xyz, as k_ssr's miss direction
-        const f3 dir = mk3(((m[0] * v.x + m[4] * v.y) + m[8] * v.z) + m[12] * 0.0f, ((m[1] * v.x + m[5] * v.y) + m[9] * v.z) + m[13] * 0.0f,
-                           ((m[2] * v.x + m[6] * v.y) + m[10] * v.z) + m[14] * 0.0f);
-        const f3 c = dir * (0.5f / fmaxf(fmaxf(fabsf(dir.x), fabsf(dir.y)), fabsf(dir.z)));
+        float sx = ((float)x + 0.5f) / (float)a.w * 2.0f - 1.0f, sy = ((float)y + 0.5f) / (float)a.h * 2.0f - 1.0f;
+        const f3 dir = sky_direction(a, sx, sy);
+        f3 c;
+        if constexpr (kVrs) {
+            // TexCoord on the pixel's own cube face (the axis of its largest |dir|, x before y before z), at the fragment centre
+            const float ax = fabsf(dir.x), ay = fabsf(dir.y), az = fabsf(dir.z);
+            const int axis = ax >= ay && ax >= az ? 0 : ay >= az ? 1 : 2;
+            sx = xc / (float)a.w * 2.0f - 1.0f;
+            sy = yc / (float)a.h * 2.0f - 1.0f;
+            const f3 dc = sky_direction(a, sx, sy);
+            c = dc * (0.5f / fabsf(axis == 0 ? dc.x : axis == 1 ? dc.y : dc.z));
+        } else {
+            c = dir * (0.5f / fmaxf(fmaxf(fabsf(dir.x), fabsf(dir.y)), fabsf(dir.z)));
+        }
         const f3 sky = sample_sky(a.sc, c);
         const float* pv = a.prevView;                                // mat3(PrevView) * c, then Projection * (., 1)
         const f3 pc = mk3((pv[0] * c.x + pv[4] * c.y) + pv[8] * c.z, (pv[1] * c.x + pv[5] * c.y) + pv[9] * c.z, (pv[2] * c.x + pv[6] * c.y) + pv[10] * c.z);
@@ -164,4 +206,20 @@ __global__ void __launch_bounds__(256) k_lights_skybox(LightsSkyboxArgs a) {
         a.velocity[p] = make_float2(gbuffer_half((sx - q.x / q.w) * 0.5f), gbuffer_half((sy - q.y / q.w) * 0.5f));
         a.color[p] = make_float4(sky.x, sky.y, sky.z, 1.0f);
     }
+}
+
+__global__ void __launch_bounds__(256) k_lights_skybox(LightsSkyboxArgs a) {
+    __shared__ GpuLight s_lights[IDK_GPU_MAX_UBO_LIGHT_COUNT];
+    for (int i = threadIdx.x; i < a.lightCount; i += blockDim.x) s_lights[i] = a.lights[i];
+    __syncthreads();
+    lights_skybox_pixel<false>(a, s_lights, nullptr);
+}
+
+// The same draws under the context's rate image: one thread per pixel as k_lights_skybox, each reading its tile's rate byte.
+// Coverage is per pixel, so there is no fragment list (k_vrs_scan) to build.
+__global__ void __launch_bounds__(256) k_lights_skybox_vrs(LightsSkyboxArgs a, const uint8_t* __restrict__ rates) {
+    __shared__ GpuLight s_lights[IDK_GPU_MAX_UBO_LIGHT_COUNT];
+    for (int i = threadIdx.x; i < a.lightCount; i += blockDim.x) s_lights[i] = a.lights[i];
+    __syncthreads();
+    lights_skybox_pixel<true>(a, s_lights, rates);
 }

@@ -1589,7 +1589,7 @@ static int preload_kernels(IdkPtCtx* ctx) {
     IDK_PRELOAD(k_ssao); IDK_PRELOAD(k_deferred_lighting); IDK_PRELOAD(k_ssr); IDK_PRELOAD(k_taa_resolve);
     IDK_PRELOAD(k_shading_rate); IDK_PRELOAD(k_vrs_scan); IDK_PRELOAD(k_deferred_lighting_vrs); IDK_PRELOAD(k_gbuffer);
     IDK_PRELOAD(k_transparency<false>); IDK_PRELOAD(k_transparency<true>); IDK_PRELOAD(k_lights_skybox);
-    IDK_PRELOAD(k_sky_atmosphere); IDK_PRELOAD(k_sky_equirect);
+    IDK_PRELOAD(k_lights_skybox_vrs); IDK_PRELOAD(k_sky_atmosphere); IDK_PRELOAD(k_sky_equirect);
 #undef IDK_PRELOAD
     return IDKPT_OK;
 }
@@ -3542,16 +3542,20 @@ IDKPT_API int idkpt_transparency(IdkPtCtx* ctx, const GpuPerFrameData* frame, co
     return IDKPT_OK;
 }
 
+} // extern "C"
+
 // ---- the light spheres and the skybox (RasterPipeline.Render's "Draw lights" + "Draw skybox") ---------------------------------
-IDKPT_API int idkpt_lights_and_skybox(IdkPtCtx* ctx, const GpuPerFrameData* frame, const float* taaJitter, float* outRgba32f,
-                                      float* kernelMs) {
-    static const char* who = "idkpt_lights_and_skybox";
-    if (!ctx || !frame) return fail(ctx, IDKPT_ERR_INVALID_ARGUMENT, "idkpt_lights_and_skybox: null argument");
+// Both entry points: per pixel, or (vrs) under the rate image of the last idkpt_shading_rate call.
+static int lights_and_skybox(IdkPtCtx* ctx, const char* who, bool vrs, const GpuPerFrameData* frame, const float* taaJitter,
+                             float* outRgba32f, float* kernelMs) {
+    if (!ctx || !frame) return fail(ctx, IDKPT_ERR_INVALID_ARGUMENT, (std::string(who) + ": null argument").c_str());
     if (!ctx->haveScene) return fail(ctx, who, IDKPT_ERR_NO_SCENE, "no scene");
     const RasterState& r = ctx->raster;
     if (!r.gb.valid()) return fail(ctx, who, IDKPT_ERR_INVALID_ARGUMENT, "call idkpt_gbuffer first");
     if (!r.deferred.valid_at(r.gb.w, r.gb.h))
         return fail(ctx, who, IDKPT_ERR_INVALID_ARGUMENT, "needs an idkpt_deferred_lighting image of the G-buffer's size");
+    if (vrs && !r.vrs.valid_at(r.gb.w, r.gb.h))
+        return fail(ctx, who, IDKPT_ERR_INVALID_ARGUMENT, "needs an idkpt_shading_rate image of the G-buffer's size");
     LightsSkyboxArgs a;
     if (!read_jitter(taaJitter, a.jitter)) return fail(ctx, who, IDKPT_ERR_INVALID_ARGUMENT, "jitter not finite");
     CK(cudaSetDevice(ctx->device));
@@ -3575,9 +3579,22 @@ IDKPT_API int idkpt_lights_and_skybox(IdkPtCtx* ctx, const GpuPerFrameData* fram
     a.velocity = (float2*)(base + off[5]);
     a.color = (float4*)r.deferred.buf[0].p;
     return run_timed(ctx, who, kernelMs, [&]() -> int {
-        k_lights_skybox<<<tile_blocks(w, h), 256, 0, ctx->stream>>>(a);
+        if (vrs) k_lights_skybox_vrs<<<tile_blocks(w, h), 256, 0, ctx->stream>>>(a, (const uint8_t*)r.vrs.buf[0].p);
+        else k_lights_skybox<<<tile_blocks(w, h), 256, 0, ctx->stream>>>(a);
         return IDKPT_OK;
     }, outRgba32f, r.deferred.buf[0].p, outRgba32f ? (size_t)w * h * 16 : 0);
+}
+
+extern "C" {
+
+IDKPT_API int idkpt_lights_and_skybox(IdkPtCtx* ctx, const GpuPerFrameData* frame, const float* taaJitter, float* outRgba32f,
+                                      float* kernelMs) {
+    return lights_and_skybox(ctx, "idkpt_lights_and_skybox", false, frame, taaJitter, outRgba32f, kernelMs);
+}
+
+IDKPT_API int idkpt_lights_and_skybox_vrs(IdkPtCtx* ctx, const GpuPerFrameData* frame, const float* taaJitter, float* outRgba32f,
+                                          float* kernelMs) {
+    return lights_and_skybox(ctx, "idkpt_lights_and_skybox_vrs", true, frame, taaJitter, outRgba32f, kernelMs);
 }
 
 } // extern "C"

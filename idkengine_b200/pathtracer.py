@@ -740,11 +740,12 @@ class PathTracer:
         return out
 
     # ---- the light spheres and the skybox (RasterPipeline.Render's "Draw lights" + "Draw skybox")
-    def LightsAndSkybox(self, frame, jitter=None, download=True):
+    def LightsAndSkybox(self, frame, jitter=None, download=True, vrs=False):
         """Draws the light spheres and the skybox into the images of the last GBuffer call and the last DeferredLighting image
         (which must have the G-buffer's size), in place (DESIGN.md 8f.1i): later DEFERRED reads, GBufferDevicePtrs and
-        GBuffer downloads see them. jitter: taaDataUBO.Jitter in NDC units (None = 0). Returns the lit image, float32 [H, W, 4],
-        or None with download=False. Kernel ms in last_lights_and_skybox_ms."""
+        GBuffer downloads see them. jitter: taaDataUBO.Jitter in NDC units (None = 0). vrs=True draws them as the engine does
+        with IsVariableRateShading, under the rate image of the last ShadingRate call (which must have the G-buffer's size).
+        Returns the lit image, float32 [H, W, 4], or None with download=False. Kernel ms in last_lights_and_skybox_ms."""
         jit = self._jitter(jitter)
         frame = np.ascontiguousarray(frame)
         out = None
@@ -752,8 +753,9 @@ class PathTracer:
             g, _ = self.GBufferDevicePtrs()
             out = np.zeros((g.Height, g.Width, 4), np.float32)
         ms = ctypes.c_float()
-        self._check(self._lib.idkpt_lights_and_skybox(self._ctx, frame.ctypes.data, jit, out.ctypes.data if download else None,
-                                                      ctypes.byref(ms)), "idkpt_lights_and_skybox")
+        name = "idkpt_lights_and_skybox_vrs" if vrs else "idkpt_lights_and_skybox"
+        self._check(getattr(self._lib, name)(self._ctx, frame.ctypes.data, jit, out.ctypes.data if download else None, ctypes.byref(ms)),
+                    name)
         self.last_lights_and_skybox_ms = ms.value
         return out
 

@@ -590,6 +590,17 @@ IDKPT_API int idkpt_transparency(IdkPtCtx* ctx, const GpuPerFrameData* frame, co
  * The call is synchronous and ordered after the samples idkpt_compute has queued. */
 IDKPT_API int idkpt_lights_and_skybox(IdkPtCtx* ctx, const GpuPerFrameData* frame, const float* taa_jitter, float* out_rgba32f,
                                       float* kernel_ms);
+/* idkpt_lights_and_skybox_vrs: the same two draws with RasterPipeline.IsVariableRateShading on, under the rate image of the last
+ *   idkpt_shading_rate call (palette 1x1, 2x1, 2x2, 4x2, 4x4; pixel (x, y) takes texel (x/16, y/16)). Coverage, the depth test
+ *   and the written depth stay per pixel, so the depth and emissive planes and which pixels the lights and the sky cover are
+ *   those of idkpt_lights_and_skybox. The light's normal and velocity and the sky's colour and velocity are evaluated once per
+ *   coarse fragment, at its centre: a light pixel uses the centre's ray against the plane of the triangle the pixel itself won,
+ *   a sky pixel the cube face its own direction leaves through. An all-1x1 rate image gives idkpt_lights_and_skybox's bytes.
+ *   The rules are in DESIGN.md 8f.1i. Besides idkpt_lights_and_skybox's checks the call needs a rate image of the G-buffer's
+ *   size (idkpt_set_scene drops it); otherwise it returns IDKPT_ERR_INVALID_ARGUMENT and changes no byte. Arguments, ordering
+ *   and idempotence as idkpt_lights_and_skybox. */
+IDKPT_API int idkpt_lights_and_skybox_vrs(IdkPtCtx* ctx, const GpuPerFrameData* frame, const float* taa_jitter, float* out_rgba32f,
+                                          float* kernel_ms);
 
 /* ---- dynamic geometry (SURVEY.md 8f.2): ModelManager.Update = skin -> refit -> TLAS (ModelManager.cs:236-261) ----
  * idkpt_set_skinning_data: unskinnedVertexSSBO upload (52-byte GpuUnskinnedVertex records).

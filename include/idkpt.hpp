@@ -410,6 +410,12 @@ public:
         check(idkpt_lights_and_skybox(ctx_, &frame, taaJitter, outRgba32f, &ms), "idkpt_lights_and_skybox");
         return ms;
     }
+    // The same draws with IsVariableRateShading, under the rate image of the last ShadingRate call (DESIGN.md 8f.1i).
+    float LightsAndSkyboxVrs(const GpuPerFrameData& frame, const float* taaJitter = nullptr, float* outRgba32f = nullptr) {
+        float ms = 0.0f;
+        check(idkpt_lights_and_skybox_vrs(ctx_, &frame, taaJitter, outRgba32f, &ms), "idkpt_lights_and_skybox_vrs");
+        return ms;
+    }
     void SetSkinningData(const GpuUnskinnedVertex* vertices, uint64_t count) { check(idkpt_set_skinning_data(ctx_, vertices, count), "idkpt_set_skinning_data"); }
     void SkinVertices(const float* jointMatrices3x4, uint64_t jointCount, const IdkPtSkinningCmd* cmds, uint32_t cmdCount) {
         check(idkpt_skin_vertices(ctx_, jointMatrices3x4, jointCount, cmds, cmdCount, nullptr), "idkpt_skin_vertices");
