@@ -205,11 +205,13 @@ def post_process(result, settings=None, want_bloom=False, threads=None):
 
 
 def tex_sample(pixels, uv, srgb=False, wrap_s=10497, wrap_t=10497, flags=0):
-    px = np.ascontiguousarray(pixels, np.uint8)
+    """TexSample at float32 uv [N, 2] of RGBA8 pixels, or of a texture dict as host.Scene.textures holds it (uncompressed
+    formats only: the oracle takes block-compressed textures decoded)."""
+    tex = pixels if isinstance(pixels, dict) else dict(pixels=pixels, srgb=srgb, wrap_s=wrap_s, wrap_t=wrap_t, flags=flags)
+    arr, keep = capi.texture_descs([tex])
     uv = np.ascontiguousarray(uv, np.float32)
-    t = capi.IdkPtTextureDesc(px.ctypes.data, px.shape[1], px.shape[0], 1 if srgb else 0, wrap_s, wrap_t, flags)
     out = np.zeros((len(uv), 4), np.float32)
-    lib().oracle_tex_sample(ctypes.byref(t), uv.ctypes.data, len(uv), out.ctypes.data)
+    lib().oracle_tex_sample(arr, uv.ctypes.data, len(uv), out.ctypes.data)
     return out
 
 

@@ -10,6 +10,8 @@ from idkengine_b200 import scenes
 from idkengine_b200.host import Model, Scene, trs_matrix
 
 W, H = 48, 32
+# float32 barycentrics move the interpolated texcoord by at most this much here (about 64 float32 ulps of the texcoords' span)
+TC_SPREAD = 64 * 2.0 ** -24 * 2.0
 CAM = dict(position=(0.0, 1.0, 3.0), view_dir=(0.0, 0.0, -1.0), fov_y_deg=60.0)
 
 
@@ -166,8 +168,21 @@ def float64_gbuffer(scene, frame, w, h, jitter=(0.0, 0.0)):
             t = scene.blas_triangles[k]
             ids = [t["X"], t["Y"], t["Z"]]
             tris.append((ids, (M @ np.c_[P[ids], np.ones(3)].T).T[:, :3], (Mp @ np.c_[P[ids], np.ones(3)].T).T[:, :3], int(t["MeshId"])))
+    import surface_ref64           # it takes encode_unit_vec and ufloat64 from this module
     out = dict(depth=np.ones((h, w)), normal=np.zeros((h, w, 2)), albedo=np.zeros((h, w, 3)), mr=np.zeros((h, w, 2)),
-               emissive=np.zeros((h, w, 3)), velocity=np.zeros((h, w, 2)), mesh=np.full((h, w), -1), edge=np.full((h, w), np.inf))
+               emissive=np.zeros((h, w, 3)), velocity=np.zeros((h, w, 2)), mesh=np.full((h, w), -1), edge=np.full((h, w), np.inf),
+               albedo_lo=np.zeros((h, w, 3)), albedo_hi=np.zeros((h, w, 3)))
+
+    def base_colour(mat, b, ids):
+        """(texel at the hit, lowest and highest texel over the texcoords within TC_SPREAD of it) of the base-colour texture."""
+        if not mat["BaseColorTexture"]:
+            return np.ones(4), np.ones(4), np.ones(4)
+        tc = b @ scene.vertices["TexCoord"][ids].astype(np.float64)
+        tex = scene.textures[int(mat["BaseColorTexture"]) - 1]
+        at = surface_ref64.sample(tex, tc.astype(np.float32)[None], spread=False)[0][0]
+        around = (tc + TC_SPREAD * np.stack(np.meshgrid([-1, 0, 1], [-1, 0, 1]), -1).reshape(-1, 2)).astype(np.float32)
+        lo, hi = surface_ref64.sample(tex, around)
+        return at, lo.min(0), hi.max(0)
     for y in range(h):
         for x in range(w):
             ndc = np.array([(x + 0.5) / w * 2 - 1 - jitter[0], (y + 0.5) / h * 2 - 1 - jitter[1], 1.0, 1.0])
@@ -200,20 +215,20 @@ def float64_gbuffer(scene, frame, w, h, jitter=(0.0, 0.0)):
                     continue
                 c = int(mat["BaseColorFactor"])
                 alpha = ((c >> 24) & 255) / 255.0
-                if mat["BaseColorTexture"]:
-                    tc = b @ scene.vertices["TexCoord"][ids].astype(np.float64)
-                    tex = scene.textures[int(mat["BaseColorTexture"]) - 1]
-                    alpha *= ol.tex_sample(tex["pixels"], tc.astype(np.float32)[None], srgb=tex["srgb"])[0, 3]
+                alpha *= base_colour(mat, b, ids)[0][3]
                 if alpha < mat["AlphaCutoff"]:
                     continue
-                best = (t, b, wp, pp, n, mesh_id, depth)
+                best = (t, b, wp, pp, n, mesh_id, depth, ids)
             if best is None:
                 continue
-            t, b, wp, pp, n, mesh_id, depth = best
+            t, b, wp, pp, n, mesh_id, depth, ids = best
             mesh = scene.meshes[mesh_id]
             mat = scene.materials[mesh["MaterialId"]]
             c = int(mat["BaseColorFactor"])
-            albedo = np.array([(c >> s) & 255 for s in (0, 8, 16)]) / 255.0
+            factor = np.array([(c >> s) & 255 for s in (0, 8, 16)]) / 255.0
+            texel, tlo, thi = base_colour(mat, b, ids)
+            albedo = factor * texel[:3]
+            out["albedo_lo"][y, x], out["albedo_hi"][y, x] = factor * tlo[:3], factor * thi[:3]
             nrm = n / np.linalg.norm(n) * (1.0 if np.dot(n, d) < 0 else -1.0)    # flat quads: the vertex normals are the face's
             clip_prev = (ppv @ np.c_[pp, np.ones(3)].T).T
             pc = b @ clip_prev
@@ -250,10 +265,15 @@ def test_oracle_matches_float64_brute_force(jitter):
     m = far & hit
     assert np.allclose(g[0][m], ref["depth"][m], rtol=0, atol=2e-6)
     assert np.array_equal(g[0][far & ~hit], np.ones((far & ~hit).sum(), np.float32))
-    untextured = m & (ref["mesh"] != 5)    # the cut-out's colour is its texture's (the GPU tests compare it with the oracle)
-    for k, want in ((2, ref["albedo"]), (4, ref["emissive"])):
-        q = np.stack([ufloat64(want[..., c], 6 if c < 2 else 5, 65024.0 if c < 2 else 64512.0) for c in range(3)], -1)
-        assert np.array_equal(g[k][untextured], q[untextured].astype(np.float32))
+    store = lambda v: np.stack([ufloat64(v[..., c], 6 if c < 2 else 5, 65024.0 if c < 2 else 64512.0) for c in range(3)], -1)
+    assert np.array_equal(g[4][m], store(ref["emissive"])[m].astype(np.float32))
+    # the albedo lies between the stores of the base colour's range over the texcoords float32 allows; untextured meshes
+    # have one value, and so does every textured pixel whose range does not straddle a store boundary
+    lo, hi = store(ref["albedo_lo"]), store(ref["albedo_hi"])
+    assert np.all((g[2][m] >= lo[m]) & (g[2][m] <= hi[m]))
+    assert np.array_equal(store(ref["albedo"])[m & (ref["mesh"] != 5)], lo[m & (ref["mesh"] != 5)])
+    cut = m & (ref["mesh"] == 5)
+    assert int(cut.sum()) == 12 and int((lo != hi)[cut].any(-1).sum()) == 1   # pinned: textured; one range straddles a store boundary
     assert np.array_equal(g[3][m], rg8(ref["mr"])[m].astype(np.float32))
     boundary = np.abs(ref["normal"] * 255 - np.floor(ref["normal"] * 255) - 0.5) < 1e-3
     nm = m[..., None] & ~boundary

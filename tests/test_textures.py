@@ -5,6 +5,7 @@ import numpy as np
 import pytest
 
 import oracle_lib as ol
+import surface_ref64
 from idkengine_b200 import capi, scenes
 
 
@@ -14,30 +15,8 @@ def textured():
 
 
 def ref_sample(px, uv, srgb, wrap_s, wrap_t):
-    """float64 restatement of GL bilinear sampling at lod 0 with the three wrap modes."""
-    h, w = px.shape[:2]
-    tex = px.astype(np.float64) / 255.0
-    if srgb:
-        c = tex[..., :3]
-        tex[..., :3] = np.where(c <= 0.04045, c / 12.92, ((c + 0.055) / 1.055) ** 2.4)
-
-    def wrap(i, n, mode):
-        if mode == 33071:
-            return np.clip(i, 0, n - 1)
-        if mode == 33648:
-            m = np.mod(i, 2 * n)
-            return np.where(m < n, m, 2 * n - 1 - m)
-        return np.mod(i, n)
-
-    u, v = uv[:, 0].astype(np.float64), uv[:, 1].astype(np.float64)
-    x, y = u * w - 0.5, v * h - 0.5
-    x0, y0 = np.floor(x), np.floor(y)
-    fx, fy = (x - x0)[:, None], (y - y0)[:, None]
-    xa, xb = wrap(x0.astype(int), w, wrap_s), wrap(x0.astype(int) + 1, w, wrap_s)
-    ya, yb = wrap(y0.astype(int), h, wrap_t), wrap(y0.astype(int) + 1, h, wrap_t)
-    top = tex[ya, xa] * (1 - fx) + tex[ya, xb] * fx
-    bot = tex[yb, xa] * (1 - fx) + tex[yb, xb] * fx
-    return top * (1 - fy) + bot * fy
+    """float64 GL bilinear sampling at lod 0 with the three wrap modes (tests/surface_ref64.py)."""
+    return surface_ref64.sample(dict(pixels=px, srgb=srgb, wrap_s=wrap_s, wrap_t=wrap_t), uv, spread=False)[0]
 
 
 @pytest.mark.parametrize("srgb", [False, True])
