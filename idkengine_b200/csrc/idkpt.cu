@@ -11,6 +11,8 @@
 #include <algorithm>
 #include <cmath>
 #include <functional>
+#include <array>
+#include <optional>
 
 #include "../../include/idkpt.h"
 #include "idk_kernels.cuh"
@@ -44,6 +46,35 @@ struct DevBuf {
     void* p = nullptr;
     size_t bytes = 0;
 };
+
+static void release(DevBuf& b) {
+    if (b.p) cudaFree(b.p);
+    b.p = nullptr;
+    b.bytes = 0;
+}
+
+// The scene's device arrays. The path tracer holds one set; idkpt_blas_rebuild and idkpt_add_models build the arrays they
+// replace into a staged set and swap it in (commit_scene), which then frees the replaced ones. The voxeliser's own copy
+// (idkvx_set_scene) fills the arrays it reads and leaves the others empty.
+struct SceneArrays;
+static void release(SceneArrays& a);
+struct SceneArrays {
+    DevBuf nodes;                  // [nodes | triRec]: one allocation, so that one L2 access-policy window covers both
+    DevBuf blasTris, positions, descs, instances, xforms, meshes, materials, vertices, lights, tlas, vtxFrame, surfRec;
+    size_t nodeBytes = 0;          // the node part of `nodes`, 256-byte aligned: the triangle records start here
+    SceneArrays() = default;
+    SceneArrays(const SceneArrays&) = delete;
+    SceneArrays& operator=(const SceneArrays&) = delete;
+    ~SceneArrays() { release(*this); }
+    std::array<DevBuf*, 13> buffers() {
+        return {&nodes, &blasTris, &positions, &descs, &instances, &xforms, &meshes, &materials, &vertices, &lights, &tlas, &vtxFrame, &surfRec};
+    }
+};
+
+static void release(SceneArrays& a) {
+    for (DevBuf* b : a.buffers()) release(*b);
+    a.nodeBytes = 0;
+}
 
 // What the path tracer (IdkPtCtx) and the voxeliser (IdkVxCtx) contexts share: device, stream, last error, and the events
 // run_timed brackets synchronous work with.
@@ -142,7 +173,7 @@ struct IdkPtCtx : IdkCtxBase {
     bool haveScene = false;
     DeviceScene sc = {};
     IdkPtSceneDesc counts = {};    // element counts only (pointers unused)
-    DevBuf nodes, triRec, blasTris, positions, descs, instances, xforms, meshes, materials, vertices, lights, tlas, vtxFrame, surfRec;
+    SceneArrays scene;
     std::vector<GpuLight> hostLights;   // host mirror of `lights` (idkpt_set_scene, idkpt_update_range): shadow-index checks
     float sky[3] = {0.0f, 0.0f, 0.0f};
     DevBuf skyFaces;
@@ -176,7 +207,6 @@ struct IdkPtCtx : IdkCtxBase {
     std::vector<uint32_t> unskinnedMaxJoint;   // per vertex max(JointIndices), host copy for range validation
     std::vector<GpuBlasDesc> hostDescs;
     std::vector<GpuBlasInstance> hostInstances;   // host mirror of `instances` (idkpt_set_scene): a bound voxeliser's draw list
-    size_t nodeBytes = 0;
     // prevVertexPositionSSBO (ModelManager.cs:620): the positions before the last skin of each range. Created from the
     // positions at the first idkpt_skin_vertices or idkpt_prev_positions_device_ptr after idkpt_set_scene or idkpt_add_models,
     // which release it.
@@ -270,12 +300,6 @@ static cudaError_t ensure(DevBuf& b, size_t bytes) {
     return e;
 }
 
-static void release(DevBuf& b) {
-    if (b.p) cudaFree(b.p);
-    b.p = nullptr;
-    b.bytes = 0;
-}
-
 static void release_textures(TextureTable& t) {
     for (DevBuf& b : t.pools) release(b);
     t.pools.clear();
@@ -352,10 +376,18 @@ static const FirstHitKernel kFirstHit[2][2][2] = {
     {{k_first_hit<false, false, false>, k_first_hit<false, false, true>}, {k_first_hit<true, false, false>, k_first_hit<true, false, true>}},
     {{k_first_hit<false, true, false>, k_first_hit<false, true, true>}, {k_first_hit<true, true, false>, k_first_hit<true, true, true>}}};
 
+// The shared-memory traversal stack of a block (IDK_BLOCK threads x stackSize entries) must fit the 200 KB the kernels are
+// given. `who` prefixes the refusal when given.
+static int check_stack_size(IdkPtCtx* ctx, const char* who, int stackSize) {
+    if ((size_t)std::max(1, stackSize) * IDK_BLOCK * sizeof(uint32_t) <= 200 * 1024) return IDKPT_OK;
+    const char* what = "BlasStackSize too large for the shared-memory traversal stack";
+    return who ? fail(ctx, who, IDKPT_ERR_UNSUPPORTED, what) : fail(ctx, IDKPT_ERR_UNSUPPORTED, what);
+}
+
 static int configure_launches(IdkPtCtx* ctx) {
     const int stackSize = std::max(1, ctx->sc.stackSize);
     ctx->stackBytes = (size_t)stackSize * IDK_BLOCK * sizeof(uint32_t);
-    if (ctx->stackBytes > 200 * 1024) return fail(ctx, IDKPT_ERR_UNSUPPORTED, "BlasStackSize too large for the shared-memory traversal stack");
+    if (int rc = check_stack_size(ctx, nullptr, stackSize)) return rc;
     CK(cudaFuncSetAttribute(k_trace_rays, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)ctx->stackBytes));
     CK(cudaFuncSetAttribute(k_trace_rays_any, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)ctx->stackBytes));
     CK(cudaFuncSetAttribute(k_shadows_ray_traced, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)ctx->stackBytes));
@@ -537,6 +569,16 @@ static int texture_error(IdkCtxBase* ctx, const char* who, const char* terr) {
     return fail(ctx, who, strstr(terr, "not supported") ? IDKPT_ERR_UNSUPPORTED : IDKPT_ERR_INVALID_ARGUMENT, terr);
 }
 
+// Every triangle's vertex ids below vertexCount, and with a mesh bound its MeshId in [0, meshCount).
+static bool triangles_valid(const GpuBlasTriangle* t, uint64_t count, uint64_t vertexCount, std::optional<uint64_t> meshCount = std::nullopt) {
+    for (uint64_t i = 0; i < count; i++) {
+        if ((uint64_t)(uint32_t)t[i].X >= vertexCount || (uint64_t)(uint32_t)t[i].Y >= vertexCount || (uint64_t)(uint32_t)t[i].Z >= vertexCount)
+            return false;
+        if (meshCount && (t[i].MeshId < 0 || (uint64_t)t[i].MeshId >= *meshCount)) return false;
+    }
+    return true;
+}
+
 // Checks idkpt_set_scene and idkvx_set_scene share: every index the kernels chase must be in range (a malformed host array
 // must become an error code, never a device fault).
 static int validate_scene(IdkCtxBase* ctx, const char* who, const IdkPtSceneDesc* s) {
@@ -553,12 +595,8 @@ static int validate_scene(IdkCtxBase* ctx, const char* who, const IdkPtSceneDesc
     }
     // triangle vertex ids must index the position / vertex arrays (checked on the host copy: cheap relative to the BVH build
     // that produced it)
-    const uint64_t lim = std::min(s->VertexPositionCount, s->VertexCount);
-    for (uint64_t i = 0; i < s->BlasTriangleCount; i++) {
-        const GpuBlasTriangle& t = s->BlasTriangles[i];
-        if ((uint64_t)(uint32_t)t.X >= lim || (uint64_t)(uint32_t)t.Y >= lim || (uint64_t)(uint32_t)t.Z >= lim || t.MeshId < 0 || (uint64_t)t.MeshId >= s->MeshCount)
-            return fail(ctx, who, IDKPT_ERR_INVALID_ARGUMENT, "GpuBlasTriangle index out of range");
-    }
+    if (!triangles_valid(s->BlasTriangles, s->BlasTriangleCount, std::min(s->VertexPositionCount, s->VertexCount), s->MeshCount))
+        return fail(ctx, who, IDKPT_ERR_INVALID_ARGUMENT, "GpuBlasTriangle index out of range");
     for (uint64_t i = 0; i < s->MeshCount; i++)
         if (s->Meshes[i].MaterialId < 0 || (uint64_t)s->Meshes[i].MaterialId >= s->MaterialCount) return fail(ctx, who, IDKPT_ERR_INVALID_ARGUMENT, "GpuMesh.MaterialId out of range");
     if (const char* terr = idk_validate_textures(s)) return texture_error(ctx, who, terr);
@@ -657,7 +695,7 @@ static int keep_prev_positions(IdkPtCtx* ctx) {
     if (ctx->prevPositions.p) return IDKPT_OK;
     const size_t bytes = ctx->counts.VertexPositionCount * sizeof(PackedVec3);
     CK(ensure(ctx->prevPositions, std::max<size_t>(bytes, 16)));
-    const cudaError_t e = bytes ? cudaMemcpyAsync(ctx->prevPositions.p, ctx->positions.p, bytes, cudaMemcpyDeviceToDevice, ctx->stream) : cudaSuccess;
+    const cudaError_t e = bytes ? cudaMemcpyAsync(ctx->prevPositions.p, ctx->scene.positions.p, bytes, cudaMemcpyDeviceToDevice, ctx->stream) : cudaSuccess;
     if (e != cudaSuccess) release(ctx->prevPositions);
     CK(e);
     return IDKPT_OK;
@@ -700,6 +738,101 @@ static int blas_build_params(IdkPtCtx* ctx, const char* who, const IdkPtBlasBuil
     if (s.StopSplittingThreshold < 1) return fail(ctx, who, IDKPT_ERR_INVALID_ARGUMENT, "StopSplittingThreshold must be at least 1");
     p = {s.StopSplittingThreshold, s.MaxLeafTriangleCount, s.TriangleCost, s.StackOptThreshold, s.StackOptSahIncreaseAcceptance,
          s.SplitFactor, s.DoPreSplit ? 1 : 0};
+    return IDKPT_OK;
+}
+
+// The scene view the kernels read (DeviceScene) from the context's arrays, counts, sky and texture table, and nothing else: every
+// call that changes one of them derives it again, and deriving it twice changes nothing.
+static void derive_view(IdkPtCtx* ctx) {
+    const SceneArrays& a = ctx->scene;
+    const IdkPtSceneDesc& c = ctx->counts;
+    DeviceScene& sc = ctx->sc;
+    sc.nodes = (const float4*)a.nodes.p;
+    sc.triRec = (const float4*)((char*)a.nodes.p + a.nodeBytes);
+    sc.blasTris = (const int4*)a.blasTris.p;
+    sc.descs = (const GpuBlasDesc*)a.descs.p;
+    sc.instances = (const GpuBlasInstance*)a.instances.p;
+    sc.xforms = (const float4*)a.xforms.p;
+    sc.meshes = (const GpuMesh*)a.meshes.p;
+    sc.materials = (const GpuMaterial*)a.materials.p;
+    sc.vertices = (const uint4*)a.vertices.p;
+    sc.lights = (const GpuLight*)a.lights.p;
+    sc.instanceCount = (uint32_t)c.BlasInstanceCount;
+    sc.lightCount = (uint32_t)c.LightCount;
+    sc.skyR = ctx->sky[0]; sc.skyG = ctx->sky[1]; sc.skyB = ctx->sky[2];
+    sc.skyFaces = ctx->skyFaceSize ? (const float4*)ctx->skyFaces.p : nullptr;
+    sc.skyFaceSize = ctx->skyFaceSize;
+    sc.stackSize = std::max(1, c.BlasStackSize);
+    sc.tlasNodes = (const float4*)a.tlas.p;
+    sc.useTlas = c.UseTlas ? 1 : 0;
+    sc.vtxFrame = (const float4*)a.vtxFrame.p;
+    sc.surfRec = (const float4*)a.surfRec.p;
+    sc.textures = (const TexRec*)ctx->tex.recs.p;
+    sc.textureCount = (uint32_t)c.TextureCount;
+    sc.srgbLut = (const float*)ctx->tex.srgbLut.p;
+}
+
+// Bytes of [nodes | triRec] the L2 window covers for `triangleCount` triangle records behind `nodeBytes` of nodes.
+static size_t bvh_bytes(size_t nodeBytes, uint64_t triangleCount) { return nodeBytes + std::max<size_t>(triangleCount, 1) * 64; }
+
+// Swaps `staged` into the scene (idkpt_blas_rebuild, idkpt_add_models): every array it holds replaces the scene's, whose
+// other arrays stay. The launch configuration and the L2 window for the new arrays come first and are both restored if either
+// fails, leaving the scene as it was. Then the counts, BLAS descs and view become the new scene's, and `staged` holds the
+// replaced arrays, which it frees.
+static int commit_scene(IdkPtCtx* ctx, SceneArrays& staged, const IdkPtSceneDesc& counts, std::vector<GpuBlasDesc>&& descs) {
+    const int oldStack = ctx->sc.stackSize;
+    ctx->sc.stackSize = std::max(1, counts.BlasStackSize);
+    int rc;
+    if ((rc = configure_launches(ctx)) || (rc = set_l2_window(ctx, staged.nodes.p, bvh_bytes(staged.nodeBytes, counts.BlasTriangleCount)))) {
+        const std::string err = ctx->lastError;
+        ctx->sc.stackSize = oldStack;
+        configure_launches(ctx);
+        set_l2_window(ctx, ctx->scene.nodes.p, bvh_bytes(ctx->scene.nodeBytes, ctx->counts.BlasTriangleCount));
+        ctx->lastError = err;
+        return rc;
+    }
+    const std::array<DevBuf*, 13> mine = ctx->scene.buffers(), theirs = staged.buffers();
+    for (size_t i = 0; i < mine.size(); i++)
+        if (theirs[i]->p) std::swap(*mine[i], *theirs[i]);
+    std::swap(ctx->scene.nodeBytes, staged.nodeBytes);
+    ctx->counts = counts;
+    ctx->hostDescs = std::move(descs);
+    derive_view(ctx);
+    ctx->sceneGeneration++;                              // a bound voxeliser re-sizes its work queue for the new draw list
+    ctx->accumulatedSamples = 0;
+    return IDKPT_OK;
+}
+
+// idkbb::build's status as the library's
+static int blas_build_fail(IdkPtCtx* ctx, const char* who, int rc, const std::string& err) {
+    if (rc == idkbb::BB_CUDA) cudaStreamSynchronize(ctx->stream);
+    return fail(ctx, who, rc == idkbb::BB_CUDA ? IDKPT_ERR_CUDA : IDKPT_ERR_UNSUPPORTED, err.c_str());
+}
+
+// The builder's input for each of `count` BLAS descs: its triangle range, pre-split unless it is refittable (BVH.cs:325).
+static std::vector<idkbb::Input> blas_inputs(const GpuBlasDesc* descs, size_t count) {
+    std::vector<idkbb::Input> in(count);
+    for (size_t k = 0; k < count; k++) in[k] = {descs[k].TriangleOffset, descs[k].TriangleCount, descs[k].IsRefittable ? 0 : 1};
+    return in;
+}
+
+// One batched idkbb::build_device over device triangles, enqueued on the context's stream, with its stage timer and fragment
+// print. On success descs[k] holds BLAS k's new NodeCount, TriangleCount and RequiredStackSize.
+static int build_blases(IdkPtCtx* ctx, const char* who, const PackedVec3* positions, const GpuBlasTriangle* tris, const std::vector<idkbb::Input>& in,
+                        const idkbvh::Params& p, idkbb::Arena& staged, idkbb::DeviceResult& built, GpuBlasDesc* descs) {
+    idkbb::StageTimer tm(ctx->stream);
+    tm.mark("start");
+    std::string err;
+    const int brc = idkbb::build_device(ctx->stream, positions, tris, in, p, staged, built, tm, err);
+    if (brc != idkbb::BB_OK) return blas_build_fail(ctx, who, brc, err);
+    long long fragments = 0;
+    for (int c : built.fragmentCount) fragments += c;
+    tm.print((int)in.size(), fragments);
+    for (size_t k = 0; k < in.size(); k++) {
+        descs[k].NodeCount = built.nodeStart[k + 1] - built.nodeStart[k];
+        descs[k].TriangleCount = built.triStart[k + 1] - built.triStart[k];
+        descs[k].RequiredStackSize = built.requiredStackSize[k];
+    }
     return IDKPT_OK;
 }
 
@@ -771,9 +904,8 @@ IDKPT_API void idkpt_destroy(IdkPtCtx* ctx) {
     cudaSetDevice(ctx->device);
     drain(ctx);
     unbind_voxelizers(ctx);
-    DevBuf* all[] = {&ctx->nodes, &ctx->triRec, &ctx->blasTris, &ctx->positions, &ctx->descs, &ctx->instances, &ctx->xforms,
-                     &ctx->meshes, &ctx->materials, &ctx->vertices, &ctx->lights, &ctx->tlas, &ctx->vtxFrame, &ctx->surfRec,
-                     &ctx->images[0], &ctx->images[1], &ctx->images[2], &ctx->counters, &ctx->countLog, &ctx->skyFaces,
+    release(ctx->scene);
+    DevBuf* all[] = {&ctx->images[0], &ctx->images[1], &ctx->images[2], &ctx->counters, &ctx->countLog, &ctx->skyFaces,
                      &ctx->bloomDown, &ctx->bloomUp, &ctx->postConsts, &ctx->ldr,
                      &ctx->unskinned, &ctx->joints, &ctx->refitParents, &ctx->refitLocks, &ctx->scratch[0], &ctx->scratch[1], &ctx->scratch[2],
                      &ctx->tlasScratch, &ctx->sahScratch, &ctx->oidn[0], &ctx->oidn[1], &ctx->oidn[2], &ctx->oidn[3], &ctx->denoiseWork[0], &ctx->denoiseWork[1], &ctx->denoised,
@@ -817,8 +949,7 @@ IDKPT_API int idkpt_set_scene(IdkPtCtx* ctx, const IdkPtSceneDesc* s) {
             return fail(ctx, IDKPT_ERR_INVALID_ARGUMENT, "idkpt_set_scene: BlasStackSize smaller than a BLAS's RequiredStackSize");
         if (const char* err = validate_blas(s->BlasNodes + d.NodeOffset, d, s->BlasStackSize)) return fail(ctx, IDKPT_ERR_INVALID_ARGUMENT, err);
     }
-    if ((size_t)std::max(1, s->BlasStackSize) * IDK_BLOCK * sizeof(uint32_t) > 200 * 1024)
-        return fail(ctx, IDKPT_ERR_UNSUPPORTED, "BlasStackSize too large for the shared-memory traversal stack");
+    if (int rc = check_stack_size(ctx, nullptr, s->BlasStackSize)) return rc;
 
     // Every host-side check has passed; from here on device arrays are overwritten / reallocated. Until the new scene is
     // complete the context has NO scene: a failure below (CUDA error, out of memory) must not leave the previous scene's
@@ -831,73 +962,48 @@ IDKPT_API int idkpt_set_scene(IdkPtCtx* ctx, const IdkPtSceneDesc* s) {
     release_raster(ctx->raster);   // the raster images belong to the old scene too
     release_anim(ctx->anim);       // and the animation set
     int rc;
-    // nodes and triangle records share one allocation ("bvh"): [nodes | triRec], so that one L2 access-policy window covers both
     const size_t nodeBytes = ((s->BlasNodeCount * sizeof(GpuBlasNode)) + 255) & ~(size_t)255;
-    const size_t triRecBytes = std::max<size_t>(s->BlasTriangleCount, 1) * 64;
-    CK(ensure(ctx->nodes, nodeBytes + triRecBytes));
-    CK(cudaMemcpyAsync(ctx->nodes.p, s->BlasNodes, s->BlasNodeCount * sizeof(GpuBlasNode), cudaMemcpyHostToDevice, ctx->stream));
-    if ((rc = upload(ctx, ctx->blasTris, s->BlasTriangles, s->BlasTriangleCount * sizeof(GpuBlasTriangle)))) return rc;
-    if ((rc = upload(ctx, ctx->positions, s->VertexPositions, s->VertexPositionCount * sizeof(PackedVec3)))) return rc;
-    if ((rc = upload(ctx, ctx->descs, s->BlasDescs, s->BlasDescCount * sizeof(GpuBlasDesc)))) return rc;
-    if ((rc = upload(ctx, ctx->instances, s->BlasInstances, s->BlasInstanceCount * sizeof(GpuBlasInstance)))) return rc;
-    if ((rc = upload(ctx, ctx->xforms, s->MeshTransforms, s->MeshTransformCount * sizeof(GpuMeshTransform)))) return rc;
-    if ((rc = upload(ctx, ctx->meshes, s->Meshes, s->MeshCount * sizeof(GpuMesh)))) return rc;
-    if ((rc = upload(ctx, ctx->materials, s->Materials, s->MaterialCount * sizeof(GpuMaterial)))) return rc;
-    if ((rc = upload(ctx, ctx->vertices, s->Vertices, s->VertexCount * sizeof(GpuVertex)))) return rc;
-    if ((rc = upload(ctx, ctx->lights, s->Lights, s->LightCount * sizeof(GpuLight)))) return rc;
-    if ((rc = upload(ctx, ctx->tlas, s->TlasNodes, s->UseTlas ? s->TlasNodeCount * sizeof(GpuTlasNode) : 0))) return rc;
+    CK(ensure(ctx->scene.nodes, bvh_bytes(nodeBytes, s->BlasTriangleCount)));
+    CK(cudaMemcpyAsync(ctx->scene.nodes.p, s->BlasNodes, s->BlasNodeCount * sizeof(GpuBlasNode), cudaMemcpyHostToDevice, ctx->stream));
+    if ((rc = upload(ctx, ctx->scene.blasTris, s->BlasTriangles, s->BlasTriangleCount * sizeof(GpuBlasTriangle)))) return rc;
+    if ((rc = upload(ctx, ctx->scene.positions, s->VertexPositions, s->VertexPositionCount * sizeof(PackedVec3)))) return rc;
+    if ((rc = upload(ctx, ctx->scene.descs, s->BlasDescs, s->BlasDescCount * sizeof(GpuBlasDesc)))) return rc;
+    if ((rc = upload(ctx, ctx->scene.instances, s->BlasInstances, s->BlasInstanceCount * sizeof(GpuBlasInstance)))) return rc;
+    if ((rc = upload(ctx, ctx->scene.xforms, s->MeshTransforms, s->MeshTransformCount * sizeof(GpuMeshTransform)))) return rc;
+    if ((rc = upload(ctx, ctx->scene.meshes, s->Meshes, s->MeshCount * sizeof(GpuMesh)))) return rc;
+    if ((rc = upload(ctx, ctx->scene.materials, s->Materials, s->MaterialCount * sizeof(GpuMaterial)))) return rc;
+    if ((rc = upload(ctx, ctx->scene.vertices, s->Vertices, s->VertexCount * sizeof(GpuVertex)))) return rc;
+    if ((rc = upload(ctx, ctx->scene.lights, s->Lights, s->LightCount * sizeof(GpuLight)))) return rc;
+    if ((rc = upload(ctx, ctx->scene.tlas, s->TlasNodes, s->UseTlas ? s->TlasNodeCount * sizeof(GpuTlasNode) : 0))) return rc;
     if ((rc = upload_textures(ctx, ctx->tex, s->Textures, s->TextureCount))) return rc;
     ctx->hostMaterialMaxHandle.assign(s->MaterialCount, 0);
     for (uint64_t i = 0; i < s->MaterialCount; i++) ctx->hostMaterialMaxHandle[i] = material_max_handle(s->Materials[i]);
 
-    CK(ensure(ctx->vtxFrame, std::max<size_t>(s->VertexCount, 1) * 32));
-    CK(ensure(ctx->surfRec, std::max<size_t>(s->MeshCount, 1) * 80));
+    CK(ensure(ctx->scene.vtxFrame, std::max<size_t>(s->VertexCount, 1) * 32));
+    CK(ensure(ctx->scene.surfRec, std::max<size_t>(s->MeshCount, 1) * 80));
     if (s->VertexCount) {
         const uint32_t nv = (uint32_t)s->VertexCount;
-        k_prepare_vertices<<<(nv + 255) / 256, 256, 0, ctx->stream>>>((const uint4*)ctx->vertices.p, (float4*)ctx->vtxFrame.p, nv);
+        k_prepare_vertices<<<(nv + 255) / 256, 256, 0, ctx->stream>>>((const uint4*)ctx->scene.vertices.p, (float4*)ctx->scene.vtxFrame.p, nv);
     }
     if (s->MeshCount) {
         const uint32_t nm = (uint32_t)s->MeshCount;
-        k_prepare_surfaces<<<(nm + 255) / 256, 256, 0, ctx->stream>>>((const GpuMesh*)ctx->meshes.p, (const GpuMaterial*)ctx->materials.p, (float4*)ctx->surfRec.p, nm);
+        k_prepare_surfaces<<<(nm + 255) / 256, 256, 0, ctx->stream>>>((const GpuMesh*)ctx->scene.meshes.p, (const GpuMaterial*)ctx->scene.materials.p, (float4*)ctx->scene.surfRec.p, nm);
     }
     CK(cudaGetLastError());
     if (s->BlasTriangleCount) {
         const uint32_t n = (uint32_t)s->BlasTriangleCount;
-        k_prepare_triangles<<<(n + 255) / 256, 256, 0, ctx->stream>>>((const int4*)ctx->blasTris.p, (const float*)ctx->positions.p, (float4*)((char*)ctx->nodes.p + nodeBytes), n);
+        k_prepare_triangles<<<(n + 255) / 256, 256, 0, ctx->stream>>>((const int4*)ctx->scene.blasTris.p, (const float*)ctx->scene.positions.p, (float4*)((char*)ctx->scene.nodes.p + nodeBytes), n);
         CK(cudaGetLastError());
     }
 
-    DeviceScene& sc = ctx->sc;
-    sc.nodes = (const float4*)ctx->nodes.p;
-    sc.triRec = (const float4*)((char*)ctx->nodes.p + nodeBytes);
-    sc.blasTris = (const int4*)ctx->blasTris.p;
-    sc.descs = (const GpuBlasDesc*)ctx->descs.p;
-    sc.instances = (const GpuBlasInstance*)ctx->instances.p;
-    sc.xforms = (const float4*)ctx->xforms.p;
-    sc.meshes = (const GpuMesh*)ctx->meshes.p;
-    sc.materials = (const GpuMaterial*)ctx->materials.p;
-    sc.vertices = (const uint4*)ctx->vertices.p;
-    sc.lights = (const GpuLight*)ctx->lights.p;
-    sc.instanceCount = (uint32_t)s->BlasInstanceCount;
-    sc.lightCount = (uint32_t)s->LightCount;
-    sc.skyR = ctx->sky[0]; sc.skyG = ctx->sky[1]; sc.skyB = ctx->sky[2];
-    sc.skyFaces = ctx->skyFaceSize ? (const float4*)ctx->skyFaces.p : nullptr;
-    sc.skyFaceSize = ctx->skyFaceSize;
-    sc.stackSize = std::max(1, s->BlasStackSize);
-    sc.tlasNodes = (const float4*)ctx->tlas.p;
-    sc.useTlas = s->UseTlas ? 1 : 0;
-    sc.vtxFrame = (const float4*)ctx->vtxFrame.p;
-    sc.surfRec = (const float4*)ctx->surfRec.p;
-    sc.textures = (const TexRec*)ctx->tex.recs.p;
-    sc.textureCount = (uint32_t)s->TextureCount;
-    sc.srgbLut = (const float*)ctx->tex.srgbLut.p;
     ctx->counts = *s;
     ctx->hostLights.assign(s->Lights, s->Lights + s->LightCount);
     ctx->hostDescs.assign(s->BlasDescs, s->BlasDescs + s->BlasDescCount);
     ctx->hostInstances.assign(s->BlasInstances, s->BlasInstances + s->BlasInstanceCount);
-    ctx->nodeBytes = nodeBytes;
+    ctx->scene.nodeBytes = nodeBytes;
+    derive_view(ctx);
     if ((rc = configure_launches(ctx))) return rc;
-    if ((rc = set_l2_window(ctx, ctx->nodes.p, nodeBytes + triRecBytes))) return rc;
+    if ((rc = set_l2_window(ctx, ctx->scene.nodes.p, bvh_bytes(nodeBytes, s->BlasTriangleCount)))) return rc;
     CK(cudaStreamSynchronize(ctx->stream));
     ctx->haveScene = true;
     ctx->accumulatedSamples = 0;
@@ -913,11 +1019,11 @@ IDKPT_API int idkpt_update_range(IdkPtCtx* ctx, IdkPtArrayId which, uint64_t fir
     size_t elem = 0;
     uint64_t limit = 0;
     switch (which) {
-        case IDKPT_ARRAY_MESH_TRANSFORMS: b = &ctx->xforms; elem = sizeof(GpuMeshTransform); limit = ctx->counts.MeshTransformCount; break;
-        case IDKPT_ARRAY_MESHES: b = &ctx->meshes; elem = sizeof(GpuMesh); limit = ctx->counts.MeshCount; break;
-        case IDKPT_ARRAY_MATERIALS: b = &ctx->materials; elem = sizeof(GpuMaterial); limit = ctx->counts.MaterialCount; break;
-        case IDKPT_ARRAY_LIGHTS: b = &ctx->lights; elem = sizeof(GpuLight); limit = ctx->counts.LightCount; break;
-        case IDKPT_ARRAY_TLAS_NODES: b = &ctx->tlas; elem = sizeof(GpuTlasNode); limit = ctx->counts.UseTlas ? ctx->counts.TlasNodeCount : 0; break;
+        case IDKPT_ARRAY_MESH_TRANSFORMS: b = &ctx->scene.xforms; elem = sizeof(GpuMeshTransform); limit = ctx->counts.MeshTransformCount; break;
+        case IDKPT_ARRAY_MESHES: b = &ctx->scene.meshes; elem = sizeof(GpuMesh); limit = ctx->counts.MeshCount; break;
+        case IDKPT_ARRAY_MATERIALS: b = &ctx->scene.materials; elem = sizeof(GpuMaterial); limit = ctx->counts.MaterialCount; break;
+        case IDKPT_ARRAY_LIGHTS: b = &ctx->scene.lights; elem = sizeof(GpuLight); limit = ctx->counts.LightCount; break;
+        case IDKPT_ARRAY_TLAS_NODES: b = &ctx->scene.tlas; elem = sizeof(GpuTlasNode); limit = ctx->counts.UseTlas ? ctx->counts.TlasNodeCount : 0; break;
         default: return fail(ctx, IDKPT_ERR_INVALID_ARGUMENT, "idkpt_update_range: unknown array id");
     }
     if (first > limit || count > limit - first) return fail(ctx, IDKPT_ERR_INVALID_ARGUMENT, "idkpt_update_range: range outside the array");
@@ -945,7 +1051,7 @@ IDKPT_API int idkpt_update_range(IdkPtCtx* ctx, IdkPtArrayId which, uint64_t fir
     if (which == IDKPT_ARRAY_LIGHTS) std::copy((const GpuLight*)data, (const GpuLight*)data + count, ctx->hostLights.begin() + first);
     if ((which == IDKPT_ARRAY_MESHES || which == IDKPT_ARRAY_MATERIALS) && ctx->counts.MeshCount) {
         const uint32_t nm = (uint32_t)ctx->counts.MeshCount;   // refresh the per-mesh surface records
-        k_prepare_surfaces<<<(nm + 255) / 256, 256, 0, ctx->stream>>>((const GpuMesh*)ctx->meshes.p, (const GpuMaterial*)ctx->materials.p, (float4*)ctx->surfRec.p, nm);
+        k_prepare_surfaces<<<(nm + 255) / 256, 256, 0, ctx->stream>>>((const GpuMesh*)ctx->scene.meshes.p, (const GpuMaterial*)ctx->scene.materials.p, (float4*)ctx->scene.surfRec.p, nm);
         CK(cudaGetLastError());
     }
     CK(cudaStreamSynchronize(ctx->stream));
@@ -967,9 +1073,7 @@ IDKPT_API int idkpt_set_sky(IdkPtCtx* ctx, const IdkPtSkyDesc* sky) {
     }
     ctx->skyFaceSize = sky->FaceSize;
     for (int i = 0; i < 3; i++) ctx->sky[i] = sky->Color[i];
-    ctx->sc.skyR = ctx->sky[0]; ctx->sc.skyG = ctx->sky[1]; ctx->sc.skyB = ctx->sky[2];
-    ctx->sc.skyFaces = ctx->skyFaceSize ? (const float4*)ctx->skyFaces.p : nullptr;
-    ctx->sc.skyFaceSize = ctx->skyFaceSize;
+    derive_view(ctx);
     ctx->accumulatedSamples = 0;
     return IDKPT_OK;
 }
@@ -993,8 +1097,7 @@ static int sky_generate(IdkPtCtx* ctx, const char* who, int n, float* kernelMs, 
     if (rc != IDKPT_OK) { release(fresh); return rc; }
     if (fresh.p) { release(ctx->skyFaces); ctx->skyFaces = fresh; }
     ctx->skyFaceSize = n;
-    ctx->sc.skyFaces = (const float4*)ctx->skyFaces.p;
-    ctx->sc.skyFaceSize = n;
+    derive_view(ctx);
     ctx->accumulatedSamples = 0;
     return IDKPT_OK;
 }
@@ -1077,10 +1180,8 @@ IDKPT_API int idkpt_set_textures(IdkPtCtx* ctx, const IdkPtTextureDesc* textures
     CK(cudaStreamSynchronize(ctx->stream));
     int rc = upload_textures(ctx, ctx->tex, textures, count);
     if (rc) return rc;
-    ctx->sc.textures = (const TexRec*)ctx->tex.recs.p;
-    ctx->sc.textureCount = (uint32_t)count;
-    ctx->sc.srgbLut = (const float*)ctx->tex.srgbLut.p;
     ctx->counts.TextureCount = count;
+    derive_view(ctx);
     ctx->accumulatedSamples = 0;
     return IDKPT_OK;
 }
@@ -1970,10 +2071,10 @@ static int enqueue_skin(IdkPtCtx* ctx, const void* joints, const IdkPtSkinningCm
         // Skinning/compute.glsl:42, prevVertexPositionSSBO = vertexPositionSSBO over the command's output range, dispatch by
         // dispatch: with overlapping commands the kept positions are those the previous command left, as in the engine
         const size_t off = (size_t)cmds[c].OutputVertexOffset * sizeof(PackedVec3), n = (size_t)cmds[c].VertexCount * sizeof(PackedVec3);
-        CK(cudaMemcpyAsync((char*)ctx->prevPositions.p + off, (const char*)ctx->positions.p + off, n, cudaMemcpyDeviceToDevice, ctx->stream));
+        CK(cudaMemcpyAsync((char*)ctx->prevPositions.p + off, (const char*)ctx->scene.positions.p + off, n, cudaMemcpyDeviceToDevice, ctx->stream));
         SkinArgs a;
         a.unskinned = (const uint32_t*)ctx->unskinned.p; a.joints = (const float4*)joints;
-        a.positions = (float*)ctx->positions.p; a.vertices = (uint4*)ctx->vertices.p; a.vtxFrame = (float4*)ctx->vtxFrame.p;
+        a.positions = (float*)ctx->scene.positions.p; a.vertices = (uint4*)ctx->scene.vertices.p; a.vtxFrame = (float4*)ctx->scene.vtxFrame.p;
         a.inOffset = cmds[c].InputVertexOffset; a.outOffset = cmds[c].OutputVertexOffset; a.jointOffset = cmds[c].JointMatricesOffset; a.count = cmds[c].VertexCount;
         k_skin_vertices<<<(a.count + 255) / 256, 256, 0, ctx->stream>>>(a);
     }
@@ -2004,9 +2105,9 @@ static int enqueue_refit(IdkPtCtx* ctx, uint32_t first, uint32_t count) {
     for (uint32_t b = first; b < first + count; b++) {
         const GpuBlasDesc& d = ctx->hostDescs[b];
         RefitArgs a;
-        a.nodes = (float4*)ctx->nodes.p + 2 * (size_t)d.NodeOffset;
-        a.blasTris = (const int4*)ctx->blasTris.p; a.positions = (const float*)ctx->positions.p;
-        a.triRec = (float4*)((char*)ctx->nodes.p + ctx->nodeBytes);
+        a.nodes = (float4*)ctx->scene.nodes.p + 2 * (size_t)d.NodeOffset;
+        a.blasTris = (const int4*)ctx->scene.blasTris.p; a.positions = (const float*)ctx->scene.positions.p;
+        a.triRec = (float4*)((char*)ctx->scene.nodes.p + ctx->scene.nodeBytes);
         a.parents = (int32_t*)ctx->refitParents.p; a.locks = (uint32_t*)ctx->refitLocks.p;
         a.nodeCount = (uint32_t)d.NodeCount; a.triOffset = (uint32_t)d.TriangleOffset; a.triCount = (uint32_t)d.TriangleCount;
         k_refit_prepare<<<(a.nodeCount + 255) / 256, 256, 0, ctx->stream>>>(a);
@@ -2086,6 +2187,22 @@ static int enqueue_tlas_build(IdkPtCtx* ctx, const void* blasNodes, const void* 
     return IDKPT_OK;
 }
 
+// Reads enqueue_tlas_build's status word once the stream has finished and refuses a tree the walk cannot use. `inPlace`: the
+// build wrote the scene's own TLAS (idkpt_tlas_build, idkpt_update_models), so a refusal leaves the scene invalidated;
+// otherwise (idkpt_add_models) it wrote staging memory and a refusal changes nothing.
+static int check_tlas_built(IdkPtCtx* ctx, const char* who, const int* needDev, bool inPlace) {
+    int need = 0;
+    CK(cudaMemcpy(&need, needDev, 4, cudaMemcpyDeviceToHost));
+    if (need >= 0 && need <= IDK_TLAS_STACK_SIZE) return IDKPT_OK;
+    if (inPlace) ctx->haveScene = false;
+    if (need < 0)                         // the PLOC loop merged nothing: the node array is not a tree
+        return fail(ctx, who, IDKPT_ERR_INVALID_ARGUMENT, inPlace ? "an instance's world box is not finite or its half area overflows (ModelMatrix or BLAS root); scene invalidated; set it again"
+                                                                  : "an instance's world box is not finite or its half area overflows (ModelMatrix or BLAS root)");
+    // the walk's stack is fixed (BVHIntersect.glsl:4): refuse to trace through a TLAS it cannot hold
+    return fail(ctx, who, IDKPT_ERR_UNSUPPORTED, inPlace ? "the built TLAS is deeper than the 24-entry traversal stack of the TLAS walk (scene invalidated; set it again)"
+                                                         : "the TLAS is deeper than the 24-entry traversal stack of the TLAS walk (BVHIntersect.glsl:4)");
+}
+
 // BVH.TlasBuild on the device (BVH.cs:278-298, TLAS.cs:28-141): see k_tlas_ploc. Shared by idkpt_tlas_build and
 // idkpt_update_models, whose refusals are the same.
 // `pre` enqueues work that must come before the build (idkpt_update_models' skin and refit) inside the same timed, synchronised
@@ -2100,21 +2217,11 @@ static int tlas_build_scene(IdkPtCtx* ctx, const char* who, int32_t searchRadius
     const int rc = run_timed(ctx, who, kernelMs, [&]() -> int {
         if (pre)
             if (int r = pre()) return r;
-        return enqueue_tlas_build(ctx, ctx->nodes.p, ctx->descs.p, ctx->instances.p, ctx->xforms.p, ctx->tlas.p, n, searchRadius, &needDev);
+        return enqueue_tlas_build(ctx, ctx->scene.nodes.p, ctx->scene.descs.p, ctx->scene.instances.p, ctx->scene.xforms.p, ctx->scene.tlas.p, n, searchRadius, &needDev);
     });
     if (rc) return rc;
     ctx->accumulatedSamples = 0;
-    int need = 0;
-    CK(cudaMemcpy(&need, needDev, 4, cudaMemcpyDeviceToHost));
-    if (need < 0) {                       // the PLOC loop merged nothing: the node array is not a tree
-        ctx->haveScene = false;
-        return fail(ctx, who, IDKPT_ERR_INVALID_ARGUMENT, "an instance's world box is not finite or its half area overflows (ModelMatrix or BLAS root); scene invalidated; set it again");
-    }
-    if (need > IDK_TLAS_STACK_SIZE) {     // the walk's stack is fixed (BVHIntersect.glsl:4): refuse to trace through a TLAS it cannot hold
-        ctx->haveScene = false;
-        return fail(ctx, who, IDKPT_ERR_UNSUPPORTED, "the built TLAS is deeper than the 24-entry traversal stack of the TLAS walk (scene invalidated; set it again)");
-    }
-    return IDKPT_OK;
+    return check_tlas_built(ctx, who, needDev, true);
 }
 
 IDKPT_API int idkpt_tlas_build(IdkPtCtx* ctx, int32_t searchRadius, float* kernelMs) {
@@ -2125,10 +2232,24 @@ IDKPT_API int idkpt_tlas_build(IdkPtCtx* ctx, int32_t searchRadius, float* kerne
     return tlas_build_scene(ctx, "idkpt_tlas_build", searchRadius, kernelMs);
 }
 
-// idkbb::build's status as the library's
-static int blas_build_fail(IdkPtCtx* ctx, const char* who, int rc, const std::string& err) {
-    if (rc == idkbb::BB_CUDA) cudaStreamSynchronize(ctx->stream);
-    return fail(ctx, who, rc == idkbb::BB_CUDA ? IDKPT_ERR_CUDA : IDKPT_ERR_UNSUPPORTED, err.c_str());
+// The build of checked host inputs into a new handle: what idkpt_blas_build and idkpt_blas_build_batch share after their
+// argument checks.
+static int blas_build_host(IdkPtCtx* ctx, const char* who, const PackedVec3* positions, uint64_t vertexCount, const GpuBlasTriangle* triangles,
+                           uint64_t triangleCount, const std::vector<idkbb::Input>& in, const std::vector<GpuBlasDesc>& descs,
+                           const idkbvh::Params& p, IdkPtBlasBuild** out, float* kernelMs) {
+    DRAIN_PENDING(who);
+    CK(cudaSetDevice(ctx->device));
+    IdkPtBlasBuild* b = new IdkPtBlasBuild();
+    std::string err;
+    float ms = 0.0f;
+    const int rc = idkbb::build(ctx->stream, positions, vertexCount, triangles, triangleCount, in, descs, p, *b, ms, err);
+    if (rc != idkbb::BB_OK) {
+        delete b;
+        return blas_build_fail(ctx, who, rc, err);
+    }
+    *out = b;
+    if (kernelMs) *kernelMs = ms;
+    return IDKPT_OK;
 }
 
 // BLAS.Build + PreSplitting.PreSplit on the device (BVH.BlasesBuild's loop body, BVH.cs:315-377): a batch of one, see
@@ -2144,25 +2265,9 @@ IDKPT_API int idkpt_blas_build(IdkPtCtx* ctx, const PackedVec3* positions, uint6
     if (int rc = blas_build_params(ctx, "idkpt_blas_build", settings, p)) return rc;
     if (triangleCount > (uint64_t)idkbb::MAX_FRAGMENTS)
         return fail(ctx, IDKPT_ERR_UNSUPPORTED, "idkpt_blas_build: more than 2^24 triangles");
-    for (uint64_t i = 0; i < triangleCount; i++) {
-        const GpuBlasTriangle& t = triangles[i];
-        if ((uint64_t)(uint32_t)t.X >= vertexCount || (uint64_t)(uint32_t)t.Y >= vertexCount || (uint64_t)(uint32_t)t.Z >= vertexCount)
-            return fail(ctx, IDKPT_ERR_INVALID_ARGUMENT, "idkpt_blas_build: vertex id out of range");
-    }
-    DRAIN_PENDING("idkpt_blas_build");
-    CK(cudaSetDevice(ctx->device));
-    IdkPtBlasBuild* b = new IdkPtBlasBuild();
-    std::string err;
-    float ms = 0.0f;
-    const std::vector<idkbb::Input> in = {{0, (int)triangleCount, p.doPreSplit}};
-    const int rc = idkbb::build(ctx->stream, positions, vertexCount, triangles, triangleCount, in, std::vector<GpuBlasDesc>(1), p, *b, ms, err);
-    if (rc != idkbb::BB_OK) {
-        delete b;
-        return blas_build_fail(ctx, "idkpt_blas_build", rc, err);
-    }
-    *out = b;
-    if (kernelMs) *kernelMs = ms;
-    return IDKPT_OK;
+    if (!triangles_valid(triangles, triangleCount, vertexCount)) return fail(ctx, IDKPT_ERR_INVALID_ARGUMENT, "idkpt_blas_build: vertex id out of range");
+    return blas_build_host(ctx, "idkpt_blas_build", positions, vertexCount, triangles, triangleCount, {{0, (int)triangleCount, p.doPreSplit}},
+                           std::vector<GpuBlasDesc>(1), p, out, kernelMs);
 }
 
 // BVH.BlasesBuild's parallel loop (BVH.cs:315-377) as one batch: see idk_blas_build.cuh.
@@ -2177,7 +2282,6 @@ IDKPT_API int idkpt_blas_build_batch(IdkPtCtx* ctx, const PackedVec3* positions,
     if (descCount == 0) return fail(ctx, who, IDKPT_ERR_INVALID_ARGUMENT, "no BLASes");
     idkbvh::Params p;
     if (int rc = blas_build_params(ctx, who, settings, p)) return rc;
-    std::vector<idkbb::Input> in(descCount);
     std::vector<int> counts(descCount);
     for (uint32_t s = 0; s < descCount; s++) {
         const GpuBlasDesc& d = descs[s];
@@ -2185,31 +2289,14 @@ IDKPT_API int idkpt_blas_build_batch(IdkPtCtx* ctx, const PackedVec3* positions,
         if (d.TriangleOffset < 0 || (uint64_t)d.TriangleOffset + (uint64_t)d.TriangleCount > triangleCount)
             return fail(ctx, who, IDKPT_ERR_INVALID_ARGUMENT, "GpuBlasDesc triangle range outside the array");
         if (d.TriangleCount > idkbb::MAX_FRAGMENTS) return fail(ctx, who, IDKPT_ERR_UNSUPPORTED, "a BLAS of more than 2^24 triangles");
-        in[s] = {d.TriangleOffset, d.TriangleCount, d.IsRefittable ? 0 : 1};   // BVH.cs:325
         counts[s] = d.TriangleCount;
     }
     if (idkbb::nodeIdCount(counts, descCount) < 0) return fail(ctx, who, IDKPT_ERR_UNSUPPORTED, "the batch needs 2^31 or more node ids");
-    for (uint32_t s = 0; s < descCount; s++) {
-        for (int i = 0; i < descs[s].TriangleCount; i++) {
-            const GpuBlasTriangle& t = triangles[(size_t)descs[s].TriangleOffset + i];
-            if ((uint64_t)(uint32_t)t.X >= vertexCount || (uint64_t)(uint32_t)t.Y >= vertexCount || (uint64_t)(uint32_t)t.Z >= vertexCount)
-                return fail(ctx, who, IDKPT_ERR_INVALID_ARGUMENT, "vertex id out of range");
-        }
-    }
-    DRAIN_PENDING("idkpt_blas_build_batch");
-    CK(cudaSetDevice(ctx->device));
-    IdkPtBlasBuild* b = new IdkPtBlasBuild();
-    std::string err;
-    float ms = 0.0f;
-    const int rc = idkbb::build(ctx->stream, positions, vertexCount, triangles, triangleCount, in,
-                                std::vector<GpuBlasDesc>(descs, descs + descCount), p, *b, ms, err);
-    if (rc != idkbb::BB_OK) {
-        delete b;
-        return blas_build_fail(ctx, who, rc, err);
-    }
-    *out = b;
-    if (kernelMs) *kernelMs = ms;
-    return IDKPT_OK;
+    for (uint32_t s = 0; s < descCount; s++)
+        if (!triangles_valid(triangles + descs[s].TriangleOffset, (uint64_t)descs[s].TriangleCount, vertexCount))
+            return fail(ctx, who, IDKPT_ERR_INVALID_ARGUMENT, "vertex id out of range");
+    return blas_build_host(ctx, who, positions, vertexCount, triangles, triangleCount, blas_inputs(descs, descCount),
+                           std::vector<GpuBlasDesc>(descs, descs + descCount), p, out, kernelMs);
 }
 
 // Totals over the batch: the largest RequiredStackSize (BVH.UpdateBlasStackSize) and the SAHs added in BLAS order.
@@ -2280,37 +2367,20 @@ IDKPT_API int idkpt_blas_rebuild(IdkPtCtx* ctx, uint32_t first, uint32_t count, 
     }
     if (nodes_end(old[nd - 1]) != (int64_t)ctx->counts.BlasNodeCount || triangles_end(old[nd - 1]) != (int64_t)ctx->counts.BlasTriangleCount)
         return fail(ctx, IDKPT_ERR_INVALID_ARGUMENT, "idkpt_blas_rebuild: the last BLAS does not end the node and triangle arrays");
-    std::vector<idkbb::Input> in(count);
-    for (uint32_t k = 0; k < count; k++) {
-        const GpuBlasDesc& d = old[first + k];
-        if (d.TriangleCount > idkbb::MAX_FRAGMENTS) return fail(ctx, IDKPT_ERR_UNSUPPORTED, "idkpt_blas_rebuild: a BLAS of more than 2^24 triangles");
-        in[k] = {d.TriangleOffset, d.TriangleCount, d.IsRefittable ? 0 : 1};   // BVH.cs:325
-    }
+    for (uint32_t k = 0; k < count; k++)
+        if (old[first + k].TriangleCount > idkbb::MAX_FRAGMENTS) return fail(ctx, IDKPT_ERR_UNSUPPORTED, "idkpt_blas_rebuild: a BLAS of more than 2^24 triangles");
+    const std::vector<idkbb::Input> in = blas_inputs(old.data() + first, count);
     CK(cudaSetDevice(ctx->device));
 
     std::vector<GpuBlasDesc> descs = old;
     idkbb::Arena staged;                                  // the rebuilt BLASes, until they are committed
     idkbb::DeviceResult built;
-    DevBuf bvh, tris, descBuf;                            // the new [nodes | triRec], triangles and descs
-    struct Drop { DevBuf* b[3]; ~Drop() { for (DevBuf* x : b) release(*x); } } drop = {{&bvh, &tris, &descBuf}};
-    size_t nodeBytes = 0, triRecBytes = 0;
-    int stackSize = 0;
+    SceneArrays next;                                     // the new [nodes | triRec], triangles and descs
+    IdkPtSceneDesc counts = ctx->counts;
     int rc = run_timed(ctx, "idkpt_blas_rebuild", kernelMs, [&]() -> int {
-        idkbb::StageTimer tm(ctx->stream);
-        tm.mark("start");
-        std::string err;
-        const int brc = idkbb::build_device(ctx->stream, (const PackedVec3*)ctx->positions.p, (const GpuBlasTriangle*)ctx->blasTris.p,
-                                            in, p, staged, built, tm, err);
-        if (brc != idkbb::BB_OK) return blas_build_fail(ctx, "idkpt_blas_rebuild", brc, err);
-        long long fragments = 0;
-        for (int c : built.fragmentCount) fragments += c;
-        tm.print((int)count, fragments);
-        for (uint32_t k = 0; k < count; k++) {
-            GpuBlasDesc& d = descs[first + k];
-            d.NodeCount = built.nodeStart[k + 1] - built.nodeStart[k];
-            d.TriangleCount = built.triStart[k + 1] - built.triStart[k];
-            d.RequiredStackSize = built.requiredStackSize[k];
-        }
+        if (int brc = build_blases(ctx, "idkpt_blas_rebuild", (const PackedVec3*)ctx->scene.positions.p, (const GpuBlasTriangle*)ctx->scene.blasTris.p,
+                                   in, p, staged, built, descs.data() + first))
+            return brc;
         int64_t nodeEnd = 0, triEnd = 0;
         for (size_t i = first; i < nd; i++) {
             const int64_t no = i ? nodes_end(descs[i - 1]) : 0, to = i ? triangles_end(descs[i - 1]) : 0;
@@ -2320,25 +2390,27 @@ IDKPT_API int idkpt_blas_rebuild(IdkPtCtx* ctx, uint32_t first, uint32_t count, 
             descs[i].NodeOffset = (int32_t)no;
             descs[i].TriangleOffset = (int32_t)to;
         }
-        for (const GpuBlasDesc& d : descs) stackSize = std::max(stackSize, d.RequiredStackSize);   // BVH.UpdateBlasStackSize
-        if ((size_t)std::max(1, stackSize) * IDK_BLOCK * sizeof(uint32_t) > 200 * 1024)
-            return fail(ctx, IDKPT_ERR_UNSUPPORTED, "idkpt_blas_rebuild: BlasStackSize too large for the shared-memory traversal stack");
+        counts.BlasStackSize = 0;
+        for (const GpuBlasDesc& d : descs) counts.BlasStackSize = std::max(counts.BlasStackSize, d.RequiredStackSize);   // BVH.UpdateBlasStackSize
+        if (int r = check_stack_size(ctx, "idkpt_blas_rebuild", counts.BlasStackSize)) return r;
+        counts.BlasNodeCount = (uint64_t)nodeEnd;
+        counts.BlasTriangleCount = (uint64_t)triEnd;
 
         // the new arrays: the kept prefix, the rebuilt BLASes, the moved tail
         const GpuBlasDesc &r0 = descs[first], &rl = descs[first + count - 1];
         const int64_t oldEndN = nodes_end(old[first + count - 1]), oldEndT = triangles_end(old[first + count - 1]);
         const int64_t tailN = (int64_t)ctx->counts.BlasNodeCount - oldEndN, tailT = (int64_t)ctx->counts.BlasTriangleCount - oldEndT;
-        nodeBytes = (((size_t)nodeEnd * sizeof(GpuBlasNode)) + 255) & ~(size_t)255;
-        triRecBytes = std::max<size_t>((size_t)triEnd, 1) * 64;
-        if (ensure(bvh, nodeBytes + triRecBytes) != cudaSuccess || ensure(tris, std::max<size_t>((size_t)triEnd * sizeof(GpuBlasTriangle), 16)) != cudaSuccess ||
-            ensure(descBuf, std::max<size_t>(nd * sizeof(GpuBlasDesc), 16)) != cudaSuccess)
+        next.nodeBytes = (((size_t)nodeEnd * sizeof(GpuBlasNode)) + 255) & ~(size_t)255;
+        if (ensure(next.nodes, bvh_bytes(next.nodeBytes, (size_t)triEnd)) != cudaSuccess ||
+            ensure(next.blasTris, std::max<size_t>((size_t)triEnd * sizeof(GpuBlasTriangle), 16)) != cudaSuccess ||
+            ensure(next.descs, std::max<size_t>(nd * sizeof(GpuBlasDesc), 16)) != cudaSuccess)
             return fail(ctx, IDKPT_ERR_OUT_OF_MEMORY, "idkpt_blas_rebuild: device allocation failed");
-        GpuBlasNode* nodesNew = (GpuBlasNode*)bvh.p;
-        const GpuBlasNode* nodesOld = (const GpuBlasNode*)ctx->nodes.p;
-        float4* recNew = (float4*)((char*)bvh.p + nodeBytes);
-        const float4* recOld = (const float4*)((const char*)ctx->nodes.p + ctx->nodeBytes);
-        GpuBlasTriangle* trisNew = (GpuBlasTriangle*)tris.p;
-        const GpuBlasTriangle* trisOld = (const GpuBlasTriangle*)ctx->blasTris.p;
+        GpuBlasNode* nodesNew = (GpuBlasNode*)next.nodes.p;
+        const GpuBlasNode* nodesOld = (const GpuBlasNode*)ctx->scene.nodes.p;
+        float4* recNew = (float4*)((char*)next.nodes.p + next.nodeBytes);
+        const float4* recOld = (const float4*)((const char*)ctx->scene.nodes.p + ctx->scene.nodeBytes);
+        GpuBlasTriangle* trisNew = (GpuBlasTriangle*)next.blasTris.p;
+        const GpuBlasTriangle* trisOld = (const GpuBlasTriangle*)ctx->scene.blasTris.p;
         auto d2d = [&](void* dst, const void* src, size_t bytes) { return bytes ? cudaMemcpyAsync(dst, src, bytes, cudaMemcpyDeviceToDevice, ctx->stream) : cudaSuccess; };
         CK(d2d(nodesNew, nodesOld, (size_t)keepNodes * sizeof(GpuBlasNode)));
         CK(d2d(trisNew, trisOld, (size_t)keepTris * sizeof(GpuBlasTriangle)));
@@ -2349,39 +2421,13 @@ IDKPT_API int idkpt_blas_rebuild(IdkPtCtx* ctx, uint32_t first, uint32_t count, 
         CK(d2d(trisNew + triangles_end(rl), trisOld + oldEndT, (size_t)tailT * sizeof(GpuBlasTriangle)));
         CK(d2d(recNew + 4 * triangles_end(rl), recOld + 4 * oldEndT, (size_t)tailT * 64));
         if (const uint32_t n = (uint32_t)(triangles_end(rl) - r0.TriangleOffset))   // the rebuilt BLASes' triangle records
-            k_prepare_triangles<<<(n + 255) / 256, 256, 0, ctx->stream>>>((const int4*)(trisNew + r0.TriangleOffset), (const float*)ctx->positions.p,
+            k_prepare_triangles<<<(n + 255) / 256, 256, 0, ctx->stream>>>((const int4*)(trisNew + r0.TriangleOffset), (const float*)ctx->scene.positions.p,
                                                                           recNew + 4 * (size_t)r0.TriangleOffset, n);
-        CK(cudaMemcpyAsync(descBuf.p, descs.data(), nd * sizeof(GpuBlasDesc), cudaMemcpyHostToDevice, ctx->stream));
+        CK(cudaMemcpyAsync(next.descs.p, descs.data(), nd * sizeof(GpuBlasDesc), cudaMemcpyHostToDevice, ctx->stream));
         return IDKPT_OK;
     });
     if (rc) return rc;
-
-    // commit: launch configuration and L2 window for the new arrays first (restored if either fails), then the swap
-    const int oldStack = ctx->sc.stackSize;
-    ctx->sc.stackSize = std::max(1, stackSize);
-    if ((rc = configure_launches(ctx)) || (rc = set_l2_window(ctx, bvh.p, nodeBytes + triRecBytes))) {
-        const std::string err = ctx->lastError;
-        ctx->sc.stackSize = oldStack;
-        configure_launches(ctx);
-        set_l2_window(ctx, ctx->nodes.p, ctx->nodeBytes + std::max<size_t>(ctx->counts.BlasTriangleCount, 1) * 64);
-        ctx->lastError = err;
-        return rc;
-    }
-    std::swap(ctx->nodes, bvh);
-    std::swap(ctx->blasTris, tris);
-    std::swap(ctx->descs, descBuf);                      // `drop` frees the old arrays
-    ctx->nodeBytes = nodeBytes;
-    ctx->sc.nodes = (const float4*)ctx->nodes.p;
-    ctx->sc.triRec = (const float4*)((char*)ctx->nodes.p + nodeBytes);
-    ctx->sc.blasTris = (const int4*)ctx->blasTris.p;
-    ctx->sc.descs = (const GpuBlasDesc*)ctx->descs.p;
-    ctx->counts.BlasNodeCount = (uint64_t)nodes_end(descs[nd - 1]);
-    ctx->counts.BlasTriangleCount = (uint64_t)triangles_end(descs[nd - 1]);
-    ctx->counts.BlasStackSize = stackSize;
-    ctx->hostDescs = std::move(descs);
-    ctx->sceneGeneration++;                              // a bound voxeliser re-sizes its work queue for the new triangle counts
-    ctx->accumulatedSamples = 0;
-    return IDKPT_OK;
+    return commit_scene(ctx, next, counts, std::move(descs));
 }
 
 // validate_scene's checks for idkpt_add_models's own arrays, every id local to them: O(model), never O(scene).
@@ -2409,12 +2455,8 @@ static int validate_add_models(IdkPtCtx* ctx, const char* who, const IdkPtAddMod
             return invalid("GpuBlasDesc triangle range outside the call's triangles");
         if (d.TriangleCount > idkbb::MAX_FRAGMENTS) return fail(ctx, who, IDKPT_ERR_UNSUPPORTED, "a BLAS of more than 2^24 triangles");
     }
-    for (uint64_t i = 0; i < m->TriangleCount; i++) {
-        const GpuBlasTriangle& t = m->Triangles[i];
-        if ((uint64_t)(uint32_t)t.X >= m->VertexCount || (uint64_t)(uint32_t)t.Y >= m->VertexCount || (uint64_t)(uint32_t)t.Z >= m->VertexCount ||
-            t.MeshId < 0 || (uint64_t)t.MeshId >= m->MeshCount)
-            return invalid("GpuBlasTriangle index outside the call's vertices or meshes");
-    }
+    if (!triangles_valid(m->Triangles, m->TriangleCount, m->VertexCount, m->MeshCount))
+        return invalid("GpuBlasTriangle index outside the call's vertices or meshes");
     for (uint64_t i = 0; i < m->MeshCount; i++)
         if (m->Meshes[i].MaterialId < 0 || (uint64_t)m->Meshes[i].MaterialId >= m->MaterialCount)
             return invalid("GpuMesh.MaterialId outside the call's materials");
@@ -2451,24 +2493,19 @@ IDKPT_API int idkpt_add_models(IdkPtCtx* ctx, const IdkPtAddModelsDesc* m, const
     const uint64_t nI = old.BlasInstanceCount + m->BlasInstanceCount, nB = old.BlasDescCount + m->BlasDescCount;
     const uint64_t nTex = old.TextureCount + m->TextureCount, nU = ctx->unskinnedCount + m->UnskinnedVertexCount;
     const uint32_t B = (uint32_t)m->BlasDescCount;
-    std::vector<idkbb::Input> in(B);
-    for (uint32_t k = 0; k < B; k++) {
-        const GpuBlasDesc& d = m->BlasDescs[k];
-        in[k] = {d.TriangleOffset, d.TriangleCount, d.IsRefittable ? 0 : 1};   // BVH.cs:325
-    }
+    const std::vector<idkbb::Input> in = blas_inputs(m->BlasDescs, B);
 
-    // the grown arrays ([nodes | triRec] in `bvh`), the new texture pool and records, and the staged records with ids
-    DevBuf positions, vertices, xforms, meshes, materials, instances, vtxFrame, surfRec, descBuf, tris, bvh, tlas, recs, pool, unskinned, stage;
+    // the grown scene arrays, the new texture pool and records, the grown skinning data and the staged records with ids
+    SceneArrays next;
+    DevBuf recs, pool, unskinned, stage;
     struct Drop {
-        DevBuf* b[16];
+        DevBuf* b[4];
         ~Drop() { for (DevBuf* x : b) release(*x); }
-    } drop = {{&positions, &vertices, &xforms, &meshes, &materials, &instances, &vtxFrame, &surfRec, &descBuf, &tris, &bvh, &tlas, &recs,
-               &pool, &unskinned, &stage}};
+    } drop = {{&recs, &pool, &unskinned, &stage}};
     std::vector<GpuBlasDesc> descs = ctx->hostDescs;
     std::vector<TexRec> newRecs;
-    idkbb::Arena staged;                                  // the new BLASes, until they are copied into `bvh`
+    idkbb::Arena staged;                                  // the new BLASes, until they are copied into `next`
     idkbb::DeviceResult built;
-    size_t nodeBytes = 0, triRecBytes = 0;
     uint64_t nN = old.BlasNodeCount, nT = old.BlasTriangleCount;
     int stackSize = 0;
     int* needDev = nullptr;
@@ -2480,24 +2517,24 @@ IDKPT_API int idkpt_add_models(IdkPtCtx* ctx, const IdkPtAddModelsDesc* m, const
         auto a256 = [](size_t x) { return (x + 255) & ~(size_t)255; };
         const size_t stTris = 0, stMeshes = a256(m->TriangleCount * sizeof(GpuBlasTriangle)), stMaterials = stMeshes + a256(m->MeshCount * sizeof(GpuMesh));
         const size_t stInstances = stMaterials + a256(m->MaterialCount * sizeof(GpuMaterial)), stEnd = stInstances + m->BlasInstanceCount * sizeof(GpuBlasInstance);
-        if (!alloc(stage, stEnd) || !alloc(positions, nV * sizeof(PackedVec3)) || !alloc(vertices, nV * sizeof(GpuVertex)) ||
-            !alloc(xforms, nX * sizeof(GpuMeshTransform)) || !alloc(meshes, nM * sizeof(GpuMesh)) || !alloc(materials, nMat * sizeof(GpuMaterial)) ||
-            !alloc(instances, nI * sizeof(GpuBlasInstance)) || !alloc(vtxFrame, std::max<uint64_t>(nV, 1) * 32) || !alloc(surfRec, std::max<uint64_t>(nM, 1) * 80) ||
-            !alloc(descBuf, nB * sizeof(GpuBlasDesc)) || (m->UnskinnedVertexCount && !alloc(unskinned, nU * sizeof(GpuUnskinnedVertex))))
+        if (!alloc(stage, stEnd) || !alloc(next.positions, nV * sizeof(PackedVec3)) || !alloc(next.vertices, nV * sizeof(GpuVertex)) ||
+            !alloc(next.xforms, nX * sizeof(GpuMeshTransform)) || !alloc(next.meshes, nM * sizeof(GpuMesh)) || !alloc(next.materials, nMat * sizeof(GpuMaterial)) ||
+            !alloc(next.instances, nI * sizeof(GpuBlasInstance)) || !alloc(next.vtxFrame, std::max<uint64_t>(nV, 1) * 32) || !alloc(next.surfRec, std::max<uint64_t>(nM, 1) * 80) ||
+            !alloc(next.descs, nB * sizeof(GpuBlasDesc)) || (m->UnskinnedVertexCount && !alloc(unskinned, nU * sizeof(GpuUnskinnedVertex))))
             return fail(ctx, who, IDKPT_ERR_OUT_OF_MEMORY, "device allocation failed");
 
         // the scene's arrays move device to device; the call's arrays come over once, those with ids into the staging buffer
-        CK(d2d(positions.p, ctx->positions.p, old.VertexCount * sizeof(PackedVec3)));
-        CK(d2d(vertices.p, ctx->vertices.p, old.VertexCount * sizeof(GpuVertex)));
-        CK(d2d(vtxFrame.p, ctx->vtxFrame.p, old.VertexCount * 32));
-        CK(d2d(xforms.p, ctx->xforms.p, old.MeshTransformCount * sizeof(GpuMeshTransform)));
-        CK(d2d(meshes.p, ctx->meshes.p, old.MeshCount * sizeof(GpuMesh)));
-        CK(d2d(surfRec.p, ctx->surfRec.p, old.MeshCount * 80));
-        CK(d2d(materials.p, ctx->materials.p, old.MaterialCount * sizeof(GpuMaterial)));
-        CK(d2d(instances.p, ctx->instances.p, old.BlasInstanceCount * sizeof(GpuBlasInstance)));
-        CK(h2d(at(positions, old.VertexCount * sizeof(PackedVec3)), m->VertexPositions, m->VertexCount * sizeof(PackedVec3)));
-        CK(h2d(at(vertices, old.VertexCount * sizeof(GpuVertex)), m->Vertices, m->VertexCount * sizeof(GpuVertex)));
-        CK(h2d(at(xforms, old.MeshTransformCount * sizeof(GpuMeshTransform)), m->MeshTransforms, m->MeshTransformCount * sizeof(GpuMeshTransform)));
+        CK(d2d(next.positions.p, ctx->scene.positions.p, old.VertexCount * sizeof(PackedVec3)));
+        CK(d2d(next.vertices.p, ctx->scene.vertices.p, old.VertexCount * sizeof(GpuVertex)));
+        CK(d2d(next.vtxFrame.p, ctx->scene.vtxFrame.p, old.VertexCount * 32));
+        CK(d2d(next.xforms.p, ctx->scene.xforms.p, old.MeshTransformCount * sizeof(GpuMeshTransform)));
+        CK(d2d(next.meshes.p, ctx->scene.meshes.p, old.MeshCount * sizeof(GpuMesh)));
+        CK(d2d(next.surfRec.p, ctx->scene.surfRec.p, old.MeshCount * 80));
+        CK(d2d(next.materials.p, ctx->scene.materials.p, old.MaterialCount * sizeof(GpuMaterial)));
+        CK(d2d(next.instances.p, ctx->scene.instances.p, old.BlasInstanceCount * sizeof(GpuBlasInstance)));
+        CK(h2d(at(next.positions, old.VertexCount * sizeof(PackedVec3)), m->VertexPositions, m->VertexCount * sizeof(PackedVec3)));
+        CK(h2d(at(next.vertices, old.VertexCount * sizeof(GpuVertex)), m->Vertices, m->VertexCount * sizeof(GpuVertex)));
+        CK(h2d(at(next.xforms, old.MeshTransformCount * sizeof(GpuMeshTransform)), m->MeshTransforms, m->MeshTransformCount * sizeof(GpuMeshTransform)));
         CK(h2d(at(stage, stTris), m->Triangles, m->TriangleCount * sizeof(GpuBlasTriangle)));
         CK(h2d(at(stage, stMeshes), m->Meshes, m->MeshCount * sizeof(GpuMesh)));
         CK(h2d(at(stage, stMaterials), m->Materials, m->MaterialCount * sizeof(GpuMaterial)));
@@ -2508,19 +2545,19 @@ IDKPT_API int idkpt_add_models(IdkPtCtx* ctx, const IdkPtAddModelsDesc* m, const
         }
         SceneAddArgs a;
         a.tris = (GpuBlasTriangle*)at(stage, stTris);
-        a.meshesIn = (const GpuMesh*)at(stage, stMeshes); a.meshesOut = (GpuMesh*)meshes.p + old.MeshCount;
-        a.materialsIn = (const GpuMaterial*)at(stage, stMaterials); a.materialsOut = (GpuMaterial*)materials.p + old.MaterialCount;
-        a.instancesIn = (const GpuBlasInstance*)at(stage, stInstances); a.instancesOut = (GpuBlasInstance*)instances.p + old.BlasInstanceCount;
+        a.meshesIn = (const GpuMesh*)at(stage, stMeshes); a.meshesOut = (GpuMesh*)next.meshes.p + old.MeshCount;
+        a.materialsIn = (const GpuMaterial*)at(stage, stMaterials); a.materialsOut = (GpuMaterial*)next.materials.p + old.MaterialCount;
+        a.instancesIn = (const GpuBlasInstance*)at(stage, stInstances); a.instancesOut = (GpuBlasInstance*)next.instances.p + old.BlasInstanceCount;
         a.triCount = m->TriangleCount; a.meshCount = m->MeshCount; a.materialCount = m->MaterialCount; a.instanceCount = m->BlasInstanceCount;
         a.vertexOffset = (int32_t)old.VertexCount; a.meshOffset = (int32_t)old.MeshCount; a.materialOffset = (int32_t)old.MaterialCount;
         a.blasOffset = (uint32_t)old.BlasDescCount; a.transformOffset = (uint32_t)old.MeshTransformCount; a.textureOffset = old.TextureCount;
         if (const uint64_t total = a.triCount + a.meshCount + a.materialCount + a.instanceCount)
             k_scene_add_rebase<<<(unsigned)((total + 255) / 256), 256, 0, ctx->stream>>>(a);
         if (const uint32_t n = (uint32_t)m->VertexCount)      // per element: a launch over the appended range equals the full one
-            k_prepare_vertices<<<(n + 255) / 256, 256, 0, ctx->stream>>>((const uint4*)vertices.p + old.VertexCount, (float4*)vtxFrame.p + 2 * old.VertexCount, n);
+            k_prepare_vertices<<<(n + 255) / 256, 256, 0, ctx->stream>>>((const uint4*)next.vertices.p + old.VertexCount, (float4*)next.vtxFrame.p + 2 * old.VertexCount, n);
         if (const uint32_t n = (uint32_t)m->MeshCount)
-            k_prepare_surfaces<<<(n + 255) / 256, 256, 0, ctx->stream>>>((const GpuMesh*)meshes.p + old.MeshCount, (const GpuMaterial*)materials.p,
-                                                                         (float4*)surfRec.p + 5 * old.MeshCount, n);
+            k_prepare_surfaces<<<(n + 255) / 256, 256, 0, ctx->stream>>>((const GpuMesh*)next.meshes.p + old.MeshCount, (const GpuMaterial*)next.materials.p,
+                                                                         (float4*)next.surfRec.p + 5 * old.MeshCount, n);
         CK(cudaGetLastError());
 
         if (m->TextureCount) {                            // decoded once, into a pool of their own; the old records keep theirs
@@ -2536,120 +2573,62 @@ IDKPT_API int idkpt_add_models(IdkPtCtx* ctx, const IdkPtAddModelsDesc* m, const
 
         // the new BLASes: one batch over the staged, rebased triangles and the grown positions
         if (B) {
-            idkbb::StageTimer tm(ctx->stream);
-            tm.mark("start");
-            std::string err;
-            const int brc = idkbb::build_device(ctx->stream, (const PackedVec3*)positions.p, (const GpuBlasTriangle*)at(stage, stTris), in, p,
-                                                staged, built, tm, err);
-            if (brc != idkbb::BB_OK) return blas_build_fail(ctx, who, brc, err);
-            long long fragments = 0;
-            for (int c : built.fragmentCount) fragments += c;
-            tm.print((int)B, fragments);
+            descs.insert(descs.end(), m->BlasDescs, m->BlasDescs + B);
+            GpuBlasDesc* added = descs.data() + old.BlasDescCount;
+            if (int brc = build_blases(ctx, who, (const PackedVec3*)next.positions.p, (const GpuBlasTriangle*)at(stage, stTris), in, p, staged, built, added))
+                return brc;
             nN += (uint64_t)built.nodeStart[B];
             nT += (uint64_t)built.triStart[B];
             if (nN >= (1ull << 31) || nT >= (1ull << 31)) return fail(ctx, who, IDKPT_ERR_INVALID_ARGUMENT, "scene too large");
             for (uint32_t k = 0; k < B; k++) {            // BVH.cs:363-386
-                GpuBlasDesc d = m->BlasDescs[k];
-                d.NodeOffset = (int32_t)(old.BlasNodeCount + built.nodeStart[k]);
-                d.NodeCount = built.nodeStart[k + 1] - built.nodeStart[k];
-                d.TriangleOffset = (int32_t)(old.BlasTriangleCount + built.triStart[k]);
-                d.TriangleCount = built.triStart[k + 1] - built.triStart[k];
-                d.RequiredStackSize = built.requiredStackSize[k];
-                descs.push_back(d);
+                added[k].NodeOffset = (int32_t)(old.BlasNodeCount + built.nodeStart[k]);
+                added[k].TriangleOffset = (int32_t)(old.BlasTriangleCount + built.triStart[k]);
             }
         }
         for (const GpuBlasDesc& d : descs) stackSize = std::max(stackSize, d.RequiredStackSize);   // BVH.UpdateBlasStackSize
-        if ((size_t)std::max(1, stackSize) * IDK_BLOCK * sizeof(uint32_t) > 200 * 1024)
-            return fail(ctx, who, IDKPT_ERR_UNSUPPORTED, "BlasStackSize too large for the shared-memory traversal stack");
-        nodeBytes = ((nN * sizeof(GpuBlasNode)) + 255) & ~(size_t)255;
-        triRecBytes = std::max<size_t>(nT, 1) * 64;
-        if (!alloc(bvh, nodeBytes + triRecBytes) || !alloc(tris, nT * sizeof(GpuBlasTriangle)))
+        if (int r = check_stack_size(ctx, who, stackSize)) return r;
+        next.nodeBytes = ((nN * sizeof(GpuBlasNode)) + 255) & ~(size_t)255;
+        if (!alloc(next.nodes, bvh_bytes(next.nodeBytes, nT)) || !alloc(next.blasTris, nT * sizeof(GpuBlasTriangle)))
             return fail(ctx, who, IDKPT_ERR_OUT_OF_MEMORY, "device allocation failed");
-        float4* recNew = (float4*)at(bvh, nodeBytes);
-        CK(d2d(bvh.p, ctx->nodes.p, old.BlasNodeCount * sizeof(GpuBlasNode)));
-        CK(d2d(recNew, (const char*)ctx->nodes.p + ctx->nodeBytes, old.BlasTriangleCount * 64));
-        CK(d2d(tris.p, ctx->blasTris.p, old.BlasTriangleCount * sizeof(GpuBlasTriangle)));
-        CK(d2d(descBuf.p, ctx->descs.p, old.BlasDescCount * sizeof(GpuBlasDesc)));
+        float4* recNew = (float4*)at(next.nodes, next.nodeBytes);
+        CK(d2d(next.nodes.p, ctx->scene.nodes.p, old.BlasNodeCount * sizeof(GpuBlasNode)));
+        CK(d2d(recNew, (const char*)ctx->scene.nodes.p + ctx->scene.nodeBytes, old.BlasTriangleCount * 64));
+        CK(d2d(next.blasTris.p, ctx->scene.blasTris.p, old.BlasTriangleCount * sizeof(GpuBlasTriangle)));
+        CK(d2d(next.descs.p, ctx->scene.descs.p, old.BlasDescCount * sizeof(GpuBlasDesc)));
         if (B) {
-            CK(d2d((GpuBlasNode*)bvh.p + old.BlasNodeCount, built.nodes, (size_t)built.nodeStart[B] * sizeof(GpuBlasNode)));
-            CK(d2d((GpuBlasTriangle*)tris.p + old.BlasTriangleCount, built.tris, (size_t)built.triStart[B] * sizeof(GpuBlasTriangle)));
+            CK(d2d((GpuBlasNode*)next.nodes.p + old.BlasNodeCount, built.nodes, (size_t)built.nodeStart[B] * sizeof(GpuBlasNode)));
+            CK(d2d((GpuBlasTriangle*)next.blasTris.p + old.BlasTriangleCount, built.tris, (size_t)built.triStart[B] * sizeof(GpuBlasTriangle)));
             if (const uint32_t n = (uint32_t)built.triStart[B])
-                k_prepare_triangles<<<(n + 255) / 256, 256, 0, ctx->stream>>>((const int4*)tris.p + old.BlasTriangleCount, (const float*)positions.p,
+                k_prepare_triangles<<<(n + 255) / 256, 256, 0, ctx->stream>>>((const int4*)next.blasTris.p + old.BlasTriangleCount, (const float*)next.positions.p,
                                                                               recNew + 4 * old.BlasTriangleCount, n);
-            CK(h2d(at(descBuf, old.BlasDescCount * sizeof(GpuBlasDesc)), descs.data() + old.BlasDescCount, B * sizeof(GpuBlasDesc)));
+            CK(h2d(at(next.descs, old.BlasDescCount * sizeof(GpuBlasDesc)), descs.data() + old.BlasDescCount, B * sizeof(GpuBlasDesc)));
         }
 
         // BVH.TlasBuild(true) in ModelManager.Add: the device PLOC build over every instance, TLAS.BuildSettings.SearchRadius 15
         if (old.UseTlas) {
-            if (!alloc(tlas, (2 * nI - 1) * sizeof(GpuTlasNode))) return fail(ctx, who, IDKPT_ERR_OUT_OF_MEMORY, "device allocation failed");
-            if (int trc = enqueue_tlas_build(ctx, bvh.p, descBuf.p, instances.p, xforms.p, tlas.p, nI, 15, &needDev)) return trc;
+            if (!alloc(next.tlas, (2 * nI - 1) * sizeof(GpuTlasNode))) return fail(ctx, who, IDKPT_ERR_OUT_OF_MEMORY, "device allocation failed");
+            if (int trc = enqueue_tlas_build(ctx, next.nodes.p, next.descs.p, next.instances.p, next.xforms.p, next.tlas.p, nI, 15, &needDev)) return trc;
         }
         return IDKPT_OK;
     });
     if (rc) return rc;
-    if (needDev) {
-        int need = 0;
-        CK(cudaMemcpy(&need, needDev, 4, cudaMemcpyDeviceToHost));
-        if (need < 0)
-            return fail(ctx, who, IDKPT_ERR_INVALID_ARGUMENT, "an instance's world box is not finite or its half area overflows (ModelMatrix or BLAS root)");
-        if (need > IDK_TLAS_STACK_SIZE)
-            return fail(ctx, who, IDKPT_ERR_UNSUPPORTED, "the TLAS is deeper than the 24-entry traversal stack of the TLAS walk (BVHIntersect.glsl:4)");
-    }
+    if (needDev)
+        if ((rc = check_tlas_built(ctx, who, needDev, false))) return rc;
 
-    // commit: launch configuration and L2 window for the new arrays first (restored if either fails), then the swap
-    const int oldStack = ctx->sc.stackSize;
-    ctx->sc.stackSize = std::max(1, stackSize);
-    if ((rc = configure_launches(ctx)) || (rc = set_l2_window(ctx, bvh.p, nodeBytes + triRecBytes))) {
-        const std::string err = ctx->lastError;
-        ctx->sc.stackSize = oldStack;
-        configure_launches(ctx);
-        set_l2_window(ctx, ctx->nodes.p, ctx->nodeBytes + std::max<size_t>(ctx->counts.BlasTriangleCount, 1) * 64);
-        ctx->lastError = err;
-        return rc;
-    }
-    std::swap(ctx->positions, positions);                // `drop` frees the old arrays
-    std::swap(ctx->vertices, vertices);
-    std::swap(ctx->xforms, xforms);
-    std::swap(ctx->meshes, meshes);
-    std::swap(ctx->materials, materials);
-    std::swap(ctx->instances, instances);
-    std::swap(ctx->vtxFrame, vtxFrame);
-    std::swap(ctx->surfRec, surfRec);
-    std::swap(ctx->descs, descBuf);
-    std::swap(ctx->blasTris, tris);
-    std::swap(ctx->nodes, bvh);
-    if (old.UseTlas) std::swap(ctx->tlas, tlas);
-    if (m->TextureCount) {
-        std::swap(ctx->tex.recs, recs);
-        ctx->tex.pools.push_back(pool);
-        pool = DevBuf{};
-    }
-    if (m->UnskinnedVertexCount) std::swap(ctx->unskinned, unskinned);
-    release(ctx->prevPositions);                         // re-created from the positions at its next use (ModelManager.cs:620)
-
-    DeviceScene& sc = ctx->sc;
-    sc.nodes = (const float4*)ctx->nodes.p;
-    sc.triRec = (const float4*)((char*)ctx->nodes.p + nodeBytes);
-    sc.blasTris = (const int4*)ctx->blasTris.p;
-    sc.descs = (const GpuBlasDesc*)ctx->descs.p;
-    sc.instances = (const GpuBlasInstance*)ctx->instances.p;
-    sc.xforms = (const float4*)ctx->xforms.p;
-    sc.meshes = (const GpuMesh*)ctx->meshes.p;
-    sc.materials = (const GpuMaterial*)ctx->materials.p;
-    sc.vertices = (const uint4*)ctx->vertices.p;
-    sc.instanceCount = (uint32_t)nI;
-    sc.tlasNodes = (const float4*)ctx->tlas.p;
-    sc.vtxFrame = (const float4*)ctx->vtxFrame.p;
-    sc.surfRec = (const float4*)ctx->surfRec.p;
-    sc.textures = (const TexRec*)ctx->tex.recs.p;
-    sc.textureCount = (uint32_t)nTex;
-    IdkPtSceneDesc& c = ctx->counts;
+    IdkPtSceneDesc c = old;
     c.BlasNodeCount = nN; c.BlasTriangleCount = nT; c.BlasDescCount = nB; c.BlasInstanceCount = nI;
     if (old.UseTlas) c.TlasNodeCount = 2 * nI - 1;
     c.MeshTransformCount = nX; c.MeshCount = nM; c.MaterialCount = nMat; c.VertexCount = nV; c.VertexPositionCount = nV;
     c.BlasStackSize = stackSize; c.TextureCount = nTex;
-    ctx->nodeBytes = nodeBytes;
-    ctx->hostDescs = std::move(descs);
+    if ((rc = commit_scene(ctx, next, c, std::move(descs)))) return rc;
+    if (m->TextureCount) {                               // the records of the new pool's textures follow the old ones
+        std::swap(ctx->tex.recs, recs);
+        ctx->tex.pools.push_back(pool);
+        pool = DevBuf{};
+        derive_view(ctx);
+    }
+    if (m->UnskinnedVertexCount) std::swap(ctx->unskinned, unskinned);
+    release(ctx->prevPositions);                         // re-created from the positions at its next use (ModelManager.cs:620)
     for (uint64_t i = 0; i < m->BlasInstanceCount; i++)
         ctx->hostInstances.push_back({m->BlasInstances[i].BlasId + (uint32_t)old.BlasDescCount, m->BlasInstances[i].MeshTransformId + (uint32_t)old.MeshTransformCount});
     for (uint64_t i = 0; i < m->MaterialCount; i++) {
@@ -2661,8 +2640,6 @@ IDKPT_API int idkpt_add_models(IdkPtCtx* ctx, const IdkPtAddModelsDesc* m, const
         ctx->unskinnedMaxJoint.push_back(std::max(std::max(j[0], j[1]), std::max(j[2], j[3])));
     }
     ctx->unskinnedCount = nU;
-    ctx->sceneGeneration++;                              // a bound voxeliser re-sizes its work queue for the new draw list
-    ctx->accumulatedSamples = 0;
     return IDKPT_OK;
 }
 
@@ -2684,7 +2661,7 @@ IDKPT_API int idkpt_blas_sah(IdkPtCtx* ctx, uint32_t first, uint32_t count, cons
     int* stack = (int*)(out + count);
     return run_timed(ctx, "idkpt_blas_sah", nullptr, [&]() -> int {
         for (uint32_t k = 0; k < count; k++)
-            idkbb::k_global_sah<<<1, 1, 0, ctx->stream>>>((const GpuBlasNode*)ctx->nodes.p + ctx->hostDescs[first + k].NodeOffset, stack, triangleCost, out + k);
+            idkbb::k_global_sah<<<1, 1, 0, ctx->stream>>>((const GpuBlasNode*)ctx->scene.nodes.p + ctx->hostDescs[first + k].NodeOffset, stack, triangleCost, out + k);
         return IDKPT_OK;
     }, sahOut, out, (size_t)count * sizeof(double));
 }
@@ -2696,13 +2673,13 @@ IDKPT_API int idkpt_read_range(IdkPtCtx* ctx, IdkPtArrayId which, uint64_t first
     size_t elem = 0;
     uint64_t limit = 0;
     switch (which) {
-        case IDKPT_ARRAY_BLAS_NODES: b = &ctx->nodes; elem = sizeof(GpuBlasNode); limit = ctx->counts.BlasNodeCount; break;
-        case IDKPT_ARRAY_VERTEX_POSITIONS: b = &ctx->positions; elem = sizeof(PackedVec3); limit = ctx->counts.VertexPositionCount; break;
-        case IDKPT_ARRAY_VERTICES: b = &ctx->vertices; elem = sizeof(GpuVertex); limit = ctx->counts.VertexCount; break;
-        case IDKPT_ARRAY_TLAS_NODES: b = &ctx->tlas; elem = sizeof(GpuTlasNode); limit = ctx->counts.UseTlas ? ctx->counts.TlasNodeCount : 0; break;
-        case IDKPT_ARRAY_BLAS_TRIANGLES: b = &ctx->blasTris; elem = sizeof(GpuBlasTriangle); limit = ctx->counts.BlasTriangleCount; break;
-        case IDKPT_ARRAY_BLAS_DESCS: b = &ctx->descs; elem = sizeof(GpuBlasDesc); limit = ctx->counts.BlasDescCount; break;
-        case IDKPT_ARRAY_MESH_TRANSFORMS: b = &ctx->xforms; elem = sizeof(GpuMeshTransform); limit = ctx->counts.MeshTransformCount; break;
+        case IDKPT_ARRAY_BLAS_NODES: b = &ctx->scene.nodes; elem = sizeof(GpuBlasNode); limit = ctx->counts.BlasNodeCount; break;
+        case IDKPT_ARRAY_VERTEX_POSITIONS: b = &ctx->scene.positions; elem = sizeof(PackedVec3); limit = ctx->counts.VertexPositionCount; break;
+        case IDKPT_ARRAY_VERTICES: b = &ctx->scene.vertices; elem = sizeof(GpuVertex); limit = ctx->counts.VertexCount; break;
+        case IDKPT_ARRAY_TLAS_NODES: b = &ctx->scene.tlas; elem = sizeof(GpuTlasNode); limit = ctx->counts.UseTlas ? ctx->counts.TlasNodeCount : 0; break;
+        case IDKPT_ARRAY_BLAS_TRIANGLES: b = &ctx->scene.blasTris; elem = sizeof(GpuBlasTriangle); limit = ctx->counts.BlasTriangleCount; break;
+        case IDKPT_ARRAY_BLAS_DESCS: b = &ctx->scene.descs; elem = sizeof(GpuBlasDesc); limit = ctx->counts.BlasDescCount; break;
+        case IDKPT_ARRAY_MESH_TRANSFORMS: b = &ctx->scene.xforms; elem = sizeof(GpuMeshTransform); limit = ctx->counts.MeshTransformCount; break;
         case IDKPT_ARRAY_NODE_LOCAL_TRANSFORMS: b = &ctx->anim.locals; elem = sizeof(IdkPtNodeLocal); limit = ctx->anim.plan.nodes.size(); break;
         case IDKPT_ARRAY_NODE_GLOBAL_TRANSFORMS: b = &ctx->anim.globals; elem = 64; limit = ctx->anim.plan.nodes.size(); break;
         case IDKPT_ARRAY_JOINT_MATRICES: b = &ctx->anim.joints; elem = 48; limit = ctx->anim.plan.jointMatrixCount; break;
@@ -3420,7 +3397,7 @@ IDKPT_API int idkpt_gbuffer(IdkPtCtx* ctx, const GpuPerFrameData* frame, int32_t
     if (hostPrev && prevBytes) CK(cudaMemcpyAsync(r.gbPrev.p, prevPositions, prevBytes, cudaMemcpyHostToDevice, ctx->stream));
     char* base = (char*)r.gb.buf[0].p;
     a.sc = ctx->sc;
-    a.positions = (const float*)ctx->positions.p;
+    a.positions = (const float*)ctx->scene.positions.p;
     a.prevPositions = kept ? (const float*)ctx->prevPositions.p : hostPrev ? (const float*)r.gbPrev.p : a.positions;
     memcpy(a.projView, frame->ProjView, sizeof(a.projView));
     memcpy(a.prevProjView, frame->PrevProjView, sizeof(a.prevProjView));
@@ -3517,7 +3494,7 @@ IDKPT_API int idkpt_transparency(IdkPtCtx* ctx, const GpuPerFrameData* frame, co
     const size_t n = (size_t)g->Width * g->Height;
     const bool hostArray = source == IDKPT_LIT_SOURCE_ARRAY && !g->OnDevice;
     a.sc = ctx->sc;
-    a.positions = (const float*)ctx->positions.p;
+    a.positions = (const float*)ctx->scene.positions.p;
     memcpy(a.projView, frame->ProjView, sizeof(a.projView));
     memcpy(a.invProjView, frame->InvProjView, sizeof(a.invProjView));
     for (int k = 0; k < 3; k++) a.viewPos[k] = frame->ViewPos[k];
@@ -3704,7 +3681,7 @@ IDKPT_API int idkpt_update_models(IdkPtCtx* ctx, float time, int32_t searchRadiu
     g.jointSlotSkin = (const uint32_t*)a.jointSlotSkin.p; g.jointSlotJoint = (const uint32_t*)a.jointSlotJoint.p; g.owner = (const int32_t*)a.owner.p;
     g.locals = (IdkPtNodeLocal*)a.scratchLocals.p; g.globals = (const idkanim::M4*)a.globals.p; g.newGlobals = (idkanim::M4*)a.newGlobals.p;
     g.diffs = (idkanim::M4*)a.diffs.p; g.invSkin = (idkanim::M4*)a.invSkin.p; g.dirty = (uint8_t*)a.dirty.p; g.inSet = (uint8_t*)a.inSet.p;
-    g.movedBits = (uint8_t*)a.movedBits.p; g.xforms = (GpuMeshTransform*)ctx->xforms.p; g.joints = (float*)a.joints.p; g.flags = (uint32_t*)a.flags.p;
+    g.movedBits = (uint8_t*)a.movedBits.p; g.xforms = (GpuMeshTransform*)ctx->scene.xforms.p; g.joints = (float*)a.joints.p; g.flags = (uint32_t*)a.flags.p;
     g.time = time;
     g.groupCount = (uint32_t)p.groups.size(); g.levelCount = (uint32_t)p.levelStart.size() - 1; g.skinCount = (uint32_t)p.skins.size();
     g.transformCount = (uint32_t)p.owner.size(); g.jointMatrixCount = p.jointMatrixCount;

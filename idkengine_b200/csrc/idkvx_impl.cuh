@@ -20,7 +20,7 @@ struct IdkVxCtx : IdkCtxBase {
     IdkPtSceneDesc counts = {};
     std::vector<GpuBlasDesc> hostDescs;
     std::vector<GpuBlasInstance> hostInstances;
-    DevBuf positions, vertices, tris, descs, instances, xforms, meshes, materials, lights;
+    SceneArrays scene;                    // idkvx_set_scene's copy: no nodes, triangle records, TLAS or prepared records
     TextureTable tex;
     DevBuf queue, queueCount, counters;
     size_t queueCapacity = 0;
@@ -70,12 +70,21 @@ static void unbind_voxelizers(IdkPtCtx* pt) {
     pt->boundVoxelizers.clear();
 }
 
-// The scene arrays idkvx_set_scene copies, the texture table included.
-static void release_scene(IdkVxCtx* ctx) {
-    for (DevBuf* b : {&ctx->positions, &ctx->vertices, &ctx->tris, &ctx->descs, &ctx->instances, &ctx->xforms, &ctx->meshes,
-                      &ctx->materials, &ctx->lights})
-        release(*b);
-    release_textures(ctx->tex);
+// VxScene's arrays: a scene's arrays and texture table, the path tracer's (bind_source) or the voxeliser's own copy
+// (idkvx_set_scene).
+static void vx_view(VxScene& sc, const SceneArrays& a, const TextureTable& t, uint64_t lightCount) {
+    sc.positions = (const float*)a.positions.p;
+    sc.vertices = (const uint4*)a.vertices.p;
+    sc.blasTris = (const int4*)a.blasTris.p;
+    sc.descs = (const GpuBlasDesc*)a.descs.p;
+    sc.instances = (const GpuBlasInstance*)a.instances.p;
+    sc.xforms = (const float4*)a.xforms.p;
+    sc.meshes = (const GpuMesh*)a.meshes.p;
+    sc.materials = (const GpuMaterial*)a.materials.p;
+    sc.lights = (const GpuLight*)a.lights.p;
+    sc.textures = (const TexRec*)t.recs.p;
+    sc.srgbLut = (const float*)t.srgbLut.p;
+    sc.lightCount = (uint32_t)lightCount;
 }
 
 // Work items of the large-triangle queue for a draw list: (triangle, tile) items of large triangles.
@@ -89,26 +98,15 @@ static int size_queue(IdkVxCtx* ctx, const std::vector<GpuBlasDesc>& descs, cons
 
 // idkvx_voxelize of a bound voxeliser: VxScene's pointers, the light count and the shadowed-light bound from the path tracer's
 // scene as it stands now. Every path-tracer call that writes these arrays (idkpt_set_scene, idkpt_update_range,
-// idkpt_set_textures, idkpt_skin_vertices, idkpt_blas_refit, idkpt_tlas_build) ends in a synchronise of its stream, and so
+// idkpt_set_textures, idkpt_skin_vertices, idkpt_blas_refit, idkpt_tlas_build, idkpt_blas_rebuild, idkpt_add_models,
+// idkpt_update_models) ends in a synchronise of its stream, and so
 // does idkvx_voxelize; samples idkpt_compute has queued only read them. So the voxelisation reads a finished scene without
 // waiting for the path tracer, and a pointer is never kept past the call that could reallocate it.
 static int bind_source(IdkVxCtx* ctx) {
     IdkPtCtx* pt = ctx->source;
     if (!pt->haveScene)
         return fail(ctx, IDKPT_ERR_NO_SCENE, "idkvx_voxelize: the path-tracer context bound with idkvx_set_scene_from has no scene (idkpt_set_scene)");
-    VxScene& sc = ctx->sc;
-    sc.positions = (const float*)pt->positions.p;
-    sc.vertices = (const uint4*)pt->vertices.p;
-    sc.blasTris = (const int4*)pt->blasTris.p;
-    sc.descs = (const GpuBlasDesc*)pt->descs.p;
-    sc.instances = (const GpuBlasInstance*)pt->instances.p;
-    sc.xforms = (const float4*)pt->xforms.p;
-    sc.meshes = (const GpuMesh*)pt->meshes.p;
-    sc.materials = (const GpuMaterial*)pt->materials.p;
-    sc.lights = (const GpuLight*)pt->lights.p;
-    sc.textures = (const TexRec*)pt->tex.recs.p;
-    sc.srgbLut = (const float*)pt->tex.srgbLut.p;
-    sc.lightCount = (uint32_t)pt->counts.LightCount;
+    vx_view(ctx->sc, pt->scene, pt->tex, pt->counts.LightCount);
     ctx->maxPointShadowIndex = -1;   // idkpt_update_range(LIGHTS) may have changed it
     for (const GpuLight& L : pt->hostLights) ctx->maxPointShadowIndex = std::max(ctx->maxPointShadowIndex, L.PointShadowIndex);
     ctx->shadowedLights = ctx->maxPointShadowIndex >= 0;
@@ -182,7 +180,8 @@ IDKPT_API void idkvx_destroy(IdkVxCtx* ctx) {
     cudaSetDevice(ctx->device);
     if (ctx->stream) cudaStreamSynchronize(ctx->stream);
     unbind_source(ctx);
-    release_scene(ctx);
+    release(ctx->scene);
+    release_textures(ctx->tex);
     DevBuf* all[] = {&ctx->gridMem, &ctx->queue, &ctx->queueCount, &ctx->counters, &ctx->stage, &ctx->cone.buf[0], &ctx->debugImage, &ctx->debugMask};
     for (DevBuf* b : all) release(*b);
     destroy_stream(ctx);
@@ -210,33 +209,21 @@ IDKPT_API int idkvx_set_scene(IdkVxCtx* ctx, const IdkPtSceneDesc* s) {
     for (uint64_t i = 0; i < s->LightCount; i++) ctx->maxPointShadowIndex = std::max(ctx->maxPointShadowIndex, s->Lights[i].PointShadowIndex);
     ctx->shadowedLights = ctx->maxPointShadowIndex >= 0;
     int rc;
-    if ((rc = upload(ctx, ctx->positions, s->VertexPositions, s->VertexPositionCount * sizeof(PackedVec3)))) return rc;
-    if ((rc = upload(ctx, ctx->vertices, s->Vertices, s->VertexCount * sizeof(GpuVertex)))) return rc;
-    if ((rc = upload(ctx, ctx->tris, s->BlasTriangles, s->BlasTriangleCount * sizeof(GpuBlasTriangle)))) return rc;
-    if ((rc = upload(ctx, ctx->descs, s->BlasDescs, s->BlasDescCount * sizeof(GpuBlasDesc)))) return rc;
-    if ((rc = upload(ctx, ctx->instances, s->BlasInstances, s->BlasInstanceCount * sizeof(GpuBlasInstance)))) return rc;
-    if ((rc = upload(ctx, ctx->xforms, s->MeshTransforms, s->MeshTransformCount * sizeof(GpuMeshTransform)))) return rc;
-    if ((rc = upload(ctx, ctx->meshes, s->Meshes, s->MeshCount * sizeof(GpuMesh)))) return rc;
-    if ((rc = upload(ctx, ctx->materials, s->Materials, s->MaterialCount * sizeof(GpuMaterial)))) return rc;
-    if ((rc = upload(ctx, ctx->lights, s->Lights, s->LightCount * sizeof(GpuLight)))) return rc;
+    if ((rc = upload(ctx, ctx->scene.positions, s->VertexPositions, s->VertexPositionCount * sizeof(PackedVec3)))) return rc;
+    if ((rc = upload(ctx, ctx->scene.vertices, s->Vertices, s->VertexCount * sizeof(GpuVertex)))) return rc;
+    if ((rc = upload(ctx, ctx->scene.blasTris, s->BlasTriangles, s->BlasTriangleCount * sizeof(GpuBlasTriangle)))) return rc;
+    if ((rc = upload(ctx, ctx->scene.descs, s->BlasDescs, s->BlasDescCount * sizeof(GpuBlasDesc)))) return rc;
+    if ((rc = upload(ctx, ctx->scene.instances, s->BlasInstances, s->BlasInstanceCount * sizeof(GpuBlasInstance)))) return rc;
+    if ((rc = upload(ctx, ctx->scene.xforms, s->MeshTransforms, s->MeshTransformCount * sizeof(GpuMeshTransform)))) return rc;
+    if ((rc = upload(ctx, ctx->scene.meshes, s->Meshes, s->MeshCount * sizeof(GpuMesh)))) return rc;
+    if ((rc = upload(ctx, ctx->scene.materials, s->Materials, s->MaterialCount * sizeof(GpuMaterial)))) return rc;
+    if ((rc = upload(ctx, ctx->scene.lights, s->Lights, s->LightCount * sizeof(GpuLight)))) return rc;
     // material textures (BaseColor / Emissive are the slots the voxeliser's fragment stage uses)
     if ((rc = upload_textures(ctx, ctx->tex, s->Textures, s->TextureCount))) return rc;
     ctx->hostDescs.assign(s->BlasDescs, s->BlasDescs + s->BlasDescCount);
     ctx->hostInstances.assign(s->BlasInstances, s->BlasInstances + s->BlasInstanceCount);
     if ((rc = size_queue(ctx, ctx->hostDescs, ctx->hostInstances))) return rc;
-    VxScene& sc = ctx->sc;
-    sc.positions = (const float*)ctx->positions.p;
-    sc.vertices = (const uint4*)ctx->vertices.p;
-    sc.blasTris = (const int4*)ctx->tris.p;
-    sc.descs = (const GpuBlasDesc*)ctx->descs.p;
-    sc.instances = (const GpuBlasInstance*)ctx->instances.p;
-    sc.xforms = (const float4*)ctx->xforms.p;
-    sc.meshes = (const GpuMesh*)ctx->meshes.p;
-    sc.materials = (const GpuMaterial*)ctx->materials.p;
-    sc.lights = (const GpuLight*)ctx->lights.p;
-    sc.textures = (const TexRec*)ctx->tex.recs.p;
-    sc.srgbLut = (const float*)ctx->tex.srgbLut.p;
-    sc.lightCount = (uint32_t)s->LightCount;
+    vx_view(ctx->sc, ctx->scene, ctx->tex, s->LightCount);
     ctx->counts = *s;
     CK(cudaStreamSynchronize(ctx->stream));
     ctx->haveScene = true;
@@ -249,7 +236,8 @@ IDKPT_API int idkvx_set_scene_from(IdkVxCtx* ctx, IdkPtCtx* pathTracer) {
         return fail(ctx, IDKPT_ERR_UNSUPPORTED, "idkvx_set_scene_from: the path-tracer context is on another device");
     CK(cudaSetDevice(ctx->device));
     unbind_source(ctx);
-    release_scene(ctx);
+    release(ctx->scene);
+    release_textures(ctx->tex);
     ctx->haveScene = false;
     ctx->hostDescs.clear();
     ctx->hostInstances.clear();
