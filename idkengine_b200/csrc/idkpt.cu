@@ -32,13 +32,14 @@
 #include "idk_blas_build.cuh"
 #include "idk_scene_add.cuh"
 #include "idk_animation.cuh"
+#include "idk_collision.cuh"
 #include "idk_textures_host.h"
 
 #define IDKPT_ABI_VERSION 4u   // 2: IdkPtSceneDesc gained Textures / TextureCount; 3: IdkPtStats gained CompactMs / AccumulateMs, host-buffer registration;
                                // 4: gather handle blob is 5 IPC handles (320 bytes), IDKPT_CREATE_GLOBAL_SLOTS, idkpt_gather_connect.
                                // Entry points added since (point-shadow cube maps, idkvx_set_shadow_maps, volumetric lighting, SSAO
                                // and deferred lighting, SSR and the TAA resolve, the shading-rate classifier, the G-buffer pass,
-                               // transparency, the light spheres and the skybox) are
+                               // transparency, the light spheres and the skybox, scene-versus-sphere collision) are
                                // additive and keep 4;
                                // IdkPtDeferredSettings grew a trailing IsVariableRateShading.
 
@@ -395,6 +396,7 @@ static int configure_launches(IdkPtCtx* ctx) {
     CK(cudaFuncSetAttribute(k_gbuffer, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)ctx->stackBytes));
     CK(cudaFuncSetAttribute(k_transparency<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)ctx->stackBytes));
     CK(cudaFuncSetAttribute(k_transparency<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)ctx->stackBytes));
+    CK(cudaFuncSetAttribute(k_collide_spheres, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)ctx->stackBytes));
     ctx->traverse2Smem = (size_t)stackSize * IDK_T2_BLOCK * sizeof(uint32_t);
     CK(cudaFuncSetAttribute(k_traverse2<false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)ctx->traverse2Smem));
     CK(cudaFuncSetAttribute(k_traverse2<true, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)ctx->traverse2Smem));
@@ -1690,7 +1692,7 @@ static int preload_kernels(IdkPtCtx* ctx) {
     IDK_PRELOAD(k_ssao); IDK_PRELOAD(k_deferred_lighting); IDK_PRELOAD(k_ssr); IDK_PRELOAD(k_taa_resolve);
     IDK_PRELOAD(k_shading_rate); IDK_PRELOAD(k_vrs_scan); IDK_PRELOAD(k_deferred_lighting_vrs); IDK_PRELOAD(k_gbuffer);
     IDK_PRELOAD(k_transparency<false>); IDK_PRELOAD(k_transparency<true>); IDK_PRELOAD(k_lights_skybox);
-    IDK_PRELOAD(k_lights_skybox_vrs); IDK_PRELOAD(k_sky_atmosphere); IDK_PRELOAD(k_sky_equirect);
+    IDK_PRELOAD(k_lights_skybox_vrs); IDK_PRELOAD(k_sky_atmosphere); IDK_PRELOAD(k_sky_equirect); IDK_PRELOAD(k_collide_spheres);
 #undef IDK_PRELOAD
     return IDKPT_OK;
 }
@@ -2724,6 +2726,47 @@ IDKPT_API int idkpt_trace_rays(IdkPtCtx* ctx, const IdkPtRay* rays, uint64_t cou
 
 IDKPT_API int idkpt_trace_rays_any(IdkPtCtx* ctx, const IdkPtRay* rays, uint64_t count, int32_t traceLights, IdkPtHit* hitsOut, float* kernelMs) {
     return trace_rays_impl(ctx, rays, count, traceLights, hitsOut, kernelMs, true);
+}
+
+IDKPT_API int idkpt_collide_spheres(IdkPtCtx* ctx, const IdkPtMovingSphere* spheres, uint64_t count, const IdkPtCollisionSettings* settings,
+                                    IdkPtSphereCollision* out, float* kernelMs) {
+    const char* who = "idkpt_collide_spheres";
+    if (!ctx) return fail(ctx, IDKPT_ERR_INVALID_ARGUMENT, "idkpt_collide_spheres: null argument");
+    if (!settings || (count && (!spheres || !out))) return fail(ctx, who, IDKPT_ERR_INVALID_ARGUMENT, "null argument");
+    if (!ctx->haveScene) return fail(ctx, who, IDKPT_ERR_NO_SCENE, "no scene");
+    if (count >= (1ull << 31)) return fail(ctx, who, IDKPT_ERR_INVALID_ARGUMENT, "too many spheres");
+    const IdkPtCollisionSettings st = *settings;
+    if (st.TestSteps < 1) return fail(ctx, who, IDKPT_ERR_INVALID_ARGUMENT, "TestSteps must be at least 1");
+    if (st.RecursiveSteps < 0 || st.RecursiveSteps > IDKPT_MAX_COLLISION_RECURSIVE_STEPS)
+        return fail(ctx, who, IDKPT_ERR_INVALID_ARGUMENT, "RecursiveSteps outside 0..IDKPT_MAX_COLLISION_RECURSIVE_STEPS");
+    if (st.Response != IDKPT_COLLISION_SLIDE && st.Response != IDKPT_COLLISION_REFLECT)
+        return fail(ctx, who, IDKPT_ERR_INVALID_ARGUMENT, "unknown Response");
+    for (uint64_t i = 0; i < count; i++)
+        if (!(spheres[i].Radius >= 0.0f) || !std::isfinite(spheres[i].Radius))
+            return fail(ctx, who, IDKPT_ERR_INVALID_ARGUMENT, "a Radius is negative or not finite");
+    if (kernelMs) *kernelMs = 0.0f;
+    if (count == 0) return IDKPT_OK;
+    CK(cudaSetDevice(ctx->device));
+    DevBuf &din = ctx->scratch[0], &dout = ctx->scratch[1];
+    if (ensure(din, count * sizeof(IdkPtMovingSphere)) != cudaSuccess || ensure(dout, count * sizeof(IdkPtSphereCollision)) != cudaSuccess)
+        return fail(ctx, who, IDKPT_ERR_OUT_OF_MEMORY, "device allocation failed");
+    CK(cudaMemcpyAsync(din.p, spheres, count * sizeof(IdkPtMovingSphere), cudaMemcpyHostToDevice, ctx->stream));
+    CollideArgs a;
+    a.nodes = ctx->sc.nodes;
+    a.blasTris = ctx->sc.blasTris;
+    a.positions = (const float*)ctx->scene.positions.p;
+    a.descs = ctx->sc.descs;
+    a.instances = ctx->sc.instances;
+    a.xforms = ctx->sc.xforms;
+    a.instanceCount = ctx->sc.instanceCount;
+    a.spheres = (const IdkPtMovingSphere*)din.p;
+    a.out = (IdkPtSphereCollision*)dout.p;
+    a.count = (uint32_t)count;
+    a.st = st;
+    return run_timed(ctx, who, kernelMs, [&]() -> int {
+        k_collide_spheres<<<(unsigned)((count + IDK_BLOCK - 1) / IDK_BLOCK), IDK_BLOCK, ctx->stackBytes, ctx->stream>>>(a);
+        return IDKPT_OK;
+    }, out, dout.p, count * sizeof(IdkPtSphereCollision));
 }
 
 // ---- point-shadow cube maps (PointShadowManager.UpdateBuffer / RenderShadowMaps) ----------------------------------------------

@@ -53,6 +53,10 @@ IdkPtGpuSettings = np.dtype([("FocalLength", f4), ("LenseRadius", f4), ("DoDebug
 IdkPtRay = np.dtype([("Origin", f4, 3), ("TMax", f4), ("Direction", f4, 3), ("_pad0", f4)])
 IdkPtHit = np.dtype([("BaryX", f4), ("BaryY", f4), ("T", f4), ("TriangleId", u4), ("MeshTransformId", u4),
                      ("NodePairFetches", u4), ("TriangleTests", u4), ("_pad0", u4)])
+IdkPtCollisionSettings = np.dtype([("TestSteps", i4), ("RecursiveSteps", i4), ("EpsilonNormalOffset", f4), ("Response", i4)])
+IdkPtMovingSphere = np.dtype([("PrevPosition", f4, 3), ("Radius", f4), ("Position", f4, 3), ("_pad0", f4), ("Velocity", f4, 3),
+                              ("_pad1", f4)])
+IdkPtSphereCollision = np.dtype([("Position", f4, 3), ("Hits", i4), ("Velocity", f4, 3), ("_pad0", f4)])
 # idkpt_add_models's argument record: its pointers as u8 (capi.IdkPtAddModelsDesc is the ctypes twin the calls pass)
 IdkPtAddModelsDesc = np.dtype([(n, u8) for n in (
     "Triangles", "TriangleCount", "BlasDescs", "BlasDescCount", "BlasInstances", "BlasInstanceCount", "MeshTransforms",

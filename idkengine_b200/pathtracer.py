@@ -20,6 +20,12 @@ class IdkPtError(RuntimeError):
     pass
 
 
+# Intersections.SceneVsMovingSphereSettings (TestSteps, RecursiveSteps, EpsilonNormalOffset) and the response of the caller's
+# callback: the lights' (LightManager.cs:237-258) and the camera's (Camera.cs:152-169) collision.
+LIGHT_COLLISION = (1, 8, 0.001, capi.IDKPT_COLLISION_REFLECT)
+CAMERA_COLLISION = (3, 12, 0.001, capi.IDKPT_COLLISION_SLIDE)
+
+
 class PathTracer:
     def __init__(self, width, height, settings=None, device=0, tile=(8, 0, 1), lib_path=None, lanes=0, global_slots=False):
         """global_slots: IDKPT_CREATE_GLOBAL_SLOTS -- a tiled (multi-GPU) context numbers its alive rays over the WHOLE image, so the
@@ -455,6 +461,19 @@ class PathTracer:
         self._check(self._lib.idkpt_trace_rays_any(self._ctx, rays.ctypes.data, len(rays), int(trace_lights),
                                                    hits.ctypes.data, ctypes.byref(ms)), "idkpt_trace_rays_any")
         return hits, ms.value
+
+    def CollideSpheres(self, spheres, settings=None):
+        """Intersections.SceneVsMovingSphereCollisionRoutine for each IdkPtMovingSphere against the current device scene.
+        settings: (TestSteps, RecursiveSteps, EpsilonNormalOffset, Response) or an IdkPtCollisionSettings record, default
+        LIGHT_COLLISION. Returns (IdkPtSphereCollision records, kernel ms)."""
+        spheres = np.ascontiguousarray(spheres)
+        assert spheres.dtype == gt.IdkPtMovingSphere
+        st = np.array(tuple(LIGHT_COLLISION if settings is None else settings), gt.IdkPtCollisionSettings)
+        out = np.zeros(len(spheres), gt.IdkPtSphereCollision)
+        ms = ctypes.c_float()
+        self._check(self._lib.idkpt_collide_spheres(self._ctx, spheres.ctypes.data, len(spheres), st.ctypes.data, out.ctypes.data,
+                                                    ctypes.byref(ms)), "idkpt_collide_spheres")
+        return out, ms.value
 
     def ShadowsRayTraced(self, frame, depth, normal_rg, light_index, samples=1, noise_index=0, jitter=(0.0, 0.0), visibility=None):
         """PointShadowManager.ComputeRayTracedShadowMaps for one light: visibility image from a G-buffer (host arrays)."""

@@ -308,6 +308,49 @@ IDKPT_API int idkpt_trace_rays(IdkPtCtx* ctx, const IdkPtRay* rays, uint64_t cou
  * is 1 if the ray is occluded, 0 otherwise; T/TriangleId/Bary describe the first accepted (not the closest) hit. */
 IDKPT_API int idkpt_trace_rays_any(IdkPtCtx* ctx, const IdkPtRay* rays, uint64_t count, int32_t trace_lights, IdkPtHit* hits_out, float* kernel_ms);
 
+/* ---- scene versus moving spheres: Intersections.SceneVsMovingSphereCollisionRoutine (Intersections.cs:492-593) ----
+ * The response the caller's callback applies on each hit: Camera.CollisionDetection (Camera.cs:152-169) slides,
+ * LightManager.CollisionDetection (LightManager.cs:237-258) reflects. */
+typedef enum IdkPtCollisionResponse {
+    IDKPT_COLLISION_SLIDE = 0,     /* Plane.Project of the remaining step and of the velocity */
+    IDKPT_COLLISION_REFLECT = 1    /* Plane.Reflect of the remaining step and of the velocity */
+} IdkPtCollisionResponse;
+
+#define IDKPT_MAX_COLLISION_RECURSIVE_STEPS 64
+
+typedef struct IdkPtCollisionSettings {   /* Intersections.SceneVsMovingSphereSettings + the response */
+    int32_t TestSteps;                    /* >= 1; the camera uses 3, the lights 1 */
+    int32_t RecursiveSteps;               /* 0 .. IDKPT_MAX_COLLISION_RECURSIVE_STEPS; the camera uses 12, the lights 8 */
+    float   EpsilonNormalOffset;          /* 0.001 for both */
+    int32_t Response;                     /* IdkPtCollisionResponse */
+} IdkPtCollisionSettings;
+IDK_STATIC_ASSERT(sizeof(IdkPtCollisionSettings) == 16, "IdkPtCollisionSettings must be 16 bytes");
+
+typedef struct IdkPtMovingSphere {
+    float PrevPosition[3]; float Radius;  /* where the sphere starts: Camera.PrevPosition / GpuLight.PrevPosition; Radius >= 0 */
+    float Position[3];     float _pad0;   /* where it heads after the velocity integration: Camera.Position / GpuLight.Position */
+    float Velocity[3];     float _pad1;
+} IdkPtMovingSphere;
+IDK_STATIC_ASSERT(sizeof(IdkPtMovingSphere) == 48, "IdkPtMovingSphere must be 48 bytes");
+
+typedef struct IdkPtSphereCollision {
+    float Position[3]; int32_t Hits;      /* Hits: recursive steps that found a collision; 0 = Position and Velocity unchanged */
+    float Velocity[3]; float _pad0;
+} IdkPtSphereCollision;
+IDK_STATIC_ASSERT(sizeof(IdkPtSphereCollision) == 32, "IdkPtSphereCollision must be 32 bytes");
+
+/* Moves each sphere from PrevPosition towards Position through the scene as it is on the device now -- after every
+ * idkpt_update_range, idkpt_skin_vertices / idkpt_blas_refit, idkpt_update_models, idkpt_blas_rebuild and idkpt_add_models
+ * before it -- exactly as the engine's routine does with BVH.CpuUseTlas == false: instances in index order, each BLAS walked
+ * with the sphere's box in instance space (Box.Transformed by InvModelMatrix), the first candidate at the smallest distance
+ * wins. Per sphere, independently: out = the final destination, the final velocity and the number of hits. Lights are not
+ * colliders. Synchronous, host arrays in and out; the call changes nothing in the context.
+ * IDKPT_ERR_NO_SCENE without a scene. IDKPT_ERR_INVALID_ARGUMENT, with `out` untouched: a null pointer with count > 0, a null
+ * settings pointer, count >= 2^31, TestSteps < 1, RecursiveSteps outside 0 .. IDKPT_MAX_COLLISION_RECURSIVE_STEPS, an
+ * unknown Response, a negative or non-finite Radius. kernel_ms (may be NULL): device time of the kernel. */
+IDKPT_API int idkpt_collide_spheres(IdkPtCtx* ctx, const IdkPtMovingSphere* spheres, uint64_t count, const IdkPtCollisionSettings* settings,
+                                    IdkPtSphereCollision* out, float* kernel_ms);
+
 /* Ray-traced point-light shadows: ShadowsRayTraced/compute.glsl for one light (PointShadowManager.ComputeRayTracedShadowMaps,
  * Source/Render/PointShadowManager.cs:53-75). Host arrays: depth [w*h], octahedral normal rg [w*h*2]; visibility_out [w*h] is
  * read-modify-write (pixels with depth == 1 are left untouched, as the shader returns early). noise_index = the
