@@ -109,8 +109,8 @@ EXPORTS = [
     "idkpt_register_host_buffer", "idkpt_unregister_host_buffer",
     "idkpt_gather_export", "idkpt_gather_import", "idkpt_gather_connect", "idkpt_gather_device_ptr",
     "idkpt_result_device_ptr", "idkpt_tile_rows",
-    "idkpt_read_wavefront_rays", "idkpt_trace_rays", "idkpt_trace_rays_any", "idkpt_collide_spheres", "idkpt_shadows_ray_traced",
-    "idkpt_shadows_ray_traced_gbuffer", "idkpt_shadows_device_ptr", "idkpt_volumetric_lighting_gbuffer",
+    "idkpt_read_wavefront_rays", "idkpt_trace_rays", "idkpt_trace_rays_any", "idkpt_collide_spheres", "idkpt_collide_spheres_tlas",
+    "idkpt_shadows_ray_traced", "idkpt_shadows_ray_traced_gbuffer", "idkpt_shadows_device_ptr", "idkpt_volumetric_lighting_gbuffer",
     "idkpt_set_animations", "idkpt_enable_animations", "idkpt_set_node_transforms", "idkpt_update_models",
     "idkpt_set_skinning_data", "idkpt_skin_vertices", "idkpt_blas_refit", "idkpt_read_range", "idkpt_post_process", "idkpt_ldr_device_ptr", "idkpt_abi_version",
     "idkpt_denoise", "idkpt_denoise_device_ptrs", "idkpt_denoise_import_output", "idkpt_tlas_build",
@@ -493,6 +493,8 @@ def load(path=None):
     L.idkpt_trace_rays_any.argtypes = [c_vp, c_vp, c_u64, c_i32, c_vp, P(c_f)]
     L.idkpt_collide_spheres.restype = c_i32
     L.idkpt_collide_spheres.argtypes = [c_vp, c_vp, c_u64, c_vp, c_vp, P(c_f)]
+    L.idkpt_collide_spheres_tlas.restype = c_i32
+    L.idkpt_collide_spheres_tlas.argtypes = [c_vp, c_vp, c_u64, c_vp, c_vp, P(c_f)]
     L.idkpt_shadows_ray_traced.restype = c_i32
     L.idkpt_shadows_ray_traced.argtypes = [c_vp, c_vp, c_vp, c_vp, c_i32, c_i32, c_i32, c_i32, c_u32, c_vp, c_vp, P(c_f)]
     L.idkpt_shadows_ray_traced_gbuffer.restype = c_i32

@@ -397,6 +397,7 @@ static int configure_launches(IdkPtCtx* ctx) {
     CK(cudaFuncSetAttribute(k_transparency<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)ctx->stackBytes));
     CK(cudaFuncSetAttribute(k_transparency<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)ctx->stackBytes));
     CK(cudaFuncSetAttribute(k_collide_spheres, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)ctx->stackBytes));
+    CK(cudaFuncSetAttribute(k_collide_spheres_tlas, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)ctx->stackBytes));
     ctx->traverse2Smem = (size_t)stackSize * IDK_T2_BLOCK * sizeof(uint32_t);
     CK(cudaFuncSetAttribute(k_traverse2<false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)ctx->traverse2Smem));
     CK(cudaFuncSetAttribute(k_traverse2<true, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)ctx->traverse2Smem));
@@ -1693,6 +1694,7 @@ static int preload_kernels(IdkPtCtx* ctx) {
     IDK_PRELOAD(k_shading_rate); IDK_PRELOAD(k_vrs_scan); IDK_PRELOAD(k_deferred_lighting_vrs); IDK_PRELOAD(k_gbuffer);
     IDK_PRELOAD(k_transparency<false>); IDK_PRELOAD(k_transparency<true>); IDK_PRELOAD(k_lights_skybox);
     IDK_PRELOAD(k_lights_skybox_vrs); IDK_PRELOAD(k_sky_atmosphere); IDK_PRELOAD(k_sky_equirect); IDK_PRELOAD(k_collide_spheres);
+    IDK_PRELOAD(k_collide_spheres_tlas);
 #undef IDK_PRELOAD
     return IDKPT_OK;
 }
@@ -2728,12 +2730,13 @@ IDKPT_API int idkpt_trace_rays_any(IdkPtCtx* ctx, const IdkPtRay* rays, uint64_t
     return trace_rays_impl(ctx, rays, count, traceLights, hitsOut, kernelMs, true);
 }
 
-IDKPT_API int idkpt_collide_spheres(IdkPtCtx* ctx, const IdkPtMovingSphere* spheres, uint64_t count, const IdkPtCollisionSettings* settings,
-                                    IdkPtSphereCollision* out, float* kernelMs) {
-    const char* who = "idkpt_collide_spheres";
-    if (!ctx) return fail(ctx, IDKPT_ERR_INVALID_ARGUMENT, "idkpt_collide_spheres: null argument");
+static int collide_spheres_impl(IdkPtCtx* ctx, const IdkPtMovingSphere* spheres, uint64_t count, const IdkPtCollisionSettings* settings,
+                                IdkPtSphereCollision* out, float* kernelMs, bool tlas) {
+    const char* who = tlas ? "idkpt_collide_spheres_tlas" : "idkpt_collide_spheres";
+    if (!ctx) return fail(ctx, IDKPT_ERR_INVALID_ARGUMENT, tlas ? "idkpt_collide_spheres_tlas: null argument" : "idkpt_collide_spheres: null argument");
     if (!settings || (count && (!spheres || !out))) return fail(ctx, who, IDKPT_ERR_INVALID_ARGUMENT, "null argument");
     if (!ctx->haveScene) return fail(ctx, who, IDKPT_ERR_NO_SCENE, "no scene");
+    if (tlas && !ctx->counts.UseTlas) return fail(ctx, who, IDKPT_ERR_INVALID_ARGUMENT, "the scene was set without UseTlas (no TLAS to walk)");
     if (count >= (1ull << 31)) return fail(ctx, who, IDKPT_ERR_INVALID_ARGUMENT, "too many spheres");
     const IdkPtCollisionSettings st = *settings;
     if (st.TestSteps < 1) return fail(ctx, who, IDKPT_ERR_INVALID_ARGUMENT, "TestSteps must be at least 1");
@@ -2763,10 +2766,23 @@ IDKPT_API int idkpt_collide_spheres(IdkPtCtx* ctx, const IdkPtMovingSphere* sphe
     a.out = (IdkPtSphereCollision*)dout.p;
     a.count = (uint32_t)count;
     a.st = st;
+    a.tlasNodes = ctx->sc.tlasNodes;
     return run_timed(ctx, who, kernelMs, [&]() -> int {
-        k_collide_spheres<<<(unsigned)((count + IDK_BLOCK - 1) / IDK_BLOCK), IDK_BLOCK, ctx->stackBytes, ctx->stream>>>(a);
+        const unsigned blocks = (unsigned)((count + IDK_BLOCK - 1) / IDK_BLOCK);
+        if (tlas) k_collide_spheres_tlas<<<blocks, IDK_BLOCK, ctx->stackBytes, ctx->stream>>>(a);
+        else k_collide_spheres<<<blocks, IDK_BLOCK, ctx->stackBytes, ctx->stream>>>(a);
         return IDKPT_OK;
     }, out, dout.p, count * sizeof(IdkPtSphereCollision));
+}
+
+IDKPT_API int idkpt_collide_spheres(IdkPtCtx* ctx, const IdkPtMovingSphere* spheres, uint64_t count, const IdkPtCollisionSettings* settings,
+                                    IdkPtSphereCollision* out, float* kernelMs) {
+    return collide_spheres_impl(ctx, spheres, count, settings, out, kernelMs, false);
+}
+
+IDKPT_API int idkpt_collide_spheres_tlas(IdkPtCtx* ctx, const IdkPtMovingSphere* spheres, uint64_t count, const IdkPtCollisionSettings* settings,
+                                         IdkPtSphereCollision* out, float* kernelMs) {
+    return collide_spheres_impl(ctx, spheres, count, settings, out, kernelMs, true);
 }
 
 // ---- point-shadow cube maps (PointShadowManager.UpdateBuffer / RenderShadowMaps) ----------------------------------------------

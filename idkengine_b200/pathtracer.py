@@ -462,17 +462,20 @@ class PathTracer:
                                                    hits.ctypes.data, ctypes.byref(ms)), "idkpt_trace_rays_any")
         return hits, ms.value
 
-    def CollideSpheres(self, spheres, settings=None):
+    def CollideSpheres(self, spheres, settings=None, use_tlas=False):
         """Intersections.SceneVsMovingSphereCollisionRoutine for each IdkPtMovingSphere against the current device scene.
         settings: (TestSteps, RecursiveSteps, EpsilonNormalOffset, Response) or an IdkPtCollisionSettings record, default
-        LIGHT_COLLISION. Returns (IdkPtSphereCollision records, kernel ms)."""
+        LIGHT_COLLISION. use_tlas: walk the device TLAS as the engine does with BVH.CpuUseTlas (idkpt_collide_spheres_tlas;
+        the scene must have been set with UseTlas) instead of every instance in index order. Returns (IdkPtSphereCollision
+        records, kernel ms)."""
         spheres = np.ascontiguousarray(spheres)
         assert spheres.dtype == gt.IdkPtMovingSphere
         st = np.array(tuple(LIGHT_COLLISION if settings is None else settings), gt.IdkPtCollisionSettings)
         out = np.zeros(len(spheres), gt.IdkPtSphereCollision)
         ms = ctypes.c_float()
-        self._check(self._lib.idkpt_collide_spheres(self._ctx, spheres.ctypes.data, len(spheres), st.ctypes.data, out.ctypes.data,
-                                                    ctypes.byref(ms)), "idkpt_collide_spheres")
+        name = "idkpt_collide_spheres_tlas" if use_tlas else "idkpt_collide_spheres"
+        self._check(getattr(self._lib, name)(self._ctx, spheres.ctypes.data, len(spheres), st.ctypes.data, out.ctypes.data,
+                                             ctypes.byref(ms)), name)
         return out, ms.value
 
     def ShadowsRayTraced(self, frame, depth, normal_rg, light_index, samples=1, noise_index=0, jitter=(0.0, 0.0), visibility=None):

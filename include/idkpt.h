@@ -351,6 +351,20 @@ IDK_STATIC_ASSERT(sizeof(IdkPtSphereCollision) == 32, "IdkPtSphereCollision must
 IDKPT_API int idkpt_collide_spheres(IdkPtCtx* ctx, const IdkPtMovingSphere* spheres, uint64_t count, const IdkPtCollisionSettings* settings,
                                     IdkPtSphereCollision* out, float* kernel_ms);
 
+/* idkpt_collide_spheres with the engine's BVH.CpuUseTlas == true: each test step walks the TLAS as TLAS.Intersect(Box)
+ * (TLAS.cs:209-264) does. From node 0, whose own box is not tested, an interior node's children (id, id + 1) are each tested
+ * with BoxVsBox against the sphere's world box; the walk goes left when both overlap and visits the right child later, so
+ * instances are walked in depth-first TLAS leaf order, and an instance whose TLAS leaf box misses the sphere's box is never
+ * walked. A leaf walks its instance exactly as idkpt_collide_spheres does. The first candidate at the smallest distance still
+ * wins, so a tie between instances goes to the one first in depth-first order rather than the lower instance index, and the
+ * result can differ from idkpt_collide_spheres there. The walk reads the TLAS nodes as they are on the device now (as set by
+ * idkpt_set_scene, idkpt_update_range(IDKPT_ARRAY_TLAS_NODES), idkpt_tlas_build, idkpt_update_models or idkpt_add_models)
+ * and never rebuilds them: after a transform upload without a TLAS rebuild the TLAS is stale, as the engine's is.
+ * Refusals and their order are those of idkpt_collide_spheres, with texts naming this call, plus
+ * IDKPT_ERR_INVALID_ARGUMENT (out untouched) when the scene was set without UseTlas. */
+IDKPT_API int idkpt_collide_spheres_tlas(IdkPtCtx* ctx, const IdkPtMovingSphere* spheres, uint64_t count, const IdkPtCollisionSettings* settings,
+                                         IdkPtSphereCollision* out, float* kernel_ms);
+
 /* Ray-traced point-light shadows: ShadowsRayTraced/compute.glsl for one light (PointShadowManager.ComputeRayTracedShadowMaps,
  * Source/Render/PointShadowManager.cs:53-75). Host arrays: depth [w*h], octahedral normal rg [w*h*2]; visibility_out [w*h] is
  * read-modify-write (pixels with depth == 1 are left untouched, as the shader returns early). noise_index = the

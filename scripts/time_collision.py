@@ -1,13 +1,15 @@
-"""Timing of scene-versus-moving-sphere collision on the device (idkpt_collide_spheres, DESIGN 8f "Collision").
+"""Timing of scene-versus-moving-sphere collision on the device (idkpt_collide_spheres and idkpt_collide_spheres_tlas,
+DESIGN 8f "Collision").
 
-    python scripts/time_collision.py [--reps 5] [--counts 1,257,65536] [--scenes atrium,instances] [--out FILE]
+    python scripts/time_collision.py [--reps 5] [--counts 1,257,65536] [--scenes atrium,instances] [--modes linear,tlas] [--out FILE]
 
-Scenes: the 262 k-triangle atrium (one instance, no TLAS) and the 262 144-instance grid of the TLAS timings (instance_grid(2)'s
-BLASes, scale 0.4, 1.25 apart) with its TLAS built on the device. Spheres, seeded: a start anywhere in the scene's bounds, a
-destination up to 0.5 away, radius 0.02 .. 0.5. For each scene, sphere count and preset (the lights' 1 test step and 8
-recursive steps with Plane.Reflect, the camera's 3 and 12 with Plane.Project):
+Scenes: the 262 k-triangle atrium (one instance; its TLAS is that instance's leaf) and the 262 144-instance grid of the TLAS
+timings (instance_grid(2)'s BLASes, scale 0.4, 1.25 apart) with its TLAS built on the device. Spheres, seeded: a start
+anywhere in the scene's bounds, a destination up to 0.5 away, radius 0.02 .. 0.5. For each scene, mode, sphere count and
+preset (the lights' 1 test step and 8 recursive steps with Plane.Reflect, the camera's 3 and 12 with Plane.Project):
   device   PathTracer.CollideSpheres: the kernel's device time (kernel_ms) and the host clock around the call (upload, kernel,
-           download), median over --reps calls after two warm-ups.
+           download), median over --reps calls after two warm-ups. Mode `linear` visits every instance in index order
+           (CpuUseTlas == false), mode `tlas` walks the TLAS (CpuUseTlas == true); a scene without a TLAS has no tlas rows.
 Beside each scene: the bytes of the read-backs the call makes unnecessary, from the scene's shapes: the vertex positions, the
 BLAS nodes and triangles (the host BVH that BVH.Intersect walks) and the mesh transforms. The card name and power limit are
 read in the same run.
@@ -30,7 +32,7 @@ PRESETS = {"lights": LIGHT_COLLISION, "camera": CAMERA_COLLISION}
 def make_scene(name):
     if name == "atrium":
         sc, _ = scenes.atrium(262144, threads=os.cpu_count())
-        return sc
+        return sc.build_tlas()
     return scenes._instanced(scenes._grid_matrices(262144))
 
 
@@ -65,6 +67,7 @@ def main():
     ap.add_argument("--reps", type=int, default=5)
     ap.add_argument("--counts", default="1,257,65536")
     ap.add_argument("--scenes", default="atrium,instances")
+    ap.add_argument("--modes", default="linear,tlas")
     ap.add_argument("--out", default="")
     a = ap.parse_args()
     dev = card()
@@ -81,20 +84,21 @@ def main():
             pt.SetScene(sc)
             if sc.use_tlas:
                 pt.TlasBuild()
-            for n in (int(x) for x in a.counts.split(",")):
-                s = spheres(sc, n, seed=n)
-                for preset, st in PRESETS.items():
-                    kernel, host = [], []
-                    for _ in range(a.reps + 2):
-                        t0 = time.perf_counter()
-                        out, ms = pt.CollideSpheres(s, st)
-                        host.append((time.perf_counter() - t0) * 1e3)
-                        kernel.append(ms)
-                    row = dict(spheres=n, preset=preset, kernel_ms=float(np.median(kernel[2:])), call_ms=float(np.median(host[2:])),
-                               hit_spheres=int((out["Hits"] > 0).sum()), hits=int(out["Hits"].sum()))
-                    rows.append(row)
-                    print(f"  {n:6d} spheres  {preset:6s}  kernel {row['kernel_ms']:9.3f} ms  call {row['call_ms']:9.3f} ms  "
-                          f"({row['hit_spheres']} spheres hit, {row['hits']} hits)")
+            for mode in (m for m in a.modes.split(",") if m == "linear" or sc.use_tlas):
+                for n in (int(x) for x in a.counts.split(",")):
+                    s = spheres(sc, n, seed=n)
+                    for preset, st in PRESETS.items():
+                        kernel, host = [], []
+                        for _ in range(a.reps + 2):
+                            t0 = time.perf_counter()
+                            out, ms = pt.CollideSpheres(s, st, use_tlas=mode == "tlas")
+                            host.append((time.perf_counter() - t0) * 1e3)
+                            kernel.append(ms)
+                        row = dict(mode=mode, spheres=n, preset=preset, kernel_ms=float(np.median(kernel[2:])),
+                                   call_ms=float(np.median(host[2:])), hit_spheres=int((out["Hits"] > 0).sum()), hits=int(out["Hits"].sum()))
+                        rows.append(row)
+                        print(f"  {mode:6s}  {n:6d} spheres  {preset:6s}  kernel {row['kernel_ms']:9.3f} ms  call {row['call_ms']:9.3f} ms  "
+                              f"({row['hit_spheres']} spheres hit, {row['hits']} hits)")
         result["scenes"][name] = dict(readback_bytes=rb, triangles=len(sc.blas_triangles), instances=len(sc.blas_instances), rows=rows)
     write_out(a.out, result)
 
