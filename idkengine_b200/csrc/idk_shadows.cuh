@@ -38,7 +38,7 @@ __device__ __forceinline__ f3 sample_sphere_light(f3 toSphere, float sphereRadiu
     const float phi = phiMax * rnd0;
     const float cosTheta = mix1(cosThetaMax, 1.0f, fmaxf(rnd1, 0.001f));
     const float sinTheta = sqrtf(fmaxf(1.0f - cosTheta * cosTheta, 0.0f));
-    distanceToSphere = sqrtf(dot3(toSphere, toSphere)) * cosTheta - sqrtf(radiusSq - distanceSq * sinTheta * sinTheta);
+    distanceToSphere = sqrtf(dot3(toSphere, toSphere)) * cosTheta - sqrtf(fmaxf(radiusSq - distanceSq * sinTheta * sinTheta, 0.0f));
     const f3 normal = normalize3(toSphere);
     float sinPhi, cosPhi;
     det_sincos(phi, &sinPhi, &cosPhi);

@@ -1463,7 +1463,7 @@ static vec3 SampleSphereLight(vec3 toSphere, float sphereRadius, float rnd0, flo
     float phi = phiMax * rnd0;
     float cosTheta = mixf(cosThetaMax, 1.0f, fmaxf(rnd1, 0.001f));
     float sinTheta = sqrtf(fmaxf(1.0f - cosTheta * cosTheta, 0.0f));
-    distanceToSphere = sqrtf(dot(toSphere, toSphere)) * cosTheta - sqrtf(radiusSq - distanceSq * sinTheta * sinTheta);
+    distanceToSphere = sqrtf(dot(toSphere, toSphere)) * cosTheta - sqrtf(fmaxf(radiusSq - distanceSq * sinTheta * sinTheta, 0.0f));
     vec3 normal = normalize(toSphere);
     float sinPhi, cosPhi;
     det_sincos(phi, &sinPhi, &cosPhi);

@@ -196,10 +196,14 @@ class Tables:
         self.lights = scene.lights
 
 
-def closest(tb, O, D):
+def closest(tb, O, D, tmax=None, spread=None, want_strict=False):
     """Float64 closest hit of rays (O, D) against every source triangle, with edge_lib's strict / lenient margins.
     Returns (kind, tri, t, eps_t, barycentrics) with kind 1 = unambiguous hit (the nearest strict triangle, every other lenient candidate
-    clearly farther), 0 = clear miss (no lenient candidate), -1 = not judged."""
+    clearly farther), 0 = clear miss (no lenient candidate), -1 = not judged.
+    tmax: per-ray (limit, its uncertainty) [N]: only hits with t < limit count, and a hit within the uncertainty of it is not
+    judged. spread: per-ray (a, b) [N]: the float32 ray may start up to a away from O and point up to b radians away from D,
+    which widens every margin by the displacement a + b t on the triangle's plane. want_strict: also return whether any
+    triangle is in the strict set (an any-hit verdict that holds whichever of them is the closest)."""
     O, D = np.asarray(O, np.float64), np.asarray(D, np.float64)
     N = len(O)
     p0, e1, e2, n = tb.p[:, 0], tb.e1, tb.e2, tb.n
@@ -218,11 +222,23 @@ def closest(tb, O, D):
         S = np.linalg.norm(rop0, axis=2) + np.linalg.norm(O, axis=1)[:, None] + np.linalg.norm(p0, axis=1)[None]
         eb = EPS + K * U32 * kappa * (1.0 + S / lmin[None])
         et = EPS * np.abs(t) + K * U32 * area2[None] * S / np.abs(det)
+        dpos = 0.0
+        if spread is not None:
+            # a displacement d of the ray moves its hit on the plane by d / cos, a barycentric by that over the lowest height
+            dpos = np.asarray(spread[0], np.float64)[:, None] + np.asarray(spread[1], np.float64)[:, None] * np.abs(t)
+            lmax = np.maximum(np.maximum(l1, l2), np.linalg.norm(tb.p[:, 2] - tb.p[:, 1], axis=1))
+            dn = np.linalg.norm(D, axis=1)[:, None] / np.abs(det)
+            eb = eb + dpos * lmax[None] * dn
+            et = et + dpos * np.linalg.norm(n, axis=1)[None] * dn
         bmin = np.minimum(np.minimum(b0, b1), b2)
         graze = ~(kappa <= GRAZE_KAPPA)
         strict = ~graze & (bmin >= eb) & (t >= et)
         dist = np.abs(np.einsum("mk,rmk->rm", n, rop0)) / np.linalg.norm(n, axis=1)[None]
-        lenient = (~graze & (bmin >= -eb) & (t >= -et)) | (graze & (dist <= EPS * lmin[None] + K * U32 * S))
+        lenient = (~graze & (bmin >= -eb) & (t >= -et)) | (graze & (dist <= EPS * lmin[None] + K * U32 * S + dpos))
+        if tmax is not None:
+            lim, elim = (np.asarray(v, np.float64)[:, None] for v in tmax)
+            strict &= t + et < lim - elim
+            lenient &= graze | (t - et < lim + elim)
     ts = np.where(strict, t, np.inf)
     best = np.argmin(ts, 1)
     r = np.arange(N)
@@ -234,6 +250,8 @@ def closest(tb, O, D):
     miss = ~lenient.any(1)
     kind = np.where(hit, 1, np.where(miss, 0, -1))
     bary = np.stack([b0[r, best], b1[r, best], b2[r, best]], 1)
+    if want_strict:
+        return kind, best, tb_, eb_, bary, np.isfinite(ts[r, best])
     return kind, best, tb_, eb_, bary
 
 
