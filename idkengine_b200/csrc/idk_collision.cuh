@@ -22,7 +22,7 @@
 // Float semantics: OpenTK's Vector3 formulas in fp32, left to right, no contraction (the library is built with -fmad=false):
 // Dot = x*x' + y*y' + z*z', Distance = sqrt of the sum of the squared differences, Vector3 / float divides each component,
 // Vector4(p, 1) * Matrix4 = ((x*m0 + y*m1) + z*m2) + m3 per row of the stored 3x4. The CPU oracle
-// (tests/cpp/collision_oracle.cpp) restates the same rules; the two agree bit for bit.
+// (oracle_collide_spheres) restates the same rules; the two agree bit for bit.
 #pragma once
 #include "idk_kernels.cuh"
 

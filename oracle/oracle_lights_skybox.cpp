@@ -54,7 +54,7 @@ inline vec3 LsWorld(const GpuLight& L, const float* position, vec3 p) {
 
 struct LsPixel { float depth, normal[2], emissive[3], velocity[2], color[4]; int winner; bool light, sky; };
 
-LsPixel LsShadePixel(const Scene& s, const GpuPerFrameData& f, int x, int y, int w, int h, const float jitter[2], float gDepth) {
+ORACLE_INLINE LsPixel LsShadePixel(const Scene& s, const GpuPerFrameData& f, int x, int y, int w, int h, const float jitter[2], float gDepth) {
     LsPixel px = {};
     px.depth = gDepth;
     px.winner = -1;

@@ -1,10 +1,10 @@
 // ORACLE (TEST INFRASTRUCTURE ONLY) -- the light spheres and the skybox under the shading-rate image (idkpt_lights_and_skybox_vrs).
 //
-// The root of its own library, liboracle_lights_skybox_vrs.so, which tests/lights_skybox_vrs_oracle.py builds and wraps. It
-// includes the per-pixel oracle (oracle_lights_skybox.cpp, and with it oracle_gbuffer.cpp and oracle.cpp) and the
-// variable-rate deferred oracle (oracle_vrs.cpp) and reuses LsShadePixel's coverage, depth test and winner, the sphere mesh,
-// RayTriangleIntersect, EncodeUnitVec, SampleSky, the attachment conversions and VrsFragmentSize unchanged. What the fragment
-// shaders compute at the coarse fragment's centre is restated here.
+// Part of liboracle.so (wrapped by tests/lights_skybox_vrs_oracle.py). It includes the per-pixel oracle
+// (oracle_lights_skybox.cpp, and with it oracle_gbuffer.cpp and oracle.cpp) and the variable-rate deferred oracle
+// (oracle_vrs.cpp) and reuses LsShadePixel's coverage, depth test and winner, the sphere mesh, RayTriangleIntersect,
+// EncodeUnitVec, SampleSky, the attachment conversions and VrsFragmentSize unchanged. What the fragment shaders compute at the
+// coarse fragment's centre is restated here.
 //
 // Restated sources (relative to the reference repository's IDKEngine):
 //   Source/Render/RasterPipeline.cs:465-516                    "Draw lights" and "Draw skybox" with VariableRateShadingNV
@@ -83,12 +83,13 @@ void LsShadeAtCentre(const Scene& s, const GpuPerFrameData& f, int x, int y, int
 
 } // namespace
 
+extern "C" {
+
 // idkpt_lights_and_skybox_vrs: oracle_lights_skybox's arguments and, before `threads`, rates [ceil(h/16)][ceil(w/16)] (palette
-// indices 0..4). Returns 0, or 1 for an argument the library rejects. Its ctypes signature is declared with its wrapper,
-// tests/lights_skybox_vrs_oracle.py, which also builds this library.
-extern "C" ORACLE_API int oracle_lights_skybox_vrs(const IdkPtSceneDesc* scene, const IdkPtSkyDesc* sky, const GpuPerFrameData* frame,
-                                                   int w, int h, const float* jitter, float* depth, float* normal, float* emissive,
-                                                   float* velocity, float* color, int32_t* winner, const uint8_t* rates, int threads) {
+// indices 0..4). Returns 0, or 1 for an argument the library rejects.
+ORACLE_API int oracle_lights_skybox_vrs(const IdkPtSceneDesc* scene, const IdkPtSkyDesc* sky, const GpuPerFrameData* frame, int w, int h,
+                                        const float* jitter, float* depth, float* normal, float* emissive, float* velocity, float* color,
+                                        int32_t* winner, const uint8_t* rates, int threads) {
     if (!scene || !frame || !rates || w < 1 || h < 1) return 1;
     const int tilesX = (w + 15) / 16;
     for (size_t t = 0; t < (size_t)tilesX * ((h + 15) / 16); t++)
@@ -118,3 +119,5 @@ extern "C" ORACLE_API int oracle_lights_skybox_vrs(const IdkPtSceneDesc* scene, 
     });
     return 0;
 }
+
+} // extern "C"

@@ -1,52 +1,11 @@
 """ctypes wrapper of the variable-rate light-sphere and skybox oracle (oracle/oracle_lights_skybox_vrs.cpp), which
-tests/test_lights_skybox_vrs*.py use. The oracle is the root of its own library, liboracle_lights_skybox_vrs.so, built here
-with oracle/build.py's compiler flags; the export's signature is declared here, beside the wrapper."""
+tests/test_lights_skybox_vrs*.py use."""
 import ctypes
-import glob
-import os
-import subprocess
-import tempfile
 
 import numpy as np
 
 import oracle_lib as ol
 from idkengine_b200 import capi
-
-ORACLE_DIR = os.path.join(ol.REPO, "oracle")
-SOURCE = os.path.join(ORACLE_DIR, "oracle_lights_skybox_vrs.cpp")
-
-# name -> (restype, argtypes) of the exports this module declares
-SIGNATURES = {
-    "oracle_lights_skybox_vrs": (ctypes.c_int32, [ctypes.POINTER(capi.IdkPtSceneDesc), ctypes.POINTER(capi.IdkPtSkyDesc)] +
-                                 [ctypes.c_void_p, ctypes.c_int32, ctypes.c_int32] + [ctypes.c_void_p] * 8 + [ctypes.c_int32]),
-}
-
-_fn = None
-
-
-def build():
-    """The library beside liboracle.so (or, where the tree is read-only, in the temporary directory), rebuilt when an oracle
-    source or public header is newer than it."""
-    out_dir = ORACLE_DIR if os.access(ORACLE_DIR, os.W_OK) else tempfile.gettempdir()
-    target = os.path.join(out_dir, "liboracle_lights_skybox_vrs.so")
-    deps = [f for pattern in ("*.cpp", "*.inc") for f in glob.glob(os.path.join(ORACLE_DIR, pattern))] + \
-        glob.glob(os.path.join(ol.REPO, "include", "*.h"))
-    if os.path.exists(target) and all(os.path.getmtime(d) <= os.path.getmtime(target) for d in deps):
-        return target
-    tmp = "%s.%d.tmp" % (target, os.getpid())
-    subprocess.run(["g++", "-O2", "-std=c++17", "-ffp-contract=off", "-fno-fast-math", "-fPIC", "-shared", "-pthread",
-                    "-fvisibility=hidden", "-I", ORACLE_DIR, "-o", tmp, SOURCE], check=True)
-    os.replace(tmp, target)    # a process that loads the library meanwhile sees the old file or the new one, never half of one
-    return target
-
-
-def _oracle():
-    global _fn
-    if _fn is None:
-        fn = ctypes.CDLL(build()).oracle_lights_skybox_vrs
-        fn.restype, fn.argtypes = SIGNATURES["oracle_lights_skybox_vrs"]
-        _fn = fn
-    return _fn
 
 
 def tiles_of(w, h):
@@ -66,9 +25,10 @@ def lights_and_skybox_vrs(scene, frame, gbuffer, color, rates, jitter=None, sky=
     winner = np.zeros((h, w), np.int32)
     jit = None if jitter is None else np.ascontiguousarray(jitter, np.float32)
     sd = None if sky is None else capi.sky_desc(sky)
-    rc = _oracle()(ctypes.byref(d), ctypes.byref(sd) if sd is not None else None, fr.ctypes.data, w, h,
-                   jit.ctypes.data if jit is not None else None, g[0].ctypes.data, g[1].ctypes.data, g[4].ctypes.data,
-                   g[5].ctypes.data, col.ctypes.data, winner.ctypes.data, r.ctypes.data, threads or ol.default_threads())
+    rc = ol.lib().oracle_lights_skybox_vrs(ctypes.byref(d), ctypes.byref(sd) if sd is not None else None, fr.ctypes.data, w, h,
+                                          jit.ctypes.data if jit is not None else None, g[0].ctypes.data, g[1].ctypes.data,
+                                          g[4].ctypes.data, g[5].ctypes.data, col.ctypes.data, winner.ctypes.data, r.ctypes.data,
+                                          threads or ol.default_threads())
     assert rc == 0, rc
     del keep
     return tuple(g), col, winner

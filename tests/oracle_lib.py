@@ -75,6 +75,8 @@ def _signatures():
         # oracle_lights_skybox.cpp
         "oracle_lights_skybox": (i32, [SCENE, vp, vp, i32, i32, vp, vp, vp, vp, vp, vp, vp, i32]),
         "oracle_sphere_mesh": (None, [vp, vp]),
+        # oracle_lights_skybox_vrs.cpp
+        "oracle_lights_skybox_vrs": (i32, [SCENE, SKY, vp, i32, i32] + [vp] * 8 + [i32]),
         # oracle_volumetric.cpp
         "oracle_volumetric_lighting": (i32, [vp, u64, vp, P(capi.IdkPtVolumetricSettings), vp, vp, vp, i32, vp, i32, i32, i32, i32,
                                              vp, vp, vp, vp]),
@@ -91,6 +93,8 @@ def _signatures():
         "oracle_vx_voxelize_conservative_shadow_maps": (i32, [SCENE, CI, vp, vp, vp, i32, vp, u64, P(u64), i32]),
         # oracle_vxgi_debug.cpp
         "oracle_vx_debug_render": (i32, [vp, vp, vp, vp, f32, f32, i32, i32, vp, P(u64), i32]),
+        # oracle_collision.cpp
+        "oracle_collide_spheres": (i32, [SCENE, vp, u64, vp, vp, vp, vp, i32, i32]),
     }
 
 

@@ -1,23 +1,22 @@
-"""The C#-semantics scene-versus-moving-sphere oracle (oracle_collide_spheres, the checker of idkpt_collide_spheres) against
-closed forms and a float64 brute force, and the collision records' layout."""
+"""The C#-semantics scene-versus-moving-sphere oracle (oracle_collide_spheres, the checker of idkpt_collide_spheres and
+idkpt_collide_spheres_tlas) against closed forms and a float64 brute force, and the collision records' layout.
+
+The oracle's TLAS walk (BVH.CpuUseTlas, TLAS.Intersect(Box)) is checked against its linear walk. The two walks test the same
+triangles with the same arithmetic; they differ only in which instances they reach and in what order, so the winner of a test
+step can differ only between candidates at the same distance."""
 import numpy as np
 import pytest
 
 import collision_oracle as co
 import oracle_lib as ol
+from collision_oracle import random_spheres, spheres, visit_order_case, with_tlas
 from edge_lib import world_triangles
 from idkengine_b200 import capi, gpu_types as gt, scenes
 from idkengine_b200.pathtracer import CAMERA_COLLISION, LIGHT_COLLISION
 
 EPS = 0.001
 SLIDE, REFLECT = capi.IDKPT_COLLISION_SLIDE, capi.IDKPT_COLLISION_REFLECT
-
-
-def spheres(prev, dest, radius, vel=None):
-    s = np.zeros(len(prev), gt.IdkPtMovingSphere)
-    s["PrevPosition"], s["Position"], s["Radius"] = prev, dest, radius
-    s["Velocity"] = 0.0 if vel is None else vel
-    return s
+PRESETS = pytest.mark.parametrize("settings", [LIGHT_COLLISION, CAMERA_COLLISION], ids=["lights", "camera"])
 
 
 def test_record_layouts():
@@ -132,3 +131,57 @@ def test_chosen_triangle_and_distance_match_a_float64_brute_force():
         assert abs(float(dist[i]) - best) <= 1e-5 * max(1.0, float(np.abs(c).max())), (i, dist[i], best)
         checked += 1
     assert checked >= n // 2, checked
+
+
+# ---- the TLAS walk ----------------------------------------------------------------------------------------------------------
+SINGLE = {
+    "closed_box": lambda: with_tlas(scenes.closed_box(subdiv=4, threads=1)[0]),
+    "open_floor": lambda: with_tlas(scenes.open_floor(threads=1)[0]),
+    "atrium": lambda: with_tlas(scenes.atrium(target_tris=20000, threads=1)[0]),
+}
+
+
+@PRESETS
+@pytest.mark.parametrize("name", list(SINGLE))
+def test_single_instance_tlas_equals_the_linear_walk(name, settings):
+    """With one instance the TLAS root is that instance's leaf: both walks visit the same BLAS, so every byte agrees."""
+    sc = SINGLE[name]()
+    assert len(sc.tlas_nodes) == 1 and sc.tlas_nodes["IsLeafAndChildOrInstanceId"][0] == 0x80000000
+    s = random_spheres(sc, 2048, seed=len(name))
+    lin = co.collide_spheres(sc, s, settings)
+    tl = co.collide_spheres(sc, s, settings, use_tlas=True)
+    for a, b in zip(lin, tl):
+        assert a.tobytes() == b.tobytes()
+    assert (lin[0]["Hits"] > 0).sum() >= 16
+
+
+INSTANCED = {
+    "instance_grid": lambda: scenes.instance_grid(3, threads=1)[0],
+    "grid_4096": lambda: with_tlas(scenes._instanced(scenes._grid_matrices(4096))),
+}
+
+
+@PRESETS
+@pytest.mark.parametrize("name", list(INSTANCED))
+def test_instanced_first_winner_agrees_up_to_ties(name, settings):
+    """The first recursive step's winner is the linear walk's, or a different candidate at exactly the same distance."""
+    sc = INSTANCED[name]()
+    s = random_spheres(sc, 4096, seed=17 + len(name))
+    _, lf, ld = co.collide_spheres(sc, s, settings)
+    out, tf, td = co.collide_spheres(sc, s, settings, use_tlas=True)
+    same = (lf == tf).all(1)
+    assert (ld[~same].view(np.uint32) == td[~same].view(np.uint32)).all(), np.flatnonzero(~same)[:8]
+    assert ((lf[:, 0] >= 0) == (tf[:, 0] >= 0)).all()
+    assert (out["Hits"] > 0).sum() >= 16
+
+
+@PRESETS
+def test_ties_go_to_the_depth_first_instance(settings):
+    sc, s, want = visit_order_case()
+    assert len(want) >= 2, want
+    _, lf, ld = co.collide_spheres(sc, s, settings)
+    _, tf, td = co.collide_spheres(sc, s, settings, use_tlas=True)
+    assert (ld == 0.5).all() and (td == 0.5).all()
+    assert tf[:, 1].tolist() == [w[0] for w in want]      # the TLAS walk: the leaf it reaches first
+    assert lf[:, 1].tolist() == [w[1] for w in want]      # the linear walk: the lower instance index
+    assert (tf[:, 1] != lf[:, 1]).all()

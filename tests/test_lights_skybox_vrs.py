@@ -4,16 +4,12 @@ per-pixel oracle and an independent float64 restatement of the fragment-centre r
 As in tests/test_lights_skybox.py the oracle reads a hand-made G-buffer over the Cornell box's scene record, with its own lights
 and cameras; the rate images come from the classifier oracle (five rates) or are written directly."""
 import copy
-import glob
-import os
-import re
 
 import numpy as np
 import pytest
 
 import lights_skybox_oracle as lo
 import lights_skybox_vrs_oracle as lvo
-import oracle_lib as ol
 import vrs_oracle as vo
 from idkengine_b200 import gpu_types as gt
 from idkengine_b200 import host, scenes
@@ -123,17 +119,6 @@ def sky_dirs64(frame, px, py, w, h):
     v = ndc @ mat(frame, "InvProjection").T
     v = v[..., :3] / v[..., 3:]
     return v @ mat(frame, "InvView")[:3, :3].T
-
-
-# ---- the oracle's export ----------------------------------------------------------------------------------------------------
-def test_every_oracle_export_has_a_signature():
-    """Each export of the oracle sources, however its line starts, is declared by oracle_lib's table or by its wrapper's."""
-    names = set()
-    for path in glob.glob(os.path.join(ol.REPO, "oracle", "*.cpp")) + glob.glob(os.path.join(ol.REPO, "oracle", "*.inc")):
-        with open(path) as f:
-            names |= set(re.findall(r"\bORACLE_API\b[^(;]*?\b(oracle_\w+)\(", f.read()))
-    assert "oracle_lights_skybox_vrs" in names
-    assert names == set(ol.SIGNATURES) | set(lvo.SIGNATURES), names ^ (set(ol.SIGNATURES) | set(lvo.SIGNATURES))
 
 
 # ---- full rate and coverage -------------------------------------------------------------------------------------------------

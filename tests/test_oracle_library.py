@@ -11,7 +11,7 @@ def test_signature_table_covers_every_export():
     names = set()
     for path in glob.glob(os.path.join(ol.REPO, "oracle", "*.cpp")) + glob.glob(os.path.join(ol.REPO, "oracle", "*.inc")):
         with open(path) as f:
-            names |= set(re.findall(r"^ORACLE_API\b[^(]*?\b(oracle_\w+)\(", f.read(), re.M))
+            names |= set(re.findall(r"\bORACLE_API\b[^(;]*?\b(oracle_\w+)\(", f.read()))
     assert names == set(ol.SIGNATURES), names ^ set(ol.SIGNATURES)
     L = ol.lib()
     missing = sorted(name for name in names if not hasattr(L, name))
